@@ -14,6 +14,11 @@ One step = one frame of the hot path (pathtag .. fine) over the synthetic scene.
            full image D2H inside the timed region.
 Timing   : CUDA events on the renderer's stream around every step; L2 is flushed (256 MiB write) between
            steps outside the event pairs; max over ranks; clocks sampled with nvidia-smi during the run.
+--dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step rendered (the RGBA8 frame a caller of
+           vb_render_resident receives) as DIR/*.npy, so that two builds can be compared output for output:
+             frame_row_sums.npy      float64 (H, 4)  per-row sums of every channel value of the whole frame
+             frame_sample.npy        float32 (N, 4)  channel values (0..255) of N <= 2^20 pixels drawn with a fixed seed
+             frame_sample_index.npy  float64 (N,)    their row-major pixel indices
 """
 import argparse
 import ctypes as C
@@ -39,7 +44,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 def build_scene(args):
@@ -57,7 +62,7 @@ def build_scene(args):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         self.index = index
@@ -154,6 +159,19 @@ def run_cpu_arm(args, packed, as_reference):
         1000.0 * sum(times) / len(times), len(times), frame
 
 
+def dump_frame(out_dir, r, device_ptr, h, w):
+    """Write the frame at `device_ptr` (h x w RGBA8 on the renderer's device) as the arrays --dump-outputs documents."""
+    frame = np.zeros((h, w, 4), dtype=np.uint8)
+    assert r.lib.vb_copy_to_host(r.handle, C.c_void_p(device_ptr), C.c_void_p(frame.ctypes.data), C.c_size_t(frame.nbytes)) == 0
+    flat = frame.reshape(-1, 4)
+    n = min(flat.shape[0], 1 << 20)
+    idx = np.sort(np.random.default_rng(0).choice(flat.shape[0], size=n, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "frame_row_sums.npy"), frame.sum(axis=1, dtype=np.float64))
+    np.save(os.path.join(out_dir, "frame_sample.npy"), flat[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "frame_sample_index.npy"), idx.astype(np.float64))
+
+
 _REAL_STDOUT = None
 
 
@@ -188,6 +206,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-exchange", action="store_true", help="N > 1: every rank flattens the whole scene (round-1 behaviour)")
     ap.add_argument("--profile-only", action="store_true", help="just run warmup+steps resident frames (for ncu)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's frame (row sums + a fixed, seeded pixel sample) as DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if not args.profile_only else args.warmup
 
@@ -452,9 +472,12 @@ def main():
     total_ms = float(step_ms.sum().item())
     fps = args.steps / (total_ms / 1000.0)
     rank_totals = [v[0] for v in allgather_floats([my_total])]
+    if args.dump_outputs and rank == 0:
+        assert world == 1 or p2p_frame, "--dump-outputs: the stripes were not assembled into one frame on this box"
+        dump_frame(args.dump_outputs, r, frame_base, H, args.size)
 
     # ---- the same K steps with the stripes LEFT ON THEIR GPUS (every rank paints into its own buffer, no NVLink traffic): at
-    # 16384^2 the assembly of 1 GiB per frame on one GPU is bound by that GPU's NVLink ingest (~0.8 TB/s), SURVEY.md 8e asks
+    # 16384^2 the assembly of 1 GiB per frame on one GPU is bound by that GPU's NVLink ingest, SURVEY.md 8e asks
     # for both figures
     distributed = None
     if world > 1:
@@ -520,7 +543,7 @@ def main():
             assert rc == 0 and fs.failed == 0
         assert r.lib.vb_readback_wait(r.handle) == 0  # every frame's pixels are in host memory when the clock stops
 
-    e2e_steps = max(6, args.steps // 2)
+    e2e_steps = args.steps
     e2e_fps_by_mode = {}
     for mode in ("sync", "stream"):
         for _ in range(3):
@@ -618,23 +641,7 @@ def main():
                 "whole_list": {"bytes": 4 * px + 4 * full_words + 24 * full_segs, "fill_cmds": full_fills},
                 "note": "bytes = pixels + the PTCL words and segments fine reads from each tile's occlusion start (last opaque "
                 "full-tile cover, noted by coarse); whole_list = the same count over the complete lists the reference executes. "
-                "MSAA16 fine is issue / shared-memory-atomic bound, not HBM bound (SURVEY.md 8d caveat): see issue_bound"}
-    # dram traffic and warp-instruction count of k_fine are ncu measurements: they are quoted only when the capture under
-    # profiles/ was made with THIS k_fine.cu at THIS configuration (hash + workload recorded beside the numbers), else null
-    try:
-        import hashlib
-        meta = json.load(open(os.path.join(ROOT, "profiles", "fine_ncu.json")))
-        src_hash = hashlib.sha256(open(os.path.join(ROOT, "vello_b200", "csrc", "k_fine.cu"), "rb").read()).hexdigest()[:16]
-        if meta.get("k_fine_sha16") == src_hash and meta.get("workload") == config["workload"] and world == 1:
-            roofline["traffic"] = meta.get("dram_bytes_per_launch")
-            wi = meta.get("warp_instructions")
-            if wi and clocks and clocks.get("sm_mhz"):
-                issue_peak = 148 * 4 * clocks["sm_mhz"] * 1e6  # warp instructions / s: 4 schedulers per SM, one issue per cycle
-                roofline["issue_bound"] = {"warp_instructions": wi, "achieved_per_s": wi / fine_s, "peak_per_s": issue_peak,
-                                           "frac": wi / fine_s / issue_peak, "source": meta.get("source")}
-    except Exception:
-        pass
-
+                "MSAA16 fine is issue / shared-memory-atomic bound, not HBM bound (SURVEY.md 8d caveat)"}
     cpu_baseline, parity = None, {"checked": False}
     if not args.no_cpu_baseline and world == 1:  # rank 0 at N = 1 only (contract)
         # the CPU arm renders this very frame: keep it and compare the GPU's pixels with it (the oracle is the checker here,

@@ -1,4 +1,4 @@
-/* vello_b200.h -- C ABI of libvello_b200.so: a Blackwell (sm_100a) drop-in for the GPU compute
+/* vello_b200.h -- C ABI of libvello_b200.so: a Hopper (sm_90a) drop-in for the GPU compute
  * path behind vello's `Renderer::render_to_texture`.
  *
  * What each entry point replaces in the reference (linebender/vello @ 3fabef93):

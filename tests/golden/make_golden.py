@@ -9,7 +9,7 @@
   (examples/scenes/src/pico_svg.rs:134-195): per <path> the fill / stroke colours, stroke width
   and the path data string. The SVG itself is not copied.
 
-Usage: python tests/golden/make_golden.py [/root/reference]
+Usage: python tests/golden/make_golden.py <checkout of linebender/vello @ 3fabef93>
 """
 import gzip
 import json
@@ -24,7 +24,7 @@ from PIL import Image
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def main(ref="/root/reference"):
+def main(ref):
     smoke = os.path.join(ref, "vello_tests/snapshots/smoke")
     for name in ["filled_square", "filled_circle", "layer_size", "gradient_color_alpha_premultiplied",
                  "gradient_color_alpha_unpremultiplied", "data_image_roundtrip"]:

@@ -1,5 +1,5 @@
 """GPU parity tests proper: the CUDA path (through the C ABI) against the CPU oracle and the golden
-vectors. Run on the B200 box with `pytest -m gpu`.
+vectors. Run on an H100 with `pytest -m gpu`.
 
 Bar: bit-exact for every integer / index buffer and for MSAA pixels (integer sample counts);
 area-AA pixels within +-1 LSB per 8-bit channel (float sums in atomic slot order).

@@ -1,11 +1,10 @@
-"""Static checks of the compiled sm_100a code (cuobjdump / nvdisasm on the objects `build()` produces; no GPU needed).
+"""Static checks of the compiled sm_90a code (cuobjdump / nvdisasm on the objects `build()` produces; no GPU needed).
 
 * `k_fine` must keep the lane's pixels in registers: no local-memory instruction may be attributed to the MSAA fill
-  (`fill_path_ms`) or to the interpreter's CMD_FILL / CMD_SOLID / CMD_COLOR cases. Until round 2 build k four
-  `#pragma unroll 1` brush loops kept `rgba[]` / `area[]` in local memory: 132 M L2 sectors of local traffic per frame, the
-  kernel's top stall (profiles/README.md).
+  (`fill_path_ms`) or to the interpreter's CMD_FILL / CMD_SOLID / CMD_COLOR cases. Four `#pragma unroll 1` brush loops
+  once kept `rgba[]` / `area[]` in local memory, which made local traffic the kernel's top stall.
 * `k_fine` stages its mask LUT and command windows with bulk copies signalled on mbarriers (SASS UBLKCP / SYNCS), the
-  sm_100a-specific path DESIGN.md claims.
+  Hopper (sm_90a) path DESIGN.md claims.
 * no kernel of the pipeline spills more than a few registers."""
 import os
 import re

@@ -1,5 +1,5 @@
-import sys, numpy as np
-sys.path.insert(0, '/root/repo')
+import os, sys, numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from vello_b200 import scenes
 from vello_b200.config import RenderParams
 from vello_b200.encoding import BLACK, resolve

@@ -13,9 +13,9 @@ for o in build/*.o; do
   [ $skip == 0 ] && objs="$objs $o"
 done
 for f in "$@"; do
-  nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -fmad=false -Xcompiler -fPIC $extra -c $f -o /tmp/mkvariant_$name/${f%.cu}.o &
+  nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -fmad=false -Xcompiler -fPIC $extra -c $f -o /tmp/mkvariant_$name/${f%.cu}.o &
 done
 wait
 for f in "$@"; do objs="$objs /tmp/mkvariant_$name/${f%.cu}.o"; done
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../../variants/$name.so $objs
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../variants/$name.so $objs
 echo built variants/$name.so

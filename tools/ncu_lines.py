@@ -36,7 +36,7 @@ key_ix = 1 if os.environ.get("BY_SAMPLES") else 0
 for k, v in sorted(agg.items(), key=lambda kv: -kv[1][key_ix])[:top]:
     f, ln = k if k else ("?", 0)
     if f not in src:
-        try: src[f] = open("/root/repo/vello_b200/csrc/" + f).read().splitlines()
+        try: src[f] = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "vello_b200", "csrc", f)).read().splitlines()
         except Exception: src[f] = []
     text = src[f][ln - 1].strip()[:90] if 0 < ln <= len(src[f]) else ""
     print(f"{100*v[0]/ti:5.1f}% inst {100*v[1]/max(ts,1):5.1f}% smp  {f}:{ln:<5d} {text}")

@@ -1,6 +1,6 @@
-"""SASS evidence of a kernel: resource usage, opcode histogram and the instructions that prove the Blackwell-native paths
+"""SASS evidence of a kernel: resource usage, opcode histogram and the instructions that prove the Hopper-native paths
 (UBLKCP = cp.async.bulk / TMA, SYNCS = mbarrier, ATOMS / REDUX / VOTE / MATCH = warp-level protocol).
-usage: python tools/sass_summary.py <object or .so> <mangled kernel name> > profiles/sass_<kernel>.txt"""
+usage: python tools/sass_summary.py <object or .so> <mangled kernel name>"""
 import re
 import subprocess
 import sys
@@ -12,7 +12,7 @@ start = next(i for i, l in enumerate(sass) if "Function : " + kname in l)
 end = next((i for i in range(start + 1, len(sass)) if "Function : " in sass[i]), len(sass))
 body = [l for l in sass[start:end] if re.match(r"\s+/\*[0-9a-f]{4,}\*/", l)]
 ins = [re.sub(r"^\s+/\*[0-9a-f]+\*/\s+", "", l).split(";")[0].strip() for l in body]
-print(f"# SASS summary of {kname} in {obj} (cuobjdump -sass, sm_100a)")
+print(f"# SASS summary of {kname} in {obj} (cuobjdump -sass, sm_90a)")
 for i, l in enumerate(res.splitlines()):
     if kname in l:
         print("# " + l.strip())

@@ -1,4 +1,4 @@
-"""vello_b200 -- a Blackwell-native drop-in for the GPU compute path behind
+"""vello_b200 -- a Hopper-native (H100, sm_90a) drop-in for the GPU compute path behind
 `vello::Renderer::render_to_texture` (see DESIGN.md and include/vello_b200.h)."""
 from .config import AA_AREA, AA_MSAA8, AA_MSAA16, RenderParams  # noqa: F401
 from .encoding import Scene, Packed, resolve  # noqa: F401

@@ -5,7 +5,7 @@
 // stack, unlimited depth). Outputs are the reference's: clip_bboxes[i] and the patched
 // draw_monoids of EndClip objects (clip_leaf.wgsl:195-213).
 //
-// B200 design: the matching problem is restated as "nearest position to the left whose depth is
+// Design: the matching problem is restated as "nearest position to the left whose depth is
 // <= v" on the depth sequence B (B[i] = number of open clips before op i):
 //   * the BeginClip matching an EndClip at i is the last j < i with B[j] <= B[i] - 1;
 //   * the enclosing BeginClip of a BeginClip at i is the last j < i with B[j] <= B[i] - 1.

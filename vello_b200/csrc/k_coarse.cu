@@ -6,7 +6,7 @@
 // The per-tile command SEQUENCE is identical to the reference's; segment slices and dynamic PTCL
 // chunks come from atomic bump allocators, so their absolute offsets are allocation-order
 // dependent (as in the reference). Only bins inside the stripe window are launched.
-// Parallelism: the WGSL launches one workgroup per bin (256 at 4096^2 -- far fewer than a B200 can hold), and the
+// Parallelism: the WGSL launches one workgroup per bin (256 at 4096^2 -- far fewer than an H100 can hold), and the
 // per-bin coverage loop is a chain of dependent global loads. Here every bin is split into four 8x8-tile QUADRANTS,
 // each handled by its own CTA (all 256 threads share the (draw, tile) coverage loop, threads 0..63 own a tile each for
 // emission), and the coverage loop keeps two independent tile loads in flight.

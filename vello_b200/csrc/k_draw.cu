@@ -4,7 +4,7 @@
 // Reference: vello_shaders/shader/draw_reduce.wgsl:22-55, draw_leaf.wgsl:53-303,
 // shared/drawtag.wgsl:47-54, shared/transform.wgsl; CPU twins cpu/draw_reduce.rs, cpu/draw_leaf.rs.
 //
-// B200 design: one pass, decoupled look-back over the 4-field monoid (the WGSL strides <= 256
+// Design: one pass, decoupled look-back over the 4-field monoid (the WGSL strides <= 256
 // workgroups over the tags and rescans the reduced prefix in every workgroup).
 #include "vb_device.cuh"
 

@@ -1,8 +1,8 @@
 // k_exchange.cu -- flatten sharded by tag range across the GPUs of one box, with the line soup exchanged through peer memory.
 //
 // SURVEY.md 8(e) option B. In the stripe split every GPU needs the lines that touch ITS tile rows and the bounding box of
-// every path; computing them is the stage that does not shrink with the stripe (the replicated floor of round 1: 0.13 ms
-// of a 0.46 ms frame at 8 GPUs, 0.29 of 0.65 ms on the cubic-heavy workload). Here GPU r flattens only partitions
+// every path; computing them is the stage that does not shrink with the stripe (the replicated floor of round 1,
+// largest on the cubic-heavy workload). Here GPU r flattens only partitions
 // [P*r/G, P*(r+1)/G) of the tag stream and the results are exchanged over NVLink / NVSwitch WITHOUT a host round trip or a
 // library collective -- peers read each other's memory directly and synchronise through flags in that memory:
 //

@@ -5,10 +5,10 @@
 // fine; our oracle (oracle/vbo_fine.c) restates the WGSL and this kernel must match it bit for bit
 // (MSAA: integer sample counts -> exact; area: float sums in slice order).
 //
-// B200 design (v3): PERSISTENT WARPS, ONE WARP PER TILE, TMA-STAGED COMMAND WINDOWS.
+// Design (v3): PERSISTENT WARPS, ONE WARP PER TILE, TMA-STAGED COMMAND WINDOWS.
 //  * The grid is sized to the machine (2 CTAs of FI_MAX_WARPS warps per SM) and every warp pulls tile indices from a
 //    global queue (one atomic per tile, issued two tiles ahead), so a long tile no longer idles the other warp
-//    slots of its CTA (v2: 32,768 two-warp CTAs, 36 % achieved occupancy against 50 % theoretical).
+//    slots of its CTA (v2 launched one two-warp CTA per pair of tiles).
 //  * The half-plane mask LUT (8 KB for MSAA16) is copied ONCE per CTA into shared memory with one bulk copy
 //    (cp.async.bulk + mbarrier, the TMA path; v2 fetched it with __ldg per pixel touch).
 //  * Each warp owns two 256-byte command windows in shared memory. A window is filled by one bulk copy signalled on
@@ -24,9 +24,8 @@
 //    the winding words. The integer arithmetic per touched pixel is the WGSL's, word for word.
 //  * Each tile starts at its occlusion start (the last opaque full-tile cover, noted by coarse).
 //  * The lane's 8 pixels (rgba[8], area[8]: 40 registers) are only ever indexed by compile-time constants, so they live in
-//    registers for the whole tile; the rarely used brushes that loop over them without unrolling work on a copy. (Until
-//    round 2 build k a dynamically indexed loop kept them in local memory: 132 M L2 sectors of local traffic per frame,
-//    ncu `memory_l2_theoretical_sectors_local`, against 6.5 M sectors of global traffic -- the top stall of the kernel.)
+//    registers for the whole tile; the rarely used brushes that loop over them without unrolling work on a copy. (A dynamically
+//    indexed loop once kept them in local memory, and that local traffic was the top stall of the kernel.)
 // Conventions fixed where WGSL leaves latitude: see oracle/vbo_fine.c.
 // Algorithmic bytes: 4 B/pixel stored + 4 B per PTCL word + 24 B per segment referenced.
 #include <cuda_fp16.h>

@@ -4,7 +4,7 @@
 // caps :521-545, joins :547-631, segment decode :683-766, main :831-923) and its CPU twin
 // vello_shaders/src/cpu/{flatten,euler}.rs. Also folds in bbox_clear.wgsl.
 //
-// B200 design (differs from the WGSL on purpose; the pieces are described where they are defined below):
+// Design (differs from the WGSL on purpose; the pieces are described where they are defined below):
 //  * The WGSL bump-allocates every line with a global atomicAdd, so the line order is a race. Here line order is
 //    deterministic -- tag order, then emission order, i.e. the serial CPU shader's -- and independent of any atomic:
 //    k_flatten (thread per TAG) emits literal-line and job records plus per-warp counts, k_flatten_scan turns the counts
@@ -864,8 +864,7 @@ __device__ __forceinline__ int fl_ceil_i(float v) { return v != v ? (int)0x80000
 
 // A: thread per tag. Outputs: per-warp line count, per-tag offset inside its warp's block, literal records, jobs,
 // and the bbox contribution of the literal lines. (History: a single-pass look-back kernel was gated by the slowest
-// tag in flight, ncu r1: 18 % issue utilisation; a count+emit kernel computed long tags twice and its 200 KB of code
-// thrashed the instruction cache, ncu r1_f: no_instruction = top stall.)
+// tag in flight; a count+emit kernel computed long tags twice and its 200 KB of code thrashed the instruction cache.)
 __global__ void __launch_bounds__(FL_THREADS, FL_MINB)
 k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids,
           VbPathBbox *path_bboxes, FlCtx ctx, uint32_t *part_count, uint32_t *tag_off, uint32_t part_base, uint32_t part_end) {
@@ -940,7 +939,7 @@ k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *_
 
 // B: exclusive scan of part_count -> destination offsets; publishes bump.lines. One CTA per 8192 partitions (8 values per
 // thread, 128-bit accesses); the carry between CTAs is the single-pass look-back of vb_device.cuh (round 1 walked the whole
-// array with ONE CTA: 17 us on the critical path of every frame and of every rank of a multi-GPU frame).
+// array with ONE CTA, on the critical path of every frame and of every rank of a multi-GPU frame).
 #define FS_THREADS 1024
 #define FS_PER_THREAD 8
 static_assert(FS_PER_THREAD == 8, "k_flatten_scan is written for 8 values per thread");
@@ -1116,7 +1115,7 @@ k_flatten_place(VbConfig cfg, const uint32_t *__restrict__ scene, FlCtx ctx, con
 extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, const VbTagMonoid *tag_monoids,
                                   VbPathBbox *path_bboxes, VbBump *bump, VbLineSoup *lines, void *lit_arena, void *job_arena,
                                   uint32_t *part_mem /* 34 * n_parts + 8 words */, uint32_t *ctrs, uint32_t n_parts, int clear_bboxes,
-                                  uint32_t part_base, uint32_t part_end /* 0, n_parts: everything */, cudaStream_t st) {
+                                  uint32_t part_base, uint32_t part_end /* 0, n_parts: everything */, int sm_count, cudaStream_t st) {
     uint32_t n_paths = cfg->layout.n_paths;
     // whole frames reset the boxes in k_frame_init (vb_api.cu); a stage range that starts later does it here
     if (n_paths && clear_bboxes) k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
@@ -1139,7 +1138,7 @@ extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, co
                                                                                              part_count, tag_off, part_base, part_end);
         const uint32_t n_blocks = n_own ? (n_own + FS_THREADS * FS_PER_THREAD - 1u) / (FS_THREADS * FS_PER_THREAD) : 1u;
         k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(*cfg, n_own, part_count + part_base, part_dst + part_base, bump, ctrs + 4, n_blocks);
-        k_flatten_place<<<148 * 4, FP_THREADS, 0, st>>>(*cfg, scene, ctx, part_dst, tag_off, path_bboxes, lines);
+        k_flatten_place<<<(uint32_t)sm_count * 4u, FP_THREADS, 0, st>>>(*cfg, scene, ctx, part_dst, tag_off, path_bboxes, lines);
     }
 }
 extern "C" uint32_t vb_flatten_parts(uint32_t n_tag_words) { return (n_tag_words * 4u + 31u) / 32u; }

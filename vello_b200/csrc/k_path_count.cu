@@ -5,10 +5,10 @@
 // the WGSL where the CPU twin differs (`s1.y <= bbox.y`, `max(s0.x,s1.x) <= bbox.x`); WGSL
 // round() is ties-to-even -> rintf.
 //
-// B200 design: one thread per line as in the WGSL, but (i) no indirect dispatch -- the grid is
+// Design: one thread per line as in the WGSL, but (i) no indirect dispatch -- the grid is
 // sized from the arena capacity and reads bump.lines on the device, (ii) the seg_counts
-// allocation is aggregated per CTA: one atomicAdd per 256 lines instead of one per line (same-address atomics cost
-// ~2 ns each on this part: per-warp aggregation, 133 k atomics a frame, measured 0.26 ms against 0.14 ms),
+// allocation is aggregated per CTA: one atomicAdd per 256 lines instead of one per line (same-address atomics serialise;
+// per-warp aggregation still left ~133 k of them a frame and was slower),
 // (iii) backdrop / count updates are fire-and-forget RED operations except the slot fetch.
 // Per-tile slot order (seg_within_slice) is atomic-order dependent exactly as in the reference.
 #include "vb_device.cuh"

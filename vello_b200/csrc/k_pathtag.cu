@@ -5,7 +5,7 @@
 // Output: tag_monoids[w] = exclusive prefix of the 5-field monoid before tag word w (20 B each),
 // bit-identical to the reference's.
 //
-// B200 design: ONE pass. A CTA takes a ticket, scans 1024 tag words (256 threads x 4 words) with
+// Design: ONE pass. A CTA takes a ticket, scans 1024 tag words (256 threads x 4 words) with
 // warp shuffles, publishes its aggregate and resolves its prefix by decoupled look-back.
 // Algorithmic traffic: 4 B read + 20 B written per tag word (HBM-bound, no tensor cores).
 #include "vb_device.cuh"

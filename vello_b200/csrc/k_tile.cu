@@ -3,7 +3,7 @@
 // Reference: vello_shaders/shader/tile_alloc.wgsl:36-123 (CPU twin cpu/tile_alloc.rs),
 // backdrop_dyn.wgsl:29-86 (CPU twin cpu/backdrop.rs).
 //
-// B200 design: tile_alloc's per-workgroup atomicAdd(bump.tile) becomes a decoupled look-back scan,
+// Design: tile_alloc's per-workgroup atomicAdd(bump.tile) becomes a decoupled look-back scan,
 // so `Path.tiles` offsets are deterministic and equal to the serial CPU shader's -- `tiles[]` can be
 // compared byte for byte. The allocated range is zeroed by a grid-wide pass (k_tile_zero). backdrop streams the
 // arena as contiguous per-CTA ranges (see k_backdrop).
@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(256) k_tile_zero(VbConfig cfg, const VbBump *_
 }
 
 // backdrop: per (path, tile row) inclusive prefix sum along x (backdrop_dyn.wgsl:66-84).
-// B200 design: the WGSL assigns one thread per row, walking 8-byte tiles at a stride of the row width (uncoalesced).
+// Design: the WGSL assigns one thread per row, walking 8-byte tiles at a stride of the row width (uncoalesced).
 // tile_alloc hands out tiles in draw order, so the tiles of 32 consecutive paths are ONE contiguous range of the arena,
 // made of rows laid end to end. A CTA owns that range; it is cut into 8 x gridDim.y pieces of equal size, each piece
 // moved to whole-row boundaries, and one warp streams its piece 128 consecutive tiles at a time (four independent
@@ -164,17 +164,17 @@ k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile 
 }
 
 extern "C" void vb_launch_tile_alloc(const VbConfig *cfg, const uint32_t *scene, const VbBbox4 *draw_bboxes, VbBump *bump,
-                                     VbPath *paths, VbTile *tiles, uint32_t *lb_mem, uint32_t n_parts, cudaStream_t st) {
+                                     VbPath *paths, VbTile *tiles, uint32_t *lb_mem, uint32_t n_parts, int sm_count, cudaStream_t st) {
     if (n_parts == 0) return;
     k_tile_alloc<<<n_parts, TA_THREADS, 0, st>>>(*cfg, scene, draw_bboxes, bump, paths, tiles, lb_mem, n_parts);
-    k_tile_zero<<<148 * 4, 256, 0, st>>>(*cfg, bump, tiles);
+    k_tile_zero<<<(uint32_t)sm_count * 4u, 256, 0, st>>>(*cfg, bump, tiles);
 }
 extern "C" uint32_t vb_tile_alloc_parts(uint32_t n_draw) { return (n_draw + TA_THREADS - 1) / TA_THREADS; }
-extern "C" void vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, cudaStream_t st) {
+extern "C" void vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, int sm_count, cudaStream_t st) {
     uint32_t n = cfg->layout.n_draw_objects;
     if (n == 0) return;
     const uint32_t groups = (n + BD_PATHS - 1) / BD_PATHS;
-    uint32_t split = (148u * 4u + groups - 1u) / groups;
+    uint32_t split = ((uint32_t)sm_count * 4u + groups - 1u) / groups;
     if (split > 64u) split = 64u;
     k_backdrop<<<dim3(groups, split), BD_THREADS, 0, st>>>(*cfg, bump, paths, tiles);
 }

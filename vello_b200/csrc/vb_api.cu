@@ -24,7 +24,7 @@ extern "C" {
 void vb_launch_pathtag(const VbConfig *, const uint32_t *, VbTagMonoid *, uint32_t *, uint32_t, cudaStream_t);
 uint32_t vb_pathtag_parts(uint32_t);
 void vb_launch_flatten(const VbConfig *, const uint32_t *, const VbTagMonoid *, VbPathBbox *, VbBump *, VbLineSoup *, void *, void *, uint32_t *,
-                       uint32_t *, uint32_t, int, uint32_t, uint32_t, cudaStream_t);
+                       uint32_t *, uint32_t, int, uint32_t, uint32_t, int, cudaStream_t);
 uint32_t vb_flatten_parts(uint32_t);
 void vb_flatten_arena_bytes(uint32_t, size_t *, size_t *);
 void vb_launch_draw(const VbConfig *, const uint32_t *, const VbPathBbox *, VbDrawMonoid *, uint32_t *, VbClipInp *, uint32_t *, uint32_t,
@@ -35,10 +35,10 @@ uint32_t vb_clip_parts(uint32_t);
 size_t vb_clip_scratch_words(uint32_t);
 void vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathBbox *, const VbBbox4 *, VbBbox4 *, VbBump *, uint32_t *,
                        VbBinHeader *, cudaStream_t);
-void vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t,
+void vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
                           cudaStream_t);
 uint32_t vb_tile_alloc_parts(uint32_t);
-void vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, cudaStream_t);
+void vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, int, cudaStream_t);
 void vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
                           cudaStream_t);
 void vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
@@ -150,7 +150,7 @@ struct vb_renderer {
     bool timing = false;
     uint32_t max_retries = 6;
     std::string err;
-    int sm_count = 148;
+    int sm_count = 132;
 
     // scene
     bool have_scene = false;
@@ -601,7 +601,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
     const uint32_t n_draw = c.layout.n_draw_objects;
     if (first == 0) {
         // a kernel, not cudaMemsetAsync: small memsets / copies are served by a copy engine and would queue behind a
-        // 64 MiB read-back still draining from the previous frame (measured: +1.2 ms per streamed frame)
+        // 64 MiB read-back still draining from the previous frame
         const unsigned ctl_blocks = (unsigned)((r->ctl_words + 1023) / 1024), bb_blocks = (c.layout.n_paths + 255u) / 256u;
         uint32_t *xepoch = r->xc.enabled ? (uint32_t *)r->xc.arena.p + vb_exchange_epoch_word() : nullptr;
         k_frame_init<<<ctl_blocks + bb_blocks, 256, 0, st>>>(ctl, (uint32_t)r->ctl_words, ctl_blocks, (VbPathBbox *)r->path_bboxes.p, c.layout.n_paths,
@@ -633,7 +633,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
                 const uint32_t p1 = k + 1u == G ? P : ((uint32_t)((uint64_t)P * (k + 1u) / G) & ~7u);
                 vb_launch_flatten(&cx, (const uint32_t *)r->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p, bump,
                                   (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
-                                  ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, p0, p1, st);
+                                  ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, p0, p1, r->sm_count, st);
                 XPeersHost X;
                 xpeers_of(r, &X);
                 vb_launch_exchange_send(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, ctl + VB_CTL_XCHG_SCRATCH,
@@ -643,7 +643,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
             }
             vb_launch_flatten(&c, (const uint32_t *)r->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p, bump,
                               (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
-                              ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, 0u, r->parts_flatten, st);
+                              ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, 0u, r->parts_flatten, r->sm_count, st);
             launches += (first != 0 && c.layout.n_paths ? 1 : 0) + (r->parts_flatten ? 3 : 0);
             break;
         case VB_STAGE_ID_DRAW:
@@ -671,7 +671,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
             break;
         case VB_STAGE_ID_TILE_ALLOC:
             vb_launch_tile_alloc(&c, (const uint32_t *)r->scene.p, (const VbBbox4 *)r->draw_bboxes.p, bump, (VbPath *)r->paths.p,
-                                 (VbTile *)r->tiles.p, ctl + r->off_lb_tile, r->parts_tile, st);
+                                 (VbTile *)r->tiles.p, ctl + r->off_lb_tile, r->parts_tile, r->sm_count, st);
             launches += r->parts_tile ? 2 : 0;
             break;
         case VB_STAGE_ID_PATH_COUNT: {
@@ -684,7 +684,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
             break;
         }
         case VB_STAGE_ID_BACKDROP:
-            vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, st);
+            vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, r->sm_count, st);
             launches += n_draw ? 1 : 0;
             break;
         case VB_STAGE_ID_COARSE:
@@ -746,8 +746,8 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
 
 // ---- whole-frame CUDA graphs ---------------------------------------------------------------------------------------------
 // A frame is ~20 kernel launches. Each launch makes the GPU fetch a command buffer from host memory over PCIe; while a
-// 64 MiB read-back of the previous frame is streaming the other way that fetch queues behind it (measured with
-// tools/e2e_probe.py: every stage of a streamed frame started ~10 us late per launch, +0.3 ms per frame). In steady state
+// 64 MiB read-back of the previous frame is streaming the other way that fetch queues behind it (tools/e2e_probe.py
+// shows every stage of a streamed frame starting late). In steady state
 // the launches of a frame are identical -- same kernels, grids, arena pointers, config -- so they are captured once into a
 // graph and replayed with ONE submission. The key is everything a launch argument is derived from; growing an arena or
 // changing the scene layout / frame size / window simply misses the cache and re-captures.

@@ -66,7 +66,7 @@ def load_library() -> C.CDLL:
     path = os.environ.get("VELLO_B200_LIB", LIB_PATH)  # development knob: A/B a differently tuned build
     if not os.path.exists(path):
         raise VelloB200Error(f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                             "(nvcc, sm_100a). vello_b200 has no CPU fallback.")
+                             "(nvcc, sm_90a). vello_b200 has no CPU fallback.")
     lib = C.CDLL(path)
     vp = C.c_void_p
     lib.vb_renderer_new.argtypes = [C.POINTER(_Options), C.POINTER(vp)]

@@ -1,6 +1,6 @@
 """Geometry helpers standing in for the parts of `kurbo 0.13.1` the scene builder touches.
 
-kurbo is a third-party dependency that is *not* under /root/reference (Cargo.lock pins
+kurbo is a third-party dependency that is *not* in the reference repository (Cargo.lock pins
 kurbo 0.13.1); what is restated here is its published algorithm for turning shapes into path
 elements (`Shape::path_elements(tolerance)`), which `PathEncoder::shape` calls with
 tolerance 0.1 (vello_encoding/src/path.rs:655-657):
@@ -461,7 +461,7 @@ def parse_svg_path(d: str) -> List[tuple]:
 
 # ---------------------------------------------------------------------------------------------
 # kurbo::dash (kurbo 0.13.1 stroke.rs `DashIterator`), which vello applies on the CPU before encoding a dashed stroke
-# (vello/src/scene.rs:404-438). kurbo is a Cargo dependency that is not under /root/reference: the state machine below
+# (vello/src/scene.rs:404-438). kurbo is a Cargo dependency that is not in the reference repository: the state machine below
 # restates its published algorithm (stash the first dash of a closed subpath so that it can be joined to the last one,
 # walk arc length with `dash_remaining` / `seg_remaining`, split segments with subsegment / inv_arclen). Lines -- the
 # reference's `longpathdash` scene -- use closed forms and are exact; for curves kurbo's arclen / inv_arclen (adaptive
