@@ -7,8 +7,9 @@
 // Design (differs from the WGSL on purpose; the pieces are described where they are defined below):
 //  * The WGSL bump-allocates every line with a global atomicAdd, so the line order is a race. Here line order is
 //    deterministic -- tag order, then emission order, i.e. the serial CPU shader's -- and independent of any atomic:
-//    k_flatten (thread per TAG) emits literal-line and job records plus per-warp counts, k_flatten_scan turns the counts
-//    into offsets, k_flatten_place (thread per LINE) writes every line at its final position.
+//    the tag pass (thread per TAG: k_flatten_lean, then k_flatten for the partitions that need the general path) emits
+//    literal-line and job records plus per-warp counts, k_flatten_scan turns the counts into offsets, k_flatten_place
+//    (thread per LINE) writes every line at its final position.
 //  * Fast paths for line-tos (filled: one line; stroked: one line per side) behind guards that are derived in place,
 //    property-tested on the CPU against the oracle and compared bit for bit on the GPU.
 //  * With a stripe window set (multi-GPU), tags that cannot reach the window's rows are skipped.
@@ -99,7 +100,9 @@ __device__ __noinline__ void fl_spill_line(const FlCtx c, uint32_t tag_ix, uint3
     }
 }
 
-struct Flat {
+// SPILL = false (k_flatten_lean): a tag never has more than FL_CACHE literal lines, so there is no overflow path.
+template <bool SPILL>
+struct FlatT {
     FlCtx c;
     uint32_t tag_ix, path_ix, trans_ix;
     uint32_t ix;   // lines of this tag so far
@@ -113,7 +116,7 @@ struct Flat {
         by0 = fminf(by0, fminf(p0.y, p1.y));
         bx1 = fmaxf(bx1, fmaxf(p0.x, p1.x));
         by1 = fmaxf(by1, fmaxf(p0.y, p1.y));
-        if (nlit < FL_CACHE) {
+        if (!SPILL || nlit < FL_CACHE) {
             cache[nlit * FL_THREADS] = make_float4(p0.x, p0.y, p1.x, p1.y);
             cache_rel[nlit * FL_THREADS] = ix;
         } else {
@@ -139,6 +142,7 @@ struct Flat {
         force = true;
     }
 };
+using Flat = FlatT<true>;
 
 #define DERIV_THRESH 1e-6f
 #define DERIV_THRESH_SQUARED (DERIV_THRESH * DERIV_THRESH)
@@ -497,17 +501,34 @@ __device__ fv2 fl_arc_point(const FlJob &j, uint32_t i, const FXform &t) {
     return fx_apply(t, center + r);
 }
 
-__device__ void flatten_arc(Flat &f, fv2 begin, fv2 end, fv2 center, float angle, const FXform &t) {
-    fv2 p0 = fx_apply(t, begin);
-    fv2 r = begin - center;
+// How an arc is flattened: its first point (device space), the rotation step, its line count and whether it is deferred.
+struct ArcSteps {
+    fv2 p0;
+    float s, c;
+    uint32_t n_lines;
+    bool job;
+};
+__device__ __forceinline__ ArcSteps arc_steps(fv2 begin, fv2 end, fv2 center, float angle, const FXform &t) {
+    ArcSteps a;
+    a.p0 = fx_apply(t, begin);
     const float MIN_THETA = 0.0001f;
     const float tol = 0.25f;
-    float radius = fmaxf(tol, flen(p0 - fx_apply(t, center)));
+    float radius = fmaxf(tol, flen(a.p0 - fx_apply(t, center)));
     float theta = fmaxf(MIN_THETA, 2.f * vb_acosf(1.f - tol / radius));
-    uint32_t n_lines = max(1u, vb_f2u_sat(ceilf(angle / theta)));
-    float s, c;
-    vb_sincosf(theta, &s, &c);
-    if (n_lines >= FL_DEFER_MIN && n_lines <= FL_ARC_MAX && !feq(p0, fx_apply(t, end))) {
+    a.n_lines = max(1u, vb_f2u_sat(ceilf(angle / theta)));
+    vb_sincosf(theta, &a.s, &a.c);
+    a.job = a.n_lines >= FL_DEFER_MIN && a.n_lines <= FL_ARC_MAX && !feq(a.p0, fx_apply(t, end));
+    return a;
+}
+
+template <class F>
+__device__ void flatten_arc(F &f, fv2 begin, fv2 end, fv2 center, float angle, const FXform &t) {
+    const ArcSteps a = arc_steps(begin, end, center, angle, t);
+    fv2 p0 = a.p0;
+    fv2 r = begin - center;
+    const uint32_t n_lines = a.n_lines;
+    const float s = a.s, c = a.c;
+    if (a.job) {
         FlJob j;
         j.p0x = begin.x; j.p0y = begin.y; j.p1x = end.x; j.p1y = end.y;
         j.th0 = center.x; j.k0 = center.y; j.k1 = c; j.ch = s;
@@ -710,13 +731,26 @@ __device__ CubicPoints read_path_segment(const VbConfig &cfg, const uint32_t *__
     return r;
 }
 
-// Everything one tag byte produces.
-__device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__restrict__ scene,
-                            const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix, uint32_t style_flags) {
-    uint32_t seg_type = tag.tag_byte & 3u;
-    if (seg_type == 0u) return;
-    bool is_stroke = (style_flags & STYLE_FLAGS_STYLE) != 0u;
+// What one tag byte produces, decided before anything is emitted: 0, 1 or 2 offset curves for the Euler machinery (none
+// when a line-to fast path applies), then the tail of a cap or join. Both tag kernels plan with this one function.
+struct TagPlan {
     FXform transform;
+    CubicPoints pts;
+    bool is_stroke, fast_stroke; // fast_stroke: one line per side, (p0 + n_start, p3 + n_prev) and (p3 - n_prev, p0 - n_start)
+    int n_sides;
+    float offset;
+    fv2 n_start, n_prev;
+    TailOps tail;
+};
+
+// false: the tag emits nothing.
+__device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, const uint32_t *__restrict__ scene,
+                                         const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix,
+                                         uint32_t style_flags) {
+    uint32_t seg_type = tag.tag_byte & 3u;
+    if (seg_type == 0u) return false;
+    bool is_stroke = (style_flags & STYLE_FLAGS_STYLE) != 0u;
+    FXform &transform = plan.transform;
     {
         uint32_t b = cfg.layout.transform_base + tag.trans_ix * 6u;
         transform.m0 = __uint_as_float(vb_scene(scene, cfg, b));
@@ -726,7 +760,8 @@ __device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__rest
         transform.tx = __uint_as_float(vb_scene(scene, cfg, b + 4));
         transform.ty = __uint_as_float(vb_scene(scene, cfg, b + 5));
     }
-    CubicPoints pts = read_path_segment(cfg, scene, tag, is_stroke);
+    CubicPoints &pts = plan.pts;
+    pts = read_path_segment(cfg, scene, tag, is_stroke);
     if (cfg.win_cull != 0u) {
         // Stripe rendering (one bin-row window per GPU): everything this tag emits lies within R of the convex hull of
         // its control points (R = half width x max(miter limit, sqrt 2) for strokes), so a tag whose hull, grown by R
@@ -744,14 +779,19 @@ __device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__rest
             grow += 0.5f * fabsf(lw) * lim * (fabsf(transform.m0) + fabsf(transform.m1) + fabsf(transform.m2) + fabsf(transform.m3));
         }
         const float lo = fminf(fminf(y_0, y_1), fminf(y_2, y_3)) - grow, hi = fmaxf(fmaxf(y_0, y_1), fmaxf(y_2, y_3)) + grow;
-        if (hi < (float)(cfg.win_ty0 * VB_TILE_HEIGHT) || lo > (float)(cfg.win_ty1 * VB_TILE_HEIGHT)) return; // NaN: kept
+        if (hi < (float)(cfg.win_ty0 * VB_TILE_HEIGHT) || lo > (float)(cfg.win_ty1 * VB_TILE_HEIGHT)) return false; // NaN: kept
     }
     // the offset curves to flatten (0, 1 or 2 of them) and what follows them
-    int n_sides = 0;
-    bool fast_stroke = false;
-    float offset = 0.f;
-    fv2 n_start = F2(0.f, 0.f), n_prev = F2(0.f, 0.f);
-    TailOps tail;
+    plan.is_stroke = is_stroke;
+    int &n_sides = plan.n_sides;
+    bool &fast_stroke = plan.fast_stroke;
+    float &offset = plan.offset;
+    fv2 &n_start = plan.n_start, &n_prev = plan.n_prev;
+    TailOps &tail = plan.tail;
+    n_sides = 0;
+    fast_stroke = false;
+    offset = 0.f;
+    n_start = n_prev = F2(0.f, 0.f);
     tail.have_arc = false; tail.n_lines = 0u; tail.arc_angle = 0.f;
     tail.arc_begin = tail.arc_end = tail.arc_center = F2(0.f, 0.f);
     tail.a0 = tail.b0 = tail.a1 = tail.b1 = tail.a2 = tail.b2 = F2(0.f, 0.f);
@@ -830,22 +870,41 @@ __device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__rest
             }
         }
     }
-    if (fast_stroke) {
-        f.line_xf(pts.p0 + n_start, pts.p3 + n_prev, transform);
-        f.line_xf(pts.p3 - n_prev, pts.p0 - n_start, transform);
-        n_sides = 0;
-    }
-#pragma unroll 1
-    for (int side = 0; side < n_sides; side++) { // one copy of the Euler machinery in the instruction stream
-        const bool fwd = side == 0;
-        flatten_euler(f, pts, transform, fwd ? offset : -offset, fwd ? pts.p0 + n_start : pts.p0 - n_start,
-                      fwd ? pts.p3 + n_prev : pts.p3 - n_prev);
-    }
-    if (tail.have_arc) flatten_arc(f, tail.arc_begin, tail.arc_end, tail.arc_center, tail.arc_angle, transform);
+    if (fast_stroke) n_sides = 0;
+    return true;
+}
+
+// A tag's output in order: the lines of the stroke fast path, the offset curves (flatten_tag only), the tail.
+template <class F>
+__device__ __forceinline__ void emit_fast_stroke(F &f, const TagPlan &p) {
+    if (!p.fast_stroke) return;
+    f.line_xf(p.pts.p0 + p.n_start, p.pts.p3 + p.n_prev, p.transform);
+    f.line_xf(p.pts.p3 - p.n_prev, p.pts.p0 - p.n_start, p.transform);
+}
+template <class F>
+__device__ __forceinline__ void emit_tail(F &f, const TagPlan &p) {
+    const TailOps &tail = p.tail;
+    if (tail.have_arc) flatten_arc(f, tail.arc_begin, tail.arc_end, tail.arc_center, tail.arc_angle, p.transform);
     // the fast-path line of a fill is in device space already; cap / join lines are in local space
-    if (tail.n_lines > 0u) f.write_line(is_stroke ? fx_apply(transform, tail.a0) : tail.a0, is_stroke ? fx_apply(transform, tail.b0) : tail.b0);
-    if (tail.n_lines > 1u) f.line_xf(tail.a1, tail.b1, transform);
-    if (tail.n_lines > 2u) f.line_xf(tail.a2, tail.b2, transform);
+    if (tail.n_lines > 0u)
+        f.write_line(p.is_stroke ? fx_apply(p.transform, tail.a0) : tail.a0, p.is_stroke ? fx_apply(p.transform, tail.b0) : tail.b0);
+    if (tail.n_lines > 1u) f.line_xf(tail.a1, tail.b1, p.transform);
+    if (tail.n_lines > 2u) f.line_xf(tail.a2, tail.b2, p.transform);
+}
+
+// Everything one tag byte produces.
+__device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__restrict__ scene,
+                            const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix, uint32_t style_flags) {
+    TagPlan p;
+    if (!plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags)) return;
+    emit_fast_stroke(f, p);
+#pragma unroll 1
+    for (int side = 0; side < p.n_sides; side++) { // one copy of the Euler machinery in the instruction stream
+        const bool fwd = side == 0;
+        flatten_euler(f, p.pts, p.transform, fwd ? p.offset : -p.offset, fwd ? p.pts.p0 + p.n_start : p.pts.p0 - p.n_start,
+                      fwd ? p.pts.p3 + p.n_prev : p.pts.p3 - p.n_prev);
+    }
+    emit_tail(f, p);
 }
 
 // bbox_clear.wgsl: path bboxes start at (+INT_MAX, -INT_MAX)
@@ -862,23 +921,14 @@ __global__ void k_bbox_clear(uint32_t n_paths, VbPathBbox *path_bboxes) {
 __device__ __forceinline__ int fl_floor_i(float v) { return v != v ? 0x7fffffff : vb_f2i_sat(floorf(v)); }
 __device__ __forceinline__ int fl_ceil_i(float v) { return v != v ? (int)0x80000000 : vb_f2i_sat(ceilf(v)); }
 
-// A: thread per tag. Outputs: per-warp line count, per-tag offset inside its warp's block, literal records, jobs,
-// and the bbox contribution of the literal lines. (History: a single-pass look-back kernel was gated by the slowest
-// tag in flight; a count+emit kernel computed long tags twice and its 200 KB of code thrashed the instruction cache.)
-__global__ void __launch_bounds__(FL_THREADS, FL_MINB)
-k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids,
-          VbPathBbox *path_bboxes, FlCtx ctx, uint32_t *part_count, uint32_t *tag_off, uint32_t part_base, uint32_t part_end) {
-    // [part_base, part_end): the partitions (32 tags each) this launch covers -- all of them, or this GPU's share of a
-    // frame whose flatten is sharded by tag range (k_exchange.cu); every array is indexed by the GLOBAL partition / tag
-    const uint32_t lane = vb_lane();
-    const uint32_t part = part_base + blockIdx.x * (FL_THREADS / 32) + (threadIdx.x >> 5);
-    if (part >= part_end) return;
-    const uint32_t ix = part * 32u + lane;
+// Per-partition prologue of both tag kernels: this lane's tag and style word, the draw flags / transform of the path it
+// opens; then an empty Flat over the block's shared-memory line cache.
+__device__ __forceinline__ void fl_load_tag(PathTagData &tag, uint32_t &style_flags, const VbConfig &cfg, const uint32_t *__restrict__ scene,
+                                            const VbTagMonoid *__restrict__ tag_monoids, VbPathBbox *path_bboxes, uint32_t ix) {
     const uint32_t n_tags = cfg.n_tag_words * 4u;
     const uint32_t n_paths = cfg.layout.n_paths;
-    PathTagData tag;
     tag.tag_byte = 0; tag.trans_ix = 0; tag.pathseg_offset = 0; tag.style_ix = 0; tag.path_ix = 0;
-    uint32_t style_flags = 0;
+    style_flags = 0;
     if (ix < n_tags) {
         tag = compute_tag_monoid(cfg, scene, tag_monoids, ix);
         style_flags = vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix);
@@ -887,16 +937,24 @@ k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *_
             path_bboxes[tag.path_ix].trans_ix = tag.trans_ix;
         }
     }
-    __shared__ float4 sh_cache[FL_CACHE][FL_THREADS];
-    __shared__ uint32_t sh_rel[FL_CACHE][FL_THREADS];
-    Flat f;
+}
+template <class F>
+__device__ __forceinline__ void fl_flat_init(F &f, const FlCtx &ctx, const PathTagData &tag, uint32_t ix, float4 *cache, uint32_t *cache_rel) {
     f.c = ctx;
     f.tag_ix = ix; f.path_ix = tag.path_ix; f.trans_ix = tag.trans_ix;
     f.ix = 0u; f.nlit = 0u; f.force = false;
     f.bx0 = 1e31f; f.by0 = 1e31f; f.bx1 = -1e31f; f.by1 = -1e31f;
-    f.cache = &sh_cache[0][threadIdx.x];
-    f.cache_rel = &sh_rel[0][threadIdx.x];
-    flatten_tag(f, cfg, scene, tag_monoids, tag, ix, style_flags);
+    f.cache = cache;
+    f.cache_rel = cache_rel;
+}
+
+// Per-partition epilogue of both tag kernels: per-warp line count, per-tag offset inside its warp's block, the cached
+// literal records, and the bbox contribution of the literal lines.
+template <class F>
+__device__ __forceinline__ void fl_tag_end(F &f, const VbConfig &cfg, VbPathBbox *path_bboxes, const FlCtx &ctx, uint32_t *part_count,
+                                           uint32_t *tag_off) {
+    const uint32_t ix = f.tag_ix, path_ix = f.path_ix, part = ix >> 5, lane = ix & 31u;
+    const uint32_t n_paths = cfg.layout.n_paths;
     __syncwarp();
     const uint32_t incl = vb_warp_incl_scan(f.ix);
     if (lane == 31u) part_count[part] = incl;
@@ -906,35 +964,119 @@ k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *_
     const uint32_t ltotal = __shfl_sync(VB_FULL, lincl, 31);
     uint32_t lbase = 0u;
     if (lane == 31u && ltotal != 0u) lbase = atomicAdd(ctx.ctrs, ltotal);
-    lbase = __shfl_sync(VB_FULL, lbase, 31) + lincl - ncache;
-    for (uint32_t k = 0; k < ncache; k++) {
-        const uint32_t slot = lbase + k;
-        if (slot < ctx.lits_cap) {
-            const float4 l = sh_cache[k][threadIdx.x];
+    lbase = __shfl_sync(VB_FULL, lbase, 31);
+    // The warp's literal records are one range [lbase, lbase + ltotal), lane i's ncache records after lane i-1's. They are
+    // written lane-strided, record j of the range by lane j % 32 from its owner's cache, so that a warp's stores cover
+    // consecutive 32 B records (each lane writing its own records made every store a scatter of partial sectors).
+    const uint32_t lexcl = lincl - ncache;
+    const float4 *wcache = f.cache - lane;
+    const uint32_t *wrel = f.cache_rel - lane;
+    for (uint32_t b = 0u; b < ltotal; b += 32u) {
+        const uint32_t j = b + lane;
+        uint32_t o = 0u; // owner: the number of lanes whose records all lie before j
+#pragma unroll
+        for (uint32_t step = 16u; step > 0u; step >>= 1)
+            if (__shfl_sync(VB_FULL, lincl, o + step - 1u) <= j) o += step;
+        const uint32_t k = j - __shfl_sync(VB_FULL, lexcl, o);
+        const uint32_t o_path = __shfl_sync(VB_FULL, path_ix, o);
+        const uint32_t slot = lbase + j;
+        if (j < ltotal && slot < ctx.lits_cap) {
+            const float4 l = wcache[k * FL_THREADS + o];
             uint4 *dst = reinterpret_cast<uint4 *>(ctx.lits + slot);
-            dst[0] = make_uint4(ix, sh_rel[k][threadIdx.x], tag.path_ix, 0u);
+            dst[0] = make_uint4(ix - lane + o, wrel[k * FL_THREADS + o], o_path, 0u);
             dst[1] = make_uint4(__float_as_uint(l.x), __float_as_uint(l.y), __float_as_uint(l.z), __float_as_uint(l.w));
         }
     }
     // bbox: consecutive tags mostly belong to the same path, so reduce across the lanes of a path first (floor / ceil
     // commute with min / max) and issue one set of atomics per (warp, path) instead of one per tag
-    const bool pub = f.nlit != 0u && (f.force || f.bx1 > f.bx0 || f.by1 > f.by0) && tag.path_ix < n_paths;
+    const bool pub = f.nlit != 0u && (f.force || f.bx1 > f.bx0 || f.by1 > f.by0) && path_ix < n_paths;
     const uint32_t pubmask = __ballot_sync(VB_FULL, pub);
     if (pub) {
         int x0 = fl_floor_i(f.bx0), y0 = fl_floor_i(f.by0), x1 = fl_ceil_i(f.bx1), y1 = fl_ceil_i(f.by1);
-        const uint32_t peers = __match_any_sync(pubmask, tag.path_ix);
+        const uint32_t peers = __match_any_sync(pubmask, path_ix);
         x0 = __reduce_min_sync(peers, x0);
         y0 = __reduce_min_sync(peers, y0);
         x1 = __reduce_max_sync(peers, x1);
         y1 = __reduce_max_sync(peers, y1);
         if (lane == (uint32_t)(__ffs((int)peers) - 1)) {
-            VbPathBbox *o = path_bboxes + tag.path_ix;
+            VbPathBbox *o = path_bboxes + path_ix;
             atomicMin(&o->x0, x0);
             atomicMin(&o->y0, y0);
             atomicMax(&o->x1, x1);
             atomicMax(&o->y1, y1);
         }
     }
+}
+
+// A: the tag pass, thread per tag, warp per partition of 32 tags. It is split by what the tags need, because the general
+// path (Euler subdivision) needs 128 registers and most partitions of a map-like scene need none of it:
+//  * k_flatten_lean runs every partition [part_base, part_end) -- all of them, or this GPU's share of a frame whose
+//    flatten is sharded by tag range (k_exchange.cu); every array is indexed by the GLOBAL partition / tag. A partition
+//    whose tags all take a line-to fast path or need no lines, and whose caps and joins are straight or round arcs that
+//    are deferred or have at most 2 lines, is finished here (at most 5 literal lines per tag -- 2 + 3 straight, or
+//    2 + 2 + 1 with an arc -- so all of them stay in the shared-memory cache).
+//    Any other partition (a curve, a failed fast-path guard, an arc emitted in place) is left untouched and appended to
+//    a work list.
+//  * k_flatten runs the partitions of the work list with the general code.
+// Both plan a tag with plan_tag and emit its lines through the same functions, so a partition's outputs are the same
+// bits whichever kernel ran it.
+#ifndef FL_LEAN_MINB
+#define FL_LEAN_MINB 4
+#endif
+
+__global__ void __launch_bounds__(FL_THREADS, FL_LEAN_MINB)
+k_flatten_lean(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids, VbPathBbox *path_bboxes,
+               FlCtx ctx, uint32_t *part_count, uint32_t *tag_off, uint32_t *work, uint32_t part_base, uint32_t part_end) {
+    const uint32_t lane = vb_lane();
+    const uint32_t part = part_base + blockIdx.x * (FL_THREADS / 32) + (threadIdx.x >> 5);
+    if (part >= part_end) return;
+    const uint32_t ix = part * 32u + lane;
+    __shared__ float4 sh_cache[FL_CACHE][FL_THREADS];
+    __shared__ uint32_t sh_rel[FL_CACHE][FL_THREADS];
+    PathTagData tag;
+    uint32_t style_flags;
+    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, path_bboxes, ix);
+    TagPlan p;
+    const bool emits = plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags);
+    bool general = emits && p.n_sides != 0;
+    if (emits && !general && p.tail.have_arc) {
+        const ArcSteps a = arc_steps(p.tail.arc_begin, p.tail.arc_end, p.tail.arc_center, p.tail.arc_angle, p.transform);
+        general = !a.job && a.n_lines > 2u;
+    }
+    if (__any_sync(VB_FULL, general)) {
+        if (lane == 0u) work[atomicAdd(ctx.ctrs + 2, 1u)] = part;
+        return;
+    }
+    FlatT<false> f;
+    fl_flat_init(f, ctx, tag, ix, &sh_cache[0][threadIdx.x], &sh_rel[0][threadIdx.x]);
+    if (emits) {
+        emit_fast_stroke(f, p);
+        emit_tail(f, p);
+    }
+    fl_tag_end(f, cfg, path_bboxes, ctx, part_count, tag_off);
+}
+
+// Outputs as k_flatten_lean's, plus the job records. The grid covers every partition the lean kernel could have left;
+// the number it did leave is read on the device (frames are replayed as CUDA graphs). (History: a single-pass look-back
+// kernel was gated by the slowest tag in flight; a count+emit kernel computed long tags twice and its 200 KB of code
+// thrashed the instruction cache.)
+__global__ void __launch_bounds__(FL_THREADS, FL_MINB)
+k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids,
+          VbPathBbox *path_bboxes, FlCtx ctx, uint32_t *part_count, uint32_t *tag_off, const uint32_t *__restrict__ work) {
+    const uint32_t lane = vb_lane();
+    const uint32_t slot = blockIdx.x * (FL_THREADS / 32) + (threadIdx.x >> 5);
+    if (slot >= ctx.ctrs[2]) return;
+    const uint32_t part = work[slot];
+    const uint32_t ix = part * 32u + lane;
+    __shared__ float4 sh_cache[FL_CACHE][FL_THREADS];
+    __shared__ uint32_t sh_rel[FL_CACHE][FL_THREADS];
+    PathTagData tag;
+    uint32_t style_flags;
+    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, path_bboxes, ix);
+    Flat f;
+    fl_flat_init(f, ctx, tag, ix, &sh_cache[0][threadIdx.x], &sh_rel[0][threadIdx.x]);
+    flatten_tag(f, cfg, scene, tag_monoids, tag, ix, style_flags);
+    fl_tag_end(f, cfg, path_bboxes, ctx, part_count, tag_off);
 }
 
 // B: exclusive scan of part_count -> destination offsets; publishes bump.lines. One CTA per 8192 partitions (8 values per
@@ -1114,14 +1256,14 @@ k_flatten_place(VbConfig cfg, const uint32_t *__restrict__ scene, FlCtx ctx, con
 
 extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, const VbTagMonoid *tag_monoids,
                                   VbPathBbox *path_bboxes, VbBump *bump, VbLineSoup *lines, void *lit_arena, void *job_arena,
-                                  uint32_t *part_mem /* 34 * n_parts + 8 words */, uint32_t *ctrs, uint32_t n_parts, int clear_bboxes,
+                                  uint32_t *part_mem /* vb_flatten_part_words */, uint32_t *ctrs, uint32_t n_parts, int clear_bboxes,
                                   uint32_t part_base, uint32_t part_end /* 0, n_parts: everything */, int sm_count, cudaStream_t st) {
     uint32_t n_paths = cfg->layout.n_paths;
     // whole frames reset the boxes in k_frame_init (vb_api.cu); a stage range that starts later does it here
     if (n_paths && clear_bboxes) k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
     if (n_parts) {
         const size_t np4 = ((size_t)n_parts + 3u) & ~(size_t)3u; // 16-byte aligned sub-arrays (k_flatten_scan uses 128-bit accesses)
-        uint32_t *part_count = part_mem, *part_dst = part_mem + np4, *tag_off = part_mem + 2 * np4;
+        uint32_t *part_count = part_mem, *part_dst = part_mem + np4, *tag_off = part_mem + 2 * np4, *work = part_mem + 34 * np4;
         FlCtx ctx;
         ctx.lits = (FlLit *)lit_arena;
         ctx.jobs = (FlJob *)job_arena;
@@ -1134,14 +1276,20 @@ extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, co
             part_base = part_end = 0u;
         }
         const uint32_t n_own = part_end - part_base; // part_base is a multiple of 8: the scan's 128-bit accesses stay aligned
-        if (n_own) k_flatten<<<(n_own + warps_per_cta - 1) / warps_per_cta, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx,
-                                                                                             part_count, tag_off, part_base, part_end);
+        if (n_own) {
+            const uint32_t grid = (n_own + warps_per_cta - 1) / warps_per_cta;
+            k_flatten_lean<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work, part_base,
+                                                        part_end);
+            k_flatten<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work);
+        }
         const uint32_t n_blocks = n_own ? (n_own + FS_THREADS * FS_PER_THREAD - 1u) / (FS_THREADS * FS_PER_THREAD) : 1u;
         k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(*cfg, n_own, part_count + part_base, part_dst + part_base, bump, ctrs + 4, n_blocks);
         k_flatten_place<<<(uint32_t)sm_count * 4u, FP_THREADS, 0, st>>>(*cfg, scene, ctx, part_dst, tag_off, path_bboxes, lines);
     }
 }
 extern "C" uint32_t vb_flatten_parts(uint32_t n_tag_words) { return (n_tag_words * 4u + 31u) / 32u; }
+// part_mem: part_count, part_dst (one word per partition each), tag_off (32), the work list of k_flatten (1); 16-byte aligned
+extern "C" size_t vb_flatten_part_words(uint32_t n_parts) { return 35u * (((size_t)n_parts + 3u) & ~(size_t)3u); }
 extern "C" void vb_flatten_arena_bytes(uint32_t cap_lines, size_t *lit_bytes, size_t *job_bytes) {
     *lit_bytes = (size_t)cap_lines * sizeof(FlLit);
     *job_bytes = ((size_t)cap_lines / FL_DEFER_MIN + 1u) * sizeof(FlJob);

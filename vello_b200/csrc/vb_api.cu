@@ -26,6 +26,7 @@ uint32_t vb_pathtag_parts(uint32_t);
 void vb_launch_flatten(const VbConfig *, const uint32_t *, const VbTagMonoid *, VbPathBbox *, VbBump *, VbLineSoup *, void *, void *, uint32_t *,
                        uint32_t *, uint32_t, int, uint32_t, uint32_t, int, cudaStream_t);
 uint32_t vb_flatten_parts(uint32_t);
+size_t vb_flatten_part_words(uint32_t);
 void vb_flatten_arena_bytes(uint32_t, size_t *, size_t *);
 void vb_launch_draw(const VbConfig *, const uint32_t *, const VbPathBbox *, VbDrawMonoid *, uint32_t *, VbClipInp *, uint32_t *, uint32_t,
                     cudaStream_t);
@@ -569,14 +570,14 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     r->parts_tile = vb_tile_alloc_parts(n_draw);
     size_t off = VB_CTL_HEADER_WORDS;
     r->off_lb_pathtag = off; off += vb_lookback_words(r->parts_pathtag, 5);
-    r->off_lb_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [4..] look-back state of its partition scan
+    r->off_lb_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
     off += 4 + vb_lookback_words((r->parts_flatten + 8191u) / 8192u, 1);
     r->off_lb_draw = off; off += vb_lookback_words(r->parts_draw, 4);
     r->off_lb_tile = off; off += vb_lookback_words(r->parts_tile, 1);
     r->off_lb_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
     r->ctl_words = off;
     if ((rc = ensure(r, r->ctl, off * 4))) return rc;
-    if ((rc = ensure(r, r->flatten_parts, ((size_t)r->parts_flatten * 34 + 8) * 4))) return rc;
+    if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(r->parts_flatten) * 4))) return rc;
     return VB_OK;
 }
 
@@ -638,13 +639,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
                 xpeers_of(r, &X);
                 vb_launch_exchange_send(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, ctl + VB_CTL_XCHG_SCRATCH,
                                         (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
-                launches += (r->parts_flatten ? 3 : 0) + 4;
+                launches += (r->parts_flatten ? 4 : 0) + 4;
                 break;
             }
             vb_launch_flatten(&c, (const uint32_t *)r->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p, bump,
                               (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
                               ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, 0u, r->parts_flatten, r->sm_count, st);
-            launches += (first != 0 && c.layout.n_paths ? 1 : 0) + (r->parts_flatten ? 3 : 0);
+            launches += (first != 0 && c.layout.n_paths ? 1 : 0) + (r->parts_flatten ? 4 : 0);
             break;
         case VB_STAGE_ID_DRAW:
             if (r->xc.enabled) { // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
