@@ -150,10 +150,21 @@ void *vb_stream(vb_renderer *);
 int vb_run_stages(vb_renderer *, const vb_params *, int first, int last, void *out_device);
 /* Copy an intermediate buffer to the host: "tag_monoids","path_bboxes","lines","draw_monoids",
  * "info_bin_data","clip_inp","clip_bboxes","draw_bboxes","bin_headers","paths","tiles","seg_counts",
- * "segments","ptcl","blend_spill","bump","config". Returns bytes available in *bytes; copies min(cap, bytes). */
+ * "segments","ptcl","blend_spill","bump","config", and the guard regions of vb_debug_limit_arena ("<arena>.guard", empty
+ * while the arena has no limit). Returns bytes available in *bytes; copies min(cap, bytes). */
 int vb_debug_download(vb_renderer *, const char *name, void *dst, size_t cap, size_t *bytes);
 /* Overwrite an intermediate buffer from the host ("lines" also sets bump.lines; "path_bboxes"). */
 int vb_debug_upload(vb_renderer *, const char *name, const void *src, size_t bytes);
+/* Test-only capacity limit of one bump arena, to drive the overflow / grow-and-re-run path at a chosen boundary. `arena`:
+ * "lines", "binning", "tiles", "seg_counts", "segments", "blend" or "ptcl"; `limit` in the units of the matching
+ * VbConfig::*_size (ptcl: words of the whole arena, static area included); UINT32_MAX clears it. The kernels then see
+ * min(capacity, limit); the allocation is unchanged and its bytes past the limit become a guard region, filled with
+ * VB_GUARD_BYTE when the limit is set (after the renderer's streams are synchronised) and downloadable as "<arena>.guard"
+ * (for "lines" also "line_scratch.guard" and "flatten_jobs.guard"). A limit lasts until an attempt overflows it: growing
+ * the arenas after that attempt drops it. vb_run_stages never grows, so there it stays until cleared. VB_E_INVALID for a
+ * limit of 0, above the current allocation, or (ptcl) below the static area of the last frame's tiles. */
+int vb_debug_limit_arena(vb_renderer *, const char *arena, uint32_t limit);
+#define VB_GUARD_BYTE 0xA5
 
 /* Traffic statistics of the last frame's `fine` (for the roofline): PTCL words its interpreters read,
  * segments referenced by CMD_FILL, number of CMD_FILL commands. */

@@ -219,6 +219,8 @@ def test_arena_growth_and_retry(oracle):
     s = scenes.paris_like(3000, 1024, seed=3)
     packed = resolve(s.encoding)
     img = r.render_to_texture(packed, RenderParams(BLACK, 1024, 1024, AA_MSAA16))
+    # the first attempt overflows `lines` (VB_STAGE_FLATTEN: 426,866 lines against a first guess sized from the tag count)
+    assert r.last_stats.retries >= 1
     ref = oracle.render(packed, 1024, 1024, BLACK.premul_rgba8_u32(), AA_MSAA16)
     assert np.array_equal(img, ref)
     r.close()
@@ -491,7 +493,9 @@ def test_c4_stripes_against_oracle(big_oracle):
     """BASELINE.json configs[3]: paris-30k at 16384x16384 MSAA16 in bin-row stripes. Two of the 64 bin rows (one rank's
     share on a 32-way split; the 8-GPU split renders 8 such rows per rank) are rendered by the GPU as stripes and by the
     oracle with the same window: pixels identical. A fresh renderer is used per stripe, as a rank of the multi-GPU run
-    would start (this is also the regression test of the stale failure flag: the first attempt overflows its arenas)."""
+    would start (this is also a regression test of the stale failure flag: an attempt of each stripe overflows an arena).
+    Bin row 21's first attempt overflows `tiles` (VB_STAGE_TILE_ALLOC: 622,840 tiles against a first guess sized from the
+    draw count); bin row 63's first guesses hold it, so its second frame is forced to overflow `tiles` by one tile."""
     from vello_b200.renderer import Renderer
     size = 16384
     packed = resolve(scenes.paris_like(30000, size, seed=30000).encoding)
@@ -501,18 +505,23 @@ def test_c4_stripes_against_oracle(big_oracle):
         got = r.render_to_texture(packed, p, bin_rows=(b, b + 1))
         st = r.last_stats.as_dict()
         assert st["failed"] == 0
+        if b == 21:
+            assert st["retries"] >= 1
         ref = big_oracle.render(packed, size, size, BLACK.premul_rgba8_u32(), AA_MSAA16, bin_rows=(b, b + 1))[b * 256:(b + 1) * 256]
         assert got.shape == ref.shape
         assert np.array_equal(got, ref), f"bin row {b}: {int((got != ref).any(axis=2).sum())} pixels differ (retries={st['retries']})"
+        if b == 63:
+            r.limit_arena("tiles", st["tile"] - 1)
         again = r.render_to_texture(packed, p, bin_rows=(b, b + 1))
         assert np.array_equal(again, ref)
+        assert r.last_stats.retries == (1 if b == 63 else 0)
         r.close()
 
 
 def test_failed_attempt_leaves_no_flag_in_a_stripe(oracle):
-    """A fresh renderer whose FIRST frame is a stripe that does not contain tile 0 and whose first attempt overflows the
-    first-guess arenas: the successful re-run (and every later frame) must paint. The reference signals failure to fine
-    through ptcl[0] (path_tiling_setup.wgsl:25), which only tile 0's owner rewrites; this implementation reads bump.failed."""
+    """A stripe that does not contain tile 0 and whose first attempt overflows an arena: the successful re-run (and every
+    later frame) must paint. The reference signals failure to fine through ptcl[0] (path_tiling_setup.wgsl:25), which only
+    tile 0's owner rewrites; this implementation reads bump.failed."""
     from vello_b200.renderer import Renderer
     small, w0, h0 = scenes.filled_square()
     packed = resolve(scenes.paris_like(4000, 1024, seed=9).encoding)
@@ -521,11 +530,14 @@ def test_failed_attempt_leaves_no_flag_in_a_stripe(oracle):
     r = Renderer()
     r.upload(resolve(small.encoding))
     r.render_resident(RenderParams(BLACK, w0, h0, AA_AREA), 0, (0, 0))  # arenas sized for a tiny scene, nothing else
-    for rows in ((1, 2), (2, 4), (1, 2)):
+    # the first guesses, sized from this scene, hold the stripe: the overflow is forced on `lines` (VB_STAGE_FLATTEN) with a
+    # limit one line below the stripe's need, on arenas that already held it
+    assert np.array_equal(r.render_to_texture(packed, p, bin_rows=(1, 2)), ref[256:512])
+    r.limit_arena("lines", int(r.last_stats.lines) - 1)
+    for k, rows in enumerate(((1, 2), (2, 4), (1, 2))):
         got = r.render_to_texture(packed, p, bin_rows=rows)
         assert np.array_equal(got, ref[rows[0] * 256:rows[1] * 256]), (rows, r.last_stats.as_dict()["retries"])
-        if rows == (1, 2):
-            first_retries = r.last_stats.as_dict()["retries"]
+        assert r.last_stats.retries == (1 if k == 0 else 0), (rows, r.last_stats.retries)
     r.close()
     r2 = Renderer()  # completely fresh: first-guess arenas from the scene itself
     assert np.array_equal(r2.render_to_texture(packed, p, bin_rows=(3, 4)), ref[768:1024])

@@ -130,6 +130,10 @@ struct DevBuf {
     size_t cap = 0; // bytes
 };
 
+// the seven bump-allocated arenas, by the names vb_debug_limit_arena takes
+enum { ARENA_LINES, ARENA_BINNING, ARENA_TILES, ARENA_SEG_COUNTS, ARENA_SEGMENTS, ARENA_BLEND, ARENA_PTCL, N_ARENAS };
+static const char *const ARENA_NAMES[N_ARENAS] = {"lines", "binning", "tiles", "seg_counts", "segments", "blend", "ptcl"};
+
 // key of a captured frame: everything a launch argument is derived from (see enqueue)
 struct GraphKey {
     VbConfig cfg;
@@ -167,6 +171,8 @@ struct vb_renderer {
     DevBuf resolve_tmp; // patches, ramp descriptors and stops of vb_scene_upload_streams
     DevBuf lines, line_scratch, flatten_jobs, flatten_parts, tiles, seg_counts, segments, ptcl, blend_spill;
     uint32_t cap_lines = 0, cap_binning = 0, cap_tiles = 0, cap_seg_counts = 0, cap_segments = 0, cap_blend = 0, cap_ptcl = 0;
+    // test-only capacity limits (vb_debug_limit_arena), in the order of ARENA_NAMES; UINT32_MAX = none
+    uint32_t arena_limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
 
     // per-frame
     VbConfig cfg{};
@@ -555,13 +561,15 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     if ((rc = ensure(r, r->segments, (size_t)r->cap_segments * sizeof(VbSegment)))) return rc;
     if ((rc = ensure(r, r->blend_spill, (size_t)r->cap_blend * 4))) return rc;
     if ((rc = ensure(r, r->ptcl, (size_t)r->cap_ptcl * 4 + 512))) return rc; // + slack for fine's 256-byte command windows
-    c.lines_size = r->cap_lines;
-    c.binning_size = r->cap_binning;
-    c.tiles_size = r->cap_tiles;
-    c.seg_counts_size = r->cap_seg_counts;
-    c.segments_size = r->cap_segments;
-    c.blend_size = r->cap_blend;
-    c.ptcl_size = r->cap_ptcl;
+    // a test-only limit lowers the capacity the kernels see, never the allocation (vb_debug_limit_arena)
+    const uint32_t *lim = r->arena_limit;
+    c.lines_size = std::min(r->cap_lines, lim[ARENA_LINES]);
+    c.binning_size = std::min(r->cap_binning, lim[ARENA_BINNING]);
+    c.tiles_size = std::min(r->cap_tiles, lim[ARENA_TILES]);
+    c.seg_counts_size = std::min(r->cap_seg_counts, lim[ARENA_SEG_COUNTS]);
+    c.segments_size = std::min(r->cap_segments, lim[ARENA_SEGMENTS]);
+    c.blend_size = std::min(r->cap_blend, lim[ARENA_BLEND]);
+    c.ptcl_size = std::min(r->cap_ptcl, lim[ARENA_PTCL]);
 
     // control block: [bump (8 words, padded to 16)] [look-back states]
     r->parts_pathtag = vb_pathtag_parts(c.n_tag_words);
@@ -930,6 +938,11 @@ static void fill_stats(vb_renderer *r, vb_frame_stats *s) {
 static void grow_arenas(vb_renderer *r) {
     const VbBump &b = *r->h_bump;
     const VbConfig &c = r->cfg;
+    // a test-only limit lasts for one overflow of its arena: the re-run sees the real capacity
+    const uint64_t need[N_ARENAS] = {b.lines, b.binning, b.tile, b.seg_counts, b.segments, b.blend,
+                                     (uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC + b.ptcl};
+    for (int a = 0; a < N_ARENAS; a++)
+        if (need[a] > r->arena_limit[a]) r->arena_limit[a] = UINT32_MAX;
     if (b.lines > r->cap_lines) r->cap_lines = grow(b.lines);
     if (b.binning > r->cap_binning) r->cap_binning = grow(b.binning);
     if (b.tile > r->cap_tiles) r->cap_tiles = grow(b.tile);
@@ -1202,10 +1215,94 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
     };
 }
 
+// The guard region of a limited arena (vb_debug_limit_arena): the bytes of its allocation past the limit. `name` is an arena
+// name, or "line_scratch" / "flatten_jobs" (flatten's scratch arenas, sized from the lines capacity). Returns false for an
+// unknown name; *buf is nullptr while the arena has no limit.
+static bool guard_region(vb_renderer *r, const char *name, DevBuf **buf, size_t *off) {
+    int a = -1;
+    if (!strcmp(name, "line_scratch") || !strcmp(name, "flatten_jobs")) a = ARENA_LINES;
+    for (int i = 0; i < N_ARENAS; i++)
+        if (!strcmp(name, ARENA_NAMES[i])) a = i;
+    if (a < 0) return false;
+    *buf = nullptr;
+    *off = 0;
+    const size_t lim = r->arena_limit[a];
+    if (lim == UINT32_MAX) return true;
+    DevBuf *b = nullptr;
+    size_t o = 0;
+    switch (a) {
+    case ARENA_LINES: {
+        size_t lit_bytes, job_bytes; // flatten sees lits_cap = lines_size, jobs_cap = lines_size / FL_DEFER_MIN + 1
+        vb_flatten_arena_bytes((uint32_t)lim, &lit_bytes, &job_bytes);
+        if (!strcmp(name, "line_scratch")) b = &r->line_scratch, o = lit_bytes;
+        else if (!strcmp(name, "flatten_jobs")) b = &r->flatten_jobs, o = job_bytes;
+        else b = &r->lines, o = lim * sizeof(VbLineSoup);
+        break;
+    }
+    case ARENA_BINNING: b = &r->info_bin_data, o = ((size_t)r->layout.bin_data_start + lim) * 4; break;
+    case ARENA_TILES: b = &r->tiles, o = lim * sizeof(VbTile); break;
+    case ARENA_SEG_COUNTS: b = &r->seg_counts, o = lim * sizeof(VbSegmentCount); break;
+    case ARENA_SEGMENTS: b = &r->segments, o = lim * sizeof(VbSegment); break;
+    case ARENA_BLEND: b = &r->blend_spill, o = lim * 4; break;
+    default: b = &r->ptcl, o = lim * 4; break; // includes the 512 bytes of window slack that fine reads and never writes
+    }
+    *buf = b;
+    *off = o < b->cap ? o : b->cap;
+    return true;
+}
+
+extern "C" int vb_debug_limit_arena(vb_renderer *r, const char *arena, uint32_t limit) {
+    if (!r || !arena) return VB_E_INVALID;
+    int a = -1;
+    for (int i = 0; i < N_ARENAS; i++)
+        if (!strcmp(arena, ARENA_NAMES[i])) a = i;
+    if (a < 0) {
+        r->err = std::string("vb_debug_limit_arena: unknown arena ") + arena;
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream));
+    CK(cudaStreamSynchronize(r->copy_stream));
+    CK(cudaStreamSynchronize(r->upload_stream));
+    if (limit == UINT32_MAX) {
+        r->arena_limit[a] = UINT32_MAX;
+        return VB_OK;
+    }
+    const uint32_t caps[N_ARENAS] = {r->cap_lines, r->cap_binning, r->cap_tiles, r->cap_seg_counts, r->cap_segments, r->cap_blend, r->cap_ptcl};
+    const uint64_t ptcl_static = (uint64_t)r->cfg.width_in_tiles * r->cfg.height_in_tiles * VB_PTCL_INITIAL_ALLOC;
+    // 0 is refused too: path_count and path_tiling size their grids from the capacity
+    if (limit == 0u || limit > caps[a] || (a == ARENA_PTCL && limit < ptcl_static)) {
+        r->err = "vb_debug_limit_arena: the limit must be at least 1 (the static area for ptcl) and at most the allocation";
+        return VB_E_INVALID;
+    }
+    r->arena_limit[a] = limit;
+    const char *regions[3] = {ARENA_NAMES[a], "line_scratch", "flatten_jobs"};
+    for (int k = 0; k < (a == ARENA_LINES ? 3 : 1); k++) {
+        DevBuf *b;
+        size_t off;
+        guard_region(r, regions[k], &b, &off);
+        if (b && b->cap > off) CK(cudaMemsetAsync((char *)b->p + off, VB_GUARD_BYTE, b->cap - off, r->stream));
+    }
+    CK(cudaStreamSynchronize(r->stream));
+    return VB_OK;
+}
+
 extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, size_t cap, size_t *bytes) {
     if (!r || !name) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
+    const size_t len = strlen(name);
+    if (len > 6 && !strcmp(name + len - 6, ".guard")) {
+        const std::string base(name, len - 6);
+        DevBuf *b;
+        size_t off;
+        if (!guard_region(r, base.c_str(), &b, &off)) return VB_E_UNKNOWN_BUFFER;
+        const size_t n = b ? b->cap - off : 0;
+        if (bytes) *bytes = n;
+        const size_t c = n < cap ? n : cap;
+        if (dst && c) CK(cudaMemcpy(dst, (const char *)b->p + off, c, cudaMemcpyDeviceToHost));
+        return VB_OK;
+    }
     if (!strcmp(name, "bump")) {
         if (bytes) *bytes = sizeof(VbBump);
         if (dst && cap >= sizeof(VbBump)) CK(cudaMemcpy(dst, r->ctl.p, sizeof(VbBump), cudaMemcpyDeviceToHost));
@@ -1648,8 +1745,11 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                     redo = true;
                     rc = VB_OK;
                 } else {
-                    // grow and re-run (first frames); with a host destination the re-run queues its read-back again
+                    // grow and re-run (first frames); with a host destination the re-run queues its read-back again.
+                    // Growing first: the same attempt with the same arenas would only overflow again.
+                    grow_arenas(r);
                     rc = vb_render_resident(r, &ps[i], dst, stats ? &stats[i] : nullptr);
+                    if (stats) stats[i].retries += 1;
                 }
             }
             g->ms[i] = vb_last_frame_ms(r);

@@ -61,7 +61,7 @@ typedef struct {
 #define VB_STAGE_FLATTEN 0x4u
 #define VB_STAGE_PATH_COUNT 0x8u
 #define VB_STAGE_COARSE 0x10u
-#define VB_STAGE_FINE_SEGMENTS 0x20u /* extension: segments arena too small (checked in coarse) */
+#define VB_STAGE_FINE_SEGMENTS 0x20u /* extension: segments arena too small (reserved in coarse, checked in k_path_tiling) */
 #define VB_STAGE_EXCHANGE 0x40u      /* extension: multi-GPU line exchange (outbox too small, or a peer never signalled) */
 
 #define VB_TILE_WIDTH 16u

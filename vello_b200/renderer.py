@@ -94,6 +94,7 @@ def load_library() -> C.CDLL:
     lib.vb_run_stages.argtypes = [vp, C.POINTER(_Params), C.c_int, C.c_int, vp]
     lib.vb_debug_download.argtypes = [vp, C.c_char_p, vp, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.vb_debug_upload.argtypes = [vp, C.c_char_p, vp, C.c_size_t]
+    lib.vb_debug_limit_arena.argtypes = [vp, C.c_char_p, C.c_uint32]
     lib.vb_set_occlusion_cull.argtypes = [vp, C.c_int]
     lib.vb_debug_fine_traffic.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.vb_last_frame_ms.restype = C.c_float
@@ -130,7 +131,7 @@ def load_library() -> C.CDLL:
 
 EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_last_error", "vb_scene_upload",
                     "vb_render_resident", "vb_render_enqueue", "vb_frame_finish", "vb_render", "vb_target", "vb_copy_to_host", "vb_stream",
-                    "vb_run_stages", "vb_debug_download", "vb_debug_upload", "vb_debug_fine_traffic", "vb_set_occlusion_cull", "vb_render_begin", "vb_readback_wait", "vb_set_readback_bands", "vb_set_cuda_graph", "vb_set_timing",
+                    "vb_run_stages", "vb_debug_download", "vb_debug_upload", "vb_debug_limit_arena", "vb_debug_fine_traffic", "vb_set_occlusion_cull", "vb_render_begin", "vb_readback_wait", "vb_set_readback_bands", "vb_set_cuda_graph", "vb_set_timing",
                     "vb_scene_upload_streams", "vb_render_uploaded", "vb_last_frame_ms", "vb_frame_alloc", "vb_frame_free", "vb_ipc_export", "vb_ipc_open", "vb_ipc_close",
                     "vb_group_new", "vb_group_free", "vb_group_size", "vb_group_renderer", "vb_group_last_error", "vb_group_render",
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
@@ -165,11 +166,20 @@ class Renderer:
         self.options = options
         self.last_stats: Optional[FrameStats] = None
         self._keep = None
+        self._owner = None
+
+    @classmethod
+    def _borrowed(cls, lib, handle: int, owner):
+        """A view of a renderer owned by someone else (a RendererGroup): closing it frees nothing."""
+        r = cls.__new__(cls)
+        r.lib, r.handle, r.options, r.last_stats, r._keep = lib, C.c_void_p(handle), None, None, None
+        r._owner = owner
+        return r
 
     def close(self):
-        if getattr(self, "handle", None) and self.handle.value:
+        if getattr(self, "_owner", None) is None and getattr(self, "handle", None) and self.handle.value:
             self.lib.vb_renderer_free(self.handle)
-            self.handle = C.c_void_p()
+        self.handle = C.c_void_p()
 
     def __del__(self):
         try:
@@ -297,6 +307,20 @@ class Renderer:
         a = np.ascontiguousarray(arr)
         self._check(self.lib.vb_debug_upload(self.handle, name.encode(), a.ctypes.data, a.nbytes), f"upload {name}")
 
+    # the guard byte vb_debug_limit_arena writes past a limited arena's limit (VB_GUARD_BYTE)
+    GUARD_BYTE = 0xA5
+    NO_LIMIT = 0xFFFFFFFF
+
+    def limit_arena(self, name: str, limit: int):
+        """Test-only: the kernels see at most `limit` of arena `name` ("lines", "binning", "tiles", "seg_counts", "segments",
+        "blend", "ptcl"; ptcl in words of the whole arena) until an attempt overflows it. `NO_LIMIT` clears it. The bytes of
+        the allocation past the limit are filled with GUARD_BYTE (see download_guard)."""
+        self._check(self.lib.vb_debug_limit_arena(self.handle, name.encode(), int(limit)), f"vb_debug_limit_arena {name}")
+
+    def download_guard(self, name: str) -> np.ndarray:
+        """The guard region past a limited arena's limit as bytes ("lines", ..., "ptcl", "line_scratch", "flatten_jobs")."""
+        return self.download(f"{name}.guard", np.uint8)
+
     def set_cuda_graph(self, on: bool):
         """Replay whole frames as CUDA graphs (default on)."""
         self._check(self.lib.vb_set_cuda_graph(self.handle, 1 if on else 0), "vb_set_cuda_graph")
@@ -352,6 +376,13 @@ class RendererGroup:
     def _check(self, rc, what):
         if rc != 0:
             raise VelloB200Error(f"{what}: {self.lib.vb_strerror(rc).decode()} [{self.lib.vb_group_last_error(self.handle).decode()}]")
+
+    def renderer(self, i: int) -> Renderer:
+        """The i-th device's renderer (statistics, debugging); it belongs to the group and lives as long as the group."""
+        h = self.lib.vb_group_renderer(self.handle, int(i))
+        if not h:
+            raise VelloB200Error(f"vb_group_renderer: no renderer {i}")
+        return Renderer._borrowed(self.lib, h, self)
 
     def set_balancing(self, on: bool):
         self._check(self.lib.vb_group_set_balancing(self.handle, 1 if on else 0), "vb_group_set_balancing")
