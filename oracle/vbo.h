@@ -66,7 +66,9 @@ int vbo_bind(vbo_ctx *, const uint32_t *scene, size_t scene_words, const vbo_lay
              uint32_t atlas_h, const vbo_params *);
 
 /* Run stages first..last inclusive (stage enum above). Fine writes `out_rgba8`
- * (width*height*4 bytes, un-premultiplied, row pitch 4*width); may be NULL for earlier stages. */
+ * (width*height*4 bytes, un-premultiplied, row pitch 4*width); may be NULL for earlier stages.
+ * Returns 0; -1 fine without `out_rgba8`; -3 fine met a command, segment slice, draw-info read or
+ * blend spill outside its buffer (possible only with buffers installed by vbo_set_buffer). */
 int vbo_run(vbo_ctx *, int first_stage, int last_stage, uint8_t *out_rgba8);
 
 /* Intermediate buffers by name: "tag_monoids","path_bboxes","lines","draw_monoids","info_bin_data",
@@ -74,8 +76,12 @@ int vbo_run(vbo_ctx *, int first_stage, int last_stage, uint8_t *out_rgba8);
  * "ptcl","bump","config". Returns pointer + size in bytes (valid until the next vbo_run). */
 const void *vbo_buffer(vbo_ctx *, const char *name, size_t *bytes);
 
-/* Replace an intermediate buffer (e.g. feed the CUDA path's line soup to the oracle's tile
- * stages). Only "lines" and "path_bboxes" are supported. */
+/* Replace an intermediate buffer after vbo_bind (e.g. feed the CUDA path's line soup to the
+ * oracle's tile stages). Supported: "lines" and "path_bboxes" (inputs of the tile stages), and
+ * "ptcl", "segments", "info_bin_data" and "blend_spill" (the inputs of fine, so that running
+ * only fine replays another implementation's command lists). "blend_spill" also sets the spill
+ * size (bump.blend): pass as many words as the blend offsets in the installed ptcl were
+ * allocated against. Returns -1 for any other name. */
 int vbo_set_buffer(vbo_ctx *, const char *name, const void *data, size_t bytes);
 
 /* Number of worker threads for `fine` (per-tile independent). 1 = serial. */

@@ -38,13 +38,28 @@ static inline rgba_t over(rgba_t bg, rgba_t fg) {
     return RG(fmaf(bg.r, k, fg.r), fmaf(bg.g, k, fg.g), fmaf(bg.b, k, fg.b), fmaf(bg.a, k, fg.a));
 }
 
+/* Sizes of every buffer the interpreter reads or writes: fine may be replayed on buffers another implementation wrote
+ * (vbo_set_buffer), so each access is checked and a reference outside a buffer fails the run instead of reading or
+ * writing past it. */
 typedef struct {
     const vbo_ctx *c;
     const uint32_t *ptcl, *info;
     const Segment *segments;
     uint32_t *blend_spill;
-    uint32_t n_segments;
+    size_t n_ptcl, n_info, n_segments, n_spill;
+    int *error;
 } FineIn;
+
+static void fine_fail(const FineIn *in) { __atomic_store_n(in->error, 1, __ATOMIC_RELAXED); }
+static uint32_t cmd_words(uint32_t tag) {
+    switch (tag) {
+    case CMD_FILL: return 4u;
+    case CMD_COLOR: case CMD_IMAGE: case CMD_JUMP: return 2u;
+    case CMD_LIN_GRAD: case CMD_RAD_GRAD: case CMD_SWEEP_GRAD: case CMD_END_CLIP: case CMD_BLUR_RECT: return 3u;
+    default: return 1u;
+    }
+}
+static int in_range(size_t start, size_t n, size_t size) { return start <= size && n <= size - start; }
 
 /* ---------------- area coverage: fine.wgsl:1005-1059 ---------------- */
 static void fill_path_area(const FineIn *in, uint32_t size_and_rule, uint32_t seg_data, int32_t backdrop, float *area) {
@@ -543,15 +558,30 @@ static void fine_tile(const FineIn *in, const uint32_t *mask_lut, uint32_t tile_
     uint32_t stack_cap = 0;
     uint32_t clip_depth = 0u;
     uint32_t cmd_ix = tile_ix * 64u;
-    uint32_t blend_offset = ptcl[cmd_ix];
+    uint32_t blend_offset = in_range(cmd_ix, 1, in->n_ptcl) ? ptcl[cmd_ix] : 0u;
     cmd_ix += 1u;
     for (;;) {
+        if (!in_range(cmd_ix, 1, in->n_ptcl) || !in_range(cmd_ix, cmd_words(ptcl[cmd_ix]), in->n_ptcl)) {
+            fine_fail(in);
+            break;
+        }
         uint32_t tag = ptcl[cmd_ix];
         if (tag == CMD_END) break;
+        /* brushes that read draw info: the words they read must lie in info_bin_data */
+        uint32_t info_n = tag == CMD_LIN_GRAD ? 3u : tag == CMD_RAD_GRAD ? 9u : tag == CMD_SWEEP_GRAD ? 8u : tag == CMD_IMAGE ? 9u
+                          : tag == CMD_BLUR_RECT ? 10u : 0u;
+        if (info_n && !in_range(ptcl[cmd_ix + (tag == CMD_IMAGE || tag == CMD_BLUR_RECT ? 1u : 2u)], info_n, in->n_info)) {
+            fine_fail(in);
+            break;
+        }
         switch (tag) {
         case CMD_FILL: {
             uint32_t sr = ptcl[cmd_ix + 1], sd = ptcl[cmd_ix + 2];
             int32_t bd = (int32_t)ptcl[cmd_ix + 3];
+            if (!in_range(sd, sr >> 1, in->n_segments)) {
+                fine_fail(in);
+                goto done;
+            }
             if (aa == 0u) fill_path_area(in, sr, sd, bd, area);
             else fill_path_ms(in, mask_lut, aa == 2u, sr, sd, bd, area);
             cmd_ix += 4u;
@@ -572,11 +602,16 @@ static void fine_tile(const FineIn *in, const uint32_t *mask_lut, uint32_t tile_
                 stack_cap = stack_cap ? stack_cap * 2u : 8u;
                 stack = realloc(stack, (size_t)stack_cap * 256u * 4u);
             }
+            /* mirror the spill buffer traffic (fine.wgsl:1126-1133) at the tile's blend offset */
+            int spill = clip_depth >= 4u && in->blend_spill;
+            if (spill && !in_range((size_t)blend_offset + (clip_depth - 4u) * 256u, 256, in->n_spill)) {
+                fine_fail(in);
+                goto done;
+            }
             for (int i = 0; i < 256; i++) {
                 uint32_t packed = pack4x8unorm(rgba[i]);
                 stack[clip_depth * 256u + (uint32_t)i] = packed;
-                if (clip_depth >= 4u && in->blend_spill) /* mirror the spill buffer traffic (fine.wgsl:1126-1133) */
-                    in->blend_spill[blend_offset + (clip_depth - 4u) * 256u + (uint32_t)i] = packed;
+                if (spill) in->blend_spill[blend_offset + (clip_depth - 4u) * 256u + (uint32_t)i] = packed;
                 rgba[i] = RG(0, 0, 0, 0);
             }
             clip_depth += 1u;
@@ -586,6 +621,10 @@ static void fine_tile(const FineIn *in, const uint32_t *mask_lut, uint32_t tile_
         case CMD_END_CLIP: {
             uint32_t blend = ptcl[cmd_ix + 1];
             float alpha = u2f_bits(ptcl[cmd_ix + 2]);
+            if (clip_depth == 0u) {
+                fine_fail(in);
+                goto done;
+            }
             clip_depth -= 1u;
             for (int i = 0; i < 256; i++) {
                 rgba_t bg = unpack4x8unorm(stack[clip_depth * 256u + (uint32_t)i]);
@@ -785,6 +824,7 @@ static void fine_tile(const FineIn *in, const uint32_t *mask_lut, uint32_t tile_
             break;
         }
     }
+done:
     free(stack);
     for (int i = 0; i < 256; i++) {
         uint32_t px = tile_x * 16u + ((uint32_t)i & 15u), py = tile_y * 16u + ((uint32_t)i >> 4);
@@ -847,18 +887,20 @@ static void *fine_worker(void *arg) {
     return NULL;
 }
 
-void vbo_fine(vbo_ctx *c, uint8_t *out) {
+int vbo_fine(vbo_ctx *c, uint8_t *out) {
     static uint32_t lut8[256], lut16[2048];
     static int luts_ready = 0;
     if (!luts_ready) { make_mask_luts(lut8, lut16); luts_ready = 1; }
     uint32_t *spill = vec_resize(&c->blend_spill, c->bump.blend ? c->bump.blend : 1);
-    FineIn in = {c, c->ptcl.p, c->info_bin_data.p, c->segments.p, spill, c->bump.segments};
+    int error = 0;
+    FineIn in = {c, c->ptcl.p, c->info_bin_data.p, c->segments.p, spill,
+                 c->ptcl.n, c->info_bin_data.n, c->segments.n, c->bump.blend, &error};
     const uint32_t *lut = c->params.aa == 2u ? lut16 : lut8;
     int nt = c->threads;
     if (nt <= 1) {
         Job j = {&in, lut, out, c->win_ty0, c->win_ty1, c->cfg.width_in_tiles, 0, 1};
         fine_worker(&j);
-        return;
+        return error ? -3 : 0;
     }
     enum { MAX_THREADS = 1024 };
     static pthread_t th[MAX_THREADS]; /* vbo_fine is not re-entrant (one context renders at a time) */
@@ -872,4 +914,5 @@ void vbo_fine(vbo_ctx *c, uint8_t *out) {
         pthread_create(&th[t], NULL, fine_worker, &jobs[t]);
     }
     for (int t = 0; t < nt; t++) pthread_join(th[t], NULL);
+    return error ? -3 : 0;
 }

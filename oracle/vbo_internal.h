@@ -111,6 +111,7 @@ struct vbo_ctx {
     int threads;
 };
 
-void vbo_fine(vbo_ctx *c, uint8_t *out);
+/* 0, or -3 when a command, segment slice, draw-info read or blend spill lies outside its buffer */
+int vbo_fine(vbo_ctx *c, uint8_t *out);
 
 #endif

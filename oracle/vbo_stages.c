@@ -1579,7 +1579,7 @@ int vbo_run(vbo_ctx *c, int first, int last, uint8_t *out) {
         case VBO_STAGE_PATH_TILING: stage_path_tiling(c); break;
         case VBO_STAGE_FINE:
             if (!out) return -1;
-            vbo_fine(c, out);
+            if (vbo_fine(c, out) != 0) return -3;
             break;
         default: return -2;
         }
@@ -1626,6 +1626,36 @@ int vbo_set_buffer(vbo_ctx *c, const char *name, const void *data, size_t bytes)
         size_t n = bytes / sizeof(PathBbox);
         void *p = vec_resize(&c->path_bboxes, n);
         memcpy(p, data, n * sizeof(PathBbox));
+        return 0;
+    }
+    /* fine's inputs, so that `fine` alone interprets exactly the buffers another implementation's fine read */
+    if (!strcmp(name, "ptcl")) {
+        size_t n = bytes / 4;
+        memcpy(vec_resize(&c->ptcl, n), data, n * 4);
+        c->cfg.ptcl_size = (uint32_t)n;
+        return 0;
+    }
+    if (!strcmp(name, "segments")) {
+        size_t n = bytes / sizeof(Segment);
+        memcpy(vec_resize(&c->segments, n), data, n * sizeof(Segment));
+        c->bump.segments = (uint32_t)n;
+        c->cfg.segments_size = (uint32_t)n;
+        return 0;
+    }
+    if (!strcmp(name, "info_bin_data")) {
+        size_t n = bytes / 4;
+        memcpy(vec_resize(&c->info_bin_data, n), data, n * 4);
+        c->bump.binning = n > c->cfg.layout.bin_data_start ? (uint32_t)(n - c->cfg.layout.bin_data_start) : 0u;
+        c->cfg.binning_size = c->bump.binning;
+        return 0;
+    }
+    /* sizes the spill area from the caller's count (the blend offsets in a replayed ptcl were allocated against it): fine
+     * writes its spilled blend-stack levels there, at each tile's blend offset */
+    if (!strcmp(name, "blend_spill")) {
+        size_t n = bytes / 4;
+        memcpy(vec_resize(&c->blend_spill, n), data, n * 4);
+        c->bump.blend = (uint32_t)n;
+        c->cfg.blend_size = (uint32_t)n;
         return 0;
     }
     return -1;

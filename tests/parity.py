@@ -77,6 +77,37 @@ def unpaired_endpoints(lines: np.ndarray) -> np.ndarray:
     return u[c % 2 == 1]
 
 
+def replay_fine(r, o, packed, w, h, aa, base, window=None):
+    """The oracle's `fine` run on the buffers the GPU's `fine` read in the last frame of renderer r: its `ptcl`, `segments`
+    and `info_bin_data`, with the blend spill sized by the GPU's `bump.blend` (the blend offsets in that ptcl were allocated
+    against it). Returns the oracle's image (h, w, 4); with a bin-row `window` only that window's rows are painted.
+
+    The GPU's image must equal it byte for byte in every AA mode: the two interpreters then see the same commands and the
+    same segments in the same order, so even area AA's float sums agree (both sides are built without FMA contraction).
+    The GPU's fine starts a tile at its occlusion start and walks coarse's cost-ordered tile queue; the oracle starts every
+    tile at its head, so equality also pins the occlusion start."""
+    g = gpu_buffers(r, ["ptcl", "segments", "info_bin_data", "bump"])
+    bump = g["bump"][0]
+    assert int(bump["failed"]) == 0, "the last GPU frame failed: fine painted nothing"
+    base_u32 = base if isinstance(base, int) else base.premul_rgba8_u32()
+    o.bind(packed, w, h, base_u32, aa, window or (0, 0))
+    for n in ("ptcl", "segments", "info_bin_data"):
+        o.set_buffer(n, g[n])
+    o.set_buffer("blend_spill", np.zeros(int(bump["blend"]), np.uint32))
+    return o.run("fine", "fine")
+
+
+def assert_replay(r, o, packed, img, w, h, aa, base, window=None):
+    """`img`, the last frame of renderer r (the window's rows only, for a bin-row window), equals replay_fine's image."""
+    want = replay_fine(r, o, packed, w, h, aa, base, window)
+    if window:
+        want = want[min(window[0] * 256, h):min(window[1] * 256, h)]
+    assert img.shape == want.shape, (img.shape, want.shape)
+    bad = (img != want).any(axis=2)
+    assert not bad.any(), f"aa={aa}: {int(bad.sum())} pixels differ from the oracle's fine on the GPU's own buffers, first at " \
+                          f"{tuple(int(v) for v in np.argwhere(bad)[0])}"
+
+
 STAGES = ["pathtag", "flatten", "draw", "clip", "binning", "tile_alloc", "path_count", "backdrop", "coarse", "path_tiling", "fine"]
 # the stage that writes each compared buffer (info_bin_data: its info part; the bins part belongs to binning) and bump counter
 BUFFER_STAGE = {"tag_monoids": "pathtag", "path_bboxes": "flatten", "lines": "flatten", "draw_monoids": "draw", "clip_inp": "draw",
