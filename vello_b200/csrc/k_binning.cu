@@ -111,11 +111,12 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
     }
 }
 
-extern "C" void vb_launch_binning(const VbConfig *cfg, const VbDrawMonoid *draw_monoids, const VbPathBbox *path_bbox,
+extern "C" uint32_t vb_launch_binning(const VbConfig *cfg, const VbDrawMonoid *draw_monoids, const VbPathBbox *path_bbox,
                                   const VbBbox4 *clip_bbox, VbBbox4 *draw_bbox, VbBump *bump, uint32_t *info_bin_data,
                                   VbBinHeader *bin_header, cudaStream_t st) {
     uint32_t n = cfg->layout.n_draw_objects;
-    if (n == 0) return;
+    if (n == 0) return 0;
     k_binning<<<(n + BN_THREADS - 1) / BN_THREADS, BN_THREADS, 0, st>>>(*cfg, draw_monoids, path_bbox, clip_bbox, draw_bbox, bump,
                                                                        info_bin_data, bin_header);
+    return 1;
 }

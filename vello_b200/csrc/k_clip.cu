@@ -135,10 +135,10 @@ __global__ void k_clip_bbox(uint32_t n_clips, const VbClipInp *__restrict__ clip
 }
 
 extern "C" uint32_t vb_clip_parts(uint32_t n_clips) { return (n_clips + CL_THREADS - 1u) / CL_THREADS; }
-extern "C" void vb_launch_clip(uint32_t n_clips, const VbClipInp *clip_inp, const VbPathBbox *pbs, VbDrawMonoid *draw_monoids,
+extern "C" uint32_t vb_launch_clip(uint32_t n_clips, const VbClipInp *clip_inp, const VbPathBbox *pbs, VbDrawMonoid *draw_monoids,
                                VbBbox4 *clip_bboxes, int32_t *scratch /* B | min32 | min1024 | link */, uint32_t *lb_mem /* zeroed */,
                                cudaStream_t st) {
-    if (n_clips == 0) return;
+    if (n_clips == 0) return 0;
     int32_t *B = scratch;
     int32_t *min32 = B + n_clips;
     int32_t *min1024 = min32 + (n_clips + 31) / 32;
@@ -147,6 +147,7 @@ extern "C" void vb_launch_clip(uint32_t n_clips, const VbClipInp *clip_inp, cons
     k_clip_depth<<<n_parts, CL_THREADS, 0, st>>>(n_clips, clip_inp, B, min32, min1024, lb_mem, n_parts);
     k_clip_link<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, clip_inp, B, min32, min1024, link);
     k_clip_bbox<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, clip_inp, pbs, link, draw_monoids, clip_bboxes);
+    return 3;
 }
 extern "C" size_t vb_clip_scratch_words(uint32_t n_clips) {
     return (size_t)n_clips * 2 + (n_clips + 31) / 32 + (n_clips + 1023) / 1024 + 8;

@@ -424,12 +424,13 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
 // The segments-arena overflow check (the reference sizes `segments` statically and never checks) lives at the top of
 // k_path_tiling, the next kernel.
 
-extern "C" void vb_launch_coarse(const VbConfig *cfg, const uint32_t *scene, const VbDrawMonoid *draw_monoids,
+extern "C" uint32_t vb_launch_coarse(const VbConfig *cfg, const uint32_t *scene, const VbDrawMonoid *draw_monoids,
                                  const VbBinHeader *bin_headers, const uint32_t *info_bin_data, const VbPath *paths, VbTile *tiles,
                                  VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, void *cls_list, uint32_t cls_stride, cudaStream_t st) {
     uint32_t width_in_bins = (cfg->width_in_tiles + 15u) / 16u;
     uint32_t rows = cfg->win_by1 - cfg->win_by0;
-    if (width_in_bins == 0 || rows == 0) return;
+    if (width_in_bins == 0 || rows == 0) return 0;
     dim3 grid(width_in_bins * 2u, rows * 2u); // four quadrant CTAs per bin
     k_coarse<<<grid, CO_THREADS, 0, st>>>(*cfg, scene, draw_monoids, bin_headers, info_bin_data, paths, tiles, bump, ptcl, tile_start, (uint2 *)cls_list, cls_stride);
+    return 1;
 }

@@ -233,9 +233,10 @@ k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const VbPathBbox *__res
     }
 }
 
-extern "C" void vb_launch_draw(const VbConfig *cfg, const uint32_t *scene, const VbPathBbox *path_bbox, VbDrawMonoid *draw_monoid,
+extern "C" uint32_t vb_launch_draw(const VbConfig *cfg, const uint32_t *scene, const VbPathBbox *path_bbox, VbDrawMonoid *draw_monoid,
                                uint32_t *info, VbClipInp *clip_inp, uint32_t *lb_mem, uint32_t n_parts, cudaStream_t st) {
-    if (n_parts == 0) return;
+    if (n_parts == 0) return 0;
     k_draw<<<n_parts, DR_THREADS, 0, st>>>(*cfg, scene, path_bbox, draw_monoid, info, clip_inp, lb_mem, n_parts);
+    return 1;
 }
 extern "C" uint32_t vb_draw_parts(uint32_t n_draw) { return (n_draw + DR_THREADS - 1) / DR_THREADS; }

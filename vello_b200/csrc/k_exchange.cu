@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(256) k_lines_pull(XPeers X, VbBump *bump, uint
 // send = everything up to raising my flags; recv = wait for the peers, combine the boxes, pull my lines. They are separate
 // entry points so that a host driving several renderers on ONE device can issue every send before any recv (a wait kernel
 // never sits in front of the signal it waits for in a shared hardware queue).
-extern "C" void vb_launch_exchange_send(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines, uint32_t *scratch,
+extern "C" uint32_t vb_launch_exchange_send(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines, uint32_t *scratch,
                                         VbPathBbox *path_bboxes, int sm_count, cudaStream_t st) {
     const XPeers &X = *reinterpret_cast<const XPeers *>(peers);
     const uint32_t grid = (uint32_t)sm_count * 8u;
@@ -248,13 +248,15 @@ extern "C" void vb_launch_exchange_send(const void *peers /* XPeers */, VbBump *
     k_route_scatter<<<grid, 256, 0, st>>>(X, bump, lines_size, lines, scratch, scratch + XG_MAX);
     if (X.n_paths) k_bbox_publish<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, path_bboxes);
     k_xsignal<<<1, 32, 0, st>>>(X, scratch);
+    return X.n_paths ? 4 : 3;
 }
-extern "C" void vb_launch_exchange_recv(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines,
+extern "C" uint32_t vb_launch_exchange_recv(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines,
                                         VbPathBbox *path_bboxes, int sm_count, cudaStream_t st) {
     const XPeers &X = *reinterpret_cast<const XPeers *>(peers);
     const uint32_t grid = (uint32_t)sm_count * 8u;
     k_xwait<<<1, 32, 0, st>>>(X, bump, 4000000000ull); // ~2 s at 2 GHz
     if (X.n_paths) k_bbox_combine<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, path_bboxes);
     k_lines_pull<<<grid, 256, 0, st>>>(X, bump, lines_size, lines);
+    return X.n_paths ? 3 : 2;
 }
 extern "C" size_t vb_exchange_peers_bytes(void) { return sizeof(XPeers); }

@@ -1234,13 +1234,13 @@ extern "C" int vb_fine_init_constants(void) {
 }
 
 // `queue` = one zeroed word per launch (vb_api.cu keeps 8 of them in the control block, one per read-back band).
-extern "C" void vb_launch_fine(const VbConfig *cfg, int aa, const VbBump *bump, const VbSegment *segments, const uint32_t *ptcl, const uint32_t *info,
+extern "C" uint32_t vb_launch_fine(const VbConfig *cfg, int aa, const VbBump *bump, const VbSegment *segments, const uint32_t *ptcl, const uint32_t *info,
                                uint32_t *blend_spill, uint32_t *out, const uint32_t *ramps, const uint8_t *atlas,
                                const uint32_t *mask_lut8, const uint32_t *mask_lut16, const uint32_t *tile_start, uint32_t cull, uint32_t *queue,
                                const void *cls_list, const uint32_t *cls_count, uint32_t cls_stride, int sm_count, cudaStream_t st) {
     uint32_t rows = cfg->win_ty1 - cfg->win_ty0;
     uint32_t n = cfg->width_in_tiles * rows;
-    if (n == 0) return;
+    if (n == 0) return 0;
     // persistent grid: FI_MINB CTAs per SM; small frames get smaller CTAs so that their tiles still spread over the SMs
     uint32_t warps = FI_MAX_WARPS;
     while (warps > 2u && (n + warps - 1u) / warps < (uint32_t)sm_count * FI_MINB) warps >>= 1;
@@ -1260,4 +1260,5 @@ extern "C" void vb_launch_fine(const VbConfig *cfg, int aa, const VbBump *bump, 
     if (aa == 0) k_fine<0><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(*cfg, A);
     else if (aa == 1) k_fine<1><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(*cfg, A);
     else k_fine<2><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(*cfg, A);
+    return 1;
 }

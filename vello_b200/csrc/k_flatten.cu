@@ -1254,13 +1254,16 @@ k_flatten_place(VbConfig cfg, const uint32_t *__restrict__ scene, FlCtx ctx, con
     }
 }
 
-extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, const VbTagMonoid *tag_monoids,
+extern "C" uint32_t vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, const VbTagMonoid *tag_monoids,
                                   VbPathBbox *path_bboxes, VbBump *bump, VbLineSoup *lines, void *lit_arena, void *job_arena,
                                   uint32_t *part_mem /* vb_flatten_part_words */, uint32_t *ctrs, uint32_t n_parts, int clear_bboxes,
                                   uint32_t part_base, uint32_t part_end /* 0, n_parts: everything */, int sm_count, cudaStream_t st) {
-    uint32_t n_paths = cfg->layout.n_paths;
+    uint32_t n_paths = cfg->layout.n_paths, launches = 0;
     // whole frames reset the boxes in k_frame_init (vb_api.cu); a stage range that starts later does it here
-    if (n_paths && clear_bboxes) k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
+    if (n_paths && clear_bboxes) {
+        k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
+        launches++;
+    }
     if (n_parts) {
         const size_t np4 = ((size_t)n_parts + 3u) & ~(size_t)3u; // 16-byte aligned sub-arrays (k_flatten_scan uses 128-bit accesses)
         uint32_t *part_count = part_mem, *part_dst = part_mem + np4, *tag_off = part_mem + 2 * np4, *work = part_mem + 34 * np4;
@@ -1281,11 +1284,14 @@ extern "C" void vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, co
             k_flatten_lean<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work, part_base,
                                                         part_end);
             k_flatten<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work);
+            launches += 2;
         }
         const uint32_t n_blocks = n_own ? (n_own + FS_THREADS * FS_PER_THREAD - 1u) / (FS_THREADS * FS_PER_THREAD) : 1u;
         k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(*cfg, n_own, part_count + part_base, part_dst + part_base, bump, ctrs + 4, n_blocks);
         k_flatten_place<<<(uint32_t)sm_count * 4u, FP_THREADS, 0, st>>>(*cfg, scene, ctx, part_dst, tag_off, path_bboxes, lines);
+        launches += 2;
     }
+    return launches;
 }
 extern "C" uint32_t vb_flatten_parts(uint32_t n_tag_words) { return (n_tag_words * 4u + 31u) / 32u; }
 // part_mem: part_count, part_dst (one word per partition each), tag_off (32), the work list of k_flatten (1); 16-byte aligned

@@ -166,8 +166,9 @@ k_path_count(VbConfig cfg, VbBump *bump, const VbLineSoup *__restrict__ lines, c
 
 // The seg_counts overflow check (the WGSL does it at the top of coarse) lives at the top of k_backdrop, the next kernel.
 
-extern "C" void vb_launch_path_count(const VbConfig *cfg, VbBump *bump, const VbLineSoup *lines, const VbPath *paths, VbTile *tile,
+extern "C" uint32_t vb_launch_path_count(const VbConfig *cfg, VbBump *bump, const VbLineSoup *lines, const VbPath *paths, VbTile *tile,
                                      VbSegmentCount *seg_counts, uint32_t grid, cudaStream_t st) {
-    if (grid == 0) return;
+    if (grid == 0) return 0;
     k_path_count<<<grid, PC_THREADS, 0, st>>>(*cfg, bump, lines, paths, tile, seg_counts);
+    return 1;
 }

@@ -132,9 +132,10 @@ k_path_tiling(VbConfig cfg, VbBump *bump, const VbSegmentCount *__restrict__ seg
     }
 }
 
-extern "C" void vb_launch_path_tiling(const VbConfig *cfg, VbBump *bump, const VbSegmentCount *seg_counts,
+extern "C" uint32_t vb_launch_path_tiling(const VbConfig *cfg, VbBump *bump, const VbSegmentCount *seg_counts,
                                       const VbLineSoup *lines, const VbPath *paths, const VbTile *tiles, VbSegment *segments,
                                       uint32_t grid, cudaStream_t st) {
-    if (grid == 0) return;
+    if (grid == 0) return 0;
     k_path_tiling<<<grid, PTI_THREADS, 0, st>>>(*cfg, bump, seg_counts, lines, paths, tiles, segments);
+    return 1;
 }

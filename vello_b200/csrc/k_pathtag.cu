@@ -96,9 +96,10 @@ k_pathtag_scan(VbConfig cfg, const uint32_t *__restrict__ scene, VbTagMonoid *__
     }
 }
 
-extern "C" void vb_launch_pathtag(const VbConfig *cfg, const uint32_t *scene, VbTagMonoid *tag_monoids, uint32_t *lb_mem,
+extern "C" uint32_t vb_launch_pathtag(const VbConfig *cfg, const uint32_t *scene, VbTagMonoid *tag_monoids, uint32_t *lb_mem,
                                   uint32_t n_parts, cudaStream_t st) {
-    if (n_parts == 0) return;
+    if (n_parts == 0) return 0;
     k_pathtag_scan<<<n_parts, PT_THREADS, 0, st>>>(*cfg, scene, tag_monoids, lb_mem, n_parts);
+    return 1;
 }
 extern "C" uint32_t vb_pathtag_parts(uint32_t n_tag_words) { return (n_tag_words + PT_PART - 1) / PT_PART; }

@@ -163,18 +163,20 @@ k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile 
     }
 }
 
-extern "C" void vb_launch_tile_alloc(const VbConfig *cfg, const uint32_t *scene, const VbBbox4 *draw_bboxes, VbBump *bump,
+extern "C" uint32_t vb_launch_tile_alloc(const VbConfig *cfg, const uint32_t *scene, const VbBbox4 *draw_bboxes, VbBump *bump,
                                      VbPath *paths, VbTile *tiles, uint32_t *lb_mem, uint32_t n_parts, int sm_count, cudaStream_t st) {
-    if (n_parts == 0) return;
+    if (n_parts == 0) return 0;
     k_tile_alloc<<<n_parts, TA_THREADS, 0, st>>>(*cfg, scene, draw_bboxes, bump, paths, tiles, lb_mem, n_parts);
     k_tile_zero<<<(uint32_t)sm_count * 4u, 256, 0, st>>>(*cfg, bump, tiles);
+    return 2;
 }
 extern "C" uint32_t vb_tile_alloc_parts(uint32_t n_draw) { return (n_draw + TA_THREADS - 1) / TA_THREADS; }
-extern "C" void vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, int sm_count, cudaStream_t st) {
+extern "C" uint32_t vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, int sm_count, cudaStream_t st) {
     uint32_t n = cfg->layout.n_draw_objects;
-    if (n == 0) return;
+    if (n == 0) return 0;
     const uint32_t groups = (n + BD_PATHS - 1) / BD_PATHS;
     uint32_t split = ((uint32_t)sm_count * 4u + groups - 1u) / groups;
     if (split > 64u) split = 64u;
     k_backdrop<<<dim3(groups, split), BD_THREADS, 0, st>>>(*cfg, bump, paths, tiles);
+    return 1;
 }

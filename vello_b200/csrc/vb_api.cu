@@ -6,47 +6,47 @@
 // bump-allocated arena is sized from the scene and grown + re-run when a frame overflows.
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 #include <string>
-#include <utility>
 #include <vector>
 
 #include "../../include/vello_b200.h"
 #include "vb_device.cuh"
 #include "vb_types.h"
 
-// ---- stage launchers (k_*.cu) --------------------------------------------------------------
+// ---- stage launchers (k_*.cu); each returns the number of kernels it launched -----------------------------------------------
 extern "C" {
-void vb_launch_pathtag(const VbConfig *, const uint32_t *, VbTagMonoid *, uint32_t *, uint32_t, cudaStream_t);
+uint32_t vb_launch_pathtag(const VbConfig *, const uint32_t *, VbTagMonoid *, uint32_t *, uint32_t, cudaStream_t);
 uint32_t vb_pathtag_parts(uint32_t);
-void vb_launch_flatten(const VbConfig *, const uint32_t *, const VbTagMonoid *, VbPathBbox *, VbBump *, VbLineSoup *, void *, void *, uint32_t *,
+uint32_t vb_launch_flatten(const VbConfig *, const uint32_t *, const VbTagMonoid *, VbPathBbox *, VbBump *, VbLineSoup *, void *, void *, uint32_t *,
                        uint32_t *, uint32_t, int, uint32_t, uint32_t, int, cudaStream_t);
 uint32_t vb_flatten_parts(uint32_t);
 size_t vb_flatten_part_words(uint32_t);
 void vb_flatten_arena_bytes(uint32_t, size_t *, size_t *);
-void vb_launch_draw(const VbConfig *, const uint32_t *, const VbPathBbox *, VbDrawMonoid *, uint32_t *, VbClipInp *, uint32_t *, uint32_t,
+uint32_t vb_launch_draw(const VbConfig *, const uint32_t *, const VbPathBbox *, VbDrawMonoid *, uint32_t *, VbClipInp *, uint32_t *, uint32_t,
                     cudaStream_t);
 uint32_t vb_draw_parts(uint32_t);
-void vb_launch_clip(uint32_t, const VbClipInp *, const VbPathBbox *, VbDrawMonoid *, VbBbox4 *, int32_t *, uint32_t *, cudaStream_t);
+uint32_t vb_launch_clip(uint32_t, const VbClipInp *, const VbPathBbox *, VbDrawMonoid *, VbBbox4 *, int32_t *, uint32_t *, cudaStream_t);
 uint32_t vb_clip_parts(uint32_t);
 size_t vb_clip_scratch_words(uint32_t);
-void vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathBbox *, const VbBbox4 *, VbBbox4 *, VbBump *, uint32_t *,
+uint32_t vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathBbox *, const VbBbox4 *, VbBbox4 *, VbBump *, uint32_t *,
                        VbBinHeader *, cudaStream_t);
-void vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
+uint32_t vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
                           cudaStream_t);
 uint32_t vb_tile_alloc_parts(uint32_t);
-void vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, int, cudaStream_t);
-void vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
+uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, int, cudaStream_t);
+uint32_t vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
                           cudaStream_t);
-void vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
+uint32_t vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
                       VbTile *, VbBump *, uint32_t *, uint32_t *, void *, uint32_t, cudaStream_t);
-void vb_launch_path_tiling(const VbConfig *, VbBump *, const VbSegmentCount *, const VbLineSoup *, const VbPath *, const VbTile *,
+uint32_t vb_launch_path_tiling(const VbConfig *, VbBump *, const VbSegmentCount *, const VbLineSoup *, const VbPath *, const VbTile *,
                            VbSegment *, uint32_t, cudaStream_t);
-void vb_launch_fine(const VbConfig *, int, const VbBump *, const VbSegment *, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *,
+uint32_t vb_launch_fine(const VbConfig *, int, const VbBump *, const VbSegment *, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *,
                     const uint32_t *, const uint8_t *, const uint32_t *, const uint32_t *, const uint32_t *, uint32_t, uint32_t *, const void *,
                     const uint32_t *, uint32_t, int, cudaStream_t);
 }
@@ -62,8 +62,8 @@ struct XPeersHost { // == XPeers in k_exchange.cu
 extern "C" size_t vb_exchange_half_bytes(uint32_t n_paths, uint32_t lines_cap);
 extern "C" size_t vb_exchange_peers_bytes(void);
 extern "C" uint32_t vb_exchange_epoch_word(void);
-extern "C" void vb_launch_exchange_send(const void *, VbBump *, uint32_t, VbLineSoup *, uint32_t *, VbPathBbox *, int, cudaStream_t);
-extern "C" void vb_launch_exchange_recv(const void *, VbBump *, uint32_t, VbLineSoup *, VbPathBbox *, int, cudaStream_t);
+extern "C" uint32_t vb_launch_exchange_send(const void *, VbBump *, uint32_t, VbLineSoup *, uint32_t *, VbPathBbox *, int, cudaStream_t);
+extern "C" uint32_t vb_launch_exchange_recv(const void *, VbBump *, uint32_t, VbLineSoup *, VbPathBbox *, int, cudaStream_t);
 extern "C" void vb_launch_resolve_finish(uint32_t *, uint32_t, uint32_t, uint32_t, uint32_t, const void *, uint32_t, cudaStream_t);
 extern "C" void vb_launch_make_ramps(const void *, const void *, uint32_t, uint32_t *, cudaStream_t);
 
@@ -130,9 +130,18 @@ struct DevBuf {
     size_t cap = 0; // bytes
 };
 
-// the seven bump-allocated arenas, by the names vb_debug_limit_arena takes
+// the seven bump-allocated arenas, in the order of VbConfig::lines_size .. ptcl_size (ARENAS below)
 enum { ARENA_LINES, ARENA_BINNING, ARENA_TILES, ARENA_SEG_COUNTS, ARENA_SEGMENTS, ARENA_BLEND, ARENA_PTCL, N_ARENAS };
-static const char *const ARENA_NAMES[N_ARENAS] = {"lines", "binning", "tiles", "seg_counts", "segments", "blend", "ptcl"};
+static_assert(offsetof(VbConfig, ptcl_size) - offsetof(VbConfig, lines_size) == (N_ARENAS - 1) * sizeof(uint32_t),
+              "VbConfig's arena sizes are consecutive words in ARENA_* order");
+
+// Where a frame's pixels go: a device pointer, or the renderer's own target (target_alt when `alt`), and optionally a copy of
+// the frame in host memory, read back in `bands` row bands while fine runs.
+struct Dest {
+    void *dev = nullptr, *host = nullptr;
+    bool alt = false;
+    uint32_t bands = 1;
+};
 
 // key of a captured frame: everything a launch argument is derived from (see enqueue)
 struct GraphKey {
@@ -157,29 +166,34 @@ struct vb_renderer {
     std::string err;
     int sm_count = 132;
 
-    // scene
-    bool have_scene = false;
-    VbLayout layout{};
-    size_t scene_words = 0;
-    uint32_t n_ramps = 0, atlas_w = 0, atlas_h = 0;
-    DevBuf scene, ramps, atlas, mask8, mask16;
+    // Streaming (vb_render_begin) keeps TWO frames in flight: while frame k is rasterised, frame k+1's scene is uploaded
+    // into the other slot on its own stream and frame k-1's pixels drain to the host. `cur` is the slot frames render from.
+    struct SceneSlot {
+        bool have_scene = false;
+        VbLayout layout{};
+        size_t scene_words = 0;
+        uint32_t n_ramps = 0, atlas_w = 0, atlas_h = 0;
+        DevBuf scene, ramps, atlas;
+        VbBump *h_bump = nullptr;     // pinned + mapped: the device writes the counters straight into host memory
+        VbBump *h_bump_dev = nullptr; // device-side address of h_bump
+    } slot[2];
+    SceneSlot *cur = slot;
+    DevBuf mask8, mask16;
 
     // fixed-size intermediates
     DevBuf tag_monoids, path_bboxes, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
         ctl, target, target_alt, tile_start, cls_list;
-    // bump arenas (capacities in elements live in cap_*)
+    // bump arenas (ARENAS), capacities in elements
     DevBuf resolve_tmp; // patches, ramp descriptors and stops of vb_scene_upload_streams
     DevBuf lines, line_scratch, flatten_jobs, flatten_parts, tiles, seg_counts, segments, ptcl, blend_spill;
-    uint32_t cap_lines = 0, cap_binning = 0, cap_tiles = 0, cap_seg_counts = 0, cap_segments = 0, cap_blend = 0, cap_ptcl = 0;
-    // test-only capacity limits (vb_debug_limit_arena), in the order of ARENA_NAMES; UINT32_MAX = none
-    uint32_t arena_limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
+    uint32_t cap[N_ARENAS] = {};
+    // test-only capacity limits (vb_debug_limit_arena); UINT32_MAX = none
+    uint32_t limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
 
     // per-frame
     VbConfig cfg{};
     vb_params params{};
-    void *out_dev = nullptr;
-    VbBump *h_bump = nullptr;   // pinned + mapped: the device writes the counters straight into host memory
-    VbBump *h_bump_dev = nullptr; // device-side address of h_bump
+    Dest dest; // of the frame frame_prepare set up
     uint32_t retries = 0, launches = 0;
     size_t ctl_words = 0;
     bool use_graph = true;        // replay whole frames as CUDA graphs (see enqueue)
@@ -196,28 +210,12 @@ struct vb_renderer {
     // read-back pipeline of vb_render (host output): fine runs in row bands, each band's D2H copy overlaps the next band
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t band_ev[8]{};
-    void *host_out = nullptr; // set by vb_render for the duration of one frame
     // streaming read-back (vb_render_begin): frames alternate between two targets so that the copy of frame n can
     // still be draining while frame n+1 is rasterised
-    bool use_alt = false, stream_pending = false;
-    uint32_t stream_parity = 0;
+    bool stream_pending = false;
     cudaEvent_t copy_done[3]{};
     bool frame_pending = false;
-    bool zero_fine_queue = false; // set by vb_run_stages (see enqueue_direct)
-    bool in_stream_call = false;  // inside vb_render_begin / vb_readback_wait (their internal calls must not drain)
 
-    // Streaming (vb_render_begin) keeps TWO frames in flight: while frame k is rasterised, frame k+1's scene is uploaded
-    // into the other slot on its own stream and frame k-1's pixels drain to the host. The members above (scene, ramps,
-    // atlas, layout, ..., h_bump) are the CURRENT slot; `other` holds the parked one and swap_slot() exchanges them.
-    struct SceneSlot {
-        DevBuf scene, ramps, atlas;
-        VbLayout layout{};
-        size_t scene_words = 0;
-        uint32_t n_ramps = 0, atlas_w = 0, atlas_h = 0;
-        bool have_scene = false;
-        VbBump *h_bump = nullptr, *h_bump_dev = nullptr;
-    } other;
-    uint32_t cur_slot = 0;
     cudaStream_t upload_stream = nullptr;
     cudaEvent_t upload_done[2]{}, raster_done[2]{};
     struct RingFrame { // a streamed frame between vb_render_begin and its completion on the host
@@ -240,22 +238,18 @@ struct vb_renderer {
     } xc;
 };
 
-static void swap_slot(vb_renderer *r) {
-    std::swap(r->scene, r->other.scene);
-    std::swap(r->ramps, r->other.ramps);
-    std::swap(r->atlas, r->other.atlas);
-    std::swap(r->layout, r->other.layout);
-    std::swap(r->scene_words, r->other.scene_words);
-    std::swap(r->n_ramps, r->other.n_ramps);
-    std::swap(r->atlas_w, r->other.atlas_w);
-    std::swap(r->atlas_h, r->other.atlas_h);
-    std::swap(r->have_scene, r->other.have_scene);
-    std::swap(r->h_bump, r->other.h_bump);
-    std::swap(r->h_bump_dev, r->other.h_bump_dev);
-    r->cur_slot ^= 1u;
-}
-static void select_slot(vb_renderer *r, uint32_t slot) {
-    if (r->cur_slot != slot) swap_slot(r);
+// Every device buffer the renderer owns, each once. `keyed` marks what the launches of a frame read: the current scene slot's
+// inputs and the intermediates, whose addresses are part of a captured frame's key (graph_key). The frame's destination is
+// keyed by itself; the parked scene slot, the targets, resolve_tmp and the exchange arena are not launch arguments.
+template <class F> static void for_each_buf(vb_renderer *r, F f) {
+    vb_renderer::SceneSlot &s = *r->cur, &o = r->slot[r->cur == r->slot ? 1 : 0];
+    DevBuf *const keyed[] = {&s.scene, &s.ramps, &s.atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
+                             &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers,
+                             &r->paths, &r->ctl, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs,
+                             &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
+    DevBuf *const unkeyed[] = {&o.scene, &o.ramps, &o.atlas, &r->target, &r->target_alt, &r->resolve_tmp, &r->xc.arena};
+    for (DevBuf *b : keyed) f(*b, true);
+    for (DevBuf *b : unkeyed) f(*b, false);
 }
 
 #define CK(call)                                                                                  \
@@ -278,13 +272,50 @@ static int ensure(vb_renderer *r, DevBuf &b, size_t bytes) {
     b.cap = want;
     return VB_OK;
 }
-static size_t arena_bytes(const vb_renderer *r) {
-    const DevBuf *all[] = {&r->scene, &r->ramps, &r->atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
-                           &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths,
-                           &r->ctl, &r->target, &r->target_alt, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
-    size_t s = r->other.scene.cap + r->other.ramps.cap + r->other.atlas.cap;
-    for (auto b : all) s += b->cap;
-    return s;
+// One entry per bump arena: the name vb_debug_limit_arena takes, the buffer, its element size and its VbBump counter.
+// The special cases are in arena_offset, arena_need, ensure_arena and the first guesses of prepare.
+using RendererBuf = DevBuf vb_renderer::*;
+using BumpCounter = uint32_t VbBump::*;
+struct ArenaDesc {
+    const char *name;
+    const char *download; // vb_debug_download's name of the buffer when it differs from the arena's
+    RendererBuf buf;
+    size_t elem_bytes;
+    BumpCounter counter;
+};
+static const ArenaDesc ARENAS[N_ARENAS] = {
+    {"lines", nullptr, &vb_renderer::lines, sizeof(VbLineSoup), &VbBump::lines},
+    {"binning", "info_bin_data", &vb_renderer::info_bin_data, 4, &VbBump::binning},
+    {"tiles", nullptr, &vb_renderer::tiles, sizeof(VbTile), &VbBump::tile},
+    {"seg_counts", nullptr, &vb_renderer::seg_counts, sizeof(VbSegmentCount), &VbBump::seg_counts},
+    {"segments", nullptr, &vb_renderer::segments, sizeof(VbSegment), &VbBump::segments},
+    {"blend", "blend_spill", &vb_renderer::blend_spill, 4, &VbBump::blend},
+    {"ptcl", nullptr, &vb_renderer::ptcl, 4, &VbBump::ptcl},
+};
+static int arena_index(const char *name) {
+    for (int a = 0; a < N_ARENAS; a++)
+        if (!strcmp(name, ARENAS[a].name)) return a;
+    return -1;
+}
+// ptcl starts with a static command area of VB_PTCL_INITIAL_ALLOC words per tile; its capacity includes it, bump.ptcl does not
+static uint64_t ptcl_static(const VbConfig &c) { return (uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC; }
+// elements of the arena's buffer in front of the arena: binning lives after the draw info in info_bin_data
+static size_t arena_offset(const vb_renderer *r, int a) { return a == ARENA_BINNING ? r->cur->layout.bin_data_start : 0; }
+// what the last attempt asked of an arena, in the units of its capacity
+static uint64_t arena_need(const vb_renderer *r, int a) {
+    const uint64_t n = r->cur->h_bump->*ARENAS[a].counter;
+    return a == ARENA_PTCL ? ptcl_static(r->cfg) + n : n;
+}
+// Allocate arena a for its capacity. ptcl gets 512 bytes of slack for fine's 256-byte command windows; the lines capacity
+// also sizes flatten's scratch arenas.
+static int ensure_arena(vb_renderer *r, int a) {
+    const ArenaDesc &d = ARENAS[a];
+    int rc = ensure(r, r->*d.buf, (arena_offset(r, a) + r->cap[a]) * d.elem_bytes + (a == ARENA_PTCL ? 512 : 0));
+    if (rc || a != ARENA_LINES) return rc;
+    size_t lit_bytes, job_bytes;
+    vb_flatten_arena_bytes(r->cap[a], &lit_bytes, &job_bytes);
+    if ((rc = ensure(r, r->line_scratch, lit_bytes))) return rc;
+    return ensure(r, r->flatten_jobs, job_bytes);
 }
 
 // mask LUTs: vello_encoding/src/mask.rs:10-98 (f64 maths like the reference)
@@ -329,19 +360,18 @@ extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, r->device) == cudaSuccess) r->sm_count = prop.multiProcessorCount;
     if (cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaHostAlloc((void **)&r->h_bump, sizeof(VbBump), cudaHostAllocMapped) != cudaSuccess ||
-        cudaHostGetDevicePointer((void **)&r->h_bump_dev, r->h_bump, 0) != cudaSuccess) {
-        delete r;
-        return VB_E_CUDA;
-    }
-    memset(r->h_bump, 0, sizeof(VbBump));
-    if (cudaHostAlloc((void **)&r->other.h_bump, sizeof(VbBump), cudaHostAllocMapped) != cudaSuccess ||
-        cudaHostGetDevicePointer((void **)&r->other.h_bump_dev, r->other.h_bump, 0) != cudaSuccess ||
         cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess) {
         delete r;
         return VB_E_CUDA;
     }
-    memset(r->other.h_bump, 0, sizeof(VbBump));
+    for (auto &s : r->slot) {
+        if (cudaHostAlloc((void **)&s.h_bump, sizeof(VbBump), cudaHostAllocMapped) != cudaSuccess ||
+            cudaHostGetDevicePointer((void **)&s.h_bump_dev, s.h_bump, 0) != cudaSuccess) {
+            delete r;
+            return VB_E_CUDA;
+        }
+        memset(s.h_bump, 0, sizeof(VbBump));
+    }
     for (auto &ev : r->upload_done) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
     for (auto &ev : r->raster_done) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
     for (auto &ev : r->ev) cudaEventCreate(&ev);
@@ -374,15 +404,11 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
     if (!r) return;
     cudaSetDevice(r->device);
     if (r->stream) cudaStreamSynchronize(r->stream);
-    DevBuf *all[] = {&r->scene, &r->ramps, &r->atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
-                     &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths,
-                     &r->ctl, &r->target, &r->target_alt, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
-    for (auto b : all)
-        if (b->p) cudaFree(b->p);
-    for (DevBuf *b : {&r->other.scene, &r->other.ramps, &r->other.atlas, &r->resolve_tmp, &r->xc.arena})
-        if (b->p) cudaFree(b->p);
-    if (r->h_bump) cudaFreeHost(r->h_bump);
-    if (r->other.h_bump) cudaFreeHost(r->other.h_bump);
+    for_each_buf(r, [](DevBuf &b, bool) {
+        if (b.p) cudaFree(b.p);
+    });
+    for (auto &s : r->slot)
+        if (s.h_bump) cudaFreeHost(s.h_bump);
     if (r->ev_ok) {
         for (auto &ev : r->ev) cudaEventDestroy(ev);
         for (auto &ev : r->frame_ev) cudaEventDestroy(ev);
@@ -430,27 +456,27 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
     if (!r || !layout || (scene_len && !scene) || (scene_len & 3)) return VB_E_INVALID;
     if (ramp_h && ramp_w != 512) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
-    memcpy(&r->layout, layout, sizeof(VbLayout));
-    r->scene_words = scene_len / 4;
+    memcpy(&r->cur->layout, layout, sizeof(VbLayout));
+    r->cur->scene_words = scene_len / 4;
     int rc;
-    if ((rc = ensure(r, r->scene, scene_len + 64))) return rc;
-    if (scene_len) CK(cudaMemcpyAsync(r->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
-    r->n_ramps = ramp_h;
-    if ((rc = ensure(r, r->ramps, (size_t)ramp_h * 512 * 4))) return rc;
-    if (ramp_h) CK(cudaMemcpyAsync(r->ramps.p, ramps, (size_t)ramp_h * 512 * 4, cudaMemcpyHostToDevice, st));
-    r->atlas_w = atlas ? atlas_w : 0;
-    r->atlas_h = atlas ? atlas_h : 0;
-    if ((rc = ensure(r, r->atlas, (size_t)r->atlas_w * r->atlas_h * 4))) return rc;
-    if (r->atlas_w && r->atlas_h)
-        CK(cudaMemcpyAsync(r->atlas.p, atlas, (size_t)r->atlas_w * r->atlas_h * 4, cudaMemcpyHostToDevice, st));
-    r->have_scene = true;
+    if ((rc = ensure(r, r->cur->scene, scene_len + 64))) return rc;
+    if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
+    r->cur->n_ramps = ramp_h;
+    if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
+    if (ramp_h) CK(cudaMemcpyAsync(r->cur->ramps.p, ramps, (size_t)ramp_h * 512 * 4, cudaMemcpyHostToDevice, st));
+    r->cur->atlas_w = atlas ? atlas_w : 0;
+    r->cur->atlas_h = atlas ? atlas_h : 0;
+    if ((rc = ensure(r, r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4))) return rc;
+    if (r->cur->atlas_w && r->cur->atlas_h)
+        CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4, cudaMemcpyHostToDevice, st));
+    r->cur->have_scene = true;
     return VB_OK;
 }
 
 extern "C" int vb_readback_wait(vb_renderer *r);
 // A non-streaming entry point used while streamed frames are still in flight completes them first.
 static int drain_stream(vb_renderer *r) {
-    if (r->stream_pending && !r->in_stream_call) return vb_readback_wait(r);
+    if (r->stream_pending) return vb_readback_wait(r);
     return VB_OK;
 }
 
@@ -488,7 +514,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.target_width = p->width;
     c.target_height = p->height;
     c.base_color = p->base_color;
-    c.layout = r->layout;
+    c.layout = r->cur->layout;
     const uint32_t hb = (c.height_in_tiles + 15u) / 16u, wb = (c.width_in_tiles + 15u) / 16u;
     c.win_by0 = 0;
     c.win_by1 = hb;
@@ -507,16 +533,16 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         c.win_by1 = (c.win_ty1 + 15u) / 16u;
     }
     c.win_cull = (c.win_ty0 > 0u || c.win_ty1 < c.height_in_tiles) ? 1u : 0u;
-    c.n_tag_words = r->layout.path_data_base - r->layout.path_tag_base;
-    c.scene_words = (uint32_t)r->scene_words;
-    c.n_ramps = r->n_ramps;
-    c.atlas_w = r->atlas_w;
-    c.atlas_h = r->atlas_h;
+    c.n_tag_words = r->cur->layout.path_data_base - r->cur->layout.path_tag_base;
+    c.scene_words = (uint32_t)r->cur->scene_words;
+    c.n_ramps = r->cur->n_ramps;
+    c.atlas_w = r->cur->atlas_w;
+    c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
     r->params = *p;
 
-    const VbLayout &L = r->layout;
+    const VbLayout &L = r->cur->layout;
     const uint32_t n_draw = L.n_draw_objects, n_paths = L.n_paths, n_clips = L.n_clips;
     const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles;
     const uint32_t n_bins = wb * hb, aligned_n_bins = (n_bins + 255u) & ~255u;
@@ -533,43 +559,17 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     if ((rc = ensure(r, r->tile_start, ((size_t)n_tiles + 256) * 4))) return rc;
     if ((rc = ensure(r, r->cls_list, (size_t)VB_FINE_CLASSES * n_tiles * 8))) return rc; // fine's cost-ordered tile lists
 
-    // first-guess arena capacities (elements); they only ever grow
-    const uint32_t n_tags = c.n_tag_words * 4u;
-    auto atleast = [](uint32_t &cap, uint64_t v) {
-        if (v > 0xfffffff0ull) v = 0xfffffff0ull;
-        if (cap < (uint32_t)v) cap = (uint32_t)v;
-    };
-    atleast(r->cap_lines, (uint64_t)n_tags * 2 + 4096);
-    atleast(r->cap_binning, (uint64_t)n_draw * 4 + 4096);
-    atleast(r->cap_tiles, (uint64_t)n_draw * 16 + 4096);
-    atleast(r->cap_seg_counts, (uint64_t)r->cap_lines * 2);
-    atleast(r->cap_segments, (uint64_t)r->cap_seg_counts);
-    atleast(r->cap_blend, 256);
-    atleast(r->cap_ptcl, (uint64_t)n_tiles * VB_PTCL_INITIAL_ALLOC + (uint64_t)VB_PTCL_INCREMENT * (64 + n_tiles / 8));
-    if (r->cap_ptcl < n_tiles * VB_PTCL_INITIAL_ALLOC + VB_PTCL_INCREMENT)
-        r->cap_ptcl = n_tiles * VB_PTCL_INITIAL_ALLOC + VB_PTCL_INCREMENT;
-    if ((rc = ensure(r, r->lines, (size_t)r->cap_lines * sizeof(VbLineSoup)))) return rc;
-    {
-        size_t lit_bytes, job_bytes;
-        vb_flatten_arena_bytes(r->cap_lines, &lit_bytes, &job_bytes);
-        if ((rc = ensure(r, r->line_scratch, lit_bytes))) return rc;
-        if ((rc = ensure(r, r->flatten_jobs, job_bytes))) return rc;
+    // arena capacities (elements) start at a first guess and only ever grow; seg_counts and segments follow the capacities
+    // before them. A test-only limit lowers the capacity the kernels see, never the allocation (vb_debug_limit_arena).
+    const uint64_t guess[N_ARENAS] = {(uint64_t)(c.n_tag_words * 4u) * 2 + 4096, (uint64_t)n_draw * 4 + 4096, (uint64_t)n_draw * 16 + 4096,
+                                      0, 0, 256, ptcl_static(c) + (uint64_t)VB_PTCL_INCREMENT * (64 + n_tiles / 8)};
+    uint32_t *size = &c.lines_size;
+    for (int a = 0; a < N_ARENAS; a++) {
+        const uint64_t g = a == ARENA_SEG_COUNTS ? (uint64_t)r->cap[ARENA_LINES] * 2 : a == ARENA_SEGMENTS ? r->cap[ARENA_SEG_COUNTS] : guess[a];
+        r->cap[a] = (uint32_t)std::max<uint64_t>(r->cap[a], std::min<uint64_t>(g, 0xfffffff0ull));
+        if ((rc = ensure_arena(r, a))) return rc;
+        size[a] = std::min(r->cap[a], r->limit[a]);
     }
-    if ((rc = ensure(r, r->info_bin_data, ((size_t)L.bin_data_start + r->cap_binning) * 4))) return rc;
-    if ((rc = ensure(r, r->tiles, (size_t)r->cap_tiles * sizeof(VbTile)))) return rc;
-    if ((rc = ensure(r, r->seg_counts, (size_t)r->cap_seg_counts * sizeof(VbSegmentCount)))) return rc;
-    if ((rc = ensure(r, r->segments, (size_t)r->cap_segments * sizeof(VbSegment)))) return rc;
-    if ((rc = ensure(r, r->blend_spill, (size_t)r->cap_blend * 4))) return rc;
-    if ((rc = ensure(r, r->ptcl, (size_t)r->cap_ptcl * 4 + 512))) return rc; // + slack for fine's 256-byte command windows
-    // a test-only limit lowers the capacity the kernels see, never the allocation (vb_debug_limit_arena)
-    const uint32_t *lim = r->arena_limit;
-    c.lines_size = std::min(r->cap_lines, lim[ARENA_LINES]);
-    c.binning_size = std::min(r->cap_binning, lim[ARENA_BINNING]);
-    c.tiles_size = std::min(r->cap_tiles, lim[ARENA_TILES]);
-    c.seg_counts_size = std::min(r->cap_seg_counts, lim[ARENA_SEG_COUNTS]);
-    c.segments_size = std::min(r->cap_segments, lim[ARENA_SEGMENTS]);
-    c.blend_size = std::min(r->cap_blend, lim[ARENA_BLEND]);
-    c.ptcl_size = std::min(r->cap_ptcl, lim[ARENA_PTCL]);
 
     // control block: [bump (8 words, padded to 16)] [look-back states]
     r->parts_pathtag = vb_pathtag_parts(c.n_tag_words);
@@ -600,14 +600,36 @@ static void rec(vb_renderer *r, int i) {
     if (r->timing) cudaEventRecord(r->ev[i], r->stream);
 }
 
-// Enqueue stages first..last. Does not synchronise.
-static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
+// path_count and path_tiling: the grid comes from the arena capacity, the kernels stride over the count read on the device
+static uint32_t capacity_grid(uint32_t cap, int sm_count) {
+    const uint64_t blocks = ((uint64_t)cap + 255) / 256;
+    return (uint32_t)std::min<uint64_t>(blocks, (uint64_t)sm_count * 16);
+}
+
+// Queue the copy of tile rows ty0..ty1 of the frame to d.host on the copy stream, behind everything on the renderer's stream.
+static int queue_readback(vb_renderer *r, const VbConfig &c, uint32_t ty0, uint32_t ty1, const Dest &d, uint32_t band) {
+    size_t y0 = (size_t)ty0 * 16u, y1 = (size_t)ty1 * 16u;
+    if (y1 > c.target_height) y1 = c.target_height;
+    if (y1 <= y0) return VB_OK;
+    const size_t off = (y0 - c.out_row0) * c.out_pitch_px * 4u, bytes = (y1 - y0) * c.out_pitch_px * 4u;
+    CK(cudaEventRecord(r->band_ev[band], r->stream));
+    CK(cudaStreamWaitEvent(r->copy_stream, r->band_ev[band], 0));
+    CK(cudaMemcpyAsync((char *)d.host + off, (const char *)d.dev + off, bytes, cudaMemcpyDeviceToHost, r->copy_stream));
+    return VB_OK;
+}
+
+// Enqueue stages first..last into d.dev (and d.host). Does not synchronise. `clear_queues` (vb_run_stages): a range that
+// starts after stage 0 does not zero the control block, but fine's tile queues must start at 0 and coarse must append to
+// empty class lists.
+static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bool clear_queues) {
     const VbConfig &c = r->cfg;
     cudaStream_t st = r->stream;
     uint32_t *ctl = (uint32_t *)r->ctl.p;
     VbBump *bump = (VbBump *)ctl;
     uint32_t launches = 0;
-    const uint32_t n_draw = c.layout.n_draw_objects;
+    int rc;
+    XPeersHost X; // multi-GPU exchange
+    if (r->xc.enabled) xpeers_of(r, &X);
     if (first == 0) {
         // a kernel, not cudaMemsetAsync: small memsets / copies are served by a copy engine and would queue behind a
         // 64 MiB read-back still draining from the previous frame
@@ -617,9 +639,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
                                                              xepoch);
         launches++;
     }
-    else if (r->zero_fine_queue) {
-        // vb_run_stages starting after stage 0: the control block is not zeroed, but fine's tile queues must start at 0 and
-        // coarse must append to empty class lists
+    else if (clear_queues) {
         if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(ctl + VB_CTL_FINE_QUEUE, 0, 8 * sizeof(uint32_t), st));
         if (first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_COARSE)
             CK(cudaMemsetAsync(ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_CLASSES * sizeof(uint32_t), st));
@@ -628,117 +648,85 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
     for (int s = first; s <= last; s++) {
         switch (s) {
         case VB_STAGE_ID_PATHTAG:
-            vb_launch_pathtag(&c, (const uint32_t *)r->scene.p, (VbTagMonoid *)r->tag_monoids.p, ctl + r->off_lb_pathtag, r->parts_pathtag, st);
-            launches += r->parts_pathtag ? 1 : 0;
+            launches += vb_launch_pathtag(&c, (const uint32_t *)r->cur->scene.p, (VbTagMonoid *)r->tag_monoids.p, ctl + r->off_lb_pathtag,
+                                          r->parts_pathtag, st);
             break;
-        case VB_STAGE_ID_FLATTEN:
+        case VB_STAGE_ID_FLATTEN: {
+            // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
+            // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
+            VbConfig cf = c;
+            uint32_t p0 = 0u, p1 = r->parts_flatten;
             if (r->xc.enabled) {
-                // this GPU flattens its share of the tag stream (no stripe culling: the lines are for everybody), then the
-                // lines and path boxes are exchanged through peer memory (k_exchange.cu)
-                VbConfig cx = c;
-                cx.win_cull = 0u;
+                cf.win_cull = 0u;
                 const uint32_t P = r->parts_flatten, G = r->xc.world, k = r->xc.rank;
-                const uint32_t p0 = (uint32_t)((uint64_t)P * k / G) & ~7u;
-                const uint32_t p1 = k + 1u == G ? P : ((uint32_t)((uint64_t)P * (k + 1u) / G) & ~7u);
-                vb_launch_flatten(&cx, (const uint32_t *)r->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p, bump,
-                                  (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
-                                  ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, p0, p1, r->sm_count, st);
-                XPeersHost X;
-                xpeers_of(r, &X);
-                vb_launch_exchange_send(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, ctl + VB_CTL_XCHG_SCRATCH,
-                                        (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
-                launches += (r->parts_flatten ? 4 : 0) + 4;
-                break;
+                p0 = (uint32_t)((uint64_t)P * k / G) & ~7u;
+                p1 = k + 1u == G ? P : ((uint32_t)((uint64_t)P * (k + 1u) / G) & ~7u);
             }
-            vb_launch_flatten(&c, (const uint32_t *)r->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p, bump,
-                              (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
-                              ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, 0u, r->parts_flatten, r->sm_count, st);
-            launches += (first != 0 && c.layout.n_paths ? 1 : 0) + (r->parts_flatten ? 4 : 0);
+            launches += vb_launch_flatten(&cf, (const uint32_t *)r->cur->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p,
+                                          bump, (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
+                                          ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, p0, p1, r->sm_count, st);
+            if (r->xc.enabled)
+                launches += vb_launch_exchange_send(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, ctl + VB_CTL_XCHG_SCRATCH,
+                                                    (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
             break;
+        }
         case VB_STAGE_ID_DRAW:
-            if (r->xc.enabled) { // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
-                XPeersHost X;
-                xpeers_of(r, &X);
-                vb_launch_exchange_recv(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
-                launches += 3;
-            }
-            vb_launch_draw(&c, (const uint32_t *)r->scene.p, (const VbPathBbox *)r->path_bboxes.p, (VbDrawMonoid *)r->draw_monoids.p,
-                           (uint32_t *)r->info_bin_data.p, (VbClipInp *)r->clip_inp.p, ctl + r->off_lb_draw, r->parts_draw, st);
-            launches += r->parts_draw ? 1 : 0;
+            if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
+                launches += vb_launch_exchange_recv(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
+            launches += vb_launch_draw(&c, (const uint32_t *)r->cur->scene.p, (const VbPathBbox *)r->path_bboxes.p, (VbDrawMonoid *)r->draw_monoids.p,
+                                       (uint32_t *)r->info_bin_data.p, (VbClipInp *)r->clip_inp.p, ctl + r->off_lb_draw, r->parts_draw, st);
             break;
         case VB_STAGE_ID_CLIP:
-            vb_launch_clip(c.layout.n_clips, (const VbClipInp *)r->clip_inp.p, (const VbPathBbox *)r->path_bboxes.p,
-                           (VbDrawMonoid *)r->draw_monoids.p, (VbBbox4 *)r->clip_bboxes.p, (int32_t *)r->clip_scratch.p,
-                           ctl + r->off_lb_clip, st);
-            launches += c.layout.n_clips ? 3 : 0;
+            launches += vb_launch_clip(c.layout.n_clips, (const VbClipInp *)r->clip_inp.p, (const VbPathBbox *)r->path_bboxes.p,
+                                       (VbDrawMonoid *)r->draw_monoids.p, (VbBbox4 *)r->clip_bboxes.p, (int32_t *)r->clip_scratch.p,
+                                       ctl + r->off_lb_clip, st);
             break;
         case VB_STAGE_ID_BINNING:
-            vb_launch_binning(&c, (const VbDrawMonoid *)r->draw_monoids.p, (const VbPathBbox *)r->path_bboxes.p,
-                              (const VbBbox4 *)r->clip_bboxes.p, (VbBbox4 *)r->draw_bboxes.p, bump, (uint32_t *)r->info_bin_data.p,
-                              (VbBinHeader *)r->bin_headers.p, st);
-            launches += n_draw ? 1 : 0;
+            launches += vb_launch_binning(&c, (const VbDrawMonoid *)r->draw_monoids.p, (const VbPathBbox *)r->path_bboxes.p,
+                                          (const VbBbox4 *)r->clip_bboxes.p, (VbBbox4 *)r->draw_bboxes.p, bump, (uint32_t *)r->info_bin_data.p,
+                                          (VbBinHeader *)r->bin_headers.p, st);
             break;
         case VB_STAGE_ID_TILE_ALLOC:
-            vb_launch_tile_alloc(&c, (const uint32_t *)r->scene.p, (const VbBbox4 *)r->draw_bboxes.p, bump, (VbPath *)r->paths.p,
-                                 (VbTile *)r->tiles.p, ctl + r->off_lb_tile, r->parts_tile, r->sm_count, st);
-            launches += r->parts_tile ? 2 : 0;
+            launches += vb_launch_tile_alloc(&c, (const uint32_t *)r->cur->scene.p, (const VbBbox4 *)r->draw_bboxes.p, bump, (VbPath *)r->paths.p,
+                                             (VbTile *)r->tiles.p, ctl + r->off_lb_tile, r->parts_tile, r->sm_count, st);
             break;
-        case VB_STAGE_ID_PATH_COUNT: {
-            // grid from the arena capacity; the kernel strides over bump.lines read on the device
-            uint64_t blocks = ((uint64_t)c.lines_size + 255) / 256;
-            uint32_t grid = (uint32_t)(blocks < (uint64_t)r->sm_count * 16 ? blocks : (uint64_t)r->sm_count * 16);
-            vb_launch_path_count(&c, bump, (const VbLineSoup *)r->lines.p, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p,
-                                 (VbSegmentCount *)r->seg_counts.p, grid, st);
-            launches += 1;
+        case VB_STAGE_ID_PATH_COUNT:
+            launches += vb_launch_path_count(&c, bump, (const VbLineSoup *)r->lines.p, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p,
+                                             (VbSegmentCount *)r->seg_counts.p, capacity_grid(c.lines_size, r->sm_count), st);
             break;
-        }
         case VB_STAGE_ID_BACKDROP:
-            vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, r->sm_count, st);
-            launches += n_draw ? 1 : 0;
+            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, r->sm_count, st);
             break;
         case VB_STAGE_ID_COARSE:
-            vb_launch_coarse(&c, (const uint32_t *)r->scene.p, (const VbDrawMonoid *)r->draw_monoids.p, (const VbBinHeader *)r->bin_headers.p,
-                             (const uint32_t *)r->info_bin_data.p, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, bump,
-                             (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p, c.width_in_tiles * c.height_in_tiles, st);
-            launches += 1;
+            launches += vb_launch_coarse(&c, (const uint32_t *)r->cur->scene.p, (const VbDrawMonoid *)r->draw_monoids.p,
+                                         (const VbBinHeader *)r->bin_headers.p, (const uint32_t *)r->info_bin_data.p, (const VbPath *)r->paths.p,
+                                         (VbTile *)r->tiles.p, bump, (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p,
+                                         c.width_in_tiles * c.height_in_tiles, st);
             break;
-        case VB_STAGE_ID_PATH_TILING: {
-            uint64_t blocks = ((uint64_t)c.seg_counts_size + 255) / 256;
-            uint32_t grid = (uint32_t)(blocks < (uint64_t)r->sm_count * 16 ? blocks : (uint64_t)r->sm_count * 16);
-            vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
-                                  (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p, grid, st);
-            launches += 1;
+        case VB_STAGE_ID_PATH_TILING:
+            launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
+                                              (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p,
+                                              capacity_grid(c.seg_counts_size, r->sm_count), st);
             break;
-        }
         case VB_STAGE_ID_FINE: {
             // With a host destination (vb_render) fine is launched in up to 8 bands of tile rows and each band's
             // device->host copy is queued on a second stream behind an event, so the read-back of band k overlaps
             // the rasterisation of band k+1 (only the last band's copy is exposed).
             const uint32_t rows = c.win_ty1 - c.win_ty0;
-            uint32_t n_bands = (r->host_out && rows >= 64u) ? r->readback_bands : 1u;
+            uint32_t n_bands = (d.host && rows >= 64u) ? d.bands : 1u;
             const uint32_t band_rows = (rows + n_bands - 1u) / n_bands;
             for (uint32_t b = 0; b < n_bands; b++) {
                 VbConfig cb = c;
                 cb.win_ty0 = c.win_ty0 + b * band_rows;
                 cb.win_ty1 = cb.win_ty0 + band_rows < c.win_ty1 ? cb.win_ty0 + band_rows : c.win_ty1;
                 if (cb.win_ty0 >= cb.win_ty1) break;
-                vb_launch_fine(&cb, (int)r->params.aa, bump, (const VbSegment *)r->segments.p, (const uint32_t *)r->ptcl.p,
-                               (const uint32_t *)r->info_bin_data.p, (uint32_t *)r->blend_spill.p, (uint32_t *)out_dev,
-                               (const uint32_t *)r->ramps.p, (const uint8_t *)r->atlas.p, (const uint32_t *)r->mask8.p,
-                               (const uint32_t *)r->mask16.p, (const uint32_t *)r->tile_start.p, r->occlusion_cull,
-                               ctl + VB_CTL_FINE_QUEUE + b, r->cls_list.p, n_bands == 1u ? ctl + VB_CTL_FINE_CLASS : nullptr,
-                               c.width_in_tiles * c.height_in_tiles, r->sm_count, st);
-                launches += 1;
-                if (r->host_out) {
-                    size_t y0 = (size_t)cb.win_ty0 * 16u, y1 = (size_t)cb.win_ty1 * 16u;
-                    if (y1 > c.target_height) y1 = c.target_height;
-                    if (y1 > y0) {
-                        const size_t off = (y0 - c.out_row0) * c.out_pitch_px * 4u, bytes = (y1 - y0) * c.out_pitch_px * 4u;
-                        CK(cudaEventRecord(r->band_ev[b], st));
-                        CK(cudaStreamWaitEvent(r->copy_stream, r->band_ev[b], 0));
-                        CK(cudaMemcpyAsync((char *)r->host_out + off, (const char *)out_dev + off, bytes, cudaMemcpyDeviceToHost, r->copy_stream));
-                    }
-                }
+                launches += vb_launch_fine(&cb, (int)r->params.aa, bump, (const VbSegment *)r->segments.p, (const uint32_t *)r->ptcl.p,
+                                           (const uint32_t *)r->info_bin_data.p, (uint32_t *)r->blend_spill.p, (uint32_t *)d.dev,
+                                           (const uint32_t *)r->cur->ramps.p, (const uint8_t *)r->cur->atlas.p, (const uint32_t *)r->mask8.p,
+                                           (const uint32_t *)r->mask16.p, (const uint32_t *)r->tile_start.p, r->occlusion_cull,
+                                           ctl + VB_CTL_FINE_QUEUE + b, r->cls_list.p, n_bands == 1u ? ctl + VB_CTL_FINE_CLASS : nullptr,
+                                           c.width_in_tiles * c.height_in_tiles, r->sm_count, st);
+                if (d.host && (rc = queue_readback(r, c, cb.win_ty0, cb.win_ty1, d, b))) return rc;
             }
             break;
         }
@@ -746,7 +734,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
         }
         rec(r, s + 1);
     }
-    k_publish_bump<<<1, 32, 0, st>>>(bump, r->h_bump_dev); // zero-copy store to mapped host memory (no copy engine)
+    k_publish_bump<<<1, 32, 0, st>>>(bump, r->cur->h_bump_dev); // zero-copy store to mapped host memory (no copy engine)
     launches++;
     CK(cudaGetLastError());
     r->launches = launches;
@@ -760,17 +748,15 @@ static int enqueue_direct(vb_renderer *r, int first, int last, void *out_dev) {
 // the launches of a frame are identical -- same kernels, grids, arena pointers, config -- so they are captured once into a
 // graph and replayed with ONE submission. The key is everything a launch argument is derived from; growing an arena or
 // changing the scene layout / frame size / window simply misses the cache and re-captures.
-static void graph_key(const vb_renderer *r, int last, const void *out_dev, GraphKey *k) {
+static void graph_key(vb_renderer *r, int last, const void *out_dev, GraphKey *k) {
     memset(k, 0, sizeof *k);
     k->cfg = r->cfg;
-    const DevBuf *bufs[] = {&r->scene, &r->ramps, &r->atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
-                            &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths,
-                            &r->ctl, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles,
-                            &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
     size_t n = 0;
-    for (const DevBuf *b : bufs) k->ptrs[n++] = b->p;
+    for_each_buf(r, [&](DevBuf &b, bool keyed) {
+        if (keyed) k->ptrs[n++] = b.p;
+    });
     k->ptrs[n++] = out_dev;
-    k->ptrs[n++] = r->h_bump_dev;
+    k->ptrs[n++] = r->cur->h_bump_dev;
     k->ctl_words = r->ctl_words;
     k->aa = r->params.aa;
     k->cull = r->occlusion_cull;
@@ -782,93 +768,74 @@ static void graph_key(const vb_renderer *r, int last, const void *out_dev, Graph
     }
 }
 
-static int queue_readback(vb_renderer *r, const VbConfig &c, uint32_t ty0, uint32_t ty1, void *out_dev, uint32_t band) {
-    size_t y0 = (size_t)ty0 * 16u, y1 = (size_t)ty1 * 16u;
-    if (y1 > c.target_height) y1 = c.target_height;
-    if (y1 <= y0) return VB_OK;
-    const size_t off = (y0 - c.out_row0) * c.out_pitch_px * 4u, bytes = (y1 - y0) * c.out_pitch_px * 4u;
-    CK(cudaEventRecord(r->band_ev[band], r->stream));
-    CK(cudaStreamWaitEvent(r->copy_stream, r->band_ev[band], 0));
-    CK(cudaMemcpyAsync((char *)r->host_out + off, (const char *)out_dev + off, bytes, cudaMemcpyDeviceToHost, r->copy_stream));
-    return VB_OK;
-}
-
 // Enqueue stages first..last: through a cached graph for whole frames, directly otherwise.
-static int enqueue(vb_renderer *r, int first, int last, void *out_dev) {
+static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clear_queues) {
     const VbConfig &c = r->cfg;
-    if (!r->use_graph || r->timing || first != 0 || last != VB_N_STAGE_IDS - 1) return enqueue_direct(r, first, last, out_dev);
+    if (!r->use_graph || r->timing || first != 0 || last != VB_N_STAGE_IDS - 1) return enqueue_direct(r, first, last, d, clear_queues);
     // with a host destination split into bands, fine and its interleaved copies stay outside the graph
     const uint32_t rows = c.win_ty1 - c.win_ty0;
-    const bool banded = r->host_out && rows >= 64u && r->readback_bands > 1u;
+    const bool banded = d.host && rows >= 64u && d.bands > 1u;
     const int g_last = banded ? VB_STAGE_ID_FINE - 1 : last;
     GraphKey key;
-    graph_key(r, g_last, out_dev, &key);
+    graph_key(r, g_last, d.dev, &key);
     GraphSlot *slot = nullptr;
     for (GraphSlot &gs : r->graphs)
         if (gs.exec && memcmp(&gs.key, &key, sizeof key) == 0) slot = &gs;
-    void *host_out = r->host_out;
+    // Any refusal along the way (a tool or driver that does not allow capture here) turns graph replay off for this renderer
+    // and the frame is launched kernel by kernel: graphs are an optimisation, never a requirement.
+    auto direct = [&]() {
+        cudaGetLastError();
+        r->use_graph = false;
+        return enqueue_direct(r, first, last, d, clear_queues);
+    };
     if (!slot) {
         slot = &r->graphs[r->graph_next++ % (sizeof r->graphs / sizeof r->graphs[0])];
         if (slot->exec) {
             cudaGraphExecDestroy(slot->exec);
             slot->exec = nullptr;
         }
-        // Any refusal along the way (a tool or driver that does not allow capture here) turns graph replay off for this
-        // renderer and the frame is launched kernel by kernel: graphs are an optimisation, never a requirement.
-        if (cudaStreamBeginCapture(r->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-            cudaGetLastError();
-            r->use_graph = false;
-            return enqueue_direct(r, first, last, out_dev);
-        }
-        r->host_out = nullptr; // the captured fine is one launch; its read-back is queued after the graph, below
-        const int rc = enqueue_direct(r, 0, g_last, out_dev);
+        if (cudaStreamBeginCapture(r->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) return direct();
+        Dest captured = d;
+        captured.host = nullptr; // the captured fine is one launch; its read-back is queued after the graph, below
+        const int rc = enqueue_direct(r, 0, g_last, captured, false);
         cudaGraph_t g = nullptr;
         const cudaError_t e = cudaStreamEndCapture(r->stream, &g);
-        r->host_out = host_out;
         if (rc != VB_OK || e != cudaSuccess || !g) {
             if (g) cudaGraphDestroy(g);
-            cudaGetLastError();
-            r->use_graph = false;
-            return enqueue_direct(r, first, last, out_dev);
+            return direct();
         }
         const cudaError_t ei = cudaGraphInstantiate(&slot->exec, g, 0);
         cudaGraphDestroy(g);
         if (ei != cudaSuccess) {
             slot->exec = nullptr;
-            cudaGetLastError();
-            r->use_graph = false;
-            return enqueue_direct(r, first, last, out_dev);
+            return direct();
         }
         slot->key = key;
         slot->launches = r->launches;
     }
     if (cudaGraphLaunch(slot->exec, r->stream) != cudaSuccess) {
-        cudaGetLastError();
         cudaGraphExecDestroy(slot->exec);
         slot->exec = nullptr;
-        r->use_graph = false;
-        return enqueue_direct(r, first, last, out_dev);
+        return direct();
     }
     r->launches = slot->launches;
     if (banded) {
-        const int rc = enqueue_direct(r, VB_STAGE_ID_FINE, VB_STAGE_ID_FINE, out_dev);
+        const int rc = enqueue_direct(r, VB_STAGE_ID_FINE, VB_STAGE_ID_FINE, d, false);
         r->launches += slot->launches;
         return rc;
     }
-    if (host_out) return queue_readback(r, c, c.win_ty0, c.win_ty1, out_dev, 0);
+    if (d.host) return queue_readback(r, c, c.win_ty0, c.win_ty1, d, 0);
     return VB_OK;
 }
 
-static int pick_out(vb_renderer *r, void *out_device, void **out) {
-    if (out_device) {
-        *out = out_device;
-        return VB_OK;
-    }
+// The frame's device destination: the given pointer, or the renderer's own target (allocated for this frame's window).
+static int pick_out(vb_renderer *r, Dest *d) {
+    if (d->dev) return VB_OK;
     const VbConfig &c = r->cfg;
     size_t rows = (size_t)(c.win_ty1 - c.win_ty0) * 16u;
-    DevBuf &t = r->use_alt ? r->target_alt : r->target;
+    DevBuf &t = d->alt ? r->target_alt : r->target;
     int rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * rows);
-    *out = t.p;
+    d->dev = t.p;
     return rc;
 }
 
@@ -876,21 +843,19 @@ static int pick_out(vb_renderer *r, void *out_device, void **out) {
 // arenas, the output target), then the launches. vb_group runs step 1 for ALL its renderers before step 2 of any: with the
 // exchange on, a renderer's frame contains a kernel that waits for its peers, and a peer that shares the device (tests)
 // must not be stuck in a cudaFree behind that kernel.
-static int frame_prepare(vb_renderer *r, const vb_params *p, void *out_device) {
+static int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
     if (!r || !p) return VB_E_INVALID;
-    if (!r->have_scene) return VB_E_NO_SCENE;
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;
-    void *out;
-    if ((rc = pick_out(r, out_device, &out))) return rc;
-    r->out_dev = out;
-    return VB_OK;
+    r->dest = d;
+    return pick_out(r, &r->dest);
 }
 static int frame_launch(vb_renderer *r) {
     CK(cudaSetDevice(r->device));
     CK(cudaEventRecord(r->frame_ev[0], r->stream));
-    int rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->out_dev);
+    int rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->dest, false);
     if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
     r->frame_timed = rc == VB_OK;
     r->frame_pending = rc == VB_OK;
@@ -903,10 +868,10 @@ static int frame_launch_half(vb_renderer *r, int half) {
     CK(cudaSetDevice(r->device));
     if (half == 0) {
         CK(cudaEventRecord(r->frame_ev[0], r->stream));
-        return enqueue_direct(r, 0, VB_STAGE_ID_FLATTEN, r->out_dev);
+        return enqueue_direct(r, 0, VB_STAGE_ID_FLATTEN, r->dest, false);
     }
     uint32_t first_half = r->launches;
-    int rc = enqueue_direct(r, VB_STAGE_ID_DRAW, VB_N_STAGE_IDS - 1, r->out_dev);
+    int rc = enqueue_direct(r, VB_STAGE_ID_DRAW, VB_N_STAGE_IDS - 1, r->dest, false);
     r->launches += first_half;
     // (with a host destination enqueue_direct queues the read-back behind fine itself)
     if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
@@ -915,19 +880,22 @@ static int frame_launch_half(vb_renderer *r, int half) {
     return rc;
 }
 
-extern "C" int vb_render_enqueue(vb_renderer *r, const vb_params *p, void *out_device) {
-    int rc = frame_prepare(r, p, out_device);
+static int render_enqueue(vb_renderer *r, const vb_params *p, const Dest &d) {
+    int rc = frame_prepare(r, p, d);
     if (rc) return rc;
     return frame_launch(r);
+}
+extern "C" int vb_render_enqueue(vb_renderer *r, const vb_params *p, void *out_device) {
+    return render_enqueue(r, p, Dest{out_device});
 }
 
 static void fill_stats(vb_renderer *r, vb_frame_stats *s) {
     if (!s) return;
     memset(s, 0, sizeof *s);
-    memcpy(s, r->h_bump, sizeof(VbBump));
+    memcpy(s, r->cur->h_bump, sizeof(VbBump));
     s->retries = r->retries;
     s->kernel_launches = r->launches;
-    s->arena_bytes = arena_bytes(r);
+    for_each_buf(r, [&](DevBuf &b, bool) { s->arena_bytes += b.cap; });
     if (r->timing) {
         for (int i = 0; i < VB_N_STAGE_IDS; i++) cudaEventElapsedTime(&s->stage_ms[i], r->ev[i], r->ev[i + 1]);
         cudaEventElapsedTime(&s->total_ms, r->ev[0], r->ev[VB_N_STAGE_IDS]);
@@ -936,23 +904,16 @@ static void fill_stats(vb_renderer *r, vb_frame_stats *s) {
 
 // After a failed attempt: enlarge whatever overflowed, using the counters the kernels kept counting.
 static void grow_arenas(vb_renderer *r) {
-    const VbBump &b = *r->h_bump;
-    const VbConfig &c = r->cfg;
-    // a test-only limit lasts for one overflow of its arena: the re-run sees the real capacity
-    const uint64_t need[N_ARENAS] = {b.lines, b.binning, b.tile, b.seg_counts, b.segments, b.blend,
-                                     (uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC + b.ptcl};
-    for (int a = 0; a < N_ARENAS; a++)
-        if (need[a] > r->arena_limit[a]) r->arena_limit[a] = UINT32_MAX;
-    if (b.lines > r->cap_lines) r->cap_lines = grow(b.lines);
-    if (b.binning > r->cap_binning) r->cap_binning = grow(b.binning);
-    if (b.tile > r->cap_tiles) r->cap_tiles = grow(b.tile);
-    if (b.seg_counts > r->cap_seg_counts) r->cap_seg_counts = grow(b.seg_counts);
-    if (b.segments > r->cap_segments) r->cap_segments = grow(b.segments);
-    if (b.blend > r->cap_blend) r->cap_blend = grow(b.blend);
-    uint64_t ptcl_need = (uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC + b.ptcl + VB_PTCL_INCREMENT;
-    if (ptcl_need > r->cap_ptcl) r->cap_ptcl = grow((uint32_t)(ptcl_need > 0xf0000000ull ? 0xf0000000ull : ptcl_need));
-    if (r->cap_seg_counts < r->cap_lines) r->cap_seg_counts = r->cap_lines;
-    if (r->cap_segments < r->cap_seg_counts && (b.failed & VB_STAGE_PATH_COUNT)) r->cap_segments = r->cap_seg_counts;
+    for (int a = 0; a < N_ARENAS; a++) {
+        const uint64_t need = arena_need(r, a);
+        // a test-only limit lasts for one overflow of its arena: the re-run sees the real capacity
+        if (need > r->limit[a]) r->limit[a] = UINT32_MAX;
+        const uint64_t want = need + (a == ARENA_PTCL ? VB_PTCL_INCREMENT : 0u);
+        if (want > r->cap[a]) r->cap[a] = grow((uint32_t)std::min<uint64_t>(want, 0xf0000000ull));
+    }
+    uint32_t *cap = r->cap;
+    if (cap[ARENA_SEG_COUNTS] < cap[ARENA_LINES]) cap[ARENA_SEG_COUNTS] = cap[ARENA_LINES];
+    if (cap[ARENA_SEGMENTS] < cap[ARENA_SEG_COUNTS] && (r->cur->h_bump->failed & VB_STAGE_PATH_COUNT)) cap[ARENA_SEGMENTS] = cap[ARENA_SEG_COUNTS];
 }
 
 extern "C" int vb_frame_finish(vb_renderer *r, vb_frame_stats *stats) {
@@ -961,23 +922,20 @@ extern "C" int vb_frame_finish(vb_renderer *r, vb_frame_stats *stats) {
     CK(cudaStreamSynchronize(r->stream));
     r->frame_pending = false;
     fill_stats(r, stats);
-    return r->h_bump->failed ? VB_E_BUMP_OVERFLOW : VB_OK;
+    return r->cur->h_bump->failed ? VB_E_BUMP_OVERFLOW : VB_OK;
 }
 
-extern "C" int vb_render_resident(vb_renderer *r, const vb_params *p, void *out_device, vb_frame_stats *stats) {
-    if (!r || !p) return VB_E_INVALID;
-    {
-        int rcd = drain_stream(r);
-        if (rcd) return rcd;
-    }
-    if (!r->have_scene) return VB_E_NO_SCENE;
+// One frame, re-run with grown arenas until it fits. Streamed frames still in flight are left alone: the streaming calls
+// re-run their own frames through here.
+static int render_sync(vb_renderer *r, const vb_params *p, const Dest &d, vb_frame_stats *stats) {
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
     r->retries = 0;
     for (uint32_t attempt = 0;; attempt++) {
-        int rc = vb_render_enqueue(r, p, out_device);
+        int rc = render_enqueue(r, p, d);
         if (rc) return rc;
         CK(cudaStreamSynchronize(r->stream));
         r->frame_pending = false;
-        if (r->h_bump->failed == 0) break;
+        if (r->cur->h_bump->failed == 0) break;
         if (r->xc.enabled) {
             // every attempt of an exchanged frame is a collective step (all GPUs advance their epoch together): grow what
             // overflowed here and let the caller re-issue the frame on every GPU
@@ -998,20 +956,31 @@ extern "C" int vb_render_resident(vb_renderer *r, const vb_params *p, void *out_
     return VB_OK;
 }
 
-extern "C" int vb_render_uploaded(vb_renderer *r, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {
-    if (!r || !p || !out) return VB_E_INVALID;
-    r->host_out = out_is_device ? nullptr : out;
-    int rc = vb_render_resident(r, p, out_is_device ? out : nullptr, stats);
-    r->host_out = nullptr;
-    if (!out_is_device) {
-        // the band copies were queued behind the fine bands; a re-run after an arena overflow simply copies again
-        cudaError_t e = cudaStreamSynchronize(r->copy_stream);
-        if (rc == VB_OK && e != cudaSuccess) {
-            r->err = std::string("copy stream: ") + cudaGetErrorString(e);
-            return VB_E_CUDA;
-        }
+// render_sync with a host destination, then wait for its copies
+static int render_sync_host(vb_renderer *r, const vb_params *p, const Dest &d, vb_frame_stats *stats) {
+    int rc = render_sync(r, p, d, stats);
+    // the band copies were queued behind the fine bands; a re-run after an arena overflow simply copies again
+    cudaError_t e = cudaStreamSynchronize(r->copy_stream);
+    if (rc == VB_OK && e != cudaSuccess) {
+        r->err = std::string("copy stream: ") + cudaGetErrorString(e);
+        return VB_E_CUDA;
     }
     return rc;
+}
+
+extern "C" int vb_render_resident(vb_renderer *r, const vb_params *p, void *out_device, vb_frame_stats *stats) {
+    if (!r || !p) return VB_E_INVALID;
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    return render_sync(r, p, Dest{out_device}, stats);
+}
+
+extern "C" int vb_render_uploaded(vb_renderer *r, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {
+    if (!r || !p || !out) return VB_E_INVALID;
+    if (out_is_device) return vb_render_resident(r, p, out, stats);
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    return render_sync_host(r, p, Dest{nullptr, out, false, r->readback_bands}, stats);
 }
 
 extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
@@ -1034,21 +1003,8 @@ extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len,
 // it) is then re-run synchronously with grown arenas -- rare (first frames of a new scene size) and exact.
 static int rerun_frame_sync(vb_renderer *r, uint32_t q, vb_frame_stats *stats) {
     const uint32_t slot = r->ring[q].slot;
-    select_slot(r, slot);
-    r->host_out = r->ring[q].out_host;
-    r->use_alt = slot != 0u;
-    const uint32_t bands = r->readback_bands;
-    r->readback_bands = 1;
-    int rc = vb_render_resident(r, &r->ring[q].params, nullptr, stats);
-    r->readback_bands = bands;
-    r->host_out = nullptr;
-    r->use_alt = false;
-    cudaError_t e = cudaStreamSynchronize(r->copy_stream);
-    if (rc == VB_OK && e != cudaSuccess) {
-        r->err = std::string("copy stream: ") + cudaGetErrorString(e);
-        rc = VB_E_CUDA;
-    }
-    return rc;
+    r->cur = &r->slot[slot];
+    return render_sync_host(r, &r->ring[q].params, Dest{nullptr, r->ring[q].out_host, slot != 0u, 1u}, stats);
 }
 
 // Frame in ring entry q: wait for its kernels, look at its bump counters, re-run on overflow (together with the younger frame
@@ -1056,19 +1012,19 @@ static int rerun_frame_sync(vb_renderer *r, uint32_t q, vb_frame_stats *stats) {
 static int check_raster(vb_renderer *r, uint32_t q, int younger) {
     vb_renderer::RingFrame &f = r->ring[q];
     if (!f.pending || f.raster_checked) return VB_OK;
-    const uint32_t keep = r->cur_slot;
+    vb_renderer::SceneSlot *const keep = r->cur;
     CK(cudaEventSynchronize(r->raster_done[f.slot]));
-    select_slot(r, f.slot);
+    r->cur = &r->slot[f.slot];
     int rc = VB_OK;
-    if (r->h_bump->failed != 0u) {
+    if (r->cur->h_bump->failed != 0u) {
         CK(cudaStreamSynchronize(r->stream));
         CK(cudaStreamSynchronize(r->copy_stream));
         grow_arenas(r);
         rc = rerun_frame_sync(r, q, &f.stats);
         CK(cudaEventRecord(r->copy_done[q], r->copy_stream));
         if (rc == VB_OK && younger >= 0 && r->ring[younger].pending) {
-            select_slot(r, r->ring[younger].slot);
-            if (r->h_bump->failed != 0u) {
+            r->cur = &r->slot[r->ring[younger].slot];
+            if (r->cur->h_bump->failed != 0u) {
                 rc = rerun_frame_sync(r, (uint32_t)younger, &r->ring[younger].stats);
                 CK(cudaEventRecord(r->raster_done[r->ring[younger].slot], r->stream));
                 CK(cudaEventRecord(r->copy_done[younger], r->copy_stream));
@@ -1079,7 +1035,7 @@ static int check_raster(vb_renderer *r, uint32_t q, int younger) {
         fill_stats(r, &f.stats);
     }
     f.raster_checked = true;
-    select_slot(r, keep);
+    r->cur = keep;
     return rc;
 }
 
@@ -1099,28 +1055,17 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
     if (!r || !p || !out_host) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     if (stats) memset(stats, 0, sizeof *stats);
-    struct Guard {
-        vb_renderer *r;
-        ~Guard() { r->in_stream_call = false; }
-    } guard{r};
-    r->in_stream_call = true;
     const uint64_t k = r->stream_seq;
     const uint32_t slot = (uint32_t)(k & 1u), q = (uint32_t)(k % 3u), q1 = (uint32_t)((k + 2u) % 3u), q2 = (uint32_t)((k + 1u) % 3u);
     // frame k-2 (same scene slot, same device target) was checked by the previous call; frame k-3 (ring entry q) is complete
-    select_slot(r, slot);
+    r->cur = &r->slot[slot];
     int rc = upload_on(r, r->upload_stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h);
     if (rc) return rc;
     CK(cudaEventRecord(r->upload_done[slot], r->upload_stream));
     CK(cudaStreamWaitEvent(r->stream, r->upload_done[slot], 0));
     if (k >= 2u && r->ring[q2].pending) CK(cudaStreamWaitEvent(r->stream, r->copy_done[q2], 0)); // its read-back still reads this target
-    const uint32_t bands = r->readback_bands;
-    r->readback_bands = 1; // the whole read-back overlaps the next frames: no reason to split fine
-    r->host_out = out_host;
-    r->use_alt = slot != 0u;
-    rc = vb_render_enqueue(r, p, nullptr);
-    r->host_out = nullptr;
-    r->use_alt = false;
-    r->readback_bands = bands;
+    // one band: the whole read-back overlaps the next frames, no reason to split fine
+    rc = render_enqueue(r, p, Dest{nullptr, out_host, slot != 0u, 1u});
     if (rc) return rc;
     r->frame_pending = false;
     CK(cudaEventRecord(r->raster_done[slot], r->stream));
@@ -1145,11 +1090,6 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
 extern "C" int vb_readback_wait(vb_renderer *r) {
     if (!r) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
-    struct Guard {
-        vb_renderer *r;
-        ~Guard() { r->in_stream_call = false; }
-    } guard{r};
-    r->in_stream_call = true;
     int rc = VB_OK;
     const uint64_t k = r->stream_seq; // the next frame number: complete k-3 .. k-1 in order
     for (uint64_t j = k >= 3u ? k - 3u : 0u; j < k; j++) {
@@ -1166,19 +1106,13 @@ extern "C" int vb_readback_wait(vb_renderer *r) {
 
 extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int last, void *out_device) {
     if (!r || !p || first < 0 || last >= VB_N_STAGE_IDS || first > last) return VB_E_INVALID;
-    if (!r->have_scene) return VB_E_NO_SCENE;
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;
-    void *out = nullptr;
-    if (last == VB_STAGE_ID_FINE) {
-        if ((rc = pick_out(r, out_device, &out))) return rc;
-        r->out_dev = out;
-    }
-    r->zero_fine_queue = true;
-    rc = enqueue(r, first, last, out);
-    r->zero_fine_queue = false;
-    if (rc) return rc;
+    Dest d{out_device};
+    if (last == VB_STAGE_ID_FINE && (rc = pick_out(r, &d))) return rc;
+    if ((rc = enqueue(r, first, last, d, true))) return rc;
     CK(cudaStreamSynchronize(r->stream));
     return VB_OK;
 }
@@ -1190,61 +1124,51 @@ struct NamedBuf {
 };
 static std::vector<NamedBuf> named(vb_renderer *r) {
     const VbConfig &c = r->cfg;
-    const VbLayout &L = r->layout;
-    const VbBump &b = *r->h_bump;
-    auto mn = [](uint64_t a, uint64_t b2) { return a < b2 ? a : b2; };
+    const VbLayout &L = r->cur->layout;
     const uint32_t wb = (c.width_in_tiles + 15u) / 16u, hb = (c.height_in_tiles + 15u) / 16u;
     const uint32_t aligned_n_bins = (wb * hb + 255u) & ~255u;
-    uint64_t ptcl_words = mn((uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC + b.ptcl, c.ptcl_size);
-    return {
+    std::vector<NamedBuf> v = {
+        {"scene", &r->cur->scene, r->cur->scene_words * 4}, // the uploaded / device-resolved inputs
+        {"ramps", &r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4},
+        {"atlas", &r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4},
         {"tag_monoids", &r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)},
         {"path_bboxes", &r->path_bboxes, (size_t)L.n_paths * sizeof(VbPathBbox)},
-        {"lines", &r->lines, (size_t)mn(b.lines, c.lines_size) * sizeof(VbLineSoup)},
         {"draw_monoids", &r->draw_monoids, (size_t)L.n_draw_objects * sizeof(VbDrawMonoid)},
-        {"info_bin_data", &r->info_bin_data, ((size_t)L.bin_data_start + mn(b.binning, c.binning_size)) * 4},
         {"clip_inp", &r->clip_inp, (size_t)L.n_clips * sizeof(VbClipInp)},
         {"clip_bboxes", &r->clip_bboxes, (size_t)L.n_clips * sizeof(VbBbox4)},
         {"draw_bboxes", &r->draw_bboxes, (size_t)L.n_draw_objects * sizeof(VbBbox4)},
         {"bin_headers", &r->bin_headers, (size_t)((L.n_draw_objects + 255u) / 256u) * aligned_n_bins * sizeof(VbBinHeader)},
         {"paths", &r->paths, (size_t)L.n_draw_objects * sizeof(VbPath)},
-        {"tiles", &r->tiles, (size_t)mn(b.tile, c.tiles_size) * sizeof(VbTile)},
-        {"seg_counts", &r->seg_counts, (size_t)mn(b.seg_counts, c.seg_counts_size) * sizeof(VbSegmentCount)},
-        {"segments", &r->segments, (size_t)mn(b.segments, c.segments_size) * sizeof(VbSegment)},
-        {"ptcl", &r->ptcl, (size_t)ptcl_words * 4},
-        {"blend_spill", &r->blend_spill, (size_t)mn(b.blend, c.blend_size) * 4},
     };
+    // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
+    const uint32_t *size = &c.lines_size;
+    for (int a = 0; a < N_ARENAS; a++) {
+        const ArenaDesc &d = ARENAS[a];
+        const size_t used = (size_t)std::min<uint64_t>(arena_need(r, a), size[a]);
+        v.push_back({d.download ? d.download : d.name, &(r->*d.buf), (arena_offset(r, a) + used) * d.elem_bytes});
+    }
+    return v;
 }
 
 // The guard region of a limited arena (vb_debug_limit_arena): the bytes of its allocation past the limit. `name` is an arena
 // name, or "line_scratch" / "flatten_jobs" (flatten's scratch arenas, sized from the lines capacity). Returns false for an
 // unknown name; *buf is nullptr while the arena has no limit.
 static bool guard_region(vb_renderer *r, const char *name, DevBuf **buf, size_t *off) {
-    int a = -1;
-    if (!strcmp(name, "line_scratch") || !strcmp(name, "flatten_jobs")) a = ARENA_LINES;
-    for (int i = 0; i < N_ARENAS; i++)
-        if (!strcmp(name, ARENA_NAMES[i])) a = i;
+    DevBuf *scratch = !strcmp(name, "line_scratch") ? &r->line_scratch : !strcmp(name, "flatten_jobs") ? &r->flatten_jobs : nullptr;
+    const int a = scratch ? ARENA_LINES : arena_index(name);
     if (a < 0) return false;
     *buf = nullptr;
     *off = 0;
-    const size_t lim = r->arena_limit[a];
+    const uint32_t lim = r->limit[a];
     if (lim == UINT32_MAX) return true;
-    DevBuf *b = nullptr;
-    size_t o = 0;
-    switch (a) {
-    case ARENA_LINES: {
+    // ptcl: includes the 512 bytes of window slack that fine reads and never writes
+    DevBuf *b = &(r->*ARENAS[a].buf);
+    size_t o = (arena_offset(r, a) + lim) * ARENAS[a].elem_bytes;
+    if (scratch) {
         size_t lit_bytes, job_bytes; // flatten sees lits_cap = lines_size, jobs_cap = lines_size / FL_DEFER_MIN + 1
-        vb_flatten_arena_bytes((uint32_t)lim, &lit_bytes, &job_bytes);
-        if (!strcmp(name, "line_scratch")) b = &r->line_scratch, o = lit_bytes;
-        else if (!strcmp(name, "flatten_jobs")) b = &r->flatten_jobs, o = job_bytes;
-        else b = &r->lines, o = lim * sizeof(VbLineSoup);
-        break;
-    }
-    case ARENA_BINNING: b = &r->info_bin_data, o = ((size_t)r->layout.bin_data_start + lim) * 4; break;
-    case ARENA_TILES: b = &r->tiles, o = lim * sizeof(VbTile); break;
-    case ARENA_SEG_COUNTS: b = &r->seg_counts, o = lim * sizeof(VbSegmentCount); break;
-    case ARENA_SEGMENTS: b = &r->segments, o = lim * sizeof(VbSegment); break;
-    case ARENA_BLEND: b = &r->blend_spill, o = lim * 4; break;
-    default: b = &r->ptcl, o = lim * 4; break; // includes the 512 bytes of window slack that fine reads and never writes
+        vb_flatten_arena_bytes(lim, &lit_bytes, &job_bytes);
+        b = scratch;
+        o = scratch == &r->line_scratch ? lit_bytes : job_bytes;
     }
     *buf = b;
     *off = o < b->cap ? o : b->cap;
@@ -1253,9 +1177,7 @@ static bool guard_region(vb_renderer *r, const char *name, DevBuf **buf, size_t 
 
 extern "C" int vb_debug_limit_arena(vb_renderer *r, const char *arena, uint32_t limit) {
     if (!r || !arena) return VB_E_INVALID;
-    int a = -1;
-    for (int i = 0; i < N_ARENAS; i++)
-        if (!strcmp(arena, ARENA_NAMES[i])) a = i;
+    const int a = arena_index(arena);
     if (a < 0) {
         r->err = std::string("vb_debug_limit_arena: unknown arena ") + arena;
         return VB_E_INVALID;
@@ -1265,18 +1187,16 @@ extern "C" int vb_debug_limit_arena(vb_renderer *r, const char *arena, uint32_t 
     CK(cudaStreamSynchronize(r->copy_stream));
     CK(cudaStreamSynchronize(r->upload_stream));
     if (limit == UINT32_MAX) {
-        r->arena_limit[a] = UINT32_MAX;
+        r->limit[a] = UINT32_MAX;
         return VB_OK;
     }
-    const uint32_t caps[N_ARENAS] = {r->cap_lines, r->cap_binning, r->cap_tiles, r->cap_seg_counts, r->cap_segments, r->cap_blend, r->cap_ptcl};
-    const uint64_t ptcl_static = (uint64_t)r->cfg.width_in_tiles * r->cfg.height_in_tiles * VB_PTCL_INITIAL_ALLOC;
     // 0 is refused too: path_count and path_tiling size their grids from the capacity
-    if (limit == 0u || limit > caps[a] || (a == ARENA_PTCL && limit < ptcl_static)) {
+    if (limit == 0u || limit > r->cap[a] || (a == ARENA_PTCL && limit < ptcl_static(r->cfg))) {
         r->err = "vb_debug_limit_arena: the limit must be at least 1 (the static area for ptcl) and at most the allocation";
         return VB_E_INVALID;
     }
-    r->arena_limit[a] = limit;
-    const char *regions[3] = {ARENA_NAMES[a], "line_scratch", "flatten_jobs"};
+    r->limit[a] = limit;
+    const char *regions[3] = {ARENAS[a].name, "line_scratch", "flatten_jobs"};
     for (int k = 0; k < (a == ARENA_LINES ? 3 : 1); k++) {
         DevBuf *b;
         size_t off;
@@ -1311,14 +1231,6 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
     if (!strcmp(name, "seg_holes")) { // reserved-but-unused segment slots of the last frame (k_coarse.cu)
         if (bytes) *bytes = 4;
         if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->ctl.p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
-        return VB_OK;
-    }
-    if (!strcmp(name, "scene") || !strcmp(name, "ramps") || !strcmp(name, "atlas")) { // the uploaded / device-resolved inputs
-        const DevBuf &b = name[0] == 's' ? r->scene : (name[0] == 'r' ? r->ramps : r->atlas);
-        const size_t n = name[0] == 's' ? r->scene_words * 4 : (name[0] == 'r' ? (size_t)r->n_ramps * 512 * 4 : (size_t)r->atlas_w * r->atlas_h * 4);
-        if (bytes) *bytes = n;
-        const size_t c = n < cap ? n : cap;
-        if (dst && c) CK(cudaMemcpy(dst, b.p, c, cudaMemcpyDeviceToHost));
         return VB_OK;
     }
     if (!strcmp(name, "config")) {
@@ -1383,17 +1295,17 @@ extern "C" int vb_debug_upload(vb_renderer *r, const char *name, const void *src
     if (!r || !name || !src) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
-    if (!strcmp(name, "lines")) {
+    if (!strcmp(name, ARENAS[ARENA_LINES].name)) {
         uint32_t n = (uint32_t)(bytes / sizeof(VbLineSoup));
-        if (n > r->cap_lines) {
-            r->cap_lines = grow(n);
-            int rc = ensure(r, r->lines, (size_t)r->cap_lines * sizeof(VbLineSoup));
+        if (n > r->cap[ARENA_LINES]) {
+            r->cap[ARENA_LINES] = grow(n);
+            int rc = ensure_arena(r, ARENA_LINES);
             if (rc) return rc;
         }
         CK(cudaMemcpy(r->lines.p, src, (size_t)n * sizeof(VbLineSoup), cudaMemcpyHostToDevice));
         VbBump *bump = (VbBump *)r->ctl.p;
         CK(cudaMemcpy(&bump->lines, &n, 4, cudaMemcpyHostToDevice));
-        r->h_bump->lines = n;
+        r->cur->h_bump->lines = n;
         return VB_OK;
     }
     if (!strcmp(name, "path_bboxes")) {
@@ -1644,7 +1556,7 @@ extern "C" int vb_group_set_exchange(vb_group *g, int on) {
         return VB_OK;
     }
     for (vb_renderer *r : g->subs)
-        if (!r->have_scene) return VB_OK; // arenas are built by the next vb_group_scene_upload
+        if (!r->cur->have_scene) return VB_OK; // arenas are built by the next vb_group_scene_upload
     return group_setup_exchange(g);
 }
 
@@ -1688,6 +1600,16 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
     }
     // enqueue every device's stripe, then complete them (one host thread; the devices run side by side)
     std::vector<vb_params> ps(n, *p);
+    // device destination: straight into the frame on devices[0] when peer-mapped; otherwise (and for a host destination) the
+    // renderer's own target. Without the exchange a host destination's stripe is copied by the frame itself, on the
+    // renderer's copy stream.
+    auto dest_of = [&](size_t i) {
+        const size_t row0 = (size_t)g->bounds[i] * 16u;
+        Dest d;
+        if (!host_out && g->peer_ok[i]) d.dev = (char *)frame + row0 * pitch;
+        if (host_out && !g->exchange) d.host = (char *)host_out + row0 * pitch;
+        return d;
+    };
     int result = VB_OK;
     for (uint32_t attempt = 0;; attempt++) {
         if (g->exchange)
@@ -1705,24 +1627,16 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                 ps[i].tile_row1 = g->bounds[i + 1];
                 if (ps[i].tile_row1 <= ps[i].tile_row0) continue; // more devices than tile rows (never with the exchange on)
                 const size_t row0 = (size_t)g->bounds[i] * 16u;
-                // device destination: straight into the frame on devices[0] when peer-mapped; otherwise (and for a host
-                // destination) the renderer's own target
-                void *dst = (!host_out && g->peer_ok[i]) ? (char *)frame + row0 * pitch : nullptr;
-                if (host_out && !late_copy) { // the frame copies its stripe to the host itself, on the renderer's copy stream
-                    r->host_out = (char *)host_out + row0 * pitch;
-                    r->readback_bands = 1;
-                }
                 int rc = VB_OK;
-                if (phase == 0) rc = frame_prepare(r, &ps[i], dst);
+                if (phase == 0) rc = frame_prepare(r, &ps[i], dest_of(i));
                 else if (phase <= n_launch) rc = halves ? frame_launch_half(r, phase - 1) : frame_launch(r);
                 else {
                     const size_t h1 = std::min<size_t>((size_t)g->bounds[i + 1] * 16u, p->height);
                     cudaSetDevice(r->device);
-                    if (h1 > row0 && cudaMemcpyAsync((char *)host_out + row0 * pitch, r->out_dev, (h1 - row0) * pitch, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess)
+                    if (h1 > row0 && cudaMemcpyAsync((char *)host_out + row0 * pitch, r->dest.dev, (h1 - row0) * pitch, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess)
                         rc = VB_E_CUDA;
                 }
                 if (rc) {
-                    for (vb_renderer *q : g->subs) q->host_out = nullptr;
                     g->err = r->err;
                     return rc;
                 }
@@ -1737,7 +1651,6 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                 continue;
             }
             const size_t row0 = (size_t)g->bounds[i] * 16u;
-            void *dst = (!host_out && g->peer_ok[i]) ? (char *)frame + row0 * pitch : nullptr;
             int rc = vb_frame_finish(r, stats ? &stats[i] : nullptr);
             if (rc == VB_E_BUMP_OVERFLOW) {
                 if (g->exchange) { // an exchanged frame is re-issued on EVERY device (epochs advance together)
@@ -1748,7 +1661,7 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                     // grow and re-run (first frames); with a host destination the re-run queues its read-back again.
                     // Growing first: the same attempt with the same arenas would only overflow again.
                     grow_arenas(r);
-                    rc = vb_render_resident(r, &ps[i], dst, stats ? &stats[i] : nullptr);
+                    rc = render_sync(r, &ps[i], dest_of(i), stats ? &stats[i] : nullptr);
                     if (stats) stats[i].retries += 1;
                 }
             }
@@ -1757,12 +1670,11 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                 cudaSetDevice(r->device);
                 if (cudaStreamSynchronize(r->copy_stream) != cudaSuccess) rc = VB_E_CUDA;
             }
-            r->host_out = nullptr;
             if (rc == VB_OK && !host_out && !g->peer_ok[i]) {
                 // no peer mapping between these two devices: stage through the renderer's own target
                 const size_t h0 = row0, h1 = std::min<size_t>((size_t)g->bounds[i + 1] * 16u, p->height);
                 cudaSetDevice(r->device);
-                if (h1 > h0 && (cudaMemcpyPeerAsync((char *)frame + row0 * pitch, g->devices[0], r->out_dev, r->device, (h1 - h0) * pitch, r->stream) != cudaSuccess ||
+                if (h1 > h0 && (cudaMemcpyPeerAsync((char *)frame + row0 * pitch, g->devices[0], r->dest.dev, r->device, (h1 - h0) * pitch, r->stream) != cudaSuccess ||
                                 cudaStreamSynchronize(r->stream) != cudaSuccess))
                     rc = VB_E_CUDA;
             }
@@ -1774,7 +1686,7 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
         if (!redo || result != VB_OK) break;
         if (attempt >= 8u) {
             g->err = "bump overflow persisted in an exchanged frame; failed bits per renderer:";
-            for (vb_renderer *q : g->subs) g->err += " 0x" + std::to_string(q->h_bump->failed);
+            for (vb_renderer *q : g->subs) g->err += " 0x" + std::to_string(q->cur->h_bump->failed);
             return VB_E_BUMP_OVERFLOW;
         }
     }
@@ -1876,8 +1788,8 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
 
     // the six streams go straight to their places in the packed buffer
-    if ((rc = ensure(r, r->scene, total_words * 4 + 64))) return rc;
-    char *base = (char *)r->scene.p;
+    if ((rc = ensure(r, r->cur->scene, total_words * 4 + 64))) return rc;
+    char *base = (char *)r->cur->scene.p;
     if (e->n_path_tags) CK(cudaMemcpyAsync(base, e->path_tags, e->n_path_tags, cudaMemcpyHostToDevice, st));
     if (e->n_path_data) CK(cudaMemcpyAsync(base + (size_t)L.path_data_base * 4, e->path_data, (size_t)e->n_path_data * 4, cudaMemcpyHostToDevice, st));
     if (e->n_draw_tags) CK(cudaMemcpyAsync(base + (size_t)L.draw_tag_base * 4, e->draw_tags, (size_t)e->n_draw_tags * 4, cudaMemcpyHostToDevice, st));
@@ -1892,25 +1804,25 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (pb) CK(cudaMemcpyAsync(tmp, patches.data(), pb, cudaMemcpyHostToDevice, st));
     if (rb) CK(cudaMemcpyAsync(tmp + o_r, ramps.data(), rb, cudaMemcpyHostToDevice, st));
     if (sb) CK(cudaMemcpyAsync(tmp + o_s, stops.data(), sb, cudaMemcpyHostToDevice, st));
-    vb_launch_resolve_finish((uint32_t *)r->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags, tmp,
+    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags, tmp,
                              (uint32_t)patches.size(), st);
-    r->n_ramps = (uint32_t)ramps.size();
-    if ((rc = ensure(r, r->ramps, (size_t)r->n_ramps * 512 * 4))) return rc;
-    vb_launch_make_ramps(tmp + o_r, tmp + o_s, r->n_ramps, (uint32_t *)r->ramps.p, st);
-    r->atlas_w = atlas_w;
-    r->atlas_h = atlas_h;
-    if ((rc = ensure(r, r->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
-    CK(cudaMemsetAsync(r->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
+    r->cur->n_ramps = (uint32_t)ramps.size();
+    if ((rc = ensure(r, r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4))) return rc;
+    vb_launch_make_ramps(tmp + o_r, tmp + o_s, r->cur->n_ramps, (uint32_t *)r->cur->ramps.p, st);
+    r->cur->atlas_w = atlas_w;
+    r->cur->atlas_h = atlas_h;
+    if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
+    CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
     for (const Placed &q : placed)
         if (q.key && q.w && q.h)
-            CK(cudaMemcpy2DAsync((char *)r->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
+            CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
                                  cudaMemcpyHostToDevice, st));
     CK(cudaGetLastError());
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
-    r->layout = L;
-    r->scene_words = total_words;
-    r->have_scene = true;
+    r->cur->layout = L;
+    r->cur->scene_words = total_words;
+    r->cur->have_scene = true;
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
@@ -1920,17 +1832,17 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
 // grow_arenas() is declared above; these entry points only manage the arena and the peer table.
 extern "C" int vb_exchange_configure(vb_renderer *r, uint32_t rank, uint32_t world, void **arena, size_t *arena_bytes) {
     if (!r || world < 1u || world > 8u || rank >= world) return VB_E_INVALID;
-    if (!r->have_scene) return VB_E_NO_SCENE;
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
     vb_renderer::Exchange &x = r->xc;
     x.enabled = false;
-    const uint32_t n_tags = (r->layout.path_data_base - r->layout.path_tag_base) * 4u;
+    const uint32_t n_tags = (r->cur->layout.path_data_base - r->cur->layout.path_tag_base) * 4u;
     // my outbox holds my share of the lines (+ the ones needed by two stripes): generous and fixed, so that the arena -- which
     // the peers have mapped -- never moves
     const uint64_t cap = (uint64_t)n_tags * 4u / world * 2u + 262144u;
     x.lines_cap = cap > 0x7fffffffull ? 0x7fffffffu : (uint32_t)cap;
-    x.n_paths = r->layout.n_paths;
+    x.n_paths = r->cur->layout.n_paths;
     x.half_bytes = vb_exchange_half_bytes(x.n_paths, x.lines_cap);
     const size_t bytes = 256 + 2 * x.half_bytes;
     int rc = ensure(r, x.arena, bytes);
