@@ -3,27 +3,45 @@
 // Reference: vello_shaders/shader/coarse.wgsl:156-471 (PTCL layout shared/ptcl.wgsl:6-25, writers
 // coarse.wgsl:68-154), CPU twin cpu/coarse.rs. One CTA = one bin (16x16 tiles), one thread = one
 // tile, as in the WGSL; log-step shared-memory scans are replaced by warp-shuffle scans.
-// The per-tile command SEQUENCE is identical to the reference's; segment slices and dynamic PTCL
-// chunks come from atomic bump allocators, so their absolute offsets are allocation-order
-// dependent (as in the reference). Only bins inside the stripe window are launched.
+// The per-tile command SEQUENCE is identical to the reference's; dynamic PTCL chunks come from an
+// atomic bump allocator, so their absolute offsets are allocation-order dependent (as in the
+// reference), and segment slices are in tile order (see below). Only bins inside the stripe window are launched.
 // Parallelism: the WGSL launches one workgroup per bin (256 at 4096^2 -- far fewer than an H100 can hold), and the
 // per-bin coverage loop is a chain of dependent global loads. Here every bin is split into four 8x8-tile QUADRANTS,
 // each handled by its own CTA (all 256 threads share the (draw, tile) coverage loop, threads 0..63 own a tile each for
 // emission), and the coverage loop keeps two independent tile loads in flight.
-// Segment slices: the WGSL takes one global atomicAdd per CMD_FILL (coarse.wgsl:100), ~1.7 M same-address atomics on a
-// map-like frame, each sitting in the middle of a tile's serial emission chain (tile load -> atomic -> stores). Here
-// the coverage pass, which has every (draw, tile) record in registers anyway, sums the segment counts per tile in
-// shared memory; one atomicAdd per CTA and 256-draw chunk reserves the slices of all 64 tiles, and emission hands them
-// out with plain adds. Fills that emission then skips (inside a zero-coverage clip) leave their reserved slots unused;
-// those are counted in ctl[VB_CTL_SEG_HOLES] so that `bump.segments - holes` is the reference's number.
+// Segment slices: the WGSL takes one global atomicAdd per CMD_FILL (coarse.wgsl:100) and writes ~slice into the tile,
+// ~1.7 M same-address atomics and scattered stores on a map-like frame. Here k_backdrop has already given every
+// (path, tile) its slice in tile order (k_tile.cu), so coarse only reads them: it allocates no segments and writes no
+// tile, and k_path_tiling runs beside it. Slices of tiles that coarse turns into no CMD_FILL (a fill inside a
+// zero-coverage clip, a clip path whose END_CLIP is not emitted) stay unused: ctl[VB_CTL_SEG_HOLES] starts at
+// bump.segments and each CTA subtracts the segments of the fills it emits, so `bump.segments - holes` is the
+// reference's number.
 #include "vb_device.cuh"
 
 #define CO_THREADS 256
+#define CO_MINB 5 // CTAs per SM: 48 registers, no spills
 #define CO_N_SLICE 8
 
 struct TileState {
     uint32_t cmd_offset, cmd_limit;
 };
+
+// A tile as coarse sees it. k_backdrop wrote ~(first slot of the slice) into every tile of the arena in tile order, so a
+// tile's segment count is the distance to the next tile's slice; the arena's last tile ends at bump.segments.
+struct CoTile {
+    int32_t backdrop;
+    uint32_t seg_ix, n_segs;
+};
+__device__ __forceinline__ CoTile co_load_tile(const VbTile *tiles, uint32_t ix, uint32_t tile_end, uint32_t seg_end) {
+    const VbTile t = tiles[ix];
+    const uint32_t next = ix + 1u < tile_end ? ~tiles[ix + 1u].segment_count_or_ix : seg_end;
+    CoTile c;
+    c.backdrop = t.backdrop;
+    c.seg_ix = ~t.segment_count_or_ix;
+    c.n_segs = next - c.seg_ix;
+    return c;
+}
 
 __device__ __forceinline__ void co_alloc_cmd(TileState &s, uint32_t size, const VbConfig &cfg, VbBump *bump, uint32_t *ptcl) {
     if (s.cmd_offset + size >= s.cmd_limit) {
@@ -43,25 +61,17 @@ __device__ __forceinline__ void co_alloc_cmd(TileState &s, uint32_t size, const 
     }
 }
 
-__device__ __forceinline__ bool co_tag_writes_path(uint32_t tag) { // the draw tags whose emission calls co_write_path
-    return tag == VB_DRAWTAG_FILL_COLOR || tag == VB_DRAWTAG_BLURRED_ROUNDED_RECT || tag == VB_DRAWTAG_FILL_LIN_GRADIENT ||
-           tag == VB_DRAWTAG_FILL_RAD_GRADIENT || tag == VB_DRAWTAG_FILL_SWEEP_GRADIENT || tag == VB_DRAWTAG_FILL_IMAGE ||
-           tag == VB_DRAWTAG_END_CLIP;
-}
-
-// Returns the PTCL offset of the CMD_SOLID it wrote, or 0 when it wrote a CMD_FILL.
-__device__ __forceinline__ uint32_t co_write_path(TileState &s, const VbTile &tile, uint32_t tile_ix, uint32_t draw_flags, const VbConfig &cfg,
-                                                  VbBump *bump, uint32_t *ptcl, VbTile *tiles, uint32_t &seg_next, uint32_t &cost) {
-    const uint32_t n_segs = tile.segment_count_or_ix;
+// Returns the PTCL offset of the CMD_SOLID it wrote, or 0 when it wrote a CMD_FILL (whose segments it adds to `emitted`).
+__device__ __forceinline__ uint32_t co_write_path(TileState &s, const CoTile &tile, uint32_t draw_flags, const VbConfig &cfg, VbBump *bump,
+                                                  uint32_t *ptcl, uint32_t &emitted, uint32_t &cost) {
+    const uint32_t n_segs = tile.n_segs;
     cost += n_segs != 0u ? 8u + n_segs : 1u; // what fine will spend on it, in rough units (a fill: set-up + its segments)
     if (n_segs != 0u) {
-        const uint32_t seg_ix = seg_next; // reserved for this tile by the coverage pass
-        seg_next += n_segs;
-        tiles[tile_ix].segment_count_or_ix = ~seg_ix;
+        emitted += n_segs;
         co_alloc_cmd(s, 4u, cfg, bump, ptcl);
         ptcl[s.cmd_offset] = VB_CMD_FILL;
         ptcl[s.cmd_offset + 1u] = (n_segs << 1) | (draw_flags & 1u);
-        ptcl[s.cmd_offset + 2u] = seg_ix;
+        ptcl[s.cmd_offset + 2u] = tile.seg_ix;
         ptcl[s.cmd_offset + 3u] = (uint32_t)tile.backdrop;
         s.cmd_offset += 4u;
         return 0u;
@@ -72,10 +82,10 @@ __device__ __forceinline__ uint32_t co_write_path(TileState &s, const VbTile &ti
     return s.cmd_offset - 1u;
 }
 
-__global__ void __launch_bounds__(CO_THREADS)
+__global__ void __launch_bounds__(CO_THREADS, CO_MINB)
 k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *__restrict__ draw_monoids,
          const VbBinHeader *__restrict__ bin_headers, const uint32_t *__restrict__ info_bin_data, const VbPath *__restrict__ paths,
-         VbTile *tiles, VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, uint2 *cls_list, uint32_t cls_stride) {
+         const VbTile *__restrict__ tiles, VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, uint2 *cls_list, uint32_t cls_stride) {
     __shared__ uint32_t sh_bitmaps[CO_N_SLICE][VB_N_TILE];
     __shared__ uint32_t sh_part_count[CO_THREADS];
     __shared__ uint32_t sh_part_offsets[CO_THREADS];
@@ -92,17 +102,16 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     __shared__ uint32_t sh_di[CO_THREADS];     // info word offset
     __shared__ uint32_t sh_dflags[CO_THREADS]; // bit0 even-odd, bit1 non-trivial blend (clip objects)
     __shared__ uint32_t sh_scan[CO_THREADS / 32 + 2];
-    __shared__ uint32_t sh_tile_segs[64]; // per tile of the quadrant: segments its fills of this chunk need
-    __shared__ uint32_t sh_seg_base;
 
     const uint32_t lid = threadIdx.x;
     // Only PRIOR stages abort coarse (coarse.wgsl:164-179); read once per CTA so the decision is
-    // uniform even while other CTAs of this kernel raise VB_STAGE_COARSE.
-    if (lid == 0) sh_scan[0] = bump->failed & (VB_STAGE_BINNING | VB_STAGE_TILE_ALLOC | VB_STAGE_FLATTEN | VB_STAGE_PATH_COUNT);
+    // uniform even while other CTAs of this kernel raise VB_STAGE_COARSE (and k_path_tiling, beside it, FINE_SEGMENTS).
+    if (lid == 0) sh_scan[0] = bump->failed & VB_STAGES_BEFORE_COARSE;
     __syncthreads();
     const uint32_t prior_failed = sh_scan[0];
     __syncthreads();
     if (prior_failed != 0u) return;
+    const uint32_t tile_end = min(bump->tile, cfg.tiles_size), seg_end = bump->segments; // final since k_backdrop
     const uint32_t wg_x = blockIdx.x >> 1, wg_y = (blockIdx.y >> 1) + cfg.win_by0;
     const int32_t qx0 = (int32_t)(blockIdx.x & 1u) * 8, qy0 = (int32_t)(blockIdx.y & 1u) * 8; // quadrant origin in bin tiles
     const uint32_t width_in_bins = (cfg.width_in_tiles + VB_N_TILE_X - 1u) / VB_N_TILE_X;
@@ -122,12 +131,12 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     uint32_t render_blend_depth = 0u, max_blend_depth = 0u;
     uint32_t cull_start = 0u; // PTCL offset of the CMD_SOLID of this tile's last opaque full-tile cover (0: none)
     uint32_t cost = 0u;       // estimated work of fine on this tile from its occlusion start (orders fine's tile queue)
+    uint32_t emitted = 0u;    // segments of the CMD_FILLs written for this tile
     const uint32_t blend_offset = st.cmd_offset;
     st.cmd_offset += 1u;
 
     while (true) {
         for (int i = 0; i < CO_N_SLICE; i++) sh_bitmaps[i][lid] = 0u;
-        if (lid < 64u) sh_tile_segs[lid] = 0u;
         while (true) {
             if (ready_ix == wr_ix && partition_ix < n_partitions) {
                 part_start_ix = ready_ix;
@@ -199,7 +208,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
         __syncthreads();
         for (uint32_t ix0 = lid; ix0 < total_tile_count; ix0 += 2u * VB_N_TILE) {
             uint32_t el[2], tix[2], bit[2];
-            VbTile tl[2];
+            CoTile tl[2];
             bool ok[2];
 #pragma unroll
             for (int u = 0; u < 2; u++) {
@@ -224,7 +233,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
             }
 #pragma unroll
             for (int u = 0; u < 2; u++)
-                if (ok[u]) tl[u] = tiles[tix[u]]; // independent loads in flight
+                if (ok[u]) tl[u] = co_load_tile(tiles, tix[u], tile_end, seg_end); // independent loads in flight
 #pragma unroll
             for (int u = 0; u < 2; u++) {
                 if (!ok[u]) continue;
@@ -234,39 +243,20 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 const uint32_t fl = sh_dflags[el_ix];
                 const bool is_blend = (fl & 2u) != 0u;
                 const bool even_odd = (fl & 1u) != 0u;
-                const uint32_t n_segs = tl[u].segment_count_or_ix;
                 const bool backdrop_clear = (even_odd ? (abs(tl[u].backdrop) & 1) : tl[u].backdrop) == 0;
-                const bool include_tile = n_segs != 0u || (backdrop_clear == is_clip) || is_blend;
-                if (include_tile) {
-                    atomicOr(&sh_bitmaps[el_ix / 32u][bit[u]], 1u << (el_ix & 31u));
-                    if (n_segs != 0u && co_tag_writes_path(dtag)) atomicAdd(&sh_tile_segs[bit[u]], n_segs);
-                }
+                const bool include_tile = tl[u].n_segs != 0u || (backdrop_clear == is_clip) || is_blend;
+                if (include_tile) atomicOr(&sh_bitmaps[el_ix / 32u][bit[u]], 1u << (el_ix & 31u));
             }
         }
         __syncthreads();
-        // reserve the segment slices of this chunk: one global atomic for the CTA
-        uint32_t seg_next, seg_end;
-        {
-            const uint32_t mine = owns_tile ? sh_tile_segs[lid] : 0u; // the owners are warps 0 and 1
-            const uint32_t incl = vb_warp_incl_scan(mine);
-            if (lid == 31u || lid == 63u) sh_scan[lid >> 5] = incl;
-            __syncthreads();
-            if (lid == 0u) {
-                const uint32_t chunk_total = sh_scan[0] + sh_scan[1];
-                sh_seg_base = chunk_total != 0u ? atomicAdd(&bump->segments, chunk_total) : 0u;
-            }
-            __syncthreads();
-            seg_next = sh_seg_base + incl - mine + (lid >= 32u ? sh_scan[0] : 0u);
-            seg_end = seg_next + mine;
-        }
 
         // emission: each owner walks the set bits of its tile in draw order. The tile record of the NEXT element is
         // requested before the current one is emitted, so the walk is not a chain of exposed global-load latencies.
         uint32_t slice_ix = 0u;
         uint32_t bitmap = owns_tile ? sh_bitmaps[0][lid] : 0u;
-        uint32_t nx_el = 0u, nx_tile_ix = 0u;
-        VbTile nx_tile;
-        nx_tile.backdrop = 0; nx_tile.segment_count_or_ix = 0u;
+        uint32_t nx_el = 0u;
+        CoTile nx_tile;
+        nx_tile.backdrop = 0; nx_tile.seg_ix = 0u; nx_tile.n_segs = 0u;
         bool nx_have = false;
         auto advance = [&]() {
             nx_have = false;
@@ -279,16 +269,15 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 }
                 nx_el = slice_ix * 32u + (uint32_t)(__ffs((int)bitmap) - 1);
                 bitmap &= bitmap - 1u;
-                nx_tile_ix = sh_tile_base[nx_el] + sh_tile_stride[nx_el] * tile_y + tile_x;
-                nx_tile = tiles[nx_tile_ix];
+                nx_tile = co_load_tile(tiles, sh_tile_base[nx_el] + sh_tile_stride[nx_el] * tile_y + tile_x, tile_end, seg_end);
                 nx_have = true;
                 break;
             }
         };
         advance();
         while (nx_have) {
-            const uint32_t el_ix = nx_el, tile_ix = nx_tile_ix;
-            const VbTile tile = nx_tile;
+            const uint32_t el_ix = nx_el;
+            const CoTile tile = nx_tile;
             advance();
             const uint32_t drawtag = sh_tag[el_ix];
             const uint32_t dd = sh_dd[el_ix];
@@ -297,7 +286,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
             if (clip_zero_depth == 0u) {
                 switch (drawtag) {
                 case VB_DRAWTAG_FILL_COLOR: {
-                    const uint32_t solid_at = co_write_path(st, tile, tile_ix, draw_flags, cfg, bump, ptcl, tiles, seg_next, cost);
+                    const uint32_t solid_at = co_write_path(st, tile, draw_flags, cfg, bump, ptcl, emitted, cost);
                     const uint32_t rgba = vb_scene(scene, cfg, dd);
                     co_alloc_cmd(st, 2u, cfg, bump, ptcl);
                     ptcl[st.cmd_offset] = VB_CMD_COLOR;
@@ -312,7 +301,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                     break;
                 }
                 case VB_DRAWTAG_BLURRED_ROUNDED_RECT:
-                    co_write_path(st, tile, tile_ix, draw_flags, cfg, bump, ptcl, tiles, seg_next, cost);
+                    co_write_path(st, tile, draw_flags, cfg, bump, ptcl, emitted, cost);
                     co_alloc_cmd(st, 3u, cfg, bump, ptcl);
                     ptcl[st.cmd_offset] = VB_CMD_BLUR_RECT;
                     ptcl[st.cmd_offset + 1u] = di + 1u;
@@ -325,7 +314,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 case VB_DRAWTAG_FILL_SWEEP_GRADIENT: {
                     const uint32_t ty = drawtag == VB_DRAWTAG_FILL_LIN_GRADIENT ? VB_CMD_LIN_GRAD
                                         : drawtag == VB_DRAWTAG_FILL_RAD_GRADIENT ? VB_CMD_RAD_GRAD : VB_CMD_SWEEP_GRAD;
-                    co_write_path(st, tile, tile_ix, draw_flags, cfg, bump, ptcl, tiles, seg_next, cost);
+                    co_write_path(st, tile, draw_flags, cfg, bump, ptcl, emitted, cost);
                     co_alloc_cmd(st, 3u, cfg, bump, ptcl);
                     ptcl[st.cmd_offset] = ty;
                     ptcl[st.cmd_offset + 1u] = vb_scene(scene, cfg, dd);
@@ -335,7 +324,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                     break;
                 }
                 case VB_DRAWTAG_FILL_IMAGE:
-                    co_write_path(st, tile, tile_ix, draw_flags, cfg, bump, ptcl, tiles, seg_next, cost);
+                    co_write_path(st, tile, draw_flags, cfg, bump, ptcl, emitted, cost);
                     co_alloc_cmd(st, 2u, cfg, bump, ptcl);
                     ptcl[st.cmd_offset] = VB_CMD_IMAGE;
                     ptcl[st.cmd_offset + 1u] = di + 1u;
@@ -345,7 +334,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 case VB_DRAWTAG_BEGIN_CLIP: {
                     const bool even_odd = (draw_flags & 1u) != 0u;
                     const bool backdrop_clear = (even_odd ? (abs(tile.backdrop) & 1) : tile.backdrop) == 0;
-                    if (tile.segment_count_or_ix == 0u && backdrop_clear) {
+                    if (tile.n_segs == 0u && backdrop_clear) {
                         clip_zero_depth = clip_depth + 1u;
                     } else {
                         co_alloc_cmd(st, 1u, cfg, bump, ptcl);
@@ -360,7 +349,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 }
                 case VB_DRAWTAG_END_CLIP:
                     clip_depth -= 1u;
-                    co_write_path(st, tile, tile_ix, draw_flags, cfg, bump, ptcl, tiles, seg_next, cost);
+                    co_write_path(st, tile, draw_flags, cfg, bump, ptcl, emitted, cost);
                     co_alloc_cmd(st, 3u, cfg, bump, ptcl);
                     ptcl[st.cmd_offset] = VB_CMD_END_CLIP;
                     ptcl[st.cmd_offset + 1u] = vb_scene(scene, cfg, dd);
@@ -380,7 +369,6 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 }
             }
         }
-        if (seg_next != seg_end) atomicAdd(reinterpret_cast<uint32_t *>(bump) + VB_CTL_SEG_HOLES, seg_end - seg_next);
         rd_ix += VB_N_TILE;
         if (rd_ix >= ready_ix && partition_ix >= n_partitions) break;
         __syncthreads();
@@ -418,14 +406,17 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                 if (slot < cls_stride) cls_list[(size_t)k * cls_stride + slot] = make_uint2((ty - cfg.win_ty0) * cfg.width_in_tiles + tx, cull_start);
             }
         }
+        // the slots these fills use are not holes (k_backdrop set holes to every slot of the frame)
+        const uint32_t used = vb_warp_sum(emitted);
+        if (lane == 0u && used != 0u) atomicSub(reinterpret_cast<uint32_t *>(bump) + VB_CTL_SEG_HOLES, used);
     }
 }
 
 // The segments-arena overflow check (the reference sizes `segments` statically and never checks) lives at the top of
-// k_path_tiling, the next kernel.
+// k_path_tiling, which runs beside coarse.
 
 extern "C" uint32_t vb_launch_coarse(const VbConfig *cfg, const uint32_t *scene, const VbDrawMonoid *draw_monoids,
-                                 const VbBinHeader *bin_headers, const uint32_t *info_bin_data, const VbPath *paths, VbTile *tiles,
+                                 const VbBinHeader *bin_headers, const uint32_t *info_bin_data, const VbPath *paths, const VbTile *tiles,
                                  VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, void *cls_list, uint32_t cls_stride, cudaStream_t st) {
     uint32_t width_in_bins = (cfg->width_in_tiles + 15u) / 16u;
     uint32_t rows = cfg->win_by1 - cfg->win_by0;

@@ -3,6 +3,9 @@
 // Reference: vello_shaders/shader/path_tiling.wgsl:40-172 (+ path_tiling_setup.wgsl), CPU twin
 // cpu/path_tiling.rs. One thread per crossing (SegmentCount record); no indirect dispatch: the grid
 // is sized from the arena and strides over bump.seg_counts read on the device.
+// Slices: k_backdrop gives every (path, tile) with crossings its slice, so this kernel does not wait for coarse; the
+// two run side by side on two streams (vb_api.cu). Crossings of tiles that coarse emits no CMD_FILL for are still
+// written, into slots no command reads (the reference, which allocates in coarse, skips them).
 // Algorithmic bytes per crossing: 8 (SegmentCount) + 24 (LineSoup gather) + 32 (Path) + 8 (Tile)
 // read, 24 written (scattered into the tile's slice).
 #include "vb_device.cuh"
@@ -21,10 +24,11 @@ __global__ void __launch_bounds__(PTI_THREADS, PTI_MINB)
 k_path_tiling(VbConfig cfg, VbBump *bump, const VbSegmentCount *__restrict__ seg_counts,
               const VbLineSoup *__restrict__ lines, const VbPath *__restrict__ paths, const VbTile *__restrict__ tiles,
               VbSegment *segments) {
-    // coarse reserved more segment slots than the arena holds: flagged here (one thread), decided by every CTA alike
+    // backdrop assigned more segment slots than the arena holds: flagged here (one thread), decided by every CTA alike.
+    // Only the stages before coarse abort this kernel: coarse, running beside it, may raise its bit at any time.
     const bool seg_overflow = bump->segments > cfg.segments_size;
     if (seg_overflow && blockIdx.x == 0u && threadIdx.x == 0u) atomicOr(&bump->failed, VB_STAGE_FINE_SEGMENTS);
-    if (bump->failed != 0u || seg_overflow) return;
+    if ((bump->failed & VB_STAGES_BEFORE_COARSE) != 0u || seg_overflow) return;
     const uint32_t n_segments = min(bump->seg_counts, cfg.seg_counts_size);
     for (uint32_t g = blockIdx.x * PTI_THREADS + threadIdx.x; g < n_segments; g += gridDim.x * PTI_THREADS) {
         const VbSegmentCount sc = seg_counts[g];
@@ -62,9 +66,7 @@ k_path_tiling(VbConfig cfg, VbBump *bump, const VbSegmentCount *__restrict__ seg
         const int32_t bx0 = (int32_t)path.bbox[0], by0 = (int32_t)path.bbox[1], bx1 = (int32_t)path.bbox[2];
         const int32_t stride = bx1 - bx0;
         const int32_t tile_ix = (int32_t)path.tiles + (y - by0) * stride + x - bx0;
-        const VbTile tile = tiles[tile_ix];
-        const uint32_t seg_start = ~tile.segment_count_or_ix;
-        if ((int32_t)seg_start < 0) continue;
+        const uint32_t seg_start = ~tiles[tile_ix].segment_count_or_ix; // every tile has its slice (k_backdrop)
         const float tile_x = (float)x * 16.0f, tile_y = (float)y * 16.0f;
         const float tile_x1 = tile_x + 16.0f, tile_y1 = tile_y + 16.0f;
         if (seg_within_line > 0u) {

@@ -6,7 +6,8 @@
 // Design: tile_alloc's per-workgroup atomicAdd(bump.tile) becomes a decoupled look-back scan,
 // so `Path.tiles` offsets are deterministic and equal to the serial CPU shader's -- `tiles[]` can be
 // compared byte for byte. The allocated range is zeroed by a grid-wide pass (k_tile_zero). backdrop streams the
-// arena as contiguous per-CTA ranges (see k_backdrop).
+// arena as contiguous per-CTA ranges and also assigns every tile its segment slice, which the reference leaves to
+// coarse, so that path_tiling and coarse can run side by side (see k_backdrop).
 // Extension: tile rows are clamped to the stripe window [win_ty0, win_ty1).
 #include "vb_device.cuh"
 
@@ -74,27 +75,45 @@ __global__ void __launch_bounds__(256) k_tile_zero(VbConfig cfg, const VbBump *_
     if ((end & 1u) != 0u && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<uint2 *>(tiles)[end - 1u] = make_uint2(0u, 0u);
 }
 
-// backdrop: per (path, tile row) inclusive prefix sum along x (backdrop_dyn.wgsl:66-84).
+// backdrop: per (path, tile row) inclusive prefix sum along x (backdrop_dyn.wgsl:66-84), and the segment slices.
 // Design: the WGSL assigns one thread per row, walking 8-byte tiles at a stride of the row width (uncoalesced).
 // tile_alloc hands out tiles in draw order, so the tiles of 32 consecutive paths are ONE contiguous range of the arena,
-// made of rows laid end to end. A CTA owns that range; it is cut into 8 x gridDim.y pieces of equal size, each piece
-// moved to whole-row boundaries, and one warp streams its piece 128 consecutive tiles at a time (four independent
-// coalesced loads per lane in flight) through a segmented warp-shuffle scan whose segments are the rows. Groups whose
-// deltas are all zero -- most of the arena -- are skipped after the load. Integer sums: identical results.
+// made of rows laid end to end. A group of `split` CTAs owns that range; it is cut into 8 x split pieces of equal size,
+// each piece moved to whole-row boundaries, and one warp streams its piece 128 consecutive tiles at a time (four
+// independent coalesced loads per lane in flight) through a segmented warp-shuffle scan whose segments are the rows.
+// Groups whose deltas are all zero -- most of the arena -- skip the scan. Integer sums: identical results.
+// Segment slices (the reference allocates one per CMD_FILL in coarse, coarse.wgsl:100): path_count left each tile's
+// crossing count in `segment_count_or_ix`, so an exclusive scan of the counts in tile order gives every (path, tile) its
+// slice without waiting for coarse. Each CTA first sums the counts of its pieces, a decoupled look-back over the CTAs
+// (ticketed; CTA order = tile order) turns the sums into bases, and the backdrop pass then writes every tile whole:
+// {backdrop, ~first slot of its slice}. A tile's count is the difference to the next tile's slice start (the arena's
+// last tile ends at bump.segments), so coarse recovers it without another buffer. bump.segments is the total, which
+// includes the slices of tiles that coarse turns into no CMD_FILL; ctl[VB_CTL_SEG_HOLES] starts at the total and
+// coarse subtracts what its fills take, so `bump.segments - holes` is the reference's count.
 #define BD_THREADS 256
 #define BD_WARPS (BD_THREADS / 32)
-#define BD_PATHS 32u // paths per CTA
+#define BD_PATHS 32u // paths per CTA group
+static void bd_grid(uint32_t n_draw, int sm_count, uint32_t *groups, uint32_t *split) {
+    *groups = (n_draw + BD_PATHS - 1) / BD_PATHS;
+    const uint32_t s = *groups ? ((uint32_t)sm_count * 4u + *groups - 1u) / *groups : 1u;
+    *split = s > 64u ? 64u : s;
+}
 __global__ void __launch_bounds__(BD_THREADS)
-k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile *tiles) {
+k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile *tiles, uint32_t *lb_mem, uint32_t split) {
     __shared__ uint32_t sh_start[BD_PATHS + 1]; // first tile of each path, then the end of the range
     __shared__ uint32_t sh_width[BD_PATHS];
+    __shared__ uint32_t sh_seg[BD_WARPS]; // segments of each warp's piece, then the first slot of the piece
+    __shared__ uint32_t sh_ticket;
     // path_count's worklist overflow (the WGSL checks it at the top of coarse) is detected here, by every CTA alike, and
     // published by one thread: a separate one-thread check kernel used to sit on the frame's critical path
     const bool pc_overflow = bump->seg_counts > cfg.seg_counts_size;
-    if (pc_overflow && blockIdx.x == 0u && blockIdx.y == 0u && threadIdx.x == 0u) atomicOr(&bump->failed, VB_STAGE_PATH_COUNT);
-    if (bump->failed != 0u || pc_overflow) return;
+    if (pc_overflow && blockIdx.x == 0u && threadIdx.x == 0u) atomicOr(&bump->failed, VB_STAGE_PATH_COUNT);
+    if (bump->failed != 0u || pc_overflow) return; // uniform: every CTA returns, or none (the look-back needs all)
+    const uint32_t n_parts = gridDim.x;
+    const VbLookback lb = vb_lookback_view(lb_mem, n_parts, 1);
+    const uint32_t part = vb_take_ticket(lb, &sh_ticket);
     const uint32_t n_draw = cfg.layout.n_draw_objects;
-    const uint32_t p0 = blockIdx.x * BD_PATHS;
+    const uint32_t p0 = (part / split) * BD_PATHS;
     const uint32_t arena_end = min(bump->tile, cfg.tiles_size);
     if (threadIdx.x <= BD_PATHS) {
         const uint32_t p = p0 + threadIdx.x;
@@ -110,7 +129,6 @@ k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile 
     __syncthreads();
     const uint32_t lane = vb_lane();
     const uint32_t r0 = sh_start[0], r1 = sh_start[BD_PATHS];
-    if (r1 <= r0) return;
     // the path owning tile t (the last path starting at or before t; empty paths share their successor's start) and
     // t's column inside its row
     auto column = [&](uint32_t t, uint32_t &w) -> uint32_t {
@@ -127,38 +145,77 @@ k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile 
         const uint32_t x = column(t, w);
         return x == 0u ? t : min(t + (w - x), r1);
     };
-    const uint32_t pieces = BD_WARPS * gridDim.y;
-    const uint32_t piece = blockIdx.y * BD_WARPS + (threadIdx.x >> 5);
-    const uint32_t len = (r1 - r0 + pieces - 1u) / pieces;
-    const uint64_t na = (uint64_t)r0 + (uint64_t)piece * len;
-    if (na >= r1) return;
-    const uint32_t A = row_align((uint32_t)na);
-    const uint32_t B = row_align((uint32_t)min((uint64_t)r1, na + len));
+    // this warp's piece [A, B) (empty when the range has fewer rows than pieces)
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t pieces = BD_WARPS * split;
+    const uint32_t piece = (part % split) * BD_WARPS + warp;
+    uint32_t A = r1, B = r1;
+    if (r1 > r0) {
+        const uint32_t len = (r1 - r0 + pieces - 1u) / pieces;
+        const uint64_t na = (uint64_t)r0 + (uint64_t)piece * len;
+        if (na < r1) {
+            A = row_align((uint32_t)na);
+            B = row_align((uint32_t)min((uint64_t)r1, na + len));
+        }
+    }
+    // slices: the piece's segment count, the CTA's prefix over its warps, the look-back across CTAs
+    uint32_t n_segs = 0u;
+    for (uint32_t base = A; base < B; base += 256u) {
+        uint32_t c[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const uint32_t idx = base + (uint32_t)k * 32u + lane;
+            c[k] = idx < B ? tiles[idx].segment_count_or_ix : 0u;
+        }
+#pragma unroll
+        for (int k = 0; k < 8; k++) n_segs += c[k];
+    }
+    n_segs = vb_warp_sum(n_segs);
+    if (lane == 0u) sh_seg[warp] = n_segs;
+    __syncthreads();
+    if (warp == 0u) {
+        const uint32_t mine = lane < BD_WARPS ? sh_seg[lane] : 0u;
+        const uint32_t incl = vb_warp_incl_scan(mine);
+        uint32_t agg[1] = {__shfl_sync(VB_FULL, incl, 31)}, excl[1];
+        vb_lookback<1>(lb, part, agg, excl);
+        if (lane < BD_WARPS) sh_seg[lane] = excl[0] + incl - mine;
+        if (lane == 0u && part == n_parts - 1u) {
+            bump->segments = excl[0] + agg[0];
+            reinterpret_cast<uint32_t *>(bump)[VB_CTL_SEG_HOLES] = excl[0] + agg[0]; // coarse subtracts its fills
+        }
+    }
+    __syncthreads();
+    uint32_t seg_next = sh_seg[warp];
     int32_t carry = 0;
     for (uint32_t base = A; base < B; base += 128u) {
-        int32_t v[4];
+        int2 v[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const uint32_t idx = base + (uint32_t)k * 32u + lane;
-            v[k] = idx < B ? tiles[idx].backdrop : 0;
+            v[k] = idx < B ? reinterpret_cast<const int2 *>(tiles)[idx] : make_int2(0, 0);
         }
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const uint32_t idx = base + (uint32_t)k * 32u + lane;
-            if (!__any_sync(VB_FULL, v[k] != 0) && carry == 0) continue; // nothing to propagate in these 32 tiles
             const bool valid = idx < B;
-            uint32_t w;
-            const uint32_t x = valid ? column(idx, w) : 0u;
-            const uint32_t reach = min(x, lane); // elements of my row to my left inside this 32-tile group
-            int32_t s = v[k];
+            const uint32_t count = (uint32_t)v[k].y;
+            const uint32_t count_incl = vb_warp_incl_scan(count);
+            const uint32_t slice = seg_next + count_incl - count;
+            seg_next += __shfl_sync(VB_FULL, count_incl, 31);
+            int32_t s = v[k].x;
+            if (__any_sync(VB_FULL, s != 0) || carry != 0) { // else nothing to propagate in these 32 tiles
+                uint32_t w;
+                const uint32_t x = valid ? column(idx, w) : 0u;
+                const uint32_t reach = min(x, lane); // elements of my row to my left inside this 32-tile group
 #pragma unroll
-            for (uint32_t o = 1u; o < 32u; o <<= 1) {
-                const int32_t t = __shfl_up_sync(VB_FULL, s, o);
-                if (o <= reach) s += t;
+                for (uint32_t o = 1u; o < 32u; o <<= 1) {
+                    const int32_t t = __shfl_up_sync(VB_FULL, s, o);
+                    if (o <= reach) s += t;
+                }
+                if (x > lane) s += carry; // my row started in an earlier group
+                carry = __shfl_sync(VB_FULL, s, 31);
             }
-            if (x > lane) s += carry; // my row started in an earlier group
-            if (valid && x != 0u && s != v[k]) tiles[idx].backdrop = s;
-            carry = __shfl_sync(VB_FULL, s, 31);
+            if (valid) reinterpret_cast<int2 *>(tiles)[idx] = make_int2(s, (int32_t)~slice);
         }
     }
 }
@@ -171,12 +228,17 @@ extern "C" uint32_t vb_launch_tile_alloc(const VbConfig *cfg, const uint32_t *sc
     return 2;
 }
 extern "C" uint32_t vb_tile_alloc_parts(uint32_t n_draw) { return (n_draw + TA_THREADS - 1) / TA_THREADS; }
-extern "C" uint32_t vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, int sm_count, cudaStream_t st) {
-    uint32_t n = cfg->layout.n_draw_objects;
-    if (n == 0) return 0;
-    const uint32_t groups = (n + BD_PATHS - 1) / BD_PATHS;
-    uint32_t split = ((uint32_t)sm_count * 4u + groups - 1u) / groups;
-    if (split > 64u) split = 64u;
-    k_backdrop<<<dim3(groups, split), BD_THREADS, 0, st>>>(*cfg, bump, paths, tiles);
+// look-back partitions of k_backdrop: its CTAs
+extern "C" uint32_t vb_backdrop_parts(uint32_t n_draw, int sm_count) {
+    uint32_t groups, split;
+    bd_grid(n_draw, sm_count, &groups, &split);
+    return groups * split;
+}
+extern "C" uint32_t vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, uint32_t *lb_mem, int sm_count,
+                                       cudaStream_t st) {
+    uint32_t groups, split;
+    bd_grid(cfg->layout.n_draw_objects, sm_count, &groups, &split);
+    if (groups == 0) return 0;
+    k_backdrop<<<groups * split, BD_THREADS, 0, st>>>(*cfg, bump, paths, tiles, lb_mem, split);
     return 1;
 }

@@ -39,11 +39,12 @@ uint32_t vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathB
 uint32_t vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
                           cudaStream_t);
 uint32_t vb_tile_alloc_parts(uint32_t);
-uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, int, cudaStream_t);
+uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, uint32_t *, int, cudaStream_t);
+uint32_t vb_backdrop_parts(uint32_t, int);
 uint32_t vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
                           cudaStream_t);
 uint32_t vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
-                      VbTile *, VbBump *, uint32_t *, uint32_t *, void *, uint32_t, cudaStream_t);
+                      const VbTile *, VbBump *, uint32_t *, uint32_t *, void *, uint32_t, cudaStream_t);
 uint32_t vb_launch_path_tiling(const VbConfig *, VbBump *, const VbSegmentCount *, const VbLineSoup *, const VbPath *, const VbTile *,
                            VbSegment *, uint32_t, cudaStream_t);
 uint32_t vb_launch_fine(const VbConfig *, int, const VbBump *, const VbSegment *, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *,
@@ -201,8 +202,11 @@ struct vb_renderer {
     uint32_t graph_next = 0;
     uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
     uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
-    uint32_t parts_pathtag = 0, parts_flatten = 0, parts_draw = 0, parts_tile = 0;
-    size_t off_lb_pathtag = 0, off_lb_flatten = 0, off_lb_draw = 0, off_lb_tile = 0, off_lb_clip = 0;
+    uint32_t parts_pathtag = 0, parts_flatten = 0, parts_draw = 0, parts_tile = 0, parts_backdrop = 0;
+    size_t off_lb_pathtag = 0, off_lb_flatten = 0, off_lb_draw = 0, off_lb_tile = 0, off_lb_clip = 0, off_lb_backdrop = 0;
+    // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct)
+    cudaStream_t tiling_stream = nullptr;
+    cudaEvent_t tiling_fork = nullptr, tiling_join = nullptr;
     cudaEvent_t ev[VB_N_STAGE_IDS + 1]{};
     cudaEvent_t frame_ev[2]{}; // around every whole frame (vb_last_frame_ms: the signal stripe balancing uses)
     bool frame_timed = false;
@@ -360,7 +364,10 @@ extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, r->device) == cudaSuccess) r->sm_count = prop.multiProcessorCount;
     if (cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess) {
+        cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&r->tiling_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->tiling_fork, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess) {
         delete r;
         return VB_E_CUDA;
     }
@@ -419,6 +426,10 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
         for (auto &gs : r->graphs)
             if (gs.exec) cudaGraphExecDestroy(gs.exec);
     }
+    if (r->tiling_stream) cudaStreamSynchronize(r->tiling_stream);
+    if (r->tiling_fork) cudaEventDestroy(r->tiling_fork);
+    if (r->tiling_join) cudaEventDestroy(r->tiling_join);
+    if (r->tiling_stream) cudaStreamDestroy(r->tiling_stream);
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
     if (r->upload_stream) cudaStreamDestroy(r->upload_stream);
     if (r->stream) cudaStreamDestroy(r->stream);
@@ -576,6 +587,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     r->parts_flatten = vb_flatten_parts(c.n_tag_words);
     r->parts_draw = vb_draw_parts(n_draw);
     r->parts_tile = vb_tile_alloc_parts(n_draw);
+    r->parts_backdrop = vb_backdrop_parts(n_draw, r->sm_count);
     size_t off = VB_CTL_HEADER_WORDS;
     r->off_lb_pathtag = off; off += vb_lookback_words(r->parts_pathtag, 5);
     r->off_lb_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
@@ -583,6 +595,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     r->off_lb_draw = off; off += vb_lookback_words(r->parts_draw, 4);
     r->off_lb_tile = off; off += vb_lookback_words(r->parts_tile, 1);
     r->off_lb_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
+    r->off_lb_backdrop = off; off += vb_lookback_words(r->parts_backdrop, 1);
     r->ctl_words = off;
     if ((rc = ensure(r, r->ctl, off * 4))) return rc;
     if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(r->parts_flatten) * 4))) return rc;
@@ -643,7 +656,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(ctl + VB_CTL_FINE_QUEUE, 0, 8 * sizeof(uint32_t), st));
         if (first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_COARSE)
             CK(cudaMemsetAsync(ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_CLASSES * sizeof(uint32_t), st));
+        if (first <= VB_STAGE_ID_BACKDROP && last >= VB_STAGE_ID_BACKDROP)
+            CK(cudaMemsetAsync(ctl + r->off_lb_backdrop, 0, VB_LB_ZERO_WORDS(r->parts_backdrop) * sizeof(uint32_t), st));
     }
+    // path_tiling and coarse both depend on backdrop only (it assigns the segment slices): path_tiling is forked onto the
+    // tiling stream and joined again before the next stage, so the two kernels share the GPU. Launch counts are unchanged;
+    // with per-stage timing on, the stages stay serial so that each one's events time it alone.
+    const bool fork_tiling = !r->timing && first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_PATH_TILING;
     rec(r, 0);
     for (int s = first; s <= last; s++) {
         switch (s) {
@@ -695,15 +714,27 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
                                              (VbSegmentCount *)r->seg_counts.p, capacity_grid(c.lines_size, r->sm_count), st);
             break;
         case VB_STAGE_ID_BACKDROP:
-            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, r->sm_count, st);
+            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, ctl + r->off_lb_backdrop, r->sm_count, st);
             break;
         case VB_STAGE_ID_COARSE:
+            // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before
+            // path_tiling's grid fills the rest of the GPU
+            if (fork_tiling) CK(cudaEventRecord(r->tiling_fork, st));
             launches += vb_launch_coarse(&c, (const uint32_t *)r->cur->scene.p, (const VbDrawMonoid *)r->draw_monoids.p,
                                          (const VbBinHeader *)r->bin_headers.p, (const uint32_t *)r->info_bin_data.p, (const VbPath *)r->paths.p,
-                                         (VbTile *)r->tiles.p, bump, (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p,
+                                         (const VbTile *)r->tiles.p, bump, (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p,
                                          c.width_in_tiles * c.height_in_tiles, st);
+            if (fork_tiling) {
+                CK(cudaStreamWaitEvent(r->tiling_stream, r->tiling_fork, 0));
+                launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
+                                                  (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p,
+                                                  capacity_grid(c.seg_counts_size, r->sm_count), r->tiling_stream);
+                CK(cudaEventRecord(r->tiling_join, r->tiling_stream));
+                CK(cudaStreamWaitEvent(st, r->tiling_join, 0));
+            }
             break;
         case VB_STAGE_ID_PATH_TILING:
+            if (fork_tiling) break; // launched beside coarse
             launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
                                               (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p,
                                               capacity_grid(c.seg_counts_size, r->sm_count), st);
@@ -1228,7 +1259,7 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
         if (dst && cap >= sizeof(VbBump)) CK(cudaMemcpy(dst, r->ctl.p, sizeof(VbBump), cudaMemcpyDeviceToHost));
         return VB_OK;
     }
-    if (!strcmp(name, "seg_holes")) { // reserved-but-unused segment slots of the last frame (k_coarse.cu)
+    if (!strcmp(name, "seg_holes")) { // segment slots of the last frame that backdrop assigned and no CMD_FILL uses (k_tile.cu, k_coarse.cu)
         if (bytes) *bytes = 4;
         if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->ctl.p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
         return VB_OK;

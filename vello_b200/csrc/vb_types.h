@@ -22,8 +22,9 @@ typedef struct { int32_t backdrop; uint32_t segment_count_or_ix; } VbTile;
 typedef struct { uint32_t line_ix, counts; } VbSegmentCount;
 typedef struct { float p0[2], p1[2]; float y_edge; uint32_t _pad; } VbSegment;
 typedef struct { uint32_t failed, binning, ptcl, tile, seg_counts, segments, blend, lines; } VbBump;
-/* The control block starts with VbBump (8 words) padded to 16; word 8 counts segment slots that coarse reserved but did
- * not hand out (fills skipped inside a zero-coverage clip): bump.segments - holes = the reference's bump.segments. */
+/* The control block starts with VbBump (8 words) padded to 16; word 8 counts segment slots that backdrop assigned but no
+ * CMD_FILL of coarse uses (fills skipped inside a zero-coverage clip, ...): bump.segments - holes = the reference's
+ * bump.segments. */
 #define VB_CTL_SEG_HOLES 8
 /* words 16..23: fine's tile queues, one per launch of a frame (up to 8 read-back bands); the header is 32 words */
 #define VB_CTL_FINE_QUEUE 16
@@ -61,8 +62,10 @@ typedef struct {
 #define VB_STAGE_FLATTEN 0x4u
 #define VB_STAGE_PATH_COUNT 0x8u
 #define VB_STAGE_COARSE 0x10u
-#define VB_STAGE_FINE_SEGMENTS 0x20u /* extension: segments arena too small (reserved in coarse, checked in k_path_tiling) */
+#define VB_STAGE_FINE_SEGMENTS 0x20u /* extension: segments arena too small (assigned in k_backdrop, checked in k_path_tiling) */
 #define VB_STAGE_EXCHANGE 0x40u      /* extension: multi-GPU line exchange (outbox too small, or a peer never signalled) */
+/* the bits coarse and path_tiling skip on: every stage before them. Not each other's: the two run side by side. */
+#define VB_STAGES_BEFORE_COARSE (VB_STAGE_BINNING | VB_STAGE_TILE_ALLOC | VB_STAGE_FLATTEN | VB_STAGE_PATH_COUNT | VB_STAGE_EXCHANGE)
 
 #define VB_TILE_WIDTH 16u
 #define VB_TILE_HEIGHT 16u
