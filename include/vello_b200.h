@@ -136,7 +136,8 @@ int vb_set_timing(vb_renderer *, int on);
 void *vb_target(vb_renderer *, size_t *bytes);
 /* Copy `bytes` from a device pointer to a host pointer on the renderer's stream, then synchronise. */
 int vb_copy_to_host(vb_renderer *, const void *src_device, void *dst_host, size_t bytes);
-/* cudaStream_t the renderer enqueues on (for event timing by the caller). */
+/* cudaStream_t the renderer enqueues on (for event timing by the caller). Writes to an overridden image's device pixels
+ * (vb_override_image) that are enqueued on this stream before the copying call are ordered before the copy. */
 void *vb_stream(vb_renderer *);
 
 /* ---- stage-level access (parity tests; mirrors the reference's CPU-shader operator seam) ----
@@ -180,7 +181,8 @@ int vb_debug_fine_traffic(vb_renderer *, uint64_t *ptcl_words, uint64_t *segment
  * late-bound patches (resolve.rs:560-590): each stream is copied straight to its Layout offset inside the packed buffer in
  * device memory, and a kernel finishes the job there -- tag padding, the trailing PATH / END_CLIP tags of unclosed clips, the
  * ramp-id and atlas-position patches, and the gradient ramps themselves (one thread per texel). The images go into the atlas
- * with one 2-D copy each. Only sizes, the ramp de-duplication and the atlas shelf placement stay on the host. The resulting
+ * with one 2-D copy each from host memory, except those with an override (vb_override_image below), which come from device
+ * memory with one k_atlas_blit launch for all of them. Only sizes, the ramp de-duplication and the atlas shelf placement stay on the host. The resulting
  * device buffers are byte-identical to what vb_scene_upload receives from the host-side resolve (tests/test_gpu_parity.py).
  * Glyph runs are not part of this path (they are resolved to outlines above the boundary). */
 typedef struct { float offset, r, g, b, a; } vb_ramp_stop; /* straight-alpha colour */
@@ -209,6 +211,29 @@ typedef struct {
 int vb_scene_upload_streams(vb_renderer *, const vb_encoding_streams *, vb_layout *layout_out);
 /* Render the uploaded scene and deliver the pixels like vb_render does (host pointer with out_is_device == 0, device otherwise). */
 int vb_render_uploaded(vb_renderer *, const vb_params *, void *out, uint32_t out_is_device, vb_frame_stats *);
+
+/* ---- images drawn from device memory: Renderer::override_image / mark_override_image_dirty (vello/src/lib.rs:536-603) ----
+ * An image is named by its key: the `pixels` pointer of its vb_image / vb_image_patch (the atlas already shares one slot per
+ * key, like vello's blob id). With an override, every image of that key (and these dimensions) is copied into its atlas slot
+ * from `device_pixels` by the device resolve (vb_scene_upload_streams / vb_scene_upload_device) with one k_atlas_blit for all
+ * overridden images, instead of from the key's host memory. device_pixels: RGBA8 / BGRA8 rows (the vb_image's format decides),
+ * row_pitch_bytes apart, in memory of the renderer's device (or managed memory); pointer and pitch multiples of 4, pitch >=
+ * 4 * width, no dimension 0 -- else VB_E_INVALID (vb_last_error says why). device_pixels NULL removes the override.
+ * Setting an override marks the image dirty.
+ *
+ * vello's semantics: the device resolve records where each overridden image sits in this renderer's atlas. A dirty image is
+ * copied again in front of the next frame rendered from that scene (on vb_stream, before every kernel of the frame and outside
+ * any captured graph; the atlas does not move, so frames keep replaying); a frame with nothing dirty enqueues nothing extra and
+ * its kernel_launches do not count the copy. An image that is not marked dirty keeps the pixels copied last. Removing an override,
+ * or giving it another size, takes effect at the next device resolve. The caller finishes or orders its writes to device_pixels
+ * (e.g. on vb_stream, or with a stream synchronisation) before the call that copies them: vb_scene_upload_streams, or the next
+ * frame after vb_mark_override_image_dirty. Because the copy precedes the frame's kernels in stream order, a frame may draw its
+ * own destination buffer (e.g. the previous frame) as an image: it reads the old contents.
+ * The device resolve returns VB_E_INVALID when an override's size differs from its image's. Caller-packed atlases
+ * (vb_scene_upload, vb_render, vb_render_begin) and vb_group ignore overrides. */
+int vb_override_image(vb_renderer *, const void *key, uint32_t width, uint32_t height, const void *device_pixels, size_t row_pitch_bytes);
+/* Recopy the overridden image `key` before the next frame that renders from this renderer's atlas. VB_E_INVALID: no override. */
+int vb_mark_override_image_dirty(vb_renderer *, const void *key);
 
 /* ---- one frame on several GPUs of one box (SURVEY.md 8e, north_star: "a single frame shards across the GPUs by stripes") ----
  * The frame is cut into horizontal stripes of tile rows, one per device; every device runs the element stages on the scene and

@@ -162,6 +162,17 @@ int vb_render_scene(vb_renderer *, vb_scene *, const vb_params *, void *out, uin
 /* The first half of vb_render_scene: resolve the scene's streams on the device (vb_scene_upload_streams) and leave them uploaded. */
 int vb_scene_upload_device(vb_renderer *, vb_scene *, vb_layout *layout_out);
 
+/* Renderer::register_texture / unregister_texture (vello/src/lib.rs:578-603): draw pixels that live in device memory.
+ * vb_register_texture fills *out with a fresh key as `pixels` -- an address that no host buffer can have, kept in one
+ * process-wide registry -- and the size, and sets an override of that key to device_pixels on this renderer (vb_override_image,
+ * same checks). The pixels are RGBA8 with straight alpha (vello's assumption: format 0, alpha_type 0); quality (medium),
+ * extends (pad) and alpha (1) are defaults the caller may change. The host resolve (vb_scene_resolve) never reads through such a
+ * key and leaves its atlas region zero; a device resolve on a renderer without an override of the key returns VB_E_INVALID
+ * (vello panics), so a texture registered on one renderer is not drawn by another. vb_unregister_texture (on the registering
+ * renderer) removes the key and its override; its atlas region keeps the pixels copied last until the next device resolve. */
+int vb_register_texture(vb_renderer *, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes, vb_image *out);
+int vb_unregister_texture(vb_renderer *, const vb_image *);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,9 +10,12 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <sys/mman.h>
 
 #include <algorithm>
+#include <mutex>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/vello_b200.h"
@@ -67,6 +70,9 @@ extern "C" uint32_t vb_launch_exchange_send(const void *, VbBump *, uint32_t, Vb
 extern "C" uint32_t vb_launch_exchange_recv(const void *, VbBump *, uint32_t, VbLineSoup *, VbPathBbox *, int, cudaStream_t);
 extern "C" void vb_launch_resolve_finish(uint32_t *, uint32_t, uint32_t, uint32_t, uint32_t, const void *, uint32_t, cudaStream_t);
 extern "C" void vb_launch_make_ramps(const void *, const void *, uint32_t, uint32_t *, cudaStream_t);
+// k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch
+extern "C" uint32_t vb_atlas_blit_units_per_row(uint32_t w);
+extern "C" uint32_t vb_launch_atlas_blit(const VbBlitRect *, uint32_t, uint64_t, uint8_t *, uint32_t, cudaStream_t);
 
 // path_tiling_setup.wgsl:21-26 flags a failed frame to fine through ptcl[0] = ~0. That word is also tile 0's blend offset
 // and is only rewritten when coarse visits tile 0 -- which a stripe window with bin_row0 > 0 never does, so the flag of a
@@ -177,6 +183,16 @@ struct vb_renderer {
         DevBuf scene, ramps, atlas;
         VbBump *h_bump = nullptr;     // pinned + mapped: the device writes the counters straight into host memory
         VbBump *h_bump_dev = nullptr; // device-side address of h_bump
+        // the images of the last device resolve that were copied from an override, with their atlas places: a dirty one is
+        // copied again before the next frame (refresh_overrides), without a new resolve
+        struct OverridePlace {
+            const void *key;
+            const uint8_t *src;
+            size_t pitch;
+            uint32_t w, h, x, y;
+            bool dirty;
+        };
+        std::vector<OverridePlace> overridden;
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -184,6 +200,17 @@ struct vb_renderer {
     // fixed-size intermediates
     DevBuf tag_monoids, path_bboxes, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
         ctl, target, target_alt, tile_start, cls_list;
+    // Renderer::override_image: images (by key) whose pixels come from device memory at the device resolve
+    struct Override {
+        const uint8_t *src;
+        size_t pitch;
+        uint32_t w, h;
+    };
+    std::unordered_map<const void *, Override> overrides;
+    DevBuf blit_rects;                  // k_atlas_blit's rectangles, staged through blit_host (pinned)
+    VbBlitRect *blit_host = nullptr;
+    size_t blit_host_cap = 0;           // rectangles
+    cudaEvent_t blit_staged = nullptr;  // the last copy out of blit_host
     // bump arenas (ARENAS), capacities in elements
     DevBuf resolve_tmp; // patches, ramp descriptors and stops of vb_scene_upload_streams
     DevBuf lines, line_scratch, flatten_jobs, flatten_parts, tiles, seg_counts, segments, ptcl, blend_spill;
@@ -251,7 +278,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                              &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers,
                              &r->paths, &r->ctl, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs,
                              &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
-    DevBuf *const unkeyed[] = {&o.scene, &o.ramps, &o.atlas, &r->target, &r->target_alt, &r->resolve_tmp, &r->xc.arena};
+    DevBuf *const unkeyed[] = {&o.scene, &o.ramps, &o.atlas, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena};
     for (DevBuf *b : keyed) f(*b, true);
     for (DevBuf *b : unkeyed) f(*b, false);
 }
@@ -322,6 +349,38 @@ static int ensure_arena(vb_renderer *r, int a) {
     return ensure(r, r->flatten_jobs, job_bytes);
 }
 
+// Keys of registered textures (vb_register_texture). Each is a fresh address inside one reserved, inaccessible (PROT_NONE)
+// range of the process's address space, so no host buffer can have it, even after the texture is unregistered: the host
+// resolve recognises such a key by its address alone and never reads through it (vb_texture_key). The range is never
+// unmapped and a key is never handed out twice. `owner` is the renderer that registered the key.
+static std::mutex g_tex_mutex;
+static std::unordered_map<const void *, vb_renderer *> g_tex_owner;
+static uint8_t *g_tex_base = nullptr;
+static size_t g_tex_next = 0;
+static const size_t TEX_KEY_STRIDE = 16, TEX_RANGE_BYTES = (size_t)1 << 30;
+
+extern "C" int vb_texture_key(const void *key) { // for vb_scene.cpp's host resolve
+    const uint8_t *p = (const uint8_t *)key, *base = __atomic_load_n(&g_tex_base, __ATOMIC_ACQUIRE);
+    return base != nullptr && p >= base && p < base + TEX_RANGE_BYTES;
+}
+static const void *new_texture_key(vb_renderer *owner) {
+    std::lock_guard<std::mutex> lock(g_tex_mutex);
+    if (!g_tex_base) {
+        void *m = mmap(nullptr, TEX_RANGE_BYTES, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
+        if (m == MAP_FAILED) return nullptr;
+        __atomic_store_n(&g_tex_base, (uint8_t *)m, __ATOMIC_RELEASE);
+    }
+    if (g_tex_next + TEX_KEY_STRIDE > TEX_RANGE_BYTES) return nullptr;
+    const void *key = g_tex_base + g_tex_next;
+    g_tex_next += TEX_KEY_STRIDE;
+    g_tex_owner[key] = owner;
+    return key;
+}
+static void drop_registrations(vb_renderer *r) {
+    std::lock_guard<std::mutex> lock(g_tex_mutex);
+    for (auto it = g_tex_owner.begin(); it != g_tex_owner.end();) it = it->second == r ? g_tex_owner.erase(it) : std::next(it);
+}
+
 // mask LUTs: vello_encoding/src/mask.rs:10-98 (f64 maths like the reference)
 static uint32_t one_mask(double slope, double translation, bool is_pos, const uint8_t *pattern, int n) {
     if (is_pos) translation = 1. - translation;
@@ -367,7 +426,8 @@ extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
         cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&r->tiling_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&r->tiling_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->blit_staged, cudaEventDisableTiming) != cudaSuccess) {
         delete r;
         return VB_E_CUDA;
     }
@@ -416,6 +476,9 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
     });
     for (auto &s : r->slot)
         if (s.h_bump) cudaFreeHost(s.h_bump);
+    if (r->blit_host) cudaFreeHost(r->blit_host);
+    if (r->blit_staged) cudaEventDestroy(r->blit_staged);
+    drop_registrations(r);
     if (r->ev_ok) {
         for (auto &ev : r->ev) cudaEventDestroy(ev);
         for (auto &ev : r->frame_ev) cudaEventDestroy(ev);
@@ -480,6 +543,7 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
     if ((rc = ensure(r, r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4))) return rc;
     if (r->cur->atlas_w && r->cur->atlas_h)
         CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4, cudaMemcpyHostToDevice, st));
+    r->cur->overridden.clear(); // a caller-packed atlas: overrides do not apply
     r->cur->have_scene = true;
     return VB_OK;
 }
@@ -870,6 +934,153 @@ static int pick_out(vb_renderer *r, Dest *d) {
     return rc;
 }
 
+// ---- images from device memory: Renderer::override_image / register_texture (vello/src/lib.rs:536-603) ----------------------
+// An override names an image by its key (the `pixels` pointer of its vb_image / vb_image_patch). The device resolve
+// (vb_scene_upload_streams) copies such an image into its atlas slot from the override's device memory with k_atlas_blit and
+// records the slot; marking the image dirty later queues the same copy in front of the next frame (refresh_overrides).
+
+// A device image must be memory of this renderer's device (or managed memory), with 4-byte aligned rows of at least 4 * w bytes.
+static int check_device_pixels(vb_renderer *r, const void *px, uint32_t w, uint32_t h, size_t pitch) {
+    auto bad = [&](const char *why) {
+        r->err = std::string("device image: ") + why;
+        return VB_E_INVALID;
+    };
+    if (!w || !h) return bad("a dimension is 0");
+    if (((uintptr_t)px & 3u) || (pitch & 3u)) return bad("the pointer and the row pitch must be multiples of 4 bytes");
+    if (pitch < (size_t)w * 4u) return bad("the row pitch is less than 4 * width");
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, px) != cudaSuccess) {
+        cudaGetLastError();
+        return bad("not a CUDA pointer");
+    }
+    if (a.type == cudaMemoryTypeManaged) return VB_OK;
+    if (a.type != cudaMemoryTypeDevice || a.device != r->device) return bad("not device memory of the renderer's device");
+    return VB_OK;
+}
+
+// Copy `rects` into an atlas of atlas_w texels per row with one k_atlas_blit on the renderer's stream. The rectangles reach
+// the device through a pinned staging buffer, which is rewritten only once the previous copy out of it has run.
+static int enqueue_blits(vb_renderer *r, std::vector<VbBlitRect> &rects, void *atlas, uint32_t atlas_w) {
+    if (rects.empty()) return VB_OK;
+    uint64_t units = 0;
+    for (VbBlitRect &b : rects) {
+        b.spr = vb_atlas_blit_units_per_row(b.w);
+        b.unit0 = units;
+        units += (uint64_t)b.h * b.spr;
+    }
+    const size_t bytes = rects.size() * sizeof(VbBlitRect);
+    CK(cudaEventSynchronize(r->blit_staged));
+    if (r->blit_host_cap < rects.size()) {
+        if (r->blit_host) CK(cudaFreeHost(r->blit_host));
+        r->blit_host = nullptr;
+        r->blit_host_cap = 0;
+        CK(cudaMallocHost((void **)&r->blit_host, bytes));
+        r->blit_host_cap = rects.size();
+    }
+    memcpy(r->blit_host, rects.data(), bytes);
+    int rc = ensure(r, r->blit_rects, bytes);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(r->blit_rects.p, r->blit_host, bytes, cudaMemcpyHostToDevice, r->stream));
+    CK(cudaEventRecord(r->blit_staged, r->stream));
+    vb_launch_atlas_blit((const VbBlitRect *)r->blit_rects.p, (uint32_t)rects.size(), units, (uint8_t *)atlas, atlas_w, r->stream);
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+
+// Before a frame: copy the dirty overridden images of the current scene slot into their atlas places. The copy runs ahead of
+// every kernel of the frame (and outside any captured graph), so a frame that draws its own destination reads the old pixels.
+// The atlas does not move, so a captured frame stays valid. Nothing dirty: nothing is enqueued.
+static int refresh_overrides(vb_renderer *r) {
+    std::vector<VbBlitRect> rects;
+    for (const auto &o : r->cur->overridden)
+        if (o.dirty) rects.push_back(VbBlitRect{o.src, o.pitch, 0, o.w, o.h, o.x, o.y, 0, 0});
+    if (rects.empty()) return VB_OK;
+    const int rc = enqueue_blits(r, rects, r->cur->atlas.p, r->cur->atlas_w);
+    if (rc) return rc;
+    for (auto &o : r->cur->overridden) o.dirty = false;
+    return VB_OK;
+}
+
+extern "C" int vb_override_image(vb_renderer *r, const void *key, uint32_t width, uint32_t height, const void *device_pixels,
+                                 size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    if (!key) {
+        r->err = "vb_override_image: NULL key";
+        return VB_E_INVALID;
+    }
+    if (device_pixels) {
+        CK(cudaSetDevice(r->device));
+        const int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
+        if (rc) return rc;
+        r->overrides[key] = vb_renderer::Override{(const uint8_t *)device_pixels, row_pitch_bytes, width, height};
+    } else {
+        r->overrides.erase(key);
+    }
+    // recorded atlas places: a new source of the same size is copied before the next frame; a removed override (or one of
+    // another size) keeps the pixels copied last and takes effect at the next device resolve
+    for (auto &s : r->slot) {
+        auto &v = s.overridden;
+        v.erase(std::remove_if(v.begin(), v.end(),
+                               [&](const auto &o) { return o.key == key && (!device_pixels || o.w != width || o.h != height); }),
+                v.end());
+        for (auto &o : v)
+            if (o.key == key) {
+                o.src = (const uint8_t *)device_pixels;
+                o.pitch = row_pitch_bytes;
+                o.dirty = true;
+            }
+    }
+    return VB_OK;
+}
+
+extern "C" int vb_mark_override_image_dirty(vb_renderer *r, const void *key) {
+    if (!r) return VB_E_INVALID;
+    if (!r->overrides.count(key)) {
+        r->err = "vb_mark_override_image_dirty: no override for this key";
+        return VB_E_INVALID;
+    }
+    for (auto &s : r->slot)
+        for (auto &o : s.overridden)
+            if (o.key == key) o.dirty = true;
+    return VB_OK;
+}
+
+// Renderer::register_texture / unregister_texture; vb_register_texture / vb_unregister_texture (vb_scene.cpp, which owns vb_image)
+// wrap these two.
+extern "C" int vb_texture_register(vb_renderer *r, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes,
+                                   const void **key_out) {
+    if (!r || !key_out) return VB_E_INVALID;
+    if (!device_pixels) {
+        r->err = "vb_register_texture: NULL pixels";
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
+    if (rc) return rc;
+    const void *key = new_texture_key(r);
+    if (!key) {
+        r->err = "vb_register_texture: no texture key left";
+        return VB_E_INVALID;
+    }
+    if ((rc = vb_override_image(r, key, width, height, device_pixels, row_pitch_bytes))) return rc;
+    *key_out = key;
+    return VB_OK;
+}
+
+extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
+    if (!r) return VB_E_INVALID;
+    {
+        std::lock_guard<std::mutex> lock(g_tex_mutex);
+        auto it = vb_texture_key(key) ? g_tex_owner.find(key) : g_tex_owner.end();
+        if (it == g_tex_owner.end() || it->second != r) {
+            r->err = "vb_unregister_texture: not a texture registered on this renderer";
+            return VB_E_INVALID;
+        }
+        g_tex_owner.erase(it);
+    }
+    return vb_override_image(r, key, 0, 0, nullptr, 0);
+}
+
 // A frame is enqueued in two steps: everything that may allocate, free or otherwise synchronise with the device (config,
 // arenas, the output target), then the launches. vb_group runs step 1 for ALL its renderers before step 2 of any: with the
 // exchange on, a renderer's frame contains a kernel that waits for its peers, and a peer that shares the device (tests)
@@ -885,8 +1096,10 @@ static int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
 }
 static int frame_launch(vb_renderer *r) {
     CK(cudaSetDevice(r->device));
+    int rc = refresh_overrides(r);
+    if (rc) return rc;
     CK(cudaEventRecord(r->frame_ev[0], r->stream));
-    int rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->dest, false);
+    rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->dest, false);
     if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
     r->frame_timed = rc == VB_OK;
     r->frame_pending = rc == VB_OK;
@@ -1817,6 +2030,28 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
         patches.push_back(Patch{L.draw_data_base + im.draw_data_offset, (px << 16) | py});
     }
     const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
+    // images with an override on this renderer come from device memory (one k_atlas_blit); a registered texture needs one
+    std::vector<VbBlitRect> blits;
+    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
+    std::vector<bool> from_device(placed.size(), false);
+    for (size_t i = 0; i < placed.size(); i++) {
+        const Placed &q = placed[i];
+        const auto ov = q.key ? r->overrides.find(q.key) : r->overrides.end();
+        if (ov != r->overrides.end()) {
+            const vb_renderer::Override &o = ov->second;
+            if (o.w != q.w || o.h != q.h) {
+                r->err = "device resolve: an override's size differs from its image's (" + std::to_string(o.w) + "x" + std::to_string(o.h) +
+                         " vs " + std::to_string(q.w) + "x" + std::to_string(q.h) + ")";
+                return VB_E_INVALID;
+            }
+            blits.push_back(VbBlitRect{o.src, o.pitch, 0, q.w, q.h, q.x, q.y, 0, 0});
+            over.push_back({q.key, o.src, o.pitch, q.w, q.h, q.x, q.y, false});
+            from_device[i] = true;
+        } else if (vb_texture_key(q.key)) {
+            r->err = "device resolve: a registered texture has no override on this renderer";
+            return VB_E_INVALID;
+        }
+    }
 
     // the six streams go straight to their places in the packed buffer
     if ((rc = ensure(r, r->cur->scene, total_words * 4 + 64))) return rc;
@@ -1844,13 +2079,17 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     r->cur->atlas_h = atlas_h;
     if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
     CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
-    for (const Placed &q : placed)
-        if (q.key && q.w && q.h)
+    for (size_t i = 0; i < placed.size(); i++) {
+        const Placed &q = placed[i];
+        if (q.key && q.w && q.h && !from_device[i])
             CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
                                  cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = enqueue_blits(r, blits, r->cur->atlas.p, atlas_w))) return rc;
     CK(cudaGetLastError());
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
+    r->cur->overridden = std::move(over);
     r->cur->layout = L;
     r->cur->scene_words = total_words;
     r->cur->have_scene = true;

@@ -23,6 +23,12 @@
 
 #include "../../include/vello_b200_scene.h"
 
+// vb_api.cu: nonzero for a key vb_register_texture handed out (an address no host buffer has); the texture registry
+extern "C" int vb_texture_key(const void *key);
+extern "C" int vb_texture_register(vb_renderer *, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes,
+                                   const void **key_out);
+extern "C" int vb_texture_unregister(vb_renderer *, const void *key);
+
 namespace {
 
 constexpr uint8_t TAG_LINE_TO_F32 = 0x9, TAG_QUAD_TO_F32 = 0xA, TAG_CUBIC_TO_F32 = 0xB;
@@ -1365,8 +1371,9 @@ int vb_scene_resolve(vb_scene *s, vb_packed *out) {
     }
     const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
     s->atlas.assign((size_t)atlas_w * atlas_h * 4, 0);
+    // a registered texture's key points at nothing (its pixels exist only in device memory): its region stays zero, as for NULL
     for (const Placed &q : placed)
-        for (uint32_t row = 0; row < q.h && q.key; row++)
+        for (uint32_t row = 0; row < q.h && q.key && !vb_texture_key(q.key); row++)
             std::memcpy(&s->atlas[((size_t)(q.y + row) * atlas_w + q.x) * 4], q.key + (size_t)row * q.w * 4, (size_t)q.w * 4);
 
     // pack the six streams (resolve.rs:107-154); unclosed clips get a trailing PATH tag and END_CLIP draw tag each
@@ -1443,6 +1450,25 @@ int vb_scene_upload_device(vb_renderer *r, vb_scene *s, vb_layout *layout_out) {
     st.ramp_patches = rps.data(); st.n_ramp_patches = (uint32_t)rps.size();
     st.image_patches = ips.data(); st.n_image_patches = (uint32_t)ips.size();
     return vb_scene_upload_streams(r, &st, layout_out);
+}
+
+int vb_register_texture(vb_renderer *r, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes, vb_image *out) {
+    if (!out) return VB_E_INVALID;
+    const void *key = nullptr;
+    const int rc = vb_texture_register(r, device_pixels, width, height, row_pitch_bytes, &key);
+    if (rc) return rc;
+    std::memset(out, 0, sizeof *out);
+    out->pixels = static_cast<const uint8_t *>(key);
+    out->width = width;
+    out->height = height;
+    out->quality = 1; // peniko's default ImageQuality::Medium; RGBA8, straight alpha, pad: zeros
+    out->alpha = 1.0f;
+    return VB_OK;
+}
+
+int vb_unregister_texture(vb_renderer *r, const vb_image *image) {
+    if (!r || !image) return VB_E_INVALID;
+    return vb_texture_unregister(r, image->pixels);
 }
 
 int vb_render_scene(vb_renderer *r, vb_scene *s, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {

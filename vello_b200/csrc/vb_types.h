@@ -57,6 +57,16 @@ typedef struct {
     uint32_t win_cull;         /* 1: a stripe window is set -- flatten skips segments that cannot reach its rows */
 } VbConfig;
 
+/* One rectangle of k_atlas_blit (k_atlas.cu): w x h RGBA8 texels from device memory (rows src_pitch bytes apart, 4-byte
+ * aligned) to atlas texel (dst_x, dst_y). unit0 = exclusive prefix of h * spr over the rectangles before it. */
+typedef struct {
+    const uint8_t *src;
+    uint64_t src_pitch;
+    uint64_t unit0;
+    uint32_t w, h, dst_x, dst_y;
+    uint32_t spr, _pad; /* units (16-byte destination windows) per row: vb_atlas_blit_units_per_row(w) */
+} VbBlitRect;
+
 #define VB_STAGE_BINNING 0x1u
 #define VB_STAGE_TILE_ALLOC 0x2u
 #define VB_STAGE_FLATTEN 0x4u

@@ -191,7 +191,12 @@ class Gradient:
 
 @dataclass
 class Image:
-    """RGBA8/BGRA8 image + sampler (peniko `ImageBrush`)."""
+    """RGBA8/BGRA8 image + sampler (peniko `ImageBrush`).
+
+    `key` (optional) names the image in the atlas the way vello's blob id does: images with the same key share one atlas slot,
+    and a renderer's override of the key (`Renderer.override_image`) supplies its pixels from device memory at the device
+    resolve. A registered texture (`Renderer.register_texture`) has a key that points at no host memory and a zero-strided
+    `data` of zeros, so the host resolve leaves its atlas region zero."""
 
     data: np.ndarray  # (h, w, 4) uint8
     format: int = FORMAT_RGBA8
@@ -200,6 +205,7 @@ class Image:
     x_extend: int = EXTEND_PAD
     y_extend: int = EXTEND_PAD
     alpha: float = 1.0
+    key: Optional[int] = None
 
     @property
     def width(self) -> int:
@@ -813,7 +819,8 @@ def resolve(enc: Encoding) -> Packed:
     placed = {}
     for p in enc.image_patches:
         im = p["image"]
-        k = id(im.data)  # the image cache is keyed by the pixel blob's identity (image_cache.rs:113-114), not by the brush
+        # the image cache is keyed by the pixel blob's identity (image_cache.rs:113-114), not by the brush
+        k = ("key", im.key) if im.key is not None else ("id", id(im.data))
         if k not in placed:
             if x + im.width > MAXW:
                 y += shelf_h

@@ -15,7 +15,7 @@ from typing import Optional
 import numpy as np
 
 from .config import AA_AREA, AA_MSAA8, AA_MSAA16, RenderParams
-from .encoding import Packed, Scene, resolve
+from .encoding import Image, Packed, Scene, resolve
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvello_b200.so")
@@ -125,6 +125,8 @@ def load_library() -> C.CDLL:
     lib.vb_exchange_attach.argtypes = [vp, C.c_uint32, vp]
     lib.vb_exchange_set_bounds.argtypes = [vp, C.POINTER(C.c_uint32)]
     lib.vb_exchange_enable.argtypes = [vp, C.c_int]
+    lib.vb_override_image.argtypes = [vp, vp, C.c_uint32, C.c_uint32, vp, C.c_size_t]
+    lib.vb_mark_override_image_dirty.argtypes = [vp, vp]
     _lib = lib
     return lib
 
@@ -135,7 +137,23 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_scene_upload_streams", "vb_render_uploaded", "vb_last_frame_ms", "vb_frame_alloc", "vb_frame_free", "vb_ipc_export", "vb_ipc_open", "vb_ipc_close",
                     "vb_group_new", "vb_group_free", "vb_group_size", "vb_group_renderer", "vb_group_last_error", "vb_group_render",
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
-                    "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable"]
+                    "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
+                    "vb_override_image", "vb_mark_override_image_dirty"]
+
+
+def _device_image(t):
+    """(pointer, height, width, row pitch in bytes) of an (H, W, 4) uint8 array in device memory, from its
+    `__cuda_array_interface__` (a torch CUDA tensor, or a slice of one): texels 4 bytes apart, rows any multiple of 4 apart."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: a device image is needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 3 or shape[2] != 4 or cai["typestr"] not in ("|u1", "<u1", ">u1"):
+        raise ValueError(f"a device image is (H, W, 4) uint8, not shape {shape} of type {cai['typestr']}")
+    strides = cai.get("strides") or (shape[1] * 4, 4, 1)
+    if tuple(strides[1:]) != (4, 1) or strides[0] % 4:
+        raise ValueError(f"a device image has texel strides (4, 1) and a row stride that is a multiple of 4, not {tuple(strides)}")
+    return int(cai["data"][0]), shape[0], shape[1], int(strides[0])
 
 
 @dataclass
@@ -167,6 +185,7 @@ class Renderer:
         self.last_stats: Optional[FrameStats] = None
         self._keep = None
         self._owner = None
+        self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
 
     @classmethod
     def _borrowed(cls, lib, handle: int, owner):
@@ -174,6 +193,7 @@ class Renderer:
         r = cls.__new__(cls)
         r.lib, r.handle, r.options, r.last_stats, r._keep = lib, C.c_void_p(handle), None, None, None
         r._owner = owner
+        r._device_images = {}
         return r
 
     def close(self):
@@ -202,6 +222,50 @@ class Renderer:
                                       ramps.ctypes.data if ramps.size else None, 512, ramps.shape[0],
                                       atlas.ctypes.data, atlas.shape[1], atlas.shape[0])
         self._check(rc, "vb_scene_upload")
+
+    # -- images from device memory (Renderer::override_image / register_texture, vello/src/lib.rs:536-603) ---------------------
+    # Overrides apply where the scene is resolved on the device (NativeScene.upload_device); a host-packed scene (upload,
+    # render_to_texture, render_stream) ignores them. The caller orders its writes to a device array before the call that
+    # copies it (a torch.cuda.synchronize(), or work on `self.stream`).
+    def register_texture(self, t) -> Image:
+        """Draw the device array `t` ((H, W, 4) uint8, RGBA8 with straight alpha; e.g. a torch CUDA tensor or a column slice
+        of one) as an `Image`: a fresh key with an override of `t`. `t` is held until `unregister_texture`. The image's
+        sampler fields (quality, extends, alpha, format, alpha_type) are the caller's to change."""
+        from .scene_native import _Image, _lib as _scene_lib
+        ptr, h, w, pitch = _device_image(t)
+        im = _Image()
+        self._check(_scene_lib().vb_register_texture(self.handle, C.c_void_p(ptr), w, h, pitch, C.byref(im)), "vb_register_texture")
+        self._device_images[int(im.pixels)] = t
+        zeros = np.lib.stride_tricks.as_strided(np.zeros(4, dtype=np.uint8), shape=(h, w, 4), strides=(0, 0, 1))
+        return Image(zeros, key=int(im.pixels))
+
+    def unregister_texture(self, image: Image):
+        from .scene_native import _Image, _lib as _scene_lib
+        im = _Image(C.c_void_p(image.key) if image.key is not None else None, image.width, image.height)
+        self._check(_scene_lib().vb_unregister_texture(self.handle, C.byref(im)), "vb_unregister_texture")
+        self._device_images.pop(image.key, None)
+
+    def override_image(self, image: Image, t=None):
+        """Supply the pixels of `image` from the device array `t` at the next device resolve and the frames after it
+        (`mark_override_image_dirty` to copy them again); `t=None` removes the override. A host image without a key gets one
+        here: its data becomes a private contiguous copy whose address is the key."""
+        if t is None:
+            if image.key is not None:
+                self._check(self.lib.vb_override_image(self.handle, C.c_void_p(image.key), 0, 0, None, 0), "vb_override_image")
+                self._device_images.pop(image.key, None)
+            return
+        ptr, h, w, pitch = _device_image(t)
+        if image.key is None:
+            image.data = np.ascontiguousarray(image.data, dtype=np.uint8).copy()
+            image.key = int(image.data.ctypes.data)
+        self._check(self.lib.vb_override_image(self.handle, C.c_void_p(image.key), w, h, C.c_void_p(ptr), pitch), "vb_override_image")
+        self._device_images[image.key] = t
+
+    def mark_override_image_dirty(self, image: Image):
+        """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
+        if image.key is None:
+            raise ValueError("mark_override_image_dirty: the image has no override")
+        self._check(self.lib.vb_mark_override_image_dirty(self.handle, C.c_void_p(image.key)), "vb_mark_override_image_dirty")
 
     # -- rendering ---------------------------------------------------------------------------------
     def render_to_texture(self, scene, params: RenderParams, bin_rows=(0, 0), tile_rows=(0, 0)) -> np.ndarray:

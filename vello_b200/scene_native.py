@@ -54,7 +54,8 @@ PATHBUF_SYMBOLS = ["vb_pathbuf_new", "vb_pathbuf_free", "vb_pathbuf_clear", "vb_
                    "vb_pathbuf_svg", "vb_pathbuf_view"]
 SCENE_SYMBOLS = ["vb_scene_new", "vb_scene_free", "vb_scene_reset", "vb_scene_fill", "vb_scene_stroke", "vb_scene_push_layer",
                  "vb_scene_push_luminance_mask_layer", "vb_scene_push_clip_layer", "vb_scene_pop_layer", "vb_scene_draw_image",
-                 "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash"]
+                 "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
+                 "vb_register_texture", "vb_unregister_texture"]
 
 _bound = False
 
@@ -81,6 +82,8 @@ def _lib():
         lib.vb_render_scene.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
         lib.vb_scene_upload_device.argtypes = [vp, vp, vp]
         lib.vb_path_dash.argtypes = [vp, C.c_double, vp, C.c_uint32, vp]
+        lib.vb_register_texture.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_size_t, C.POINTER(_Image)]
+        lib.vb_unregister_texture.argtypes = [vp, C.POINTER(_Image)]
         d = C.c_double
         lib.vb_pathbuf_new.restype = vp
         lib.vb_pathbuf_free.argtypes = [vp]
@@ -136,14 +139,18 @@ class NativeScene:
         return _Color(c.r, c.g, c.b, c.a)
 
     def _image(self, im: Image) -> _Image:
-        k = id(im)
-        if k not in self._images:
-            dk = id(im.data)  # one pixel buffer per blob: the atlas is keyed by it (image_cache.rs:113-114)
-            if dk not in self._pixels:
-                self._pixels[dk] = np.ascontiguousarray(im.data, dtype=np.uint8).copy()
-            px = self._pixels[dk]
-            self._images[k] = _Image(px.ctypes.data, im.width, im.height, im.format, im.alpha_type, im.quality, im.x_extend, im.y_extend, im.alpha)
-        return self._images[k]
+        k = (id(im), im.key)
+        if k not in self._images:  # the entry holds `im` too, so that its id cannot be reused by another Image meanwhile
+            if im.key is not None:  # the key is the image's `pixels` (a host image's key points into its own data)
+                self._pixels[("key", im.key)] = im.data
+                ptr = im.key
+            else:
+                dk = id(im.data)  # one pixel buffer per blob: the atlas is keyed by it (image_cache.rs:113-114)
+                if dk not in self._pixels:
+                    self._pixels[dk] = np.ascontiguousarray(im.data, dtype=np.uint8).copy()
+                ptr = self._pixels[dk].ctypes.data
+            self._images[k] = (_Image(ptr, im.width, im.height, im.format, im.alpha_type, im.quality, im.x_extend, im.y_extend, im.alpha), im)
+        return self._images[k][0]
 
     def _brush(self, brush):
         b = _Brush()
