@@ -176,6 +176,18 @@ int vb_set_occlusion_cull(vb_renderer *, int on);
 
 int vb_debug_fine_traffic(vb_renderer *, uint64_t *ptcl_words, uint64_t *segment_refs, uint64_t *fill_cmds);
 
+/* ---- batches: many scenes of one size in one pass (an addition; vello has no batch API) ----
+ * Split the uploaded scene's draw objects into n_cells contiguous ranges (cells): draw_offsets[0] = 0 <= ... <= draw_offsets[n_cells]
+ * = layout.n_draw_objects (n_cells + 1 entries; vb_scene_batch builds such a scene and its offsets). The following frames of
+ * that scene (vb_render_resident, vb_render_enqueue, vb_render_uploaded, vb_run_stages) render cell c, alone, into a
+ * params.width x params.height frame at byte offset c * 4 * width * height of the destination: n_cells frames back to back,
+ * i.e. an [n_cells, height, width, 4] RGBA8 buffer. Every cell shares the params (size, AA, base colour); no cell's geometry
+ * reaches another's frame, and a cell's pixels are the ones its scene renders alone. Any scene upload resets the renderer to
+ * one cell; n_cells = 1 ({0, n_draw_objects}) is no batch. VB_E_INVALID (vb_last_error says why): offsets that do not start
+ * at 0, decrease, or do not end at n_draw_objects; a cell whose BEGIN_CLIP / END_CLIP do not balance; a renderer of a vb_group
+ * or with the exchange enabled; and, at the frame, bin_row / tile_row windows or a batch larger than the arenas can index. */
+int vb_set_cells(vb_renderer *, const uint32_t *draw_offsets, uint32_t n_cells);
+
 /* ---- Resolver::resolve on the DEVICE (vello_encoding/src/resolve.rs:183-399, ramp_cache.rs:119-155) ----
  * Instead of a packed scene the caller hands over the six streams of a vello_encoding::Encoding (encoding.rs:22-48) and its
  * late-bound patches (resolve.rs:560-590): each stream is copied straight to its Layout offset inside the packed buffer in

@@ -143,6 +143,12 @@ int vb_scene_draw_blurred_rounded_rect_in(vb_scene *, const vb_path *shape, cons
  * src's transforms. Images referenced by src must stay alive like dst's own. */
 int vb_scene_append(vb_scene *dst, const vb_scene *src, const double *transform);
 
+/* A batch of n scenes for vb_set_cells: dst is reset, then every scene is appended with the identity transform and its open
+ * layers are closed right behind it (the END_CLIP draw tag and PATH tag of vb_scene_pop_layer, which resolve would add at the
+ * end of a single scene). draw_offsets (n + 1 entries) receives the draw-object range of each scene. Upload dst as any scene
+ * (vb_scene_upload_device, or vb_scene_resolve + vb_scene_upload), then vb_set_cells(r, draw_offsets, n). */
+int vb_scene_batch(vb_scene *dst, const vb_scene *const *scenes, uint32_t n, uint32_t *draw_offsets);
+
 /* Resolver::resolve (resolve.rs:183-399) without glyph runs: late-bound gradient ramps (512 premultiplied RGBA8 samples
  * each) and the image atlas are built, their indices patched into the draw data, and the six streams packed. The
  * pointers stay owned by the scene and valid until it is changed, resolved again or freed. */

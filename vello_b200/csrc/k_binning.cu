@@ -43,18 +43,31 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
     }
     const int32_t width_in_bins = (int32_t)((cfg.width_in_tiles + VB_N_TILE_X - 1u) / VB_N_TILE_X);
     const int32_t height_in_bins = (int32_t)((cfg.height_in_tiles + VB_N_TILE_Y - 1u) / VB_N_TILE_Y);
-    const uint32_t n_bins = (uint32_t)(width_in_bins * height_in_bins);
+    const uint32_t n_bins = (uint32_t)(width_in_bins * height_in_bins) * cfg.n_cells;
     const uint32_t aligned_n_bins = (n_bins + VB_N_TILE - 1u) & ~(VB_N_TILE - 1u);
     x0 = vb_clampi(x0, 0, width_in_bins);
     x1 = vb_clampi(x1, 0, width_in_bins);
     y0 = vb_clampi(y0, (int32_t)cfg.win_by0, (int32_t)cfg.win_by1);
     y1 = vb_clampi(y1, (int32_t)cfg.win_by0, (int32_t)cfg.win_by1);
     if (x0 == x1) y1 = y0;
+    // Batch: the draw's rectangle, clamped to its own cell above, moves down to the cell's bin rows; this partition walks only
+    // the 256-bin blocks that hold bins of the cells its draws belong to (coarse reads no header of any other block).
+    uint32_t block_lo = 0u, block_hi = n_bins;
+    if (cfg.n_cells > 1u) {
+        const uint32_t last_ix = min(blockIdx.x * BN_THREADS + BN_THREADS, cfg.layout.n_draw_objects) - 1u;
+        const uint32_t c_first = vb_cell_of(cfg, blockIdx.x * BN_THREADS), c_last = vb_cell_of(cfg, last_ix);
+        const uint32_t cell_bins = (uint32_t)(width_in_bins * height_in_bins);
+        block_lo = (c_first * cell_bins) & ~(VB_N_TILE - 1u);
+        block_hi = (c_last + 1u) * cell_bins;
+        const int32_t row0 = (int32_t)(vb_cell_of(cfg, min(element_ix, cfg.layout.n_draw_objects - 1u)) * (uint32_t)height_in_bins);
+        y0 += row0;
+        y1 += row0;
+    }
     const int32_t y0_width = y0 * width_in_bins, y1_width = y1 * width_in_bins;
     const uint32_t my_slice = lid / 32u, my_mask = 1u << (lid & 31u);
 
-    uint32_t next_block = VB_N_TILE;
-    for (uint32_t block_start = 0u; block_start < n_bins;) {
+    uint32_t next_block = block_lo + VB_N_TILE;
+    for (uint32_t block_start = block_lo; block_start < block_hi;) {
         for (int32_t y_offset = y0_width; y_offset < y1_width; y_offset += width_in_bins) {
             uint32_t start_bin = max((uint32_t)(y_offset + x0), block_start);
             uint32_t end_bin = min((uint32_t)(y_offset + x1), next_block);
@@ -102,7 +115,7 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
             }
         }
         block_start = next_block;
-        if (next_block < aligned_n_bins) {
+        if (next_block < block_hi) {
             __syncthreads();
             for (int i = 0; i < BN_N_SLICE; i++) sh_bitmaps[i][lid] = 0u;
             __syncthreads();

@@ -45,7 +45,7 @@ __device__ __forceinline__ CoTile co_load_tile(const VbTile *tiles, uint32_t ix,
 
 __device__ __forceinline__ void co_alloc_cmd(TileState &s, uint32_t size, const VbConfig &cfg, VbBump *bump, uint32_t *ptcl) {
     if (s.cmd_offset + size >= s.cmd_limit) {
-        const uint32_t ptcl_dyn_start = cfg.width_in_tiles * cfg.height_in_tiles * VB_PTCL_INITIAL_ALLOC;
+        const uint32_t ptcl_dyn_start = cfg.width_in_tiles * cfg.tile_rows * VB_PTCL_INITIAL_ALLOC;
         uint32_t new_cmd = ptcl_dyn_start + atomicAdd(&bump->ptcl, VB_PTCL_INCREMENT);
         if (new_cmd + VB_PTCL_INCREMENT > cfg.ptcl_size) {
             // Out of PTCL space: park this tile's writes in the (unused) first dynamic chunk slot 0 of
@@ -117,17 +117,29 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     const uint32_t width_in_bins = (cfg.width_in_tiles + VB_N_TILE_X - 1u) / VB_N_TILE_X;
     const uint32_t height_in_bins = (cfg.height_in_tiles + VB_N_TILE_Y - 1u) / VB_N_TILE_Y;
     const uint32_t bin_ix = width_in_bins * wg_y + wg_x;
-    const uint32_t aligned_n_bins = (width_in_bins * height_in_bins + VB_N_TILE - 1u) & ~(VB_N_TILE - 1u);
-    const uint32_t n_partitions = (cfg.layout.n_draw_objects + VB_N_TILE - 1u) / VB_N_TILE;
-    const uint32_t bin_tile_x = VB_N_TILE_X * wg_x, bin_tile_y = VB_N_TILE_Y * wg_y;
+    const uint32_t aligned_n_bins = (width_in_bins * height_in_bins * cfg.n_cells + VB_N_TILE - 1u) & ~(VB_N_TILE - 1u);
+    // Batch: the bin row (of the tall frame) names the cell; tiles are cell-local below, except for the frame-wide tile index
+    // (PTCL, tile_start, fine's queue). Only the partitions that hold draws of the cell are read: [partition_ix, sh_part_end).
+    // (The end lives in shared memory: a register more would spill at this occupancy.)
+    __shared__ uint32_t sh_part_end;
+    uint32_t cell = 0u, partition_ix = 0u;
+    if (cfg.n_cells > 1u) {
+        cell = wg_y / height_in_bins;
+        const uint32_t d0 = __ldg(cfg.cell_draw + cell), d1 = __ldg(cfg.cell_draw + cell + 1u);
+        partition_ix = d0 / VB_N_TILE;
+        if (lid == 0u) sh_part_end = d1 > d0 ? (d1 + VB_N_TILE - 1u) / VB_N_TILE : partition_ix;
+        __syncthreads(); // uniform: n_cells is the launch's
+    }
+#define n_partitions (cfg.n_cells > 1u ? sh_part_end : (cfg.layout.n_draw_objects + VB_N_TILE - 1u) / VB_N_TILE)
+    const uint32_t bin_tile_x = VB_N_TILE_X * wg_x, bin_tile_y = VB_N_TILE_Y * (wg_y - cell * height_in_bins);
     const bool owns_tile = lid < 64u;
     const uint32_t tile_x = (uint32_t)qx0 + (lid & 7u), tile_y = (uint32_t)qy0 + ((lid >> 3) & 7u);
-    const uint32_t this_tile_ix = (bin_tile_y + tile_y) * cfg.width_in_tiles + bin_tile_x + tile_x;
+    const uint32_t this_tile_ix = (cell * cfg.height_in_tiles + bin_tile_y + tile_y) * cfg.width_in_tiles + bin_tile_x + tile_x;
     TileState st;
     st.cmd_offset = this_tile_ix * VB_PTCL_INITIAL_ALLOC;
     st.cmd_limit = st.cmd_offset + (VB_PTCL_INITIAL_ALLOC - VB_PTCL_HEADROOM);
     uint32_t clip_zero_depth = 0u, clip_depth = 0u;
-    uint32_t partition_ix = 0u, rd_ix = 0u, wr_ix = 0u, part_start_ix = 0u, ready_ix = 0u;
+    uint32_t rd_ix = 0u, wr_ix = 0u, part_start_ix = 0u, ready_ix = 0u;
     uint32_t render_blend_depth = 0u, max_blend_depth = 0u;
     uint32_t cull_start = 0u; // PTCL offset of the CMD_SOLID of this tile's last opaque full-tile cover (0: none)
     uint32_t cost = 0u;       // estimated work of fine on this tile from its occlusion start (orders fine's tile queue)
@@ -388,7 +400,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     // (one atomic per warp and class; fine walks the lists in class order, so the long tiles start at time zero instead of
     // turning up at the tail of a persistent kernel that has nothing left to overlap them with)
     if (lid < 64u) { // the two owner warps, whole
-        const uint32_t ty = bin_tile_y + tile_y, tx = bin_tile_x + tile_x;
+        const uint32_t ty = bin_tile_y + tile_y, tx = bin_tile_x + tile_x; // ty: row in the cell; the list takes frame rows
         const bool in_win = tx < cfg.width_in_tiles && ty >= cfg.win_ty0 && ty < cfg.win_ty1 && ty < cfg.height_in_tiles;
         // classes by powers of two of the estimate: >= 1024, 512, 256, 128, 64, 32, 16, rest
         const uint32_t lg = 31u - (uint32_t)__clz((int)max(cost, 1u));
@@ -403,13 +415,14 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
             base = __shfl_sync(VB_FULL, base, __ffs((int)m) - 1);
             if (in_win && cls == k) {
                 const uint32_t slot = base + (uint32_t)__popc(m & ((1u << lane) - 1u));
-                if (slot < cls_stride) cls_list[(size_t)k * cls_stride + slot] = make_uint2((ty - cfg.win_ty0) * cfg.width_in_tiles + tx, cull_start);
+                if (slot < cls_stride) cls_list[(size_t)k * cls_stride + slot] = make_uint2(this_tile_ix - cfg.win_ty0 * cfg.width_in_tiles, cull_start);
             }
         }
         // the slots these fills use are not holes (k_backdrop set holes to every slot of the frame)
         const uint32_t used = vb_warp_sum(emitted);
         if (lane == 0u && used != 0u) atomicSub(reinterpret_cast<uint32_t *>(bump) + VB_CTL_SEG_HOLES, used);
     }
+#undef n_partitions
 }
 
 // The segments-arena overflow check (the reference sizes `segments` statically and never checks) lives at the top of
@@ -420,6 +433,7 @@ extern "C" uint32_t vb_launch_coarse(const VbConfig *cfg, const uint32_t *scene,
                                  VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, void *cls_list, uint32_t cls_stride, cudaStream_t st) {
     uint32_t width_in_bins = (cfg->width_in_tiles + 15u) / 16u;
     uint32_t rows = cfg->win_by1 - cfg->win_by0;
+    if (cfg->n_cells > 1u) rows *= cfg->n_cells; // a batch has no window: every cell's bin rows, stacked
     if (width_in_bins == 0 || rows == 0) return 0;
     dim3 grid(width_in_bins * 2u, rows * 2u); // four quadrant CTAs per bin
     k_coarse<<<grid, CO_THREADS, 0, st>>>(*cfg, scene, draw_monoids, bin_headers, info_bin_data, paths, tiles, bump, ptcl, tile_start, (uint2 *)cls_list, cls_stride);

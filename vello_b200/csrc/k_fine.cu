@@ -867,7 +867,10 @@ k_fine(VbConfig cfg, FineArgs A) {
         // ---- this tile
         const uint32_t tile_x = t_cur % wt, tile_y = cfg.win_ty0 + t_cur / wt;
         const uint32_t tile_ix = tile_y * wt + tile_x;
-        const uint32_t gx = tile_x * 16u + h * 8u, gy = tile_y * 16u + ly;
+        // batch: the tile row of the tall frame names the cell; pixels (brushes, output row) are the cell's own
+        uint32_t cell = 0u;
+        if (cfg.n_cells > 1u) cell = tile_y / cfg.height_in_tiles;
+        const uint32_t gx = tile_x * 16u + h * 8u, gy = (tile_y - cell * cfg.height_in_tiles) * 16u + ly;
         // pixel coordinates are small integers: (float)(gx + i) is exactly the WGSL's xy.x + f32(i) of either 4-pixel group
 #define xyy ((float)gy)
 #define xyx0 ((float)gx)
@@ -1202,7 +1205,9 @@ k_fine(VbConfig cfg, FineArgs A) {
                     px[i] = unorm8(fg.r * a_inv) | (unorm8(fg.g * a_inv) << 8) | (unorm8(fg.b * a_inv) << 16) | (unorm8(fg.a) << 24);
                 }
             }
-            uint32_t *row = A.out + (size_t)(gy - cfg.out_row0) * cfg.out_pitch_px;
+            // the cell again, from the tile index (keeping it live across the interpreter would cost a register)
+            const uint32_t out_cell = cfg.n_cells > 1u ? tile_ix / wt / cfg.height_in_tiles : 0u;
+            uint32_t *row = A.out + ((size_t)out_cell * cfg.target_height + (gy - cfg.out_row0)) * cfg.out_pitch_px;
             if (gx + 7u < cfg.target_width && (cfg.out_pitch_px & 3u) == 0u && ((uintptr_t)A.out & 15u) == 0u) {
                 // two 128-bit stores: 32 contiguous bytes of one pixel row per lane
                 uint4 *dst = reinterpret_cast<uint4 *>(row + gx);

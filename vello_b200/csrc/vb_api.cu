@@ -218,6 +218,12 @@ struct vb_renderer {
     // test-only capacity limits (vb_debug_limit_arena); UINT32_MAX = none
     uint32_t limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
 
+    // batch (vb_set_cells): the draw-object offsets of the cells of the current scene (n_cells + 1 entries, a copy of cell_draw);
+    // empty = one cell, no batch. Every scene upload empties it.
+    std::vector<uint32_t> cells;
+    DevBuf cell_draw;
+    bool grouped = false; // a renderer of a vb_group: no batches
+
     // per-frame
     VbConfig cfg{};
     vb_params params{};
@@ -277,7 +283,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const keyed[] = {&s.scene, &s.ramps, &s.atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
                              &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers,
                              &r->paths, &r->ctl, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs,
-                             &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill};
+                             &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw};
     DevBuf *const unkeyed[] = {&o.scene, &o.ramps, &o.atlas, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena};
     for (DevBuf *b : keyed) f(*b, true);
     for (DevBuf *b : unkeyed) f(*b, false);
@@ -329,7 +335,7 @@ static int arena_index(const char *name) {
     return -1;
 }
 // ptcl starts with a static command area of VB_PTCL_INITIAL_ALLOC words per tile; its capacity includes it, bump.ptcl does not
-static uint64_t ptcl_static(const VbConfig &c) { return (uint64_t)c.width_in_tiles * c.height_in_tiles * VB_PTCL_INITIAL_ALLOC; }
+static uint64_t ptcl_static(const VbConfig &c) { return (uint64_t)c.width_in_tiles * c.tile_rows * VB_PTCL_INITIAL_ALLOC; }
 // elements of the arena's buffer in front of the arena: binning lives after the draw info in info_bin_data
 static size_t arena_offset(const vb_renderer *r, int a) { return a == ARENA_BINNING ? r->cur->layout.bin_data_start : 0; }
 // what the last attempt asked of an arena, in the units of its capacity
@@ -545,6 +551,7 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
         CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4, cudaMemcpyHostToDevice, st));
     r->cur->overridden.clear(); // a caller-packed atlas: overrides do not apply
     r->cur->have_scene = true;
+    r->cells.clear(); // a new scene is one cell until vb_set_cells says otherwise
     return VB_OK;
 }
 
@@ -575,10 +582,24 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         r->err = "vb_params: width/height must be 1..65536 and aa 0..2";
         return VB_E_INVALID;
     }
+    const uint32_t n_cells = r->cells.empty() ? 1u : (uint32_t)r->cells.size() - 1u;
+    if (n_cells > 1u) {
+        if (p->bin_row1 > p->bin_row0 || p->tile_row1 > p->tile_row0 || r->xc.enabled || r->grouped) {
+            r->err = "batch: cells cannot be combined with bin_row / tile_row windows, vb_group or the exchange";
+            return VB_E_INVALID;
+        }
+        const uint64_t hb = ((p->height + 15u) / 16u + 15u) / 16u, wb = ((p->width + 15u) / 16u + 15u) / 16u;
+        const uint64_t parts = (r->cur->layout.n_draw_objects + 255u) / 256u, bins = ((wb * hb * n_cells + 255u) & ~255ull);
+        if (hb * n_cells * 2u > 65535u || parts * bins >= 0xffffffffull) {
+            r->err = "batch: too many cells of this size (bin rows or bin headers exceed what the kernels index)";
+            return VB_E_INVALID;
+        }
+    }
     {
-        const uint64_t nt = (uint64_t)((p->width + 15u) / 16u) * ((p->height + 15u) / 16u);
+        const uint64_t nt = (uint64_t)((p->width + 15u) / 16u) * ((p->height + 15u) / 16u) * n_cells;
         if (nt * VB_PTCL_INITIAL_ALLOC + nt * (VB_PTCL_INCREMENT / 8u) + 65536u > 0xf0000000ull) {
-            r->err = "vb_params: tile count * PTCL allocation exceeds 32-bit word offsets";
+            r->err = n_cells > 1u ? "batch: tile count * PTCL allocation exceeds 32-bit word offsets"
+                                  : "vb_params: tile count * PTCL allocation exceeds 32-bit word offsets";
             return VB_E_INVALID;
         }
     }
@@ -615,12 +636,15 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
+    c.n_cells = n_cells;
+    c.tile_rows = c.height_in_tiles * n_cells;
+    c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
     r->params = *p;
 
     const VbLayout &L = r->cur->layout;
     const uint32_t n_draw = L.n_draw_objects, n_paths = L.n_paths, n_clips = L.n_clips;
-    const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles;
-    const uint32_t n_bins = wb * hb, aligned_n_bins = (n_bins + 255u) & ~255u;
+    const uint32_t n_tiles = c.width_in_tiles * c.tile_rows;
+    const uint32_t n_bins = wb * hb * n_cells, aligned_n_bins = (n_bins + 255u) & ~255u;
     int rc;
     if ((rc = ensure(r, r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)))) return rc;
     if ((rc = ensure(r, r->path_bboxes, (size_t)n_paths * sizeof(VbPathBbox)))) return rc;
@@ -687,6 +711,7 @@ static uint32_t capacity_grid(uint32_t cap, int sm_count) {
 static int queue_readback(vb_renderer *r, const VbConfig &c, uint32_t ty0, uint32_t ty1, const Dest &d, uint32_t band) {
     size_t y0 = (size_t)ty0 * 16u, y1 = (size_t)ty1 * 16u;
     if (y1 > c.target_height) y1 = c.target_height;
+    if (c.n_cells > 1u) y0 = 0, y1 = (size_t)c.n_cells * c.target_height; // a batch: all its frames, back to back
     if (y1 <= y0) return VB_OK;
     const size_t off = (y0 - c.out_row0) * c.out_pitch_px * 4u, bytes = (y1 - y0) * c.out_pitch_px * 4u;
     CK(cudaEventRecord(r->band_ev[band], r->stream));
@@ -787,7 +812,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             launches += vb_launch_coarse(&c, (const uint32_t *)r->cur->scene.p, (const VbDrawMonoid *)r->draw_monoids.p,
                                          (const VbBinHeader *)r->bin_headers.p, (const uint32_t *)r->info_bin_data.p, (const VbPath *)r->paths.p,
                                          (const VbTile *)r->tiles.p, bump, (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p,
-                                         c.width_in_tiles * c.height_in_tiles, st);
+                                         c.width_in_tiles * c.tile_rows, st);
             if (fork_tiling) {
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->tiling_fork, 0));
                 launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
@@ -807,20 +832,22 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // With a host destination (vb_render) fine is launched in up to 8 bands of tile rows and each band's
             // device->host copy is queued on a second stream behind an event, so the read-back of band k overlaps
             // the rasterisation of band k+1 (only the last band's copy is exposed).
-            const uint32_t rows = c.win_ty1 - c.win_ty0;
-            uint32_t n_bands = (d.host && rows >= 64u) ? d.bands : 1u;
+            // A batch paints every tile row of the tall frame in one launch (its cells are not rows of one image).
+            const uint32_t ty0 = c.n_cells > 1u ? 0u : c.win_ty0, ty1 = c.n_cells > 1u ? c.tile_rows : c.win_ty1;
+            const uint32_t rows = ty1 - ty0;
+            uint32_t n_bands = (d.host && rows >= 64u && c.n_cells == 1u) ? d.bands : 1u;
             const uint32_t band_rows = (rows + n_bands - 1u) / n_bands;
             for (uint32_t b = 0; b < n_bands; b++) {
                 VbConfig cb = c;
-                cb.win_ty0 = c.win_ty0 + b * band_rows;
-                cb.win_ty1 = cb.win_ty0 + band_rows < c.win_ty1 ? cb.win_ty0 + band_rows : c.win_ty1;
+                cb.win_ty0 = ty0 + b * band_rows;
+                cb.win_ty1 = cb.win_ty0 + band_rows < ty1 ? cb.win_ty0 + band_rows : ty1;
                 if (cb.win_ty0 >= cb.win_ty1) break;
                 launches += vb_launch_fine(&cb, (int)r->params.aa, bump, (const VbSegment *)r->segments.p, (const uint32_t *)r->ptcl.p,
                                            (const uint32_t *)r->info_bin_data.p, (uint32_t *)r->blend_spill.p, (uint32_t *)d.dev,
                                            (const uint32_t *)r->cur->ramps.p, (const uint8_t *)r->cur->atlas.p, (const uint32_t *)r->mask8.p,
                                            (const uint32_t *)r->mask16.p, (const uint32_t *)r->tile_start.p, r->occlusion_cull,
                                            ctl + VB_CTL_FINE_QUEUE + b, r->cls_list.p, n_bands == 1u ? ctl + VB_CTL_FINE_CLASS : nullptr,
-                                           c.width_in_tiles * c.height_in_tiles, r->sm_count, st);
+                                           c.width_in_tiles * c.tile_rows, r->sm_count, st);
                 if (d.host && (rc = queue_readback(r, c, cb.win_ty0, cb.win_ty1, d, b))) return rc;
             }
             break;
@@ -869,7 +896,7 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
     if (!r->use_graph || r->timing || first != 0 || last != VB_N_STAGE_IDS - 1) return enqueue_direct(r, first, last, d, clear_queues);
     // with a host destination split into bands, fine and its interleaved copies stay outside the graph
     const uint32_t rows = c.win_ty1 - c.win_ty0;
-    const bool banded = d.host && rows >= 64u && d.bands > 1u;
+    const bool banded = d.host && rows >= 64u && d.bands > 1u && c.n_cells == 1u;
     const int g_last = banded ? VB_STAGE_ID_FINE - 1 : last;
     GraphKey key;
     graph_key(r, g_last, d.dev, &key);
@@ -928,6 +955,7 @@ static int pick_out(vb_renderer *r, Dest *d) {
     if (d->dev) return VB_OK;
     const VbConfig &c = r->cfg;
     size_t rows = (size_t)(c.win_ty1 - c.win_ty0) * 16u;
+    if (c.n_cells > 1u) rows = (size_t)c.n_cells * c.target_height;
     DevBuf &t = d->alt ? r->target_alt : r->target;
     int rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * rows);
     d->dev = t.p;
@@ -1370,7 +1398,7 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
     const VbConfig &c = r->cfg;
     const VbLayout &L = r->cur->layout;
     const uint32_t wb = (c.width_in_tiles + 15u) / 16u, hb = (c.height_in_tiles + 15u) / 16u;
-    const uint32_t aligned_n_bins = (wb * hb + 255u) & ~255u;
+    const uint32_t aligned_n_bins = (wb * hb * std::max(c.n_cells, 1u) + 255u) & ~255u;
     std::vector<NamedBuf> v = {
         {"scene", &r->cur->scene, r->cur->scene_words * 4}, // the uploaded / device-resolved inputs
         {"ramps", &r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4},
@@ -1516,6 +1544,49 @@ extern "C" int vb_set_occlusion_cull(vb_renderer *r, int on) {
     return VB_OK;
 }
 
+// ---- batches: many scenes of one size in one pass (vb_scene_batch builds the scene) ---------------------------------------
+// The offsets split the uploaded scene's draw objects into cells. Validated here against the uploaded draw tags (one download):
+// a cell whose clips do not balance would pair a BEGIN_CLIP of one cell with an END_CLIP of the next. What depends on the
+// frame size (arena indexing) and on the call (windows) is checked when a frame is prepared.
+extern "C" int vb_set_cells(vb_renderer *r, const uint32_t *draw_offsets, uint32_t n_cells) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_set_cells: " + why;
+        return VB_E_INVALID;
+    };
+    if (!draw_offsets || n_cells == 0u) return bad("no offsets");
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
+    if (r->xc.enabled || r->grouped) return bad("a batch cannot be combined with vb_group or the exchange");
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    CK(cudaSetDevice(r->device));
+    const VbLayout &L = r->cur->layout;
+    const uint32_t n_draw = L.n_draw_objects;
+    if (draw_offsets[0] != 0u || draw_offsets[n_cells] != n_draw) return bad("offsets must start at 0 and end at the scene's draw-object count");
+    for (uint32_t c = 0; c < n_cells; c++)
+        if (draw_offsets[c + 1] < draw_offsets[c]) return bad("offsets must not decrease");
+    if (n_cells == 1u) { // the whole scene: no batch
+        r->cells.clear();
+        return VB_OK;
+    }
+    std::vector<uint32_t> tags(n_draw);
+    if (n_draw) {
+        CK(cudaMemcpyAsync(tags.data(), (const uint32_t *)r->cur->scene.p + L.draw_tag_base, (size_t)n_draw * 4, cudaMemcpyDeviceToHost, r->stream));
+        CK(cudaStreamSynchronize(r->stream));
+    }
+    for (uint32_t c = 0; c < n_cells; c++) {
+        int64_t depth = 0;
+        for (uint32_t i = draw_offsets[c]; i < draw_offsets[c + 1] && depth >= 0; i++)
+            depth += tags[i] == VB_DRAWTAG_BEGIN_CLIP ? 1 : tags[i] == VB_DRAWTAG_END_CLIP ? -1 : 0;
+        if (depth != 0) return bad("the clips of cell " + std::to_string(c) + " do not balance");
+    }
+    if ((rc = ensure(r, r->cell_draw, ((size_t)n_cells + 1u) * 4u))) return rc;
+    r->cells.assign(draw_offsets, draw_offsets + n_cells + 1u);
+    // in stream order: a frame still running reads the previous offsets
+    CK(cudaMemcpyAsync(r->cell_draw.p, r->cells.data(), r->cells.size() * 4u, cudaMemcpyHostToDevice, r->stream));
+    return VB_OK;
+}
+
 extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint64_t *segment_refs, uint64_t *fill_cmds) {
     if (!r) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
@@ -1523,8 +1594,10 @@ extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint6
     unsigned long long *d = nullptr, h[3] = {0, 0, 0};
     CK(cudaMalloc(&d, sizeof h));
     CK(cudaMemset(d, 0, sizeof h));
-    uint32_t n = r->cfg.width_in_tiles * (r->cfg.win_ty1 - r->cfg.win_ty0);
-    if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(r->cfg, (const uint32_t *)r->ptcl.p,
+    VbConfig c = r->cfg;
+    if (c.n_cells > 1u) c.win_ty0 = 0u, c.win_ty1 = c.tile_rows; // a batch: every cell
+    uint32_t n = c.width_in_tiles * (c.win_ty1 - c.win_ty0);
+    if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(c, (const uint32_t *)r->ptcl.p,
                                                                 r->occlusion_cull ? (const uint32_t *)r->tile_start.p : nullptr, d);
     CK(cudaStreamSynchronize(r->stream));
     CK(cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost));
@@ -1641,6 +1714,7 @@ extern "C" int vb_group_new(const int32_t *devices, uint32_t n, const vb_options
             vb_group_free(g);
             return rc;
         }
+        r->grouped = true;
         g->subs.push_back(r);
         g->devices.push_back(devices[i]);
         cudaEvent_t ev = nullptr;
@@ -2093,6 +2167,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     r->cur->layout = L;
     r->cur->scene_words = total_words;
     r->cur->have_scene = true;
+    r->cells.clear();
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }

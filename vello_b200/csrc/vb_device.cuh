@@ -143,3 +143,13 @@ __device__ __forceinline__ uint32_t vb_span(float a, float b) {
 __device__ __forceinline__ uint32_t vb_scene(const uint32_t *__restrict__ scene, const VbConfig &cfg, uint32_t ix) {
     return ix < cfg.scene_words ? __ldg(scene + ix) : 0u;
 }
+// Batch: the cell of draw object `ix`, the last c with cell_draw[c] <= ix (empty cells are skipped: cell_draw[c + 1] > ix).
+__device__ __forceinline__ uint32_t vb_cell_of(const VbConfig &cfg, uint32_t ix) {
+    uint32_t lo = 0u, hi = cfg.n_cells; // cell_draw[lo] <= ix < cell_draw[hi]
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(cfg.cell_draw + mid) <= ix) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}

@@ -1320,6 +1320,21 @@ int vb_scene_append(vb_scene *dst, const vb_scene *src, const double *transform)
     return VB_OK;
 }
 
+int vb_scene_batch(vb_scene *dst, const vb_scene *const *scenes, uint32_t n, uint32_t *draw_offsets) {
+    if (!dst || (n && (!scenes || !draw_offsets))) return VB_E_INVALID;
+    for (uint32_t i = 0; i < n; i++)
+        if (!scenes[i] || scenes[i] == dst) return VB_E_INVALID;
+    vb_scene_reset(dst);
+    Encoding &e = dst->e;
+    if (draw_offsets) draw_offsets[0] = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        vb_scene_append(dst, scenes[i], nullptr);
+        while (e.n_open_clips > 0) e.encode_end_clip();
+        draw_offsets[i + 1] = e.n_paths; // after resolve every draw object is a path
+    }
+    return VB_OK;
+}
+
 int vb_scene_resolve(vb_scene *s, vb_packed *out) {
     if (!s || !out) return VB_E_INVALID;
     const Encoding &e = s->e;

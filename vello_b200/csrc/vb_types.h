@@ -55,6 +55,12 @@ typedef struct {
     uint32_t out_pitch_px;     /* output row pitch in pixels */
     uint32_t out_row0;         /* first pixel row stored at out[0] (stripe outputs) */
     uint32_t win_cull;         /* 1: a stripe window is set -- flatten skips segments that cannot reach its rows */
+    /* Batch (vb_set_cells): the draw objects are split into n_cells ranges cell_draw[c] .. cell_draw[c + 1], each rendered
+     * into its own width x height frame. The tile grid is a tall frame of tile_rows = n_cells * height_in_tiles rows; cell c
+     * owns tile rows [c * height_in_tiles, (c + 1) * height_in_tiles) and bin rows [c * hB, (c + 1) * hB). width_in_tiles,
+     * height_in_tiles and the windows above stay the CELL's. n_cells = 1: no batch (cell_draw unused). */
+    uint32_t n_cells, tile_rows;
+    const uint32_t *cell_draw; /* device: n_cells + 1 draw-object offsets */
 } VbConfig;
 
 /* One rectangle of k_atlas_blit (k_atlas.cu): w x h RGBA8 texels from device memory (rows src_pitch bytes apart, 4-byte

@@ -730,6 +730,21 @@ class Scene:
             e.encode_blurred_rounded_rect(color, rect.x1 - rect.x0, rect.y1 - rect.y0, radius, std_dev)
 
 
+def batch(scenes: Sequence[Scene]) -> Tuple[Scene, List[int]]:
+    """A batch for `Renderer.set_cells` / `render_batch` (the native `vb_scene_batch`): one scene holding every scene appended
+    with the identity transform, each followed by the END_CLIP / PATH tags that close its open layers (what resolve would add
+    at the end of that scene alone), and the draw-object offsets of the scenes (len(scenes) + 1 entries)."""
+    out = Scene()
+    e = out.encoding
+    offsets = [0]
+    for s in scenes:
+        e.append(s.encoding)
+        while e.n_open_clips > 0:
+            e.encode_end_clip()
+        offsets.append(e.n_paths)  # after resolve every draw object is a path
+    return out, offsets
+
+
 # ---------------------------------------------------------------------------------------------
 # Ramps (ramp_cache.rs:119-155) and image atlas (shelf packer; atlas placement is ours, the
 # reference uses guillotiere -- only the (x, y) written into draw data matters to the pipeline)

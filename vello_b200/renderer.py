@@ -127,6 +127,8 @@ def load_library() -> C.CDLL:
     lib.vb_exchange_enable.argtypes = [vp, C.c_int]
     lib.vb_override_image.argtypes = [vp, vp, C.c_uint32, C.c_uint32, vp, C.c_size_t]
     lib.vb_mark_override_image_dirty.argtypes = [vp, vp]
+    lib.vb_set_cells.argtypes = [vp, vp, C.c_uint32]
+    lib.vb_render_uploaded.argtypes = [vp, C.POINTER(_Params), vp, C.c_uint32, C.POINTER(FrameStats)]
     _lib = lib
     return lib
 
@@ -138,7 +140,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_new", "vb_group_free", "vb_group_size", "vb_group_renderer", "vb_group_last_error", "vb_group_render",
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
-                    "vb_override_image", "vb_mark_override_image_dirty"]
+                    "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells"]
 
 
 def _device_image(t):
@@ -316,6 +318,49 @@ class Renderer:
             for o in outs[-2:]:
                 if o is not None:
                     yield o
+
+    # -- batches: many scenes of one size in one pass (vb_set_cells) ---------------------------------------------------------
+    def set_cells(self, offsets):
+        """Split the uploaded scene's draw objects into cells (`offsets`: len = cells + 1, from `encoding.batch` or
+        `NativeScene.batch`): the following frames render cell c into frame c of an [N, H, W, 4] destination. A new upload
+        resets the renderer to one cell."""
+        arr = np.ascontiguousarray(offsets, dtype=np.uint32)
+        if arr.ndim != 1 or arr.size < 2:
+            raise ValueError("set_cells: offsets need at least two entries (cells + 1)")
+        self._check(self.lib.vb_set_cells(self.handle, arr.ctypes.data, arr.size - 1), "vb_set_cells")
+
+    def render_batch(self, scenes, params: RenderParams, out=None):
+        """Render every scene of `scenes` (all `Scene`s, or all `NativeScene`s, which are resolved on the device) at
+        params.width x params.height in ONE pass and return the [N, H, W, 4] RGBA8 frames: into `out` when it is a CUDA array
+        of that shape (`__cuda_array_interface__`, e.g. a torch uint8 tensor), else a new numpy array."""
+        from .encoding import batch
+        from .scene_native import NativeScene
+        scenes = list(scenes)
+        n, h, w = len(scenes), int(params.height), int(params.width)
+        if n == 0:
+            raise ValueError("render_batch: no scenes")
+        if all(isinstance(s, NativeScene) for s in scenes):
+            b = NativeScene()
+            offsets = b.batch(scenes)
+            b.upload_device(self)
+        else:
+            bs, offsets = batch(scenes)
+            self.upload(resolve(bs.encoding))
+        self.set_cells(offsets)
+        ps = _params_struct(params)
+        st = FrameStats()
+        if out is not None and hasattr(out, "__cuda_array_interface__"):
+            cai = out.__cuda_array_interface__
+            shape = tuple(int(v) for v in cai["shape"])
+            if shape != (n, h, w, 4) or cai["typestr"] not in ("|u1", "<u1", ">u1") or cai.get("strides") not in (None, (h * w * 4, w * 4, 4, 1)):
+                raise ValueError(f"render_batch: out must be a contiguous uint8 ({n}, {h}, {w}, 4) array, not {shape} {cai['typestr']}")
+            rc = self.lib.vb_render_uploaded(self.handle, C.byref(ps), C.c_void_p(int(cai["data"][0])), 1, C.byref(st))
+        else:
+            out = np.zeros((n, h, w, 4), dtype=np.uint8)
+            rc = self.lib.vb_render_uploaded(self.handle, C.byref(ps), C.c_void_p(out.ctypes.data), 0, C.byref(st))
+        self.last_stats = st
+        self._check(rc, "vb_render_uploaded")
+        return out
 
     @staticmethod
     def stripe_rows(params: RenderParams, bin_rows=(0, 0), tile_rows=(0, 0)):

@@ -54,7 +54,7 @@ PATHBUF_SYMBOLS = ["vb_pathbuf_new", "vb_pathbuf_free", "vb_pathbuf_clear", "vb_
                    "vb_pathbuf_svg", "vb_pathbuf_view"]
 SCENE_SYMBOLS = ["vb_scene_new", "vb_scene_free", "vb_scene_reset", "vb_scene_fill", "vb_scene_stroke", "vb_scene_push_layer",
                  "vb_scene_push_luminance_mask_layer", "vb_scene_push_clip_layer", "vb_scene_pop_layer", "vb_scene_draw_image",
-                 "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
+                 "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_batch", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
                  "vb_register_texture", "vb_unregister_texture"]
 
 _bound = False
@@ -78,6 +78,7 @@ def _lib():
         lib.vb_scene_draw_blurred_rounded_rect.argtypes = [vp, vp, vp, _Color, C.c_double, C.c_double]
         lib.vb_scene_draw_blurred_rounded_rect_in.argtypes = [vp, vp, vp, vp, _Color, C.c_double, C.c_double]
         lib.vb_scene_append.argtypes = [vp, vp, vp]
+        lib.vb_scene_batch.argtypes = [vp, vp, C.c_uint32, vp]
         lib.vb_scene_resolve.argtypes = [vp, vp]
         lib.vb_render_scene.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
         lib.vb_scene_upload_device.argtypes = [vp, vp, vp]
@@ -247,6 +248,17 @@ class NativeScene:
     def append(self, other: "NativeScene", transform: Optional[Affine] = None):
         self._keep.append(other)  # its image buffers must outlive this scene's resolve
         self._check(self.lib.vb_scene_append(self.handle, other.handle, _affine(transform) if transform is not None else None))
+
+    def batch(self, scenes) -> list:
+        """`vb_scene_batch`: make this scene the batch of `scenes` (for `Renderer.set_cells`) and return its draw-object
+        offsets (len(scenes) + 1 entries)."""
+        scenes = list(scenes)
+        self._keep = list(scenes)  # their image buffers must outlive this scene's resolve
+        self._images, self._pixels = {}, {}
+        arr = (C.c_void_p * max(len(scenes), 1))(*[s.handle for s in scenes])
+        offs = (C.c_uint32 * (len(scenes) + 1))()
+        self._check(self.lib.vb_scene_batch(self.handle, arr, len(scenes), offs))
+        return [int(v) for v in offs]
 
     # -- Resolver::resolve ---------------------------------------------------------------------------
     def upload_device(self, renderer) -> Layout:
