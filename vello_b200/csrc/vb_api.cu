@@ -42,8 +42,8 @@ uint32_t vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathB
 uint32_t vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
                           cudaStream_t);
 uint32_t vb_tile_alloc_parts(uint32_t);
-uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, uint32_t *, int, cudaStream_t);
-uint32_t vb_backdrop_parts(uint32_t, int);
+uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, uint32_t *, uint32_t, cudaStream_t);
+uint32_t vb_backdrop_parts(uint32_t);
 uint32_t vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
                           cudaStream_t);
 uint32_t vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
@@ -675,7 +675,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     r->parts_flatten = vb_flatten_parts(c.n_tag_words);
     r->parts_draw = vb_draw_parts(n_draw);
     r->parts_tile = vb_tile_alloc_parts(n_draw);
-    r->parts_backdrop = vb_backdrop_parts(n_draw, r->sm_count);
+    r->parts_backdrop = vb_backdrop_parts(c.tiles_size); // follows the tile arena: set above, regrown on retry
     size_t off = VB_CTL_HEADER_WORDS;
     r->off_lb_pathtag = off; off += vb_lookback_words(r->parts_pathtag, 5);
     r->off_lb_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
@@ -683,7 +683,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     r->off_lb_draw = off; off += vb_lookback_words(r->parts_draw, 4);
     r->off_lb_tile = off; off += vb_lookback_words(r->parts_tile, 1);
     r->off_lb_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
-    r->off_lb_backdrop = off; off += vb_lookback_words(r->parts_backdrop, 1);
+    r->off_lb_backdrop = off; off += vb_lookback_words(r->parts_backdrop, 3);
     r->ctl_words = off;
     if ((rc = ensure(r, r->ctl, off * 4))) return rc;
     if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(r->parts_flatten) * 4))) return rc;
@@ -803,7 +803,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
                                              (VbSegmentCount *)r->seg_counts.p, capacity_grid(c.lines_size, r->sm_count), st);
             break;
         case VB_STAGE_ID_BACKDROP:
-            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, ctl + r->off_lb_backdrop, r->sm_count, st);
+            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, ctl + r->off_lb_backdrop, r->parts_backdrop, st);
             break;
         case VB_STAGE_ID_COARSE:
             // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before

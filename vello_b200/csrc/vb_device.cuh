@@ -1,7 +1,7 @@
 // vb_device.cuh -- device-side building blocks shared by the stage kernels.
 //
 //  * warp-shuffle scans (32-wide warps; no shared-memory log-step scans as in the WGSL)
-//  * single-pass "decoupled look-back" prefix over a K-field u32 sum monoid (Merrill & Garland):
+//  * single-pass "decoupled look-back" prefix over a K-field u32 monoid, a sum unless another is given (Merrill & Garland):
 //    partitions take a ticket (so partition p only waits on partitions that already started),
 //    publish {aggregate | inclusive prefix} descriptors, and warp 0 walks the predecessors 32 at
 //    a time. This replaces the reference's 2-3 dispatch reduce/scan chains
@@ -87,9 +87,33 @@ __device__ __forceinline__ uint32_t vb_take_ticket(const VbLookback &s, uint32_t
     return t;
 }
 
+// The monoid of a look-back: K u32 words whose identity is all zeros, and combine(a, b, r): r = a (+) b, where a is the
+// earlier operand (r may alias a or b). The default is the field-wise sum.
+struct VbSumOp {
+    static constexpr bool commutative = true;
+    template <int K> __device__ __forceinline__ static void combine(const uint32_t (&a)[K], const uint32_t (&b)[K], uint32_t (&r)[K]) {
+#pragma unroll
+        for (int k = 0; k < K; k++) r[k] = a[k] + b[k];
+    }
+};
+// Warp reduction of a non-commutative monoid in which a HIGHER lane holds an EARLIER element: every lane ends with
+// v[31] (+) v[30] (+) ... (+) v[0]. After the step of width o, a lane holds its aligned block of 2o lanes.
+template <int K, class Op> __device__ __forceinline__ void vb_warp_reduce_rev(uint32_t (&v)[K]) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t p[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) p[k] = __shfl_xor_sync(VB_FULL, v[k], o);
+        if (vb_lane() & (uint32_t)o) Op::combine(v, p, v); // my block is the earlier one
+        else Op::combine(p, v, v);
+    }
+}
+
 // Must be called by ALL threads of warp 0 (other warps skip it). `agg` = this partition's
-// aggregate (same value in every lane). On return `excl` = sum of all earlier partitions.
-template <int K>
+// aggregate (same value in every lane). On return `excl` = the combination of all earlier partitions, in partition order.
+// A non-commutative Op is reduced in that order: lane 0 of a window holds the nearest predecessor, the cutoff lane the
+// inclusive prefix of the earliest one.
+template <int K, class Op = VbSumOp>
 __device__ __forceinline__ void vb_lookback(const VbLookback &s, uint32_t part, const uint32_t (&agg)[K], uint32_t (&excl)[K]) {
     const uint32_t lane = vb_lane();
 #pragma unroll
@@ -118,15 +142,22 @@ __device__ __forceinline__ void vb_lookback(const VbLookback &s, uint32_t part, 
 #pragma unroll
             for (int k = 0; k < K; k++) v[k] = src[k];
         }
+        if constexpr (Op::commutative) {
 #pragma unroll
-        for (int k = 0; k < K; k++) excl[k] += vb_warp_sum(v[k]);
+            for (int k = 0; k < K; k++) excl[k] += vb_warp_sum(v[k]);
+        } else {
+            vb_warp_reduce_rev<K, Op>(v);
+            Op::combine(v, excl, excl); // this window lies before the nearer ones already in excl
+        }
         if (pm) break;
         idx -= 32;
     }
     if (lane == 0) {
         uint32_t *dst = s.pref + (size_t)part * K;
+        uint32_t incl[K];
+        Op::combine(excl, agg, incl);
 #pragma unroll
-        for (int k = 0; k < K; k++) dst[k] = excl[k] + agg[k];
+        for (int k = 0; k < K; k++) dst[k] = incl[k];
         vb_st_flag(s.flags + part, 2u);
     }
 }
