@@ -9,6 +9,7 @@
 // 16-byte load only when it is full and its source texels start on a 16-byte boundary; otherwise texel by texel.
 #include "vb_device.cuh"
 #include "vb_types.h"
+#include "vb_stages.h"
 
 #define AB_THREADS 256u
 #define AB_UNITS_PER_THREAD 4u

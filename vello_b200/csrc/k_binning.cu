@@ -7,6 +7,7 @@
 // chunk ORDER in bin_data is not deterministic -- consumers only go through the headers.
 // Extension: the bin-row window [win_by0, win_by1) restricts binning to this GPU's stripe.
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define BN_THREADS 256
 #define BN_N_SLICE 8
@@ -124,12 +125,10 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
     }
 }
 
-extern "C" uint32_t vb_launch_binning(const VbConfig *cfg, const VbDrawMonoid *draw_monoids, const VbPathBbox *path_bbox,
-                                  const VbBbox4 *clip_bbox, VbBbox4 *draw_bbox, VbBump *bump, uint32_t *info_bin_data,
-                                  VbBinHeader *bin_header, cudaStream_t st) {
-    uint32_t n = cfg->layout.n_draw_objects;
+extern "C" uint32_t vb_launch_binning(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    uint32_t n = cfg.layout.n_draw_objects;
     if (n == 0) return 0;
-    k_binning<<<(n + BN_THREADS - 1) / BN_THREADS, BN_THREADS, 0, st>>>(*cfg, draw_monoids, path_bbox, clip_bbox, draw_bbox, bump,
-                                                                       info_bin_data, bin_header);
+    k_binning<<<(n + BN_THREADS - 1) / BN_THREADS, BN_THREADS, 0, st>>>(cfg, b.draw_monoids, b.path_bboxes, b.clip_bboxes, b.draw_bboxes, b.bump(),
+                                                                       b.info_bin_data, b.bin_headers);
     return 1;
 }

@@ -13,6 +13,7 @@
 // Any nesting depth is supported (the reference's GPU path stops at 256), results identical
 // to the CPU shader for every depth.
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define CL_THREADS 1024
 
@@ -135,18 +136,17 @@ __global__ void k_clip_bbox(uint32_t n_clips, const VbClipInp *__restrict__ clip
 }
 
 extern "C" uint32_t vb_clip_parts(uint32_t n_clips) { return (n_clips + CL_THREADS - 1u) / CL_THREADS; }
-extern "C" uint32_t vb_launch_clip(uint32_t n_clips, const VbClipInp *clip_inp, const VbPathBbox *pbs, VbDrawMonoid *draw_monoids,
-                               VbBbox4 *clip_bboxes, int32_t *scratch /* B | min32 | min1024 | link */, uint32_t *lb_mem /* zeroed */,
-                               cudaStream_t st) {
+extern "C" uint32_t vb_launch_clip(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    const uint32_t n_clips = cfg.layout.n_clips;
     if (n_clips == 0) return 0;
-    int32_t *B = scratch;
+    int32_t *B = b.clip_scratch; // B | min32 | min1024 | link
     int32_t *min32 = B + n_clips;
     int32_t *min1024 = min32 + (n_clips + 31) / 32;
     int32_t *link = min1024 + (n_clips + 1023) / 1024;
     const uint32_t n_parts = vb_clip_parts(n_clips);
-    k_clip_depth<<<n_parts, CL_THREADS, 0, st>>>(n_clips, clip_inp, B, min32, min1024, lb_mem, n_parts);
-    k_clip_link<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, clip_inp, B, min32, min1024, link);
-    k_clip_bbox<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, clip_inp, pbs, link, draw_monoids, clip_bboxes);
+    k_clip_depth<<<n_parts, CL_THREADS, 0, st>>>(n_clips, b.clip_inp, B, min32, min1024, b.lb_clip, n_parts);
+    k_clip_link<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, B, min32, min1024, link);
+    k_clip_bbox<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, b.path_bboxes, link, b.draw_monoids, b.clip_bboxes);
     return 3;
 }
 extern "C" size_t vb_clip_scratch_words(uint32_t n_clips) {

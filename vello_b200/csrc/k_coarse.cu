@@ -18,6 +18,7 @@
 // bump.segments and each CTA subtracts the segments of the fills it emits, so `bump.segments - holes` is the
 // reference's number.
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define CO_THREADS 256
 #define CO_MINB 5 // CTAs per SM: 48 registers, no spills
@@ -428,14 +429,13 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
 // The segments-arena overflow check (the reference sizes `segments` statically and never checks) lives at the top of
 // k_path_tiling, which runs beside coarse.
 
-extern "C" uint32_t vb_launch_coarse(const VbConfig *cfg, const uint32_t *scene, const VbDrawMonoid *draw_monoids,
-                                 const VbBinHeader *bin_headers, const uint32_t *info_bin_data, const VbPath *paths, const VbTile *tiles,
-                                 VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, void *cls_list, uint32_t cls_stride, cudaStream_t st) {
-    uint32_t width_in_bins = (cfg->width_in_tiles + 15u) / 16u;
-    uint32_t rows = cfg->win_by1 - cfg->win_by0;
-    if (cfg->n_cells > 1u) rows *= cfg->n_cells; // a batch has no window: every cell's bin rows, stacked
+extern "C" uint32_t vb_launch_coarse(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    uint32_t width_in_bins = (cfg.width_in_tiles + 15u) / 16u;
+    uint32_t rows = cfg.win_by1 - cfg.win_by0;
+    if (cfg.n_cells > 1u) rows *= cfg.n_cells; // a batch has no window: every cell's bin rows, stacked
     if (width_in_bins == 0 || rows == 0) return 0;
     dim3 grid(width_in_bins * 2u, rows * 2u); // four quadrant CTAs per bin
-    k_coarse<<<grid, CO_THREADS, 0, st>>>(*cfg, scene, draw_monoids, bin_headers, info_bin_data, paths, tiles, bump, ptcl, tile_start, (uint2 *)cls_list, cls_stride);
+    k_coarse<<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
+                                          b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows);
     return 1;
 }

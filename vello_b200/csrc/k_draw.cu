@@ -7,6 +7,7 @@
 // Design: one pass, decoupled look-back over the 4-field monoid (the WGSL strides <= 256
 // workgroups over the tags and rescans the reduced prefix in every workgroup).
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define DR_THREADS 256
 
@@ -233,10 +234,9 @@ k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const VbPathBbox *__res
     }
 }
 
-extern "C" uint32_t vb_launch_draw(const VbConfig *cfg, const uint32_t *scene, const VbPathBbox *path_bbox, VbDrawMonoid *draw_monoid,
-                               uint32_t *info, VbClipInp *clip_inp, uint32_t *lb_mem, uint32_t n_parts, cudaStream_t st) {
-    if (n_parts == 0) return 0;
-    k_draw<<<n_parts, DR_THREADS, 0, st>>>(*cfg, scene, path_bbox, draw_monoid, info, clip_inp, lb_mem, n_parts);
+extern "C" uint32_t vb_launch_draw(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (b.parts_draw == 0) return 0;
+    k_draw<<<b.parts_draw, DR_THREADS, 0, st>>>(cfg, b.scene, b.path_bboxes, b.draw_monoids, b.info_bin_data, b.clip_inp, b.lb_draw, b.parts_draw);
     return 1;
 }
 extern "C" uint32_t vb_draw_parts(uint32_t n_draw) { return (n_draw + DR_THREADS - 1) / DR_THREADS; }

@@ -22,8 +22,7 @@
 // overwritten while somebody still reads it. Works across processes (arenas exported with CUDA IPC) and inside one
 // (vb_group), and -- for the tests -- between several renderers on ONE GPU.
 #include "vb_device.cuh"
-
-#define XG_MAX 8u // GPUs of one box
+#include "vb_stages.h"
 
 // layout of one arena half (bytes): [XHdr 256][VbPathBbox x n_paths][pad to 256][VbLineSoup x lines_cap]
 struct XHdr {
@@ -32,12 +31,7 @@ struct XHdr {
 };
 // An arena: [flags: XG_MAX words][epoch counter: word 16][pad to 256 B][half 0][half 1]. The epoch counter is advanced by the
 // frame's first kernel (k_frame_init, vb_api.cu) and READ by the kernels below, so a captured CUDA graph replays correctly.
-struct XPeers {
-    unsigned char *base[XG_MAX]; // peer s: its arena (own arena at [rank])
-    uint32_t rows[XG_MAX + 1];   // stripe boundaries in tile rows
-    uint32_t world, rank, n_paths, lines_cap;
-    unsigned long long half_bytes;
-};
+// The peer table (XPeers) is in vb_stages.h.
 #define X_EPOCH_WORD 16u
 __device__ __forceinline__ uint32_t x_epoch(const XPeers &X) { return *(reinterpret_cast<const volatile uint32_t *>(X.base[X.rank]) + X_EPOCH_WORD); }
 __device__ __forceinline__ unsigned char *x_half(const XPeers &X, uint32_t s, uint32_t epoch) {
@@ -47,7 +41,6 @@ __device__ __forceinline__ uint32_t *x_flags(const XPeers &X, uint32_t s) { retu
 __host__ __device__ inline size_t x_bbox_off() { return 256; }
 __host__ __device__ inline size_t x_lines_off(uint32_t n_paths) { return (256 + (size_t)n_paths * sizeof(VbPathBbox) + 255) & ~(size_t)255; }
 extern "C" size_t vb_exchange_half_bytes(uint32_t n_paths, uint32_t lines_cap) { return x_lines_off(n_paths) + (size_t)lines_cap * sizeof(VbLineSoup) + 256; }
-extern "C" size_t vb_exchange_flag_bytes(void) { return 256; }
 extern "C" uint32_t vb_exchange_epoch_word(void) { return X_EPOCH_WORD; }
 
 __device__ __forceinline__ uint32_t x_dest_mask(const XPeers &X, float y0, float y1) {
@@ -240,23 +233,19 @@ __global__ void __launch_bounds__(256) k_lines_pull(XPeers X, VbBump *bump, uint
 // send = everything up to raising my flags; recv = wait for the peers, combine the boxes, pull my lines. They are separate
 // entry points so that a host driving several renderers on ONE device can issue every send before any recv (a wait kernel
 // never sits in front of the signal it waits for in a shared hardware queue).
-extern "C" uint32_t vb_launch_exchange_send(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines, uint32_t *scratch,
-                                        VbPathBbox *path_bboxes, int sm_count, cudaStream_t st) {
-    const XPeers &X = *reinterpret_cast<const XPeers *>(peers);
-    const uint32_t grid = (uint32_t)sm_count * 8u;
-    k_route_count<<<grid, 256, 0, st>>>(X, bump, lines_size, lines, scratch);
-    k_route_scatter<<<grid, 256, 0, st>>>(X, bump, lines_size, lines, scratch, scratch + XG_MAX);
-    if (X.n_paths) k_bbox_publish<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, path_bboxes);
+extern "C" uint32_t vb_launch_exchange_send(const VbConfig &cfg, const VbFrameBufs &b, const XPeers &X, cudaStream_t st) {
+    const uint32_t grid = (uint32_t)b.sm_count * 8u;
+    uint32_t *scratch = b.ctl + VB_CTL_XCHG_SCRATCH;
+    k_route_count<<<grid, 256, 0, st>>>(X, b.bump(), cfg.lines_size, b.lines, scratch);
+    k_route_scatter<<<grid, 256, 0, st>>>(X, b.bump(), cfg.lines_size, b.lines, scratch, scratch + XG_MAX);
+    if (X.n_paths) k_bbox_publish<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, b.path_bboxes);
     k_xsignal<<<1, 32, 0, st>>>(X, scratch);
     return X.n_paths ? 4 : 3;
 }
-extern "C" uint32_t vb_launch_exchange_recv(const void *peers /* XPeers */, VbBump *bump, uint32_t lines_size, VbLineSoup *lines,
-                                        VbPathBbox *path_bboxes, int sm_count, cudaStream_t st) {
-    const XPeers &X = *reinterpret_cast<const XPeers *>(peers);
-    const uint32_t grid = (uint32_t)sm_count * 8u;
-    k_xwait<<<1, 32, 0, st>>>(X, bump, 4000000000ull); // ~2 s at 2 GHz
-    if (X.n_paths) k_bbox_combine<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, path_bboxes);
-    k_lines_pull<<<grid, 256, 0, st>>>(X, bump, lines_size, lines);
+extern "C" uint32_t vb_launch_exchange_recv(const VbConfig &cfg, const VbFrameBufs &b, const XPeers &X, cudaStream_t st) {
+    const uint32_t grid = (uint32_t)b.sm_count * 8u;
+    k_xwait<<<1, 32, 0, st>>>(X, b.bump(), 4000000000ull); // ~2 s at 2 GHz
+    if (X.n_paths) k_bbox_combine<<<(X.n_paths + 255u) / 256u, 256, 0, st>>>(X, b.path_bboxes);
+    k_lines_pull<<<grid, 256, 0, st>>>(X, b.bump(), cfg.lines_size, b.lines);
     return X.n_paths ? 3 : 2;
 }
-extern "C" size_t vb_exchange_peers_bytes(void) { return sizeof(XPeers); }

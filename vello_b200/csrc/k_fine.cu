@@ -32,6 +32,7 @@
 
 #include "vb_detmath.h"
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #ifndef FI_MAX_WARPS
 #define FI_MAX_WARPS 10 // warps (= tiles in flight) per CTA; the launcher picks 2..FI_MAX_WARPS by frame size. 2 CTAs x 10 warps leave
@@ -1238,32 +1239,32 @@ extern "C" int vb_fine_init_constants(void) {
     return (int)e;
 }
 
-// `queue` = one zeroed word per launch (vb_api.cu keeps 8 of them in the control block, one per read-back band).
-extern "C" uint32_t vb_launch_fine(const VbConfig *cfg, int aa, const VbBump *bump, const VbSegment *segments, const uint32_t *ptcl, const uint32_t *info,
-                               uint32_t *blend_spill, uint32_t *out, const uint32_t *ramps, const uint8_t *atlas,
-                               const uint32_t *mask_lut8, const uint32_t *mask_lut16, const uint32_t *tile_start, uint32_t cull, uint32_t *queue,
-                               const void *cls_list, const uint32_t *cls_count, uint32_t cls_stride, int sm_count, cudaStream_t st) {
-    uint32_t rows = cfg->win_ty1 - cfg->win_ty0;
-    uint32_t n = cfg->width_in_tiles * rows;
+// The launch's tile queue is control-block word VB_CTL_FINE_QUEUE + band, zeroed with the control block (8 of them, one per
+// read-back band).
+extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, uint32_t *out, int aa, uint32_t cull, uint32_t band, bool cls_order,
+                                   cudaStream_t st) {
+    uint32_t rows = cfg.win_ty1 - cfg.win_ty0;
+    uint32_t n = cfg.width_in_tiles * rows;
     if (n == 0) return 0;
     // persistent grid: FI_MINB CTAs per SM; small frames get smaller CTAs so that their tiles still spread over the SMs
+    const int sm_count = b.sm_count;
     uint32_t warps = FI_MAX_WARPS;
     while (warps > 2u && (n + warps - 1u) / warps < (uint32_t)sm_count * FI_MINB) warps >>= 1;
     uint32_t grid = (n + warps - 1u) / warps;
     const uint32_t resident = (uint32_t)sm_count * FI_MINB * (FI_MAX_WARPS / warps);
     if (grid > resident) grid = resident;
     FineArgs A;
-    A.segments = segments; A.ptcl = ptcl; A.info = info; A.blend_spill = blend_spill; A.out = out; A.ramps = ramps; A.atlas = atlas;
-    A.mask_lut = aa == 2 ? mask_lut16 : mask_lut8;
+    A.segments = b.segments; A.ptcl = b.ptcl; A.info = b.info_bin_data; A.blend_spill = b.blend_spill; A.out = out; A.ramps = b.ramps; A.atlas = b.atlas;
+    A.mask_lut = aa == 2 ? b.mask16 : b.mask8;
     A.cull = cull;
-    A.tile_start = tile_start;
-    A.bump = bump;
-    A.queue = queue;
-    A.cls_list = (const uint2 *)cls_list;
-    A.cls_count = cls_count;
-    A.cls_stride = cls_stride;
-    if (aa == 0) k_fine<0><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(*cfg, A);
-    else if (aa == 1) k_fine<1><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(*cfg, A);
-    else k_fine<2><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(*cfg, A);
+    A.tile_start = b.tile_start;
+    A.bump = b.bump();
+    A.queue = b.ctl + VB_CTL_FINE_QUEUE + band;
+    A.cls_list = b.cls_list;
+    A.cls_count = cls_order ? b.ctl + VB_CTL_FINE_CLASS : nullptr;
+    A.cls_stride = cfg.width_in_tiles * cfg.tile_rows;
+    if (aa == 0) k_fine<0><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, A);
+    else if (aa == 1) k_fine<1><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, A);
+    else k_fine<2><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, A);
     return 1;
 }

@@ -21,6 +21,7 @@
 
 #include "vb_detmath.h"
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #ifndef FL_THREADS
 #define FL_THREADS 256
@@ -1254,11 +1255,13 @@ k_flatten_place(VbConfig cfg, const uint32_t *__restrict__ scene, FlCtx ctx, con
     }
 }
 
-extern "C" uint32_t vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene, const VbTagMonoid *tag_monoids,
-                                  VbPathBbox *path_bboxes, VbBump *bump, VbLineSoup *lines, void *lit_arena, void *job_arena,
-                                  uint32_t *part_mem /* vb_flatten_part_words */, uint32_t *ctrs, uint32_t n_parts, int clear_bboxes,
-                                  uint32_t part_base, uint32_t part_end /* 0, n_parts: everything */, int sm_count, cudaStream_t st) {
-    uint32_t n_paths = cfg->layout.n_paths, launches = 0;
+extern "C" uint32_t vb_launch_flatten(const VbConfig &cfg, const VbFrameBufs &b, bool clear_bboxes, uint32_t part_base, uint32_t part_end,
+                                      cudaStream_t st) {
+    const uint32_t n_paths = cfg.layout.n_paths, n_parts = b.parts_flatten;
+    uint32_t launches = 0;
+    const uint32_t *scene = b.scene;
+    const VbTagMonoid *tag_monoids = b.tag_monoids;
+    VbPathBbox *path_bboxes = b.path_bboxes;
     // whole frames reset the boxes in k_frame_init (vb_api.cu); a stage range that starts later does it here
     if (n_paths && clear_bboxes) {
         k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
@@ -1266,13 +1269,14 @@ extern "C" uint32_t vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene
     }
     if (n_parts) {
         const size_t np4 = ((size_t)n_parts + 3u) & ~(size_t)3u; // 16-byte aligned sub-arrays (k_flatten_scan uses 128-bit accesses)
+        uint32_t *part_mem = b.flatten_parts; // vb_flatten_part_words
         uint32_t *part_count = part_mem, *part_dst = part_mem + np4, *tag_off = part_mem + 2 * np4, *work = part_mem + 34 * np4;
         FlCtx ctx;
-        ctx.lits = (FlLit *)lit_arena;
-        ctx.jobs = (FlJob *)job_arena;
-        ctx.lits_cap = cfg->lines_size;
-        ctx.jobs_cap = cfg->lines_size / FL_DEFER_MIN + 1u;
-        ctx.ctrs = ctrs;
+        ctx.lits = b.line_scratch;
+        ctx.jobs = b.flatten_jobs;
+        ctx.lits_cap = cfg.lines_size;
+        ctx.jobs_cap = cfg.lines_size / FL_DEFER_MIN + 1u;
+        ctx.ctrs = b.lb_flatten;
         const uint32_t warps_per_cta = FL_THREADS / 32;
         if (part_end > n_parts) part_end = n_parts;
         if (part_base >= part_end) { // an empty share still has to publish bump.lines = 0
@@ -1281,14 +1285,14 @@ extern "C" uint32_t vb_launch_flatten(const VbConfig *cfg, const uint32_t *scene
         const uint32_t n_own = part_end - part_base; // part_base is a multiple of 8: the scan's 128-bit accesses stay aligned
         if (n_own) {
             const uint32_t grid = (n_own + warps_per_cta - 1) / warps_per_cta;
-            k_flatten_lean<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work, part_base,
+            k_flatten_lean<<<grid, FL_THREADS, 0, st>>>(cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work, part_base,
                                                         part_end);
-            k_flatten<<<grid, FL_THREADS, 0, st>>>(*cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work);
+            k_flatten<<<grid, FL_THREADS, 0, st>>>(cfg, scene, tag_monoids, path_bboxes, ctx, part_count, tag_off, work);
             launches += 2;
         }
         const uint32_t n_blocks = n_own ? (n_own + FS_THREADS * FS_PER_THREAD - 1u) / (FS_THREADS * FS_PER_THREAD) : 1u;
-        k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(*cfg, n_own, part_count + part_base, part_dst + part_base, bump, ctrs + 4, n_blocks);
-        k_flatten_place<<<(uint32_t)sm_count * 4u, FP_THREADS, 0, st>>>(*cfg, scene, ctx, part_dst, tag_off, path_bboxes, lines);
+        k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(cfg, n_own, part_count + part_base, part_dst + part_base, b.bump(), ctx.ctrs + 4, n_blocks);
+        k_flatten_place<<<(uint32_t)b.sm_count * 4u, FP_THREADS, 0, st>>>(cfg, scene, ctx, part_dst, tag_off, path_bboxes, b.lines);
         launches += 2;
     }
     return launches;

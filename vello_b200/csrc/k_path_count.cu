@@ -12,6 +12,7 @@
 // (iii) backdrop / count updates are fire-and-forget RED operations except the slot fetch.
 // Per-tile slot order (seg_within_slice) is atomic-order dependent exactly as in the reference.
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #ifndef PC_THREADS
 #define PC_THREADS 256
@@ -166,9 +167,11 @@ k_path_count(VbConfig cfg, VbBump *bump, const VbLineSoup *__restrict__ lines, c
 
 // The seg_counts overflow check (the WGSL does it at the top of coarse) lives at the top of k_backdrop, the next kernel.
 
-extern "C" uint32_t vb_launch_path_count(const VbConfig *cfg, VbBump *bump, const VbLineSoup *lines, const VbPath *paths, VbTile *tile,
-                                     VbSegmentCount *seg_counts, uint32_t grid, cudaStream_t st) {
+// The grid comes from the lines capacity (at most 16 CTAs per SM); the kernel strides over the count read on the device.
+extern "C" uint32_t vb_launch_path_count(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    const uint64_t blocks = ((uint64_t)cfg.lines_size + 255) / 256, most = (uint64_t)b.sm_count * 16;
+    const uint32_t grid = (uint32_t)(blocks < most ? blocks : most);
     if (grid == 0) return 0;
-    k_path_count<<<grid, PC_THREADS, 0, st>>>(*cfg, bump, lines, paths, tile, seg_counts);
+    k_path_count<<<grid, PC_THREADS, 0, st>>>(cfg, b.bump(), b.lines, b.paths, b.tiles, b.seg_counts);
     return 1;
 }

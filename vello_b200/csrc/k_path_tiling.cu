@@ -9,6 +9,7 @@
 // Algorithmic bytes per crossing: 8 (SegmentCount) + 24 (LineSoup gather) + 32 (Path) + 8 (Tile)
 // read, 24 written (scattered into the tile's slice).
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #ifndef PTI_THREADS
 #define PTI_THREADS 256
@@ -134,10 +135,11 @@ k_path_tiling(VbConfig cfg, VbBump *bump, const VbSegmentCount *__restrict__ seg
     }
 }
 
-extern "C" uint32_t vb_launch_path_tiling(const VbConfig *cfg, VbBump *bump, const VbSegmentCount *seg_counts,
-                                      const VbLineSoup *lines, const VbPath *paths, const VbTile *tiles, VbSegment *segments,
-                                      uint32_t grid, cudaStream_t st) {
+// The grid comes from the seg_counts capacity (at most 16 CTAs per SM); the kernel strides over the count read on the device.
+extern "C" uint32_t vb_launch_path_tiling(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    const uint64_t blocks = ((uint64_t)cfg.seg_counts_size + 255) / 256, most = (uint64_t)b.sm_count * 16;
+    const uint32_t grid = (uint32_t)(blocks < most ? blocks : most);
     if (grid == 0) return 0;
-    k_path_tiling<<<grid, PTI_THREADS, 0, st>>>(*cfg, bump, seg_counts, lines, paths, tiles, segments);
+    k_path_tiling<<<grid, PTI_THREADS, 0, st>>>(cfg, b.bump(), b.seg_counts, b.lines, b.paths, b.tiles, b.segments);
     return 1;
 }

@@ -9,6 +9,7 @@
 // warp shuffles, publishes its aggregate and resolves its prefix by decoupled look-back.
 // Algorithmic traffic: 4 B read + 20 B written per tag word (HBM-bound, no tensor cores).
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define PT_THREADS 256
 #define PT_WORDS_PER_THREAD 4
@@ -96,10 +97,9 @@ k_pathtag_scan(VbConfig cfg, const uint32_t *__restrict__ scene, VbTagMonoid *__
     }
 }
 
-extern "C" uint32_t vb_launch_pathtag(const VbConfig *cfg, const uint32_t *scene, VbTagMonoid *tag_monoids, uint32_t *lb_mem,
-                                  uint32_t n_parts, cudaStream_t st) {
-    if (n_parts == 0) return 0;
-    k_pathtag_scan<<<n_parts, PT_THREADS, 0, st>>>(*cfg, scene, tag_monoids, lb_mem, n_parts);
+extern "C" uint32_t vb_launch_pathtag(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (b.parts_pathtag == 0) return 0;
+    k_pathtag_scan<<<b.parts_pathtag, PT_THREADS, 0, st>>>(cfg, b.scene, b.tag_monoids, b.lb_pathtag, b.parts_pathtag);
     return 1;
 }
 extern "C" uint32_t vb_pathtag_parts(uint32_t n_tag_words) { return (n_tag_words + PT_PART - 1) / PT_PART; }

@@ -6,10 +6,7 @@
 // resolve.rs:268-330) and the gradient ramps themselves (512 premultiplied RGBA8 texels per unique gradient).
 // Arithmetic of the ramps is the host statement's (vb_scene.cpp make_ramp), float for float; the TU is built with -fmad=false.
 #include "vb_device.cuh"
-
-struct RsRamp { uint32_t first_stop, n_stops, premul, pad; };
-struct RsStop { float offset, r, g, b, a; };
-struct RsPatch { uint32_t word, value; };
+#include "vb_stages.h"
 
 #define RS_TAG_PATH 0x10u
 #define RS_DRAWTAG_END_CLIP 0x21u
@@ -86,12 +83,12 @@ k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
 }
 
 extern "C" void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes,
-                                         uint32_t end_clip_word0, const void *patches, uint32_t n_patches, cudaStream_t st) {
+                                         uint32_t end_clip_word0, const RsPatch *patches, uint32_t n_patches, cudaStream_t st) {
     const uint32_t work = max(max(padded_tag_bytes - n_tag_bytes, n_open_clips), n_patches);
     if (work == 0u) return;
     const uint32_t grid = min((work + 255u) / 256u, 592u);
-    k_resolve_finish<<<grid, 256, 0, st>>>(scene, n_tag_bytes, n_open_clips, padded_tag_bytes, end_clip_word0, (const RsPatch *)patches, n_patches);
+    k_resolve_finish<<<grid, 256, 0, st>>>(scene, n_tag_bytes, n_open_clips, padded_tag_bytes, end_clip_word0, patches, n_patches);
 }
-extern "C" void vb_launch_make_ramps(const void *ramps, const void *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st) {
-    if (n_ramps) k_make_ramps<<<n_ramps, RS_SAMPLES, 0, st>>>((const RsRamp *)ramps, (const RsStop *)stops, out);
+extern "C" void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st) {
+    if (n_ramps) k_make_ramps<<<n_ramps, RS_SAMPLES, 0, st>>>(ramps, stops, out);
 }

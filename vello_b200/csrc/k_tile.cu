@@ -10,6 +10,7 @@
 // coarse, so that path_tiling and coarse can run side by side (see k_backdrop).
 // Extension: tile rows are clamped to the stripe window [win_ty0, win_ty1).
 #include "vb_device.cuh"
+#include "vb_stages.h"
 
 #define TA_THREADS 256
 
@@ -316,11 +317,10 @@ k_backdrop(VbConfig cfg, VbBump *bump, const VbPath *__restrict__ paths, VbTile 
     }
 }
 
-extern "C" uint32_t vb_launch_tile_alloc(const VbConfig *cfg, const uint32_t *scene, const VbBbox4 *draw_bboxes, VbBump *bump,
-                                     VbPath *paths, VbTile *tiles, uint32_t *lb_mem, uint32_t n_parts, int sm_count, cudaStream_t st) {
-    if (n_parts == 0) return 0;
-    k_tile_alloc<<<n_parts, TA_THREADS, 0, st>>>(*cfg, scene, draw_bboxes, bump, paths, tiles, lb_mem, n_parts);
-    k_tile_zero<<<(uint32_t)sm_count * 4u, 256, 0, st>>>(*cfg, bump, tiles);
+extern "C" uint32_t vb_launch_tile_alloc(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (b.parts_tile == 0) return 0;
+    k_tile_alloc<<<b.parts_tile, TA_THREADS, 0, st>>>(cfg, b.scene, b.draw_bboxes, b.bump(), b.paths, b.tiles, b.lb_tile, b.parts_tile);
+    k_tile_zero<<<(uint32_t)b.sm_count * 4u, 256, 0, st>>>(cfg, b.bump(), b.tiles);
     return 2;
 }
 extern "C" uint32_t vb_tile_alloc_parts(uint32_t n_draw) { return (n_draw + TA_THREADS - 1) / TA_THREADS; }
@@ -329,9 +329,8 @@ extern "C" uint32_t vb_backdrop_parts(uint32_t tiles_size) {
     const uint32_t n = tiles_size / BD_CHUNK + (tiles_size % BD_CHUNK != 0u ? 1u : 0u);
     return n ? n : 1u;
 }
-extern "C" uint32_t vb_launch_backdrop(const VbConfig *cfg, VbBump *bump, const VbPath *paths, VbTile *tiles, uint32_t *lb_mem, uint32_t n_parts,
-                                       cudaStream_t st) {
-    if (cfg->layout.n_draw_objects == 0) return 0;
-    k_backdrop<<<n_parts, BD_THREADS, 0, st>>>(*cfg, bump, paths, tiles, lb_mem, n_parts);
+extern "C" uint32_t vb_launch_backdrop(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (cfg.layout.n_draw_objects == 0) return 0;
+    k_backdrop<<<b.parts_backdrop, BD_THREADS, 0, st>>>(cfg, b.bump(), b.paths, b.tiles, b.lb_backdrop, b.parts_backdrop);
     return 1;
 }

@@ -20,59 +20,9 @@
 
 #include "../../include/vello_b200.h"
 #include "vb_device.cuh"
+#include "vb_stages.h"
+#include "vb_textures.h"
 #include "vb_types.h"
-
-// ---- stage launchers (k_*.cu); each returns the number of kernels it launched -----------------------------------------------
-extern "C" {
-uint32_t vb_launch_pathtag(const VbConfig *, const uint32_t *, VbTagMonoid *, uint32_t *, uint32_t, cudaStream_t);
-uint32_t vb_pathtag_parts(uint32_t);
-uint32_t vb_launch_flatten(const VbConfig *, const uint32_t *, const VbTagMonoid *, VbPathBbox *, VbBump *, VbLineSoup *, void *, void *, uint32_t *,
-                       uint32_t *, uint32_t, int, uint32_t, uint32_t, int, cudaStream_t);
-uint32_t vb_flatten_parts(uint32_t);
-size_t vb_flatten_part_words(uint32_t);
-void vb_flatten_arena_bytes(uint32_t, size_t *, size_t *);
-uint32_t vb_launch_draw(const VbConfig *, const uint32_t *, const VbPathBbox *, VbDrawMonoid *, uint32_t *, VbClipInp *, uint32_t *, uint32_t,
-                    cudaStream_t);
-uint32_t vb_draw_parts(uint32_t);
-uint32_t vb_launch_clip(uint32_t, const VbClipInp *, const VbPathBbox *, VbDrawMonoid *, VbBbox4 *, int32_t *, uint32_t *, cudaStream_t);
-uint32_t vb_clip_parts(uint32_t);
-size_t vb_clip_scratch_words(uint32_t);
-uint32_t vb_launch_binning(const VbConfig *, const VbDrawMonoid *, const VbPathBbox *, const VbBbox4 *, VbBbox4 *, VbBump *, uint32_t *,
-                       VbBinHeader *, cudaStream_t);
-uint32_t vb_launch_tile_alloc(const VbConfig *, const uint32_t *, const VbBbox4 *, VbBump *, VbPath *, VbTile *, uint32_t *, uint32_t, int,
-                          cudaStream_t);
-uint32_t vb_tile_alloc_parts(uint32_t);
-uint32_t vb_launch_backdrop(const VbConfig *, VbBump *, const VbPath *, VbTile *, uint32_t *, uint32_t, cudaStream_t);
-uint32_t vb_backdrop_parts(uint32_t);
-uint32_t vb_launch_path_count(const VbConfig *, VbBump *, const VbLineSoup *, const VbPath *, VbTile *, VbSegmentCount *, uint32_t,
-                          cudaStream_t);
-uint32_t vb_launch_coarse(const VbConfig *, const uint32_t *, const VbDrawMonoid *, const VbBinHeader *, const uint32_t *, const VbPath *,
-                      const VbTile *, VbBump *, uint32_t *, uint32_t *, void *, uint32_t, cudaStream_t);
-uint32_t vb_launch_path_tiling(const VbConfig *, VbBump *, const VbSegmentCount *, const VbLineSoup *, const VbPath *, const VbTile *,
-                           VbSegment *, uint32_t, cudaStream_t);
-uint32_t vb_launch_fine(const VbConfig *, int, const VbBump *, const VbSegment *, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *,
-                    const uint32_t *, const uint8_t *, const uint32_t *, const uint32_t *, const uint32_t *, uint32_t, uint32_t *, const void *,
-                    const uint32_t *, uint32_t, int, cudaStream_t);
-}
-
-extern "C" int vb_fine_init_constants(void);
-// k_exchange.cu: flatten sharded by tag range, lines / path boxes exchanged through peer memory
-struct XPeersHost { // == XPeers in k_exchange.cu
-    unsigned char *base[8];
-    uint32_t rows[9];
-    uint32_t world, rank, n_paths, lines_cap;
-    unsigned long long half_bytes;
-};
-extern "C" size_t vb_exchange_half_bytes(uint32_t n_paths, uint32_t lines_cap);
-extern "C" size_t vb_exchange_peers_bytes(void);
-extern "C" uint32_t vb_exchange_epoch_word(void);
-extern "C" uint32_t vb_launch_exchange_send(const void *, VbBump *, uint32_t, VbLineSoup *, uint32_t *, VbPathBbox *, int, cudaStream_t);
-extern "C" uint32_t vb_launch_exchange_recv(const void *, VbBump *, uint32_t, VbLineSoup *, VbPathBbox *, int, cudaStream_t);
-extern "C" void vb_launch_resolve_finish(uint32_t *, uint32_t, uint32_t, uint32_t, uint32_t, const void *, uint32_t, cudaStream_t);
-extern "C" void vb_launch_make_ramps(const void *, const void *, uint32_t, uint32_t *, cudaStream_t);
-// k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch
-extern "C" uint32_t vb_atlas_blit_units_per_row(uint32_t w);
-extern "C" uint32_t vb_launch_atlas_blit(const VbBlitRect *, uint32_t, uint64_t, uint8_t *, uint32_t, cudaStream_t);
 
 // path_tiling_setup.wgsl:21-26 flags a failed frame to fine through ptcl[0] = ~0. That word is also tile 0's blend offset
 // and is only rewritten when coarse visits tile 0 -- which a stripe window with bin_row0 > 0 never does, so the flag of a
@@ -150,15 +100,17 @@ struct Dest {
     uint32_t bands = 1;
 };
 
-// key of a captured frame: everything a launch argument is derived from (see enqueue)
+// key of a captured frame: the inputs of its launches (see enqueue)
 struct GraphKey {
     VbConfig cfg;
-    const void *ptrs[32];
-    uint64_t ctl_words;
+    VbFrameBufs bufs;
+    const void *out;
+    const VbBump *h_bump_dev;
     uint32_t aa, cull, last;
-    uint32_t xen, xrows[9];
-    const void *xpeer[8];
+    const void *xarena; // exchange: the arena holding the epoch counter, and the peer table; zero while it is off
+    XPeers xpeers;
 };
+static_assert(sizeof(VbFrameBufs) == offsetof(VbFrameBufs, sm_count) + sizeof(int), "VbFrameBufs has no padding (GraphKey is compared bytewise)");
 struct GraphSlot {
     GraphKey key;
     cudaGraphExec_t exec = nullptr;
@@ -229,14 +181,12 @@ struct vb_renderer {
     vb_params params{};
     Dest dest; // of the frame frame_prepare set up
     uint32_t retries = 0, launches = 0;
-    size_t ctl_words = 0;
+    VbFrameBufs bufs{};           // the buffers of the frame prepare set up, as the launchers take them
     bool use_graph = true;        // replay whole frames as CUDA graphs (see enqueue)
     GraphSlot graphs[4];
     uint32_t graph_next = 0;
     uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
     uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
-    uint32_t parts_pathtag = 0, parts_flatten = 0, parts_draw = 0, parts_tile = 0, parts_backdrop = 0;
-    size_t off_lb_pathtag = 0, off_lb_flatten = 0, off_lb_draw = 0, off_lb_tile = 0, off_lb_clip = 0, off_lb_backdrop = 0;
     // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct)
     cudaStream_t tiling_stream = nullptr;
     cudaEvent_t tiling_fork = nullptr, tiling_join = nullptr;
@@ -275,18 +225,15 @@ struct vb_renderer {
     } xc;
 };
 
-// Every device buffer the renderer owns, each once. `keyed` marks what the launches of a frame read: the current scene slot's
-// inputs and the intermediates, whose addresses are part of a captured frame's key (graph_key). The frame's destination is
-// keyed by itself; the parked scene slot, the targets, resolve_tmp and the exchange arena are not launch arguments.
+// Every device buffer the renderer owns, each once: what vb_renderer_free frees and vb_frame_stats::arena_bytes counts.
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
-    vb_renderer::SceneSlot &s = *r->cur, &o = r->slot[r->cur == r->slot ? 1 : 0];
-    DevBuf *const keyed[] = {&s.scene, &s.ramps, &s.atlas, &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids,
-                             &r->info_bin_data, &r->clip_inp, &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers,
-                             &r->paths, &r->ctl, &r->tile_start, &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs,
-                             &r->flatten_parts, &r->tiles, &r->seg_counts, &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw};
-    DevBuf *const unkeyed[] = {&o.scene, &o.ramps, &o.atlas, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena};
-    for (DevBuf *b : keyed) f(*b, true);
-    for (DevBuf *b : unkeyed) f(*b, false);
+    DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
+                           &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids, &r->info_bin_data, &r->clip_inp,
+                           &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
+                           &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
+                           &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
+                           &r->blit_rects, &r->xc.arena};
+    for (DevBuf *b : all) f(*b);
 }
 
 #define CK(call)                                                                                  \
@@ -477,7 +424,7 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
     if (!r) return;
     cudaSetDevice(r->device);
     if (r->stream) cudaStreamSynchronize(r->stream);
-    for_each_buf(r, [](DevBuf &b, bool) {
+    for_each_buf(r, [](DevBuf &b) {
         if (b.p) cudaFree(b.p);
     });
     for (auto &s : r->slot)
@@ -670,27 +617,65 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         size[a] = std::min(r->cap[a], r->limit[a]);
     }
 
-    // control block: [bump (8 words, padded to 16)] [look-back states]
-    r->parts_pathtag = vb_pathtag_parts(c.n_tag_words);
-    r->parts_flatten = vb_flatten_parts(c.n_tag_words);
-    r->parts_draw = vb_draw_parts(n_draw);
-    r->parts_tile = vb_tile_alloc_parts(n_draw);
-    r->parts_backdrop = vb_backdrop_parts(c.tiles_size); // follows the tile arena: set above, regrown on retry
+    // control block: [bump (8 words, padded to 16), header words] [look-back states]
+    VbFrameBufs &b = r->bufs;
+    memset(&b, 0, sizeof b);
+    b.parts_pathtag = vb_pathtag_parts(c.n_tag_words);
+    b.parts_flatten = vb_flatten_parts(c.n_tag_words);
+    b.parts_draw = vb_draw_parts(n_draw);
+    b.parts_tile = vb_tile_alloc_parts(n_draw);
+    b.parts_backdrop = vb_backdrop_parts(c.tiles_size); // follows the tile arena: set above, regrown on retry
     size_t off = VB_CTL_HEADER_WORDS;
-    r->off_lb_pathtag = off; off += vb_lookback_words(r->parts_pathtag, 5);
-    r->off_lb_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
-    off += 4 + vb_lookback_words((r->parts_flatten + 8191u) / 8192u, 1);
-    r->off_lb_draw = off; off += vb_lookback_words(r->parts_draw, 4);
-    r->off_lb_tile = off; off += vb_lookback_words(r->parts_tile, 1);
-    r->off_lb_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
-    r->off_lb_backdrop = off; off += vb_lookback_words(r->parts_backdrop, 3);
-    r->ctl_words = off;
+    const size_t o_pathtag = off; off += vb_lookback_words(b.parts_pathtag, 5);
+    const size_t o_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
+    off += 4 + vb_lookback_words((b.parts_flatten + 8191u) / 8192u, 1);
+    const size_t o_draw = off; off += vb_lookback_words(b.parts_draw, 4);
+    const size_t o_tile = off; off += vb_lookback_words(b.parts_tile, 1);
+    const size_t o_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
+    const size_t o_backdrop = off; off += vb_lookback_words(b.parts_backdrop, 3);
+    b.ctl_words = off;
     if ((rc = ensure(r, r->ctl, off * 4))) return rc;
-    if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(r->parts_flatten) * 4))) return rc;
+    if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(b.parts_flatten) * 4))) return rc;
+
+    // every buffer has its size: the launchers' view of them
+    b.scene = (const uint32_t *)r->cur->scene.p;
+    b.ramps = (const uint32_t *)r->cur->ramps.p;
+    b.atlas = (const uint8_t *)r->cur->atlas.p;
+    b.mask8 = (const uint32_t *)r->mask8.p;
+    b.mask16 = (const uint32_t *)r->mask16.p;
+    b.tag_monoids = (VbTagMonoid *)r->tag_monoids.p;
+    b.path_bboxes = (VbPathBbox *)r->path_bboxes.p;
+    b.draw_monoids = (VbDrawMonoid *)r->draw_monoids.p;
+    b.info_bin_data = (uint32_t *)r->info_bin_data.p;
+    b.clip_inp = (VbClipInp *)r->clip_inp.p;
+    b.clip_bboxes = (VbBbox4 *)r->clip_bboxes.p;
+    b.clip_scratch = (int32_t *)r->clip_scratch.p;
+    b.draw_bboxes = (VbBbox4 *)r->draw_bboxes.p;
+    b.bin_headers = (VbBinHeader *)r->bin_headers.p;
+    b.paths = (VbPath *)r->paths.p;
+    b.tile_start = (uint32_t *)r->tile_start.p;
+    b.cls_list = (uint2 *)r->cls_list.p;
+    b.lines = (VbLineSoup *)r->lines.p;
+    b.line_scratch = (FlLit *)r->line_scratch.p;
+    b.flatten_jobs = (FlJob *)r->flatten_jobs.p;
+    b.flatten_parts = (uint32_t *)r->flatten_parts.p;
+    b.tiles = (VbTile *)r->tiles.p;
+    b.seg_counts = (VbSegmentCount *)r->seg_counts.p;
+    b.segments = (VbSegment *)r->segments.p;
+    b.ptcl = (uint32_t *)r->ptcl.p;
+    b.blend_spill = (uint32_t *)r->blend_spill.p;
+    b.ctl = (uint32_t *)r->ctl.p;
+    b.lb_pathtag = b.ctl + o_pathtag;
+    b.lb_flatten = b.ctl + o_flatten;
+    b.lb_draw = b.ctl + o_draw;
+    b.lb_tile = b.ctl + o_tile;
+    b.lb_clip = b.ctl + o_clip;
+    b.lb_backdrop = b.ctl + o_backdrop;
+    b.sm_count = r->sm_count;
     return VB_OK;
 }
 
-static void xpeers_of(const vb_renderer *r, XPeersHost *X) {
+static void xpeers_of(const vb_renderer *r, XPeers *X) {
     memset(X, 0, sizeof *X);
     for (uint32_t i = 0; i < r->xc.world; i++) X->base[i] = (unsigned char *)r->xc.peer[i];
     for (uint32_t i = 0; i <= r->xc.world; i++) X->rows[i] = r->xc.rows[i];
@@ -701,17 +686,38 @@ static void rec(vb_renderer *r, int i) {
     if (r->timing) cudaEventRecord(r->ev[i], r->stream);
 }
 
-// path_count and path_tiling: the grid comes from the arena capacity, the kernels stride over the count read on the device
-static uint32_t capacity_grid(uint32_t cap, int sm_count) {
-    const uint64_t blocks = ((uint64_t)cap + 255) / 256;
-    return (uint32_t)std::min<uint64_t>(blocks, (uint64_t)sm_count * 16);
+// The rows fine paints: the window's tile rows, launched in `bands` row bands when the pixels also go to the host (up to 8,
+// for at least 64 rows), so that the read-back of band k overlaps the rasterisation of band k+1. A batch paints every tile
+// row of its tall frame in one launch: its cells are not rows of one image, and its pixel rows are n_cells * height.
+struct FineRows {
+    uint32_t ty0, ty1, bands; // tile rows [ty0, ty1) in `bands` launches
+    size_t y1;                // the last pixel row they cover (+1); rows from ty0 * 16
+    size_t dest_rows;         // pixel rows the destination holds, from row out_row0
+    // tile rows [*by0, *by1) of band b; false once the bands have run out of rows
+    bool band(uint32_t b, uint32_t *by0, uint32_t *by1) const {
+        const uint32_t n = (ty1 - ty0 + bands - 1u) / bands;
+        *by0 = ty0 + b * n;
+        *by1 = *by0 + n < ty1 ? *by0 + n : ty1;
+        return *by0 < *by1;
+    }
+};
+static FineRows fine_rows(const VbConfig &c, const Dest &d) {
+    const bool batch = c.n_cells > 1u;
+    FineRows f;
+    f.ty0 = batch ? 0u : c.win_ty0;
+    f.ty1 = batch ? c.tile_rows : c.win_ty1;
+    const uint32_t rows = f.ty1 - f.ty0;
+    f.bands = d.host && rows >= 64u && !batch ? d.bands : 1u;
+    f.y1 = std::min((size_t)f.ty1 * 16u, (size_t)c.n_cells * c.target_height);
+    f.dest_rows = batch ? (size_t)c.n_cells * c.target_height : (size_t)rows * 16u;
+    return f;
 }
 
-// Queue the copy of tile rows ty0..ty1 of the frame to d.host on the copy stream, behind everything on the renderer's stream.
-static int queue_readback(vb_renderer *r, const VbConfig &c, uint32_t ty0, uint32_t ty1, const Dest &d, uint32_t band) {
-    size_t y0 = (size_t)ty0 * 16u, y1 = (size_t)ty1 * 16u;
-    if (y1 > c.target_height) y1 = c.target_height;
-    if (c.n_cells > 1u) y0 = 0, y1 = (size_t)c.n_cells * c.target_height; // a batch: all its frames, back to back
+// Queue the copy of band `band`'s pixel rows to d.host on the copy stream, behind everything on the renderer's stream.
+static int queue_readback(vb_renderer *r, const VbConfig &c, const FineRows &f, uint32_t band, const Dest &d) {
+    uint32_t ty0, ty1;
+    f.band(band, &ty0, &ty1);
+    const size_t y0 = (size_t)ty0 * 16u, y1 = std::min((size_t)ty1 * 16u, f.y1);
     if (y1 <= y0) return VB_OK;
     const size_t off = (y0 - c.out_row0) * c.out_pitch_px * 4u, bytes = (y1 - y0) * c.out_pitch_px * 4u;
     CK(cudaEventRecord(r->band_ev[band], r->stream));
@@ -725,28 +731,26 @@ static int queue_readback(vb_renderer *r, const VbConfig &c, uint32_t ty0, uint3
 // empty class lists.
 static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bool clear_queues) {
     const VbConfig &c = r->cfg;
+    const VbFrameBufs &b = r->bufs;
     cudaStream_t st = r->stream;
-    uint32_t *ctl = (uint32_t *)r->ctl.p;
-    VbBump *bump = (VbBump *)ctl;
     uint32_t launches = 0;
     int rc;
-    XPeersHost X; // multi-GPU exchange
+    XPeers X; // multi-GPU exchange
     if (r->xc.enabled) xpeers_of(r, &X);
     if (first == 0) {
         // a kernel, not cudaMemsetAsync: small memsets / copies are served by a copy engine and would queue behind a
         // 64 MiB read-back still draining from the previous frame
-        const unsigned ctl_blocks = (unsigned)((r->ctl_words + 1023) / 1024), bb_blocks = (c.layout.n_paths + 255u) / 256u;
+        const unsigned ctl_blocks = (unsigned)((b.ctl_words + 1023) / 1024), bb_blocks = (c.layout.n_paths + 255u) / 256u;
         uint32_t *xepoch = r->xc.enabled ? (uint32_t *)r->xc.arena.p + vb_exchange_epoch_word() : nullptr;
-        k_frame_init<<<ctl_blocks + bb_blocks, 256, 0, st>>>(ctl, (uint32_t)r->ctl_words, ctl_blocks, (VbPathBbox *)r->path_bboxes.p, c.layout.n_paths,
-                                                             xepoch);
+        k_frame_init<<<ctl_blocks + bb_blocks, 256, 0, st>>>(b.ctl, (uint32_t)b.ctl_words, ctl_blocks, b.path_bboxes, c.layout.n_paths, xepoch);
         launches++;
     }
     else if (clear_queues) {
-        if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(ctl + VB_CTL_FINE_QUEUE, 0, 8 * sizeof(uint32_t), st));
+        if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_QUEUE, 0, 8 * sizeof(uint32_t), st));
         if (first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_COARSE)
-            CK(cudaMemsetAsync(ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_CLASSES * sizeof(uint32_t), st));
+            CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_CLASSES * sizeof(uint32_t), st));
         if (first <= VB_STAGE_ID_BACKDROP && last >= VB_STAGE_ID_BACKDROP)
-            CK(cudaMemsetAsync(ctl + r->off_lb_backdrop, 0, VB_LB_ZERO_WORDS(r->parts_backdrop) * sizeof(uint32_t), st));
+            CK(cudaMemsetAsync(b.lb_backdrop, 0, VB_LB_ZERO_WORDS(b.parts_backdrop) * sizeof(uint32_t), st));
     }
     // path_tiling and coarse both depend on backdrop only (it assigns the segment slices): path_tiling is forked onto the
     // tiling stream and joined again before the next stage, so the two kernels share the GPU. Launch counts are unchanged;
@@ -755,100 +759,56 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
     rec(r, 0);
     for (int s = first; s <= last; s++) {
         switch (s) {
-        case VB_STAGE_ID_PATHTAG:
-            launches += vb_launch_pathtag(&c, (const uint32_t *)r->cur->scene.p, (VbTagMonoid *)r->tag_monoids.p, ctl + r->off_lb_pathtag,
-                                          r->parts_pathtag, st);
-            break;
+        case VB_STAGE_ID_PATHTAG: launches += vb_launch_pathtag(c, b, st); break;
         case VB_STAGE_ID_FLATTEN: {
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
             VbConfig cf = c;
-            uint32_t p0 = 0u, p1 = r->parts_flatten;
+            uint32_t p0 = 0u, p1 = b.parts_flatten;
             if (r->xc.enabled) {
                 cf.win_cull = 0u;
-                const uint32_t P = r->parts_flatten, G = r->xc.world, k = r->xc.rank;
+                const uint32_t P = b.parts_flatten, G = r->xc.world, k = r->xc.rank;
                 p0 = (uint32_t)((uint64_t)P * k / G) & ~7u;
                 p1 = k + 1u == G ? P : ((uint32_t)((uint64_t)P * (k + 1u) / G) & ~7u);
             }
-            launches += vb_launch_flatten(&cf, (const uint32_t *)r->cur->scene.p, (const VbTagMonoid *)r->tag_monoids.p, (VbPathBbox *)r->path_bboxes.p,
-                                          bump, (VbLineSoup *)r->lines.p, r->line_scratch.p, r->flatten_jobs.p, (uint32_t *)r->flatten_parts.p,
-                                          ctl + r->off_lb_flatten, r->parts_flatten, first != 0 ? 1 : 0, p0, p1, r->sm_count, st);
-            if (r->xc.enabled)
-                launches += vb_launch_exchange_send(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, ctl + VB_CTL_XCHG_SCRATCH,
-                                                    (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
+            launches += vb_launch_flatten(cf, b, first != 0, p0, p1, st);
+            if (r->xc.enabled) launches += vb_launch_exchange_send(c, b, X, st);
             break;
         }
         case VB_STAGE_ID_DRAW:
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
-                launches += vb_launch_exchange_recv(&X, bump, c.lines_size, (VbLineSoup *)r->lines.p, (VbPathBbox *)r->path_bboxes.p, r->sm_count, st);
-            launches += vb_launch_draw(&c, (const uint32_t *)r->cur->scene.p, (const VbPathBbox *)r->path_bboxes.p, (VbDrawMonoid *)r->draw_monoids.p,
-                                       (uint32_t *)r->info_bin_data.p, (VbClipInp *)r->clip_inp.p, ctl + r->off_lb_draw, r->parts_draw, st);
+                launches += vb_launch_exchange_recv(c, b, X, st);
+            launches += vb_launch_draw(c, b, st);
             break;
-        case VB_STAGE_ID_CLIP:
-            launches += vb_launch_clip(c.layout.n_clips, (const VbClipInp *)r->clip_inp.p, (const VbPathBbox *)r->path_bboxes.p,
-                                       (VbDrawMonoid *)r->draw_monoids.p, (VbBbox4 *)r->clip_bboxes.p, (int32_t *)r->clip_scratch.p,
-                                       ctl + r->off_lb_clip, st);
-            break;
-        case VB_STAGE_ID_BINNING:
-            launches += vb_launch_binning(&c, (const VbDrawMonoid *)r->draw_monoids.p, (const VbPathBbox *)r->path_bboxes.p,
-                                          (const VbBbox4 *)r->clip_bboxes.p, (VbBbox4 *)r->draw_bboxes.p, bump, (uint32_t *)r->info_bin_data.p,
-                                          (VbBinHeader *)r->bin_headers.p, st);
-            break;
-        case VB_STAGE_ID_TILE_ALLOC:
-            launches += vb_launch_tile_alloc(&c, (const uint32_t *)r->cur->scene.p, (const VbBbox4 *)r->draw_bboxes.p, bump, (VbPath *)r->paths.p,
-                                             (VbTile *)r->tiles.p, ctl + r->off_lb_tile, r->parts_tile, r->sm_count, st);
-            break;
-        case VB_STAGE_ID_PATH_COUNT:
-            launches += vb_launch_path_count(&c, bump, (const VbLineSoup *)r->lines.p, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p,
-                                             (VbSegmentCount *)r->seg_counts.p, capacity_grid(c.lines_size, r->sm_count), st);
-            break;
-        case VB_STAGE_ID_BACKDROP:
-            launches += vb_launch_backdrop(&c, bump, (const VbPath *)r->paths.p, (VbTile *)r->tiles.p, ctl + r->off_lb_backdrop, r->parts_backdrop, st);
-            break;
+        case VB_STAGE_ID_CLIP: launches += vb_launch_clip(c, b, st); break;
+        case VB_STAGE_ID_BINNING: launches += vb_launch_binning(c, b, st); break;
+        case VB_STAGE_ID_TILE_ALLOC: launches += vb_launch_tile_alloc(c, b, st); break;
+        case VB_STAGE_ID_PATH_COUNT: launches += vb_launch_path_count(c, b, st); break;
+        case VB_STAGE_ID_BACKDROP: launches += vb_launch_backdrop(c, b, st); break;
         case VB_STAGE_ID_COARSE:
             // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before
             // path_tiling's grid fills the rest of the GPU
             if (fork_tiling) CK(cudaEventRecord(r->tiling_fork, st));
-            launches += vb_launch_coarse(&c, (const uint32_t *)r->cur->scene.p, (const VbDrawMonoid *)r->draw_monoids.p,
-                                         (const VbBinHeader *)r->bin_headers.p, (const uint32_t *)r->info_bin_data.p, (const VbPath *)r->paths.p,
-                                         (const VbTile *)r->tiles.p, bump, (uint32_t *)r->ptcl.p, (uint32_t *)r->tile_start.p, r->cls_list.p,
-                                         c.width_in_tiles * c.tile_rows, st);
+            launches += vb_launch_coarse(c, b, st);
             if (fork_tiling) {
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->tiling_fork, 0));
-                launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
-                                                  (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p,
-                                                  capacity_grid(c.seg_counts_size, r->sm_count), r->tiling_stream);
+                launches += vb_launch_path_tiling(c, b, r->tiling_stream);
                 CK(cudaEventRecord(r->tiling_join, r->tiling_stream));
                 CK(cudaStreamWaitEvent(st, r->tiling_join, 0));
             }
             break;
         case VB_STAGE_ID_PATH_TILING:
-            if (fork_tiling) break; // launched beside coarse
-            launches += vb_launch_path_tiling(&c, bump, (const VbSegmentCount *)r->seg_counts.p, (const VbLineSoup *)r->lines.p,
-                                              (const VbPath *)r->paths.p, (const VbTile *)r->tiles.p, (VbSegment *)r->segments.p,
-                                              capacity_grid(c.seg_counts_size, r->sm_count), st);
+            if (!fork_tiling) launches += vb_launch_path_tiling(c, b, st); // else launched beside coarse
             break;
         case VB_STAGE_ID_FINE: {
-            // With a host destination (vb_render) fine is launched in up to 8 bands of tile rows and each band's
-            // device->host copy is queued on a second stream behind an event, so the read-back of band k overlaps
-            // the rasterisation of band k+1 (only the last band's copy is exposed).
-            // A batch paints every tile row of the tall frame in one launch (its cells are not rows of one image).
-            const uint32_t ty0 = c.n_cells > 1u ? 0u : c.win_ty0, ty1 = c.n_cells > 1u ? c.tile_rows : c.win_ty1;
-            const uint32_t rows = ty1 - ty0;
-            uint32_t n_bands = (d.host && rows >= 64u && c.n_cells == 1u) ? d.bands : 1u;
-            const uint32_t band_rows = (rows + n_bands - 1u) / n_bands;
-            for (uint32_t b = 0; b < n_bands; b++) {
+            // with a host destination, each band's device->host copy is queued on the copy stream behind an event (only
+            // the last band's copy is exposed)
+            const FineRows f = fine_rows(c, d);
+            for (uint32_t band = 0; band < f.bands; band++) {
                 VbConfig cb = c;
-                cb.win_ty0 = ty0 + b * band_rows;
-                cb.win_ty1 = cb.win_ty0 + band_rows < ty1 ? cb.win_ty0 + band_rows : ty1;
-                if (cb.win_ty0 >= cb.win_ty1) break;
-                launches += vb_launch_fine(&cb, (int)r->params.aa, bump, (const VbSegment *)r->segments.p, (const uint32_t *)r->ptcl.p,
-                                           (const uint32_t *)r->info_bin_data.p, (uint32_t *)r->blend_spill.p, (uint32_t *)d.dev,
-                                           (const uint32_t *)r->cur->ramps.p, (const uint8_t *)r->cur->atlas.p, (const uint32_t *)r->mask8.p,
-                                           (const uint32_t *)r->mask16.p, (const uint32_t *)r->tile_start.p, r->occlusion_cull,
-                                           ctl + VB_CTL_FINE_QUEUE + b, r->cls_list.p, n_bands == 1u ? ctl + VB_CTL_FINE_CLASS : nullptr,
-                                           c.width_in_tiles * c.tile_rows, r->sm_count, st);
-                if (d.host && (rc = queue_readback(r, c, cb.win_ty0, cb.win_ty1, d, b))) return rc;
+                if (!f.band(band, &cb.win_ty0, &cb.win_ty1)) break;
+                launches += vb_launch_fine(cb, b, (uint32_t *)d.dev, (int)r->params.aa, r->occlusion_cull, band, f.bands == 1u, st);
+                if (d.host && (rc = queue_readback(r, c, f, band, d))) return rc;
             }
             break;
         }
@@ -856,7 +816,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         }
         rec(r, s + 1);
     }
-    k_publish_bump<<<1, 32, 0, st>>>(bump, r->cur->h_bump_dev); // zero-copy store to mapped host memory (no copy engine)
+    k_publish_bump<<<1, 32, 0, st>>>(b.bump(), r->cur->h_bump_dev); // zero-copy store to mapped host memory (no copy engine)
     launches++;
     CK(cudaGetLastError());
     r->launches = launches;
@@ -868,35 +828,29 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
 // 64 MiB read-back of the previous frame is streaming the other way that fetch queues behind it (tools/e2e_probe.py
 // shows every stage of a streamed frame starting late). In steady state
 // the launches of a frame are identical -- same kernels, grids, arena pointers, config -- so they are captured once into a
-// graph and replayed with ONE submission. The key is everything a launch argument is derived from; growing an arena or
-// changing the scene layout / frame size / window simply misses the cache and re-captures.
+// graph and replayed with ONE submission. The key is the inputs of the launches; growing an arena or changing the scene
+// layout / frame size / window simply misses the cache and re-captures.
 static void graph_key(vb_renderer *r, int last, const void *out_dev, GraphKey *k) {
     memset(k, 0, sizeof *k);
     k->cfg = r->cfg;
-    size_t n = 0;
-    for_each_buf(r, [&](DevBuf &b, bool keyed) {
-        if (keyed) k->ptrs[n++] = b.p;
-    });
-    k->ptrs[n++] = out_dev;
-    k->ptrs[n++] = r->cur->h_bump_dev;
-    k->ctl_words = r->ctl_words;
+    memcpy(&k->bufs, &r->bufs, sizeof k->bufs);
+    k->out = out_dev;
+    k->h_bump_dev = r->cur->h_bump_dev;
     k->aa = r->params.aa;
     k->cull = r->occlusion_cull;
     k->last = (uint32_t)last;
-    k->xen = r->xc.enabled ? 1u + r->xc.rank + (r->xc.world << 8) : 0u;
     if (r->xc.enabled) {
-        memcpy(k->xrows, r->xc.rows, sizeof k->xrows);
-        memcpy(k->xpeer, r->xc.peer, sizeof k->xpeer);
+        k->xarena = r->xc.arena.p;
+        xpeers_of(r, &k->xpeers);
     }
 }
 
 // Enqueue stages first..last: through a cached graph for whole frames, directly otherwise.
 static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clear_queues) {
-    const VbConfig &c = r->cfg;
     if (!r->use_graph || r->timing || first != 0 || last != VB_N_STAGE_IDS - 1) return enqueue_direct(r, first, last, d, clear_queues);
     // with a host destination split into bands, fine and its interleaved copies stay outside the graph
-    const uint32_t rows = c.win_ty1 - c.win_ty0;
-    const bool banded = d.host && rows >= 64u && d.bands > 1u && c.n_cells == 1u;
+    const FineRows f = fine_rows(r->cfg, d);
+    const bool banded = f.bands > 1u;
     const int g_last = banded ? VB_STAGE_ID_FINE - 1 : last;
     GraphKey key;
     graph_key(r, g_last, d.dev, &key);
@@ -932,7 +886,7 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
             slot->exec = nullptr;
             return direct();
         }
-        slot->key = key;
+        memcpy(&slot->key, &key, sizeof key); // with its (zeroed) padding: keys are compared bytewise
         slot->launches = r->launches;
     }
     if (cudaGraphLaunch(slot->exec, r->stream) != cudaSuccess) {
@@ -946,7 +900,7 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
         r->launches += slot->launches;
         return rc;
     }
-    if (d.host) return queue_readback(r, c, c.win_ty0, c.win_ty1, d, 0);
+    if (d.host) return queue_readback(r, r->cfg, f, 0, d);
     return VB_OK;
 }
 
@@ -954,10 +908,8 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
 static int pick_out(vb_renderer *r, Dest *d) {
     if (d->dev) return VB_OK;
     const VbConfig &c = r->cfg;
-    size_t rows = (size_t)(c.win_ty1 - c.win_ty0) * 16u;
-    if (c.n_cells > 1u) rows = (size_t)c.n_cells * c.target_height;
     DevBuf &t = d->alt ? r->target_alt : r->target;
-    int rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * rows);
+    int rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * fine_rows(c, *d).dest_rows);
     d->dev = t.p;
     return rc;
 }
@@ -1167,7 +1119,7 @@ static void fill_stats(vb_renderer *r, vb_frame_stats *s) {
     memcpy(s, r->cur->h_bump, sizeof(VbBump));
     s->retries = r->retries;
     s->kernel_launches = r->launches;
-    for_each_buf(r, [&](DevBuf &b, bool) { s->arena_bytes += b.cap; });
+    for_each_buf(r, [&](DevBuf &b) { s->arena_bytes += b.cap; });
     if (r->timing) {
         for (int i = 0; i < VB_N_STAGE_IDS; i++) cudaEventElapsedTime(&s->stage_ms[i], r->ev[i], r->ev[i + 1]);
         cudaEventElapsedTime(&s->total_ms, r->ev[0], r->ev[VB_N_STAGE_IDS]);
@@ -1595,7 +1547,8 @@ extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint6
     CK(cudaMalloc(&d, sizeof h));
     CK(cudaMemset(d, 0, sizeof h));
     VbConfig c = r->cfg;
-    if (c.n_cells > 1u) c.win_ty0 = 0u, c.win_ty1 = c.tile_rows; // a batch: every cell
+    const FineRows f = fine_rows(c, Dest{});
+    c.win_ty0 = f.ty0, c.win_ty1 = f.ty1;
     uint32_t n = c.width_in_tiles * (c.win_ty1 - c.win_ty0);
     if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(c, (const uint32_t *)r->ptcl.p,
                                                                 r->occlusion_cull ? (const uint32_t *)r->tile_start.p : nullptr, d);
@@ -2037,10 +1990,8 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (rc) return rc;
     CK(cudaSetDevice(r->device));
     cudaStream_t st = r->stream;
-    struct Patch { uint32_t word, value; };
-    struct Ramp { uint32_t first_stop, n_stops, premul, pad; };
-    std::vector<Patch> patches;
-    std::vector<Ramp> ramps;
+    std::vector<RsPatch> patches;
+    std::vector<RsRamp> ramps;
     std::vector<vb_ramp_stop> stops;
     std::vector<const vb_ramp_patch *> ramp_of;
     // layout: sizes only (resolve.rs:107-154)
@@ -2074,10 +2025,10 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
         }
         if (rid == ramp_of.size()) {
             ramp_of.push_back(&p);
-            ramps.push_back(Ramp{(uint32_t)stops.size(), p.n_stops, p.premul_interp ? 1u : 0u, 0u});
+            ramps.push_back(RsRamp{(uint32_t)stops.size(), p.n_stops, p.premul_interp ? 1u : 0u, 0u});
             stops.insert(stops.end(), p.stops, p.stops + p.n_stops);
         }
-        patches.push_back(Patch{L.draw_data_base + p.draw_data_offset, (rid << 2) | p.extend});
+        patches.push_back(RsPatch{L.draw_data_base + p.draw_data_offset, (rid << 2) | p.extend});
     }
     // late-bound images: shelf placement (ours; only the (x, y) written into the draw data matters to the pipeline)
     struct Placed { const uint8_t *key; uint32_t w, h, x, y; };
@@ -2101,7 +2052,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
         } else {
             px = hit->x; py = hit->y;
         }
-        patches.push_back(Patch{L.draw_data_base + im.draw_data_offset, (px << 16) | py});
+        patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (px << 16) | py});
     }
     const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
     // images with an override on this renderer come from device memory (one k_atlas_blit); a registered texture needs one
@@ -2137,18 +2088,19 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (e->n_transforms) CK(cudaMemcpyAsync(base + (size_t)L.transform_base * 4, e->transforms, (size_t)e->n_transforms * 24, cudaMemcpyHostToDevice, st));
     if (e->n_styles) CK(cudaMemcpyAsync(base + (size_t)L.style_base * 4, e->styles, (size_t)e->n_styles * 8, cudaMemcpyHostToDevice, st));
     // patches, ramp descriptors and stops in one staging buffer
-    const size_t pb = patches.size() * sizeof(Patch), rb = ramps.size() * sizeof(Ramp), sb = stops.size() * sizeof(vb_ramp_stop);
+    static_assert(sizeof(RsStop) == sizeof(vb_ramp_stop), "the stops are staged as the caller gave them");
+    const size_t pb = patches.size() * sizeof(RsPatch), rb = ramps.size() * sizeof(RsRamp), sb = stops.size() * sizeof(vb_ramp_stop);
     const size_t o_r = (pb + 15) & ~(size_t)15, o_s = (o_r + rb + 15) & ~(size_t)15;
     if ((rc = ensure(r, r->resolve_tmp, o_s + sb + 16))) return rc;
     char *tmp = (char *)r->resolve_tmp.p;
     if (pb) CK(cudaMemcpyAsync(tmp, patches.data(), pb, cudaMemcpyHostToDevice, st));
     if (rb) CK(cudaMemcpyAsync(tmp + o_r, ramps.data(), rb, cudaMemcpyHostToDevice, st));
     if (sb) CK(cudaMemcpyAsync(tmp + o_s, stops.data(), sb, cudaMemcpyHostToDevice, st));
-    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags, tmp,
-                             (uint32_t)patches.size(), st);
+    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags,
+                             (const RsPatch *)tmp, (uint32_t)patches.size(), st);
     r->cur->n_ramps = (uint32_t)ramps.size();
     if ((rc = ensure(r, r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4))) return rc;
-    vb_launch_make_ramps(tmp + o_r, tmp + o_s, r->cur->n_ramps, (uint32_t *)r->cur->ramps.p, st);
+    vb_launch_make_ramps((const RsRamp *)(tmp + o_r), (const RsStop *)(tmp + o_s), r->cur->n_ramps, (uint32_t *)r->cur->ramps.p, st);
     r->cur->atlas_w = atlas_w;
     r->cur->atlas_h = atlas_h;
     if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;

@@ -22,12 +22,7 @@
 #include <vector>
 
 #include "../../include/vello_b200_scene.h"
-
-// vb_api.cu: nonzero for a key vb_register_texture handed out (an address no host buffer has); the texture registry
-extern "C" int vb_texture_key(const void *key);
-extern "C" int vb_texture_register(vb_renderer *, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes,
-                                   const void **key_out);
-extern "C" int vb_texture_unregister(vb_renderer *, const void *key);
+#include "vb_textures.h"
 
 namespace {
 
