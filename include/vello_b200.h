@@ -154,7 +154,12 @@ int vb_run_stages(vb_renderer *, const vb_params *, int first, int last, void *o
  * "segments","ptcl","blend_spill","bump","config", and the guard regions of vb_debug_limit_arena ("<arena>.guard", empty
  * while the arena has no limit). Returns bytes available in *bytes; copies min(cap, bytes). */
 int vb_debug_download(vb_renderer *, const char *name, void *dst, size_t cap, size_t *bytes);
-/* Overwrite an intermediate buffer from the host ("lines" also sets bump.lines; "path_bboxes"). */
+/* Overwrite an intermediate buffer from the host: "lines" (also sets bump.lines), "tiles" (also sets bump.tile), "path_bboxes",
+ * "paths" (exactly layout.n_draw_objects records, else VB_E_INVALID). "lines" and "tiles" grow their arena when `bytes` exceeds
+ * it. Growing frees the arena without copying, and the control block, which holds the bump counters and backdrop's look-back
+ * state sized from the tile capacity, is only set up anew by a vb_run_stages range that starts at stage 0. So to run
+ * backdrop on uploaded tiles: upload them once (to grow the arena), run pathtag..path_count, upload "paths" and "tiles"
+ * again, then run backdrop alone. */
 int vb_debug_upload(vb_renderer *, const char *name, const void *src, size_t bytes);
 /* Test-only capacity limit of one bump arena, to drive the overflow / grow-and-re-run path at a chosen boundary. `arena`:
  * "lines", "binning", "tiles", "seg_counts", "segments", "blend" or "ptcl"; `limit` in the units of the matching
@@ -166,6 +171,21 @@ int vb_debug_upload(vb_renderer *, const char *name, const void *src, size_t byt
  * limit of 0, above the current allocation, or (ptcl) below the static area of the last frame's tiles. */
 int vb_debug_limit_arena(vb_renderer *, const char *arena, uint32_t limit);
 #define VB_GUARD_BYTE 0xA5
+/* Test-only: the decoupled look-back every scan kernel uses, run alone on the renderer's device over n_parts partitions of one
+ * warp each. Partitions take tickets in launch order; partition p waits delay_ns[p] (NULL: none; each at most
+ * VB_LOOKBACK_MAX_DELAY_NS) before it publishes agg[p], so that its successors publish aggregates only and later partitions
+ * combine whole windows of them. Writes every partition's exclusive prefix to excl[p]. agg and excl hold K words per
+ * partition, K by `op`: VB_LOOKBACK_SUM1 (a sum, K = 1), VB_LOOKBACK_SUM5 (a field-wise sum, K = 5), VB_LOOKBACK_BACKDROP
+ * (backdrop's segmented sum {crossings, row start seen, backdrop since it}, K = 3), VB_LOOKBACK_AFFINE (x -> a x + b mod
+ * 2^32 stored as {a - 1, b}, applied in partition order, K = 2). VB_E_INVALID for another op, n_parts outside
+ * 1..VB_LOOKBACK_MAX_PARTS or a longer delay. Synchronous. */
+int vb_debug_lookback(vb_renderer *, int op, uint32_t n_parts, const uint32_t *agg, const uint32_t *delay_ns, uint32_t *excl);
+#define VB_LOOKBACK_SUM1 0
+#define VB_LOOKBACK_SUM5 1
+#define VB_LOOKBACK_BACKDROP 2
+#define VB_LOOKBACK_AFFINE 3
+#define VB_LOOKBACK_MAX_PARTS 65536u
+#define VB_LOOKBACK_MAX_DELAY_NS 1000000u
 
 /* Traffic statistics of the last frame's `fine` (for the roofline): PTCL words its interpreters read,
  * segments referenced by CMD_FILL, number of CMD_FILL commands. */

@@ -73,7 +73,9 @@ int vbo_run(vbo_ctx *, int first_stage, int last_stage, uint8_t *out_rgba8);
 
 /* Intermediate buffers by name: "tag_monoids","path_bboxes","lines","draw_monoids","info_bin_data",
  * "clip_inp","clip_bboxes","draw_bboxes","bin_headers","paths","tiles","seg_counts","segments",
- * "ptcl","bump","config". Returns pointer + size in bytes (valid until the next vbo_run). */
+ * "ptcl","bump","config", and "tile_counts": one u32 per tile, its crossing count as path_count left it in
+ * `segment_count_or_ix` (coarse then overwrites that word; empty until path_count has run for the bound scene).
+ * Returns pointer + size in bytes (valid until the next vbo_run). */
 const void *vbo_buffer(vbo_ctx *, const char *name, size_t *bytes);
 
 /* Replace an intermediate buffer after vbo_bind (e.g. feed the CUDA path's line soup to the

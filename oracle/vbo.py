@@ -36,6 +36,7 @@ DTYPES = {
     "segments": np.dtype([("p0", "<f4", 2), ("p1", "<f4", 2), ("y_edge", "<f4"), ("pad", "<u4")]),
     "ptcl": np.dtype("<u4"),
     "blend_spill": np.dtype("<u4"),
+    "tile_counts": np.dtype("<u4"),
     "bump": np.dtype([("failed", "<u4"), ("binning", "<u4"), ("ptcl", "<u4"), ("tile", "<u4"),
                       ("seg_counts", "<u4"), ("segments", "<u4"), ("blend", "<u4"), ("lines", "<u4")]),
     "config": np.dtype("<u4"),

@@ -107,6 +107,7 @@ struct vbo_ctx {
     Bump bump;
     Vec tag_monoids, path_bboxes, lines, draw_monoids, info_bin_data, clip_inp, clip_bboxes, draw_bboxes,
         bin_headers, paths, tiles, seg_counts, segments, ptcl, blend_spill;
+    Vec tile_counts; /* each tile's crossing count as path_count left it (coarse later overwrites the tile's word) */
     int lines_overridden;
     int threads;
 };

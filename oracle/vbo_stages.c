@@ -1187,6 +1187,9 @@ static void stage_path_count(vbo_ctx *c) {
             last_z = z;
         }
     }
+    /* a copy of the counts for the tests: the CUDA backdrop turns them into slice starts, which coarse here overwrites */
+    uint32_t *counts = vec_resize(&c->tile_counts, c->bump.tile);
+    for (uint32_t t = 0; t < c->bump.tile; t++) counts[t] = tile[t].segment_count_or_ix;
 }
 
 /* ------------------------------------------------------------------------------------------
@@ -1525,6 +1528,7 @@ vbo_ctx *vbo_create(void) {
     vec_init(&c->segments, sizeof(Segment));
     vec_init(&c->ptcl, 4);
     vec_init(&c->blend_spill, 4);
+    vec_init(&c->tile_counts, 4);
     c->threads = 1;
     return c;
 }
@@ -1532,7 +1536,7 @@ void vbo_destroy(vbo_ctx *c) {
     if (!c) return;
     Vec *vs[] = {&c->tag_monoids, &c->path_bboxes, &c->lines, &c->draw_monoids, &c->info_bin_data, &c->clip_inp,
                  &c->clip_bboxes, &c->draw_bboxes, &c->bin_headers, &c->paths, &c->tiles, &c->seg_counts, &c->segments,
-                 &c->ptcl, &c->blend_spill};
+                 &c->ptcl, &c->blend_spill, &c->tile_counts};
     for (size_t i = 0; i < sizeof vs / sizeof vs[0]; i++) vec_free(vs[i]);
     free(c);
 }
@@ -1560,6 +1564,7 @@ int vbo_bind(vbo_ctx *c, const uint32_t *scene, size_t scene_words, const vbo_la
     c->win_ty0 = c->win_by0 * 16u;
     c->win_ty1 = c->win_by1 * 16u < c->cfg.height_in_tiles ? c->win_by1 * 16u : c->cfg.height_in_tiles;
     memset(&c->bump, 0, sizeof c->bump);
+    c->tile_counts.n = 0; /* no counts of this scene until its path_count runs */
     c->lines_overridden = 0;
     return 0;
 }
@@ -1601,7 +1606,7 @@ const void *vbo_buffer(vbo_ctx *c, const char *name, size_t *bytes) {
         {"draw_monoids", &c->draw_monoids}, {"info_bin_data", &c->info_bin_data}, {"clip_inp", &c->clip_inp},
         {"clip_bboxes", &c->clip_bboxes}, {"draw_bboxes", &c->draw_bboxes}, {"bin_headers", &c->bin_headers},
         {"paths", &c->paths}, {"tiles", &c->tiles}, {"seg_counts", &c->seg_counts}, {"segments", &c->segments},
-        {"ptcl", &c->ptcl}, {"blend_spill", &c->blend_spill}};
+        {"ptcl", &c->ptcl}, {"blend_spill", &c->blend_spill}, {"tile_counts", &c->tile_counts}};
     for (size_t i = 0; i < sizeof tab / sizeof tab[0]; i++)
         if (!strcmp(name, tab[i].n)) {
             *bytes = tab[i].v->n * tab[i].v->elem;

@@ -1,8 +1,9 @@
 """Helpers that compare the CUDA pipeline's buffers with the CPU oracle's.
 
-Deterministic buffers are compared byte for byte. Buffers whose absolute offsets depend on atomic
-allocation order in BOTH implementations' GPU design (bin_data chunks, seg_counts order, segment
-slices, dynamic PTCL chunks) are compared after canonicalisation: through the headers / per tile,
+Deterministic buffers are compared byte for byte. That includes every tile's segment slice start, which backdrop assigns
+in tile order (the oracle's coarse allocates slices in its own order, so the GPU's words are compared with the oracle's
+crossing counts instead). What depends on atomic order in the GPU design (bin_data chunks, seg_counts order, the order of
+segments inside a slice, dynamic PTCL chunks) is compared after canonicalisation: through the headers / per tile,
 following jumps, with per-slice segment multisets.
 """
 from __future__ import annotations
@@ -10,6 +11,8 @@ from __future__ import annotations
 import numpy as np
 
 from oracle.vbo import DTYPES
+
+from .backdrop_ref import slice_words
 
 CMD_SIZES = {1: 4, 3: 1, 5: 2, 6: 3, 7: 3, 8: 3, 9: 2, 10: 1, 11: 3, 13: 3}
 
@@ -152,9 +155,19 @@ def compare_all(r, o, layout, width, height, check_ptcl_tiles=None, before=None)
         assert g["info_bin_data"][:bds].tobytes() == c["info_bin_data"][:bds].tobytes(), "info differs"
     if "bin_headers" in g:
         assert bins_canonical(g["bin_headers"], g["info_bin_data"], bds) == bins_canonical(c["bin_headers"], c["info_bin_data"], bds)
-    # tiles: backdrop exact; the count/index word is ~seg_ix after coarse (allocation order) -> compare via PTCL
+    # tiles: backdrop exact, and every tile's word is ~(the first slot of its slice): the exclusive sum of the crossing counts
+    # path_count left in the tiles before it, in u32. The oracle's coarse overwrites its own words in allocation order, so the
+    # GPU's are compared with the oracle's counts. This pins every count too (a tile's count is the next word's start minus its
+    # own), also for the tiles coarse turns into no CMD_FILL, and bump.segments is their total.
     if "tiles" in g:
         assert np.array_equal(g["tiles"]["backdrop"], c["tiles"]["backdrop"]), "tile backdrops differ"
+        counts = o.buffer("tile_counts")
+        assert counts.shape == g["tiles"].shape, ("tile_counts: run the oracle's path_count on this scene", counts.shape, g["tiles"].shape)
+        want = slice_words(counts)
+        bad = np.nonzero(g["tiles"]["segment_count_or_ix"] != want)[0]
+        assert len(bad) == 0, f"{len(bad)} of {len(want)} tile slice words differ from the oracle's counts, first at tile {int(bad[0])}"
+        total = int(counts.astype(np.uint64).sum() & 0xFFFFFFFF)
+        assert int(gb["segments"]) == total, ("bump.segments is not the total of the crossing counts", int(gb["segments"]), total)
     # crossing worklist as a multiset of (line, i)
     if "seg_counts" in g:
         gs = np.stack([g["seg_counts"]["line_ix"], g["seg_counts"]["counts"] & 0xFFFF], 1)

@@ -108,19 +108,6 @@ __global__ void __launch_bounds__(256) k_tile_zero(VbConfig cfg, const VbBump *_
                                                    // accesses of 8 consecutive threads hit distinct banks
 #define BD_STAGE 256u
 
-// The look-back monoid: [0] crossings, [1] a row starts in the range (0 / 1), [2] backdrop deltas summed from the range's
-// last row start on (all of them without one). The last two form a segmented sum: associative, not commutative.
-struct BdSegOp {
-    static constexpr bool commutative = false;
-    template <int K> __device__ __forceinline__ static void combine(const uint32_t (&a)[K], const uint32_t (&b)[K], uint32_t (&r)[K]) {
-        static_assert(K == 3, "BdSegOp has three words");
-        const uint32_t c = a[0] + b[0], f = a[1] | b[1], s = b[1] ? b[2] : a[2] + b[2];
-        r[0] = c;
-        r[1] = f;
-        r[2] = s;
-    }
-};
-
 // The last path p < n whose first tile is <= t (paths[0].tiles is 0), by a warp-wide 32-ary search: ceil(log32 n) rounds
 // of one load per lane. Call from a whole warp.
 __device__ __forceinline__ uint32_t bd_find_path(const VbPath *__restrict__ paths, uint32_t n, uint32_t t) {

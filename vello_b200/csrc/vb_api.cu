@@ -1565,17 +1565,20 @@ extern "C" int vb_debug_upload(vb_renderer *r, const char *name, const void *src
     if (!r || !name || !src) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
-    if (!strcmp(name, ARENAS[ARENA_LINES].name)) {
-        uint32_t n = (uint32_t)(bytes / sizeof(VbLineSoup));
-        if (n > r->cap[ARENA_LINES]) {
-            r->cap[ARENA_LINES] = grow(n);
-            int rc = ensure_arena(r, ARENA_LINES);
+    // "lines" and "tiles": the arena's contents and its bump counter. Growing the arena frees it without copying, and the
+    // look-back state of backdrop is sized from the tile capacity when the next frame is prepared.
+    for (int a : {ARENA_LINES, ARENA_TILES}) {
+        if (strcmp(name, ARENAS[a].name)) continue;
+        const uint32_t n = (uint32_t)(bytes / ARENAS[a].elem_bytes);
+        if (n > r->cap[a]) {
+            r->cap[a] = grow(n);
+            int rc = ensure_arena(r, a);
             if (rc) return rc;
         }
-        CK(cudaMemcpy(r->lines.p, src, (size_t)n * sizeof(VbLineSoup), cudaMemcpyHostToDevice));
+        if (n) CK(cudaMemcpy((r->*ARENAS[a].buf).p, src, (size_t)n * ARENAS[a].elem_bytes, cudaMemcpyHostToDevice));
         VbBump *bump = (VbBump *)r->ctl.p;
-        CK(cudaMemcpy(&bump->lines, &n, 4, cudaMemcpyHostToDevice));
-        r->cur->h_bump->lines = n;
+        CK(cudaMemcpy(&(bump->*ARENAS[a].counter), &n, 4, cudaMemcpyHostToDevice));
+        r->cur->h_bump->*ARENAS[a].counter = n;
         return VB_OK;
     }
     if (!strcmp(name, "path_bboxes")) {
@@ -1583,7 +1586,51 @@ extern "C" int vb_debug_upload(vb_renderer *r, const char *name, const void *src
         CK(cudaMemcpy(r->path_bboxes.p, src, bytes, cudaMemcpyHostToDevice));
         return VB_OK;
     }
+    if (!strcmp(name, "paths")) { // backdrop searches exactly n_draw_objects of them
+        if (bytes != (size_t)r->cur->layout.n_draw_objects * sizeof(VbPath) || bytes > r->paths.cap) {
+            r->err = "vb_debug_upload: \"paths\" takes exactly one record per draw object, after a frame of the scene";
+            return VB_E_INVALID;
+        }
+        if (bytes) CK(cudaMemcpy(r->paths.p, src, bytes, cudaMemcpyHostToDevice));
+        return VB_OK;
+    }
     return VB_E_UNKNOWN_BUFFER;
+}
+
+extern "C" int vb_debug_lookback(vb_renderer *r, int op, uint32_t n_parts, const uint32_t *agg, const uint32_t *delay_ns, uint32_t *excl) {
+    if (!r) return VB_E_INVALID;
+    const uint32_t K = vb_debug_lookback_words(op);
+    if (!agg || !excl || K == 0u || n_parts == 0u || n_parts > VB_LOOKBACK_MAX_PARTS) {
+        r->err = "vb_debug_lookback: unknown op, no buffers, or n_parts outside 1..VB_LOOKBACK_MAX_PARTS";
+        return VB_E_INVALID;
+    }
+    for (uint32_t p = 0; delay_ns && p < n_parts; p++)
+        if (delay_ns[p] > VB_LOOKBACK_MAX_DELAY_NS) {
+            r->err = "vb_debug_lookback: a delay exceeds VB_LOOKBACK_MAX_DELAY_NS";
+            return VB_E_INVALID;
+        }
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream));
+    // one allocation: [look-back state][agg: n_parts * K][delays: n_parts][excl: n_parts * K]
+    const size_t lb_words = vb_lookback_words(n_parts, (int)K), vec = (size_t)n_parts * K;
+    DevBuf d;
+    int rc = ensure(r, d, (lb_words + 2 * vec + n_parts) * 4);
+    if (rc) return rc;
+    uint32_t *lb = (uint32_t *)d.p, *d_agg = lb + lb_words, *d_delay = d_agg + vec, *d_excl = d_delay + n_parts;
+    auto run = [&]() -> int {
+        CK(cudaMemsetAsync(lb, 0, lb_words * 4, r->stream));
+        CK(cudaMemcpyAsync(d_agg, agg, vec * 4, cudaMemcpyHostToDevice, r->stream));
+        if (delay_ns) CK(cudaMemcpyAsync(d_delay, delay_ns, (size_t)n_parts * 4, cudaMemcpyHostToDevice, r->stream));
+        else CK(cudaMemsetAsync(d_delay, 0, (size_t)n_parts * 4, r->stream));
+        vb_launch_debug_lookback(op, n_parts, lb, d_agg, d_delay, d_excl, r->stream);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(excl, d_excl, vec * 4, cudaMemcpyDeviceToHost, r->stream));
+        CK(cudaStreamSynchronize(r->stream));
+        return VB_OK;
+    };
+    rc = run();
+    cudaFree(d.p);
+    return rc;
 }
 
 

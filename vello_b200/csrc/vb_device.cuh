@@ -96,6 +96,19 @@ struct VbSumOp {
         for (int k = 0; k < K; k++) r[k] = a[k] + b[k];
     }
 };
+// backdrop's look-back monoid (k_backdrop): [0] crossings, [1] a row starts in the range (0 / 1), [2] backdrop deltas summed
+// from the range's last row start on (all of them without one). The last two form a segmented sum: associative, not
+// commutative.
+struct BdSegOp {
+    static constexpr bool commutative = false;
+    template <int K> __device__ __forceinline__ static void combine(const uint32_t (&a)[K], const uint32_t (&b)[K], uint32_t (&r)[K]) {
+        static_assert(K == 3, "BdSegOp has three words");
+        const uint32_t c = a[0] + b[0], f = a[1] | b[1], s = b[1] ? b[2] : a[2] + b[2];
+        r[0] = c;
+        r[1] = f;
+        r[2] = s;
+    }
+};
 // Warp reduction of a non-commutative monoid in which a HIGHER lane holds an EARLIER element: every lane ends with
 // v[31] (+) v[30] (+) ... (+) v[0]. After the step of width o, a lane holds its aligned block of 2o lanes.
 template <int K, class Op> __device__ __forceinline__ void vb_warp_reduce_rev(uint32_t (&v)[K]) {

@@ -112,6 +112,12 @@ void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_r
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)
 uint32_t vb_atlas_blit_units_per_row(uint32_t w);
 uint32_t vb_launch_atlas_blit(const VbBlitRect *rects, uint32_t n, uint64_t total_units, uint8_t *atlas, uint32_t atlas_w, cudaStream_t st);
+
+// k_debug_lookback.cu (test-only, vb_debug_lookback): the words per partition of look-back `op` (VB_LOOKBACK_*), 0 for an
+// unknown op; one launch of n_parts partitions over the zeroed look-back state lb_mem (vb_lookback_words(n_parts, K) words)
+uint32_t vb_debug_lookback_words(int op);
+uint32_t vb_launch_debug_lookback(int op, uint32_t n_parts, uint32_t *lb_mem, const uint32_t *agg, const uint32_t *delay_ns,
+                                  uint32_t *excl, cudaStream_t st);
 }
 
 #endif

@@ -97,6 +97,7 @@ def load_library() -> C.CDLL:
     lib.vb_debug_limit_arena.argtypes = [vp, C.c_char_p, C.c_uint32]
     lib.vb_set_occlusion_cull.argtypes = [vp, C.c_int]
     lib.vb_debug_fine_traffic.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    lib.vb_debug_lookback.argtypes = [vp, C.c_int, C.c_uint32, vp, vp, vp]
     lib.vb_last_frame_ms.restype = C.c_float
     lib.vb_last_frame_ms.argtypes = [vp]
     lib.vb_frame_alloc.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
@@ -135,7 +136,7 @@ def load_library() -> C.CDLL:
 
 EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_last_error", "vb_scene_upload",
                     "vb_render_resident", "vb_render_enqueue", "vb_frame_finish", "vb_render", "vb_target", "vb_copy_to_host", "vb_stream",
-                    "vb_run_stages", "vb_debug_download", "vb_debug_upload", "vb_debug_limit_arena", "vb_debug_fine_traffic", "vb_set_occlusion_cull", "vb_render_begin", "vb_readback_wait", "vb_set_readback_bands", "vb_set_cuda_graph", "vb_set_timing",
+                    "vb_run_stages", "vb_debug_download", "vb_debug_upload", "vb_debug_limit_arena", "vb_debug_fine_traffic", "vb_debug_lookback", "vb_set_occlusion_cull", "vb_render_begin", "vb_readback_wait", "vb_set_readback_bands", "vb_set_cuda_graph", "vb_set_timing",
                     "vb_scene_upload_streams", "vb_render_uploaded", "vb_last_frame_ms", "vb_frame_alloc", "vb_frame_free", "vb_ipc_export", "vb_ipc_open", "vb_ipc_close",
                     "vb_group_new", "vb_group_free", "vb_group_size", "vb_group_renderer", "vb_group_last_error", "vb_group_render",
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
@@ -429,6 +430,26 @@ class Renderer:
     def download_guard(self, name: str) -> np.ndarray:
         """The guard region past a limited arena's limit as bytes ("lines", ..., "ptcl", "line_scratch", "flatten_jobs")."""
         return self.download(f"{name}.guard", np.uint8)
+
+    # look-back monoids of debug_lookback (VB_LOOKBACK_*) and their words per partition
+    LOOKBACK_SUM1, LOOKBACK_SUM5, LOOKBACK_BACKDROP, LOOKBACK_AFFINE = 0, 1, 2, 3
+    LOOKBACK_WORDS = {0: 1, 1: 5, 2: 3, 3: 2}
+    LOOKBACK_MAX_DELAY_NS = 1_000_000
+
+    def debug_lookback(self, op: int, agg: np.ndarray, delay_ns=None) -> np.ndarray:
+        """Test-only: the device look-back alone (vb_debug_lookback) over len(agg) partitions, partition p waiting delay_ns[p]
+        before it publishes agg[p] ((n_parts, K) u32). Returns every partition's exclusive prefix, (n_parts, K) u32."""
+        a = np.ascontiguousarray(agg, dtype=np.uint32)
+        n = a.shape[0]
+        if a.shape != (n, self.LOOKBACK_WORDS[op]):
+            raise ValueError(f"debug_lookback: agg must be (n_parts, {self.LOOKBACK_WORDS[op]}), not {a.shape}")
+        d = None if delay_ns is None else np.ascontiguousarray(delay_ns, dtype=np.uint32)
+        if d is not None and d.shape != (n,):
+            raise ValueError("debug_lookback: one delay per partition")
+        out = np.zeros_like(a)
+        self._check(self.lib.vb_debug_lookback(self.handle, op, n, a.ctypes.data, None if d is None else d.ctypes.data, out.ctypes.data),
+                    "vb_debug_lookback")
+        return out
 
     def set_cuda_graph(self, on: bool):
         """Replay whole frames as CUDA graphs (default on)."""
