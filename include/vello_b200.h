@@ -152,7 +152,10 @@ int vb_run_stages(vb_renderer *, const vb_params *, int first, int last, void *o
 /* Copy an intermediate buffer to the host: "tag_monoids","path_bboxes","lines","draw_monoids",
  * "info_bin_data","clip_inp","clip_bboxes","draw_bboxes","bin_headers","paths","tiles","seg_counts",
  * "segments","ptcl","blend_spill","bump","config", and the guard regions of vb_debug_limit_arena ("<arena>.guard", empty
- * while the arena has no limit). Returns bytes available in *bytes; copies min(cap, bytes). */
+ * while the arena has no limit). Test-only, flatten's own state after the last attempt: "flatten_counters" (3 x u32:
+ * literal line records, deferred jobs, partitions on the general tag kernel's work list), "line_scratch" (32 B literal
+ * records) and "flatten_jobs" (96 B job records), each up to its counter and at most its capacity.
+ * Returns bytes available in *bytes; copies min(cap, bytes). */
 int vb_debug_download(vb_renderer *, const char *name, void *dst, size_t cap, size_t *bytes);
 /* Overwrite an intermediate buffer from the host: "lines" (also sets bump.lines), "tiles" (also sets bump.tile), "path_bboxes",
  * "paths" (exactly layout.n_draw_objects records, else VB_E_INVALID). "lines" and "tiles" grow their arena when `bytes` exceeds

@@ -1462,6 +1462,32 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
         if (dst && cap >= sizeof(VbConfig)) memcpy(dst, &r->cfg, sizeof(VbConfig));
         return VB_OK;
     }
+    // flatten's device counters of the last attempt (k_flatten.cu FlCtx::ctrs): literal records, jobs, and the length of
+    // the general tag kernel's work list; and its two scratch arenas up to their counters (at most their capacity)
+    const bool lits = !strcmp(name, "line_scratch"), jobs = !strcmp(name, "flatten_jobs");
+    if (!strcmp(name, "flatten_counters") || lits || jobs) {
+        uint32_t ctrs[3] = {0u, 0u, 0u};
+        if (r->bufs.lb_flatten) CK(cudaMemcpy(ctrs, r->bufs.lb_flatten, sizeof ctrs, cudaMemcpyDeviceToHost));
+        size_t n = sizeof ctrs;
+        const void *src = ctrs;
+        bool host = true;
+        if (lits || jobs) {
+            size_t lit1, job1, lit_cap, job_cap; // one record of each, and the capacities the kernels saw
+            vb_flatten_arena_bytes(1u, &lit1, &job1);
+            vb_flatten_arena_bytes(r->cfg.lines_size, &lit_cap, &job_cap);
+            const DevBuf &b = lits ? r->line_scratch : r->flatten_jobs;
+            n = std::min({(size_t)ctrs[lits ? 0 : 1] * (lits ? lit1 : job1), lits ? lit_cap : job_cap, b.cap});
+            src = b.p;
+            host = false;
+        }
+        if (bytes) *bytes = n;
+        const size_t c = n < cap ? n : cap;
+        if (dst && c) {
+            if (host) memcpy(dst, src, c);
+            else CK(cudaMemcpy(dst, src, c, cudaMemcpyDeviceToHost));
+        }
+        return VB_OK;
+    }
     for (auto &nb : named(r))
         if (!strcmp(name, nb.name)) {
             if (bytes) *bytes = nb.bytes;
