@@ -7,9 +7,11 @@
 // Design (differs from the WGSL on purpose; the pieces are described where they are defined below):
 //  * The WGSL bump-allocates every line with a global atomicAdd, so the line order is a race. Here line order is
 //    deterministic -- tag order, then emission order, i.e. the serial CPU shader's -- and independent of any atomic:
-//    the tag pass (thread per TAG: k_flatten_lean, then k_flatten for the partitions that need the general path) emits
-//    literal-line and job records plus per-warp counts, k_flatten_scan turns the counts into offsets, k_flatten_place
-//    (thread per LINE) writes every line at its final position.
+//    the tag pass (thread per TAG: k_flatten_lean, then k_flatten for the partitions that need the general path) counts
+//    every partition's lines and emits job records, and k_flatten also literal-line records; k_flatten_scan turns the
+//    counts into offsets; k_flatten_emit plans the lean partitions' tags again and writes their literal lines straight
+//    to their final positions; k_flatten_place (thread per LINE) places the general partitions' literal records and
+//    expands every job.
 //  * Fast paths for line-tos (filled: one line; stroked: one line per side) behind guards that are derived in place,
 //    property-tested on the CPU against the oracle and compared bit for bit on the GPU.
 //  * With a stripe window set (multi-GPU), tags that cannot reach the window's rows are skipped.
@@ -51,9 +53,11 @@ __device__ __forceinline__ fv2 fx_apply(const FXform &t, fv2 p) { // flatten.wgs
 //  * k_flatten (thread per tag) runs the control flow of the reference -- subdivision into Euler segments, caps,
 //    joins -- but does not evaluate long runs of lines itself: an Euler segment or arc of >= FL_DEFER_MIN lines
 //    becomes a 96 B FlJob record ("these n lines, at tag-relative offset rel"). Short output (the one line of a
-//    line-to, cap / join lines) is kept in a small shared-memory cache and leaves as 32 B FlLit records.
+//    line-to, cap / join lines) is kept in a small shared-memory cache and leaves as 32 B FlLit records. k_flatten_lean
+//    only counts the literal lines of its (lean) partitions.
 //  * k_flatten_scan turns per-warp line counts into final offsets (tag order == the serial CPU shader's order).
-//  * k_flatten_place (thread per LINE) scatters the literals and expands the jobs, 32 jobs per warp with a
+//  * k_flatten_emit re-plans the lean partitions and writes their literal lines at their final offsets.
+//  * k_flatten_place (thread per LINE) scatters k_flatten's literals and expands the jobs, 32 jobs per warp with a
 //    load-balanced lane <-> line mapping, so the cost of a frame no longer hangs on its slowest tag.
 // Every point is a pure function of (job, i); whoever evaluates it gets the same bits.
 #define FL_CACHE 6     // literal lines a thread keeps in shared memory
@@ -101,49 +105,67 @@ __device__ __noinline__ void fl_spill_line(const FlCtx c, uint32_t tag_ix, uint3
     }
 }
 
-// SPILL = false (k_flatten_lean): a tag never has more than FL_CACHE literal lines, so there is no overflow path.
-template <bool SPILL>
+// Where a tag's output goes (the sink policy of FlatT):
+//  * FL_SINK_RECORDS (k_flatten): literal lines into the shared-memory cache, spilling past it as records; the bbox of
+//    the literal lines; job records.
+//  * FL_SINK_COUNT (k_flatten_lean): the line count, the bbox of the literal lines and the job records; no literal line
+//    is stored.
+//  * FL_SINK_EMIT (k_flatten_emit): the literal lines only, staged in shared memory with their final positions; a job
+//    only advances the count past its lines.
+enum FlSink { FL_SINK_RECORDS, FL_SINK_COUNT, FL_SINK_EMIT };
+template <int SINK>
 struct FlatT {
+    static constexpr int kSink = SINK;
     FlCtx c;
     uint32_t tag_ix, path_ix, trans_ix;
     uint32_t ix;   // lines of this tag so far
     uint32_t nlit; // of which literal (cached or spilled)
+    uint32_t dst0; // FL_SINK_EMIT: final position of the tag's first line
     float bx0, by0, bx1, by1; // bbox of the literal lines
     bool force;    // a job was deferred: the tag's bbox is known to be non-degenerate
-    float4 *cache; // &cache[0][threadIdx.x], stride FL_THREADS
-    uint32_t *cache_rel;
+    float4 *cache; // RECORDS: &cache[0][threadIdx.x], stride FL_THREADS; EMIT: this lane's first staging slot, stride 1
+    uint32_t *cache_rel; // RECORDS: rel, same stride; EMIT: (final position, path_ix) pairs
     __device__ __forceinline__ void write_line(fv2 p0, fv2 p1) { // device-space end points
-        bx0 = fminf(bx0, fminf(p0.x, p1.x));
-        by0 = fminf(by0, fminf(p0.y, p1.y));
-        bx1 = fmaxf(bx1, fmaxf(p0.x, p1.x));
-        by1 = fmaxf(by1, fmaxf(p0.y, p1.y));
-        if (!SPILL || nlit < FL_CACHE) {
-            cache[nlit * FL_THREADS] = make_float4(p0.x, p0.y, p1.x, p1.y);
-            cache_rel[nlit * FL_THREADS] = ix;
-        } else {
-            fl_spill_line(c, tag_ix, ix, path_ix, p0, p1);
+        if (SINK != FL_SINK_EMIT) {
+            bx0 = fminf(bx0, fminf(p0.x, p1.x));
+            by0 = fminf(by0, fminf(p0.y, p1.y));
+            bx1 = fmaxf(bx1, fmaxf(p0.x, p1.x));
+            by1 = fmaxf(by1, fmaxf(p0.y, p1.y));
+        }
+        if (SINK == FL_SINK_RECORDS) {
+            if (nlit < FL_CACHE) {
+                cache[nlit * FL_THREADS] = make_float4(p0.x, p0.y, p1.x, p1.y);
+                cache_rel[nlit * FL_THREADS] = ix;
+            } else {
+                fl_spill_line(c, tag_ix, ix, path_ix, p0, p1);
+            }
+        } else if (SINK == FL_SINK_EMIT) {
+            cache[nlit] = make_float4(p0.x, p0.y, p1.x, p1.y);
+            reinterpret_cast<uint2 *>(cache_rel)[nlit] = make_uint2(dst0 + ix, path_ix);
         }
         nlit++;
         ix++;
     }
     __device__ __forceinline__ void line_xf(fv2 p0, fv2 p1, const FXform &t) { write_line(fx_apply(t, p0), fx_apply(t, p1)); }
     __device__ __forceinline__ void push_job(FlJob &j, uint32_t n_lines) {
-        j.tag_ix = tag_ix; j.rel = ix; j.path_ix = path_ix; j.trans_ix = trans_ix; j.pad = 0u;
-        const uint32_t slot = fl_alloc(c.ctrs + 1);
-        if (slot < c.jobs_cap) {
-            float4 *dst = reinterpret_cast<float4 *>(c.jobs + slot);
-            dst[0] = make_float4(j.p0x, j.p0y, j.p1x, j.p1y);
-            dst[1] = make_float4(j.th0, j.k0, j.k1, j.ch);
-            dst[2] = make_float4(j.noff, j.n, j.integral, j.int0);
-            dst[3] = make_float4(j.a, j.b, j.lp0x, j.lp0y);
-            dst[4] = make_float4(j.tex, j.tey, __uint_as_float(j.tag_ix), __uint_as_float(j.rel));
-            dst[5] = make_float4(__uint_as_float(j.path_ix), __uint_as_float(j.trans_ix), __uint_as_float(j.meta), 0.f);
+        if (SINK != FL_SINK_EMIT) {
+            j.tag_ix = tag_ix; j.rel = ix; j.path_ix = path_ix; j.trans_ix = trans_ix; j.pad = 0u;
+            const uint32_t slot = fl_alloc(c.ctrs + 1);
+            if (slot < c.jobs_cap) {
+                float4 *dst = reinterpret_cast<float4 *>(c.jobs + slot);
+                dst[0] = make_float4(j.p0x, j.p0y, j.p1x, j.p1y);
+                dst[1] = make_float4(j.th0, j.k0, j.k1, j.ch);
+                dst[2] = make_float4(j.noff, j.n, j.integral, j.int0);
+                dst[3] = make_float4(j.a, j.b, j.lp0x, j.lp0y);
+                dst[4] = make_float4(j.tex, j.tey, __uint_as_float(j.tag_ix), __uint_as_float(j.rel));
+                dst[5] = make_float4(__uint_as_float(j.path_ix), __uint_as_float(j.trans_ix), __uint_as_float(j.meta), 0.f);
+            }
+            force = true;
         }
         ix += n_lines;
-        force = true;
     }
 };
-using Flat = FlatT<true>;
+using Flat = FlatT<FL_SINK_RECORDS>;
 
 #define DERIV_THRESH 1e-6f
 #define DERIV_THRESH_SQUARED (DERIV_THRESH * DERIV_THRESH)
@@ -922,35 +944,35 @@ __global__ void k_bbox_clear(uint32_t n_paths, VbPathBbox *path_bboxes) {
 __device__ __forceinline__ int fl_floor_i(float v) { return v != v ? 0x7fffffff : vb_f2i_sat(floorf(v)); }
 __device__ __forceinline__ int fl_ceil_i(float v) { return v != v ? (int)0x80000000 : vb_f2i_sat(ceilf(v)); }
 
-// Per-partition prologue of both tag kernels: this lane's tag and style word, the draw flags / transform of the path it
-// opens; then an empty Flat over the block's shared-memory line cache.
+// Per-partition prologue of the tag kernels: this lane's tag and style word (fl_load_tag), the draw flags / transform of
+// the path it opens (fl_open_path, the counting kernels only); then an empty Flat over the block's shared-memory lines.
 __device__ __forceinline__ void fl_load_tag(PathTagData &tag, uint32_t &style_flags, const VbConfig &cfg, const uint32_t *__restrict__ scene,
-                                            const VbTagMonoid *__restrict__ tag_monoids, VbPathBbox *path_bboxes, uint32_t ix) {
-    const uint32_t n_tags = cfg.n_tag_words * 4u;
-    const uint32_t n_paths = cfg.layout.n_paths;
+                                            const VbTagMonoid *__restrict__ tag_monoids, uint32_t ix) {
     tag.tag_byte = 0; tag.trans_ix = 0; tag.pathseg_offset = 0; tag.style_ix = 0; tag.path_ix = 0;
     style_flags = 0;
-    if (ix < n_tags) {
+    if (ix < cfg.n_tag_words * 4u) {
         tag = compute_tag_monoid(cfg, scene, tag_monoids, ix);
         style_flags = vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix);
-        if ((tag.tag_byte & 0x10u) != 0u && tag.path_ix < n_paths) {
-            path_bboxes[tag.path_ix].draw_flags = (style_flags & STYLE_FLAGS_FILL) == 0u ? 0u : 1u;
-            path_bboxes[tag.path_ix].trans_ix = tag.trans_ix;
-        }
+    }
+}
+__device__ __forceinline__ void fl_open_path(const VbConfig &cfg, VbPathBbox *path_bboxes, const PathTagData &tag, uint32_t style_flags) {
+    if ((tag.tag_byte & 0x10u) != 0u && tag.path_ix < cfg.layout.n_paths) {
+        path_bboxes[tag.path_ix].draw_flags = (style_flags & STYLE_FLAGS_FILL) == 0u ? 0u : 1u;
+        path_bboxes[tag.path_ix].trans_ix = tag.trans_ix;
     }
 }
 template <class F>
 __device__ __forceinline__ void fl_flat_init(F &f, const FlCtx &ctx, const PathTagData &tag, uint32_t ix, float4 *cache, uint32_t *cache_rel) {
     f.c = ctx;
     f.tag_ix = ix; f.path_ix = tag.path_ix; f.trans_ix = tag.trans_ix;
-    f.ix = 0u; f.nlit = 0u; f.force = false;
+    f.ix = 0u; f.nlit = 0u; f.dst0 = 0u; f.force = false;
     f.bx0 = 1e31f; f.by0 = 1e31f; f.bx1 = -1e31f; f.by1 = -1e31f;
     f.cache = cache;
     f.cache_rel = cache_rel;
 }
 
-// Per-partition epilogue of both tag kernels: per-warp line count, per-tag offset inside its warp's block, the cached
-// literal records, and the bbox contribution of the literal lines.
+// Per-partition epilogue of both counting tag kernels: per-warp line count, per-tag offset inside its warp's block, the
+// cached literal records (k_flatten only), and the bbox contribution of the literal lines.
 template <class F>
 __device__ __forceinline__ void fl_tag_end(F &f, const VbConfig &cfg, VbPathBbox *path_bboxes, const FlCtx &ctx, uint32_t *part_count,
                                            uint32_t *tag_off) {
@@ -960,32 +982,34 @@ __device__ __forceinline__ void fl_tag_end(F &f, const VbConfig &cfg, VbPathBbox
     const uint32_t incl = vb_warp_incl_scan(f.ix);
     if (lane == 31u) part_count[part] = incl;
     tag_off[ix] = incl - f.ix;
-    const uint32_t ncache = min(f.nlit, (uint32_t)FL_CACHE);
-    const uint32_t lincl = vb_warp_incl_scan(ncache);
-    const uint32_t ltotal = __shfl_sync(VB_FULL, lincl, 31);
-    uint32_t lbase = 0u;
-    if (lane == 31u && ltotal != 0u) lbase = atomicAdd(ctx.ctrs, ltotal);
-    lbase = __shfl_sync(VB_FULL, lbase, 31);
-    // The warp's literal records are one range [lbase, lbase + ltotal), lane i's ncache records after lane i-1's. They are
-    // written lane-strided, record j of the range by lane j % 32 from its owner's cache, so that a warp's stores cover
-    // consecutive 32 B records (each lane writing its own records made every store a scatter of partial sectors).
-    const uint32_t lexcl = lincl - ncache;
-    const float4 *wcache = f.cache - lane;
-    const uint32_t *wrel = f.cache_rel - lane;
-    for (uint32_t b = 0u; b < ltotal; b += 32u) {
-        const uint32_t j = b + lane;
-        uint32_t o = 0u; // owner: the number of lanes whose records all lie before j
+    if constexpr (F::kSink == FL_SINK_RECORDS) {
+        const uint32_t ncache = min(f.nlit, (uint32_t)FL_CACHE);
+        const uint32_t lincl = vb_warp_incl_scan(ncache);
+        const uint32_t ltotal = __shfl_sync(VB_FULL, lincl, 31);
+        uint32_t lbase = 0u;
+        if (lane == 31u && ltotal != 0u) lbase = atomicAdd(ctx.ctrs, ltotal);
+        lbase = __shfl_sync(VB_FULL, lbase, 31);
+        // The warp's literal records are one range [lbase, lbase + ltotal), lane i's ncache records after lane i-1's. They are
+        // written lane-strided, record j of the range by lane j % 32 from its owner's cache, so that a warp's stores cover
+        // consecutive 32 B records (each lane writing its own records made every store a scatter of partial sectors).
+        const uint32_t lexcl = lincl - ncache;
+        const float4 *wcache = f.cache - lane;
+        const uint32_t *wrel = f.cache_rel - lane;
+        for (uint32_t b = 0u; b < ltotal; b += 32u) {
+            const uint32_t j = b + lane;
+            uint32_t o = 0u; // owner: the number of lanes whose records all lie before j
 #pragma unroll
-        for (uint32_t step = 16u; step > 0u; step >>= 1)
-            if (__shfl_sync(VB_FULL, lincl, o + step - 1u) <= j) o += step;
-        const uint32_t k = j - __shfl_sync(VB_FULL, lexcl, o);
-        const uint32_t o_path = __shfl_sync(VB_FULL, path_ix, o);
-        const uint32_t slot = lbase + j;
-        if (j < ltotal && slot < ctx.lits_cap) {
-            const float4 l = wcache[k * FL_THREADS + o];
-            uint4 *dst = reinterpret_cast<uint4 *>(ctx.lits + slot);
-            dst[0] = make_uint4(ix - lane + o, wrel[k * FL_THREADS + o], o_path, 0u);
-            dst[1] = make_uint4(__float_as_uint(l.x), __float_as_uint(l.y), __float_as_uint(l.z), __float_as_uint(l.w));
+            for (uint32_t step = 16u; step > 0u; step >>= 1)
+                if (__shfl_sync(VB_FULL, lincl, o + step - 1u) <= j) o += step;
+            const uint32_t k = j - __shfl_sync(VB_FULL, lexcl, o);
+            const uint32_t o_path = __shfl_sync(VB_FULL, path_ix, o);
+            const uint32_t slot = lbase + j;
+            if (j < ltotal && slot < ctx.lits_cap) {
+                const float4 l = wcache[k * FL_THREADS + o];
+                uint4 *dst = reinterpret_cast<uint4 *>(ctx.lits + slot);
+                dst[0] = make_uint4(ix - lane + o, wrel[k * FL_THREADS + o], o_path, 0u);
+                dst[1] = make_uint4(__float_as_uint(l.x), __float_as_uint(l.y), __float_as_uint(l.z), __float_as_uint(l.w));
+            }
         }
     }
     // bbox: consecutive tags mostly belong to the same path, so reduce across the lanes of a path first (floor / ceil
@@ -1014,16 +1038,37 @@ __device__ __forceinline__ void fl_tag_end(F &f, const VbConfig &cfg, VbPathBbox
 //  * k_flatten_lean runs every partition [part_base, part_end) -- all of them, or this GPU's share of a frame whose
 //    flatten is sharded by tag range (k_exchange.cu); every array is indexed by the GLOBAL partition / tag. A partition
 //    whose tags all take a line-to fast path or need no lines, and whose caps and joins are straight or round arcs that
-//    are deferred or have at most 2 lines, is finished here (at most 5 literal lines per tag -- 2 + 3 straight, or
-//    2 + 2 + 1 with an arc -- so all of them stay in the shared-memory cache).
+//    are deferred or have at most 2 lines, is a LEAN partition: at most 5 literal lines per tag (2 + 3 straight, or
+//    2 + 2 + 1 with an arc). Here it is counted -- line counts, bbox of its literal lines, deferred arc jobs -- and its
+//    literal lines are written after the scan by k_flatten_emit, straight to their final positions.
 //    Any other partition (a curve, a failed fast-path guard, an arc emitted in place) is left untouched and appended to
 //    a work list.
 //  * k_flatten runs the partitions of the work list with the general code.
-// Both plan a tag with plan_tag and emit its lines through the same functions, so a partition's outputs are the same
-// bits whichever kernel ran it.
+// All three plan a tag with plan_tag and emit its lines through the same functions, so a partition's outputs are the
+// same bits whichever kernel ran it, and the lean partitions' lines are the bits that were counted.
 #ifndef FL_LEAN_MINB
 #define FL_LEAN_MINB 4
 #endif
+
+// The plan of a tag in a lean kernel. Returns true when the tag needs the general kernel; otherwise nlit is the number
+// of literal lines the tag writes (its deferred arc's lines are not among them).
+__device__ __forceinline__ bool fl_plan_lean(TagPlan &p, bool &emits, uint32_t &nlit, const VbConfig &cfg, const uint32_t *__restrict__ scene,
+                                             const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix,
+                                             uint32_t style_flags) {
+    nlit = 0u;
+    emits = plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags);
+    if (!emits) return false;
+    if (p.n_sides != 0) return true;
+    nlit = (p.fast_stroke ? 2u : 0u) + p.tail.n_lines;
+    if (p.tail.have_arc) {
+        const ArcSteps a = arc_steps(p.tail.arc_begin, p.tail.arc_end, p.tail.arc_center, p.tail.arc_angle, p.transform);
+        if (!a.job) {
+            if (a.n_lines > 2u) return true;
+            nlit += a.n_lines;
+        }
+    }
+    return false;
+}
 
 __global__ void __launch_bounds__(FL_THREADS, FL_LEAN_MINB)
 k_flatten_lean(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids, VbPathBbox *path_bboxes,
@@ -1032,24 +1077,20 @@ k_flatten_lean(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMono
     const uint32_t part = part_base + blockIdx.x * (FL_THREADS / 32) + (threadIdx.x >> 5);
     if (part >= part_end) return;
     const uint32_t ix = part * 32u + lane;
-    __shared__ float4 sh_cache[FL_CACHE][FL_THREADS];
-    __shared__ uint32_t sh_rel[FL_CACHE][FL_THREADS];
     PathTagData tag;
     uint32_t style_flags;
-    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, path_bboxes, ix);
+    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, ix);
+    fl_open_path(cfg, path_bboxes, tag, style_flags);
     TagPlan p;
-    const bool emits = plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags);
-    bool general = emits && p.n_sides != 0;
-    if (emits && !general && p.tail.have_arc) {
-        const ArcSteps a = arc_steps(p.tail.arc_begin, p.tail.arc_end, p.tail.arc_center, p.tail.arc_angle, p.transform);
-        general = !a.job && a.n_lines > 2u;
-    }
+    bool emits;
+    uint32_t nlit;
+    const bool general = fl_plan_lean(p, emits, nlit, cfg, scene, tag_monoids, tag, ix, style_flags);
     if (__any_sync(VB_FULL, general)) {
         if (lane == 0u) work[atomicAdd(ctx.ctrs + 2, 1u)] = part;
         return;
     }
-    FlatT<false> f;
-    fl_flat_init(f, ctx, tag, ix, &sh_cache[0][threadIdx.x], &sh_rel[0][threadIdx.x]);
+    FlatT<FL_SINK_COUNT> f;
+    fl_flat_init(f, ctx, tag, ix, nullptr, nullptr);
     if (emits) {
         emit_fast_stroke(f, p);
         emit_tail(f, p);
@@ -1073,7 +1114,8 @@ k_flatten(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *_
     __shared__ uint32_t sh_rel[FL_CACHE][FL_THREADS];
     PathTagData tag;
     uint32_t style_flags;
-    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, path_bboxes, ix);
+    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, ix);
+    fl_open_path(cfg, path_bboxes, tag, style_flags);
     Flat f;
     fl_flat_init(f, ctx, tag, ix, &sh_cache[0][threadIdx.x], &sh_rel[0][threadIdx.x]);
     flatten_tag(f, cfg, scene, tag_monoids, tag, ix, style_flags);
@@ -1137,7 +1179,55 @@ k_flatten_scan(VbConfig cfg, uint32_t n_parts, const uint32_t *__restrict__ part
     }
 }
 
-// C: thread per LINE. Phase 1 scatters the literal records; phase 2 expands the jobs, 32 per warp: the warp scans the
+// B': the literal lines of the lean partitions, written straight to their final positions. Warp per partition, as in
+// k_flatten_lean; the partitions k_flatten ran (re-derived from the same plan) and those without lines are skipped. Each
+// tag is planned again and emits through the same functions as in the count pass, now into a per-warp staging area in
+// line order: lane i's nlit lines after lane i-1's, each with its final position part_dst + tag_off + rel. The deferred
+// arcs' lines (k_flatten_place) leave gaps in that order; between them the warp's lines are runs of consecutive LineSoup
+// records, stored as 8-byte words, word k by lane k % 32, so that a warp store covers 256 consecutive bytes where the run
+// allows.
+__global__ void __launch_bounds__(FL_THREADS, FL_LEAN_MINB)
+k_flatten_emit(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMonoid *__restrict__ tag_monoids,
+               const uint32_t *__restrict__ part_count, const uint32_t *__restrict__ part_dst, const uint32_t *__restrict__ tag_off,
+               VbLineSoup *lines, uint32_t part_base, uint32_t part_end) {
+    const uint32_t lane = vb_lane(), w = threadIdx.x >> 5;
+    const uint32_t part = part_base + blockIdx.x * (FL_THREADS / 32) + w;
+    if (part >= part_end || part_count[part] == 0u) return;
+    const uint32_t ix = part * 32u + lane;
+    __shared__ float4 sh_lines[FL_THREADS / 32][FL_CACHE * 32]; // a lean tag writes at most 5 < FL_CACHE literal lines
+    __shared__ uint2 sh_dst[FL_THREADS / 32][FL_CACHE * 32];    // (final position, path_ix)
+    PathTagData tag;
+    uint32_t style_flags;
+    fl_load_tag(tag, style_flags, cfg, scene, tag_monoids, ix);
+    TagPlan p;
+    bool emits;
+    uint32_t nlit;
+    const bool general = fl_plan_lean(p, emits, nlit, cfg, scene, tag_monoids, tag, ix, style_flags);
+    if (__any_sync(VB_FULL, general)) return; // k_flatten's literal records, placed by k_flatten_place
+    const uint32_t lincl = vb_warp_incl_scan(nlit);
+    const uint32_t ltotal = __shfl_sync(VB_FULL, lincl, 31);
+    FlatT<FL_SINK_EMIT> f;
+    fl_flat_init(f, FlCtx{}, tag, ix, &sh_lines[w][lincl - nlit], reinterpret_cast<uint32_t *>(&sh_dst[w][lincl - nlit]));
+    f.dst0 = part_dst[part] + tag_off[ix];
+    if (emits) {
+        emit_fast_stroke(f, p);
+        emit_tail(f, p);
+    }
+    __syncwarp();
+    const float2 *pts = reinterpret_cast<const float2 *>(sh_lines[w]);
+    for (uint32_t q = lane; q < 3u * ltotal; q += 32u) { // word c of line j: (path_ix, 0), p0, p1
+        const uint32_t j = q / 3u, c = q - 3u * j;
+        const uint2 d = sh_dst[w][j];
+        uint2 v = make_uint2(d.y, 0u);
+        if (c != 0u) {
+            const float2 pt = pts[2u * j + c - 1u];
+            v = make_uint2(__float_as_uint(pt.x), __float_as_uint(pt.y));
+        }
+        if (d.x < cfg.lines_size) reinterpret_cast<uint2 *>(lines + d.x)[c] = v;
+    }
+}
+
+// C: thread per LINE. Phase 1 scatters k_flatten's literal records; phase 2 expands the jobs, 32 per warp: the warp scans the
 // jobs' line counts and walks the concatenated line range 32 lines at a time, so lanes stay busy whatever the mix of
 // job sizes. A line's start point is its predecessor's end point: taken from the neighbouring lane when that lane
 // holds the predecessor, recomputed otherwise (same function, same bits).
@@ -1292,6 +1382,11 @@ extern "C" uint32_t vb_launch_flatten(const VbConfig &cfg, const VbFrameBufs &b,
         }
         const uint32_t n_blocks = n_own ? (n_own + FS_THREADS * FS_PER_THREAD - 1u) / (FS_THREADS * FS_PER_THREAD) : 1u;
         k_flatten_scan<<<n_blocks, FS_THREADS, 0, st>>>(cfg, n_own, part_count + part_base, part_dst + part_base, b.bump(), ctx.ctrs + 4, n_blocks);
+        if (n_own) {
+            k_flatten_emit<<<(n_own + warps_per_cta - 1) / warps_per_cta, FL_THREADS, 0, st>>>(cfg, scene, tag_monoids, part_count, part_dst,
+                                                                                            tag_off, b.lines, part_base, part_end);
+            launches++;
+        }
         k_flatten_place<<<(uint32_t)b.sm_count * 4u, FP_THREADS, 0, st>>>(cfg, scene, ctx, part_dst, tag_off, path_bboxes, b.lines);
         launches += 2;
     }

@@ -627,7 +627,9 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     b.parts_backdrop = vb_backdrop_parts(c.tiles_size); // follows the tile arena: set above, regrown on retry
     size_t off = VB_CTL_HEADER_WORDS;
     const size_t o_pathtag = off; off += vb_lookback_words(b.parts_pathtag, 5);
-    const size_t o_flatten = off; // flatten: [0] literal-record counter, [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
+    // flatten: [0] literal-record counter (k_flatten's partitions only; the lean ones write their lines in place, k_flatten_emit),
+    // [1] job counter, [2] work-list length, [4..] look-back state of its partition scan
+    const size_t o_flatten = off;
     off += 4 + vb_lookback_words((b.parts_flatten + 8191u) / 8192u, 1);
     const size_t o_draw = off; off += vb_lookback_words(b.parts_draw, 4);
     const size_t o_tile = off; off += vb_lookback_words(b.parts_tile, 1);
