@@ -5,11 +5,19 @@
 // the WGSL where the CPU twin differs (`s1.y <= bbox.y`, `max(s0.x,s1.x) <= bbox.x`); WGSL
 // round() is ties-to-even -> rintf.
 //
-// Design: one thread per line as in the WGSL, but (i) no indirect dispatch -- the grid is
-// sized from the arena capacity and reads bump.lines on the device, (ii) the seg_counts
-// allocation is aggregated per CTA: one atomicAdd per 256 lines instead of one per line (same-address atomics serialise;
-// per-warp aggregation still left ~133 k of them a frame and was slower),
-// (iii) backdrop / count updates are fire-and-forget RED operations except the slot fetch.
+// Design: (i) no indirect dispatch -- the grid is sized from the arena capacity and reads bump.lines on the device.
+// (ii) Lines are taken PC_THREADS at a time. The per-line phase is the WGSL's, one thread per line: setup, box cull,
+// imin / imax, and the backdrop of the rows left of the path's box. The seg_counts allocation is aggregated per CTA: one
+// atomicAdd per PC_THREADS lines (same-address atomics serialise; per-warp aggregation still left ~133 k of them a frame
+// and was slower).
+// (iii) The crossing phase spreads the block's crossings over all its threads instead of walking each line in a serial
+// loop: the state the walk needs goes to shared memory, and item k of the block's exclusive scan is crossing
+// i = imin + k - excl of the line found by a binary search over the scan. z and the previous z are recomputed from i
+// exactly as the serial loop produced them, so every (line, i) record is bit-identical and lands at cta_base + k, where the
+// serial loop put it. A line of 28 crossings no longer holds its CTA for 28 dependent atomic round trips.
+// (iv) Slots are reserved once per (warp, tile): __match_any_sync groups the lanes of a tile, the first takes
+// popc(peers) slots and the others theirs in lane order, so a tile's slots stay a permutation of 0..count-1. Backdrop
+// updates are fire-and-forget RED operations (aggregating the top-edge ones per warp as well measured no faster).
 // Per-tile slot order (seg_within_slice) is atomic-order dependent exactly as in the reference.
 #include "vb_device.cuh"
 #include "vb_stages.h"
@@ -18,18 +26,31 @@
 #define PC_THREADS 256
 #endif
 #ifndef PC_MINB
-#define PC_MINB 8
+#define PC_MINB 6
+#endif
+#ifndef PC_CTAS_PER_SM
+#define PC_CTAS_PER_SM 16
 #endif
 #define ONE_MINUS_ULP 0.99999994f
 #define ROBUST_EPSILON 2e-7f
 #define TILE_SCALE 0.0625f
+
+// What the crossing phase needs of each line of the current PC_THREADS-line block, as structure-of-arrays (14 KB).
+// Entries of lines without crossings are stale; the search over excl never lands on them.
+struct PcLines {
+    float a[PC_THREADS], b[PC_THREADS], x0[PC_THREADS], y0[PC_THREADS], s0y[PC_THREADS], x_sign[PC_THREADS];
+    int32_t bx0[PC_THREADS], by0[PC_THREADS], bx1[PC_THREADS], by1[PC_THREADS], delta[PC_THREADS];
+    uint32_t path_tiles[PC_THREADS], imin[PC_THREADS], excl[PC_THREADS];
+};
 
 __global__ void __launch_bounds__(PC_THREADS, PC_MINB)
 k_path_count(VbConfig cfg, VbBump *bump, const VbLineSoup *__restrict__ lines, const VbPath *__restrict__ paths, VbTile *tile,
              VbSegmentCount *seg_counts) {
     __shared__ uint32_t sh_scan[PC_THREADS / 32 + 2];
     __shared__ uint32_t sh_base;
+    __shared__ PcLines sh;
     if (bump->failed != 0u) return;
+    const uint32_t lane = vb_lane();
     const uint32_t n_lines = min(bump->lines, cfg.lines_size);
     for (uint32_t line_base = blockIdx.x * PC_THREADS; line_base < n_lines; line_base += gridDim.x * PC_THREADS) {
         const uint32_t line_ix = line_base + threadIdx.x;
@@ -133,37 +154,68 @@ k_path_count(VbConfig cfg, VbBump *bump, const VbLineSoup *__restrict__ lines, c
             }
         }
         const uint32_t n = active ? imax - imin : 0u;
-        // CTA-aggregated worklist allocation: one same-address atomic per 256 lines
+        if (n != 0u) {
+            const uint32_t t = threadIdx.x;
+            sh.a[t] = a; sh.b[t] = b; sh.x0[t] = x0; sh.y0[t] = y0; sh.s0y[t] = s0y; sh.x_sign[t] = x_sign;
+            sh.bx0[t] = bx0; sh.by0[t] = by0; sh.bx1[t] = bx1; sh.by1[t] = by1; sh.delta[t] = delta;
+            sh.path_tiles[t] = path_tiles; sh.imin[t] = imin;
+        }
+        // CTA-aggregated worklist allocation: one same-address atomic per PC_THREADS lines
         uint32_t cta_total;
         const uint32_t excl = vb_block_excl_scan(n, sh_scan, &cta_total);
+        sh.excl[threadIdx.x] = excl;
         if (threadIdx.x == 0 && cta_total != 0u) sh_base = atomicAdd(&bump->seg_counts, cta_total);
         __syncthreads();
         const uint32_t cta_base = sh_base;
-        if (n != 0u) {
-            const uint32_t seg_base = cta_base + excl;
-            float last_z = floorf(a * ((float)imin - 1.0f) + b);
-            for (uint32_t i = imin; i < imax; i++) {
-                const float zf = a * (float)i + b;
-                const float z = floorf(zf);
-                const int32_t y = vb_f2i_sat(y0 + (float)i - z);
-                const int32_t x = vb_f2i_sat(x0 + x_sign * z);
-                const int32_t base = (int32_t)path_tiles + (y - by0) * stride - bx0;
-                const bool top_edge = (i == 0u) ? (y0 == s0y) : (last_z == z);
+        // crossing phase: item k of the CTA is crossing i = imin + k - excl of the last line whose excl <= k. Whole warps
+        // step together (k0 is warp-uniform), so the warp-wide slot reservation below sees every lane.
+        for (uint32_t k0 = threadIdx.x & ~31u; k0 < cta_total; k0 += PC_THREADS) {
+            const uint32_t k = k0 + lane;
+            bool inside = false, top_edge = false;
+            int32_t tix = 0, x = 0, bx1j = 0, dj = 0;
+            uint32_t j = 0, i = 0;
+            if (k < cta_total) {
+#pragma unroll
+                for (uint32_t step = PC_THREADS / 2; step != 0u; step >>= 1)
+                    if (sh.excl[j + step] <= k) j += step;
+                const float aj = sh.a[j], bj = sh.b[j], y0j = sh.y0[j];
+                const uint32_t iminj = sh.imin[j];
+                i = iminj + (k - sh.excl[j]);
+                // the serial walk's carried last_z: at imin it started from imin - 1 in f32, later it is the previous z
+                const float z = floorf(aj * (float)i + bj);
+                const float last_z = (i == iminj) ? floorf(aj * ((float)iminj - 1.0f) + bj) : floorf(aj * (float)(i - 1u) + bj);
+                const int32_t y = vb_f2i_sat(y0j + (float)i - z);
+                x = vb_f2i_sat(sh.x0[j] + sh.x_sign[j] * z);
+                const int32_t bx0j = sh.bx0[j], by0j = sh.by0[j], by1j = sh.by1[j];
+                bx1j = sh.bx1[j];
+                dj = sh.delta[j];
+                tix = (int32_t)sh.path_tiles[j] + (y - by0j) * (bx1j - bx0j) - bx0j;
+                top_edge = (i == 0u) ? (y0j == sh.s0y[j]) : (last_z == z);
                 // far from the frame the f32 walk can step off the path's tile box: such a crossing touches no tile
-                const bool inside = x >= bx0 && x < bx1 && y >= by0 && y < by1;
-                if (inside && top_edge && x + 1 < bx1) {
-                    const int32_t x_bump = max(x + 1, bx0);
-                    atomicAdd(&tile[base + x_bump].backdrop, delta);
-                }
-                const uint32_t seg_within_slice = inside ? atomicAdd(&tile[base + x].segment_count_or_ix, 1u) : VB_SEG_OUTSIDE;
-                const uint32_t seg_ix = seg_base + i - imin;
+                inside = x >= bx0j && x < bx1j && y >= by0j && y < by1j;
+            }
+            if (inside && top_edge && x + 1 < bx1j) atomicAdd(&tile[tix + x + 1].backdrop, dj);
+            // one slot fetch per (warp, tile): the leader takes popc(peers) slots and hands them out in lane order, so a
+            // tile's slots stay a permutation of 0..count-1
+            const uint32_t inmask = __ballot_sync(VB_FULL, inside);
+            uint32_t peers = 0u, old = 0u;
+            int leader = (int)lane;
+            if (inside) {
+                peers = __match_any_sync(inmask, tix + x);
+                leader = __ffs((int)peers) - 1;
+                if ((int)lane == leader) old = atomicAdd(&tile[tix + x].segment_count_or_ix, (uint32_t)__popc(peers));
+            }
+            old = __shfl_sync(VB_FULL, old, leader);
+            if (k < cta_total) {
+                const uint32_t seg_within_slice = inside ? old + (uint32_t)__popc(peers & ((1u << lane) - 1u)) : VB_SEG_OUTSIDE;
+                const uint32_t seg_ix = cta_base + k;
                 if (seg_ix < cfg.seg_counts_size) {
-                    VbSegmentCount sc = {line_ix, i, seg_within_slice};
+                    VbSegmentCount sc = {line_base + j, i, seg_within_slice};
                     seg_counts[seg_ix] = sc;
                 }
-                last_z = z;
             }
         }
+        __syncthreads(); // the next iteration overwrites sh
     }
 }
 
@@ -171,7 +223,7 @@ k_path_count(VbConfig cfg, VbBump *bump, const VbLineSoup *__restrict__ lines, c
 
 // The grid comes from the lines capacity (at most 16 CTAs per SM); the kernel strides over the count read on the device.
 extern "C" uint32_t vb_launch_path_count(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    const uint64_t blocks = ((uint64_t)cfg.lines_size + 255) / 256, most = (uint64_t)b.sm_count * 16;
+    const uint64_t blocks = ((uint64_t)cfg.lines_size + 255) / 256, most = (uint64_t)b.sm_count * PC_CTAS_PER_SM;
     const uint32_t grid = (uint32_t)(blocks < most ? blocks : most);
     if (grid == 0) return 0;
     k_path_count<<<grid, PC_THREADS, 0, st>>>(cfg, b.bump(), b.lines, b.paths, b.tiles, b.seg_counts);
