@@ -132,6 +132,29 @@ int vb_set_cuda_graph(vb_renderer *, int on);
 /* Switch the per-stage CUDA events of vb_options.timing on or off for the following frames (on: plain launches, no graph). */
 int vb_set_timing(vb_renderer *, int on);
 
+/* ---- views: pan and zoom a resident scene without uploading it again (an addition; vello re-encodes the scene) ----
+ * Render the uploaded scene under a view: frames enqueued after this call render what
+ * Scene::new().append(&scene, Some(view)) would render (encoding.rs:94-174). affine = kurbo Affine coefficients
+ * [a b c d e f], converted to f32 like Transform::from_kurbo. NULL clears the view. Non-finite coefficients (in f32):
+ * VB_E_INVALID.
+ *  - A view lasts until it is changed or cleared. It survives scene uploads: it belongs to the viewer, not to the scene.
+ *  - It applies to every frame the renderer renders: vb_render_resident, vb_render_enqueue, vb_render_uploaded, vb_render,
+ *    vb_render_begin, vb_run_stages, batches (every cell, each in its own frame), bin_row / tile_row windows and vb_group
+ *    (vb_group_set_view).
+ *  - It applies in stream order: a frame already enqueued (e.g. the frames in flight of vb_render_begin) keeps the view it was
+ *    enqueued with, also when it is re-run after an arena overflow.
+ *  - The viewed transforms are written by the frame itself into renderer-owned memory past the scene (one extra kernel);
+ *    the uploaded bytes are never modified. Changing the coefficients replays a captured frame graph; setting or clearing
+ *    a view captures again. Room for the viewed transforms is taken only while a view is set (the first viewed frame after an
+ *    upload without it moves the scene and waits for the renderer's streams); clearing the view waits for the frames already
+ *    enqueued and frees what the view held.
+ *  - Setting any view, the identity included, switches on frame culling: flatten emits no lines for a tag whose hull (grown
+ *    by the stroke's reach) lies above, below or right of the frame (or the window), so a zoomed-in frame flattens fewer
+ *    lines. Pixels are those of the unculled frame. With the exchange (vb_exchange_enable) flatten does not cull; the view
+ *    still applies. NULL restores the unviewed pipeline exactly. */
+int vb_set_view(vb_renderer *, const double affine[6]);
+int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: whole-frame graphs instantiated so far */
+
 /* The renderer-owned target of the last frame (device pointer) and its size in bytes. */
 void *vb_target(vb_renderer *, size_t *bytes);
 /* Copy `bytes` from a device pointer to a host pointer on the renderer's stream, then synchronise. */
@@ -300,6 +323,7 @@ void *vb_group_frame(vb_group *, size_t *bytes);
 /* tile-row boundaries in use (n_devices + 1 entries) and the device times (ms) of the last frame (n_devices entries) */
 int vb_group_stripes(vb_group *, uint32_t *boundaries, float *device_ms);
 int vb_group_set_balancing(vb_group *, int on); /* default on */
+int vb_group_set_view(vb_group *, const double affine[6]); /* vb_set_view on every renderer of the group */
 
 /* ---- flatten sharded across the GPUs (SURVEY.md 8e option B) ----
  * By default every GPU of a multi-GPU frame flattens the whole scene (culled to its stripe). With the exchange enabled GPU k

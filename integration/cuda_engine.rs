@@ -69,6 +69,11 @@ extern "C" {
     pub fn vb_scene_upload_streams(r: *mut VbRenderer, e: *const VbEncodingStreams, layout_out: *mut Layout) -> c_int;
     pub fn vb_render_uploaded(r: *mut VbRenderer, params: *const VbParams, out: *mut c_void, out_is_device: u32, stats: *mut VbFrameStats) -> c_int;
     pub fn vb_set_occlusion_cull(r: *mut VbRenderer, on: c_int) -> c_int;
+    // pan / zoom a resident scene: with_winit's per-frame `scene.append(&fragment, Some(transform))` becomes one upload of
+    // the fragment and vb_set_view(transform.as_coeffs()) per frame (NULL clears the view)
+    pub fn vb_set_view(r: *mut VbRenderer, affine: *const [f64; 6]) -> c_int;
+    pub fn vb_group_set_view(g: *mut VbGroup, affine: *const [f64; 6]) -> c_int;
+    pub fn vb_debug_graph_captures(r: *mut VbRenderer, captures: *mut u64) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

@@ -123,6 +123,7 @@ struct FlatT {
     uint32_t dst0; // FL_SINK_EMIT: final position of the tag's first line
     float bx0, by0, bx1, by1; // bbox of the literal lines
     bool force;    // a job was deferred: the tag's bbox is known to be non-degenerate
+    bool edge;     // the tag was culled right of the frame: its bbox is the one point of emit_edge
     float4 *cache; // RECORDS: &cache[0][threadIdx.x], stride FL_THREADS; EMIT: this lane's first staging slot, stride 1
     uint32_t *cache_rel; // RECORDS: rel, same stride; EMIT: (final position, path_ix) pairs
     __device__ __forceinline__ void write_line(fv2 p0, fv2 p1) { // device-space end points
@@ -764,12 +765,15 @@ struct TagPlan {
     float offset;
     fv2 n_start, n_prev;
     TailOps tail;
+    bool edge;    // culled right of the frame: the tag's only output is the box point (16 width_in_tiles, edge_y) (emit_edge)
+    float edge_y;
 };
 
-// false: the tag emits nothing.
+// false: the tag emits nothing (and, with plan.edge, only extends its path's box).
 __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, const uint32_t *__restrict__ scene,
                                          const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix,
                                          uint32_t style_flags) {
+    plan.edge = false;
     uint32_t seg_type = tag.tag_byte & 3u;
     if (seg_type == 0u) return false;
     bool is_stroke = (style_flags & STYLE_FLAGS_STYLE) != 0u;
@@ -785,12 +789,13 @@ __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, con
     }
     CubicPoints &pts = plan.pts;
     pts = read_path_segment(cfg, scene, tag, is_stroke);
-    if (cfg.win_cull != 0u) {
-        // Stripe rendering (one bin-row window per GPU): everything this tag emits lies within R of the convex hull of
-        // its control points (R = half width x max(miter limit, sqrt 2) for strokes), so a tag whose hull, grown by R
-        // and one pixel, misses the window's rows cannot contribute a line, a backdrop or a bbox extent to them.
-        // Rows are independent in this algorithm (backdrop runs left to right inside a tile row), so the rows of the
-        // window still see every line that touches them: pixels are unchanged (test_stripes_equal_full_frame).
+    if ((cfg.win_cull | cfg.frame_cull) != 0u) {
+        // Stripe rendering (one bin-row window per GPU) and views: everything this tag emits lies within R of the convex
+        // hull of its control points (R = half width x max(miter limit, sqrt 2) for strokes), so a tag whose hull, grown
+        // by R and one pixel, misses the window's rows (the frame's, without a window) cannot contribute a line, a backdrop
+        // or a bbox extent to them. Rows are independent in this algorithm (backdrop runs left to right inside a tile row),
+        // so the rows of the window still see every line that touches them: pixels are unchanged
+        // (test_stripes_equal_full_frame, tests/test_gpu_view.py).
         const float y_0 = fmaf(transform.m1, pts.p0.x, fmaf(transform.m3, pts.p0.y, transform.ty));
         const float y_1 = fmaf(transform.m1, pts.p1.x, fmaf(transform.m3, pts.p1.y, transform.ty));
         const float y_2 = fmaf(transform.m1, pts.p2.x, fmaf(transform.m3, pts.p2.y, transform.ty));
@@ -803,6 +808,26 @@ __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, con
         }
         const float lo = fminf(fminf(y_0, y_1), fminf(y_2, y_3)) - grow, hi = fmaxf(fmaxf(y_0, y_1), fmaxf(y_2, y_3)) + grow;
         if (hi < (float)(cfg.win_ty0 * VB_TILE_HEIGHT) || lo > (float)(cfg.win_ty1 * VB_TILE_HEIGHT)) return false; // NaN: kept
+        if (cfg.frame_cull != 0u) {
+            // Views: a tag whose grown hull lies right of the frame (x > 16 width_in_tiles) emits no line either. Its lines
+            // cross no pixel of the frame, and the winding number at a frame pixel sums only crossings LEFT of it, so no
+            // frame pixel's coverage changes. What it still contributes is its path's box: coverage that enters from the
+            // left may run to the frame's right edge because of lines that are culled here (a frame-covering rectangle
+            // whose right edge is off-frame), so the tag extends the box to x = 16 width_in_tiles at the height of its
+            // first point, clamped to the window's rows. That point is an end point of the tag's own lines (fills), or lies
+            // between two of them (strokes: p0 +- the offset normal), so the box stays within the path's true extents as
+            // tile_alloc clamps them to the frame, and the tiles it allocates are the unculled frame's. Tags left of the
+            // frame are kept: they carry backdrop. NaN: kept.
+            const float x_0 = fmaf(transform.m0, pts.p0.x, fmaf(transform.m2, pts.p0.y, transform.tx));
+            const float x_1 = fmaf(transform.m0, pts.p1.x, fmaf(transform.m2, pts.p1.y, transform.tx));
+            const float x_2 = fmaf(transform.m0, pts.p2.x, fmaf(transform.m2, pts.p2.y, transform.tx));
+            const float x_3 = fmaf(transform.m0, pts.p3.x, fmaf(transform.m2, pts.p3.y, transform.tx));
+            if (fminf(fminf(x_0, x_1), fminf(x_2, x_3)) - grow > (float)(cfg.width_in_tiles * VB_TILE_WIDTH)) {
+                plan.edge = true;
+                plan.edge_y = vb_clampf(y_0, (float)(cfg.win_ty0 * VB_TILE_HEIGHT), (float)(cfg.win_ty1 * VB_TILE_HEIGHT));
+                return false;
+            }
+        }
     }
     // the offset curves to flatten (0, 1 or 2 of them) and what follows them
     plan.is_stroke = is_stroke;
@@ -915,11 +940,23 @@ __device__ __forceinline__ void emit_tail(F &f, const TagPlan &p) {
     if (tail.n_lines > 2u) f.line_xf(tail.a2, tail.b2, p.transform);
 }
 
+// The box point of a tag culled right of the frame (plan_tag).
+template <class F>
+__device__ __forceinline__ void emit_edge(F &f, const VbConfig &cfg, const TagPlan &p) {
+    if (!p.edge) return;
+    f.bx0 = f.bx1 = (float)(cfg.width_in_tiles * VB_TILE_WIDTH);
+    f.by0 = f.by1 = p.edge_y;
+    f.edge = true;
+}
+
 // Everything one tag byte produces.
 __device__ void flatten_tag(Flat &f, const VbConfig &cfg, const uint32_t *__restrict__ scene,
                             const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix, uint32_t style_flags) {
     TagPlan p;
-    if (!plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags)) return;
+    if (!plan_tag(p, cfg, scene, tag_monoids, tag, ix, style_flags)) {
+        emit_edge(f, cfg, p);
+        return;
+    }
     emit_fast_stroke(f, p);
 #pragma unroll 1
     for (int side = 0; side < p.n_sides; side++) { // one copy of the Euler machinery in the instruction stream
@@ -965,7 +1002,7 @@ template <class F>
 __device__ __forceinline__ void fl_flat_init(F &f, const FlCtx &ctx, const PathTagData &tag, uint32_t ix, float4 *cache, uint32_t *cache_rel) {
     f.c = ctx;
     f.tag_ix = ix; f.path_ix = tag.path_ix; f.trans_ix = tag.trans_ix;
-    f.ix = 0u; f.nlit = 0u; f.dst0 = 0u; f.force = false;
+    f.ix = 0u; f.nlit = 0u; f.dst0 = 0u; f.force = false; f.edge = false;
     f.bx0 = 1e31f; f.by0 = 1e31f; f.bx1 = -1e31f; f.by1 = -1e31f;
     f.cache = cache;
     f.cache_rel = cache_rel;
@@ -1014,7 +1051,7 @@ __device__ __forceinline__ void fl_tag_end(F &f, const VbConfig &cfg, VbPathBbox
     }
     // bbox: consecutive tags mostly belong to the same path, so reduce across the lanes of a path first (floor / ceil
     // commute with min / max) and issue one set of atomics per (warp, path) instead of one per tag
-    const bool pub = f.nlit != 0u && (f.force || f.bx1 > f.bx0 || f.by1 > f.by0) && path_ix < n_paths;
+    const bool pub = ((f.nlit != 0u && (f.force || f.bx1 > f.bx0 || f.by1 > f.by0)) || f.edge) && path_ix < n_paths;
     const uint32_t pubmask = __ballot_sync(VB_FULL, pub);
     if (pub) {
         int x0 = fl_floor_i(f.bx0), y0 = fl_floor_i(f.by0), x1 = fl_ceil_i(f.bx1), y1 = fl_ceil_i(f.by1);
@@ -1094,6 +1131,8 @@ k_flatten_lean(VbConfig cfg, const uint32_t *__restrict__ scene, const VbTagMono
     if (emits) {
         emit_fast_stroke(f, p);
         emit_tail(f, p);
+    } else {
+        emit_edge(f, cfg, p);
     }
     fl_tag_end(f, cfg, path_bboxes, ctx, part_count, tag_off);
 }

@@ -1,0 +1,58 @@
+// k_view.cu -- views of a resident scene (vb_set_view): every draw rendered as Scene::new().append(&scene, Some(view)) would
+// render it (vello_encoding/src/encoding.rs:94-174), without touching the uploaded bytes.
+//
+// The view V lives in device memory, written in stream order by k_view_set, so that frames enqueued before a change keep
+// the view they were enqueued with and a captured frame replays under a new view. k_view_transforms, the first kernel of a
+// viewed frame, writes V * T for every transform T of the scene into a region past the scene's streams; the frame's
+// layout.transform_base points there (prepare, vb_api.cu). The scene's own transforms are never modified, so a re-run after
+// an arena overflow, a graph replay or the next frame compose the view once.
+#include "vb_device.cuh"
+#include "vb_stages.h"
+
+struct ViewCoeffs {
+    float m[6];
+};
+
+__global__ void k_view_set(ViewCoeffs v, float *dst) {
+    if (threadIdx.x < 6u) dst[threadIdx.x] = v.m[threadIdx.x];
+}
+
+// Transform * Transform (vello_encoding/src/math.rs:51-73) in f32, in its association and without FMA contraction: the
+// arithmetic of encoding.py's Encoding.append, so the viewed transforms are the bits a host-side append produces.
+__global__ void __launch_bounds__(256) k_view_transforms(const float *__restrict__ view, const uint32_t *__restrict__ src, uint32_t *dst,
+                                                         uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float a[6], b[6];
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        a[k] = __ldg(view + k);
+        b[k] = __uint_as_float(__ldg(src + 6u * i + k));
+    }
+    float r[6];
+    r[0] = __fadd_rn(__fmul_rn(a[0], b[0]), __fmul_rn(a[2], b[1]));
+    r[1] = __fadd_rn(__fmul_rn(a[1], b[0]), __fmul_rn(a[3], b[1]));
+    r[2] = __fadd_rn(__fmul_rn(a[0], b[2]), __fmul_rn(a[2], b[3]));
+    r[3] = __fadd_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[3], b[3]));
+    r[4] = __fadd_rn(__fadd_rn(__fmul_rn(a[0], b[4]), __fmul_rn(a[2], b[5])), a[4]);
+    r[5] = __fadd_rn(__fadd_rn(__fmul_rn(a[1], b[4]), __fmul_rn(a[3], b[5])), a[5]);
+#pragma unroll
+    for (int k = 0; k < 6; k++) dst[6u * i + k] = __float_as_uint(r[k]);
+}
+
+extern "C" void vb_launch_view_set(float *dst, const float m[6], cudaStream_t st) {
+    ViewCoeffs v;
+    for (int k = 0; k < 6; k++) v.m[k] = m[k];
+    k_view_set<<<1, 32, 0, st>>>(v, dst);
+}
+
+extern "C" uint32_t vb_launch_view_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    // exactly the region prepare reserved and sized the allocation for: [transform_base, scene_words), past the uploaded
+    // streams. It is empty for a layout whose transforms do not lie inside the uploaded words, so such a layout launches
+    // nothing, and the source transforms [view_src, view_src + 6 n) lie inside the scene whenever n > 0.
+    const uint32_t n = cfg.scene_words > cfg.layout.transform_base ? (cfg.scene_words - cfg.layout.transform_base) / 6u : 0u;
+    if (n == 0u) return 0u;
+    uint32_t *dst = const_cast<uint32_t *>(b.scene) + cfg.layout.transform_base;
+    k_view_transforms<<<(n + 255u) / 256u, 256, 0, st>>>(b.view, b.scene + cfg.view_src, dst, n);
+    return 1u;
+}

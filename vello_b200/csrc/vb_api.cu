@@ -117,6 +117,12 @@ struct GraphSlot {
     uint32_t launches = 0;
 };
 
+// A view (vb_set_view): the f32 coefficients every frame enqueued while it is set renders the scene under.
+struct View {
+    bool on = false;
+    float m[6] = {};
+};
+
 struct vb_renderer {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -185,6 +191,10 @@ struct vb_renderer {
     bool use_graph = true;        // replay whole frames as CUDA graphs (see enqueue)
     GraphSlot graphs[4];
     uint32_t graph_next = 0;
+    uint64_t graph_captures = 0;  // whole-frame graphs instantiated (vb_debug_graph_captures)
+    // the view of the frames enqueued from now on; its coefficients reach view_coef in stream order (put_view)
+    View view;
+    DevBuf view_coef;
     uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
     uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
     // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct)
@@ -208,6 +218,7 @@ struct vb_renderer {
     struct RingFrame { // a streamed frame between vb_render_begin and its completion on the host
         bool pending = false, raster_checked = false;
         vb_params params{};
+        View view; // the view it was enqueued with (a re-run renders under it again)
         void *out_host = nullptr;
         uint32_t slot = 0;
         vb_frame_stats stats{};
@@ -232,7 +243,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena};
+                           &r->blit_rects, &r->xc.arena, &r->view_coef};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -478,6 +489,36 @@ extern "C" int vb_copy_to_host(vb_renderer *r, const void *src_device, void *dst
     return VB_OK;
 }
 
+// Transforms of a scene: the stream from layout.transform_base to style_base (0 for a layout that does not fit the scene).
+static uint32_t n_transforms(const VbLayout &L, size_t scene_words) {
+    if (L.style_base < L.transform_base || L.style_base > scene_words) return 0u;
+    return (L.style_base - L.transform_base) / 6u;
+}
+// A scene slot's allocation: the packed scene, then (while a view is set) room for its viewed transforms (k_view.cu), then slack.
+static size_t scene_bytes(const VbLayout &L, size_t scene_words, bool view) {
+    return (scene_words + (view ? 6u * (size_t)n_transforms(L, scene_words) : 0u)) * 4u + 64u;
+}
+// A view set after the scene's upload: move the current slot's scene into an allocation with room for its viewed transforms.
+// The scene may still be arriving on the upload stream, and frames already enqueued read the old allocation.
+static int reserve_view_room(vb_renderer *r, size_t bytes) {
+    DevBuf &sc = r->cur->scene;
+    if (sc.cap >= bytes) return VB_OK;
+    CK(cudaStreamSynchronize(r->upload_stream));
+    CK(cudaStreamSynchronize(r->stream));
+    DevBuf grown;
+    grown.cap = (bytes + 255) & ~(size_t)255;
+    CK(cudaMalloc(&grown.p, grown.cap));
+    const cudaError_t e = cudaMemcpy(grown.p, sc.p, r->cur->scene_words * 4, cudaMemcpyDeviceToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(grown.p);
+        r->err = std::string("view: moving the scene: ") + cudaGetErrorString(e);
+        return VB_E_CUDA;
+    }
+    CK(cudaFree(sc.p));
+    sc = grown;
+    return VB_OK;
+}
+
 static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
                      uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h) {
     if (!r || !layout || (scene_len && !scene) || (scene_len & 3)) return VB_E_INVALID;
@@ -486,7 +527,7 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
     memcpy(&r->cur->layout, layout, sizeof(VbLayout));
     r->cur->scene_words = scene_len / 4;
     int rc;
-    if ((rc = ensure(r, r->cur->scene, scene_len + 64))) return rc;
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(r->cur->layout, r->cur->scene_words, r->view.on)))) return rc;
     if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
     r->cur->n_ramps = ramp_h;
     if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
@@ -583,6 +624,16 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
+    if (r->view.on) {
+        // the frame reads the viewed transforms past the scene's streams: [transform_base, scene_words) is the region
+        // k_view_transforms writes, empty for a layout whose transforms do not lie inside the uploaded words
+        c.view_src = c.layout.transform_base;
+        c.layout.transform_base = c.scene_words;
+        c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
+        c.frame_cull = 1u;
+        int rc0 = reserve_view_room(r, (size_t)c.scene_words * 4u + 64u);
+        if (rc0) return rc0;
+    }
     c.n_cells = n_cells;
     c.tile_rows = c.height_in_tiles * n_cells;
     c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
@@ -645,6 +696,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     b.atlas = (const uint8_t *)r->cur->atlas.p;
     b.mask8 = (const uint32_t *)r->mask8.p;
     b.mask16 = (const uint32_t *)r->mask16.p;
+    b.view = r->view.on ? (const float *)r->view_coef.p : nullptr;
     b.tag_monoids = (VbTagMonoid *)r->tag_monoids.p;
     b.path_bboxes = (VbPathBbox *)r->path_bboxes.p;
     b.draw_monoids = (VbDrawMonoid *)r->draw_monoids.p;
@@ -765,10 +817,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_FLATTEN: {
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
+            // a viewed frame first writes its transforms (read by flatten and draw), inside flatten's stage events
+            if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             VbConfig cf = c;
             uint32_t p0 = 0u, p1 = b.parts_flatten;
             if (r->xc.enabled) {
                 cf.win_cull = 0u;
+                cf.frame_cull = 0u;
                 const uint32_t P = b.parts_flatten, G = r->xc.world, k = r->xc.rank;
                 p0 = (uint32_t)((uint64_t)P * k / G) & ~7u;
                 p1 = k + 1u == G ? P : ((uint32_t)((uint64_t)P * (k + 1u) / G) & ~7u);
@@ -778,6 +833,8 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             break;
         }
         case VB_STAGE_ID_DRAW:
+            // a range that starts here writes them again: the kernel only reads the scene's own, so the words are the same
+            if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);
             launches += vb_launch_draw(c, b, st);
@@ -890,6 +947,7 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
         }
         memcpy(&slot->key, &key, sizeof key); // with its (zeroed) padding: keys are compared bytewise
         slot->launches = r->launches;
+        r->graph_captures++;
     }
     if (cudaGraphLaunch(slot->exec, r->stream) != cudaSuccess) {
         cudaGraphExecDestroy(slot->exec);
@@ -1227,10 +1285,21 @@ extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len,
 // out_host and `stats` describes frame k-2 (zeros while there is none); vb_readback_wait completes the rest. THREE alternating
 // out_host buffers are needed. An arena overflow is found at the rasterisation check; that frame (and the one enqueued behind
 // it) is then re-run synchronously with grown arenas -- rare (first frames of a new scene size) and exact.
+static int put_view(vb_renderer *r, const View &v);
+static bool same_view(const View &a, const View &b) { return a.on == b.on && (!a.on || memcmp(a.m, b.m, sizeof a.m) == 0); }
 static int rerun_frame_sync(vb_renderer *r, uint32_t q, vb_frame_stats *stats) {
     const uint32_t slot = r->ring[q].slot;
     r->cur = &r->slot[slot];
-    return render_sync_host(r, &r->ring[q].params, Dest{nullptr, r->ring[q].out_host, slot != 0u, 1u}, stats);
+    // under the view the frame was enqueued with, even if it has changed since
+    const View now = r->view;
+    const bool other = !same_view(now, r->ring[q].view);
+    int rc = other ? put_view(r, r->ring[q].view) : VB_OK;
+    if (rc == VB_OK) rc = render_sync_host(r, &r->ring[q].params, Dest{nullptr, r->ring[q].out_host, slot != 0u, 1u}, stats);
+    if (other) {
+        const int rc2 = put_view(r, now);
+        if (rc == VB_OK) rc = rc2;
+    }
+    return rc;
 }
 
 // Frame in ring entry q: wait for its kernels, look at its bump counters, re-run on overflow (together with the younger frame
@@ -1299,6 +1368,7 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
     r->ring[q].pending = true;
     r->ring[q].raster_checked = false;
     r->ring[q].params = *p;
+    r->ring[q].view = r->view;
     r->ring[q].out_host = out_host;
     r->ring[q].slot = slot;
     memset(&r->ring[q].stats, 0, sizeof(vb_frame_stats));
@@ -1498,6 +1568,50 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
             return VB_OK;
         }
     return VB_E_UNKNOWN_BUFFER;
+}
+
+// ---- views: vb_set_view --------------------------------------------------------------------------------------------------
+// Make v the view of the frames enqueued from now on: its coefficients are written on the renderer's stream, behind every
+// frame already enqueued, so those keep theirs. Setting or clearing a view changes the frame's config (and the graph key);
+// changing the coefficients does not.
+static int put_view(vb_renderer *r, const View &v) {
+    CK(cudaSetDevice(r->device));
+    r->view = v;
+    if (!v.on) { // no view: nothing of it stays (frames already enqueued may still read the coefficients)
+        if (r->view_coef.p) {
+            CK(cudaStreamSynchronize(r->stream));
+            CK(cudaFree(r->view_coef.p));
+            r->view_coef = DevBuf{};
+        }
+        return VB_OK;
+    }
+    int rc = ensure(r, r->view_coef, 6 * sizeof(float));
+    if (rc) return rc;
+    vb_launch_view_set((float *)r->view_coef.p, v.m, r->stream);
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+static int view_of(const double *affine, View *v) {
+    v->on = affine != nullptr;
+    for (int k = 0; v->on && k < 6; k++) {
+        v->m[k] = (float)affine[k]; // Transform::from_kurbo
+        if (!isfinite(v->m[k])) return VB_E_INVALID;
+    }
+    return VB_OK;
+}
+extern "C" int vb_set_view(vb_renderer *r, const double affine[6]) {
+    if (!r) return VB_E_INVALID;
+    View v;
+    if (view_of(affine, &v)) {
+        r->err = "vb_set_view: the coefficients must be finite in f32";
+        return VB_E_INVALID;
+    }
+    return put_view(r, v);
+}
+extern "C" int vb_debug_graph_captures(vb_renderer *r, uint64_t *captures) {
+    if (!r || !captures) return VB_E_INVALID;
+    *captures = r->graph_captures;
+    return VB_OK;
 }
 
 extern "C" int vb_set_timing(vb_renderer *r, int on) {
@@ -1782,6 +1896,26 @@ extern "C" const char *vb_group_last_error(vb_group *g) { return g ? g->err.c_st
 extern "C" int vb_group_set_balancing(vb_group *g, int on) {
     if (!g) return VB_E_INVALID;
     g->balancing = on != 0;
+    return VB_OK;
+}
+extern "C" int vb_group_set_view(vb_group *g, const double affine[6]) {
+    if (!g) return VB_E_INVALID;
+    View v;
+    if (view_of(affine, &v)) {
+        g->err = "vb_group_set_view: the coefficients must be finite in f32";
+        return VB_E_INVALID;
+    }
+    // all renderers or none: on a failure the ones already switched get their earlier view back
+    std::vector<View> before;
+    for (vb_renderer *r : g->subs) before.push_back(r->view);
+    for (size_t i = 0; i < g->subs.size(); i++) {
+        const int rc = put_view(g->subs[i], v);
+        if (rc) {
+            g->err = g->subs[i]->err;
+            for (size_t j = 0; j <= i; j++) put_view(g->subs[j], before[j]);
+            return rc;
+        }
+    }
     return VB_OK;
 }
 extern "C" void *vb_group_frame(vb_group *g, size_t *bytes) {
@@ -2154,7 +2288,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     }
 
     // the six streams go straight to their places in the packed buffer
-    if ((rc = ensure(r, r->cur->scene, total_words * 4 + 64))) return rc;
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, total_words, r->view.on)))) return rc;
     char *base = (char *)r->cur->scene.p;
     if (e->n_path_tags) CK(cudaMemcpyAsync(base, e->path_tags, e->n_path_tags, cudaMemcpyHostToDevice, st));
     if (e->n_path_data) CK(cudaMemcpyAsync(base + (size_t)L.path_data_base * 4, e->path_data, (size_t)e->n_path_data * 4, cudaMemcpyHostToDevice, st));

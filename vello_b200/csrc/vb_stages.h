@@ -22,6 +22,7 @@ struct VbFrameBufs {
     const uint32_t *scene, *ramps;
     const uint8_t *atlas;
     const uint32_t *mask8, *mask16;
+    const float *view; // the view's six f32 coefficients (vb_set_view), written in stream order; read by k_view_transforms
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -102,6 +103,10 @@ size_t vb_exchange_half_bytes(uint32_t n_paths, uint32_t lines_cap);
 uint32_t vb_exchange_epoch_word(void);
 uint32_t vb_launch_exchange_send(const VbConfig &cfg, const VbFrameBufs &b, const XPeers &peers, cudaStream_t st);
 uint32_t vb_launch_exchange_recv(const VbConfig &cfg, const VbFrameBufs &b, const XPeers &peers, cudaStream_t st);
+
+// views (k_view.cu): store the coefficients m[6] at dst in stream order; write V * T of every scene transform to the view region
+void vb_launch_view_set(float *dst, const float m[6], cudaStream_t st);
+uint32_t vb_launch_view_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // device resolve (vb_scene_upload_streams)
 void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes, uint32_t end_clip_word0,

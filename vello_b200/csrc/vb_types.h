@@ -60,6 +60,10 @@ typedef struct {
     uint32_t out_pitch_px;     /* output row pitch in pixels */
     uint32_t out_row0;         /* first pixel row stored at out[0] (stripe outputs) */
     uint32_t win_cull;         /* 1: a stripe window is set -- flatten skips segments that cannot reach its rows */
+    /* View (vb_set_view): layout.transform_base points at the viewed transforms, which k_view_transforms writes past the
+     * scene's own streams (scene_words covers them) from the scene's transforms at view_src. frame_cull: flatten also skips
+     * tags above, below or right of the frame (plan_tag). Both 0 without a view. */
+    uint32_t view_src, frame_cull;
     /* Batch (vb_set_cells): the draw objects are split into n_cells ranges cell_draw[c] .. cell_draw[c + 1], each rendered
      * into its own width x height frame. The tile grid is a tall frame of tile_rows = n_cells * height_in_tiles rows; cell c
      * owns tile rows [c * height_in_tiles, (c + 1) * height_in_tiles) and bin rows [c * hB, (c + 1) * hB). width_in_tiles,

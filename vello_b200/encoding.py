@@ -809,6 +809,25 @@ class Packed:
         return int(self.scene.nbytes)
 
 
+def viewed(packed: Packed, view: Affine) -> Packed:
+    """The packed scene of `Scene().append(scene, view)`, made by mapping `packed`'s transform words: every transform T
+    becomes view * T in f32 with `Encoding.append`'s arithmetic (the product the renderer's `set_view` computes on the
+    device). Nothing else of a packed scene depends on the transforms."""
+    lay = packed.layout
+    scene = np.array(packed.scene, dtype=np.uint32)
+    t = scene[lay.transform_base:lay.style_base].view(np.float32).reshape(-1, 6)
+    a = [np.float32(v) for v in view.coeffs]
+    b = [t[:, k].copy() for k in range(6)]
+    with np.errstate(over="ignore", invalid="ignore"):  # f32 overflow is part of the arithmetic, as on the device
+        t[:, 0] = a[0] * b[0] + a[2] * b[1]
+        t[:, 1] = a[1] * b[0] + a[3] * b[1]
+        t[:, 2] = a[0] * b[2] + a[2] * b[3]
+        t[:, 3] = a[1] * b[2] + a[3] * b[3]
+        t[:, 4] = a[0] * b[4] + a[2] * b[5] + a[4]
+        t[:, 5] = a[1] * b[4] + a[3] * b[5] + a[5]
+    return Packed(scene, lay, packed.ramps, packed.atlas)
+
+
 def _align_up(n: int, a: int) -> int:
     return (n + a - 1) // a * a
 

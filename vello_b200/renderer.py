@@ -16,6 +16,7 @@ import numpy as np
 
 from .config import AA_AREA, AA_MSAA8, AA_MSAA16, RenderParams
 from .encoding import Image, Packed, Scene, resolve
+from .shapes import Affine
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvello_b200.so")
@@ -130,6 +131,9 @@ def load_library() -> C.CDLL:
     lib.vb_mark_override_image_dirty.argtypes = [vp, vp]
     lib.vb_set_cells.argtypes = [vp, vp, C.c_uint32]
     lib.vb_render_uploaded.argtypes = [vp, C.POINTER(_Params), vp, C.c_uint32, C.POINTER(FrameStats)]
+    lib.vb_set_view.argtypes = [vp, C.POINTER(C.c_double)]
+    lib.vb_group_set_view.argtypes = [vp, C.POINTER(C.c_double)]
+    lib.vb_debug_graph_captures.argtypes = [vp, C.POINTER(C.c_uint64)]
     _lib = lib
     return lib
 
@@ -141,7 +145,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_new", "vb_group_free", "vb_group_size", "vb_group_renderer", "vb_group_last_error", "vb_group_render",
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
-                    "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells"]
+                    "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
+                    "vb_debug_graph_captures"]
 
 
 def _device_image(t):
@@ -165,6 +170,11 @@ class RendererOptions:
     device: int = 0
     timing: bool = False
     max_retries: int = 6
+
+
+def _view_coeffs(affine: Optional[Affine]):
+    """The kurbo Affine coefficients [a b c d e f] as vb_set_view takes them (None: clear the view)."""
+    return None if affine is None else (C.c_double * 6)(*[float(v) for v in affine.coeffs])
 
 
 def _params_struct(p: RenderParams, bin_rows=(0, 0), tile_rows=(0, 0)) -> _Params:
@@ -455,6 +465,18 @@ class Renderer:
         """Replay whole frames as CUDA graphs (default on)."""
         self._check(self.lib.vb_set_cuda_graph(self.handle, 1 if on else 0), "vb_set_cuda_graph")
 
+    def set_view(self, affine: Optional[Affine]):
+        """Render the uploaded scene under `affine` from the next frame on, as `Scene().append(scene, affine)` would render,
+        without uploading it again (pan / zoom of a resident scene). Frames already enqueued keep their view; the view
+        survives uploads. Flatten then culls what lies above, below or right of the frame. None clears it."""
+        self._check(self.lib.vb_set_view(self.handle, _view_coeffs(affine)), "vb_set_view")
+
+    def debug_graph_captures(self) -> int:
+        """Test-only: whole-frame CUDA graphs this renderer has instantiated so far."""
+        n = C.c_uint64(0)
+        self._check(self.lib.vb_debug_graph_captures(self.handle, C.byref(n)), "vb_debug_graph_captures")
+        return int(n.value)
+
     def set_occlusion_cull(self, on: bool):
         """fine skips the commands under a tile's last opaque full-tile cover (identical pixels). Default on."""
         self._check(self.lib.vb_set_occlusion_cull(self.handle, 1 if on else 0), "vb_set_occlusion_cull")
@@ -516,6 +538,10 @@ class RendererGroup:
 
     def set_balancing(self, on: bool):
         self._check(self.lib.vb_group_set_balancing(self.handle, 1 if on else 0), "vb_group_set_balancing")
+
+    def set_view(self, affine: Optional[Affine]):
+        """`Renderer.set_view` on every device's renderer."""
+        self._check(self.lib.vb_group_set_view(self.handle, _view_coeffs(affine)), "vb_group_set_view")
 
     def set_exchange(self, on: bool):
         """Shard `flatten` by tag range across the devices and exchange lines / path boxes through peer memory
