@@ -155,6 +155,35 @@ int vb_set_timing(vb_renderer *, int on);
 int vb_set_view(vb_renderer *, const double affine[6]);
 int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: whole-frame graphs instantiated so far */
 
+/* ---- hit testing: the topmost draw object under each point of the last frame (an addition; vello's applications hit-test on
+ * the host against their own geometry) ----
+ * For each of the n points xy[2k], xy[2k + 1] writes draw_ix[k]: the index of the LAST draw object in draw order whose path
+ * covers the point in the renderer's last frame that completed successfully, or -1.
+ *  - Points are f32 pixel coordinates of that frame: x right, y down, pixel (i, j) covers [i, i+1) x [j, j+1). In a batch
+ *    (vb_set_cells) the frame is the tall [n_cells * height, width] one: a point of cell c has y in [c * height, (c+1) * height).
+ *  - Covering is geometric and exact: the winding number of the draw's flattened outline (the frame's own lines, so a view
+ *    and flatten's tolerance are those on screen; strokes are their outlines) at the point is nonzero, or odd under the
+ *    even-odd rule, and the point lies inside the clip path of every enclosing BEGIN_CLIP (each with its own fill rule).
+ *    Brush alpha, layer alpha and blend modes do not matter: a transparent fill is hit, an image or a blurred rectangle
+ *    anywhere in the rectangle it is drawn in. A point exactly on a line is decided by the half-open rules of the tile walk
+ *    (tests/tile_walk_ref.py): deterministic, with no promise of the side.
+ *  - BEGIN_CLIP / END_CLIP objects are never returned. Points outside the frame and NaN points give -1. Indices are the
+ *    scene's draw-object indices (vb_scene_n_draw_objects / Scene.n_draw_objects; global in a batch: cell c's draws are
+ *    draw_offsets[c] .. draw_offsets[c + 1]).
+ *  - on_device == 0: host pointers; synchronous (the points go through a renderer-owned device buffer). on_device != 0: both
+ *    are pointers to memory of the renderer's device; the work is enqueued on vb_stream and the call returns (order the
+ *    points' writes before the call, and read the answers after synchronising with vb_stream).
+ *  - The answers come from the frame's buffers as its kernels left them; hit tests write nothing of the frame, launch nothing
+ *    of it and capture no graph: kernel_launches, graph captures and the next frame's pixels are the same with or without them.
+ *    vb_set_view does not change the answers: they stay those of the frame rendered last until the next frame. A frame that
+ *    was re-run after an arena overflow answers from the attempt that succeeded.
+ * n = 0: nothing happens, VB_OK. VB_E_NO_SCENE: no successful frame since the last scene upload (any form), vb_set_cells,
+ * vb_run_stages, vb_debug_upload or vb_debug_limit_arena (each rewrites something the answers read), or the last frame failed.
+ * VB_E_INVALID (vb_last_error says why): NULL pointers; device pointers of another device (on_device); the last frame had a
+ * bin_row / tile_row window; a renderer of a vb_group or with the exchange enabled; a frame enqueued and not finished
+ * (vb_render_enqueue until vb_frame_finish, vb_render_begin until vb_readback_wait). */
+int vb_hit_test(vb_renderer *, const float *xy, uint32_t n, int32_t *draw_ix, uint32_t on_device);
+
 /* The renderer-owned target of the last frame (device pointer) and its size in bytes. */
 void *vb_target(vb_renderer *, size_t *bytes);
 /* Copy `bytes` from a device pointer to a host pointer on the renderer's stream, then synchronise. */

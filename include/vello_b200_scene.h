@@ -112,6 +112,10 @@ enum { VB_FILL_NON_ZERO = 0, VB_FILL_EVEN_ODD = 1 };
 vb_scene *vb_scene_new(void);        /* Scene::new, scene.rs:54 */
 void vb_scene_free(vb_scene *);
 void vb_scene_reset(vb_scene *);     /* Scene::reset, scene.rs:59 */
+/* The draw objects encoded so far (an addition; vello has no such getter): the draw-object index the next fill, stroke,
+ * draw_image, blurred rectangle or push_*_layer receives, so a caller can note the index a call gave (read it before and after
+ * the call: a shape that encodes nothing adds no draw). These are the indices vb_hit_test returns. 0 for NULL. */
+uint32_t vb_scene_n_draw_objects(const vb_scene *);
 
 /* Scene::fill, scene.rs:316-345. brush_transform may be NULL. */
 int vb_scene_fill(vb_scene *, uint32_t fill_rule, const double transform[6], const vb_brush *, const double *brush_transform,

@@ -28,22 +28,6 @@ struct TileState {
     uint32_t cmd_offset, cmd_limit;
 };
 
-// A tile as coarse sees it. k_backdrop wrote ~(first slot of the slice) into every tile of the arena in tile order, so a
-// tile's segment count is the distance to the next tile's slice; the arena's last tile ends at bump.segments.
-struct CoTile {
-    int32_t backdrop;
-    uint32_t seg_ix, n_segs;
-};
-__device__ __forceinline__ CoTile co_load_tile(const VbTile *tiles, uint32_t ix, uint32_t tile_end, uint32_t seg_end) {
-    const VbTile t = tiles[ix];
-    const uint32_t next = ix + 1u < tile_end ? ~tiles[ix + 1u].segment_count_or_ix : seg_end;
-    CoTile c;
-    c.backdrop = t.backdrop;
-    c.seg_ix = ~t.segment_count_or_ix;
-    c.n_segs = next - c.seg_ix;
-    return c;
-}
-
 __device__ __forceinline__ void co_alloc_cmd(TileState &s, uint32_t size, const VbConfig &cfg, VbBump *bump, uint32_t *ptcl) {
     if (s.cmd_offset + size >= s.cmd_limit) {
         const uint32_t ptcl_dyn_start = cfg.width_in_tiles * cfg.tile_rows * VB_PTCL_INITIAL_ALLOC;

@@ -225,6 +225,17 @@ struct vb_renderer {
     } ring[3];
     uint64_t stream_seq = 0;
 
+    // hit testing (vb_hit_test): the config and buffers of a frame, taken when it is enqueued (hit_enq) and handed to `hit` once
+    // it is known to have succeeded. `hit` stays valid until something rewrites what the answers read: the next frame, a scene
+    // upload, vb_set_cells, vb_run_stages, vb_debug_upload or vb_debug_limit_arena.
+    struct HitFrame {
+        bool valid = false;
+        bool windowed = false; // rendered with a bin_row / tile_row window
+        VbConfig cfg{};
+        VbFrameBufs bufs{};
+    } hit, hit_enq;
+    DevBuf hit_io; // the host form's points and answers
+
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
         bool configured = false, enabled = false;
@@ -243,7 +254,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena, &r->view_coef};
+                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -267,6 +278,24 @@ static int ensure(vb_renderer *r, DevBuf &b, size_t bytes) {
     b.cap = want;
     return VB_OK;
 }
+// Hit testing's record of the frame it answers for (vb_renderer::hit).
+static void hit_forget(vb_renderer *r) {
+    r->hit.valid = false;
+    r->hit_enq.valid = false;
+}
+static void hit_enqueued(vb_renderer *r) {
+    r->hit.valid = false;
+    r->hit_enq.valid = true;
+    r->hit_enq.windowed = r->params.bin_row1 > r->params.bin_row0 || r->params.tile_row1 > r->params.tile_row0;
+    r->hit_enq.cfg = r->cfg;
+    r->hit_enq.bufs = r->bufs;
+}
+// the frame enqueued last has finished, successfully or not
+static void hit_finished(vb_renderer *r, bool ok) {
+    r->hit = r->hit_enq;
+    r->hit.valid = ok && r->hit_enq.valid;
+}
+
 // One entry per bump arena: the name vb_debug_limit_arena takes, the buffer, its element size and its VbBump counter.
 // The special cases are in arena_offset, arena_need, ensure_arena and the first guesses of prepare.
 using RendererBuf = DevBuf vb_renderer::*;
@@ -540,6 +569,7 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
     r->cur->overridden.clear(); // a caller-packed atlas: overrides do not apply
     r->cur->have_scene = true;
     r->cells.clear(); // a new scene is one cell until vb_set_cells says otherwise
+    hit_forget(r);
     return VB_OK;
 }
 
@@ -1139,7 +1169,9 @@ static int frame_launch(vb_renderer *r) {
     int rc = refresh_overrides(r);
     if (rc) return rc;
     CK(cudaEventRecord(r->frame_ev[0], r->stream));
+    hit_enqueued(r);
     rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->dest, false);
+    if (rc != VB_OK) hit_forget(r); // a frame enqueued in part
     if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
     r->frame_timed = rc == VB_OK;
     r->frame_pending = rc == VB_OK;
@@ -1151,6 +1183,7 @@ static int frame_launch(vb_renderer *r) {
 static int frame_launch_half(vb_renderer *r, int half) {
     CK(cudaSetDevice(r->device));
     if (half == 0) {
+        hit_enqueued(r);
         CK(cudaEventRecord(r->frame_ev[0], r->stream));
         return enqueue_direct(r, 0, VB_STAGE_ID_FLATTEN, r->dest, false);
     }
@@ -1206,6 +1239,7 @@ extern "C" int vb_frame_finish(vb_renderer *r, vb_frame_stats *stats) {
     CK(cudaStreamSynchronize(r->stream));
     r->frame_pending = false;
     fill_stats(r, stats);
+    hit_finished(r, r->cur->h_bump->failed == 0u);
     return r->cur->h_bump->failed ? VB_E_BUMP_OVERFLOW : VB_OK;
 }
 
@@ -1220,6 +1254,7 @@ static int render_sync(vb_renderer *r, const vb_params *p, const Dest &d, vb_fra
         CK(cudaStreamSynchronize(r->stream));
         r->frame_pending = false;
         if (r->cur->h_bump->failed == 0) break;
+        hit_finished(r, false);
         if (r->xc.enabled) {
             // every attempt of an exchanged frame is a collective step (all GPUs advance their epoch together): grow what
             // overflowed here and let the caller re-issue the frame on every GPU
@@ -1237,6 +1272,7 @@ static int render_sync(vb_renderer *r, const vb_params *p, const Dest &d, vb_fra
         r->retries++;
     }
     fill_stats(r, stats);
+    hit_finished(r, true);
     return VB_OK;
 }
 
@@ -1387,6 +1423,7 @@ extern "C" int vb_readback_wait(vb_renderer *r) {
     if (!r) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     int rc = VB_OK;
+    const bool streamed = r->stream_pending;
     const uint64_t k = r->stream_seq; // the next frame number: complete k-3 .. k-1 in order
     for (uint64_t j = k >= 3u ? k - 3u : 0u; j < k; j++) {
         const uint32_t q = (uint32_t)(j % 3u);
@@ -1397,12 +1434,15 @@ extern "C" int vb_readback_wait(vb_renderer *r) {
     }
     CK(cudaStreamSynchronize(r->copy_stream));
     r->stream_pending = false;
+    // the intermediates hold the frame enqueued last (a re-run after an overflow is enqueued anew)
+    if (streamed) hit_finished(r, rc == VB_OK);
     return rc;
 }
 
 extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int last, void *out_device) {
     if (!r || !p || first < 0 || last >= VB_N_STAGE_IDS || first > last) return VB_E_INVALID;
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
+    hit_forget(r);
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;
@@ -1478,6 +1518,7 @@ extern "C" int vb_debug_limit_arena(vb_renderer *r, const char *arena, uint32_t 
         r->err = std::string("vb_debug_limit_arena: unknown arena ") + arena;
         return VB_E_INVALID;
     }
+    hit_forget(r);
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
     CK(cudaStreamSynchronize(r->copy_stream));
@@ -1568,6 +1609,52 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
             return VB_OK;
         }
     return VB_E_UNKNOWN_BUFFER;
+}
+
+// ---- hit testing: vb_hit_test ---------------------------------------------------------------------------------------------
+// The answers read the buffers of the frame recorded in r->hit (k_hit.cu); nothing of the frame is written, launched or
+// captured, so kernel_launches, the graph key and the next frame are the same with or without hit tests in between.
+static bool device_memory_of(vb_renderer *r, const void *p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return a.type == cudaMemoryTypeManaged || (a.type == cudaMemoryTypeDevice && a.device == r->device);
+}
+extern "C" int vb_hit_test(vb_renderer *r, const float *xy, uint32_t n, int32_t *draw_ix, uint32_t on_device) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_hit_test: ") + why;
+        return VB_E_INVALID;
+    };
+    if (n == 0u) return VB_OK;
+    if (!xy || !draw_ix) return bad("NULL points or answers");
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending || r->stream_pending) return bad("a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)");
+    if (!r->hit.valid) {
+        r->err = "vb_hit_test: no successful frame since the last scene upload, vb_set_cells, vb_run_stages or vb_debug_* call";
+        return VB_E_NO_SCENE;
+    }
+    if (r->hit.windowed) return bad("the last frame had a bin_row / tile_row window");
+    CK(cudaSetDevice(r->device));
+    if (on_device) {
+        if (!device_memory_of(r, xy) || !device_memory_of(r, draw_ix)) return bad("on_device: the pointers must be memory of the renderer's device");
+        vb_launch_hit_test(r->hit.cfg, r->hit.bufs, xy, n, draw_ix, r->stream);
+        CK(cudaGetLastError());
+        return VB_OK;
+    }
+    const size_t xy_bytes = (size_t)n * 2u * sizeof(float);
+    int rc = ensure(r, r->hit_io, xy_bytes + (size_t)n * sizeof(int32_t));
+    if (rc) return rc;
+    float *d_xy = (float *)r->hit_io.p;
+    int32_t *d_ix = (int32_t *)((char *)r->hit_io.p + xy_bytes);
+    CK(cudaMemcpyAsync(d_xy, xy, xy_bytes, cudaMemcpyHostToDevice, r->stream));
+    vb_launch_hit_test(r->hit.cfg, r->hit.bufs, d_xy, n, d_ix, r->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(draw_ix, d_ix, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, r->stream));
+    CK(cudaStreamSynchronize(r->stream));
+    return VB_OK;
 }
 
 // ---- views: vb_set_view --------------------------------------------------------------------------------------------------
@@ -1661,6 +1748,7 @@ extern "C" int vb_set_cells(vb_renderer *r, const uint32_t *draw_offsets, uint32
         if (draw_offsets[c + 1] < draw_offsets[c]) return bad("offsets must not decrease");
     if (n_cells == 1u) { // the whole scene: no batch
         r->cells.clear();
+        hit_forget(r);
         return VB_OK;
     }
     std::vector<uint32_t> tags(n_draw);
@@ -1674,6 +1762,7 @@ extern "C" int vb_set_cells(vb_renderer *r, const uint32_t *draw_offsets, uint32
             depth += tags[i] == VB_DRAWTAG_BEGIN_CLIP ? 1 : tags[i] == VB_DRAWTAG_END_CLIP ? -1 : 0;
         if (depth != 0) return bad("the clips of cell " + std::to_string(c) + " do not balance");
     }
+    hit_forget(r); // cell_draw, which the answers read, is rewritten below
     if ((rc = ensure(r, r->cell_draw, ((size_t)n_cells + 1u) * 4u))) return rc;
     r->cells.assign(draw_offsets, draw_offsets + n_cells + 1u);
     // in stream order: a frame still running reads the previous offsets
@@ -1705,6 +1794,7 @@ extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint6
 
 extern "C" int vb_debug_upload(vb_renderer *r, const char *name, const void *src, size_t bytes) {
     if (!r || !name || !src) return VB_E_INVALID;
+    hit_forget(r);
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
     // "lines" and "tiles": the arena's contents and its bump counter. Growing the arena frees it without copying, and the
@@ -2329,6 +2419,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     r->cur->scene_words = total_words;
     r->cur->have_scene = true;
     r->cells.clear();
+    hit_forget(r);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }

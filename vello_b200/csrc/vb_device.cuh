@@ -187,6 +187,22 @@ __device__ __forceinline__ uint32_t vb_span(float a, float b) {
 __device__ __forceinline__ uint32_t vb_scene(const uint32_t *__restrict__ scene, const VbConfig &cfg, uint32_t ix) {
     return ix < cfg.scene_words ? __ldg(scene + ix) : 0u;
 }
+// A tile after backdrop, as coarse and hit testing read it. k_backdrop wrote ~(first slot of the slice) into every tile of the
+// arena in tile order, so a tile's segment count is the distance to the next tile's slice; the arena's last tile ends at
+// bump.segments.
+struct CoTile {
+    int32_t backdrop;
+    uint32_t seg_ix, n_segs;
+};
+__device__ __forceinline__ CoTile co_load_tile(const VbTile *tiles, uint32_t ix, uint32_t tile_end, uint32_t seg_end) {
+    const VbTile t = tiles[ix];
+    const uint32_t next = ix + 1u < tile_end ? ~tiles[ix + 1u].segment_count_or_ix : seg_end;
+    CoTile c;
+    c.backdrop = t.backdrop;
+    c.seg_ix = ~t.segment_count_or_ix;
+    c.n_segs = next - c.seg_ix;
+    return c;
+}
 // Batch: the cell of draw object `ix`, the last c with cell_draw[c] <= ix (empty cells are skipped: cell_draw[c + 1] > ix).
 __device__ __forceinline__ uint32_t vb_cell_of(const VbConfig &cfg, uint32_t ix) {
     uint32_t lo = 0u, hi = cfg.n_cells; // cell_draw[lo] <= ix < cell_draw[hi]

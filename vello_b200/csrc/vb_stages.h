@@ -108,6 +108,10 @@ uint32_t vb_launch_exchange_recv(const VbConfig &cfg, const VbFrameBufs &b, cons
 void vb_launch_view_set(float *dst, const float m[6], cudaStream_t st);
 uint32_t vb_launch_view_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// hit testing (k_hit.cu): for n points xy (interleaved f32 pairs, device memory) the last draw object covering each of them
+// in the finished frame `cfg` / `b` describe, or -1 (vb_hit_test); reads the frame's buffers and writes only draw_ix
+uint32_t vb_launch_hit_test(const VbConfig &cfg, const VbFrameBufs &b, const float *xy, uint32_t n, int32_t *draw_ix, cudaStream_t st);
+
 // device resolve (vb_scene_upload_streams)
 void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes, uint32_t end_clip_word0,
                               const RsPatch *patches, uint32_t n_patches, cudaStream_t st);

@@ -645,6 +645,13 @@ class Scene:
     def __init__(self):
         self.encoding = Encoding()
 
+    @property
+    def n_draw_objects(self) -> int:
+        """The draw objects encoded so far: the draw-object index the next fill, stroke, draw_image, blurred rectangle or
+        push_*_layer receives (read it before and after a call to note the index that call gave; a shape that encodes nothing
+        adds no draw). `Renderer.hit_test` answers with these indices."""
+        return len(self.encoding.draw_tags)
+
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
         e = self.encoding
         e.encode_transform(transform)

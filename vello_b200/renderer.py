@@ -134,6 +134,7 @@ def load_library() -> C.CDLL:
     lib.vb_set_view.argtypes = [vp, C.POINTER(C.c_double)]
     lib.vb_group_set_view.argtypes = [vp, C.POINTER(C.c_double)]
     lib.vb_debug_graph_captures.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.vb_hit_test.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
     _lib = lib
     return lib
 
@@ -146,7 +147,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
-                    "vb_debug_graph_captures"]
+                    "vb_debug_graph_captures", "vb_hit_test"]
 
 
 def _device_image(t):
@@ -162,6 +163,22 @@ def _device_image(t):
     if tuple(strides[1:]) != (4, 1) or strides[0] % 4:
         raise ValueError(f"a device image has texel strides (4, 1) and a row stride that is a multiple of 4, not {tuple(strides)}")
     return int(cai["data"][0]), shape[0], shape[1], int(strides[0])
+
+
+def _device_vector(t, width, typestrs, what):
+    """(pointer, rows) of a contiguous (rows, width) -- or (rows,) for width 1 -- device array from its
+    `__cuda_array_interface__`."""
+    cai = t.__cuda_array_interface__
+    shape = tuple(int(v) for v in cai["shape"])
+    want = 2 if width > 1 else 1
+    if len(shape) != want or (width > 1 and shape[1] != width) or cai["typestr"] not in typestrs:
+        raise ValueError(f"hit_test: {what} must be {'(n, %d)' % width if width > 1 else '(n,)'} {typestrs[0]}, "
+                         f"not {shape} {cai['typestr']}")
+    item = int(cai["typestr"][2:])
+    strides = cai.get("strides")
+    if strides is not None and tuple(strides) != ((width * item, item) if width > 1 else (item,)) and shape[0] > 1:
+        raise ValueError(f"hit_test: {what} must be contiguous, not strides {tuple(strides)}")
+    return int(cai["data"][0]), shape[0]
 
 
 @dataclass
@@ -470,6 +487,37 @@ class Renderer:
         without uploading it again (pan / zoom of a resident scene). Frames already enqueued keep their view; the view
         survives uploads. Flatten then culls what lies above, below or right of the frame. None clears it."""
         self._check(self.lib.vb_set_view(self.handle, _view_coeffs(affine)), "vb_set_view")
+
+    def hit_test(self, points, out=None):
+        """The topmost draw object under each point of the last frame that completed (`vb_hit_test`): for every (x, y) in
+        pixel coordinates of that frame (a batch's tall [N * H, W] frame), the index of the last draw object in draw order
+        whose outline covers the point inside all its enclosing clips (`Scene.n_draw_objects` tells which index a call got),
+        or -1. Alpha and blend modes do not matter; clips are never returned; points outside the frame and NaN give -1.
+
+        A numpy (n, 2) float32 array (or anything numpy turns into one) returns a numpy int32 (n,) array (into `out` when it
+        is one), synchronously. A device array (`__cuda_array_interface__`, e.g. a torch CUDA tensor) of n x 2 float32 needs
+        `out`, a device int32 array of n: the work is enqueued on `self.stream` and `out` is returned at once (order the
+        points' writes before the call and synchronise with that stream before reading `out`)."""
+        if hasattr(points, "__cuda_array_interface__"):
+            ptr, n = _device_vector(points, 2, ("<f4",), "points")
+            if out is None or not hasattr(out, "__cuda_array_interface__"):
+                raise ValueError("hit_test: device points need a device int32 array `out`")
+            optr, m = _device_vector(out, 1, ("<i4",), "out")
+            if m != n:
+                raise ValueError(f"hit_test: out holds {m} answers for {n} points")
+            self._check(self.lib.vb_hit_test(self.handle, C.c_void_p(ptr), n, C.c_void_p(optr), 1), "vb_hit_test")
+            return out
+        pts = np.ascontiguousarray(points, dtype=np.float32)
+        if pts.ndim != 2 or pts.shape[1] != 2:
+            raise ValueError(f"hit_test: points must be (n, 2), not {pts.shape}")
+        n = pts.shape[0]
+        if out is None:
+            out = np.empty(n, dtype=np.int32)
+        elif not (isinstance(out, np.ndarray) and out.dtype == np.int32 and out.shape == (n,) and out.flags.c_contiguous):
+            raise ValueError(f"hit_test: out must be a contiguous int32 numpy array of shape ({n},)")
+        if n:
+            self._check(self.lib.vb_hit_test(self.handle, pts.ctypes.data, n, out.ctypes.data, 0), "vb_hit_test")
+        return out
 
     def debug_graph_captures(self) -> int:
         """Test-only: whole-frame CUDA graphs this renderer has instantiated so far."""
