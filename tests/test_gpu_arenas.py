@@ -220,6 +220,70 @@ def test_cascade_retry_budget(packed, oracle):
     r.close()
 
 
+def test_cascade_retry_budget_streamed(packed, oracle):
+    """render_stream under the same budget: the frame that meets every limit reports its len(CASCADE) re-runs (the frame
+    enqueued behind it, which overflowed too, one); with one re-run fewer the stream fails, and the same renderer then
+    renders the next frame exactly."""
+    from vello_b200.renderer import VelloB200Error
+    ref = oracle.render(packed, W, H, BLACK.premul_rgba8_u32(), AA_MSAA16)
+    r, p, _ = ample(packed, AA_MSAA16, max_retries=len(CASCADE))
+    limit_all(r)
+    retries = []
+    for img in r.render_stream([packed] * 4, p):
+        assert np.array_equal(img, ref)
+        retries.append(int(r.last_stats.retries))  # frame len(retries) - 1, for all but the last two frames
+    assert retries[:2] == [len(CASCADE), 1]
+    r.close()
+    r, p, _ = ample(packed, AA_MSAA16, max_retries=len(CASCADE) - 1)
+    limit_all(r)
+    with pytest.raises(VelloB200Error, match="bump arena overflow") as e:
+        list(r.render_stream([packed] * 4, p))
+    assert "[bump overflow persisted]" in str(e.value)
+    assert np.array_equal(r.render_to_texture(packed, p), ref)
+    r.close()
+
+
+@pytest.mark.parametrize("exchange", [False, True])
+def test_cascade_retry_budget_in_a_group(packed, oracle, exchange):
+    """RendererGroup([0] * 3) with every arena of renderer 1 limited: renderer 1 re-runs its stripe alone (exchange off) or
+    every renderer re-issues the frame (exchange on, where the sharded flatten may change the cascade), N times in all.
+    With max_retries = N the frame is exact and reports N; with N - 1 it fails, and the group then renders the next frame
+    exactly."""
+    from vello_b200.renderer import RendererGroup, RendererOptions, VelloB200Error
+    ref = oracle.render(packed, W, H, BLACK.premul_rgba8_u32(), AA_MSAA16)
+    p = RenderParams(BLACK, W, H, AA_MSAA16)
+
+    def limited_group(max_retries):
+        g = RendererGroup([0] * 3, RendererOptions(max_retries=max_retries))
+        g.set_balancing(False)  # the same stripes every frame: renderer 1's arenas hold its next frame
+        g.set_exchange(exchange)
+        for attempt in range(3):  # a small max_retries may need more than one call to grow from the first guesses
+            try:
+                g.render_to_texture(packed, p)
+                break
+            except VelloB200Error:
+                assert attempt < 2
+        limit_all(g.renderer(1))
+        return g
+
+    g = limited_group(16)
+    assert np.array_equal(g.render_to_texture(packed, p), ref)
+    n = int(g.last_stats[1].retries)
+    want = [n] * 3 if exchange else [0, n, 0]
+    assert [int(s.retries) for s in g.last_stats] == want
+    assert n == len(CASCADE) or (exchange and n >= 2), n
+    g.close()
+    g = limited_group(n)
+    assert np.array_equal(g.render_to_texture(packed, p), ref)
+    assert [int(s.retries) for s in g.last_stats] == want
+    g.close()
+    g = limited_group(n - 1)
+    with pytest.raises(VelloB200Error, match="bump arena overflow"):
+        g.render_to_texture(packed, p)
+    assert np.array_equal(g.render_to_texture(packed, p), ref)
+    g.close()
+
+
 # ---- the other entry points, for one early arena (lines: flatten) and one late one (ptcl: coarse) -----------------------
 ENTRY_ARENAS = ["lines", "ptcl"]
 
@@ -266,6 +330,8 @@ def test_one_overflow_with_and_without_graphs(packed, oracle, arena, graph):
     r.limit_arena(arena, need[arena] - 1)
     assert r.render_resident(p).retries == 1
     assert np.array_equal(r.download_target(p), ref)
+    r.enqueue(p)  # an enqueued frame reports no re-runs, whatever the frame before it needed
+    assert r.finish().retries == 0
     assert r.render_resident(p).retries == 0
     assert np.array_equal(r.download_target(p), ref)
     r.close()
@@ -275,11 +341,12 @@ def test_one_overflow_with_and_without_graphs(packed, oracle, arena, graph):
 @pytest.mark.parametrize("younger_overflows", [False, True])
 def test_one_overflow_while_streaming(packed, arena, younger_overflows):
     """render_stream with the limit set before frame k. The frame enqueued behind it either fits (only k is re-run) or
-    overflows too (both are re-run). Either way every frame arrives, in order, equal to the blocking frame."""
+    overflows too (both are re-run). Either way every frame arrives, in order, equal to the blocking frame, and a re-run
+    frame reports its one re-run."""
     from vello_b200.renderer import Renderer
     light = resolve(scenes.paris_like(150, 512, seed=12).encoding)
     k = 3
-    seq = [packed, light, packed, packed, packed if younger_overflows else light, packed]
+    seq = [packed, light, packed, packed, packed if younger_overflows else light, packed, light]
     p = RenderParams(BLACK, W, H, AA_MSAA16)
     r = Renderer()
     want, need = [], {}
@@ -288,14 +355,16 @@ def test_one_overflow_while_streaming(packed, arena, younger_overflows):
         need[id(s)] = stats_need(r.last_stats)
     limit = need[id(packed)][arena] - 1
     assert (need[id(seq[k + 1])][arena] > limit) == younger_overflows
-    got = []
+    got, retries = [], []
     for img in r.render_stream(seq, p):
         got.append(img.copy())
+        retries.append(int(r.last_stats.retries))  # frame len(got) - 1, for all but the last two frames
         if len(got) == k - 2:  # vb_render_begin(k - 1) has returned; frame k is the next one submitted
             r.limit_arena(arena, limit)
     assert len(got) == len(want)
     for i, (a, b) in enumerate(zip(got, want)):
         assert np.array_equal(a, b), i
+    assert retries[:len(seq) - 2] == [0, 0, 0, 1, 1 if younger_overflows else 0]
     assert np.array_equal(r.render_to_texture(packed, p), want[0])
     assert r.last_stats.retries == 0
     r.close()
@@ -317,8 +386,8 @@ def test_one_overflow_in_a_group(packed, oracle, arena, exchange):
     need = stats_need(g.last_stats[1])
     g.renderer(1).limit_arena(arena, need[arena] - 1)
     assert np.array_equal(g.render_to_texture(packed, p), ref)
-    if not exchange:
-        assert [int(s.retries) for s in g.last_stats] == [0, 1, 0]
+    # with the exchange on, every renderer re-issues the frame
+    assert [int(s.retries) for s in g.last_stats] == ([1, 1, 1] if exchange else [0, 1, 0])
     assert np.array_equal(g.render_to_texture(packed, p), ref)
     assert all(int(s.retries) == 0 and int(s.failed) == 0 for s in g.last_stats)
     g.close()

@@ -123,6 +123,15 @@ struct View {
     float m[6] = {};
 };
 
+// Everything a frame needs to be issued again (issue): a re-run renders under the view and from the scene slot the frame
+// was first issued with, even if the renderer's have changed since.
+struct Frame {
+    vb_params params{};
+    Dest dest;
+    View view;
+    uint32_t slot = 0;
+};
+
 struct vb_renderer {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -186,7 +195,7 @@ struct vb_renderer {
     VbConfig cfg{};
     vb_params params{};
     Dest dest; // of the frame frame_prepare set up
-    uint32_t retries = 0, launches = 0;
+    uint32_t launches = 0;
     VbFrameBufs bufs{};           // the buffers of the frame prepare set up, as the launchers take them
     bool use_graph = true;        // replay whole frames as CUDA graphs (see enqueue)
     GraphSlot graphs[4];
@@ -217,10 +226,7 @@ struct vb_renderer {
     cudaEvent_t upload_done[2]{}, raster_done[2]{};
     struct RingFrame { // a streamed frame between vb_render_begin and its completion on the host
         bool pending = false, raster_checked = false;
-        vb_params params{};
-        View view; // the view it was enqueued with (a re-run renders under it again)
-        void *out_host = nullptr;
-        uint32_t slot = 0;
+        Frame frame;
         vb_frame_stats stats{};
     } ring[3];
     uint64_t stream_seq = 0;
@@ -1164,53 +1170,63 @@ static int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
     r->dest = d;
     return pick_out(r, &r->dest);
 }
-static int frame_launch(vb_renderer *r) {
+// Enqueue stages first..last of the frame frame_prepare set up. A range from stage 0 starts the frame: the dirty overridden
+// images are copied and the hit record and the frame's first event are taken. A range after stage 0 continues the frame and
+// adds to its launches. A range that ends at fine completes it: the frame's last event, and the frame is pending.
+static int launch(vb_renderer *r, int first, int last) {
     CK(cudaSetDevice(r->device));
-    int rc = refresh_overrides(r);
-    if (rc) return rc;
-    CK(cudaEventRecord(r->frame_ev[0], r->stream));
-    hit_enqueued(r);
-    rc = enqueue(r, 0, VB_N_STAGE_IDS - 1, r->dest, false);
-    if (rc != VB_OK) hit_forget(r); // a frame enqueued in part
-    if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
-    r->frame_timed = rc == VB_OK;
-    r->frame_pending = rc == VB_OK;
-    return rc;
-}
-
-// The same frame in two submissions (plain launches): up to and including flatten + the sending half of the exchange, then
-// the rest. Used by vb_group when renderers share a device, see k_exchange.cu.
-static int frame_launch_half(vb_renderer *r, int half) {
-    CK(cudaSetDevice(r->device));
-    if (half == 0) {
-        hit_enqueued(r);
+    const uint32_t before = r->launches;
+    int rc;
+    if (first == 0) {
+        if ((rc = refresh_overrides(r))) return rc;
         CK(cudaEventRecord(r->frame_ev[0], r->stream));
-        return enqueue_direct(r, 0, VB_STAGE_ID_FLATTEN, r->dest, false);
+        hit_enqueued(r);
     }
-    uint32_t first_half = r->launches;
-    int rc = enqueue_direct(r, VB_STAGE_ID_DRAW, VB_N_STAGE_IDS - 1, r->dest, false);
-    r->launches += first_half;
-    // (with a host destination enqueue_direct queues the read-back behind fine itself)
-    if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
-    r->frame_timed = rc == VB_OK;
-    r->frame_pending = rc == VB_OK;
+    rc = enqueue(r, first, last, r->dest, false);
+    if (first != 0) r->launches += before;
+    if (rc != VB_OK) hit_forget(r); // a frame enqueued in part
+    if (last == VB_N_STAGE_IDS - 1) {
+        if (rc == VB_OK) CK(cudaEventRecord(r->frame_ev[1], r->stream));
+        r->frame_timed = rc == VB_OK;
+        r->frame_pending = rc == VB_OK;
+    }
     return rc;
 }
 
-static int render_enqueue(vb_renderer *r, const vb_params *p, const Dest &d) {
-    int rc = frame_prepare(r, p, d);
-    if (rc) return rc;
-    return frame_launch(r);
-}
-extern "C" int vb_render_enqueue(vb_renderer *r, const vb_params *p, void *out_device) {
-    return render_enqueue(r, p, Dest{out_device});
+// A frame of the renderer's current scene slot, under its current view.
+static Frame frame_of(const vb_renderer *r, const vb_params *p, const Dest &d) {
+    return Frame{*p, d, r->view, (uint32_t)(r->cur - r->slot)};
 }
 
-static void fill_stats(vb_renderer *r, vb_frame_stats *s) {
+static int put_view(vb_renderer *r, const View &v);
+static bool same_view(const View &a, const View &b) { return a.on == b.on && (!a.on || memcmp(a.m, b.m, sizeof a.m) == 0); }
+// Enqueue frame f from its scene slot and under its view; the renderer's current slot and view are restored afterwards.
+static int issue(vb_renderer *r, const Frame &f) {
+    vb_renderer::SceneSlot *const keep = r->cur;
+    const View now = r->view;
+    const bool other = !same_view(now, f.view);
+    r->cur = &r->slot[f.slot];
+    int rc = other ? put_view(r, f.view) : VB_OK;
+    if (rc == VB_OK) rc = frame_prepare(r, &f.params, f.dest);
+    if (rc == VB_OK) rc = launch(r, 0, VB_N_STAGE_IDS - 1);
+    if (other) {
+        const int rc2 = put_view(r, now);
+        if (rc == VB_OK) rc = rc2;
+    }
+    r->cur = keep;
+    return rc;
+}
+
+extern "C" int vb_render_enqueue(vb_renderer *r, const vb_params *p, void *out_device) {
+    if (!r || !p) return VB_E_INVALID;
+    return issue(r, frame_of(r, p, Dest{out_device}));
+}
+
+static void fill_stats(vb_renderer *r, vb_frame_stats *s, uint32_t retries) {
     if (!s) return;
     memset(s, 0, sizeof *s);
     memcpy(s, r->cur->h_bump, sizeof(VbBump));
-    s->retries = r->retries;
+    s->retries = retries;
     s->kernel_launches = r->launches;
     for_each_buf(r, [&](DevBuf &b) { s->arena_bytes += b.cap; });
     if (r->timing) {
@@ -1238,69 +1254,73 @@ extern "C" int vb_frame_finish(vb_renderer *r, vb_frame_stats *stats) {
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
     r->frame_pending = false;
-    fill_stats(r, stats);
+    fill_stats(r, stats, 0u); // an enqueued frame is not re-run
     hit_finished(r, r->cur->h_bump->failed == 0u);
     return r->cur->h_bump->failed ? VB_E_BUMP_OVERFLOW : VB_OK;
 }
 
-// One frame, re-run with grown arenas until it fits. Streamed frames still in flight are left alone: the streaming calls
-// re-run their own frames through here.
-static int render_sync(vb_renderer *r, const vb_params *p, const Dest &d, vb_frame_stats *stats) {
-    if (!r->cur->have_scene) return VB_E_NO_SCENE;
-    r->retries = 0;
-    for (uint32_t attempt = 0;; attempt++) {
-        int rc = render_enqueue(r, p, d);
-        if (rc) return rc;
-        CK(cudaStreamSynchronize(r->stream));
-        r->frame_pending = false;
-        if (r->cur->h_bump->failed == 0) break;
+// Wait for frame f, issued last, and for its read-back when it has a host destination.
+static int finish(vb_renderer *r, const Frame &f) {
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream));
+    r->frame_pending = false;
+    // the band copies were queued behind the fine bands; a re-run after an arena overflow simply copies again
+    if (f.dest.host) CK(cudaStreamSynchronize(r->copy_stream));
+    return VB_OK;
+}
+// Issue frame f and wait for it (for the band copies of a frame enqueued in part too).
+static int run(vb_renderer *r, const Frame &f) {
+    const int rc = issue(r, f);
+    const int rc2 = finish(r, f);
+    return rc ? rc : rc2;
+}
+
+// The grow-and-re-run loop of every entry point. Frame f has finished an attempt (r->cur is its scene slot); while the
+// attempt overflowed, grow the arenas and run f again, at most max_retries times. Then report f in *stats.
+static int settle(vb_renderer *r, const Frame &f, vb_frame_stats *stats) {
+    uint32_t retries = 0;
+    while (r->cur->h_bump->failed != 0u) {
         hit_finished(r, false);
         if (r->xc.enabled) {
             // every attempt of an exchanged frame is a collective step (all GPUs advance their epoch together): grow what
             // overflowed here and let the caller re-issue the frame on every GPU
             grow_arenas(r);
-            fill_stats(r, stats);
+            fill_stats(r, stats, retries);
             r->err = "bump overflow in an exchanged frame: re-issue the frame on every GPU";
             return VB_E_BUMP_OVERFLOW;
         }
-        if (attempt >= r->max_retries) {
-            fill_stats(r, stats);
+        if (retries >= r->max_retries) {
+            fill_stats(r, stats, retries);
             r->err = "bump overflow persisted";
             return VB_E_BUMP_OVERFLOW;
         }
         grow_arenas(r);
-        r->retries++;
+        retries++;
+        const int rc = run(r, f);
+        if (rc) return rc;
     }
-    fill_stats(r, stats);
+    fill_stats(r, stats, retries);
     hit_finished(r, true);
     return VB_OK;
 }
 
-// render_sync with a host destination, then wait for its copies
-static int render_sync_host(vb_renderer *r, const vb_params *p, const Dest &d, vb_frame_stats *stats) {
-    int rc = render_sync(r, p, d, stats);
-    // the band copies were queued behind the fine bands; a re-run after an arena overflow simply copies again
-    cudaError_t e = cudaStreamSynchronize(r->copy_stream);
-    if (rc == VB_OK && e != cudaSuccess) {
-        r->err = std::string("copy stream: ") + cudaGetErrorString(e);
-        return VB_E_CUDA;
-    }
-    return rc;
+// One frame, after the streamed frames still in flight, re-run with grown arenas until it fits.
+static int render_sync(vb_renderer *r, const vb_params *p, const Dest &d, vb_frame_stats *stats) {
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    const Frame f = frame_of(r, p, d);
+    rc = run(r, f);
+    return rc ? rc : settle(r, f, stats);
 }
 
 extern "C" int vb_render_resident(vb_renderer *r, const vb_params *p, void *out_device, vb_frame_stats *stats) {
     if (!r || !p) return VB_E_INVALID;
-    int rc = drain_stream(r);
-    if (rc) return rc;
     return render_sync(r, p, Dest{out_device}, stats);
 }
 
 extern "C" int vb_render_uploaded(vb_renderer *r, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {
     if (!r || !p || !out) return VB_E_INVALID;
-    if (out_is_device) return vb_render_resident(r, p, out, stats);
-    int rc = drain_stream(r);
-    if (rc) return rc;
-    return render_sync_host(r, p, Dest{nullptr, out, false, r->readback_bands}, stats);
+    return render_sync(r, p, out_is_device ? Dest{out} : Dest{nullptr, out, false, r->readback_bands}, stats);
 }
 
 extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
@@ -1321,22 +1341,6 @@ extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len,
 // out_host and `stats` describes frame k-2 (zeros while there is none); vb_readback_wait completes the rest. THREE alternating
 // out_host buffers are needed. An arena overflow is found at the rasterisation check; that frame (and the one enqueued behind
 // it) is then re-run synchronously with grown arenas -- rare (first frames of a new scene size) and exact.
-static int put_view(vb_renderer *r, const View &v);
-static bool same_view(const View &a, const View &b) { return a.on == b.on && (!a.on || memcmp(a.m, b.m, sizeof a.m) == 0); }
-static int rerun_frame_sync(vb_renderer *r, uint32_t q, vb_frame_stats *stats) {
-    const uint32_t slot = r->ring[q].slot;
-    r->cur = &r->slot[slot];
-    // under the view the frame was enqueued with, even if it has changed since
-    const View now = r->view;
-    const bool other = !same_view(now, r->ring[q].view);
-    int rc = other ? put_view(r, r->ring[q].view) : VB_OK;
-    if (rc == VB_OK) rc = render_sync_host(r, &r->ring[q].params, Dest{nullptr, r->ring[q].out_host, slot != 0u, 1u}, stats);
-    if (other) {
-        const int rc2 = put_view(r, now);
-        if (rc == VB_OK) rc = rc2;
-    }
-    return rc;
-}
 
 // Frame in ring entry q: wait for its kernels, look at its bump counters, re-run on overflow (together with the younger frame
 // enqueued behind it, ring entry `younger`, or -1).
@@ -1344,26 +1348,26 @@ static int check_raster(vb_renderer *r, uint32_t q, int younger) {
     vb_renderer::RingFrame &f = r->ring[q];
     if (!f.pending || f.raster_checked) return VB_OK;
     vb_renderer::SceneSlot *const keep = r->cur;
-    CK(cudaEventSynchronize(r->raster_done[f.slot]));
-    r->cur = &r->slot[f.slot];
+    CK(cudaEventSynchronize(r->raster_done[f.frame.slot]));
+    r->cur = &r->slot[f.frame.slot];
     int rc = VB_OK;
     if (r->cur->h_bump->failed != 0u) {
         CK(cudaStreamSynchronize(r->stream));
         CK(cudaStreamSynchronize(r->copy_stream));
-        grow_arenas(r);
-        rc = rerun_frame_sync(r, q, &f.stats);
+        rc = settle(r, f.frame, &f.stats);
         CK(cudaEventRecord(r->copy_done[q], r->copy_stream));
-        if (rc == VB_OK && younger >= 0 && r->ring[younger].pending) {
-            r->cur = &r->slot[r->ring[younger].slot];
+        vb_renderer::RingFrame *const y = younger >= 0 ? &r->ring[younger] : nullptr;
+        if (rc == VB_OK && y && y->pending) {
+            r->cur = &r->slot[y->frame.slot];
             if (r->cur->h_bump->failed != 0u) {
-                rc = rerun_frame_sync(r, (uint32_t)younger, &r->ring[younger].stats);
-                CK(cudaEventRecord(r->raster_done[r->ring[younger].slot], r->stream));
+                rc = settle(r, y->frame, &y->stats);
+                CK(cudaEventRecord(r->raster_done[y->frame.slot], r->stream));
                 CK(cudaEventRecord(r->copy_done[younger], r->copy_stream));
+                y->raster_checked = true; // its stats are the re-run's
             }
         }
     } else {
-        r->retries = 0;
-        fill_stats(r, &f.stats);
+        fill_stats(r, &f.stats, 0u);
     }
     f.raster_checked = true;
     r->cur = keep;
@@ -1396,17 +1400,15 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
     CK(cudaStreamWaitEvent(r->stream, r->upload_done[slot], 0));
     if (k >= 2u && r->ring[q2].pending) CK(cudaStreamWaitEvent(r->stream, r->copy_done[q2], 0)); // its read-back still reads this target
     // one band: the whole read-back overlaps the next frames, no reason to split fine
-    rc = render_enqueue(r, p, Dest{nullptr, out_host, slot != 0u, 1u});
+    const Frame f = frame_of(r, p, Dest{nullptr, out_host, slot != 0u, 1u});
+    rc = issue(r, f);
     if (rc) return rc;
     r->frame_pending = false;
     CK(cudaEventRecord(r->raster_done[slot], r->stream));
     CK(cudaEventRecord(r->copy_done[q], r->copy_stream));
     r->ring[q].pending = true;
     r->ring[q].raster_checked = false;
-    r->ring[q].params = *p;
-    r->ring[q].view = r->view;
-    r->ring[q].out_host = out_host;
-    r->ring[q].slot = slot;
+    r->ring[q].frame = f;
     memset(&r->ring[q].stats, 0, sizeof(vb_frame_stats));
     r->stream_seq = k + 1u;
     r->stream_pending = true;
@@ -2169,21 +2171,24 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
         frame = g->frame;
     }
     // enqueue every device's stripe, then complete them (one host thread; the devices run side by side)
-    std::vector<vb_params> ps(n, *p);
     // device destination: straight into the frame on devices[0] when peer-mapped; otherwise (and for a host destination) the
     // renderer's own target. Without the exchange a host destination's stripe is copied by the frame itself, on the
     // renderer's copy stream.
-    auto dest_of = [&](size_t i) {
-        const size_t row0 = (size_t)g->bounds[i] * 16u;
-        Dest d;
-        if (!host_out && g->peer_ok[i]) d.dev = (char *)frame + row0 * pitch;
-        if (host_out && !g->exchange) d.host = (char *)host_out + row0 * pitch;
-        return d;
-    };
+    std::vector<Frame> fs;
+    for (size_t i = 0; i < n; i++) {
+        Frame f = frame_of(g->subs[i], p, Dest{});
+        f.params.tile_row0 = g->bounds[i];
+        f.params.tile_row1 = g->bounds[i + 1];
+        if (!host_out && g->peer_ok[i]) f.dest.dev = (char *)frame + (size_t)g->bounds[i] * 16u * pitch;
+        if (host_out && !g->exchange) f.dest.host = (char *)host_out + (size_t)g->bounds[i] * 16u * pitch;
+        fs.push_back(f);
+    }
     int result = VB_OK;
     for (uint32_t attempt = 0;; attempt++) {
         if (g->exchange)
             for (vb_renderer *r : g->subs) vb_exchange_set_bounds(r, g->bounds.data());
+        // renderers that share a device (tests) launch the frame in two submissions: up to and including flatten + the
+        // sending half of the exchange, then the rest (see k_exchange.cu)
         const bool halves = g->exchange && g->shared_device;
         // phases: 0 = configs and arenas of every renderer, 1 (and 2) = the launches, last = the read-backs of a host
         // destination. A copy into pageable host memory blocks the host until it is done, so it must not be issued before
@@ -2193,13 +2198,12 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
         for (int phase = 0; phase < 1 + n_launch + (late_copy ? 1 : 0); phase++) {
             for (size_t i = 0; i < n; i++) {
                 vb_renderer *r = g->subs[i];
-                ps[i].tile_row0 = g->bounds[i];
-                ps[i].tile_row1 = g->bounds[i + 1];
-                if (ps[i].tile_row1 <= ps[i].tile_row0) continue; // more devices than tile rows (never with the exchange on)
+                if (g->bounds[i + 1] <= g->bounds[i]) continue; // more devices than tile rows (never with the exchange on)
                 const size_t row0 = (size_t)g->bounds[i] * 16u;
                 int rc = VB_OK;
-                if (phase == 0) rc = frame_prepare(r, &ps[i], dest_of(i));
-                else if (phase <= n_launch) rc = halves ? frame_launch_half(r, phase - 1) : frame_launch(r);
+                if (phase == 0) rc = frame_prepare(r, &fs[i].params, fs[i].dest);
+                else if (phase <= n_launch)
+                    rc = launch(r, phase == 2 ? VB_STAGE_ID_DRAW : 0, halves && phase == 1 ? VB_STAGE_ID_FLATTEN : VB_N_STAGE_IDS - 1);
                 else {
                     const size_t h1 = std::min<size_t>((size_t)g->bounds[i + 1] * 16u, p->height);
                     cudaSetDevice(r->device);
@@ -2216,30 +2220,21 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
         bool redo = false;
         for (size_t i = 0; i < n; i++) {
             vb_renderer *r = g->subs[i];
-            if (ps[i].tile_row1 <= ps[i].tile_row0) {
+            if (g->bounds[i + 1] <= g->bounds[i]) {
                 if (stats) memset(&stats[i], 0, sizeof(vb_frame_stats));
                 continue;
             }
             const size_t row0 = (size_t)g->bounds[i] * 16u;
-            int rc = vb_frame_finish(r, stats ? &stats[i] : nullptr);
-            if (rc == VB_E_BUMP_OVERFLOW) {
-                if (g->exchange) { // an exchanged frame is re-issued on EVERY device (epochs advance together)
-                    grow_arenas(r);
-                    redo = true;
-                    rc = VB_OK;
-                } else {
-                    // grow and re-run (first frames); with a host destination the re-run queues its read-back again.
-                    // Growing first: the same attempt with the same arenas would only overflow again.
-                    grow_arenas(r);
-                    rc = render_sync(r, &ps[i], dest_of(i), stats ? &stats[i] : nullptr);
-                    if (stats) stats[i].retries += 1;
-                }
+            // a stripe that overflowed is re-run by its renderer alone (first frames); with the exchange on, settle only grows
+            // the arenas and the frame is re-issued on EVERY device (epochs advance together)
+            int rc = finish(r, fs[i]);
+            if (rc == VB_OK) rc = settle(r, fs[i], stats ? &stats[i] : nullptr);
+            if (rc == VB_E_BUMP_OVERFLOW && g->exchange) {
+                redo = true;
+                rc = VB_OK;
             }
+            if (stats) stats[i].retries += attempt; // the re-issues of an exchanged frame
             g->ms[i] = vb_last_frame_ms(r);
-            if (rc == VB_OK && host_out && !late_copy) {
-                cudaSetDevice(r->device);
-                if (cudaStreamSynchronize(r->copy_stream) != cudaSuccess) rc = VB_E_CUDA;
-            }
             if (rc == VB_OK && !host_out && !g->peer_ok[i]) {
                 // no peer mapping between these two devices: stage through the renderer's own target
                 const size_t h0 = row0, h1 = std::min<size_t>((size_t)g->bounds[i + 1] * 16u, p->height);
@@ -2254,7 +2249,7 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
             }
         }
         if (!redo || result != VB_OK) break;
-        if (attempt >= 8u) {
+        if (attempt >= g->subs[0]->max_retries) {
             g->err = "bump overflow persisted in an exchanged frame; failed bits per renderer:";
             for (vb_renderer *q : g->subs) g->err += " 0x" + std::to_string(q->cur->h_bump->failed);
             return VB_E_BUMP_OVERFLOW;
