@@ -322,6 +322,49 @@ int vb_override_image(vb_renderer *, const void *key, uint32_t width, uint32_t h
 /* Recopy the overridden image `key` before the next frame that renders from this renderer's atlas. VB_E_INVALID: no override. */
 int vb_mark_override_image_dirty(vb_renderer *, const void *key);
 
+/* ---- composition: frames built on the device from resident fragments (an addition; vello builds every frame on the host as
+ * Scene::new() + scene.append(&fragment, Some(transform)) per fragment, vello/src/scene.rs:464-469, encoding.rs:94-174) ----
+ * vb_fragment_upload copies a fragment's streams (the vb_encoding_streams of vb_scene_upload_streams) into one renderer-owned
+ * device allocation, together with the host pixels of its images (one copy per key, as the device resolve keys them: the
+ * `pixels` pointer and the size) and its gradient stops. Synchronous; the caller's memory is not needed afterwards, so a key's
+ * address may later hold other pixels: images of different fragments share an atlas slot only when their pointer, size AND
+ * pixels (a 64-bit hash taken at upload) agree. Registered texture keys are never read (their pixels exist only in device
+ * memory) and NULL keys give a zero region, as in a resolve; both are one image per pointer.
+ * *fragment_out receives its id; ids are never reused.
+ * vb_fragment_free returns at once: the fragment's id is invalid from then on, and its memory is released once the work
+ * already enqueued that reads it has finished (checked at the next vb_fragment_* / vb_compose call). A composed scene is a
+ * copy: it does not change.
+ * vb_compose makes the renderer's current scene exactly
+ *     s = Scene::new(); for k: s.append(&fragment[inst[k].fragment], inst[k].has_transform ? Some(T_k) : None); resolve(s)
+ * without reading stream, stop or pixel data from the host: the packed scene, the Layout (*layout_out, optional), the ramps
+ * and the atlas are byte-identical to vb_scene_append + vb_scene_resolve of those scenes (ramp de-duplication by (stops,
+ * interpolation space) across fragments, one atlas slot per image key in first-seen order, the trailing PATH / END_CLIP tags
+ * of open clips, the f32 transform product of Encoding::append). transform = kurbo Affine [a b c d e f], converted to f32
+ * like Transform::from_kurbo. draw_offsets (n + 1 entries, or NULL): draw_offsets[k] = the draw-object index of instance k's
+ * first draw, draw_offsets[n] = the total before the trailing END_CLIPs; a vb_hit_test answer i belongs to the instance k
+ * with draw_offsets[k] <= i < draw_offsets[k + 1].
+ *  - Afterwards the renderer is as after any scene upload: frames render the composed scene, a view applies on top, vb_set_cells
+ *    may split it, vb_hit_test answers VB_E_NO_SCENE until the next frame, and overridden images refresh when marked dirty.
+ *  - Images: a key with an override on this renderer (vb_override_image) is copied from the override's device memory (a size
+ *    mismatch is VB_E_INVALID); any other from its fragment's copy; a registered texture key without an override is VB_E_INVALID.
+ *  - Asynchronous: the work is enqueued on vb_stream and the call returns without waiting, except when the scene, ramp or atlas
+ *    buffers have to grow. Streamed frames still in flight (vb_render_begin) are completed first.
+ *  - The ramps are regenerated only when the ordered list of distinct ramps changes, the atlas only when the ordered list of
+ *    placed images changes or an override applies. A compose that changes only transforms keeps the layout and the buffers,
+ *    so the captured frame graph replays.
+ *  - n = 0 composes the empty scene.
+ * VB_E_INVALID (vb_last_error says why), with the previous scene left as it was: NULL pointers; an unknown or freed fragment;
+ * a transform that is not finite in f32; a scene past 32-bit word offsets; a renderer of a vb_group or with the exchange
+ * enabled; a call between vb_render_enqueue and vb_frame_finish. */
+typedef struct {
+    uint32_t fragment;      /* id from vb_fragment_upload */
+    uint32_t has_transform; /* 0: Encoding::append(&frag, None); 1: Some(transform) */
+    double transform[6];    /* kurbo Affine [a b c d e f], converted to f32 like Transform::from_kurbo */
+} vb_instance;
+int vb_fragment_upload(vb_renderer *, const vb_encoding_streams *, uint32_t *fragment_out);
+int vb_fragment_free(vb_renderer *, uint32_t fragment);
+int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
+
 /* ---- one frame on several GPUs of one box (SURVEY.md 8e, north_star: "a single frame shards across the GPUs by stripes") ----
  * The frame is cut into horizontal stripes of tile rows, one per device; every device runs the element stages on the scene and
  * the tile stages on its stripe (no winding seam exists between horizontal stripes, DESIGN.md 6), and `fine` on device k stores

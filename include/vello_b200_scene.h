@@ -171,6 +171,9 @@ int vb_scene_resolve(vb_scene *, vb_packed *out);
 int vb_render_scene(vb_renderer *, vb_scene *, const vb_params *, void *out, uint32_t out_is_device, vb_frame_stats *);
 /* The first half of vb_render_scene: resolve the scene's streams on the device (vb_scene_upload_streams) and leave them uploaded. */
 int vb_scene_upload_device(vb_renderer *, vb_scene *, vb_layout *layout_out);
+/* The scene as a resident fragment of the renderer (vb_fragment_upload; compose frames from fragments with vb_compose). The
+ * scene, and the image pixels it refers to, are not needed afterwards. */
+int vb_scene_upload_fragment(vb_renderer *, vb_scene *, uint32_t *fragment_out);
 
 /* Renderer::register_texture / unregister_texture (vello/src/lib.rs:578-603): draw pixels that live in device memory.
  * vb_register_texture fills *out with a fresh key as `pixels` -- an address that no host buffer can have, kept in one

@@ -33,6 +33,8 @@ pub struct VbFrameStats {
 #[repr(C)] pub struct VbRampStop { pub offset: f32, pub r: f32, pub g: f32, pub b: f32, pub a: f32 }
 #[repr(C)] pub struct VbRampPatch { pub draw_data_offset: u32, pub extend: u32, pub premul_interp: u32, pub n_stops: u32, pub stops: *const VbRampStop }
 #[repr(C)] pub struct VbImagePatch { pub draw_data_offset: u32, pub width: u32, pub height: u32, pub pixels: *const u8 }
+// one appended fragment of vb_compose: Encoding::append(&fragment, has_transform != 0 ? Some(transform) : None)
+#[repr(C)] pub struct VbInstance { pub fragment: u32, pub has_transform: u32, pub transform: [f64; 6] }
 /// == the six streams of vello_encoding::Encoding (encoding.rs:22-48) + its patches (resolve.rs:560-590)
 #[repr(C)]
 pub struct VbEncodingStreams {
@@ -74,6 +76,11 @@ extern "C" {
     pub fn vb_set_view(r: *mut VbRenderer, affine: *const [f64; 6]) -> c_int;
     pub fn vb_group_set_view(g: *mut VbGroup, affine: *const [f64; 6]) -> c_int;
     pub fn vb_debug_graph_captures(r: *mut VbRenderer, captures: *mut u64) -> c_int;
+    // compose frames on the device from resident fragments: a toolkit's per-frame `Scene::new()` + `scene.append(&fragment,
+    // Some(transform))` per widget becomes one vb_fragment_upload per fragment and one vb_compose of (id, transform) pairs
+    pub fn vb_fragment_upload(r: *mut VbRenderer, e: *const VbEncodingStreams, fragment_out: *mut u32) -> c_int;
+    pub fn vb_fragment_free(r: *mut VbRenderer, fragment: u32) -> c_int;
+    pub fn vb_compose(r: *mut VbRenderer, instances: *const VbInstance, n: u32, layout_out: *mut Layout, draw_offsets: *mut u32) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

@@ -17,8 +17,7 @@ __global__ void k_view_set(ViewCoeffs v, float *dst) {
     if (threadIdx.x < 6u) dst[threadIdx.x] = v.m[threadIdx.x];
 }
 
-// Transform * Transform (vello_encoding/src/math.rs:51-73) in f32, in its association and without FMA contraction: the
-// arithmetic of encoding.py's Encoding.append, so the viewed transforms are the bits a host-side append produces.
+// V * T with Encoding::append's arithmetic (vb_affine_mul), so the viewed transforms are the bits a host-side append produces.
 __global__ void __launch_bounds__(256) k_view_transforms(const float *__restrict__ view, const uint32_t *__restrict__ src, uint32_t *dst,
                                                          uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -30,12 +29,7 @@ __global__ void __launch_bounds__(256) k_view_transforms(const float *__restrict
         b[k] = __uint_as_float(__ldg(src + 6u * i + k));
     }
     float r[6];
-    r[0] = __fadd_rn(__fmul_rn(a[0], b[0]), __fmul_rn(a[2], b[1]));
-    r[1] = __fadd_rn(__fmul_rn(a[1], b[0]), __fmul_rn(a[3], b[1]));
-    r[2] = __fadd_rn(__fmul_rn(a[0], b[2]), __fmul_rn(a[2], b[3]));
-    r[3] = __fadd_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[3], b[3]));
-    r[4] = __fadd_rn(__fadd_rn(__fmul_rn(a[0], b[4]), __fmul_rn(a[2], b[5])), a[4]);
-    r[5] = __fadd_rn(__fadd_rn(__fmul_rn(a[1], b[4]), __fmul_rn(a[3], b[5])), a[5]);
+    vb_affine_mul(a, b, r);
 #pragma unroll
     for (int k = 0; k < 6; k++) dst[6u * i + k] = __float_as_uint(r[k]);
 }

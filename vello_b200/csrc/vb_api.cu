@@ -13,8 +13,11 @@
 #include <sys/mman.h>
 
 #include <algorithm>
+#include <map>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -132,6 +135,43 @@ struct Frame {
     uint32_t slot = 0;
 };
 
+// Composition (vb_compose). A ramp key is one distinct gradient ramp, (stops, interpolation space) compared as the host
+// resolve compares them (floats by ==); an image key is one atlas slot, (pixels pointer, width, height, hash of the pixels). Fragments hold
+// references to the keys of their patches, so de-duplicating a composed scene's ramps and images is a walk over the
+// instances' patch lists (stamp / local: the ramp id or atlas slot the key got in the compose numbered stamp).
+struct RampKey {
+    std::vector<vb_ramp_stop> stops;
+    bool premul = false;
+    bool self_equal = true; // false when a stop holds a NaN: such a ramp equals no other ramp, itself included
+    uint32_t id = 0, refs = 0;
+    uint32_t pool = 0;      // its first stop in the renderer's stop pool
+    uint64_t stamp = 0;
+    uint32_t local = 0;
+};
+struct ImageKey {
+    const void *key = nullptr;
+    uint32_t w = 0, h = 0, id = 0, refs = 0;
+    uint64_t pixels_hash = 0; // of the pixels read at upload (0 for a NULL or registered-texture key, which are not read)
+    uint64_t stamp = 0;
+    uint32_t local = 0;
+};
+// A resident fragment: its streams in one device allocation, back to back behind a header of their word offsets (k_compose.cu
+// reads it), followed by a copy of the pixels of each image key it draws. Patch words are as the encoder wrote them.
+enum { CMP_TAGS, CMP_PATH_DATA, CMP_DRAW_TAGS, CMP_DRAW_DATA, CMP_TRANSFORMS, CMP_STYLES, CMP_STREAMS };
+#define CMP_HEADER_WORDS 8u
+#define CMP_FROM_OVERRIDE 0xffffffffu // the source of an atlas slot filled from an override (fragment ids start at 1, count up)
+struct Fragment {
+    uint32_t id = 0;
+    void *mem = nullptr;
+    size_t bytes = 0;
+    uint32_t len[CMP_STREAMS] = {}; // tag bytes, path data words, draw tags, draw data words, transforms, style words
+    uint32_t n_paths = 0, n_clips = 0, n_open_clips = 0, info = 0;
+    struct Ramp { uint32_t dd, extend; RampKey *key; };
+    struct Image { uint32_t dd; ImageKey *key; const uint8_t *pixels; }; // pixels: in mem, or nullptr for a NULL / texture key
+    std::vector<Ramp> ramps;
+    std::vector<Image> images;
+};
+
 struct vb_renderer {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -160,6 +200,12 @@ struct vb_renderer {
             bool dirty;
         };
         std::vector<OverridePlace> overridden;
+        // set by vb_compose, cleared by every other upload: what the slot's ramps and atlas were made from, so that a compose
+        // regenerates them only when that changes (ramp-key ids in ramp order; (image-key id << 32 | source fragment) in
+        // placement order)
+        bool composed = false;
+        std::vector<uint32_t> ramp_keys;
+        std::vector<uint64_t> atlas_keys;
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -242,6 +288,27 @@ struct vb_renderer {
     } hit, hit_enq;
     DevBuf hit_io; // the host form's points and answers
 
+    // composition (vb_fragment_upload / vb_compose): the resident fragments by id, and the keys their ramps and images are
+    // de-duplicated by across fragments
+    std::unordered_map<uint32_t, std::unique_ptr<Fragment>> fragments;
+    uint32_t next_fragment = 1;
+    size_t fragment_bytes = 0;
+    std::unordered_map<uint64_t, std::vector<RampKey *>> ramp_by_hash; // ramps whose stops compare equal to themselves
+    std::unordered_map<uint32_t, std::unique_ptr<RampKey>> ramp_keys;
+    uint32_t next_ramp_key = 1;
+    DevBuf stop_pool;      // the stops of every ramp key, RampKey::pool apart
+    uint32_t pool_used = 0; // stops
+    std::map<std::tuple<const void *, uint32_t, uint32_t, uint64_t>, std::unique_ptr<ImageKey>> image_keys;
+    // freed fragments whose memory composes already enqueued may still read: released once `done` has completed
+    struct FreedFragment { void *mem; size_t bytes; cudaEvent_t done; };
+    std::vector<FreedFragment> freed;
+    uint32_t next_image_key = 1;
+    uint64_t compose_seq = 0;
+    DevBuf compose_tmp;                  // compose's tables, staged through compose_host (pinned)
+    uint8_t *compose_host = nullptr;
+    size_t compose_host_cap = 0;
+    cudaEvent_t compose_staged = nullptr; // the last copy out of compose_host
+
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
         bool configured = false, enabled = false;
@@ -260,7 +327,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io};
+                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -426,7 +493,8 @@ extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
         cudaStreamCreateWithFlags(&r->tiling_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&r->tiling_fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->blit_staged, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&r->blit_staged, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->compose_staged, cudaEventDisableTiming) != cudaSuccess) {
         delete r;
         return VB_E_CUDA;
     }
@@ -477,6 +545,13 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
         if (s.h_bump) cudaFreeHost(s.h_bump);
     if (r->blit_host) cudaFreeHost(r->blit_host);
     if (r->blit_staged) cudaEventDestroy(r->blit_staged);
+    for (auto &f : r->fragments) cudaFree(f.second->mem);
+    for (auto &f : r->freed) {
+        cudaFree(f.mem);
+        cudaEventDestroy(f.done);
+    }
+    if (r->compose_host) cudaFreeHost(r->compose_host);
+    if (r->compose_staged) cudaEventDestroy(r->compose_staged);
     drop_registrations(r);
     if (r->ev_ok) {
         for (auto &ev : r->ev) cudaEventDestroy(ev);
@@ -573,6 +648,7 @@ static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size
     if (r->cur->atlas_w && r->cur->atlas_h)
         CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4, cudaMemcpyHostToDevice, st));
     r->cur->overridden.clear(); // a caller-packed atlas: overrides do not apply
+    r->cur->composed = false;
     r->cur->have_scene = true;
     r->cells.clear(); // a new scene is one cell until vb_set_cells says otherwise
     hit_forget(r);
@@ -1229,6 +1305,7 @@ static void fill_stats(vb_renderer *r, vb_frame_stats *s, uint32_t retries) {
     s->retries = retries;
     s->kernel_launches = r->launches;
     for_each_buf(r, [&](DevBuf &b) { s->arena_bytes += b.cap; });
+    s->arena_bytes += r->fragment_bytes;
     if (r->timing) {
         for (int i = 0; i < VB_N_STAGE_IDS; i++) cudaEventElapsedTime(&s->stage_ms[i], r->ev[i], r->ev[i + 1]);
         cudaEventElapsedTime(&s->total_ms, r->ev[0], r->ev[VB_N_STAGE_IDS]);
@@ -2410,9 +2487,518 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
     r->cur->overridden = std::move(over);
+    r->cur->composed = false;
     r->cur->layout = L;
     r->cur->scene_words = total_words;
     r->cur->have_scene = true;
+    r->cells.clear();
+    hit_forget(r);
+    if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
+    return VB_OK;
+}
+
+// ---- composition of resident fragments: vb_fragment_upload / vb_fragment_free / vb_compose (k_compose.cu) ---------------------
+static void stop_fields(const vb_ramp_stop &s, float v[5]) {
+    v[0] = s.offset; v[1] = s.r; v[2] = s.g; v[3] = s.b; v[4] = s.a;
+}
+// Stops compared as vb_scene_resolve compares them: float by float with ==, so -0 equals 0 (the hash maps both to 0).
+static uint64_t ramp_hash(const vb_ramp_stop *stops, uint32_t n, bool premul) {
+    uint64_t h = 1469598103934665603ull;
+    auto mix = [&](uint32_t v) { h = (h ^ v) * 1099511628211ull; };
+    mix(premul ? 1u : 0u);
+    mix(n);
+    for (uint32_t i = 0; i < n; i++) {
+        float v[5];
+        stop_fields(stops[i], v);
+        for (float x : v) {
+            uint32_t bits = 0u;
+            if (x != 0.0f) memcpy(&bits, &x, 4);
+            mix(bits);
+        }
+    }
+    return h;
+}
+static bool same_stops(const RampKey &k, const vb_ramp_patch &p) {
+    if (k.premul != (p.premul_interp != 0u) || k.stops.size() != p.n_stops) return false;
+    for (uint32_t i = 0; i < p.n_stops; i++) {
+        float a[5], b[5];
+        stop_fields(k.stops[i], a);
+        stop_fields(p.stops[i], b);
+        for (int c = 0; c < 5; c++)
+            if (!(a[c] == b[c])) return false;
+    }
+    return true;
+}
+// The ramp key of patch p, with one more reference. A key made here is appended to `fresh`: its stops still need a place in
+// the stop pool (place_stops).
+static RampKey *intern_ramp(vb_renderer *r, const vb_ramp_patch &p, std::vector<RampKey *> &fresh) {
+    bool self_equal = true;
+    for (uint32_t i = 0; i < p.n_stops; i++) {
+        float v[5];
+        stop_fields(p.stops[i], v);
+        for (float x : v) self_equal = self_equal && x == x;
+    }
+    const uint64_t h = ramp_hash(p.stops, p.n_stops, p.premul_interp != 0u);
+    if (self_equal) {
+        const auto it = r->ramp_by_hash.find(h);
+        if (it != r->ramp_by_hash.end())
+            for (RampKey *k : it->second)
+                if (same_stops(*k, p)) {
+                    k->refs++;
+                    return k;
+                }
+    }
+    std::unique_ptr<RampKey> k(new RampKey());
+    k->stops.assign(p.stops, p.stops + p.n_stops);
+    k->premul = p.premul_interp != 0u;
+    k->self_equal = self_equal;
+    k->id = r->next_ramp_key++;
+    k->refs = 1;
+    RampKey *raw = k.get();
+    if (self_equal) r->ramp_by_hash[h].push_back(raw);
+    r->ramp_keys[raw->id] = std::move(k);
+    fresh.push_back(raw);
+    return raw;
+}
+static void release_ramp(vb_renderer *r, RampKey *k) {
+    if (--k->refs) return;
+    if (k->self_equal) {
+        auto it = r->ramp_by_hash.find(ramp_hash(k->stops.data(), (uint32_t)k->stops.size(), k->premul));
+        it->second.erase(std::find(it->second.begin(), it->second.end(), k));
+        if (it->second.empty()) r->ramp_by_hash.erase(it);
+    }
+    r->ramp_keys.erase(k->id); // its stops stay in the pool until the pool is rebuilt
+}
+// An image key names one set of pixels. The caller's buffer need not outlive vb_fragment_upload, so its address may come back
+// holding other pixels in a later fragment: host pixels are told apart by a hash of their bytes as well as by the pointer,
+// and only a pointer that holds the same pixels again shares an atlas slot. NULL and registered-texture keys are never read
+// (hash 0): they are one image per pointer, as in a resolve.
+static bool readable_image(const void *key, uint32_t w, uint32_t h) { return key && w && h && !vb_texture_key(key); }
+static uint64_t hash_pixels(const void *key, uint32_t w, uint32_t h) {
+    const uint8_t *p = (const uint8_t *)key;
+    const size_t n = (size_t)w * h * 4u;
+    uint64_t a = 0x9e3779b97f4a7c15ull ^ n, b = 0xc2b2ae3d27d4eb4full;
+    size_t i = 0;
+    for (; i + 16u <= n; i += 16u) {
+        uint64_t x, y;
+        memcpy(&x, p + i, 8);
+        memcpy(&y, p + i + 8, 8);
+        a = (a ^ x) * 0xff51afd7ed558ccdull;
+        b = (b ^ y) * 0xc4ceb9fe1a85ec53ull;
+        a ^= a >> 29;
+        b ^= b >> 31;
+    }
+    for (; i < n; i += 4u) { // w * h * 4 is a multiple of 4
+        uint32_t x;
+        memcpy(&x, p + i, 4);
+        a = (a ^ x) * 0xff51afd7ed558ccdull;
+        a ^= a >> 29;
+    }
+    const uint64_t h64 = (a ^ (b * 0x9e3779b97f4a7c15ull)) * 0xff51afd7ed558ccdull;
+    return h64 ^ (h64 >> 32);
+}
+static ImageKey *intern_image(vb_renderer *r, const void *key, uint32_t w, uint32_t h, uint64_t pixels_hash) {
+    std::unique_ptr<ImageKey> &k = r->image_keys[std::make_tuple(key, w, h, pixels_hash)];
+    if (!k) {
+        k.reset(new ImageKey());
+        k->key = key;
+        k->w = w;
+        k->h = h;
+        k->pixels_hash = pixels_hash;
+        k->id = r->next_image_key++;
+    }
+    k->refs++;
+    return k.get();
+}
+static void release_image(vb_renderer *r, ImageKey *k) {
+    if (--k->refs == 0u) r->image_keys.erase(std::make_tuple(k->key, k->w, k->h, k->pixels_hash));
+}
+static void release_keys(vb_renderer *r, const Fragment &f) {
+    for (const Fragment::Ramp &x : f.ramps) release_ramp(r, x.key);
+    for (const Fragment::Image &x : f.images) release_image(r, x.key);
+}
+
+// Copy the stops of new ramp keys into the stop pool. When they do not fit, the pool is made anew from the live keys (their
+// stops are on the host), after the work already enqueued, which may read the old pool, has finished.
+static int place_stops(vb_renderer *r, const std::vector<RampKey *> &fresh) {
+    size_t add = 0;
+    for (const RampKey *k : fresh) add += k->stops.size();
+    if (add == 0) return VB_OK;
+    std::vector<vb_ramp_stop> host;
+    size_t first = r->pool_used;
+    if ((r->pool_used + add) * sizeof(vb_ramp_stop) <= r->stop_pool.cap) {
+        for (RampKey *k : fresh) {
+            k->pool = (uint32_t)(first + host.size());
+            host.insert(host.end(), k->stops.begin(), k->stops.end());
+        }
+    } else {
+        size_t live = 0;
+        for (const auto &e : r->ramp_keys) live += e.second->stops.size();
+        if (live > 0x7fffffffu) {
+            r->err = "vb_fragment_upload: more gradient stops than 32-bit indices reach";
+            return VB_E_INVALID;
+        }
+        CK(cudaStreamSynchronize(r->stream));
+        CK(cudaFree(r->stop_pool.p));
+        r->stop_pool = DevBuf{};
+        int rc = ensure(r, r->stop_pool, 2 * live * sizeof(vb_ramp_stop));
+        if (rc) return rc;
+        first = 0;
+        for (auto &e : r->ramp_keys) {
+            e.second->pool = (uint32_t)host.size();
+            host.insert(host.end(), e.second->stops.begin(), e.second->stops.end());
+        }
+    }
+    CK(cudaMemcpy((vb_ramp_stop *)r->stop_pool.p + first, host.data(), host.size() * sizeof(vb_ramp_stop), cudaMemcpyHostToDevice));
+    r->pool_used = (uint32_t)(first + host.size());
+    return VB_OK;
+}
+
+// Release the memory of freed fragments that no enqueued work reads any more.
+static void reap_freed(vb_renderer *r) {
+    auto &v = r->freed;
+    for (size_t i = 0; i < v.size();) {
+        if (cudaEventQuery(v[i].done) != cudaSuccess) {
+            cudaGetLastError(); // cudaErrorNotReady is not an error of the next call
+            i++;
+            continue;
+        }
+        cudaFree(v[i].mem);
+        cudaEventDestroy(v[i].done);
+        r->fragment_bytes -= v[i].bytes;
+        v[i] = v.back();
+        v.pop_back();
+    }
+}
+
+extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, uint32_t *fragment_out) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_fragment_upload: ") + why;
+        return VB_E_INVALID;
+    };
+    if (!e || !fragment_out) return bad("NULL streams or id");
+    if ((e->n_path_tags && !e->path_tags) || (e->n_path_data && !e->path_data) || (e->n_draw_tags && !e->draw_tags) ||
+        (e->n_draw_data && !e->draw_data) || (e->n_transforms && !e->transforms) || (e->n_styles && !e->styles) ||
+        (e->n_ramp_patches && !e->ramp_patches) || (e->n_image_patches && !e->image_patches))
+        return bad("a stream with elements and no pointer");
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return bad("a ramp patch without stops or outside the draw data");
+    }
+    for (uint32_t i = 0; i < e->n_image_patches; i++)
+        if (e->image_patches[i].draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+    // the allocation: header, the six streams (tags padded to whole words), then one copy of each image key's pixels
+    uint64_t off[CMP_HEADER_WORDS] = {};
+    uint64_t w = CMP_HEADER_WORDS;
+    const uint64_t words[CMP_STREAMS] = {((uint64_t)e->n_path_tags + 3u) / 4u, e->n_path_data, e->n_draw_tags, e->n_draw_data,
+                                         6ull * e->n_transforms, 2ull * e->n_styles};
+    for (int s = 0; s < CMP_STREAMS; s++) {
+        off[s] = w;
+        w += words[s];
+    }
+    if (w + 4u > 0xfffffff0ull) return bad("the fragment's streams exceed 32-bit word offsets");
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    std::unique_ptr<Fragment> f(new Fragment());
+    size_t bytes = (size_t)(w + 4u) * 4u;
+    bytes = (bytes + 15u) & ~(size_t)15u;
+    std::vector<std::pair<size_t, const Fragment::Image *>> copies; // (offset in the allocation, image) per key with pixels
+    std::unordered_map<const ImageKey *, size_t> at;
+    std::map<std::tuple<const void *, uint32_t, uint32_t>, uint64_t> hashed; // each of this fragment's images is read once
+    for (uint32_t i = 0; i < e->n_image_patches; i++) {
+        const vb_image_patch &im = e->image_patches[i];
+        uint64_t hv = 0;
+        if (readable_image(im.pixels, im.width, im.height)) {
+            const auto t = std::make_tuple((const void *)im.pixels, im.width, im.height);
+            const auto it = hashed.find(t);
+            hv = it != hashed.end() ? it->second : (hashed[t] = hash_pixels(im.pixels, im.width, im.height));
+        }
+        f->images.push_back(Fragment::Image{im.draw_data_offset, intern_image(r, im.pixels, im.width, im.height, hv), nullptr});
+    }
+    for (Fragment::Image &x : f->images) {
+        // a registered texture's key points at nothing: its pixels exist only in device memory (an override, at compose)
+        if (!readable_image(x.key->key, x.key->w, x.key->h) || at.count(x.key)) continue;
+        at[x.key] = bytes;
+        copies.push_back({bytes, &x});
+        bytes += ((size_t)x.key->w * x.key->h * 4u + 15u) & ~(size_t)15u;
+    }
+    std::vector<RampKey *> fresh;
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        f->ramps.push_back(Fragment::Ramp{p.draw_data_offset, p.extend, intern_ramp(r, p, fresh)});
+    }
+    int rc = place_stops(r, fresh);
+    cudaError_t ce = rc ? cudaSuccess : cudaMalloc(&f->mem, bytes);
+    if (rc || ce != cudaSuccess) {
+        release_keys(r, *f);
+        if (ce != cudaSuccess) {
+            r->err = std::string("vb_fragment_upload: cudaMalloc: ") + cudaGetErrorString(ce);
+            return VB_E_CUDA;
+        }
+        return rc;
+    }
+    f->bytes = bytes;
+    for (Fragment::Image &x : f->images) {
+        const auto it = at.find(x.key);
+        if (it != at.end()) x.pixels = (const uint8_t *)f->mem + it->second;
+    }
+    uint32_t header[CMP_HEADER_WORDS];
+    for (int s = 0; s < (int)CMP_HEADER_WORDS; s++) header[s] = (uint32_t)off[s];
+    char *base = (char *)f->mem;
+    const void *src[CMP_STREAMS] = {e->path_tags, e->path_data, e->draw_tags, e->draw_data, e->transforms, e->styles};
+    const size_t len_bytes[CMP_STREAMS] = {e->n_path_tags, (size_t)e->n_path_data * 4, (size_t)e->n_draw_tags * 4, (size_t)e->n_draw_data * 4,
+                                           (size_t)e->n_transforms * 24, (size_t)e->n_styles * 8};
+    cudaStream_t st = r->upload_stream;
+    ce = cudaMemcpyAsync(base, header, sizeof header, cudaMemcpyHostToDevice, st);
+    for (int s = 0; s < CMP_STREAMS && ce == cudaSuccess; s++)
+        if (len_bytes[s]) ce = cudaMemcpyAsync(base + off[s] * 4u, src[s], len_bytes[s], cudaMemcpyHostToDevice, st);
+    for (size_t i = 0; i < copies.size() && ce == cudaSuccess; i++) {
+        const ImageKey &k = *copies[i].second->key;
+        ce = cudaMemcpyAsync(base + copies[i].first, k.key, (size_t)k.w * k.h * 4u, cudaMemcpyHostToDevice, st);
+    }
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) {
+        cudaFree(f->mem);
+        release_keys(r, *f);
+        r->err = std::string("vb_fragment_upload: copying the streams: ") + cudaGetErrorString(ce);
+        return VB_E_CUDA;
+    }
+    f->len[CMP_TAGS] = e->n_path_tags;
+    f->len[CMP_PATH_DATA] = e->n_path_data;
+    f->len[CMP_DRAW_TAGS] = e->n_draw_tags;
+    f->len[CMP_DRAW_DATA] = e->n_draw_data;
+    f->len[CMP_TRANSFORMS] = e->n_transforms;
+    f->len[CMP_STYLES] = 2u * e->n_styles;
+    f->n_paths = e->n_paths;
+    f->n_clips = e->n_clips;
+    f->n_open_clips = e->n_open_clips;
+    for (uint32_t i = 0; i < e->n_draw_tags; i++) f->info += (e->draw_tags[i] >> 6) & 0xFu;
+    f->id = r->next_fragment++;
+    r->fragment_bytes += bytes;
+    *fragment_out = f->id;
+    r->fragments[f->id] = std::move(f);
+    return VB_OK;
+}
+
+extern "C" int vb_fragment_free(vb_renderer *r, uint32_t fragment) {
+    if (!r) return VB_E_INVALID;
+    const auto it = r->fragments.find(fragment);
+    if (it == r->fragments.end()) {
+        r->err = "vb_fragment_free: unknown or freed fragment " + std::to_string(fragment);
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    // composes already enqueued read the memory: it is released once the stream has passed this point (reap_freed)
+    cudaEvent_t done;
+    CK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    const cudaError_t ce = cudaEventRecord(done, r->stream);
+    if (ce != cudaSuccess) {
+        cudaEventDestroy(done);
+        r->err = std::string("vb_fragment_free: ") + cudaGetErrorString(ce);
+        return VB_E_CUDA;
+    }
+    r->freed.push_back({it->second->mem, it->second->bytes, done});
+    release_keys(r, *it->second);
+    r->fragments.erase(it);
+    return VB_OK;
+}
+
+// Grow a buffer compose writes. Work already enqueued may read it: growing waits for the renderer's stream.
+static int compose_room(vb_renderer *r, DevBuf &b, size_t bytes) {
+    if (b.cap >= std::max<size_t>(bytes, 256)) return VB_OK;
+    CK(cudaStreamSynchronize(r->stream));
+    return ensure(r, b, bytes);
+}
+
+extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_compose: " + why;
+        return VB_E_INVALID;
+    };
+    if (n && !inst) return bad("NULL instances");
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    // validate everything and size the scene before anything is written
+    std::vector<const Fragment *> fr(n);
+    std::vector<CmpXform> xf(n);
+    uint64_t tot[CMP_STREAMS] = {}, n_paths = 0, n_clips = 0, n_open = 0, info = 0;
+    for (uint32_t k = 0; k < n; k++) {
+        const auto it = r->fragments.find(inst[k].fragment);
+        if (it == r->fragments.end()) return bad("unknown or freed fragment " + std::to_string(inst[k].fragment));
+        fr[k] = it->second.get();
+        memset(&xf[k], 0, sizeof xf[k]);
+        xf[k].on = inst[k].has_transform ? 1u : 0u;
+        for (int c = 0; c < 6 && xf[k].on; c++) {
+            xf[k].m[c] = (float)inst[k].transform[c]; // Transform::from_kurbo
+            if (!isfinite(xf[k].m[c])) return bad("instance " + std::to_string(k) + ": the transform must be finite in f32");
+        }
+        for (int s = 0; s < CMP_STREAMS; s++) tot[s] += fr[k]->len[s];
+        n_paths += fr[k]->n_paths;
+        n_clips += fr[k]->n_clips;
+        n_open += fr[k]->n_open_clips;
+        info += fr[k]->info;
+    }
+    const uint64_t n_tags = tot[CMP_TAGS] + n_open, padded = (n_tags + 1023u) & ~1023ull;
+    const uint64_t total_words = padded / 4u + tot[CMP_PATH_DATA] + tot[CMP_DRAW_TAGS] + n_open + tot[CMP_DRAW_DATA] +
+                                 6u * tot[CMP_TRANSFORMS] + tot[CMP_STYLES];
+    // room for a view's transforms too (prepare), which share the scene's 32-bit word offsets
+    if (padded > 0xffffffffull || total_words + 6u * tot[CMP_TRANSFORMS] > 0xfffffff0ull || n_paths > 0xffffffffull || info > 0xffffffffull)
+        return bad("the composed scene exceeds 32-bit word offsets");
+    VbLayout L;
+    memset(&L, 0, sizeof L);
+    L.n_paths = L.n_draw_objects = (uint32_t)n_paths;
+    L.n_clips = (uint32_t)n_clips;
+    L.bin_data_start = (uint32_t)info;
+    uint32_t o = (uint32_t)(padded / 4u);
+    L.path_tag_base = 0;
+    L.path_data_base = o; o += (uint32_t)tot[CMP_PATH_DATA];
+    L.draw_tag_base = o; o += (uint32_t)(tot[CMP_DRAW_TAGS] + n_open);
+    L.draw_data_base = o; o += (uint32_t)tot[CMP_DRAW_DATA];
+    L.transform_base = o; o += 6u * (uint32_t)tot[CMP_TRANSFORMS];
+    L.style_base = o;
+
+    // late-bound ramps and images of every instance in order: the host resolve's de-duplication and shelf placement, keyed
+    // by the keys the fragments hold
+    const uint64_t seq = ++r->compose_seq;
+    std::vector<RsPatch> patches;
+    std::vector<RsRamp> ramps;
+    std::vector<uint32_t> ramp_ids;
+    struct Placed { const ImageKey *key; const uint8_t *src; uint32_t x, y, frag; };
+    std::vector<Placed> placed;
+    uint32_t atlas_w = 1, x = 0, y = 0, shelf_h = 0;
+    const uint32_t MAXW = 2048;
+    uint32_t dd0 = L.draw_data_base;
+    for (uint32_t k = 0; k < n; k++) {
+        const Fragment &f = *fr[k];
+        for (const Fragment::Ramp &p : f.ramps) {
+            RampKey *key = p.key;
+            if (key->stamp != seq || !key->self_equal) {
+                key->stamp = seq;
+                key->local = (uint32_t)ramps.size();
+                ramps.push_back(RsRamp{key->pool, (uint32_t)key->stops.size(), key->premul ? 1u : 0u, 0u});
+                ramp_ids.push_back(key->id);
+            }
+            patches.push_back(RsPatch{dd0 + p.dd, (key->local << 2) | p.extend});
+        }
+        for (const Fragment::Image &im : f.images) {
+            ImageKey *key = im.key;
+            if (key->stamp != seq) {
+                if (x + key->w > MAXW) { y += shelf_h; x = 0; shelf_h = 0; }
+                key->stamp = seq;
+                key->local = (uint32_t)placed.size();
+                placed.push_back(Placed{key, im.pixels, x, y, f.id});
+                x += key->w;
+                if (key->h > shelf_h) shelf_h = key->h;
+                if (x > atlas_w) atlas_w = x;
+            }
+            const Placed &q = placed[key->local];
+            patches.push_back(RsPatch{dd0 + im.dd, (q.x << 16) | q.y});
+        }
+        dd0 += f.len[CMP_DRAW_DATA];
+    }
+    const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
+    // images with an override on this renderer come from its device memory, the others from their fragment's copy
+    std::vector<VbBlitRect> blits;
+    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
+    std::vector<uint64_t> atlas_keys;
+    for (const Placed &q : placed) {
+        const ImageKey &k = *q.key;
+        const auto ov = k.key ? r->overrides.find(k.key) : r->overrides.end();
+        // where the slot's pixels come from: the fragment, an override (never a fragment id), or nowhere (a zero region)
+        const uint32_t src_of = ov != r->overrides.end() ? CMP_FROM_OVERRIDE : q.src ? q.frag : 0u;
+        if (ov != r->overrides.end()) {
+            const vb_renderer::Override &ob = ov->second;
+            if (ob.w != k.w || ob.h != k.h)
+                return bad("an override's size differs from its image's (" + std::to_string(ob.w) + "x" + std::to_string(ob.h) + " vs " +
+                           std::to_string(k.w) + "x" + std::to_string(k.h) + ")");
+            blits.push_back(VbBlitRect{ob.src, ob.pitch, 0, k.w, k.h, q.x, q.y, 0, 0});
+            over.push_back({k.key, ob.src, ob.pitch, k.w, k.h, q.x, q.y, false});
+        } else if (vb_texture_key(k.key)) {
+            return bad("a registered texture has no override on this renderer");
+        } else if (q.src) {
+            blits.push_back(VbBlitRect{q.src, (uint64_t)k.w * 4u, 0, k.w, k.h, q.x, q.y, 0, 0});
+        }
+        atlas_keys.push_back((uint64_t)k.id << 32 | src_of);
+    }
+
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    cudaStream_t st = r->stream;
+    vb_renderer::SceneSlot &slot = *r->cur;
+    const bool new_ramps = !slot.composed || ramp_ids != slot.ramp_keys;
+    const bool new_atlas = !slot.composed || atlas_keys != slot.atlas_keys || !over.empty();
+    // the tables, staged through pinned memory: prefixes, fragment addresses, transforms, patches, ramp descriptors
+    auto up16 = [](size_t v) { return (v + 15u) & ~(size_t)15u; };
+    const size_t o_src = up16((size_t)CMP_STREAMS * (n + 1u) * 4u), o_xf = up16(o_src + (size_t)n * 8u), o_pat = up16(o_xf + (size_t)n * sizeof(CmpXform));
+    const size_t o_ramp = up16(o_pat + patches.size() * sizeof(RsPatch)), staged = o_ramp + ramps.size() * sizeof(RsRamp);
+    CK(cudaEventSynchronize(r->compose_staged));
+    if (r->compose_host_cap < staged) {
+        if (r->compose_host) CK(cudaFreeHost(r->compose_host));
+        r->compose_host = nullptr;
+        r->compose_host_cap = 0;
+        CK(cudaMallocHost((void **)&r->compose_host, staged));
+        r->compose_host_cap = staged;
+    }
+    uint8_t *h = r->compose_host;
+    uint32_t *pre = (uint32_t *)h;
+    for (int s = 0; s < CMP_STREAMS; s++) {
+        uint32_t *P = pre + (size_t)s * (n + 1u);
+        P[0] = 0u;
+        for (uint32_t k = 0; k < n; k++) P[k + 1] = P[k] + fr[k]->len[s];
+    }
+    unsigned long long *srcs = (unsigned long long *)(h + o_src);
+    for (uint32_t k = 0; k < n; k++) srcs[k] = (unsigned long long)(uintptr_t)fr[k]->mem;
+    if (n) memcpy(h + o_xf, xf.data(), (size_t)n * sizeof(CmpXform));
+    if (!patches.empty()) memcpy(h + o_pat, patches.data(), patches.size() * sizeof(RsPatch));
+    if (!ramps.empty()) memcpy(h + o_ramp, ramps.data(), ramps.size() * sizeof(RsRamp));
+    if (draw_offsets) memcpy(draw_offsets, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+
+    if ((rc = compose_room(r, r->compose_tmp, staged))) return rc;
+    if ((rc = compose_room(r, slot.scene, scene_bytes(L, total_words, r->view.on)))) return rc;
+    if (new_ramps && (rc = compose_room(r, slot.ramps, ramps.size() * 512u * 4u))) return rc;
+    if (new_atlas && (rc = compose_room(r, slot.atlas, (size_t)atlas_w * atlas_h * 4u))) return rc;
+    char *tmp = (char *)r->compose_tmp.p;
+    if (staged) CK(cudaMemcpyAsync(tmp, h, staged, cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(r->compose_staged, st));
+    uint32_t *scene = (uint32_t *)slot.scene.p;
+    CmpArgs a;
+    memset(&a, 0, sizeof a);
+    a.scene = scene;
+    a.prefix = (const uint32_t *)tmp;
+    a.src = (const unsigned long long *)(tmp + o_src);
+    a.xf = (const CmpXform *)(tmp + o_xf);
+    a.n = n;
+    const uint32_t dst[CMP_STREAMS] = {L.path_tag_base, L.path_data_base, L.draw_tag_base, L.draw_data_base, L.transform_base, L.style_base};
+    const uint32_t units[CMP_STREAMS] = {(uint32_t)((tot[CMP_TAGS] + 3u) / 4u), (uint32_t)tot[CMP_PATH_DATA], (uint32_t)tot[CMP_DRAW_TAGS],
+                                         (uint32_t)tot[CMP_DRAW_DATA], (uint32_t)tot[CMP_TRANSFORMS], (uint32_t)tot[CMP_STYLES]};
+    memcpy(a.dst, dst, sizeof dst);
+    memcpy(a.units, units, sizeof units);
+    vb_launch_compose(a, st);
+    vb_launch_resolve_finish(scene, (uint32_t)tot[CMP_TAGS], (uint32_t)n_open, (uint32_t)padded, L.draw_tag_base + (uint32_t)tot[CMP_DRAW_TAGS],
+                             (const RsPatch *)(tmp + o_pat), (uint32_t)patches.size(), st);
+    if (new_ramps) {
+        vb_launch_make_ramps((const RsRamp *)(tmp + o_ramp), (const RsStop *)r->stop_pool.p, (uint32_t)ramps.size(), (uint32_t *)slot.ramps.p, st);
+        slot.ramp_keys = std::move(ramp_ids);
+    }
+    if (new_atlas) {
+        CK(cudaMemsetAsync(slot.atlas.p, 0, (size_t)atlas_w * atlas_h * 4u, st));
+        if ((rc = enqueue_blits(r, blits, slot.atlas.p, atlas_w))) return rc;
+        slot.atlas_keys = std::move(atlas_keys);
+    }
+    CK(cudaGetLastError());
+    slot.composed = true;
+    slot.overridden = std::move(over);
+    slot.n_ramps = (uint32_t)ramps.size();
+    slot.atlas_w = atlas_w;
+    slot.atlas_h = atlas_h;
+    slot.layout = L;
+    slot.scene_words = total_words;
+    slot.have_scene = true;
     r->cells.clear();
     hit_forget(r);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));

@@ -213,3 +213,14 @@ __device__ __forceinline__ uint32_t vb_cell_of(const VbConfig &cfg, uint32_t ix)
     }
     return lo;
 }
+// Transform * Transform (vello_encoding/src/math.rs:51-73) in f32, in its association and without FMA contraction: the
+// arithmetic of Encoding::append (encoding.py's Encoding.append, vb_scene.cpp's vb_scene_append), so a transform composed on
+// the device has the bits a host-side append produces. r = a * b; used by views (k_view.cu) and composition (k_compose.cu).
+__device__ __forceinline__ void vb_affine_mul(const float a[6], const float b[6], float r[6]) {
+    r[0] = __fadd_rn(__fmul_rn(a[0], b[0]), __fmul_rn(a[2], b[1]));
+    r[1] = __fadd_rn(__fmul_rn(a[1], b[0]), __fmul_rn(a[3], b[1]));
+    r[2] = __fadd_rn(__fmul_rn(a[0], b[2]), __fmul_rn(a[2], b[3]));
+    r[3] = __fadd_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[3], b[3]));
+    r[4] = __fadd_rn(__fadd_rn(__fmul_rn(a[0], b[4]), __fmul_rn(a[2], b[5])), a[4]);
+    r[5] = __fadd_rn(__fadd_rn(__fmul_rn(a[1], b[4]), __fmul_rn(a[3], b[5])), a[5]);
+}

@@ -1437,30 +1437,44 @@ int vb_scene_resolve(vb_scene *s, vb_packed *out) {
     return VB_OK;
 }
 
+// The scene's streams as vb_encoding_streams, pointing into the scene (rps / ips hold its patches).
+static void streams_of(const Encoding &e, std::vector<vb_ramp_patch> &rps, std::vector<vb_image_patch> &ips, vb_encoding_streams *st) {
+    static_assert(sizeof(Stop) == sizeof(vb_ramp_stop) && sizeof(Xform) == 24 && sizeof(Style) == 8, "stream record layouts");
+    for (const RampPatch &p : e.ramp_patches)
+        rps.push_back(vb_ramp_patch{p.draw_data_offset, p.extend, p.premul ? 1u : 0u, (uint32_t)p.stops.size(),
+                                    reinterpret_cast<const vb_ramp_stop *>(p.stops.data())});
+    for (const ImagePatch &p : e.image_patches) ips.push_back(vb_image_patch{p.draw_data_offset, p.image.width, p.image.height, p.image.pixels});
+    std::memset(st, 0, sizeof *st);
+    st->path_tags = e.path_tags.data(); st->n_path_tags = (uint32_t)e.path_tags.size();
+    st->path_data = reinterpret_cast<const uint32_t *>(e.path_data.data()); st->n_path_data = (uint32_t)e.path_data.size();
+    st->draw_tags = e.draw_tags.data(); st->n_draw_tags = (uint32_t)e.draw_tags.size();
+    st->draw_data = e.draw_data.data(); st->n_draw_data = (uint32_t)e.draw_data.size();
+    st->transforms = reinterpret_cast<const float *>(e.transforms.data()); st->n_transforms = (uint32_t)e.transforms.size();
+    st->styles = reinterpret_cast<const uint32_t *>(e.styles.data()); st->n_styles = (uint32_t)e.styles.size();
+    st->n_paths = e.n_paths; st->n_clips = e.n_clips; st->n_open_clips = e.n_open_clips;
+    st->ramp_patches = rps.data(); st->n_ramp_patches = (uint32_t)rps.size();
+    st->image_patches = ips.data(); st->n_image_patches = (uint32_t)ips.size();
+}
+
 // Shapes to pixels: the scene's streams are resolved ON THE DEVICE (vb_scene_upload_streams: stream copies to their Layout offsets,
 // patch / padding / ramp kernels), then rendered.
 int vb_scene_upload_device(vb_renderer *r, vb_scene *s, vb_layout *layout_out) {
     if (!r || !s) return VB_E_INVALID;
-    const Encoding &e = s->e;
-    static_assert(sizeof(Stop) == sizeof(vb_ramp_stop) && sizeof(Xform) == 24 && sizeof(Style) == 8, "stream record layouts");
     std::vector<vb_ramp_patch> rps;
-    for (const RampPatch &p : e.ramp_patches)
-        rps.push_back(vb_ramp_patch{p.draw_data_offset, p.extend, p.premul ? 1u : 0u, (uint32_t)p.stops.size(),
-                                    reinterpret_cast<const vb_ramp_stop *>(p.stops.data())});
     std::vector<vb_image_patch> ips;
-    for (const ImagePatch &p : e.image_patches) ips.push_back(vb_image_patch{p.draw_data_offset, p.image.width, p.image.height, p.image.pixels});
     vb_encoding_streams st;
-    std::memset(&st, 0, sizeof st);
-    st.path_tags = e.path_tags.data(); st.n_path_tags = (uint32_t)e.path_tags.size();
-    st.path_data = reinterpret_cast<const uint32_t *>(e.path_data.data()); st.n_path_data = (uint32_t)e.path_data.size();
-    st.draw_tags = e.draw_tags.data(); st.n_draw_tags = (uint32_t)e.draw_tags.size();
-    st.draw_data = e.draw_data.data(); st.n_draw_data = (uint32_t)e.draw_data.size();
-    st.transforms = reinterpret_cast<const float *>(e.transforms.data()); st.n_transforms = (uint32_t)e.transforms.size();
-    st.styles = reinterpret_cast<const uint32_t *>(e.styles.data()); st.n_styles = (uint32_t)e.styles.size();
-    st.n_paths = e.n_paths; st.n_clips = e.n_clips; st.n_open_clips = e.n_open_clips;
-    st.ramp_patches = rps.data(); st.n_ramp_patches = (uint32_t)rps.size();
-    st.image_patches = ips.data(); st.n_image_patches = (uint32_t)ips.size();
+    streams_of(s->e, rps, ips, &st);
     return vb_scene_upload_streams(r, &st, layout_out);
+}
+
+// The scene as a resident fragment for vb_compose (vb_fragment_upload copies everything it needs).
+int vb_scene_upload_fragment(vb_renderer *r, vb_scene *s, uint32_t *fragment_out) {
+    if (!r || !s) return VB_E_INVALID;
+    std::vector<vb_ramp_patch> rps;
+    std::vector<vb_image_patch> ips;
+    vb_encoding_streams st;
+    streams_of(s->e, rps, ips, &st);
+    return vb_fragment_upload(r, &st, fragment_out);
 }
 
 int vb_register_texture(vb_renderer *r, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes, vb_image *out) {

@@ -117,6 +117,21 @@ void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_
                               const RsPatch *patches, uint32_t n_patches, cudaStream_t st);
 void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st);
 
+// k_compose.cu: the six streams of a composition of resident fragments (vb_compose), staged by vb_api.cu
+struct CmpXform { float m[6]; uint32_t on, pad; }; // an instance's transform (on == 0: appended without one)
+struct CmpArgs {
+    uint32_t *scene;              // the packed scene being composed
+    const uint32_t *prefix;       // 6 x (n + 1): per stream, the exclusive prefix of the instances' lengths (path tags in bytes,
+                                  // transforms in transforms, the other streams in words)
+    const unsigned long long *src; // n: each instance's fragment allocation, which starts with the word offsets of its streams
+    const CmpXform *xf;           // n
+    uint32_t n;
+    uint32_t dst[6];              // the streams' Layout offsets in words
+    uint32_t units[6];            // destination units per stream: tag words, words, transforms (stream 4), words
+    uint32_t cta0[6];             // first CTA of each stream (set by the launcher)
+};
+uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
+
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)
 uint32_t vb_atlas_blit_units_per_row(uint32_t w);

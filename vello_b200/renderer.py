@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 from dataclasses import dataclass
 from typing import Optional
 
@@ -41,6 +42,31 @@ class _Layout(C.Structure):
 
 class _Params(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("base_color", "width", "height", "aa", "bin_row0", "bin_row1", "tile_row0", "tile_row1")]
+
+
+class _RampStop(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("offset", "r", "g", "b", "a")]
+
+
+class _RampPatch(C.Structure):
+    _fields_ = [("draw_data_offset", C.c_uint32), ("extend", C.c_uint32), ("premul_interp", C.c_uint32), ("n_stops", C.c_uint32),
+                ("stops", C.c_void_p)]
+
+
+class _ImagePatch(C.Structure):
+    _fields_ = [("draw_data_offset", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("pixels", C.c_void_p)]
+
+
+class _EncodingStreams(C.Structure):
+    _fields_ = [("path_tags", C.c_void_p), ("n_path_tags", C.c_uint32), ("path_data", C.c_void_p), ("n_path_data", C.c_uint32),
+                ("draw_tags", C.c_void_p), ("n_draw_tags", C.c_uint32), ("draw_data", C.c_void_p), ("n_draw_data", C.c_uint32),
+                ("transforms", C.c_void_p), ("n_transforms", C.c_uint32), ("styles", C.c_void_p), ("n_styles", C.c_uint32),
+                ("n_paths", C.c_uint32), ("n_clips", C.c_uint32), ("n_open_clips", C.c_uint32),
+                ("ramp_patches", C.c_void_p), ("n_ramp_patches", C.c_uint32), ("image_patches", C.c_void_p), ("n_image_patches", C.c_uint32)]
+
+
+class _Instance(C.Structure):
+    _fields_ = [("fragment", C.c_uint32), ("has_transform", C.c_uint32), ("transform", C.c_double * 6)]
 
 
 class FrameStats(C.Structure):
@@ -135,6 +161,9 @@ def load_library() -> C.CDLL:
     lib.vb_group_set_view.argtypes = [vp, C.POINTER(C.c_double)]
     lib.vb_debug_graph_captures.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.vb_hit_test.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
+    lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
+    lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
+    lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     _lib = lib
     return lib
 
@@ -147,7 +176,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
-                    "vb_debug_graph_captures", "vb_hit_test"]
+                    "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose"]
 
 
 def _device_image(t):
@@ -194,6 +223,36 @@ def _view_coeffs(affine: Optional[Affine]):
     return None if affine is None else (C.c_double * 6)(*[float(v) for v in affine.coeffs])
 
 
+def _encoding_streams(enc, key_of):
+    """`enc` (an `encoding.Encoding`) as vb_encoding_streams, and the arrays it points into (keep them alive for the call).
+    key_of(image) gives the pointer an image is keyed and read by."""
+    from .encoding import _f32_bits, _path_data_array
+    tags = np.asarray(enc.path_tags, dtype=np.uint8)
+    pd = _path_data_array(enc.path_data).view(np.uint32)
+    dtags = np.asarray(enc.draw_tags, dtype=np.uint32)
+    ddata = np.asarray(enc.draw_data, dtype=np.uint32)
+    tr = np.asarray(enc.transforms, dtype=np.float32).reshape(-1)
+    st = np.zeros(2 * len(enc.styles), dtype=np.uint32)
+    for i, (fl, lw) in enumerate(enc.styles):
+        st[2 * i], st[2 * i + 1] = fl, _f32_bits(lw)
+    keep = [tags, pd, dtags, ddata, tr, st]
+    rps = (_RampPatch * max(len(enc.ramp_patches), 1))()
+    for i, p in enumerate(enc.ramp_patches):
+        stops = (_RampStop * len(p["stops"]))(*[_RampStop(o, c.r, c.g, c.b, c.a) for o, c in p["stops"]])
+        keep.append(stops)
+        rps[i] = _RampPatch(p["draw_data_offset"], p["extend"], 1 if p["premul"] else 0, len(p["stops"]), C.cast(stops, C.c_void_p))
+    ips = (_ImagePatch * max(len(enc.image_patches), 1))()
+    for i, p in enumerate(enc.image_patches):
+        im = p["image"]
+        ips[i] = _ImagePatch(p["draw_data_offset"], im.width, im.height, key_of(im))
+    keep += [rps, ips]
+    ptr = lambda a: a.ctypes.data if a.size else None  # noqa: E731
+    e = _EncodingStreams(ptr(tags), tags.size, ptr(pd), pd.size, ptr(dtags), dtags.size, ptr(ddata), ddata.size, ptr(tr), len(enc.transforms),
+                         ptr(st), len(enc.styles), enc.n_paths, enc.n_clips, enc.n_open_clips, C.cast(rps, C.c_void_p), len(enc.ramp_patches),
+                         C.cast(ips, C.c_void_p), len(enc.image_patches))
+    return e, keep
+
+
 def _params_struct(p: RenderParams, bin_rows=(0, 0), tile_rows=(0, 0)) -> _Params:
     return _Params(p.base_color.premul_rgba8_u32(), int(p.width), int(p.height), int(p.antialiasing_method),
                    int(bin_rows[0]), int(bin_rows[1]), int(tile_rows[0]), int(tile_rows[1]))
@@ -216,6 +275,7 @@ class Renderer:
         self._keep = None
         self._owner = None
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
+        self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
 
     @classmethod
     def _borrowed(cls, lib, handle: int, owner):
@@ -224,6 +284,7 @@ class Renderer:
         r.lib, r.handle, r.options, r.last_stats, r._keep = lib, C.c_void_p(handle), None, None, None
         r._owner = owner
         r._device_images = {}
+        r._fragment_pixels = {}
         return r
 
     def close(self):
@@ -290,6 +351,62 @@ class Renderer:
             image.key = int(image.data.ctypes.data)
         self._check(self.lib.vb_override_image(self.handle, C.c_void_p(image.key), w, h, C.c_void_p(ptr), pitch), "vb_override_image")
         self._device_images[image.key] = t
+
+    # -- composition: frames built on the device from resident fragments (vb_fragment_upload / vb_compose) -------------------
+    def upload_fragment(self, scene) -> int:
+        """Copy `scene` (a `Scene` or a `NativeScene`) to the device as a fragment, with its images' pixels and its gradient
+        stops, and return its id for `compose`. The scene is not needed afterwards; editing it does not change the fragment."""
+        from .scene_native import NativeScene, _lib as _scene_lib
+        fid = C.c_uint32(0)
+        if isinstance(scene, NativeScene):
+            self._check(_scene_lib().vb_scene_upload_fragment(self.handle, scene.handle, C.byref(fid)), "vb_scene_upload_fragment")
+            return int(fid.value)
+        e, keep = _encoding_streams(scene.encoding, self._image_key)
+        self._check(self.lib.vb_fragment_upload(self.handle, C.byref(e), C.byref(fid)), "vb_fragment_upload")
+        return int(fid.value)
+
+    def _image_key(self, im: Image) -> Optional[int]:
+        """The pointer an image of a `Scene` is keyed and read by: its key, else its pixel array (as resolve keys images by
+        the array's identity; for a non-contiguous array, a contiguous copy kept while the array lives, so that the key stays the
+        same)."""
+        if im.key is not None:
+            return int(im.key)
+        d = im.data
+        if isinstance(d, np.ndarray) and d.dtype == np.uint8 and d.flags.c_contiguous:
+            return int(d.ctypes.data)
+        copy = self._fragment_pixels.get(id(d))
+        if copy is None:
+            copy = np.ascontiguousarray(d, dtype=np.uint8).copy()
+            try:  # held while `d` lives, so that the key stays the same for it (and no other array can have its id)
+                weakref.finalize(d, self._fragment_pixels.pop, id(d), None)
+                self._fragment_pixels[id(d)] = copy
+            except TypeError:  # not weakly referenceable: a copy for this upload only
+                pass
+        return int(copy.ctypes.data)
+
+    def free_fragment(self, fragment: int):
+        """Release a fragment (after the work already enqueued that reads it). Composed scenes are copies: they stay."""
+        self._check(self.lib.vb_fragment_free(self.handle, int(fragment)), "vb_fragment_free")
+
+    def compose(self, instances):
+        """Make the renderer's scene `Scene()` with every `(fragment id, Affine or None)` of `instances` appended in order,
+        resolved, built on the device from the resident fragments (`vb_compose`; asynchronous on `self.stream`). Returns
+        (Layout, draw_offsets): instance k's draws are draw objects draw_offsets[k] .. draw_offsets[k + 1] - 1."""
+        from .encoding import Layout
+        inst = list(instances)
+        arr = (_Instance * max(len(inst), 1))()
+        for k, (fid, t) in enumerate(inst):
+            arr[k].fragment = int(fid)
+            if t is not None:
+                arr[k].has_transform = 1
+                for i, v in enumerate(t.coeffs):
+                    arr[k].transform[i] = float(v)
+        L = _Layout()
+        offs = (C.c_uint32 * (len(inst) + 1))()
+        self._check(self.lib.vb_compose(self.handle, arr, len(inst), C.byref(L), offs), "vb_compose")
+        lay = Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
+                     L.draw_data_base, L.transform_base, L.style_base)
+        return lay, [int(v) for v in offs]
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""

@@ -55,7 +55,7 @@ PATHBUF_SYMBOLS = ["vb_pathbuf_new", "vb_pathbuf_free", "vb_pathbuf_clear", "vb_
 SCENE_SYMBOLS = ["vb_scene_new", "vb_scene_free", "vb_scene_reset", "vb_scene_fill", "vb_scene_stroke", "vb_scene_push_layer",
                  "vb_scene_push_luminance_mask_layer", "vb_scene_push_clip_layer", "vb_scene_pop_layer", "vb_scene_draw_image",
                  "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_batch", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
-                 "vb_register_texture", "vb_unregister_texture", "vb_scene_n_draw_objects"]
+                 "vb_register_texture", "vb_unregister_texture", "vb_scene_n_draw_objects", "vb_scene_upload_fragment"]
 
 _bound = False
 
@@ -84,6 +84,7 @@ def _lib():
         lib.vb_scene_resolve.argtypes = [vp, vp]
         lib.vb_render_scene.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
         lib.vb_scene_upload_device.argtypes = [vp, vp, vp]
+        lib.vb_scene_upload_fragment.argtypes = [vp, vp, vp]
         lib.vb_path_dash.argtypes = [vp, C.c_double, vp, C.c_uint32, vp]
         lib.vb_register_texture.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_size_t, C.POINTER(_Image)]
         lib.vb_unregister_texture.argtypes = [vp, C.POINTER(_Image)]
