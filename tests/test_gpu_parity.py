@@ -642,7 +642,8 @@ def test_device_resolve_equals_host_resolve(renderer, oracle):
     """Resolver::resolve on the device (vb_scene_upload_streams: stream copies to their Layout offsets + the patch / padding /
     ramp kernels, k_resolve.cu): packed scene, gradient ramps and image atlas are byte-identical to the host-side resolve --
     all brush kinds, duplicated gradients (one ramp) and images (one atlas slot), premultiplied and straight interpolation,
-    unclosed clips (trailing PATH / END_CLIP tags), dashed strokes -- and so are the pixels."""
+    unclosed clips (trailing PATH / END_CLIP tags), dashed strokes -- and so are the pixels. Stops are compared as floats with
+    ==, by both resolves: -0 equals 0, and a stop holding a NaN equals nothing, itself included."""
     from vello_b200.scene_native import NativeScene
     from vello_b200.shapes import Affine, Circle, Rect, RoundedRect
     from vello_b200.encoding import FILL_NON_ZERO, FILL_EVEN_ODD, Gradient, Image, Stroke, EXTEND_REPEAT, MIX_SCREEN, COMPOSE_SRC_OVER
@@ -656,6 +657,11 @@ def test_device_resolve_equals_host_resolve(renderer, oracle):
         nat.fill(FILL_NON_ZERO, Affine.translate(10.0 * k, 0.0), g, None, Rect(10, 10, 290, 190))
     nat.fill(FILL_EVEN_ODD, Affine.IDENTITY, Gradient.radial((150, 100), 5.0, (160, 110), 80.0, stops[:2]), None, Circle(150.0, 100.0, 90.0))
     nat.fill(FILL_NON_ZERO, Affine.scale(1.2), Gradient.sweep((80, 60), 0.0, 6.0, stops), None, RoundedRect(30, 20, 150, 110, 9.0))
+    # the stops of the first ramp but for the sign of a zero, in an offset and in a colour channel: the same ramp
+    c1 = stops[1][1]
+    assert stops[0][0] == 0.0 and c1.r == 0.0
+    for zs in ([(-0.0, stops[0][1])] + stops[1:], stops[:1] + [(0.3, Color(-0.0, c1.g, c1.b, c1.a))] + stops[2:]):
+        nat.fill(FILL_NON_ZERO, Affine.translate(0.0, 15.0), Gradient.linear((0, 0), (300, 200), zs, EXTEND_REPEAT), None, Rect(20, 150, 120, 190))
     for im in (img_a, img_b, img_a):
         nat.draw_image(Image(im), Affine.translate(float(rng.uniform(0, 200)), float(rng.uniform(0, 100))) * Affine.scale(3.0))
     nat.stroke(Stroke(3.0, dash_pattern=(9.0, 4.0, 2.0), dash_offset=3.0), Affine.IDENTITY, Color.from_rgba8(255, 255, 255), None, Circle(200.0, 120.0, 60.0))
@@ -678,6 +684,17 @@ def test_device_resolve_equals_host_resolve(renderer, oracle):
         got = renderer.render_resident(p) and renderer.download_target(p)
         assert np.array_equal(got, want)
         assert_pixels(got, oracle.render(host, w, h, p.base_color.premul_rgba8_u32(), aa), aa)
+    # two patches with the same NaN-holding stops: two ramps (their texels are not compared: host make_ramp and k_make_ramps
+    # are not promised to agree on NaN)
+    nan_stops = [(0.0, Color(float("nan"), 0.5, 0.5)), (1.0, Color.from_rgba8(0, 0, 255))]
+    nan = NativeScene()
+    for k in range(2):
+        nan.fill(FILL_NON_ZERO, Affine.translate(20.0 * k, 0.0), Gradient.linear((0, 0), (100, 0), nan_stops), None, Rect(0, 0, 100, 50))
+    host = nan.resolve()
+    assert host.ramps.shape[0] == 2
+    assert nan.upload_device(renderer).as_array().tolist() == host.layout.as_array().tolist()
+    assert renderer.download("scene", np.uint32).tobytes() == host.scene.tobytes()
+    assert renderer.download("ramps", np.uint32).size == host.ramps.size
 
 
 @pytest.mark.parametrize("n", [2, 3, 5])

@@ -23,6 +23,7 @@
 
 #include "../../include/vello_b200.h"
 #include "vb_device.cuh"
+#include "vb_resolve.h"
 #include "vb_stages.h"
 #include "vb_textures.h"
 #include "vb_types.h"
@@ -135,8 +136,8 @@ struct Frame {
     uint32_t slot = 0;
 };
 
-// Composition (vb_compose). A ramp key is one distinct gradient ramp, (stops, interpolation space) compared as the host
-// resolve compares them (floats by ==); an image key is one atlas slot, (pixels pointer, width, height, hash of the pixels). Fragments hold
+// Composition (vb_compose). A ramp key is one distinct gradient ramp, (stops, interpolation space) compared as every
+// resolve compares them (vb_same_ramp); an image key is one atlas slot, (pixels pointer, width, height, hash of the pixels). Fragments hold
 // references to the keys of their patches, so de-duplicating a composed scene's ramps and images is a walk over the
 // instances' patch lists (stamp / local: the ramp id or atlas slot the key got in the compose numbered stamp).
 struct RampKey {
@@ -629,29 +630,39 @@ static int reserve_view_room(vb_renderer *r, size_t bytes) {
     return VB_OK;
 }
 
+// Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
+// until vb_set_cells says otherwise, and hit testing has no frame of it yet.
+static void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
+                      std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
+    vb_renderer::SceneSlot &s = *r->cur;
+    s.layout = L;
+    s.scene_words = scene_words;
+    s.n_ramps = n_ramps;
+    s.atlas_w = atlas_w;
+    s.atlas_h = atlas_h;
+    s.overridden = std::move(overridden);
+    s.composed = composed;
+    s.have_scene = true;
+    r->cells.clear();
+    hit_forget(r);
+}
+
 static int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
                      uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h) {
     if (!r || !layout || (scene_len && !scene) || (scene_len & 3)) return VB_E_INVALID;
     if (ramp_h && ramp_w != 512) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
-    memcpy(&r->cur->layout, layout, sizeof(VbLayout));
-    r->cur->scene_words = scene_len / 4;
+    VbLayout L;
+    memcpy(&L, layout, sizeof L);
+    if (!atlas) atlas_w = atlas_h = 0;
     int rc;
-    if ((rc = ensure(r, r->cur->scene, scene_bytes(r->cur->layout, r->cur->scene_words, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, scene_len / 4, r->view.on)))) return rc;
     if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
-    r->cur->n_ramps = ramp_h;
     if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
     if (ramp_h) CK(cudaMemcpyAsync(r->cur->ramps.p, ramps, (size_t)ramp_h * 512 * 4, cudaMemcpyHostToDevice, st));
-    r->cur->atlas_w = atlas ? atlas_w : 0;
-    r->cur->atlas_h = atlas ? atlas_h : 0;
-    if ((rc = ensure(r, r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4))) return rc;
-    if (r->cur->atlas_w && r->cur->atlas_h)
-        CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4, cudaMemcpyHostToDevice, st));
-    r->cur->overridden.clear(); // a caller-packed atlas: overrides do not apply
-    r->cur->composed = false;
-    r->cur->have_scene = true;
-    r->cells.clear(); // a new scene is one cell until vb_set_cells says otherwise
-    hit_forget(r);
+    if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
+    if (atlas_w && atlas_h) CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)atlas_w * atlas_h * 4, cudaMemcpyHostToDevice, st));
+    set_scene(r, L, scene_len / 4, ramp_h, atlas_w, atlas_h, {}, false); // a caller-packed atlas: overrides do not apply
     return VB_OK;
 }
 
@@ -2351,103 +2362,106 @@ extern "C" int vb_group_render(vb_group *g, const uint8_t *scene, size_t scene_l
 
 
 // ---- Resolver::resolve on the device (resolve.rs:183-399): see include/vello_b200.h and k_resolve.cu ---------------------------
-extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams *e, vb_layout *layout_out) {
-    if (!r || !e) return VB_E_INVALID;
+// Streams a resolve can read: a pointer for every stream with elements, stops for every ramp patch, every patch in the draw data.
+static int check_streams(vb_renderer *r, const vb_encoding_streams *e, const char *who) {
+    auto bad = [&](const char *why) {
+        r->err = std::string(who) + ": " + why;
+        return VB_E_INVALID;
+    };
     if ((e->n_path_tags && !e->path_tags) || (e->n_path_data && !e->path_data) || (e->n_draw_tags && !e->draw_tags) ||
         (e->n_draw_data && !e->draw_data) || (e->n_transforms && !e->transforms) || (e->n_styles && !e->styles) ||
         (e->n_ramp_patches && !e->ramp_patches) || (e->n_image_patches && !e->image_patches))
+        return bad("a stream with elements and no pointer");
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return bad("a ramp patch without stops or outside the draw data");
+    }
+    for (uint32_t i = 0; i < e->n_image_patches; i++)
+        if (e->image_patches[i].draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+    return VB_OK;
+}
+
+// The pixels of an image placed at (x, y): with an override on this renderer, a blit from its memory, kept in `over` for
+// refresh_overrides (*overridden). Otherwise the caller's to copy; a registered texture has pixels only as an override's.
+static int image_source(vb_renderer *r, const char *who, const void *key, uint32_t w, uint32_t h, uint32_t x, uint32_t y,
+                        std::vector<VbBlitRect> &blits, std::vector<vb_renderer::SceneSlot::OverridePlace> &over, bool *overridden) {
+    const auto ov = key ? r->overrides.find(key) : r->overrides.end();
+    *overridden = ov != r->overrides.end();
+    if (*overridden) {
+        const vb_renderer::Override &o = ov->second;
+        if (o.w != w || o.h != h) {
+            r->err = std::string(who) + ": an override's size differs from its image's (" + std::to_string(o.w) + "x" + std::to_string(o.h) + " vs " +
+                     std::to_string(w) + "x" + std::to_string(h) + ")";
+            return VB_E_INVALID;
+        }
+        blits.push_back(VbBlitRect{o.src, o.pitch, 0, w, h, x, y, 0, 0});
+        over.push_back({key, o.src, o.pitch, w, h, x, y, false});
+    } else if (vb_texture_key(key)) {
+        r->err = std::string(who) + ": a registered texture has no override on this renderer";
         return VB_E_INVALID;
-    int rc = drain_stream(r);
+    }
+    return VB_OK;
+}
+
+extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams *e, vb_layout *layout_out) {
+    if (!r || !e) return VB_E_INVALID;
+    int rc = check_streams(r, e, "vb_scene_upload_streams");
     if (rc) return rc;
+    VbLayout L;
+    uint32_t padded;
+    size_t total_words;
+    if (!vb_resolve_layout(e->n_path_tags, e->n_path_data, e->n_draw_tags, e->n_draw_data, e->n_transforms, e->n_styles, e->n_open_clips, e->n_paths,
+                           e->n_clips, vb_draw_info_sum(e->draw_tags, e->n_draw_tags), &L, &padded, &total_words)) {
+        r->err = "vb_scene_upload_streams: the scene exceeds 32-bit word offsets";
+        return VB_E_INVALID;
+    }
+    if ((rc = drain_stream(r))) return rc;
     CK(cudaSetDevice(r->device));
     cudaStream_t st = r->stream;
     std::vector<RsPatch> patches;
     std::vector<RsRamp> ramps;
     std::vector<vb_ramp_stop> stops;
+    // late-bound gradient ramps, de-duplicated by (stops, interpolation space) as the host resolve does
     std::vector<const vb_ramp_patch *> ramp_of;
-    // layout: sizes only (resolve.rs:107-154)
-    VbLayout L;
-    memset(&L, 0, sizeof L);
-    L.n_paths = e->n_paths;
-    L.n_clips = e->n_clips;
-    L.n_draw_objects = e->n_paths;
-    const uint32_t n_tags = e->n_path_tags + e->n_open_clips;
-    const uint32_t padded = (n_tags + 1023u) & ~1023u; // 4 * PATH_REDUCE_WG bytes (resolve.rs:625, config.rs:237)
-    uint32_t off = padded / 4u;
-    L.path_tag_base = 0;
-    L.path_data_base = off; off += e->n_path_data;
-    L.draw_tag_base = off; off += e->n_draw_tags + e->n_open_clips;
-    L.draw_data_base = off; off += e->n_draw_data;
-    L.transform_base = off; off += e->n_transforms * 6u;
-    L.style_base = off; off += e->n_styles * 2u;
-    const size_t total_words = off;
-    uint32_t info = 0;
-    for (uint32_t i = 0; i < e->n_draw_tags; i++) info += (e->draw_tags[i] >> 6) & 0xFu;
-    L.bin_data_start = info;
-    // late-bound gradient ramps, de-duplicated by (stops, interpolation space) as the ramp cache does
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
     for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
         const vb_ramp_patch &p = e->ramp_patches[i];
-        if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return VB_E_INVALID;
+        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(p.stops, p.n_stops, p.premul_interp != 0u)];
         uint32_t rid = (uint32_t)ramp_of.size();
-        for (uint32_t k = 0; k < ramp_of.size(); k++) {
+        for (uint32_t k : same_hash) {
             const vb_ramp_patch &q = *ramp_of[k];
-            if ((q.premul_interp != 0u) == (p.premul_interp != 0u) && q.n_stops == p.n_stops &&
-                memcmp(q.stops, p.stops, sizeof(vb_ramp_stop) * p.n_stops) == 0) { rid = k; break; }
+            if (vb_same_ramp(q.stops, q.n_stops, q.premul_interp != 0u, p.stops, p.n_stops, p.premul_interp != 0u)) { rid = k; break; }
         }
         if (rid == ramp_of.size()) {
+            same_hash.push_back(rid);
             ramp_of.push_back(&p);
             ramps.push_back(RsRamp{(uint32_t)stops.size(), p.n_stops, p.premul_interp ? 1u : 0u, 0u});
             stops.insert(stops.end(), p.stops, p.stops + p.n_stops);
         }
         patches.push_back(RsPatch{L.draw_data_base + p.draw_data_offset, (rid << 2) | p.extend});
     }
-    // late-bound images: shelf placement (ours; only the (x, y) written into the draw data matters to the pipeline)
-    struct Placed { const uint8_t *key; uint32_t w, h, x, y; };
+    // late-bound images: each distinct (pixels, width, height) placed once in the atlas, filled from an override on this
+    // renderer (one k_atlas_blit) or from the host
+    struct Placed { const uint8_t *key; uint32_t w, h, x, y; bool from_device; };
     std::vector<Placed> placed;
-    uint32_t atlas_w = 1, x = 0, y = 0, shelf_h = 0;
-    const uint32_t MAXW = 2048;
+    std::vector<VbBlitRect> blits;
+    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
+    VbShelfPacker shelf;
     for (uint32_t i = 0; i < e->n_image_patches; i++) {
         const vb_image_patch &im = e->image_patches[i];
-        if (im.draw_data_offset >= e->n_draw_data) return VB_E_INVALID;
         const Placed *hit = nullptr;
         for (const Placed &q : placed)
             if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
-        uint32_t px, py;
         if (!hit) {
-            if (x + im.width > MAXW) { y += shelf_h; x = 0; shelf_h = 0; }
-            placed.push_back(Placed{im.pixels, im.width, im.height, x, y});
-            px = x; py = y;
-            x += im.width;
-            if (im.height > shelf_h) shelf_h = im.height;
-            if (x > atlas_w) atlas_w = x;
-        } else {
-            px = hit->x; py = hit->y;
+            Placed q{im.pixels, im.width, im.height, 0, 0, false};
+            shelf.place(q.w, q.h, &q.x, &q.y);
+            if ((rc = image_source(r, "device resolve", q.key, q.w, q.h, q.x, q.y, blits, over, &q.from_device))) return rc;
+            placed.push_back(q);
+            hit = &placed.back();
         }
-        patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (px << 16) | py});
+        patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (hit->x << 16) | hit->y});
     }
-    const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
-    // images with an override on this renderer come from device memory (one k_atlas_blit); a registered texture needs one
-    std::vector<VbBlitRect> blits;
-    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
-    std::vector<bool> from_device(placed.size(), false);
-    for (size_t i = 0; i < placed.size(); i++) {
-        const Placed &q = placed[i];
-        const auto ov = q.key ? r->overrides.find(q.key) : r->overrides.end();
-        if (ov != r->overrides.end()) {
-            const vb_renderer::Override &o = ov->second;
-            if (o.w != q.w || o.h != q.h) {
-                r->err = "device resolve: an override's size differs from its image's (" + std::to_string(o.w) + "x" + std::to_string(o.h) +
-                         " vs " + std::to_string(q.w) + "x" + std::to_string(q.h) + ")";
-                return VB_E_INVALID;
-            }
-            blits.push_back(VbBlitRect{o.src, o.pitch, 0, q.w, q.h, q.x, q.y, 0, 0});
-            over.push_back({q.key, o.src, o.pitch, q.w, q.h, q.x, q.y, false});
-            from_device[i] = true;
-        } else if (vb_texture_key(q.key)) {
-            r->err = "device resolve: a registered texture has no override on this renderer";
-            return VB_E_INVALID;
-        }
-    }
+    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
 
     // the six streams go straight to their places in the packed buffer
     if ((rc = ensure(r, r->cur->scene, scene_bytes(L, total_words, r->view.on)))) return rc;
@@ -2469,16 +2483,12 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (sb) CK(cudaMemcpyAsync(tmp + o_s, stops.data(), sb, cudaMemcpyHostToDevice, st));
     vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags,
                              (const RsPatch *)tmp, (uint32_t)patches.size(), st);
-    r->cur->n_ramps = (uint32_t)ramps.size();
-    if ((rc = ensure(r, r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4))) return rc;
-    vb_launch_make_ramps((const RsRamp *)(tmp + o_r), (const RsStop *)(tmp + o_s), r->cur->n_ramps, (uint32_t *)r->cur->ramps.p, st);
-    r->cur->atlas_w = atlas_w;
-    r->cur->atlas_h = atlas_h;
+    if ((rc = ensure(r, r->cur->ramps, ramps.size() * 512 * 4))) return rc;
+    vb_launch_make_ramps((const RsRamp *)(tmp + o_r), (const RsStop *)(tmp + o_s), (uint32_t)ramps.size(), (uint32_t *)r->cur->ramps.p, st);
     if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
     CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
-    for (size_t i = 0; i < placed.size(); i++) {
-        const Placed &q = placed[i];
-        if (q.key && q.w && q.h && !from_device[i])
+    for (const Placed &q : placed) {
+        if (q.key && q.w && q.h && !q.from_device)
             CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
                                  cudaMemcpyHostToDevice, st));
     }
@@ -2486,71 +2496,30 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     CK(cudaGetLastError());
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
-    r->cur->overridden = std::move(over);
-    r->cur->composed = false;
-    r->cur->layout = L;
-    r->cur->scene_words = total_words;
-    r->cur->have_scene = true;
-    r->cells.clear();
-    hit_forget(r);
+    set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), false);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
 
 // ---- composition of resident fragments: vb_fragment_upload / vb_fragment_free / vb_compose (k_compose.cu) ---------------------
-static void stop_fields(const vb_ramp_stop &s, float v[5]) {
-    v[0] = s.offset; v[1] = s.r; v[2] = s.g; v[3] = s.b; v[4] = s.a;
-}
-// Stops compared as vb_scene_resolve compares them: float by float with ==, so -0 equals 0 (the hash maps both to 0).
-static uint64_t ramp_hash(const vb_ramp_stop *stops, uint32_t n, bool premul) {
-    uint64_t h = 1469598103934665603ull;
-    auto mix = [&](uint32_t v) { h = (h ^ v) * 1099511628211ull; };
-    mix(premul ? 1u : 0u);
-    mix(n);
-    for (uint32_t i = 0; i < n; i++) {
-        float v[5];
-        stop_fields(stops[i], v);
-        for (float x : v) {
-            uint32_t bits = 0u;
-            if (x != 0.0f) memcpy(&bits, &x, 4);
-            mix(bits);
-        }
-    }
-    return h;
-}
-static bool same_stops(const RampKey &k, const vb_ramp_patch &p) {
-    if (k.premul != (p.premul_interp != 0u) || k.stops.size() != p.n_stops) return false;
-    for (uint32_t i = 0; i < p.n_stops; i++) {
-        float a[5], b[5];
-        stop_fields(k.stops[i], a);
-        stop_fields(p.stops[i], b);
-        for (int c = 0; c < 5; c++)
-            if (!(a[c] == b[c])) return false;
-    }
-    return true;
-}
 // The ramp key of patch p, with one more reference. A key made here is appended to `fresh`: its stops still need a place in
 // the stop pool (place_stops).
 static RampKey *intern_ramp(vb_renderer *r, const vb_ramp_patch &p, std::vector<RampKey *> &fresh) {
-    bool self_equal = true;
-    for (uint32_t i = 0; i < p.n_stops; i++) {
-        float v[5];
-        stop_fields(p.stops[i], v);
-        for (float x : v) self_equal = self_equal && x == x;
-    }
-    const uint64_t h = ramp_hash(p.stops, p.n_stops, p.premul_interp != 0u);
+    const bool premul = p.premul_interp != 0u;
+    const bool self_equal = vb_same_ramp(p.stops, p.n_stops, premul, p.stops, p.n_stops, premul);
+    const uint64_t h = vb_ramp_hash(p.stops, p.n_stops, premul);
     if (self_equal) {
         const auto it = r->ramp_by_hash.find(h);
         if (it != r->ramp_by_hash.end())
             for (RampKey *k : it->second)
-                if (same_stops(*k, p)) {
+                if (vb_same_ramp(k->stops.data(), (uint32_t)k->stops.size(), k->premul, p.stops, p.n_stops, premul)) {
                     k->refs++;
                     return k;
                 }
     }
     std::unique_ptr<RampKey> k(new RampKey());
     k->stops.assign(p.stops, p.stops + p.n_stops);
-    k->premul = p.premul_interp != 0u;
+    k->premul = premul;
     k->self_equal = self_equal;
     k->id = r->next_ramp_key++;
     k->refs = 1;
@@ -2563,7 +2532,7 @@ static RampKey *intern_ramp(vb_renderer *r, const vb_ramp_patch &p, std::vector<
 static void release_ramp(vb_renderer *r, RampKey *k) {
     if (--k->refs) return;
     if (k->self_equal) {
-        auto it = r->ramp_by_hash.find(ramp_hash(k->stops.data(), (uint32_t)k->stops.size(), k->premul));
+        auto it = r->ramp_by_hash.find(vb_ramp_hash(k->stops.data(), (uint32_t)k->stops.size(), k->premul));
         it->second.erase(std::find(it->second.begin(), it->second.end(), k));
         if (it->second.empty()) r->ramp_by_hash.erase(it);
     }
@@ -2678,16 +2647,7 @@ extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, 
         return VB_E_INVALID;
     };
     if (!e || !fragment_out) return bad("NULL streams or id");
-    if ((e->n_path_tags && !e->path_tags) || (e->n_path_data && !e->path_data) || (e->n_draw_tags && !e->draw_tags) ||
-        (e->n_draw_data && !e->draw_data) || (e->n_transforms && !e->transforms) || (e->n_styles && !e->styles) ||
-        (e->n_ramp_patches && !e->ramp_patches) || (e->n_image_patches && !e->image_patches))
-        return bad("a stream with elements and no pointer");
-    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
-        const vb_ramp_patch &p = e->ramp_patches[i];
-        if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return bad("a ramp patch without stops or outside the draw data");
-    }
-    for (uint32_t i = 0; i < e->n_image_patches; i++)
-        if (e->image_patches[i].draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+    if (check_streams(r, e, "vb_fragment_upload")) return VB_E_INVALID;
     // the allocation: header, the six streams (tags padded to whole words), then one copy of each image key's pixels
     uint64_t off[CMP_HEADER_WORDS] = {};
     uint64_t w = CMP_HEADER_WORDS;
@@ -2773,7 +2733,7 @@ extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, 
     f->n_paths = e->n_paths;
     f->n_clips = e->n_clips;
     f->n_open_clips = e->n_open_clips;
-    for (uint32_t i = 0; i < e->n_draw_tags; i++) f->info += (e->draw_tags[i] >> 6) & 0xFu;
+    f->info = (uint32_t)vb_draw_info_sum(e->draw_tags, e->n_draw_tags);
     f->id = r->next_fragment++;
     r->fragment_bytes += bytes;
     *fragment_out = f->id;
@@ -2841,24 +2801,12 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
         n_open += fr[k]->n_open_clips;
         info += fr[k]->info;
     }
-    const uint64_t n_tags = tot[CMP_TAGS] + n_open, padded = (n_tags + 1023u) & ~1023ull;
-    const uint64_t total_words = padded / 4u + tot[CMP_PATH_DATA] + tot[CMP_DRAW_TAGS] + n_open + tot[CMP_DRAW_DATA] +
-                                 6u * tot[CMP_TRANSFORMS] + tot[CMP_STYLES];
-    // room for a view's transforms too (prepare), which share the scene's 32-bit word offsets
-    if (padded > 0xffffffffull || total_words + 6u * tot[CMP_TRANSFORMS] > 0xfffffff0ull || n_paths > 0xffffffffull || info > 0xffffffffull)
-        return bad("the composed scene exceeds 32-bit word offsets");
     VbLayout L;
-    memset(&L, 0, sizeof L);
-    L.n_paths = L.n_draw_objects = (uint32_t)n_paths;
-    L.n_clips = (uint32_t)n_clips;
-    L.bin_data_start = (uint32_t)info;
-    uint32_t o = (uint32_t)(padded / 4u);
-    L.path_tag_base = 0;
-    L.path_data_base = o; o += (uint32_t)tot[CMP_PATH_DATA];
-    L.draw_tag_base = o; o += (uint32_t)(tot[CMP_DRAW_TAGS] + n_open);
-    L.draw_data_base = o; o += (uint32_t)tot[CMP_DRAW_DATA];
-    L.transform_base = o; o += 6u * (uint32_t)tot[CMP_TRANSFORMS];
-    L.style_base = o;
+    uint32_t padded;
+    size_t total_words;
+    if (!vb_resolve_layout(tot[CMP_TAGS], tot[CMP_PATH_DATA], tot[CMP_DRAW_TAGS], tot[CMP_DRAW_DATA], tot[CMP_TRANSFORMS], tot[CMP_STYLES] / 2u, n_open,
+                           n_paths, n_clips, info, &L, &padded, &total_words))
+        return bad("the composed scene exceeds 32-bit word offsets");
 
     // late-bound ramps and images of every instance in order: the host resolve's de-duplication and shelf placement, keyed
     // by the keys the fragments hold
@@ -2868,8 +2816,7 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     std::vector<uint32_t> ramp_ids;
     struct Placed { const ImageKey *key; const uint8_t *src; uint32_t x, y, frag; };
     std::vector<Placed> placed;
-    uint32_t atlas_w = 1, x = 0, y = 0, shelf_h = 0;
-    const uint32_t MAXW = 2048;
+    VbShelfPacker shelf;
     uint32_t dd0 = L.draw_data_base;
     for (uint32_t k = 0; k < n; k++) {
         const Fragment &f = *fr[k];
@@ -2886,46 +2833,32 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
         for (const Fragment::Image &im : f.images) {
             ImageKey *key = im.key;
             if (key->stamp != seq) {
-                if (x + key->w > MAXW) { y += shelf_h; x = 0; shelf_h = 0; }
                 key->stamp = seq;
                 key->local = (uint32_t)placed.size();
-                placed.push_back(Placed{key, im.pixels, x, y, f.id});
-                x += key->w;
-                if (key->h > shelf_h) shelf_h = key->h;
-                if (x > atlas_w) atlas_w = x;
+                placed.push_back(Placed{key, im.pixels, 0, 0, f.id});
+                shelf.place(key->w, key->h, &placed.back().x, &placed.back().y);
             }
             const Placed &q = placed[key->local];
             patches.push_back(RsPatch{dd0 + im.dd, (q.x << 16) | q.y});
         }
         dd0 += f.len[CMP_DRAW_DATA];
     }
-    const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
+    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
     // images with an override on this renderer come from its device memory, the others from their fragment's copy
     std::vector<VbBlitRect> blits;
     std::vector<vb_renderer::SceneSlot::OverridePlace> over;
     std::vector<uint64_t> atlas_keys;
+    int rc;
     for (const Placed &q : placed) {
         const ImageKey &k = *q.key;
-        const auto ov = k.key ? r->overrides.find(k.key) : r->overrides.end();
+        bool overridden;
+        if ((rc = image_source(r, "vb_compose", k.key, k.w, k.h, q.x, q.y, blits, over, &overridden))) return rc;
+        if (!overridden && q.src) blits.push_back(VbBlitRect{q.src, (uint64_t)k.w * 4u, 0, k.w, k.h, q.x, q.y, 0, 0});
         // where the slot's pixels come from: the fragment, an override (never a fragment id), or nowhere (a zero region)
-        const uint32_t src_of = ov != r->overrides.end() ? CMP_FROM_OVERRIDE : q.src ? q.frag : 0u;
-        if (ov != r->overrides.end()) {
-            const vb_renderer::Override &ob = ov->second;
-            if (ob.w != k.w || ob.h != k.h)
-                return bad("an override's size differs from its image's (" + std::to_string(ob.w) + "x" + std::to_string(ob.h) + " vs " +
-                           std::to_string(k.w) + "x" + std::to_string(k.h) + ")");
-            blits.push_back(VbBlitRect{ob.src, ob.pitch, 0, k.w, k.h, q.x, q.y, 0, 0});
-            over.push_back({k.key, ob.src, ob.pitch, k.w, k.h, q.x, q.y, false});
-        } else if (vb_texture_key(k.key)) {
-            return bad("a registered texture has no override on this renderer");
-        } else if (q.src) {
-            blits.push_back(VbBlitRect{q.src, (uint64_t)k.w * 4u, 0, k.w, k.h, q.x, q.y, 0, 0});
-        }
-        atlas_keys.push_back((uint64_t)k.id << 32 | src_of);
+        atlas_keys.push_back((uint64_t)k.id << 32 | (overridden ? CMP_FROM_OVERRIDE : q.src ? q.frag : 0u));
     }
 
-    int rc = drain_stream(r);
-    if (rc) return rc;
+    if ((rc = drain_stream(r))) return rc;
     CK(cudaSetDevice(r->device));
     reap_freed(r);
     cudaStream_t st = r->stream;
@@ -2979,7 +2912,7 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     memcpy(a.dst, dst, sizeof dst);
     memcpy(a.units, units, sizeof units);
     vb_launch_compose(a, st);
-    vb_launch_resolve_finish(scene, (uint32_t)tot[CMP_TAGS], (uint32_t)n_open, (uint32_t)padded, L.draw_tag_base + (uint32_t)tot[CMP_DRAW_TAGS],
+    vb_launch_resolve_finish(scene, (uint32_t)tot[CMP_TAGS], (uint32_t)n_open, padded, L.draw_tag_base + (uint32_t)tot[CMP_DRAW_TAGS],
                              (const RsPatch *)(tmp + o_pat), (uint32_t)patches.size(), st);
     if (new_ramps) {
         vb_launch_make_ramps((const RsRamp *)(tmp + o_ramp), (const RsStop *)r->stop_pool.p, (uint32_t)ramps.size(), (uint32_t *)slot.ramps.p, st);
@@ -2991,16 +2924,7 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
         slot.atlas_keys = std::move(atlas_keys);
     }
     CK(cudaGetLastError());
-    slot.composed = true;
-    slot.overridden = std::move(over);
-    slot.n_ramps = (uint32_t)ramps.size();
-    slot.atlas_w = atlas_w;
-    slot.atlas_h = atlas_h;
-    slot.layout = L;
-    slot.scene_words = total_words;
-    slot.have_scene = true;
-    r->cells.clear();
-    hit_forget(r);
+    set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), true);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }

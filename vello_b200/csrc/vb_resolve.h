@@ -1,0 +1,89 @@
+// vb_resolve.h -- the decisions the library's three Resolver::resolve share, so that their output stays byte-identical: the host
+// resolve (vb_scene_resolve, vb_scene.cpp), the device resolve (vb_scene_upload_streams) and composition (vb_compose, vb_api.cu).
+// Internal to the library, and plain C++: vb_scene.cpp is built without the CUDA headers.
+#ifndef VB_RESOLVE_H
+#define VB_RESOLVE_H
+#include <stddef.h>
+#include <stdint.h>
+#include <string.h>
+
+#include "../../include/vello_b200.h"
+
+// The info words of a scene's draw tags (layout.bin_data_start).
+static inline uint64_t vb_draw_info_sum(const uint32_t *draw_tags, size_t n) {
+    uint64_t info = 0;
+    for (size_t i = 0; i < n; i++) info += (draw_tags[i] >> 6) & 0xFu;
+    return info;
+}
+
+// The packed scene's layout from the sizes of its streams (resolve.rs:107-154): the tag bytes and one PATH tag per open clip,
+// padded to 4 * PATH_REDUCE_WG bytes (resolve.rs:625, config.rs:237); path data; draw tags and one END_CLIP per open clip; draw
+// data; 6 words per transform; 2 per style. Sets *padded_tags (bytes) and *words (the whole scene). False when the scene, with
+// room behind it for a view's transforms, passes 32-bit word offsets. Layout: vb_layout, or vb_api.cu's VbLayout (the same record).
+template <class Layout>
+static inline bool vb_resolve_layout(uint64_t path_tags, uint64_t path_data, uint64_t draw_tags, uint64_t draw_data, uint64_t transforms,
+                                     uint64_t styles, uint64_t open_clips, uint64_t paths, uint64_t clips, uint64_t info, Layout *L,
+                                     uint32_t *padded_tags, size_t *words) {
+    const uint64_t padded = (path_tags + open_clips + 1023u) & ~1023ull;
+    const uint64_t total = padded / 4u + path_data + draw_tags + open_clips + draw_data + 6u * transforms + 2u * styles;
+    if (padded > 0xffffffffull || total + 6u * transforms > 0xfffffff0ull || paths > 0xffffffffull || info > 0xffffffffull) return false;
+    memset(L, 0, sizeof *L);
+    L->n_paths = L->n_draw_objects = (uint32_t)paths;
+    L->n_clips = (uint32_t)clips;
+    L->bin_data_start = (uint32_t)info;
+    L->path_tag_base = 0;
+    L->path_data_base = (uint32_t)(padded / 4u);
+    L->draw_tag_base = L->path_data_base + (uint32_t)path_data;
+    L->draw_data_base = L->draw_tag_base + (uint32_t)(draw_tags + open_clips);
+    L->transform_base = L->draw_data_base + (uint32_t)draw_data;
+    L->style_base = L->transform_base + 6u * (uint32_t)transforms;
+    *padded_tags = (uint32_t)padded;
+    *words = (size_t)total;
+    return true;
+}
+
+// Two gradient ramps are one when their interpolation spaces match and their stops compare float by float with ==: -0 equals 0,
+// and a stop holding a NaN equals nothing, itself included. vb_ramp_hash agrees (equal ramps hash alike).
+static inline bool vb_same_ramp(const vb_ramp_stop *a, uint32_t na, bool premul_a, const vb_ramp_stop *b, uint32_t nb, bool premul_b) {
+    if (premul_a != premul_b || na != nb) return false;
+    for (uint32_t i = 0; i < na; i++)
+        if (!(a[i].offset == b[i].offset && a[i].r == b[i].r && a[i].g == b[i].g && a[i].b == b[i].b && a[i].a == b[i].a)) return false;
+    return true;
+}
+static inline uint64_t vb_ramp_hash(const vb_ramp_stop *s, uint32_t n, bool premul) {
+    uint64_t h = 1469598103934665603ull;
+    auto mix = [&](uint32_t v) { h = (h ^ v) * 1099511628211ull; };
+    mix(premul ? 1u : 0u);
+    mix(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const float v[5] = {s[i].offset, s[i].r, s[i].g, s[i].b, s[i].a};
+        for (float x : v) {
+            uint32_t bits = 0u; // -0 and 0 alike
+            if (x != 0.0f) memcpy(&bits, &x, 4);
+            mix(bits);
+        }
+    }
+    return h;
+}
+
+// Shelf placement in the atlas (ours: only the (x, y) written into the draw data matters to the pipeline). Images go left to
+// right in rows up to 2048 wide; one that does not fit starts a new row below the tallest image of the last. The caller places
+// each distinct image once, in first-seen order.
+struct VbShelfPacker {
+    uint32_t width = 1, x = 0, y = 0, shelf_h = 0;
+    void place(uint32_t w, uint32_t h, uint32_t *px, uint32_t *py) {
+        if (x + w > 2048u) {
+            y += shelf_h;
+            x = 0;
+            shelf_h = 0;
+        }
+        *px = x;
+        *py = y;
+        x += w;
+        if (h > shelf_h) shelf_h = h;
+        if (x > width) width = x;
+    }
+    uint32_t height() const { return y + shelf_h > 1u ? y + shelf_h : 1u; }
+};
+
+#endif

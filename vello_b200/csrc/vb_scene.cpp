@@ -19,9 +19,11 @@
 #include <cstring>
 #include <initializer_list>
 #include <new>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/vello_b200_scene.h"
+#include "vb_resolve.h"
 #include "vb_textures.h"
 
 namespace {
@@ -32,7 +34,6 @@ constexpr uint32_t DRAWTAG_COLOR = 0x44, DRAWTAG_LINEAR_GRADIENT = 0x114, DRAWTA
                    DRAWTAG_IMAGE = 0x28C, DRAWTAG_BLUR_RECT = 0x2D4, DRAWTAG_BEGIN_CLIP = 0x49, DRAWTAG_END_CLIP = 0x21;
 constexpr uint32_t STYLE_FLAGS_STYLE_BIT = 0x80000000u, STYLE_FLAGS_FILL_BIT = 0x40000000u;
 constexpr uint32_t CLIP_BLEND_MODE = 0x8003u, LUMINANCE_MASK_BLEND_MODE = 0x10000u; // draw.rs:215-216
-constexpr uint32_t PATH_REDUCE_WG = 256;                                            // config.rs
 constexpr uint32_t N_RAMP_SAMPLES = 512;
 constexpr float EPS = 1e-12f; // path.rs:841
 
@@ -58,7 +59,6 @@ uint32_t f32_to_f16(float val) { // math.rs:93-127 (float_to_half_fast3)
 }
 
 struct Color { float r, g, b, a; };
-inline bool operator==(const Color &x, const Color &y) { return x.r == y.r && x.g == y.g && x.b == y.b && x.a == y.a; }
 inline Color multiply_alpha(Color c, float m) { return Color{c.r, c.g, c.b, c.a * m}; }
 uint32_t premul_rgba8(Color c) { // premultiply().to_rgba8().to_u32(), draw.rs:76-84; r is the low byte
     const float comps[4] = {c.r * c.a, c.g * c.a, c.b * c.a, c.a};
@@ -89,6 +89,7 @@ inline Affine mul(const Affine &a, const Affine &b) { // kurbo Affine * Affine
 
 struct Stop { float offset; Color color; };
 struct RampPatch { uint32_t draw_data_offset; std::vector<Stop> stops; uint32_t extend; bool premul; };
+inline const vb_ramp_stop *ramp_stops(const RampPatch &p) { return reinterpret_cast<const vb_ramp_stop *>(p.stops.data()); } // one record (streams_of)
 struct ImagePatch { uint32_t draw_data_offset; vb_image image; };
 struct Style { uint32_t flags; float width; };
 struct Xform { float c[6]; };
@@ -519,7 +520,6 @@ int push_layer_inner(vb_scene *s, uint32_t blend_mode, float alpha, uint32_t fil
 }
 
 inline float clamp01(float a) { return a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a); }
-inline uint32_t align_up(uint32_t n, uint32_t a) { return (n + a - 1) / a * a; }
 
 } // namespace
 
@@ -1334,97 +1334,75 @@ int vb_scene_batch(vb_scene *dst, const vb_scene *const *scenes, uint32_t n, uin
 int vb_scene_resolve(vb_scene *s, vb_packed *out) {
     if (!s || !out) return VB_E_INVALID;
     const Encoding &e = s->e;
-    std::vector<uint32_t> draw_data = e.draw_data;
+    vb_layout L;
+    uint32_t padded;
+    size_t total;
+    if (!vb_resolve_layout(e.path_tags.size(), e.path_data.size(), e.draw_tags.size(), e.draw_data.size(), e.transforms.size(), e.styles.size(),
+                           e.n_open_clips, e.n_paths, e.n_clips, vb_draw_info_sum(e.draw_tags.data(), e.draw_tags.size()), &L, &padded, &total))
+        return VB_E_INVALID;
+
+    // pack the six streams (resolve.rs:107-154); unclosed clips get a trailing PATH tag and END_CLIP draw tag each
+    s->packed.assign(total, 0u);
+    uint8_t *tag_bytes = reinterpret_cast<uint8_t *>(s->packed.data());
+    if (!e.path_tags.empty()) std::memcpy(tag_bytes, e.path_tags.data(), e.path_tags.size());
+    for (uint32_t i = 0; i < e.n_open_clips; i++) tag_bytes[e.path_tags.size() + i] = TAG_PATH;
+    if (!e.path_data.empty()) std::memcpy(&s->packed[L.path_data_base], e.path_data.data(), e.path_data.size() * 4);
+    uint32_t off = L.draw_tag_base;
+    for (uint32_t t : e.draw_tags) s->packed[off++] = t;
+    for (uint32_t i = 0; i < e.n_open_clips; i++) s->packed[off++] = DRAWTAG_END_CLIP;
+    if (!e.draw_data.empty()) std::memcpy(&s->packed[L.draw_data_base], e.draw_data.data(), e.draw_data.size() * 4);
+    off = L.transform_base;
+    for (const Xform &t : e.transforms)
+        for (int i = 0; i < 6; i++) s->packed[off++] = f32_bits(t.c[i]);
+    for (const Style &st : e.styles) {
+        s->packed[off++] = st.flags;
+        s->packed[off++] = f32_bits(st.width);
+    }
+    uint32_t *draw_data = s->packed.data() + L.draw_data_base;
+
     // late-bound gradient ramps, de-duplicated by (stops, interpolation space) -- ramp_cache.rs
     std::vector<const RampPatch *> ramp_of;
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
     s->ramps.clear();
     for (const RampPatch &p : e.ramp_patches) {
+        const uint32_t n = (uint32_t)p.stops.size();
+        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(ramp_stops(p), n, p.premul)];
         uint32_t rid = (uint32_t)ramp_of.size();
-        for (uint32_t k = 0; k < ramp_of.size(); k++) {
+        for (uint32_t k : same_hash) {
             const RampPatch &q = *ramp_of[k];
-            bool same = q.premul == p.premul && q.stops.size() == p.stops.size();
-            for (size_t i = 0; same && i < p.stops.size(); i++) same = q.stops[i].offset == p.stops[i].offset && q.stops[i].color == p.stops[i].color;
-            if (same) { rid = k; break; }
+            if (vb_same_ramp(ramp_stops(q), (uint32_t)q.stops.size(), q.premul, ramp_stops(p), n, p.premul)) { rid = k; break; }
         }
         if (rid == ramp_of.size()) {
+            same_hash.push_back(rid);
             ramp_of.push_back(&p);
             s->ramps.resize(s->ramps.size() + N_RAMP_SAMPLES);
             make_ramp(p.stops, p.premul, s->ramps.data() + (size_t)rid * N_RAMP_SAMPLES);
         }
         draw_data[p.draw_data_offset] = (rid << 2) | p.extend;
     }
-    // late-bound images: shelf-packed atlas (placement is ours; only the (x, y) written into the draw data matters)
+    // late-bound images: each distinct (pixels, width, height) placed once in the atlas
     struct Placed { const uint8_t *key; uint32_t w, h, x, y; };
     std::vector<Placed> placed;
-    uint32_t atlas_w = 1, x = 0, y = 0, shelf_h = 0;
-    const uint32_t MAXW = 2048;
+    VbShelfPacker shelf;
     for (const ImagePatch &p : e.image_patches) {
         const vb_image &im = p.image;
         const Placed *hit = nullptr;
         for (const Placed &q : placed)
             if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
-        uint32_t px, py;
         if (!hit) {
-            if (x + im.width > MAXW) {
-                y += shelf_h;
-                x = 0;
-                shelf_h = 0;
-            }
-            placed.push_back(Placed{im.pixels, im.width, im.height, x, y});
-            px = x; py = y;
-            x += im.width;
-            if (im.height > shelf_h) shelf_h = im.height;
-            if (x > atlas_w) atlas_w = x;
-        } else {
-            px = hit->x; py = hit->y;
+            placed.push_back(Placed{im.pixels, im.width, im.height, 0, 0});
+            shelf.place(im.width, im.height, &placed.back().x, &placed.back().y);
+            hit = &placed.back();
         }
-        draw_data[p.draw_data_offset] = (px << 16) | py;
+        draw_data[p.draw_data_offset] = (hit->x << 16) | hit->y;
     }
-    const uint32_t atlas_h = (y + shelf_h) > 1u ? (y + shelf_h) : 1u;
+    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
     s->atlas.assign((size_t)atlas_w * atlas_h * 4, 0);
     // a registered texture's key points at nothing (its pixels exist only in device memory): its region stays zero, as for NULL
     for (const Placed &q : placed)
         for (uint32_t row = 0; row < q.h && q.key && !vb_texture_key(q.key); row++)
             std::memcpy(&s->atlas[((size_t)(q.y + row) * atlas_w + q.x) * 4], q.key + (size_t)row * q.w * 4, (size_t)q.w * 4);
 
-    // pack the six streams (resolve.rs:107-154); unclosed clips get a trailing PATH tag and END_CLIP draw tag each
-    vb_layout L;
-    std::memset(&L, 0, sizeof L);
-    L.n_paths = e.n_paths;
-    L.n_clips = e.n_clips;
-    const uint32_t n_tags = (uint32_t)e.path_tags.size() + e.n_open_clips;
-    const uint32_t padded = align_up(n_tags, 4 * PATH_REDUCE_WG);
-    const size_t total = (size_t)padded / 4 + e.path_data.size() + e.draw_tags.size() + e.n_open_clips + draw_data.size() + e.transforms.size() * 6 +
-                         e.styles.size() * 2;
-    s->packed.assign(total, 0u);
-    uint8_t *tag_bytes = reinterpret_cast<uint8_t *>(s->packed.data());
-    if (!e.path_tags.empty()) std::memcpy(tag_bytes, e.path_tags.data(), e.path_tags.size());
-    for (uint32_t i = 0; i < e.n_open_clips; i++) tag_bytes[e.path_tags.size() + i] = TAG_PATH;
-    uint32_t off = padded / 4;
-    L.path_tag_base = 0;
-    L.path_data_base = off;
-    if (!e.path_data.empty()) std::memcpy(&s->packed[off], e.path_data.data(), e.path_data.size() * 4);
-    off += (uint32_t)e.path_data.size();
-    L.draw_tag_base = off;
-    uint32_t info = 0;
-    for (uint32_t t : e.draw_tags) {
-        s->packed[off++] = t;
-        info += (t >> 6) & 0xFu;
-    }
-    for (uint32_t i = 0; i < e.n_open_clips; i++) s->packed[off++] = DRAWTAG_END_CLIP;
-    L.bin_data_start = info;
-    L.draw_data_base = off;
-    if (!draw_data.empty()) std::memcpy(&s->packed[off], draw_data.data(), draw_data.size() * 4);
-    off += (uint32_t)draw_data.size();
-    L.transform_base = off;
-    for (const Xform &t : e.transforms)
-        for (int i = 0; i < 6; i++) s->packed[off++] = f32_bits(t.c[i]);
-    L.style_base = off;
-    for (const Style &st : e.styles) {
-        s->packed[off++] = st.flags;
-        s->packed[off++] = f32_bits(st.width);
-    }
-    L.n_draw_objects = L.n_paths;
     out->scene = reinterpret_cast<const uint8_t *>(s->packed.data());
     out->scene_len = s->packed.size() * 4;
     out->layout = L;
@@ -1441,8 +1419,7 @@ int vb_scene_resolve(vb_scene *s, vb_packed *out) {
 static void streams_of(const Encoding &e, std::vector<vb_ramp_patch> &rps, std::vector<vb_image_patch> &ips, vb_encoding_streams *st) {
     static_assert(sizeof(Stop) == sizeof(vb_ramp_stop) && sizeof(Xform) == 24 && sizeof(Style) == 8, "stream record layouts");
     for (const RampPatch &p : e.ramp_patches)
-        rps.push_back(vb_ramp_patch{p.draw_data_offset, p.extend, p.premul ? 1u : 0u, (uint32_t)p.stops.size(),
-                                    reinterpret_cast<const vb_ramp_stop *>(p.stops.data())});
+        rps.push_back(vb_ramp_patch{p.draw_data_offset, p.extend, p.premul ? 1u : 0u, (uint32_t)p.stops.size(), ramp_stops(p)});
     for (const ImagePatch &p : e.image_patches) ips.push_back(vb_image_patch{p.draw_data_offset, p.image.width, p.image.height, p.image.pixels});
     std::memset(st, 0, sizeof *st);
     st->path_tags = e.path_tags.data(); st->n_path_tags = (uint32_t)e.path_tags.size();
