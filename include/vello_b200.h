@@ -364,6 +364,36 @@ typedef struct {
 int vb_fragment_upload(vb_renderer *, const vb_encoding_streams *, uint32_t *fragment_out);
 int vb_fragment_free(vb_renderer *, uint32_t fragment);
 int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
+/* Bind the instance transforms of the composed scene to device memory (an addition; no vello counterpart). A simulation, an
+ * animation or a layout model that writes its instances' transforms on the GPU moves them without a host call per frame:
+ *  - Rows. Row k is at device_transforms + k * row_pitch_bytes. It holds six f32 values [a b c d e f] in kurbo Affine order.
+ *  - What a frame renders. While the array is bound, every frame renders the scene that vb_compose would have made with the
+ *    same fragments in the same order, with instance k as Some(row k). This includes instances that were composed with
+ *    has_transform = 0. The scene's products row_k * T are bit-identical to vb_compose given transform = (double)row_k for
+ *    every instance: both use the same f32 product (Encoding::append's, without FMA).
+ *  - When the array is read. A frame reads the array when it runs on vb_stream, in the frame's first stage (like a view's
+ *    coefficients). The caller orders its writes before the frame, on vb_stream or with a synchronisation, and does not write
+ *    the array while a frame that reads it is running. A blocking frame that is re-run after an arena overflow reads the same
+ *    contents again; an enqueued frame is never re-run (vb_frame_finish). The caller keeps the memory alive while it is bound.
+ *    Changing only the contents replays the captured frame graph; nothing crosses PCIe per frame.
+ *  - Non-finite rows. If a row has a coefficient that is not finite, that instance keeps the transform it was composed with
+ *    (Some(T_k) or None) for that frame.
+ *  - Views. A view applies on top: a viewed frame renders V * (row_k * T), the same two f32 products as vb_compose followed by
+ *    vb_set_view. Culling to the frame stays tied to the view: on exactly while a view is set (set the identity view to cull
+ *    without panning).
+ *  - Other state. The binding survives vb_set_cells, vb_set_view and vb_hit_test; hit tests answer from the last frame, bound or
+ *    not. Every scene installation unbinds: every upload form, vb_render, vb_render_begin and vb_compose. device_transforms NULL
+ *    unbinds; frames then render the scene as composed.
+ *  - Fragments. The call copies what it needs from the fragments (their untransformed transforms) and from the compose (each
+ *    instance's transform prefix and compose-time transform): freeing fragments afterwards does not affect bound frames.
+ *  - Binding, unbinding, or binding another pointer, pitch or n changes the frame's key, so the next frame captures its graph
+ *    anew.
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: the current scene was not made by
+ * vb_compose; n is 0 or not the last compose's instance count; a pointer that is not device memory of the renderer's device
+ * (or managed memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 24, or 4 GiB or more; a fragment of
+ * that compose freed before the call; a renderer of a vb_group or with the exchange enabled; a call between vb_render_enqueue
+ * and vb_frame_finish; a scene whose bound transforms plus a view's would pass 32-bit word offsets. */
+int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- one frame on several GPUs of one box (SURVEY.md 8e, north_star: "a single frame shards across the GPUs by stripes") ----
  * The frame is cut into horizontal stripes of tile rows, one per device; every device runs the element stages on the scene and

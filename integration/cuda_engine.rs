@@ -81,6 +81,9 @@ extern "C" {
     pub fn vb_fragment_upload(r: *mut VbRenderer, e: *const VbEncodingStreams, fragment_out: *mut u32) -> c_int;
     pub fn vb_fragment_free(r: *mut VbRenderer, fragment: u32) -> c_int;
     pub fn vb_compose(r: *mut VbRenderer, instances: *const VbInstance, n: u32, layout_out: *mut Layout, draw_offsets: *mut u32) -> c_int;
+    // every frame reads instance k's transform from row k of device memory ([a b c d e f] f32, row_pitch_bytes apart), so a
+    // simulation that writes its transforms on vb_stream moves the instances without a compose per frame; NULL unbinds
+    pub fn vb_bind_instance_transforms(r: *mut VbRenderer, device_transforms: *const f32, n: u32, row_pitch_bytes: usize) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

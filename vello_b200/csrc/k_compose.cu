@@ -14,6 +14,9 @@
 // the last tag are stored as zero; k_resolve_finish, which runs next, writes the padding and the PATH tags of open clips.
 // Transforms are written whole, multiplied by the instance's transform (vb_affine_mul: Encoding::append's f32 product) when
 // it has one. Patch words of the draw data are copied as the encoder left them; k_resolve_finish patches them too.
+//
+// k_instance_transforms, at the end, is the per-frame half of bound instance transforms: the transform stream again, with each
+// instance's transform read from device memory when the frame runs.
 #include "vb_device.cuh"
 #include "vb_stages.h"
 
@@ -126,6 +129,52 @@ __global__ void __launch_bounds__(CP_THREADS) k_compose_streams(const CmpArgs a)
             if (u < u1) out[u] = v[j];
         }
     }
+}
+
+// Bound instance transforms (vb_bind_instance_transforms): transform u of the composed scene belongs to instance
+// k = cp_find(prefix, u) and is rendered as row_k * T, the product vb_compose makes for transform = row k, T being the
+// fragment's untransformed transform. A row with a coefficient that is not finite leaves its instance as composed (the
+// compose-time transform, or T itself for an instance appended without one), so that no NaN reaches flatten.
+__global__ void __launch_bounds__(256) k_instance_transforms(const uint8_t *__restrict__ rows, uint32_t pitch, const uint32_t *__restrict__ prefix,
+                                                             const CmpXform *__restrict__ xf, const uint32_t *__restrict__ src, uint32_t *dst,
+                                                             uint32_t n, uint32_t n_transforms) {
+    const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= n_transforms) return;
+    const uint32_t k = cp_find(prefix, 0u, n - 1u, u);
+    const float *row = reinterpret_cast<const float *>(rows + (size_t)k * pitch);
+    float m[6], t[6], r[6];
+    bool finite = true;
+#pragma unroll
+    for (int i = 0; i < 6; i++) {
+        m[i] = __ldg(row + i);
+        finite = finite && isfinite(m[i]);
+        t[i] = __uint_as_float(__ldg(src + 6u * u + i));
+    }
+    bool on = true;
+    if (!finite) {
+        const CmpXform x = xf[k];
+        on = x.on != 0u;
+#pragma unroll
+        for (int i = 0; i < 6; i++) m[i] = x.m[i];
+    }
+    if (on) {
+        vb_affine_mul(m, t, r);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 6; i++) r[i] = t[i];
+    }
+#pragma unroll
+    for (int i = 0; i < 6; i++) dst[6u * u + i] = __float_as_uint(r[i]);
+}
+
+extern "C" uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (!b.inst_rows) return 0u;
+    // the bound region prepare reserved: [transform_base, scene_words), or the view's source with a view on top of it
+    const uint32_t n = (cfg.scene_words - cfg.layout.transform_base) / 6u;
+    if (n == 0u) return 0u;
+    uint32_t *dst = const_cast<uint32_t *>(b.scene) + (b.view ? cfg.view_src : cfg.layout.transform_base);
+    k_instance_transforms<<<(n + 255u) / 256u, 256, 0, st>>>(b.inst_rows, b.inst_pitch, b.inst_prefix, b.inst_xf, b.inst_src, dst, b.inst_n, n);
+    return 1u;
 }
 
 extern "C" uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st) {

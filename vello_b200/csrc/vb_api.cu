@@ -207,6 +207,9 @@ struct vb_renderer {
         bool composed = false;
         std::vector<uint32_t> ramp_keys;
         std::vector<uint64_t> atlas_keys;
+        // the composed scene's instances, for vb_bind_instance_transforms: each one's fragment id and compose-time transform
+        std::vector<uint32_t> inst_frag;
+        std::vector<CmpXform> inst_xf;
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -309,6 +312,15 @@ struct vb_renderer {
     uint8_t *compose_host = nullptr;
     size_t compose_host_cap = 0;
     cudaEvent_t compose_staged = nullptr; // the last copy out of compose_host
+    // bound instance transforms (vb_bind_instance_transforms) of the current scene: the caller's rows (nullptr: unbound), and
+    // the binding's tables in inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n), at
+    // o_xf] [the fragments' untransformed transforms, at o_src]. Every scene installation unbinds (set_scene).
+    struct Binding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+        size_t o_xf = 0, o_src = 0;
+    } bound;
+    DevBuf inst_tables;
 
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
@@ -328,7 +340,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp};
+                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -605,13 +617,15 @@ static uint32_t n_transforms(const VbLayout &L, size_t scene_words) {
     if (L.style_base < L.transform_base || L.style_base > scene_words) return 0u;
     return (L.style_base - L.transform_base) / 6u;
 }
-// A scene slot's allocation: the packed scene, then (while a view is set) room for its viewed transforms (k_view.cu), then slack.
-static size_t scene_bytes(const VbLayout &L, size_t scene_words, bool view) {
-    return (scene_words + (view ? 6u * (size_t)n_transforms(L, scene_words) : 0u)) * 4u + 64u;
+// A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
+// transforms, k_compose.cu; viewed transforms, k_view.cu), then slack.
+static size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions) {
+    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words)) * 4u + 64u;
 }
-// A view set after the scene's upload: move the current slot's scene into an allocation with room for its viewed transforms.
-// The scene may still be arriving on the upload stream, and frames already enqueued read the old allocation.
-static int reserve_view_room(vb_renderer *r, size_t bytes) {
+// A view set or transforms bound after the scene's upload: move the current slot's scene into an allocation with room for the
+// transforms frames write. The scene may still be arriving on the upload stream, and frames already enqueued read the old
+// allocation.
+static int reserve_transform_room(vb_renderer *r, size_t bytes) {
     DevBuf &sc = r->cur->scene;
     if (sc.cap >= bytes) return VB_OK;
     CK(cudaStreamSynchronize(r->upload_stream));
@@ -622,7 +636,7 @@ static int reserve_view_room(vb_renderer *r, size_t bytes) {
     const cudaError_t e = cudaMemcpy(grown.p, sc.p, r->cur->scene_words * 4, cudaMemcpyDeviceToDevice);
     if (e != cudaSuccess) {
         cudaFree(grown.p);
-        r->err = std::string("view: moving the scene: ") + cudaGetErrorString(e);
+        r->err = std::string("moving the scene: ") + cudaGetErrorString(e);
         return VB_E_CUDA;
     }
     CK(cudaFree(sc.p));
@@ -631,7 +645,7 @@ static int reserve_view_room(vb_renderer *r, size_t bytes) {
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
-// until vb_set_cells says otherwise, and hit testing has no frame of it yet.
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms are bound to it.
 static void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                       std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
     vb_renderer::SceneSlot &s = *r->cur;
@@ -642,8 +656,11 @@ static void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uin
     s.atlas_h = atlas_h;
     s.overridden = std::move(overridden);
     s.composed = composed;
+    s.inst_frag.clear(); // vb_compose fills them afterwards
+    s.inst_xf.clear();
     s.have_scene = true;
     r->cells.clear();
+    r->bound = vb_renderer::Binding{};
     hit_forget(r);
 }
 
@@ -747,14 +764,23 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
+    const uint32_t n_regions = (r->bound.rows ? 1u : 0u) + (r->view.on ? 1u : 0u);
+    if (r->bound.rows) {
+        // the frame reads its instances' transforms past the scene's streams: [transform_base, scene_words) is the region
+        // k_instance_transforms writes from the caller's rows
+        c.layout.transform_base = c.scene_words;
+        c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
+    }
     if (r->view.on) {
-        // the frame reads the viewed transforms past the scene's streams: [transform_base, scene_words) is the region
-        // k_view_transforms writes, empty for a layout whose transforms do not lie inside the uploaded words
+        // the frame reads the viewed transforms past the scene's streams (and the bound region): [transform_base, scene_words)
+        // is the region k_view_transforms writes, empty for a layout whose transforms do not lie inside the uploaded words
         c.view_src = c.layout.transform_base;
         c.layout.transform_base = c.scene_words;
         c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
         c.frame_cull = 1u;
-        int rc0 = reserve_view_room(r, (size_t)c.scene_words * 4u + 64u);
+    }
+    if (n_regions) {
+        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions));
         if (rc0) return rc0;
     }
     c.n_cells = n_cells;
@@ -820,6 +846,15 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     b.mask8 = (const uint32_t *)r->mask8.p;
     b.mask16 = (const uint32_t *)r->mask16.p;
     b.view = r->view.on ? (const float *)r->view_coef.p : nullptr;
+    if (r->bound.rows) {
+        const char *t = (const char *)r->inst_tables.p;
+        b.inst_rows = r->bound.rows;
+        b.inst_prefix = (const uint32_t *)t;
+        b.inst_xf = (const CmpXform *)(t + r->bound.o_xf);
+        b.inst_src = (const uint32_t *)(t + r->bound.o_src);
+        b.inst_n = r->bound.n;
+        b.inst_pitch = r->bound.pitch;
+    }
     b.tag_monoids = (VbTagMonoid *)r->tag_monoids.p;
     b.path_bboxes = (VbPathBbox *)r->path_bboxes.p;
     b.draw_monoids = (VbDrawMonoid *)r->draw_monoids.p;
@@ -940,7 +975,9 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_FLATTEN: {
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
-            // a viewed frame first writes its transforms (read by flatten and draw), inside flatten's stage events
+            // a frame with bound instance transforms or a view first writes its transforms (read by flatten and draw), the
+            // bound ones first (the view's source), inside flatten's stage events
+            launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             VbConfig cf = c;
             uint32_t p0 = 0u, p1 = b.parts_flatten;
@@ -956,7 +993,9 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             break;
         }
         case VB_STAGE_ID_DRAW:
-            // a range that starts here writes them again: the kernel only reads the scene's own, so the words are the same
+            // a range that starts here writes them again: the kernels only read the scene's own and the caller's rows, so the
+            // words are the same
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);
@@ -1547,6 +1586,7 @@ struct NamedBuf {
     const char *name;
     DevBuf *buf;
     size_t bytes;
+    size_t off = 0; // where the bytes start in buf
 };
 static std::vector<NamedBuf> named(vb_renderer *r) {
     const VbConfig &c = r->cfg;
@@ -1566,6 +1606,9 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
         {"bin_headers", &r->bin_headers, (size_t)((L.n_draw_objects + 255u) / 256u) * aligned_n_bins * sizeof(VbBinHeader)},
         {"paths", &r->paths, (size_t)L.n_draw_objects * sizeof(VbPath)},
     };
+    // the transform words the last frame read from its transform_base: the bound or viewed region, else the scene's stream
+    const size_t t_off = (size_t)c.layout.transform_base * 4u, t_cap = r->cur->scene.cap > t_off ? r->cur->scene.cap - t_off : 0u;
+    v.push_back({"transforms", &r->cur->scene, std::min<size_t>(24u * (size_t)n_transforms(L, r->cur->scene_words), t_cap), t_off});
     // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
     const uint32_t *size = &c.lines_size;
     for (int a = 0; a < N_ARENAS; a++) {
@@ -1695,7 +1738,7 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
         if (!strcmp(name, nb.name)) {
             if (bytes) *bytes = nb.bytes;
             size_t n = nb.bytes < cap ? nb.bytes : cap;
-            if (dst && n) CK(cudaMemcpy(dst, nb.buf->p, n, cudaMemcpyDeviceToHost));
+            if (dst && n) CK(cudaMemcpy(dst, (const char *)nb.buf->p + nb.off, n, cudaMemcpyDeviceToHost));
             return VB_OK;
         }
     return VB_E_UNKNOWN_BUFFER;
@@ -2925,7 +2968,97 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     }
     CK(cudaGetLastError());
     set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), true);
+    slot.inst_frag.resize(n);
+    for (uint32_t k = 0; k < n; k++) slot.inst_frag[k] = fr[k]->id;
+    slot.inst_xf = std::move(xf);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
+    return VB_OK;
+}
+
+// ---- bound instance transforms: vb_bind_instance_transforms (k_compose.cu) ----------------------------------------------------
+// The binding's tables are made once, here: the transform prefix and compose-time transforms from the slot's instance records,
+// the untransformed transforms by one k_compose_streams over the transform stream alone (no transforms applied, destination 0).
+// Every frame after that reads the caller's rows in its k_instance_transforms.
+extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_transforms, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_instance_transforms: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_transforms) {
+        r->bound = vb_renderer::Binding{};
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene || !slot.composed) return bad("the renderer's current scene was not made by vb_compose");
+    if (n == 0u || n != slot.inst_frag.size())
+        return bad(std::to_string(n) + " rows for a composed scene of " + std::to_string(slot.inst_frag.size()) + " instances");
+    if ((uintptr_t)device_transforms & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 24u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 24 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_transforms)) return bad("the rows must be memory of the renderer's device");
+    std::vector<const Fragment *> fr(n);
+    for (uint32_t k = 0; k < n; k++) {
+        const auto it = r->fragments.find(slot.inst_frag[k]);
+        if (it == r->fragments.end()) return bad("fragment " + std::to_string(slot.inst_frag[k]) + " of the composed scene was freed");
+        fr[k] = it->second.get();
+    }
+    // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one)
+    const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr > 0xfffffff0ull)
+        return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
+
+    // staged through pinned memory: [the copy's tables: prefix (6 x (n + 1), transform row only), fragment addresses, zero
+    // transforms] [the binding's tables: prefix (n + 1), compose-time transforms]
+    reap_freed(r);
+    auto up16 = [](size_t v) { return (v + 15u) & ~(size_t)15u; };
+    const size_t o_src = up16((size_t)CMP_STREAMS * (n + 1u) * 4u), o_xf0 = up16(o_src + (size_t)n * 8u);
+    const size_t tmp_bytes = up16(o_xf0 + (size_t)n * sizeof(CmpXform));
+    const size_t o_xf = up16(((size_t)n + 1u) * 4u), o_tr = up16(o_xf + (size_t)n * sizeof(CmpXform));
+    const size_t staged = tmp_bytes + o_tr;
+    CK(cudaEventSynchronize(r->compose_staged));
+    if (r->compose_host_cap < staged) {
+        if (r->compose_host) CK(cudaFreeHost(r->compose_host));
+        r->compose_host = nullptr;
+        r->compose_host_cap = 0;
+        CK(cudaMallocHost((void **)&r->compose_host, staged));
+        r->compose_host_cap = staged;
+    }
+    uint8_t *h = r->compose_host;
+    memset(h, 0, tmp_bytes);
+    uint32_t *P = (uint32_t *)h + (size_t)CMP_TRANSFORMS * (n + 1u), *Pb = (uint32_t *)(h + tmp_bytes);
+    for (uint32_t k = 0; k < n; k++) P[k + 1] = P[k] + fr[k]->len[CMP_TRANSFORMS];
+    memcpy(Pb, P, ((size_t)n + 1u) * 4u);
+    unsigned long long *srcs = (unsigned long long *)(h + o_src);
+    for (uint32_t k = 0; k < n; k++) srcs[k] = (unsigned long long)(uintptr_t)fr[k]->mem;
+    memcpy(h + tmp_bytes + o_xf, slot.inst_xf.data(), (size_t)n * sizeof(CmpXform));
+
+    int rc;
+    if ((rc = compose_room(r, r->compose_tmp, tmp_bytes))) return rc;
+    if ((rc = compose_room(r, r->inst_tables, o_tr + (size_t)n_tr * 24u))) return rc;
+    cudaStream_t st = r->stream;
+    char *tmp = (char *)r->compose_tmp.p, *tables = (char *)r->inst_tables.p;
+    CK(cudaMemcpyAsync(tmp, h, tmp_bytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tables, h + tmp_bytes, o_tr, cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(r->compose_staged, st));
+    CmpArgs a;
+    memset(&a, 0, sizeof a);
+    a.scene = (uint32_t *)(tables + o_tr);
+    a.prefix = (const uint32_t *)tmp;
+    a.src = (const unsigned long long *)(tmp + o_src);
+    a.xf = (const CmpXform *)(tmp + o_xf0);
+    a.n = n;
+    a.units[CMP_TRANSFORMS] = n_tr;
+    vb_launch_compose(a, st);
+    CK(cudaGetLastError());
+    r->bound.rows = (const uint8_t *)device_transforms;
+    r->bound.n = n;
+    r->bound.pitch = (uint32_t)row_pitch_bytes;
+    r->bound.o_xf = o_xf;
+    r->bound.o_src = o_tr;
     return VB_OK;
 }
 

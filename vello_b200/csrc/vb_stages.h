@@ -13,6 +13,7 @@
 
 struct FlLit; // flatten's scratch records (k_flatten.cu)
 struct FlJob;
+struct CmpXform; // an instance's transform (k_compose.cu, below)
 
 // The device buffers a frame's launches read and write: the current scene slot's inputs, every intermediate and arena, and
 // the look-back regions of the control block with their partition counts. prepare() (vb_api.cu) fills it once every buffer
@@ -23,6 +24,13 @@ struct VbFrameBufs {
     const uint8_t *atlas;
     const uint32_t *mask8, *mask16;
     const float *view; // the view's six f32 coefficients (vb_set_view), written in stream order; read by k_view_transforms
+    // bound instance transforms (vb_bind_instance_transforms), read by k_instance_transforms: the caller's rows (instance k's
+    // at inst_rows + k * inst_pitch bytes) and the binding's tables: the exclusive prefix of the instances' transform counts
+    // (inst_n + 1), their compose-time transforms (inst_n) and the fragments' untransformed transforms. Null while unbound.
+    const uint8_t *inst_rows;
+    const uint32_t *inst_prefix;
+    const CmpXform *inst_xf;
+    const uint32_t *inst_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -50,6 +58,7 @@ struct VbFrameBufs {
     size_t ctl_words;
     uint32_t *lb_pathtag, *lb_flatten, *lb_draw, *lb_tile, *lb_clip, *lb_backdrop;
     uint32_t parts_pathtag, parts_flatten, parts_draw, parts_tile, parts_backdrop;
+    uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
     int sm_count; // the grids of the persistent and grid-stride kernels are sized from it
 
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
@@ -131,6 +140,9 @@ struct CmpArgs {
     uint32_t cta0[6];             // first CTA of each stream (set by the launcher)
 };
 uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
+// bound instance transforms: row_k * T of every transform T of the composed scene into the frame's bound region (prepare,
+// vb_api.cu), in flatten's stage before the view's transforms; nothing while unbound
+uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)

@@ -164,6 +164,7 @@ def load_library() -> C.CDLL:
     lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
+    lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     _lib = lib
     return lib
 
@@ -176,7 +177,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
-                    "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose"]
+                    "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
+                    "vb_bind_instance_transforms"]
 
 
 def _device_image(t):
@@ -276,6 +278,7 @@ class Renderer:
         self._owner = None
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
+        self._bound = None  # the device array of bind_instance_transforms
 
     @classmethod
     def _borrowed(cls, lib, handle: int, owner):
@@ -285,6 +288,7 @@ class Renderer:
         r._owner = owner
         r._device_images = {}
         r._fragment_pixels = {}
+        r._bound = None
         return r
 
     def close(self):
@@ -407,6 +411,31 @@ class Renderer:
         lay = Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
                      L.draw_data_base, L.transform_base, L.style_base)
         return lay, [int(v) for v in offs]
+
+    def bind_instance_transforms(self, t):
+        """Render instance k of the last `compose` under row k of the device array `t` in every frame from now on, read when
+        the frame runs (`vb_bind_instance_transforms`): `t` is float32 (n, 6) [a b c d e f] rows, one per composed instance, with
+        `__cuda_array_interface__` (e.g. a torch CUDA tensor, or columns of a larger one such as `state[:, 2:8]`). Write it on
+        `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. A row that is not
+        finite leaves its instance as composed. `t` is held while bound; None unbinds. A new scene (upload, compose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_instance_transforms(self.handle, None, 0, 0), "vb_bind_instance_transforms")
+            self._bound = None
+            return
+        cai = getattr(t, "__cuda_array_interface__", None)
+        if cai is None:
+            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device transforms are needed")
+        shape = tuple(int(v) for v in cai["shape"])
+        if len(shape) != 2 or shape[0] == 0 or shape[1] != 6 or cai["typestr"] != "<f4":
+            raise ValueError(f"bind_instance_transforms: transforms must be (n, 6) float32, not {shape} {cai['typestr']}")
+        strides = cai.get("strides") or (24, 4)
+        pitch = int(strides[0]) if shape[0] > 1 else 24  # the pitch of a single row is never used
+        if int(strides[1]) != 4 or pitch % 4 or pitch < 24:
+            raise ValueError(f"bind_instance_transforms: columns 4 bytes apart and rows a multiple of 4 bytes, at least 24, apart; "
+                             f"not strides {tuple(strides)}")
+        self._check(self.lib.vb_bind_instance_transforms(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
+                    "vb_bind_instance_transforms")
+        self._bound = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
