@@ -395,6 +395,46 @@ int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout
  * and vb_frame_finish; a scene whose bound transforms plus a view's would pass 32-bit word offsets. */
 int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, uint32_t n, size_t row_pitch_bytes);
 
+/* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
+ * repaints every frame in full) ----
+ * While tracking is on, a frame written into the destination of the renderer's last successful frame re-renders only its
+ * damaged 16 x 16 tiles and writes no other pixel; the damaged tiles are byte-identical to a full frame. Off (the default)
+ * changes nothing: not the pixels, the launches or the captured graphs.
+ *  - Incremental frames. A frame is incremental when tracking is on; the scene installation is the same (no upload form,
+ *    vb_compose, vb_render or vb_render_begin since); width, height, AA, base colour and the device destination pointer are
+ *    those of the last successful frame (NULL counts as the renderer's own target); the view, the binding and vb_set_cells are
+ *    unchanged; it has one cell and no bin_row / tile_row window; and the renderer is not in a vb_group and has no exchange.
+ *    Every other frame is full: it reports every tile as damaged and becomes the base of the next one (a batch or a windowed
+ *    frame becomes no base). Host destinations (vb_render_uploaded with a host pointer, vb_render) are always full; use
+ *    vb_last_damage to read back only what changed.
+ *  - Automatic damage, for composed scenes with bound instance transforms (vb_bind_instance_transforms). Instance k changed if
+ *    any transform word the frame reads for it (its bound products, or their viewed ones under a view) differs bit for bit
+ *    from the last successful frame's: a non-finite row that falls back to its composed transform is no change. The damage is
+ *    the tiles of the clipped boxes of its draw objects (draw_offsets[k] .. draw_offsets[k + 1] of vb_compose) in the last
+ *    frame and in this one. A moved open clip or blend layer is covered by its own box. The comparison and the snapshot it
+ *    needs are kernels of the frame: moving rows replays the captured graph.
+ *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
+ *    renderer of a vb_group or with the exchange configured.
+ *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
+ *    tiles, added to the next frame's damage in stream order (like vb_set_view's coefficients) on top of the automatic
+ *    damage. This is the explicit invalidate: use it for a scene re-uploaded with local edits (which is a full frame anyway,
+ *    unless the edit is written into the resident scene in place), dirty image overrides, or a destination the caller
+ *    changed. A frame after vb_mark_override_image_dirty / vb_override_image is full unless rectangles were added since the
+ *    last successful frame. No effect while tracking is off or before the first tracked frame. VB_E_INVALID: NULL rects
+ *    with n > 0; a frame enqueued and not finished (vb_render_enqueue until vb_frame_finish, vb_render_begin until
+ *    vb_readback_wait), since the rectangles are meant for the frame after it.
+ *  - vb_last_damage: one byte per tile of the last frame that completed successfully, row-major (height_in_tiles x
+ *    width_in_tiles), 1 for a tile that frame rendered, and their count in *n_damaged (either output may be NULL).
+ *    Synchronous. VB_E_INVALID: no completed frame, a frame enqueued and not finished, or cap below the tile count; also
+ *    when a tracked frame after the last successful one failed for good or was streamed (vb_render_begin), as it rewrote the
+ *    mask.
+ *  - Unchanged by tracking: flatten, path_count, backdrop and path_tiling run in full, so vb_hit_test answers on an
+ *    incremental frame equal those on a full one. vb_debug_fine_traffic counts the damaged tiles only, and after an
+ *    incremental frame vb_debug_download("seg_holes") also counts the segment slots of the tiles coarse skipped. */
+int vb_set_damage_tracking(vb_renderer *, int on);
+int vb_add_damage(vb_renderer *, const uint32_t *rects, uint32_t n);
+int vb_last_damage(vb_renderer *, uint8_t *tile_mask, size_t cap, uint32_t *n_damaged);
+
 /* ---- one frame on several GPUs of one box (SURVEY.md 8e, north_star: "a single frame shards across the GPUs by stripes") ----
  * The frame is cut into horizontal stripes of tile rows, one per device; every device runs the element stages on the scene and
  * the tile stages on its stripe (no winding seam exists between horizontal stripes, DESIGN.md 6), and `fine` on device k stores

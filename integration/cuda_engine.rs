@@ -84,6 +84,11 @@ extern "C" {
     // every frame reads instance k's transform from row k of device memory ([a b c d e f] f32, row_pitch_bytes apart), so a
     // simulation that writes its transforms on vb_stream moves the instances without a compose per frame; NULL unbinds
     pub fn vb_bind_instance_transforms(r: *mut VbRenderer, device_transforms: *const f32, n: u32, row_pitch_bytes: usize) -> c_int;
+    // damage tracking: a frame into the same destination as the last one repaints only the damaged tiles (moved bound instances,
+    // plus the x0 y0 x1 y1 pixel rectangles added for the next frame); vb_last_damage gives one byte per tile of the last frame
+    pub fn vb_set_damage_tracking(r: *mut VbRenderer, on: c_int) -> c_int;
+    pub fn vb_add_damage(r: *mut VbRenderer, rects: *const u32, n: u32) -> c_int;
+    pub fn vb_last_damage(r: *mut VbRenderer, tile_mask: *mut u8, cap: usize, n_damaged: *mut u32) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

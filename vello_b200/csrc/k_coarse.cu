@@ -67,10 +67,15 @@ __device__ __forceinline__ uint32_t co_write_path(TileState &s, const CoTile &ti
     return s.cmd_offset - 1u;
 }
 
+// DMG (damage tracking, k_damage.cu): `dmg` holds one byte per tile of the frame, non-zero for a tile the frame paints again.
+// A quadrant without such a tile returns at once; the others emit every tile but list only the damaged ones for fine, so fine
+// paints no other pixel. Without it (the default) the kernel is the one it was before damage tracking existed.
+template <bool DMG>
 __global__ void __launch_bounds__(CO_THREADS, CO_MINB)
 k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *__restrict__ draw_monoids,
          const VbBinHeader *__restrict__ bin_headers, const uint32_t *__restrict__ info_bin_data, const VbPath *__restrict__ paths,
-         const VbTile *__restrict__ tiles, VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, uint2 *cls_list, uint32_t cls_stride) {
+         const VbTile *__restrict__ tiles, VbBump *bump, uint32_t *ptcl, uint32_t *tile_start, uint2 *cls_list, uint32_t cls_stride,
+         const uint8_t *__restrict__ dmg) {
     __shared__ uint32_t sh_bitmaps[CO_N_SLICE][VB_N_TILE];
     __shared__ uint32_t sh_part_count[CO_THREADS];
     __shared__ uint32_t sh_part_offsets[CO_THREADS];
@@ -89,6 +94,16 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     __shared__ uint32_t sh_scan[CO_THREADS / 32 + 2];
 
     const uint32_t lid = threadIdx.x;
+    // DMG: one cell and no window (vb_api.cu), so the quadrant's tiles follow from the block alone. The owners' flags stay in
+    // shared memory until the tile lists (registers live across the loop would spill at this occupancy).
+    __shared__ uint8_t sh_damaged[64];
+    if (DMG) {
+        const uint32_t tx = (blockIdx.x >> 1) * VB_N_TILE_X + (blockIdx.x & 1u) * 8u + (lid & 7u);
+        const uint32_t ty = (blockIdx.y >> 1) * VB_N_TILE_Y + (blockIdx.y & 1u) * 8u + ((lid >> 3) & 7u);
+        const bool damaged = lid < 64u && tx < cfg.width_in_tiles && ty < cfg.height_in_tiles && dmg[ty * cfg.width_in_tiles + tx] != 0u;
+        if (lid < 64u) sh_damaged[lid] = damaged;
+        if (__syncthreads_or(damaged) == 0) return;
+    }
     // Only PRIOR stages abort coarse (coarse.wgsl:164-179); read once per CTA so the decision is
     // uniform even while other CTAs of this kernel raise VB_STAGE_COARSE (and k_path_tiling, beside it, FINE_SEGMENTS).
     if (lid == 0) sh_scan[0] = bump->failed & VB_STAGES_BEFORE_COARSE;
@@ -386,7 +401,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     // turning up at the tail of a persistent kernel that has nothing left to overlap them with)
     if (lid < 64u) { // the two owner warps, whole
         const uint32_t ty = bin_tile_y + tile_y, tx = bin_tile_x + tile_x; // ty: row in the cell; the list takes frame rows
-        const bool in_win = tx < cfg.width_in_tiles && ty >= cfg.win_ty0 && ty < cfg.win_ty1 && ty < cfg.height_in_tiles;
+        const bool in_win = tx < cfg.width_in_tiles && ty >= cfg.win_ty0 && ty < cfg.win_ty1 && ty < cfg.height_in_tiles && (!DMG || sh_damaged[lid] != 0u);
         // classes by powers of two of the estimate: >= 1024, 512, 256, 128, 64, 32, 16, rest
         const uint32_t lg = 31u - (uint32_t)__clz((int)max(cost, 1u));
         const uint32_t cls = lg >= 10u ? 0u : (lg <= 3u ? 7u : 10u - lg);
@@ -419,7 +434,11 @@ extern "C" uint32_t vb_launch_coarse(const VbConfig &cfg, const VbFrameBufs &b, 
     if (cfg.n_cells > 1u) rows *= cfg.n_cells; // a batch has no window: every cell's bin rows, stacked
     if (width_in_bins == 0 || rows == 0) return 0;
     dim3 grid(width_in_bins * 2u, rows * 2u); // four quadrant CTAs per bin
-    k_coarse<<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
-                                          b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows);
+    if (b.dmg_mode == VB_DMG_INCREMENTAL)
+        k_coarse<true><<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
+                                                    b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows, b.dmg_mask);
+    else
+        k_coarse<false><<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
+                                                     b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows, nullptr);
     return 1;
 }

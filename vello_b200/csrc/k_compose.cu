@@ -24,17 +24,6 @@
 #define CP_ITEMS 4u
 #define CP_UNITS_PER_CTA (CP_THREADS * CP_ITEMS)
 
-// the instance holding element x of a stream: the last k in [lo, hi] with P[k] <= x (an instance without elements has
-// P[k] == P[k + 1] and is never the answer for an x below the stream's total)
-__device__ __forceinline__ uint32_t cp_find(const uint32_t *__restrict__ P, uint32_t lo, uint32_t hi, uint32_t x) {
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1u) >> 1;
-        if (__ldg(P + mid) <= x) lo = mid;
-        else hi = mid - 1u;
-    }
-    return lo;
-}
-
 // stream s of instance k in its fragment's allocation: the fragment starts with the word offsets of its six streams
 __device__ __forceinline__ const uint32_t *cp_stream(const CmpArgs &a, uint32_t k, uint32_t s) {
     const uint32_t *base = reinterpret_cast<const uint32_t *>(__ldg(a.src + k));

@@ -1,0 +1,159 @@
+// k_damage.cu -- damage tracking: which tiles a frame must paint again when it goes into the destination of the last
+// successful frame (vb_set_damage_tracking).
+//
+// A tile's pixels depend only on the draw objects whose tile box covers it, and every stage is deterministic, so a tile that
+// no changed draw object touches gets the same pixels again. The damage of a frame is
+//   the caller's rectangles (vb_add_damage, staged into `pending` in stream order)
+//   + for every bound instance whose transform words (the ones flatten reads: the bound region, or the viewed one) differ bit
+//     for bit from the last successful frame's, the tile boxes of its draw objects in that frame and in this one.
+// Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
+// pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
+// and new box, which its BEGIN_CLIP contributes.
+//
+// The comparison needs the last successful frame's words and boxes: the snapshot holds two slots behind a generation word.
+// A frame reads slot gen & 1 and writes its own words and boxes into the other one; k_damage_commit, the frame's last kernel,
+// advances the generation only when bump.failed is 0. A re-run after an arena overflow therefore compares against the same
+// slot and computes the same damage, and the frame's launches never change: moving instances keeps replaying one graph.
+#include <string.h>
+
+#include <algorithm>
+
+#include "vb_device.cuh"
+#include "vb_stages.h"
+
+#define DM_THREADS 256u
+#define DM_HEADER_WORDS 4u // [generation, pad x3]
+#define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
+
+extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw) {
+    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw);
+}
+
+// the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
+__device__ __forceinline__ void dm_slots(uint32_t *snap, size_t slot_words, const uint32_t **old, uint32_t **nxt) {
+    const uint32_t gen = *(volatile uint32_t *)snap;
+    *old = snap + DM_HEADER_WORDS + (gen & 1u) * slot_words;
+    *nxt = snap + DM_HEADER_WORDS + ((gen + 1u) & 1u) * slot_words;
+}
+
+// A full frame damages every tile; otherwise the frame starts from the caller's rectangles. No instance has changed yet.
+__global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, const uint8_t *__restrict__ pending, uint32_t n_tiles, uint32_t full,
+                                                             uint32_t *changed, uint32_t n_inst) {
+    const uint32_t i = blockIdx.x * DM_THREADS + threadIdx.x;
+    if (i < n_tiles) mask[i] = full ? 1u : pending[i];
+    if (i < n_inst) changed[i] = 0u;
+}
+
+// One thread per transform u of the frame: its six words against the snapshot, and into the next slot. A difference marks
+// the instance holding u (the binding's prefix of the instances' transform counts).
+__global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__restrict__ xf, uint32_t *snap, size_t slot_words, uint32_t n_xf,
+                                                            uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed) {
+    const uint32_t u = blockIdx.x * DM_THREADS + threadIdx.x;
+    if (u >= n_xf) return;
+    const uint32_t *old;
+    uint32_t *nxt;
+    dm_slots(snap, slot_words, &old, &nxt);
+    bool diff = false;
+#pragma unroll
+    for (uint32_t i = 0; i < 6u; i++) {
+        const uint32_t w = __ldg(xf + 6u * u + i);
+        diff = diff || w != old[6u * u + i];
+        nxt[6u * u + i] = w;
+    }
+    if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
+}
+
+// Set the tiles of box b (pixels) in mask: the warp's lanes take its tiles in turn.
+__device__ __forceinline__ void dm_or_box(uint8_t *mask, const VbBbox4 b, uint32_t wt, uint32_t ht, uint32_t lane) {
+    if (!(b.x0 < b.x1 && b.y0 < b.y1)) return; // empty (or NaN): no tiles, as in tile_alloc
+    const float S = 1.0f / 16.0f;
+    const int32_t x0 = vb_clampi(vb_f2i_sat(floorf(b.x0 * S)), 0, (int32_t)wt), x1 = vb_clampi(vb_f2i_sat(ceilf(b.x1 * S)), 0, (int32_t)wt);
+    const int32_t y0 = vb_clampi(vb_f2i_sat(floorf(b.y0 * S)), 0, (int32_t)ht), y1 = vb_clampi(vb_f2i_sat(ceilf(b.y1 * S)), 0, (int32_t)ht);
+    if (x1 <= x0 || y1 <= y0) return;
+    const uint32_t w = (uint32_t)(x1 - x0), n = w * (uint32_t)(y1 - y0);
+    for (uint32_t i = lane; i < n; i += 32u) mask[((uint32_t)y0 + i / w) * wt + (uint32_t)x0 + i % w] = 1u;
+}
+
+// One warp per draw object: its box into the next slot, and, when its instance changed, its old and new boxes into the mask.
+__global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
+                                                       uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
+                                                       const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht) {
+    const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+    if (d >= n_draw) return;
+    const uint32_t *old;
+    uint32_t *nxt;
+    dm_slots(snap, slot_words, &old, &nxt);
+    const VbBbox4 now = draw_bboxes[d];
+    const VbBbox4 was = reinterpret_cast<const VbBbox4 *>(old + 6u * (size_t)n_xf)[d];
+    __syncwarp();
+    if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
+    // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
+    if (!compare || d >= __ldg(inst_draw + n_inst)) return;
+    if (changed[cp_find(inst_draw, 0u, n_inst - 1u, d)] == 0u) return;
+    dm_or_box(mask, was, wt, ht, lane);
+    dm_or_box(mask, now, wt, ht, lane);
+}
+
+// The frame's last kernel: a frame that succeeded becomes the base of the next one (its snapshot slot is current, the caller's
+// rectangles are consumed). A failed attempt changes nothing, so its re-run computes the same damage. An unbound scene keeps
+// no snapshot (snap is null).
+__global__ void __launch_bounds__(DM_THREADS) k_damage_commit(const VbBump *bump, uint32_t *snap, uint8_t *pending, uint32_t n_tiles) {
+    if (bump->failed != 0u) return;
+    const uint32_t i = blockIdx.x * DM_THREADS + threadIdx.x;
+    if (i == 0u && snap) snap[0] += 1u;
+    if (i < n_tiles) pending[i] = 0u;
+}
+
+struct DmRects {
+    uint32_t r[DM_RECTS][4]; // tile ranges x0 y0 x1 y1, clipped to the frame
+    uint32_t wt;
+};
+// One CTA per rectangle.
+__global__ void __launch_bounds__(DM_THREADS) k_damage_rects(uint8_t *pending, DmRects a) {
+    const uint32_t *q = a.r[blockIdx.x];
+    const uint32_t w = q[2] - q[0], n = w * (q[3] - q[1]);
+    for (uint32_t i = threadIdx.x; i < n; i += DM_THREADS) pending[(q[1] + i / w) * a.wt + q[0] + i % w] = 1u;
+}
+
+extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (b.dmg_mode == VB_DMG_OFF) return 0u;
+    const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = b.inst_n;
+    const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
+    const uint32_t n = std::max(n_tiles, n_inst);
+    k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst);
+    if (n_inst == 0u) return 1u; // not bound: the transforms never change without a call that makes the frame full
+    const size_t slot_words = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw;
+    uint32_t launches = 1u;
+    if (b.dmg_n_xf) {
+        k_damage_mark<<<(b.dmg_n_xf + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
+                                                                                            b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed);
+        launches++;
+    }
+    if (n_draw) {
+        const uint32_t per = DM_THREADS / 32u;
+        k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
+                                                                   n_inst, b.dmg_changed, b.dmg_mask, wt, ht);
+        launches++;
+    }
+    return launches;
+}
+
+extern "C" uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (b.dmg_mode == VB_DMG_OFF) return 0u;
+    const uint32_t n_tiles = cfg.width_in_tiles * cfg.height_in_tiles;
+    k_damage_commit<<<(n_tiles + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.bump(), b.dmg_snap, b.dmg_pending, n_tiles);
+    return 1u;
+}
+
+extern "C" uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st) {
+    uint32_t launches = 0u;
+    for (uint32_t i = 0; i < n; i += DM_RECTS) {
+        DmRects a;
+        const uint32_t m = std::min(DM_RECTS, n - i);
+        memcpy(a.r, tile_rects + 4u * (size_t)i, (size_t)m * 16u);
+        a.wt = width_in_tiles;
+        k_damage_rects<<<m, DM_THREADS, 0, st>>>(pending, a);
+        launches++;
+    }
+    return launches;
+}

@@ -769,9 +769,15 @@ struct FineSmem {
 };
 static_assert(sizeof(WarpIo) % 16 == 0 && sizeof(WarpMs<1>) % 16 == 0 && sizeof(WarpMs<2>) % 16 == 0, "16-byte aligned smem blocks");
 
-template <int AA>
+// MODE: the AA mode (0 area, 1 MSAA8, 2 MSAA16), plus FI_DMG for damage tracking (k_damage.cu): coarse listed only the
+// damaged tiles, and those lists are the whole queue, so no other pixel is written. Without FI_DMG the kernel is the one it was
+// before damage tracking existed.
+#define FI_DMG 16
+template <int MODE>
 __global__ void __launch_bounds__(FI_MAX_THREADS, FI_MINB)
 k_fine(VbConfig cfg, FineArgs A) {
+    constexpr int AA = MODE & 15;
+    constexpr bool DMG = (MODE & FI_DMG) != 0;
     extern __shared__ __align__(16) unsigned char smem[];
     typedef WarpMs<AA == 0 ? 1 : AA> Ms;
     const uint32_t *__restrict__ ptcl = A.ptcl;
@@ -804,7 +810,7 @@ k_fine(VbConfig cfg, FineArgs A) {
     // window of tile k+1 is in flight (bulk copy), the occlusion start of tile k+2 is being loaded and the queue
     // ticket of tile k+3 is being taken, so none of those latencies is exposed.
     const uint32_t wt = cfg.width_in_tiles;
-    const uint32_t n_tiles = wt * (cfg.win_ty1 - cfg.win_ty0);
+    uint32_t n_tiles = wt * (cfg.win_ty1 - cfg.win_ty0);
     const uint32_t G = gridDim.x * n_warps, g = blockIdx.x * n_warps + warp;
     const uint32_t first_tile = cfg.win_ty0 * wt;
 #define START_OF(t, s0) ((s0) != 0u && A.cull != 0u ? (s0) : (first_tile + (t)) * VB_PTCL_INITIAL_ALLOC + 1u)
@@ -820,7 +826,8 @@ k_fine(VbConfig cfg, FineArgs A) {
             cpre[k] = acc;
             acc += min(__ldg(A.cls_count + k), A.cls_stride);
         }
-        ordered = acc == n_tiles; // a launch over part of the window (read-back bands) keeps the natural order
+        if (DMG) n_tiles = acc;
+        ordered = DMG || acc == n_tiles; // a launch over part of the window (read-back bands) keeps the natural order
     }
     auto entry_of = [&](uint32_t pos) -> uint2 {
         if (ordered) {
@@ -1234,8 +1241,11 @@ extern "C" int vb_fine_init_constants(void) {
     cudaError_t e = cudaMemcpyToSymbol(c_unorm, h, sizeof h);
     // the kernels use more than the default 48 KB of dynamic shared memory per CTA
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<0>::bytes(FI_MAX_WARPS));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<0 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<0>::bytes(FI_MAX_WARPS));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<1>::bytes(FI_MAX_WARPS));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<1 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<1>::bytes(FI_MAX_WARPS));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<2>::bytes(FI_MAX_WARPS));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<2 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<2>::bytes(FI_MAX_WARPS));
     return (int)e;
 }
 
@@ -1263,6 +1273,12 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, ui
     A.cls_list = b.cls_list;
     A.cls_count = cls_order ? b.ctl + VB_CTL_FINE_CLASS : nullptr;
     A.cls_stride = cfg.width_in_tiles * cfg.tile_rows;
+    if (b.dmg_mode == VB_DMG_INCREMENTAL && cls_order) { // the damaged tiles of coarse's lists only
+        if (aa == 0) k_fine<0 + FI_DMG><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, A);
+        else if (aa == 1) k_fine<1 + FI_DMG><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, A);
+        else k_fine<2 + FI_DMG><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, A);
+        return 1;
+    }
     if (aa == 0) k_fine<0><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, A);
     else if (aa == 1) k_fine<1><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, A);
     else k_fine<2><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, A);

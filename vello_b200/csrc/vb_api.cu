@@ -35,12 +35,14 @@
 
 // Statistics for the roofline of `fine`: PTCL words each tile's interpreter reads and segments it
 // references (one thread per tile walks its command stream, as fine does).
+// Under damage tracking (`damage` non-null) only the tiles fine painted count.
 __global__ void k_ptcl_stats(VbConfig cfg, const uint32_t *__restrict__ ptcl, const uint32_t *__restrict__ tile_start,
-                             unsigned long long *out) {
+                             const uint8_t *__restrict__ damage, unsigned long long *out) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t wt = cfg.width_in_tiles, rows = cfg.win_ty1 - cfg.win_ty0;
     if (t >= wt * rows) return;
     uint32_t tile_ix = (cfg.win_ty0 + t / wt) * wt + t % wt;
+    if (damage && !damage[tile_ix]) return;
     uint32_t ix = tile_ix * VB_PTCL_INITIAL_ALLOC + 1u;
     unsigned long long words = 1, segs = 0, fills = 0;
     if (tile_start && tile_start[tile_ix]) { // occlusion start: the interpreter begins at the tile's last opaque cover
@@ -210,6 +212,7 @@ struct vb_renderer {
         // the composed scene's instances, for vb_bind_instance_transforms: each one's fragment id and compose-time transform
         std::vector<uint32_t> inst_frag;
         std::vector<CmpXform> inst_xf;
+        std::vector<uint32_t> inst_draw; // the exclusive prefix of the instances' draw objects (n + 1), for damage tracking
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -315,12 +318,34 @@ struct vb_renderer {
     // bound instance transforms (vb_bind_instance_transforms) of the current scene: the caller's rows (nullptr: unbound), and
     // the binding's tables in inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n), at
     // o_xf] [the fragments' untransformed transforms, at o_src]. Every scene installation unbinds (set_scene).
+    // [the instances' draw prefix (n + 1), at o_draw]
     struct Binding {
         const uint8_t *rows = nullptr;
         uint32_t n = 0, pitch = 0;
-        size_t o_xf = 0, o_src = 0;
+        size_t o_xf = 0, o_src = 0, o_draw = 0;
     } bound;
     DevBuf inst_tables;
+
+    // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
+    // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
+    // matches `base`, the last successful frame, in epoch, size, AA, base colour and device destination. The device keeps the
+    // base's snapshot (dmg_snap) and advances it itself, so base changes only when the host learns that a frame succeeded.
+    struct DamageFrame {
+        uint32_t mode = VB_DMG_OFF;
+        bool can_base = false; // one cell, no window, device destination: the frame can be the next one's base
+        uint32_t w = 0, h = 0, aa = 0, base_color = 0;
+        const void *dest = nullptr;
+        uint64_t epoch = 0;
+    };
+    struct Damage {
+        bool on = false;
+        uint64_t epoch = 0;
+        bool have_base = false, have_last = false;
+        bool rects = false;      // vb_add_damage since the last successful frame (dirty overrides then do not force a full frame)
+        bool force_full = false; // dirty overrides without rectangles: the frame and its re-runs are full
+        DamageFrame base, frame, last; // frame: the one prepared last; last: the last successful one
+    } dmg;
+    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
 
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
@@ -340,7 +365,8 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables};
+                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -658,9 +684,11 @@ static void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uin
     s.composed = composed;
     s.inst_frag.clear(); // vb_compose fills them afterwards
     s.inst_xf.clear();
+    s.inst_draw.clear();
     s.have_scene = true;
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
+    r->dmg.epoch++;
     hit_forget(r);
 }
 
@@ -1007,6 +1035,8 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_PATH_COUNT: launches += vb_launch_path_count(c, b, st); break;
         case VB_STAGE_ID_BACKDROP: launches += vb_launch_backdrop(c, b, st); break;
         case VB_STAGE_ID_COARSE:
+            // damage tracking: the frame's damaged tiles, from binning's draw boxes, before coarse reads them
+            launches += vb_launch_damage(c, b, st);
             // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before
             // path_tiling's grid fills the rest of the GPU
             if (fork_tiling) CK(cudaEventRecord(r->tiling_fork, st));
@@ -1037,6 +1067,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         }
         rec(r, s + 1);
     }
+    if (last == VB_STAGE_ID_FINE) launches += vb_launch_damage_commit(c, b, st); // after fine: the frame's success is known
     k_publish_bump<<<1, 32, 0, st>>>(b.bump(), r->cur->h_bump_dev); // zero-copy store to mapped host memory (no copy engine)
     launches++;
     CK(cudaGetLastError());
@@ -1287,6 +1318,8 @@ extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
 // arenas, the output target), then the launches. vb_group runs step 1 for ALL its renderers before step 2 of any: with the
 // exchange on, a renderer's frame contains a kernel that waits for its peers, and a peer that shares the device (tests)
 // must not be stuck in a cudaFree behind that kernel.
+static int damage_prepare(vb_renderer *r);
+static void damage_succeeded(vb_renderer *r);
 static int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
     if (!r || !p) return VB_E_INVALID;
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
@@ -1294,7 +1327,8 @@ static int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
     int rc = prepare(r, p);
     if (rc) return rc;
     r->dest = d;
-    return pick_out(r, &r->dest);
+    if ((rc = pick_out(r, &r->dest))) return rc;
+    return damage_prepare(r);
 }
 // Enqueue stages first..last of the frame frame_prepare set up. A range from stage 0 starts the frame: the dirty overridden
 // images are copied and the hit record and the frame's first event are taken. A range after stage 0 continues the frame and
@@ -1383,6 +1417,7 @@ extern "C" int vb_frame_finish(vb_renderer *r, vb_frame_stats *stats) {
     r->frame_pending = false;
     fill_stats(r, stats, 0u); // an enqueued frame is not re-run
     hit_finished(r, r->cur->h_bump->failed == 0u);
+    if (r->cur->h_bump->failed == 0u) damage_succeeded(r);
     return r->cur->h_bump->failed ? VB_E_BUMP_OVERFLOW : VB_OK;
 }
 
@@ -1428,6 +1463,7 @@ static int settle(vb_renderer *r, const Frame &f, vb_frame_stats *stats) {
     }
     fill_stats(r, stats, retries);
     hit_finished(r, true);
+    damage_succeeded(r);
     return VB_OK;
 }
 
@@ -1698,7 +1734,9 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
         if (dst && cap >= sizeof(VbBump)) CK(cudaMemcpy(dst, r->ctl.p, sizeof(VbBump), cudaMemcpyDeviceToHost));
         return VB_OK;
     }
-    if (!strcmp(name, "seg_holes")) { // segment slots of the last frame that backdrop assigned and no CMD_FILL uses (k_tile.cu, k_coarse.cu)
+    // segment slots of the last frame that backdrop assigned and no CMD_FILL uses (k_tile.cu, k_coarse.cu); after an incremental
+    // frame (damage tracking) also the slots of the quadrants coarse skipped, so not the reference's count
+    if (!strcmp(name, "seg_holes")) {
         if (bytes) *bytes = 4;
         if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->ctl.p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
         return VB_OK;
@@ -1826,8 +1864,142 @@ extern "C" int vb_set_view(vb_renderer *r, const double affine[6]) {
         r->err = "vb_set_view: the coefficients must be finite in f32";
         return VB_E_INVALID;
     }
+    if (!same_view(r->view, v)) r->dmg.epoch++;
     return put_view(r, v);
 }
+// ---- damage tracking: vb_set_damage_tracking / vb_add_damage / vb_last_damage (k_damage.cu) -------------------------------
+// After prepare and pick_out: is the frame incremental, full, or outside damage tracking (a batch, a window, the exchange:
+// mode VB_DMG_OFF, and no base for the next frame)? The decision is the same for every re-run of the frame, because the base
+// and the forcing flags change only when a frame succeeds (damage_succeeded). Allocates the mask, the staged rectangles and
+// the snapshot; their sizes follow from the frame size and the scene, so they never move under an incremental frame.
+static int damage_prepare(vb_renderer *r) {
+    vb_renderer::Damage &D = r->dmg;
+    const VbConfig &c = r->cfg;
+    vb_renderer::DamageFrame f;
+    f.w = c.target_width;
+    f.h = c.target_height;
+    f.aa = r->params.aa;
+    f.base_color = c.base_color;
+    f.dest = r->dest.dev;
+    f.epoch = D.epoch;
+    const bool windowed = r->params.bin_row1 > r->params.bin_row0 || r->params.tile_row1 > r->params.tile_row0;
+    f.can_base = D.on && c.n_cells == 1u && !windowed && !r->xc.enabled && !r->grouped;
+    D.frame = f;
+    if (!f.can_base) return VB_OK;
+    // an overridden image copied again changes pixels nothing here can locate: the frame is full unless the caller named them
+    for (const auto &o : r->cur->overridden)
+        if (o.dirty && !D.rects) D.force_full = true;
+    const vb_renderer::DamageFrame &B = D.base;
+    const bool incremental = D.have_base && !D.force_full && !r->dest.host && B.epoch == f.epoch && B.w == f.w && B.h == f.h && B.aa == f.aa &&
+                             B.base_color == f.base_color && B.dest == f.dest;
+    f.mode = incremental ? VB_DMG_INCREMENTAL : VB_DMG_FULL;
+    // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
+    // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
+    if (D.last.mode == VB_DMG_INCREMENTAL) D.have_last = false;
+    const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles, n_draw = r->cur->layout.n_draw_objects;
+    const uint32_t n_xf = r->bound.rows ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
+    int rc;
+    if ((rc = ensure(r, r->dmg_mask, n_tiles))) return rc;
+    if ((rc = ensure(r, r->dmg_pending, n_tiles))) return rc;
+    if (r->bound.rows) {
+        if ((rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw) * 4u))) return rc;
+        if ((rc = ensure(r, r->dmg_changed, (size_t)r->bound.n * 4u))) return rc;
+    }
+    VbFrameBufs &b = r->bufs;
+    b.dmg_mask = (uint8_t *)r->dmg_mask.p;
+    b.dmg_pending = (uint8_t *)r->dmg_pending.p;
+    if (r->bound.rows) {
+        b.dmg_snap = (uint32_t *)r->dmg_snap.p;
+        b.dmg_changed = (uint32_t *)r->dmg_changed.p;
+        b.inst_draw = (const uint32_t *)((const char *)r->inst_tables.p + r->bound.o_draw);
+    }
+    b.dmg_mode = f.mode;
+    b.dmg_n_xf = n_xf;
+    D.frame = f;
+    return VB_OK;
+}
+// The frame prepared last succeeded: it is the one vb_last_damage reports, and the base of the next frame when it was tracked.
+static void damage_succeeded(vb_renderer *r) {
+    vb_renderer::Damage &D = r->dmg;
+    D.last = D.frame;
+    D.have_last = true;
+    D.have_base = D.frame.mode != VB_DMG_OFF;
+    if (D.have_base) D.base = D.frame;
+    D.rects = false;
+    D.force_full = false;
+}
+
+extern "C" int vb_set_damage_tracking(vb_renderer *r, int on) {
+    if (!r) return VB_E_INVALID;
+    if (on && (r->grouped || r->xc.configured)) {
+        r->err = "vb_set_damage_tracking: not available for a renderer of a vb_group or with the exchange";
+        return VB_E_INVALID;
+    }
+    r->dmg.on = on != 0;
+    r->dmg.epoch++; // switched on (or on again): the next frame is full
+    if (!on) r->dmg.have_base = false;
+    return VB_OK;
+}
+
+extern "C" int vb_add_damage(vb_renderer *r, const uint32_t *rects, uint32_t n) {
+    if (!r) return VB_E_INVALID;
+    if (n && !rects) {
+        r->err = "vb_add_damage: NULL rectangles";
+        return VB_E_INVALID;
+    }
+    // the rectangles belong to the frame after the one in flight, whose size and success are not known yet
+    if (r->frame_pending || r->stream_pending) {
+        r->err = "vb_add_damage: a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)";
+        return VB_E_INVALID;
+    }
+    vb_renderer::Damage &D = r->dmg;
+    if (!D.on || n == 0u) return VB_OK;
+    D.rects = true;
+    if (!D.have_base) return VB_OK; // the next frame is a full one
+    // clamped to the frame the next incremental frame must match, rounded out to tiles
+    const uint32_t w = D.base.w, h = D.base.h, wt = (w + 15u) / 16u;
+    std::vector<uint32_t> t;
+    t.reserve((size_t)n * 4u);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t *q = rects + 4u * (size_t)i;
+        const uint32_t x0 = std::min(q[0], w), y0 = std::min(q[1], h), x1 = std::min(q[2], w), y1 = std::min(q[3], h);
+        if (x1 <= x0 || y1 <= y0) continue;
+        t.insert(t.end(), {x0 / 16u, y0 / 16u, (x1 + 15u) / 16u, (y1 + 15u) / 16u});
+    }
+    if (t.empty()) return VB_OK;
+    CK(cudaSetDevice(r->device));
+    vb_launch_damage_rects((uint8_t *)r->dmg_pending.p, wt, t.data(), (uint32_t)(t.size() / 4u), r->stream); // in stream order
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+
+extern "C" int vb_last_damage(vb_renderer *r, uint8_t *tile_mask, size_t cap, uint32_t *n_damaged) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_last_damage: ") + why;
+        return VB_E_INVALID;
+    };
+    if (r->frame_pending || r->stream_pending) return bad("a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)");
+    const vb_renderer::Damage &D = r->dmg;
+    if (!D.have_last) return bad("no completed frame to report (none yet, or a later tracked frame failed or was streamed)");
+    const size_t n_tiles = (size_t)((D.last.w + 15u) / 16u) * ((D.last.h + 15u) / 16u);
+    if (tile_mask && cap < n_tiles) return bad("the mask holds fewer bytes than the frame has tiles");
+    std::vector<uint8_t> m(n_tiles, 1u); // a frame that was not incremental rendered every tile
+    if (D.last.mode == VB_DMG_INCREMENTAL) {
+        CK(cudaSetDevice(r->device));
+        CK(cudaMemcpyAsync(m.data(), r->dmg_mask.p, n_tiles, cudaMemcpyDeviceToHost, r->stream));
+        CK(cudaStreamSynchronize(r->stream));
+    }
+    uint32_t count = 0;
+    for (uint8_t &v : m) {
+        v = v ? 1u : 0u;
+        count += v;
+    }
+    if (tile_mask) memcpy(tile_mask, m.data(), n_tiles);
+    if (n_damaged) *n_damaged = count;
+    return VB_OK;
+}
+
 extern "C" int vb_debug_graph_captures(vb_renderer *r, uint64_t *captures) {
     if (!r || !captures) return VB_E_INVALID;
     *captures = r->graph_captures;
@@ -1879,6 +2051,7 @@ extern "C" int vb_set_cells(vb_renderer *r, const uint32_t *draw_offsets, uint32
     if (draw_offsets[0] != 0u || draw_offsets[n_cells] != n_draw) return bad("offsets must start at 0 and end at the scene's draw-object count");
     for (uint32_t c = 0; c < n_cells; c++)
         if (draw_offsets[c + 1] < draw_offsets[c]) return bad("offsets must not decrease");
+    r->dmg.epoch++;
     if (n_cells == 1u) { // the whole scene: no batch
         r->cells.clear();
         hit_forget(r);
@@ -1914,8 +2087,9 @@ extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint6
     const FineRows f = fine_rows(c, Dest{});
     c.win_ty0 = f.ty0, c.win_ty1 = f.ty1;
     uint32_t n = c.width_in_tiles * (c.win_ty1 - c.win_ty0);
+    const uint8_t *damage = r->dmg.have_last && r->dmg.last.mode == VB_DMG_INCREMENTAL ? (const uint8_t *)r->dmg_mask.p : nullptr;
     if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(c, (const uint32_t *)r->ptcl.p,
-                                                                r->occlusion_cull ? (const uint32_t *)r->tile_start.p : nullptr, d);
+                                                                r->occlusion_cull ? (const uint32_t *)r->tile_start.p : nullptr, damage, d);
     CK(cudaStreamSynchronize(r->stream));
     CK(cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost));
     cudaFree(d);
@@ -2971,6 +3145,7 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     slot.inst_frag.resize(n);
     for (uint32_t k = 0; k < n; k++) slot.inst_frag[k] = fr[k]->id;
     slot.inst_xf = std::move(xf);
+    slot.inst_draw.assign(pre + (size_t)CMP_DRAW_TAGS * (n + 1u), pre + (size_t)(CMP_DRAW_TAGS + 1) * (n + 1u));
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
@@ -2989,6 +3164,7 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
     if (!device_transforms) {
         r->bound = vb_renderer::Binding{};
+        r->dmg.epoch++;
         return VB_OK;
     }
     const vb_renderer::SceneSlot &slot = *r->cur;
@@ -3018,7 +3194,8 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     const size_t o_src = up16((size_t)CMP_STREAMS * (n + 1u) * 4u), o_xf0 = up16(o_src + (size_t)n * 8u);
     const size_t tmp_bytes = up16(o_xf0 + (size_t)n * sizeof(CmpXform));
     const size_t o_xf = up16(((size_t)n + 1u) * 4u), o_tr = up16(o_xf + (size_t)n * sizeof(CmpXform));
-    const size_t staged = tmp_bytes + o_tr;
+    const size_t o_draw = up16(o_tr + (size_t)n_tr * 24u), draw_bytes = ((size_t)n + 1u) * 4u; // staged right after the tables
+    const size_t staged = tmp_bytes + o_tr + draw_bytes;
     CK(cudaEventSynchronize(r->compose_staged));
     if (r->compose_host_cap < staged) {
         if (r->compose_host) CK(cudaFreeHost(r->compose_host));
@@ -3035,14 +3212,16 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     unsigned long long *srcs = (unsigned long long *)(h + o_src);
     for (uint32_t k = 0; k < n; k++) srcs[k] = (unsigned long long)(uintptr_t)fr[k]->mem;
     memcpy(h + tmp_bytes + o_xf, slot.inst_xf.data(), (size_t)n * sizeof(CmpXform));
+    memcpy(h + tmp_bytes + o_tr, slot.inst_draw.data(), draw_bytes);
 
     int rc;
     if ((rc = compose_room(r, r->compose_tmp, tmp_bytes))) return rc;
-    if ((rc = compose_room(r, r->inst_tables, o_tr + (size_t)n_tr * 24u))) return rc;
+    if ((rc = compose_room(r, r->inst_tables, o_draw + draw_bytes))) return rc;
     cudaStream_t st = r->stream;
     char *tmp = (char *)r->compose_tmp.p, *tables = (char *)r->inst_tables.p;
     CK(cudaMemcpyAsync(tmp, h, tmp_bytes, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(tables, h + tmp_bytes, o_tr, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tables + o_draw, h + tmp_bytes + o_tr, draw_bytes, cudaMemcpyHostToDevice, st));
     CK(cudaEventRecord(r->compose_staged, st));
     CmpArgs a;
     memset(&a, 0, sizeof a);
@@ -3059,6 +3238,8 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     r->bound.pitch = (uint32_t)row_pitch_bytes;
     r->bound.o_xf = o_xf;
     r->bound.o_src = o_tr;
+    r->bound.o_draw = o_draw;
+    r->dmg.epoch++;
     return VB_OK;
 }
 

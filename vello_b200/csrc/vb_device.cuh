@@ -177,6 +177,17 @@ __device__ __forceinline__ void vb_lookback(const VbLookback &s, uint32_t part, 
 
 // ---- misc -----------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t vb_f2u_sat(float f) { return __float2uint_rz(f); }  // saturating, NaN -> 0
+// composition (k_compose.cu, k_damage.cu): the instance holding element x of a stream: the last k in [lo, hi] with P[k] <= x (an instance without elements has
+// P[k] == P[k + 1] and is never the answer for an x below the stream's total)
+__device__ __forceinline__ uint32_t cp_find(const uint32_t *__restrict__ P, uint32_t lo, uint32_t hi, uint32_t x) {
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (__ldg(P + mid) <= x) lo = mid;
+        else hi = mid - 1u;
+    }
+    return lo;
+}
+
 __device__ __forceinline__ int32_t vb_f2i_sat(float f) { return __float2int_rz(f); }    // saturating, NaN -> 0
 __device__ __forceinline__ float vb_signf(float x) { return (x > 0.0f) ? 1.0f : ((x < 0.0f) ? -1.0f : 0.0f); }
 __device__ __forceinline__ float vb_clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }

@@ -53,12 +53,22 @@ struct VbFrameBufs {
     VbSegmentCount *seg_counts;
     VbSegment *segments;
     uint32_t *ptcl, *blend_spill;
+    // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
+    // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
+    // of the frame's transform words and draw boxes), one changed flag per bound instance, and the composed scene's draw prefix
+    // (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k + 1]; null while unbound)
+    uint8_t *dmg_mask, *dmg_pending;
+    uint32_t *dmg_snap, *dmg_changed;
+    const uint32_t *inst_draw;
     // control block: [VbBump, header words (vb_types.h)] [look-back states], zeroed at the start of every frame
     uint32_t *ctl;
     size_t ctl_words;
     uint32_t *lb_pathtag, *lb_flatten, *lb_draw, *lb_tile, *lb_clip, *lb_backdrop;
     uint32_t parts_pathtag, parts_flatten, parts_draw, parts_tile, parts_backdrop;
     uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
+    // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
+    // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
+    uint32_t dmg_mode, dmg_n_xf;
     int sm_count; // the grids of the persistent and grid-stride kernels are sized from it
 
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
@@ -143,6 +153,17 @@ uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
 // bound instance transforms: row_k * T of every transform T of the composed scene into the frame's bound region (prepare,
 // vb_api.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
+// k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
+// the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame
+// succeeded. vb_launch_damage_rects stages caller rectangles (tile ranges x0 y0 x1 y1, clipped) into `pending` in stream order.
+#define VB_DMG_OFF 0u
+#define VB_DMG_FULL 1u
+#define VB_DMG_INCREMENTAL 2u
+uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
+size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw);
 
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)

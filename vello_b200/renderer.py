@@ -165,6 +165,9 @@ def load_library() -> C.CDLL:
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
+    lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
+    lib.vb_last_damage.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_uint32)]
     _lib = lib
     return lib
 
@@ -178,7 +181,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
                     "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
-                    "vb_bind_instance_transforms"]
+                    "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage"]
 
 
 def _device_image(t):
@@ -279,6 +282,7 @@ class Renderer:
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
         self._bound = None  # the device array of bind_instance_transforms
+        self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
 
     @classmethod
     def _borrowed(cls, lib, handle: int, owner):
@@ -289,6 +293,7 @@ class Renderer:
         r._device_images = {}
         r._fragment_pixels = {}
         r._bound = None
+        r._frame_size = None
         return r
 
     def close(self):
@@ -462,6 +467,7 @@ class Renderer:
                                 atlas.ctypes.data, atlas.shape[1], atlas.shape[0], C.byref(ps), out.ctypes.data, 0, C.byref(st))
         self.last_stats = st
         self._check(rc, "vb_render")
+        self._frame_size = (int(params.width), int(params.height))
         return out
 
     def render_stream(self, scenes, params: RenderParams):
@@ -534,6 +540,7 @@ class Renderer:
             rc = self.lib.vb_render_uploaded(self.handle, C.byref(ps), C.c_void_p(out.ctypes.data), 0, C.byref(st))
         self.last_stats = st
         self._check(rc, "vb_render_uploaded")
+        self._frame_size = (w, h)
         return out
 
     @staticmethod
@@ -551,17 +558,20 @@ class Renderer:
         rc = self.lib.vb_render_resident(self.handle, C.byref(ps), C.c_void_p(out_device_ptr or None), C.byref(st))
         self.last_stats = st
         self._check(rc, "vb_render_resident")
+        self._frame_size = (int(params.width), int(params.height))
         return st
 
     def enqueue(self, params: RenderParams, out_device_ptr: int = 0, bin_rows=(0, 0), tile_rows=(0, 0)):
         ps = _params_struct(params, bin_rows, tile_rows)
         self._check(self.lib.vb_render_enqueue(self.handle, C.byref(ps), C.c_void_p(out_device_ptr or None)), "vb_render_enqueue")
+        self._enqueued_size = (int(params.width), int(params.height))
 
     def finish(self) -> FrameStats:
         st = FrameStats()
         rc = self.lib.vb_frame_finish(self.handle, C.byref(st))
         self.last_stats = st
         self._check(rc, "vb_frame_finish")
+        self._frame_size = getattr(self, "_enqueued_size", self._frame_size)
         return st
 
     @property
@@ -674,6 +684,29 @@ class Renderer:
     def set_occlusion_cull(self, on: bool):
         """fine skips the commands under a tile's last opaque full-tile cover (identical pixels). Default on."""
         self._check(self.lib.vb_set_occlusion_cull(self.handle, 1 if on else 0), "vb_set_occlusion_cull")
+
+    def set_damage_tracking(self, on: bool):
+        """Damage tracking (`vb_set_damage_tracking`, default off): a frame rendered into the same device destination as the
+        last successful one, with the same scene, size, AA, base colour and view, repaints only the tiles that changed and
+        writes no other pixel. With bound instance transforms, the instances whose transforms changed are found on the device;
+        `add_damage` names anything else. Switching it on (again) makes the next frame full."""
+        self._check(self.lib.vb_set_damage_tracking(self.handle, 1 if on else 0), "vb_set_damage_tracking")
+
+    def add_damage(self, rects):
+        """Add half-open pixel rectangles (x0, y0, x1, y1), an (n, 4) array, to the next frame's damage (`vb_add_damage`),
+        in stream order. Clamped to the frame; no effect while tracking is off."""
+        arr = np.ascontiguousarray(rects, dtype=np.uint32).reshape(-1, 4)
+        self._check(self.lib.vb_add_damage(self.handle, arr.ctypes.data if arr.size else None, arr.shape[0]), "vb_add_damage")
+
+    def last_damage(self) -> np.ndarray:
+        """The tiles the last successful frame rendered (`vb_last_damage`): bool [tiles_h, tiles_w], all True for a full frame."""
+        if self._frame_size is None:
+            raise VelloB200Error("last_damage: no frame rendered yet")
+        w, h = self._frame_size
+        out = np.zeros(((h + 15) // 16, (w + 15) // 16), dtype=np.uint8)
+        n = C.c_uint32(0)
+        self._check(self.lib.vb_last_damage(self.handle, out.ctypes.data, out.size, C.byref(n)), "vb_last_damage")
+        return out.astype(bool)
 
     def fine_traffic(self):
         """(ptcl_words, segment_refs, fill_cmds) of the last frame -- inputs of the fine roofline."""
