@@ -364,6 +364,32 @@ typedef struct {
 int vb_fragment_upload(vb_renderer *, const vb_encoding_streams *, uint32_t *fragment_out);
 int vb_fragment_free(vb_renderer *, uint32_t fragment);
 int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
+/* vb_recompose: vb_compose, followed by a frame that repaints only what the new instance list changed (an addition; no vello
+ * counterpart). It installs exactly the scene vb_compose would (scene, layout, ramps, atlas and draw offsets, byte for byte),
+ * with the same errors; on an error the previous scene and the damage state are left as they were. A toolkit recomposes for
+ * every edit: a hover colour is a new fragment in the same slot, a popup an inserted instance, a closed dialog a removed one,
+ * a raised window a move in z-order. With damage tracking (below) the next frame is then incremental, with the damage between
+ * the composition the base frame rendered and the new one, when all of these hold:
+ *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, unbound, with no scene
+ *    installation, binding, view, cell split or tracking switch since, and hit tests answering from it (no failed frame,
+ *    vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
+ *  - no other vb_recompose / vb_compose since that frame, and no vb_run_stages before the next one;
+ *  - the next frame meets every condition of an incremental frame (size, AA, base colour, destination, one cell, no window).
+ * Otherwise it is vb_compose: the next frame is full, and still correct. vb_compose itself always makes the next frame full.
+ * The damage: instance k's key is (fragment, has_transform, the six f32 transform words). The old and new instance lists are
+ * matched in order between equal keys: common prefix and suffix, then Myers' diff of the middle up to VB_RECOMPOSE_MAX_EDITS
+ * insertions and deletions, past that the middle by position. A matched instance counts as changed when one of its images got
+ * another atlas slot, pixel source or place, or comes from an override (the compose copies its pixels again); a different
+ * ramp row does not count (a ramp's row holds the same bytes wherever it is). The damaged tiles are those of the clipped
+ * draw boxes of unmatched and changed instances (old boxes in the base frame, new ones in this frame); both boxes of a matched
+ * draw object whose box is not bit for bit the old one (an enclosing open clip came or went); the END_CLIPs after the last
+ * instance, paired from the end, when unpaired or when their boxes differ; and vb_add_damage rectangles as usual. The host work
+ * is O(instances + patches) like vb_compose's; the frame adds one kernel and the recompose one device copy of the old boxes. */
+#define VB_RECOMPOSE_MAX_EDITS 32u
+int vb_recompose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
+/* test-only: vb_recompose's matching on plain keys. match[j] = the old index paired with new key j, or 0xffffffff; returns the
+ * middle's edit count, or VB_RECOMPOSE_MAX_EDITS + 1 when it was paired by position */
+uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t n_old, const uint32_t *new_keys, uint32_t n_new, uint32_t *match);
 /* Bind the instance transforms of the composed scene to device memory (an addition; no vello counterpart). A simulation, an
  * animation or a layout model that writes its instances' transforms on the GPU moves them without a host call per frame:
  *  - Rows. Row k is at device_transforms + k * row_pitch_bytes. It holds six f32 values [a b c d e f] in kurbo Affine order.
@@ -401,7 +427,7 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  * damaged 16 x 16 tiles and writes no other pixel; the damaged tiles are byte-identical to a full frame. Off (the default)
  * changes nothing: not the pixels, the launches or the captured graphs.
  *  - Incremental frames. A frame is incremental when tracking is on; the scene installation is the same (no upload form,
- *    vb_compose, vb_render or vb_render_begin since); width, height, AA, base colour and the device destination pointer are
+ *    vb_compose, vb_render or vb_render_begin since; vb_recompose, see there, can keep the frame after it incremental); width, height, AA, base colour and the device destination pointer are
  *    those of the last successful frame (NULL counts as the renderer's own target); the view, the binding and vb_set_cells are
  *    unchanged; it has one cell and no bin_row / tile_row window; and the renderer is not in a vb_group and has no exchange.
  *    Every other frame is full: it reports every tile as damaged and becomes the base of the next one (a batch or a windowed

@@ -89,6 +89,9 @@ extern "C" {
     pub fn vb_set_damage_tracking(r: *mut VbRenderer, on: c_int) -> c_int;
     pub fn vb_add_damage(r: *mut VbRenderer, rects: *const u32, n: u32) -> c_int;
     pub fn vb_last_damage(r: *mut VbRenderer, tile_mask: *mut u8, cap: usize, n_damaged: *mut u32) -> c_int;
+    // vb_compose, after which the next tracked frame repaints only the instances added, removed or changed since the composition
+    // the last frame rendered (matched in order by fragment and transform); vb_compose itself makes the next frame full
+    pub fn vb_recompose(r: *mut VbRenderer, instances: *const VbInstance, n: u32, layout_out: *mut Layout, draw_offsets: *mut u32) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

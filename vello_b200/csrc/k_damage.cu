@@ -63,17 +63,6 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
     if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
 }
 
-// Set the tiles of box b (pixels) in mask: the warp's lanes take its tiles in turn.
-__device__ __forceinline__ void dm_or_box(uint8_t *mask, const VbBbox4 b, uint32_t wt, uint32_t ht, uint32_t lane) {
-    if (!(b.x0 < b.x1 && b.y0 < b.y1)) return; // empty (or NaN): no tiles, as in tile_alloc
-    const float S = 1.0f / 16.0f;
-    const int32_t x0 = vb_clampi(vb_f2i_sat(floorf(b.x0 * S)), 0, (int32_t)wt), x1 = vb_clampi(vb_f2i_sat(ceilf(b.x1 * S)), 0, (int32_t)wt);
-    const int32_t y0 = vb_clampi(vb_f2i_sat(floorf(b.y0 * S)), 0, (int32_t)ht), y1 = vb_clampi(vb_f2i_sat(ceilf(b.y1 * S)), 0, (int32_t)ht);
-    if (x1 <= x0 || y1 <= y0) return;
-    const uint32_t w = (uint32_t)(x1 - x0), n = w * (uint32_t)(y1 - y0);
-    for (uint32_t i = lane; i < n; i += 32u) mask[((uint32_t)y0 + i / w) * wt + (uint32_t)x0 + i % w] = 1u;
-}
-
 // One warp per draw object: its box into the next slot, and, when its instance changed, its old and new boxes into the mask.
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
                                                        uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,

@@ -23,6 +23,7 @@
 
 #include "../../include/vello_b200.h"
 #include "vb_device.cuh"
+#include "vb_diff.h"
 #include "vb_resolve.h"
 #include "vb_stages.h"
 #include "vb_textures.h"
@@ -163,6 +164,11 @@ struct ImageKey {
 enum { CMP_TAGS, CMP_PATH_DATA, CMP_DRAW_TAGS, CMP_DRAW_DATA, CMP_TRANSFORMS, CMP_STYLES, CMP_STREAMS };
 #define CMP_HEADER_WORDS 8u
 #define CMP_FROM_OVERRIDE 0xffffffffu // the source of an atlas slot filled from an override (fragment ids start at 1, count up)
+// An image's atlas slot in a composition: (image-key id << 32 | pixel source), as in SceneSlot::atlas_keys, and x << 16 | y.
+struct ImgPlace {
+    uint64_t key;
+    uint32_t xy;
+};
 struct Fragment {
     uint32_t id = 0;
     void *mem = nullptr;
@@ -213,6 +219,9 @@ struct vb_renderer {
         std::vector<uint32_t> inst_frag;
         std::vector<CmpXform> inst_xf;
         std::vector<uint32_t> inst_draw; // the exclusive prefix of the instances' draw objects (n + 1), for damage tracking
+        // for vb_recompose: the atlas places of the instances' images in patch order, instance k's from inst_img[k] (n + 1)
+        std::vector<uint32_t> inst_img;
+        std::vector<ImgPlace> img_place;
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -344,8 +353,17 @@ struct vb_renderer {
         bool rects = false;      // vb_add_damage since the last successful frame (dirty overrides then do not force a full frame)
         bool force_full = false; // dirty overrides without rectangles: the frame and its re-runs are full
         DamageFrame base, frame, last; // frame: the one prepared last; last: the last successful one
+        // vb_recompose that tracking follows: the next frame of epoch `epoch` (the recompose's installation) is incremental
+        // against `base` and runs k_recompose_damage on the tables in rcmp; consumed when a frame succeeds
+        struct Diff {
+            bool armed = false;
+            uint64_t epoch = 0;
+            uint32_t n_old = 0, n_new = 0, old_draws = 0, new_draws = 0;
+            size_t o_tables = 0;
+        } diff;
     } dmg;
     DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
+    DevBuf rcmp; // vb_recompose: [the base frame's draw boxes] [the tables, at dmg.diff.o_tables] (VbFrameBufs::rcmp_tables)
 
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
@@ -366,7 +384,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
                            &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed};
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->rcmp};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -685,6 +703,8 @@ static void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uin
     s.inst_frag.clear(); // vb_compose fills them afterwards
     s.inst_xf.clear();
     s.inst_draw.clear();
+    s.inst_img.clear();
+    s.img_place.clear();
     s.have_scene = true;
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
@@ -1037,6 +1057,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_COARSE:
             // damage tracking: the frame's damaged tiles, from binning's draw boxes, before coarse reads them
             launches += vb_launch_damage(c, b, st);
+            launches += vb_launch_recompose_damage(c, b, st); // the first frame after vb_recompose: what the recompose changed
             // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before
             // path_tiling's grid fills the rest of the GPU
             if (fork_tiling) CK(cudaEventRecord(r->tiling_fork, st));
@@ -1608,6 +1629,7 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     if (!r || !p || first < 0 || last >= VB_N_STAGE_IDS || first > last) return VB_E_INVALID;
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
     hit_forget(r);
+    r->dmg.diff.armed = false; // the stages may write the destination: the frame after them is full
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;
@@ -1890,8 +1912,9 @@ static int damage_prepare(vb_renderer *r) {
     for (const auto &o : r->cur->overridden)
         if (o.dirty && !D.rects) D.force_full = true;
     const vb_renderer::DamageFrame &B = D.base;
-    const bool incremental = D.have_base && !D.force_full && !r->dest.host && B.epoch == f.epoch && B.w == f.w && B.h == f.h && B.aa == f.aa &&
-                             B.base_color == f.base_color && B.dest == f.dest;
+    const bool diff = D.diff.armed && D.diff.epoch == f.epoch; // the scene is a recompose of the base's (vb_recompose)
+    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff) && B.w == f.w && B.h == f.h &&
+                             B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
     f.mode = incremental ? VB_DMG_INCREMENTAL : VB_DMG_FULL;
     // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
     // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
@@ -1915,6 +1938,14 @@ static int damage_prepare(vb_renderer *r) {
     }
     b.dmg_mode = f.mode;
     b.dmg_n_xf = n_xf;
+    if (incremental && diff) {
+        b.rcmp_old_boxes = (const VbBbox4 *)r->rcmp.p;
+        b.rcmp_tables = (const uint32_t *)((const char *)r->rcmp.p + D.diff.o_tables);
+        b.rcmp_n_old = D.diff.n_old;
+        b.rcmp_n_new = D.diff.n_new;
+        b.rcmp_old_draws = D.diff.old_draws;
+        b.rcmp_new_draws = D.diff.new_draws;
+    }
     D.frame = f;
     return VB_OK;
 }
@@ -1927,6 +1958,7 @@ static void damage_succeeded(vb_renderer *r) {
     if (D.have_base) D.base = D.frame;
     D.rects = false;
     D.force_full = false;
+    D.diff.armed = false;
 }
 
 extern "C" int vb_set_damage_tracking(vb_renderer *r, int on) {
@@ -2989,10 +3021,22 @@ static int compose_room(vb_renderer *r, DevBuf &b, size_t bytes) {
     return ensure(r, b, bytes);
 }
 
-extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+// vb_compose and vb_recompose. A recompose that damage tracking can follow (recompose_armed) also matches the instances
+// against the current scene's, stages the tables of k_recompose_damage and copies the base frame's draw boxes.
+static bool recompose_armed(const vb_renderer *r) {
+    const vb_renderer::Damage &D = r->dmg;
+    const vb_renderer::SceneSlot &s = *r->cur;
+    // the base rendered the current scene (no installation, binding, view, cells or tracking switch since: the epoch), unbound,
+    // and its draw boxes are intact (hit tests answer from it: no frame, failure, vb_run_stages or debug write since)
+    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && s.composed && !r->bound.rows && r->hit.valid &&
+           !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects &&
+           s.inst_draw.size() == s.inst_frag.size() + 1u && s.inst_img.size() == s.inst_frag.size() + 1u;
+}
+static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets,
+                   bool recompose) {
     if (!r) return VB_E_INVALID;
     auto bad = [&](const std::string &why) {
-        r->err = "vb_compose: " + why;
+        r->err = std::string(fn) + ": " + why;
         return VB_E_INVALID;
     };
     if (n && !inst) return bad("NULL instances");
@@ -3033,10 +3077,12 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     std::vector<uint32_t> ramp_ids;
     struct Placed { const ImageKey *key; const uint8_t *src; uint32_t x, y, frag; };
     std::vector<Placed> placed;
+    std::vector<uint32_t> img_pre(n + 1u, 0u), img_local; // each instance's images: their place in `placed`
     VbShelfPacker shelf;
     uint32_t dd0 = L.draw_data_base;
     for (uint32_t k = 0; k < n; k++) {
         const Fragment &f = *fr[k];
+        img_pre[k + 1] = img_pre[k] + (uint32_t)f.images.size();
         for (const Fragment::Ramp &p : f.ramps) {
             RampKey *key = p.key;
             if (key->stamp != seq || !key->self_equal) {
@@ -3057,6 +3103,7 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
             }
             const Placed &q = placed[key->local];
             patches.push_back(RsPatch{dd0 + im.dd, (q.x << 16) | q.y});
+            img_local.push_back(key->local);
         }
         dd0 += f.len[CMP_DRAW_DATA];
     }
@@ -3069,10 +3116,36 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     for (const Placed &q : placed) {
         const ImageKey &k = *q.key;
         bool overridden;
-        if ((rc = image_source(r, "vb_compose", k.key, k.w, k.h, q.x, q.y, blits, over, &overridden))) return rc;
+        if ((rc = image_source(r, fn, k.key, k.w, k.h, q.x, q.y, blits, over, &overridden))) return rc;
         if (!overridden && q.src) blits.push_back(VbBlitRect{q.src, (uint64_t)k.w * 4u, 0, k.w, k.h, q.x, q.y, 0, 0});
         // where the slot's pixels come from: the fragment, an override (never a fragment id), or nowhere (a zero region)
         atlas_keys.push_back((uint64_t)k.id << 32 | (overridden ? CMP_FROM_OVERRIDE : q.src ? q.frag : 0u));
+    }
+    std::vector<ImgPlace> img_place(img_local.size());
+    for (size_t t = 0; t < img_local.size(); t++) {
+        const Placed &q = placed[img_local[t]];
+        img_place[t] = ImgPlace{atlas_keys[img_local[t]], (q.x << 16) | q.y};
+    }
+
+    // vb_recompose: match the new instances to the current scene's (vb_diff.h). A matched instance whose images moved in the
+    // atlas, or come from an override (copied again by this compose), is unmatched: fine samples in atlas coordinates.
+    const vb_renderer::SceneSlot &was = *r->cur;
+    const bool arm = recompose && recompose_armed(r);
+    const uint32_t n_old = arm ? (uint32_t)was.inst_frag.size() : 0u, old_draws = arm ? was.layout.n_draw_objects : 0u;
+    std::vector<uint32_t> match(arm ? n : 0u), unmatched(n_old, 1u);
+    if (arm) {
+        vb_diff_match(
+            n_old, n,
+            [&](uint32_t i, uint32_t j) { return was.inst_frag[i] == fr[j]->id && memcmp(&was.inst_xf[i], &xf[j], sizeof(CmpXform)) == 0; },
+            match.data());
+        for (uint32_t j = 0; j < n; j++) {
+            const uint32_t i = match[j];
+            if (i == VB_DIFF_NONE) continue;
+            const ImgPlace *a = was.img_place.data() + was.inst_img[i], *b = img_place.data() + img_pre[j];
+            for (uint32_t t = 0; t < img_pre[j + 1] - img_pre[j] && match[j] != VB_DIFF_NONE; t++)
+                if (a[t].key != b[t].key || a[t].xy != b[t].xy || (uint32_t)b[t].key == CMP_FROM_OVERRIDE) match[j] = VB_DIFF_NONE;
+            if (match[j] != VB_DIFF_NONE) unmatched[i] = 0u;
+        }
     }
 
     if ((rc = drain_stream(r))) return rc;
@@ -3086,13 +3159,16 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     auto up16 = [](size_t v) { return (v + 15u) & ~(size_t)15u; };
     const size_t o_src = up16((size_t)CMP_STREAMS * (n + 1u) * 4u), o_xf = up16(o_src + (size_t)n * 8u), o_pat = up16(o_xf + (size_t)n * sizeof(CmpXform));
     const size_t o_ramp = up16(o_pat + patches.size() * sizeof(RsPatch)), staged = o_ramp + ramps.size() * sizeof(RsRamp);
+    // vb_recompose's tables (VbFrameBufs::rcmp_tables), staged after compose's, and where they go in rcmp: after the old boxes
+    const size_t o_rc = up16(staged), rc_bytes = arm ? ((size_t)n_old + 1u + n + 1u + n + n_old) * 4u : 0u;
+    const size_t o_tables = up16((size_t)old_draws * sizeof(VbBbox4)), host_bytes = o_rc + rc_bytes;
     CK(cudaEventSynchronize(r->compose_staged));
-    if (r->compose_host_cap < staged) {
+    if (r->compose_host_cap < host_bytes) {
         if (r->compose_host) CK(cudaFreeHost(r->compose_host));
         r->compose_host = nullptr;
         r->compose_host_cap = 0;
-        CK(cudaMallocHost((void **)&r->compose_host, staged));
-        r->compose_host_cap = staged;
+        CK(cudaMallocHost((void **)&r->compose_host, host_bytes));
+        r->compose_host_cap = host_bytes;
     }
     uint8_t *h = r->compose_host;
     uint32_t *pre = (uint32_t *)h;
@@ -3107,6 +3183,14 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     if (!patches.empty()) memcpy(h + o_pat, patches.data(), patches.size() * sizeof(RsPatch));
     if (!ramps.empty()) memcpy(h + o_ramp, ramps.data(), ramps.size() * sizeof(RsRamp));
     if (draw_offsets) memcpy(draw_offsets, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+    if (arm) {
+        uint32_t *t = (uint32_t *)(h + o_rc);
+        memcpy(t, was.inst_draw.data(), ((size_t)n_old + 1u) * 4u);
+        memcpy(t + n_old + 1u, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+        if (n) memcpy(t + n_old + 1u + n + 1u, match.data(), (size_t)n * 4u);
+        if (n_old) memcpy(t + n_old + 1u + n + 1u + n, unmatched.data(), (size_t)n_old * 4u);
+        if ((rc = compose_room(r, r->rcmp, o_tables + rc_bytes))) return rc;
+    }
 
     if ((rc = compose_room(r, r->compose_tmp, staged))) return rc;
     if ((rc = compose_room(r, slot.scene, scene_bytes(L, total_words, r->view.on)))) return rc;
@@ -3114,6 +3198,10 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     if (new_atlas && (rc = compose_room(r, slot.atlas, (size_t)atlas_w * atlas_h * 4u))) return rc;
     char *tmp = (char *)r->compose_tmp.p;
     if (staged) CK(cudaMemcpyAsync(tmp, h, staged, cudaMemcpyHostToDevice, st));
+    if (arm) { // the base frame's boxes, before anything can rewrite them, and the tables
+        if (old_draws) CK(cudaMemcpyAsync(r->rcmp.p, r->hit.bufs.draw_bboxes, (size_t)old_draws * sizeof(VbBbox4), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync((char *)r->rcmp.p + o_tables, h + o_rc, rc_bytes, cudaMemcpyHostToDevice, st));
+    }
     CK(cudaEventRecord(r->compose_staged, st));
     uint32_t *scene = (uint32_t *)slot.scene.p;
     CmpArgs a;
@@ -3146,8 +3234,30 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     for (uint32_t k = 0; k < n; k++) slot.inst_frag[k] = fr[k]->id;
     slot.inst_xf = std::move(xf);
     slot.inst_draw.assign(pre + (size_t)CMP_DRAW_TAGS * (n + 1u), pre + (size_t)(CMP_DRAW_TAGS + 1) * (n + 1u));
+    slot.inst_img = std::move(img_pre);
+    slot.img_place = std::move(img_place);
+    vb_renderer::Damage::Diff &X = r->dmg.diff;
+    X.armed = arm;
+    if (arm) { // the next frame of this installation's epoch is incremental (damage_prepare)
+        X.epoch = r->dmg.epoch;
+        X.n_old = n_old;
+        X.n_new = n;
+        X.old_draws = old_draws;
+        X.new_draws = L.n_draw_objects;
+        X.o_tables = o_tables;
+    }
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
+}
+
+extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+    return compose(r, "vb_compose", inst, n, layout_out, draw_offsets, false);
+}
+extern "C" int vb_recompose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+    return compose(r, "vb_recompose", inst, n, layout_out, draw_offsets, true);
+}
+extern "C" uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t n_old, const uint32_t *new_keys, uint32_t n_new, uint32_t *match) {
+    return vb_diff_match(n_old, n_new, [&](uint32_t i, uint32_t j) { return old_keys[i] == new_keys[j]; }, match);
 }
 
 // ---- bound instance transforms: vb_bind_instance_transforms (k_compose.cu) ----------------------------------------------------

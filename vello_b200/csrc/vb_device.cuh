@@ -177,7 +177,7 @@ __device__ __forceinline__ void vb_lookback(const VbLookback &s, uint32_t part, 
 
 // ---- misc -----------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t vb_f2u_sat(float f) { return __float2uint_rz(f); }  // saturating, NaN -> 0
-// composition (k_compose.cu, k_damage.cu): the instance holding element x of a stream: the last k in [lo, hi] with P[k] <= x (an instance without elements has
+// composition (k_compose.cu, k_damage.cu, k_recompose.cu): the instance holding element x of a stream: the last k in [lo, hi] with P[k] <= x (an instance without elements has
 // P[k] == P[k + 1] and is never the answer for an x below the stream's total)
 __device__ __forceinline__ uint32_t cp_find(const uint32_t *__restrict__ P, uint32_t lo, uint32_t hi, uint32_t x) {
     while (lo < hi) {
@@ -192,6 +192,17 @@ __device__ __forceinline__ int32_t vb_f2i_sat(float f) { return __float2int_rz(f
 __device__ __forceinline__ float vb_signf(float x) { return (x > 0.0f) ? 1.0f : ((x < 0.0f) ? -1.0f : 0.0f); }
 __device__ __forceinline__ float vb_clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
 __device__ __forceinline__ int32_t vb_clampi(int32_t x, int32_t lo, int32_t hi) { return min(max(x, lo), hi); }
+// damage tracking (k_damage.cu, k_recompose.cu): set the tiles of box b (pixels) in mask, rounded out exactly as tile_alloc
+// rounds a draw object's box; the warp's lanes take its tiles in turn
+__device__ __forceinline__ void dm_or_box(uint8_t *mask, const VbBbox4 b, uint32_t wt, uint32_t ht, uint32_t lane) {
+    if (!(b.x0 < b.x1 && b.y0 < b.y1)) return; // empty (or NaN): no tiles, as in tile_alloc
+    const float S = 1.0f / 16.0f;
+    const int32_t x0 = vb_clampi(vb_f2i_sat(floorf(b.x0 * S)), 0, (int32_t)wt), x1 = vb_clampi(vb_f2i_sat(ceilf(b.x1 * S)), 0, (int32_t)wt);
+    const int32_t y0 = vb_clampi(vb_f2i_sat(floorf(b.y0 * S)), 0, (int32_t)ht), y1 = vb_clampi(vb_f2i_sat(ceilf(b.y1 * S)), 0, (int32_t)ht);
+    if (x1 <= x0 || y1 <= y0) return;
+    const uint32_t w = (uint32_t)(x1 - x0), n = w * (uint32_t)(y1 - y0);
+    for (uint32_t i = lane; i < n; i += 32u) mask[((uint32_t)y0 + i / w) * wt + (uint32_t)x0 + i % w] = 1u;
+}
 __device__ __forceinline__ uint32_t vb_span(float a, float b) {
     return vb_f2u_sat(fmaxf(ceilf(fmaxf(a, b)) - floorf(fminf(a, b)), 1.0f));
 }

@@ -60,6 +60,11 @@ struct VbFrameBufs {
     uint8_t *dmg_mask, *dmg_pending;
     uint32_t *dmg_snap, *dmg_changed;
     const uint32_t *inst_draw;
+    // recompose damage (vb_recompose; k_recompose.cu), set only for the first frame after a recompose that tracking follows,
+    // null otherwise: the base frame's draw boxes (rcmp_old_draws), and the tables [old draw prefix (rcmp_n_old + 1)] [new draw
+    // prefix (rcmp_n_new + 1)] [new instance -> old instance, or VB_RCMP_NONE (rcmp_n_new)] [old instance unmatched (rcmp_n_old)]
+    const VbBbox4 *rcmp_old_boxes;
+    const uint32_t *rcmp_tables;
     // control block: [VbBump, header words (vb_types.h)] [look-back states], zeroed at the start of every frame
     uint32_t *ctl;
     size_t ctl_words;
@@ -69,6 +74,8 @@ struct VbFrameBufs {
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
+    // recompose damage: the old and new compositions' instances and draw objects (the END_CLIPs after the last instance included)
+    uint32_t rcmp_n_old, rcmp_n_new, rcmp_old_draws, rcmp_new_draws;
     int sm_count; // the grids of the persistent and grid-stride kernels are sized from it
 
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
@@ -164,6 +171,11 @@ uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
 size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw);
+// k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
+// of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
+// are null
+#define VB_RCMP_NONE 0xffffffffu
+uint32_t vb_launch_recompose_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)

@@ -164,6 +164,9 @@ def load_library() -> C.CDLL:
     lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
+    lib.vb_recompose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
+    lib.vb_debug_match_instances.argtypes = [vp, C.c_uint32, vp, C.c_uint32, vp]
+    lib.vb_debug_match_instances.restype = C.c_uint32
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -181,7 +184,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
                     "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
-                    "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage"]
+                    "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
+                    "vb_recompose"]
 
 
 def _device_image(t):
@@ -401,6 +405,16 @@ class Renderer:
         """Make the renderer's scene `Scene()` with every `(fragment id, Affine or None)` of `instances` appended in order,
         resolved, built on the device from the resident fragments (`vb_compose`; asynchronous on `self.stream`). Returns
         (Layout, draw_offsets): instance k's draws are draw objects draw_offsets[k] .. draw_offsets[k + 1] - 1."""
+        return self._compose(instances, "vb_compose")
+
+    def recompose(self, instances):
+        """`compose`, after which the next frame repaints only what changed (`vb_recompose`): with damage tracking on and the
+        last frame rendered from the composition being replaced, the old and new instance lists are matched in order, and only
+        the tiles of the instances added, removed or changed (and of draws whose enclosing clip changed) are damaged. Otherwise,
+        and for `compose` itself, the next frame is full. Same return value as `compose`."""
+        return self._compose(instances, "vb_recompose")
+
+    def _compose(self, instances, fn):
         from .encoding import Layout
         inst = list(instances)
         arr = (_Instance * max(len(inst), 1))()
@@ -412,7 +426,7 @@ class Renderer:
                     arr[k].transform[i] = float(v)
         L = _Layout()
         offs = (C.c_uint32 * (len(inst) + 1))()
-        self._check(self.lib.vb_compose(self.handle, arr, len(inst), C.byref(L), offs), "vb_compose")
+        self._check(getattr(self.lib, fn)(self.handle, arr, len(inst), C.byref(L), offs), fn)
         lay = Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
                      L.draw_data_base, L.transform_base, L.style_base)
         return lay, [int(v) for v in offs]
