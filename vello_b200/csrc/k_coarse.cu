@@ -94,7 +94,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     __shared__ uint32_t sh_scan[CO_THREADS / 32 + 2];
 
     const uint32_t lid = threadIdx.x;
-    // DMG: one cell and no window (vb_api.cu), so the quadrant's tiles follow from the block alone. The owners' flags stay in
+    // DMG: one cell and no window (vb_damage.cu), so the quadrant's tiles follow from the block alone. The owners' flags stay in
     // shared memory until the tile lists (registers live across the loop would spill at this occupancy).
     __shared__ uint8_t sh_damaged[64];
     if (DMG) {

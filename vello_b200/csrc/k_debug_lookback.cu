@@ -3,7 +3,7 @@
 // A look-back that finds an inclusive prefix at its nearest predecessor never combines more than one window, and never
 // reduces a window of aggregates. Which case a frame kernel meets depends on timing. Here partition p, by ticket, first
 // waits delay_ns[p]: a delayed partition keeps the ones after it from finishing, so they publish aggregates only and a later
-// partition has to combine whole windows of them, in order. No frame kernel uses this file (vb_debug_lookback, vb_api.cu).
+// partition has to combine whole windows of them, in order. No frame kernel uses this file (vb_debug_lookback, vb_debug.cu).
 #include "../../include/vello_b200.h"
 #include "vb_device.cuh"
 #include "vb_stages.h"

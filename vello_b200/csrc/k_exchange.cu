@@ -30,7 +30,7 @@ struct XHdr {
     uint32_t pad[64 - (XG_MAX + 1)];
 };
 // An arena: [flags: XG_MAX words][epoch counter: word 16][pad to 256 B][half 0][half 1]. The epoch counter is advanced by the
-// frame's first kernel (k_frame_init, vb_api.cu) and READ by the kernels below, so a captured CUDA graph replays correctly.
+// frame's first kernel (k_frame_init, vb_frame.cu) and READ by the kernels below, so a captured CUDA graph replays correctly.
 // The peer table (XPeers) is in vb_stages.h.
 #define X_EPOCH_WORD 16u
 __device__ __forceinline__ uint32_t x_epoch(const XPeers &X) { return *(reinterpret_cast<const volatile uint32_t *>(X.base[X.rank]) + X_EPOCH_WORD); }

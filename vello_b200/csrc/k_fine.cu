@@ -782,7 +782,7 @@ k_fine(VbConfig cfg, FineArgs A) {
     typedef WarpMs<AA == 0 ? 1 : AA> Ms;
     const uint32_t *__restrict__ ptcl = A.ptcl;
     const uint32_t *__restrict__ info = A.info;
-    if (A.bump->failed != 0u) return; // upstream failure (the reference flags it through ptcl[0], path_tiling_setup.wgsl:25; see vb_api.cu)
+    if (A.bump->failed != 0u) return; // upstream failure (the reference flags it through ptcl[0], path_tiling_setup.wgsl:25; see vb_frame.cu)
     const uint32_t lane = vb_lane(), warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
     uint32_t *lut = reinterpret_cast<uint32_t *>(smem);
     uint64_t *lut_bar = reinterpret_cast<uint64_t *>(smem + FineSmem<AA>::LUT_WORDS * 4u);

@@ -1391,7 +1391,7 @@ extern "C" uint32_t vb_launch_flatten(const VbConfig &cfg, const VbFrameBufs &b,
     const uint32_t *scene = b.scene;
     const VbTagMonoid *tag_monoids = b.tag_monoids;
     VbPathBbox *path_bboxes = b.path_bboxes;
-    // whole frames reset the boxes in k_frame_init (vb_api.cu); a stage range that starts later does it here
+    // whole frames reset the boxes in k_frame_init (vb_frame.cu); a stage range that starts later does it here
     if (n_paths && clear_bboxes) {
         k_bbox_clear<<<(n_paths + 255) / 256, 256, 0, st>>>(n_paths, path_bboxes);
         launches++;

@@ -4,7 +4,7 @@
 // cpu/path_tiling.rs. One thread per crossing (SegmentCount record); no indirect dispatch: the grid
 // is sized from the arena and strides over bump.seg_counts read on the device.
 // Slices: k_backdrop gives every (path, tile) with crossings its slice, so this kernel does not wait for coarse; the
-// two run side by side on two streams (vb_api.cu). Crossings of tiles that coarse emits no CMD_FILL for are still
+// two run side by side on two streams (vb_frame.cu). Crossings of tiles that coarse emits no CMD_FILL for are still
 // written, into slots no command reads (the reference, which allocates in coarse, skips them).
 // Algorithmic bytes per crossing: 12 (SegmentCount) + 24 (LineSoup gather) + 32 (Path) + 8 (Tile)
 // read, 24 written (scattered into the tile's slice).

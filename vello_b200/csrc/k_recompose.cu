@@ -1,7 +1,7 @@
 // k_recompose.cu -- the damage of the first frame after vb_recompose: which tiles differ between the composition the base
 // frame rendered and the new one.
 //
-// The host (vb_api.cu) matches the old instances to the new ones in order, by fragment id and transform, and unmatches an
+// The host (vb_compose.cu) matches the old instances to the new ones in order, by fragment id and transform, and unmatches an
 // instance whose images moved in the atlas. A tile's pixels are a function of the ordered draw objects whose clipped box covers
 // it, so it is damaged only by
 //   - the draw objects of unmatched instances: their boxes in the base frame (old) and in this frame (new);

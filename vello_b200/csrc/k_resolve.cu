@@ -1,6 +1,6 @@
 // k_resolve.cu -- the device half of Resolver::resolve (vello_encoding/src/resolve.rs:183-399, ramp_cache.rs:119-155).
 //
-// vb_scene_upload_streams (vb_api.cu) copies the six encoding streams straight to their Layout offsets inside the packed scene
+// vb_scene_upload_streams (vb_upload.cu) copies the six encoding streams straight to their Layout offsets inside the packed scene
 // buffer on the device; what is left of `resolve` runs here: the zero padding of the tag stream and the trailing PATH tags /
 // END_CLIP draw tags of unclosed clips (resolve.rs:127-141), the late-bound patches (gradient ramp id | extend, atlas x | y:
 // resolve.rs:268-330) and the gradient ramps themselves (512 premultiplied RGBA8 texels per unique gradient).

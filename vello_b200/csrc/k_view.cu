@@ -4,7 +4,7 @@
 // The view V lives in device memory, written in stream order by k_view_set, so that frames enqueued before a change keep
 // the view they were enqueued with and a captured frame replays under a new view. k_view_transforms, the first kernel of a
 // viewed frame, writes V * T for every transform T of the scene into a region past the scene's streams; the frame's
-// layout.transform_base points there (prepare, vb_api.cu). The scene's own transforms are never modified, so a re-run after
+// layout.transform_base points there (prepare, vb_frame.cu). The scene's own transforms are never modified, so a re-run after
 // an arena overflow, a graph replay or the next frame compose the view once.
 #include "vb_device.cuh"
 #include "vb_stages.h"

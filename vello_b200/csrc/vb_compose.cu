@@ -1,0 +1,615 @@
+// vb_compose.cu -- composition of resident fragments: vb_fragment_upload / vb_fragment_free, vb_compose and vb_recompose
+// (k_compose.cu, k_recompose.cu), and bound instance transforms (vb_bind_instance_transforms).
+#include <cuda_runtime.h>
+#include <math.h>
+#include <string.h>
+
+#include <algorithm>
+
+#include "vb_diff.h"
+#include "vb_renderer.h"
+#include "vb_resolve.h"
+#include "vb_textures.h"
+
+// ---- composition of resident fragments: vb_fragment_upload / vb_fragment_free / vb_compose (k_compose.cu) ---------------------
+// The ramp key of patch p, with one more reference. A key made here is appended to `fresh`: its stops still need a place in
+// the stop pool (place_stops).
+static RampKey *intern_ramp(vb_renderer *r, const vb_ramp_patch &p, std::vector<RampKey *> &fresh) {
+    const bool premul = p.premul_interp != 0u;
+    const bool self_equal = vb_same_ramp(p.stops, p.n_stops, premul, p.stops, p.n_stops, premul);
+    const uint64_t h = vb_ramp_hash(p.stops, p.n_stops, premul);
+    if (self_equal) {
+        const auto it = r->ramp_by_hash.find(h);
+        if (it != r->ramp_by_hash.end())
+            for (RampKey *k : it->second)
+                if (vb_same_ramp(k->stops.data(), (uint32_t)k->stops.size(), k->premul, p.stops, p.n_stops, premul)) {
+                    k->refs++;
+                    return k;
+                }
+    }
+    std::unique_ptr<RampKey> k(new RampKey());
+    k->stops.assign(p.stops, p.stops + p.n_stops);
+    k->premul = premul;
+    k->self_equal = self_equal;
+    k->id = r->next_ramp_key++;
+    k->refs = 1;
+    RampKey *raw = k.get();
+    if (self_equal) r->ramp_by_hash[h].push_back(raw);
+    r->ramp_keys[raw->id] = std::move(k);
+    fresh.push_back(raw);
+    return raw;
+}
+static void release_ramp(vb_renderer *r, RampKey *k) {
+    if (--k->refs) return;
+    if (k->self_equal) {
+        auto it = r->ramp_by_hash.find(vb_ramp_hash(k->stops.data(), (uint32_t)k->stops.size(), k->premul));
+        it->second.erase(std::find(it->second.begin(), it->second.end(), k));
+        if (it->second.empty()) r->ramp_by_hash.erase(it);
+    }
+    r->ramp_keys.erase(k->id); // its stops stay in the pool until the pool is rebuilt
+}
+// An image key names one set of pixels. The caller's buffer need not outlive vb_fragment_upload, so its address may come back
+// holding other pixels in a later fragment: host pixels are told apart by a hash of their bytes as well as by the pointer,
+// and only a pointer that holds the same pixels again shares an atlas slot. NULL and registered-texture keys are never read
+// (hash 0): they are one image per pointer, as in a resolve.
+static bool readable_image(const void *key, uint32_t w, uint32_t h) { return key && w && h && !vb_texture_key(key); }
+static uint64_t hash_pixels(const void *key, uint32_t w, uint32_t h) {
+    const uint8_t *p = (const uint8_t *)key;
+    const size_t n = (size_t)w * h * 4u;
+    uint64_t a = 0x9e3779b97f4a7c15ull ^ n, b = 0xc2b2ae3d27d4eb4full;
+    size_t i = 0;
+    for (; i + 16u <= n; i += 16u) {
+        uint64_t x, y;
+        memcpy(&x, p + i, 8);
+        memcpy(&y, p + i + 8, 8);
+        a = (a ^ x) * 0xff51afd7ed558ccdull;
+        b = (b ^ y) * 0xc4ceb9fe1a85ec53ull;
+        a ^= a >> 29;
+        b ^= b >> 31;
+    }
+    for (; i < n; i += 4u) { // w * h * 4 is a multiple of 4
+        uint32_t x;
+        memcpy(&x, p + i, 4);
+        a = (a ^ x) * 0xff51afd7ed558ccdull;
+        a ^= a >> 29;
+    }
+    const uint64_t h64 = (a ^ (b * 0x9e3779b97f4a7c15ull)) * 0xff51afd7ed558ccdull;
+    return h64 ^ (h64 >> 32);
+}
+static ImageKey *intern_image(vb_renderer *r, const void *key, uint32_t w, uint32_t h, uint64_t pixels_hash) {
+    std::unique_ptr<ImageKey> &k = r->image_keys[std::make_tuple(key, w, h, pixels_hash)];
+    if (!k) {
+        k.reset(new ImageKey());
+        k->key = key;
+        k->w = w;
+        k->h = h;
+        k->pixels_hash = pixels_hash;
+        k->id = r->next_image_key++;
+    }
+    k->refs++;
+    return k.get();
+}
+static void release_image(vb_renderer *r, ImageKey *k) {
+    if (--k->refs == 0u) r->image_keys.erase(std::make_tuple(k->key, k->w, k->h, k->pixels_hash));
+}
+static void release_keys(vb_renderer *r, const Fragment &f) {
+    for (const Fragment::Ramp &x : f.ramps) release_ramp(r, x.key);
+    for (const Fragment::Image &x : f.images) release_image(r, x.key);
+}
+
+// Copy the stops of new ramp keys into the stop pool. When they do not fit, the pool is made anew from the live keys (their
+// stops are on the host), after the work already enqueued, which may read the old pool, has finished.
+static int place_stops(vb_renderer *r, const std::vector<RampKey *> &fresh) {
+    size_t add = 0;
+    for (const RampKey *k : fresh) add += k->stops.size();
+    if (add == 0) return VB_OK;
+    std::vector<vb_ramp_stop> host;
+    size_t first = r->pool_used;
+    if ((r->pool_used + add) * sizeof(vb_ramp_stop) <= r->stop_pool.cap) {
+        for (RampKey *k : fresh) {
+            k->pool = (uint32_t)(first + host.size());
+            host.insert(host.end(), k->stops.begin(), k->stops.end());
+        }
+    } else {
+        size_t live = 0;
+        for (const auto &e : r->ramp_keys) live += e.second->stops.size();
+        if (live > 0x7fffffffu) {
+            r->err = "vb_fragment_upload: more gradient stops than 32-bit indices reach";
+            return VB_E_INVALID;
+        }
+        CK(cudaStreamSynchronize(r->stream));
+        CK(cudaFree(r->stop_pool.p));
+        r->stop_pool = DevBuf{};
+        int rc = ensure(r, r->stop_pool, 2 * live * sizeof(vb_ramp_stop));
+        if (rc) return rc;
+        first = 0;
+        for (auto &e : r->ramp_keys) {
+            e.second->pool = (uint32_t)host.size();
+            host.insert(host.end(), e.second->stops.begin(), e.second->stops.end());
+        }
+    }
+    CK(cudaMemcpy((vb_ramp_stop *)r->stop_pool.p + first, host.data(), host.size() * sizeof(vb_ramp_stop), cudaMemcpyHostToDevice));
+    r->pool_used = (uint32_t)(first + host.size());
+    return VB_OK;
+}
+
+// Release the memory of freed fragments that no enqueued work reads any more.
+static void reap_freed(vb_renderer *r) {
+    auto &v = r->freed;
+    for (size_t i = 0; i < v.size();) {
+        if (cudaEventQuery(v[i].done) != cudaSuccess) {
+            cudaGetLastError(); // cudaErrorNotReady is not an error of the next call
+            i++;
+            continue;
+        }
+        cudaFree(v[i].mem);
+        cudaEventDestroy(v[i].done);
+        r->fragment_bytes -= v[i].bytes;
+        v[i] = v.back();
+        v.pop_back();
+    }
+}
+
+extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, uint32_t *fragment_out) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_fragment_upload: ") + why;
+        return VB_E_INVALID;
+    };
+    if (!e || !fragment_out) return bad("NULL streams or id");
+    if (check_streams(r, e, "vb_fragment_upload")) return VB_E_INVALID;
+    // the allocation: header, the six streams (tags padded to whole words), then one copy of each image key's pixels
+    uint64_t off[CMP_HEADER_WORDS] = {};
+    uint64_t w = CMP_HEADER_WORDS;
+    const uint64_t words[CMP_STREAMS] = {((uint64_t)e->n_path_tags + 3u) / 4u, e->n_path_data, e->n_draw_tags, e->n_draw_data,
+                                         6ull * e->n_transforms, 2ull * e->n_styles};
+    for (int s = 0; s < CMP_STREAMS; s++) {
+        off[s] = w;
+        w += words[s];
+    }
+    if (w + 4u > 0xfffffff0ull) return bad("the fragment's streams exceed 32-bit word offsets");
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    std::unique_ptr<Fragment> f(new Fragment());
+    size_t bytes = (size_t)(w + 4u) * 4u;
+    bytes = (bytes + 15u) & ~(size_t)15u;
+    std::vector<std::pair<size_t, const Fragment::Image *>> copies; // (offset in the allocation, image) per key with pixels
+    std::unordered_map<const ImageKey *, size_t> at;
+    std::map<std::tuple<const void *, uint32_t, uint32_t>, uint64_t> hashed; // each of this fragment's images is read once
+    for (uint32_t i = 0; i < e->n_image_patches; i++) {
+        const vb_image_patch &im = e->image_patches[i];
+        uint64_t hv = 0;
+        if (readable_image(im.pixels, im.width, im.height)) {
+            const auto t = std::make_tuple((const void *)im.pixels, im.width, im.height);
+            const auto it = hashed.find(t);
+            hv = it != hashed.end() ? it->second : (hashed[t] = hash_pixels(im.pixels, im.width, im.height));
+        }
+        f->images.push_back(Fragment::Image{im.draw_data_offset, intern_image(r, im.pixels, im.width, im.height, hv), nullptr});
+    }
+    for (Fragment::Image &x : f->images) {
+        // a registered texture's key points at nothing: its pixels exist only in device memory (an override, at compose)
+        if (!readable_image(x.key->key, x.key->w, x.key->h) || at.count(x.key)) continue;
+        at[x.key] = bytes;
+        copies.push_back({bytes, &x});
+        bytes += ((size_t)x.key->w * x.key->h * 4u + 15u) & ~(size_t)15u;
+    }
+    std::vector<RampKey *> fresh;
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        f->ramps.push_back(Fragment::Ramp{p.draw_data_offset, p.extend, intern_ramp(r, p, fresh)});
+    }
+    int rc = place_stops(r, fresh);
+    cudaError_t ce = rc ? cudaSuccess : cudaMalloc(&f->mem, bytes);
+    if (rc || ce != cudaSuccess) {
+        release_keys(r, *f);
+        if (ce != cudaSuccess) {
+            r->err = std::string("vb_fragment_upload: cudaMalloc: ") + cudaGetErrorString(ce);
+            return VB_E_CUDA;
+        }
+        return rc;
+    }
+    f->bytes = bytes;
+    for (Fragment::Image &x : f->images) {
+        const auto it = at.find(x.key);
+        if (it != at.end()) x.pixels = (const uint8_t *)f->mem + it->second;
+    }
+    uint32_t header[CMP_HEADER_WORDS];
+    for (int s = 0; s < (int)CMP_HEADER_WORDS; s++) header[s] = (uint32_t)off[s];
+    char *base = (char *)f->mem;
+    const void *src[CMP_STREAMS] = {e->path_tags, e->path_data, e->draw_tags, e->draw_data, e->transforms, e->styles};
+    const size_t len_bytes[CMP_STREAMS] = {e->n_path_tags, (size_t)e->n_path_data * 4, (size_t)e->n_draw_tags * 4, (size_t)e->n_draw_data * 4,
+                                           (size_t)e->n_transforms * 24, (size_t)e->n_styles * 8};
+    cudaStream_t st = r->upload_stream;
+    ce = cudaMemcpyAsync(base, header, sizeof header, cudaMemcpyHostToDevice, st);
+    for (int s = 0; s < CMP_STREAMS && ce == cudaSuccess; s++)
+        if (len_bytes[s]) ce = cudaMemcpyAsync(base + off[s] * 4u, src[s], len_bytes[s], cudaMemcpyHostToDevice, st);
+    for (size_t i = 0; i < copies.size() && ce == cudaSuccess; i++) {
+        const ImageKey &k = *copies[i].second->key;
+        ce = cudaMemcpyAsync(base + copies[i].first, k.key, (size_t)k.w * k.h * 4u, cudaMemcpyHostToDevice, st);
+    }
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) {
+        cudaFree(f->mem);
+        release_keys(r, *f);
+        r->err = std::string("vb_fragment_upload: copying the streams: ") + cudaGetErrorString(ce);
+        return VB_E_CUDA;
+    }
+    f->len[CMP_TAGS] = e->n_path_tags;
+    f->len[CMP_PATH_DATA] = e->n_path_data;
+    f->len[CMP_DRAW_TAGS] = e->n_draw_tags;
+    f->len[CMP_DRAW_DATA] = e->n_draw_data;
+    f->len[CMP_TRANSFORMS] = e->n_transforms;
+    f->len[CMP_STYLES] = 2u * e->n_styles;
+    f->n_paths = e->n_paths;
+    f->n_clips = e->n_clips;
+    f->n_open_clips = e->n_open_clips;
+    f->info = (uint32_t)vb_draw_info_sum(e->draw_tags, e->n_draw_tags);
+    f->id = r->next_fragment++;
+    r->fragment_bytes += bytes;
+    *fragment_out = f->id;
+    r->fragments[f->id] = std::move(f);
+    return VB_OK;
+}
+
+extern "C" int vb_fragment_free(vb_renderer *r, uint32_t fragment) {
+    if (!r) return VB_E_INVALID;
+    const auto it = r->fragments.find(fragment);
+    if (it == r->fragments.end()) {
+        r->err = "vb_fragment_free: unknown or freed fragment " + std::to_string(fragment);
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    // composes already enqueued read the memory: it is released once the stream has passed this point (reap_freed)
+    cudaEvent_t done;
+    CK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    const cudaError_t ce = cudaEventRecord(done, r->stream);
+    if (ce != cudaSuccess) {
+        cudaEventDestroy(done);
+        r->err = std::string("vb_fragment_free: ") + cudaGetErrorString(ce);
+        return VB_E_CUDA;
+    }
+    r->freed.push_back({it->second->mem, it->second->bytes, done});
+    release_keys(r, *it->second);
+    r->fragments.erase(it);
+    return VB_OK;
+}
+
+// Grow a buffer compose writes. Work already enqueued may read it: growing waits for the renderer's stream.
+static int compose_room(vb_renderer *r, DevBuf &b, size_t bytes) {
+    if (b.cap >= std::max<size_t>(bytes, 256)) return VB_OK;
+    CK(cudaStreamSynchronize(r->stream));
+    return ensure(r, b, bytes);
+}
+
+// The resident fragment of an id; nullptr when there is none (never uploaded, or freed).
+static const Fragment *find_fragment(const vb_renderer *r, uint32_t id) {
+    const auto it = r->fragments.find(id);
+    return it == r->fragments.end() ? nullptr : it->second.get();
+}
+
+static size_t up16(size_t v) { return (v + 15u) & ~(size_t)15u; }
+// The tables k_compose_streams reads for n instances: [the per-stream exclusive prefix of the instances' lengths,
+// CMP_STREAMS x (n + 1) words] [the fragments' addresses, at o_src] [the transforms, at o_xf]; `bytes` in all.
+struct CmpTables {
+    size_t o_src, o_xf, bytes;
+};
+static CmpTables cmp_tables(size_t n) {
+    CmpTables t;
+    t.o_src = up16((size_t)CMP_STREAMS * (n + 1u) * 4u);
+    t.o_xf = up16(t.o_src + n * 8u);
+    t.bytes = up16(t.o_xf + n * sizeof(CmpXform));
+    return t;
+}
+// Write the tables for instances fr with transforms xf (nullptr: none applied) at h, and return the CmpArgs that read their
+// copy at dev. The caller sets the scene, the destinations and the units.
+static CmpArgs stage_cmp_tables(const std::vector<const Fragment *> &fr, const CmpXform *xf, uint8_t *h, const char *dev) {
+    const uint32_t n = (uint32_t)fr.size();
+    const CmpTables t = cmp_tables(n);
+    for (int s = 0; s < CMP_STREAMS; s++) {
+        uint32_t *P = (uint32_t *)h + (size_t)s * (n + 1u);
+        P[0] = 0u;
+        for (uint32_t k = 0; k < n; k++) P[k + 1] = P[k] + fr[k]->len[s];
+    }
+    unsigned long long *srcs = (unsigned long long *)(h + t.o_src);
+    for (uint32_t k = 0; k < n; k++) srcs[k] = (unsigned long long)(uintptr_t)fr[k]->mem;
+    if (xf) memcpy(h + t.o_xf, xf, (size_t)n * sizeof(CmpXform));
+    else memset(h + t.o_xf, 0, (size_t)n * sizeof(CmpXform));
+    CmpArgs a;
+    memset(&a, 0, sizeof a);
+    a.prefix = (const uint32_t *)dev;
+    a.src = (const unsigned long long *)(dev + t.o_src);
+    a.xf = (const CmpXform *)(dev + t.o_xf);
+    a.n = n;
+    return a;
+}
+
+// vb_compose and vb_recompose. A recompose that damage tracking can follow (recompose_armed) also matches the instances
+// against the current scene's, stages the tables of k_recompose_damage and copies the base frame's draw boxes.
+static bool recompose_armed(const vb_renderer *r) {
+    const vb_renderer::Damage &D = r->dmg;
+    const vb_renderer::SceneSlot &s = *r->cur;
+    // the base rendered the current scene (no installation, binding, view, cells or tracking switch since: the epoch), unbound,
+    // and its draw boxes are intact (hit tests answer from it: no frame, failure, vb_run_stages or debug write since)
+    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && s.composed && !r->bound.rows && r->hit.valid &&
+           !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects &&
+           s.inst_draw.size() == s.inst_frag.size() + 1u && s.inst_img.size() == s.inst_frag.size() + 1u;
+}
+static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets,
+                   bool recompose) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = std::string(fn) + ": " + why;
+        return VB_E_INVALID;
+    };
+    if (n && !inst) return bad("NULL instances");
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    // validate everything and size the scene before anything is written
+    std::vector<const Fragment *> fr(n);
+    std::vector<CmpXform> xf(n);
+    uint64_t tot[CMP_STREAMS] = {}, n_paths = 0, n_clips = 0, n_open = 0, info = 0;
+    for (uint32_t k = 0; k < n; k++) {
+        if (!(fr[k] = find_fragment(r, inst[k].fragment))) return bad("unknown or freed fragment " + std::to_string(inst[k].fragment));
+        memset(&xf[k], 0, sizeof xf[k]);
+        xf[k].on = inst[k].has_transform ? 1u : 0u;
+        for (int c = 0; c < 6 && xf[k].on; c++) {
+            xf[k].m[c] = (float)inst[k].transform[c]; // Transform::from_kurbo
+            if (!isfinite(xf[k].m[c])) return bad("instance " + std::to_string(k) + ": the transform must be finite in f32");
+        }
+        for (int s = 0; s < CMP_STREAMS; s++) tot[s] += fr[k]->len[s];
+        n_paths += fr[k]->n_paths;
+        n_clips += fr[k]->n_clips;
+        n_open += fr[k]->n_open_clips;
+        info += fr[k]->info;
+    }
+    VbLayout L;
+    uint32_t padded;
+    size_t total_words;
+    if (!vb_resolve_layout(tot[CMP_TAGS], tot[CMP_PATH_DATA], tot[CMP_DRAW_TAGS], tot[CMP_DRAW_DATA], tot[CMP_TRANSFORMS], tot[CMP_STYLES] / 2u, n_open,
+                           n_paths, n_clips, info, &L, &padded, &total_words))
+        return bad("the composed scene exceeds 32-bit word offsets");
+
+    // late-bound ramps and images of every instance in order: the host resolve's de-duplication and shelf placement, keyed
+    // by the keys the fragments hold
+    const uint64_t seq = ++r->compose_seq;
+    std::vector<RsPatch> patches;
+    std::vector<RsRamp> ramps;
+    std::vector<uint32_t> ramp_ids;
+    struct Placed { const ImageKey *key; const uint8_t *src; uint32_t x, y, frag; };
+    std::vector<Placed> placed;
+    std::vector<uint32_t> img_pre(n + 1u, 0u), img_local; // each instance's images: their place in `placed`
+    VbShelfPacker shelf;
+    uint32_t dd0 = L.draw_data_base;
+    for (uint32_t k = 0; k < n; k++) {
+        const Fragment &f = *fr[k];
+        img_pre[k + 1] = img_pre[k] + (uint32_t)f.images.size();
+        for (const Fragment::Ramp &p : f.ramps) {
+            RampKey *key = p.key;
+            if (key->stamp != seq || !key->self_equal) {
+                key->stamp = seq;
+                key->local = (uint32_t)ramps.size();
+                ramps.push_back(RsRamp{key->pool, (uint32_t)key->stops.size(), key->premul ? 1u : 0u, 0u});
+                ramp_ids.push_back(key->id);
+            }
+            patches.push_back(RsPatch{dd0 + p.dd, (key->local << 2) | p.extend});
+        }
+        for (const Fragment::Image &im : f.images) {
+            ImageKey *key = im.key;
+            if (key->stamp != seq) {
+                key->stamp = seq;
+                key->local = (uint32_t)placed.size();
+                placed.push_back(Placed{key, im.pixels, 0, 0, f.id});
+                shelf.place(key->w, key->h, &placed.back().x, &placed.back().y);
+            }
+            const Placed &q = placed[key->local];
+            patches.push_back(RsPatch{dd0 + im.dd, (q.x << 16) | q.y});
+            img_local.push_back(key->local);
+        }
+        dd0 += f.len[CMP_DRAW_DATA];
+    }
+    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
+    // images with an override on this renderer come from its device memory, the others from their fragment's copy
+    std::vector<VbBlitRect> blits;
+    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
+    std::vector<uint64_t> atlas_keys;
+    int rc;
+    for (const Placed &q : placed) {
+        const ImageKey &k = *q.key;
+        bool overridden;
+        if ((rc = image_source(r, fn, k.key, k.w, k.h, q.x, q.y, blits, over, &overridden))) return rc;
+        if (!overridden && q.src) blits.push_back(VbBlitRect{q.src, (uint64_t)k.w * 4u, 0, k.w, k.h, q.x, q.y, 0, 0});
+        // where the slot's pixels come from: the fragment, an override (never a fragment id), or nowhere (a zero region)
+        atlas_keys.push_back((uint64_t)k.id << 32 | (overridden ? CMP_FROM_OVERRIDE : q.src ? q.frag : 0u));
+    }
+    std::vector<ImgPlace> img_place(img_local.size());
+    for (size_t t = 0; t < img_local.size(); t++) {
+        const Placed &q = placed[img_local[t]];
+        img_place[t] = ImgPlace{atlas_keys[img_local[t]], (q.x << 16) | q.y};
+    }
+
+    // vb_recompose: match the new instances to the current scene's (vb_diff.h). A matched instance whose images moved in the
+    // atlas, or come from an override (copied again by this compose), is unmatched: fine samples in atlas coordinates.
+    const vb_renderer::SceneSlot &was = *r->cur;
+    const bool arm = recompose && recompose_armed(r);
+    const uint32_t n_old = arm ? (uint32_t)was.inst_frag.size() : 0u, old_draws = arm ? was.layout.n_draw_objects : 0u;
+    std::vector<uint32_t> match(arm ? n : 0u), unmatched(n_old, 1u);
+    if (arm) {
+        vb_diff_match(
+            n_old, n,
+            [&](uint32_t i, uint32_t j) { return was.inst_frag[i] == fr[j]->id && memcmp(&was.inst_xf[i], &xf[j], sizeof(CmpXform)) == 0; },
+            match.data());
+        for (uint32_t j = 0; j < n; j++) {
+            const uint32_t i = match[j];
+            if (i == VB_DIFF_NONE) continue;
+            const ImgPlace *a = was.img_place.data() + was.inst_img[i], *b = img_place.data() + img_pre[j];
+            for (uint32_t t = 0; t < img_pre[j + 1] - img_pre[j] && match[j] != VB_DIFF_NONE; t++)
+                if (a[t].key != b[t].key || a[t].xy != b[t].xy || (uint32_t)b[t].key == CMP_FROM_OVERRIDE) match[j] = VB_DIFF_NONE;
+            if (match[j] != VB_DIFF_NONE) unmatched[i] = 0u;
+        }
+    }
+
+    if ((rc = drain_stream(r))) return rc;
+    CK(cudaSetDevice(r->device));
+    reap_freed(r);
+    cudaStream_t st = r->stream;
+    vb_renderer::SceneSlot &slot = *r->cur;
+    const bool new_ramps = !slot.composed || ramp_ids != slot.ramp_keys;
+    const bool new_atlas = !slot.composed || atlas_keys != slot.atlas_keys || !over.empty();
+    // the tables, staged through pinned memory: k_compose_streams' (cmp_tables), patches, ramp descriptors
+    const size_t o_pat = cmp_tables(n).bytes;
+    const size_t o_ramp = up16(o_pat + patches.size() * sizeof(RsPatch)), staged = o_ramp + ramps.size() * sizeof(RsRamp);
+    // vb_recompose's tables (VbFrameBufs::rcmp_tables), staged after compose's, and where they go in rcmp: after the old boxes
+    const size_t o_rc = up16(staged), rc_bytes = arm ? ((size_t)n_old + 1u + n + 1u + n + n_old) * 4u : 0u;
+    const size_t o_tables = up16((size_t)old_draws * sizeof(VbBbox4)), host_bytes = o_rc + rc_bytes;
+    if ((rc = compose_room(r, r->compose_tmp, staged))) return rc;
+    char *tmp = (char *)r->compose_tmp.p;
+    PinnedStage &stage = r->pinned[PIN_COMPOSE];
+    uint8_t *h;
+    if ((rc = stage_host(r, stage, host_bytes, &h))) return rc;
+    CmpArgs a = stage_cmp_tables(fr, xf.data(), h, tmp);
+    const uint32_t *pre = (const uint32_t *)h;
+    if (!patches.empty()) memcpy(h + o_pat, patches.data(), patches.size() * sizeof(RsPatch));
+    if (!ramps.empty()) memcpy(h + o_ramp, ramps.data(), ramps.size() * sizeof(RsRamp));
+    if (draw_offsets) memcpy(draw_offsets, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+    if (arm) {
+        uint32_t *t = (uint32_t *)(h + o_rc);
+        memcpy(t, was.inst_draw.data(), ((size_t)n_old + 1u) * 4u);
+        memcpy(t + n_old + 1u, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+        if (n) memcpy(t + n_old + 1u + n + 1u, match.data(), (size_t)n * 4u);
+        if (n_old) memcpy(t + n_old + 1u + n + 1u + n, unmatched.data(), (size_t)n_old * 4u);
+        if ((rc = compose_room(r, r->rcmp, o_tables + rc_bytes))) return rc;
+    }
+
+    if ((rc = compose_room(r, slot.scene, scene_bytes(L, total_words, r->view.on)))) return rc;
+    if (new_ramps && (rc = compose_room(r, slot.ramps, ramps.size() * 512u * 4u))) return rc;
+    if (new_atlas && (rc = compose_room(r, slot.atlas, (size_t)atlas_w * atlas_h * 4u))) return rc;
+    if (staged) CK(cudaMemcpyAsync(tmp, h, staged, cudaMemcpyHostToDevice, st));
+    if (arm) { // the base frame's boxes, before anything can rewrite them, and the tables
+        if (old_draws) CK(cudaMemcpyAsync(r->rcmp.p, r->hit.bufs.draw_bboxes, (size_t)old_draws * sizeof(VbBbox4), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync((char *)r->rcmp.p + o_tables, h + o_rc, rc_bytes, cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = stage_copied(r, stage))) return rc;
+    uint32_t *scene = (uint32_t *)slot.scene.p;
+    a.scene = scene;
+    const uint32_t dst[CMP_STREAMS] = {L.path_tag_base, L.path_data_base, L.draw_tag_base, L.draw_data_base, L.transform_base, L.style_base};
+    const uint32_t units[CMP_STREAMS] = {(uint32_t)((tot[CMP_TAGS] + 3u) / 4u), (uint32_t)tot[CMP_PATH_DATA], (uint32_t)tot[CMP_DRAW_TAGS],
+                                         (uint32_t)tot[CMP_DRAW_DATA], (uint32_t)tot[CMP_TRANSFORMS], (uint32_t)tot[CMP_STYLES]};
+    memcpy(a.dst, dst, sizeof dst);
+    memcpy(a.units, units, sizeof units);
+    vb_launch_compose(a, st);
+    vb_launch_resolve_finish(scene, (uint32_t)tot[CMP_TAGS], (uint32_t)n_open, padded, L.draw_tag_base + (uint32_t)tot[CMP_DRAW_TAGS],
+                             (const RsPatch *)(tmp + o_pat), (uint32_t)patches.size(), st);
+    if (new_ramps) {
+        vb_launch_make_ramps((const RsRamp *)(tmp + o_ramp), (const RsStop *)r->stop_pool.p, (uint32_t)ramps.size(), (uint32_t *)slot.ramps.p, st);
+        slot.ramp_keys = std::move(ramp_ids);
+    }
+    if (new_atlas) {
+        CK(cudaMemsetAsync(slot.atlas.p, 0, (size_t)atlas_w * atlas_h * 4u, st));
+        if ((rc = enqueue_blits(r, blits, slot.atlas.p, atlas_w))) return rc;
+        slot.atlas_keys = std::move(atlas_keys);
+    }
+    CK(cudaGetLastError());
+    set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), true);
+    slot.inst_frag.resize(n);
+    for (uint32_t k = 0; k < n; k++) slot.inst_frag[k] = fr[k]->id;
+    slot.inst_xf = std::move(xf);
+    slot.inst_draw.assign(pre + (size_t)CMP_DRAW_TAGS * (n + 1u), pre + (size_t)(CMP_DRAW_TAGS + 1) * (n + 1u));
+    slot.inst_img = std::move(img_pre);
+    slot.img_place = std::move(img_place);
+    vb_renderer::Damage::Diff &X = r->dmg.diff;
+    X.armed = arm;
+    if (arm) { // the next frame of this installation's epoch is incremental (damage_prepare)
+        X.epoch = r->dmg.epoch;
+        X.n_old = n_old;
+        X.n_new = n;
+        X.old_draws = old_draws;
+        X.new_draws = L.n_draw_objects;
+        X.o_tables = o_tables;
+    }
+    if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
+    return VB_OK;
+}
+
+extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+    return compose(r, "vb_compose", inst, n, layout_out, draw_offsets, false);
+}
+extern "C" int vb_recompose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
+    return compose(r, "vb_recompose", inst, n, layout_out, draw_offsets, true);
+}
+extern "C" uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t n_old, const uint32_t *new_keys, uint32_t n_new, uint32_t *match) {
+    return vb_diff_match(n_old, n_new, [&](uint32_t i, uint32_t j) { return old_keys[i] == new_keys[j]; }, match);
+}
+
+// ---- bound instance transforms: vb_bind_instance_transforms (k_compose.cu) ----------------------------------------------------
+// The binding's tables are made once, here: the transform prefix and compose-time transforms from the slot's instance records,
+// the untransformed transforms by one k_compose_streams over the transform stream alone (no transforms applied, destination 0).
+// Every frame after that reads the caller's rows in its k_instance_transforms.
+extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_transforms, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_instance_transforms: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_transforms) {
+        r->bound = vb_renderer::Binding{};
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene || !slot.composed) return bad("the renderer's current scene was not made by vb_compose");
+    if (n == 0u || n != slot.inst_frag.size())
+        return bad(std::to_string(n) + " rows for a composed scene of " + std::to_string(slot.inst_frag.size()) + " instances");
+    if ((uintptr_t)device_transforms & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 24u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 24 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_transforms)) return bad("the rows must be memory of the renderer's device");
+    std::vector<const Fragment *> fr(n);
+    for (uint32_t k = 0; k < n; k++)
+        if (!(fr[k] = find_fragment(r, slot.inst_frag[k]))) return bad("fragment " + std::to_string(slot.inst_frag[k]) + " of the composed scene was freed");
+    // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one)
+    const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr > 0xfffffff0ull)
+        return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
+
+    // staged through pinned memory: [the copy's tables (cmp_tables), with no transforms] [the binding's tables: transform
+    // prefix (n + 1), compose-time transforms] [the instances' draw prefix (n + 1)]
+    reap_freed(r);
+    const size_t tmp_bytes = cmp_tables(n).bytes;
+    const size_t o_xf = up16(((size_t)n + 1u) * 4u), o_tr = up16(o_xf + (size_t)n * sizeof(CmpXform));
+    const size_t o_draw = up16(o_tr + (size_t)n_tr * 24u), draw_bytes = ((size_t)n + 1u) * 4u; // staged right after the tables
+    const size_t staged = tmp_bytes + o_tr + draw_bytes;
+    int rc;
+    if ((rc = compose_room(r, r->compose_tmp, tmp_bytes))) return rc;
+    char *tmp = (char *)r->compose_tmp.p;
+    PinnedStage &stage = r->pinned[PIN_COMPOSE];
+    uint8_t *h;
+    if ((rc = stage_host(r, stage, staged, &h))) return rc;
+    CmpArgs a = stage_cmp_tables(fr, nullptr, h, tmp);
+    memcpy(h + tmp_bytes, (const uint32_t *)h + (size_t)CMP_TRANSFORMS * (n + 1u), ((size_t)n + 1u) * 4u);
+    memcpy(h + tmp_bytes + o_xf, slot.inst_xf.data(), (size_t)n * sizeof(CmpXform));
+    memcpy(h + tmp_bytes + o_tr, slot.inst_draw.data(), draw_bytes);
+
+    if ((rc = compose_room(r, r->inst_tables, o_draw + draw_bytes))) return rc;
+    cudaStream_t st = r->stream;
+    char *tables = (char *)r->inst_tables.p;
+    CK(cudaMemcpyAsync(tmp, h, tmp_bytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tables, h + tmp_bytes, o_tr, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tables + o_draw, h + tmp_bytes + o_tr, draw_bytes, cudaMemcpyHostToDevice, st));
+    if ((rc = stage_copied(r, stage))) return rc;
+    a.scene = (uint32_t *)(tables + o_tr);
+    a.units[CMP_TRANSFORMS] = n_tr;
+    vb_launch_compose(a, st);
+    CK(cudaGetLastError());
+    r->bound.rows = (const uint8_t *)device_transforms;
+    r->bound.n = n;
+    r->bound.pitch = (uint32_t)row_pitch_bytes;
+    r->bound.o_xf = o_xf;
+    r->bound.o_src = o_tr;
+    r->bound.o_draw = o_draw;
+    r->dmg.epoch++;
+    return VB_OK;
+}

@@ -1,0 +1,150 @@
+// vb_damage.cu -- damage tracking (k_damage.cu): which frames are incremental, and the C ABI around it.
+#include <cuda_runtime.h>
+#include <string.h>
+
+#include <algorithm>
+
+#include "vb_renderer.h"
+
+// ---- damage tracking: vb_set_damage_tracking / vb_add_damage / vb_last_damage (k_damage.cu) -------------------------------
+// After prepare and pick_out: is the frame incremental, full, or outside damage tracking (a batch, a window, the exchange:
+// mode VB_DMG_OFF, and no base for the next frame)? The decision is the same for every re-run of the frame, because the base
+// and the forcing flags change only when a frame succeeds (damage_succeeded). Allocates the mask, the staged rectangles and
+// the snapshot; their sizes follow from the frame size and the scene, so they never move under an incremental frame.
+int vb_host::damage_prepare(vb_renderer *r) {
+    vb_renderer::Damage &D = r->dmg;
+    const VbConfig &c = r->cfg;
+    vb_renderer::DamageFrame f;
+    f.w = c.target_width;
+    f.h = c.target_height;
+    f.aa = r->params.aa;
+    f.base_color = c.base_color;
+    f.dest = r->dest.dev;
+    f.epoch = D.epoch;
+    const bool windowed = r->params.bin_row1 > r->params.bin_row0 || r->params.tile_row1 > r->params.tile_row0;
+    f.can_base = D.on && c.n_cells == 1u && !windowed && !r->xc.enabled && !r->grouped;
+    D.frame = f;
+    if (!f.can_base) return VB_OK;
+    // an overridden image copied again changes pixels nothing here can locate: the frame is full unless the caller named them
+    for (const auto &o : r->cur->overridden)
+        if (o.dirty && !D.rects) D.force_full = true;
+    const vb_renderer::DamageFrame &B = D.base;
+    const bool diff = D.diff.armed && D.diff.epoch == f.epoch; // the scene is a recompose of the base's (vb_recompose)
+    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff) && B.w == f.w && B.h == f.h &&
+                             B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
+    f.mode = incremental ? VB_DMG_INCREMENTAL : VB_DMG_FULL;
+    // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
+    // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
+    if (D.last.mode == VB_DMG_INCREMENTAL) D.have_last = false;
+    const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles, n_draw = r->cur->layout.n_draw_objects;
+    const uint32_t n_xf = r->bound.rows ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
+    int rc;
+    if ((rc = ensure(r, r->dmg_mask, n_tiles))) return rc;
+    if ((rc = ensure(r, r->dmg_pending, n_tiles))) return rc;
+    if (r->bound.rows) {
+        if ((rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw) * 4u))) return rc;
+        if ((rc = ensure(r, r->dmg_changed, (size_t)r->bound.n * 4u))) return rc;
+    }
+    VbFrameBufs &b = r->bufs;
+    b.dmg_mask = (uint8_t *)r->dmg_mask.p;
+    b.dmg_pending = (uint8_t *)r->dmg_pending.p;
+    if (r->bound.rows) {
+        b.dmg_snap = (uint32_t *)r->dmg_snap.p;
+        b.dmg_changed = (uint32_t *)r->dmg_changed.p;
+        b.inst_draw = (const uint32_t *)((const char *)r->inst_tables.p + r->bound.o_draw);
+    }
+    b.dmg_mode = f.mode;
+    b.dmg_n_xf = n_xf;
+    if (incremental && diff) {
+        b.rcmp_old_boxes = (const VbBbox4 *)r->rcmp.p;
+        b.rcmp_tables = (const uint32_t *)((const char *)r->rcmp.p + D.diff.o_tables);
+        b.rcmp_n_old = D.diff.n_old;
+        b.rcmp_n_new = D.diff.n_new;
+        b.rcmp_old_draws = D.diff.old_draws;
+        b.rcmp_new_draws = D.diff.new_draws;
+    }
+    D.frame = f;
+    return VB_OK;
+}
+// The frame prepared last succeeded: it is the one vb_last_damage reports, and the base of the next frame when it was tracked.
+void vb_host::damage_succeeded(vb_renderer *r) {
+    vb_renderer::Damage &D = r->dmg;
+    D.last = D.frame;
+    D.have_last = true;
+    D.have_base = D.frame.mode != VB_DMG_OFF;
+    if (D.have_base) D.base = D.frame;
+    D.rects = false;
+    D.force_full = false;
+    D.diff.armed = false;
+}
+
+extern "C" int vb_set_damage_tracking(vb_renderer *r, int on) {
+    if (!r) return VB_E_INVALID;
+    if (on && (r->grouped || r->xc.configured)) {
+        r->err = "vb_set_damage_tracking: not available for a renderer of a vb_group or with the exchange";
+        return VB_E_INVALID;
+    }
+    r->dmg.on = on != 0;
+    r->dmg.epoch++; // switched on (or on again): the next frame is full
+    if (!on) r->dmg.have_base = false;
+    return VB_OK;
+}
+
+extern "C" int vb_add_damage(vb_renderer *r, const uint32_t *rects, uint32_t n) {
+    if (!r) return VB_E_INVALID;
+    if (n && !rects) {
+        r->err = "vb_add_damage: NULL rectangles";
+        return VB_E_INVALID;
+    }
+    // the rectangles belong to the frame after the one in flight, whose size and success are not known yet
+    if (r->frame_pending || r->stream_pending) {
+        r->err = "vb_add_damage: a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)";
+        return VB_E_INVALID;
+    }
+    vb_renderer::Damage &D = r->dmg;
+    if (!D.on || n == 0u) return VB_OK;
+    D.rects = true;
+    if (!D.have_base) return VB_OK; // the next frame is a full one
+    // clamped to the frame the next incremental frame must match, rounded out to tiles
+    const uint32_t w = D.base.w, h = D.base.h, wt = (w + 15u) / 16u;
+    std::vector<uint32_t> t;
+    t.reserve((size_t)n * 4u);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t *q = rects + 4u * (size_t)i;
+        const uint32_t x0 = std::min(q[0], w), y0 = std::min(q[1], h), x1 = std::min(q[2], w), y1 = std::min(q[3], h);
+        if (x1 <= x0 || y1 <= y0) continue;
+        t.insert(t.end(), {x0 / 16u, y0 / 16u, (x1 + 15u) / 16u, (y1 + 15u) / 16u});
+    }
+    if (t.empty()) return VB_OK;
+    CK(cudaSetDevice(r->device));
+    vb_launch_damage_rects((uint8_t *)r->dmg_pending.p, wt, t.data(), (uint32_t)(t.size() / 4u), r->stream); // in stream order
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+
+extern "C" int vb_last_damage(vb_renderer *r, uint8_t *tile_mask, size_t cap, uint32_t *n_damaged) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_last_damage: ") + why;
+        return VB_E_INVALID;
+    };
+    if (r->frame_pending || r->stream_pending) return bad("a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)");
+    const vb_renderer::Damage &D = r->dmg;
+    if (!D.have_last) return bad("no completed frame to report (none yet, or a later tracked frame failed or was streamed)");
+    const size_t n_tiles = (size_t)((D.last.w + 15u) / 16u) * ((D.last.h + 15u) / 16u);
+    if (tile_mask && cap < n_tiles) return bad("the mask holds fewer bytes than the frame has tiles");
+    std::vector<uint8_t> m(n_tiles, 1u); // a frame that was not incremental rendered every tile
+    if (D.last.mode == VB_DMG_INCREMENTAL) {
+        CK(cudaSetDevice(r->device));
+        CK(cudaMemcpyAsync(m.data(), r->dmg_mask.p, n_tiles, cudaMemcpyDeviceToHost, r->stream));
+        CK(cudaStreamSynchronize(r->stream));
+    }
+    uint32_t count = 0;
+    for (uint8_t &v : m) {
+        v = v ? 1u : 0u;
+        count += v;
+    }
+    if (tile_mask) memcpy(tile_mask, m.data(), n_tiles);
+    if (n_damaged) *n_damaged = count;
+    return VB_OK;
+}

@@ -1,4 +1,4 @@
-// vb_diff.h -- the order-preserving matching of a recompose (vb_recompose, vb_api.cu): which instances of the old composition
+// vb_diff.h -- the order-preserving matching of a recompose (vb_recompose, vb_compose.cu): which instances of the old composition
 // reappear, unchanged, in the new one. Plain C++, no CUDA.
 //
 // match[j] = i pairs new element j with old element i (VB_DIFF_NONE: unpaired). Pairs are between equal elements only, and

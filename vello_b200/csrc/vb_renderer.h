@@ -1,0 +1,419 @@
+// vb_renderer.h -- the renderer's host state (struct vb_renderer) and the helpers its host files share. Internal to the library.
+//
+// The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
+// (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
+// instance transforms), vb_damage.cu (damage tracking), vb_debug.cu (debug downloads and uploads) and vb_group.cu (vb_group,
+// the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in namespace vb_host, hidden
+// from the shared library's symbol table, so that a host program's own functions of the same names cannot interpose on them.
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include <map>
+#include <memory>
+#include <string>
+#include <tuple>
+#include <unordered_map>
+#include <vector>
+
+#include "../../include/vello_b200.h"
+#include "vb_stages.h"
+#include "vb_types.h"
+
+struct DevBuf {
+    void *p = nullptr;
+    size_t cap = 0; // bytes
+};
+
+// Pinned host memory that tables reach the device through (stage_host / stage_copied). It is rewritten only once the last
+// copy out of it has run.
+struct PinnedStage {
+    uint8_t *host = nullptr;
+    size_t cap = 0;                 // bytes
+    cudaEvent_t copied = nullptr;   // the last copy out of host
+};
+// The renderer's stages: the rectangles of k_atlas_blit, and the tables of compose and bind. They are separate because compose
+// enqueues its blits while its own tables are still being copied.
+enum { PIN_BLITS, PIN_COMPOSE, N_PINNED };
+
+// the seven bump-allocated arenas, in the order of VbConfig::lines_size .. ptcl_size (ARENAS below)
+enum { ARENA_LINES, ARENA_BINNING, ARENA_TILES, ARENA_SEG_COUNTS, ARENA_SEGMENTS, ARENA_BLEND, ARENA_PTCL, N_ARENAS };
+static_assert(offsetof(VbConfig, ptcl_size) - offsetof(VbConfig, lines_size) == (N_ARENAS - 1) * sizeof(uint32_t),
+              "VbConfig's arena sizes are consecutive words in ARENA_* order");
+
+// Where a frame's pixels go: a device pointer, or the renderer's own target (target_alt when `alt`), and optionally a copy of
+// the frame in host memory, read back in `bands` row bands while fine runs.
+struct Dest {
+    void *dev = nullptr, *host = nullptr;
+    bool alt = false;
+    uint32_t bands = 1;
+};
+
+// key of a captured frame: the inputs of its launches (see enqueue)
+struct GraphKey {
+    VbConfig cfg;
+    VbFrameBufs bufs;
+    const void *out;
+    const VbBump *h_bump_dev;
+    uint32_t aa, cull, last;
+    const void *xarena; // exchange: the arena holding the epoch counter, and the peer table; zero while it is off
+    XPeers xpeers;
+};
+static_assert(sizeof(VbFrameBufs) == offsetof(VbFrameBufs, sm_count) + sizeof(int), "VbFrameBufs has no padding (GraphKey is compared bytewise)");
+struct GraphSlot {
+    GraphKey key;
+    cudaGraphExec_t exec = nullptr;
+    uint32_t launches = 0;
+};
+
+// A view (vb_set_view): the f32 coefficients every frame enqueued while it is set renders the scene under.
+struct View {
+    bool on = false;
+    float m[6] = {};
+};
+
+// Everything a frame needs to be issued again (issue): a re-run renders under the view and from the scene slot the frame
+// was first issued with, even if the renderer's have changed since.
+struct Frame {
+    vb_params params{};
+    Dest dest;
+    View view;
+    uint32_t slot = 0;
+};
+
+// Composition (vb_compose). A ramp key is one distinct gradient ramp, (stops, interpolation space) compared as every
+// resolve compares them (vb_same_ramp); an image key is one atlas slot, (pixels pointer, width, height, hash of the pixels). Fragments hold
+// references to the keys of their patches, so de-duplicating a composed scene's ramps and images is a walk over the
+// instances' patch lists (stamp / local: the ramp id or atlas slot the key got in the compose numbered stamp).
+struct RampKey {
+    std::vector<vb_ramp_stop> stops;
+    bool premul = false;
+    bool self_equal = true; // false when a stop holds a NaN: such a ramp equals no other ramp, itself included
+    uint32_t id = 0, refs = 0;
+    uint32_t pool = 0;      // its first stop in the renderer's stop pool
+    uint64_t stamp = 0;
+    uint32_t local = 0;
+};
+struct ImageKey {
+    const void *key = nullptr;
+    uint32_t w = 0, h = 0, id = 0, refs = 0;
+    uint64_t pixels_hash = 0; // of the pixels read at upload (0 for a NULL or registered-texture key, which are not read)
+    uint64_t stamp = 0;
+    uint32_t local = 0;
+};
+// A resident fragment: its streams in one device allocation, back to back behind a header of their word offsets (k_compose.cu
+// reads it), followed by a copy of the pixels of each image key it draws. Patch words are as the encoder wrote them.
+enum { CMP_TAGS, CMP_PATH_DATA, CMP_DRAW_TAGS, CMP_DRAW_DATA, CMP_TRANSFORMS, CMP_STYLES, CMP_STREAMS };
+#define CMP_HEADER_WORDS 8u
+#define CMP_FROM_OVERRIDE 0xffffffffu // the source of an atlas slot filled from an override (fragment ids start at 1, count up)
+// An image's atlas slot in a composition: (image-key id << 32 | pixel source), as in SceneSlot::atlas_keys, and x << 16 | y.
+struct ImgPlace {
+    uint64_t key;
+    uint32_t xy;
+};
+struct Fragment {
+    uint32_t id = 0;
+    void *mem = nullptr;
+    size_t bytes = 0;
+    uint32_t len[CMP_STREAMS] = {}; // tag bytes, path data words, draw tags, draw data words, transforms, style words
+    uint32_t n_paths = 0, n_clips = 0, n_open_clips = 0, info = 0;
+    struct Ramp { uint32_t dd, extend; RampKey *key; };
+    struct Image { uint32_t dd; ImageKey *key; const uint8_t *pixels; }; // pixels: in mem, or nullptr for a NULL / texture key
+    std::vector<Ramp> ramps;
+    std::vector<Image> images;
+};
+
+struct vb_renderer {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    bool timing = false;
+    uint32_t max_retries = 6;
+    std::string err;
+    int sm_count = 132;
+
+    // Streaming (vb_render_begin) keeps TWO frames in flight: while frame k is rasterised, frame k+1's scene is uploaded
+    // into the other slot on its own stream and frame k-1's pixels drain to the host. `cur` is the slot frames render from.
+    struct SceneSlot {
+        bool have_scene = false;
+        VbLayout layout{};
+        size_t scene_words = 0;
+        uint32_t n_ramps = 0, atlas_w = 0, atlas_h = 0;
+        DevBuf scene, ramps, atlas;
+        VbBump *h_bump = nullptr;     // pinned + mapped: the device writes the counters straight into host memory
+        VbBump *h_bump_dev = nullptr; // device-side address of h_bump
+        // the images of the last device resolve that were copied from an override, with their atlas places: a dirty one is
+        // copied again before the next frame (refresh_overrides), without a new resolve
+        struct OverridePlace {
+            const void *key;
+            const uint8_t *src;
+            size_t pitch;
+            uint32_t w, h, x, y;
+            bool dirty;
+        };
+        std::vector<OverridePlace> overridden;
+        // set by vb_compose, cleared by every other upload: what the slot's ramps and atlas were made from, so that a compose
+        // regenerates them only when that changes (ramp-key ids in ramp order; (image-key id << 32 | source fragment) in
+        // placement order)
+        bool composed = false;
+        std::vector<uint32_t> ramp_keys;
+        std::vector<uint64_t> atlas_keys;
+        // the composed scene's instances, for vb_bind_instance_transforms: each one's fragment id and compose-time transform
+        std::vector<uint32_t> inst_frag;
+        std::vector<CmpXform> inst_xf;
+        std::vector<uint32_t> inst_draw; // the exclusive prefix of the instances' draw objects (n + 1), for damage tracking
+        // for vb_recompose: the atlas places of the instances' images in patch order, instance k's from inst_img[k] (n + 1)
+        std::vector<uint32_t> inst_img;
+        std::vector<ImgPlace> img_place;
+    } slot[2];
+    SceneSlot *cur = slot;
+    DevBuf mask8, mask16;
+
+    // fixed-size intermediates
+    DevBuf tag_monoids, path_bboxes, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
+        ctl, target, target_alt, tile_start, cls_list;
+    // Renderer::override_image: images (by key) whose pixels come from device memory at the device resolve
+    struct Override {
+        const uint8_t *src;
+        size_t pitch;
+        uint32_t w, h;
+    };
+    std::unordered_map<const void *, Override> overrides;
+    DevBuf blit_rects;                  // k_atlas_blit's rectangles, staged through pinned[PIN_BLITS]
+    PinnedStage pinned[N_PINNED];
+    // bump arenas (ARENAS), capacities in elements
+    DevBuf resolve_tmp; // patches, ramp descriptors and stops of vb_scene_upload_streams
+    DevBuf lines, line_scratch, flatten_jobs, flatten_parts, tiles, seg_counts, segments, ptcl, blend_spill;
+    uint32_t cap[N_ARENAS] = {};
+    // test-only capacity limits (vb_debug_limit_arena); UINT32_MAX = none
+    uint32_t limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
+
+    // batch (vb_set_cells): the draw-object offsets of the cells of the current scene (n_cells + 1 entries, a copy of cell_draw);
+    // empty = one cell, no batch. Every scene upload empties it.
+    std::vector<uint32_t> cells;
+    DevBuf cell_draw;
+    bool grouped = false; // a renderer of a vb_group: no batches
+
+    // per-frame
+    VbConfig cfg{};
+    vb_params params{};
+    Dest dest; // of the frame frame_prepare set up
+    uint32_t launches = 0;
+    VbFrameBufs bufs{};           // the buffers of the frame prepare set up, as the launchers take them
+    bool use_graph = true;        // replay whole frames as CUDA graphs (see enqueue)
+    GraphSlot graphs[4];
+    uint32_t graph_next = 0;
+    uint64_t graph_captures = 0;  // whole-frame graphs instantiated (vb_debug_graph_captures)
+    // the view of the frames enqueued from now on; its coefficients reach view_coef in stream order (put_view)
+    View view;
+    DevBuf view_coef;
+    uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
+    uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
+    // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct)
+    cudaStream_t tiling_stream = nullptr;
+    cudaEvent_t tiling_fork = nullptr, tiling_join = nullptr;
+    cudaEvent_t ev[VB_N_STAGE_IDS + 1]{};
+    cudaEvent_t frame_ev[2]{}; // around every whole frame (vb_last_frame_ms: the signal stripe balancing uses)
+    bool frame_timed = false;
+    bool ev_ok = false;
+    // read-back pipeline of vb_render (host output): fine runs in row bands, each band's D2H copy overlaps the next band
+    cudaStream_t copy_stream = nullptr;
+    cudaEvent_t band_ev[8]{};
+    // streaming read-back (vb_render_begin): frames alternate between two targets so that the copy of frame n can
+    // still be draining while frame n+1 is rasterised
+    bool stream_pending = false;
+    cudaEvent_t copy_done[3]{};
+    bool frame_pending = false;
+
+    cudaStream_t upload_stream = nullptr;
+    cudaEvent_t upload_done[2]{}, raster_done[2]{};
+    struct RingFrame { // a streamed frame between vb_render_begin and its completion on the host
+        bool pending = false, raster_checked = false;
+        Frame frame;
+        vb_frame_stats stats{};
+    } ring[3];
+    uint64_t stream_seq = 0;
+
+    // hit testing (vb_hit_test): the config and buffers of a frame, taken when it is enqueued (hit_enq) and handed to `hit` once
+    // it is known to have succeeded. `hit` stays valid until something rewrites what the answers read: the next frame, a scene
+    // upload, vb_set_cells, vb_run_stages, vb_debug_upload or vb_debug_limit_arena.
+    struct HitFrame {
+        bool valid = false;
+        bool windowed = false; // rendered with a bin_row / tile_row window
+        VbConfig cfg{};
+        VbFrameBufs bufs{};
+    } hit, hit_enq;
+    DevBuf hit_io; // the host form's points and answers
+
+    // composition (vb_fragment_upload / vb_compose): the resident fragments by id, and the keys their ramps and images are
+    // de-duplicated by across fragments
+    std::unordered_map<uint32_t, std::unique_ptr<Fragment>> fragments;
+    uint32_t next_fragment = 1;
+    size_t fragment_bytes = 0;
+    std::unordered_map<uint64_t, std::vector<RampKey *>> ramp_by_hash; // ramps whose stops compare equal to themselves
+    std::unordered_map<uint32_t, std::unique_ptr<RampKey>> ramp_keys;
+    uint32_t next_ramp_key = 1;
+    DevBuf stop_pool;      // the stops of every ramp key, RampKey::pool apart
+    uint32_t pool_used = 0; // stops
+    std::map<std::tuple<const void *, uint32_t, uint32_t, uint64_t>, std::unique_ptr<ImageKey>> image_keys;
+    // freed fragments whose memory composes already enqueued may still read: released once `done` has completed
+    struct FreedFragment { void *mem; size_t bytes; cudaEvent_t done; };
+    std::vector<FreedFragment> freed;
+    uint32_t next_image_key = 1;
+    uint64_t compose_seq = 0;
+    DevBuf compose_tmp;                  // compose's tables, staged through pinned[PIN_COMPOSE]
+    // bound instance transforms (vb_bind_instance_transforms) of the current scene: the caller's rows (nullptr: unbound), and
+    // the binding's tables in inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n), at
+    // o_xf] [the fragments' untransformed transforms, at o_src]. Every scene installation unbinds (set_scene).
+    // [the instances' draw prefix (n + 1), at o_draw]
+    struct Binding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+        size_t o_xf = 0, o_src = 0, o_draw = 0;
+    } bound;
+    DevBuf inst_tables;
+
+    // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
+    // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
+    // matches `base`, the last successful frame, in epoch, size, AA, base colour and device destination. The device keeps the
+    // base's snapshot (dmg_snap) and advances it itself, so base changes only when the host learns that a frame succeeded.
+    struct DamageFrame {
+        uint32_t mode = VB_DMG_OFF;
+        bool can_base = false; // one cell, no window, device destination: the frame can be the next one's base
+        uint32_t w = 0, h = 0, aa = 0, base_color = 0;
+        const void *dest = nullptr;
+        uint64_t epoch = 0;
+    };
+    struct Damage {
+        bool on = false;
+        uint64_t epoch = 0;
+        bool have_base = false, have_last = false;
+        bool rects = false;      // vb_add_damage since the last successful frame (dirty overrides then do not force a full frame)
+        bool force_full = false; // dirty overrides without rectangles: the frame and its re-runs are full
+        DamageFrame base, frame, last; // frame: the one prepared last; last: the last successful one
+        // vb_recompose that tracking follows: the next frame of epoch `epoch` (the recompose's installation) is incremental
+        // against `base` and runs k_recompose_damage on the tables in rcmp; consumed when a frame succeeds
+        struct Diff {
+            bool armed = false;
+            uint64_t epoch = 0;
+            uint32_t n_old = 0, n_new = 0, old_draws = 0, new_draws = 0;
+            size_t o_tables = 0;
+        } diff;
+    } dmg;
+    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
+    DevBuf rcmp; // vb_recompose: [the base frame's draw boxes] [the tables, at dmg.diff.o_tables] (VbFrameBufs::rcmp_tables)
+
+    // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
+    struct Exchange {
+        bool configured = false, enabled = false;
+        uint32_t rank = 0, world = 1, lines_cap = 0, n_paths = 0;
+        size_t half_bytes = 0;
+        DevBuf arena;
+        void *peer[8] = {};
+        uint32_t rows[9] = {};
+    } xc;
+};
+
+// Every device buffer the renderer owns, each once: what vb_renderer_free frees and vb_frame_stats::arena_bytes counts.
+template <class F> static void for_each_buf(vb_renderer *r, F f) {
+    DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
+                           &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids, &r->info_bin_data, &r->clip_inp,
+                           &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
+                           &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
+                           &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
+                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->rcmp};
+    for (DevBuf *b : all) f(*b);
+}
+
+#define CK(call)                                                                                  \
+    do {                                                                                          \
+        cudaError_t e_ = (call);                                                                  \
+        if (e_ != cudaSuccess) {                                                                  \
+            r->err = std::string(#call) + ": " + cudaGetErrorString(e_);                          \
+            return VB_E_CUDA;                                                                     \
+        }                                                                                         \
+    } while (0)
+
+// One entry per bump arena: the name vb_debug_limit_arena takes, the buffer, its element size and its VbBump counter.
+// The special cases are in arena_offset, arena_need, ensure_arena and the first guesses of prepare.
+using RendererBuf = DevBuf vb_renderer::*;
+using BumpCounter = uint32_t VbBump::*;
+struct ArenaDesc {
+    const char *name;
+    const char *download; // vb_debug_download's name of the buffer when it differs from the arena's
+    RendererBuf buf;
+    size_t elem_bytes;
+    BumpCounter counter;
+};
+
+// The rows fine paints: the window's tile rows, launched in `bands` row bands when the pixels also go to the host (up to 8,
+// for at least 64 rows), so that the read-back of band k overlaps the rasterisation of band k+1. A batch paints every tile
+// row of its tall frame in one launch: its cells are not rows of one image, and its pixel rows are n_cells * height.
+struct FineRows {
+    uint32_t ty0, ty1, bands; // tile rows [ty0, ty1) in `bands` launches
+    size_t y1;                // the last pixel row they cover (+1); rows from ty0 * 16
+    size_t dest_rows;         // pixel rows the destination holds, from row out_row0
+    // tile rows [*by0, *by1) of band b; false once the bands have run out of rows
+    bool band(uint32_t b, uint32_t *by0, uint32_t *by1) const {
+        const uint32_t n = (ty1 - ty0 + bands - 1u) / bands;
+        *by0 = ty0 + b * n;
+        *by1 = *by0 + n < ty1 ? *by0 + n : ty1;
+        return *by0 < *by1;
+    }
+};
+
+namespace vb_host __attribute__((visibility("hidden"))) {
+
+// Transforms of a scene: the stream from layout.transform_base to style_base (0 for a layout that does not fit the scene).
+inline uint32_t n_transforms(const VbLayout &L, size_t scene_words) {
+    if (L.style_base < L.transform_base || L.style_base > scene_words) return 0u;
+    return (L.style_base - L.transform_base) / 6u;
+}
+// A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
+// transforms, k_compose.cu; viewed transforms, k_view.cu), then slack.
+inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions) {
+    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words)) * 4u + 64u;
+}
+
+// vb_frame.cu
+int ensure(vb_renderer *r, DevBuf &b, size_t bytes);
+int stage_host(vb_renderer *r, PinnedStage &s, size_t bytes, uint8_t **host);
+int stage_copied(vb_renderer *r, PinnedStage &s);
+void hit_forget(vb_renderer *r);
+extern const ArenaDesc ARENAS[N_ARENAS];
+int arena_index(const char *name);
+uint64_t ptcl_static(const VbConfig &c);
+size_t arena_offset(const vb_renderer *r, int a);
+uint64_t arena_need(const vb_renderer *r, int a);
+int ensure_arena(vb_renderer *r, int a);
+uint32_t grow(uint32_t need);
+int drain_stream(vb_renderer *r);
+FineRows fine_rows(const VbConfig &c, const Dest &d);
+int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d);
+int launch(vb_renderer *r, int first, int last);
+Frame frame_of(const vb_renderer *r, const vb_params *p, const Dest &d);
+int finish(vb_renderer *r, const Frame &f);
+int settle(vb_renderer *r, const Frame &f, vb_frame_stats *stats);
+bool device_memory_of(vb_renderer *r, const void *p);
+int put_view(vb_renderer *r, const View &v);
+int view_of(const double *affine, View *v);
+
+// vb_upload.cu
+void drop_registrations(vb_renderer *r);
+void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
+               std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed);
+int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
+              uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h);
+int enqueue_blits(vb_renderer *r, std::vector<VbBlitRect> &rects, void *atlas, uint32_t atlas_w);
+int refresh_overrides(vb_renderer *r);
+int check_streams(vb_renderer *r, const vb_encoding_streams *e, const char *who);
+int image_source(vb_renderer *r, const char *who, const void *key, uint32_t w, uint32_t h, uint32_t x, uint32_t y,
+                 std::vector<VbBlitRect> &blits, std::vector<vb_renderer::SceneSlot::OverridePlace> &over, bool *overridden);
+
+// vb_damage.cu
+int damage_prepare(vb_renderer *r);
+void damage_succeeded(vb_renderer *r);
+
+} // namespace vb_host
+using namespace vb_host;

@@ -1,5 +1,5 @@
 // vb_resolve.h -- the decisions the library's three Resolver::resolve share, so that their output stays byte-identical: the host
-// resolve (vb_scene_resolve, vb_scene.cpp), the device resolve (vb_scene_upload_streams) and composition (vb_compose, vb_api.cu).
+// resolve (vb_scene_resolve, vb_scene.cpp), the device resolve (vb_scene_upload_streams) and composition (vb_compose, vb_compose.cu).
 // Internal to the library, and plain C++: vb_scene.cpp is built without the CUDA headers.
 #ifndef VB_RESOLVE_H
 #define VB_RESOLVE_H
@@ -19,7 +19,7 @@ static inline uint64_t vb_draw_info_sum(const uint32_t *draw_tags, size_t n) {
 // The packed scene's layout from the sizes of its streams (resolve.rs:107-154): the tag bytes and one PATH tag per open clip,
 // padded to 4 * PATH_REDUCE_WG bytes (resolve.rs:625, config.rs:237); path data; draw tags and one END_CLIP per open clip; draw
 // data; 6 words per transform; 2 per style. Sets *padded_tags (bytes) and *words (the whole scene). False when the scene, with
-// room behind it for a view's transforms, passes 32-bit word offsets. Layout: vb_layout, or vb_api.cu's VbLayout (the same record).
+// room behind it for a view's transforms, passes 32-bit word offsets. Layout: vb_layout, or the host files' VbLayout (the same record).
 template <class Layout>
 static inline bool vb_resolve_layout(uint64_t path_tags, uint64_t path_data, uint64_t draw_tags, uint64_t draw_data, uint64_t transforms,
                                      uint64_t styles, uint64_t open_clips, uint64_t paths, uint64_t clips, uint64_t info, Layout *L,

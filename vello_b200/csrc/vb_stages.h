@@ -1,6 +1,6 @@
-// vb_stages.h -- the stage launchers of k_*.cu and the records they share with the host code (vb_api.cu).
+// vb_stages.h -- the stage launchers of k_*.cu and the records they share with the host code (vb_renderer.h).
 //
-// Internal to the library. vb_api.cu and every k_*.cu that defines a launcher include it, so a definition that disagrees with
+// Internal to the library. The host files and every k_*.cu that defines a launcher include it, so a definition that disagrees with
 // its declaration here does not compile. Stage launchers take the frame's config, its device buffers (VbFrameBufs) and their
 // own per-call scalars, derive their grids themselves and return the number of kernels they launched.
 #ifndef VB_STAGES_H
@@ -16,7 +16,7 @@ struct FlJob;
 struct CmpXform; // an instance's transform (k_compose.cu, below)
 
 // The device buffers a frame's launches read and write: the current scene slot's inputs, every intermediate and arena, and
-// the look-back regions of the control block with their partition counts. prepare() (vb_api.cu) fills it once every buffer
+// the look-back regions of the control block with their partition counts. prepare() (vb_frame.cu) fills it once every buffer
 // has its size. It is part of the key of a captured frame (GraphKey), so it holds launch inputs only, and no padding.
 struct VbFrameBufs {
     // scene slot and the renderer's fixed tables
@@ -143,7 +143,7 @@ void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_
                               const RsPatch *patches, uint32_t n_patches, cudaStream_t st);
 void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st);
 
-// k_compose.cu: the six streams of a composition of resident fragments (vb_compose), staged by vb_api.cu
+// k_compose.cu: the six streams of a composition of resident fragments (vb_compose), staged by vb_compose.cu
 struct CmpXform { float m[6]; uint32_t on, pad; }; // an instance's transform (on == 0: appended without one)
 struct CmpArgs {
     uint32_t *scene;              // the packed scene being composed
@@ -158,7 +158,7 @@ struct CmpArgs {
 };
 uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
 // bound instance transforms: row_k * T of every transform T of the composed scene into the frame's bound region (prepare,
-// vb_api.cu), in flatten's stage before the view's transforms; nothing while unbound
+// vb_frame.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot

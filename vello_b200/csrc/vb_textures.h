@@ -1,4 +1,4 @@
-// vb_textures.h -- the texture registry of vb_api.cu, as the native scene front end (vb_scene.cpp) uses it.
+// vb_textures.h -- the texture registry of vb_upload.cu, as the native scene front end (vb_scene.cpp) uses it.
 // Internal to the library, and plain C++: vb_scene.cpp is built without the CUDA headers.
 #ifndef VB_TEXTURES_H
 #define VB_TEXTURES_H

@@ -1,0 +1,423 @@
+// vb_upload.cu -- scenes into a renderer: uploads of packed scenes, the device resolve (vb_scene_upload_streams), images from
+// device memory (overrides and registered textures, copied into the atlas by k_atlas_blit) and batches of cells.
+#include <cuda_runtime.h>
+#include <string.h>
+#include <sys/mman.h>
+
+#include <algorithm>
+#include <mutex>
+
+#include "vb_renderer.h"
+#include "vb_resolve.h"
+#include "vb_textures.h"
+
+// Keys of registered textures (vb_register_texture). Each is a fresh address inside one reserved, inaccessible (PROT_NONE)
+// range of the process's address space, so no host buffer can have it, even after the texture is unregistered: the host
+// resolve recognises such a key by its address alone and never reads through it (vb_texture_key). The range is never
+// unmapped and a key is never handed out twice. `owner` is the renderer that registered the key.
+static std::mutex g_tex_mutex;
+static std::unordered_map<const void *, vb_renderer *> g_tex_owner;
+static uint8_t *g_tex_base = nullptr;
+static size_t g_tex_next = 0;
+static const size_t TEX_KEY_STRIDE = 16, TEX_RANGE_BYTES = (size_t)1 << 30;
+
+extern "C" int vb_texture_key(const void *key) { // for vb_scene.cpp's host resolve
+    const uint8_t *p = (const uint8_t *)key, *base = __atomic_load_n(&g_tex_base, __ATOMIC_ACQUIRE);
+    return base != nullptr && p >= base && p < base + TEX_RANGE_BYTES;
+}
+static const void *new_texture_key(vb_renderer *owner) {
+    std::lock_guard<std::mutex> lock(g_tex_mutex);
+    if (!g_tex_base) {
+        void *m = mmap(nullptr, TEX_RANGE_BYTES, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
+        if (m == MAP_FAILED) return nullptr;
+        __atomic_store_n(&g_tex_base, (uint8_t *)m, __ATOMIC_RELEASE);
+    }
+    if (g_tex_next + TEX_KEY_STRIDE > TEX_RANGE_BYTES) return nullptr;
+    const void *key = g_tex_base + g_tex_next;
+    g_tex_next += TEX_KEY_STRIDE;
+    g_tex_owner[key] = owner;
+    return key;
+}
+void vb_host::drop_registrations(vb_renderer *r) {
+    std::lock_guard<std::mutex> lock(g_tex_mutex);
+    for (auto it = g_tex_owner.begin(); it != g_tex_owner.end();) it = it->second == r ? g_tex_owner.erase(it) : std::next(it);
+}
+
+// Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms are bound to it.
+void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
+                      std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
+    vb_renderer::SceneSlot &s = *r->cur;
+    s.layout = L;
+    s.scene_words = scene_words;
+    s.n_ramps = n_ramps;
+    s.atlas_w = atlas_w;
+    s.atlas_h = atlas_h;
+    s.overridden = std::move(overridden);
+    s.composed = composed;
+    s.inst_frag.clear(); // vb_compose fills them afterwards
+    s.inst_xf.clear();
+    s.inst_draw.clear();
+    s.inst_img.clear();
+    s.img_place.clear();
+    s.have_scene = true;
+    r->cells.clear();
+    r->bound = vb_renderer::Binding{};
+    r->dmg.epoch++;
+    hit_forget(r);
+}
+
+int vb_host::upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
+                     uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h) {
+    if (!r || !layout || (scene_len && !scene) || (scene_len & 3)) return VB_E_INVALID;
+    if (ramp_h && ramp_w != 512) return VB_E_INVALID;
+    CK(cudaSetDevice(r->device));
+    VbLayout L;
+    memcpy(&L, layout, sizeof L);
+    if (!atlas) atlas_w = atlas_h = 0;
+    int rc;
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, scene_len / 4, r->view.on)))) return rc;
+    if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
+    if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
+    if (ramp_h) CK(cudaMemcpyAsync(r->cur->ramps.p, ramps, (size_t)ramp_h * 512 * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
+    if (atlas_w && atlas_h) CK(cudaMemcpyAsync(r->cur->atlas.p, atlas, (size_t)atlas_w * atlas_h * 4, cudaMemcpyHostToDevice, st));
+    set_scene(r, L, scene_len / 4, ramp_h, atlas_w, atlas_h, {}, false); // a caller-packed atlas: overrides do not apply
+    return VB_OK;
+}
+
+extern "C" int vb_scene_upload(vb_renderer *r, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
+                               uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h) {
+    if (!r) return VB_E_INVALID;
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    return upload_on(r, r->stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h);
+}
+
+// ---- images from device memory: Renderer::override_image / register_texture (vello/src/lib.rs:536-603) ----------------------
+// An override names an image by its key (the `pixels` pointer of its vb_image / vb_image_patch). The device resolve
+// (vb_scene_upload_streams) copies such an image into its atlas slot from the override's device memory with k_atlas_blit and
+// records the slot; marking the image dirty later queues the same copy in front of the next frame (refresh_overrides).
+
+// A device image must be memory of this renderer's device (or managed memory), with 4-byte aligned rows of at least 4 * w bytes.
+static int check_device_pixels(vb_renderer *r, const void *px, uint32_t w, uint32_t h, size_t pitch) {
+    auto bad = [&](const char *why) {
+        r->err = std::string("device image: ") + why;
+        return VB_E_INVALID;
+    };
+    if (!w || !h) return bad("a dimension is 0");
+    if (((uintptr_t)px & 3u) || (pitch & 3u)) return bad("the pointer and the row pitch must be multiples of 4 bytes");
+    if (pitch < (size_t)w * 4u) return bad("the row pitch is less than 4 * width");
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, px) != cudaSuccess) {
+        cudaGetLastError();
+        return bad("not a CUDA pointer");
+    }
+    if (a.type == cudaMemoryTypeManaged) return VB_OK;
+    if (a.type != cudaMemoryTypeDevice || a.device != r->device) return bad("not device memory of the renderer's device");
+    return VB_OK;
+}
+
+// Copy `rects` into an atlas of atlas_w texels per row with one k_atlas_blit on the renderer's stream. The rectangles reach
+// the device through a pinned staging buffer, which is rewritten only once the previous copy out of it has run.
+int vb_host::enqueue_blits(vb_renderer *r, std::vector<VbBlitRect> &rects, void *atlas, uint32_t atlas_w) {
+    if (rects.empty()) return VB_OK;
+    uint64_t units = 0;
+    for (VbBlitRect &b : rects) {
+        b.spr = vb_atlas_blit_units_per_row(b.w);
+        b.unit0 = units;
+        units += (uint64_t)b.h * b.spr;
+    }
+    const size_t bytes = rects.size() * sizeof(VbBlitRect);
+    PinnedStage &s = r->pinned[PIN_BLITS];
+    uint8_t *h;
+    int rc = stage_host(r, s, bytes, &h);
+    if (rc) return rc;
+    memcpy(h, rects.data(), bytes);
+    if ((rc = ensure(r, r->blit_rects, bytes))) return rc;
+    CK(cudaMemcpyAsync(r->blit_rects.p, h, bytes, cudaMemcpyHostToDevice, r->stream));
+    if ((rc = stage_copied(r, s))) return rc;
+    vb_launch_atlas_blit((const VbBlitRect *)r->blit_rects.p, (uint32_t)rects.size(), units, (uint8_t *)atlas, atlas_w, r->stream);
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+
+// Before a frame: copy the dirty overridden images of the current scene slot into their atlas places. The copy runs ahead of
+// every kernel of the frame (and outside any captured graph), so a frame that draws its own destination reads the old pixels.
+// The atlas does not move, so a captured frame stays valid. Nothing dirty: nothing is enqueued.
+int vb_host::refresh_overrides(vb_renderer *r) {
+    std::vector<VbBlitRect> rects;
+    for (const auto &o : r->cur->overridden)
+        if (o.dirty) rects.push_back(VbBlitRect{o.src, o.pitch, 0, o.w, o.h, o.x, o.y, 0, 0});
+    if (rects.empty()) return VB_OK;
+    const int rc = enqueue_blits(r, rects, r->cur->atlas.p, r->cur->atlas_w);
+    if (rc) return rc;
+    for (auto &o : r->cur->overridden) o.dirty = false;
+    return VB_OK;
+}
+
+extern "C" int vb_override_image(vb_renderer *r, const void *key, uint32_t width, uint32_t height, const void *device_pixels,
+                                 size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    if (!key) {
+        r->err = "vb_override_image: NULL key";
+        return VB_E_INVALID;
+    }
+    if (device_pixels) {
+        CK(cudaSetDevice(r->device));
+        const int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
+        if (rc) return rc;
+        r->overrides[key] = vb_renderer::Override{(const uint8_t *)device_pixels, row_pitch_bytes, width, height};
+    } else {
+        r->overrides.erase(key);
+    }
+    // recorded atlas places: a new source of the same size is copied before the next frame; a removed override (or one of
+    // another size) keeps the pixels copied last and takes effect at the next device resolve
+    for (auto &s : r->slot) {
+        auto &v = s.overridden;
+        v.erase(std::remove_if(v.begin(), v.end(),
+                               [&](const auto &o) { return o.key == key && (!device_pixels || o.w != width || o.h != height); }),
+                v.end());
+        for (auto &o : v)
+            if (o.key == key) {
+                o.src = (const uint8_t *)device_pixels;
+                o.pitch = row_pitch_bytes;
+                o.dirty = true;
+            }
+    }
+    return VB_OK;
+}
+
+extern "C" int vb_mark_override_image_dirty(vb_renderer *r, const void *key) {
+    if (!r) return VB_E_INVALID;
+    if (!r->overrides.count(key)) {
+        r->err = "vb_mark_override_image_dirty: no override for this key";
+        return VB_E_INVALID;
+    }
+    for (auto &s : r->slot)
+        for (auto &o : s.overridden)
+            if (o.key == key) o.dirty = true;
+    return VB_OK;
+}
+
+// Renderer::register_texture / unregister_texture; vb_register_texture / vb_unregister_texture (vb_scene.cpp, which owns vb_image)
+// wrap these two.
+extern "C" int vb_texture_register(vb_renderer *r, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes,
+                                   const void **key_out) {
+    if (!r || !key_out) return VB_E_INVALID;
+    if (!device_pixels) {
+        r->err = "vb_register_texture: NULL pixels";
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
+    if (rc) return rc;
+    const void *key = new_texture_key(r);
+    if (!key) {
+        r->err = "vb_register_texture: no texture key left";
+        return VB_E_INVALID;
+    }
+    if ((rc = vb_override_image(r, key, width, height, device_pixels, row_pitch_bytes))) return rc;
+    *key_out = key;
+    return VB_OK;
+}
+
+extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
+    if (!r) return VB_E_INVALID;
+    {
+        std::lock_guard<std::mutex> lock(g_tex_mutex);
+        auto it = vb_texture_key(key) ? g_tex_owner.find(key) : g_tex_owner.end();
+        if (it == g_tex_owner.end() || it->second != r) {
+            r->err = "vb_unregister_texture: not a texture registered on this renderer";
+            return VB_E_INVALID;
+        }
+        g_tex_owner.erase(it);
+    }
+    return vb_override_image(r, key, 0, 0, nullptr, 0);
+}
+
+// ---- batches: many scenes of one size in one pass (vb_scene_batch builds the scene) ---------------------------------------
+// The offsets split the uploaded scene's draw objects into cells. Validated here against the uploaded draw tags (one download):
+// a cell whose clips do not balance would pair a BEGIN_CLIP of one cell with an END_CLIP of the next. What depends on the
+// frame size (arena indexing) and on the call (windows) is checked when a frame is prepared.
+extern "C" int vb_set_cells(vb_renderer *r, const uint32_t *draw_offsets, uint32_t n_cells) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_set_cells: " + why;
+        return VB_E_INVALID;
+    };
+    if (!draw_offsets || n_cells == 0u) return bad("no offsets");
+    if (!r->cur->have_scene) return VB_E_NO_SCENE;
+    if (r->xc.enabled || r->grouped) return bad("a batch cannot be combined with vb_group or the exchange");
+    int rc = drain_stream(r);
+    if (rc) return rc;
+    CK(cudaSetDevice(r->device));
+    const VbLayout &L = r->cur->layout;
+    const uint32_t n_draw = L.n_draw_objects;
+    if (draw_offsets[0] != 0u || draw_offsets[n_cells] != n_draw) return bad("offsets must start at 0 and end at the scene's draw-object count");
+    for (uint32_t c = 0; c < n_cells; c++)
+        if (draw_offsets[c + 1] < draw_offsets[c]) return bad("offsets must not decrease");
+    r->dmg.epoch++;
+    if (n_cells == 1u) { // the whole scene: no batch
+        r->cells.clear();
+        hit_forget(r);
+        return VB_OK;
+    }
+    std::vector<uint32_t> tags(n_draw);
+    if (n_draw) {
+        CK(cudaMemcpyAsync(tags.data(), (const uint32_t *)r->cur->scene.p + L.draw_tag_base, (size_t)n_draw * 4, cudaMemcpyDeviceToHost, r->stream));
+        CK(cudaStreamSynchronize(r->stream));
+    }
+    for (uint32_t c = 0; c < n_cells; c++) {
+        int64_t depth = 0;
+        for (uint32_t i = draw_offsets[c]; i < draw_offsets[c + 1] && depth >= 0; i++)
+            depth += tags[i] == VB_DRAWTAG_BEGIN_CLIP ? 1 : tags[i] == VB_DRAWTAG_END_CLIP ? -1 : 0;
+        if (depth != 0) return bad("the clips of cell " + std::to_string(c) + " do not balance");
+    }
+    hit_forget(r); // cell_draw, which the answers read, is rewritten below
+    if ((rc = ensure(r, r->cell_draw, ((size_t)n_cells + 1u) * 4u))) return rc;
+    r->cells.assign(draw_offsets, draw_offsets + n_cells + 1u);
+    // in stream order: a frame still running reads the previous offsets
+    CK(cudaMemcpyAsync(r->cell_draw.p, r->cells.data(), r->cells.size() * 4u, cudaMemcpyHostToDevice, r->stream));
+    return VB_OK;
+}
+
+// ---- Resolver::resolve on the device (resolve.rs:183-399): see include/vello_b200.h and k_resolve.cu ---------------------------
+// Streams a resolve can read: a pointer for every stream with elements, stops for every ramp patch, every patch in the draw data.
+int vb_host::check_streams(vb_renderer *r, const vb_encoding_streams *e, const char *who) {
+    auto bad = [&](const char *why) {
+        r->err = std::string(who) + ": " + why;
+        return VB_E_INVALID;
+    };
+    if ((e->n_path_tags && !e->path_tags) || (e->n_path_data && !e->path_data) || (e->n_draw_tags && !e->draw_tags) ||
+        (e->n_draw_data && !e->draw_data) || (e->n_transforms && !e->transforms) || (e->n_styles && !e->styles) ||
+        (e->n_ramp_patches && !e->ramp_patches) || (e->n_image_patches && !e->image_patches))
+        return bad("a stream with elements and no pointer");
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return bad("a ramp patch without stops or outside the draw data");
+    }
+    for (uint32_t i = 0; i < e->n_image_patches; i++)
+        if (e->image_patches[i].draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+    return VB_OK;
+}
+
+// The pixels of an image placed at (x, y): with an override on this renderer, a blit from its memory, kept in `over` for
+// refresh_overrides (*overridden). Otherwise the caller's to copy; a registered texture has pixels only as an override's.
+int vb_host::image_source(vb_renderer *r, const char *who, const void *key, uint32_t w, uint32_t h, uint32_t x, uint32_t y,
+                        std::vector<VbBlitRect> &blits, std::vector<vb_renderer::SceneSlot::OverridePlace> &over, bool *overridden) {
+    const auto ov = key ? r->overrides.find(key) : r->overrides.end();
+    *overridden = ov != r->overrides.end();
+    if (*overridden) {
+        const vb_renderer::Override &o = ov->second;
+        if (o.w != w || o.h != h) {
+            r->err = std::string(who) + ": an override's size differs from its image's (" + std::to_string(o.w) + "x" + std::to_string(o.h) + " vs " +
+                     std::to_string(w) + "x" + std::to_string(h) + ")";
+            return VB_E_INVALID;
+        }
+        blits.push_back(VbBlitRect{o.src, o.pitch, 0, w, h, x, y, 0, 0});
+        over.push_back({key, o.src, o.pitch, w, h, x, y, false});
+    } else if (vb_texture_key(key)) {
+        r->err = std::string(who) + ": a registered texture has no override on this renderer";
+        return VB_E_INVALID;
+    }
+    return VB_OK;
+}
+
+extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams *e, vb_layout *layout_out) {
+    if (!r || !e) return VB_E_INVALID;
+    int rc = check_streams(r, e, "vb_scene_upload_streams");
+    if (rc) return rc;
+    VbLayout L;
+    uint32_t padded;
+    size_t total_words;
+    if (!vb_resolve_layout(e->n_path_tags, e->n_path_data, e->n_draw_tags, e->n_draw_data, e->n_transforms, e->n_styles, e->n_open_clips, e->n_paths,
+                           e->n_clips, vb_draw_info_sum(e->draw_tags, e->n_draw_tags), &L, &padded, &total_words)) {
+        r->err = "vb_scene_upload_streams: the scene exceeds 32-bit word offsets";
+        return VB_E_INVALID;
+    }
+    if ((rc = drain_stream(r))) return rc;
+    CK(cudaSetDevice(r->device));
+    cudaStream_t st = r->stream;
+    std::vector<RsPatch> patches;
+    std::vector<RsRamp> ramps;
+    std::vector<vb_ramp_stop> stops;
+    // late-bound gradient ramps, de-duplicated by (stops, interpolation space) as the host resolve does
+    std::vector<const vb_ramp_patch *> ramp_of;
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(p.stops, p.n_stops, p.premul_interp != 0u)];
+        uint32_t rid = (uint32_t)ramp_of.size();
+        for (uint32_t k : same_hash) {
+            const vb_ramp_patch &q = *ramp_of[k];
+            if (vb_same_ramp(q.stops, q.n_stops, q.premul_interp != 0u, p.stops, p.n_stops, p.premul_interp != 0u)) { rid = k; break; }
+        }
+        if (rid == ramp_of.size()) {
+            same_hash.push_back(rid);
+            ramp_of.push_back(&p);
+            ramps.push_back(RsRamp{(uint32_t)stops.size(), p.n_stops, p.premul_interp ? 1u : 0u, 0u});
+            stops.insert(stops.end(), p.stops, p.stops + p.n_stops);
+        }
+        patches.push_back(RsPatch{L.draw_data_base + p.draw_data_offset, (rid << 2) | p.extend});
+    }
+    // late-bound images: each distinct (pixels, width, height) placed once in the atlas, filled from an override on this
+    // renderer (one k_atlas_blit) or from the host
+    struct Placed { const uint8_t *key; uint32_t w, h, x, y; bool from_device; };
+    std::vector<Placed> placed;
+    std::vector<VbBlitRect> blits;
+    std::vector<vb_renderer::SceneSlot::OverridePlace> over;
+    VbShelfPacker shelf;
+    for (uint32_t i = 0; i < e->n_image_patches; i++) {
+        const vb_image_patch &im = e->image_patches[i];
+        const Placed *hit = nullptr;
+        for (const Placed &q : placed)
+            if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
+        if (!hit) {
+            Placed q{im.pixels, im.width, im.height, 0, 0, false};
+            shelf.place(q.w, q.h, &q.x, &q.y);
+            if ((rc = image_source(r, "device resolve", q.key, q.w, q.h, q.x, q.y, blits, over, &q.from_device))) return rc;
+            placed.push_back(q);
+            hit = &placed.back();
+        }
+        patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (hit->x << 16) | hit->y});
+    }
+    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
+
+    // the six streams go straight to their places in the packed buffer
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, total_words, r->view.on)))) return rc;
+    char *base = (char *)r->cur->scene.p;
+    if (e->n_path_tags) CK(cudaMemcpyAsync(base, e->path_tags, e->n_path_tags, cudaMemcpyHostToDevice, st));
+    if (e->n_path_data) CK(cudaMemcpyAsync(base + (size_t)L.path_data_base * 4, e->path_data, (size_t)e->n_path_data * 4, cudaMemcpyHostToDevice, st));
+    if (e->n_draw_tags) CK(cudaMemcpyAsync(base + (size_t)L.draw_tag_base * 4, e->draw_tags, (size_t)e->n_draw_tags * 4, cudaMemcpyHostToDevice, st));
+    if (e->n_draw_data) CK(cudaMemcpyAsync(base + (size_t)L.draw_data_base * 4, e->draw_data, (size_t)e->n_draw_data * 4, cudaMemcpyHostToDevice, st));
+    if (e->n_transforms) CK(cudaMemcpyAsync(base + (size_t)L.transform_base * 4, e->transforms, (size_t)e->n_transforms * 24, cudaMemcpyHostToDevice, st));
+    if (e->n_styles) CK(cudaMemcpyAsync(base + (size_t)L.style_base * 4, e->styles, (size_t)e->n_styles * 8, cudaMemcpyHostToDevice, st));
+    // patches, ramp descriptors and stops in one staging buffer
+    static_assert(sizeof(RsStop) == sizeof(vb_ramp_stop), "the stops are staged as the caller gave them");
+    const size_t pb = patches.size() * sizeof(RsPatch), rb = ramps.size() * sizeof(RsRamp), sb = stops.size() * sizeof(vb_ramp_stop);
+    const size_t o_r = (pb + 15) & ~(size_t)15, o_s = (o_r + rb + 15) & ~(size_t)15;
+    if ((rc = ensure(r, r->resolve_tmp, o_s + sb + 16))) return rc;
+    char *tmp = (char *)r->resolve_tmp.p;
+    if (pb) CK(cudaMemcpyAsync(tmp, patches.data(), pb, cudaMemcpyHostToDevice, st));
+    if (rb) CK(cudaMemcpyAsync(tmp + o_r, ramps.data(), rb, cudaMemcpyHostToDevice, st));
+    if (sb) CK(cudaMemcpyAsync(tmp + o_s, stops.data(), sb, cudaMemcpyHostToDevice, st));
+    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags,
+                             (const RsPatch *)tmp, (uint32_t)patches.size(), st);
+    if ((rc = ensure(r, r->cur->ramps, ramps.size() * 512 * 4))) return rc;
+    vb_launch_make_ramps((const RsRamp *)(tmp + o_r), (const RsStop *)(tmp + o_s), (uint32_t)ramps.size(), (uint32_t *)r->cur->ramps.p, st);
+    if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
+    CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
+    for (const Placed &q : placed) {
+        if (q.key && q.w && q.h && !q.from_device)
+            CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
+                                 cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = enqueue_blits(r, blits, r->cur->atlas.p, atlas_w))) return rc;
+    CK(cudaGetLastError());
+    // the host vectors above are read by the asynchronous copies: they must outlive them
+    CK(cudaStreamSynchronize(st));
+    set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), false);
+    if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
+    return VB_OK;
+}
