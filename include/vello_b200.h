@@ -427,7 +427,7 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  * damaged 16 x 16 tiles and writes no other pixel; the damaged tiles are byte-identical to a full frame. Off (the default)
  * changes nothing: not the pixels, the launches or the captured graphs.
  *  - Incremental frames. A frame is incremental when tracking is on; the scene installation is the same (no upload form,
- *    vb_compose, vb_render or vb_render_begin since; vb_recompose, see there, can keep the frame after it incremental); width, height, AA, base colour and the device destination pointer are
+ *    vb_compose, vb_render or vb_render_begin since; vb_recompose, and uploads with vb_set_upload_diff on, see there, can keep the frame after them incremental); width, height, AA, base colour and the device destination pointer are
  *    those of the last successful frame (NULL counts as the renderer's own target); the view, the binding and vb_set_cells are
  *    unchanged; it has one cell and no bin_row / tile_row window; and the renderer is not in a vb_group and has no exchange.
  *    Every other frame is full: it reports every tile as damaged and becomes the base of the next one (a batch or a windowed
@@ -444,7 +444,7 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
  *    tiles, added to the next frame's damage in stream order (like vb_set_view's coefficients) on top of the automatic
  *    damage. This is the explicit invalidate: use it for a scene re-uploaded with local edits (which is a full frame anyway,
- *    unless the edit is written into the resident scene in place), dirty image overrides, or a destination the caller
+ *    unless vb_set_upload_diff is on or the edit is written into the resident scene in place), dirty image overrides, or a destination the caller
  *    changed. A frame after vb_mark_override_image_dirty / vb_override_image is full unless rectangles were added since the
  *    last successful frame. No effect while tracking is off or before the first tracked frame. VB_E_INVALID: NULL rects
  *    with n > 0; a frame enqueued and not finished (vb_render_enqueue until vb_frame_finish, vb_render_begin until
@@ -458,6 +458,34 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  *    incremental frame equal those on a full one. vb_debug_fine_traffic counts the damaged tiles only, and after an
  *    incremental frame vb_debug_download("seg_holes") also counts the segment slots of the tiles coarse skipped. */
 int vb_set_damage_tracking(vb_renderer *, int on);
+/* vb_set_upload_diff: diff re-uploaded scenes against the scene the base frame rendered (an addition; off by default, and off
+ * changes nothing). An application that re-encodes its whole scene every frame (vb_render, vb_scene_upload_streams) then gets
+ * incremental frames without naming the damage itself. While it and damage tracking are on, a scene installed by
+ * vb_scene_upload, vb_scene_upload_streams, vb_scene_upload_device, or the upload inside vb_render / vb_render_scene is compared
+ * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
+ * all of these hold:
+ *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound, one cell, no
+ *    scene installation, binding, view, cell split or tracking switch since, and hit tests answering from it (no failed frame,
+ *    vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
+ *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
+ *    frame full), and no vb_run_stages before the next one;
+ *  - the next frame meets every condition of an incremental frame (size, AA, base colour, device destination, one cell, no
+ *    window).
+ * Otherwise the next frame is full, and still correct. vb_compose stays full, vb_recompose keeps its own diff, streamed frames
+ * (vb_render_begin) and host destinations stay full; vb_add_damage rectangles and dirty overrides apply as usual.
+ * The damage: draw objects are equal when their draw tag and draw data, their path's tag bytes (from the byte after the
+ * previous path's end tag through its own) and path data, and the transforms and styles those tags read are the same words,
+ * a gradient's ramp row holds the same bytes (a ramp that moved to another row is equal), and an image sits at the same atlas
+ * place with the same texels. With m the smaller draw-object count, p the common prefix and s the common suffix (at most
+ * m - p), new draw object j pairs with old j below p, with old j + n_old - n_new from n_new - s on, with old j in between when
+ * the two are equal, and with nothing otherwise: an order-preserving matching of equal draw objects. The damaged tiles are
+ * those of the clipped boxes of unmatched draw objects (old boxes in the base frame, new ones in this frame) and both boxes of
+ * a matched pair whose boxes differ. The upload keeps the base's scene, ramps and atlas (a spare set of buffers it writes
+ * instead, swapped without a copy; counted in arena_bytes and freed when the switch is turned off), copies the base's draw
+ * boxes and records its draw objects on the device; the frame adds three kernels before vb_recompose's damage kernel. Frames
+ * without such an upload launch nothing new. VB_E_INVALID (switching on) for a renderer of a vb_group or with the exchange
+ * configured. */
+int vb_set_upload_diff(vb_renderer *, int on);
 int vb_add_damage(vb_renderer *, const uint32_t *rects, uint32_t n);
 int vb_last_damage(vb_renderer *, uint8_t *tile_mask, size_t cap, uint32_t *n_damaged);
 

@@ -92,6 +92,9 @@ extern "C" {
     // vb_compose, after which the next tracked frame repaints only the instances added, removed or changed since the composition
     // the last frame rendered (matched in order by fragment and transform); vb_compose itself makes the next frame full
     pub fn vb_recompose(r: *mut VbRenderer, instances: *const VbInstance, n: u32, layout_out: *mut Layout, draw_offsets: *mut u32) -> c_int;
+    // with tracking on: each uploaded scene (vb_render, vb_scene_upload, vb_scene_upload_streams) is compared on the device with
+    // the one the last frame rendered, and the next frame into a device destination repaints only the draw objects that changed
+    pub fn vb_set_upload_diff(r: *mut VbRenderer, on: c_int) -> c_int;
     // one frame on several GPUs of one box
     pub fn vb_group_new(devices: *const i32, n: u32, opt: *const VbOptions, out: *mut *mut VbGroup) -> c_int;
     pub fn vb_group_free(g: *mut VbGroup);

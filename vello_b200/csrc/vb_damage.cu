@@ -30,8 +30,9 @@ int vb_host::damage_prepare(vb_renderer *r) {
         if (o.dirty && !D.rects) D.force_full = true;
     const vb_renderer::DamageFrame &B = D.base;
     const bool diff = D.diff.armed && D.diff.epoch == f.epoch; // the scene is a recompose of the base's (vb_recompose)
-    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff) && B.w == f.w && B.h == f.h &&
-                             B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
+    const bool udiff = D.udiff.armed && D.udiff.epoch == f.epoch; // an upload diffed against the base's scene (vb_set_upload_diff)
+    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff || udiff) && B.w == f.w &&
+                             B.h == f.h && B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
     f.mode = incremental ? VB_DMG_INCREMENTAL : VB_DMG_FULL;
     // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
     // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
@@ -63,6 +64,14 @@ int vb_host::damage_prepare(vb_renderer *r) {
         b.rcmp_old_draws = D.diff.old_draws;
         b.rcmp_new_draws = D.diff.new_draws;
     }
+    if (incremental && udiff) { // one draw object per "instance" of k_recompose_damage's tables, which k_upload_diff.cu builds
+        const VbUdLayout U = vb_udiff_layout(D.udiff.n_old, D.udiff.n_new);
+        b.udiff = (VbUdiff *)r->udiff.p;
+        b.rcmp_old_boxes = (const VbBbox4 *)((const char *)r->udiff.p + U.boxes);
+        b.rcmp_tables = (const uint32_t *)((const char *)r->udiff.p + U.tables);
+        b.rcmp_n_old = b.rcmp_old_draws = D.udiff.n_old;
+        b.rcmp_n_new = b.rcmp_new_draws = D.udiff.n_new;
+    }
     D.frame = f;
     return VB_OK;
 }
@@ -76,6 +85,7 @@ void vb_host::damage_succeeded(vb_renderer *r) {
     D.rects = false;
     D.force_full = false;
     D.diff.armed = false;
+    D.udiff.armed = false;
 }
 
 extern "C" int vb_set_damage_tracking(vb_renderer *r, int on) {

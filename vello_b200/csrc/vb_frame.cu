@@ -606,6 +606,9 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_COARSE:
             // damage tracking: the frame's damaged tiles, from binning's draw boxes, before coarse reads them
             launches += vb_launch_damage(c, b, st);
+            // the first frame after an upload that tracking follows: which draw objects the upload changed, as the tables
+            // that k_recompose_damage reads
+            launches += vb_launch_upload_diff(c, b, st);
             launches += vb_launch_recompose_damage(c, b, st); // the first frame after vb_recompose: what the recompose changed
             // coarse is enqueued first, so that its CTAs (one per bin quadrant, all resident at once) are placed before
             // path_tiling's grid fills the rest of the GPU
@@ -977,7 +980,7 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
     const uint32_t slot = (uint32_t)(k & 1u), q = (uint32_t)(k % 3u), q1 = (uint32_t)((k + 2u) % 3u), q2 = (uint32_t)((k + 1u) % 3u);
     // frame k-2 (same scene slot, same device target) was checked by the previous call; frame k-3 (ring entry q) is complete
     r->cur = &r->slot[slot];
-    int rc = upload_on(r, r->upload_stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h);
+    int rc = upload_on(r, r->upload_stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h, false);
     if (rc) return rc;
     CK(cudaEventRecord(r->upload_done[slot], r->upload_stream));
     CK(cudaStreamWaitEvent(r->stream, r->upload_done[slot], 0));
@@ -1029,6 +1032,7 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
     hit_forget(r);
     r->dmg.diff.armed = false; // the stages may write the destination: the frame after them is full
+    r->dmg.udiff.armed = false;
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;

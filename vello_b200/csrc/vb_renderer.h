@@ -299,9 +299,23 @@ struct vb_renderer {
             uint32_t n_old = 0, n_new = 0, old_draws = 0, new_draws = 0;
             size_t o_tables = 0;
         } diff;
+        // an upload that tracking follows (vb_set_upload_diff): `pending` from upload_diff_begin until the upload installs its
+        // scene (set_scene), then `armed` for the next frame of epoch `epoch`, which is incremental against `base` and runs
+        // k_upload_diff.cu on `udiff`; consumed when a frame succeeds
+        struct UploadDiff {
+            bool pending = false, armed = false;
+            uint64_t epoch = 0;
+            uint32_t n_old = 0, n_new = 0;
+        } udiff;
     } dmg;
     DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
     DevBuf rcmp; // vb_recompose: [the base frame's draw boxes] [the tables, at dmg.diff.o_tables] (VbFrameBufs::rcmp_tables)
+    // upload diff (vb_set_upload_diff): the switch; the spare scene, ramps and atlas buffers an upload that tracking follows
+    // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set; and the diff's buffer
+    // (VbUdiff and vb_udiff_layout), whose head is written from ud_head
+    bool upload_diff = false;
+    DevBuf spare_scene, spare_ramps, spare_atlas, udiff;
+    VbUdiff ud_head{};
 
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
     struct Exchange {
@@ -322,7 +336,8 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
                            &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->rcmp};
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->rcmp, &r->spare_scene, &r->spare_ramps,
+                           &r->spare_atlas, &r->udiff};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -403,8 +418,9 @@ int view_of(const double *affine, View *v);
 void drop_registrations(vb_renderer *r);
 void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed);
+// diff: the upload may be diffed against the base frame's scene (vb_set_upload_diff); not for streamed frames
 int upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
-              uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h);
+              uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h, bool diff);
 int enqueue_blits(vb_renderer *r, std::vector<VbBlitRect> &rects, void *atlas, uint32_t atlas_w);
 int refresh_overrides(vb_renderer *r);
 int check_streams(vb_renderer *r, const vb_encoding_streams *e, const char *who);

@@ -14,6 +14,7 @@
 struct FlLit; // flatten's scratch records (k_flatten.cu)
 struct FlJob;
 struct CmpXform; // an instance's transform (k_compose.cu, below)
+struct VbUdiff;  // the upload diff's state (k_upload_diff.cu, below)
 
 // The device buffers a frame's launches read and write: the current scene slot's inputs, every intermediate and arena, and
 // the look-back regions of the control block with their partition counts. prepare() (vb_frame.cu) fills it once every buffer
@@ -65,6 +66,10 @@ struct VbFrameBufs {
     // prefix (rcmp_n_new + 1)] [new instance -> old instance, or VB_RCMP_NONE (rcmp_n_new)] [old instance unmatched (rcmp_n_old)]
     const VbBbox4 *rcmp_old_boxes;
     const uint32_t *rcmp_tables;
+    // upload diff (vb_set_upload_diff; k_upload_diff.cu), set only for the first frame after an upload that tracking follows,
+    // null otherwise: the diff's buffer (VbUdiff, then vb_udiff_layout). The rcmp_* fields then point into it and describe one
+    // draw object per "instance", so that k_recompose_damage computes the damage.
+    VbUdiff *udiff;
     // control block: [VbBump, header words (vb_types.h)] [look-back states], zeroed at the start of every frame
     uint32_t *ctl;
     size_t ctl_words;
@@ -176,6 +181,50 @@ size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw);
 // are null
 #define VB_RCMP_NONE 0xffffffffu
 uint32_t vb_launch_recompose_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
+// k_upload_diff.cu: the damage of the first frame after an upload that tracking follows (vb_set_upload_diff). The upload keeps
+// the base frame's scene (the renderer's spare buffers), copies its draw boxes and runs vb_launch_upload_records on its
+// intermediates; the frame runs vb_launch_upload_diff in coarse's stage, between vb_launch_damage and
+// vb_launch_recompose_damage, which then ORs the damage of the tables it built.
+// One draw object's inputs, relative to its scene's streams: path tag bytes [tag0, tag1), path data words [pd0, pd1),
+// transforms [t0, t1), style words [s0, s1), its draw tag and its draw-data offset in words.
+struct VbUdRec { uint32_t tag0, tag1, pd0, pd1, t0, t1, s0, s1, dtag, dd; };
+// One side of the diff, as uploaded (layout.transform_base is the scene's own transforms, never a view's).
+struct VbUdSide {
+    const uint32_t *scene, *ramps;
+    const uint8_t *atlas;
+    VbLayout layout;
+    uint32_t n_ramps, atlas_w, atlas_h, pad;
+};
+// The head of the diff's buffer: the base frame's scene and the uploaded one, written by the upload; and the common prefix and
+// suffix lengths, which the frame finds (atomicMin) before it builds the tables.
+struct VbUdiff {
+    VbUdSide old_side, new_side;
+    uint32_t prefix, suffix, pad[2];
+};
+// The diff's buffer after the head: the base frame's draw boxes (n_old), the records of both scenes (n_old, n_new), the
+// positional equality flags (min(n_old, n_new)) and k_recompose_damage's tables (rcmp_tables: identity draw prefixes,
+// new -> old or VB_RCMP_NONE, old unmatched).
+struct VbUdLayout { size_t boxes, old_rec, new_rec, eq, tables, bytes; };
+static inline VbUdLayout vb_udiff_layout(uint32_t n_old, uint32_t n_new) {
+    const size_t m = n_old < n_new ? n_old : n_new;
+    VbUdLayout u;
+    u.boxes = (sizeof(VbUdiff) + 15u) & ~(size_t)15u;
+    u.old_rec = u.boxes + (size_t)n_old * sizeof(VbBbox4);
+    u.new_rec = u.old_rec + (size_t)n_old * sizeof(VbUdRec);
+    u.eq = u.new_rec + (size_t)n_new * sizeof(VbUdRec);
+    u.tables = u.eq + m * 4u;
+    u.bytes = u.tables + ((size_t)n_old + 1u + n_new + 1u + n_new + n_old) * 4u;
+    return u;
+}
+// the records of a scene's n_draw draw objects from its tag and draw monoids; `init` (nullable) gets [m, m], the starting
+// prefix and suffix of the frame's matching
+uint32_t vb_launch_upload_records(const uint32_t *scene, uint32_t path_tag_base, uint32_t draw_tag_base, uint32_t n_tag_words, uint32_t n_draw,
+                                  const VbTagMonoid *tag_monoids, const VbDrawMonoid *draw_monoids, VbUdRec *out, uint32_t *init, uint32_t m,
+                                  cudaStream_t st);
+// the new scene's records, the equality of the draw objects paired by position and from the end, and the tables; nothing while
+// b.udiff is null
+uint32_t vb_launch_upload_diff(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
 // tools/atlas_blit_probe.py: keep the symbol and its C signature)

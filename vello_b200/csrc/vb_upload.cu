@@ -64,11 +64,104 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
     r->dmg.epoch++;
+    // an upload that tracking follows (upload_diff_begin) makes the next frame of this epoch incremental; anything else ends it
+    vb_renderer::Damage::UploadDiff &U = r->dmg.udiff;
+    U.armed = U.pending;
+    U.pending = false;
+    U.epoch = r->dmg.epoch;
     hit_forget(r);
 }
 
+// ---- upload diff: vb_set_upload_diff (k_upload_diff.cu) ----------------------------------------------------------------------
+// Can the frame after an upload diff it against the scene the base frame rendered? Tracking and the switch are on, and there
+// is a base frame of the current scene (the epoch unchanged since: no installation, binding, view, cells or tracking switch),
+// unbound, of one cell, whose intermediates are intact: hit tests answer from it (no failed frame, vb_run_stages or debug write
+// since). As recompose_armed (vb_compose.cu).
+static bool upload_diff_armed(const vb_renderer *r) {
+    const vb_renderer::Damage &D = r->dmg;
+    const vb_renderer::SceneSlot &s = *r->cur;
+    return r->upload_diff && D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !r->bound.rows && r->hit.valid &&
+           !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects &&
+           r->hit.bufs.scene == (const uint32_t *)s.scene.p;
+}
+
+static void swap_spare(vb_renderer *r) {
+    std::swap(r->cur->scene, r->spare_scene);
+    std::swap(r->cur->ramps, r->spare_ramps);
+    std::swap(r->cur->atlas, r->spare_atlas);
+}
+
+// An upload that tracking follows swaps the spare set in; if it fails before it installs its scene, this swaps the base's back,
+// so the renderer keeps the scene it had.
+struct DiffedUpload {
+    vb_renderer *r = nullptr;
+    ~DiffedUpload() {
+        if (r && r->dmg.udiff.pending) {
+            swap_spare(r);
+            r->dmg.udiff.pending = false;
+        }
+    }
+};
+
+// Before an upload of layout L writes the current slot: when the next frame can diff it (upload_diff_armed), keep the base
+// frame's scene. On the upload's stream, before anything overwrites the base frame's intermediates: one copy of its draw boxes
+// and its records (from its tag and draw monoids and its scene, read through the uploaded layout, not the view's). Then the
+// slot's scene, ramps and atlas are swapped with the spare set, sized here for the upload, which the upload then writes; the
+// base's buffers become the spare set, without a copy. The diff's head names both.
+static int upload_diff_begin(vb_renderer *r, cudaStream_t st, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w,
+                             uint32_t atlas_h, DiffedUpload &guard) {
+    r->dmg.udiff.pending = false;
+    if (!upload_diff_armed(r)) return VB_OK;
+    vb_renderer::SceneSlot &s = *r->cur;
+    const uint32_t n_old = s.layout.n_draw_objects, n_new = L.n_draw_objects;
+    const VbUdLayout U = vb_udiff_layout(n_old, n_new);
+    int rc;
+    if ((rc = ensure(r, r->udiff, U.bytes))) return rc;
+    if ((rc = ensure(r, r->spare_scene, scene_bytes(L, scene_words, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->spare_ramps, (size_t)n_ramps * 512 * 4))) return rc;
+    if ((rc = ensure(r, r->spare_atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
+    char *ud = (char *)r->udiff.p;
+    if (n_old) CK(cudaMemcpyAsync(ud + U.boxes, r->hit.bufs.draw_bboxes, (size_t)n_old * sizeof(VbBbox4), cudaMemcpyDeviceToDevice, st));
+    vb_launch_upload_records((const uint32_t *)s.scene.p, s.layout.path_tag_base, s.layout.draw_tag_base, r->hit.cfg.n_tag_words, n_old,
+                             r->hit.bufs.tag_monoids, r->hit.bufs.draw_monoids, (VbUdRec *)(ud + U.old_rec), nullptr, 0u, st);
+    CK(cudaGetLastError());
+    VbUdiff &h = r->ud_head;
+    memset(&h, 0, sizeof h);
+    h.old_side = VbUdSide{(const uint32_t *)s.scene.p, (const uint32_t *)s.ramps.p, (const uint8_t *)s.atlas.p, s.layout, s.n_ramps, s.atlas_w,
+                          s.atlas_h, 0u};
+    h.new_side = VbUdSide{(const uint32_t *)r->spare_scene.p, (const uint32_t *)r->spare_ramps.p, (const uint8_t *)r->spare_atlas.p, L, n_ramps,
+                          atlas_w, atlas_h, 0u};
+    CK(cudaMemcpyAsync(ud, &h, sizeof h, cudaMemcpyHostToDevice, st));
+    swap_spare(r);
+    vb_renderer::Damage::UploadDiff &D = r->dmg.udiff;
+    D.pending = true;
+    D.n_old = n_old;
+    D.n_new = n_new;
+    guard.r = r;
+    return VB_OK;
+}
+
+extern "C" int vb_set_upload_diff(vb_renderer *r, int on) {
+    if (!r) return VB_E_INVALID;
+    if (on && (r->grouped || r->xc.configured)) {
+        r->err = "vb_set_upload_diff: not available for a renderer of a vb_group or with the exchange configured";
+        return VB_E_INVALID;
+    }
+    r->upload_diff = on != 0;
+    if (on) return VB_OK;
+    // off: the next frame cannot diff (it is full, as the upload's installation already said), and the spare set goes
+    r->dmg.udiff.armed = false;
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream)); // an enqueued frame may still read them
+    for (DevBuf *b : {&r->spare_scene, &r->spare_ramps, &r->spare_atlas, &r->udiff}) {
+        if (b->p) CK(cudaFree(b->p));
+        *b = DevBuf{};
+    }
+    return VB_OK;
+}
+
 int vb_host::upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, size_t scene_len, const vb_layout *layout, const uint32_t *ramps,
-                     uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h) {
+                     uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h, bool diff) {
     if (!r || !layout || (scene_len && !scene) || (scene_len & 3)) return VB_E_INVALID;
     if (ramp_h && ramp_w != 512) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
@@ -76,6 +169,8 @@ int vb_host::upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, si
     memcpy(&L, layout, sizeof L);
     if (!atlas) atlas_w = atlas_h = 0;
     int rc;
+    DiffedUpload guard;
+    if (diff && (rc = upload_diff_begin(r, st, L, scene_len / 4, ramp_h, atlas_w, atlas_h, guard))) return rc;
     if ((rc = ensure(r, r->cur->scene, scene_bytes(L, scene_len / 4, r->view.on)))) return rc;
     if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
     if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
@@ -91,7 +186,7 @@ extern "C" int vb_scene_upload(vb_renderer *r, const uint8_t *scene, size_t scen
     if (!r) return VB_E_INVALID;
     int rc = drain_stream(r);
     if (rc) return rc;
-    return upload_on(r, r->stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h);
+    return upload_on(r, r->stream, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h, true);
 }
 
 // ---- images from device memory: Renderer::override_image / register_texture (vello/src/lib.rs:536-603) ----------------------
@@ -383,6 +478,8 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
         patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (hit->x << 16) | hit->y});
     }
     const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
+    DiffedUpload guard;
+    if ((rc = upload_diff_begin(r, st, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, guard))) return rc;
 
     // the six streams go straight to their places in the packed buffer
     if ((rc = ensure(r, r->cur->scene, scene_bytes(L, total_words, r->view.on)))) return rc;

@@ -169,6 +169,7 @@ def load_library() -> C.CDLL:
     lib.vb_debug_match_instances.restype = C.c_uint32
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
+    lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
     lib.vb_last_damage.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_uint32)]
     _lib = lib
@@ -185,7 +186,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
                     "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
-                    "vb_recompose"]
+                    "vb_recompose", "vb_set_upload_diff"]
 
 
 def _device_image(t):
@@ -705,6 +706,13 @@ class Renderer:
         writes no other pixel. With bound instance transforms, the instances whose transforms changed are found on the device;
         `add_damage` names anything else. Switching it on (again) makes the next frame full."""
         self._check(self.lib.vb_set_damage_tracking(self.handle, 1 if on else 0), "vb_set_damage_tracking")
+
+    def set_upload_diff(self, on: bool):
+        """Diff re-uploaded scenes against the scene the last tracked frame rendered (`vb_set_upload_diff`, default off): with
+        damage tracking on, the frame after `upload`, `NativeScene.upload_device` or a device-destination `vb_render` repaints
+        only the tiles of the draw objects that were added, removed or changed, found on the device. Turning it off frees the
+        spare scene buffers it keeps."""
+        self._check(self.lib.vb_set_upload_diff(self.handle, 1 if on else 0), "vb_set_upload_diff")
 
     def add_damage(self, rects):
         """Add half-open pixel rectangles (x0, y0, x1, y1), an (n, 4) array, to the next frame's damage (`vb_add_damage`),
