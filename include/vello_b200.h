@@ -271,7 +271,11 @@ int vb_set_cells(vb_renderer *, const uint32_t *draw_offsets, uint32_t n_cells);
  * with one 2-D copy each from host memory, except those with an override (vb_override_image below), which come from device
  * memory with one k_atlas_blit launch for all of them. Only sizes, the ramp de-duplication and the atlas shelf placement stay on the host. The resulting
  * device buffers are byte-identical to what vb_scene_upload receives from the host-side resolve (tests/test_gpu_parity.py).
- * Glyph runs are not part of this path (they are resolved to outlines above the boundary). */
+ * Glyph runs are not part of this path (they are resolved to outlines above the boundary).
+ * Atlas limit (every resolve: vb_scene_resolve, this one, vb_fragment_upload, vb_compose / vb_recompose): the draw data holds
+ * an image's atlas place and size as 16-bit fields, so an image with a side over 65535 texels, or one the 2048-wide shelves
+ * would place below row 65535, is refused with VB_E_INVALID (vb_last_error says why where the call has a renderer) and the
+ * renderer's scene is left as it was; vb_register_texture refuses a side over 65535 too. */
 typedef struct { float offset, r, g, b, a; } vb_ramp_stop; /* straight-alpha colour */
 typedef struct {
     uint32_t draw_data_offset; /* word in the draw-data stream that receives (ramp id << 2) | extend */

@@ -400,7 +400,8 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
                 key->stamp = seq;
                 key->local = (uint32_t)placed.size();
                 placed.push_back(Placed{key, im.pixels, 0, 0, f.id});
-                shelf.place(key->w, key->h, &placed.back().x, &placed.back().y);
+                if (!shelf.place(key->w, key->h, &placed.back().x, &placed.back().y))
+                    return bad("the composed atlas places an image below row 65535, past the draw data's 16-bit field");
             }
             const Placed &q = placed[key->local];
             patches.push_back(RsPatch{dd0 + im.dd, (q.x << 16) | q.y});

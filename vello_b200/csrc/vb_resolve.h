@@ -66,13 +66,23 @@ static inline uint64_t vb_ramp_hash(const vb_ramp_stop *s, uint32_t n, bool prem
     return h;
 }
 
+// The draw data holds an image's atlas place as (x << 16) | y and its size as (w << 16) | h: each is a 16-bit field, so no
+// side may pass VB_ATLAS_MAX_COORD and no place may start below row VB_ATLAS_MAX_COORD. The atlas itself may reach past that
+// row (an image placed at y = 65535 extends below it).
+#define VB_ATLAS_MAX_COORD 65535u
+static inline bool vb_atlas_side_fits(uint32_t w, uint32_t h) { return w <= VB_ATLAS_MAX_COORD && h <= VB_ATLAS_MAX_COORD; }
+
 // Shelf placement in the atlas (ours: only the (x, y) written into the draw data matters to the pipeline). Images go left to
 // right in rows up to 2048 wide; one that does not fit starts a new row below the tallest image of the last. The caller places
-// each distinct image once, in first-seen order.
+// each distinct image once, in first-seen order. place() is false, and the packer unchanged, for an image with a side over
+// VB_ATLAS_MAX_COORD or one whose place would start below row VB_ATLAS_MAX_COORD; the caller refuses the scene.
 struct VbShelfPacker {
     uint32_t width = 1, x = 0, y = 0, shelf_h = 0;
-    void place(uint32_t w, uint32_t h, uint32_t *px, uint32_t *py) {
-        if (x + w > 2048u) {
+    bool place(uint32_t w, uint32_t h, uint32_t *px, uint32_t *py) {
+        if (!vb_atlas_side_fits(w, h)) return false;
+        const bool new_shelf = x + w > 2048u;
+        if (new_shelf && y + shelf_h > VB_ATLAS_MAX_COORD) return false;
+        if (new_shelf) {
             y += shelf_h;
             x = 0;
             shelf_h = 0;
@@ -82,6 +92,7 @@ struct VbShelfPacker {
         x += w;
         if (h > shelf_h) shelf_h = h;
         if (x > width) width = x;
+        return true;
     }
     uint32_t height() const { return y + shelf_h > 1u ? y + shelf_h : 1u; }
 };

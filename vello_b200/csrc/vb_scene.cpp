@@ -1380,7 +1380,8 @@ int vb_scene_resolve(vb_scene *s, vb_packed *out) {
         }
         draw_data[p.draw_data_offset] = (rid << 2) | p.extend;
     }
-    // late-bound images: each distinct (pixels, width, height) placed once in the atlas
+    // late-bound images: each distinct (pixels, width, height) placed once in the atlas; a scene whose atlas places do not fit
+    // the draw data's 16-bit fields is refused (VbShelfPacker)
     struct Placed { const uint8_t *key; uint32_t w, h, x, y; };
     std::vector<Placed> placed;
     VbShelfPacker shelf;
@@ -1391,7 +1392,7 @@ int vb_scene_resolve(vb_scene *s, vb_packed *out) {
             if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
         if (!hit) {
             placed.push_back(Placed{im.pixels, im.width, im.height, 0, 0});
-            shelf.place(im.width, im.height, &placed.back().x, &placed.back().y);
+            if (!shelf.place(im.width, im.height, &placed.back().x, &placed.back().y)) return VB_E_INVALID;
             hit = &placed.back();
         }
         draw_data[p.draw_data_offset] = (hit->x << 16) | hit->y;

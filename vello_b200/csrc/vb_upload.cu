@@ -304,6 +304,10 @@ extern "C" int vb_texture_register(vb_renderer *r, const void *device_pixels, ui
         r->err = "vb_register_texture: NULL pixels";
         return VB_E_INVALID;
     }
+    if (!vb_atlas_side_fits(width, height)) {
+        r->err = "vb_register_texture: a side over 65535 texels (an image's size is two 16-bit fields)";
+        return VB_E_INVALID;
+    }
     CK(cudaSetDevice(r->device));
     int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
     if (rc) return rc;
@@ -392,8 +396,11 @@ int vb_host::check_streams(vb_renderer *r, const vb_encoding_streams *e, const c
         const vb_ramp_patch &p = e->ramp_patches[i];
         if (!p.n_stops || !p.stops || p.draw_data_offset >= e->n_draw_data) return bad("a ramp patch without stops or outside the draw data");
     }
-    for (uint32_t i = 0; i < e->n_image_patches; i++)
-        if (e->image_patches[i].draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+    for (uint32_t i = 0; i < e->n_image_patches; i++) {
+        const vb_image_patch &im = e->image_patches[i];
+        if (im.draw_data_offset >= e->n_draw_data) return bad("an image patch outside the draw data");
+        if (!vb_atlas_side_fits(im.width, im.height)) return bad("an image with a side over 65535 texels");
+    }
     return VB_OK;
 }
 
@@ -470,7 +477,11 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
             if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
         if (!hit) {
             Placed q{im.pixels, im.width, im.height, 0, 0, false};
-            shelf.place(q.w, q.h, &q.x, &q.y);
+            if (!shelf.place(q.w, q.h, &q.x, &q.y)) {
+                r->err = "device resolve: an image's atlas place or size passes 16 bits (at most 65535 rows of shelves and 65535 "
+                         "texels a side)";
+                return VB_E_INVALID;
+            }
             if ((rc = image_source(r, "device resolve", q.key, q.w, q.h, q.x, q.y, blits, over, &q.from_device))) return rc;
             placed.push_back(q);
             hit = &placed.back();

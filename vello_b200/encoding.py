@@ -757,6 +757,7 @@ def batch(scenes: Sequence[Scene]) -> Tuple[Scene, List[int]]:
 # reference uses guillotiere -- only the (x, y) written into draw data matters to the pipeline)
 # ---------------------------------------------------------------------------------------------
 N_RAMP_SAMPLES = 512
+ATLAS_MAX_COORD = 65535  # the largest atlas x, y, width and height the draw data's 16-bit fields hold
 
 
 def make_ramp(stops: Sequence[Tuple[float, Color]], premul_interp: bool) -> np.ndarray:
@@ -852,7 +853,8 @@ def resolve(enc: Encoding) -> Packed:
             ramp_rows.append(make_ramp(p["stops"], p["premul"]))
         rid = ramp_keys[key]
         draw_data[p["draw_data_offset"]] = ((rid << 2) | p["extend"]) & 0xFFFFFFFF
-    # late-bound: images -> simple shelf atlas
+    # late-bound: images -> simple shelf atlas (VbShelfPacker, vb_resolve.h); the draw data holds a place and a size as
+    # 16-bit fields, so an image with a side over ATLAS_MAX_COORD, or a place below row ATLAS_MAX_COORD, is refused
     atlas_w = 1
     shelves: List[Tuple[int, int, Image]] = []
     x = y = shelf_h = 0
@@ -863,7 +865,11 @@ def resolve(enc: Encoding) -> Packed:
         # the image cache is keyed by the pixel blob's identity (image_cache.rs:113-114), not by the brush
         k = ("key", im.key) if im.key is not None else ("id", id(im.data))
         if k not in placed:
+            if im.width > ATLAS_MAX_COORD or im.height > ATLAS_MAX_COORD:
+                raise ValueError(f"resolve: a {im.width}x{im.height} image has a side over {ATLAS_MAX_COORD} texels")
             if x + im.width > MAXW:
+                if y + shelf_h > ATLAS_MAX_COORD:
+                    raise ValueError(f"resolve: the atlas would place an image at row {y + shelf_h}, past {ATLAS_MAX_COORD}")
                 y += shelf_h
                 x = 0
                 shelf_h = 0
