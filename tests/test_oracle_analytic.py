@@ -12,8 +12,9 @@ Porter-Duff operators, radial and sweep gradients, luminance masks -- to first p
   edges are the LUT-quantised half planes, asserted within 2 samples of the exact area;
 * a stroke's total coverage == width x length (+ the caps' area);
 * a clipped fill == clip coverage x fill coverage;
-* every blend mode == the W3C `Compositing and Blending Level 1` formula evaluated in float64 here (restated from the
-  specification text, not from blend.wgsl), within 2 LSB (the backdrop passes through one 8-bit store on the blend stack);
+* every blend mode == the W3C `Compositing and Blending Level 1` formula evaluated in float64 by blend_ref.py (restated
+  from the specification text, not from blend.wgsl), within 2 LSB at a few colour pairs (test_blend_ref.py checks every
+  branch of the same formulas exactly, over 65536 pairs per mode);
 * radial / sweep gradients == the ramp colour at the analytically computed parameter.
 """
 import math
@@ -25,6 +26,8 @@ from vello_b200.config import AA_AREA, AA_MSAA8, AA_MSAA16
 from vello_b200.encoding import (BLACK, COMPOSE_SRC_OVER, FILL_EVEN_ODD, FILL_NON_ZERO, MIX_NORMAL, STYLE_CAP_BUTT, STYLE_CAP_ROUND,
                                  STYLE_CAP_SQUARE, STYLE_JOIN_BEVEL, TRANSPARENT, Color, Gradient, Scene, Stroke, resolve)
 from vello_b200.shapes import Affine, BezPath, Line, Rect
+
+from .blend_ref import MIXES, w3c_composite
 
 WHITE = Color.from_rgba8(255, 255, 255)
 
@@ -177,104 +180,7 @@ def test_clip_is_the_product_of_coverages(oracle):
     assert np.abs(got - a * b).max() <= 1.5 / 255
 
 
-# ---- W3C compositing and blending, restated from the specification ----------------------------------------------------------------
-def _lum(c):
-    return 0.3 * c[0] + 0.59 * c[1] + 0.11 * c[2]
-
-
-def _clip_color(c):
-    l, n, x = _lum(c), min(c), max(c)
-    if n < 0:
-        c = [l + (v - l) * l / (l - n) for v in c]
-    if x > 1:
-        c = [l + (v - l) * (1 - l) / (x - l) for v in c]
-    return c
-
-
-def _set_lum(c, l):
-    d = l - _lum(c)
-    return _clip_color([v + d for v in c])
-
-
-def _sat(c):
-    return max(c) - min(c)
-
-
-def _set_sat(c, s):
-    order = sorted(range(3), key=lambda i: c[i])  # spec: Cmin, Cmid, Cmax
-    lo, mid, hi = order
-    out = [0.0, 0.0, 0.0]
-    if c[hi] > c[lo]:
-        out[mid] = (c[mid] - c[lo]) * s / (c[hi] - c[lo])
-        out[hi] = s
-    return out
-
-
-def _sep(mode, cb, cs):
-    if mode == "multiply":
-        return cb * cs
-    if mode == "screen":
-        return cb + cs - cb * cs
-    if mode == "hard_light":
-        return cb * 2 * cs if cs <= 0.5 else _sep("screen", cb, 2 * cs - 1)
-    if mode == "overlay":
-        return _sep("hard_light", cs, cb)
-    if mode == "darken":
-        return min(cb, cs)
-    if mode == "lighten":
-        return max(cb, cs)
-    if mode == "color_dodge":
-        return 0.0 if cb == 0 else (1.0 if cs == 1 else min(1.0, cb / (1 - cs)))
-    if mode == "color_burn":
-        return 1.0 if cb == 1 else (0.0 if cs == 0 else 1 - min(1.0, (1 - cb) / cs))
-    if mode == "soft_light":
-        if cs <= 0.5:
-            return cb - (1 - 2 * cs) * cb * (1 - cb)
-        d = ((16 * cb - 12) * cb + 4) * cb if cb <= 0.25 else math.sqrt(cb)
-        return cb + (2 * cs - 1) * (d - cb)
-    if mode == "difference":
-        return abs(cb - cs)
-    if mode == "exclusion":
-        return cb + cs - 2 * cb * cs
-    raise KeyError(mode)
-
-
-MIXES = ["normal", "multiply", "screen", "overlay", "darken", "lighten", "color_dodge", "color_burn", "hard_light", "soft_light",
-         "difference", "exclusion", "hue", "saturation", "color", "luminosity"]  # peniko::Mix values 0..15
-
-
-def w3c_mix(mode, cb, cs):
-    if mode == "normal":
-        return list(cs)
-    if mode == "hue":
-        return _set_lum(_set_sat(cs, _sat(cb)), _lum(cb))
-    if mode == "saturation":
-        return _set_lum(_set_sat(cb, _sat(cs)), _lum(cb))
-    if mode == "color":
-        return _set_lum(cs, _lum(cb))
-    if mode == "luminosity":
-        return _set_lum(cb, _lum(cs))
-    return [_sep(mode, cb[i], cs[i]) for i in range(3)]
-
-
-# peniko::Compose values 0..13 -> Porter-Duff (Fa, Fb) as functions of (alpha_s, alpha_b)
-PD = [lambda s, b: (0, 0), lambda s, b: (1, 0), lambda s, b: (0, 1), lambda s, b: (1, 1 - s), lambda s, b: (1 - b, 1), lambda s, b: (b, 0),
-      lambda s, b: (0, s), lambda s, b: (1 - b, 0), lambda s, b: (0, 1 - s), lambda s, b: (b, 1 - s), lambda s, b: (1 - b, s),
-      lambda s, b: (1 - b, 1 - s), lambda s, b: (1, 1), lambda s, b: (1, 1)]
-
-
-def w3c_composite(mix, compose, cb, ab, cs, as_):
-    """Unpremultiplied backdrop / source colours and alphas -> premultiplied result (r, g, b, a)."""
-    bm = w3c_mix(MIXES[mix], cb, cs)
-    cm = [(1 - ab) * cs[i] + ab * bm[i] for i in range(3)]
-    fa, fb = PD[compose](as_, ab)
-    co = [as_ * fa * cm[i] + ab * fb * cb[i] for i in range(3)]
-    ao = as_ * fa + ab * fb
-    if compose == 13:  # plus-lighter: clamped sum
-        co = [min(1.0, v) for v in co]
-    return co + [min(1.0, ao)]
-
-
+# ---- W3C compositing and blending: the float64 restatement of the specification lives in blend_ref.py -------------------
 def _blend_scene(mix, compose, backdrop: Color, source: Color, layer_alpha=1.0):
     s = Scene()
     r = Rect(0.0, 0.0, 16.0, 16.0)
