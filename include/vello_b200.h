@@ -96,9 +96,9 @@ const char *vb_last_error(vb_renderer *);
 int vb_scene_upload(vb_renderer *, const uint8_t *scene, size_t scene_len, const vb_layout *, const uint32_t *ramps,
                     uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas_rgba8, uint32_t atlas_w, uint32_t atlas_h);
 
-/* Render the uploaded scene. `out` is a DEVICE pointer (RGBA8, un-premultiplied, pitch 4*width) or NULL
- * to render into the renderer's own target (see vb_target). Blocks until the frame is complete and
- * arenas were large enough (re-running if not). */
+/* Render the uploaded scene. `out` is a DEVICE pointer (RGBA8, un-premultiplied, pitch 4*width), the key of a registered
+ * destination (vb_register_destination: a pitched buffer or a CUDA array, RGBA8 or BGRA8), or NULL to render into the
+ * renderer's own target (see vb_target). Blocks until the frame is complete and arenas were large enough (re-running if not). */
 int vb_render_resident(vb_renderer *, const vb_params *, void *out_device, vb_frame_stats *);
 
 /* Asynchronous variant for pipelined use / benchmarks: enqueue one attempt and return. The frame is
@@ -188,6 +188,49 @@ int vb_hit_test(vb_renderer *, const float *xy, uint32_t n, int32_t *draw_ix, ui
 void *vb_target(vb_renderer *, size_t *bytes);
 /* Copy `bytes` from a device pointer to a host pointer on the renderer's stream, then synchronise. */
 int vb_copy_to_host(vb_renderer *, const void *src_device, void *dst_host, size_t bytes);
+/* ---- registered destinations: frames straight into CUDA arrays (interop images) and pitched buffers (an addition) ----
+ * vello's render_to_texture writes a storage texture. A Vulkan or GL image imported into CUDA is a CUDA array, not a device
+ * pointer: cudaImportExternalMemory, cudaExternalMemoryGetMappedMipmappedArray (with cudaArraySurfaceLoadStore), then
+ * cudaGetMipmappedArrayLevel(.., 0). vb_register_destination turns such an array, or linear device memory at any row pitch,
+ * into a key, which goes wherever a device destination pointer goes: vb_render_resident, vb_render_enqueue / vb_frame_finish,
+ * vb_render_uploaded, vb_render and vb_render_scene with out_is_device = 1, and vb_run_stages.
+ *  - Pixel (px, py) of a frame lands at texel (x + px, y + py) of the array, or at ptr + py * row_pitch_bytes + 4 * px. The
+ *    bytes are the frame's un-premultiplied RGBA8, with r and b swapped for VB_DEST_BGRA8. No colour conversion is done: an
+ *    _SRGB image receives vello's bytes as they are (already sRGB-encoded values).
+ *  - A destination holds the whole frame, so a bin_row / tile_row window writes only its rows, at their own rows of the
+ *    destination. (A plain pointer differs: its first row is the window's first row.)
+ *  - Damage tracking: a frame into the same key as the last successful frame can be incremental, writing only its damaged
+ *    tiles into the destination. Whole-frame graphs are keyed by the key like a pointer.
+ *  - Keys come from the same reserved, inaccessible address range as vb_register_texture's keys: no buffer has a key's
+ *    address, a key is never handed out twice, and a key used as an image key reads as an unregistered texture key does.
+ * VB_E_INVALID (vb_last_error says why), each checked on the host before anything is enqueued:
+ *  - registering: NULL arguments; an unknown kind or format; a renderer of a vb_group or with the exchange configured;
+ *    LINEAR: ptr NULL, not 4-byte aligned, or not device or managed memory of the renderer's device; a row pitch that is not a
+ *    multiple of 4 or is 2^34 bytes or more; ARRAY: not a 2-D array (1-D, layered, cubemap, 3-D), channels other than four
+ *    8-bit cudaChannelFormatKindUnsigned ones, no cudaArraySurfaceLoadStore flag;
+ *  - a frame into a key: the key is unregistered, another renderer's or a texture key; the frame does not fit (x + width or
+ *    y + its last row past the array's extent, a row pitch below 4 * width); a batch (vb_set_cells with more than one cell);
+ *  - a key where a host pointer or a plain device pointer is needed: vb_render / vb_render_uploaded / vb_render_scene with
+ *    out_is_device = 0, vb_render_begin's out_host, vb_copy_to_host, image pixels (vb_override_image, vb_register_texture),
+ *    vb_group destinations.
+ * The caller keeps the memory or array alive and on the renderer's device while the key is registered. No CUDA call tells
+ * cheaply which device an array belongs to, so an array of another device is a caller error, as a freed pointer is.
+ * vb_unregister_destination returns once the frames already enqueued into the key have completed; VB_E_INVALID for a key that
+ * is not a destination of this renderer. vb_renderer_free releases the destinations still registered. */
+#define VB_DEST_LINEAR 0 /* device memory, row_pitch_bytes apart */
+#define VB_DEST_ARRAY 1  /* a 2-D CUDA array (cudaArray_t / CUarray), written through a surface object */
+#define VB_DEST_RGBA8 0  /* byte order of a stored pixel: vello's Rgba8Unorm (r in the low byte) */
+#define VB_DEST_BGRA8 1  /* b, g, r, a */
+typedef struct {
+    uint32_t kind, format;
+    void *ptr;              /* LINEAR: where pixel (0, 0) of a frame goes */
+    size_t row_pitch_bytes; /* LINEAR */
+    void *array;            /* ARRAY: level-0 array of the renderer's device */
+    uint32_t x, y;          /* ARRAY: the texel pixel (0, 0) of a frame lands on */
+} vb_destination;
+int vb_register_destination(vb_renderer *, const vb_destination *, void **key_out);
+int vb_unregister_destination(vb_renderer *, void *key);
+
 /* cudaStream_t the renderer enqueues on (for event timing by the caller). Writes to an overridden image's device pixels
  * (vb_override_image) that are enqueued on this stream before the copying call are ordered before the copy. */
 void *vb_stream(vb_renderer *);

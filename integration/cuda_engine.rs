@@ -49,6 +49,11 @@ pub struct VbEncodingStreams {
     pub image_patches: *const VbImagePatch, pub n_image_patches: u32,
 }
 
+/// a registered destination (vb_register_destination): VB_DEST_LINEAR 0 / VB_DEST_ARRAY 1, VB_DEST_RGBA8 0 / VB_DEST_BGRA8 1.
+/// For a wgpu/Vulkan storage texture: the image's memory imported into CUDA, level 0 of its mipmapped array in `array`.
+#[repr(C)]
+pub struct VbDestination { pub kind: u32, pub format: u32, pub ptr: *mut c_void, pub row_pitch_bytes: usize, pub array: *mut c_void, pub x: u32, pub y: u32 }
+
 pub enum VbRenderer {}
 pub enum VbGroup {}
 
@@ -89,6 +94,9 @@ extern "C" {
     pub fn vb_set_damage_tracking(r: *mut VbRenderer, on: c_int) -> c_int;
     pub fn vb_add_damage(r: *mut VbRenderer, rects: *const u32, n: u32) -> c_int;
     pub fn vb_last_damage(r: *mut VbRenderer, tile_mask: *mut u8, cap: usize, n_damaged: *mut u32) -> c_int;
+    // frames straight into a storage texture (a CUDA array) or a pitched buffer: the key goes where out_device goes
+    pub fn vb_register_destination(r: *mut VbRenderer, d: *const VbDestination, key_out: *mut *mut c_void) -> c_int;
+    pub fn vb_unregister_destination(r: *mut VbRenderer, key: *mut c_void) -> c_int;
     // vb_compose, after which the next tracked frame repaints only the instances added, removed or changed since the composition
     // the last frame rendered (matched in order by fragment and transform); vb_compose itself makes the next frame full
     pub fn vb_recompose(r: *mut VbRenderer, instances: *const VbInstance, n: u32, layout_out: *mut Layout, draw_offsets: *mut u32) -> c_int;

@@ -30,6 +30,8 @@
 // Algorithmic bytes: 4 B/pixel stored + 4 B per PTCL word + 24 B per segment referenced.
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "vb_detmath.h"
 #include "vb_device.cuh"
 #include "vb_stages.h"
@@ -87,6 +89,14 @@ struct FineArgs {
     const uint32_t *cls_count;  // their fill counts (control block); NULL: natural tile order
     uint32_t cls_stride;
     uint32_t cull;              // 1: start each tile there
+};
+// The arguments of the FI_DST instantiations: FineArgs, then a registered destination's (vb_launch_fine's VbFineOut): the
+// __byte_perm selector of the stored byte order, and either linear memory at `out` or, with `array`, the surface of a CUDA
+// array, pixel (x, y) of the frame at texel (x0 + x, y0 + y). The other instantiations take FineArgs alone, so that their code
+// is exactly what it was before destinations existed (a larger parameter block alone changes ptxas's register assignment).
+struct FineDstArgs : FineArgs {
+    cudaSurfaceObject_t surf;
+    uint32_t swz, array, x0, y0;
 };
 
 // ---------------- mbarrier + bulk-copy (TMA) primitives: PTX as in cute/arch/copy_sm90_tma.hpp, cutlass/arch/barrier.h ----------------
@@ -771,13 +781,17 @@ static_assert(sizeof(WarpIo) % 16 == 0 && sizeof(WarpMs<1>) % 16 == 0 && sizeof(
 
 // MODE: the AA mode (0 area, 1 MSAA8, 2 MSAA16), plus FI_DMG for damage tracking (k_damage.cu): coarse listed only the
 // damaged tiles, and those lists are the whole queue, so no other pixel is written. Without FI_DMG the kernel is the one it was
-// before damage tracking existed.
+// before damage tracking existed. FI_DST: a registered destination (vb_register_destination) in BGRA8 order or in a CUDA array;
+// only the store differs.
 #define FI_DMG 16
+#define FI_DST 32
+template <int MODE> using FineArgsOf = typename std::conditional<(MODE & FI_DST) != 0, FineDstArgs, FineArgs>::type;
 template <int MODE>
 __global__ void __launch_bounds__(FI_MAX_THREADS, FI_MINB)
-k_fine(VbConfig cfg, FineArgs A) {
+k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
     constexpr int AA = MODE & 15;
     constexpr bool DMG = (MODE & FI_DMG) != 0;
+    constexpr bool DST = (MODE & FI_DST) != 0;
     extern __shared__ __align__(16) unsigned char smem[];
     typedef WarpMs<AA == 0 ? 1 : AA> Ms;
     const uint32_t *__restrict__ ptcl = A.ptcl;
@@ -1213,18 +1227,40 @@ k_fine(VbConfig cfg, FineArgs A) {
                     px[i] = unorm8(fg.r * a_inv) | (unorm8(fg.g * a_inv) << 8) | (unorm8(fg.b * a_inv) << 16) | (unorm8(fg.a) << 24);
                 }
             }
-            // the cell again, from the tile index (keeping it live across the interpreter would cost a register)
-            const uint32_t out_cell = cfg.n_cells > 1u ? tile_ix / wt / cfg.height_in_tiles : 0u;
-            uint32_t *row = A.out + ((size_t)out_cell * cfg.target_height + (gy - cfg.out_row0)) * cfg.out_pitch_px;
-            if (gx + 7u < cfg.target_width && (cfg.out_pitch_px & 3u) == 0u && ((uintptr_t)A.out & 15u) == 0u) {
-                // two 128-bit stores: 32 contiguous bytes of one pixel row per lane
-                uint4 *dst = reinterpret_cast<uint4 *>(row + gx);
-                dst[0] = make_uint4(px[0], px[1], px[2], px[3]);
-                dst[1] = make_uint4(px[4], px[5], px[6], px[7]);
-            } else {
+            bool stored = false;
+            if constexpr (DST) {
 #pragma unroll
-                for (int i = 0; i < PX; i++)
-                    if (gx + i < cfg.target_width) row[gx + i] = px[i];
+                for (int i = 0; i < PX; i++) px[i] = __byte_perm(px[i], 0u, A.swz);
+                if (A.array) {
+                    // gy is the frame's own row, also in a window. Texels out of the array's range are dropped
+                    // (cudaBoundaryModeZero), though the host refuses a frame that does not fit before it is enqueued.
+                    const uint32_t x = A.x0 + gx, y = A.y0 + gy;
+                    if (gx + 7u < cfg.target_width && (x & 3u) == 0u) {
+                        // two 128-bit stores: 32 contiguous bytes of one texel row per lane
+                        surf2Dwrite(make_uint4(px[0], px[1], px[2], px[3]), A.surf, (int)(x * 4u), (int)y, cudaBoundaryModeZero);
+                        surf2Dwrite(make_uint4(px[4], px[5], px[6], px[7]), A.surf, (int)(x * 4u + 16u), (int)y, cudaBoundaryModeZero);
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < PX; i++)
+                            if (gx + i < cfg.target_width) surf2Dwrite(px[i], A.surf, (int)((x + i) * 4u), (int)y, cudaBoundaryModeZero);
+                    }
+                    stored = true;
+                }
+            }
+            if (!stored) {
+                // the cell again, from the tile index (keeping it live across the interpreter would cost a register)
+                const uint32_t out_cell = cfg.n_cells > 1u ? tile_ix / wt / cfg.height_in_tiles : 0u;
+                uint32_t *row = A.out + ((size_t)out_cell * cfg.target_height + (gy - cfg.out_row0)) * cfg.out_pitch_px;
+                if (gx + 7u < cfg.target_width && (cfg.out_pitch_px & 3u) == 0u && ((uintptr_t)A.out & 15u) == 0u) {
+                    // two 128-bit stores: 32 contiguous bytes of one pixel row per lane
+                    uint4 *dst = reinterpret_cast<uint4 *>(row + gx);
+                    dst[0] = make_uint4(px[0], px[1], px[2], px[3]);
+                    dst[1] = make_uint4(px[4], px[5], px[6], px[7]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < PX; i++)
+                        if (gx + i < cfg.target_width) row[gx + i] = px[i];
+                }
             }
         }
         __syncwarp();
@@ -1235,24 +1271,35 @@ k_fine(VbConfig cfg, FineArgs A) {
 #undef START_OF
 }
 
+template <int MODE> static cudaError_t fine_smem_limit() {
+    return cudaFuncSetAttribute(k_fine<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<MODE & 15>::bytes(FI_MAX_WARPS));
+}
 extern "C" int vb_fine_init_constants(void) {
     float h[256];
     for (int i = 0; i < 256; i++) h[i] = (float)i / 255.0f;
     cudaError_t e = cudaMemcpyToSymbol(c_unorm, h, sizeof h);
     // the kernels use more than the default 48 KB of dynamic shared memory per CTA
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<0>::bytes(FI_MAX_WARPS));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<0 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<0>::bytes(FI_MAX_WARPS));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<1>::bytes(FI_MAX_WARPS));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<1 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<1>::bytes(FI_MAX_WARPS));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<2>::bytes(FI_MAX_WARPS));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_fine<2 + FI_DMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<2>::bytes(FI_MAX_WARPS));
+    const decltype(&fine_smem_limit<0>) set[] = {
+        fine_smem_limit<0>, fine_smem_limit<0 + FI_DMG>, fine_smem_limit<0 + FI_DST>, fine_smem_limit<0 + FI_DST + FI_DMG>,
+        fine_smem_limit<1>, fine_smem_limit<1 + FI_DMG>, fine_smem_limit<1 + FI_DST>, fine_smem_limit<1 + FI_DST + FI_DMG>,
+        fine_smem_limit<2>, fine_smem_limit<2 + FI_DMG>, fine_smem_limit<2 + FI_DST>, fine_smem_limit<2 + FI_DST + FI_DMG>};
+    for (auto f : set)
+        if (e == cudaSuccess) e = f();
     return (int)e;
+}
+
+// k_fine<aa + FLAGS>, with FineArgs alone unless FLAGS has FI_DST
+template <int FLAGS> static void launch_fine(int aa, uint32_t grid, uint32_t warps, cudaStream_t st, const VbConfig &cfg, const FineDstArgs &A) {
+    const FineArgsOf<FLAGS> &a = A;
+    if (aa == 0) k_fine<0 + FLAGS><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, a);
+    else if (aa == 1) k_fine<1 + FLAGS><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, a);
+    else k_fine<2 + FLAGS><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, a);
 }
 
 // The launch's tile queue is control-block word VB_CTL_FINE_QUEUE + band, zeroed with the control block (8 of them, one per
 // read-back band).
-extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, uint32_t *out, int aa, uint32_t cull, uint32_t band, bool cls_order,
-                                   cudaStream_t st) {
+extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, int aa, uint32_t cull, uint32_t band,
+                                   bool cls_order, cudaStream_t st) {
     uint32_t rows = cfg.win_ty1 - cfg.win_ty0;
     uint32_t n = cfg.width_in_tiles * rows;
     if (n == 0) return 0;
@@ -1263,8 +1310,8 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, ui
     uint32_t grid = (n + warps - 1u) / warps;
     const uint32_t resident = (uint32_t)sm_count * FI_MINB * (FI_MAX_WARPS / warps);
     if (grid > resident) grid = resident;
-    FineArgs A;
-    A.segments = b.segments; A.ptcl = b.ptcl; A.info = b.info_bin_data; A.blend_spill = b.blend_spill; A.out = out; A.ramps = b.ramps; A.atlas = b.atlas;
+    FineDstArgs A;
+    A.segments = b.segments; A.ptcl = b.ptcl; A.info = b.info_bin_data; A.blend_spill = b.blend_spill; A.out = o.out; A.ramps = b.ramps; A.atlas = b.atlas;
     A.mask_lut = aa == 2 ? b.mask16 : b.mask8;
     A.cull = cull;
     A.tile_start = b.tile_start;
@@ -1273,14 +1320,18 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, ui
     A.cls_list = b.cls_list;
     A.cls_count = cls_order ? b.ctl + VB_CTL_FINE_CLASS : nullptr;
     A.cls_stride = cfg.width_in_tiles * cfg.tile_rows;
-    if (b.dmg_mode == VB_DMG_INCREMENTAL && cls_order) { // the damaged tiles of coarse's lists only
-        if (aa == 0) k_fine<0 + FI_DMG><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, A);
-        else if (aa == 1) k_fine<1 + FI_DMG><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, A);
-        else k_fine<2 + FI_DMG><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, A);
-        return 1;
+    A.surf = o.surf;
+    A.swz = o.swz;
+    A.array = o.array;
+    A.x0 = o.x0;
+    A.y0 = o.y0;
+    const bool dmg = b.dmg_mode == VB_DMG_INCREMENTAL && cls_order; // the damaged tiles of coarse's lists only
+    if (o.dst) {
+        if (dmg) launch_fine<FI_DST + FI_DMG>(aa, grid, warps, st, cfg, A);
+        else launch_fine<FI_DST>(aa, grid, warps, st, cfg, A);
+    } else {
+        if (dmg) launch_fine<FI_DMG>(aa, grid, warps, st, cfg, A);
+        else launch_fine<0>(aa, grid, warps, st, cfg, A);
     }
-    if (aa == 0) k_fine<0><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, A);
-    else if (aa == 1) k_fine<1><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, A);
-    else k_fine<2><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, A);
     return 1;
 }

@@ -15,6 +15,7 @@
 
 #include "vb_device.cuh"
 #include "vb_renderer.h"
+#include "vb_textures.h"
 
 // path_tiling_setup.wgsl:21-26 flags a failed frame to fine through ptcl[0] = ~0. That word is also tile 0's blend offset
 // and is only rewritten when coarse visits tile 0 -- which a stripe window with bin_row0 > 0 never does, so the flag of a
@@ -273,8 +274,15 @@ extern "C" void *vb_target(vb_renderer *r, size_t *bytes) {
     if (bytes) *bytes = r->target.cap;
     return r->target.p;
 }
+// A key given where a host pointer or a plain device pointer is needed: refused, since a key is an inaccessible address.
+static int refuse_key(vb_renderer *r, const void *p, const char *who) {
+    if (!vb_texture_key(p)) return VB_OK;
+    r->err = std::string(who) + ": a texture or destination key is not a host or device pointer here";
+    return VB_E_INVALID;
+}
 extern "C" int vb_copy_to_host(vb_renderer *r, const void *src_device, void *dst_host, size_t bytes) {
     if (!r || !src_device || !dst_host) return VB_E_INVALID;
+    if (refuse_key(r, src_device, "vb_copy_to_host") || refuse_key(r, dst_host, "vb_copy_to_host")) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     CK(cudaMemcpyAsync(dst_host, src_device, bytes, cudaMemcpyDeviceToHost, r->stream));
     CK(cudaStreamSynchronize(r->stream));
@@ -631,7 +639,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             for (uint32_t band = 0; band < f.bands; band++) {
                 VbConfig cb = c;
                 if (!f.band(band, &cb.win_ty0, &cb.win_ty1)) break;
-                launches += vb_launch_fine(cb, b, (uint32_t *)d.dev, (int)r->params.aa, r->occlusion_cull, band, f.bands == 1u, st);
+                launches += vb_launch_fine(cb, b, d.out, (int)r->params.aa, r->occlusion_cull, band, f.bands == 1u, st);
                 if (d.host && (rc = queue_readback(r, c, f, band, d))) return rc;
             }
             break;
@@ -730,13 +738,19 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
     return VB_OK;
 }
 
-// The frame's device destination: the given pointer, or the renderer's own target (allocated for this frame's window).
+// The frame's device destination: a registered destination's key, the given pointer, or the renderer's own target (allocated
+// for this frame's window).
 static int pick_out(vb_renderer *r, Dest *d) {
-    if (d->dev) return VB_OK;
-    const VbConfig &c = r->cfg;
-    DevBuf &t = d->alt ? r->target_alt : r->target;
-    int rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * fine_rows(c, *d).dest_rows);
-    d->dev = t.p;
+    if (vb_texture_key(d->dev)) return resolve_destination(r, d);
+    int rc = VB_OK;
+    if (!d->dev) {
+        const VbConfig &c = r->cfg;
+        DevBuf &t = d->alt ? r->target_alt : r->target;
+        rc = ensure(r, t, (size_t)c.out_pitch_px * 4u * fine_rows(c, *d).dest_rows);
+        d->dev = t.p;
+    }
+    d->out = VbFineOut{};
+    d->out.out = (uint32_t *)d->dev;
     return rc;
 }
 
@@ -906,6 +920,7 @@ extern "C" int vb_render_resident(vb_renderer *r, const vb_params *p, void *out_
 
 extern "C" int vb_render_uploaded(vb_renderer *r, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {
     if (!r || !p || !out) return VB_E_INVALID;
+    if (!out_is_device && refuse_key(r, out, "vb_render_uploaded")) return VB_E_INVALID;
     return render_sync(r, p, out_is_device ? Dest{out} : Dest{nullptr, out, false, r->readback_bands}, stats);
 }
 
@@ -913,6 +928,7 @@ extern "C" int vb_render(vb_renderer *r, const uint8_t *scene, size_t scene_len,
                          uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h, const vb_params *p,
                          void *out, uint32_t out_is_device, vb_frame_stats *stats) {
     if (!r || !p || !out) return VB_E_INVALID;
+    if (!out_is_device && refuse_key(r, out, "vb_render")) return VB_E_INVALID;
     int rc = vb_scene_upload(r, scene, scene_len, layout, ramps, ramp_w, ramp_h, atlas, atlas_w, atlas_h);
     if (rc) return rc;
     return vb_render_uploaded(r, p, out, out_is_device, stats);
@@ -974,6 +990,7 @@ extern "C" int vb_render_begin(vb_renderer *r, const uint8_t *scene, size_t scen
                                uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas, uint32_t atlas_w, uint32_t atlas_h,
                                const vb_params *p, void *out_host, vb_frame_stats *stats) {
     if (!r || !p || !out_host) return VB_E_INVALID;
+    if (refuse_key(r, out_host, "vb_render_begin")) return VB_E_INVALID;
     CK(cudaSetDevice(r->device));
     if (stats) memset(stats, 0, sizeof *stats);
     const uint64_t k = r->stream_seq;
@@ -1037,7 +1054,7 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     int rc = prepare(r, p);
     if (rc) return rc;
     Dest d{out_device};
-    if (last == VB_STAGE_ID_FINE && (rc = pick_out(r, &d))) return rc;
+    if ((last == VB_STAGE_ID_FINE || vb_texture_key(d.dev)) && (rc = pick_out(r, &d))) return rc;
     if ((rc = enqueue(r, first, last, d, true))) return rc;
     CK(cudaStreamSynchronize(r->stream));
     return VB_OK;

@@ -6,6 +6,7 @@
 #include <algorithm>
 
 #include "vb_renderer.h"
+#include "vb_textures.h"
 
 // ---- CUDA IPC helpers (one process per GPU: the frame buffer of rank 0 mapped into the other ranks) ----------------------
 extern "C" int vb_frame_alloc(vb_renderer *r, size_t bytes, void **device_ptr) {
@@ -277,6 +278,10 @@ extern "C" int vb_group_scene_upload(vb_group *g, const uint8_t *scene, size_t s
 // out: nullptr (group frame), a device pointer on devices[0], or (host_out) a host pointer
 static int group_render(vb_group *g, const vb_params *p, void *out_device, void *host_out, vb_frame_stats *stats) {
     if (!g || !p || p->bin_row1 > p->bin_row0 || p->tile_row1 > p->tile_row0) return VB_E_INVALID;
+    if (vb_texture_key(out_device) || vb_texture_key(host_out)) {
+        g->err = "a vb_group renders into plain host or device pointers, not into registered destinations or texture keys";
+        return VB_E_INVALID;
+    }
     const size_t n = g->subs.size();
     const uint32_t ht = (p->height + 15u) / 16u;
     if (g->exchange && ht < n) {

@@ -42,12 +42,26 @@ enum { ARENA_LINES, ARENA_BINNING, ARENA_TILES, ARENA_SEG_COUNTS, ARENA_SEGMENTS
 static_assert(offsetof(VbConfig, ptcl_size) - offsetof(VbConfig, lines_size) == (N_ARENAS - 1) * sizeof(uint32_t),
               "VbConfig's arena sizes are consecutive words in ARENA_* order");
 
-// Where a frame's pixels go: a device pointer, or the renderer's own target (target_alt when `alt`), and optionally a copy of
-// the frame in host memory, read back in `bands` row bands while fine runs.
+// Where a frame's pixels go: a device pointer, a registered destination's key, or the renderer's own target (target_alt when
+// `alt`), and optionally a copy of the frame in host memory, read back in `bands` row bands while fine runs. `out` is where
+// fine stores, set from `dev` for each attempt by pick_out (dev itself stays the identity of the destination: the graph key's
+// and damage tracking's).
 struct Dest {
     void *dev = nullptr, *host = nullptr;
     bool alt = false;
     uint32_t bands = 1;
+    VbFineOut out{};
+};
+
+// A registered destination (vb_register_destination), found by its key in vb_renderer::dests. LINEAR: pixel (x, y) of a frame
+// at ptr + y * pitch + 4 * x. ARRAY: at texel (x + x0, y + y0) of a w x h array, written through surf.
+struct Destination {
+    uint32_t kind = VB_DEST_LINEAR, format = VB_DEST_RGBA8;
+    uint8_t *ptr = nullptr;
+    size_t pitch = 0;
+    cudaSurfaceObject_t surf = 0;
+    uint32_t x0 = 0, y0 = 0;
+    size_t w = 0, h = 0;
 };
 
 // key of a captured frame: the inputs of its launches (see enqueue)
@@ -179,6 +193,7 @@ struct vb_renderer {
         uint32_t w, h;
     };
     std::unordered_map<const void *, Override> overrides;
+    std::unordered_map<const void *, Destination> dests; // by key
     DevBuf blit_rects;                  // k_atlas_blit's rectangles, staged through pinned[PIN_BLITS]
     PinnedStage pinned[N_PINNED];
     // bump arenas (ARENAS), capacities in elements
@@ -416,6 +431,8 @@ int view_of(const double *affine, View *v);
 
 // vb_upload.cu
 void drop_registrations(vb_renderer *r);
+// a registered destination's key: where fine stores (d->out), after the frame-time checks
+int resolve_destination(vb_renderer *r, Dest *d);
 void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed);
 // diff: the upload may be diffed against the base frame's scene (vb_set_upload_diff); not for streamed frames

@@ -1475,6 +1475,8 @@ int vb_unregister_texture(vb_renderer *r, const vb_image *image) {
 }
 
 int vb_render_scene(vb_renderer *r, vb_scene *s, const vb_params *p, void *out, uint32_t out_is_device, vb_frame_stats *stats) {
+    // a key as the host destination: vb_render_uploaded refuses it (with its message) before anything is uploaded
+    if (!out_is_device && vb_texture_key(out)) return vb_render_uploaded(r, p, out, out_is_device, stats);
     const int rc = vb_scene_upload_device(r, s, nullptr);
     if (rc) return rc;
     return vb_render_uploaded(r, p, out, out_is_device, stats);

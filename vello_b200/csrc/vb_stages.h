@@ -123,10 +123,19 @@ uint32_t vb_launch_backdrop(const VbConfig &cfg, const VbFrameBufs &b, cudaStrea
 uint32_t vb_backdrop_parts(uint32_t tiles_size);
 uint32_t vb_launch_coarse(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_path_tiling(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
-// tile rows cfg.win_ty0..win_ty1 into `out`; `band` picks the launch's tile queue (one of 8 control-block words) and
+// Where fine stores a frame. Without `dst`: RGBA8 at `out`, cfg.out_pitch_px pixels a row, frame row cfg.out_row0 at out[0].
+// With `dst` (a registered destination in BGRA8 order or in a CUDA array; the FI_DST instantiations): each pixel's bytes are
+// permuted by __byte_perm selector `swz`, then stored as without `dst`, or with `array` through `surf`, frame pixel (x, y) at
+// texel (x0 + x, y0 + y).
+struct VbFineOut {
+    uint32_t *out;
+    cudaSurfaceObject_t surf;
+    uint32_t dst, swz, array, x0, y0;
+};
+// tile rows cfg.win_ty0..win_ty1 into `o`; `band` picks the launch's tile queue (one of 8 control-block words) and
 // cls_order starts the tiles in coarse's cost order
-uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, uint32_t *out, int aa, uint32_t cull, uint32_t band, bool cls_order,
-                        cudaStream_t st);
+uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, int aa, uint32_t cull, uint32_t band,
+                        bool cls_order, cudaStream_t st);
 int vb_fine_init_constants(void);
 
 // multi-GPU exchange: send = everything up to raising my flags, recv = wait for the peers, combine the boxes, pull my lines

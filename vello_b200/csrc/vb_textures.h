@@ -8,7 +8,8 @@
 #include "../../include/vello_b200.h"
 
 extern "C" {
-// nonzero for a key vb_texture_register handed out (an address no host buffer has: the host resolve never reads through it)
+// nonzero for an address of the reserved key range, from which vb_texture_register and vb_register_destination take their
+// keys (no host buffer has such an address: the host resolve never reads through it)
 int vb_texture_key(const void *key);
 // Renderer::register_texture / unregister_texture; vb_register_texture / vb_unregister_texture (vb_scene.cpp) wrap them
 int vb_texture_register(vb_renderer *r, const void *device_pixels, uint32_t width, uint32_t height, size_t row_pitch_bytes, const void **key_out);

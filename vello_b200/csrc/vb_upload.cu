@@ -11,12 +11,18 @@
 #include "vb_resolve.h"
 #include "vb_textures.h"
 
-// Keys of registered textures (vb_register_texture). Each is a fresh address inside one reserved, inaccessible (PROT_NONE)
-// range of the process's address space, so no host buffer can have it, even after the texture is unregistered: the host
-// resolve recognises such a key by its address alone and never reads through it (vb_texture_key). The range is never
-// unmapped and a key is never handed out twice. `owner` is the renderer that registered the key.
+// Keys of registered textures (vb_register_texture) and destinations (vb_register_destination). Each is a fresh address inside
+// one reserved, inaccessible (PROT_NONE) range of the process's address space, so no host or device buffer can have it, even
+// after it is unregistered: the host resolve recognises such a key by its address alone and never reads through it
+// (vb_texture_key), and the entry points that take a plain host or device pointer refuse it. The range is never unmapped and a
+// key is never handed out twice. `g_key_owner` holds the renderer that registered each key and what kind of key it is.
+enum { KEY_TEXTURE, KEY_DESTINATION };
+struct KeyOwner {
+    vb_renderer *r;
+    int kind;
+};
 static std::mutex g_tex_mutex;
-static std::unordered_map<const void *, vb_renderer *> g_tex_owner;
+static std::unordered_map<const void *, KeyOwner> g_key_owner;
 static uint8_t *g_tex_base = nullptr;
 static size_t g_tex_next = 0;
 static const size_t TEX_KEY_STRIDE = 16, TEX_RANGE_BYTES = (size_t)1 << 30;
@@ -25,7 +31,7 @@ extern "C" int vb_texture_key(const void *key) { // for vb_scene.cpp's host reso
     const uint8_t *p = (const uint8_t *)key, *base = __atomic_load_n(&g_tex_base, __ATOMIC_ACQUIRE);
     return base != nullptr && p >= base && p < base + TEX_RANGE_BYTES;
 }
-static const void *new_texture_key(vb_renderer *owner) {
+static const void *new_key(vb_renderer *owner, int kind) {
     std::lock_guard<std::mutex> lock(g_tex_mutex);
     if (!g_tex_base) {
         void *m = mmap(nullptr, TEX_RANGE_BYTES, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
@@ -35,12 +41,23 @@ static const void *new_texture_key(vb_renderer *owner) {
     if (g_tex_next + TEX_KEY_STRIDE > TEX_RANGE_BYTES) return nullptr;
     const void *key = g_tex_base + g_tex_next;
     g_tex_next += TEX_KEY_STRIDE;
-    g_tex_owner[key] = owner;
+    g_key_owner[key] = KeyOwner{owner, kind};
     return key;
 }
-void vb_host::drop_registrations(vb_renderer *r) {
+// Forget `key` if it is a key of `kind` that r registered.
+static bool drop_key(vb_renderer *r, const void *key, int kind) {
     std::lock_guard<std::mutex> lock(g_tex_mutex);
-    for (auto it = g_tex_owner.begin(); it != g_tex_owner.end();) it = it->second == r ? g_tex_owner.erase(it) : std::next(it);
+    auto it = vb_texture_key(key) ? g_key_owner.find(key) : g_key_owner.end();
+    if (it == g_key_owner.end() || it->second.r != r || it->second.kind != kind) return false;
+    g_key_owner.erase(it);
+    return true;
+}
+void vb_host::drop_registrations(vb_renderer *r) {
+    for (auto &d : r->dests)
+        if (d.second.surf) cudaDestroySurfaceObject(d.second.surf);
+    r->dests.clear();
+    std::lock_guard<std::mutex> lock(g_tex_mutex);
+    for (auto it = g_key_owner.begin(); it != g_key_owner.end();) it = it->second.r == r ? g_key_owner.erase(it) : std::next(it);
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
@@ -201,6 +218,7 @@ static int check_device_pixels(vb_renderer *r, const void *px, uint32_t w, uint3
         return VB_E_INVALID;
     };
     if (!w || !h) return bad("a dimension is 0");
+    if (vb_texture_key(px)) return bad("a texture or destination key is not device memory");
     if (((uintptr_t)px & 3u) || (pitch & 3u)) return bad("the pointer and the row pitch must be multiples of 4 bytes");
     if (pitch < (size_t)w * 4u) return bad("the row pitch is less than 4 * width");
     cudaPointerAttributes a;
@@ -311,7 +329,7 @@ extern "C" int vb_texture_register(vb_renderer *r, const void *device_pixels, ui
     CK(cudaSetDevice(r->device));
     int rc = check_device_pixels(r, device_pixels, width, height, row_pitch_bytes);
     if (rc) return rc;
-    const void *key = new_texture_key(r);
+    const void *key = new_key(r, KEY_TEXTURE);
     if (!key) {
         r->err = "vb_register_texture: no texture key left";
         return VB_E_INVALID;
@@ -323,16 +341,118 @@ extern "C" int vb_texture_register(vb_renderer *r, const void *device_pixels, ui
 
 extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
     if (!r) return VB_E_INVALID;
-    {
-        std::lock_guard<std::mutex> lock(g_tex_mutex);
-        auto it = vb_texture_key(key) ? g_tex_owner.find(key) : g_tex_owner.end();
-        if (it == g_tex_owner.end() || it->second != r) {
-            r->err = "vb_unregister_texture: not a texture registered on this renderer";
-            return VB_E_INVALID;
-        }
-        g_tex_owner.erase(it);
+    if (!drop_key(r, key, KEY_TEXTURE)) {
+        r->err = "vb_unregister_texture: not a texture registered on this renderer";
+        return VB_E_INVALID;
     }
     return vb_override_image(r, key, 0, 0, nullptr, 0);
+}
+
+// ---- registered destinations: vb_register_destination / vb_unregister_destination ------------------------------------------
+// Frames into a destination's key store through k_fine's FI_DST instantiations, except linear RGBA8, which is the default store
+// at another pitch and origin. Every check is made here or in resolve_destination, on the host, before a frame is enqueued.
+extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, void **key_out) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_register_destination: ") + why;
+        return VB_E_INVALID;
+    };
+    if (!d || !key_out) return bad("NULL destination or key_out");
+    if (d->kind != VB_DEST_LINEAR && d->kind != VB_DEST_ARRAY) return bad("unknown kind");
+    if (d->format != VB_DEST_RGBA8 && d->format != VB_DEST_BGRA8) return bad("unknown format");
+    if (r->grouped || r->xc.configured) return bad("not available for a renderer of a vb_group or with the exchange configured");
+    CK(cudaSetDevice(r->device));
+    Destination D;
+    D.kind = d->kind;
+    D.format = d->format;
+    if (d->kind == VB_DEST_LINEAR) {
+        if (!d->ptr) return bad("NULL ptr");
+        if ((uintptr_t)d->ptr & 3u) return bad("ptr is not 4-byte aligned");
+        if (vb_texture_key(d->ptr) || !device_memory_of(r, d->ptr)) return bad("ptr is not device or managed memory of the renderer's device");
+        if (d->row_pitch_bytes & 3u) return bad("row_pitch_bytes is not a multiple of 4");
+        if (d->row_pitch_bytes >= ((size_t)1 << 34)) return bad("row_pitch_bytes is 2^34 or more");
+        D.ptr = (uint8_t *)d->ptr;
+        D.pitch = d->row_pitch_bytes;
+    } else {
+        if (!d->array) return bad("NULL array");
+        cudaChannelFormatDesc fd;
+        cudaExtent ext;
+        unsigned int flags = 0;
+        if (cudaArrayGetInfo(&fd, &ext, &flags, (cudaArray_t)d->array) != cudaSuccess) {
+            cudaGetLastError();
+            return bad("not a CUDA array");
+        }
+        if (ext.depth != 0 || ext.height == 0 || (flags & (cudaArrayLayered | cudaArrayCubemap)))
+            return bad("a 1-D, layered, cubemap or 3-D array (a 2-D array is needed)");
+        if (fd.f != cudaChannelFormatKindUnsigned || fd.x != 8 || fd.y != 8 || fd.z != 8 || fd.w != 8)
+            return bad("the array's channels are not four 8-bit unsigned ones");
+        if (!(flags & cudaArraySurfaceLoadStore)) return bad("the array was not created with cudaArraySurfaceLoadStore");
+        cudaResourceDesc rd;
+        memset(&rd, 0, sizeof rd);
+        rd.resType = cudaResourceTypeArray;
+        rd.res.array.array = (cudaArray_t)d->array;
+        CK(cudaCreateSurfaceObject(&D.surf, &rd));
+        D.x0 = d->x;
+        D.y0 = d->y;
+        D.w = ext.width;
+        D.h = ext.height;
+    }
+    const void *key = new_key(r, KEY_DESTINATION);
+    if (!key) {
+        if (D.surf) cudaDestroySurfaceObject(D.surf);
+        return bad("no key left");
+    }
+    r->dests[key] = D;
+    *key_out = (void *)key;
+    return VB_OK;
+}
+
+extern "C" int vb_unregister_destination(vb_renderer *r, void *key) {
+    if (!r) return VB_E_INVALID;
+    auto it = r->dests.find(key);
+    if (it == r->dests.end()) {
+        r->err = "vb_unregister_destination: not a destination registered on this renderer";
+        return VB_E_INVALID;
+    }
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream)); // the frames enqueued into it
+    if (it->second.surf) CK(cudaDestroySurfaceObject(it->second.surf));
+    r->dests.erase(it);
+    drop_key(r, key, KEY_DESTINATION);
+    return VB_OK;
+}
+
+// The frame r prepared goes to d->dev, a key: check that the frame fits the destination, and say where fine stores (d->out).
+// A linear destination holds the whole frame, so a window's rows land at their own rows: out[0] is the window's first row.
+int vb_host::resolve_destination(vb_renderer *r, Dest *d) {
+    auto bad = [&](const char *why) {
+        r->err = std::string("registered destination: ") + why;
+        return VB_E_INVALID;
+    };
+    const auto it = r->dests.find(d->dev);
+    if (it == r->dests.end()) return bad("the key is not a destination registered on this renderer");
+    if (d->host) return bad("a key is not host memory");
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    VbConfig &c = r->cfg;
+    if (c.n_cells > 1u) return bad("a batch (vb_set_cells with more than one cell) cannot render into a registered destination");
+    const Destination &D = it->second;
+    VbFineOut o{};
+    o.swz = D.format == VB_DEST_BGRA8 ? 0x3012u : 0x3210u;
+    o.dst = D.format == VB_DEST_BGRA8 || D.kind == VB_DEST_ARRAY;
+    if (D.kind == VB_DEST_LINEAR) {
+        if (D.pitch < (size_t)c.target_width * 4u) return bad("the row pitch is below 4 * width");
+        c.out_pitch_px = (uint32_t)(D.pitch / 4u);
+        o.out = (uint32_t *)(D.ptr + (size_t)c.out_row0 * D.pitch);
+    } else {
+        if ((uint64_t)D.x0 + c.target_width > D.w || (uint64_t)D.y0 + fine_rows(c, *d).y1 > D.h)
+            return bad("the frame does not fit the array at its origin");
+        o.surf = D.surf;
+        o.array = 1u;
+        o.x0 = D.x0;
+        o.y0 = D.y0;
+    }
+    d->out = o;
+    return VB_OK;
 }
 
 // ---- batches: many scenes of one size in one pass (vb_scene_batch builds the scene) ---------------------------------------

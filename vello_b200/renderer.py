@@ -69,6 +69,11 @@ class _Instance(C.Structure):
     _fields_ = [("fragment", C.c_uint32), ("has_transform", C.c_uint32), ("transform", C.c_double * 6)]
 
 
+class _Destination(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("format", C.c_uint32), ("ptr", C.c_void_p), ("row_pitch_bytes", C.c_size_t),
+                ("array", C.c_void_p), ("x", C.c_uint32), ("y", C.c_uint32)]
+
+
 class FrameStats(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("failed", "binning", "ptcl", "tile", "seg_counts", "segments", "blend", "lines",
                                           "retries", "kernel_launches")] + \
@@ -172,6 +177,8 @@ def load_library() -> C.CDLL:
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
     lib.vb_last_damage.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_uint32)]
+    lib.vb_register_destination.argtypes = [vp, C.POINTER(_Destination), C.POINTER(vp)]
+    lib.vb_unregister_destination.argtypes = [vp, vp]
     _lib = lib
     return lib
 
@@ -186,12 +193,13 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
                     "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
-                    "vb_recompose", "vb_set_upload_diff"]
+                    "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination"]
 
 
 def _device_image(t):
     """(pointer, height, width, row pitch in bytes) of an (H, W, 4) uint8 array in device memory, from its
-    `__cuda_array_interface__` (a torch CUDA tensor, or a slice of one): texels 4 bytes apart, rows any multiple of 4 apart."""
+    `__cuda_array_interface__` (a torch CUDA tensor, or a slice of one): texels 4 bytes apart, rows any multiple of 4 apart.
+    Device images and linear destinations (`Renderer.register_destination`) are read this way."""
     cai = getattr(t, "__cuda_array_interface__", None)
     if cai is None:
         raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: a device image is needed")
@@ -287,6 +295,7 @@ class Renderer:
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
         self._bound = None  # the device array of bind_instance_transforms
+        self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
 
     @classmethod
@@ -297,6 +306,7 @@ class Renderer:
         r._owner = owner
         r._device_images = {}
         r._fragment_pixels = {}
+        r._destinations = {}
         r._bound = None
         r._frame_size = None
         return r
@@ -565,6 +575,39 @@ class Renderer:
         if bin_rows[1] > bin_rows[0]:
             return min(bin_rows[0] * 256, params.height), min(bin_rows[1] * 256, params.height)
         return 0, params.height
+
+    DEST_FORMATS = {"rgba8": 0, "bgra8": 1}
+
+    def register_destination(self, target=None, *, array=None, format: str = "rgba8", origin=(0, 0)) -> int:
+        """Register where frames can be rendered straight to (`vb_register_destination`) and return its key, which goes
+        wherever `out_device_ptr` goes (`render_resident`, `enqueue`, `run_stages`).
+
+        `target`: an (H, W, 4) uint8 device array (`__cuda_array_interface__`: a torch CUDA tensor, or a slice of a larger
+        one) with strides (pitch, 4, 1); pixel (x, y) of a frame lands at element [y, x]. It must hold the frames rendered
+        into it: the row pitch is checked at each frame, the rows are the caller's to provide. `array`: an integer
+        `cudaArray_t` handle of a 2-D array of four 8-bit unsigned channels created with `cudaArraySurfaceLoadStore` (such as
+        level 0 of an imported Vulkan image); pixel (x, y) lands at texel (origin[0] + x, origin[1] + y), and a frame that
+        does not fit is refused. `format`: "rgba8" (vello's byte order) or "bgra8". A bin_row / tile_row window writes its
+        rows at their own rows. Damage-tracked frames into the same key are incremental."""
+        fmt = self.DEST_FORMATS.get(format)
+        if fmt is None:
+            raise ValueError(f"register_destination: format is one of {sorted(self.DEST_FORMATS)}, not {format!r}")
+        if (target is None) == (array is None):
+            raise ValueError("register_destination: give either a target or an array")
+        if target is not None:
+            ptr, _, _, pitch = _device_image(target)
+            d = _Destination(0, fmt, ptr, pitch, None, 0, 0)
+        else:
+            d = _Destination(1, fmt, None, 0, int(array), int(origin[0]), int(origin[1]))
+        key = C.c_void_p()
+        self._check(self.lib.vb_register_destination(self.handle, C.byref(d), C.byref(key)), "vb_register_destination")
+        self._destinations[int(key.value)] = target
+        return int(key.value)
+
+    def unregister_destination(self, key: int):
+        """Unregister a destination (`vb_unregister_destination`), once the frames enqueued into it have completed."""
+        self._check(self.lib.vb_unregister_destination(self.handle, C.c_void_p(key)), "vb_unregister_destination")
+        self._destinations.pop(int(key), None)
 
     def render_resident(self, params: RenderParams, out_device_ptr: int = 0, bin_rows=(0, 0), tile_rows=(0, 0)) -> FrameStats:
         """Render the uploaded scene into a device buffer (0 = the renderer's own target)."""
