@@ -3,8 +3,9 @@
 // Reference: vello_shaders/shader/binning.wgsl:55-203, CPU twin cpu/binning.rs.
 // Output layout is the reference's: draw_bboxes[draw], bin_headers[partition][bin]{count,offset},
 // bin_data (appended after `info` in info_bin_data). Within one (partition, bin) chunk the draw
-// indices are ascending; chunk offsets come from an atomic bump allocator (as in the WGSL), so
-// chunk ORDER in bin_data is not deterministic -- consumers only go through the headers.
+// indices are ascending; chunk offsets come from an atomic bump allocator (as in the WGSL, but one
+// allocation per partition and bin block, with its chunks in bin order), so chunk ORDER in bin_data is
+// not deterministic -- consumers only go through the headers.
 // Extension: the bin-row window [win_by0, win_by1) restricts binning to this GPU's stripe.
 #include "vb_device.cuh"
 #include "vb_stages.h"
@@ -20,6 +21,7 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
     __shared__ uint32_t sh_bitmaps[BN_N_SLICE][VB_N_TILE];
     __shared__ uint32_t sh_count[BN_N_SUBSLICE][VB_N_TILE];
     __shared__ uint32_t sh_chunk_offset[VB_N_TILE];
+    __shared__ uint32_t sh_scan[BN_THREADS / 32 + 1];
     const uint32_t lid = threadIdx.x;
     for (int i = 0; i < BN_N_SLICE; i++) sh_bitmaps[i][lid] = 0u;
     if (bump->failed & VB_STAGE_FLATTEN) return; // uniform
@@ -83,13 +85,16 @@ k_binning(VbConfig cfg, const VbDrawMonoid *__restrict__ draw_monoids, const VbP
             element_count += __popc(sh_bitmaps[i * 2u + 1u][lid]);
             sh_count[i][lid] = lo | (element_count << 16);
         }
-        uint32_t chunk_offset = 0u;
-        if (element_count != 0u) {
-            chunk_offset = atomicAdd(&bump->binning, element_count);
-            if (chunk_offset + element_count > cfg.binning_size) {
-                chunk_offset = 0u;
-                atomicOr(&bump->failed, VB_STAGE_BINNING);
-            }
+        // the block's chunks are one allocation, laid out in bin order: one atomic per block instead of one per bin on the
+        // same counter (a block of map-like draws reaches most of its 256 bins)
+        uint32_t block_total;
+        uint32_t chunk_offset = vb_block_excl_scan(element_count, sh_scan, &block_total);
+        if (lid == 0u) sh_scan[0] = block_total != 0u ? atomicAdd(&bump->binning, block_total) : 0u;
+        __syncthreads();
+        chunk_offset = element_count != 0u ? sh_scan[0] + chunk_offset : 0u;
+        if (element_count != 0u && chunk_offset + element_count > cfg.binning_size) {
+            chunk_offset = 0u;
+            atomicOr(&bump->failed, VB_STAGE_BINNING);
         }
         sh_chunk_offset[lid] = chunk_offset;
         const uint32_t header_ix = blockIdx.x * aligned_n_bins + cur_bin_ix;

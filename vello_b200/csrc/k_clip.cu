@@ -136,18 +136,35 @@ __global__ void k_clip_bbox(uint32_t n_clips, const VbClipInp *__restrict__ clip
 }
 
 extern "C" uint32_t vb_clip_parts(uint32_t n_clips) { return (n_clips + CL_THREADS - 1u) / CL_THREADS; }
-extern "C" uint32_t vb_launch_clip(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+// clip_scratch: B | min32 | min1024 | link
+struct ClScratch {
+    int32_t *B, *min32, *min1024, *link;
+};
+static ClScratch cl_scratch(const VbFrameBufs &b, uint32_t n_clips) {
+    ClScratch s;
+    s.B = b.clip_scratch;
+    s.min32 = s.B + n_clips;
+    s.min1024 = s.min32 + (n_clips + 31) / 32;
+    s.link = s.min1024 + (n_clips + 1023) / 1024;
+    return s;
+}
+// the depth scan and the links: they read only draw's clip_inp, so they may run beside flatten
+extern "C" uint32_t vb_launch_clip_links(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
     const uint32_t n_clips = cfg.layout.n_clips;
     if (n_clips == 0) return 0;
-    int32_t *B = b.clip_scratch; // B | min32 | min1024 | link
-    int32_t *min32 = B + n_clips;
-    int32_t *min1024 = min32 + (n_clips + 31) / 32;
-    int32_t *link = min1024 + (n_clips + 1023) / 1024;
+    const ClScratch s = cl_scratch(b, n_clips);
     const uint32_t n_parts = vb_clip_parts(n_clips);
-    k_clip_depth<<<n_parts, CL_THREADS, 0, st>>>(n_clips, b.clip_inp, B, min32, min1024, b.lb_clip, n_parts);
-    k_clip_link<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, B, min32, min1024, link);
-    k_clip_bbox<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, b.path_bboxes, link, b.draw_monoids, b.clip_bboxes);
-    return 3;
+    k_clip_depth<<<n_parts, CL_THREADS, 0, st>>>(n_clips, b.clip_inp, s.B, s.min32, s.min1024, b.lb_clip, n_parts);
+    k_clip_link<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, s.B, s.min32, s.min1024, s.link);
+    return 2;
+}
+// the boxes: they read flatten's path boxes too
+extern "C" uint32_t vb_launch_clip_bboxes(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    const uint32_t n_clips = cfg.layout.n_clips;
+    if (n_clips == 0) return 0;
+    const ClScratch s = cl_scratch(b, n_clips);
+    k_clip_bbox<<<(n_clips + 255) / 256, 256, 0, st>>>(n_clips, b.clip_inp, b.path_bboxes, s.link, b.draw_monoids, b.clip_bboxes);
+    return 1;
 }
 extern "C" size_t vb_clip_scratch_words(uint32_t n_clips) {
     return (size_t)n_clips * 2 + (n_clips + 31) / 32 + (n_clips + 1023) / 1024 + 8;

@@ -64,7 +64,7 @@ __device__ __forceinline__ void put_xform(uint32_t *info, const DXform &x) {
 }
 
 __global__ void __launch_bounds__(DR_THREADS)
-k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const VbPathBbox *__restrict__ path_bbox, VbDrawMonoid *draw_monoid,
+k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const uint2 *__restrict__ path_draw, VbDrawMonoid *draw_monoid,
        uint32_t *info, VbClipInp *clip_inp, uint32_t *lb_mem, uint32_t n_parts) {
     __shared__ uint32_t sh_ticket;
     __shared__ uint32_t sh_warp[4][DR_THREADS / 32];
@@ -118,11 +118,10 @@ k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const VbPathBbox *__res
     if (tag_word == VB_DRAWTAG_FILL_COLOR || tag_word == VB_DRAWTAG_FILL_LIN_GRADIENT || tag_word == VB_DRAWTAG_FILL_RAD_GRADIENT ||
         tag_word == VB_DRAWTAG_FILL_SWEEP_GRADIENT || tag_word == VB_DRAWTAG_FILL_IMAGE || tag_word == VB_DRAWTAG_BEGIN_CLIP ||
         tag_word == VB_DRAWTAG_BLURRED_ROUNDED_RECT) {
-        VbPathBbox bbox = path_bbox[m.path_ix];
-        const uint32_t draw_flags = bbox.draw_flags;
-        info[di] = draw_flags;
+        const uint2 pd = path_draw[m.path_ix]; // {style_ix, trans_ix}: the draw flags are the style's fill rule (fl_open_path)
+        info[di] = (vb_scene(scene, cfg, cfg.layout.style_base + pd.x) & STYLE_FLAGS_FILL) == 0u ? 0u : 1u;
         if (tag_word != VB_DRAWTAG_FILL_COLOR && tag_word != VB_DRAWTAG_BEGIN_CLIP) {
-            DXform transform = dx_read(cfg, scene, bbox.trans_ix);
+            DXform transform = dx_read(cfg, scene, pd.y);
             switch (tag_word) {
             case VB_DRAWTAG_FILL_LIN_GRADIENT: {
                 float p0x, p0y, p1x, p1y;
@@ -236,7 +235,7 @@ k_draw(VbConfig cfg, const uint32_t *__restrict__ scene, const VbPathBbox *__res
 
 extern "C" uint32_t vb_launch_draw(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
     if (b.parts_draw == 0) return 0;
-    k_draw<<<b.parts_draw, DR_THREADS, 0, st>>>(cfg, b.scene, b.path_bboxes, b.draw_monoids, b.info_bin_data, b.clip_inp, b.lb_draw, b.parts_draw);
+    k_draw<<<b.parts_draw, DR_THREADS, 0, st>>>(cfg, b.scene, b.path_draw, b.draw_monoids, b.info_bin_data, b.clip_inp, b.lb_draw, b.parts_draw);
     return 1;
 }
 extern "C" uint32_t vb_draw_parts(uint32_t n_draw) { return (n_draw + DR_THREADS - 1) / DR_THREADS; }

@@ -573,7 +573,6 @@ __device__ void flatten_arc(F &f, fv2 begin, fv2 end, fv2 center, float angle, c
 }
 
 #define STYLE_FLAGS_STYLE 0x80000000u
-#define STYLE_FLAGS_FILL 0x40000000u
 #define STYLE_MITER_LIMIT_MASK 0xFFFFu
 #define STYLE_FLAGS_START_CAP_MASK 0x0C000000u
 #define STYLE_FLAGS_END_CAP_MASK 0x03000000u
@@ -992,6 +991,7 @@ __device__ __forceinline__ void fl_load_tag(PathTagData &tag, uint32_t &style_fl
         style_flags = vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix);
     }
 }
+// (draw does not read these: it finds the same style and transform through pathtag's path table, k_pathtag.cu)
 __device__ __forceinline__ void fl_open_path(const VbConfig &cfg, VbPathBbox *path_bboxes, const PathTagData &tag, uint32_t style_flags) {
     if ((tag.tag_byte & 0x10u) != 0u && tag.path_ix < cfg.layout.n_paths) {
         path_bboxes[tag.path_ix].draw_flags = (style_flags & STYLE_FLAGS_FILL) == 0u ? 0u : 1u;

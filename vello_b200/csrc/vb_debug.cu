@@ -57,6 +57,7 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
         {"atlas", &r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4},
         {"tag_monoids", &r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)},
         {"path_bboxes", &r->path_bboxes, (size_t)L.n_paths * sizeof(VbPathBbox)},
+        {"path_draw", &r->path_draw, (size_t)L.n_paths * 8u},
         {"draw_monoids", &r->draw_monoids, (size_t)L.n_draw_objects * sizeof(VbDrawMonoid)},
         {"clip_inp", &r->clip_inp, (size_t)L.n_clips * sizeof(VbClipInp)},
         {"clip_bboxes", &r->clip_bboxes, (size_t)L.n_clips * sizeof(VbBbox4)},

@@ -172,7 +172,9 @@ extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
         cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&r->tiling_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&r->tiling_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->draw_fork, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&r->draw_join, cudaEventDisableTiming) != cudaSuccess) {
         delete r;
         return VB_E_CUDA;
     }
@@ -249,6 +251,8 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
     if (r->tiling_stream) cudaStreamSynchronize(r->tiling_stream);
     if (r->tiling_fork) cudaEventDestroy(r->tiling_fork);
     if (r->tiling_join) cudaEventDestroy(r->tiling_join);
+    if (r->draw_fork) cudaEventDestroy(r->draw_fork);
+    if (r->draw_join) cudaEventDestroy(r->draw_join);
     if (r->tiling_stream) cudaStreamDestroy(r->tiling_stream);
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
     if (r->upload_stream) cudaStreamDestroy(r->upload_stream);
@@ -415,6 +419,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     int rc;
     if ((rc = ensure(r, r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)))) return rc;
     if ((rc = ensure(r, r->path_bboxes, (size_t)n_paths * sizeof(VbPathBbox)))) return rc;
+    if ((rc = ensure(r, r->path_draw, (size_t)n_paths * sizeof(uint2)))) return rc;
     if ((rc = ensure(r, r->draw_monoids, (size_t)n_draw * sizeof(VbDrawMonoid)))) return rc;
     if ((rc = ensure(r, r->clip_inp, (size_t)n_clips * sizeof(VbClipInp)))) return rc;
     if ((rc = ensure(r, r->clip_bboxes, (size_t)n_clips * sizeof(VbBbox4)))) return rc;
@@ -477,6 +482,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     }
     b.tag_monoids = (VbTagMonoid *)r->tag_monoids.p;
     b.path_bboxes = (VbPathBbox *)r->path_bboxes.p;
+    b.path_draw = (uint2 *)r->path_draw.p;
     b.draw_monoids = (VbDrawMonoid *)r->draw_monoids.p;
     b.info_bin_data = (uint32_t *)r->info_bin_data.p;
     b.clip_inp = (VbClipInp *)r->clip_inp.p;
@@ -573,6 +579,12 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
     // tiling stream and joined again before the next stage, so the two kernels share the GPU. Launch counts are unchanged;
     // with per-stage timing on, the stages stay serial so that each one's events time it alone.
     const bool fork_tiling = !r->timing && first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_PATH_TILING;
+    // draw reads pathtag's path table and the transforms, not flatten's output, and clip's depth scan and links read only
+    // draw's clip inputs: they are forked onto the tiling stream once the transforms are written, beside flatten, and
+    // joined before clip's boxes (which read the path boxes). Launch counts are unchanged. Serial with per-stage timing, with
+    // the exchange (draw waits for its second half) and for partial ranges: only whole frames fork, whose fine may follow
+    // separately (a host destination's bands after the captured graph).
+    const bool fork_draw = !r->timing && !r->xc.enabled && first == VB_STAGE_ID_PATHTAG && last >= VB_STAGE_ID_FINE - 1;
     rec(r, 0);
     for (int s = first; s <= last; s++) {
         switch (s) {
@@ -584,6 +596,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // bound ones first (the view's source), inside flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
+            if (fork_draw) {
+                CK(cudaEventRecord(r->draw_fork, st));
+                CK(cudaStreamWaitEvent(r->tiling_stream, r->draw_fork, 0));
+                launches += vb_launch_draw(c, b, r->tiling_stream);
+                launches += vb_launch_clip_links(c, b, r->tiling_stream);
+                CK(cudaEventRecord(r->draw_join, r->tiling_stream));
+            }
             VbConfig cf = c;
             uint32_t p0 = 0u, p1 = b.parts_flatten;
             if (r->xc.enabled) {
@@ -604,9 +623,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);
-            launches += vb_launch_draw(c, b, st);
+            if (fork_draw) CK(cudaStreamWaitEvent(st, r->draw_join, 0)); // launched beside flatten
+            else launches += vb_launch_draw(c, b, st);
             break;
-        case VB_STAGE_ID_CLIP: launches += vb_launch_clip(c, b, st); break;
+        case VB_STAGE_ID_CLIP:
+            if (!fork_draw) launches += vb_launch_clip_links(c, b, st); // else launched beside flatten
+            launches += vb_launch_clip_bboxes(c, b, st);
+            break;
         case VB_STAGE_ID_BINNING: launches += vb_launch_binning(c, b, st); break;
         case VB_STAGE_ID_TILE_ALLOC: launches += vb_launch_tile_alloc(c, b, st); break;
         case VB_STAGE_ID_PATH_COUNT: launches += vb_launch_path_count(c, b, st); break;

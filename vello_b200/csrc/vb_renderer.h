@@ -184,7 +184,7 @@ struct vb_renderer {
     DevBuf mask8, mask16;
 
     // fixed-size intermediates
-    DevBuf tag_monoids, path_bboxes, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
+    DevBuf tag_monoids, path_bboxes, path_draw, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
         ctl, target, target_alt, tile_start, cls_list;
     // Renderer::override_image: images (by key) whose pixels come from device memory at the device resolve
     struct Override {
@@ -224,9 +224,11 @@ struct vb_renderer {
     DevBuf view_coef;
     uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
     uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
-    // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct)
+    // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct). Earlier in
+    // the frame, draw and clip's links run on the same stream beside flatten: forked after the transforms, joined before clip's
+    // boxes (draw_fork / draw_join).
     cudaStream_t tiling_stream = nullptr;
-    cudaEvent_t tiling_fork = nullptr, tiling_join = nullptr;
+    cudaEvent_t tiling_fork = nullptr, tiling_join = nullptr, draw_fork = nullptr, draw_join = nullptr;
     cudaEvent_t ev[VB_N_STAGE_IDS + 1]{};
     cudaEvent_t frame_ev[2]{}; // around every whole frame (vb_last_frame_ms: the signal stripe balancing uses)
     bool frame_timed = false;
@@ -346,7 +348,7 @@ struct vb_renderer {
 // Every device buffer the renderer owns, each once: what vb_renderer_free frees and vb_frame_stats::arena_bytes counts.
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
-                           &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->draw_monoids, &r->info_bin_data, &r->clip_inp,
+                           &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->path_draw, &r->draw_monoids, &r->info_bin_data, &r->clip_inp,
                            &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,

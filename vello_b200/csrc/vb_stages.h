@@ -35,6 +35,7 @@ struct VbFrameBufs {
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
+    uint2 *path_draw; // per path: {style_ix, trans_ix}, written by pathtag for draw (what flatten's path_bboxes fields come from)
     VbDrawMonoid *draw_monoids;
     uint32_t *info_bin_data;
     VbClipInp *clip_inp;
@@ -112,7 +113,9 @@ size_t vb_flatten_part_words(uint32_t n_parts);
 void vb_flatten_arena_bytes(uint32_t cap_lines, size_t *lit_bytes, size_t *job_bytes);
 uint32_t vb_launch_draw(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_draw_parts(uint32_t n_draw);
-uint32_t vb_launch_clip(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+// clip in two launchers: the depth scan and the links read only draw's clip_inp, the boxes also the path boxes flatten writes
+uint32_t vb_launch_clip_links(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+uint32_t vb_launch_clip_bboxes(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_clip_parts(uint32_t n_clips);
 size_t vb_clip_scratch_words(uint32_t n_clips);
 uint32_t vb_launch_binning(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
