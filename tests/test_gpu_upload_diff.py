@@ -416,6 +416,40 @@ def test_full_frame_fallbacks(rr):
     assert r.last_stats.arena_bytes > 0
 
 
+def test_recompose_and_diffed_upload_without_a_frame_between(rr):
+    """A recompose and a diffed upload without a frame between them, in either order: the frame is full, and still exact."""
+    r, ref = rr
+    s = Diffed(r, ref)
+    g = np.random.default_rng(47)
+    items = rand_items(g, 60, [])
+    pa = resolve(build(items).encoding)
+    pb = recoloured(pa, colour_draws(pa)[3:4], g)
+    frags = [build(items[k:k + 10]) for k in range(0, 60, 10)]
+    ids, rids = [r.upload_fragment(f) for f in frags], [ref.upload_fragment(f) for f in frags]
+    moved_last = [(k, Affine.translate(6, 3) if k == 5 else None) for k in range(6)]
+
+    def compose(how, inst):
+        getattr(r, how)([(ids[k], t) for k, t in inst])
+        ref.compose([(rids[k], t) for k, t in inst])
+
+    def frame(what, full):
+        img, want = s.frame()
+        dmg = r.last_damage()
+        assert (img == want).all(), f"{what}: {int((img != want).any(axis=2).sum())} pixels differ from the full frame"
+        assert dmg.all() if full else not dmg.all(), f"{what}: expected {'a full' if full else 'an incremental'} frame"
+
+    compose("compose", [(k, None) for k in range(6)])
+    frame("composed", True)
+    compose("recompose", moved_last)
+    frame("a recompose alone", False)
+    compose("recompose", [(k, None) for k in range(6)])
+    s.step(pa, diffed=False, what="a recompose, then a diffed upload")
+    s.step(pb, what="a diffed upload alone")
+    s.upload(pa)
+    compose("recompose", moved_last)
+    frame("a diffed upload, then a recompose", True)
+
+
 # ---- overflow re-runs, hit tests, graphs ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("arena", ["ptcl", "segments"])
 def test_overflow_rerun_keeps_the_damage(rr, arena):

@@ -324,17 +324,8 @@ static CmpArgs stage_cmp_tables(const std::vector<const Fragment *> &fr, const C
     return a;
 }
 
-// vb_compose and vb_recompose. A recompose that damage tracking can follow (recompose_armed) also matches the instances
-// against the current scene's, stages the tables of k_recompose_damage and copies the base frame's draw boxes.
-static bool recompose_armed(const vb_renderer *r) {
-    const vb_renderer::Damage &D = r->dmg;
-    const vb_renderer::SceneSlot &s = *r->cur;
-    // the base rendered the current scene (no installation, binding, view, cells or tracking switch since: the epoch), unbound,
-    // and its draw boxes are intact (hit tests answer from it: no frame, failure, vb_run_stages or debug write since)
-    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && s.composed && !r->bound.rows && r->hit.valid &&
-           !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects &&
-           s.inst_draw.size() == s.inst_frag.size() + 1u && s.inst_img.size() == s.inst_frag.size() + 1u;
-}
+// vb_compose and vb_recompose. A recompose that damage tracking can follow (a composed base: base_diffable) also matches the
+// instances against the current scene's, and begins the diff (diff_begin) with the tables of k_recompose_damage.
 static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets,
                    bool recompose) {
     if (!r) return VB_E_INVALID;
@@ -432,8 +423,9 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     // vb_recompose: match the new instances to the current scene's (vb_diff.h). A matched instance whose images moved in the
     // atlas, or come from an override (copied again by this compose), is unmatched: fine samples in atlas coordinates.
     const vb_renderer::SceneSlot &was = *r->cur;
-    const bool arm = recompose && recompose_armed(r);
-    const uint32_t n_old = arm ? (uint32_t)was.inst_frag.size() : 0u, old_draws = arm ? was.layout.n_draw_objects : 0u;
+    const bool arm = recompose && was.composed && was.inst_draw.size() == was.inst_frag.size() + 1u &&
+                     was.inst_img.size() == was.inst_frag.size() + 1u && base_diffable(r);
+    const uint32_t n_old = arm ? (uint32_t)was.inst_frag.size() : 0u;
     std::vector<uint32_t> match(arm ? n : 0u), unmatched(n_old, 1u);
     if (arm) {
         vb_diff_match(
@@ -460,9 +452,8 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     // the tables, staged through pinned memory: k_compose_streams' (cmp_tables), patches, ramp descriptors
     const size_t o_pat = cmp_tables(n).bytes;
     const size_t o_ramp = up16(o_pat + patches.size() * sizeof(RsPatch)), staged = o_ramp + ramps.size() * sizeof(RsRamp);
-    // vb_recompose's tables (VbFrameBufs::rcmp_tables), staged after compose's, and where they go in rcmp: after the old boxes
-    const size_t o_rc = up16(staged), rc_bytes = arm ? ((size_t)n_old + 1u + n + 1u + n + n_old) * 4u : 0u;
-    const size_t o_tables = up16((size_t)old_draws * sizeof(VbBbox4)), host_bytes = o_rc + rc_bytes;
+    // vb_recompose's tables (VbFrameBufs::rcmp_tables), staged after compose's
+    const size_t o_rc = up16(staged), rc_bytes = arm ? ((size_t)n_old + 1u + n + 1u + n + n_old) * 4u : 0u, host_bytes = o_rc + rc_bytes;
     if ((rc = compose_room(r, r->compose_tmp, staged))) return rc;
     char *tmp = (char *)r->compose_tmp.p;
     PinnedStage &stage = r->pinned[PIN_COMPOSE];
@@ -479,16 +470,15 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
         memcpy(t + n_old + 1u, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
         if (n) memcpy(t + n_old + 1u + n + 1u, match.data(), (size_t)n * 4u);
         if (n_old) memcpy(t + n_old + 1u + n + 1u + n, unmatched.data(), (size_t)n_old * 4u);
-        if ((rc = compose_room(r, r->rcmp, o_tables + rc_bytes))) return rc;
     }
 
     if ((rc = compose_room(r, slot.scene, scene_bytes(L, total_words, r->view.on)))) return rc;
     if (new_ramps && (rc = compose_room(r, slot.ramps, ramps.size() * 512u * 4u))) return rc;
     if (new_atlas && (rc = compose_room(r, slot.atlas, (size_t)atlas_w * atlas_h * 4u))) return rc;
     if (staged) CK(cudaMemcpyAsync(tmp, h, staged, cudaMemcpyHostToDevice, st));
-    if (arm) { // the base frame's boxes, before anything can rewrite them, and the tables
-        if (old_draws) CK(cudaMemcpyAsync(r->rcmp.p, r->hit.bufs.draw_bboxes, (size_t)old_draws * sizeof(VbBbox4), cudaMemcpyDeviceToDevice, st));
-        CK(cudaMemcpyAsync((char *)r->rcmp.p + o_tables, h + o_rc, rc_bytes, cudaMemcpyHostToDevice, st));
+    if (arm) {
+        if ((rc = diff_begin(r, st, false, n_old, n, L.n_draw_objects))) return rc;
+        CK(cudaMemcpyAsync((char *)r->dmg_diff.p + r->dmg.diff.o_tables, h + o_rc, rc_bytes, cudaMemcpyHostToDevice, st));
     }
     if ((rc = stage_copied(r, stage))) return rc;
     uint32_t *scene = (uint32_t *)slot.scene.p;
@@ -518,16 +508,6 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     slot.inst_draw.assign(pre + (size_t)CMP_DRAW_TAGS * (n + 1u), pre + (size_t)(CMP_DRAW_TAGS + 1) * (n + 1u));
     slot.inst_img = std::move(img_pre);
     slot.img_place = std::move(img_place);
-    vb_renderer::Damage::Diff &X = r->dmg.diff;
-    X.armed = arm;
-    if (arm) { // the next frame of this installation's epoch is incremental (damage_prepare)
-        X.epoch = r->dmg.epoch;
-        X.n_old = n_old;
-        X.n_new = n;
-        X.old_draws = old_draws;
-        X.new_draws = L.n_draw_objects;
-        X.o_tables = o_tables;
-    }
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
@@ -536,7 +516,9 @@ extern "C" int vb_compose(vb_renderer *r, const vb_instance *inst, uint32_t n, v
     return compose(r, "vb_compose", inst, n, layout_out, draw_offsets, false);
 }
 extern "C" int vb_recompose(vb_renderer *r, const vb_instance *inst, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets) {
-    return compose(r, "vb_recompose", inst, n, layout_out, draw_offsets, true);
+    const int rc = compose(r, "vb_recompose", inst, n, layout_out, draw_offsets, true);
+    if (r) r->dmg.diff.pending = false; // a recompose that failed after diff_begin installed nothing: its diff must not be armed
+    return rc;
 }
 extern "C" uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t n_old, const uint32_t *new_keys, uint32_t n_new, uint32_t *match) {
     return vb_diff_match(n_old, n_new, [&](uint32_t i, uint32_t j) { return old_keys[i] == new_keys[j]; }, match);

@@ -29,10 +29,10 @@ int vb_host::damage_prepare(vb_renderer *r) {
     for (const auto &o : r->cur->overridden)
         if (o.dirty && !D.rects) D.force_full = true;
     const vb_renderer::DamageFrame &B = D.base;
-    const bool diff = D.diff.armed && D.diff.epoch == f.epoch; // the scene is a recompose of the base's (vb_recompose)
-    const bool udiff = D.udiff.armed && D.udiff.epoch == f.epoch; // an upload diffed against the base's scene (vb_set_upload_diff)
-    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff || udiff) && B.w == f.w &&
-                             B.h == f.h && B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
+    const vb_renderer::Damage::Diff &X = D.diff;
+    const bool diff = X.armed && X.epoch == f.epoch; // the scene was diffed against the base's (vb_recompose, vb_set_upload_diff)
+    const bool incremental = D.have_base && !D.force_full && !r->dest.host && (B.epoch == f.epoch || diff) && B.w == f.w && B.h == f.h &&
+                             B.aa == f.aa && B.base_color == f.base_color && B.dest == f.dest;
     f.mode = incremental ? VB_DMG_INCREMENTAL : VB_DMG_FULL;
     // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
     // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
@@ -56,23 +56,43 @@ int vb_host::damage_prepare(vb_renderer *r) {
     }
     b.dmg_mode = f.mode;
     b.dmg_n_xf = n_xf;
-    if (incremental && diff) {
-        b.rcmp_old_boxes = (const VbBbox4 *)r->rcmp.p;
-        b.rcmp_tables = (const uint32_t *)((const char *)r->rcmp.p + D.diff.o_tables);
-        b.rcmp_n_old = D.diff.n_old;
-        b.rcmp_n_new = D.diff.n_new;
-        b.rcmp_old_draws = D.diff.old_draws;
-        b.rcmp_new_draws = D.diff.new_draws;
-    }
-    if (incremental && udiff) { // one draw object per "instance" of k_recompose_damage's tables, which k_upload_diff.cu builds
-        const VbUdLayout U = vb_udiff_layout(D.udiff.n_old, D.udiff.n_new);
-        b.udiff = (VbUdiff *)r->udiff.p;
-        b.rcmp_old_boxes = (const VbBbox4 *)((const char *)r->udiff.p + U.boxes);
-        b.rcmp_tables = (const uint32_t *)((const char *)r->udiff.p + U.tables);
-        b.rcmp_n_old = b.rcmp_old_draws = D.udiff.n_old;
-        b.rcmp_n_new = b.rcmp_new_draws = D.udiff.n_new;
+    if (incremental && diff) { // k_recompose_damage's inputs; an upload's tables are built by the frame (k_upload_diff.cu)
+        const char *p = (const char *)r->dmg_diff.p;
+        if (X.upload) b.udiff = (VbUdiff *)r->dmg_diff.p;
+        b.rcmp_old_boxes = (const VbBbox4 *)(p + X.o_boxes);
+        b.rcmp_tables = (const uint32_t *)(p + X.o_tables);
+        b.rcmp_n_old = X.n_old;
+        b.rcmp_n_new = X.n_new;
+        b.rcmp_old_draws = X.old_draws;
+        b.rcmp_new_draws = X.new_draws;
     }
     D.frame = f;
+    return VB_OK;
+}
+
+// There is a tracked base frame of the current scene (the epoch unchanged since: no installation, binding, view, cells or
+// tracking switch), unbound, of one cell, whose intermediates are intact: hit tests answer from it (no failed frame,
+// vb_run_stages or debug write since).
+bool vb_host::base_diffable(const vb_renderer *r) {
+    const vb_renderer::Damage &D = r->dmg;
+    const vb_renderer::SceneSlot &s = *r->cur;
+    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !r->bound.rows && r->hit.valid && !r->hit.windowed &&
+           r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects;
+}
+
+// Size dmg_diff (an upload's laid out by vb_udiff_layout; a recompose's as [boxes] [tables, 16-byte aligned]), enqueue on st the
+// copy of the base frame's draw boxes, before anything can rewrite them, and mark the record pending for set_scene to arm.
+int vb_host::diff_begin(vb_renderer *r, cudaStream_t st, bool upload, uint32_t n_old, uint32_t n_new, uint32_t new_draws) {
+    const uint32_t old_draws = r->cur->layout.n_draw_objects;
+    const size_t box_bytes = (size_t)old_draws * sizeof(VbBbox4);
+    const VbUdLayout U = vb_udiff_layout(n_old, n_new);
+    const size_t o_boxes = upload ? U.boxes : 0u, o_tables = upload ? U.tables : (box_bytes + 15u) & ~(size_t)15u;
+    const size_t bytes = o_tables + ((size_t)n_old + 1u + n_new + 1u + n_new + n_old) * 4u; // k_recompose_damage's tables
+    if (r->dmg_diff.cap < bytes) CK(cudaStreamSynchronize(st)); // growing: copies enqueued into it may not have run yet
+    int rc;
+    if ((rc = ensure(r, r->dmg_diff, bytes))) return rc;
+    if (old_draws) CK(cudaMemcpyAsync((char *)r->dmg_diff.p + o_boxes, r->hit.bufs.draw_bboxes, box_bytes, cudaMemcpyDeviceToDevice, st));
+    r->dmg.diff = vb_renderer::Damage::Diff{true, false, upload, 0u, n_old, n_new, old_draws, new_draws, o_boxes, o_tables}; // pending
     return VB_OK;
 }
 // The frame prepared last succeeded: it is the one vb_last_damage reports, and the base of the next frame when it was tracked.
@@ -85,7 +105,6 @@ void vb_host::damage_succeeded(vb_renderer *r) {
     D.rects = false;
     D.force_full = false;
     D.diff.armed = false;
-    D.udiff.armed = false;
 }
 
 extern "C" int vb_set_damage_tracking(vb_renderer *r, int on) {

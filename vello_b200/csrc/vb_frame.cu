@@ -1072,7 +1072,6 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
     hit_forget(r);
     r->dmg.diff.armed = false; // the stages may write the destination: the frame after them is full
-    r->dmg.udiff.armed = false;
     CK(cudaSetDevice(r->device));
     int rc = prepare(r, p);
     if (rc) return rc;

@@ -308,30 +308,25 @@ struct vb_renderer {
         bool rects = false;      // vb_add_damage since the last successful frame (dirty overrides then do not force a full frame)
         bool force_full = false; // dirty overrides without rectangles: the frame and its re-runs are full
         DamageFrame base, frame, last; // frame: the one prepared last; last: the last successful one
-        // vb_recompose that tracking follows: the next frame of epoch `epoch` (the recompose's installation) is incremental
-        // against `base` and runs k_recompose_damage on the tables in rcmp; consumed when a frame succeeds
+        // A draw-object diff that tracking follows, of n_old instances (old_draws draw objects) of the base frame's scene against
+        // n_new (new_draws) of the next one: a vb_recompose, or with `upload` an upload under vb_set_upload_diff (one draw object
+        // per instance; the frame builds the tables, k_upload_diff.cu). `pending` from diff_begin until the installation
+        // (set_scene), then `armed` for the next frame of epoch `epoch`, which is incremental against `base` and runs
+        // k_recompose_damage on the base frame's boxes and the tables in dmg_diff; consumed when a frame succeeds.
         struct Diff {
-            bool armed = false;
+            bool pending = false, armed = false, upload = false;
             uint64_t epoch = 0;
             uint32_t n_old = 0, n_new = 0, old_draws = 0, new_draws = 0;
-            size_t o_tables = 0;
+            size_t o_boxes = 0, o_tables = 0;
         } diff;
-        // an upload that tracking follows (vb_set_upload_diff): `pending` from upload_diff_begin until the upload installs its
-        // scene (set_scene), then `armed` for the next frame of epoch `epoch`, which is incremental against `base` and runs
-        // k_upload_diff.cu on `udiff`; consumed when a frame succeeds
-        struct UploadDiff {
-            bool pending = false, armed = false;
-            uint64_t epoch = 0;
-            uint32_t n_old = 0, n_new = 0;
-        } udiff;
     } dmg;
     DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
-    DevBuf rcmp; // vb_recompose: [the base frame's draw boxes] [the tables, at dmg.diff.o_tables] (VbFrameBufs::rcmp_tables)
-    // upload diff (vb_set_upload_diff): the switch; the spare scene, ramps and atlas buffers an upload that tracking follows
-    // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set; and the diff's buffer
-    // (VbUdiff and vb_udiff_layout), whose head is written from ud_head
+    DevBuf dmg_diff; // the diff's buffer: [the base frame's draw boxes, at o_boxes] [the tables, at o_tables] (VbFrameBufs::rcmp_*)
+    // upload diff (vb_set_upload_diff): the switch; and the spare scene, ramps and atlas buffers an upload that tracking follows
+    // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set. The diff's buffer is laid
+    // out by vb_udiff_layout, behind a head (VbUdiff) written from ud_head.
     bool upload_diff = false;
-    DevBuf spare_scene, spare_ramps, spare_atlas, udiff;
+    DevBuf spare_scene, spare_ramps, spare_atlas;
     VbUdiff ud_head{};
 
     // multi-GPU exchange (flatten sharded by tag range; k_exchange.cu)
@@ -353,8 +348,8 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
                            &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
                            &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->rcmp, &r->spare_scene, &r->spare_ramps,
-                           &r->spare_atlas, &r->udiff};
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps,
+                           &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
 }
 
@@ -449,6 +444,11 @@ int image_source(vb_renderer *r, const char *who, const void *key, uint32_t w, u
 // vb_damage.cu
 int damage_prepare(vb_renderer *r);
 void damage_succeeded(vb_renderer *r);
+// Can the next installation be diffed against the scene the base frame rendered? What each diff source needs besides, it checks.
+bool base_diffable(const vb_renderer *r);
+// Begin the diff of the next installation (dmg.diff): n_old instances of the current scene's draw objects against n_new of
+// new_draws; with `upload`, one draw object per instance. The caller stages the tables, or an upload's head and records.
+int diff_begin(vb_renderer *r, cudaStream_t st, bool upload, uint32_t n_old, uint32_t n_new, uint32_t new_draws);
 
 } // namespace vb_host
 using namespace vb_host;

@@ -81,27 +81,15 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
     r->dmg.epoch++;
-    // an upload that tracking follows (upload_diff_begin) makes the next frame of this epoch incremental; anything else ends it
-    vb_renderer::Damage::UploadDiff &U = r->dmg.udiff;
-    U.armed = U.pending;
-    U.pending = false;
-    U.epoch = r->dmg.epoch;
+    // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
+    vb_renderer::Damage::Diff &X = r->dmg.diff;
+    X.armed = X.pending;
+    X.pending = false;
+    X.epoch = r->dmg.epoch;
     hit_forget(r);
 }
 
 // ---- upload diff: vb_set_upload_diff (k_upload_diff.cu) ----------------------------------------------------------------------
-// Can the frame after an upload diff it against the scene the base frame rendered? Tracking and the switch are on, and there
-// is a base frame of the current scene (the epoch unchanged since: no installation, binding, view, cells or tracking switch),
-// unbound, of one cell, whose intermediates are intact: hit tests answer from it (no failed frame, vb_run_stages or debug write
-// since). As recompose_armed (vb_compose.cu).
-static bool upload_diff_armed(const vb_renderer *r) {
-    const vb_renderer::Damage &D = r->dmg;
-    const vb_renderer::SceneSlot &s = *r->cur;
-    return r->upload_diff && D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !r->bound.rows && r->hit.valid &&
-           !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects &&
-           r->hit.bufs.scene == (const uint32_t *)s.scene.p;
-}
-
 static void swap_spare(vb_renderer *r) {
     std::swap(r->cur->scene, r->spare_scene);
     std::swap(r->cur->ramps, r->spare_ramps);
@@ -113,48 +101,42 @@ static void swap_spare(vb_renderer *r) {
 struct DiffedUpload {
     vb_renderer *r = nullptr;
     ~DiffedUpload() {
-        if (r && r->dmg.udiff.pending) {
+        if (r && r->dmg.diff.pending) {
             swap_spare(r);
-            r->dmg.udiff.pending = false;
+            r->dmg.diff.pending = false;
         }
     }
 };
 
-// Before an upload of layout L writes the current slot: when the next frame can diff it (upload_diff_armed), keep the base
-// frame's scene. On the upload's stream, before anything overwrites the base frame's intermediates: one copy of its draw boxes
-// and its records (from its tag and draw monoids and its scene, read through the uploaded layout, not the view's). Then the
-// slot's scene, ramps and atlas are swapped with the spare set, sized here for the upload, which the upload then writes; the
-// base's buffers become the spare set, without a copy. The diff's head names both.
+// Before an upload of layout L writes the current slot: when the next frame can diff it against the scene the base frame
+// rendered (the switch is on, base_diffable, and the base read this slot's scene buffer), begin the diff (diff_begin) and keep
+// that scene. The slot's scene, ramps and atlas are swapped with the spare set, sized here for the upload, which the upload then
+// writes; the base's buffers become the spare set, without a copy. On the upload's stream, before anything overwrites the base
+// frame's intermediates, its records (from its tag and draw monoids and its scene, read through the uploaded layout, not the
+// view's); and the diff's head, which names both sides.
 static int upload_diff_begin(vb_renderer *r, cudaStream_t st, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w,
                              uint32_t atlas_h, DiffedUpload &guard) {
-    r->dmg.udiff.pending = false;
-    if (!upload_diff_armed(r)) return VB_OK;
     vb_renderer::SceneSlot &s = *r->cur;
+    if (!r->upload_diff || r->hit.bufs.scene != (const uint32_t *)s.scene.p || !base_diffable(r)) return VB_OK;
     const uint32_t n_old = s.layout.n_draw_objects, n_new = L.n_draw_objects;
-    const VbUdLayout U = vb_udiff_layout(n_old, n_new);
     int rc;
-    if ((rc = ensure(r, r->udiff, U.bytes))) return rc;
     if ((rc = ensure(r, r->spare_scene, scene_bytes(L, scene_words, r->view.on)))) return rc;
     if ((rc = ensure(r, r->spare_ramps, (size_t)n_ramps * 512 * 4))) return rc;
     if ((rc = ensure(r, r->spare_atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
-    char *ud = (char *)r->udiff.p;
-    if (n_old) CK(cudaMemcpyAsync(ud + U.boxes, r->hit.bufs.draw_bboxes, (size_t)n_old * sizeof(VbBbox4), cudaMemcpyDeviceToDevice, st));
-    vb_launch_upload_records((const uint32_t *)s.scene.p, s.layout.path_tag_base, s.layout.draw_tag_base, r->hit.cfg.n_tag_words, n_old,
-                             r->hit.bufs.tag_monoids, r->hit.bufs.draw_monoids, (VbUdRec *)(ud + U.old_rec), nullptr, 0u, st);
-    CK(cudaGetLastError());
+    if ((rc = diff_begin(r, st, true, n_old, n_new, n_new))) return rc;
+    swap_spare(r); // s keeps the base's layout and sizes until set_scene
+    guard.r = r;
     VbUdiff &h = r->ud_head;
     memset(&h, 0, sizeof h);
-    h.old_side = VbUdSide{(const uint32_t *)s.scene.p, (const uint32_t *)s.ramps.p, (const uint8_t *)s.atlas.p, s.layout, s.n_ramps, s.atlas_w,
-                          s.atlas_h, 0u};
-    h.new_side = VbUdSide{(const uint32_t *)r->spare_scene.p, (const uint32_t *)r->spare_ramps.p, (const uint8_t *)r->spare_atlas.p, L, n_ramps,
-                          atlas_w, atlas_h, 0u};
+    h.old_side = VbUdSide{(const uint32_t *)r->spare_scene.p, (const uint32_t *)r->spare_ramps.p, (const uint8_t *)r->spare_atlas.p, s.layout,
+                          s.n_ramps, s.atlas_w, s.atlas_h, 0u};
+    h.new_side = VbUdSide{(const uint32_t *)s.scene.p, (const uint32_t *)s.ramps.p, (const uint8_t *)s.atlas.p, L, n_ramps, atlas_w, atlas_h, 0u};
+    char *ud = (char *)r->dmg_diff.p;
+    vb_launch_upload_records(h.old_side.scene, s.layout.path_tag_base, s.layout.draw_tag_base, r->hit.cfg.n_tag_words, n_old,
+                             r->hit.bufs.tag_monoids, r->hit.bufs.draw_monoids, (VbUdRec *)(ud + vb_udiff_layout(n_old, n_new).old_rec), nullptr,
+                             0u, st);
+    CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ud, &h, sizeof h, cudaMemcpyHostToDevice, st));
-    swap_spare(r);
-    vb_renderer::Damage::UploadDiff &D = r->dmg.udiff;
-    D.pending = true;
-    D.n_old = n_old;
-    D.n_new = n_new;
-    guard.r = r;
     return VB_OK;
 }
 
@@ -166,11 +148,11 @@ extern "C" int vb_set_upload_diff(vb_renderer *r, int on) {
     }
     r->upload_diff = on != 0;
     if (on) return VB_OK;
-    // off: the next frame cannot diff (it is full, as the upload's installation already said), and the spare set goes
-    r->dmg.udiff.armed = false;
+    // off: the spare set goes, and with it the old side of an upload's diff, whose frame is then full
+    if (r->dmg.diff.upload) r->dmg.diff.armed = false;
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream)); // an enqueued frame may still read them
-    for (DevBuf *b : {&r->spare_scene, &r->spare_ramps, &r->spare_atlas, &r->udiff}) {
+    for (DevBuf *b : {&r->spare_scene, &r->spare_ramps, &r->spare_atlas}) {
         if (b->p) CK(cudaFree(b->p));
         *b = DevBuf{};
     }
