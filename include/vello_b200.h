@@ -183,6 +183,15 @@ int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: wh
  * bin_row / tile_row window; a renderer of a vb_group or with the exchange enabled; a frame enqueued and not finished
  * (vb_render_enqueue until vb_frame_finish, vb_render_begin until vb_readback_wait). */
 int vb_hit_test(vb_renderer *, const float *xy, uint32_t n, int32_t *draw_ix, uint32_t on_device);
+/* Hit maps: vb_hit_test's answer at every pixel centre of a rectangle of the same frame. Row j, column i of the output, at
+ * (char *)draw_ix + j * pitch_bytes + 4 * i, is the answer for the point (x0 + i + 0.5f, y0 + j + 0.5f), equal int for int;
+ * only those h rows of w values are written. Everything above carries over: the frame, its state rules and error codes, the
+ * tall frame of a batch, on_device (draw_ix alone is the pointer checked), and a map leaves the frame alone as a hit test
+ * does. One CTA per 16 x 16 tile reads the tile's draw list and segments once for its 256 pixels (DESIGN.md §1, "Hit maps").
+ * w = 0 or h = 0: nothing happens, VB_OK. VB_E_INVALID also for NULL draw_ix; a rectangle not inside the last frame
+ * (x0 + w > width or y0 + h > n_cells * height); pitch_bytes not a multiple of 4 or below 4 * w. */
+int vb_hit_map(vb_renderer *, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, int32_t *draw_ix, size_t pitch_bytes,
+               uint32_t on_device);
 
 /* The renderer-owned target of the last frame (device pointer) and its size in bytes. */
 void *vb_target(vb_renderer *, size_t *bytes);

@@ -2,9 +2,12 @@
 test of 1, 1,024, 65,536 and 10^6 uniformly random points in the frame, in the host form (numpy in, numpy out, synchronous)
 and the device form (CUDA tensors in and out, enqueued on the renderer's stream), both with CUDA events around the call on
 that stream, after warm-up; prints the median of --steps calls beside the frame's own device time. Also reports where the
-time of a point goes: the longest draw list of a bin and the longest segment slice of a tile. Prints the card, its power
-limit and SM clock first. With --out, the rows also go to DIR/hit_probe.jsonl:
-    python tools/hit_probe.py [--steps 20] [--out DIR]"""
+time of a point goes: the longest draw list of a bin and the longest segment slice of a tile. Then hit maps
+(Renderer.hit_map, device form): the whole 4096^2 frame and a 1024^2 sub-rectangle, beside the device form of hit_test
+over the same 16.7 M pixel centres (--test-steps calls: it is slow), with a check that its answers equal the map's. Prints
+the card, its power limit and SM clock first, and again after the map rows. With --out, the rows also go to
+DIR/hit_probe.jsonl:
+    python tools/hit_probe.py [--steps 20] [--test-steps 3] [--out DIR]"""
 import argparse
 import json
 import os
@@ -31,11 +34,11 @@ def card():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
-def timed(r, fn, steps):
+def timed(r, fn, steps, warmup=3):
     """Median device time in ms of fn() between two events on the renderer's stream."""
     st = torch.cuda.ExternalStream(r.stream)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(3):
+    for _ in range(warmup):
         fn()
     ms = []
     for _ in range(steps):
@@ -50,6 +53,7 @@ def timed(r, fn, steps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--test-steps", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -91,6 +95,29 @@ def main():
                    hit_share=round(float((out >= 0).mean()), 3), device_equals_host=same)
         rows.append(row)
         print(json.dumps(row), flush=True)
+    # hit maps: the whole frame and a 1024^2 sub-rectangle, against hit_test over the same pixel centres
+    dmap = torch.empty((SIZE, SIZE), dtype=torch.int32, device="cuda")
+    sub = (1536, 1536, 1024, 1024)
+    dsub = torch.empty((sub[3], sub[2]), dtype=torch.int32, device="cuda")
+    torch.cuda.synchronize()
+    map_ms = timed(r, lambda: r.hit_map(out=dmap), a.steps)
+    sub_ms = timed(r, lambda: r.hit_map(sub, out=dsub), a.steps)
+    torch.cuda.synchronize()
+    c = torch.arange(SIZE, dtype=torch.float32, device="cuda") + 0.5
+    centres = torch.stack([c.repeat(SIZE), c.repeat_interleave(SIZE)], 1).contiguous()  # row by row
+    dtest = torch.empty(SIZE * SIZE, dtype=torch.int32, device="cuda")
+    torch.cuda.synchronize()
+    test_ms = timed(r, lambda: r.hit_test(centres, dtest), a.test_steps, warmup=1)
+    torch.cuda.synchronize()
+    same = bool(torch.equal(dtest.view(SIZE, SIZE), dmap))
+    same_sub = bool(torch.equal(dsub, dmap[sub[1]:sub[1] + sub[3], sub[0]:sub[0] + sub[2]]))
+    row = dict(map=f"{SIZE}x{SIZE}", map_ms=round(map_ms, 4), map_frames=round(map_ms / frame_ms, 3),
+               sub_map=f"{sub[2]}x{sub[3]}", sub_map_ms=round(sub_ms, 4), hit_test_same_centres_ms=round(test_ms, 2),
+               speedup=round(test_ms / map_ms, 1), map_equals_hit_test=same, sub_map_equals_map=same_sub,
+               frame_ms=round(frame_ms, 3), hit_share=round(float((dmap >= 0).float().mean()), 3))
+    rows.append(row)
+    print(json.dumps(row), flush=True)
+    print("card after the maps (name, power limit, SM clock, max SM clock):", card(), flush=True)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "hit_probe.jsonl"), "w") as f:

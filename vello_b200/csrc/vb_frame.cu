@@ -1082,9 +1082,9 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     return VB_OK;
 }
 
-// ---- hit testing: vb_hit_test ---------------------------------------------------------------------------------------------
+// ---- hit testing: vb_hit_test, vb_hit_map ---------------------------------------------------------------------------------
 // The answers read the buffers of the frame recorded in r->hit (k_hit.cu); nothing of the frame is written, launched or
-// captured, so kernel_launches, the graph key and the next frame are the same with or without hit tests in between.
+// captured, so kernel_launches, the graph key and the next frame are the same with or without hit tests or maps in between.
 bool vb_host::device_memory_of(vb_renderer *r, const void *p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -1092,6 +1092,21 @@ bool vb_host::device_memory_of(vb_renderer *r, const void *p) {
         return false;
     }
     return a.type == cudaMemoryTypeManaged || (a.type == cudaMemoryTypeDevice && a.device == r->device);
+}
+// The renderer's state checks both calls make, in this order, with `fn` naming the call in vb_last_error.
+static int hit_state(vb_renderer *r, const char *fn) {
+    auto bad = [&](const char *why) {
+        r->err = std::string(fn) + ": " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
+    if (r->frame_pending || r->stream_pending) return bad("a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)");
+    if (!r->hit.valid) {
+        r->err = std::string(fn) + ": no successful frame since the last scene upload, vb_set_cells, vb_run_stages or vb_debug_* call";
+        return VB_E_NO_SCENE;
+    }
+    if (r->hit.windowed) return bad("the last frame had a bin_row / tile_row window");
+    return VB_OK;
 }
 extern "C" int vb_hit_test(vb_renderer *r, const float *xy, uint32_t n, int32_t *draw_ix, uint32_t on_device) {
     if (!r) return VB_E_INVALID;
@@ -1101,13 +1116,7 @@ extern "C" int vb_hit_test(vb_renderer *r, const float *xy, uint32_t n, int32_t 
     };
     if (n == 0u) return VB_OK;
     if (!xy || !draw_ix) return bad("NULL points or answers");
-    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
-    if (r->frame_pending || r->stream_pending) return bad("a frame is in flight (finish it with vb_frame_finish / vb_readback_wait)");
-    if (!r->hit.valid) {
-        r->err = "vb_hit_test: no successful frame since the last scene upload, vb_set_cells, vb_run_stages or vb_debug_* call";
-        return VB_E_NO_SCENE;
-    }
-    if (r->hit.windowed) return bad("the last frame had a bin_row / tile_row window");
+    if (int rc = hit_state(r, "vb_hit_test")) return rc;
     CK(cudaSetDevice(r->device));
     if (on_device) {
         if (!device_memory_of(r, xy) || !device_memory_of(r, draw_ix)) return bad("on_device: the pointers must be memory of the renderer's device");
@@ -1124,6 +1133,38 @@ extern "C" int vb_hit_test(vb_renderer *r, const float *xy, uint32_t n, int32_t 
     vb_launch_hit_test(r->hit.cfg, r->hit.bufs, d_xy, n, d_ix, r->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(draw_ix, d_ix, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, r->stream));
+    CK(cudaStreamSynchronize(r->stream));
+    return VB_OK;
+}
+extern "C" int vb_hit_map(vb_renderer *r, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, int32_t *draw_ix, size_t pitch_bytes,
+                          uint32_t on_device) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const char *why) {
+        r->err = std::string("vb_hit_map: ") + why;
+        return VB_E_INVALID;
+    };
+    if (w == 0u || h == 0u) return VB_OK;
+    if (!draw_ix) return bad("NULL answers");
+    if (int rc = hit_state(r, "vb_hit_map")) return rc;
+    const VbConfig &cfg = r->hit.cfg;
+    if ((uint64_t)x0 + w > cfg.target_width || (uint64_t)y0 + h > (uint64_t)cfg.n_cells * cfg.target_height)
+        return bad("the rectangle does not lie inside the last frame");
+    const size_t row = (size_t)w * sizeof(int32_t);
+    if (pitch_bytes % sizeof(int32_t) != 0u || pitch_bytes < row) return bad("pitch_bytes must be a multiple of 4 and at least 4 * w");
+    if ((size_t)(h - 1u) > (SIZE_MAX - row) / pitch_bytes) return bad("the rows do not fit in the address space");
+    CK(cudaSetDevice(r->device));
+    if (on_device) {
+        if (!device_memory_of(r, draw_ix)) return bad("on_device: draw_ix must be memory of the renderer's device");
+        vb_launch_hit_map(cfg, r->hit.bufs, x0, y0, w, h, draw_ix, pitch_bytes, r->stream);
+        CK(cudaGetLastError());
+        return VB_OK;
+    }
+    int rc = ensure(r, r->hit_io, row * h);
+    if (rc) return rc;
+    int32_t *d_ix = (int32_t *)r->hit_io.p;
+    vb_launch_hit_map(cfg, r->hit.bufs, x0, y0, w, h, d_ix, row, r->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpy2DAsync(draw_ix, pitch_bytes, d_ix, row, row, h, cudaMemcpyDeviceToHost, r->stream));
     CK(cudaStreamSynchronize(r->stream));
     return VB_OK;
 }

@@ -251,7 +251,7 @@ struct vb_renderer {
     } ring[3];
     uint64_t stream_seq = 0;
 
-    // hit testing (vb_hit_test): the config and buffers of a frame, taken when it is enqueued (hit_enq) and handed to `hit` once
+    // hit testing (vb_hit_test, vb_hit_map): the config and buffers of a frame, taken when it is enqueued (hit_enq) and handed to `hit` once
     // it is known to have succeeded. `hit` stays valid until something rewrites what the answers read: the next frame, a scene
     // upload, vb_set_cells, vb_run_stages, vb_debug_upload or vb_debug_limit_arena.
     struct HitFrame {
@@ -260,7 +260,7 @@ struct vb_renderer {
         VbConfig cfg{};
         VbFrameBufs bufs{};
     } hit, hit_enq;
-    DevBuf hit_io; // the host form's points and answers
+    DevBuf hit_io; // the host forms' points and answers, and maps
 
     // composition (vb_fragment_upload / vb_compose): the resident fragments by id, and the keys their ramps and images are
     // de-duplicated by across fragments

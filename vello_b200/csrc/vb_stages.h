@@ -154,6 +154,10 @@ uint32_t vb_launch_view_transforms(const VbConfig &cfg, const VbFrameBufs &b, cu
 // hit testing (k_hit.cu): for n points xy (interleaved f32 pairs, device memory) the last draw object covering each of them
 // in the finished frame `cfg` / `b` describe, or -1 (vb_hit_test); reads the frame's buffers and writes only draw_ix
 uint32_t vb_launch_hit_test(const VbConfig &cfg, const VbFrameBufs &b, const float *xy, uint32_t n, int32_t *draw_ix, cudaStream_t st);
+// hit maps (k_hit.cu): the same answer at every pixel centre of the rectangle [x0, x0 + w) x [y0, y0 + h) of the tall frame,
+// pixel (i, j) at (char *)draw_ix + j * pitch + 4 * i (vb_hit_map); the rectangle must lie inside the frame
+uint32_t vb_launch_hit_map(const VbConfig &cfg, const VbFrameBufs &b, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, int32_t *draw_ix,
+                           size_t pitch, cudaStream_t st);
 
 // device resolve (vb_scene_upload_streams)
 void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes, uint32_t end_clip_word0,

@@ -166,6 +166,7 @@ def load_library() -> C.CDLL:
     lib.vb_group_set_view.argtypes = [vp, C.POINTER(C.c_double)]
     lib.vb_debug_graph_captures.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.vb_hit_test.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
+    lib.vb_hit_map.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, C.c_size_t, C.c_uint32]
     lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
@@ -191,7 +192,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_group_scene_upload", "vb_group_render_resident", "vb_group_frame", "vb_group_stripes", "vb_group_set_balancing",
                     "vb_group_set_exchange", "vb_exchange_configure", "vb_exchange_attach", "vb_exchange_set_bounds", "vb_exchange_enable",
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
-                    "vb_debug_graph_captures", "vb_hit_test", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
+                    "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination"]
 
@@ -297,6 +298,8 @@ class Renderer:
         self._bound = None  # the device array of bind_instance_transforms
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
+        self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
+        self._hit_extent = None  # (width, cells * height) of the last frame that succeeded: hit_map's whole frame
 
     @classmethod
     def _borrowed(cls, lib, handle: int, owner):
@@ -309,6 +312,8 @@ class Renderer:
         r._destinations = {}
         r._bound = None
         r._frame_size = None
+        r._cells = 1
+        r._hit_extent = None
         return r
 
     def close(self):
@@ -333,6 +338,7 @@ class Renderer:
         atlas = np.ascontiguousarray(packed.atlas, dtype=np.uint8)
         lay = _Layout(*[int(v) for v in packed.layout.as_array()])
         self._keep = (scene, ramps, atlas)
+        self._cells = 1
         rc = self.lib.vb_scene_upload(self.handle, scene.ctypes.data, scene.nbytes, C.byref(lay),
                                       ramps.ctypes.data if ramps.size else None, 512, ramps.shape[0],
                                       atlas.ctypes.data, atlas.shape[1], atlas.shape[0])
@@ -438,6 +444,7 @@ class Renderer:
         L = _Layout()
         offs = (C.c_uint32 * (len(inst) + 1))()
         self._check(getattr(self.lib, fn)(self.handle, arr, len(inst), C.byref(L), offs), fn)
+        self._cells = 1
         lay = Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
                      L.draw_data_base, L.transform_base, L.style_base)
         return lay, [int(v) for v in offs]
@@ -493,6 +500,7 @@ class Renderer:
         self.last_stats = st
         self._check(rc, "vb_render")
         self._frame_size = (int(params.width), int(params.height))
+        self._cells, self._hit_extent = 1, self._frame_size
         return out
 
     def render_stream(self, scenes, params: RenderParams):
@@ -515,6 +523,7 @@ class Renderer:
                                           atlas.ctypes.data, atlas.shape[1], atlas.shape[0], C.byref(ps), out.ctypes.data, C.byref(st))
             self.last_stats = st
             self._check(rc, "vb_render_begin")
+            self._cells, self._hit_extent = 1, (int(params.width), int(params.height))  # once it completes
             if k >= 2:
                 yield outs[k - 2]  # complete: vb_render_begin returned for the frame two later
                 outs[k - 2] = None
@@ -533,6 +542,7 @@ class Renderer:
         if arr.ndim != 1 or arr.size < 2:
             raise ValueError("set_cells: offsets need at least two entries (cells + 1)")
         self._check(self.lib.vb_set_cells(self.handle, arr.ctypes.data, arr.size - 1), "vb_set_cells")
+        self._cells = arr.size - 1
 
     def render_batch(self, scenes, params: RenderParams, out=None):
         """Render every scene of `scenes` (all `Scene`s, or all `NativeScene`s, which are resolved on the device) at
@@ -566,6 +576,7 @@ class Renderer:
         self.last_stats = st
         self._check(rc, "vb_render_uploaded")
         self._frame_size = (w, h)
+        self._hit_extent = (w, n * h)
         return out
 
     @staticmethod
@@ -617,12 +628,14 @@ class Renderer:
         self.last_stats = st
         self._check(rc, "vb_render_resident")
         self._frame_size = (int(params.width), int(params.height))
+        self._hit_extent = (int(params.width), self._cells * int(params.height))
         return st
 
     def enqueue(self, params: RenderParams, out_device_ptr: int = 0, bin_rows=(0, 0), tile_rows=(0, 0)):
         ps = _params_struct(params, bin_rows, tile_rows)
         self._check(self.lib.vb_render_enqueue(self.handle, C.byref(ps), C.c_void_p(out_device_ptr or None)), "vb_render_enqueue")
         self._enqueued_size = (int(params.width), int(params.height))
+        self._enqueued_extent = (int(params.width), self._cells * int(params.height))
 
     def finish(self) -> FrameStats:
         st = FrameStats()
@@ -630,6 +643,7 @@ class Renderer:
         self.last_stats = st
         self._check(rc, "vb_frame_finish")
         self._frame_size = getattr(self, "_enqueued_size", self._frame_size)
+        self._hit_extent = getattr(self, "_enqueued_extent", self._hit_extent)
         return st
 
     @property
@@ -731,6 +745,41 @@ class Renderer:
             raise ValueError(f"hit_test: out must be a contiguous int32 numpy array of shape ({n},)")
         if n:
             self._check(self.lib.vb_hit_test(self.handle, pts.ctypes.data, n, out.ctypes.data, 0), "vb_hit_test")
+        return out
+
+    def hit_map(self, rect=None, out=None):
+        """`hit_test` at every pixel centre of a rectangle of the last frame that completed (`vb_hit_map`): element [j, i] is
+        the answer for the point (x0 + i + 0.5, y0 + j + 0.5), equal int for int. `rect` = (x0, y0, w, h) must lie inside that
+        frame; None is the whole frame, (0, 0, W, N * H) for a batch of N cells (reshape it to (N, H, W)).
+
+        With no `out`, or a numpy `out` (int32 (h, w) with element stride 4, so a slice of a larger array works), the call is
+        synchronous and returns the numpy map. A device `out` (`__cuda_array_interface__`, e.g. a torch int32 CUDA tensor or a
+        row slice of one) of the same shape and element stride gets the map enqueued on `self.stream` and is returned at once
+        (synchronise with that stream before reading it). Only the h rows of w answers are written."""
+        if rect is None:
+            if self._hit_extent is None:
+                raise VelloB200Error("hit_map: no frame has completed on this renderer")
+            rect = (0, 0) + tuple(self._hit_extent)
+        x0, y0, w, h = (int(v) for v in rect)
+        if not all(0 <= v < 2 ** 32 for v in (x0, y0, w, h)):
+            raise ValueError(f"hit_map: rect must be four unsigned 32-bit integers, not {tuple(rect)}")
+        device = out is not None and hasattr(out, "__cuda_array_interface__")
+        if device:
+            cai = out.__cuda_array_interface__
+            shape, typestr, ptr = tuple(int(v) for v in cai["shape"]), cai["typestr"], int(cai["data"][0])
+            strides = cai.get("strides") or (4 * w, 4)
+        else:
+            if out is None:
+                out = np.empty((h, w), dtype=np.int32)
+            if not isinstance(out, np.ndarray):
+                raise ValueError("hit_map: out must be a numpy array or a device array")
+            shape, typestr, ptr, strides = out.shape, out.dtype.str, out.ctypes.data, out.strides
+        if shape != (h, w) or typestr != "<i4":
+            raise ValueError(f"hit_map: out must be int32 of shape ({h}, {w}), not {shape} {typestr}")
+        pitch = int(strides[0]) if h > 1 else 4 * w  # one row: its pitch is never used
+        if (w > 1 and strides[1] != 4) or (h > 1 and (pitch % 4 or pitch < 4 * w)):
+            raise ValueError(f"hit_map: out needs element stride 4 and a row stride of at least 4 * w, not strides {tuple(strides)}")
+        self._check(self.lib.vb_hit_map(self.handle, x0, y0, w, h, C.c_void_p(ptr), pitch, 1 if device else 0), "vb_hit_map")
         return out
 
     def debug_graph_captures(self) -> int:

@@ -274,6 +274,7 @@ class NativeScene:
         offsets, kernels apply the patches / padding and generate the gradient ramps) and leave it uploaded there."""
         L = _Layout()
         self._check(self.lib.vb_scene_upload_device(renderer.handle, self.handle, C.byref(L)))
+        renderer._cells = 1  # a new scene is one cell (Renderer.hit_map's whole frame)
         return Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
                       L.draw_data_base, L.transform_base, L.style_base)
 
