@@ -48,32 +48,23 @@ struct NamedBuf {
 };
 static std::vector<NamedBuf> named(vb_renderer *r) {
     const VbConfig &c = r->cfg;
-    const VbLayout &L = r->cur->layout;
-    const uint32_t wb = (c.width_in_tiles + 15u) / 16u, hb = (c.height_in_tiles + 15u) / 16u;
-    const uint32_t aligned_n_bins = (wb * hb * std::max(c.n_cells, 1u) + 255u) & ~255u;
     std::vector<NamedBuf> v = {
         {"scene", &r->cur->scene, r->cur->scene_words * 4}, // the uploaded / device-resolved inputs
         {"ramps", &r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4},
         {"atlas", &r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4},
-        {"tag_monoids", &r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)},
-        {"path_bboxes", &r->path_bboxes, (size_t)L.n_paths * sizeof(VbPathBbox)},
-        {"path_draw", &r->path_draw, (size_t)L.n_paths * 8u},
-        {"draw_monoids", &r->draw_monoids, (size_t)L.n_draw_objects * sizeof(VbDrawMonoid)},
-        {"clip_inp", &r->clip_inp, (size_t)L.n_clips * sizeof(VbClipInp)},
-        {"clip_bboxes", &r->clip_bboxes, (size_t)L.n_clips * sizeof(VbBbox4)},
-        {"draw_bboxes", &r->draw_bboxes, (size_t)L.n_draw_objects * sizeof(VbBbox4)},
-        {"bin_headers", &r->bin_headers, (size_t)((L.n_draw_objects + 255u) / 256u) * aligned_n_bins * sizeof(VbBinHeader)},
-        {"paths", &r->paths, (size_t)L.n_draw_objects * sizeof(VbPath)},
     };
+    // the fixed-size intermediates of the frame prepared last
+    for (int i = 0; i < N_FIXED_BUFS; i++)
+        if (FRAME_BUFS[i].downloadable) v.push_back({FRAME_BUFS[i].name, &r->fb[i], FRAME_BUFS[i].bytes(r->counts, true)});
     // the transform words the last frame read from its transform_base: the bound or viewed region, else the scene's stream
     const size_t t_off = (size_t)c.layout.transform_base * 4u, t_cap = r->cur->scene.cap > t_off ? r->cur->scene.cap - t_off : 0u;
-    v.push_back({"transforms", &r->cur->scene, std::min<size_t>(24u * (size_t)n_transforms(L, r->cur->scene_words), t_cap), t_off});
+    v.push_back({"transforms", &r->cur->scene, std::min<size_t>(24u * (size_t)n_transforms(r->cur->layout, r->cur->scene_words), t_cap), t_off});
     // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
     const uint32_t *size = &c.lines_size;
     for (int a = 0; a < N_ARENAS; a++) {
         const ArenaDesc &d = ARENAS[a];
         const size_t used = (size_t)std::min<uint64_t>(arena_need(r, a), size[a]);
-        v.push_back({d.download ? d.download : d.name, &(r->*d.buf), (arena_offset(r, a) + used) * d.elem_bytes});
+        v.push_back({FRAME_BUFS[d.buf].name, &r->fb[d.buf], (arena_offset(r, a) + used) * d.elem_bytes});
     }
     return v;
 }
@@ -82,7 +73,7 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
 // name, or "line_scratch" / "flatten_jobs" (flatten's scratch arenas, sized from the lines capacity). Returns false for an
 // unknown name; *buf is nullptr while the arena has no limit.
 static bool guard_region(vb_renderer *r, const char *name, DevBuf **buf, size_t *off) {
-    DevBuf *scratch = !strcmp(name, "line_scratch") ? &r->line_scratch : !strcmp(name, "flatten_jobs") ? &r->flatten_jobs : nullptr;
+    DevBuf *scratch = !strcmp(name, "line_scratch") ? &r->fb[FB_LINE_SCRATCH] : !strcmp(name, "flatten_jobs") ? &r->fb[FB_FLATTEN_JOBS] : nullptr;
     const int a = scratch ? ARENA_LINES : arena_index(name);
     if (a < 0) return false;
     *buf = nullptr;
@@ -90,13 +81,13 @@ static bool guard_region(vb_renderer *r, const char *name, DevBuf **buf, size_t 
     const uint32_t lim = r->limit[a];
     if (lim == UINT32_MAX) return true;
     // ptcl: includes the 512 bytes of window slack that fine reads and never writes
-    DevBuf *b = &(r->*ARENAS[a].buf);
+    DevBuf *b = &r->fb[ARENAS[a].buf];
     size_t o = (arena_offset(r, a) + lim) * ARENAS[a].elem_bytes;
     if (scratch) {
         size_t lit_bytes, job_bytes; // flatten sees lits_cap = lines_size, jobs_cap = lines_size / FL_DEFER_MIN + 1
         vb_flatten_arena_bytes(lim, &lit_bytes, &job_bytes);
         b = scratch;
-        o = scratch == &r->line_scratch ? lit_bytes : job_bytes;
+        o = scratch == &r->fb[FB_LINE_SCRATCH] ? lit_bytes : job_bytes;
     }
     *buf = b;
     *off = o < b->cap ? o : b->cap;
@@ -154,14 +145,14 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
     }
     if (!strcmp(name, "bump")) {
         if (bytes) *bytes = sizeof(VbBump);
-        if (dst && cap >= sizeof(VbBump)) CK(cudaMemcpy(dst, r->ctl.p, sizeof(VbBump), cudaMemcpyDeviceToHost));
+        if (dst && cap >= sizeof(VbBump)) CK(cudaMemcpy(dst, r->fb[FB_CTL].p, sizeof(VbBump), cudaMemcpyDeviceToHost));
         return VB_OK;
     }
     // segment slots of the last frame that backdrop assigned and no CMD_FILL uses (k_tile.cu, k_coarse.cu); after an incremental
     // frame (damage tracking) also the slots of the quadrants coarse skipped, so not the reference's count
     if (!strcmp(name, "seg_holes")) {
         if (bytes) *bytes = 4;
-        if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->ctl.p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
+        if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->fb[FB_CTL].p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
         return VB_OK;
     }
     if (!strcmp(name, "config")) {
@@ -182,7 +173,7 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
             size_t lit1, job1, lit_cap, job_cap; // one record of each, and the capacities the kernels saw
             vb_flatten_arena_bytes(1u, &lit1, &job1);
             vb_flatten_arena_bytes(r->cfg.lines_size, &lit_cap, &job_cap);
-            const DevBuf &b = lits ? r->line_scratch : r->flatten_jobs;
+            const DevBuf &b = r->fb[lits ? FB_LINE_SCRATCH : FB_FLATTEN_JOBS];
             n = std::min({(size_t)ctrs[lits ? 0 : 1] * (lits ? lit1 : job1), lits ? lit_cap : job_cap, b.cap});
             src = b.p;
             host = false;
@@ -223,8 +214,8 @@ extern "C" int vb_debug_fine_traffic(vb_renderer *r, uint64_t *ptcl_words, uint6
     c.win_ty0 = f.ty0, c.win_ty1 = f.ty1;
     uint32_t n = c.width_in_tiles * (c.win_ty1 - c.win_ty0);
     const uint8_t *damage = r->dmg.have_last && r->dmg.last.mode == VB_DMG_INCREMENTAL ? (const uint8_t *)r->dmg_mask.p : nullptr;
-    if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(c, (const uint32_t *)r->ptcl.p,
-                                                                r->occlusion_cull ? (const uint32_t *)r->tile_start.p : nullptr, damage, d);
+    if (n) k_ptcl_stats<<<(n + 127) / 128, 128, 0, r->stream>>>(c, (const uint32_t *)r->fb[FB_PTCL].p,
+                                                                r->occlusion_cull ? (const uint32_t *)r->fb[FB_TILE_START].p : nullptr, damage, d);
     CK(cudaStreamSynchronize(r->stream));
     CK(cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost));
     cudaFree(d);
@@ -249,23 +240,23 @@ extern "C" int vb_debug_upload(vb_renderer *r, const char *name, const void *src
             int rc = ensure_arena(r, a);
             if (rc) return rc;
         }
-        if (n) CK(cudaMemcpy((r->*ARENAS[a].buf).p, src, (size_t)n * ARENAS[a].elem_bytes, cudaMemcpyHostToDevice));
-        VbBump *bump = (VbBump *)r->ctl.p;
+        if (n) CK(cudaMemcpy(r->fb[ARENAS[a].buf].p, src, (size_t)n * ARENAS[a].elem_bytes, cudaMemcpyHostToDevice));
+        VbBump *bump = (VbBump *)r->fb[FB_CTL].p;
         CK(cudaMemcpy(&(bump->*ARENAS[a].counter), &n, 4, cudaMemcpyHostToDevice));
         r->cur->h_bump->*ARENAS[a].counter = n;
         return VB_OK;
     }
     if (!strcmp(name, "path_bboxes")) {
-        if (bytes > r->path_bboxes.cap) return VB_E_INVALID;
-        CK(cudaMemcpy(r->path_bboxes.p, src, bytes, cudaMemcpyHostToDevice));
+        if (bytes > r->fb[FB_PATH_BBOXES].cap) return VB_E_INVALID;
+        CK(cudaMemcpy(r->fb[FB_PATH_BBOXES].p, src, bytes, cudaMemcpyHostToDevice));
         return VB_OK;
     }
     if (!strcmp(name, "paths")) { // backdrop searches exactly n_draw_objects of them
-        if (bytes != (size_t)r->cur->layout.n_draw_objects * sizeof(VbPath) || bytes > r->paths.cap) {
+        if (bytes != (size_t)r->cur->layout.n_draw_objects * sizeof(VbPath) || bytes > r->fb[FB_PATHS].cap) {
             r->err = "vb_debug_upload: \"paths\" takes exactly one record per draw object, after a frame of the scene";
             return VB_E_INVALID;
         }
-        if (bytes) CK(cudaMemcpy(r->paths.p, src, bytes, cudaMemcpyHostToDevice));
+        if (bytes) CK(cudaMemcpy(r->fb[FB_PATHS].p, src, bytes, cudaMemcpyHostToDevice));
         return VB_OK;
     }
     return VB_E_UNKNOWN_BUFFER;

@@ -92,14 +92,46 @@ static void hit_finished(vb_renderer *r, bool ok) {
     r->hit.valid = ok && r->hit_enq.valid;
 }
 
+#define FIELD(f) offsetof(VbFrameBufs, f)
+const FrameBufDesc vb_host::FRAME_BUFS[N_FRAME_BUFS] = {
+    {"tag_monoids", FIELD(tag_monoids), true, [](const FrameCounts &n, bool) { return n.tag_words * sizeof(VbTagMonoid); }},
+    {"path_bboxes", FIELD(path_bboxes), true, [](const FrameCounts &n, bool) { return n.paths * sizeof(VbPathBbox); }},
+    {"path_draw", FIELD(path_draw), true, [](const FrameCounts &n, bool) { return n.paths * sizeof(uint2); }},
+    {"draw_monoids", FIELD(draw_monoids), true, [](const FrameCounts &n, bool) { return n.draws * sizeof(VbDrawMonoid); }},
+    {"clip_inp", FIELD(clip_inp), true, [](const FrameCounts &n, bool) { return n.clips * sizeof(VbClipInp); }},
+    {"clip_bboxes", FIELD(clip_bboxes), true, [](const FrameCounts &n, bool) { return n.clips * sizeof(VbBbox4); }},
+    {"clip_scratch", FIELD(clip_scratch), false, [](const FrameCounts &n, bool) { return vb_clip_scratch_words(n.clips) * 4; }},
+    {"draw_bboxes", FIELD(draw_bboxes), true, [](const FrameCounts &n, bool) { return n.draws * sizeof(VbBbox4); }},
+    {"bin_headers", FIELD(bin_headers), true,
+     [](const FrameCounts &n, bool) { return (size_t)n.draw_parts * n.aligned_bins * sizeof(VbBinHeader); }},
+    // allocated in whole partitions; the kernels write and read the first n_draw_objects records, and only those are downloaded
+    {"paths", FIELD(paths), true,
+     [](const FrameCounts &n, bool download) { return (download ? n.draws : (size_t)n.draw_parts * 256u) * sizeof(VbPath); }},
+    {"tile_start", FIELD(tile_start), false, [](const FrameCounts &n, bool) { return ((size_t)n.tiles + 256) * 4; }},
+    // fine's cost-ordered tile lists
+    {"cls_list", FIELD(cls_list), false, [](const FrameCounts &n, bool) { return (size_t)VB_FINE_CLASSES * n.tiles * 8; }},
+    {"flatten_parts", FIELD(flatten_parts), false, [](const FrameCounts &n, bool) { return vb_flatten_part_words(n.flatten_parts) * 4; }},
+    {"ctl", FIELD(ctl), false, [](const FrameCounts &n, bool) { return n.ctl_words * 4; }},
+    // the arenas' buffers, from FB_LINES on
+    {"lines", FIELD(lines)},
+    {"info_bin_data", FIELD(info_bin_data)},
+    {"tiles", FIELD(tiles)},
+    {"seg_counts", FIELD(seg_counts)},
+    {"segments", FIELD(segments)},
+    {"blend_spill", FIELD(blend_spill)},
+    {"ptcl", FIELD(ptcl)},
+    {"line_scratch", FIELD(line_scratch)},
+    {"flatten_jobs", FIELD(flatten_jobs)},
+};
+#undef FIELD
 const ArenaDesc vb_host::ARENAS[N_ARENAS] = {
-    {"lines", nullptr, &vb_renderer::lines, sizeof(VbLineSoup), &VbBump::lines},
-    {"binning", "info_bin_data", &vb_renderer::info_bin_data, 4, &VbBump::binning},
-    {"tiles", nullptr, &vb_renderer::tiles, sizeof(VbTile), &VbBump::tile},
-    {"seg_counts", nullptr, &vb_renderer::seg_counts, sizeof(VbSegmentCount), &VbBump::seg_counts},
-    {"segments", nullptr, &vb_renderer::segments, sizeof(VbSegment), &VbBump::segments},
-    {"blend", "blend_spill", &vb_renderer::blend_spill, 4, &VbBump::blend},
-    {"ptcl", nullptr, &vb_renderer::ptcl, 4, &VbBump::ptcl},
+    {"lines", FB_LINES, sizeof(VbLineSoup), &VbBump::lines},
+    {"binning", FB_INFO_BIN_DATA, 4, &VbBump::binning},
+    {"tiles", FB_TILES, sizeof(VbTile), &VbBump::tile},
+    {"seg_counts", FB_SEG_COUNTS, sizeof(VbSegmentCount), &VbBump::seg_counts},
+    {"segments", FB_SEGMENTS, sizeof(VbSegment), &VbBump::segments},
+    {"blend", FB_BLEND_SPILL, 4, &VbBump::blend},
+    {"ptcl", FB_PTCL, 4, &VbBump::ptcl},
 };
 int vb_host::arena_index(const char *name) {
     for (int a = 0; a < N_ARENAS; a++)
@@ -119,12 +151,12 @@ uint64_t vb_host::arena_need(const vb_renderer *r, int a) {
 // also sizes flatten's scratch arenas.
 int vb_host::ensure_arena(vb_renderer *r, int a) {
     const ArenaDesc &d = ARENAS[a];
-    int rc = ensure(r, r->*d.buf, (arena_offset(r, a) + r->cap[a]) * d.elem_bytes + (a == ARENA_PTCL ? 512 : 0));
+    int rc = ensure(r, r->fb[d.buf], (arena_offset(r, a) + r->cap[a]) * d.elem_bytes + (a == ARENA_PTCL ? 512 : 0));
     if (rc || a != ARENA_LINES) return rc;
     size_t lit_bytes, job_bytes;
     vb_flatten_arena_bytes(r->cap[a], &lit_bytes, &job_bytes);
-    if ((rc = ensure(r, r->line_scratch, lit_bytes))) return rc;
-    return ensure(r, r->flatten_jobs, job_bytes);
+    if ((rc = ensure(r, r->fb[FB_LINE_SCRATCH], lit_bytes))) return rc;
+    return ensure(r, r->fb[FB_FLATTEN_JOBS], job_bytes);
 }
 
 // mask LUTs: vello_encoding/src/mask.rs:10-98 (f64 maths like the reference)
@@ -154,109 +186,88 @@ static void make_mask_luts(std::vector<uint32_t> &l8, std::vector<uint32_t> &l16
     }
 }
 
+// The renderer's streams and events, each once, with the flags they are created with: what vb_renderer_new creates and
+// vb_renderer_free destroys.
+template <class S, class E> static void for_each_handle(vb_renderer *r, S stream, E event) {
+    for (cudaStream_t *s : {&r->stream, &r->upload_stream, &r->tiling_stream, &r->copy_stream}) stream(*s);
+    for (cudaEvent_t *e : {&r->tiling_fork, &r->tiling_join, &r->draw_fork, &r->draw_join}) event(*e, cudaEventDisableTiming);
+    for (PinnedStage &s : r->pinned) event(s.copied, cudaEventDisableTiming);
+    for (cudaEvent_t &e : r->upload_done) event(e, cudaEventDisableTiming);
+    for (cudaEvent_t &e : r->raster_done) event(e, cudaEventDisableTiming);
+    for (cudaEvent_t &e : r->band_ev) event(e, cudaEventDisableTiming);
+    for (cudaEvent_t &e : r->copy_done) event(e, cudaEventDisableTiming);
+    for (cudaEvent_t &e : r->ev) event(e, cudaEventDefault);
+    for (cudaEvent_t &e : r->frame_ev) event(e, cudaEventDefault);
+}
+
+// Everything vb_renderer_new creates; on failure vb_renderer_free releases what was created.
+static int renderer_init(vb_renderer *r) {
+    const cudaError_t e = cudaSetDevice(r->device);
+    if (e != cudaSuccess) {
+        fprintf(stderr, "vello_b200: cudaSetDevice(%d): %s\n", r->device, cudaGetErrorString(e));
+        return VB_E_CUDA;
+    }
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, r->device) == cudaSuccess) r->sm_count = prop.multiProcessorCount;
+    cudaError_t created = cudaSuccess;
+    for_each_handle(
+        r, [&](cudaStream_t &s) { if (created == cudaSuccess) created = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); },
+        [&](cudaEvent_t &ev, unsigned flags) { if (created == cudaSuccess) created = cudaEventCreateWithFlags(&ev, flags); });
+    CK(created);
+    for (auto &s : r->slot) {
+        CK(cudaHostAlloc((void **)&s.h_bump, sizeof(VbBump), cudaHostAllocMapped));
+        CK(cudaHostGetDevicePointer((void **)&s.h_bump_dev, s.h_bump, 0));
+        memset(s.h_bump, 0, sizeof(VbBump));
+    }
+    if (vb_fine_init_constants() != 0) return VB_E_CUDA;
+    std::vector<uint32_t> l8, l16;
+    make_mask_luts(l8, l16);
+    int rc;
+    if ((rc = ensure(r, r->mask8, l8.size() * 4)) || (rc = ensure(r, r->mask16, l16.size() * 4))) return rc;
+    CK(cudaMemcpy(r->mask8.p, l8.data(), l8.size() * 4, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(r->mask16.p, l16.data(), l16.size() * 4, cudaMemcpyHostToDevice));
+    return VB_OK;
+}
+
 extern "C" int vb_renderer_new(const vb_options *opt, vb_renderer **out) {
     if (!out) return VB_E_INVALID;
     vb_renderer *r = new vb_renderer();
     r->device = opt ? opt->device : 0;
     r->timing = opt && opt->timing;
     if (opt && opt->max_retries) r->max_retries = opt->max_retries;
-    cudaError_t e = cudaSetDevice(r->device);
-    if (e != cudaSuccess) {
-        fprintf(stderr, "vello_b200: cudaSetDevice(%d): %s\n", r->device, cudaGetErrorString(e));
-        delete r;
-        return VB_E_CUDA;
-    }
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, r->device) == cudaSuccess) r->sm_count = prop.multiProcessorCount;
-    if (cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&r->tiling_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->tiling_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->tiling_join, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->draw_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&r->draw_join, cudaEventDisableTiming) != cudaSuccess) {
-        delete r;
-        return VB_E_CUDA;
-    }
-    for (PinnedStage &s : r->pinned)
-        if (cudaEventCreateWithFlags(&s.copied, cudaEventDisableTiming) != cudaSuccess) {
-            delete r;
-            return VB_E_CUDA;
-        }
-    for (auto &s : r->slot) {
-        if (cudaHostAlloc((void **)&s.h_bump, sizeof(VbBump), cudaHostAllocMapped) != cudaSuccess ||
-            cudaHostGetDevicePointer((void **)&s.h_bump_dev, s.h_bump, 0) != cudaSuccess) {
-            delete r;
-            return VB_E_CUDA;
-        }
-        memset(s.h_bump, 0, sizeof(VbBump));
-    }
-    for (auto &ev : r->upload_done) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-    for (auto &ev : r->raster_done) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-    for (auto &ev : r->ev) cudaEventCreate(&ev);
-    for (auto &ev : r->frame_ev) cudaEventCreate(&ev);
-    for (auto &ev : r->band_ev) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-    for (auto &ev : r->copy_done) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
     if (getenv("VELLO_B200_NO_GRAPH")) r->use_graph = false;
-    if (cudaStreamCreateWithFlags(&r->copy_stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete r;
-        return VB_E_CUDA;
+    const int rc = renderer_init(r);
+    if (rc) {
+        vb_renderer_free(r);
+        return rc;
     }
-    r->ev_ok = true;
-    if (vb_fine_init_constants() != 0) {
-        delete r;
-        return VB_E_CUDA;
-    }
-    std::vector<uint32_t> l8, l16;
-    make_mask_luts(l8, l16);
-    if (ensure(r, r->mask8, l8.size() * 4) || ensure(r, r->mask16, l16.size() * 4)) {
-        delete r;
-        return VB_E_CUDA;
-    }
-    cudaMemcpy(r->mask8.p, l8.data(), l8.size() * 4, cudaMemcpyHostToDevice);
-    cudaMemcpy(r->mask16.p, l16.data(), l16.size() * 4, cudaMemcpyHostToDevice);
     *out = r;
     return VB_OK;
 }
 
+// Also frees a renderer that vb_renderer_new left partly built: every handle is checked.
 extern "C" void vb_renderer_free(vb_renderer *r) {
     if (!r) return;
     cudaSetDevice(r->device);
     if (r->stream) cudaStreamSynchronize(r->stream);
+    if (r->tiling_stream) cudaStreamSynchronize(r->tiling_stream);
     for_each_buf(r, [](DevBuf &b) {
         if (b.p) cudaFree(b.p);
     });
     for (auto &s : r->slot)
         if (s.h_bump) cudaFreeHost(s.h_bump);
-    for (PinnedStage &s : r->pinned) {
+    for (PinnedStage &s : r->pinned)
         if (s.host) cudaFreeHost(s.host);
-        if (s.copied) cudaEventDestroy(s.copied);
-    }
     for (auto &f : r->fragments) cudaFree(f.second->mem);
     for (auto &f : r->freed) {
         cudaFree(f.mem);
         cudaEventDestroy(f.done);
     }
     drop_registrations(r);
-    if (r->ev_ok) {
-        for (auto &ev : r->ev) cudaEventDestroy(ev);
-        for (auto &ev : r->frame_ev) cudaEventDestroy(ev);
-        for (auto &ev : r->band_ev) cudaEventDestroy(ev);
-        for (auto &ev : r->copy_done) cudaEventDestroy(ev);
-        for (auto &ev : r->upload_done) cudaEventDestroy(ev);
-        for (auto &ev : r->raster_done) cudaEventDestroy(ev);
-        for (auto &gs : r->graphs)
-            if (gs.exec) cudaGraphExecDestroy(gs.exec);
-    }
-    if (r->tiling_stream) cudaStreamSynchronize(r->tiling_stream);
-    if (r->tiling_fork) cudaEventDestroy(r->tiling_fork);
-    if (r->tiling_join) cudaEventDestroy(r->tiling_join);
-    if (r->draw_fork) cudaEventDestroy(r->draw_fork);
-    if (r->draw_join) cudaEventDestroy(r->draw_join);
-    if (r->tiling_stream) cudaStreamDestroy(r->tiling_stream);
-    if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
-    if (r->upload_stream) cudaStreamDestroy(r->upload_stream);
-    if (r->stream) cudaStreamDestroy(r->stream);
+    for (auto &gs : r->graphs)
+        if (gs.exec) cudaGraphExecDestroy(gs.exec);
+    for_each_handle(
+        r, [](cudaStream_t &s) { if (s) cudaStreamDestroy(s); }, [](cudaEvent_t &ev, unsigned) { if (ev) cudaEventDestroy(ev); });
     delete r;
 }
 
@@ -335,14 +346,15 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         return VB_E_INVALID;
     }
     const uint32_t n_cells = r->cells.empty() ? 1u : (uint32_t)r->cells.size() - 1u;
+    const uint32_t hb = ((p->height + 15u) / 16u + 15u) / 16u, wb = ((p->width + 15u) / 16u + 15u) / 16u;
+    // bin_headers: one row of headers per partition of 256 draw objects, each row the bins of every cell rounded up to 256
+    const uint64_t draw_parts = (r->cur->layout.n_draw_objects + 255ull) / 256u, aligned_bins = ((uint64_t)wb * hb * n_cells + 255u) & ~255ull;
     if (n_cells > 1u) {
         if (p->bin_row1 > p->bin_row0 || p->tile_row1 > p->tile_row0 || r->xc.enabled || r->grouped) {
             r->err = "batch: cells cannot be combined with bin_row / tile_row windows, vb_group or the exchange";
             return VB_E_INVALID;
         }
-        const uint64_t hb = ((p->height + 15u) / 16u + 15u) / 16u, wb = ((p->width + 15u) / 16u + 15u) / 16u;
-        const uint64_t parts = (r->cur->layout.n_draw_objects + 255u) / 256u, bins = ((wb * hb * n_cells + 255u) & ~255ull);
-        if (hb * n_cells * 2u > 65535u || parts * bins >= 0xffffffffull) {
+        if ((uint64_t)hb * n_cells * 2u > 65535u || draw_parts * aligned_bins >= 0xffffffffull) {
             r->err = "batch: too many cells of this size (bin rows or bin headers exceed what the kernels index)";
             return VB_E_INVALID;
         }
@@ -363,7 +375,6 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.target_height = p->height;
     c.base_color = p->base_color;
     c.layout = r->cur->layout;
-    const uint32_t hb = (c.height_in_tiles + 15u) / 16u, wb = (c.width_in_tiles + 15u) / 16u;
     c.win_by0 = 0;
     c.win_by1 = hb;
     if (p->bin_row1 > p->bin_row0) {
@@ -412,23 +423,8 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
     r->params = *p;
 
-    const VbLayout &L = r->cur->layout;
-    const uint32_t n_draw = L.n_draw_objects, n_paths = L.n_paths, n_clips = L.n_clips;
-    const uint32_t n_tiles = c.width_in_tiles * c.tile_rows;
-    const uint32_t n_bins = wb * hb * n_cells, aligned_n_bins = (n_bins + 255u) & ~255u;
+    const uint32_t n_draw = c.layout.n_draw_objects, n_tiles = c.width_in_tiles * c.tile_rows;
     int rc;
-    if ((rc = ensure(r, r->tag_monoids, (size_t)c.n_tag_words * sizeof(VbTagMonoid)))) return rc;
-    if ((rc = ensure(r, r->path_bboxes, (size_t)n_paths * sizeof(VbPathBbox)))) return rc;
-    if ((rc = ensure(r, r->path_draw, (size_t)n_paths * sizeof(uint2)))) return rc;
-    if ((rc = ensure(r, r->draw_monoids, (size_t)n_draw * sizeof(VbDrawMonoid)))) return rc;
-    if ((rc = ensure(r, r->clip_inp, (size_t)n_clips * sizeof(VbClipInp)))) return rc;
-    if ((rc = ensure(r, r->clip_bboxes, (size_t)n_clips * sizeof(VbBbox4)))) return rc;
-    if ((rc = ensure(r, r->clip_scratch, vb_clip_scratch_words(n_clips) * 4))) return rc;
-    if ((rc = ensure(r, r->draw_bboxes, (size_t)n_draw * sizeof(VbBbox4)))) return rc;
-    if ((rc = ensure(r, r->bin_headers, (size_t)((n_draw + 255u) / 256u) * aligned_n_bins * sizeof(VbBinHeader)))) return rc;
-    if ((rc = ensure(r, r->paths, (size_t)((n_draw + 255u) & ~255u) * sizeof(VbPath)))) return rc;
-    if ((rc = ensure(r, r->tile_start, ((size_t)n_tiles + 256) * 4))) return rc;
-    if ((rc = ensure(r, r->cls_list, (size_t)VB_FINE_CLASSES * n_tiles * 8))) return rc; // fine's cost-ordered tile lists
 
     // arena capacities (elements) start at a first guess and only ever grow; seg_counts and segments follow the capacities
     // before them. A test-only limit lowers the capacity the kernels see, never the allocation (vb_debug_limit_arena).
@@ -458,13 +454,18 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     off += 4 + vb_lookback_words((b.parts_flatten + 8191u) / 8192u, 1);
     const size_t o_draw = off; off += vb_lookback_words(b.parts_draw, 4);
     const size_t o_tile = off; off += vb_lookback_words(b.parts_tile, 1);
-    const size_t o_clip = off; off += vb_lookback_words(vb_clip_parts(n_clips), 1);
+    const size_t o_clip = off; off += vb_lookback_words(vb_clip_parts(c.layout.n_clips), 1);
     const size_t o_backdrop = off; off += vb_lookback_words(b.parts_backdrop, 3);
     b.ctl_words = off;
-    if ((rc = ensure(r, r->ctl, off * 4))) return rc;
-    if ((rc = ensure(r, r->flatten_parts, vb_flatten_part_words(b.parts_flatten) * 4))) return rc;
+
+    // the fixed-size intermediates (FRAME_BUFS)
+    r->counts = {c.n_tag_words, c.layout.n_paths, n_draw, c.layout.n_clips, n_tiles, (uint32_t)draw_parts, (uint32_t)aligned_bins,
+                 b.parts_flatten, b.ctl_words};
+    for (int i = 0; i < N_FIXED_BUFS; i++)
+        if ((rc = ensure(r, r->fb[i], FRAME_BUFS[i].bytes(r->counts, false)))) return rc;
 
     // every buffer has its size: the launchers' view of them
+    for (int i = 0; i < N_FRAME_BUFS; i++) memcpy((char *)&b + FRAME_BUFS[i].field, &r->fb[i].p, sizeof(void *));
     b.scene = (const uint32_t *)r->cur->scene.p;
     b.ramps = (const uint32_t *)r->cur->ramps.p;
     b.atlas = (const uint8_t *)r->cur->atlas.p;
@@ -480,29 +481,6 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.inst_n = r->bound.n;
         b.inst_pitch = r->bound.pitch;
     }
-    b.tag_monoids = (VbTagMonoid *)r->tag_monoids.p;
-    b.path_bboxes = (VbPathBbox *)r->path_bboxes.p;
-    b.path_draw = (uint2 *)r->path_draw.p;
-    b.draw_monoids = (VbDrawMonoid *)r->draw_monoids.p;
-    b.info_bin_data = (uint32_t *)r->info_bin_data.p;
-    b.clip_inp = (VbClipInp *)r->clip_inp.p;
-    b.clip_bboxes = (VbBbox4 *)r->clip_bboxes.p;
-    b.clip_scratch = (int32_t *)r->clip_scratch.p;
-    b.draw_bboxes = (VbBbox4 *)r->draw_bboxes.p;
-    b.bin_headers = (VbBinHeader *)r->bin_headers.p;
-    b.paths = (VbPath *)r->paths.p;
-    b.tile_start = (uint32_t *)r->tile_start.p;
-    b.cls_list = (uint2 *)r->cls_list.p;
-    b.lines = (VbLineSoup *)r->lines.p;
-    b.line_scratch = (FlLit *)r->line_scratch.p;
-    b.flatten_jobs = (FlJob *)r->flatten_jobs.p;
-    b.flatten_parts = (uint32_t *)r->flatten_parts.p;
-    b.tiles = (VbTile *)r->tiles.p;
-    b.seg_counts = (VbSegmentCount *)r->seg_counts.p;
-    b.segments = (VbSegment *)r->segments.p;
-    b.ptcl = (uint32_t *)r->ptcl.p;
-    b.blend_spill = (uint32_t *)r->blend_spill.p;
-    b.ctl = (uint32_t *)r->ctl.p;
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
     b.lb_draw = b.ctl + o_draw;

@@ -42,6 +42,23 @@ enum { ARENA_LINES, ARENA_BINNING, ARENA_TILES, ARENA_SEG_COUNTS, ARENA_SEGMENTS
 static_assert(offsetof(VbConfig, ptcl_size) - offsetof(VbConfig, lines_size) == (N_ARENAS - 1) * sizeof(uint32_t),
               "VbConfig's arena sizes are consecutive words in ARENA_* order");
 
+// The device buffers prepare sizes for each frame, in vb_renderer::fb (FRAME_BUFS below): the fixed-size intermediates, then
+// the bump arenas' buffers (ARENAS) and flatten's two scratch arenas, which ensure_arena sizes.
+enum {
+    FB_TAG_MONOIDS, FB_PATH_BBOXES, FB_PATH_DRAW, FB_DRAW_MONOIDS, FB_CLIP_INP, FB_CLIP_BBOXES, FB_CLIP_SCRATCH, FB_DRAW_BBOXES,
+    FB_BIN_HEADERS, FB_PATHS, FB_TILE_START, FB_CLS_LIST, FB_FLATTEN_PARTS, FB_CTL, N_FIXED_BUFS,
+    FB_LINES = N_FIXED_BUFS, FB_INFO_BIN_DATA, FB_TILES, FB_SEG_COUNTS, FB_SEGMENTS, FB_BLEND_SPILL, FB_PTCL, FB_LINE_SCRATCH,
+    FB_FLATTEN_JOBS, N_FRAME_BUFS
+};
+// The counts the fixed-size intermediates of a frame are sized from, set by prepare (vb_renderer::counts).
+struct FrameCounts {
+    uint32_t tag_words, paths, draws, clips, tiles;
+    uint32_t draw_parts;    // partitions of 256 draw objects (binning's and tile_alloc's)
+    uint32_t aligned_bins;  // the bins of every cell, rounded up to 256: a partition's stride in bin_headers
+    uint32_t flatten_parts; // VbFrameBufs::parts_flatten
+    size_t ctl_words;       // VbFrameBufs::ctl_words: the control block, look-back states included
+};
+
 // Where a frame's pixels go: a device pointer, a registered destination's key, or the renderer's own target (target_alt when
 // `alt`), and optionally a copy of the frame in host memory, read back in `bands` row bands while fine runs. `out` is where
 // fine stores, set from `dev` for each attempt by pick_out (dev itself stays the identity of the destination: the graph key's
@@ -183,9 +200,8 @@ struct vb_renderer {
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
 
-    // fixed-size intermediates
-    DevBuf tag_monoids, path_bboxes, path_draw, draw_monoids, info_bin_data, clip_inp, clip_bboxes, clip_scratch, draw_bboxes, bin_headers, paths,
-        ctl, target, target_alt, tile_start, cls_list;
+    DevBuf fb[N_FRAME_BUFS]; // the frame's intermediates and arenas (FB_*)
+    DevBuf target, target_alt;
     // Renderer::override_image: images (by key) whose pixels come from device memory at the device resolve
     struct Override {
         const uint8_t *src;
@@ -196,9 +212,8 @@ struct vb_renderer {
     std::unordered_map<const void *, Destination> dests; // by key
     DevBuf blit_rects;                  // k_atlas_blit's rectangles, staged through pinned[PIN_BLITS]
     PinnedStage pinned[N_PINNED];
-    // bump arenas (ARENAS), capacities in elements
     DevBuf resolve_tmp; // patches, ramp descriptors and stops of vb_scene_upload_streams
-    DevBuf lines, line_scratch, flatten_jobs, flatten_parts, tiles, seg_counts, segments, ptcl, blend_spill;
+    // bump arenas (ARENAS), capacities in elements
     uint32_t cap[N_ARENAS] = {};
     // test-only capacity limits (vb_debug_limit_arena); UINT32_MAX = none
     uint32_t limit[N_ARENAS] = {UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX, UINT32_MAX};
@@ -211,6 +226,7 @@ struct vb_renderer {
 
     // per-frame
     VbConfig cfg{};
+    FrameCounts counts{}; // of the frame prepare set up last: vb_debug_download returns that much of its intermediates
     vb_params params{};
     Dest dest; // of the frame frame_prepare set up
     uint32_t launches = 0;
@@ -232,7 +248,6 @@ struct vb_renderer {
     cudaEvent_t ev[VB_N_STAGE_IDS + 1]{};
     cudaEvent_t frame_ev[2]{}; // around every whole frame (vb_last_frame_ms: the signal stripe balancing uses)
     bool frame_timed = false;
-    bool ev_ok = false;
     // read-back pipeline of vb_render (host output): fine runs in row bands, each band's D2H copy overlaps the next band
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t band_ev[8]{};
@@ -343,14 +358,11 @@ struct vb_renderer {
 // Every device buffer the renderer owns, each once: what vb_renderer_free frees and vb_frame_stats::arena_bytes counts.
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
-                           &r->mask8, &r->mask16, &r->tag_monoids, &r->path_bboxes, &r->path_draw, &r->draw_monoids, &r->info_bin_data, &r->clip_inp,
-                           &r->clip_bboxes, &r->clip_scratch, &r->draw_bboxes, &r->bin_headers, &r->paths, &r->ctl, &r->tile_start,
-                           &r->cls_list, &r->lines, &r->line_scratch, &r->flatten_jobs, &r->flatten_parts, &r->tiles, &r->seg_counts,
-                           &r->segments, &r->ptcl, &r->blend_spill, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp,
-                           &r->blit_rects, &r->xc.arena, &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps,
-                           &r->spare_atlas};
+                           &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->dmg_mask, &r->dmg_pending,
+                           &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
+    for (DevBuf &b : r->fb) f(b);
 }
 
 #define CK(call)                                                                                  \
@@ -362,14 +374,22 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
         }                                                                                         \
     } while (0)
 
-// One entry per bump arena: the name vb_debug_limit_arena takes, the buffer, its element size and its VbBump counter.
+// One entry per frame buffer (FB_*): its name, where its pointer goes in VbFrameBufs and, for a fixed-size intermediate, its
+// size in a frame of counts `n`: the bytes prepare allocates, or with `download` the bytes vb_debug_download returns by that
+// name (for a downloadable one). The arenas' buffers have no size here: ensure_arena sizes them from the arenas' capacities.
+struct FrameBufDesc {
+    const char *name;
+    size_t field; // offsetof(VbFrameBufs, ...)
+    bool downloadable;
+    size_t (*bytes)(const FrameCounts &n, bool download);
+};
+
+// One entry per bump arena: the name vb_debug_limit_arena takes, the buffer (FB_*), its element size and its VbBump counter.
 // The special cases are in arena_offset, arena_need, ensure_arena and the first guesses of prepare.
-using RendererBuf = DevBuf vb_renderer::*;
 using BumpCounter = uint32_t VbBump::*;
 struct ArenaDesc {
     const char *name;
-    const char *download; // vb_debug_download's name of the buffer when it differs from the arena's
-    RendererBuf buf;
+    int buf;
     size_t elem_bytes;
     BumpCounter counter;
 };
@@ -408,6 +428,7 @@ int ensure(vb_renderer *r, DevBuf &b, size_t bytes);
 int stage_host(vb_renderer *r, PinnedStage &s, size_t bytes, uint8_t **host);
 int stage_copied(vb_renderer *r, PinnedStage &s);
 void hit_forget(vb_renderer *r);
+extern const FrameBufDesc FRAME_BUFS[N_FRAME_BUFS];
 extern const ArenaDesc ARENAS[N_ARENAS];
 int arena_index(const char *name);
 uint64_t ptcl_static(const VbConfig &c);
