@@ -1,11 +1,15 @@
-// vb_resolve.h -- the decisions the library's three Resolver::resolve share, so that their output stays byte-identical: the host
-// resolve (vb_scene_resolve, vb_scene.cpp), the device resolve (vb_scene_upload_streams) and composition (vb_compose, vb_compose.cu).
+// vb_resolve.h -- what the library's three Resolver::resolve share, so that their output stays byte-identical. The host resolve
+// (vb_scene_resolve, vb_scene.cpp) and the device resolve (vb_scene_upload_streams) apply one plan (vb_resolve_plan). Composition
+// (vb_compose.cu) de-duplicates by its fragments' keys, so it shares only the decisions: layout, ramp equality, shelf placement.
 // Internal to the library, and plain C++: vb_scene.cpp is built without the CUDA headers.
 #ifndef VB_RESOLVE_H
 #define VB_RESOLVE_H
 #include <stddef.h>
 #include <stdint.h>
 #include <string.h>
+
+#include <unordered_map>
+#include <vector>
 
 #include "../../include/vello_b200.h"
 
@@ -96,5 +100,59 @@ struct VbShelfPacker {
     }
     uint32_t height() const { return y + shelf_h > 1u ? y + shelf_h : 1u; }
 };
+
+struct RsPatch { uint32_t word, value; }; // one late-bound word of the packed scene, scene[word] = value (k_resolve_finish's input)
+
+// How a scene's streams resolve (resolve.rs:183-399). Two ramp patches share a ramp when vb_same_ramp holds (ramp_cache.rs), two
+// image patches an atlas place when their pixels pointer, width and height match.
+struct VbResolvePlan {
+    struct Image { const uint8_t *pixels; uint32_t w, h, x, y; }; // a distinct image and its atlas place
+    vb_layout layout;
+    uint32_t padded_tags = 0; // bytes
+    size_t words = 0;         // the whole scene
+    std::vector<RsPatch> patches; // every ramp patch's (ramp id << 2) | extend, then every image patch's (x << 16) | y, in stream order
+    std::vector<const vb_ramp_patch *> ramps; // the distinct ramps in ramp-id order, each as its first patch
+    std::vector<Image> images;                // the distinct images in placement order
+    uint32_t atlas_w = 0, atlas_h = 0;
+};
+
+// VB_PLAN_LAYOUT: the scene passes 32-bit word offsets (vb_resolve_layout); nothing else is planned. VB_PLAN_ATLAS: the shelf
+// packer refused an image; the images placed before it stay in the plan, the rest of it is incomplete.
+enum { VB_PLAN_OK, VB_PLAN_LAYOUT, VB_PLAN_ATLAS };
+static inline int vb_resolve_plan(const vb_encoding_streams &e, VbResolvePlan *p) {
+    if (!vb_resolve_layout(e.n_path_tags, e.n_path_data, e.n_draw_tags, e.n_draw_data, e.n_transforms, e.n_styles, e.n_open_clips, e.n_paths,
+                           e.n_clips, vb_draw_info_sum(e.draw_tags, e.n_draw_tags), &p->layout, &p->padded_tags, &p->words))
+        return VB_PLAN_LAYOUT;
+    const uint32_t dd = p->layout.draw_data_base;
+    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
+    for (uint32_t i = 0; i < e.n_ramp_patches; i++) {
+        const vb_ramp_patch &rp = e.ramp_patches[i];
+        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(rp.stops, rp.n_stops, rp.premul_interp != 0u)];
+        uint32_t rid = (uint32_t)p->ramps.size();
+        for (uint32_t k : same_hash) {
+            const vb_ramp_patch &q = *p->ramps[k];
+            if (vb_same_ramp(q.stops, q.n_stops, q.premul_interp != 0u, rp.stops, rp.n_stops, rp.premul_interp != 0u)) { rid = k; break; }
+        }
+        if (rid == p->ramps.size()) {
+            same_hash.push_back(rid);
+            p->ramps.push_back(&rp);
+        }
+        p->patches.push_back(RsPatch{dd + rp.draw_data_offset, (rid << 2) | rp.extend});
+    }
+    VbShelfPacker shelf;
+    for (uint32_t i = 0; i < e.n_image_patches; i++) {
+        const vb_image_patch &im = e.image_patches[i];
+        size_t k = 0;
+        while (k < p->images.size() && !(p->images[k].pixels == im.pixels && p->images[k].w == im.width && p->images[k].h == im.height)) k++;
+        if (k == p->images.size()) {
+            VbResolvePlan::Image q{im.pixels, im.width, im.height, 0, 0};
+            if (!shelf.place(q.w, q.h, &q.x, &q.y)) return VB_PLAN_ATLAS;
+            p->images.push_back(q);
+        }
+        p->patches.push_back(RsPatch{dd + im.draw_data_offset, (p->images[k].x << 16) | p->images[k].y});
+    }
+    p->atlas_w = shelf.width, p->atlas_h = shelf.height();
+    return VB_PLAN_OK;
+}
 
 #endif

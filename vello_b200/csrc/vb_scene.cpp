@@ -19,7 +19,6 @@
 #include <cstring>
 #include <initializer_list>
 #include <new>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/vello_b200_scene.h"
@@ -308,18 +307,18 @@ private:
 };
 
 // ramp_cache.rs:119-155: 512 premultiplied RGBA8 samples
-void make_ramp(const std::vector<Stop> &stops, bool premul, uint32_t *out) {
+void make_ramp(const vb_ramp_stop *stops, uint32_t n, bool premul, uint32_t *out) {
     float last_u = 0.0f, this_u = 0.0f;
-    Color last_c = stops[0].color, this_c = last_c;
-    size_t j = 0;
+    Color last_c{stops[0].r, stops[0].g, stops[0].b, stops[0].a}, this_c = last_c;
+    uint32_t j = 0;
     for (uint32_t i = 0; i < N_RAMP_SAMPLES; i++) {
         const float u = (float)i / (float)(N_RAMP_SAMPLES - 1);
         while (u > this_u) {
             last_u = this_u;
             last_c = this_c;
-            if (j + 1 < stops.size()) {
+            if (j + 1 < n) {
                 this_u = stops[j + 1].offset;
-                this_c = stops[j + 1].color;
+                this_c = Color{stops[j + 1].r, stops[j + 1].g, stops[j + 1].b, stops[j + 1].a};
                 j += 1;
             } else {
                 break;
@@ -1331,91 +1330,6 @@ int vb_scene_batch(vb_scene *dst, const vb_scene *const *scenes, uint32_t n, uin
     return VB_OK;
 }
 
-int vb_scene_resolve(vb_scene *s, vb_packed *out) {
-    if (!s || !out) return VB_E_INVALID;
-    const Encoding &e = s->e;
-    vb_layout L;
-    uint32_t padded;
-    size_t total;
-    if (!vb_resolve_layout(e.path_tags.size(), e.path_data.size(), e.draw_tags.size(), e.draw_data.size(), e.transforms.size(), e.styles.size(),
-                           e.n_open_clips, e.n_paths, e.n_clips, vb_draw_info_sum(e.draw_tags.data(), e.draw_tags.size()), &L, &padded, &total))
-        return VB_E_INVALID;
-
-    // pack the six streams (resolve.rs:107-154); unclosed clips get a trailing PATH tag and END_CLIP draw tag each
-    s->packed.assign(total, 0u);
-    uint8_t *tag_bytes = reinterpret_cast<uint8_t *>(s->packed.data());
-    if (!e.path_tags.empty()) std::memcpy(tag_bytes, e.path_tags.data(), e.path_tags.size());
-    for (uint32_t i = 0; i < e.n_open_clips; i++) tag_bytes[e.path_tags.size() + i] = TAG_PATH;
-    if (!e.path_data.empty()) std::memcpy(&s->packed[L.path_data_base], e.path_data.data(), e.path_data.size() * 4);
-    uint32_t off = L.draw_tag_base;
-    for (uint32_t t : e.draw_tags) s->packed[off++] = t;
-    for (uint32_t i = 0; i < e.n_open_clips; i++) s->packed[off++] = DRAWTAG_END_CLIP;
-    if (!e.draw_data.empty()) std::memcpy(&s->packed[L.draw_data_base], e.draw_data.data(), e.draw_data.size() * 4);
-    off = L.transform_base;
-    for (const Xform &t : e.transforms)
-        for (int i = 0; i < 6; i++) s->packed[off++] = f32_bits(t.c[i]);
-    for (const Style &st : e.styles) {
-        s->packed[off++] = st.flags;
-        s->packed[off++] = f32_bits(st.width);
-    }
-    uint32_t *draw_data = s->packed.data() + L.draw_data_base;
-
-    // late-bound gradient ramps, de-duplicated by (stops, interpolation space) -- ramp_cache.rs
-    std::vector<const RampPatch *> ramp_of;
-    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
-    s->ramps.clear();
-    for (const RampPatch &p : e.ramp_patches) {
-        const uint32_t n = (uint32_t)p.stops.size();
-        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(ramp_stops(p), n, p.premul)];
-        uint32_t rid = (uint32_t)ramp_of.size();
-        for (uint32_t k : same_hash) {
-            const RampPatch &q = *ramp_of[k];
-            if (vb_same_ramp(ramp_stops(q), (uint32_t)q.stops.size(), q.premul, ramp_stops(p), n, p.premul)) { rid = k; break; }
-        }
-        if (rid == ramp_of.size()) {
-            same_hash.push_back(rid);
-            ramp_of.push_back(&p);
-            s->ramps.resize(s->ramps.size() + N_RAMP_SAMPLES);
-            make_ramp(p.stops, p.premul, s->ramps.data() + (size_t)rid * N_RAMP_SAMPLES);
-        }
-        draw_data[p.draw_data_offset] = (rid << 2) | p.extend;
-    }
-    // late-bound images: each distinct (pixels, width, height) placed once in the atlas; a scene whose atlas places do not fit
-    // the draw data's 16-bit fields is refused (VbShelfPacker)
-    struct Placed { const uint8_t *key; uint32_t w, h, x, y; };
-    std::vector<Placed> placed;
-    VbShelfPacker shelf;
-    for (const ImagePatch &p : e.image_patches) {
-        const vb_image &im = p.image;
-        const Placed *hit = nullptr;
-        for (const Placed &q : placed)
-            if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
-        if (!hit) {
-            placed.push_back(Placed{im.pixels, im.width, im.height, 0, 0});
-            if (!shelf.place(im.width, im.height, &placed.back().x, &placed.back().y)) return VB_E_INVALID;
-            hit = &placed.back();
-        }
-        draw_data[p.draw_data_offset] = (hit->x << 16) | hit->y;
-    }
-    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
-    s->atlas.assign((size_t)atlas_w * atlas_h * 4, 0);
-    // a registered texture's key points at nothing (its pixels exist only in device memory): its region stays zero, as for NULL
-    for (const Placed &q : placed)
-        for (uint32_t row = 0; row < q.h && q.key && !vb_texture_key(q.key); row++)
-            std::memcpy(&s->atlas[((size_t)(q.y + row) * atlas_w + q.x) * 4], q.key + (size_t)row * q.w * 4, (size_t)q.w * 4);
-
-    out->scene = reinterpret_cast<const uint8_t *>(s->packed.data());
-    out->scene_len = s->packed.size() * 4;
-    out->layout = L;
-    out->ramps = s->ramps.empty() ? nullptr : s->ramps.data();
-    out->ramp_w = N_RAMP_SAMPLES;
-    out->ramp_h = (uint32_t)(s->ramps.size() / N_RAMP_SAMPLES);
-    out->atlas = s->atlas.data();
-    out->atlas_w = atlas_w;
-    out->atlas_h = atlas_h;
-    return VB_OK;
-}
-
 // The scene's streams as vb_encoding_streams, pointing into the scene (rps / ips hold its patches).
 static void streams_of(const Encoding &e, std::vector<vb_ramp_patch> &rps, std::vector<vb_image_patch> &ips, vb_encoding_streams *st) {
     static_assert(sizeof(Stop) == sizeof(vb_ramp_stop) && sizeof(Xform) == 24 && sizeof(Style) == 8, "stream record layouts");
@@ -1432,6 +1346,60 @@ static void streams_of(const Encoding &e, std::vector<vb_ramp_patch> &rps, std::
     st->n_paths = e.n_paths; st->n_clips = e.n_clips; st->n_open_clips = e.n_open_clips;
     st->ramp_patches = rps.data(); st->n_ramp_patches = (uint32_t)rps.size();
     st->image_patches = ips.data(); st->n_image_patches = (uint32_t)ips.size();
+}
+
+int vb_scene_resolve(vb_scene *s, vb_packed *out) {
+    if (!s || !out) return VB_E_INVALID;
+    const Encoding &e = s->e;
+    // streams_of counts each stream in 32 bits: a longer one passes 32-bit word offsets, as the plan would find
+    for (size_t n : {e.path_tags.size(), e.path_data.size(), e.draw_tags.size(), e.draw_data.size(), e.transforms.size(), e.styles.size()})
+        if (n > UINT32_MAX) return VB_E_INVALID;
+    std::vector<vb_ramp_patch> rps;
+    std::vector<vb_image_patch> ips;
+    vb_encoding_streams st;
+    streams_of(e, rps, ips, &st);
+    VbResolvePlan plan;
+    if (vb_resolve_plan(st, &plan) != VB_PLAN_OK) return VB_E_INVALID;
+    const vb_layout &L = plan.layout;
+
+    // pack the six streams (resolve.rs:107-154); unclosed clips get a trailing PATH tag and END_CLIP draw tag each
+    s->packed.assign(plan.words, 0u);
+    uint8_t *tag_bytes = reinterpret_cast<uint8_t *>(s->packed.data());
+    if (!e.path_tags.empty()) std::memcpy(tag_bytes, e.path_tags.data(), e.path_tags.size());
+    for (uint32_t i = 0; i < e.n_open_clips; i++) tag_bytes[e.path_tags.size() + i] = TAG_PATH;
+    if (!e.path_data.empty()) std::memcpy(&s->packed[L.path_data_base], e.path_data.data(), e.path_data.size() * 4);
+    uint32_t off = L.draw_tag_base;
+    for (uint32_t t : e.draw_tags) s->packed[off++] = t;
+    for (uint32_t i = 0; i < e.n_open_clips; i++) s->packed[off++] = DRAWTAG_END_CLIP;
+    if (!e.draw_data.empty()) std::memcpy(&s->packed[L.draw_data_base], e.draw_data.data(), e.draw_data.size() * 4);
+    off = L.transform_base;
+    for (const Xform &t : e.transforms)
+        for (int i = 0; i < 6; i++) s->packed[off++] = f32_bits(t.c[i]);
+    for (const Style &st : e.styles) {
+        s->packed[off++] = st.flags;
+        s->packed[off++] = f32_bits(st.width);
+    }
+    // the late-bound words, the ramps and the atlas, as planned
+    for (const RsPatch &p : plan.patches) s->packed[p.word] = p.value;
+    s->ramps.resize(plan.ramps.size() * N_RAMP_SAMPLES);
+    for (size_t k = 0; k < plan.ramps.size(); k++)
+        make_ramp(plan.ramps[k]->stops, plan.ramps[k]->n_stops, plan.ramps[k]->premul_interp != 0u, s->ramps.data() + k * N_RAMP_SAMPLES);
+    s->atlas.assign((size_t)plan.atlas_w * plan.atlas_h * 4, 0);
+    // a registered texture's key points at nothing (its pixels exist only in device memory): its region stays zero, as for NULL
+    for (const VbResolvePlan::Image &q : plan.images)
+        for (uint32_t row = 0; row < q.h && q.pixels && !vb_texture_key(q.pixels); row++)
+            std::memcpy(&s->atlas[((size_t)(q.y + row) * plan.atlas_w + q.x) * 4], q.pixels + (size_t)row * q.w * 4, (size_t)q.w * 4);
+
+    out->scene = reinterpret_cast<const uint8_t *>(s->packed.data());
+    out->scene_len = s->packed.size() * 4;
+    out->layout = L;
+    out->ramps = s->ramps.empty() ? nullptr : s->ramps.data();
+    out->ramp_w = N_RAMP_SAMPLES;
+    out->ramp_h = (uint32_t)plan.ramps.size();
+    out->atlas = s->atlas.data();
+    out->atlas_w = plan.atlas_w;
+    out->atlas_h = plan.atlas_h;
+    return VB_OK;
 }
 
 // Shapes to pixels: the scene's streams are resolved ON THE DEVICE (vb_scene_upload_streams: stream copies to their Layout offsets,

@@ -9,6 +9,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "vb_resolve.h"
 #include "vb_types.h"
 
 struct FlLit; // flatten's scratch records (k_flatten.cu)
@@ -96,8 +97,7 @@ struct XPeers {
     unsigned long long half_bytes;
 };
 
-// k_resolve.cu: records of the device resolve, staged by vb_scene_upload_streams
-struct RsPatch { uint32_t word, value; };                        // scene[word] = value
+// k_resolve.cu: records of the device resolve, staged by vb_scene_upload_streams and vb_compose (and RsPatch, vb_resolve.h)
 struct RsRamp { uint32_t first_stop, n_stops, premul, pad; };     // one gradient ramp: its stops and interpolation space
 struct RsStop { float offset, r, g, b, a; };                      // == vb_ramp_stop
 

@@ -532,70 +532,43 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (!r || !e) return VB_E_INVALID;
     int rc = check_streams(r, e, "vb_scene_upload_streams");
     if (rc) return rc;
-    VbLayout L;
-    uint32_t padded;
-    size_t total_words;
-    if (!vb_resolve_layout(e->n_path_tags, e->n_path_data, e->n_draw_tags, e->n_draw_data, e->n_transforms, e->n_styles, e->n_open_clips, e->n_paths,
-                           e->n_clips, vb_draw_info_sum(e->draw_tags, e->n_draw_tags), &L, &padded, &total_words)) {
+    VbResolvePlan plan;
+    const int planned = vb_resolve_plan(*e, &plan);
+    if (planned == VB_PLAN_LAYOUT) {
         r->err = "vb_scene_upload_streams: the scene exceeds 32-bit word offsets";
         return VB_E_INVALID;
     }
+    VbLayout L;
+    memcpy(&L, &plan.layout, sizeof L);
     if ((rc = drain_stream(r))) return rc;
     CK(cudaSetDevice(r->device));
     cudaStream_t st = r->stream;
-    std::vector<RsPatch> patches;
-    std::vector<RsRamp> ramps;
-    std::vector<vb_ramp_stop> stops;
-    // late-bound gradient ramps, de-duplicated by (stops, interpolation space) as the host resolve does
-    std::vector<const vb_ramp_patch *> ramp_of;
-    std::unordered_map<uint64_t, std::vector<uint32_t>> ramp_ids; // by vb_ramp_hash
-    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
-        const vb_ramp_patch &p = e->ramp_patches[i];
-        std::vector<uint32_t> &same_hash = ramp_ids[vb_ramp_hash(p.stops, p.n_stops, p.premul_interp != 0u)];
-        uint32_t rid = (uint32_t)ramp_of.size();
-        for (uint32_t k : same_hash) {
-            const vb_ramp_patch &q = *ramp_of[k];
-            if (vb_same_ramp(q.stops, q.n_stops, q.premul_interp != 0u, p.stops, p.n_stops, p.premul_interp != 0u)) { rid = k; break; }
-        }
-        if (rid == ramp_of.size()) {
-            same_hash.push_back(rid);
-            ramp_of.push_back(&p);
-            ramps.push_back(RsRamp{(uint32_t)stops.size(), p.n_stops, p.premul_interp ? 1u : 0u, 0u});
-            stops.insert(stops.end(), p.stops, p.stops + p.n_stops);
-        }
-        patches.push_back(RsPatch{L.draw_data_base + p.draw_data_offset, (rid << 2) | p.extend});
-    }
-    // late-bound images: each distinct (pixels, width, height) placed once in the atlas, filled from an override on this
-    // renderer (one k_atlas_blit) or from the host
-    struct Placed { const uint8_t *key; uint32_t w, h, x, y; bool from_device; };
-    std::vector<Placed> placed;
+    // each planned image is filled from an override on this renderer (one k_atlas_blit) or from the host; the images placed
+    // before one the atlas refused are checked first, as when each image is placed and checked in turn
     std::vector<VbBlitRect> blits;
     std::vector<vb_renderer::SceneSlot::OverridePlace> over;
-    VbShelfPacker shelf;
-    for (uint32_t i = 0; i < e->n_image_patches; i++) {
-        const vb_image_patch &im = e->image_patches[i];
-        const Placed *hit = nullptr;
-        for (const Placed &q : placed)
-            if (q.key == im.pixels && q.w == im.width && q.h == im.height) { hit = &q; break; }
-        if (!hit) {
-            Placed q{im.pixels, im.width, im.height, 0, 0, false};
-            if (!shelf.place(q.w, q.h, &q.x, &q.y)) {
-                r->err = "device resolve: an image's atlas place or size passes 16 bits (at most 65535 rows of shelves and 65535 "
-                         "texels a side)";
-                return VB_E_INVALID;
-            }
-            if ((rc = image_source(r, "device resolve", q.key, q.w, q.h, q.x, q.y, blits, over, &q.from_device))) return rc;
-            placed.push_back(q);
-            hit = &placed.back();
-        }
-        patches.push_back(RsPatch{L.draw_data_base + im.draw_data_offset, (hit->x << 16) | hit->y});
+    std::vector<const VbResolvePlan::Image *> from_host;
+    for (const VbResolvePlan::Image &q : plan.images) {
+        bool overridden;
+        if ((rc = image_source(r, "device resolve", q.pixels, q.w, q.h, q.x, q.y, blits, over, &overridden))) return rc;
+        if (!overridden && q.pixels && q.w && q.h) from_host.push_back(&q);
     }
-    const uint32_t atlas_w = shelf.width, atlas_h = shelf.height();
+    if (planned == VB_PLAN_ATLAS) {
+        r->err = "device resolve: an image's atlas place or size passes 16 bits (at most 65535 rows of shelves and 65535 "
+                 "texels a side)";
+        return VB_E_INVALID;
+    }
+    std::vector<RsRamp> ramps;
+    std::vector<vb_ramp_stop> stops;
+    for (const vb_ramp_patch *p : plan.ramps) {
+        ramps.push_back(RsRamp{(uint32_t)stops.size(), p->n_stops, p->premul_interp ? 1u : 0u, 0u});
+        stops.insert(stops.end(), p->stops, p->stops + p->n_stops);
+    }
     DiffedUpload guard;
-    if ((rc = upload_diff_begin(r, st, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, guard))) return rc;
+    if ((rc = upload_diff_begin(r, st, L, plan.words, (uint32_t)ramps.size(), plan.atlas_w, plan.atlas_h, guard))) return rc;
 
     // the six streams go straight to their places in the packed buffer
-    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, total_words, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, plan.words, r->view.on)))) return rc;
     char *base = (char *)r->cur->scene.p;
     if (e->n_path_tags) CK(cudaMemcpyAsync(base, e->path_tags, e->n_path_tags, cudaMemcpyHostToDevice, st));
     if (e->n_path_data) CK(cudaMemcpyAsync(base + (size_t)L.path_data_base * 4, e->path_data, (size_t)e->n_path_data * 4, cudaMemcpyHostToDevice, st));
@@ -605,29 +578,27 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if (e->n_styles) CK(cudaMemcpyAsync(base + (size_t)L.style_base * 4, e->styles, (size_t)e->n_styles * 8, cudaMemcpyHostToDevice, st));
     // patches, ramp descriptors and stops in one staging buffer
     static_assert(sizeof(RsStop) == sizeof(vb_ramp_stop), "the stops are staged as the caller gave them");
-    const size_t pb = patches.size() * sizeof(RsPatch), rb = ramps.size() * sizeof(RsRamp), sb = stops.size() * sizeof(vb_ramp_stop);
+    const size_t pb = plan.patches.size() * sizeof(RsPatch), rb = ramps.size() * sizeof(RsRamp), sb = stops.size() * sizeof(vb_ramp_stop);
     const size_t o_r = (pb + 15) & ~(size_t)15, o_s = (o_r + rb + 15) & ~(size_t)15;
     if ((rc = ensure(r, r->resolve_tmp, o_s + sb + 16))) return rc;
     char *tmp = (char *)r->resolve_tmp.p;
-    if (pb) CK(cudaMemcpyAsync(tmp, patches.data(), pb, cudaMemcpyHostToDevice, st));
+    if (pb) CK(cudaMemcpyAsync(tmp, plan.patches.data(), pb, cudaMemcpyHostToDevice, st));
     if (rb) CK(cudaMemcpyAsync(tmp + o_r, ramps.data(), rb, cudaMemcpyHostToDevice, st));
     if (sb) CK(cudaMemcpyAsync(tmp + o_s, stops.data(), sb, cudaMemcpyHostToDevice, st));
-    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, padded, L.draw_tag_base + e->n_draw_tags,
-                             (const RsPatch *)tmp, (uint32_t)patches.size(), st);
+    vb_launch_resolve_finish((uint32_t *)r->cur->scene.p, e->n_path_tags, e->n_open_clips, plan.padded_tags, L.draw_tag_base + e->n_draw_tags,
+                             (const RsPatch *)tmp, (uint32_t)plan.patches.size(), st);
     if ((rc = ensure(r, r->cur->ramps, ramps.size() * 512 * 4))) return rc;
     vb_launch_make_ramps((const RsRamp *)(tmp + o_r), (const RsStop *)(tmp + o_s), (uint32_t)ramps.size(), (uint32_t *)r->cur->ramps.p, st);
-    if ((rc = ensure(r, r->cur->atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
-    CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)atlas_w * atlas_h * 4, st));
-    for (const Placed &q : placed) {
-        if (q.key && q.w && q.h && !q.from_device)
-            CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q.y * atlas_w + q.x) * 4, (size_t)atlas_w * 4, q.key, (size_t)q.w * 4, (size_t)q.w * 4, q.h,
-                                 cudaMemcpyHostToDevice, st));
-    }
-    if ((rc = enqueue_blits(r, blits, r->cur->atlas.p, atlas_w))) return rc;
+    if ((rc = ensure(r, r->cur->atlas, (size_t)plan.atlas_w * plan.atlas_h * 4))) return rc;
+    CK(cudaMemsetAsync(r->cur->atlas.p, 0, (size_t)plan.atlas_w * plan.atlas_h * 4, st));
+    for (const VbResolvePlan::Image *q : from_host)
+        CK(cudaMemcpy2DAsync((char *)r->cur->atlas.p + ((size_t)q->y * plan.atlas_w + q->x) * 4, (size_t)plan.atlas_w * 4, q->pixels, (size_t)q->w * 4,
+                             (size_t)q->w * 4, q->h, cudaMemcpyHostToDevice, st));
+    if ((rc = enqueue_blits(r, blits, r->cur->atlas.p, plan.atlas_w))) return rc;
     CK(cudaGetLastError());
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
-    set_scene(r, L, total_words, (uint32_t)ramps.size(), atlas_w, atlas_h, std::move(over), false);
+    set_scene(r, L, plan.words, (uint32_t)ramps.size(), plan.atlas_w, plan.atlas_h, std::move(over), false);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
