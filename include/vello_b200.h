@@ -97,7 +97,7 @@ int vb_scene_upload(vb_renderer *, const uint8_t *scene, size_t scene_len, const
                     uint32_t ramp_w, uint32_t ramp_h, const uint8_t *atlas_rgba8, uint32_t atlas_w, uint32_t atlas_h);
 
 /* Render the uploaded scene. `out` is a DEVICE pointer (RGBA8, un-premultiplied, pitch 4*width), the key of a registered
- * destination (vb_register_destination: a pitched buffer or a CUDA array, RGBA8 or BGRA8), or NULL to render into the
+ * destination (vb_register_destination: a pitched buffer or a CUDA array, RGBA8, BGRA8, RGBA16F or RGBA32F), or NULL to render into the
  * renderer's own target (see vb_target). Blocks until the frame is complete and arenas were large enough (re-running if not). */
 int vb_render_resident(vb_renderer *, const vb_params *, void *out_device, vb_frame_stats *);
 
@@ -203,9 +203,17 @@ int vb_copy_to_host(vb_renderer *, const void *src_device, void *dst_host, size_
  * cudaGetMipmappedArrayLevel(.., 0). vb_register_destination turns such an array, or linear device memory at any row pitch,
  * into a key, which goes wherever a device destination pointer goes: vb_render_resident, vb_render_enqueue / vb_frame_finish,
  * vb_render_uploaded, vb_render and vb_render_scene with out_is_device = 1, and vb_run_stages.
- *  - Pixel (px, py) of a frame lands at texel (x + px, y + py) of the array, or at ptr + py * row_pitch_bytes + 4 * px. The
- *    bytes are the frame's un-premultiplied RGBA8, with r and b swapped for VB_DEST_BGRA8. No colour conversion is done: an
- *    _SRGB image receives vello's bytes as they are (already sRGB-encoded values).
+ *  - Pixel (px, py) of a frame lands at texel (x + px, y + py) of the array, or at ptr + py * row_pitch_bytes + T * px, where
+ *    the texel size T is 4 (RGBA8, BGRA8), 8 (RGBA16F) or 16 (RGBA32F).
+ *  - Values: let c be fine's premultiplied f32 pixel and clamp01(v) = fminf(1, fmaxf(0, v)) (NaN gives 0). With straight
+ *    alpha (the default, vello's) a texel is clamp01(c.rgb * (1 / fmaxf(c.a, 1e-6f))) and clamp01(c.a); with
+ *    VB_DEST_PREMULTIPLIED in format (for the compositors that take premultiplied pixels) it is clamp01(c). RGBA8 and BGRA8
+ *    store floor(0.5 + 255 * value) of those (the RGBA8 straight bytes are exactly a plain pointer's), with r and b swapped
+ *    for BGRA8; RGBA16F stores them rounded to the nearest half (ties to even); RGBA32F stores them as they are. No colour
+ *    conversion is done: an _SRGB or a float image receives vello's sRGB-encoded values as they are.
+ *  - What the float formats add: coverage at edges, blurs, filtered images and translucent overlaps keep their f32 values.
+ *    Layers (the blend stack), gradient ramps and images are 8-bit inside fine, as in vello, so a flat gradient fill or an
+ *    unscaled image gains nothing.
  *  - A destination holds the whole frame, so a bin_row / tile_row window writes only its rows, at their own rows of the
  *    destination. (A plain pointer differs: its first row is the window's first row.)
  *  - Damage tracking: a frame into the same key as the last successful frame can be incremental, writing only its damaged
@@ -213,12 +221,14 @@ int vb_copy_to_host(vb_renderer *, const void *src_device, void *dst_host, size_
  *  - Keys come from the same reserved, inaccessible address range as vb_register_texture's keys: no buffer has a key's
  *    address, a key is never handed out twice, and a key used as an image key reads as an unregistered texture key does.
  * VB_E_INVALID (vb_last_error says why), each checked on the host before anything is enqueued:
- *  - registering: NULL arguments; an unknown kind or format; a renderer of a vb_group or with the exchange configured;
- *    LINEAR: ptr NULL, not 4-byte aligned, or not device or managed memory of the renderer's device; a row pitch that is not a
- *    multiple of 4 or is 2^34 bytes or more; ARRAY: not a 2-D array (1-D, layered, cubemap, 3-D), channels other than four
- *    8-bit cudaChannelFormatKindUnsigned ones, no cudaArraySurfaceLoadStore flag;
+ *  - registering: NULL arguments; an unknown kind, format or flag bit; a renderer of a vb_group or with the exchange
+ *    configured; LINEAR: ptr NULL, not a multiple of the texel size T, or not device or managed memory of the renderer's
+ *    device; a row pitch that is not a multiple of T or is 2^34 bytes or more; ARRAY: not a 2-D array (1-D, layered,
+ *    cubemap, 3-D), channels that do not match the format (four 8-bit cudaChannelFormatKindUnsigned ones for RGBA8 and
+ *    BGRA8, four 16-bit cudaChannelFormatKindFloat ones for RGBA16F, four 32-bit ones for RGBA32F), no
+ *    cudaArraySurfaceLoadStore flag;
  *  - a frame into a key: the key is unregistered, another renderer's or a texture key; the frame does not fit (x + width or
- *    y + its last row past the array's extent, a row pitch below 4 * width); a batch (vb_set_cells with more than one cell);
+ *    y + its last row past the array's extent, a row pitch below T * width); a batch (vb_set_cells with more than one cell);
  *  - a key where a host pointer or a plain device pointer is needed: vb_render / vb_render_uploaded / vb_render_scene with
  *    out_is_device = 0, vb_render_begin's out_host, vb_copy_to_host, image pixels (vb_override_image, vb_register_texture),
  *    vb_group destinations.
@@ -230,6 +240,9 @@ int vb_copy_to_host(vb_renderer *, const void *src_device, void *dst_host, size_
 #define VB_DEST_ARRAY 1  /* a 2-D CUDA array (cudaArray_t / CUarray), written through a surface object */
 #define VB_DEST_RGBA8 0  /* byte order of a stored pixel: vello's Rgba8Unorm (r in the low byte) */
 #define VB_DEST_BGRA8 1  /* b, g, r, a */
+#define VB_DEST_RGBA16F 2 /* four IEEE half floats r, g, b, a: 8 bytes a texel */
+#define VB_DEST_RGBA32F 3 /* four floats r, g, b, a: 16 bytes a texel */
+#define VB_DEST_PREMULTIPLIED 0x100 /* OR'd into format: premultiplied alpha instead of straight */
 typedef struct {
     uint32_t kind, format;
     void *ptr;              /* LINEAR: where pixel (0, 0) of a frame goes */

@@ -49,8 +49,10 @@ pub struct VbEncodingStreams {
     pub image_patches: *const VbImagePatch, pub n_image_patches: u32,
 }
 
-/// a registered destination (vb_register_destination): VB_DEST_LINEAR 0 / VB_DEST_ARRAY 1, VB_DEST_RGBA8 0 / VB_DEST_BGRA8 1.
-/// For a wgpu/Vulkan storage texture: the image's memory imported into CUDA, level 0 of its mipmapped array in `array`.
+/// a registered destination (vb_register_destination): VB_DEST_LINEAR 0 / VB_DEST_ARRAY 1, VB_DEST_RGBA8 0 / VB_DEST_BGRA8 1 /
+/// VB_DEST_RGBA16F 2 / VB_DEST_RGBA32F 3, optionally | VB_DEST_PREMULTIPLIED 0x100 (premultiplied instead of straight alpha).
+/// For a wgpu/Vulkan storage texture: the image's memory imported into CUDA, level 0 of its mipmapped array in `array`
+/// (an Rgba16Float / R16G16B16A16_SFLOAT image takes VB_DEST_RGBA16F).
 #[repr(C)]
 pub struct VbDestination { pub kind: u32, pub format: u32, pub ptr: *mut c_void, pub row_pitch_bytes: usize, pub array: *mut c_void, pub x: u32, pub y: u32 }
 

@@ -91,13 +91,67 @@ struct FineArgs {
     uint32_t cull;              // 1: start each tile there
 };
 // The arguments of the FI_DST instantiations: FineArgs, then a registered destination's (vb_launch_fine's VbFineOut): the
-// __byte_perm selector of the stored byte order, and either linear memory at `out` or, with `array`, the surface of a CUDA
-// array, pixel (x, y) of the frame at texel (x0 + x, y0 + y). The other instantiations take FineArgs alone, so that their code
-// is exactly what it was before destinations existed (a larger parameter block alone changes ptxas's register assignment).
+// __byte_perm selector of the stored byte order, the texel size (4: 8-bit, 8: RGBA16F, 16: RGBA32F), premultiplied or straight
+// alpha, and either linear memory at `out` or, with `array`, the surface of a CUDA array, pixel (x, y) of the frame at texel
+// (x0 + x, y0 + y). The other instantiations take FineArgs alone, so that their code is exactly what it was before destinations
+// existed (a larger parameter block alone changes ptxas's register assignment).
 struct FineDstArgs : FineArgs {
     cudaSurfaceObject_t surf;
-    uint32_t swz, array, x0, y0;
+    uint32_t swz, array, x0, y0, texel, premul;
 };
+
+// The store of a float destination (FI_DST, texel 8 or 16), for a lane's PX pixels at frame row gy, columns gx..gx+7 (gx a
+// multiple of 8). Each texel is clamp01 (unorm8's clamp, NaN to 0) of the premultiplied pixel, or of its straight colour
+// rgb * (1 / max(a, 1e-6)) and alpha: the values the 8-bit store rounds. When every pixel of the warp is opaque the factor is
+// exactly 1 and is skipped, as there. RGBA16F rounds them to nearest even halves. cfg.out_pitch_px is the pitch in texels.
+__device__ __forceinline__ float clamp01(float x) { return fminf(1.0f, fmaxf(0.0f, x)); }
+__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
+    return (uint32_t)__half_as_ushort(__float2half_rn(lo)) | ((uint32_t)__half_as_ushort(__float2half_rn(hi)) << 16);
+}
+__device__ __forceinline__ void store_float(const FineDstArgs &A, const VbConfig &cfg, rgba_t (&rgba)[PX], uint32_t gx, uint32_t gy,
+                                            bool all_opaque) {
+    const bool straight = A.premul == 0u && !all_opaque;
+#pragma unroll
+    for (int i = 0; i < PX; i++) {
+        const rgba_t c = rgba[i];
+        const float k = straight ? 1.0f / fmaxf(c.a, 1e-6f) : 1.0f;
+        rgba[i] = straight ? RG(clamp01(c.r * k), clamp01(c.g * k), clamp01(c.b * k), clamp01(c.a))
+                           : RG(clamp01(c.r), clamp01(c.g), clamp01(c.b), clamp01(c.a));
+    }
+    const bool full = gx + 7u < cfg.target_width;
+    const uint32_t x = A.x0 + gx, y = A.y0 + gy;
+    char *row = (char *)A.out + (size_t)(gy - cfg.out_row0) * cfg.out_pitch_px * A.texel;
+    if (A.texel == 16u) {
+        // one 128-bit store per texel: the registered pointer and pitch are multiples of 16
+#pragma unroll
+        for (int i = 0; i < PX; i++) {
+            if (!full && gx + i >= cfg.target_width) continue;
+            const float4 v = make_float4(rgba[i].r, rgba[i].g, rgba[i].b, rgba[i].a);
+            if (A.array) surf2Dwrite(v, A.surf, (int)((x + i) * 16u), (int)y, cudaBoundaryModeZero);
+            else reinterpret_cast<float4 *>(row)[gx + i] = v;
+        }
+        return;
+    }
+    uint2 t[PX];
+#pragma unroll
+    for (int i = 0; i < PX; i++) t[i] = make_uint2(half2_bits(rgba[i].r, rgba[i].g), half2_bits(rgba[i].b, rgba[i].a));
+    if (full && (A.array ? (x & 1u) == 0u : (cfg.out_pitch_px & 1u) == 0u && ((uintptr_t)A.out & 15u) == 0u)) {
+        // four 128-bit stores of two texels each: the lane's 64 contiguous bytes
+#pragma unroll
+        for (int i = 0; i < PX; i += 2) {
+            const uint4 v = make_uint4(t[i].x, t[i].y, t[i + 1].x, t[i + 1].y);
+            if (A.array) surf2Dwrite(v, A.surf, (int)((x + i) * 8u), (int)y, cudaBoundaryModeZero);
+            else reinterpret_cast<uint4 *>(row)[(gx + i) / 2u] = v;
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < PX; i++) {
+            if (gx + i >= cfg.target_width) continue;
+            if (A.array) surf2Dwrite(t[i], A.surf, (int)((x + i) * 8u), (int)y, cudaBoundaryModeZero);
+            else reinterpret_cast<uint2 *>(row)[gx + i] = t[i];
+        }
+    }
+}
 
 // ---------------- mbarrier + bulk-copy (TMA) primitives: PTX as in cute/arch/copy_sm90_tma.hpp, cutlass/arch/barrier.h ----------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -781,8 +835,8 @@ static_assert(sizeof(WarpIo) % 16 == 0 && sizeof(WarpMs<1>) % 16 == 0 && sizeof(
 
 // MODE: the AA mode (0 area, 1 MSAA8, 2 MSAA16), plus FI_DMG for damage tracking (k_damage.cu): coarse listed only the
 // damaged tiles, and those lists are the whole queue, so no other pixel is written. Without FI_DMG the kernel is the one it was
-// before damage tracking existed. FI_DST: a registered destination (vb_register_destination) in BGRA8 order or in a CUDA array;
-// only the store differs.
+// before damage tracking existed. FI_DST: a registered destination (vb_register_destination) in BGRA8 order, with premultiplied
+// alpha, in a float format or in a CUDA array; only the store differs.
 #define FI_DMG 16
 #define FI_DST 32
 template <int MODE> using FineArgsOf = typename std::conditional<(MODE & FI_DST) != 0, FineDstArgs, FineArgs>::type;
@@ -1209,16 +1263,27 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
 #undef xyx0
 #undef xyx1
         // ---- store: rgba8unorm with separated alpha (fine.wgsl:1386-1397). When every pixel of the warp is opaque
-        // (the common case) a_inv is exactly 1 and the three multiplications are identities, so they are skipped.
+        // (the common case) a_inv is exactly 1 and the three multiplications are identities, so they are skipped. FI_DST also
+        // stores premultiplied alpha (unorm8 of each channel) and float texels (store_float).
         bool opaque = true;
 #pragma unroll
         for (int i = 0; i < PX; i++) opaque = opaque && rgba[i].a == 1.0f;
         const bool all_opaque = __all_sync(VB_FULL, opaque);
-        if (gy < cfg.target_height && gy >= cfg.out_row0) {
+        bool float_texels = false, premul = false; // FI_DST: a float destination, premultiplied alpha
+        if constexpr (DST) {
+            float_texels = A.texel != 4u;
+            premul = A.premul != 0u;
+        }
+        if (float_texels && gy < cfg.target_height && gy >= cfg.out_row0) {
+            if constexpr (DST) store_float(A, cfg, rgba, gx, gy, all_opaque);
+        } else if (gy < cfg.target_height && gy >= cfg.out_row0) {
             uint32_t px[PX];
             if (all_opaque) {
 #pragma unroll
                 for (int i = 0; i < PX; i++) px[i] = unorm8(rgba[i].r) | (unorm8(rgba[i].g) << 8) | (unorm8(rgba[i].b) << 16) | 0xff000000u;
+            } else if (premul) {
+#pragma unroll
+                for (int i = 0; i < PX; i++) px[i] = pack4x8unorm(rgba[i]);
             } else {
 #pragma unroll
                 for (int i = 0; i < PX; i++) {
@@ -1325,6 +1390,8 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     A.array = o.array;
     A.x0 = o.x0;
     A.y0 = o.y0;
+    A.texel = o.texel;
+    A.premul = o.premul;
     const bool dmg = b.dmg_mode == VB_DMG_INCREMENTAL && cls_order; // the damaged tiles of coarse's lists only
     if (o.dst) {
         if (dmg) launch_fine<FI_DST + FI_DMG>(aa, grid, warps, st, cfg, A);

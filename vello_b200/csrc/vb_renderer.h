@@ -71,9 +71,12 @@ struct Dest {
 };
 
 // A registered destination (vb_register_destination), found by its key in vb_renderer::dests. LINEAR: pixel (x, y) of a frame
-// at ptr + y * pitch + 4 * x. ARRAY: at texel (x + x0, y + y0) of a w x h array, written through surf.
+// at ptr + y * pitch + texel() * x. ARRAY: at texel (x + x0, y + y0) of a w x h array, written through surf. `format` is the
+// texel format alone; `premul` is VB_DEST_PREMULTIPLIED.
 struct Destination {
     uint32_t kind = VB_DEST_LINEAR, format = VB_DEST_RGBA8;
+    bool premul = false;
+    uint32_t texel() const { return format == VB_DEST_RGBA32F ? 16u : format == VB_DEST_RGBA16F ? 8u : 4u; } // bytes
     uint8_t *ptr = nullptr;
     size_t pitch = 0;
     cudaSurfaceObject_t surf = 0;

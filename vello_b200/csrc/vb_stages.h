@@ -127,13 +127,14 @@ uint32_t vb_backdrop_parts(uint32_t tiles_size);
 uint32_t vb_launch_coarse(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_path_tiling(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 // Where fine stores a frame. Without `dst`: RGBA8 at `out`, cfg.out_pitch_px pixels a row, frame row cfg.out_row0 at out[0].
-// With `dst` (a registered destination in BGRA8 order or in a CUDA array; the FI_DST instantiations): each pixel's bytes are
-// permuted by __byte_perm selector `swz`, then stored as without `dst`, or with `array` through `surf`, frame pixel (x, y) at
-// texel (x0 + x, y0 + y).
+// With `dst` (a registered destination other than linear RGBA8 with straight alpha; the FI_DST instantiations): texels of
+// `texel` bytes (4: 8-bit, 8: RGBA16F, 16: RGBA32F) with straight or, with `premul`, premultiplied alpha, cfg.out_pitch_px
+// texels a row. An 8-bit pixel's bytes are permuted by __byte_perm selector `swz`. They are stored as without `dst`, or with
+// `array` through `surf`, frame pixel (x, y) at texel (x0 + x, y0 + y).
 struct VbFineOut {
     uint32_t *out;
     cudaSurfaceObject_t surf;
-    uint32_t dst, swz, array, x0, y0;
+    uint32_t dst, swz, array, x0, y0, texel, premul;
 };
 // tile rows cfg.win_ty0..win_ty1 into `o`; `band` picks the launch's tile queue (one of 8 control-block words) and
 // cls_order starts the tiles in coarse's cost order

@@ -331,27 +331,31 @@ extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
 }
 
 // ---- registered destinations: vb_register_destination / vb_unregister_destination ------------------------------------------
-// Frames into a destination's key store through k_fine's FI_DST instantiations, except linear RGBA8, which is the default store
-// at another pitch and origin. Every check is made here or in resolve_destination, on the host, before a frame is enqueued.
+// Frames into a destination's key store through k_fine's FI_DST instantiations, except linear RGBA8 with straight alpha, which
+// is the default store at another pitch and origin. Every check is made here or in resolve_destination, on the host, before a
+// frame is enqueued. The texel size (Destination::texel) sets the alignment, pitch and channel checks and fine's store.
 extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, void **key_out) {
     if (!r) return VB_E_INVALID;
-    auto bad = [&](const char *why) {
+    auto bad = [&](const std::string &why) {
         r->err = std::string("vb_register_destination: ") + why;
         return VB_E_INVALID;
     };
     if (!d || !key_out) return bad("NULL destination or key_out");
     if (d->kind != VB_DEST_LINEAR && d->kind != VB_DEST_ARRAY) return bad("unknown kind");
-    if (d->format != VB_DEST_RGBA8 && d->format != VB_DEST_BGRA8) return bad("unknown format");
+    const uint32_t fmt = d->format & ~(uint32_t)VB_DEST_PREMULTIPLIED;
+    if (fmt > VB_DEST_RGBA32F) return bad("unknown format or flag");
     if (r->grouped || r->xc.configured) return bad("not available for a renderer of a vb_group or with the exchange configured");
     CK(cudaSetDevice(r->device));
     Destination D;
     D.kind = d->kind;
-    D.format = d->format;
+    D.format = fmt;
+    D.premul = (d->format & VB_DEST_PREMULTIPLIED) != 0u;
+    const uint32_t T = D.texel();
     if (d->kind == VB_DEST_LINEAR) {
         if (!d->ptr) return bad("NULL ptr");
-        if ((uintptr_t)d->ptr & 3u) return bad("ptr is not 4-byte aligned");
+        if ((uintptr_t)d->ptr % T) return bad("ptr is not " + std::to_string(T) + "-byte aligned");
         if (vb_texture_key(d->ptr) || !device_memory_of(r, d->ptr)) return bad("ptr is not device or managed memory of the renderer's device");
-        if (d->row_pitch_bytes & 3u) return bad("row_pitch_bytes is not a multiple of 4");
+        if (d->row_pitch_bytes % T) return bad("row_pitch_bytes is not a multiple of " + std::to_string(T));
         if (d->row_pitch_bytes >= ((size_t)1 << 34)) return bad("row_pitch_bytes is 2^34 or more");
         D.ptr = (uint8_t *)d->ptr;
         D.pitch = d->row_pitch_bytes;
@@ -366,8 +370,11 @@ extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, 
         }
         if (ext.depth != 0 || ext.height == 0 || (flags & (cudaArrayLayered | cudaArrayCubemap)))
             return bad("a 1-D, layered, cubemap or 3-D array (a 2-D array is needed)");
-        if (fd.f != cudaChannelFormatKindUnsigned || fd.x != 8 || fd.y != 8 || fd.z != 8 || fd.w != 8)
-            return bad("the array's channels are not four 8-bit unsigned ones");
+        // four channels of T / 4 bytes each: unsigned for the 8-bit formats, float for the others
+        const int bits = (int)(2u * T);
+        if (fd.f != (T == 4u ? cudaChannelFormatKindUnsigned : cudaChannelFormatKindFloat) || fd.x != bits || fd.y != bits ||
+            fd.z != bits || fd.w != bits)
+            return bad("the array's channels are not four " + std::to_string(bits) + (T == 4u ? "-bit unsigned ones" : "-bit float ones"));
         if (!(flags & cudaArraySurfaceLoadStore)) return bad("the array was not created with cudaArraySurfaceLoadStore");
         cudaResourceDesc rd;
         memset(&rd, 0, sizeof rd);
@@ -407,7 +414,7 @@ extern "C" int vb_unregister_destination(vb_renderer *r, void *key) {
 // The frame r prepared goes to d->dev, a key: check that the frame fits the destination, and say where fine stores (d->out).
 // A linear destination holds the whole frame, so a window's rows land at their own rows: out[0] is the window's first row.
 int vb_host::resolve_destination(vb_renderer *r, Dest *d) {
-    auto bad = [&](const char *why) {
+    auto bad = [&](const std::string &why) {
         r->err = std::string("registered destination: ") + why;
         return VB_E_INVALID;
     };
@@ -420,10 +427,12 @@ int vb_host::resolve_destination(vb_renderer *r, Dest *d) {
     const Destination &D = it->second;
     VbFineOut o{};
     o.swz = D.format == VB_DEST_BGRA8 ? 0x3012u : 0x3210u;
-    o.dst = D.format == VB_DEST_BGRA8 || D.kind == VB_DEST_ARRAY;
+    o.texel = D.texel();
+    o.premul = D.premul;
+    o.dst = D.format != VB_DEST_RGBA8 || D.premul || D.kind == VB_DEST_ARRAY;
     if (D.kind == VB_DEST_LINEAR) {
-        if (D.pitch < (size_t)c.target_width * 4u) return bad("the row pitch is below 4 * width");
-        c.out_pitch_px = (uint32_t)(D.pitch / 4u);
+        if (D.pitch < (size_t)c.target_width * o.texel) return bad("the row pitch is below " + std::to_string(o.texel) + " * width");
+        c.out_pitch_px = (uint32_t)(D.pitch / o.texel);
         o.out = (uint32_t *)(D.ptr + (size_t)c.out_row0 * D.pitch);
     } else {
         if ((uint64_t)D.x0 + c.target_width > D.w || (uint64_t)D.y0 + fine_rows(c, *d).y1 > D.h)

@@ -197,19 +197,24 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination"]
 
 
-def _device_image(t):
-    """(pointer, height, width, row pitch in bytes) of an (H, W, 4) uint8 array in device memory, from its
-    `__cuda_array_interface__` (a torch CUDA tensor, or a slice of one): texels 4 bytes apart, rows any multiple of 4 apart.
-    Device images and linear destinations (`Renderer.register_destination`) are read this way."""
+def _device_image(t, typestr="|u1"):
+    """(pointer, height, width, row pitch in bytes) of an (H, W, 4) device array of element type `typestr` ("|u1" uint8,
+    "<f2" float16 or "<f4" float32), from its `__cuda_array_interface__` (a torch CUDA tensor, or a slice of one): elements
+    e bytes apart, texels 4e bytes apart, rows any multiple of 4e apart. Device images (uint8) and linear destinations
+    (`Renderer.register_destination`) are read this way."""
     cai = getattr(t, "__cuda_array_interface__", None)
     if cai is None:
         raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: a device image is needed")
     shape = tuple(int(v) for v in cai["shape"])
-    if len(shape) != 3 or shape[2] != 4 or cai["typestr"] not in ("|u1", "<u1", ">u1"):
-        raise ValueError(f"a device image is (H, W, 4) uint8, not shape {shape} of type {cai['typestr']}")
-    strides = cai.get("strides") or (shape[1] * 4, 4, 1)
-    if tuple(strides[1:]) != (4, 1) or strides[0] % 4:
-        raise ValueError(f"a device image has texel strides (4, 1) and a row stride that is a multiple of 4, not {tuple(strides)}")
+    same = ("|u1", "<u1", ">u1") if typestr == "|u1" else (typestr,)
+    if len(shape) != 3 or shape[2] != 4 or cai["typestr"] not in same:
+        name = {"|u1": "uint8", "<f2": "float16", "<f4": "float32"}[typestr]
+        raise ValueError(f"a device image is (H, W, 4) {name}, not shape {shape} of type {cai['typestr']}")
+    e = int(typestr[2:])
+    strides = cai.get("strides") or (shape[1] * 4 * e, 4 * e, e)
+    if tuple(strides[1:]) != (4 * e, e) or strides[0] % (4 * e):
+        raise ValueError(f"a device image has texel strides ({4 * e}, {e}) and a row stride that is a multiple of {4 * e}, "
+                         f"not {tuple(strides)}")
     return int(cai["data"][0]), shape[0], shape[1], int(strides[0])
 
 
@@ -587,26 +592,36 @@ class Renderer:
             return min(bin_rows[0] * 256, params.height), min(bin_rows[1] * 256, params.height)
         return 0, params.height
 
-    DEST_FORMATS = {"rgba8": 0, "bgra8": 1}
+    # format: (vb_destination.format, element type of a linear target)
+    DEST_FORMATS = {"rgba8": (0, "|u1"), "bgra8": (1, "|u1"), "rgba16f": (2, "<f2"), "rgba32f": (3, "<f4")}
+    DEST_ALPHA = {"straight": 0, "premultiplied": 0x100}
 
-    def register_destination(self, target=None, *, array=None, format: str = "rgba8", origin=(0, 0)) -> int:
+    def register_destination(self, target=None, *, array=None, format: str = "rgba8", alpha: str = "straight",
+                             origin=(0, 0)) -> int:
         """Register where frames can be rendered straight to (`vb_register_destination`) and return its key, which goes
         wherever `out_device_ptr` goes (`render_resident`, `enqueue`, `run_stages`).
 
         `target`: an (H, W, 4) uint8 device array (`__cuda_array_interface__`: a torch CUDA tensor, or a slice of a larger
-        one) with strides (pitch, 4, 1); pixel (x, y) of a frame lands at element [y, x]. It must hold the frames rendered
-        into it: the row pitch is checked at each frame, the rows are the caller's to provide. `array`: an integer
-        `cudaArray_t` handle of a 2-D array of four 8-bit unsigned channels created with `cudaArraySurfaceLoadStore` (such as
-        level 0 of an imported Vulkan image); pixel (x, y) lands at texel (origin[0] + x, origin[1] + y), and a frame that
-        does not fit is refused. `format`: "rgba8" (vello's byte order) or "bgra8". A bin_row / tile_row window writes its
-        rows at their own rows. Damage-tracked frames into the same key are incremental."""
-        fmt = self.DEST_FORMATS.get(format)
-        if fmt is None:
+        one) with strides (pitch, 4, 1), or float16 / float32 for the float formats, with strides (pitch, 8, 2) /
+        (pitch, 16, 4); pixel (x, y) of a frame lands at element [y, x]. It must hold the frames rendered into it: the row
+        pitch is checked at each frame, the rows are the caller's to provide. `array`: an integer `cudaArray_t` handle of a
+        2-D array created with `cudaArraySurfaceLoadStore` (such as level 0 of an imported Vulkan image), of four channels
+        that match the format (8-bit unsigned, 16-bit float or 32-bit float); pixel (x, y) lands at texel
+        (origin[0] + x, origin[1] + y), and a frame that does not fit is refused. `format`: "rgba8" (vello's byte order),
+        "bgra8", "rgba16f" or "rgba32f". `alpha`: "straight" (vello's) or "premultiplied". The values are fine's f32 pixels
+        clamped to [0, 1], rounded to 8 bits or to halves for the narrower formats (see `vb_register_destination`). A
+        bin_row / tile_row window writes its rows at their own rows. Damage-tracked frames into the same key are
+        incremental."""
+        if format not in self.DEST_FORMATS:
             raise ValueError(f"register_destination: format is one of {sorted(self.DEST_FORMATS)}, not {format!r}")
+        if alpha not in self.DEST_ALPHA:
+            raise ValueError(f"register_destination: alpha is one of {sorted(self.DEST_ALPHA)}, not {alpha!r}")
+        fmt, typestr = self.DEST_FORMATS[format]
+        fmt |= self.DEST_ALPHA[alpha]
         if (target is None) == (array is None):
             raise ValueError("register_destination: give either a target or an array")
         if target is not None:
-            ptr, _, _, pitch = _device_image(target)
+            ptr, _, _, pitch = _device_image(target, typestr)
             d = _Destination(0, fmt, ptr, pitch, None, 0, 0)
         else:
             d = _Destination(1, fmt, None, 0, int(array), int(origin[0]), int(origin[1]))
