@@ -165,7 +165,8 @@ int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: wh
  *    and flatten's tolerance are those on screen; strokes are their outlines) at the point is nonzero, or odd under the
  *    even-odd rule, and the point lies inside the clip path of every enclosing BEGIN_CLIP (each with its own fill rule).
  *    Brush alpha, layer alpha and blend modes do not matter: a transparent fill is hit, an image or a blurred rectangle
- *    anywhere in the rectangle it is drawn in. A point exactly on a line is decided by the half-open rules of the tile walk
+ *    anywhere in the rectangle it is drawn in. Colour never matters, so bound draw colours (vb_bind_draw_colors) do not change
+ *    the answers. A point exactly on a line is decided by the half-open rules of the tile walk
  *    (tests/tile_walk_ref.py): deterministic, with no promise of the side.
  *  - BEGIN_CLIP / END_CLIP objects are never returned. Points outside the frame and NaN points give -1. Indices are the
  *    scene's draw-object indices (vb_scene_n_draw_objects / Scene.n_draw_objects; global in a batch: cell c's draws are
@@ -187,7 +188,8 @@ int vb_hit_test(vb_renderer *, const float *xy, uint32_t n, int32_t *draw_ix, ui
  * (char *)draw_ix + j * pitch_bytes + 4 * i, is the answer for the point (x0 + i + 0.5f, y0 + j + 0.5f), equal int for int;
  * only those h rows of w values are written. Everything above carries over: the frame, its state rules and error codes, the
  * tall frame of a batch, on_device (draw_ix alone is the pointer checked), and a map leaves the frame alone as a hit test
- * does. One CTA per 16 x 16 tile reads the tile's draw list and segments once for its 256 pixels (DESIGN.md §1, "Hit maps").
+ * does. Like hit tests, maps do not depend on colour, bound draw colours included. One CTA per 16 x 16 tile reads the tile's draw
+ * list and segments once for its 256 pixels (DESIGN.md §1, "Hit maps").
  * w = 0 or h = 0: nothing happens, VB_OK. VB_E_INVALID also for NULL draw_ix; a rectangle not inside the last frame
  * (x0 + w > width or y0 + h > n_cells * height); pitch_bytes not a multiple of 4 or below 4 * w. */
 int vb_hit_map(vb_renderer *, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, int32_t *draw_ix, size_t pitch_bytes,
@@ -268,8 +270,9 @@ void *vb_stream(vb_renderer *);
 int vb_run_stages(vb_renderer *, const vb_params *, int first, int last, void *out_device);
 /* Copy an intermediate buffer to the host: "tag_monoids","path_bboxes","lines","draw_monoids",
  * "info_bin_data","clip_inp","clip_bboxes","draw_bboxes","bin_headers","paths","tiles","seg_counts",
- * "segments","ptcl","blend_spill","bump","config", and the guard regions of vb_debug_limit_arena ("<arena>.guard", empty
- * while the arena has no limit). Test-only, flatten's own state after the last attempt: "flatten_counters" (3 x u32:
+ * "segments","ptcl","blend_spill","bump","config"; "transforms" and "draw_data", the transform and draw-data words the last
+ * frame read (its bound or viewed region, else the scene's own stream); and the guard regions of vb_debug_limit_arena
+ * ("<arena>.guard", empty while the arena has no limit). Test-only, flatten's own state after the last attempt: "flatten_counters" (3 x u32:
  * literal line records, deferred jobs, partitions on the general tag kernel's work list), "line_scratch" (32 B literal
  * records) and "flatten_jobs" (96 B job records), each up to its counter and at most its capacity.
  * Returns bytes available in *bytes; copies min(cap, bytes). */
@@ -439,9 +442,9 @@ int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout
  * every edit: a hover colour is a new fragment in the same slot, a popup an inserted instance, a closed dialog a removed one,
  * a raised window a move in z-order. With damage tracking (below) the next frame is then incremental, with the damage between
  * the composition the base frame rendered and the new one, when all of these hold:
- *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, unbound, with no scene
- *    installation, binding, view, cell split or tracking switch since, and hit tests answering from it (no failed frame,
- *    vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
+ *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, with neither instance
+ *    transforms nor draw colours bound, with no scene installation, binding, view, cell split or tracking switch since, and
+ *    hit tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - no other vb_recompose / vb_compose since that frame, and no vb_run_stages before the next one;
  *  - the next frame meets every condition of an incremental frame (size, AA, base colour, destination, one cell, no window).
  * Otherwise it is vb_compose: the next frame is full, and still correct. vb_compose itself always makes the next frame full.
@@ -489,6 +492,38 @@ uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t n_old, cons
  * that compose freed before the call; a renderer of a vb_group or with the exchange enabled; a call between vb_render_enqueue
  * and vb_frame_finish; a scene whose bound transforms plus a view's would pass 32-bit word offsets. */
 int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, uint32_t n, size_t row_pitch_bytes);
+/* Bind the colours of the installed scene's draw objects to device memory (an addition; no vello counterpart). A hover or
+ * selection highlight, a choropleth coloured by a model's output, a particle view coloured by simulation state or a fade changes
+ * colours without re-encoding or re-uploading the scene, and without a host call per frame:
+ *  - Rows. Row k is at device_rgba + k * row_pitch_bytes. It holds four f32 values r, g, b, a: straight-alpha, sRGB-encoded
+ *    components, exactly a vello / peniko Color. Row k belongs to draw object k of the installed scene: the indices vb_hit_test
+ *    returns and vb_scene_n_draw_objects / Scene.n_draw_objects counts. In a composed scene they are global (instance i's draws
+ *    are draw_offsets[i] ..), and in a batch too (cell c's draws are draw_offsets[c] ..).
+ *  - What a frame renders. While rows are bound, every frame renders the scene it would render if draw object k, for every
+ *    k < n, had been encoded with Color(row k). This applies to draw objects whose paint is one colour: DRAWTAG_COLOR (solid
+ *    fills and strokes) and BLUR_RECT (the colour of draw_blurred_rounded_rect[_in]). Rows of every other draw object
+ *    (gradients, images, BEGIN_CLIP, END_CLIP) are ignored. Draw objects from n on keep the colour they were encoded with.
+ *  - Conversion. The colour word is exactly the encoder's premultiply().to_rgba8().to_u32(): p = (r*a, g*a, b*a, a) in f32, and
+ *    each channel is clamp(floor(p*255 + 0.5), 0, 255), where p*255 and + 0.5 are rounded separately in f32; r is the low byte.
+ *    So a bound frame is byte-identical to uploading the scene re-encoded with those colours.
+ *  - Non-finite rows. If any of a row's four values is NaN or +-inf, that draw object keeps its encoded colour for that frame.
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, in the frame's first stage, like bound transforms.
+ *    The caller orders its writes before the frame, on vb_stream or with a synchronisation, and does not write the rows while a
+ *    frame that reads them is running. A blocking frame that is re-run after an arena overflow reads the same rows again; an
+ *    enqueued frame is never re-run. The caller keeps the memory alive while it is bound. Changing only the contents replays the
+ *    captured frame graph, with no host call and no PCIe traffic. Binding, unbinding, or binding another pointer, n or pitch
+ *    changes the frame's key, so the next frame captures its graph anew. With nothing bound a frame launches, configures and
+ *    captures exactly what it would without this call.
+ *  - Scope. Every scene installation unbinds: every upload form, vb_render, vb_render_begin, vb_compose and vb_recompose. The
+ *    binding survives vb_set_view, vb_set_cells, vb_bind_instance_transforms and hit tests; transforms and colours can be bound
+ *    together. device_rgba NULL unbinds; frames then render the scene as encoded.
+ *  - Hit tests and hit maps do not change: colour never mattered to them. Damage tracking follows the rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the installed layout's n_draw_objects; a pointer that is not device memory of the renderer's device (or
+ * managed memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 16, or 4 GiB or more; a renderer of a
+ * vb_group or with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose draw data and
+ * transform regions past its streams would pass 32-bit word offsets. */
+int vb_bind_draw_colors(vb_renderer *, const float *device_rgba, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -497,7 +532,7 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  * changes nothing: not the pixels, the launches or the captured graphs.
  *  - Incremental frames. A frame is incremental when tracking is on; the scene installation is the same (no upload form,
  *    vb_compose, vb_render or vb_render_begin since; vb_recompose, and uploads with vb_set_upload_diff on, see there, can keep the frame after them incremental); width, height, AA, base colour and the device destination pointer are
- *    those of the last successful frame (NULL counts as the renderer's own target); the view, the binding and vb_set_cells are
+ *    those of the last successful frame (NULL counts as the renderer's own target); the view, the bindings and vb_set_cells are
  *    unchanged; it has one cell and no bin_row / tile_row window; and the renderer is not in a vb_group and has no exchange.
  *    Every other frame is full: it reports every tile as damaged and becomes the base of the next one (a batch or a windowed
  *    frame becomes no base). Host destinations (vb_render_uploaded with a host pointer, vb_render) are always full; use
@@ -508,6 +543,11 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  *    the tiles of the clipped boxes of its draw objects (draw_offsets[k] .. draw_offsets[k + 1] of vb_compose) in the last
  *    frame and in this one. A moved open clip or blend layer is covered by its own box. The comparison and the snapshot it
  *    needs are kernels of the frame: moving rows replays the captured graph.
+ *  - Automatic damage, for bound draw colours (vb_bind_draw_colors). Draw object d changed if the colour word the frame reads
+ *    for it differs bit for bit from the last successful frame's: a row that converts to the same word, or a non-finite row
+ *    that falls back to an unchanged encoded word, is no change. The damage is the tiles of its clipped box in the last frame
+ *    and in this one, and nothing else; the two boxes are equal unless bound transforms also moved it. A change of opacity can
+ *    move fine's occlusion start only inside the draw's own box, so the box covers it. Changing rows replays the captured graph.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
@@ -533,9 +573,9 @@ int vb_set_damage_tracking(vb_renderer *, int on);
  * vb_scene_upload, vb_scene_upload_streams, vb_scene_upload_device, or the upload inside vb_render / vb_render_scene is compared
  * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
  * all of these hold:
- *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound, one cell, no
- *    scene installation, binding, view, cell split or tracking switch since, and hit tests answering from it (no failed frame,
- *    vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
+ *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound (no draw
+ *    colours bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
+ *    tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
  *    frame full), and no vb_run_stages before the next one;
  *  - the next frame meets every condition of an incremental frame (size, AA, base colour, device destination, one cell, no

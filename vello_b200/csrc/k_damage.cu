@@ -5,7 +5,9 @@
 // no changed draw object touches gets the same pixels again. The damage of a frame is
 //   the caller's rectangles (vb_add_damage, staged into `pending` in stream order)
 //   + for every bound instance whose transform words (the ones flatten reads: the bound region, or the viewed one) differ bit
-//     for bit from the last successful frame's, the tile boxes of its draw objects in that frame and in this one.
+//     for bit from the last successful frame's, the tile boxes of its draw objects in that frame and in this one
+//   + for every draw object with a bound colour (vb_bind_draw_colors) whose colour word (the one coarse reads from the frame's
+//     draw data) differs bit for bit from the last successful frame's, its tile box in that frame and in this one.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -25,8 +27,9 @@
 #define DM_HEADER_WORDS 4u // [generation, pad x3]
 #define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
 
-extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw) {
-    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw);
+// a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects]
+extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col) {
+    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col);
 }
 
 // the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
@@ -63,10 +66,14 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
     if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
 }
 
-// One warp per draw object: its box into the next slot, and, when its instance changed, its old and new boxes into the mask.
+// One warp per draw object: its box and, below n_col, its colour word into the next slot; when its instance (n_inst > 0) or its
+// colour word changed, its old and new boxes into the mask. A draw object whose paint is not one colour has colour word 0:
+// its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
                                                        uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
-                                                       const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht) {
+                                                       const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht,
+                                                       const uint32_t *__restrict__ draw_tags, const uint32_t *__restrict__ dd,
+                                                       const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col) {
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (d >= n_draw) return;
     const uint32_t *old;
@@ -74,11 +81,23 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict
     dm_slots(snap, slot_words, &old, &nxt);
     const VbBbox4 now = draw_bboxes[d];
     const VbBbox4 was = reinterpret_cast<const VbBbox4 *>(old + 6u * (size_t)n_xf)[d];
+    bool hit = false;
+    if (d < n_col) {
+        const uint32_t tag = __ldg(draw_tags + d);
+        const bool one_colour = tag == VB_DRAWTAG_FILL_COLOR || tag == VB_DRAWTAG_BLURRED_ROUNDED_RECT;
+        const uint32_t col = one_colour ? __ldg(dd + draw_monoids[d].scene_offset) : 0u;
+        const size_t at = 6u * (size_t)n_xf + 4u * (size_t)n_draw + d;
+        hit = col != old[at];
+        if (lane == 0u) nxt[at] = col;
+    }
     __syncwarp();
     if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
-    // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
-    if (!compare || d >= __ldg(inst_draw + n_inst)) return;
-    if (changed[cp_find(inst_draw, 0u, n_inst - 1u, d)] == 0u) return;
+    if (!compare) return;
+    if (!hit) {
+        // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
+        if (n_inst == 0u || d >= __ldg(inst_draw + n_inst)) return;
+        if (changed[cp_find(inst_draw, 0u, n_inst - 1u, d)] == 0u) return;
+    }
     dm_or_box(mask, was, wt, ht, lane);
     dm_or_box(mask, now, wt, ht, lane);
 }
@@ -110,8 +129,9 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
     const uint32_t n = std::max(n_tiles, n_inst);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst);
-    if (n_inst == 0u) return 1u; // not bound: the transforms never change without a call that makes the frame full
-    const size_t slot_words = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw;
+    // neither transforms nor colours bound: nothing changes without a call that makes the frame full
+    if (n_inst == 0u && b.col_n == 0u) return 1u;
+    const size_t slot_words = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n;
     uint32_t launches = 1u;
     if (b.dmg_n_xf) {
         k_damage_mark<<<(b.dmg_n_xf + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
@@ -121,7 +141,8 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     if (n_draw) {
         const uint32_t per = DM_THREADS / 32u;
         k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
-                                                                   n_inst, b.dmg_changed, b.dmg_mask, wt, ht);
+                                                                   n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
+                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n);
         launches++;
     }
     return launches;

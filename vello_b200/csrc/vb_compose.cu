@@ -1,5 +1,6 @@
 // vb_compose.cu -- composition of resident fragments: vb_fragment_upload / vb_fragment_free, vb_compose and vb_recompose
-// (k_compose.cu, k_recompose.cu), and bound instance transforms (vb_bind_instance_transforms).
+// (k_compose.cu, k_recompose.cu), bound instance transforms (vb_bind_instance_transforms) and bound draw colours
+// (vb_bind_draw_colors, k_colors.cu).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
@@ -553,9 +554,11 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     std::vector<const Fragment *> fr(n);
     for (uint32_t k = 0; k < n; k++)
         if (!(fr[k] = find_fragment(r, slot.inst_frag[k]))) return bad("fragment " + std::to_string(slot.inst_frag[k]) + " of the composed scene was freed");
-    // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one)
+    // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one), and
+    // bound colours' draw data after them
     const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr > 0xfffffff0ull)
+    const uint64_t n_dd = r->colors.rows ? n_draw_data(slot.layout, slot.scene_words) : 0u;
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd > 0xfffffff0ull)
         return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
 
     // staged through pinned memory: [the copy's tables (cmp_tables), with no transforms] [the binding's tables: transform
@@ -593,6 +596,52 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     r->bound.o_xf = o_xf;
     r->bound.o_src = o_tr;
     r->bound.o_draw = o_draw;
+    r->dmg.epoch++;
+    return VB_OK;
+}
+
+// ---- bound draw colours: vb_bind_draw_colors (k_colors.cu) ----------------------------------------------------------------------
+// The slot table is made once, here, on the renderer's stream: every word VB_COLOR_NONE, then one k_draw_color_slots over the
+// first n draw tags. It stays valid while the rows are bound, because every scene installation unbinds. Every frame after that
+// reads the caller's rows in its k_draw_colors.
+extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_draw_colors: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_rgba) {
+        r->colors = vb_renderer::ColorBinding{};
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene) return bad("no scene installed");
+    const VbLayout &L = slot.layout;
+    if (n == 0u || n > L.n_draw_objects)
+        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(L.n_draw_objects) + " draw objects (1 .. n_draw_objects)");
+    if ((uintptr_t)device_rgba & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 16u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 16 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_rgba)) return bad("the rows must be memory of the renderer's device");
+    // a frame writes the bound draw data past the scene, after the bound and viewed transforms (prepare, vb_frame.cu)
+    const uint32_t n_dd = n_draw_data(L, slot.scene_words);
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_dd > 0xfffffff0ull)
+        return bad("the scene with its bound draw data and its bound and viewed transforms exceeds 32-bit word offsets");
+    if ((uint64_t)L.draw_tag_base + n > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
+    int rc;
+    if ((rc = compose_room(r, r->color_slots, (size_t)n_dd * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    uint32_t *slots = (uint32_t *)r->color_slots.p;
+    if (n_dd) CK(cudaMemsetAsync(slots, 0xff, (size_t)n_dd * 4u, st));
+    vb_launch_draw_color_slots((const uint32_t *)slot.scene.p + L.draw_tag_base, n, slots, n_dd, st);
+    CK(cudaGetLastError());
+    r->colors.rows = (const uint8_t *)device_rgba;
+    r->colors.n = n;
+    r->colors.pitch = (uint32_t)row_pitch_bytes;
     r->dmg.epoch++;
     return VB_OK;
 }

@@ -59,6 +59,9 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
     // the transform words the last frame read from its transform_base: the bound or viewed region, else the scene's stream
     const size_t t_off = (size_t)c.layout.transform_base * 4u, t_cap = r->cur->scene.cap > t_off ? r->cur->scene.cap - t_off : 0u;
     v.push_back({"transforms", &r->cur->scene, std::min<size_t>(24u * (size_t)n_transforms(r->cur->layout, r->cur->scene_words), t_cap), t_off});
+    // the draw-data words the last frame read from its draw_data_base: the bound colours' region, else the scene's stream
+    const size_t d_off = (size_t)c.layout.draw_data_base * 4u, d_cap = r->cur->scene.cap > d_off ? r->cur->scene.cap - d_off : 0u;
+    v.push_back({"draw_data", &r->cur->scene, std::min<size_t>(4u * (size_t)n_draw_data(r->cur->layout, r->cur->scene_words), d_cap), d_off});
     // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
     const uint32_t *size = &c.lines_size;
     for (int a = 0; a < N_ARENAS; a++) {

@@ -304,9 +304,9 @@ extern "C" int vb_copy_to_host(vb_renderer *r, const void *src_device, void *dst
     return VB_OK;
 }
 
-// A view set or transforms bound after the scene's upload: move the current slot's scene into an allocation with room for the
-// transforms frames write. The scene may still be arriving on the upload stream, and frames already enqueued read the old
-// allocation.
+// A view set, or transforms or colours bound, after the scene's upload: move the current slot's scene into an allocation with
+// room for the transforms and draw data frames write. The scene may still be arriving on the upload stream, and frames already
+// enqueued read the old allocation.
 static int reserve_transform_room(vb_renderer *r, size_t bytes) {
     DevBuf &sc = r->cur->scene;
     if (sc.cap >= bytes) return VB_OK;
@@ -414,8 +414,14 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
         c.frame_cull = 1u;
     }
-    if (n_regions) {
-        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions));
+    if (r->colors.rows) {
+        // the frame reads its draw data past the scene's streams and the transform regions: [draw_data_base, scene_words) is
+        // the region k_draw_colors writes from the scene's draw data and the caller's rows
+        c.layout.draw_data_base = c.scene_words;
+        c.scene_words += n_draw_data(r->cur->layout, r->cur->scene_words);
+    }
+    if (n_regions || r->colors.rows) {
+        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, r->colors.rows != nullptr));
         if (rc0) return rc0;
     }
     c.n_cells = n_cells;
@@ -480,6 +486,13 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.inst_src = (const uint32_t *)(t + r->bound.o_src);
         b.inst_n = r->bound.n;
         b.inst_pitch = r->bound.pitch;
+    }
+    if (r->colors.rows) {
+        b.col_rows = r->colors.rows;
+        b.col_slots = (const uint32_t *)r->color_slots.p;
+        b.col_n = r->colors.n;
+        b.col_pitch = r->colors.pitch;
+        b.col_src = b.scene + r->cur->layout.draw_data_base;
     }
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
@@ -571,9 +584,11 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
             // a frame with bound instance transforms or a view first writes its transforms (read by flatten and draw), the
-            // bound ones first (the view's source), inside flatten's stage events
+            // bound ones first (the view's source), and a frame with bound colours its draw data (read by draw, coarse and
+            // fine), inside flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
+            launches += vb_launch_draw_colors(c, b, st);
             if (fork_draw) {
                 CK(cudaEventRecord(r->draw_fork, st));
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->draw_fork, 0));
@@ -599,6 +614,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // words are the same
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_colors(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);
             if (fork_draw) CK(cudaStreamWaitEvent(st, r->draw_join, 0)); // launched beside flatten

@@ -2,9 +2,10 @@
 //
 // The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
 // (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
-// instance transforms), vb_damage.cu (damage tracking), vb_debug.cu (debug downloads and uploads) and vb_group.cu (vb_group,
-// the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in namespace vb_host, hidden
-// from the shared library's symbol table, so that a host program's own functions of the same names cannot interpose on them.
+// instance transforms and draw colours), vb_damage.cu (damage tracking), vb_debug.cu (debug downloads and uploads) and
+// vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
+// namespace vb_host, hidden from the shared library's symbol table, so that a host program's own functions of the same names
+// cannot interpose on them.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -307,6 +308,14 @@ struct vb_renderer {
         size_t o_xf = 0, o_src = 0, o_draw = 0;
     } bound;
     DevBuf inst_tables;
+    // bound draw colours (vb_bind_draw_colors) of the current scene: the caller's rows (nullptr: unbound), and in color_slots
+    // one word per draw-data word of the scene: the row whose converted colour replaces that word, or VB_COLOR_NONE (k_colors.cu).
+    // Every scene installation unbinds (set_scene).
+    struct ColorBinding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+    } colors;
+    DevBuf color_slots;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -362,8 +371,8 @@ struct vb_renderer {
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
-                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->dmg_mask, &r->dmg_pending,
-                           &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->dmg_mask,
+                           &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
 }
@@ -420,10 +429,16 @@ inline uint32_t n_transforms(const VbLayout &L, size_t scene_words) {
     if (L.style_base < L.transform_base || L.style_base > scene_words) return 0u;
     return (L.style_base - L.transform_base) / 6u;
 }
+// Draw-data words of a scene: the stream from layout.draw_data_base to transform_base (0 for a layout that does not fit the scene).
+inline uint32_t n_draw_data(const VbLayout &L, size_t scene_words) {
+    if (L.transform_base < L.draw_data_base || L.transform_base > scene_words) return 0u;
+    return L.transform_base - L.draw_data_base;
+}
 // A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
-// transforms, k_compose.cu; viewed transforms, k_view.cu), then slack.
-inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions) {
-    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words)) * 4u + 64u;
+// transforms, k_compose.cu; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
+// k_colors.cu), then slack.
+inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions, bool colors = false) {
+    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words) + (colors ? n_draw_data(L, scene_words) : 0u)) * 4u + 64u;
 }
 
 // vb_frame.cu

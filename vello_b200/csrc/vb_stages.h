@@ -33,6 +33,11 @@ struct VbFrameBufs {
     const uint32_t *inst_prefix;
     const CmpXform *inst_xf;
     const uint32_t *inst_src;
+    // bound draw colours (vb_bind_draw_colors), read by k_draw_colors: the caller's rows (draw object k's at col_rows + k *
+    // col_pitch bytes), the binding's slot table (per draw-data word of the scene, the row whose colour replaces it, or
+    // VB_COLOR_NONE) and the scene's own draw data, the region's source. Null while unbound.
+    const uint8_t *col_rows;
+    const uint32_t *col_slots, *col_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -58,7 +63,8 @@ struct VbFrameBufs {
     uint32_t *ptcl, *blend_spill;
     // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
     // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
-    // of the frame's transform words and draw boxes), one changed flag per bound instance, and the composed scene's draw prefix
+    // of the frame's transform words, draw boxes and colour words of the col_n bound draw objects), one changed flag per bound
+    // instance, and the composed scene's draw prefix
     // (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k + 1]; null while unbound)
     uint8_t *dmg_mask, *dmg_pending;
     uint32_t *dmg_snap, *dmg_changed;
@@ -78,6 +84,7 @@ struct VbFrameBufs {
     uint32_t *lb_pathtag, *lb_flatten, *lb_draw, *lb_tile, *lb_clip, *lb_backdrop;
     uint32_t parts_pathtag, parts_flatten, parts_draw, parts_tile, parts_backdrop;
     uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
+    uint32_t col_n, col_pitch; // bound colour rows and their pitch in bytes; 0 while unbound
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
@@ -183,6 +190,15 @@ uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
 // vb_frame.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// k_colors.cu: bound draw colours (vb_bind_draw_colors). The binding's slot table, once at bind time: slots[w] = k for the colour
+// word w (relative to the draw data) of each draw object k < n whose paint is one colour (FILL_COLOR, BLURRED_ROUNDED_RECT),
+// from the scene's draw tags at `tags`; the caller sets the n_words words of the table to VB_COLOR_NONE first. Per frame, in
+// flatten's stage after the transforms (prepare reserved the region, vb_frame.cu): the scene's draw data into the frame's
+// region at layout.draw_data_base, each slot's word replaced by its row's premultiplied RGBA8 word; nothing while unbound.
+#define VB_COLOR_NONE 0xffffffffu
+uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n, uint32_t *slots, uint32_t n_words, cudaStream_t st);
+uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
 // the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame
 // succeeded. vb_launch_damage_rects stages caller rectangles (tile ranges x0 y0 x1 y1, clipped) into `pending` in stream order.
@@ -192,7 +208,7 @@ uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b
 uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
-size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw);
+size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col);
 // k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
 // of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
 // are null

@@ -174,6 +174,7 @@ def load_library() -> C.CDLL:
     lib.vb_debug_match_instances.argtypes = [vp, C.c_uint32, vp, C.c_uint32, vp]
     lib.vb_debug_match_instances.restype = C.c_uint32
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_draw_colors.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -194,7 +195,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_override_image", "vb_mark_override_image_dirty", "vb_set_cells", "vb_set_view", "vb_group_set_view",
                     "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
-                    "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination"]
+                    "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
+                    "vb_bind_draw_colors"]
 
 
 def _device_image(t, typestr="|u1"):
@@ -301,6 +303,7 @@ class Renderer:
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
         self._bound = None  # the device array of bind_instance_transforms
+        self._colors = None  # the device array of bind_draw_colors
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
         self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
@@ -316,6 +319,7 @@ class Renderer:
         r._fragment_pixels = {}
         r._destinations = {}
         r._bound = None
+        r._colors = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -478,6 +482,34 @@ class Renderer:
         self._check(self.lib.vb_bind_instance_transforms(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
                     "vb_bind_instance_transforms")
         self._bound = t
+
+    def bind_draw_colors(self, t):
+        """Render draw object k of the installed scene, for every row k of the device array `t`, as if it had been encoded with
+        `Color(row k)`, in every frame from now on, read when the frame runs (`vb_bind_draw_colors`): `t` is float32 (n, 4)
+        straight-alpha r g b a rows, n at most `Scene.n_draw_objects`, with `__cuda_array_interface__` (e.g. a torch CUDA tensor,
+        or columns of a larger one such as `state[:, 3:7]`). Row k belongs to draw object k, the index `hit_test` returns (global
+        in a composed scene or a batch). It applies to solid fills, strokes and blurred rectangles; rows of other draw objects
+        are ignored, and draw objects from n on keep their encoded colour, as does one whose row is not finite. Write it on
+        `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. `t` is held
+        while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_draw_colors(self.handle, None, 0, 0), "vb_bind_draw_colors")
+            self._colors = None
+            return
+        cai = getattr(t, "__cuda_array_interface__", None)
+        if cai is None:
+            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device colours are needed")
+        shape = tuple(int(v) for v in cai["shape"])
+        if len(shape) != 2 or shape[0] == 0 or shape[1] != 4 or cai["typestr"] != "<f4":
+            raise ValueError(f"bind_draw_colors: colours must be (n, 4) float32, not {shape} {cai['typestr']}")
+        strides = cai.get("strides") or (16, 4)
+        pitch = int(strides[0]) if shape[0] > 1 else 16  # the pitch of a single row is never used
+        if int(strides[1]) != 4 or pitch % 4 or pitch < 16:
+            raise ValueError(f"bind_draw_colors: columns 4 bytes apart and rows a multiple of 4 bytes, at least 16, apart; "
+                             f"not strides {tuple(strides)}")
+        self._check(self.lib.vb_bind_draw_colors(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
+                    "vb_bind_draw_colors")
+        self._colors = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
