@@ -166,7 +166,8 @@ int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: wh
  *    even-odd rule, and the point lies inside the clip path of every enclosing BEGIN_CLIP (each with its own fill rule).
  *    Brush alpha, layer alpha and blend modes do not matter: a transparent fill is hit, an image or a blurred rectangle
  *    anywhere in the rectangle it is drawn in. Colour never matters, so bound draw colours (vb_bind_draw_colors) do not change
- *    the answers. A point exactly on a line is decided by the half-open rules of the tile walk
+ *    the answers. Bound path points (vb_bind_path_points) are part of the frame's geometry: the answers follow the points the
+ *    frame read. A point exactly on a line is decided by the half-open rules of the tile walk
  *    (tests/tile_walk_ref.py): deterministic, with no promise of the side.
  *  - BEGIN_CLIP / END_CLIP objects are never returned. Points outside the frame and NaN points give -1. Indices are the
  *    scene's draw-object indices (vb_scene_n_draw_objects / Scene.n_draw_objects; global in a batch: cell c's draws are
@@ -270,8 +271,8 @@ void *vb_stream(vb_renderer *);
 int vb_run_stages(vb_renderer *, const vb_params *, int first, int last, void *out_device);
 /* Copy an intermediate buffer to the host: "tag_monoids","path_bboxes","lines","draw_monoids",
  * "info_bin_data","clip_inp","clip_bboxes","draw_bboxes","bin_headers","paths","tiles","seg_counts",
- * "segments","ptcl","blend_spill","bump","config"; "transforms" and "draw_data", the transform and draw-data words the last
- * frame read (its bound or viewed region, else the scene's own stream); and the guard regions of vb_debug_limit_arena
+ * "segments","ptcl","blend_spill","bump","config"; "transforms", "draw_data" and "path_data", the transform, draw-data and
+ * path-data words the last frame read (its bound or viewed region, else the scene's own stream); and the guard regions of vb_debug_limit_arena
  * ("<arena>.guard", empty while the arena has no limit). Test-only, flatten's own state after the last attempt: "flatten_counters" (3 x u32:
  * literal line records, deferred jobs, partitions on the general tag kernel's work list), "line_scratch" (32 B literal
  * records) and "flatten_jobs" (96 B job records), each up to its counter and at most its capacity.
@@ -442,8 +443,8 @@ int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout
  * every edit: a hover colour is a new fragment in the same slot, a popup an inserted instance, a closed dialog a removed one,
  * a raised window a move in z-order. With damage tracking (below) the next frame is then incremental, with the damage between
  * the composition the base frame rendered and the new one, when all of these hold:
- *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, with neither instance
- *    transforms nor draw colours bound, with no scene installation, binding, view, cell split or tracking switch since, and
+ *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, with no instance
+ *    transforms, draw colours or path points bound, with no scene installation, binding, view, cell split or tracking switch since, and
  *    hit tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - no other vb_recompose / vb_compose since that frame, and no vb_run_stages before the next one;
  *  - the next frame meets every condition of an incremental frame (size, AA, base colour, destination, one cell, no window).
@@ -524,6 +525,49 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  * vb_group or with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose draw data and
  * transform regions past its streams would pass 32-bit word offsets. */
 int vb_bind_draw_colors(vb_renderer *, const float *device_rgba, uint32_t n, size_t row_pitch_bytes);
+/* Bind the points of the installed scene's paths to device memory (an addition; no vello counterpart). A live chart of a GPU
+ * time series, a simulation mesh or cloth outline, polygons a model predicts, a morph between outlines or a graph layout whose
+ * edges follow their nodes moves its geometry every frame without re-encoding or re-uploading the scene, and without a host
+ * call per frame:
+ *  - Rows. Row k is at device_xy + k * row_pitch_bytes and holds two f32 values x, y. Row k is point k of the installed scene's
+ *    path-data stream: path-data words 2k and 2k + 1. Points are global in a composed scene or a batch (fragments and cells in
+ *    stream order), and they are in the coordinates they were encoded in: the path's transform, bound instance transforms and
+ *    a view all still apply on top. vb_scene_n_points / Scene.n_points counts them, read before and after a call to learn the
+ *    rows that call produced. The encoders lay points out so:
+ *     - a move-to writes 1 point, a line-to, quad-to and cubic-to 1, 2 and 3 (the end point last); a repeated move-to replaces
+ *       the one before it, and a segment of zero length writes nothing;
+ *     - a closed fill (every fill subpath closes) repeats its start point, as a line-to, when its last point differs from it;
+ *     - a stroke ends each subpath with a cap marker: a closed one with a line-to (1 point, the end of its start tangent), an
+ *       open one with a quad-to (2 points: its start point, then the end of its start tangent);
+ *     - a dash's pieces are separate subpaths; arcs, circles and ellipses are a move-to and cubics, a rounded rectangle a
+ *       move-to, then per corner a line-to and its cubics;
+ *     - a fill or stroke whose shape encodes nothing writes no point (and no draw object); a push_*_layer whose clip encodes
+ *       nothing writes the empty path in its place, 2 points: a line-to from (0, 0) to (0, 0).
+ *  - What a frame renders. While rows are bound, every frame renders byte for byte what uploading the scene would render after
+ *    overwriting path-data words 2k and 2k + 1, for every k < n, with the f32 bits of row k. The definition is at stream level:
+ *    binding never changes tags, so it is not always re-encoding a moved shape, which may drop a repeated move-to or add a
+ *    closing point the bound scene does not have. Points from n on keep their encoded values.
+ *  - Non-finite rows. If x or y of a row is NaN or +-inf, that point keeps its encoded words for that frame.
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage, and every
+ *    vb_run_stages range that contains flatten reads them again. The caller orders its writes before the frame, on vb_stream
+ *    or with a synchronisation, and does not write the rows while a frame that reads them is running. A blocking frame that is
+ *    re-run after an arena overflow reads the same rows again; an enqueued frame is never re-run. The caller keeps the memory
+ *    alive while it is bound. Changing only the contents replays the captured frame graph, with no host call and no PCIe
+ *    traffic. Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next frame captures
+ *    its graph anew. With nothing bound a frame launches, configures and captures exactly what it would without this call.
+ *  - Scope. Every scene installation unbinds: every upload form, vb_render, vb_render_begin, vb_compose and vb_recompose. The
+ *    binding survives vb_set_view, vb_set_cells, vb_bind_instance_transforms, vb_bind_draw_colors and hit tests; all three
+ *    bindings can be active together. device_xy NULL unbinds; frames then render the scene as encoded.
+ *  - The call finds each path's first point once, with one kernel over the path tags, and synchronises with vb_stream once to
+ *    read back whether the scene has a 16-bit segment. Hit tests and hit maps answer from the bound geometry, and damage
+ *    tracking follows the rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the scene's point count (its path-data words / 2); a pointer that is not device memory of the renderer's
+ * device (or managed memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 8, or 4 GiB or more; a renderer
+ * of a vb_group or with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene with a 16-bit
+ * segment (a segment tag without the F32 bit: its points are not f32 pairs; neither encoder emits one); a scene whose path
+ * data, draw data and transform regions past its streams would pass 32-bit word offsets. */
+int vb_bind_path_points(vb_renderer *, const float *device_xy, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -548,6 +592,11 @@ int vb_bind_draw_colors(vb_renderer *, const float *device_rgba, uint32_t n, siz
  *    that falls back to an unchanged encoded word, is no change. The damage is the tiles of its clipped box in the last frame
  *    and in this one, and nothing else; the two boxes are equal unless bound transforms also moved it. A change of opacity can
  *    move fine's occlusion start only inside the draw's own box, so the box covers it. Changing rows replays the captured graph.
+ *  - Automatic damage, for bound path points (vb_bind_path_points). Path p changed if the words of one of its bound points that
+ *    the frame reads differ bit for bit from the last successful frame's: a non-finite row that falls back to an unchanged
+ *    encoded point is no change. The damage is the tiles of the clipped box of draw object p (path p is draw object p) in the
+ *    last frame and in this one. A changed clip path changes the boxes of the draws inside it only within its BEGIN_CLIP's own
+ *    old and new box, which that draw object contributes.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
@@ -574,7 +623,7 @@ int vb_set_damage_tracking(vb_renderer *, int on);
  * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
  * all of these hold:
  *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound (no draw
- *    colours bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
+ *    colours or path points bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
  *    tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
  *    frame full), and no vb_run_stages before the next one;

@@ -116,6 +116,14 @@ void vb_scene_reset(vb_scene *);     /* Scene::reset, scene.rs:59 */
  * draw_image, blurred rectangle or push_*_layer receives, so a caller can note the index a call gave (read it before and after
  * the call: a shape that encodes nothing adds no draw). These are the indices vb_hit_test returns. 0 for NULL. */
 uint32_t vb_scene_n_draw_objects(const vb_scene *);
+/* The path points encoded so far (an addition): the path-data words / 2, the row vb_bind_path_points reads for the next point
+ * a call encodes. Read it before and after a call to learn the rows that call produced. Every point is an f32 pair: a move-to
+ * writes 1 point, a line-to, quad-to and cubic-to 1, 2 and 3, a closed fill subpath repeats its start point when its last point
+ * differs, a stroke subpath ends with a cap marker (closed: a line-to, 1 point; open: a quad-to, 2 points), a dash's pieces are
+ * separate subpaths, arcs, circles and ellipses are cubics. A fill or stroke whose shape encodes nothing adds no point; a
+ * push_*_layer whose clip encodes nothing adds 2, the empty path (0, 0) -> (0, 0) that stands in for the clip (the full layout
+ * is at vb_bind_path_points in vello_b200.h). 0 for NULL. */
+uint32_t vb_scene_n_points(const vb_scene *);
 
 /* Scene::fill, scene.rs:316-345. brush_transform may be NULL. */
 int vb_scene_fill(vb_scene *, uint32_t fill_rule, const double transform[6], const vb_brush *, const double *brush_transform,

@@ -7,7 +7,10 @@
 //   + for every bound instance whose transform words (the ones flatten reads: the bound region, or the viewed one) differ bit
 //     for bit from the last successful frame's, the tile boxes of its draw objects in that frame and in this one
 //   + for every draw object with a bound colour (vb_bind_draw_colors) whose colour word (the one coarse reads from the frame's
-//     draw data) differs bit for bit from the last successful frame's, its tile box in that frame and in this one.
+//     draw data) differs bit for bit from the last successful frame's, its tile box in that frame and in this one
+//   + for every path with a bound point (vb_bind_path_points) whose two words (the ones flatten reads from the frame's path
+//     data) differ bit for bit from the last successful frame's, the tile box of its draw object (path i is draw object i) in
+//     that frame and in this one. A changed clip path is covered by its BEGIN_CLIP's boxes, as a moved clip is below.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -27,9 +30,10 @@
 #define DM_HEADER_WORDS 4u // [generation, pad x3]
 #define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
 
-// a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects]
-extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col) {
-    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col);
+// a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects] [the
+// words of the first n_pt points (2 n_pt)]
+extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt) {
+    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt);
 }
 
 // the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
@@ -39,41 +43,58 @@ __device__ __forceinline__ void dm_slots(uint32_t *snap, size_t slot_words, cons
     *nxt = snap + DM_HEADER_WORDS + ((gen + 1u) & 1u) * slot_words;
 }
 
-// A full frame damages every tile; otherwise the frame starts from the caller's rectangles. No instance has changed yet.
+// A full frame damages every tile; otherwise the frame starts from the caller's rectangles. No instance or path has changed yet.
 __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, const uint8_t *__restrict__ pending, uint32_t n_tiles, uint32_t full,
-                                                             uint32_t *changed, uint32_t n_inst) {
+                                                             uint32_t *changed, uint32_t n_inst, uint32_t *paths, uint32_t n_paths) {
     const uint32_t i = blockIdx.x * DM_THREADS + threadIdx.x;
     if (i < n_tiles) mask[i] = full ? 1u : pending[i];
     if (i < n_inst) changed[i] = 0u;
+    if (i < n_paths) paths[i] = 0u;
 }
 
 // One thread per transform u of the frame: its six words against the snapshot, and into the next slot. A difference marks
-// the instance holding u (the binding's prefix of the instances' transform counts).
+// the instance holding u (the binding's prefix of the instances' transform counts). The same thread takes bound point u, when
+// there is one: its two words in the frame's path data (`pd`, the bound region), at `at_pt` of the slot (after the colour
+// words). A difference marks the path holding u (`first`, the binding's first point of each path). A non-finite row left the
+// encoded words in the region, so it is a change only if the words are.
 __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__restrict__ xf, uint32_t *snap, size_t slot_words, uint32_t n_xf,
-                                                            uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed) {
+                                                            uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed,
+                                                            const uint32_t *__restrict__ pd, size_t at_pt, uint32_t n_pt,
+                                                            const uint32_t *__restrict__ first, uint32_t n_paths, uint32_t *paths) {
     const uint32_t u = blockIdx.x * DM_THREADS + threadIdx.x;
-    if (u >= n_xf) return;
+    if (u >= n_xf && u >= n_pt) return;
     const uint32_t *old;
     uint32_t *nxt;
     dm_slots(snap, slot_words, &old, &nxt);
-    bool diff = false;
+    if (u < n_xf) {
+        bool diff = false;
 #pragma unroll
-    for (uint32_t i = 0; i < 6u; i++) {
-        const uint32_t w = __ldg(xf + 6u * u + i);
-        diff = diff || w != old[6u * u + i];
-        nxt[6u * u + i] = w;
+        for (uint32_t i = 0; i < 6u; i++) {
+            const uint32_t w = __ldg(xf + 6u * u + i);
+            diff = diff || w != old[6u * u + i];
+            nxt[6u * u + i] = w;
+        }
+        if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
     }
-    if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
+    if (u < n_pt) {
+        const uint32_t x = __ldg(pd + 2u * u), y = __ldg(pd + 2u * u + 1u);
+        const size_t o = at_pt + 2u * (size_t)u;
+        const bool diff = x != old[o] || y != old[o + 1u];
+        nxt[o] = x;
+        nxt[o + 1u] = y;
+        if (compare && diff) paths[cp_find(first, 0u, n_paths - 1u, u)] = 1u;
+    }
 }
 
-// One warp per draw object: its box and, below n_col, its colour word into the next slot; when its instance (n_inst > 0) or its
-// colour word changed, its old and new boxes into the mask. A draw object whose paint is not one colour has colour word 0:
-// its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
+// One warp per draw object: its box and, below n_col, its colour word into the next slot; when its instance (n_inst > 0), its
+// colour word or its path's points (`paths`, non-null with points bound) changed, its old and new boxes into the mask. A draw
+// object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
                                                        uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
                                                        const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht,
                                                        const uint32_t *__restrict__ draw_tags, const uint32_t *__restrict__ dd,
-                                                       const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col) {
+                                                       const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col,
+                                                       const uint32_t *__restrict__ paths, uint32_t n_paths) {
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (d >= n_draw) return;
     const uint32_t *old;
@@ -93,6 +114,7 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict
     __syncwarp();
     if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
     if (!compare) return;
+    if (!hit && paths && d < n_paths) hit = paths[d] != 0u; // path d is draw object d
     if (!hit) {
         // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
         if (n_inst == 0u || d >= __ldg(inst_draw + n_inst)) return;
@@ -127,22 +149,29 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     if (b.dmg_mode == VB_DMG_OFF) return 0u;
     const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = b.inst_n;
     const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
-    const uint32_t n = std::max(n_tiles, n_inst);
-    k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst);
-    // neither transforms nor colours bound: nothing changes without a call that makes the frame full
-    if (n_inst == 0u && b.col_n == 0u) return 1u;
-    const size_t slot_words = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n;
+    const uint32_t n_paths = b.dmg_paths ? cfg.layout.n_paths : 0u;
+    const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
+    k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst,
+                                                                              b.dmg_paths, n_paths);
+    // neither transforms, colours nor points bound: nothing changes without a call that makes the frame full
+    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u) return 1u;
+    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n;
+    const size_t slot_words = at_pt + 2u * (size_t)b.pt_n;
     uint32_t launches = 1u;
-    if (b.dmg_n_xf) {
-        k_damage_mark<<<(b.dmg_n_xf + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
-                                                                                            b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed);
+    const uint32_t n_pt = n_paths ? b.pt_n : 0u, n_mark = std::max(b.dmg_n_xf, n_pt);
+    if (n_mark) {
+        k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
+                                                                                      b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed,
+                                                                                      b.scene + cfg.layout.path_data_base, at_pt, n_pt, b.pt_first,
+                                                                                      n_paths, b.dmg_paths);
         launches++;
     }
     if (n_draw) {
         const uint32_t per = DM_THREADS / 32u;
         k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
                                                                    n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
-                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n);
+                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n, b.dmg_paths,
+                                                                   n_paths);
         launches++;
     }
     return launches;

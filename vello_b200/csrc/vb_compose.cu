@@ -1,6 +1,6 @@
 // vb_compose.cu -- composition of resident fragments: vb_fragment_upload / vb_fragment_free, vb_compose and vb_recompose
-// (k_compose.cu, k_recompose.cu), bound instance transforms (vb_bind_instance_transforms) and bound draw colours
-// (vb_bind_draw_colors, k_colors.cu).
+// (k_compose.cu, k_recompose.cu), bound instance transforms (vb_bind_instance_transforms), bound draw colours
+// (vb_bind_draw_colors, k_colors.cu) and bound path points (vb_bind_path_points, k_points.cu).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
@@ -555,10 +555,11 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     for (uint32_t k = 0; k < n; k++)
         if (!(fr[k] = find_fragment(r, slot.inst_frag[k]))) return bad("fragment " + std::to_string(slot.inst_frag[k]) + " of the composed scene was freed");
     // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one), and
-    // bound colours' draw data after them
+    // bound colours' draw data and bound points' path data after them
     const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
     const uint64_t n_dd = r->colors.rows ? n_draw_data(slot.layout, slot.scene_words) : 0u;
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd > 0xfffffff0ull)
+    const uint64_t n_pd = r->points.rows ? n_path_data(slot.layout, slot.scene_words) : 0u;
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd + n_pd > 0xfffffff0ull)
         return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
 
     // staged through pinned memory: [the copy's tables (cmp_tables), with no transforms] [the binding's tables: transform
@@ -627,9 +628,11 @@ extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uin
         return bad("the row pitch must be a multiple of 4 bytes, at least 16 and below 4 GiB");
     CK(cudaSetDevice(r->device));
     if (!device_memory_of(r, device_rgba)) return bad("the rows must be memory of the renderer's device");
-    // a frame writes the bound draw data past the scene, after the bound and viewed transforms (prepare, vb_frame.cu)
+    // a frame writes the bound draw data past the scene, after the bound and viewed transforms, and bound points' path data
+    // after it (prepare, vb_frame.cu)
     const uint32_t n_dd = n_draw_data(L, slot.scene_words);
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_dd > 0xfffffff0ull)
+    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_dd + n_pd > 0xfffffff0ull)
         return bad("the scene with its bound draw data and its bound and viewed transforms exceeds 32-bit word offsets");
     if ((uint64_t)L.draw_tag_base + n > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
     int rc;
@@ -642,6 +645,58 @@ extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uin
     r->colors.rows = (const uint8_t *)device_rgba;
     r->colors.n = n;
     r->colors.pitch = (uint32_t)row_pitch_bytes;
+    r->dmg.epoch++;
+    return VB_OK;
+}
+
+// ---- bound path points: vb_bind_path_points (k_points.cu) -----------------------------------------------------------------------
+// The table of each path's first point is made once, here, on the renderer's stream by one k_path_point_slots over the scene's
+// path tags, and its 16-bit flag is read back (the call's one synchronisation). It stays valid while the rows are bound,
+// because every scene installation unbinds. Every frame after that reads the caller's rows in its k_path_points.
+extern "C" int vb_bind_path_points(vb_renderer *r, const float *device_xy, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_path_points: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_xy) {
+        r->points = vb_renderer::PointBinding{};
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene) return bad("no scene installed");
+    const VbLayout &L = slot.layout;
+    const uint32_t n_pd = n_path_data(L, slot.scene_words), n_points = n_pd / 2u;
+    if (n == 0u || n > n_points)
+        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_points) + " points (1 .. n_points)");
+    if ((uintptr_t)device_xy & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 8u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 8 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_xy)) return bad("the rows must be memory of the renderer's device");
+    // a frame writes the bound path data past the scene, after the bound and viewed transforms and the bound draw data (prepare,
+    // vb_frame.cu)
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_draw_data(L, slot.scene_words) + n_pd > 0xfffffff0ull)
+        return bad("the scene with its bound path data, draw data and bound and viewed transforms exceeds 32-bit word offsets");
+    if (L.path_data_base < L.path_tag_base || L.path_data_base > slot.scene_words) return bad("the scene's path tags do not lie inside its words");
+    const uint32_t n_tag_words = L.path_data_base - L.path_tag_base;
+    int rc;
+    if ((rc = compose_room(r, r->point_slots, ((size_t)L.n_paths + 2u) * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    uint32_t *first = (uint32_t *)r->point_slots.p, *flag = first + L.n_paths + 1u;
+    CK(cudaMemsetAsync(first, 0, ((size_t)L.n_paths + 2u) * 4u, st));
+    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, n_tag_words, L.n_paths, first, flag, st);
+    CK(cudaGetLastError());
+    uint32_t i16 = 0u;
+    CK(cudaMemcpyAsync(&i16, flag, 4u, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (i16) return bad("the scene has 16-bit path segments, whose points are not f32 pairs");
+    r->points.rows = (const uint8_t *)device_xy;
+    r->points.n = n;
+    r->points.pitch = (uint32_t)row_pitch_bytes;
     r->dmg.epoch++;
     return VB_OK;
 }

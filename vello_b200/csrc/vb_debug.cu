@@ -62,6 +62,9 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
     // the draw-data words the last frame read from its draw_data_base: the bound colours' region, else the scene's stream
     const size_t d_off = (size_t)c.layout.draw_data_base * 4u, d_cap = r->cur->scene.cap > d_off ? r->cur->scene.cap - d_off : 0u;
     v.push_back({"draw_data", &r->cur->scene, std::min<size_t>(4u * (size_t)n_draw_data(r->cur->layout, r->cur->scene_words), d_cap), d_off});
+    // the path-data words the last frame read from its path_data_base: the bound points' region, else the scene's stream
+    const size_t p_off = (size_t)c.layout.path_data_base * 4u, p_cap = r->cur->scene.cap > p_off ? r->cur->scene.cap - p_off : 0u;
+    v.push_back({"path_data", &r->cur->scene, std::min<size_t>(4u * (size_t)n_path_data(r->cur->layout, r->cur->scene_words), p_cap), p_off});
     // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
     const uint32_t *size = &c.lines_size;
     for (int a = 0; a < N_ARENAS; a++) {

@@ -304,9 +304,9 @@ extern "C" int vb_copy_to_host(vb_renderer *r, const void *src_device, void *dst
     return VB_OK;
 }
 
-// A view set, or transforms or colours bound, after the scene's upload: move the current slot's scene into an allocation with
-// room for the transforms and draw data frames write. The scene may still be arriving on the upload stream, and frames already
-// enqueued read the old allocation.
+// A view set, or transforms, colours or points bound, after the scene's upload: move the current slot's scene into an
+// allocation with room for the transforms, draw data and path data frames write. The scene may still be arriving on the
+// upload stream, and frames already enqueued read the old allocation.
 static int reserve_transform_room(vb_renderer *r, size_t bytes) {
     DevBuf &sc = r->cur->scene;
     if (sc.cap >= bytes) return VB_OK;
@@ -416,12 +416,19 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     }
     if (r->colors.rows) {
         // the frame reads its draw data past the scene's streams and the transform regions: [draw_data_base, scene_words) is
-        // the region k_draw_colors writes from the scene's draw data and the caller's rows
+        // the region k_draw_colors writes from the scene's draw data and the caller's rows (bound path data follows it)
         c.layout.draw_data_base = c.scene_words;
         c.scene_words += n_draw_data(r->cur->layout, r->cur->scene_words);
     }
-    if (n_regions || r->colors.rows) {
-        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, r->colors.rows != nullptr));
+    if (r->points.rows) {
+        // the frame reads its path data past the scene's streams and the regions before: [path_data_base, scene_words) is the
+        // region k_path_points writes from the scene's path data and the caller's rows
+        c.layout.path_data_base = c.scene_words;
+        c.scene_words += n_path_data(r->cur->layout, r->cur->scene_words);
+    }
+    if (n_regions || r->colors.rows || r->points.rows) {
+        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, r->colors.rows != nullptr,
+                                                        r->points.rows != nullptr));
         if (rc0) return rc0;
     }
     c.n_cells = n_cells;
@@ -493,6 +500,13 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.col_n = r->colors.n;
         b.col_pitch = r->colors.pitch;
         b.col_src = b.scene + r->cur->layout.draw_data_base;
+    }
+    if (r->points.rows) {
+        b.pt_rows = r->points.rows;
+        b.pt_first = (const uint32_t *)r->point_slots.p;
+        b.pt_n = r->points.n;
+        b.pt_pitch = r->points.pitch;
+        b.pt_src = b.scene + r->cur->layout.path_data_base;
     }
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
@@ -584,11 +598,12 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
             // a frame with bound instance transforms or a view first writes its transforms (read by flatten and draw), the
-            // bound ones first (the view's source), and a frame with bound colours its draw data (read by draw, coarse and
-            // fine), inside flatten's stage events
+            // bound ones first (the view's source), a frame with bound colours its draw data (read by draw, coarse and
+            // fine), and a frame with bound points its path data (read by flatten alone), inside flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             launches += vb_launch_draw_colors(c, b, st);
+            launches += vb_launch_path_points(c, b, st);
             if (fork_draw) {
                 CK(cudaEventRecord(r->draw_fork, st));
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->draw_fork, 0));

@@ -316,6 +316,14 @@ struct vb_renderer {
         uint32_t n = 0, pitch = 0;
     } colors;
     DevBuf color_slots;
+    // bound path points (vb_bind_path_points) of the current scene: the caller's rows (nullptr: unbound), and in point_slots the
+    // first point of each path (layout.n_paths + 1 words) and then the bind-time flag of a 16-bit segment (k_points.cu). Every
+    // scene installation unbinds (set_scene).
+    struct PointBinding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+    } points;
+    DevBuf point_slots;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -347,7 +355,7 @@ struct vb_renderer {
             size_t o_boxes = 0, o_tables = 0;
         } diff;
     } dmg;
-    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed;
+    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed, dmg_paths;
     DevBuf dmg_diff; // the diff's buffer: [the base frame's draw boxes, at o_boxes] [the tables, at o_tables] (VbFrameBufs::rcmp_*)
     // upload diff (vb_set_upload_diff): the switch; and the spare scene, ramps and atlas buffers an upload that tracking follows
     // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set. The diff's buffer is laid
@@ -371,8 +379,8 @@ struct vb_renderer {
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
-                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->dmg_mask,
-                           &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
 }
@@ -434,11 +442,17 @@ inline uint32_t n_draw_data(const VbLayout &L, size_t scene_words) {
     if (L.transform_base < L.draw_data_base || L.transform_base > scene_words) return 0u;
     return L.transform_base - L.draw_data_base;
 }
+// Path-data words of a scene: the stream from layout.path_data_base to draw_tag_base (0 for a layout that does not fit the scene).
+inline uint32_t n_path_data(const VbLayout &L, size_t scene_words) {
+    if (L.draw_tag_base < L.path_data_base || L.draw_tag_base > scene_words) return 0u;
+    return L.draw_tag_base - L.path_data_base;
+}
 // A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
 // transforms, k_compose.cu; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
-// k_colors.cu), then slack.
-inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions, bool colors = false) {
-    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words) + (colors ? n_draw_data(L, scene_words) : 0u)) * 4u + 64u;
+// k_colors.cu) and with `points` a region of path data after those (bound path points, k_points.cu), then slack.
+inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions, bool colors = false, bool points = false) {
+    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words) + (colors ? n_draw_data(L, scene_words) : 0u) +
+            (points ? n_path_data(L, scene_words) : 0u)) * 4u + 64u;
 }
 
 // vb_frame.cu

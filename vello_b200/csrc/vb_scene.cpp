@@ -1170,6 +1170,7 @@ void vb_scene_reset(vb_scene *s) {
     if (s) *s = vb_scene();
 }
 uint32_t vb_scene_n_draw_objects(const vb_scene *s) { return s ? (uint32_t)s->e.draw_tags.size() : 0u; }
+uint32_t vb_scene_n_points(const vb_scene *s) { return s ? (uint32_t)(s->e.path_data.size() / 2u) : 0u; }
 
 int vb_scene_fill(vb_scene *s, uint32_t fill_rule, const double transform[6], const vb_brush *brush, const double *brush_transform,
                   const vb_path *path) {

@@ -38,6 +38,11 @@ struct VbFrameBufs {
     // VB_COLOR_NONE) and the scene's own draw data, the region's source. Null while unbound.
     const uint8_t *col_rows;
     const uint32_t *col_slots, *col_src;
+    // bound path points (vb_bind_path_points), read by k_path_points: the caller's rows (point k's at pt_rows + k * pt_pitch
+    // bytes), the binding's table of each path's first point (layout.n_paths + 1; k_damage maps changed points to paths with
+    // it) and the scene's own path data, the region's source. Null while unbound.
+    const uint8_t *pt_rows;
+    const uint32_t *pt_first, *pt_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -63,11 +68,11 @@ struct VbFrameBufs {
     uint32_t *ptcl, *blend_spill;
     // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
     // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
-    // of the frame's transform words, draw boxes and colour words of the col_n bound draw objects), one changed flag per bound
-    // instance, and the composed scene's draw prefix
+    // of the frame's transform words, draw boxes, colour words of the col_n bound draw objects and words of the pt_n bound
+    // points), one changed flag per bound instance and, with points bound, one per path, and the composed scene's draw prefix
     // (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k + 1]; null while unbound)
     uint8_t *dmg_mask, *dmg_pending;
-    uint32_t *dmg_snap, *dmg_changed;
+    uint32_t *dmg_snap, *dmg_changed, *dmg_paths;
     const uint32_t *inst_draw;
     // recompose damage (vb_recompose; k_recompose.cu), set only for the first frame after a recompose that tracking follows,
     // null otherwise: the base frame's draw boxes (rcmp_old_draws), and the tables [old draw prefix (rcmp_n_old + 1)] [new draw
@@ -85,6 +90,7 @@ struct VbFrameBufs {
     uint32_t parts_pathtag, parts_flatten, parts_draw, parts_tile, parts_backdrop;
     uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
     uint32_t col_n, col_pitch; // bound colour rows and their pitch in bytes; 0 while unbound
+    uint32_t pt_n, pt_pitch;   // bound point rows and their pitch in bytes; 0 while unbound
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
@@ -94,6 +100,17 @@ struct VbFrameBufs {
 
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
 };
+
+// The regions prepare (vb_frame.cu) reserves past the scene's streams, in this order: the bound instance transforms, the viewed
+// transforms, the bound draw data, the bound path data, each present only with its binding or view. A region ends where the
+// next present one begins, the last at scene_words. Each launcher that writes one takes its length from here, never from
+// scene_words alone, so that it writes its own region and no later one.
+static inline uint32_t vb_transform_regions_end(const VbConfig &cfg, const VbFrameBufs &b) {
+    return b.col_rows ? cfg.layout.draw_data_base : b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
+}
+static inline uint32_t vb_draw_data_region_end(const VbConfig &cfg, const VbFrameBufs &b) {
+    return b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
+}
 
 // k_exchange.cu: flatten sharded by tag range, lines and path boxes exchanged through peer memory
 #define XG_MAX 8u // GPUs of one box
@@ -199,6 +216,14 @@ uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b
 uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n, uint32_t *slots, uint32_t n_words, cudaStream_t st);
 uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// k_points.cu: bound path points (vb_bind_path_points). The binding's table, once at bind time, from the n_words path tag words
+// at `tags`: first[p] = the first point of path p for p <= n_paths (first[n_paths]: the scene's points), and *i16 = 1 when a
+// segment tag lacks the F32 bit. Per frame, in flatten's stage after the draw data (prepare reserved the region, vb_frame.cu):
+// the scene's path data into the frame's region at layout.path_data_base, the words of each bound point with a finite row
+// replaced by the row's bits; nothing while unbound.
+uint32_t vb_launch_path_point_slots(const uint32_t *tags, uint32_t n_words, uint32_t n_paths, uint32_t *first, uint32_t *i16, cudaStream_t st);
+uint32_t vb_launch_path_points(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
 // the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame
 // succeeded. vb_launch_damage_rects stages caller rectangles (tile ranges x0 y0 x1 y1, clipped) into `pending` in stream order.
@@ -208,7 +233,7 @@ uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaSt
 uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
-size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col);
+size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt);
 // k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
 // of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
 // are null

@@ -61,8 +61,8 @@ void vb_host::drop_registrations(vb_renderer *r) {
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
-// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms or draw colours are bound
-// to it.
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours or path points
+// are bound to it.
 void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                       std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
     vb_renderer::SceneSlot &s = *r->cur;
@@ -82,6 +82,7 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
     r->colors = vb_renderer::ColorBinding{};
+    r->points = vb_renderer::PointBinding{};
     r->dmg.epoch++;
     // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
     vb_renderer::Damage::Diff &X = r->dmg.diff;

@@ -652,6 +652,16 @@ class Scene:
         adds no draw). `Renderer.hit_test` answers with these indices."""
         return len(self.encoding.draw_tags)
 
+    @property
+    def n_points(self) -> int:
+        """The path points encoded so far (path-data words / 2): the row `Renderer.bind_path_points` reads for the next point
+        a call encodes (read it before and after a call to learn the rows that call produced). A fill or stroke whose shape
+        encodes nothing adds no point; a push_*_layer whose clip encodes nothing adds 2, the empty path (0, 0) -> (0, 0) that
+        stands in for the clip. A move-to writes 1 point, a line-to, quad-to and cubic-to 1, 2 and 3; a closed fill subpath repeats its start
+        point when its last point differs; a stroke subpath ends with a cap marker (closed: a line-to, 1 point; open: a quad-to,
+        2 points); a dash's pieces are separate subpaths; arcs, circles and ellipses are cubics."""
+        return len(self.encoding.path_data) // 2
+
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
         e = self.encoding
         e.encode_transform(transform)

@@ -175,6 +175,7 @@ def load_library() -> C.CDLL:
     lib.vb_debug_match_instances.restype = C.c_uint32
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_draw_colors.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_path_points.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -196,7 +197,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
-                    "vb_bind_draw_colors"]
+                    "vb_bind_draw_colors", "vb_bind_path_points"]
 
 
 def _device_image(t, typestr="|u1"):
@@ -304,6 +305,7 @@ class Renderer:
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
         self._bound = None  # the device array of bind_instance_transforms
         self._colors = None  # the device array of bind_draw_colors
+        self._points = None  # the device array of bind_path_points
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
         self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
@@ -320,6 +322,7 @@ class Renderer:
         r._destinations = {}
         r._bound = None
         r._colors = None
+        r._points = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -510,6 +513,33 @@ class Renderer:
         self._check(self.lib.vb_bind_draw_colors(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
                     "vb_bind_draw_colors")
         self._colors = t
+
+    def bind_path_points(self, t):
+        """Take point k of the installed scene's path data from row k of the device array `t` in every frame from now on, read
+        when the frame runs (`vb_bind_path_points`): `t` is float32 (n, 2) x y rows, n at most the scene's `Scene.n_points`, with `__cuda_array_interface__` (e.g. a torch CUDA tensor, or columns of a larger one such as
+        `state[:, 4:6]`). Row k is path-data words 2k and 2k + 1 (global in a composed scene or a batch), in the coordinates the
+        point was encoded in: the path's transform, bound instance transforms and a view still apply. Every frame renders what
+        uploading the scene with those words overwritten would render; points from n on, and a point whose row is not finite,
+        keep their encoded values. Write it on `self.stream` (or synchronise) before a frame, never while one runs; frames then
+        need no further call. `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_path_points(self.handle, None, 0, 0), "vb_bind_path_points")
+            self._points = None
+            return
+        cai = getattr(t, "__cuda_array_interface__", None)
+        if cai is None:
+            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device points are needed")
+        shape = tuple(int(v) for v in cai["shape"])
+        if len(shape) != 2 or shape[0] == 0 or shape[1] != 2 or cai["typestr"] != "<f4":
+            raise ValueError(f"bind_path_points: points must be (n, 2) float32, not {shape} {cai['typestr']}")
+        strides = cai.get("strides") or (8, 4)
+        pitch = int(strides[0]) if shape[0] > 1 else 8  # the pitch of a single row is never used
+        if int(strides[1]) != 4 or pitch % 4 or pitch < 8:
+            raise ValueError(f"bind_path_points: columns 4 bytes apart and rows a multiple of 4 bytes, at least 8, apart; "
+                             f"not strides {tuple(strides)}")
+        self._check(self.lib.vb_bind_path_points(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
+                    "vb_bind_path_points")
+        self._points = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""

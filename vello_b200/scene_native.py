@@ -55,7 +55,8 @@ PATHBUF_SYMBOLS = ["vb_pathbuf_new", "vb_pathbuf_free", "vb_pathbuf_clear", "vb_
 SCENE_SYMBOLS = ["vb_scene_new", "vb_scene_free", "vb_scene_reset", "vb_scene_fill", "vb_scene_stroke", "vb_scene_push_layer",
                  "vb_scene_push_luminance_mask_layer", "vb_scene_push_clip_layer", "vb_scene_pop_layer", "vb_scene_draw_image",
                  "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_batch", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
-                 "vb_register_texture", "vb_unregister_texture", "vb_scene_n_draw_objects", "vb_scene_upload_fragment"]
+                 "vb_register_texture", "vb_unregister_texture", "vb_scene_n_draw_objects", "vb_scene_upload_fragment",
+                 "vb_scene_n_points"]
 
 _bound = False
 
@@ -70,6 +71,8 @@ def _lib():
         lib.vb_scene_reset.argtypes = [vp]
         lib.vb_scene_n_draw_objects.restype = C.c_uint32
         lib.vb_scene_n_draw_objects.argtypes = [vp]
+        lib.vb_scene_n_points.restype = C.c_uint32
+        lib.vb_scene_n_points.argtypes = [vp]
         lib.vb_scene_fill.argtypes = [vp, C.c_uint32, vp, vp, vp, vp]
         lib.vb_scene_stroke.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.vb_scene_push_layer.argtypes = [vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_float, vp, vp]
@@ -201,6 +204,11 @@ class NativeScene:
     def n_draw_objects(self) -> int:
         """`vb_scene_n_draw_objects`: the draw objects encoded so far, as `Scene.n_draw_objects`."""
         return int(self.lib.vb_scene_n_draw_objects(self.handle))
+
+    @property
+    def n_points(self) -> int:
+        """`vb_scene_n_points`: the path points encoded so far, as `Scene.n_points`."""
+        return int(self.lib.vb_scene_n_points(self.handle))
 
     # -- vello::Scene surface ------------------------------------------------------------------------
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
