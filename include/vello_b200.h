@@ -166,7 +166,7 @@ int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: wh
  *    even-odd rule, and the point lies inside the clip path of every enclosing BEGIN_CLIP (each with its own fill rule).
  *    Brush alpha, layer alpha and blend modes do not matter: a transparent fill is hit, an image or a blurred rectangle
  *    anywhere in the rectangle it is drawn in. Colour never matters, so bound draw colours (vb_bind_draw_colors) do not change
- *    the answers. Bound path points (vb_bind_path_points) are part of the frame's geometry: the answers follow the points the
+ *    the answers, nor do bound gradient stops (vb_bind_gradient_stops). Bound path points (vb_bind_path_points) are part of the frame's geometry: the answers follow the points the
  *    frame read. A point exactly on a line is decided by the half-open rules of the tile walk
  *    (tests/tile_walk_ref.py): deterministic, with no promise of the side.
  *  - BEGIN_CLIP / END_CLIP objects are never returned. Points outside the frame and NaN points give -1. Indices are the
@@ -503,7 +503,8 @@ int vb_bind_instance_transforms(vb_renderer *, const float *device_transforms, u
  *  - What a frame renders. While rows are bound, every frame renders the scene it would render if draw object k, for every
  *    k < n, had been encoded with Color(row k). This applies to draw objects whose paint is one colour: DRAWTAG_COLOR (solid
  *    fills and strokes) and BLUR_RECT (the colour of draw_blurred_rounded_rect[_in]). Rows of every other draw object
- *    (gradients, images, BEGIN_CLIP, END_CLIP) are ignored. Draw objects from n on keep the colour they were encoded with.
+ *    (gradients, images, BEGIN_CLIP, END_CLIP) are ignored; gradients take bound stops instead (vb_bind_gradient_stops).
+ *    Draw objects from n on keep the colour they were encoded with.
  *  - Conversion. The colour word is exactly the encoder's premultiply().to_rgba8().to_u32(): p = (r*a, g*a, b*a, a) in f32, and
  *    each channel is clamp(floor(p*255 + 0.5), 0, 255), where p*255 and + 0.5 are rounded separately in f32; r is the low byte.
  *    So a bound frame is byte-identical to uploading the scene re-encoded with those colours.
@@ -556,8 +557,8 @@ int vb_bind_draw_colors(vb_renderer *, const float *device_rgba, uint32_t n, siz
  *    traffic. Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next frame captures
  *    its graph anew. With nothing bound a frame launches, configures and captures exactly what it would without this call.
  *  - Scope. Every scene installation unbinds: every upload form, vb_render, vb_render_begin, vb_compose and vb_recompose. The
- *    binding survives vb_set_view, vb_set_cells, vb_bind_instance_transforms, vb_bind_draw_colors and hit tests; all three
- *    bindings can be active together. device_xy NULL unbinds; frames then render the scene as encoded.
+ *    binding survives vb_set_view, vb_set_cells, vb_bind_instance_transforms, vb_bind_draw_colors, vb_bind_gradient_stops and
+ *    hit tests; all four bindings can be active together. device_xy NULL unbinds; frames then render the scene as encoded.
  *  - The call finds each path's first point once, with one kernel over the path tags, and synchronises with vb_stream once to
  *    read back whether the scene has a 16-bit segment. Hit tests and hit maps answer from the bound geometry, and damage
  *    tracking follows the rows (see below).
@@ -568,6 +569,42 @@ int vb_bind_draw_colors(vb_renderer *, const float *device_rgba, uint32_t n, siz
  * segment (a segment tag without the F32 bit: its points are not f32 pairs; neither encoder emits one); a scene whose path
  * data, draw data and transform regions past its streams would pass 32-bit word offsets. */
 int vb_bind_path_points(vb_renderer *, const float *device_xy, uint32_t n, size_t row_pitch_bytes);
+/* Bind the stops of the installed scene's gradients to device memory (an addition; no vello counterpart). A heat-map legend or
+ * choropleth whose colour scale a model moves, a progress bar or shimmer that slides a stop, gradient-filled chart bars
+ * recoloured by live data or the fade of a gradient-filled widget changes its ramps without re-encoding or re-uploading the
+ * scene, and without a host call per frame:
+ *  - Rows. Row k is at device_stops + k * row_pitch_bytes and holds five f32 values offset, r, g, b, a: a vb_ramp_stop, i.e.
+ *    a straight-alpha, sRGB-encoded peniko ColorStop after the brush alpha the encoder applies. Row k is stop k of the
+ *    installed scene's ramp patches, concatenated in draw-data order (vello's Resources::color_stops); global in instance order
+ *    in a composed scene and in cell order in a batch. vb_scene_n_stops / Scene.n_stops counts them, read before and after a
+ *    call to learn the rows that call produced. Only gradients that keep a ramp have stops: a gradient with no stop or one
+ *    stop, and a degenerate radial or sweep gradient, is encoded as a colour (vb_bind_draw_colors binds it).
+ *  - What a frame renders. While rows are bound, every frame renders byte for byte what vb_scene_upload_streams renders for
+ *    the same streams with stop k of the patches replaced by row k, for every k < n. Each gradient keeps its extend mode,
+ *    interpolation alpha space and geometry. Offsets may be any finite values (out of order, equal, outside [0, 1]): make_ramp's
+ *    walk defines the ramp, on the device exactly as on the host. Stops from n on keep their encoded values.
+ *  - Non-finite rows. If any of a row's five values is NaN or +-inf, that stop keeps its encoded values for that frame.
+ *  - Scenes. Only a scene whose stops the renderer keeps can be bound: one installed from its streams (vb_scene_upload_streams,
+ *    vb_scene_upload_device, vb_render_scene) or by vb_compose / vb_recompose. A scene installed as packed bytes
+ *    (vb_scene_upload, vb_render, vb_render_begin) has only its resolved ramps.
+ *  - How. Resolves share one ramp row between gradients whose stops are equal, and bound rows may part them, so each bound
+ *    gradient (a patch with a stop below n) renders from a row of its own, after the scene's ramps. vb_debug_download("ramps")
+ *    returns the rows the last frame read: the scene's, then one per bound gradient in patch order.
+ *  - When rows are read, graphs and keys, scope: as vb_bind_draw_colors. Rows are read when the frame runs on vb_stream, in its
+ *    first stage (and again by a vb_run_stages range that starts at draw); a blocking re-run after an overflow reads them
+ *    again; changing only the contents replays the captured graph; binding, unbinding, or another pointer, n or pitch changes
+ *    the frame's key. Every scene installation unbinds; the binding survives views, cells, the three other bindings and hit
+ *    tests. device_stops NULL unbinds. With nothing bound a frame launches, configures and captures exactly what it would
+ *    without this call.
+ *  - The call copies the scene's ramps once on the device and synchronises with vb_stream once. Hit tests and hit maps do not
+ *    change, and damage tracking follows the rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed, or one installed as
+ * packed bytes; n = 0 with a non-NULL pointer, or n above the scene's stop count; a pointer that is not device memory of the
+ * renderer's device (or managed memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 20, or 4 GiB or
+ * more; a renderer of a vb_group or with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene
+ * whose ramps and one per bound gradient would pass the 30 bits of the (ramp id << 2) | extend word, or whose regions past its
+ * streams would pass 32-bit word offsets. */
+int vb_bind_gradient_stops(vb_renderer *, const float *device_stops, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -597,6 +634,9 @@ int vb_bind_path_points(vb_renderer *, const float *device_xy, uint32_t n, size_
  *    encoded point is no change. The damage is the tiles of the clipped box of draw object p (path p is draw object p) in the
  *    last frame and in this one. A changed clip path changes the boxes of the draws inside it only within its BEGIN_CLIP's own
  *    old and new box, which that draw object contributes.
+ *  - Automatic damage, for bound gradient stops (vb_bind_gradient_stops). A bound gradient changed if its 512-texel ramp row
+ *    differs byte for byte from the last successful frame's: rows that convert to the same texels are no change. The damage is
+ *    the tiles of its draw object's clipped box in the last frame and in this one.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
@@ -623,7 +663,7 @@ int vb_set_damage_tracking(vb_renderer *, int on);
  * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
  * all of these hold:
  *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound (no draw
- *    colours or path points bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
+ *    colours, path points or gradient stops bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
  *    tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
  *    frame full), and no vb_run_stages before the next one;

@@ -124,6 +124,11 @@ uint32_t vb_scene_n_draw_objects(const vb_scene *);
  * push_*_layer whose clip encodes nothing adds 2, the empty path (0, 0) -> (0, 0) that stands in for the clip (the full layout
  * is at vb_bind_path_points in vello_b200.h). 0 for NULL. */
 uint32_t vb_scene_n_points(const vb_scene *);
+/* The gradient stops encoded so far (an addition): the stops of the scene's ramp patches, concatenated in draw-data order,
+ * the row vb_bind_gradient_stops reads for the next stop a call encodes. Read it before and after a call to learn the rows
+ * that call produced. Only a gradient that keeps a ramp adds stops (its stops after the brush alpha); a gradient with no stop
+ * or one stop, and a degenerate radial or sweep gradient, is encoded as a colour and adds none. 0 for NULL. */
+uint32_t vb_scene_n_stops(const vb_scene *);
 
 /* Scene::fill, scene.rs:316-345. brush_transform may be NULL. */
 int vb_scene_fill(vb_scene *, uint32_t fill_rule, const double transform[6], const vb_brush *, const double *brush_transform,

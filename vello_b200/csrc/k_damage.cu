@@ -10,7 +10,9 @@
 //     draw data) differs bit for bit from the last successful frame's, its tile box in that frame and in this one
 //   + for every path with a bound point (vb_bind_path_points) whose two words (the ones flatten reads from the frame's path
 //     data) differ bit for bit from the last successful frame's, the tile box of its draw object (path i is draw object i) in
-//     that frame and in this one. A changed clip path is covered by its BEGIN_CLIP's boxes, as a moved clip is below.
+//     that frame and in this one. A changed clip path is covered by its BEGIN_CLIP's boxes, as a moved clip is below
+//   + for every bound gradient (vb_bind_gradient_stops) whose ramp row (the 512 texels fine reads) differs bit for bit from the
+//     last successful frame's, the tile box of its draw object in that frame and in this one.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -31,9 +33,9 @@
 #define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
 
 // a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects] [the
-// words of the first n_pt points (2 n_pt)]
-extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt) {
-    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt);
+// words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)]
+extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads) {
+    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt + 512u * (size_t)n_grads);
 }
 
 // the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
@@ -86,15 +88,18 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
     }
 }
 
-// One warp per draw object: its box and, below n_col, its colour word into the next slot; when its instance (n_inst > 0), its
-// colour word or its path's points (`paths`, non-null with points bound) changed, its old and new boxes into the mask. A draw
-// object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
+// One warp per draw object: its box, below n_col its colour word and, for a bound gradient (`grad`: the draw object's gradient
+// g or VB_COLOR_NONE, non-null with stops bound), its ramp row (`rows` + 512 g, at `at_rg` + 512 g of the slot) into the next
+// slot; when its instance (n_inst > 0), its colour word, its ramp row or its path's points (`paths`, non-null with points
+// bound) changed, its old and new boxes into the mask. A draw object whose paint is not one colour has colour word 0: its
+// bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
                                                        uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
                                                        const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht,
                                                        const uint32_t *__restrict__ draw_tags, const uint32_t *__restrict__ dd,
                                                        const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col,
-                                                       const uint32_t *__restrict__ paths, uint32_t n_paths) {
+                                                       const uint32_t *__restrict__ paths, uint32_t n_paths, const uint32_t *__restrict__ grad,
+                                                       const uint32_t *__restrict__ rows, size_t at_rg) {
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (d >= n_draw) return;
     const uint32_t *old;
@@ -110,6 +115,18 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict
         const size_t at = 6u * (size_t)n_xf + 4u * (size_t)n_draw + d;
         hit = col != old[at];
         if (lane == 0u) nxt[at] = col;
+    }
+    const uint32_t g = grad ? __ldg(grad + d) : VB_COLOR_NONE;
+    if (g != VB_COLOR_NONE) {
+        const uint32_t *row = rows + 512u * (size_t)g;
+        const size_t at = at_rg + 512u * (size_t)g;
+        bool diff = false;
+        for (uint32_t i = lane; i < 512u; i += 32u) {
+            const uint32_t w = __ldg(row + i);
+            diff = diff || w != old[at + i];
+            nxt[at + i] = w;
+        }
+        hit = __any_sync(0xffffffffu, diff) || hit;
     }
     __syncwarp();
     if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
@@ -153,10 +170,10 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst,
                                                                               b.dmg_paths, n_paths);
-    // neither transforms, colours nor points bound: nothing changes without a call that makes the frame full
-    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u) return 1u;
-    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n;
-    const size_t slot_words = at_pt + 2u * (size_t)b.pt_n;
+    // neither transforms, colours, points nor stops bound: nothing changes without a call that makes the frame full
+    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u) return 1u;
+    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n, at_rg = at_pt + 2u * (size_t)b.pt_n;
+    const size_t slot_words = at_rg + 512u * (size_t)b.rs_grads_n;
     uint32_t launches = 1u;
     const uint32_t n_pt = n_paths ? b.pt_n : 0u, n_mark = std::max(b.dmg_n_xf, n_pt);
     if (n_mark) {
@@ -171,7 +188,8 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
         k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
                                                                    n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
                                                                    b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n, b.dmg_paths,
-                                                                   n_paths);
+                                                                   n_paths, b.rs_grads_n ? b.rs_draw : nullptr,
+                                                                   b.ramps + 512u * (size_t)b.rs_ramp0, at_rg);
         launches++;
     }
     return launches;

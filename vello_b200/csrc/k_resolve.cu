@@ -3,7 +3,8 @@
 // vb_scene_upload_streams (vb_upload.cu) copies the six encoding streams straight to their Layout offsets inside the packed scene
 // buffer on the device; what is left of `resolve` runs here: the zero padding of the tag stream and the trailing PATH tags /
 // END_CLIP draw tags of unclosed clips (resolve.rs:127-141), the late-bound patches (gradient ramp id | extend, atlas x | y:
-// resolve.rs:268-330) and the gradient ramps themselves (512 premultiplied RGBA8 texels per unique gradient).
+// resolve.rs:268-330) and the gradient ramps themselves (512 premultiplied RGBA8 texels per unique gradient). The ramps of
+// bound gradient stops (vb_bind_gradient_stops) are made here too, every frame, by the same walk.
 // Arithmetic of the ramps is the host statement's (vb_scene.cpp make_ramp), float for float; the TU is built with -fmad=false.
 #include "vb_device.cuh"
 #include "vb_stages.h"
@@ -34,24 +35,25 @@ __device__ __forceinline__ uint32_t rs_premul_rgba8(float r, float g, float b, f
     return out;
 }
 
-// one CTA per ramp, one thread per texel. The host loop advances its stop cursor monotonically with u; starting from the
-// initial state for every texel reaches the same cursor (every advance made for a smaller u is also made for this one).
-__global__ void __launch_bounds__(RS_SAMPLES)
-k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
-    const RsRamp rp = ramps[blockIdx.x];
-    const RsStop *st = stops + rp.first_stop;
-    const uint32_t i = threadIdx.x;
+// Texel i of a ramp of n_stops stops, stop j read as stop(j): make_ramp's walk and conversion (vb_scene.cpp), which every
+// ramp on the device runs. Each product and sum is rounded on its own (the TU is built with -fmad=false), as on the host. The
+// host loop advances its stop cursor monotonically with u; starting from the initial state for every texel reaches the same
+// cursor (every advance made for a smaller u is also made for this one).
+template <class StopAt>
+__device__ __forceinline__ uint32_t rs_ramp_texel(uint32_t i, uint32_t n_stops, uint32_t premul, StopAt stop) {
     const float u = (float)i / (float)(RS_SAMPLES - 1u);
     float last_u = 0.0f, this_u = 0.0f;
-    float lr = st[0].r, lg = st[0].g, lb = st[0].b, la = st[0].a;
+    const RsStop s0 = stop(0u);
+    float lr = s0.r, lg = s0.g, lb = s0.b, la = s0.a;
     float tr = lr, tg = lg, tb = lb, ta = la;
     uint32_t j = 0u;
     while (u > this_u) {
         last_u = this_u;
         lr = tr; lg = tg; lb = tb; la = ta;
-        if (j + 1u < rp.n_stops) {
-            this_u = st[j + 1u].offset;
-            tr = st[j + 1u].r; tg = st[j + 1u].g; tb = st[j + 1u].b; ta = st[j + 1u].a;
+        if (j + 1u < n_stops) {
+            const RsStop sj = stop(j + 1u);
+            this_u = sj.offset;
+            tr = sj.r; tg = sj.g; tb = sj.b; ta = sj.a;
             j += 1u;
         } else {
             break;
@@ -63,7 +65,7 @@ k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
         cr = tr; cg = tg; cb = tb; ca = ta;
     } else {
         const float t = (u - last_u) / du;
-        if (rp.premul != 0u) { // AlphaColor::lerp: premultiply, lerp_rect, un-premultiply (color crate)
+        if (premul != 0u) { // AlphaColor::lerp: premultiply, lerp_rect, un-premultiply (color crate)
             const float pa[4] = {lr * la, lg * la, lb * la, la};
             const float pb[4] = {tr * ta, tg * ta, tb * ta, ta};
             float pc[4];
@@ -79,7 +81,67 @@ k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
             cr = lr + (tr - lr) * t; cg = lg + (tg - lg) * t; cb = lb + (tb - lb) * t; ca = la + (ta - la) * t;
         }
     }
-    out[(size_t)blockIdx.x * RS_SAMPLES + i] = rs_premul_rgba8(cr, cg, cb, ca);
+    return rs_premul_rgba8(cr, cg, cb, ca);
+}
+
+// one CTA per ramp, one thread per texel
+__global__ void __launch_bounds__(RS_SAMPLES)
+k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
+    const RsRamp rp = ramps[blockIdx.x];
+    const RsStop *st = stops + rp.first_stop;
+    const uint32_t i = threadIdx.x;
+    out[(size_t)blockIdx.x * RS_SAMPLES + i] = rs_ramp_texel(i, rp.n_stops, rp.premul, [&](uint32_t j) { return st[j]; });
+}
+
+// ---- bound gradient stops (vb_bind_gradient_stops) ------------------------------------------------------------------------------
+// A bound gradient renders from a ramp row of its own: resolves share one row between gradients whose stops are equal, and
+// bound rows may part them. The binding gives bound gradient g row ramp0 + g of a renderer-owned copy of the scene's ramps,
+// and k_draw_colors writes that row into the gradient's ramp word in the frame's draw data (VB_GRAD_SLOT). No pipeline kernel
+// changes: fine reads the row as any other, bounded by cfg.n_ramps.
+
+// One CTA: the bound gradients' ramp words into the draw-data slot table, then a walk over every draw tag (the exclusive scan
+// of their draw-data sizes, as k_draw_color_slots has it) that finds the draw object each of those words belongs to.
+#define RS_SLOT_THREADS 1024u
+__global__ void __launch_bounds__(RS_SLOT_THREADS) k_gradient_slots(const uint32_t *__restrict__ tags, uint32_t n_draw, const uint32_t *__restrict__ dd,
+                                                                    uint32_t n_grads, uint32_t *slots, uint32_t n_words, uint32_t *draw_grad) {
+    __shared__ uint32_t sh[RS_SLOT_THREADS / 32u + 1u];
+    for (uint32_t g = threadIdx.x; g < n_grads; g += RS_SLOT_THREADS) {
+        const uint32_t w = __ldg(dd + g);
+        if (w < n_words) slots[w] = VB_GRAD_SLOT | g;
+    }
+    __syncthreads();
+    uint32_t base = 0u;
+    for (uint32_t c = 0u; c < n_draw; c += RS_SLOT_THREADS) {
+        const uint32_t k = c + threadIdx.x;
+        const uint32_t tag = k < n_draw ? __ldg(tags + k) : VB_DRAWTAG_NOP;
+        uint32_t total;
+        const uint32_t off = base + vb_block_excl_scan((tag >> 2) & 7u, sh, &total);
+        const bool gradient = tag == VB_DRAWTAG_FILL_LIN_GRADIENT || tag == VB_DRAWTAG_FILL_RAD_GRADIENT || tag == VB_DRAWTAG_FILL_SWEEP_GRADIENT;
+        if (gradient && off < n_words) {
+            const uint32_t s = slots[off];
+            if (s != VB_COLOR_NONE && (s & VB_GRAD_SLOT)) draw_grad[k] = s & ~VB_GRAD_SLOT;
+        }
+        base += total;
+    }
+}
+
+// One CTA per bound gradient, one thread per texel: its ramp row from its stops, stop k (global over the scene's ramp patches)
+// read from the caller's row when k < n_rows and all five values are finite, else as encoded.
+__global__ void __launch_bounds__(RS_SAMPLES) k_bound_ramps(const RsRamp *__restrict__ grads, const RsStop *__restrict__ enc,
+                                                            const uint8_t *__restrict__ rows, uint32_t n_rows, uint32_t pitch, uint32_t *out) {
+    const RsRamp rp = grads[blockIdx.x];
+    const uint32_t i = threadIdx.x;
+    auto stop = [&](uint32_t j) {
+        const uint32_t k = rp.first_stop + j;
+        RsStop s = enc[k];
+        if (k < n_rows) {
+            const float *row = reinterpret_cast<const float *>(rows + (size_t)k * pitch);
+            const RsStop t = {__ldg(row), __ldg(row + 1), __ldg(row + 2), __ldg(row + 3), __ldg(row + 4)};
+            if (isfinite(t.offset) && isfinite(t.r) && isfinite(t.g) && isfinite(t.b) && isfinite(t.a)) s = t;
+        }
+        return s;
+    };
+    out[(size_t)blockIdx.x * RS_SAMPLES + i] = rs_ramp_texel(i, rp.n_stops, rp.premul, stop);
 }
 
 extern "C" void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes,
@@ -91,4 +153,16 @@ extern "C" void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, 
 }
 extern "C" void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st) {
     if (n_ramps) k_make_ramps<<<n_ramps, RS_SAMPLES, 0, st>>>(ramps, stops, out);
+}
+extern "C" uint32_t vb_launch_gradient_slots(const uint32_t *tags, uint32_t n_draw, const uint32_t *dd, uint32_t n_grads, uint32_t *slots,
+                                             uint32_t n_words, uint32_t *draw_grad, cudaStream_t st) {
+    if (n_grads == 0u) return 0u;
+    k_gradient_slots<<<1, RS_SLOT_THREADS, 0, st>>>(tags, n_draw, dd, n_grads, slots, n_words, draw_grad);
+    return 1u;
+}
+extern "C" uint32_t vb_launch_bound_ramps(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
+    if (!b.rs_rows || b.rs_grads_n == 0u) return 0u;
+    uint32_t *out = const_cast<uint32_t *>(b.ramps) + (size_t)b.rs_ramp0 * RS_SAMPLES;
+    k_bound_ramps<<<b.rs_grads_n, RS_SAMPLES, 0, st>>>(b.rs_grads, b.rs_stops, b.rs_rows, b.rs_n, b.rs_pitch, out);
+    return 1u;
 }

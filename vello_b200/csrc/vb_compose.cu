@@ -509,6 +509,17 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     slot.inst_draw.assign(pre + (size_t)CMP_DRAW_TAGS * (n + 1u), pre + (size_t)(CMP_DRAW_TAGS + 1) * (n + 1u));
     slot.inst_img = std::move(img_pre);
     slot.img_place = std::move(img_place);
+    // the instances' ramp patches with their keys' stops, in instance order, for vb_bind_gradient_stops (host copies)
+    uint32_t dd_rel = 0u;
+    for (uint32_t k = 0; k < n; k++) {
+        for (const Fragment::Ramp &p : fr[k]->ramps) {
+            const RampKey &key = *p.key;
+            slot.stop_patches.push_back({dd_rel + p.dd, (uint32_t)key.stops.size(), key.premul ? 1u : 0u, (uint32_t)slot.stops.size()});
+            slot.stops.insert(slot.stops.end(), key.stops.begin(), key.stops.end());
+        }
+        dd_rel += fr[k]->len[CMP_DRAW_DATA];
+    }
+    slot.have_stops = true;
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }
@@ -557,7 +568,7 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one), and
     // bound colours' draw data and bound points' path data after them
     const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
-    const uint64_t n_dd = r->colors.rows ? n_draw_data(slot.layout, slot.scene_words) : 0u;
+    const uint64_t n_dd = draw_data_bound(r) ? n_draw_data(slot.layout, slot.scene_words) : 0u;
     const uint64_t n_pd = r->points.rows ? n_path_data(slot.layout, slot.scene_words) : 0u;
     if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd + n_pd > 0xfffffff0ull)
         return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
@@ -602,9 +613,32 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
 }
 
 // ---- bound draw colours: vb_bind_draw_colors (k_colors.cu) ----------------------------------------------------------------------
-// The slot table is made once, here, on the renderer's stream: every word VB_COLOR_NONE, then one k_draw_color_slots over the
-// first n draw tags. It stays valid while the rows are bound, because every scene installation unbinds. Every frame after that
-// reads the caller's rows in its k_draw_colors.
+// The draw-data slot table is made here, on the renderer's stream, whenever bound colours or bound gradient stops change: every
+// word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col draw tags and one k_gradient_slots for the n_grads bound
+// gradients, whose ramp words are at grad_dd and whose draw objects it writes to draw_grad. It stays valid while the rows are
+// bound, because every scene installation unbinds. Every frame after that reads the caller's rows in its k_draw_colors.
+static int draw_data_slots(vb_renderer *r, uint32_t n_col, uint32_t n_grads, const uint32_t *grad_dd, uint32_t *draw_grad) {
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    const VbLayout &L = slot.layout;
+    const uint32_t n_dd = n_draw_data(L, slot.scene_words);
+    int rc;
+    if ((rc = compose_room(r, r->color_slots, (size_t)n_dd * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    uint32_t *slots = (uint32_t *)r->color_slots.p;
+    if (n_dd) CK(cudaMemsetAsync(slots, 0xff, (size_t)n_dd * 4u, st));
+    const uint32_t *tags = (const uint32_t *)slot.scene.p + L.draw_tag_base;
+    vb_launch_draw_color_slots(tags, n_col, slots, n_dd, st);
+    vb_launch_gradient_slots(tags, L.n_draw_objects, grad_dd, n_grads, slots, n_dd, draw_grad, st);
+    CK(cudaGetLastError());
+    return VB_OK;
+}
+// draw_data_slots for the bound gradients (none while unbound) and n_col colour rows
+static int draw_data_slots(vb_renderer *r, uint32_t n_col) {
+    const char *t = (const char *)r->stop_tables.p;
+    if (!r->stops.rows) return draw_data_slots(r, n_col, 0u, nullptr, nullptr);
+    return draw_data_slots(r, n_col, r->stops.n_grads, (const uint32_t *)(t + r->stops.o_dd), (uint32_t *)(t + r->stops.o_draw));
+}
+
 extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uint32_t n, size_t row_pitch_bytes) {
     if (!r) return VB_E_INVALID;
     auto bad = [&](const std::string &why) {
@@ -614,6 +648,12 @@ extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uin
     if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
     if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
     if (!device_rgba) {
+        // bound gradient stops keep the region: its colour slots go
+        if (r->colors.rows && r->stops.rows) {
+            CK(cudaSetDevice(r->device));
+            const int rc = draw_data_slots(r, 0u);
+            if (rc) return rc;
+        }
         r->colors = vb_renderer::ColorBinding{};
         r->dmg.epoch++;
         return VB_OK;
@@ -635,13 +675,8 @@ extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uin
     if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_dd + n_pd > 0xfffffff0ull)
         return bad("the scene with its bound draw data and its bound and viewed transforms exceeds 32-bit word offsets");
     if ((uint64_t)L.draw_tag_base + n > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
-    int rc;
-    if ((rc = compose_room(r, r->color_slots, (size_t)n_dd * 4u))) return rc;
-    cudaStream_t st = r->stream;
-    uint32_t *slots = (uint32_t *)r->color_slots.p;
-    if (n_dd) CK(cudaMemsetAsync(slots, 0xff, (size_t)n_dd * 4u, st));
-    vb_launch_draw_color_slots((const uint32_t *)slot.scene.p + L.draw_tag_base, n, slots, n_dd, st);
-    CK(cudaGetLastError());
+    const int rc = draw_data_slots(r, n);
+    if (rc) return rc;
     r->colors.rows = (const uint8_t *)device_rgba;
     r->colors.n = n;
     r->colors.pitch = (uint32_t)row_pitch_bytes;
@@ -697,6 +732,93 @@ extern "C" int vb_bind_path_points(vb_renderer *r, const float *device_xy, uint3
     r->points.rows = (const uint8_t *)device_xy;
     r->points.n = n;
     r->points.pitch = (uint32_t)row_pitch_bytes;
+    r->dmg.epoch++;
+    return VB_OK;
+}
+
+// ---- bound gradient stops: vb_bind_gradient_stops (k_resolve.cu) ---------------------------------------------------------------
+// The bound gradients are the scene's first n_grads ramp patches: those with a stop below n (the stops are concatenated in patch
+// order). Made once, here, on the renderer's stream: the binding's tables (stop_tables), the scene's ramps copied into the
+// first rows of stop_ramps, and the draw-data slot table with the gradients' ramp words (draw_data_slots). The call's one
+// synchronisation waits for the tables' copy. They stay valid while the rows are bound, because every scene installation
+// unbinds. Every frame after that writes the gradients' rows from the caller's rows in its k_bound_ramps.
+extern "C" int vb_bind_gradient_stops(vb_renderer *r, const float *device_stops, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_gradient_stops: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_stops) {
+        const bool had = r->stops.rows != nullptr;
+        r->stops = vb_renderer::StopBinding{};
+        // bound colours keep the region: the gradients' slots go
+        if (had && r->colors.rows) {
+            CK(cudaSetDevice(r->device));
+            const int rc = draw_data_slots(r, r->colors.n);
+            if (rc) return rc;
+        }
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene) return bad("no scene installed");
+    if (!slot.have_stops)
+        return bad("the scene was installed as packed bytes, whose gradients exist only as resolved ramps; install it from its "
+                   "streams (vb_scene_upload_streams, vb_scene_upload_device, vb_render_scene) or with vb_compose");
+    const VbLayout &L = slot.layout;
+    const size_t n_stops = slot.stops.size();
+    if (n == 0u || n > n_stops)
+        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_stops) + " gradient stops (1 .. n_stops)");
+    if ((uintptr_t)device_stops & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 20u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 20 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_stops)) return bad("the rows must be memory of the renderer's device");
+    uint32_t n_grads = 0u;
+    while (n_grads < slot.stop_patches.size() && slot.stop_patches[n_grads].first < n) n_grads++;
+    if ((uint64_t)slot.n_ramps + n_grads > (1ull << 30))
+        return bad("the scene's ramps and one per bound gradient pass the 30 bits of the ramp word");
+    // a frame writes the bound draw data past the scene, after the bound and viewed transforms, and bound points' path data
+    // after it (prepare, vb_frame.cu)
+    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_draw_data(L, slot.scene_words) + n_pd > 0xfffffff0ull)
+        return bad("the scene with its bound draw data, path data and bound and viewed transforms exceeds 32-bit word offsets");
+    if ((uint64_t)L.draw_tag_base + L.n_draw_objects > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
+
+    // the tables: [gradients (RsRamp)] [their stops as encoded, at o_stops] [ramp words, at o_dd] [draw object -> gradient, at o_draw]
+    const vb_renderer::SceneSlot::StopPatch *last = n_grads ? &slot.stop_patches[n_grads - 1u] : nullptr;
+    const size_t s_used = last ? (size_t)last->first + last->n_stops : 0u;
+    vb_renderer::StopBinding nb;
+    nb.rows = (const uint8_t *)device_stops;
+    nb.n = n;
+    nb.pitch = (uint32_t)row_pitch_bytes;
+    nb.n_grads = n_grads;
+    nb.ramp0 = slot.n_ramps;
+    nb.o_stops = up16((size_t)n_grads * sizeof(RsRamp));
+    nb.o_dd = up16(nb.o_stops + s_used * sizeof(RsStop));
+    nb.o_draw = up16(nb.o_dd + (size_t)n_grads * 4u);
+    const size_t bytes = nb.o_draw + (size_t)L.n_draw_objects * 4u;
+    std::vector<uint8_t> h(bytes, 0u);
+    RsRamp *grads = (RsRamp *)h.data();
+    uint32_t *dd = (uint32_t *)(h.data() + nb.o_dd);
+    for (uint32_t g = 0; g < n_grads; g++) {
+        const vb_renderer::SceneSlot::StopPatch &p = slot.stop_patches[g];
+        grads[g] = RsRamp{p.first, p.n_stops, p.premul, 0u};
+        dd[g] = p.dd;
+    }
+    if (s_used) memcpy(h.data() + nb.o_stops, slot.stops.data(), s_used * sizeof(RsStop));
+    memset(h.data() + nb.o_draw, 0xff, (size_t)L.n_draw_objects * 4u);
+    int rc;
+    if ((rc = compose_room(r, r->stop_tables, bytes))) return rc;
+    if ((rc = compose_room(r, r->stop_ramps, ((size_t)slot.n_ramps + n_grads) * 512u * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    CK(cudaMemcpyAsync(r->stop_tables.p, h.data(), bytes, cudaMemcpyHostToDevice, st));
+    if (slot.n_ramps) CK(cudaMemcpyAsync(r->stop_ramps.p, slot.ramps.p, (size_t)slot.n_ramps * 512u * 4u, cudaMemcpyDeviceToDevice, st));
+    r->stops = nb;
+    if ((rc = draw_data_slots(r, r->colors.rows ? r->colors.n : 0u))) return rc;
+    CK(cudaStreamSynchronize(st)); // h is read by the copy
     r->dmg.epoch++;
     return VB_OK;
 }

@@ -53,6 +53,8 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
         {"ramps", &r->cur->ramps, (size_t)r->cur->n_ramps * 512 * 4},
         {"atlas", &r->cur->atlas, (size_t)r->cur->atlas_w * r->cur->atlas_h * 4},
     };
+    // the ramps the last frame read: with bound gradient stops the binding's, the scene's and then one row per gradient
+    if (r->bufs.ramps && r->bufs.ramps == (const uint32_t *)r->stop_ramps.p) v[1] = {"ramps", &r->stop_ramps, (size_t)c.n_ramps * 512 * 4};
     // the fixed-size intermediates of the frame prepared last
     for (int i = 0; i < N_FIXED_BUFS; i++)
         if (FRAME_BUFS[i].downloadable) v.push_back({FRAME_BUFS[i].name, &r->fb[i], FRAME_BUFS[i].bytes(r->counts, true)});

@@ -395,6 +395,8 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.n_tag_words = r->cur->layout.path_data_base - r->cur->layout.path_tag_base;
     c.scene_words = (uint32_t)r->cur->scene_words;
     c.n_ramps = r->cur->n_ramps;
+    // bound gradient stops: the frame reads the binding's ramps, the scene's and then one row per bound gradient
+    if (r->stops.rows) c.n_ramps = r->stops.ramp0 + r->stops.n_grads;
     c.atlas_w = r->cur->atlas_w;
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
@@ -414,9 +416,10 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
         c.frame_cull = 1u;
     }
-    if (r->colors.rows) {
+    if (draw_data_bound(r)) {
         // the frame reads its draw data past the scene's streams and the transform regions: [draw_data_base, scene_words) is
-        // the region k_draw_colors writes from the scene's draw data and the caller's rows (bound path data follows it)
+        // the region k_draw_colors writes from the scene's draw data, the caller's colour rows and the bound gradients' ramp
+        // rows (bound path data follows it)
         c.layout.draw_data_base = c.scene_words;
         c.scene_words += n_draw_data(r->cur->layout, r->cur->scene_words);
     }
@@ -426,8 +429,8 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         c.layout.path_data_base = c.scene_words;
         c.scene_words += n_path_data(r->cur->layout, r->cur->scene_words);
     }
-    if (n_regions || r->colors.rows || r->points.rows) {
-        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, r->colors.rows != nullptr,
+    if (n_regions || draw_data_bound(r) || r->points.rows) {
+        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, draw_data_bound(r),
                                                         r->points.rows != nullptr));
         if (rc0) return rc0;
     }
@@ -494,12 +497,26 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.inst_n = r->bound.n;
         b.inst_pitch = r->bound.pitch;
     }
+    if (draw_data_bound(r)) {
+        b.col_slots = (const uint32_t *)r->color_slots.p;
+        b.col_src = b.scene + r->cur->layout.draw_data_base;
+    }
     if (r->colors.rows) {
         b.col_rows = r->colors.rows;
-        b.col_slots = (const uint32_t *)r->color_slots.p;
         b.col_n = r->colors.n;
         b.col_pitch = r->colors.pitch;
-        b.col_src = b.scene + r->cur->layout.draw_data_base;
+    }
+    if (r->stops.rows) {
+        const char *t = (const char *)r->stop_tables.p;
+        b.ramps = (const uint32_t *)r->stop_ramps.p;
+        b.rs_rows = r->stops.rows;
+        b.rs_grads = (const RsRamp *)t;
+        b.rs_stops = (const RsStop *)(t + r->stops.o_stops);
+        b.rs_draw = (const uint32_t *)(t + r->stops.o_draw);
+        b.rs_n = r->stops.n;
+        b.rs_pitch = r->stops.pitch;
+        b.rs_grads_n = r->stops.n_grads;
+        b.rs_ramp0 = r->stops.ramp0;
     }
     if (r->points.rows) {
         b.pt_rows = r->points.rows;
@@ -598,11 +615,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
             // a frame with bound instance transforms or a view first writes its transforms (read by flatten and draw), the
-            // bound ones first (the view's source), a frame with bound colours its draw data (read by draw, coarse and
-            // fine), and a frame with bound points its path data (read by flatten alone), inside flatten's stage events
+            // bound ones first (the view's source), a frame with bound colours or stops its draw data (read by draw, coarse
+            // and fine) and with bound stops its gradients' ramp rows (read by fine), and a frame with bound points its path
+            // data (read by flatten alone), inside flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             launches += vb_launch_draw_colors(c, b, st);
+            launches += vb_launch_bound_ramps(c, b, st);
             launches += vb_launch_path_points(c, b, st);
             if (fork_draw) {
                 CK(cudaEventRecord(r->draw_fork, st));
@@ -630,6 +649,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_instance_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_colors(c, b, st);
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_ramps(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);
             if (fork_draw) CK(cudaStreamWaitEvent(st, r->draw_join, 0)); // launched beside flatten

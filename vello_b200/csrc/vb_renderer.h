@@ -2,8 +2,8 @@
 //
 // The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
 // (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
-// instance transforms and draw colours), vb_damage.cu (damage tracking), vb_debug.cu (debug downloads and uploads) and
-// vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
+// instance transforms, draw colours, path points and gradient stops), vb_damage.cu (damage tracking), vb_debug.cu (debug
+// downloads and uploads) and vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
 // namespace vb_host, hidden from the shared library's symbol table, so that a host program's own functions of the same names
 // cannot interpose on them.
 #pragma once
@@ -200,6 +200,13 @@ struct vb_renderer {
         // for vb_recompose: the atlas places of the instances' images in patch order, instance k's from inst_img[k] (n + 1)
         std::vector<uint32_t> inst_img;
         std::vector<ImgPlace> img_place;
+        // for vb_bind_gradient_stops: the scene's ramp patches in draw-data order, each with its ramp word (relative to the
+        // draw data), its stop count, interpolation space and first stop in `stops`, the encoded stops concatenated. Kept by
+        // streams installations and vb_compose (have_stops), cleared by packed uploads, whose stops exist only as resolved ramps.
+        struct StopPatch { uint32_t dd, n_stops, premul, first; };
+        bool have_stops = false;
+        std::vector<StopPatch> stop_patches;
+        std::vector<vb_ramp_stop> stops;
     } slot[2];
     SceneSlot *cur = slot;
     DevBuf mask8, mask16;
@@ -324,6 +331,18 @@ struct vb_renderer {
         uint32_t n = 0, pitch = 0;
     } points;
     DevBuf point_slots;
+    // bound gradient stops (vb_bind_gradient_stops) of the current scene: the caller's rows (nullptr: unbound). The first
+    // n_grads ramp patches are bound (those with a stop below n); gradient g reads ramp row ramp0 + g of stop_ramps, whose rows
+    // below ramp0 are a copy of the scene's ramps. stop_tables holds [the gradients as RsRamp (first stop, count, premul)]
+    // [their encoded stops, at o_stops] [each one's ramp word in the draw data, at o_dd] [per draw object its gradient or
+    // VB_COLOR_NONE, at o_draw] (k_resolve.cu). The draw-data slot table (color_slots) marks the gradients' ramp words. Every
+    // scene installation unbinds (set_scene).
+    struct StopBinding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0, n_grads = 0, ramp0 = 0;
+        size_t o_stops = 0, o_dd = 0, o_draw = 0;
+    } stops;
+    DevBuf stop_tables, stop_ramps;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -380,6 +399,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
                            &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
+                           &r->stop_tables, &r->stop_ramps,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
@@ -447,6 +467,8 @@ inline uint32_t n_path_data(const VbLayout &L, size_t scene_words) {
     if (L.draw_tag_base < L.path_data_base || L.draw_tag_base > scene_words) return 0u;
     return L.draw_tag_base - L.path_data_base;
 }
+// Whether frames read their draw data from the region past the scene's streams: with bound colours or bound gradient stops.
+inline bool draw_data_bound(const vb_renderer *r) { return r->colors.rows || r->stops.rows; }
 // A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
 // transforms, k_compose.cu; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
 // k_colors.cu) and with `points` a region of path data after those (bound path points, k_points.cu), then slack.

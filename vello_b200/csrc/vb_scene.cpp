@@ -1171,6 +1171,12 @@ void vb_scene_reset(vb_scene *s) {
 }
 uint32_t vb_scene_n_draw_objects(const vb_scene *s) { return s ? (uint32_t)s->e.draw_tags.size() : 0u; }
 uint32_t vb_scene_n_points(const vb_scene *s) { return s ? (uint32_t)(s->e.path_data.size() / 2u) : 0u; }
+uint32_t vb_scene_n_stops(const vb_scene *s) {
+    size_t n = 0;
+    if (s)
+        for (const RampPatch &p : s->e.ramp_patches) n += p.stops.size();
+    return (uint32_t)n;
+}
 
 int vb_scene_fill(vb_scene *s, uint32_t fill_rule, const double transform[6], const vb_brush *brush, const double *brush_transform,
                   const vb_path *path) {

@@ -12,6 +12,10 @@
 #include "vb_resolve.h"
 #include "vb_types.h"
 
+// k_resolve.cu: records of the device resolve, staged by vb_scene_upload_streams and vb_compose (and RsPatch, vb_resolve.h)
+struct RsRamp { uint32_t first_stop, n_stops, premul, pad; };     // one gradient ramp: its stops and interpolation space
+struct RsStop { float offset, r, g, b, a; };                      // == vb_ramp_stop
+
 struct FlLit; // flatten's scratch records (k_flatten.cu)
 struct FlJob;
 struct CmpXform; // an instance's transform (k_compose.cu, below)
@@ -33,11 +37,21 @@ struct VbFrameBufs {
     const uint32_t *inst_prefix;
     const CmpXform *inst_xf;
     const uint32_t *inst_src;
-    // bound draw colours (vb_bind_draw_colors), read by k_draw_colors: the caller's rows (draw object k's at col_rows + k *
-    // col_pitch bytes), the binding's slot table (per draw-data word of the scene, the row whose colour replaces it, or
-    // VB_COLOR_NONE) and the scene's own draw data, the region's source. Null while unbound.
+    // the bound draw-data region, written by k_draw_colors with bound colours (vb_bind_draw_colors) or bound gradient stops
+    // (vb_bind_gradient_stops): the caller's colour rows (draw object k's at col_rows + k * col_pitch bytes; null while colours
+    // are unbound), the slot table (per draw-data word of the scene: the colour row whose conversion replaces it, VB_GRAD_SLOT
+    // | g for bound gradient g's ramp word, or VB_COLOR_NONE) and the scene's own draw data, the region's source. col_slots and
+    // col_src are null while neither is bound.
     const uint8_t *col_rows;
     const uint32_t *col_slots, *col_src;
+    // bound gradient stops (vb_bind_gradient_stops), read by k_bound_ramps: the caller's rows (stop k's at rs_rows + k *
+    // rs_pitch bytes), the bound gradients (rs_grads_n RsRamp records over the scene's stop indices) with their encoded stops,
+    // and per draw object its bound gradient or VB_COLOR_NONE (k_damage). Gradient g's ramp row is ramps + (rs_ramp0 + g) *
+    // 512. Null while unbound.
+    const uint8_t *rs_rows;
+    const RsRamp *rs_grads;
+    const RsStop *rs_stops;
+    const uint32_t *rs_draw;
     // bound path points (vb_bind_path_points), read by k_path_points: the caller's rows (point k's at pt_rows + k * pt_pitch
     // bytes), the binding's table of each path's first point (layout.n_paths + 1; k_damage maps changed points to paths with
     // it) and the scene's own path data, the region's source. Null while unbound.
@@ -91,6 +105,8 @@ struct VbFrameBufs {
     uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
     uint32_t col_n, col_pitch; // bound colour rows and their pitch in bytes; 0 while unbound
     uint32_t pt_n, pt_pitch;   // bound point rows and their pitch in bytes; 0 while unbound
+    uint32_t rs_n, rs_pitch;   // bound stop rows and their pitch in bytes; 0 while unbound
+    uint32_t rs_grads_n, rs_ramp0; // bound gradients and the ramp row of the first; 0 while unbound
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
@@ -106,7 +122,7 @@ struct VbFrameBufs {
 // next present one begins, the last at scene_words. Each launcher that writes one takes its length from here, never from
 // scene_words alone, so that it writes its own region and no later one.
 static inline uint32_t vb_transform_regions_end(const VbConfig &cfg, const VbFrameBufs &b) {
-    return b.col_rows ? cfg.layout.draw_data_base : b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
+    return b.col_slots ? cfg.layout.draw_data_base : b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
 }
 static inline uint32_t vb_draw_data_region_end(const VbConfig &cfg, const VbFrameBufs &b) {
     return b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
@@ -121,9 +137,6 @@ struct XPeers {
     unsigned long long half_bytes;
 };
 
-// k_resolve.cu: records of the device resolve, staged by vb_scene_upload_streams and vb_compose (and RsPatch, vb_resolve.h)
-struct RsRamp { uint32_t first_stop, n_stops, premul, pad; };     // one gradient ramp: its stops and interpolation space
-struct RsStop { float offset, r, g, b, a; };                      // == vb_ramp_stop
 
 extern "C" {
 // stages, in pipeline order
@@ -188,6 +201,15 @@ uint32_t vb_launch_hit_map(const VbConfig &cfg, const VbFrameBufs &b, uint32_t x
 void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes, uint32_t end_clip_word0,
                               const RsPatch *patches, uint32_t n_patches, cudaStream_t st);
 void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st);
+// bound gradient stops (vb_bind_gradient_stops). The binding's tables, once at bind time: slots[dd[g]] = VB_GRAD_SLOT | g for
+// each of the n_grads bound gradients (dd: its ramp word, relative to the draw data), then from the scene's n_draw draw tags at
+// `tags`, draw_grad[k] = g for the gradient draw object k whose ramp word that is; the caller sets both tables to
+// VB_COLOR_NONE first. Per frame, in flatten's stage after the draw data (vb_frame.cu): each bound gradient's ramp row from its
+// stops, each read from the caller's row when it is bound and finite, else as encoded; nothing while unbound.
+#define VB_GRAD_SLOT 0x80000000u
+uint32_t vb_launch_gradient_slots(const uint32_t *tags, uint32_t n_draw, const uint32_t *dd, uint32_t n_grads, uint32_t *slots, uint32_t n_words,
+                                  uint32_t *draw_grad, cudaStream_t st);
+uint32_t vb_launch_bound_ramps(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_compose.cu: the six streams of a composition of resident fragments (vb_compose), staged by vb_compose.cu
 struct CmpXform { float m[6]; uint32_t on, pad; }; // an instance's transform (on == 0: appended without one)
@@ -211,7 +233,8 @@ uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b
 // word w (relative to the draw data) of each draw object k < n whose paint is one colour (FILL_COLOR, BLURRED_ROUNDED_RECT),
 // from the scene's draw tags at `tags`; the caller sets the n_words words of the table to VB_COLOR_NONE first. Per frame, in
 // flatten's stage after the transforms (prepare reserved the region, vb_frame.cu): the scene's draw data into the frame's
-// region at layout.draw_data_base, each slot's word replaced by its row's premultiplied RGBA8 word; nothing while unbound.
+// region at layout.draw_data_base, each colour slot's word replaced by its row's premultiplied RGBA8 word and each gradient
+// slot's ramp id by its bound row (b.rs_ramp0 + g; VB_GRAD_SLOT, k_resolve.cu); nothing while neither is bound.
 #define VB_COLOR_NONE 0xffffffffu
 uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n, uint32_t *slots, uint32_t n_words, cudaStream_t st);
 uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
@@ -233,7 +256,7 @@ uint32_t vb_launch_path_points(const VbConfig &cfg, const VbFrameBufs &b, cudaSt
 uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
-size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt);
+size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads);
 // k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
 // of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
 // are null

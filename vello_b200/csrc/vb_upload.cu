@@ -61,8 +61,8 @@ void vb_host::drop_registrations(vb_renderer *r) {
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
-// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours or path points
-// are bound to it.
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours, path points
+// or gradient stops are bound to it. Its stops are unknown until the installer that has them keeps them (keep_stops).
 void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                       std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
     vb_renderer::SceneSlot &s = *r->cur;
@@ -78,11 +78,15 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     s.inst_draw.clear();
     s.inst_img.clear();
     s.img_place.clear();
+    s.have_stops = false;
+    s.stop_patches.clear();
+    s.stops.clear();
     s.have_scene = true;
     r->cells.clear();
     r->bound = vb_renderer::Binding{};
     r->colors = vb_renderer::ColorBinding{};
     r->points = vb_renderer::PointBinding{};
+    r->stops = vb_renderer::StopBinding{};
     r->dmg.epoch++;
     // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
     vb_renderer::Damage::Diff &X = r->dmg.diff;
@@ -540,6 +544,18 @@ int vb_host::image_source(vb_renderer *r, const char *who, const void *key, uint
     return VB_OK;
 }
 
+// The installed scene's ramp patches and their encoded stops, for vb_bind_gradient_stops: host copies, no device work.
+static void keep_stops(vb_renderer *r, const vb_encoding_streams *e) {
+    vb_renderer::SceneSlot &s = *r->cur;
+    s.stop_patches.reserve(e->n_ramp_patches);
+    for (uint32_t i = 0; i < e->n_ramp_patches; i++) {
+        const vb_ramp_patch &p = e->ramp_patches[i];
+        s.stop_patches.push_back({p.draw_data_offset, p.n_stops, p.premul_interp ? 1u : 0u, (uint32_t)s.stops.size()});
+        s.stops.insert(s.stops.end(), p.stops, p.stops + p.n_stops);
+    }
+    s.have_stops = true;
+}
+
 extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams *e, vb_layout *layout_out) {
     if (!r || !e) return VB_E_INVALID;
     int rc = check_streams(r, e, "vb_scene_upload_streams");
@@ -611,6 +627,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     // the host vectors above are read by the asynchronous copies: they must outlive them
     CK(cudaStreamSynchronize(st));
     set_scene(r, L, plan.words, (uint32_t)ramps.size(), plan.atlas_w, plan.atlas_h, std::move(over), false);
+    keep_stops(r, e);
     if (layout_out) memcpy(layout_out, &L, sizeof(vb_layout));
     return VB_OK;
 }

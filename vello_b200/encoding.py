@@ -662,6 +662,14 @@ class Scene:
         2 points); a dash's pieces are separate subpaths; arcs, circles and ellipses are cubics."""
         return len(self.encoding.path_data) // 2
 
+    @property
+    def n_stops(self) -> int:
+        """The gradient stops encoded so far: the stops of the ramp patches, concatenated in draw-data order, and the row
+        `Renderer.bind_gradient_stops` reads for the next stop a call encodes (read it before and after a call to learn the
+        rows that call produced). Only a gradient that keeps a ramp adds stops, after the brush alpha; a gradient with no stop
+        or one stop, and a degenerate radial or sweep gradient, is encoded as a colour and adds none."""
+        return sum(len(p["stops"]) for p in self.encoding.ramp_patches)
+
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
         e = self.encoding
         e.encode_transform(transform)

@@ -176,6 +176,7 @@ def load_library() -> C.CDLL:
     lib.vb_bind_instance_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_draw_colors.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_path_points.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_gradient_stops.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -197,7 +198,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
-                    "vb_bind_draw_colors", "vb_bind_path_points"]
+                    "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops"]
 
 
 def _device_image(t, typestr="|u1"):
@@ -306,6 +307,7 @@ class Renderer:
         self._bound = None  # the device array of bind_instance_transforms
         self._colors = None  # the device array of bind_draw_colors
         self._points = None  # the device array of bind_path_points
+        self._stops = None  # the device array of bind_gradient_stops
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
         self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
@@ -323,6 +325,7 @@ class Renderer:
         r._bound = None
         r._colors = None
         r._points = None
+        r._stops = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -355,6 +358,17 @@ class Renderer:
                                       ramps.ctypes.data if ramps.size else None, 512, ramps.shape[0],
                                       atlas.ctypes.data, atlas.shape[1], atlas.shape[0])
         self._check(rc, "vb_scene_upload")
+
+    def upload_scene(self, scene) -> "Layout":
+        """Resolve the `Scene` `scene` on the device and install it (`vb_scene_upload_streams`), keeping its gradient stops, so
+        that `bind_gradient_stops` can bind them (a packed `upload` keeps only resolved ramps). Returns its Layout."""
+        from .encoding import Layout
+        e, keep = _encoding_streams(scene.encoding, self._image_key)
+        L = _Layout()
+        self._check(self.lib.vb_scene_upload_streams(self.handle, C.byref(e), C.byref(L)), "vb_scene_upload_streams")
+        self._cells = 1
+        return Layout(L.n_draw_objects, L.n_paths, L.n_clips, L.bin_data_start, L.path_tag_base, L.path_data_base, L.draw_tag_base,
+                      L.draw_data_base, L.transform_base, L.style_base)
 
     # -- images from device memory (Renderer::override_image / register_texture, vello/src/lib.rs:536-603) ---------------------
     # Overrides apply where the scene is resolved on the device (NativeScene.upload_device); a host-packed scene (upload,
@@ -540,6 +554,35 @@ class Renderer:
         self._check(self.lib.vb_bind_path_points(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
                     "vb_bind_path_points")
         self._points = t
+
+    def bind_gradient_stops(self, t):
+        """Take stop k of the installed scene's gradients from row k of the device array `t` in every frame from now on, read
+        when the frame runs (`vb_bind_gradient_stops`): `t` is float32 (n, 5) offset r g b a rows (straight alpha, after the
+        brush alpha), n at most the scene's `Scene.n_stops`, with `__cuda_array_interface__` (e.g. a torch CUDA tensor, or
+        columns of a larger one such as `state[:, 2:7]`). Row k is stop k of the ramp patches in draw-data order (global in a
+        composed scene or a batch). Every frame renders what uploading the scene's streams with those stops would render; stops
+        from n on, and a stop whose row is not finite, keep their encoded values. The scene must have been installed with its
+        stops (`upload_scene`, `NativeScene.upload_device`, `compose`), not as packed bytes. Write it on `self.stream` (or
+        synchronise) before a frame, never while one runs; frames then need no further call. `t` is held while bound; None
+        unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_gradient_stops(self.handle, None, 0, 0), "vb_bind_gradient_stops")
+            self._stops = None
+            return
+        cai = getattr(t, "__cuda_array_interface__", None)
+        if cai is None:
+            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device stops are needed")
+        shape = tuple(int(v) for v in cai["shape"])
+        if len(shape) != 2 or shape[0] == 0 or shape[1] != 5 or cai["typestr"] != "<f4":
+            raise ValueError(f"bind_gradient_stops: stops must be (n, 5) float32, not {shape} {cai['typestr']}")
+        strides = cai.get("strides") or (20, 4)
+        pitch = int(strides[0]) if shape[0] > 1 else 20  # the pitch of a single row is never used
+        if int(strides[1]) != 4 or pitch % 4 or pitch < 20:
+            raise ValueError(f"bind_gradient_stops: columns 4 bytes apart and rows a multiple of 4 bytes, at least 20, apart; "
+                             f"not strides {tuple(strides)}")
+        self._check(self.lib.vb_bind_gradient_stops(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
+                    "vb_bind_gradient_stops")
+        self._stops = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
