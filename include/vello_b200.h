@@ -167,7 +167,7 @@ int vb_debug_graph_captures(vb_renderer *, uint64_t *captures); /* test-only: wh
  *    Brush alpha, layer alpha and blend modes do not matter: a transparent fill is hit, an image or a blurred rectangle
  *    anywhere in the rectangle it is drawn in. Colour never matters, so bound draw colours (vb_bind_draw_colors) do not change
  *    the answers, nor do bound gradient stops (vb_bind_gradient_stops). Bound path points (vb_bind_path_points) are part of the frame's geometry: the answers follow the points the
- *    frame read. A point exactly on a line is decided by the half-open rules of the tile walk
+ *    frame read, and so are bound transforms (vb_bind_transforms): the answers follow the transforms the frame read. A point exactly on a line is decided by the half-open rules of the tile walk
  *    (tests/tile_walk_ref.py): deterministic, with no promise of the side.
  *  - BEGIN_CLIP / END_CLIP objects are never returned. Points outside the frame and NaN points give -1. Indices are the
  *    scene's draw-object indices (vb_scene_n_draw_objects / Scene.n_draw_objects; global in a batch: cell c's draws are
@@ -444,7 +444,7 @@ int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout
  * a raised window a move in z-order. With damage tracking (below) the next frame is then incremental, with the damage between
  * the composition the base frame rendered and the new one, when all of these hold:
  *  - tracking is on and there is a base frame, which rendered the scene being replaced: a composition, with no instance
- *    transforms, draw colours or path points bound, with no scene installation, binding, view, cell split or tracking switch since, and
+ *    transforms, draw colours, path points, gradient stops or transforms bound, with no scene installation, binding, view, cell split or tracking switch since, and
  *    hit tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - no other vb_recompose / vb_compose since that frame, and no vb_run_stages before the next one;
  *  - the next frame meets every condition of an incremental frame (size, AA, base colour, destination, one cell, no window).
@@ -605,6 +605,54 @@ int vb_bind_path_points(vb_renderer *, const float *device_xy, uint32_t n, size_
  * whose ramps and one per bound gradient would pass the 30 bits of the (ramp id << 2) | extend word, or whose regions past its
  * streams would pass 32-bit word offsets. */
 int vb_bind_gradient_stops(vb_renderer *, const float *device_stops, uint32_t n, size_t row_pitch_bytes);
+/* Bind the transform stream of the installed scene to device memory (an addition; no vello counterpart). Sprites, markers,
+ * map symbols or widgets a simulation or a layout model places on the GPU move, rotate and scale every frame without
+ * re-encoding or re-uploading the scene, and without a host call per frame. Unlike moving their points (vb_bind_path_points),
+ * a transform also scales and shears a stroke's width, joins and dashes, and it also places gradients and images (brush
+ * transforms, draw_image), clip layers and blurred rectangles:
+ *  - Rows. Row k is at device_affines + k * row_pitch_bytes and holds six f32 values [a b c d e f] in kurbo Affine order. Row k
+ *    is transform-stream entry k of the installed scene: global in instance order in a composed scene and in cell order in a
+ *    batch. vb_scene_n_transforms / Scene.n_transforms counts the entries, read before and after a call to learn the rows that
+ *    call produced. The encoders lay the entries out so:
+ *     - a call pushes its transform only when it differs from the last entry, so consecutive fills, strokes or layers with
+ *       equal transforms share one row, and moving that row moves all of them;
+ *     - a brush transform (fill / stroke with brush_transform) is an entry of its own after the shape's, holding the product
+ *       transform * brush_transform; the gradient or image is placed by it (it is pushed, like any entry, only when it differs
+ *       from the last one). A blurred rectangle likewise pushes transform * translate(centre of its rectangle) after its
+ *       shape's. draw_image is a fill with no brush transform: its one entry places both the rectangle and the image;
+ *     - a fill whose shape encodes nothing still pushes its transform (and no brush transform), and so does a push_*_layer
+ *       with a fill-style clip; a stroke of width 0 pushes nothing.
+ *  - What a frame renders. While rows are bound, every frame renders byte for byte what installing the same scene would render
+ *    after overwriting transform entry k with the f32 bits of row k, for every finite row k < n. The definition is at stream
+ *    level: binding never adds or drops transform tags, so rows that share an entry stay shared. Entries from n on keep their
+ *    values. Rows are copied as bits, never multiplied or converted.
+ *  - Non-finite rows. If any of a row's six values is NaN or +-inf, that entry keeps, for that frame, the value the frame would
+ *    read without this binding (the encoded transform, or the product of bound instance transforms).
+ *  - With bound instance transforms (vb_bind_instance_transforms) both bindings apply: a finite row k replaces the product
+ *    row_i * T that instance i's binding makes for entry k.
+ *  - Views. A view applies on top: a viewed frame renders V * row_k, the same f32 product vb_set_view applies to the scene's
+ *    own transforms. Culling to the frame stays tied to the view.
+ *  - Singular rows (a zero scale mid-animation) are legal: such a frame renders what the patched upload renders.
+ *  - Scenes. Every installation form can be bound, packed bytes included: a packed scene carries its transform stream.
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage, and a vb_run_stages
+ *    range that starts at draw reads them again. The caller orders its writes before the frame, on vb_stream or with a
+ *    synchronisation, and does not write the rows while a frame that reads them is running. A blocking frame that is re-run
+ *    after an arena overflow reads the same rows again; an enqueued frame is never re-run. The caller keeps the memory alive
+ *    while it is bound. Changing only the contents replays the captured frame graph, with no host call and no PCIe traffic.
+ *    Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next frame captures its graph
+ *    anew. With nothing bound a frame launches, configures and captures exactly what it would without this call.
+ *  - Scope. Every scene installation unbinds: every upload form, vb_render, vb_render_begin, vb_compose and vb_recompose. The
+ *    binding survives vb_set_view, vb_set_cells, the four other bindings and hit tests; all five can be active together.
+ *    device_affines NULL unbinds; frames then render the scene as encoded.
+ *  - The call finds each path's transform range once, with one kernel over the path tags, for damage tracking; it does not
+ *    synchronise. Hit tests and hit maps answer from the frame's geometry, so they follow the bound transforms, and damage
+ *    tracking follows the rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the scene's transform count; a pointer that is not device memory of the renderer's device (or managed
+ * memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 24, or 4 GiB or more; a renderer of a vb_group or
+ * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose transform, draw-data and
+ * path-data regions past its streams would pass 32-bit word offsets. */
+int vb_bind_transforms(vb_renderer *, const float *device_affines, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -637,6 +685,12 @@ int vb_bind_gradient_stops(vb_renderer *, const float *device_stops, uint32_t n,
  *  - Automatic damage, for bound gradient stops (vb_bind_gradient_stops). A bound gradient changed if its 512-texel ramp row
  *    differs byte for byte from the last successful frame's: rows that convert to the same texels are no change. The damage is
  *    the tiles of its draw object's clipped box in the last frame and in this one.
+ *  - Automatic damage, for bound transforms (vb_bind_transforms). Transform k changed if the six words the frame reads for it
+ *    (the bound region, or the viewed one under a view) differ bit for bit from the last successful frame's: a non-finite row
+ *    that falls back to an unchanged word is no change. Path p reads the transforms t_lo(p) .. t_hi(p): t_lo is the one in
+ *    effect at its first segment tag (its geometry's), t_hi the one at its end tag (where its brush is placed: a brush
+ *    transform, or the same one). When one of them changed, the damage is the tiles of the clipped box of draw object p in the
+ *    last frame and in this one. So moving one sprite of two neighbours damages only that sprite's old and new boxes.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
@@ -663,7 +717,7 @@ int vb_set_damage_tracking(vb_renderer *, int on);
  * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
  * all of these hold:
  *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound (no draw
- *    colours, path points or gradient stops bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
+ *    colours, path points, gradient stops or transforms bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
  *    tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
  *    frame full), and no vb_run_stages before the next one;

@@ -129,6 +129,11 @@ uint32_t vb_scene_n_points(const vb_scene *);
  * that call produced. Only a gradient that keeps a ramp adds stops (its stops after the brush alpha); a gradient with no stop
  * or one stop, and a degenerate radial or sweep gradient, is encoded as a colour and adds none. 0 for NULL. */
 uint32_t vb_scene_n_stops(const vb_scene *);
+/* The transform-stream entries encoded so far (an addition): the row vb_bind_transforms reads for the next entry a call pushes.
+ * Read it before and after a call to learn the rows that call produced. A call pushes its transform only when it differs from
+ * the last entry (so equal consecutive transforms share one row), a brush transform is an entry of its own holding transform *
+ * brush_transform, and a fill whose shape encodes nothing still pushes its transform. 0 for NULL. */
+uint32_t vb_scene_n_transforms(const vb_scene *);
 
 /* Scene::fill, scene.rs:316-345. brush_transform may be NULL. */
 int vb_scene_fill(vb_scene *, uint32_t fill_rule, const double transform[6], const vb_brush *, const double *brush_transform,

@@ -12,7 +12,10 @@
 //     data) differ bit for bit from the last successful frame's, the tile box of its draw object (path i is draw object i) in
 //     that frame and in this one. A changed clip path is covered by its BEGIN_CLIP's boxes, as a moved clip is below
 //   + for every bound gradient (vb_bind_gradient_stops) whose ramp row (the 512 texels fine reads) differs bit for bit from the
-//     last successful frame's, the tile box of its draw object in that frame and in this one.
+//     last successful frame's, the tile box of its draw object in that frame and in this one
+//   + with bound transforms (vb_bind_transforms), for every path one of whose transforms [t_lo, t_hi] (the binding's range: from
+//     the one in effect at its first segment to the one at its TAG_PATH, where draw reads its brush) differs bit for bit from
+//     the last successful frame's, the tile box of its draw object in that frame and in this one.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -58,11 +61,13 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
 // the instance holding u (the binding's prefix of the instances' transform counts). The same thread takes bound point u, when
 // there is one: its two words in the frame's path data (`pd`, the bound region), at `at_pt` of the slot (after the colour
 // words). A difference marks the path holding u (`first`, the binding's first point of each path). A non-finite row left the
-// encoded words in the region, so it is a change only if the words are.
+// encoded words in the region, so it is a change only if the words are. With bound transforms, xf_changed[u] records whether
+// transform u differs (a non-finite row that left an unchanged word does not).
 __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__restrict__ xf, uint32_t *snap, size_t slot_words, uint32_t n_xf,
                                                             uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed,
                                                             const uint32_t *__restrict__ pd, size_t at_pt, uint32_t n_pt,
-                                                            const uint32_t *__restrict__ first, uint32_t n_paths, uint32_t *paths) {
+                                                            const uint32_t *__restrict__ first, uint32_t n_paths, uint32_t *paths,
+                                                            uint32_t *xf_changed) {
     const uint32_t u = blockIdx.x * DM_THREADS + threadIdx.x;
     if (u >= n_xf && u >= n_pt) return;
     const uint32_t *old;
@@ -76,7 +81,8 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
             diff = diff || w != old[6u * u + i];
             nxt[6u * u + i] = w;
         }
-        if (compare && diff) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
+        if (compare && diff && n_inst) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
+        if (compare && xf_changed) xf_changed[u] = diff ? 1u : 0u;
     }
     if (u < n_pt) {
         const uint32_t x = __ldg(pd + 2u * u), y = __ldg(pd + 2u * u + 1u);
@@ -91,15 +97,18 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
 // One warp per draw object: its box, below n_col its colour word and, for a bound gradient (`grad`: the draw object's gradient
 // g or VB_COLOR_NONE, non-null with stops bound), its ramp row (`rows` + 512 g, at `at_rg` + 512 g of the slot) into the next
 // slot; when its instance (n_inst > 0), its colour word, its ramp row or its path's points (`paths`, non-null with points
-// bound) changed, its old and new boxes into the mask. A draw object whose paint is not one colour has colour word 0: its
-// bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data (`dd`, the bound region).
+// bound) or one of its path's transforms (`xf_range`, non-null with transforms bound: path d reads transforms xf_range[d].x ..
+// .y, each flagged in `xf_changed`) changed, its old and new boxes into the mask. A draw object whose paint is not one colour
+// has colour word 0: its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data
+// (`dd`, the bound region).
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
                                                        uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
                                                        const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht,
                                                        const uint32_t *__restrict__ draw_tags, const uint32_t *__restrict__ dd,
                                                        const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col,
                                                        const uint32_t *__restrict__ paths, uint32_t n_paths, const uint32_t *__restrict__ grad,
-                                                       const uint32_t *__restrict__ rows, size_t at_rg) {
+                                                       const uint32_t *__restrict__ rows, size_t at_rg, const uint2 *__restrict__ xf_range,
+                                                       const uint32_t *__restrict__ xf_changed) {
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (d >= n_draw) return;
     const uint32_t *old;
@@ -132,6 +141,13 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict
     if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
     if (!compare) return;
     if (!hit && paths && d < n_paths) hit = paths[d] != 0u; // path d is draw object d
+    if (!hit && xf_range && d < n_paths && n_xf) {
+        const uint2 t = xf_range[d];
+        const uint64_t hi = t.y < n_xf ? t.y : n_xf - 1u;
+        bool any = false;
+        for (uint64_t i = (uint64_t)t.x + lane; i <= hi; i += 32u) any = any || xf_changed[i] != 0u;
+        hit = __any_sync(0xffffffffu, any);
+    }
     if (!hit) {
         // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
         if (n_inst == 0u || d >= __ldg(inst_draw + n_inst)) return;
@@ -170,8 +186,9 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst,
                                                                               b.dmg_paths, n_paths);
-    // neither transforms, colours, points nor stops bound: nothing changes without a call that makes the frame full
-    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u) return 1u;
+    // neither instance transforms, colours, points, stops nor transforms bound: nothing changes without a call that makes the
+    // frame full
+    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u && b.xf_n == 0u) return 1u;
     const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n, at_rg = at_pt + 2u * (size_t)b.pt_n;
     const size_t slot_words = at_rg + 512u * (size_t)b.rs_grads_n;
     uint32_t launches = 1u;
@@ -180,7 +197,7 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
         k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
                                                                                       b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed,
                                                                                       b.scene + cfg.layout.path_data_base, at_pt, n_pt, b.pt_first,
-                                                                                      n_paths, b.dmg_paths);
+                                                                                      n_paths, b.dmg_paths, b.xf_rows ? b.dmg_xf : nullptr);
         launches++;
     }
     if (n_draw) {
@@ -188,8 +205,9 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
         k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
                                                                    n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
                                                                    b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n, b.dmg_paths,
-                                                                   n_paths, b.rs_grads_n ? b.rs_draw : nullptr,
-                                                                   b.ramps + 512u * (size_t)b.rs_ramp0, at_rg);
+                                                                   cfg.layout.n_paths, b.rs_grads_n ? b.rs_draw : nullptr,
+                                                                   b.ramps + 512u * (size_t)b.rs_ramp0, at_rg, b.xf_rows ? b.xf_range : nullptr,
+                                                                   b.dmg_xf);
         launches++;
     }
     return launches;

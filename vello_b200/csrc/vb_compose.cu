@@ -1,6 +1,7 @@
 // vb_compose.cu -- composition of resident fragments: vb_fragment_upload / vb_fragment_free, vb_compose and vb_recompose
 // (k_compose.cu, k_recompose.cu), bound instance transforms (vb_bind_instance_transforms), bound draw colours
-// (vb_bind_draw_colors, k_colors.cu) and bound path points (vb_bind_path_points, k_points.cu).
+// (vb_bind_draw_colors, k_colors.cu), bound path points (vb_bind_path_points, k_points.cu), bound gradient stops
+// (vb_bind_gradient_stops, k_resolve.cu) and bound transforms (vb_bind_transforms, k_transforms.cu).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
@@ -723,7 +724,7 @@ extern "C" int vb_bind_path_points(vb_renderer *r, const float *device_xy, uint3
     cudaStream_t st = r->stream;
     uint32_t *first = (uint32_t *)r->point_slots.p, *flag = first + L.n_paths + 1u;
     CK(cudaMemsetAsync(first, 0, ((size_t)L.n_paths + 2u) * 4u, st));
-    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, n_tag_words, L.n_paths, first, flag, st);
+    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, n_tag_words, L.n_paths, first, flag, nullptr, st);
     CK(cudaGetLastError());
     uint32_t i16 = 0u;
     CK(cudaMemcpyAsync(&i16, flag, 4u, cudaMemcpyDeviceToHost, st));
@@ -819,6 +820,56 @@ extern "C" int vb_bind_gradient_stops(vb_renderer *r, const float *device_stops,
     r->stops = nb;
     if ((rc = draw_data_slots(r, r->colors.rows ? r->colors.n : 0u))) return rc;
     CK(cudaStreamSynchronize(st)); // h is read by the copy
+    r->dmg.epoch++;
+    return VB_OK;
+}
+
+// ---- bound transforms: vb_bind_transforms (k_transforms.cu) ------------------------------------------------------------------
+// Each path's transform range, which damage tracking reads, is made once, here, on the renderer's stream by one
+// k_path_point_slots over the scene's path tags (the walk bound points use). It stays valid while the rows are bound, because
+// every scene installation unbinds. Every frame after that reads the caller's rows in its k_bound_transforms.
+extern "C" int vb_bind_transforms(vb_renderer *r, const float *device_affines, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_transforms: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_affines) {
+        r->xforms = vb_renderer::TransformBinding{};
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene) return bad("no scene installed");
+    const VbLayout &L = slot.layout;
+    const uint32_t n_tr = n_transforms(L, slot.scene_words);
+    if (n == 0u || n > n_tr)
+        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_tr) + " transforms (1 .. n_transforms)");
+    if ((uintptr_t)device_affines & 3u) return bad("the pointer must be 4-byte aligned");
+    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 24u || row_pitch_bytes > 0xfffffffcu)
+        return bad("the row pitch must be a multiple of 4 bytes, at least 24 and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_affines)) return bad("the rows must be memory of the renderer's device");
+    // a frame writes the bound region and, under a view, the viewed one past the scene, and bound draw data and path data after
+    // them (prepare, vb_frame.cu)
+    const uint64_t n_dd = draw_data_bound(r) ? n_draw_data(L, slot.scene_words) : 0u;
+    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
+    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd + n_pd > 0xfffffff0ull)
+        return bad("the scene with its bound and viewed transforms, draw data and path data exceeds 32-bit word offsets");
+    if (L.path_data_base < L.path_tag_base || L.path_data_base > slot.scene_words) return bad("the scene's path tags do not lie inside its words");
+    int rc;
+    if ((rc = compose_room(r, r->xform_ranges, (size_t)L.n_paths * 8u))) return rc;
+    cudaStream_t st = r->stream;
+    uint2 *range = (uint2 *)r->xform_ranges.p;
+    if (L.n_paths) CK(cudaMemsetAsync(range, 0xff, (size_t)L.n_paths * 8u, st));
+    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, L.path_data_base - L.path_tag_base, L.n_paths, nullptr,
+                               nullptr, range, st);
+    CK(cudaGetLastError());
+    r->xforms.rows = (const uint8_t *)device_affines;
+    r->xforms.n = n;
+    r->xforms.pitch = (uint32_t)row_pitch_bytes;
     r->dmg.epoch++;
     return VB_OK;
 }

@@ -401,10 +401,11 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
-    const uint32_t n_regions = (r->bound.rows ? 1u : 0u) + (r->view.on ? 1u : 0u);
-    if (r->bound.rows) {
-        // the frame reads its instances' transforms past the scene's streams: [transform_base, scene_words) is the region
-        // k_instance_transforms writes from the caller's rows
+    const bool bound_xf = r->bound.rows || r->xforms.rows;
+    const uint32_t n_regions = (bound_xf ? 1u : 0u) + (r->view.on ? 1u : 0u);
+    if (bound_xf) {
+        // the frame reads its transforms past the scene's streams: [transform_base, scene_words) is the region
+        // k_instance_transforms writes from the caller's instance rows and k_bound_transforms from the bound rows, after it
         c.layout.transform_base = c.scene_words;
         c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
     }
@@ -525,6 +526,13 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.pt_pitch = r->points.pitch;
         b.pt_src = b.scene + r->cur->layout.path_data_base;
     }
+    if (r->xforms.rows) {
+        b.xf_rows = r->xforms.rows;
+        b.xf_range = (const uint2 *)r->xform_ranges.p;
+        b.xf_n = r->xforms.n;
+        b.xf_pitch = r->xforms.pitch;
+        b.xf_src = b.scene + r->cur->layout.transform_base;
+    }
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
     b.lb_draw = b.ctl + o_draw;
@@ -614,11 +622,12 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_FLATTEN: {
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
-            // a frame with bound instance transforms or a view first writes its transforms (read by flatten and draw), the
-            // bound ones first (the view's source), a frame with bound colours or stops its draw data (read by draw, coarse
+            // a frame with bound instance transforms, bound transforms or a view first writes its transforms (read by flatten
+            // and draw), the bound ones first (instances, then rows: the view's source), a frame with bound colours or stops its draw data (read by draw, coarse
             // and fine) and with bound stops its gradients' ramp rows (read by fine), and a frame with bound points its path
             // data (read by flatten alone), inside flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
+            launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             launches += vb_launch_draw_colors(c, b, st);
             launches += vb_launch_bound_ramps(c, b, st);
@@ -647,6 +656,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // a range that starts here writes them again: the kernels only read the scene's own and the caller's rows, so the
             // words are the same
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_instance_transforms(c, b, st);
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_colors(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_ramps(c, b, st);

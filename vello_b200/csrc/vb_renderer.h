@@ -2,7 +2,7 @@
 //
 // The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
 // (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
-// instance transforms, draw colours, path points and gradient stops), vb_damage.cu (damage tracking), vb_debug.cu (debug
+// instance transforms, draw colours, path points, gradient stops and transforms), vb_damage.cu (damage tracking), vb_debug.cu (debug
 // downloads and uploads) and vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
 // namespace vb_host, hidden from the shared library's symbol table, so that a host program's own functions of the same names
 // cannot interpose on them.
@@ -343,6 +343,14 @@ struct vb_renderer {
         size_t o_stops = 0, o_dd = 0, o_draw = 0;
     } stops;
     DevBuf stop_tables, stop_ramps;
+    // bound transforms (vb_bind_transforms) of the current scene: the caller's rows (nullptr: unbound), and in xform_ranges each
+    // path's transform range {t_lo, t_hi} (layout.n_paths uint2, k_points.cu) for damage tracking. Every scene installation
+    // unbinds (set_scene).
+    struct TransformBinding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+    } xforms;
+    DevBuf xform_ranges;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -374,7 +382,7 @@ struct vb_renderer {
             size_t o_boxes = 0, o_tables = 0;
         } diff;
     } dmg;
-    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed, dmg_paths;
+    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed, dmg_paths, dmg_xf;
     DevBuf dmg_diff; // the diff's buffer: [the base frame's draw boxes, at o_boxes] [the tables, at o_tables] (VbFrameBufs::rcmp_*)
     // upload diff (vb_set_upload_diff): the switch; and the spare scene, ramps and atlas buffers an upload that tracking follows
     // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set. The diff's buffer is laid
@@ -399,8 +407,8 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
                            &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
-                           &r->stop_tables, &r->stop_ramps,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
+                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges,
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_xf, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
 }
@@ -470,7 +478,7 @@ inline uint32_t n_path_data(const VbLayout &L, size_t scene_words) {
 // Whether frames read their draw data from the region past the scene's streams: with bound colours or bound gradient stops.
 inline bool draw_data_bound(const vb_renderer *r) { return r->colors.rows || r->stops.rows; }
 // A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
-// transforms, k_compose.cu; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
+// transforms, k_compose.cu, or bound transforms, k_transforms.cu, one region for either or both; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
 // k_colors.cu) and with `points` a region of path data after those (bound path points, k_points.cu), then slack.
 inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions, bool colors = false, bool points = false) {
     return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words) + (colors ? n_draw_data(L, scene_words) : 0u) +

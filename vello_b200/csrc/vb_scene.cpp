@@ -1171,6 +1171,7 @@ void vb_scene_reset(vb_scene *s) {
 }
 uint32_t vb_scene_n_draw_objects(const vb_scene *s) { return s ? (uint32_t)s->e.draw_tags.size() : 0u; }
 uint32_t vb_scene_n_points(const vb_scene *s) { return s ? (uint32_t)(s->e.path_data.size() / 2u) : 0u; }
+uint32_t vb_scene_n_transforms(const vb_scene *s) { return s ? (uint32_t)s->e.transforms.size() : 0u; }
 uint32_t vb_scene_n_stops(const vb_scene *s) {
     size_t n = 0;
     if (s)

@@ -57,6 +57,12 @@ struct VbFrameBufs {
     // it) and the scene's own path data, the region's source. Null while unbound.
     const uint8_t *pt_rows;
     const uint32_t *pt_first, *pt_src;
+    // bound transforms (vb_bind_transforms), read by k_bound_transforms: the caller's rows (entry k's at xf_rows + k * xf_pitch
+    // bytes), the binding's range of transforms each path reads (layout.n_paths: {t_lo, t_hi}; k_damage) and the scene's own
+    // transforms, the bound region's source without bound instance transforms. Null while unbound.
+    const uint8_t *xf_rows;
+    const uint2 *xf_range;
+    const uint32_t *xf_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -83,10 +89,11 @@ struct VbFrameBufs {
     // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
     // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
     // of the frame's transform words, draw boxes, colour words of the col_n bound draw objects and words of the pt_n bound
-    // points), one changed flag per bound instance and, with points bound, one per path, and the composed scene's draw prefix
-    // (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k + 1]; null while unbound)
+    // points), one changed flag per bound instance, with points bound one per path and with transforms bound one per
+    // transform, and the composed scene's draw prefix (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k +
+    // 1]; null while unbound)
     uint8_t *dmg_mask, *dmg_pending;
-    uint32_t *dmg_snap, *dmg_changed, *dmg_paths;
+    uint32_t *dmg_snap, *dmg_changed, *dmg_paths, *dmg_xf;
     const uint32_t *inst_draw;
     // recompose damage (vb_recompose; k_recompose.cu), set only for the first frame after a recompose that tracking follows,
     // null otherwise: the base frame's draw boxes (rcmp_old_draws), and the tables [old draw prefix (rcmp_n_old + 1)] [new draw
@@ -105,6 +112,7 @@ struct VbFrameBufs {
     uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
     uint32_t col_n, col_pitch; // bound colour rows and their pitch in bytes; 0 while unbound
     uint32_t pt_n, pt_pitch;   // bound point rows and their pitch in bytes; 0 while unbound
+    uint32_t xf_n, xf_pitch;   // bound transform rows and their pitch in bytes; 0 while unbound
     uint32_t rs_n, rs_pitch;   // bound stop rows and their pitch in bytes; 0 while unbound
     uint32_t rs_grads_n, rs_ramp0; // bound gradients and the ramp row of the first; 0 while unbound
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
@@ -244,8 +252,17 @@ uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaSt
 // segment tag lacks the F32 bit. Per frame, in flatten's stage after the draw data (prepare reserved the region, vb_frame.cu):
 // the scene's path data into the frame's region at layout.path_data_base, the words of each bound point with a finite row
 // replaced by the row's bits; nothing while unbound.
-uint32_t vb_launch_path_point_slots(const uint32_t *tags, uint32_t n_words, uint32_t n_paths, uint32_t *first, uint32_t *i16, cudaStream_t st);
+// With xf_range (bound transforms; first and i16 may then be null), xf_range[p] = {t_lo, t_hi}: the transforms path p reads are
+// t_lo (in effect at its first segment tag) .. t_hi (at its TAG_PATH); the caller sets xf_range to all ones first.
+uint32_t vb_launch_path_point_slots(const uint32_t *tags, uint32_t n_words, uint32_t n_paths, uint32_t *first, uint32_t *i16, uint2 *xf_range,
+                                    cudaStream_t st);
 uint32_t vb_launch_path_points(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
+// k_transforms.cu: bound transforms (vb_bind_transforms). Per frame, in flatten's stage after the bound instance transforms and
+// before the view's (prepare reserved the region, vb_frame.cu): the bound region's entries below b.xf_n with a finite row get
+// the row's bits, the others the scene's own transforms, or keep the bound instance transforms' products; nothing while
+// unbound.
+uint32_t vb_launch_bound_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
 // the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame

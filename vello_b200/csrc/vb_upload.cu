@@ -61,8 +61,8 @@ void vb_host::drop_registrations(vb_renderer *r) {
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
-// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours, path points
-// or gradient stops are bound to it. Its stops are unknown until the installer that has them keeps them (keep_stops).
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours, path points,
+// gradient stops or transforms are bound to it. Its stops are unknown until the installer that has them keeps them (keep_stops).
 void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                       std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
     vb_renderer::SceneSlot &s = *r->cur;
@@ -87,6 +87,7 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     r->colors = vb_renderer::ColorBinding{};
     r->points = vb_renderer::PointBinding{};
     r->stops = vb_renderer::StopBinding{};
+    r->xforms = vb_renderer::TransformBinding{};
     r->dmg.epoch++;
     // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
     vb_renderer::Damage::Diff &X = r->dmg.diff;

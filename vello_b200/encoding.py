@@ -670,6 +670,16 @@ class Scene:
         or one stop, and a degenerate radial or sweep gradient, is encoded as a colour and adds none."""
         return sum(len(p["stops"]) for p in self.encoding.ramp_patches)
 
+    @property
+    def n_transforms(self) -> int:
+        """The transform-stream entries encoded so far: the row `Renderer.bind_transforms` reads for the next entry a call
+        pushes (read it before and after a call to learn the rows that call produced). A call pushes its transform only when it
+        differs from the last entry, so consecutive calls with equal transforms share one row. A brush transform is an entry of
+        its own, after the shape's, holding `transform * brush_transform`; a blurred rectangle pushes `transform *
+        translate(centre)` the same way, and `draw_image` pushes only its transform. A fill whose shape encodes nothing still
+        pushes its transform; a stroke of width 0 pushes nothing."""
+        return len(self.encoding.transforms)
+
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
         e = self.encoding
         e.encode_transform(transform)

@@ -177,6 +177,7 @@ def load_library() -> C.CDLL:
     lib.vb_bind_draw_colors.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_path_points.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_gradient_stops.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -198,7 +199,25 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
-                    "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops"]
+                    "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms"]
+
+
+def _device_rows(t, who: str, what: str, cols: int):
+    """(pointer, rows, row pitch in bytes) of an (n, cols) float32 device array bound by a `bind_*` method, from its
+    `__cuda_array_interface__` (a torch CUDA tensor, or columns of a larger one): columns 4 bytes apart and rows any multiple of
+    4 bytes, at least 4 * cols, apart. `who` names the method and `what` the rows in the errors."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device {what} are needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 2 or shape[0] == 0 or shape[1] != cols or cai["typestr"] != "<f4":
+        raise ValueError(f"{who}: {what} must be (n, {cols}) float32, not {shape} {cai['typestr']}")
+    strides = cai.get("strides") or (4 * cols, 4)
+    pitch = int(strides[0]) if shape[0] > 1 else 4 * cols  # the pitch of a single row is never used
+    if int(strides[1]) != 4 or pitch % 4 or pitch < 4 * cols:
+        raise ValueError(f"{who}: columns 4 bytes apart and rows a multiple of 4 bytes, at least {4 * cols}, apart; "
+                         f"not strides {tuple(strides)}")
+    return C.c_void_p(int(cai["data"][0])), shape[0], pitch
 
 
 def _device_image(t, typestr="|u1"):
@@ -308,6 +327,7 @@ class Renderer:
         self._colors = None  # the device array of bind_draw_colors
         self._points = None  # the device array of bind_path_points
         self._stops = None  # the device array of bind_gradient_stops
+        self._xforms = None  # the device array of bind_transforms
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
         self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
@@ -326,6 +346,7 @@ class Renderer:
         r._colors = None
         r._points = None
         r._stops = None
+        r._xforms = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -485,19 +506,8 @@ class Renderer:
             self._check(self.lib.vb_bind_instance_transforms(self.handle, None, 0, 0), "vb_bind_instance_transforms")
             self._bound = None
             return
-        cai = getattr(t, "__cuda_array_interface__", None)
-        if cai is None:
-            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device transforms are needed")
-        shape = tuple(int(v) for v in cai["shape"])
-        if len(shape) != 2 or shape[0] == 0 or shape[1] != 6 or cai["typestr"] != "<f4":
-            raise ValueError(f"bind_instance_transforms: transforms must be (n, 6) float32, not {shape} {cai['typestr']}")
-        strides = cai.get("strides") or (24, 4)
-        pitch = int(strides[0]) if shape[0] > 1 else 24  # the pitch of a single row is never used
-        if int(strides[1]) != 4 or pitch % 4 or pitch < 24:
-            raise ValueError(f"bind_instance_transforms: columns 4 bytes apart and rows a multiple of 4 bytes, at least 24, apart; "
-                             f"not strides {tuple(strides)}")
-        self._check(self.lib.vb_bind_instance_transforms(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
-                    "vb_bind_instance_transforms")
+        ptr, n, pitch = _device_rows(t, "bind_instance_transforms", "transforms", 6)
+        self._check(self.lib.vb_bind_instance_transforms(self.handle, ptr, n, pitch), "vb_bind_instance_transforms")
         self._bound = t
 
     def bind_draw_colors(self, t):
@@ -513,19 +523,8 @@ class Renderer:
             self._check(self.lib.vb_bind_draw_colors(self.handle, None, 0, 0), "vb_bind_draw_colors")
             self._colors = None
             return
-        cai = getattr(t, "__cuda_array_interface__", None)
-        if cai is None:
-            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device colours are needed")
-        shape = tuple(int(v) for v in cai["shape"])
-        if len(shape) != 2 or shape[0] == 0 or shape[1] != 4 or cai["typestr"] != "<f4":
-            raise ValueError(f"bind_draw_colors: colours must be (n, 4) float32, not {shape} {cai['typestr']}")
-        strides = cai.get("strides") or (16, 4)
-        pitch = int(strides[0]) if shape[0] > 1 else 16  # the pitch of a single row is never used
-        if int(strides[1]) != 4 or pitch % 4 or pitch < 16:
-            raise ValueError(f"bind_draw_colors: columns 4 bytes apart and rows a multiple of 4 bytes, at least 16, apart; "
-                             f"not strides {tuple(strides)}")
-        self._check(self.lib.vb_bind_draw_colors(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
-                    "vb_bind_draw_colors")
+        ptr, n, pitch = _device_rows(t, "bind_draw_colors", "colours", 4)
+        self._check(self.lib.vb_bind_draw_colors(self.handle, ptr, n, pitch), "vb_bind_draw_colors")
         self._colors = t
 
     def bind_path_points(self, t):
@@ -540,19 +539,8 @@ class Renderer:
             self._check(self.lib.vb_bind_path_points(self.handle, None, 0, 0), "vb_bind_path_points")
             self._points = None
             return
-        cai = getattr(t, "__cuda_array_interface__", None)
-        if cai is None:
-            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device points are needed")
-        shape = tuple(int(v) for v in cai["shape"])
-        if len(shape) != 2 or shape[0] == 0 or shape[1] != 2 or cai["typestr"] != "<f4":
-            raise ValueError(f"bind_path_points: points must be (n, 2) float32, not {shape} {cai['typestr']}")
-        strides = cai.get("strides") or (8, 4)
-        pitch = int(strides[0]) if shape[0] > 1 else 8  # the pitch of a single row is never used
-        if int(strides[1]) != 4 or pitch % 4 or pitch < 8:
-            raise ValueError(f"bind_path_points: columns 4 bytes apart and rows a multiple of 4 bytes, at least 8, apart; "
-                             f"not strides {tuple(strides)}")
-        self._check(self.lib.vb_bind_path_points(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
-                    "vb_bind_path_points")
+        ptr, n, pitch = _device_rows(t, "bind_path_points", "points", 2)
+        self._check(self.lib.vb_bind_path_points(self.handle, ptr, n, pitch), "vb_bind_path_points")
         self._points = t
 
     def bind_gradient_stops(self, t):
@@ -569,20 +557,28 @@ class Renderer:
             self._check(self.lib.vb_bind_gradient_stops(self.handle, None, 0, 0), "vb_bind_gradient_stops")
             self._stops = None
             return
-        cai = getattr(t, "__cuda_array_interface__", None)
-        if cai is None:
-            raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device stops are needed")
-        shape = tuple(int(v) for v in cai["shape"])
-        if len(shape) != 2 or shape[0] == 0 or shape[1] != 5 or cai["typestr"] != "<f4":
-            raise ValueError(f"bind_gradient_stops: stops must be (n, 5) float32, not {shape} {cai['typestr']}")
-        strides = cai.get("strides") or (20, 4)
-        pitch = int(strides[0]) if shape[0] > 1 else 20  # the pitch of a single row is never used
-        if int(strides[1]) != 4 or pitch % 4 or pitch < 20:
-            raise ValueError(f"bind_gradient_stops: columns 4 bytes apart and rows a multiple of 4 bytes, at least 20, apart; "
-                             f"not strides {tuple(strides)}")
-        self._check(self.lib.vb_bind_gradient_stops(self.handle, C.c_void_p(int(cai["data"][0])), shape[0], pitch),
-                    "vb_bind_gradient_stops")
+        ptr, n, pitch = _device_rows(t, "bind_gradient_stops", "stops", 5)
+        self._check(self.lib.vb_bind_gradient_stops(self.handle, ptr, n, pitch), "vb_bind_gradient_stops")
         self._stops = t
+
+    def bind_transforms(self, t):
+        """Take transform-stream entry k of the installed scene from row k of the device array `t` in every frame from now on,
+        read when the frame runs (`vb_bind_transforms`): `t` is float32 (n, 6) [a b c d e f] rows (kurbo Affine order), n at
+        most the scene's `Scene.n_transforms`, with `__cuda_array_interface__` (e.g. a torch CUDA tensor, or columns of a larger
+        one such as `state[:, 2:8]`). Row k is entry k of the transform stream (global in a composed scene or a batch): calls
+        with equal consecutive transforms share one entry, and a brush transform is an entry of its own holding `transform *
+        brush_transform`. Every frame renders what installing the scene with those entries overwritten would render; entries
+        from n on, and an entry whose row is not finite, keep the value the frame would read unbound. Bound instance transforms
+        and a view still apply (a view on top). Any installed scene can be bound, packed ones included. Write it on
+        `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. `t` is held
+        while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_transforms(self.handle, None, 0, 0), "vb_bind_transforms")
+            self._xforms = None
+            return
+        ptr, n, pitch = _device_rows(t, "bind_transforms", "transforms", 6)
+        self._check(self.lib.vb_bind_transforms(self.handle, ptr, n, pitch), "vb_bind_transforms")
+        self._xforms = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""

@@ -56,7 +56,7 @@ SCENE_SYMBOLS = ["vb_scene_new", "vb_scene_free", "vb_scene_reset", "vb_scene_fi
                  "vb_scene_push_luminance_mask_layer", "vb_scene_push_clip_layer", "vb_scene_pop_layer", "vb_scene_draw_image",
                  "vb_scene_draw_blurred_rounded_rect", "vb_scene_draw_blurred_rounded_rect_in", "vb_scene_append", "vb_scene_batch", "vb_scene_resolve", "vb_render_scene", "vb_scene_upload_device", "vb_path_dash",
                  "vb_register_texture", "vb_unregister_texture", "vb_scene_n_draw_objects", "vb_scene_upload_fragment",
-                 "vb_scene_n_points", "vb_scene_n_stops"]
+                 "vb_scene_n_points", "vb_scene_n_stops", "vb_scene_n_transforms"]
 
 _bound = False
 
@@ -75,6 +75,8 @@ def _lib():
         lib.vb_scene_n_points.argtypes = [vp]
         lib.vb_scene_n_stops.restype = C.c_uint32
         lib.vb_scene_n_stops.argtypes = [vp]
+        lib.vb_scene_n_transforms.restype = C.c_uint32
+        lib.vb_scene_n_transforms.argtypes = [vp]
         lib.vb_scene_fill.argtypes = [vp, C.c_uint32, vp, vp, vp, vp]
         lib.vb_scene_stroke.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.vb_scene_push_layer.argtypes = [vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_float, vp, vp]
@@ -216,6 +218,11 @@ class NativeScene:
     def n_stops(self) -> int:
         """`vb_scene_n_stops`: the gradient stops encoded so far, as `Scene.n_stops`."""
         return int(self.lib.vb_scene_n_stops(self.handle))
+
+    @property
+    def n_transforms(self) -> int:
+        """`vb_scene_n_transforms`: the transform-stream entries encoded so far, as `Scene.n_transforms`."""
+        return int(self.lib.vb_scene_n_transforms(self.handle))
 
     # -- vello::Scene surface ------------------------------------------------------------------------
     def fill(self, style: int, transform: Affine, brush, brush_transform: Optional[Affine], shape):
