@@ -256,6 +256,48 @@ typedef struct {
 int vb_register_destination(vb_renderer *, const vb_destination *, void **key_out);
 int vb_unregister_destination(vb_renderer *, void *key);
 
+/* ---- backgrounds: frames drawn over the pixels of a device buffer or a CUDA array (an addition) ----
+ * vello's render_to_texture starts every pixel at the base colour: the destination is overwritten, never drawn on. With a
+ * background set, every frame enqueued from then on starts pixel (x, y) at the background's value instead, and the base colour
+ * is ignored: 2-D content over a 3-D view or a video frame without a second image and a blend, annotations drawn over a batch
+ * of images, a cached static layer under a few moving objects. The descriptor is a vb_destination:
+ *  - LINEAR: pixel (x, y) at ptr + y * row_pitch_bytes + T * x (T as for destinations: 4, 8 or 16). With vb_set_cells and
+ *    n_cells > 1, cell c's pixel (x, y) at ptr + (c * height + y) * row_pitch_bytes + T * x, so an [N, H, W, 4] tensor works.
+ *    ARRAY: texel (background->x + x, background->y + y) of a 2-D CUDA array, read through a surface object.
+ *  - format: VB_DEST_RGBA8, VB_DEST_BGRA8, VB_DEST_RGBA16F or VB_DEST_RGBA32F, optionally OR'd with VB_DEST_PREMULTIPLIED.
+ *  - Like a destination, a background holds the whole frame: a bin_row / tile_row window or a read-back band reads its rows.
+ * The load, per pixel: each channel as f32 (byte / 255.0f for the 8-bit formats, with r and b swapped back for BGRA8; the half
+ * converted exactly; the float as stored), then clamp01 (fminf(1, fmaxf(0, v)), the store's clamp: NaN gives 0), then for
+ * straight alpha (r * a, g * a, b * a, a), each product rounded on its own; premultiplied values are taken as they are. The
+ * store, layers, blend modes and luminance masks are unchanged: the background is the bottom of the blend stack, as the base
+ * colour was. So:
+ *  - a premultiplied RGBA8 background filled with the base colour's bytes renders byte for byte the frame without one;
+ *  - a tile whose command list starts with an opaque cover of the whole tile does not read the background (fine skips the
+ *    load), and vb_set_occlusion_cull does not change the pixels;
+ *  - with an empty scene, a premultiplied background stored into a destination of the same format comes back bit for bit
+ *    (float texels: those already in [0, 1], with -0 read as +0); a straight texel with alpha 0 loses its colour.
+ * Scope: every single-renderer frame (vb_render_resident, vb_render_enqueue / vb_frame_finish, vb_render_uploaded, vb_render,
+ * vb_render_scene, vb_render_begin, whose destination is host memory, and vb_run_stages ranges that contain fine). The
+ * background may be the frame's destination itself (the same pointer or array): each pixel is read and then written by the
+ * same thread, and no other thread touches it. A background is renderer state, like a view: it survives uploads, compose,
+ * recompose, bindings and vb_set_cells. A frame keeps the background it was issued with, when it is re-run after an arena
+ * overflow and when vb_set_background is called while it is in flight. Whole-frame graphs are keyed by the descriptor, not
+ * the pixels: new contents replay the captured graph. A frame with a background is full under damage tracking and is no base
+ * for the next frame, which is full as well. Hit tests and hit maps answer from geometry and do not depend on it.
+ * NULL clears the background. VB_E_INVALID (vb_last_error says why):
+ *  - setting: everything vb_register_destination refuses for the same descriptor (an unknown kind, format or flag bit; a
+ *    renderer of a vb_group or with the exchange configured; LINEAR: ptr NULL, misaligned, a texture or destination key, or
+ *    not device or managed memory of the renderer's device; a bad row pitch; ARRAY: not a 2-D array, channels that do not
+ *    match the format, no cudaArraySurfaceLoadStore); vb_exchange_configure refuses a renderer with a background;
+ *  - a frame the background cannot cover: a row pitch below T * width, an array too small for the frame at its origin, an
+ *    array background with more than one cell.
+ * The caller keeps the memory or array alive and its pixels unchanged until the frames that read it have completed. A LINEAR
+ * background must hold every row of every cell a frame reads (the descriptor has no height to check it by). Clearing the
+ * background, or replacing an array background, returns once the frames that read the old array have completed (streamed
+ * frames included); the renderer's surface object is destroyed then. If completing them fails (a streamed frame's error is
+ * returned), the renderer is left without a background. */
+int vb_set_background(vb_renderer *, const vb_destination *background);
+
 /* cudaStream_t the renderer enqueues on (for event timing by the caller). Writes to an overridden image's device pixels
  * (vb_override_image) that are enqueued on this stream before the copying call are ordered before the copy. */
 void *vb_stream(vb_renderer *);

@@ -99,6 +99,10 @@ struct FineDstArgs : FineArgs {
     cudaSurfaceObject_t surf;
     uint32_t swz, array, x0, y0, texel, premul;
 };
+// The arguments of the FI_BG instantiations: FineDstArgs, then the background every tile starts from (vb_set_background).
+struct FineBgArgs : FineDstArgs {
+    VbFineBg bg;
+};
 
 // The store of a float destination (FI_DST, texel 8 or 16), for a lane's PX pixels at frame row gy, columns gx..gx+7 (gx a
 // multiple of 8). Each texel is clamp01 (unorm8's clamp, NaN to 0) of the premultiplied pixel, or of its straight colour
@@ -150,6 +154,92 @@ __device__ __forceinline__ void store_float(const FineDstArgs &A, const VbConfig
             if (A.array) surf2Dwrite(t[i], A.surf, (int)((x + i) * 8u), (int)y, cudaBoundaryModeZero);
             else reinterpret_cast<uint2 *>(row)[gx + i] = t[i];
         }
+    }
+}
+
+// The background's texels of a lane's PX pixels (FI_BG), frame row gy of cell `cell`, columns gx..gx+7, as stored: pixel i's in
+// w[i] (8-bit formats), w[2i..2i+1] (RGBA16F) or w[4i..4i+3] (RGBA32F). A pixel right of the frame reads nothing and stays 0.
+// Plain (coherent) loads, never the non-coherent path: the background may be the destination, which this kernel writes. A lane
+// reads its 8 pixels with 128-bit loads where the row is 16-byte aligned, or through the array's surface in 16-byte texel groups.
+__device__ __forceinline__ void load_bg_texels(const VbFineBg &B, const VbConfig &cfg, uint32_t cell, uint32_t gx, uint32_t gy,
+                                               uint32_t (&w)[4 * PX]) {
+#pragma unroll
+    for (int k = 0; k < 4 * PX; k++) w[k] = 0u;
+    const bool full = gx + 7u < cfg.target_width;
+    const uint32_t T = B.texel;
+    if (B.array) {
+        const uint32_t x = B.x0 + gx;
+        const int y = (int)(B.y0 + gy);
+        if (full && (x & (16u / T - 1u)) == 0u) {
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                if ((uint32_t)k * 16u >= PX * T) break;
+                const uint4 v = surf2Dread<uint4>(B.surf, (int)(x * T + (uint32_t)k * 16u), y, cudaBoundaryModeZero);
+                w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < PX; i++) {
+                if (gx + i >= cfg.target_width) continue;
+                const int bx = (int)((x + i) * T);
+                if (T == 16u) {
+                    const uint4 v = surf2Dread<uint4>(B.surf, bx, y, cudaBoundaryModeZero);
+                    w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
+                } else if (T == 8u) {
+                    const uint2 v = surf2Dread<uint2>(B.surf, bx, y, cudaBoundaryModeZero);
+                    w[2 * i] = v.x; w[2 * i + 1] = v.y;
+                } else {
+                    w[i] = surf2Dread<uint32_t>(B.surf, bx, y, cudaBoundaryModeZero);
+                }
+            }
+        }
+        return;
+    }
+    const uint8_t *row = B.ptr + ((size_t)cell * cfg.target_height + gy) * B.pitch + (size_t)gx * T;
+    if (full && ((uintptr_t)row & 15u) == 0u) {
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            if ((uint32_t)k * 16u >= PX * T) break;
+            const uint4 v = __ldcg(reinterpret_cast<const uint4 *>(row) + k);
+            w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < PX; i++) {
+            if (gx + i >= cfg.target_width) continue;
+            if (T == 16u) {
+                const uint4 v = __ldcg(reinterpret_cast<const uint4 *>(row) + i);
+                w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
+            } else if (T == 8u) {
+                const uint2 v = __ldcg(reinterpret_cast<const uint2 *>(row) + i);
+                w[2 * i] = v.x; w[2 * i + 1] = v.y;
+            } else {
+                w[i] = __ldcg(reinterpret_cast<const unsigned int *>(row) + i);
+            }
+        }
+    }
+}
+// The background's pixels as fine's starting pixels: each channel as f32 (byte / 255.0f with r and b swapped back for BGRA8, the
+// half converted exactly, the float as stored), clamp01 of it (the store's clamp: NaN gives 0, and nothing outside [0, 1] enters
+// the blend arithmetic), then for straight alpha (r * a, g * a, b * a, a), each product rounded on its own.
+__device__ __forceinline__ void load_bg(const VbFineBg &B, const VbConfig &cfg, uint32_t cell, uint32_t gx, uint32_t gy, rgba_t (&rgba)[PX]) {
+    uint32_t w[4 * PX];
+    load_bg_texels(B, cfg, cell, gx, gy, w);
+#pragma unroll
+    for (int i = 0; i < PX; i++) {
+        rgba_t c;
+        if (B.texel == 16u) {
+            c = RG(__uint_as_float(w[4 * i]), __uint_as_float(w[4 * i + 1]), __uint_as_float(w[4 * i + 2]), __uint_as_float(w[4 * i + 3]));
+        } else if (B.texel == 8u) {
+            c = RG(__half2float(__ushort_as_half((unsigned short)(w[2 * i] & 0xffffu))), __half2float(__ushort_as_half((unsigned short)(w[2 * i] >> 16))),
+                   __half2float(__ushort_as_half((unsigned short)(w[2 * i + 1] & 0xffffu))),
+                   __half2float(__ushort_as_half((unsigned short)(w[2 * i + 1] >> 16))));
+        } else {
+            c = unpack4x8unorm(w[i]);
+            if (B.bgra) c = RG(c.b, c.g, c.r, c.a);
+        }
+        c = RG(clamp01(c.r), clamp01(c.g), clamp01(c.b), clamp01(c.a));
+        rgba[i] = B.premul ? c : RG(c.r * c.a, c.g * c.a, c.b * c.a, c.a);
     }
 }
 
@@ -836,16 +926,23 @@ static_assert(sizeof(WarpIo) % 16 == 0 && sizeof(WarpMs<1>) % 16 == 0 && sizeof(
 // MODE: the AA mode (0 area, 1 MSAA8, 2 MSAA16), plus FI_DMG for damage tracking (k_damage.cu): coarse listed only the
 // damaged tiles, and those lists are the whole queue, so no other pixel is written. Without FI_DMG the kernel is the one it was
 // before damage tracking existed. FI_DST: a registered destination (vb_register_destination) in BGRA8 order, with premultiplied
-// alpha, in a float format or in a CUDA array; only the store differs.
+// alpha, in a float format or in a CUDA array; only the store differs. FI_BG (always with FI_DST, never with FI_DMG): every tile
+// starts from a background's pixels (vb_set_background) instead of the base colour. These three instantiations are compiled
+// into k_fine_bg.o (VB_FINE_BG), so that k_fine.o holds exactly the others.
 #define FI_DMG 16
 #define FI_DST 32
-template <int MODE> using FineArgsOf = typename std::conditional<(MODE & FI_DST) != 0, FineDstArgs, FineArgs>::type;
+#define FI_BG 64
+template <int MODE>
+using FineArgsOf = typename std::conditional<(MODE & FI_BG) != 0, FineBgArgs,
+                                             typename std::conditional<(MODE & FI_DST) != 0, FineDstArgs, FineArgs>::type>::type;
 template <int MODE>
 __global__ void __launch_bounds__(FI_MAX_THREADS, FI_MINB)
 k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
     constexpr int AA = MODE & 15;
     constexpr bool DMG = (MODE & FI_DMG) != 0;
     constexpr bool DST = (MODE & FI_DST) != 0;
+    constexpr bool BG = (MODE & FI_BG) != 0;
+    static_assert(!BG || (DST && !DMG), "FI_BG goes with FI_DST and without FI_DMG");
     extern __shared__ __align__(16) unsigned char smem[];
     typedef WarpMs<AA == 0 ? 1 : AA> Ms;
     const uint32_t *__restrict__ ptcl = A.ptcl;
@@ -957,6 +1054,12 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
             const rgba_t base = unpack4x8unorm_uniform(cfg.base_color);
 #pragma unroll
             for (int i = 0; i < PX; i++) { rgba[i] = base; area[i] = 0.0f; }
+        }
+        // FI_BG: the tile starts from the background's pixels, loaded before the wait for the command window. A tile that
+        // starts at its occlusion start skips them: its first commands paint every pixel opaque, and over(bg, fg) =
+        // fmaf(bg, 0, fg) = fg for any finite bg.
+        if constexpr (BG) {
+            if (gy < cfg.target_height && start_cur == tile_ix * VB_PTCL_INITIAL_ALLOC + 1u) load_bg(A.bg, cfg, cell, gx, gy, rgba);
         }
         // first BLEND_STACK_SPLIT levels of the blend stack: thread-private (local memory, L1 resident); deeper
         // levels spill to blend_spill exactly as in the reference
@@ -1336,35 +1439,56 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
 #undef START_OF
 }
 
+typedef cudaError_t (*FineInit)();
 template <int MODE> static cudaError_t fine_smem_limit() {
     return cudaFuncSetAttribute(k_fine<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<MODE & 15>::bytes(FI_MAX_WARPS));
 }
-extern "C" int vb_fine_init_constants(void) {
+// c_unorm of this object (k_fine.o and k_fine_bg.o each have their own), and the shared-memory limits of the kernels in `set`
+static cudaError_t fine_init(const FineInit *set, int n) {
     float h[256];
     for (int i = 0; i < 256; i++) h[i] = (float)i / 255.0f;
     cudaError_t e = cudaMemcpyToSymbol(c_unorm, h, sizeof h);
     // the kernels use more than the default 48 KB of dynamic shared memory per CTA
-    const decltype(&fine_smem_limit<0>) set[] = {
-        fine_smem_limit<0>, fine_smem_limit<0 + FI_DMG>, fine_smem_limit<0 + FI_DST>, fine_smem_limit<0 + FI_DST + FI_DMG>,
-        fine_smem_limit<1>, fine_smem_limit<1 + FI_DMG>, fine_smem_limit<1 + FI_DST>, fine_smem_limit<1 + FI_DST + FI_DMG>,
-        fine_smem_limit<2>, fine_smem_limit<2 + FI_DMG>, fine_smem_limit<2 + FI_DST>, fine_smem_limit<2 + FI_DST + FI_DMG>};
-    for (auto f : set)
-        if (e == cudaSuccess) e = f();
-    return (int)e;
+    for (int k = 0; k < n; k++)
+        if (e == cudaSuccess) e = set[k]();
+    return e;
 }
 
-// k_fine<aa + FLAGS>, with FineArgs alone unless FLAGS has FI_DST
-template <int FLAGS> static void launch_fine(int aa, uint32_t grid, uint32_t warps, cudaStream_t st, const VbConfig &cfg, const FineDstArgs &A) {
+// k_fine<aa + FLAGS>, with FineArgs alone unless FLAGS has FI_DST, and FineDstArgs unless it has FI_BG
+template <int FLAGS> static void launch_fine(int aa, uint32_t grid, uint32_t warps, cudaStream_t st, const VbConfig &cfg, const FineBgArgs &A) {
     const FineArgsOf<FLAGS> &a = A;
     if (aa == 0) k_fine<0 + FLAGS><<<grid, 32u * warps, FineSmem<0>::bytes(warps), st>>>(cfg, a);
     else if (aa == 1) k_fine<1 + FLAGS><<<grid, 32u * warps, FineSmem<1>::bytes(warps), st>>>(cfg, a);
     else k_fine<2 + FLAGS><<<grid, 32u * warps, FineSmem<2>::bytes(warps), st>>>(cfg, a);
 }
 
+#ifdef VB_FINE_BG
+// k_fine_bg.o: the FI_BG instantiations, launched by vb_launch_fine
+extern "C" int vb_fine_bg_init(void) {
+    const FineInit set[] = {fine_smem_limit<0 + FI_DST + FI_BG>, fine_smem_limit<1 + FI_DST + FI_BG>,
+                                                 fine_smem_limit<2 + FI_DST + FI_BG>};
+    return (int)fine_init(set, 3);
+}
+extern "C" void vb_launch_fine_bg(int aa, uint32_t grid, uint32_t warps, cudaStream_t st, const VbConfig &cfg, const FineBgArgs &A) {
+    launch_fine<FI_DST + FI_BG>(aa, grid, warps, st, cfg, A);
+}
+#else
+extern "C" int vb_fine_bg_init(void);
+extern "C" void vb_launch_fine_bg(int aa, uint32_t grid, uint32_t warps, cudaStream_t st, const VbConfig &cfg, const FineBgArgs &A);
+
+extern "C" int vb_fine_init_constants(void) {
+    const FineInit set[] = {
+        fine_smem_limit<0>, fine_smem_limit<0 + FI_DMG>, fine_smem_limit<0 + FI_DST>, fine_smem_limit<0 + FI_DST + FI_DMG>,
+        fine_smem_limit<1>, fine_smem_limit<1 + FI_DMG>, fine_smem_limit<1 + FI_DST>, fine_smem_limit<1 + FI_DST + FI_DMG>,
+        fine_smem_limit<2>, fine_smem_limit<2 + FI_DMG>, fine_smem_limit<2 + FI_DST>, fine_smem_limit<2 + FI_DST + FI_DMG>};
+    const cudaError_t e = fine_init(set, 12);
+    return e != cudaSuccess ? (int)e : vb_fine_bg_init();
+}
+
 // The launch's tile queue is control-block word VB_CTL_FINE_QUEUE + band, zeroed with the control block (8 of them, one per
 // read-back band).
-extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, int aa, uint32_t cull, uint32_t band,
-                                   bool cls_order, cudaStream_t st) {
+extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, const VbFineBg &bg, int aa, uint32_t cull,
+                                   uint32_t band, bool cls_order, cudaStream_t st) {
     uint32_t rows = cfg.win_ty1 - cfg.win_ty0;
     uint32_t n = cfg.width_in_tiles * rows;
     if (n == 0) return 0;
@@ -1375,7 +1499,7 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     uint32_t grid = (n + warps - 1u) / warps;
     const uint32_t resident = (uint32_t)sm_count * FI_MINB * (FI_MAX_WARPS / warps);
     if (grid > resident) grid = resident;
-    FineDstArgs A;
+    FineBgArgs A;
     A.segments = b.segments; A.ptcl = b.ptcl; A.info = b.info_bin_data; A.blend_spill = b.blend_spill; A.out = o.out; A.ramps = b.ramps; A.atlas = b.atlas;
     A.mask_lut = aa == 2 ? b.mask16 : b.mask8;
     A.cull = cull;
@@ -1392,8 +1516,17 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     A.y0 = o.y0;
     A.texel = o.texel;
     A.premul = o.premul;
+    A.bg = bg;
     const bool dmg = b.dmg_mode == VB_DMG_INCREMENTAL && cls_order; // the damaged tiles of coarse's lists only
-    if (o.dst) {
+    if (bg.on) {
+        // always the FI_DST store (a plain pointer as linear RGBA8, straight alpha, bytes in place), never FI_DMG: a frame with a
+        // background is full (damage_prepare)
+        if (!o.dst) {
+            A.swz = 0x3210u;
+            A.texel = 4u;
+        }
+        vb_launch_fine_bg(aa, grid, warps, st, cfg, A);
+    } else if (o.dst) {
         if (dmg) launch_fine<FI_DST + FI_DMG>(aa, grid, warps, st, cfg, A);
         else launch_fine<FI_DST>(aa, grid, warps, st, cfg, A);
     } else {
@@ -1402,3 +1535,4 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     }
     return 1;
 }
+#endif

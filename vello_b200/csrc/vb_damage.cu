@@ -7,8 +7,9 @@
 #include "vb_renderer.h"
 
 // ---- damage tracking: vb_set_damage_tracking / vb_add_damage / vb_last_damage (k_damage.cu) -------------------------------
-// After prepare and pick_out: is the frame incremental, full, or outside damage tracking (a batch, a window, the exchange:
-// mode VB_DMG_OFF, and no base for the next frame)? The decision is the same for every re-run of the frame, because the base
+// After prepare, pick_out and resolve_background: is the frame incremental, full, or outside damage tracking (a batch, a window,
+// a background, the exchange: mode VB_DMG_OFF, and no base for the next frame)? A background frame is full because nothing tells
+// which of the background's pixels changed since the base frame. The decision is the same for every re-run of the frame, because the base
 // and the forcing flags change only when a frame succeeds (damage_succeeded). Allocates the mask, the staged rectangles and
 // the snapshot; their sizes follow from the frame size and the scene, so they never move under an incremental frame.
 int vb_host::damage_prepare(vb_renderer *r) {
@@ -22,7 +23,7 @@ int vb_host::damage_prepare(vb_renderer *r) {
     f.dest = r->dest.dev;
     f.epoch = D.epoch;
     const bool windowed = r->params.bin_row1 > r->params.bin_row0 || r->params.tile_row1 > r->params.tile_row0;
-    f.can_base = D.on && c.n_cells == 1u && !windowed && !r->xc.enabled && !r->grouped;
+    f.can_base = D.on && c.n_cells == 1u && !windowed && !r->dest.bg.on && !r->xc.enabled && !r->grouped;
     D.frame = f;
     if (!f.can_base) return VB_OK;
     // an overridden image copied again changes pixels nothing here can locate: the frame is full unless the caller named them

@@ -264,6 +264,7 @@ extern "C" void vb_renderer_free(vb_renderer *r) {
         cudaEventDestroy(f.done);
     }
     drop_registrations(r);
+    if (r->bg.d.surf) cudaDestroySurfaceObject(r->bg.d.surf);
     for (auto &gs : r->graphs)
         if (gs.exec) cudaGraphExecDestroy(gs.exec);
     for_each_handle(
@@ -701,7 +702,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             for (uint32_t band = 0; band < f.bands; band++) {
                 VbConfig cb = c;
                 if (!f.band(band, &cb.win_ty0, &cb.win_ty1)) break;
-                launches += vb_launch_fine(cb, b, d.out, (int)r->params.aa, r->occlusion_cull, band, f.bands == 1u, st);
+                launches += vb_launch_fine(cb, b, d.out, d.bg, (int)r->params.aa, r->occlusion_cull, band, f.bands == 1u, st);
                 if (d.host && (rc = queue_readback(r, c, f, band, d))) return rc;
             }
             break;
@@ -725,11 +726,12 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
 // the launches of a frame are identical -- same kernels, grids, arena pointers, config -- so they are captured once into a
 // graph and replayed with ONE submission. The key is the inputs of the launches; growing an arena or changing the scene
 // layout / frame size / window simply misses the cache and re-captures.
-static void graph_key(vb_renderer *r, int last, const void *out_dev, GraphKey *k) {
+static void graph_key(vb_renderer *r, int last, const Dest &d, GraphKey *k) {
     memset(k, 0, sizeof *k);
     k->cfg = r->cfg;
     memcpy(&k->bufs, &r->bufs, sizeof k->bufs);
-    k->out = out_dev;
+    k->bg = d.bg;
+    k->out = d.dev;
     k->h_bump_dev = r->cur->h_bump_dev;
     k->aa = r->params.aa;
     k->cull = r->occlusion_cull;
@@ -748,7 +750,7 @@ static int enqueue(vb_renderer *r, int first, int last, const Dest &d, bool clea
     const bool banded = f.bands > 1u;
     const int g_last = banded ? VB_STAGE_ID_FINE - 1 : last;
     GraphKey key;
-    graph_key(r, g_last, d.dev, &key);
+    graph_key(r, g_last, d, &key);
     GraphSlot *slot = nullptr;
     for (GraphSlot &gs : r->graphs)
         if (gs.exec && memcmp(&gs.key, &key, sizeof key) == 0) slot = &gs;
@@ -820,14 +822,14 @@ static int pick_out(vb_renderer *r, Dest *d) {
 // arenas, the output target), then the launches. vb_group runs step 1 for ALL its renderers before step 2 of any: with the
 // exchange on, a renderer's frame contains a kernel that waits for its peers, and a peer that shares the device (tests)
 // must not be stuck in a cudaFree behind that kernel.
-int vb_host::frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d) {
-    if (!r || !p) return VB_E_INVALID;
+int vb_host::frame_prepare(vb_renderer *r, const Frame &f) {
+    if (!r) return VB_E_INVALID;
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
     CK(cudaSetDevice(r->device));
-    int rc = prepare(r, p);
+    int rc = prepare(r, &f.params);
     if (rc) return rc;
-    r->dest = d;
-    if ((rc = pick_out(r, &r->dest))) return rc;
+    r->dest = f.dest;
+    if ((rc = pick_out(r, &r->dest)) || (rc = resolve_background(r, f.bg, &r->dest))) return rc;
     return damage_prepare(r);
 }
 // Enqueue stages first..last of the frame frame_prepare set up. A range from stage 0 starts the frame: the dirty overridden
@@ -853,9 +855,9 @@ int vb_host::launch(vb_renderer *r, int first, int last) {
     return rc;
 }
 
-// A frame of the renderer's current scene slot, under its current view.
+// A frame of the renderer's current scene slot, under its current view and over its current background.
 Frame vb_host::frame_of(const vb_renderer *r, const vb_params *p, const Dest &d) {
-    return Frame{*p, d, r->view, (uint32_t)(r->cur - r->slot)};
+    return Frame{*p, d, r->view, r->bg, (uint32_t)(r->cur - r->slot)};
 }
 
 static bool same_view(const View &a, const View &b) { return a.on == b.on && (!a.on || memcmp(a.m, b.m, sizeof a.m) == 0); }
@@ -866,7 +868,7 @@ static int issue(vb_renderer *r, const Frame &f) {
     const bool other = !same_view(now, f.view);
     r->cur = &r->slot[f.slot];
     int rc = other ? put_view(r, f.view) : VB_OK;
-    if (rc == VB_OK) rc = frame_prepare(r, &f.params, f.dest);
+    if (rc == VB_OK) rc = frame_prepare(r, f);
     if (rc == VB_OK) rc = launch(r, 0, VB_N_STAGE_IDS - 1);
     if (other) {
         const int rc2 = put_view(r, now);
@@ -1116,6 +1118,7 @@ extern "C" int vb_run_stages(vb_renderer *r, const vb_params *p, int first, int 
     if (rc) return rc;
     Dest d{out_device};
     if ((last == VB_STAGE_ID_FINE || vb_texture_key(d.dev)) && (rc = pick_out(r, &d))) return rc;
+    if (last == VB_STAGE_ID_FINE && (rc = resolve_background(r, r->bg, &d))) return rc;
     if ((rc = enqueue(r, first, last, d, true))) return rc;
     CK(cudaStreamSynchronize(r->stream));
     return VB_OK;

@@ -334,7 +334,7 @@ static int group_render(vb_group *g, const vb_params *p, void *out_device, void 
                 if (g->bounds[i + 1] <= g->bounds[i]) continue; // more devices than tile rows (never with the exchange on)
                 const size_t row0 = (size_t)g->bounds[i] * 16u;
                 int rc = VB_OK;
-                if (phase == 0) rc = frame_prepare(r, &fs[i].params, fs[i].dest);
+                if (phase == 0) rc = frame_prepare(r, fs[i]);
                 else if (phase <= n_launch)
                     rc = launch(r, phase == 2 ? VB_STAGE_ID_DRAW : 0, halves && phase == 1 ? VB_STAGE_ID_FLATTEN : VB_N_STAGE_IDS - 1);
                 else {
@@ -410,6 +410,10 @@ extern "C" int vb_group_render(vb_group *g, const uint8_t *scene, size_t scene_l
 extern "C" int vb_exchange_configure(vb_renderer *r, uint32_t rank, uint32_t world, void **arena, size_t *arena_bytes) {
     if (!r || world < 1u || world > 8u || rank >= world) return VB_E_INVALID;
     if (!r->cur->have_scene) return VB_E_NO_SCENE;
+    if (r->bg.on) {
+        r->err = "vb_exchange_configure: not available for a renderer with a background (vb_set_background)";
+        return VB_E_INVALID;
+    }
     CK(cudaSetDevice(r->device));
     CK(cudaStreamSynchronize(r->stream));
     vb_renderer::Exchange &x = r->xc;

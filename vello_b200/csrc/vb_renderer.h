@@ -69,6 +69,7 @@ struct Dest {
     bool alt = false;
     uint32_t bands = 1;
     VbFineOut out{};
+    VbFineBg bg{}; // what fine's tiles start from: the frame's background, set for each attempt by resolve_background
 };
 
 // A registered destination (vb_register_destination), found by its key in vb_renderer::dests. LINEAR: pixel (x, y) of a frame
@@ -84,11 +85,18 @@ struct Destination {
     uint32_t x0 = 0, y0 = 0;
     size_t w = 0, h = 0;
 };
+// A background (vb_set_background): the pixels every frame enqueued while it is set starts from, described and checked as a
+// registered destination is (destination_of). Pixel (x, y) of cell c of a LINEAR one at ptr + (c * height + y) * pitch + T * x.
+struct Background {
+    bool on = false;
+    Destination d;
+};
 
 // key of a captured frame: the inputs of its launches (see enqueue)
 struct GraphKey {
     VbConfig cfg;
     VbFrameBufs bufs;
+    VbFineBg bg; // the background's descriptor; its pixels are read at replay
     const void *out;
     const VbBump *h_bump_dev;
     uint32_t aa, cull, last;
@@ -108,12 +116,13 @@ struct View {
     float m[6] = {};
 };
 
-// Everything a frame needs to be issued again (issue): a re-run renders under the view and from the scene slot the frame
-// was first issued with, even if the renderer's have changed since.
+// Everything a frame needs to be issued again (issue): a re-run renders under the view, over the background and from the scene
+// slot the frame was first issued with, even if the renderer's have changed since.
 struct Frame {
     vb_params params{};
     Dest dest;
     View view;
+    Background bg;
     uint32_t slot = 0;
 };
 
@@ -249,6 +258,7 @@ struct vb_renderer {
     // the view of the frames enqueued from now on; its coefficients reach view_coef in stream order (put_view)
     View view;
     DevBuf view_coef;
+    Background bg; // of the frames enqueued from now on (vb_set_background); an array's surface object is the renderer's
     uint32_t readback_bands = 8; // fine launches per frame when the pixels go to the host (vb_render); 1 while streaming
     uint32_t occlusion_cull = 1; // fine starts each tile at its last opaque full-tile cover
     // path_tiling runs on its own stream beside coarse: forked after backdrop, joined before fine (enqueue_direct). Earlier in
@@ -500,7 +510,7 @@ int ensure_arena(vb_renderer *r, int a);
 uint32_t grow(uint32_t need);
 int drain_stream(vb_renderer *r);
 FineRows fine_rows(const VbConfig &c, const Dest &d);
-int frame_prepare(vb_renderer *r, const vb_params *p, const Dest &d);
+int frame_prepare(vb_renderer *r, const Frame &f);
 int launch(vb_renderer *r, int first, int last);
 Frame frame_of(const vb_renderer *r, const vb_params *p, const Dest &d);
 int finish(vb_renderer *r, const Frame &f);
@@ -513,6 +523,11 @@ int view_of(const double *affine, View *v);
 void drop_registrations(vb_renderer *r);
 // a registered destination's key: where fine stores (d->out), after the frame-time checks
 int resolve_destination(vb_renderer *r, Dest *d);
+// The checks vb_register_destination and vb_set_background make of a descriptor (`who` names the call in vb_last_error), and the
+// Destination it describes, with a new surface object for an array.
+int destination_of(vb_renderer *r, const vb_destination *d, const char *who, Destination *out);
+// what fine's tiles start from in the frame r prepared (d->bg): the background bg, after the frame-time checks, or the base colour
+int resolve_background(vb_renderer *r, const Background &bg, Dest *d);
 void set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed);
 // diff: the upload may be diffed against the base frame's scene (vb_set_upload_diff); not for streamed frames

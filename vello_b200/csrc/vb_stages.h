@@ -181,10 +181,20 @@ struct VbFineOut {
     cudaSurfaceObject_t surf;
     uint32_t dst, swz, array, x0, y0, texel, premul;
 };
-// tile rows cfg.win_ty0..win_ty1 into `o`; `band` picks the launch's tile queue (one of 8 control-block words) and
-// cls_order starts the tiles in coarse's cost order
-uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, int aa, uint32_t cull, uint32_t band,
-                        bool cls_order, cudaStream_t st);
+// What fine's tiles start from with `on` (vb_set_background; the FI_BG instantiations), instead of the base colour: texels of
+// `texel` bytes (as VbFineOut's), straight or, with `premul`, premultiplied, r and b swapped with `bgra`. Linear: pixel (x, y) of
+// cell c at ptr + (c * target_height + y) * pitch + texel * x. With `array`, through `surf`, pixel (x, y) at texel (x0 + x, y0 + y).
+// No padding: it is part of the graph key.
+struct VbFineBg {
+    const uint8_t *ptr;
+    cudaSurfaceObject_t surf;
+    unsigned long long pitch; // bytes
+    uint32_t on, array, x0, y0, texel, premul, bgra, pad;
+};
+// tile rows cfg.win_ty0..win_ty1 into `o`, over `bg` when bg.on; `band` picks the launch's tile queue (one of 8 control-block
+// words) and cls_order starts the tiles in coarse's cost order
+uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, const VbFineBg &bg, int aa, uint32_t cull,
+                        uint32_t band, bool cls_order, cudaStream_t st);
 int vb_fine_init_constants(void);
 
 // multi-GPU exchange: send = everything up to raising my flags, recv = wait for the peers, combine the boxes, pull my lines

@@ -342,13 +342,11 @@ extern "C" int vb_texture_unregister(vb_renderer *r, const void *key) {
 // Frames into a destination's key store through k_fine's FI_DST instantiations, except linear RGBA8 with straight alpha, which
 // is the default store at another pitch and origin. Every check is made here or in resolve_destination, on the host, before a
 // frame is enqueued. The texel size (Destination::texel) sets the alignment, pitch and channel checks and fine's store.
-extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, void **key_out) {
-    if (!r) return VB_E_INVALID;
+int vb_host::destination_of(vb_renderer *r, const vb_destination *d, const char *who, Destination *out) {
     auto bad = [&](const std::string &why) {
-        r->err = std::string("vb_register_destination: ") + why;
+        r->err = std::string(who) + ": " + why;
         return VB_E_INVALID;
     };
-    if (!d || !key_out) return bad("NULL destination or key_out");
     if (d->kind != VB_DEST_LINEAR && d->kind != VB_DEST_ARRAY) return bad("unknown kind");
     const uint32_t fmt = d->format & ~(uint32_t)VB_DEST_PREMULTIPLIED;
     if (fmt > VB_DEST_RGBA32F) return bad("unknown format or flag");
@@ -394,10 +392,23 @@ extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, 
         D.w = ext.width;
         D.h = ext.height;
     }
+    *out = D;
+    return VB_OK;
+}
+
+extern "C" int vb_register_destination(vb_renderer *r, const vb_destination *d, void **key_out) {
+    if (!r) return VB_E_INVALID;
+    if (!d || !key_out) {
+        r->err = "vb_register_destination: NULL destination or key_out";
+        return VB_E_INVALID;
+    }
+    Destination D;
+    if (int rc = destination_of(r, d, "vb_register_destination", &D)) return rc;
     const void *key = new_key(r, KEY_DESTINATION);
     if (!key) {
         if (D.surf) cudaDestroySurfaceObject(D.surf);
-        return bad("no key left");
+        r->err = "vb_register_destination: no key left";
+        return VB_E_INVALID;
     }
     r->dests[key] = D;
     *key_out = (void *)key;
@@ -451,6 +462,73 @@ int vb_host::resolve_destination(vb_renderer *r, Dest *d) {
         o.y0 = D.y0;
     }
     d->out = o;
+    return VB_OK;
+}
+
+// ---- backgrounds: vb_set_background -----------------------------------------------------------------------------------------
+// The descriptor is checked as vb_register_destination checks it (destination_of); whether it covers a frame, in
+// resolve_background. Frames keep the background they were issued with (Frame::bg), so an array's surface object is destroyed
+// only once every frame that can read it, a streamed frame's re-run included, has completed. Rule: r->bg never names a
+// destroyed surface. Once the old one is released, r->bg is cleared, and the new background is installed only if every step
+// succeeded; on a failure the renderer is left without a background.
+extern "C" int vb_set_background(vb_renderer *r, const vb_destination *d) {
+    if (!r) return VB_E_INVALID;
+    Background b;
+    if (d) {
+        if (int rc = destination_of(r, d, "vb_set_background", &b.d)) return rc;
+        b.on = true;
+    }
+    if (r->bg.d.surf) {
+        // complete the frames that read the old array, whatever they report (a streamed frame may have failed for good)
+        int rc = drain_stream(r);
+        cudaError_t e = cudaSetDevice(r->device);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+        // a stream that did not complete may still read the old surface: it is then forgotten, not destroyed
+        if (e == cudaSuccess) e = cudaDestroySurfaceObject(r->bg.d.surf);
+        r->bg = Background{};
+        if (rc == VB_OK && e != cudaSuccess) {
+            r->err = std::string("vb_set_background: ") + cudaGetErrorString(e);
+            rc = VB_E_CUDA;
+        }
+        if (rc) {
+            if (b.d.surf) cudaDestroySurfaceObject(b.d.surf);
+            return rc;
+        }
+    }
+    r->bg = b;
+    return VB_OK;
+}
+
+// The frame r prepared starts from bg: check that bg covers it, and say what fine reads (d->bg). Like a destination, a
+// background holds the whole frame, so a window or a read-back band reads its own rows.
+int vb_host::resolve_background(vb_renderer *r, const Background &bg, Dest *d) {
+    d->bg = VbFineBg{};
+    if (!bg.on) return VB_OK;
+    auto bad = [&](const std::string &why) {
+        r->err = std::string("background: ") + why;
+        return VB_E_INVALID;
+    };
+    const VbConfig &c = r->cfg;
+    const Destination &D = bg.d;
+    VbFineBg g{};
+    g.on = 1u;
+    g.texel = D.texel();
+    g.premul = D.premul;
+    g.bgra = D.format == VB_DEST_BGRA8;
+    if (D.kind == VB_DEST_LINEAR) {
+        if (D.pitch < (size_t)c.target_width * g.texel) return bad("the row pitch is below " + std::to_string(g.texel) + " * width");
+        g.ptr = D.ptr;
+        g.pitch = D.pitch;
+    } else {
+        if (c.n_cells > 1u) return bad("an array cannot be the background of a batch (vb_set_cells with more than one cell)");
+        if ((uint64_t)D.x0 + c.target_width > D.w || (uint64_t)D.y0 + fine_rows(c, *d).y1 > D.h)
+            return bad("the frame does not fit the array at its origin");
+        g.surf = D.surf;
+        g.array = 1u;
+        g.x0 = D.x0;
+        g.y0 = D.y0;
+    }
+    d->bg = g;
     return VB_OK;
 }
 

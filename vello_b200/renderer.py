@@ -184,6 +184,7 @@ def load_library() -> C.CDLL:
     lib.vb_last_damage.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_uint32)]
     lib.vb_register_destination.argtypes = [vp, C.POINTER(_Destination), C.POINTER(vp)]
     lib.vb_unregister_destination.argtypes = [vp, vp]
+    lib.vb_set_background.argtypes = [vp, C.POINTER(_Destination)]
     _lib = lib
     return lib
 
@@ -199,7 +200,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_debug_graph_captures", "vb_hit_test", "vb_hit_map", "vb_fragment_upload", "vb_fragment_free", "vb_compose",
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
-                    "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms"]
+                    "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
+                    "vb_set_background"]
 
 
 def _device_rows(t, who: str, what: str, cols: int):
@@ -239,6 +241,26 @@ def _device_image(t, typestr="|u1"):
         raise ValueError(f"a device image has texel strides ({4 * e}, {e}) and a row stride that is a multiple of {4 * e}, "
                          f"not {tuple(strides)}")
     return int(cai["data"][0]), shape[0], shape[1], int(strides[0])
+
+
+def _background_image(t, typestr):
+    """(pointer, row pitch in bytes) of a background (`Renderer.set_background`): an (H, W, 4) device array as `_device_image`
+    reads it, or an (N, H, W, 4) one whose cells are H row pitches apart."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None or len(cai["shape"]) != 4:
+        ptr, _, _, pitch = _device_image(t, typestr)
+        return ptr, pitch
+    shape = tuple(int(v) for v in cai["shape"])
+    e = int(typestr[2:])
+    strides = tuple(int(v) for v in (cai.get("strides") or (shape[1] * shape[2] * 4 * e, shape[2] * 4 * e, 4 * e, e)))
+
+    class _Cell:
+        __cuda_array_interface__ = dict(cai, shape=shape[1:], strides=strides[1:])
+    ptr, h, _, pitch = _device_image(_Cell(), typestr)
+    if shape[0] > 1 and strides[0] != h * pitch:
+        raise ValueError(f"set_background: the cells of an (N, H, W, 4) background are H row pitches ({h * pitch} bytes) apart, "
+                         f"not {strides[0]}")
+    return ptr, pitch
 
 
 def _device_vector(t, width, typestrs, what):
@@ -329,6 +351,8 @@ class Renderer:
         self._stops = None  # the device array of bind_gradient_stops
         self._xforms = None  # the device array of bind_transforms
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
+        self._background = None  # the device array of set_background
+        self._background_shape = None  # (cells, H, W, 4-D) of a linear background: what _check_background compares frames with
         self._frame_size = None  # (width, height) of the last frame that succeeded: the shape of last_damage
         self._cells = 1  # cells of the installed scene (set_cells; every installation is one cell)
         self._hit_extent = None  # (width, cells * height) of the last frame that succeeded: hit_map's whole frame
@@ -342,6 +366,8 @@ class Renderer:
         r._device_images = {}
         r._fragment_pixels = {}
         r._destinations = {}
+        r._background = None
+        r._background_shape = None
         r._bound = None
         r._colors = None
         r._points = None
@@ -591,6 +617,7 @@ class Renderer:
         """Render `scene` (a `Scene`, or an already resolved `Packed`) and return the RGBA8 image
         (h, w, 4) -- un-premultiplied, like the reference's Rgba8Unorm storage texture. Goes through
         the one-call C entry point `vb_render` with host buffers (upload + render + readback)."""
+        self._check_background(params, 1)
         packed = scene if isinstance(scene, Packed) else resolve(scene.encoding)
         scene_w = np.ascontiguousarray(packed.scene, dtype=np.uint32)
         ramps = np.ascontiguousarray(packed.ramps, dtype=np.uint32)
@@ -613,6 +640,7 @@ class Renderer:
         """Render a sequence of scenes through the streaming entry points (vb_render_begin / vb_readback_wait): a generator
         of RGBA8 images, each complete when yielded. Three frames are in flight (upload | rasterise | read back), so frame k-2
         is yielded after frame k has been submitted."""
+        self._check_background(params, 1)
         outs = []
         for k, scene in enumerate(scenes):
             packed = scene if isinstance(scene, Packed) else resolve(scene.encoding)
@@ -660,6 +688,7 @@ class Renderer:
         n, h, w = len(scenes), int(params.height), int(params.width)
         if n == 0:
             raise ValueError("render_batch: no scenes")
+        self._check_background(params, n)
         if all(isinstance(s, NativeScene) for s in scenes):
             b = NativeScene()
             offsets = b.batch(scenes)
@@ -736,8 +765,60 @@ class Renderer:
         self._check(self.lib.vb_unregister_destination(self.handle, C.c_void_p(key)), "vb_unregister_destination")
         self._destinations.pop(int(key), None)
 
+    def set_background(self, target=None, *, array=None, format: str = "rgba8", alpha: str = "straight", origin=(0, 0)):
+        """Draw the frames enqueued from now on over a background instead of over the base colour (`vb_set_background`);
+        with neither `target` nor `array`, clear it.
+
+        `target`: an (H, W, 4) device array (`__cuda_array_interface__`) of the format's element type, as
+        `register_destination` takes it, or an (N, H, W, 4) one whose cells are H row pitches apart: cell c of a batch
+        (`set_cells`) starts from target[c]. Pixel (x, y) of a frame starts from element [y, x]. `array`: an integer
+        `cudaArray_t` handle, read at texel (origin[0] + x, origin[1] + y). `format` and `alpha` describe the texels as
+        for `register_destination`. Each texel is read as f32, clamped to [0, 1] and, for straight alpha, premultiplied. The
+        background may be the frame's destination itself. It must stay alive, with its pixels as the frames should see them,
+        until the frames that read it have completed. A target's shape must cover the frames rendered over it: every
+        rendering method refuses a frame (ValueError) whose rows, columns or cells it does not hold (`_check_background`).
+        An array's extent is checked by the library."""
+        if format not in self.DEST_FORMATS:
+            raise ValueError(f"set_background: format is one of {sorted(self.DEST_FORMATS)}, not {format!r}")
+        if alpha not in self.DEST_ALPHA:
+            raise ValueError(f"set_background: alpha is one of {sorted(self.DEST_ALPHA)}, not {alpha!r}")
+        fmt, typestr = self.DEST_FORMATS[format]
+        fmt |= self.DEST_ALPHA[alpha]
+        if target is not None and array is not None:
+            raise ValueError("set_background: give a target, an array or neither")
+        if target is None and array is None:
+            self._background, self._background_shape = None, None
+            self._check(self.lib.vb_set_background(self.handle, None), "vb_set_background")
+            return
+        shape = None
+        if target is not None:
+            ptr, pitch = _background_image(target, typestr)
+            d = _Destination(0, fmt, ptr, pitch, None, 0, 0)
+            dims = tuple(int(v) for v in target.__cuda_array_interface__["shape"])
+            shape = (dims[0], dims[1], dims[2], True) if len(dims) == 4 else (1, dims[0], dims[1], False)
+        else:
+            d = _Destination(1, fmt, None, 0, int(array), int(origin[0]), int(origin[1]))
+        # a failed call leaves the renderer without a background when it had to release an array's (vb_set_background)
+        self._background, self._background_shape = None, None
+        self._check(self.lib.vb_set_background(self.handle, C.byref(d)), "vb_set_background")
+        self._background, self._background_shape = target, shape
+
+    def _check_background(self, params: RenderParams, cells: int):
+        """A linear background must hold every row of every cell a frame reads; the C descriptor has no height, so the shape
+        of the target given to set_background is compared here. Cell c is read from row c * height: an (H, W, 4) target
+        needs cells * height rows, and an (N, H, W, 4) one N >= cells and, with more than one cell, H == height."""
+        if self._background_shape is None:
+            return
+        n, h, w, four_d = self._background_shape
+        height, width = int(params.height), int(params.width)
+        fits = w >= width and (h >= height and n >= cells and (cells == 1 or h == height) if four_d else h >= cells * height)
+        if not fits:
+            have = f"({n}, {h}, {w}, 4)" if four_d else f"({h}, {w}, 4)"
+            raise ValueError(f"set_background: a {have} background cannot hold {cells} cell(s) of {width}x{height}")
+
     def render_resident(self, params: RenderParams, out_device_ptr: int = 0, bin_rows=(0, 0), tile_rows=(0, 0)) -> FrameStats:
         """Render the uploaded scene into a device buffer (0 = the renderer's own target)."""
+        self._check_background(params, self._cells)
         ps = _params_struct(params, bin_rows, tile_rows)
         st = FrameStats()
         rc = self.lib.vb_render_resident(self.handle, C.byref(ps), C.c_void_p(out_device_ptr or None), C.byref(st))
@@ -748,6 +829,7 @@ class Renderer:
         return st
 
     def enqueue(self, params: RenderParams, out_device_ptr: int = 0, bin_rows=(0, 0), tile_rows=(0, 0)):
+        self._check_background(params, self._cells)
         ps = _params_struct(params, bin_rows, tile_rows)
         self._check(self.lib.vb_render_enqueue(self.handle, C.byref(ps), C.c_void_p(out_device_ptr or None)), "vb_render_enqueue")
         self._enqueued_size = (int(params.width), int(params.height))
@@ -772,6 +854,8 @@ class Renderer:
 
     # -- stage-level access (parity tests) -----------------------------------------------------------
     def run_stages(self, params: RenderParams, first: str, last: str, out_device_ptr: int = 0, bin_rows=(0, 0)):
+        if last == "fine":
+            self._check_background(params, self._cells)
         ps = _params_struct(params, bin_rows)
         rc = self.lib.vb_run_stages(self.handle, C.byref(ps), STAGES.index(first), STAGES.index(last), C.c_void_p(out_device_ptr or None))
         self._check(rc, "vb_run_stages")
