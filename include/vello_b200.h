@@ -695,6 +695,45 @@ int vb_bind_gradient_stops(vb_renderer *, const float *device_stops, uint32_t n,
  * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose transform, draw-data and
  * path-data regions past its streams would pass 32-bit word offsets. */
 int vb_bind_transforms(vb_renderer *, const float *device_affines, uint32_t n, size_t row_pitch_bytes);
+/* Bind the visibility of the installed scene's draw objects to device memory (an addition; no vello counterpart). A particle or
+ * marker view whose live count changes every frame (compose the maximum, show the live ones), a chart or map whose filter a
+ * model changes, and panels, tooltips and selection overlays that appear and disappear change which draw objects are drawn
+ * without re-encoding or re-uploading the scene (which would unbind every binding), and without a host call per frame. Unlike
+ * a bound colour with alpha 0, hiding works for every paint and for layers, a hidden draw object takes no hit test, and its
+ * path costs nothing after flatten:
+ *  - Rows. Row k is the byte at device_flags + k * row_pitch_bytes and belongs to draw object k of the installed scene, with
+ *    the indices of vb_hit_test and Scene.n_draw_objects: global in a composed scene (instance i owns draw_offsets[i] ..) and
+ *    in cell order in a batch. A nonzero byte shows draw object k and 0 hides it. Draw objects from n on are shown.
+ *  - What a frame renders. While rows are bound, every frame renders what installing the scene re-encoded without the hidden
+ *    draw objects renders: byte for byte in MSAA8 and MSAA16, and in Area up to the last-bit differences the order of a
+ *    tile's segments makes in its area sums. Hiding a BEGIN_CLIP (any push_*_layer) hides the whole layer: the push, everything up to its END_CLIP and the
+ *    layer's blend or compose effect. The row of an END_CLIP is ignored.
+ *  - How. At the start of flatten's stage the frame packs the rows into a bit mask of its own, and flatten emits nothing for the
+ *    tags of a hidden path: no line and, under a view, no box point either. Its path box stays empty, so binning, tile_alloc,
+ *    coarse and fine never see it, and a hidden BEGIN_CLIP's empty clip empties its layer. Hidden tags still pass the tag scan
+ *    and flatten's tag threads, and draw, clip and binning still see every draw object. The draws inside a hidden layer are
+ *    flattened unless their own rows hide them too; hide them as well to skip their lines.
+ *  - Hit tests and hit maps answer from the frame, so they never return a hidden draw object, nor anything inside a hidden
+ *    layer.
+ *  - A hidden path is hidden also when its points or transforms are bound (vb_bind_path_points, vb_bind_transforms).
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage, like bound points,
+ *    and a vb_run_stages range that contains flatten reads them again. The caller orders its writes before the frame, on
+ *    vb_stream or with a synchronisation. A blocking frame that is re-run after an arena overflow reads the rows again; an
+ *    enqueued frame is never re-run. Flatten and damage tracking read only the frame's mask, so rows written while a frame runs
+ *    cannot make its kernels disagree. The caller keeps the memory alive while it is bound. Changing only the contents replays
+ *    the captured frame graph. Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next
+ *    frame captures its graph anew. With nothing bound a frame launches, configures and captures exactly what it would without
+ *    this call; bound, it launches one kernel more.
+ *  - Scope. Every scene installation unbinds: every upload form, vb_render, vb_render_begin, vb_compose and vb_recompose. The
+ *    binding survives vb_set_view, vb_set_cells, the five other bindings and hit tests; all six can be active together.
+ *    device_flags NULL unbinds; frames then render every draw object.
+ *  - The call makes nothing but the mask's buffer, and does not synchronise unless that grows. Damage tracking follows the rows
+ *    (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the scene's draw-object count; a pointer that is not device memory of the renderer's device (or managed
+ * memory); a pitch of 0, or of 4 GiB or more; a renderer of a vb_group or with the exchange configured; a call between
+ * vb_render_enqueue and vb_frame_finish. */
+int vb_bind_draw_visibility(vb_renderer *, const uint8_t *device_flags, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -733,6 +772,10 @@ int vb_bind_transforms(vb_renderer *, const float *device_affines, uint32_t n, s
  *    effect at its first segment tag (its geometry's), t_hi the one at its end tag (where its brush is placed: a brush
  *    transform, or the same one). When one of them changed, the damage is the tiles of the clipped box of draw object p in the
  *    last frame and in this one. So moving one sprite of two neighbours damages only that sprite's old and new boxes.
+ *  - Automatic damage, for bound visibility (vb_bind_draw_visibility). Draw object d changed if its bit of the frame's mask
+ *    differs from the last successful frame's: only shown or hidden counts, so a row going from 1 to 2 is no change. The damage
+ *    is the tiles of its clipped box in the last frame and in this one; a hidden draw object's box is empty, so that is the box
+ *    it has while shown. A shown or hidden layer is covered by its BEGIN_CLIP's box, which holds everything inside the layer.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to
@@ -759,7 +802,7 @@ int vb_set_damage_tracking(vb_renderer *, int on);
  * draw object by draw object, on the device, with the scene the base frame rendered, and the next frame is incremental when
  * all of these hold:
  *  - tracking and the switch are on, and there is a base frame, which rendered the scene being replaced: unbound (no draw
- *    colours, path points, gradient stops or transforms bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
+ *    colours, path points, gradient stops, transforms or visibility bound either), one cell, no scene installation, binding, view, cell split or tracking switch since, and hit
  *    tests answering from it (no failed frame, vb_run_stages, vb_debug_upload or vb_debug_limit_arena since);
  *  - the upload is the only scene change since that frame (two uploads without a successful frame between them make the next
  *    frame full), and no vb_run_stages before the next one;

@@ -15,7 +15,11 @@
 //     last successful frame's, the tile box of its draw object in that frame and in this one
 //   + with bound transforms (vb_bind_transforms), for every path one of whose transforms [t_lo, t_hi] (the binding's range: from
 //     the one in effect at its first segment to the one at its TAG_PATH, where draw reads its brush) differs bit for bit from
-//     the last successful frame's, the tile box of its draw object in that frame and in this one.
+//     the last successful frame's, the tile box of its draw object in that frame and in this one
+//   + with bound visibility (vb_bind_draw_visibility), for every draw object whose bit of the frame's mask (the one flatten
+//     reads) differs from the last successful frame's, its tile box in that frame and in this one. A hidden draw object's box
+//     is empty, so the union is the box it has while shown; a hidden layer is covered by its BEGIN_CLIP's box, which holds
+//     every box inside the layer and the pixels its blend touches.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -36,9 +40,11 @@
 #define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
 
 // a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects] [the
-// words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)]
-extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads) {
-    return DM_HEADER_WORDS + 2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt + 512u * (size_t)n_grads);
+// words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)] [the n_vis words of the
+// visibility mask]
+extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads, uint32_t n_vis) {
+    return DM_HEADER_WORDS +
+           2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt + 512u * (size_t)n_grads + n_vis);
 }
 
 // the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
@@ -62,14 +68,17 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
 // there is one: its two words in the frame's path data (`pd`, the bound region), at `at_pt` of the slot (after the colour
 // words). A difference marks the path holding u (`first`, the binding's first point of each path). A non-finite row left the
 // encoded words in the region, so it is a change only if the words are. With bound transforms, xf_changed[u] records whether
-// transform u differs (a non-finite row that left an unchanged word does not).
+// transform u differs (a non-finite row that left an unchanged word does not). The same thread takes word u of the visibility
+// mask (`vis`, n_vis words, at `at_vis` of the slot), when there is one: each bit that differs marks its draw object, path d
+// being draw object d. The mask holds normalised bits, so a row going from 1 to 2 is no change.
 __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__restrict__ xf, uint32_t *snap, size_t slot_words, uint32_t n_xf,
                                                             uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed,
                                                             const uint32_t *__restrict__ pd, size_t at_pt, uint32_t n_pt,
                                                             const uint32_t *__restrict__ first, uint32_t n_paths, uint32_t *paths,
-                                                            uint32_t *xf_changed) {
+                                                            uint32_t *xf_changed, const uint32_t *__restrict__ vis, size_t at_vis,
+                                                            uint32_t n_vis) {
     const uint32_t u = blockIdx.x * DM_THREADS + threadIdx.x;
-    if (u >= n_xf && u >= n_pt) return;
+    if (u >= n_xf && u >= n_pt && u >= n_vis) return;
     const uint32_t *old;
     uint32_t *nxt;
     dm_slots(snap, slot_words, &old, &nxt);
@@ -91,6 +100,16 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
         nxt[o] = x;
         nxt[o + 1u] = y;
         if (compare && diff) paths[cp_find(first, 0u, n_paths - 1u, u)] = 1u;
+    }
+    if (u < n_vis) {
+        const uint32_t w = __ldg(vis + u);
+        uint32_t flips = compare ? w ^ old[at_vis + u] : 0u;
+        nxt[at_vis + u] = w;
+        while (flips != 0u) {
+            const uint32_t d = 32u * u + (uint32_t)(__ffs((int)flips) - 1);
+            flips &= flips - 1u;
+            if (d < n_paths) paths[d] = 1u;
+        }
     }
 }
 
@@ -182,22 +201,23 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     if (b.dmg_mode == VB_DMG_OFF) return 0u;
     const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = b.inst_n;
     const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
-    const uint32_t n_paths = b.dmg_paths ? cfg.layout.n_paths : 0u;
+    const uint32_t n_paths = b.dmg_paths ? cfg.layout.n_paths : 0u, n_vis = cfg.vis ? vb_vis_words(cfg.layout) : 0u;
     const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst,
                                                                               b.dmg_paths, n_paths);
-    // neither instance transforms, colours, points, stops nor transforms bound: nothing changes without a call that makes the
-    // frame full
-    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u && b.xf_n == 0u) return 1u;
+    // neither instance transforms, colours, points, stops, transforms nor visibility bound: nothing changes without a call that
+    // makes the frame full
+    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u && b.xf_n == 0u && n_vis == 0u) return 1u;
     const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n, at_rg = at_pt + 2u * (size_t)b.pt_n;
-    const size_t slot_words = at_rg + 512u * (size_t)b.rs_grads_n;
+    const size_t at_vis = at_rg + 512u * (size_t)b.rs_grads_n, slot_words = at_vis + n_vis;
     uint32_t launches = 1u;
-    const uint32_t n_pt = n_paths ? b.pt_n : 0u, n_mark = std::max(b.dmg_n_xf, n_pt);
+    const uint32_t n_pt = n_paths ? b.pt_n : 0u, n_mark = std::max(std::max(b.dmg_n_xf, n_pt), n_vis);
     if (n_mark) {
         k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
                                                                                       b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed,
                                                                                       b.scene + cfg.layout.path_data_base, at_pt, n_pt, b.pt_first,
-                                                                                      n_paths, b.dmg_paths, b.xf_rows ? b.dmg_xf : nullptr);
+                                                                                      n_paths, b.dmg_paths, b.xf_rows ? b.dmg_xf : nullptr,
+                                                                                      cfg.vis, at_vis, n_vis);
         launches++;
     }
     if (n_draw) {

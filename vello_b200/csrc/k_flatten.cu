@@ -775,6 +775,9 @@ __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, con
     plan.edge = false;
     uint32_t seg_type = tag.tag_byte & 3u;
     if (seg_type == 0u) return false;
+    // bound visibility: a hidden draw object's tags emit no line and no box point, so its path box stays empty and nothing
+    // after flatten sees it (a hidden BEGIN_CLIP's empty clip box empties its whole layer)
+    if (cfg.vis != nullptr && ((__ldg(cfg.vis + (tag.path_ix >> 5)) >> (tag.path_ix & 31u)) & 1u) == 0u) return false;
     bool is_stroke = (style_flags & STYLE_FLAGS_STYLE) != 0u;
     FXform &transform = plan.transform;
     {

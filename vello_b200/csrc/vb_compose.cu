@@ -873,3 +873,37 @@ extern "C" int vb_bind_transforms(vb_renderer *r, const float *device_affines, u
     r->dmg.epoch++;
     return VB_OK;
 }
+
+// ---- bound visibility: vb_bind_draw_visibility (k_visibility.cu) ----------------------------------------------------------------
+// The mask is sized here, once per binding; every frame after that packs the caller's rows into it in its k_draw_visibility, and
+// flatten culls the hidden draw objects' tags. Nothing else is made at bind time, and the call does not synchronise unless the
+// mask grows.
+extern "C" int vb_bind_draw_visibility(vb_renderer *r, const uint8_t *device_flags, uint32_t n, size_t row_pitch_bytes) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_bind_draw_visibility: " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    if (!device_flags) {
+        r->vis = vb_renderer::VisBinding{};
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const vb_renderer::SceneSlot &slot = *r->cur;
+    if (!slot.have_scene) return bad("no scene installed");
+    const VbLayout &L = slot.layout;
+    if (n == 0u || n > L.n_draw_objects)
+        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(L.n_draw_objects) + " draw objects (1 .. n_draw_objects)");
+    if (row_pitch_bytes == 0u || row_pitch_bytes > 0xffffffffu) return bad("the row pitch must be at least 1 byte and below 4 GiB");
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, device_flags)) return bad("the rows must be memory of the renderer's device");
+    const int rc = compose_room(r, r->vis_mask, (size_t)vb_vis_words(L) * 4u);
+    if (rc) return rc;
+    r->vis.rows = device_flags;
+    r->vis.n = n;
+    r->vis.pitch = (uint32_t)row_pitch_bytes;
+    r->dmg.epoch++;
+    return VB_OK;
+}

@@ -41,20 +41,20 @@ int vb_host::damage_prepare(vb_renderer *r) {
     const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles, n_draw = r->cur->layout.n_draw_objects;
     const uint32_t n_xf = r->bound.rows || r->xforms.rows ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
     const uint32_t n_col = r->colors.rows ? r->colors.n : 0u, n_pt = r->points.rows ? r->points.n : 0u;
-    const uint32_t n_grads = r->stops.rows ? r->stops.n_grads : 0u;
-    const bool snap = r->bound.rows || r->colors.rows || r->points.rows || r->stops.rows || r->xforms.rows;
+    const uint32_t n_grads = r->stops.rows ? r->stops.n_grads : 0u, n_vis = r->vis.rows ? vb_vis_words(r->cur->layout) : 0u;
+    const bool snap = any_binding(r), per_path = r->points.rows || r->vis.rows;
     int rc;
     if ((rc = ensure(r, r->dmg_mask, n_tiles))) return rc;
     if ((rc = ensure(r, r->dmg_pending, n_tiles))) return rc;
-    if (snap && (rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw, n_col, n_pt, n_grads) * 4u))) return rc;
+    if (snap && (rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw, n_col, n_pt, n_grads, n_vis) * 4u))) return rc;
     if (r->bound.rows && (rc = ensure(r, r->dmg_changed, (size_t)r->bound.n * 4u))) return rc;
-    if (r->points.rows && (rc = ensure(r, r->dmg_paths, (size_t)r->cur->layout.n_paths * 4u))) return rc;
+    if (per_path && (rc = ensure(r, r->dmg_paths, (size_t)r->cur->layout.n_paths * 4u))) return rc;
     if (r->xforms.rows && (rc = ensure(r, r->dmg_xf, (size_t)n_xf * 4u))) return rc;
     VbFrameBufs &b = r->bufs;
     b.dmg_mask = (uint8_t *)r->dmg_mask.p;
     b.dmg_pending = (uint8_t *)r->dmg_pending.p;
     if (snap) b.dmg_snap = (uint32_t *)r->dmg_snap.p;
-    if (r->points.rows) b.dmg_paths = (uint32_t *)r->dmg_paths.p;
+    if (per_path) b.dmg_paths = (uint32_t *)r->dmg_paths.p;
     if (r->xforms.rows) b.dmg_xf = (uint32_t *)r->dmg_xf.p;
     if (r->bound.rows) {
         b.dmg_changed = (uint32_t *)r->dmg_changed.p;
@@ -77,13 +77,12 @@ int vb_host::damage_prepare(vb_renderer *r) {
 }
 
 // There is a tracked base frame of the current scene (the epoch unchanged since: no installation, binding, view, cells or
-// tracking switch), unbound (no instance transforms, colours, points, stops or transforms: a diff compares scenes, not what a binding made of
-// them), of one cell, whose intermediates are intact: hit tests answer from it (no failed frame, vb_run_stages or debug write
+// tracking switch), unbound (any_binding: a diff compares scenes, not what a binding made of them), of one cell, whose intermediates are intact: hit tests answer from it (no failed frame, vb_run_stages or debug write
 // since).
 bool vb_host::base_diffable(const vb_renderer *r) {
     const vb_renderer::Damage &D = r->dmg;
     const vb_renderer::SceneSlot &s = *r->cur;
-    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !r->bound.rows && !r->colors.rows && !r->points.rows && !r->stops.rows && !r->xforms.rows &&
+    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !any_binding(r) &&
            r->hit.valid && !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects;
 }
 

@@ -439,6 +439,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.n_cells = n_cells;
     c.tile_rows = c.height_in_tiles * n_cells;
     c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
+    c.vis = r->vis.rows ? (const uint32_t *)r->vis_mask.p : nullptr; // bound visibility: the mask k_draw_visibility writes
     r->params = *p;
 
     const uint32_t n_draw = c.layout.n_draw_objects, n_tiles = c.width_in_tiles * c.tile_rows;
@@ -534,6 +535,11 @@ static int prepare(vb_renderer *r, const vb_params *p) {
         b.xf_pitch = r->xforms.pitch;
         b.xf_src = b.scene + r->cur->layout.transform_base;
     }
+    if (r->vis.rows) {
+        b.vis_rows = r->vis.rows;
+        b.vis_n = r->vis.n;
+        b.vis_pitch = r->vis.pitch;
+    }
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
     b.lb_draw = b.ctl + o_draw;
@@ -626,13 +632,15 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // a frame with bound instance transforms, bound transforms or a view first writes its transforms (read by flatten
             // and draw), the bound ones first (instances, then rows: the view's source), a frame with bound colours or stops its draw data (read by draw, coarse
             // and fine) and with bound stops its gradients' ramp rows (read by fine), and a frame with bound points its path
-            // data (read by flatten alone), inside flatten's stage events
+            // data (read by flatten alone), and a frame with bound visibility its mask (read by flatten and damage tracking), inside
+            // flatten's stage events
             launches += vb_launch_instance_transforms(c, b, st);
             launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             launches += vb_launch_draw_colors(c, b, st);
             launches += vb_launch_bound_ramps(c, b, st);
             launches += vb_launch_path_points(c, b, st);
+            launches += vb_launch_draw_visibility(c, b, st);
             if (fork_draw) {
                 CK(cudaEventRecord(r->draw_fork, st));
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->draw_fork, 0));

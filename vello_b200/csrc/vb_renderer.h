@@ -2,7 +2,7 @@
 //
 // The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
 // (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
-// instance transforms, draw colours, path points, gradient stops and transforms), vb_damage.cu (damage tracking), vb_debug.cu (debug
+// instance transforms, draw colours, path points, gradient stops, transforms and visibility), vb_damage.cu (damage tracking), vb_debug.cu (debug
 // downloads and uploads) and vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
 // namespace vb_host, hidden from the shared library's symbol table, so that a host program's own functions of the same names
 // cannot interpose on them.
@@ -361,6 +361,13 @@ struct vb_renderer {
         uint32_t n = 0, pitch = 0;
     } xforms;
     DevBuf xform_ranges;
+    // bound visibility (vb_bind_draw_visibility) of the current scene: the caller's rows (nullptr: unbound), and vis_mask, the
+    // bit mask (vb_vis_words) each frame packs them into (k_visibility.cu). Every scene installation unbinds (set_scene).
+    struct VisBinding {
+        const uint8_t *rows = nullptr;
+        uint32_t n = 0, pitch = 0;
+    } vis;
+    DevBuf vis_mask;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -417,7 +424,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
                            &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
-                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges,
+                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_xf, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
@@ -484,6 +491,11 @@ inline uint32_t n_draw_data(const VbLayout &L, size_t scene_words) {
 inline uint32_t n_path_data(const VbLayout &L, size_t scene_words) {
     if (L.draw_tag_base < L.path_data_base || L.draw_tag_base > scene_words) return 0u;
     return L.draw_tag_base - L.path_data_base;
+}
+// Whether anything of the current scene is bound to device rows: instance transforms, draw colours, path points, gradient
+// stops, transforms or visibility. Such frames keep a damage snapshot, and are no base for an upload diff.
+inline bool any_binding(const vb_renderer *r) {
+    return r->bound.rows || r->colors.rows || r->points.rows || r->stops.rows || r->xforms.rows || r->vis.rows;
 }
 // Whether frames read their draw data from the region past the scene's streams: with bound colours or bound gradient stops.
 inline bool draw_data_bound(const vb_renderer *r) { return r->colors.rows || r->stops.rows; }

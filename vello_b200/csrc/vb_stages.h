@@ -63,6 +63,9 @@ struct VbFrameBufs {
     const uint8_t *xf_rows;
     const uint2 *xf_range;
     const uint32_t *xf_src;
+    // bound visibility (vb_bind_draw_visibility), read by k_draw_visibility into the mask at VbConfig::vis: the caller's rows
+    // (draw object k's byte at vis_rows + k * vis_pitch). Null while unbound.
+    const uint8_t *vis_rows;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -88,8 +91,9 @@ struct VbFrameBufs {
     uint32_t *ptcl, *blend_spill;
     // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
     // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
-    // of the frame's transform words, draw boxes, colour words of the col_n bound draw objects and words of the pt_n bound
-    // points), one changed flag per bound instance, with points bound one per path and with transforms bound one per
+    // of the frame's transform words, draw boxes, colour words of the col_n bound draw objects, words of the pt_n bound
+    // points, ramp rows of the bound gradients and the visibility mask), one changed flag per bound instance, with points or
+    // visibility bound one per path and with transforms bound one per
     // transform, and the composed scene's draw prefix (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k +
     // 1]; null while unbound)
     uint8_t *dmg_mask, *dmg_pending;
@@ -115,6 +119,7 @@ struct VbFrameBufs {
     uint32_t xf_n, xf_pitch;   // bound transform rows and their pitch in bytes; 0 while unbound
     uint32_t rs_n, rs_pitch;   // bound stop rows and their pitch in bytes; 0 while unbound
     uint32_t rs_grads_n, rs_ramp0; // bound gradients and the ramp row of the first; 0 while unbound
+    uint32_t vis_n, vis_pitch;     // bound visibility rows and their pitch in bytes; 0 while unbound
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
@@ -131,6 +136,10 @@ struct VbFrameBufs {
 // scene_words alone, so that it writes its own region and no later one.
 static inline uint32_t vb_transform_regions_end(const VbConfig &cfg, const VbFrameBufs &b) {
     return b.col_slots ? cfg.layout.draw_data_base : b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
+}
+// The words of the visibility mask of a scene: one bit per draw object, and per path (path p is draw object p).
+static inline uint32_t vb_vis_words(const VbLayout &L) {
+    return ((L.n_draw_objects > L.n_paths ? L.n_draw_objects : L.n_paths) + 31u) / 32u;
 }
 static inline uint32_t vb_draw_data_region_end(const VbConfig &cfg, const VbFrameBufs &b) {
     return b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
@@ -274,6 +283,11 @@ uint32_t vb_launch_path_points(const VbConfig &cfg, const VbFrameBufs &b, cudaSt
 // unbound.
 uint32_t vb_launch_bound_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// k_visibility.cu: bound visibility (vb_bind_draw_visibility). Per frame, at the start of flatten's stage after the path data:
+// the caller's rows packed into the mask at cfg.vis (vb_vis_words words; bit k set for a nonzero byte k below b.vis_n and for
+// every k from b.vis_n on), which flatten and damage tracking read; nothing while unbound.
+uint32_t vb_launch_draw_visibility(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
 // the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame
 // succeeded. vb_launch_damage_rects stages caller rectangles (tile ranges x0 y0 x1 y1, clipped) into `pending` in stream order.
@@ -283,7 +297,7 @@ uint32_t vb_launch_bound_transforms(const VbConfig &cfg, const VbFrameBufs &b, c
 uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
-size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads);
+size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads, uint32_t n_vis);
 // k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
 // of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
 // are null

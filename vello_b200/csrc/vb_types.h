@@ -70,6 +70,10 @@ typedef struct {
      * height_in_tiles and the windows above stay the CELL's. n_cells = 1: no batch (cell_draw unused). */
     uint32_t n_cells, tile_rows;
     const uint32_t *cell_draw; /* device: n_cells + 1 draw-object offsets */
+    /* Bound visibility (vb_bind_draw_visibility): one bit per draw object (path p is draw object p), written by
+     * k_draw_visibility at the start of flatten's stage; flatten emits nothing for a tag of a path whose bit is clear
+     * (plan_tag). Null while unbound. */
+    const uint32_t *vis;
 } VbConfig;
 
 /* One rectangle of k_atlas_blit (k_atlas.cu): w x h RGBA8 texels from device memory (rows src_pitch bytes apart, 4-byte

@@ -88,6 +88,7 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     r->points = vb_renderer::PointBinding{};
     r->stops = vb_renderer::StopBinding{};
     r->xforms = vb_renderer::TransformBinding{};
+    r->vis = vb_renderer::VisBinding{};
     r->dmg.epoch++;
     // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
     vb_renderer::Damage::Diff &X = r->dmg.diff;

@@ -178,6 +178,7 @@ def load_library() -> C.CDLL:
     lib.vb_bind_path_points.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_gradient_stops.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_draw_visibility.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -201,7 +202,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
-                    "vb_set_background"]
+                    "vb_set_background", "vb_bind_draw_visibility"]
 
 
 def _device_rows(t, who: str, what: str, cols: int):
@@ -219,6 +220,23 @@ def _device_rows(t, who: str, what: str, cols: int):
     if int(strides[1]) != 4 or pitch % 4 or pitch < 4 * cols:
         raise ValueError(f"{who}: columns 4 bytes apart and rows a multiple of 4 bytes, at least {4 * cols}, apart; "
                          f"not strides {tuple(strides)}")
+    return C.c_void_p(int(cai["data"][0])), shape[0], pitch
+
+
+def _device_flags(t, who: str):
+    """(pointer, rows, row pitch in bytes) of a 1-D bool or uint8 device array bound by a `bind_*` method, from its
+    `__cuda_array_interface__` (a torch CUDA tensor, or a column of a larger uint8 one): one byte per row, rows any positive
+    number of bytes apart. `who` names the method in the errors."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device flags are needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 1 or shape[0] == 0 or cai["typestr"] not in ("|b1", "|u1", "<u1", ">u1"):
+        raise ValueError(f"{who}: flags must be (n,) bool or uint8, not {shape} {cai['typestr']}")
+    strides = cai.get("strides") or (1,)
+    pitch = int(strides[0]) if shape[0] > 1 else 1  # the pitch of a single row is never used
+    if pitch <= 0:
+        raise ValueError(f"{who}: rows a positive number of bytes apart, not strides {tuple(strides)}")
     return C.c_void_p(int(cai["data"][0])), shape[0], pitch
 
 
@@ -350,6 +368,7 @@ class Renderer:
         self._points = None  # the device array of bind_path_points
         self._stops = None  # the device array of bind_gradient_stops
         self._xforms = None  # the device array of bind_transforms
+        self._visibility = None  # the device array of bind_draw_visibility
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._background = None  # the device array of set_background
         self._background_shape = None  # (cells, H, W, 4-D) of a linear background: what _check_background compares frames with
@@ -373,6 +392,7 @@ class Renderer:
         r._points = None
         r._stops = None
         r._xforms = None
+        r._visibility = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -605,6 +625,30 @@ class Renderer:
         ptr, n, pitch = _device_rows(t, "bind_transforms", "transforms", 6)
         self._check(self.lib.vb_bind_transforms(self.handle, ptr, n, pitch), "vb_bind_transforms")
         self._xforms = t
+
+    def bind_draw_visibility(self, t):
+        """Show draw object k of the installed scene only while byte k of the device array `t` is nonzero, in every frame from
+        now on, read when the frame runs (`vb_bind_draw_visibility`): `t` is a 1-D bool or uint8 array of n flags, n at most
+        the scene's `Scene.n_draw_objects`, with `__cuda_array_interface__` and any positive byte stride (e.g. a torch CUDA
+        tensor, or a column of a larger uint8 state tensor such as `state[:, 3]`). Index k is the draw object of `hit_test`,
+        global in a composed scene (instance i owns `draw_offsets[i] ..`) or a batch; draw objects from n on are shown. Every
+        frame renders what uploading the scene re-encoded without the hidden draw objects would render. Hiding a push_*_layer's
+        draw object hides the whole layer, up to its pop_layer (whose flag is ignored), and its blend; hide the layer's own
+        draws too to skip their flattening. Hit tests and hit maps
+        never return a hidden draw object. Write `t` on `self.stream` (or synchronise) before a frame; frames then need no
+        further call. Per instance of a composed scene, one device op makes the flags from an (instances,) bool mask and the
+        instances' draw counts (`counts = draw_offsets[1:] - draw_offsets[:-1]` as a device tensor):
+
+            r.bind_draw_visibility(mask_inst.repeat_interleave(counts))
+
+        `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        if t is None:
+            self._check(self.lib.vb_bind_draw_visibility(self.handle, None, 0, 0), "vb_bind_draw_visibility")
+            self._visibility = None
+            return
+        ptr, n, pitch = _device_flags(t, "bind_draw_visibility")
+        self._check(self.lib.vb_bind_draw_visibility(self.handle, ptr, n, pitch), "vb_bind_draw_visibility")
+        self._visibility = t
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
