@@ -72,12 +72,13 @@ extern "C" uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n,
 }
 
 extern "C" uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.col_slots) return 0u;
-    // the region prepare reserved past the scene's streams and the transform regions, up to the bound path data's (vb_stages.h)
-    const uint32_t n = vb_draw_data_region_end(cfg, b) - cfg.layout.draw_data_base;
+    if (!b.bound.col_slots) return 0u;
+    // the region prepare reserved past the scene's streams and the transform regions
+    const uint32_t n = b.dd_len;
     if (n == 0u) return 0u;
     uint32_t *dst = const_cast<uint32_t *>(b.scene) + cfg.layout.draw_data_base;
-    k_draw_colors<<<(n + DC_THREADS - 1u) / DC_THREADS, DC_THREADS, 0, st>>>(b.col_rows, b.col_pitch, b.col_slots, b.col_src, dst, n,
-                                                                              b.rs_ramp0);
+    const VbRows &rows = b.bound.rows[VB_BIND_COLORS];
+    k_draw_colors<<<(n + DC_THREADS - 1u) / DC_THREADS, DC_THREADS, 0, st>>>(rows.rows, rows.pitch, b.bound.col_slots, b.col_src, dst, n,
+                                                                              b.bound.rs_ramp0);
     return 1u;
 }

@@ -157,13 +157,14 @@ __global__ void __launch_bounds__(256) k_instance_transforms(const uint8_t *__re
 }
 
 extern "C" uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.inst_rows) return 0u;
-    // the bound region prepare reserved, as long as the region at transform_base: that one itself, or the viewed region with a
-    // view on top of it, whose source (view_src) is the bound one; it ends where the draw-data or path-data region begins
-    const uint32_t n = (vb_transform_regions_end(cfg, b) - cfg.layout.transform_base) / 6u;
+    const VbRows &rows = b.bound.rows[VB_BIND_INSTANCES];
+    if (!rows.rows) return 0u;
+    // the bound region prepare reserved: at transform_base, or with a view on top of it at the view's source (view_src)
+    const uint32_t n = b.xf_len;
     if (n == 0u) return 0u;
     uint32_t *dst = const_cast<uint32_t *>(b.scene) + (b.view ? cfg.view_src : cfg.layout.transform_base);
-    k_instance_transforms<<<(n + 255u) / 256u, 256, 0, st>>>(b.inst_rows, b.inst_pitch, b.inst_prefix, b.inst_xf, b.inst_src, dst, b.inst_n, n);
+    k_instance_transforms<<<(n + 255u) / 256u, 256, 0, st>>>(rows.rows, rows.pitch, b.bound.inst_prefix, b.bound.inst_xf, b.bound.inst_src, dst,
+                                                             rows.n, n);
     return 1u;
 }
 

@@ -199,7 +199,10 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_rects(uint8_t *pending, D
 
 extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
     if (b.dmg_mode == VB_DMG_OFF) return 0u;
-    const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = b.inst_n;
+    const VbBound &B = b.bound;
+    const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = B.rows[VB_BIND_INSTANCES].n;
+    const uint32_t n_col = B.rows[VB_BIND_COLORS].n, n_pt_rows = B.rows[VB_BIND_POINTS].n;
+    const bool xf_bound = B.rows[VB_BIND_TRANSFORMS].rows != nullptr;
     const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
     const uint32_t n_paths = b.dmg_paths ? cfg.layout.n_paths : 0u, n_vis = cfg.vis ? vb_vis_words(cfg.layout) : 0u;
     const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
@@ -207,26 +210,26 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
                                                                               b.dmg_paths, n_paths);
     // neither instance transforms, colours, points, stops, transforms nor visibility bound: nothing changes without a call that
     // makes the frame full
-    if (n_inst == 0u && b.col_n == 0u && b.pt_n == 0u && b.rs_grads_n == 0u && b.xf_n == 0u && n_vis == 0u) return 1u;
-    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + b.col_n, at_rg = at_pt + 2u * (size_t)b.pt_n;
-    const size_t at_vis = at_rg + 512u * (size_t)b.rs_grads_n, slot_words = at_vis + n_vis;
+    if (n_inst == 0u && n_col == 0u && n_pt_rows == 0u && B.rs_grads_n == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && n_vis == 0u) return 1u;
+    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + n_col, at_rg = at_pt + 2u * (size_t)n_pt_rows;
+    const size_t at_vis = at_rg + 512u * (size_t)B.rs_grads_n, slot_words = at_vis + n_vis;
     uint32_t launches = 1u;
-    const uint32_t n_pt = n_paths ? b.pt_n : 0u, n_mark = std::max(std::max(b.dmg_n_xf, n_pt), n_vis);
+    const uint32_t n_pt = n_paths ? n_pt_rows : 0u, n_mark = std::max(std::max(b.dmg_n_xf, n_pt), n_vis);
     if (n_mark) {
         k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
-                                                                                      b.dmg_n_xf, !full, b.inst_prefix, n_inst, b.dmg_changed,
-                                                                                      b.scene + cfg.layout.path_data_base, at_pt, n_pt, b.pt_first,
-                                                                                      n_paths, b.dmg_paths, b.xf_rows ? b.dmg_xf : nullptr,
+                                                                                      b.dmg_n_xf, !full, B.inst_prefix, n_inst, b.dmg_changed,
+                                                                                      b.scene + cfg.layout.path_data_base, at_pt, n_pt, B.pt_first,
+                                                                                      n_paths, b.dmg_paths, xf_bound ? b.dmg_xf : nullptr,
                                                                                       cfg.vis, at_vis, n_vis);
         launches++;
     }
     if (n_draw) {
         const uint32_t per = DM_THREADS / 32u;
-        k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, b.inst_draw,
+        k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, B.inst_draw,
                                                                    n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
-                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, b.col_n, b.dmg_paths,
-                                                                   cfg.layout.n_paths, b.rs_grads_n ? b.rs_draw : nullptr,
-                                                                   b.ramps + 512u * (size_t)b.rs_ramp0, at_rg, b.xf_rows ? b.xf_range : nullptr,
+                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, n_col, b.dmg_paths,
+                                                                   cfg.layout.n_paths, B.rs_grads_n ? B.rs_draw : nullptr,
+                                                                   b.ramps + 512u * (size_t)B.rs_ramp0, at_rg, xf_bound ? B.xf_range : nullptr,
                                                                    b.dmg_xf);
         launches++;
     }

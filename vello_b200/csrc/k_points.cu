@@ -122,12 +122,13 @@ extern "C" uint32_t vb_launch_path_point_slots(const uint32_t *tags, uint32_t n_
 }
 
 extern "C" uint32_t vb_launch_path_points(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.pt_rows) return 0u;
-    // the region prepare reserved: [path_data_base, scene_words), the last one past the scene's streams
-    const uint32_t n_words = cfg.scene_words - cfg.layout.path_data_base;
+    const VbRows &rows = b.bound.rows[VB_BIND_POINTS];
+    if (!rows.rows) return 0u;
+    // the region prepare reserved past the scene's streams, the last one
+    const uint32_t n_words = b.pd_len;
     if (n_words == 0u) return 0u;
     uint32_t *dst = const_cast<uint32_t *>(b.scene) + cfg.layout.path_data_base;
     const uint32_t n_points = (n_words + 1u) / 2u;
-    k_path_points<<<(n_points + PP_THREADS - 1u) / PP_THREADS, PP_THREADS, 0, st>>>(b.pt_rows, b.pt_pitch, b.pt_n, b.pt_src, dst, n_words);
+    k_path_points<<<(n_points + PP_THREADS - 1u) / PP_THREADS, PP_THREADS, 0, st>>>(rows.rows, rows.pitch, rows.n, b.pt_src, dst, n_words);
     return 1u;
 }

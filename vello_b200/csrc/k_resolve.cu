@@ -161,8 +161,9 @@ extern "C" uint32_t vb_launch_gradient_slots(const uint32_t *tags, uint32_t n_dr
     return 1u;
 }
 extern "C" uint32_t vb_launch_bound_ramps(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.rs_rows || b.rs_grads_n == 0u) return 0u;
-    uint32_t *out = const_cast<uint32_t *>(b.ramps) + (size_t)b.rs_ramp0 * RS_SAMPLES;
-    k_bound_ramps<<<b.rs_grads_n, RS_SAMPLES, 0, st>>>(b.rs_grads, b.rs_stops, b.rs_rows, b.rs_n, b.rs_pitch, out);
+    const VbRows &rows = b.bound.rows[VB_BIND_STOPS];
+    if (!rows.rows || b.bound.rs_grads_n == 0u) return 0u;
+    uint32_t *out = const_cast<uint32_t *>(b.ramps) + (size_t)b.bound.rs_ramp0 * RS_SAMPLES;
+    k_bound_ramps<<<b.bound.rs_grads_n, RS_SAMPLES, 0, st>>>(b.bound.rs_grads, b.bound.rs_stops, rows.rows, rows.n, rows.pitch, out);
     return 1u;
 }

@@ -41,13 +41,13 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_transforms(const uint8_t *
 }
 
 extern "C" uint32_t vb_launch_bound_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.xf_rows) return 0u;
-    // the bound region prepare reserved, as long as the region at transform_base (vb_launch_instance_transforms): that one
-    // itself, or with a view the view's source
-    const uint32_t n = (vb_transform_regions_end(cfg, b) - cfg.layout.transform_base) / 6u;
+    const VbRows &rows = b.bound.rows[VB_BIND_TRANSFORMS];
+    if (!rows.rows) return 0u;
+    // the bound region prepare reserved (vb_launch_instance_transforms): at transform_base, or with a view at the view's source
+    const uint32_t n = b.xf_len;
     if (n == 0u) return 0u;
     uint32_t *dst = const_cast<uint32_t *>(b.scene) + (b.view ? cfg.view_src : cfg.layout.transform_base);
-    const uint32_t *src = b.inst_rows ? nullptr : b.xf_src;
-    k_bound_transforms<<<(n + BT_THREADS - 1u) / BT_THREADS, BT_THREADS, 0, st>>>(b.xf_rows, b.xf_pitch, b.xf_n, src, dst, n);
+    const uint32_t *src = b.bound.rows[VB_BIND_INSTANCES].rows ? nullptr : b.xf_src;
+    k_bound_transforms<<<(n + BT_THREADS - 1u) / BT_THREADS, BT_THREADS, 0, st>>>(rows.rows, rows.pitch, rows.n, src, dst, n);
     return 1u;
 }

@@ -41,12 +41,10 @@ extern "C" void vb_launch_view_set(float *dst, const float m[6], cudaStream_t st
 }
 
 extern "C" uint32_t vb_launch_view_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    // exactly the region prepare reserved and sized the allocation for: [transform_base, end), past the uploaded streams and
-    // before any bound draw-data or path-data region. It is empty for a layout whose transforms do not lie inside the uploaded
-    // words, so such a layout launches nothing, and the source transforms [view_src, view_src + 6 n) lie inside the scene
-    // whenever n > 0.
-    const uint32_t end = vb_transform_regions_end(cfg, b);
-    const uint32_t n = end > cfg.layout.transform_base ? (end - cfg.layout.transform_base) / 6u : 0u;
+    // exactly the region prepare reserved and sized the allocation for: n transforms at transform_base, past the uploaded
+    // streams. It is empty for a layout whose transforms do not lie inside the uploaded words, so such a layout launches
+    // nothing, and the source transforms [view_src, view_src + 6 n) lie inside the scene whenever n > 0.
+    const uint32_t n = b.xf_len;
     if (n == 0u) return 0u;
     uint32_t *dst = const_cast<uint32_t *>(b.scene) + cfg.layout.transform_base;
     k_view_transforms<<<(n + 255u) / 256u, 256, 0, st>>>(b.view, b.scene + cfg.view_src, dst, n);

@@ -30,7 +30,8 @@ extern "C" uint32_t vb_launch_draw_visibility(const VbConfig &cfg, const VbFrame
     const uint32_t n_words = vb_vis_words(cfg.layout);
     if (n_words == 0u) return 0u;
     const uint32_t n_bits = n_words * 32u;
-    k_draw_visibility<<<(n_bits + VIS_THREADS - 1u) / VIS_THREADS, VIS_THREADS, 0, st>>>(b.vis_rows, b.vis_pitch, b.vis_n,
+    const VbRows &rows = b.bound.rows[VB_BIND_VISIBILITY];
+    k_draw_visibility<<<(n_bits + VIS_THREADS - 1u) / VIS_THREADS, VIS_THREADS, 0, st>>>(rows.rows, rows.pitch, rows.n,
                                                                                         const_cast<uint32_t *>(cfg.vis), n_words);
     return 1u;
 }

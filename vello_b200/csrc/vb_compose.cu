@@ -474,7 +474,7 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
         if (n_old) memcpy(t + n_old + 1u + n + 1u + n, unmatched.data(), (size_t)n_old * 4u);
     }
 
-    if ((rc = compose_room(r, slot.scene, scene_bytes(L, total_words, r->view.on)))) return rc;
+    if ((rc = compose_room(r, slot.scene, regions_of(L, total_words, false, r->view.on, false, false).bytes))) return rc;
     if (new_ramps && (rc = compose_room(r, slot.ramps, ramps.size() * 512u * 4u))) return rc;
     if (new_atlas && (rc = compose_room(r, slot.atlas, (size_t)atlas_w * atlas_h * 4u))) return rc;
     if (staged) CK(cudaMemcpyAsync(tmp, h, staged, cudaMemcpyHostToDevice, st));
@@ -537,43 +537,72 @@ extern "C" uint32_t vb_debug_match_instances(const uint32_t *old_keys, uint32_t 
     return vb_diff_match(n_old, n_new, [&](uint32_t i, uint32_t j) { return old_keys[i] == new_keys[j]; }, match);
 }
 
-// ---- bound instance transforms: vb_bind_instance_transforms (k_compose.cu) ----------------------------------------------------
-// The binding's tables are made once, here: the transform prefix and compose-time transforms from the slot's instance records,
-// the untransformed transforms by one k_compose_streams over the transform stream alone (no transforms applied, destination 0).
-// Every frame after that reads the caller's rows in its k_instance_transforms.
-extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_transforms, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_instance_transforms: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange enabled");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_transforms) {
-        r->bound = vb_renderer::Binding{};
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene || !slot.composed) return bad("the renderer's current scene was not made by vb_compose");
-    if (n == 0u || n != slot.inst_frag.size())
-        return bad(std::to_string(n) + " rows for a composed scene of " + std::to_string(slot.inst_frag.size()) + " instances");
-    if ((uintptr_t)device_transforms & 3u) return bad("the pointer must be 4-byte aligned");
-    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 24u || row_pitch_bytes > 0xfffffffcu)
-        return bad("the row pitch must be a multiple of 4 bytes, at least 24 and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_transforms)) return bad("the rows must be memory of the renderer's device");
-    std::vector<const Fragment *> fr(n);
-    for (uint32_t k = 0; k < n; k++)
-        if (!(fr[k] = find_fragment(r, slot.inst_frag[k]))) return bad("fragment " + std::to_string(slot.inst_frag[k]) + " of the composed scene was freed");
-    // a frame writes the bound region and, under a view, the viewed one past the scene (vb_resolve_layout reserved one), and
-    // bound colours' draw data and bound points' path data after them
-    const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
-    const uint64_t n_dd = draw_data_bound(r) ? n_draw_data(slot.layout, slot.scene_words) : 0u;
-    const uint64_t n_pd = r->points.rows ? n_path_data(slot.layout, slot.scene_words) : 0u;
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd + n_pd > 0xfffffff0ull)
-        return bad("the scene with its bound and viewed transforms exceeds 32-bit word offsets");
+// ---- bindings to device rows: vb_bind_* -----------------------------------------------------------------------------------------
+// A binding points the installed scene at device rows that every frame reads (VbBound). Every kind is bound by one path,
+// bind_rows: the checks they share, and what differs between them from BIND_KINDS: the scene a kind needs, how many rows it
+// takes and at what pitch, its own checks, and the tables it makes once, here, on the renderer's stream. The tables stay valid
+// while the rows are bound, because every scene installation unbinds; every frame after that reads the caller's rows.
+using Slot = vb_renderer::SceneSlot;
 
+// The scene a kind binds to, or why there is none (steps 4 and 5 of bind_rows)
+static const char *any_scene(const Slot &s) { return s.have_scene ? nullptr : "no scene installed"; }
+static const char *composed_scene(const Slot &s) {
+    return s.have_scene && s.composed ? nullptr : "the renderer's current scene was not made by vb_compose";
+}
+static const char *scene_with_stops(const Slot &s) {
+    if (!s.have_scene) return "no scene installed";
+    if (!s.have_stops)
+        return "the scene was installed as packed bytes, whose gradients exist only as resolved ramps; install it from its "
+               "streams (vb_scene_upload_streams, vb_scene_upload_device, vb_render_scene) or with vb_compose";
+    return nullptr;
+}
+
+// The rows a scene takes at most (instances: exactly)
+static uint64_t n_instances(const Slot &s) { return s.inst_frag.size(); }
+static uint64_t n_draws(const Slot &s) { return s.layout.n_draw_objects; }
+static uint64_t n_points(const Slot &s) { return n_path_data(s.layout, s.scene_words) / 2u; }
+static uint64_t n_stops(const Slot &s) { return s.stops.size(); }
+static uint64_t n_xforms(const Slot &s) { return n_transforms(s.layout, s.scene_words); }
+
+// The kinds' own checks, after the shared ones: why n rows cannot be bound, or nothing
+static std::string freed_fragment(const vb_renderer *r, uint32_t) {
+    for (uint32_t id : r->cur->inst_frag)
+        if (!find_fragment(r, id)) return "fragment " + std::to_string(id) + " of the composed scene was freed";
+    return {};
+}
+static std::string draw_tags_outside(const Slot &s, uint64_t n) {
+    if ((uint64_t)s.layout.draw_tag_base + n > s.scene_words) return "the scene's draw tags do not lie inside its words";
+    return {};
+}
+static std::string colors_check(const vb_renderer *r, uint32_t n) { return draw_tags_outside(*r->cur, n); }
+static std::string path_tags_outside(const vb_renderer *r, uint32_t) {
+    const VbLayout &L = r->cur->layout;
+    if (L.path_data_base < L.path_tag_base || L.path_data_base > r->cur->scene_words) return "the scene's path tags do not lie inside its words";
+    return {};
+}
+// bound gradient stops bind the scene's first ramp patches: those with a stop below n (the stops are concatenated in patch order)
+static uint32_t bound_grads(const Slot &s, uint32_t n) {
+    uint32_t g = 0u;
+    while (g < s.stop_patches.size() && s.stop_patches[g].first < n) g++;
+    return g;
+}
+static std::string stops_check(const vb_renderer *r, uint32_t n) {
+    const Slot &s = *r->cur;
+    if ((uint64_t)s.n_ramps + bound_grads(s, n) > (1ull << 30)) return "the scene's ramps and one per bound gradient pass the 30 bits of the ramp word";
+    return draw_tags_outside(s, s.layout.n_draw_objects);
+}
+static std::string no_check(const vb_renderer *, uint32_t) { return {}; }
+
+// The kinds' bind-time work: the tables of n rows in b. `why` is set for a refusal that only the work finds.
+
+// Bound instance transforms (k_compose.cu): the transform prefix and compose-time transforms from the slot's instance records,
+// the untransformed transforms by one k_compose_streams over the transform stream alone (no transforms applied, destination
+// 0), and the instances' draw prefix, for damage tracking.
+static int instance_tables(vb_renderer *r, uint32_t n, VbBound &b, std::string &) {
+    const Slot &slot = *r->cur;
+    std::vector<const Fragment *> fr(n);
+    for (uint32_t k = 0; k < n; k++) fr[k] = find_fragment(r, slot.inst_frag[k]);
+    const uint32_t n_tr = n_transforms(slot.layout, slot.scene_words);
     // staged through pinned memory: [the copy's tables (cmp_tables), with no transforms] [the binding's tables: transform
     // prefix (n + 1), compose-time transforms] [the instances' draw prefix (n + 1)]
     reap_freed(r);
@@ -603,23 +632,105 @@ extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_t
     a.units[CMP_TRANSFORMS] = n_tr;
     vb_launch_compose(a, st);
     CK(cudaGetLastError());
-    r->bound.rows = (const uint8_t *)device_transforms;
-    r->bound.n = n;
-    r->bound.pitch = (uint32_t)row_pitch_bytes;
-    r->bound.o_xf = o_xf;
-    r->bound.o_src = o_tr;
-    r->bound.o_draw = o_draw;
-    r->dmg.epoch++;
+    b.inst_prefix = (const uint32_t *)tables;
+    b.inst_xf = (const CmpXform *)(tables + o_xf);
+    b.inst_src = (const uint32_t *)(tables + o_tr);
+    b.inst_draw = (const uint32_t *)(tables + o_draw);
     return VB_OK;
 }
 
-// ---- bound draw colours: vb_bind_draw_colors (k_colors.cu) ----------------------------------------------------------------------
-// The draw-data slot table is made here, on the renderer's stream, whenever bound colours or bound gradient stops change: every
-// word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col draw tags and one k_gradient_slots for the n_grads bound
-// gradients, whose ramp words are at grad_dd and whose draw objects it writes to draw_grad. It stays valid while the rows are
-// bound, because every scene installation unbinds. Every frame after that reads the caller's rows in its k_draw_colors.
-static int draw_data_slots(vb_renderer *r, uint32_t n_col, uint32_t n_grads, const uint32_t *grad_dd, uint32_t *draw_grad) {
-    const vb_renderer::SceneSlot &slot = *r->cur;
+// Bound path points (k_points.cu): the table of each path's first point, by one k_path_point_slots over the scene's path tags,
+// and its 16-bit flag, read back (the call's one synchronisation).
+static int point_tables(vb_renderer *r, uint32_t, VbBound &b, std::string &why) {
+    const Slot &slot = *r->cur;
+    const VbLayout &L = slot.layout;
+    int rc;
+    if ((rc = compose_room(r, r->point_slots, ((size_t)L.n_paths + 2u) * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    uint32_t *first = (uint32_t *)r->point_slots.p, *flag = first + L.n_paths + 1u;
+    CK(cudaMemsetAsync(first, 0, ((size_t)L.n_paths + 2u) * 4u, st));
+    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, L.path_data_base - L.path_tag_base, L.n_paths, first, flag,
+                               nullptr, st);
+    CK(cudaGetLastError());
+    uint32_t i16 = 0u;
+    CK(cudaMemcpyAsync(&i16, flag, 4u, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (i16) {
+        why = "the scene has 16-bit path segments, whose points are not f32 pairs";
+        return VB_E_INVALID;
+    }
+    b.pt_first = first;
+    return VB_OK;
+}
+
+// Bound gradient stops (k_resolve.cu): the tables, and the scene's ramps copied into the first rows of stop_ramps. The call's
+// one synchronisation waits for the tables' copy. The draw-data slot table follows (bind_rows).
+static int stop_tables(vb_renderer *r, uint32_t n, VbBound &b, std::string &) {
+    const Slot &slot = *r->cur;
+    const VbLayout &L = slot.layout;
+    const uint32_t n_grads = bound_grads(slot, n);
+    // the tables: [each gradient's ramp word, relative to the draw data] [the gradients (RsRamp), at o_grads] [their stops as
+    // encoded, at o_stops] [draw object -> gradient, at o_draw]
+    const Slot::StopPatch *last = n_grads ? &slot.stop_patches[n_grads - 1u] : nullptr;
+    const size_t s_used = last ? (size_t)last->first + last->n_stops : 0u;
+    const size_t o_grads = up16((size_t)n_grads * 4u), o_stops = up16(o_grads + (size_t)n_grads * sizeof(RsRamp));
+    const size_t o_draw = up16(o_stops + s_used * sizeof(RsStop)), bytes = o_draw + (size_t)L.n_draw_objects * 4u;
+    std::vector<uint8_t> h(bytes, 0u);
+    uint32_t *dd = (uint32_t *)h.data();
+    RsRamp *grads = (RsRamp *)(h.data() + o_grads);
+    for (uint32_t g = 0; g < n_grads; g++) {
+        const Slot::StopPatch &p = slot.stop_patches[g];
+        grads[g] = RsRamp{p.first, p.n_stops, p.premul, 0u};
+        dd[g] = p.dd;
+    }
+    if (s_used) memcpy(h.data() + o_stops, slot.stops.data(), s_used * sizeof(RsStop));
+    memset(h.data() + o_draw, 0xff, (size_t)L.n_draw_objects * 4u);
+    int rc;
+    if ((rc = compose_room(r, r->stop_tables, bytes))) return rc;
+    if ((rc = compose_room(r, r->stop_ramps, ((size_t)slot.n_ramps + n_grads) * 512u * 4u))) return rc;
+    cudaStream_t st = r->stream;
+    const char *t = (const char *)r->stop_tables.p;
+    CK(cudaMemcpyAsync(r->stop_tables.p, h.data(), bytes, cudaMemcpyHostToDevice, st));
+    if (slot.n_ramps) CK(cudaMemcpyAsync(r->stop_ramps.p, slot.ramps.p, (size_t)slot.n_ramps * 512u * 4u, cudaMemcpyDeviceToDevice, st));
+    CK(cudaStreamSynchronize(st)); // h is read by the copy
+    b.rs_grads = (const RsRamp *)(t + o_grads);
+    b.rs_stops = (const RsStop *)(t + o_stops);
+    b.rs_draw = (const uint32_t *)(t + o_draw);
+    b.rs_grads_n = n_grads;
+    b.rs_ramp0 = slot.n_ramps;
+    return VB_OK;
+}
+
+// Bound transforms (k_transforms.cu): each path's transform range, which damage tracking reads, by one k_path_point_slots over
+// the scene's path tags (the walk bound points use).
+static int transform_tables(vb_renderer *r, uint32_t, VbBound &b, std::string &) {
+    const VbLayout &L = r->cur->layout;
+    int rc;
+    if ((rc = compose_room(r, r->xform_ranges, (size_t)L.n_paths * 8u))) return rc;
+    cudaStream_t st = r->stream;
+    uint2 *range = (uint2 *)r->xform_ranges.p;
+    if (L.n_paths) CK(cudaMemsetAsync(range, 0xff, (size_t)L.n_paths * 8u, st));
+    vb_launch_path_point_slots((const uint32_t *)r->cur->scene.p + L.path_tag_base, L.path_data_base - L.path_tag_base, L.n_paths, nullptr,
+                               nullptr, range, st);
+    CK(cudaGetLastError());
+    b.xf_range = range;
+    return VB_OK;
+}
+
+// Bound visibility (k_visibility.cu): only the mask is sized, which every frame packs the caller's rows into, and which flatten
+// culls the hidden draw objects' tags by. The call does not synchronise unless the mask grows.
+static int visibility_mask(vb_renderer *r, uint32_t, VbBound &, std::string &) {
+    return compose_room(r, r->vis_mask, (size_t)vb_vis_words(r->cur->layout) * 4u);
+}
+static int no_tables(vb_renderer *, uint32_t, VbBound &, std::string &) { return VB_OK; }
+
+// The draw-data slot table of bound colours and bound gradient stops (k_colors.cu), made from b whenever either changes and
+// one of them stays bound: every word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col draw tags and one
+// k_gradient_slots for the bound gradients, whose draw objects it writes to rs_draw.
+static int draw_data_slots(vb_renderer *r, VbBound &b) {
+    b.col_slots = nullptr;
+    if (!draw_data_bound(b)) return VB_OK;
+    const Slot &slot = *r->cur;
     const VbLayout &L = slot.layout;
     const uint32_t n_dd = n_draw_data(L, slot.scene_words);
     int rc;
@@ -628,282 +739,115 @@ static int draw_data_slots(vb_renderer *r, uint32_t n_col, uint32_t n_grads, con
     uint32_t *slots = (uint32_t *)r->color_slots.p;
     if (n_dd) CK(cudaMemsetAsync(slots, 0xff, (size_t)n_dd * 4u, st));
     const uint32_t *tags = (const uint32_t *)slot.scene.p + L.draw_tag_base;
-    vb_launch_draw_color_slots(tags, n_col, slots, n_dd, st);
-    vb_launch_gradient_slots(tags, L.n_draw_objects, grad_dd, n_grads, slots, n_dd, draw_grad, st);
+    const bool stops = b.rows[VB_BIND_STOPS].rows != nullptr;
+    vb_launch_draw_color_slots(tags, b.rows[VB_BIND_COLORS].n, slots, n_dd, st);
+    vb_launch_gradient_slots(tags, L.n_draw_objects, stops ? (const uint32_t *)r->stop_tables.p : nullptr, b.rs_grads_n, slots, n_dd,
+                             const_cast<uint32_t *>(b.rs_draw), st);
     CK(cudaGetLastError());
+    b.col_slots = slots;
     return VB_OK;
 }
-// draw_data_slots for the bound gradients (none while unbound) and n_col colour rows
-static int draw_data_slots(vb_renderer *r, uint32_t n_col) {
-    const char *t = (const char *)r->stop_tables.p;
-    if (!r->stops.rows) return draw_data_slots(r, n_col, 0u, nullptr, nullptr);
-    return draw_data_slots(r, n_col, r->stops.n_grads, (const uint32_t *)(t + r->stops.o_dd), (uint32_t *)(t + r->stops.o_draw));
+
+// What differs between the kinds of binding, in VB_BIND_* order
+struct BindKind {
+    const char *fn;                                   // the entry point, which vb_last_error names
+    bool enabled_only;                                // refused with the exchange enabled only, not once it is configured
+    const char *(*scene)(const Slot &s);              // why the installed scene cannot be bound, or nullptr
+    uint64_t (*rows)(const Slot &s);                  // the rows it takes at most (`exact`: exactly)
+    bool exact;
+    const char *unit;                                 // what a row is, in the row-count error
+    uint32_t min_pitch;                               // bytes; 1: byte rows at any pitch and alignment
+    bool region;                                      // frames write a region past the scene for it (regions_of)
+    std::string (*check)(const vb_renderer *r, uint32_t n);
+    int (*tables)(vb_renderer *r, uint32_t n, VbBound &b, std::string &why);
+};
+static const BindKind BIND_KINDS[VB_N_BINDINGS] = {
+    {"vb_bind_instance_transforms", true, composed_scene, n_instances, true, " instances", 24u, true, freed_fragment, instance_tables},
+    {"vb_bind_draw_colors", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 16u, true, colors_check, no_tables},
+    {"vb_bind_path_points", false, any_scene, n_points, false, " points (1 .. n_points)", 8u, true, path_tags_outside, point_tables},
+    {"vb_bind_gradient_stops", false, scene_with_stops, n_stops, false, " gradient stops (1 .. n_stops)", 20u, true, stops_check, stop_tables},
+    {"vb_bind_transforms", false, any_scene, n_xforms, false, " transforms (1 .. n_transforms)", 24u, true, path_tags_outside, transform_tables},
+    {"vb_bind_draw_visibility", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 1u, false, no_check, visibility_mask},
+};
+
+// Unbind `kind` in b: its rows and the tables only it reads
+static void unbind(VbBound &b, int kind) {
+    b.rows[kind] = VbRows{};
+    if (kind == VB_BIND_INSTANCES) b.inst_prefix = b.inst_src = b.inst_draw = nullptr, b.inst_xf = nullptr;
+    if (kind == VB_BIND_POINTS) b.pt_first = nullptr;
+    if (kind == VB_BIND_STOPS) b.rs_grads = nullptr, b.rs_stops = nullptr, b.rs_draw = nullptr, b.rs_grads_n = b.rs_ramp0 = 0u;
+    if (kind == VB_BIND_TRANSFORMS) b.xf_range = nullptr;
 }
 
+// Bind n rows of `pitch` bytes from `ptr` as `kind` (null: unbind it), for every frame from now on
+static int bind_rows(vb_renderer *r, int kind, const void *ptr, uint32_t n, size_t pitch) {
+    if (!r) return VB_E_INVALID;
+    const BindKind &K = BIND_KINDS[kind];
+    auto bad = [&](const std::string &why) {
+        r->err = std::string(K.fn) + ": " + why;
+        return VB_E_INVALID;
+    };
+    if (r->grouped || r->xc.enabled || (!K.enabled_only && r->xc.configured))
+        return bad(K.enabled_only ? "not available for a renderer of a vb_group or with the exchange enabled"
+                                  : "not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    VbBound nb = r->bound;
+    const bool draw_data = kind == VB_BIND_COLORS || kind == VB_BIND_STOPS; // the draw-data slot table follows them
+    int rc;
+    if (!ptr) {
+        const bool was = nb.rows[kind].rows != nullptr;
+        unbind(nb, kind);
+        if (draw_data && was) {
+            CK(cudaSetDevice(r->device));
+            if ((rc = draw_data_slots(r, nb))) return rc;
+        }
+        r->bound = nb;
+        r->dmg.epoch++;
+        return VB_OK;
+    }
+    const Slot &slot = *r->cur;
+    if (const char *why = K.scene(slot)) return bad(why);
+    const uint64_t max = K.rows(slot);
+    if (n == 0u || (K.exact ? n != max : n > max))
+        return bad(std::to_string(n) + (K.exact ? " rows for a composed scene of " : " rows for a scene of ") + std::to_string(max) + K.unit);
+    if (K.min_pitch == 1u) {
+        if (pitch == 0u || pitch > 0xffffffffu) return bad("the row pitch must be at least 1 byte and below 4 GiB");
+    } else {
+        if ((uintptr_t)ptr & 3u) return bad("the pointer must be 4-byte aligned");
+        if ((pitch & 3u) || pitch < K.min_pitch || pitch > 0xfffffffcu)
+            return bad("the row pitch must be a multiple of 4 bytes, at least " + std::to_string(K.min_pitch) + " and below 4 GiB");
+    }
+    CK(cudaSetDevice(r->device));
+    if (!device_memory_of(r, ptr)) return bad("the rows must be memory of the renderer's device");
+    std::string why = K.check(r, n);
+    if (!why.empty()) return bad(why);
+    nb.rows[kind] = VbRows{(const uint8_t *)ptr, n, (uint32_t)pitch};
+    // a frame writes its regions past the scene (regions_of); both transform regions count, since a view can be set later
+    if (K.region && regions_of(slot.layout, slot.scene_words, true, true, draw_data_bound(nb), nb.rows[VB_BIND_POINTS].rows != nullptr).words >
+                        0xfffffff0ull)
+        return bad("the scene with the regions its frames write past it exceeds 32-bit word offsets");
+    if ((rc = K.tables(r, n, nb, why))) return why.empty() ? rc : bad(why);
+    if (draw_data && (rc = draw_data_slots(r, nb))) return rc;
+    r->bound = nb;
+    r->dmg.epoch++;
+    return VB_OK;
+}
+
+extern "C" int vb_bind_instance_transforms(vb_renderer *r, const float *device_transforms, uint32_t n, size_t row_pitch_bytes) {
+    return bind_rows(r, VB_BIND_INSTANCES, device_transforms, n, row_pitch_bytes);
+}
 extern "C" int vb_bind_draw_colors(vb_renderer *r, const float *device_rgba, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_draw_colors: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_rgba) {
-        // bound gradient stops keep the region: its colour slots go
-        if (r->colors.rows && r->stops.rows) {
-            CK(cudaSetDevice(r->device));
-            const int rc = draw_data_slots(r, 0u);
-            if (rc) return rc;
-        }
-        r->colors = vb_renderer::ColorBinding{};
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene) return bad("no scene installed");
-    const VbLayout &L = slot.layout;
-    if (n == 0u || n > L.n_draw_objects)
-        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(L.n_draw_objects) + " draw objects (1 .. n_draw_objects)");
-    if ((uintptr_t)device_rgba & 3u) return bad("the pointer must be 4-byte aligned");
-    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 16u || row_pitch_bytes > 0xfffffffcu)
-        return bad("the row pitch must be a multiple of 4 bytes, at least 16 and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_rgba)) return bad("the rows must be memory of the renderer's device");
-    // a frame writes the bound draw data past the scene, after the bound and viewed transforms, and bound points' path data
-    // after it (prepare, vb_frame.cu)
-    const uint32_t n_dd = n_draw_data(L, slot.scene_words);
-    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_dd + n_pd > 0xfffffff0ull)
-        return bad("the scene with its bound draw data and its bound and viewed transforms exceeds 32-bit word offsets");
-    if ((uint64_t)L.draw_tag_base + n > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
-    const int rc = draw_data_slots(r, n);
-    if (rc) return rc;
-    r->colors.rows = (const uint8_t *)device_rgba;
-    r->colors.n = n;
-    r->colors.pitch = (uint32_t)row_pitch_bytes;
-    r->dmg.epoch++;
-    return VB_OK;
+    return bind_rows(r, VB_BIND_COLORS, device_rgba, n, row_pitch_bytes);
 }
-
-// ---- bound path points: vb_bind_path_points (k_points.cu) -----------------------------------------------------------------------
-// The table of each path's first point is made once, here, on the renderer's stream by one k_path_point_slots over the scene's
-// path tags, and its 16-bit flag is read back (the call's one synchronisation). It stays valid while the rows are bound,
-// because every scene installation unbinds. Every frame after that reads the caller's rows in its k_path_points.
 extern "C" int vb_bind_path_points(vb_renderer *r, const float *device_xy, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_path_points: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_xy) {
-        r->points = vb_renderer::PointBinding{};
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene) return bad("no scene installed");
-    const VbLayout &L = slot.layout;
-    const uint32_t n_pd = n_path_data(L, slot.scene_words), n_points = n_pd / 2u;
-    if (n == 0u || n > n_points)
-        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_points) + " points (1 .. n_points)");
-    if ((uintptr_t)device_xy & 3u) return bad("the pointer must be 4-byte aligned");
-    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 8u || row_pitch_bytes > 0xfffffffcu)
-        return bad("the row pitch must be a multiple of 4 bytes, at least 8 and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_xy)) return bad("the rows must be memory of the renderer's device");
-    // a frame writes the bound path data past the scene, after the bound and viewed transforms and the bound draw data (prepare,
-    // vb_frame.cu)
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_draw_data(L, slot.scene_words) + n_pd > 0xfffffff0ull)
-        return bad("the scene with its bound path data, draw data and bound and viewed transforms exceeds 32-bit word offsets");
-    if (L.path_data_base < L.path_tag_base || L.path_data_base > slot.scene_words) return bad("the scene's path tags do not lie inside its words");
-    const uint32_t n_tag_words = L.path_data_base - L.path_tag_base;
-    int rc;
-    if ((rc = compose_room(r, r->point_slots, ((size_t)L.n_paths + 2u) * 4u))) return rc;
-    cudaStream_t st = r->stream;
-    uint32_t *first = (uint32_t *)r->point_slots.p, *flag = first + L.n_paths + 1u;
-    CK(cudaMemsetAsync(first, 0, ((size_t)L.n_paths + 2u) * 4u, st));
-    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, n_tag_words, L.n_paths, first, flag, nullptr, st);
-    CK(cudaGetLastError());
-    uint32_t i16 = 0u;
-    CK(cudaMemcpyAsync(&i16, flag, 4u, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (i16) return bad("the scene has 16-bit path segments, whose points are not f32 pairs");
-    r->points.rows = (const uint8_t *)device_xy;
-    r->points.n = n;
-    r->points.pitch = (uint32_t)row_pitch_bytes;
-    r->dmg.epoch++;
-    return VB_OK;
+    return bind_rows(r, VB_BIND_POINTS, device_xy, n, row_pitch_bytes);
 }
-
-// ---- bound gradient stops: vb_bind_gradient_stops (k_resolve.cu) ---------------------------------------------------------------
-// The bound gradients are the scene's first n_grads ramp patches: those with a stop below n (the stops are concatenated in patch
-// order). Made once, here, on the renderer's stream: the binding's tables (stop_tables), the scene's ramps copied into the
-// first rows of stop_ramps, and the draw-data slot table with the gradients' ramp words (draw_data_slots). The call's one
-// synchronisation waits for the tables' copy. They stay valid while the rows are bound, because every scene installation
-// unbinds. Every frame after that writes the gradients' rows from the caller's rows in its k_bound_ramps.
 extern "C" int vb_bind_gradient_stops(vb_renderer *r, const float *device_stops, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_gradient_stops: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_stops) {
-        const bool had = r->stops.rows != nullptr;
-        r->stops = vb_renderer::StopBinding{};
-        // bound colours keep the region: the gradients' slots go
-        if (had && r->colors.rows) {
-            CK(cudaSetDevice(r->device));
-            const int rc = draw_data_slots(r, r->colors.n);
-            if (rc) return rc;
-        }
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene) return bad("no scene installed");
-    if (!slot.have_stops)
-        return bad("the scene was installed as packed bytes, whose gradients exist only as resolved ramps; install it from its "
-                   "streams (vb_scene_upload_streams, vb_scene_upload_device, vb_render_scene) or with vb_compose");
-    const VbLayout &L = slot.layout;
-    const size_t n_stops = slot.stops.size();
-    if (n == 0u || n > n_stops)
-        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_stops) + " gradient stops (1 .. n_stops)");
-    if ((uintptr_t)device_stops & 3u) return bad("the pointer must be 4-byte aligned");
-    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 20u || row_pitch_bytes > 0xfffffffcu)
-        return bad("the row pitch must be a multiple of 4 bytes, at least 20 and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_stops)) return bad("the rows must be memory of the renderer's device");
-    uint32_t n_grads = 0u;
-    while (n_grads < slot.stop_patches.size() && slot.stop_patches[n_grads].first < n) n_grads++;
-    if ((uint64_t)slot.n_ramps + n_grads > (1ull << 30))
-        return bad("the scene's ramps and one per bound gradient pass the 30 bits of the ramp word");
-    // a frame writes the bound draw data past the scene, after the bound and viewed transforms, and bound points' path data
-    // after it (prepare, vb_frame.cu)
-    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_transforms(L, slot.scene_words) + n_draw_data(L, slot.scene_words) + n_pd > 0xfffffff0ull)
-        return bad("the scene with its bound draw data, path data and bound and viewed transforms exceeds 32-bit word offsets");
-    if ((uint64_t)L.draw_tag_base + L.n_draw_objects > slot.scene_words) return bad("the scene's draw tags do not lie inside its words");
-
-    // the tables: [gradients (RsRamp)] [their stops as encoded, at o_stops] [ramp words, at o_dd] [draw object -> gradient, at o_draw]
-    const vb_renderer::SceneSlot::StopPatch *last = n_grads ? &slot.stop_patches[n_grads - 1u] : nullptr;
-    const size_t s_used = last ? (size_t)last->first + last->n_stops : 0u;
-    vb_renderer::StopBinding nb;
-    nb.rows = (const uint8_t *)device_stops;
-    nb.n = n;
-    nb.pitch = (uint32_t)row_pitch_bytes;
-    nb.n_grads = n_grads;
-    nb.ramp0 = slot.n_ramps;
-    nb.o_stops = up16((size_t)n_grads * sizeof(RsRamp));
-    nb.o_dd = up16(nb.o_stops + s_used * sizeof(RsStop));
-    nb.o_draw = up16(nb.o_dd + (size_t)n_grads * 4u);
-    const size_t bytes = nb.o_draw + (size_t)L.n_draw_objects * 4u;
-    std::vector<uint8_t> h(bytes, 0u);
-    RsRamp *grads = (RsRamp *)h.data();
-    uint32_t *dd = (uint32_t *)(h.data() + nb.o_dd);
-    for (uint32_t g = 0; g < n_grads; g++) {
-        const vb_renderer::SceneSlot::StopPatch &p = slot.stop_patches[g];
-        grads[g] = RsRamp{p.first, p.n_stops, p.premul, 0u};
-        dd[g] = p.dd;
-    }
-    if (s_used) memcpy(h.data() + nb.o_stops, slot.stops.data(), s_used * sizeof(RsStop));
-    memset(h.data() + nb.o_draw, 0xff, (size_t)L.n_draw_objects * 4u);
-    int rc;
-    if ((rc = compose_room(r, r->stop_tables, bytes))) return rc;
-    if ((rc = compose_room(r, r->stop_ramps, ((size_t)slot.n_ramps + n_grads) * 512u * 4u))) return rc;
-    cudaStream_t st = r->stream;
-    CK(cudaMemcpyAsync(r->stop_tables.p, h.data(), bytes, cudaMemcpyHostToDevice, st));
-    if (slot.n_ramps) CK(cudaMemcpyAsync(r->stop_ramps.p, slot.ramps.p, (size_t)slot.n_ramps * 512u * 4u, cudaMemcpyDeviceToDevice, st));
-    r->stops = nb;
-    if ((rc = draw_data_slots(r, r->colors.rows ? r->colors.n : 0u))) return rc;
-    CK(cudaStreamSynchronize(st)); // h is read by the copy
-    r->dmg.epoch++;
-    return VB_OK;
+    return bind_rows(r, VB_BIND_STOPS, device_stops, n, row_pitch_bytes);
 }
-
-// ---- bound transforms: vb_bind_transforms (k_transforms.cu) ------------------------------------------------------------------
-// Each path's transform range, which damage tracking reads, is made once, here, on the renderer's stream by one
-// k_path_point_slots over the scene's path tags (the walk bound points use). It stays valid while the rows are bound, because
-// every scene installation unbinds. Every frame after that reads the caller's rows in its k_bound_transforms.
 extern "C" int vb_bind_transforms(vb_renderer *r, const float *device_affines, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_transforms: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_affines) {
-        r->xforms = vb_renderer::TransformBinding{};
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene) return bad("no scene installed");
-    const VbLayout &L = slot.layout;
-    const uint32_t n_tr = n_transforms(L, slot.scene_words);
-    if (n == 0u || n > n_tr)
-        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(n_tr) + " transforms (1 .. n_transforms)");
-    if ((uintptr_t)device_affines & 3u) return bad("the pointer must be 4-byte aligned");
-    if ((row_pitch_bytes & 3u) || row_pitch_bytes < 24u || row_pitch_bytes > 0xfffffffcu)
-        return bad("the row pitch must be a multiple of 4 bytes, at least 24 and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_affines)) return bad("the rows must be memory of the renderer's device");
-    // a frame writes the bound region and, under a view, the viewed one past the scene, and bound draw data and path data after
-    // them (prepare, vb_frame.cu)
-    const uint64_t n_dd = draw_data_bound(r) ? n_draw_data(L, slot.scene_words) : 0u;
-    const uint64_t n_pd = r->points.rows ? n_path_data(L, slot.scene_words) : 0u;
-    if ((uint64_t)slot.scene_words + 12u * (uint64_t)n_tr + n_dd + n_pd > 0xfffffff0ull)
-        return bad("the scene with its bound and viewed transforms, draw data and path data exceeds 32-bit word offsets");
-    if (L.path_data_base < L.path_tag_base || L.path_data_base > slot.scene_words) return bad("the scene's path tags do not lie inside its words");
-    int rc;
-    if ((rc = compose_room(r, r->xform_ranges, (size_t)L.n_paths * 8u))) return rc;
-    cudaStream_t st = r->stream;
-    uint2 *range = (uint2 *)r->xform_ranges.p;
-    if (L.n_paths) CK(cudaMemsetAsync(range, 0xff, (size_t)L.n_paths * 8u, st));
-    vb_launch_path_point_slots((const uint32_t *)slot.scene.p + L.path_tag_base, L.path_data_base - L.path_tag_base, L.n_paths, nullptr,
-                               nullptr, range, st);
-    CK(cudaGetLastError());
-    r->xforms.rows = (const uint8_t *)device_affines;
-    r->xforms.n = n;
-    r->xforms.pitch = (uint32_t)row_pitch_bytes;
-    r->dmg.epoch++;
-    return VB_OK;
+    return bind_rows(r, VB_BIND_TRANSFORMS, device_affines, n, row_pitch_bytes);
 }
-
-// ---- bound visibility: vb_bind_draw_visibility (k_visibility.cu) ----------------------------------------------------------------
-// The mask is sized here, once per binding; every frame after that packs the caller's rows into it in its k_draw_visibility, and
-// flatten culls the hidden draw objects' tags. Nothing else is made at bind time, and the call does not synchronise unless the
-// mask grows.
 extern "C" int vb_bind_draw_visibility(vb_renderer *r, const uint8_t *device_flags, uint32_t n, size_t row_pitch_bytes) {
-    if (!r) return VB_E_INVALID;
-    auto bad = [&](const std::string &why) {
-        r->err = "vb_bind_draw_visibility: " + why;
-        return VB_E_INVALID;
-    };
-    if (r->grouped || r->xc.configured || r->xc.enabled) return bad("not available for a renderer of a vb_group or with the exchange");
-    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
-    if (!device_flags) {
-        r->vis = vb_renderer::VisBinding{};
-        r->dmg.epoch++;
-        return VB_OK;
-    }
-    const vb_renderer::SceneSlot &slot = *r->cur;
-    if (!slot.have_scene) return bad("no scene installed");
-    const VbLayout &L = slot.layout;
-    if (n == 0u || n > L.n_draw_objects)
-        return bad(std::to_string(n) + " rows for a scene of " + std::to_string(L.n_draw_objects) + " draw objects (1 .. n_draw_objects)");
-    if (row_pitch_bytes == 0u || row_pitch_bytes > 0xffffffffu) return bad("the row pitch must be at least 1 byte and below 4 GiB");
-    CK(cudaSetDevice(r->device));
-    if (!device_memory_of(r, device_flags)) return bad("the rows must be memory of the renderer's device");
-    const int rc = compose_room(r, r->vis_mask, (size_t)vb_vis_words(L) * 4u);
-    if (rc) return rc;
-    r->vis.rows = device_flags;
-    r->vis.n = n;
-    r->vis.pitch = (uint32_t)row_pitch_bytes;
-    r->dmg.epoch++;
-    return VB_OK;
+    return bind_rows(r, VB_BIND_VISIBILITY, device_flags, n, row_pitch_bytes);
 }

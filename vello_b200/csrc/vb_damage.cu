@@ -39,27 +39,26 @@ int vb_host::damage_prepare(vb_renderer *r) {
     // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
     if (D.last.mode == VB_DMG_INCREMENTAL) D.have_last = false;
     const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles, n_draw = r->cur->layout.n_draw_objects;
-    const uint32_t n_xf = r->bound.rows || r->xforms.rows ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
-    const uint32_t n_col = r->colors.rows ? r->colors.n : 0u, n_pt = r->points.rows ? r->points.n : 0u;
-    const uint32_t n_grads = r->stops.rows ? r->stops.n_grads : 0u, n_vis = r->vis.rows ? vb_vis_words(r->cur->layout) : 0u;
-    const bool snap = any_binding(r), per_path = r->points.rows || r->vis.rows;
+    const VbRows *rows = r->bound.rows;
+    const bool xf = rows[VB_BIND_TRANSFORMS].rows != nullptr;
+    const uint32_t n_xf = rows[VB_BIND_INSTANCES].rows || xf ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
+    const uint32_t n_vis = rows[VB_BIND_VISIBILITY].rows ? vb_vis_words(r->cur->layout) : 0u;
+    const bool snap = any_binding(r->bound), per_path = rows[VB_BIND_POINTS].rows || rows[VB_BIND_VISIBILITY].rows;
     int rc;
     if ((rc = ensure(r, r->dmg_mask, n_tiles))) return rc;
     if ((rc = ensure(r, r->dmg_pending, n_tiles))) return rc;
-    if (snap && (rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw, n_col, n_pt, n_grads, n_vis) * 4u))) return rc;
-    if (r->bound.rows && (rc = ensure(r, r->dmg_changed, (size_t)r->bound.n * 4u))) return rc;
+    if (snap && (rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw, rows[VB_BIND_COLORS].n, rows[VB_BIND_POINTS].n,
+                                                                      r->bound.rs_grads_n, n_vis) * 4u))) return rc;
+    if (rows[VB_BIND_INSTANCES].rows && (rc = ensure(r, r->dmg_changed, (size_t)rows[VB_BIND_INSTANCES].n * 4u))) return rc;
     if (per_path && (rc = ensure(r, r->dmg_paths, (size_t)r->cur->layout.n_paths * 4u))) return rc;
-    if (r->xforms.rows && (rc = ensure(r, r->dmg_xf, (size_t)n_xf * 4u))) return rc;
+    if (xf && (rc = ensure(r, r->dmg_xf, (size_t)n_xf * 4u))) return rc;
     VbFrameBufs &b = r->bufs;
     b.dmg_mask = (uint8_t *)r->dmg_mask.p;
     b.dmg_pending = (uint8_t *)r->dmg_pending.p;
     if (snap) b.dmg_snap = (uint32_t *)r->dmg_snap.p;
     if (per_path) b.dmg_paths = (uint32_t *)r->dmg_paths.p;
-    if (r->xforms.rows) b.dmg_xf = (uint32_t *)r->dmg_xf.p;
-    if (r->bound.rows) {
-        b.dmg_changed = (uint32_t *)r->dmg_changed.p;
-        b.inst_draw = (const uint32_t *)((const char *)r->inst_tables.p + r->bound.o_draw);
-    }
+    if (xf) b.dmg_xf = (uint32_t *)r->dmg_xf.p;
+    if (rows[VB_BIND_INSTANCES].rows) b.dmg_changed = (uint32_t *)r->dmg_changed.p;
     b.dmg_mode = f.mode;
     b.dmg_n_xf = n_xf;
     if (incremental && diff) { // k_recompose_damage's inputs; an upload's tables are built by the frame (k_upload_diff.cu)
@@ -82,7 +81,7 @@ int vb_host::damage_prepare(vb_renderer *r) {
 bool vb_host::base_diffable(const vb_renderer *r) {
     const vb_renderer::Damage &D = r->dmg;
     const vb_renderer::SceneSlot &s = *r->cur;
-    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !any_binding(r) &&
+    return D.on && D.have_base && D.base.epoch == D.epoch && s.have_scene && !any_binding(r->bound) &&
            r->hit.valid && !r->hit.windowed && r->hit.cfg.n_cells == 1u && r->hit.cfg.layout.n_draw_objects == s.layout.n_draw_objects;
 }
 

@@ -397,49 +397,34 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.scene_words = (uint32_t)r->cur->scene_words;
     c.n_ramps = r->cur->n_ramps;
     // bound gradient stops: the frame reads the binding's ramps, the scene's and then one row per bound gradient
-    if (r->stops.rows) c.n_ramps = r->stops.ramp0 + r->stops.n_grads;
+    const VbBound &B = r->bound;
+    if (B.rows[VB_BIND_STOPS].rows) c.n_ramps = B.rs_ramp0 + B.rs_grads_n;
     c.atlas_w = r->cur->atlas_w;
     c.atlas_h = r->cur->atlas_h;
     c.out_pitch_px = p->width;
     c.out_row0 = c.win_ty0 * 16u;
-    const bool bound_xf = r->bound.rows || r->xforms.rows;
-    const uint32_t n_regions = (bound_xf ? 1u : 0u) + (r->view.on ? 1u : 0u);
-    if (bound_xf) {
-        // the frame reads its transforms past the scene's streams: [transform_base, scene_words) is the region
-        // k_instance_transforms writes from the caller's instance rows and k_bound_transforms from the bound rows, after it
-        c.layout.transform_base = c.scene_words;
-        c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
-    }
+    // The frame reads its transforms, draw data and path data from the regions past the scene's streams that it writes itself
+    // (regions_of): the bound transforms from the caller's instance rows and transform rows, the viewed transforms from the
+    // transforms before them (view_src; the region is empty for a layout whose transforms do not lie inside the uploaded words),
+    // the draw data from the scene's, the colour rows and the bound gradients' ramp rows, the path data from the scene's and
+    // the point rows. Reserving them can move the scene.
+    const bool bound_xf = B.rows[VB_BIND_INSTANCES].rows || B.rows[VB_BIND_TRANSFORMS].rows;
+    const Regions g = regions_of(r->cur->layout, r->cur->scene_words, bound_xf, r->view.on, draw_data_bound(B),
+                                 B.rows[VB_BIND_POINTS].rows != nullptr);
+    if (bound_xf) c.layout.transform_base = (uint32_t)g.base[REGION_BOUND_XF];
     if (r->view.on) {
-        // the frame reads the viewed transforms past the scene's streams (and the bound region): [transform_base, scene_words)
-        // is the region k_view_transforms writes, empty for a layout whose transforms do not lie inside the uploaded words
         c.view_src = c.layout.transform_base;
-        c.layout.transform_base = c.scene_words;
-        c.scene_words += 6u * n_transforms(r->cur->layout, r->cur->scene_words);
+        c.layout.transform_base = (uint32_t)g.base[REGION_VIEW];
         c.frame_cull = 1u;
     }
-    if (draw_data_bound(r)) {
-        // the frame reads its draw data past the scene's streams and the transform regions: [draw_data_base, scene_words) is
-        // the region k_draw_colors writes from the scene's draw data, the caller's colour rows and the bound gradients' ramp
-        // rows (bound path data follows it)
-        c.layout.draw_data_base = c.scene_words;
-        c.scene_words += n_draw_data(r->cur->layout, r->cur->scene_words);
-    }
-    if (r->points.rows) {
-        // the frame reads its path data past the scene's streams and the regions before: [path_data_base, scene_words) is the
-        // region k_path_points writes from the scene's path data and the caller's rows
-        c.layout.path_data_base = c.scene_words;
-        c.scene_words += n_path_data(r->cur->layout, r->cur->scene_words);
-    }
-    if (n_regions || draw_data_bound(r) || r->points.rows) {
-        int rc0 = reserve_transform_room(r, scene_bytes(r->cur->layout, r->cur->scene_words, n_regions, draw_data_bound(r),
-                                                        r->points.rows != nullptr));
-        if (rc0) return rc0;
-    }
+    if (draw_data_bound(B)) c.layout.draw_data_base = (uint32_t)g.base[REGION_DRAW_DATA];
+    if (B.rows[VB_BIND_POINTS].rows) c.layout.path_data_base = (uint32_t)g.base[REGION_PATH_DATA];
+    c.scene_words = (uint32_t)g.words;
+    if (int rc0 = reserve_transform_room(r, g.bytes)) return rc0; // nothing to do without regions: installations allocate as much
     c.n_cells = n_cells;
     c.tile_rows = c.height_in_tiles * n_cells;
     c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
-    c.vis = r->vis.rows ? (const uint32_t *)r->vis_mask.p : nullptr; // bound visibility: the mask k_draw_visibility writes
+    c.vis = B.rows[VB_BIND_VISIBILITY].rows ? (const uint32_t *)r->vis_mask.p : nullptr; // the mask k_draw_visibility writes
     r->params = *p;
 
     const uint32_t n_draw = c.layout.n_draw_objects, n_tiles = c.width_in_tiles * c.tile_rows;
@@ -491,55 +476,15 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     b.mask8 = (const uint32_t *)r->mask8.p;
     b.mask16 = (const uint32_t *)r->mask16.p;
     b.view = r->view.on ? (const float *)r->view_coef.p : nullptr;
-    if (r->bound.rows) {
-        const char *t = (const char *)r->inst_tables.p;
-        b.inst_rows = r->bound.rows;
-        b.inst_prefix = (const uint32_t *)t;
-        b.inst_xf = (const CmpXform *)(t + r->bound.o_xf);
-        b.inst_src = (const uint32_t *)(t + r->bound.o_src);
-        b.inst_n = r->bound.n;
-        b.inst_pitch = r->bound.pitch;
-    }
-    if (draw_data_bound(r)) {
-        b.col_slots = (const uint32_t *)r->color_slots.p;
-        b.col_src = b.scene + r->cur->layout.draw_data_base;
-    }
-    if (r->colors.rows) {
-        b.col_rows = r->colors.rows;
-        b.col_n = r->colors.n;
-        b.col_pitch = r->colors.pitch;
-    }
-    if (r->stops.rows) {
-        const char *t = (const char *)r->stop_tables.p;
-        b.ramps = (const uint32_t *)r->stop_ramps.p;
-        b.rs_rows = r->stops.rows;
-        b.rs_grads = (const RsRamp *)t;
-        b.rs_stops = (const RsStop *)(t + r->stops.o_stops);
-        b.rs_draw = (const uint32_t *)(t + r->stops.o_draw);
-        b.rs_n = r->stops.n;
-        b.rs_pitch = r->stops.pitch;
-        b.rs_grads_n = r->stops.n_grads;
-        b.rs_ramp0 = r->stops.ramp0;
-    }
-    if (r->points.rows) {
-        b.pt_rows = r->points.rows;
-        b.pt_first = (const uint32_t *)r->point_slots.p;
-        b.pt_n = r->points.n;
-        b.pt_pitch = r->points.pitch;
-        b.pt_src = b.scene + r->cur->layout.path_data_base;
-    }
-    if (r->xforms.rows) {
-        b.xf_rows = r->xforms.rows;
-        b.xf_range = (const uint2 *)r->xform_ranges.p;
-        b.xf_n = r->xforms.n;
-        b.xf_pitch = r->xforms.pitch;
-        b.xf_src = b.scene + r->cur->layout.transform_base;
-    }
-    if (r->vis.rows) {
-        b.vis_rows = r->vis.rows;
-        b.vis_n = r->vis.n;
-        b.vis_pitch = r->vis.pitch;
-    }
+    // the bindings, and what depends on where the scene lives now: the regions' sources and lengths, the bound gradients' ramps
+    b.bound = B;
+    if (draw_data_bound(B)) b.col_src = b.scene + r->cur->layout.draw_data_base;
+    if (B.rows[VB_BIND_POINTS].rows) b.pt_src = b.scene + r->cur->layout.path_data_base;
+    if (B.rows[VB_BIND_TRANSFORMS].rows) b.xf_src = b.scene + r->cur->layout.transform_base;
+    if (B.rows[VB_BIND_STOPS].rows) b.ramps = (const uint32_t *)r->stop_ramps.p;
+    b.xf_len = (uint32_t)(std::max(g.len[REGION_BOUND_XF], g.len[REGION_VIEW]) / 6u); // the two are as long when both are present
+    b.dd_len = (uint32_t)g.len[REGION_DRAW_DATA];
+    b.pd_len = (uint32_t)g.len[REGION_PATH_DATA];
     b.lb_pathtag = b.ctl + o_pathtag;
     b.lb_flatten = b.ctl + o_flatten;
     b.lb_draw = b.ctl + o_draw;
@@ -629,11 +574,11 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         case VB_STAGE_ID_FLATTEN: {
             // with the exchange on, this GPU flattens its share of the tag stream (no stripe culling: the lines are for
             // everybody), then the lines and path boxes are exchanged through peer memory (k_exchange.cu)
-            // a frame with bound instance transforms, bound transforms or a view first writes its transforms (read by flatten
-            // and draw), the bound ones first (instances, then rows: the view's source), a frame with bound colours or stops its draw data (read by draw, coarse
-            // and fine) and with bound stops its gradients' ramp rows (read by fine), and a frame with bound points its path
-            // data (read by flatten alone), and a frame with bound visibility its mask (read by flatten and damage tracking), inside
-            // flatten's stage events
+            // first, inside flatten's stage events, what the bindings (VbBound) and the view make of the scene: the regions past
+            // its streams in regions_of's order, the bound transforms before the viewed ones (their source; instances, then
+            // transform rows), the draw data (read by draw, coarse and fine) and the path data (read by flatten alone); the bound
+            // gradients' ramp rows (read by fine); and the visibility mask (read by flatten and damage tracking). Each launcher
+            // launches nothing while its binding is unbound.
             launches += vb_launch_instance_transforms(c, b, st);
             launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);

@@ -1,9 +1,9 @@
 // vb_renderer.h -- the renderer's host state (struct vb_renderer) and the helpers its host files share. Internal to the library.
 //
 // The host code is split by concern: vb_frame.cu (renderer lifetime, arenas, the frame path, views, hit testing), vb_upload.cu
-// (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, bound
-// instance transforms, draw colours, path points, gradient stops, transforms and visibility), vb_damage.cu (damage tracking), vb_debug.cu (debug
-// downloads and uploads) and vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
+// (scene uploads, the device resolve, image overrides and textures, cells), vb_compose.cu (fragments, compose, recompose, and the
+// bindings to device rows: VbBound, one bind path for every kind), vb_damage.cu (damage tracking), vb_debug.cu (debug downloads
+// and uploads) and vb_group.cu (vb_group, the exchange, CUDA IPC). Each helper declared at the end is defined in one of them. They live in
 // namespace vb_host, hidden from the shared library's symbol table, so that a host program's own functions of the same names
 // cannot interpose on them.
 #pragma once
@@ -315,59 +315,18 @@ struct vb_renderer {
     uint32_t next_image_key = 1;
     uint64_t compose_seq = 0;
     DevBuf compose_tmp;                  // compose's tables, staged through pinned[PIN_COMPOSE]
-    // bound instance transforms (vb_bind_instance_transforms) of the current scene: the caller's rows (nullptr: unbound), and
-    // the binding's tables in inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n), at
-    // o_xf] [the fragments' untransformed transforms, at o_src]. Every scene installation unbinds (set_scene).
-    // [the instances' draw prefix (n + 1), at o_draw]
-    struct Binding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0;
-        size_t o_xf = 0, o_src = 0, o_draw = 0;
-    } bound;
-    DevBuf inst_tables;
-    // bound draw colours (vb_bind_draw_colors) of the current scene: the caller's rows (nullptr: unbound), and in color_slots
-    // one word per draw-data word of the scene: the row whose converted colour replaces that word, or VB_COLOR_NONE (k_colors.cu).
-    // Every scene installation unbinds (set_scene).
-    struct ColorBinding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0;
-    } colors;
-    DevBuf color_slots;
-    // bound path points (vb_bind_path_points) of the current scene: the caller's rows (nullptr: unbound), and in point_slots the
-    // first point of each path (layout.n_paths + 1 words) and then the bind-time flag of a 16-bit segment (k_points.cu). Every
-    // scene installation unbinds (set_scene).
-    struct PointBinding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0;
-    } points;
-    DevBuf point_slots;
-    // bound gradient stops (vb_bind_gradient_stops) of the current scene: the caller's rows (nullptr: unbound). The first
-    // n_grads ramp patches are bound (those with a stop below n); gradient g reads ramp row ramp0 + g of stop_ramps, whose rows
-    // below ramp0 are a copy of the scene's ramps. stop_tables holds [the gradients as RsRamp (first stop, count, premul)]
-    // [their encoded stops, at o_stops] [each one's ramp word in the draw data, at o_dd] [per draw object its gradient or
-    // VB_COLOR_NONE, at o_draw] (k_resolve.cu). The draw-data slot table (color_slots) marks the gradients' ramp words. Every
-    // scene installation unbinds (set_scene).
-    struct StopBinding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0, n_grads = 0, ramp0 = 0;
-        size_t o_stops = 0, o_dd = 0, o_draw = 0;
-    } stops;
-    DevBuf stop_tables, stop_ramps;
-    // bound transforms (vb_bind_transforms) of the current scene: the caller's rows (nullptr: unbound), and in xform_ranges each
-    // path's transform range {t_lo, t_hi} (layout.n_paths uint2, k_points.cu) for damage tracking. Every scene installation
-    // unbinds (set_scene).
-    struct TransformBinding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0;
-    } xforms;
-    DevBuf xform_ranges;
-    // bound visibility (vb_bind_draw_visibility) of the current scene: the caller's rows (nullptr: unbound), and vis_mask, the
-    // bit mask (vb_vis_words) each frame packs them into (k_visibility.cu). Every scene installation unbinds (set_scene).
-    struct VisBinding {
-        const uint8_t *rows = nullptr;
-        uint32_t n = 0, pitch = 0;
-    } vis;
-    DevBuf vis_mask;
+    // What is bound to device rows (vb_bind_*, vb_compose.cu), with the device tables the bindings made at bind time (VbBound,
+    // vb_stages.h), which point into the buffers below. Every scene installation unbinds (set_scene).
+    //  - inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n)] [the fragments'
+    //    untransformed transforms] [the instances' draw prefix (n + 1)]
+    //  - color_slots: one word per draw-data word of the scene (VbBound::col_slots), while colours or stops are bound
+    //  - point_slots: the first point of each path (layout.n_paths + 1 words), then the bind-time flag of a 16-bit segment
+    //  - stop_tables: [each bound gradient's ramp word in the draw data] [the gradients (RsRamp)] [their encoded stops] [per
+    //    draw object its gradient or VB_COLOR_NONE]; stop_ramps: the scene's ramps, then a row per bound gradient (k_resolve.cu)
+    //  - xform_ranges: each path's transform range {t_lo, t_hi} (layout.n_paths uint2, k_points.cu)
+    //  - vis_mask: the bit mask (vb_vis_words) each frame packs the visibility rows into (k_visibility.cu)
+    VbBound bound{};
+    DevBuf inst_tables, color_slots, point_slots, stop_tables, stop_ramps, xform_ranges, vis_mask;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -492,19 +451,41 @@ inline uint32_t n_path_data(const VbLayout &L, size_t scene_words) {
     if (L.draw_tag_base < L.path_data_base || L.draw_tag_base > scene_words) return 0u;
     return L.draw_tag_base - L.path_data_base;
 }
-// Whether anything of the current scene is bound to device rows: instance transforms, draw colours, path points, gradient
-// stops, transforms or visibility. Such frames keep a damage snapshot, and are no base for an upload diff.
-inline bool any_binding(const vb_renderer *r) {
-    return r->bound.rows || r->colors.rows || r->points.rows || r->stops.rows || r->xforms.rows || r->vis.rows;
+// Whether anything of the current scene is bound to device rows (VbBound). Such frames keep a damage snapshot, and are no base
+// for an upload diff.
+inline bool any_binding(const VbBound &b) {
+    for (const VbRows &k : b.rows)
+        if (k.rows) return true;
+    return false;
 }
 // Whether frames read their draw data from the region past the scene's streams: with bound colours or bound gradient stops.
-inline bool draw_data_bound(const vb_renderer *r) { return r->colors.rows || r->stops.rows; }
-// A scene slot's allocation: the packed scene, then `regions` regions of transforms that frames write past it (bound instance
-// transforms, k_compose.cu, or bound transforms, k_transforms.cu, one region for either or both; viewed transforms, k_view.cu), with `colors` a region of draw data after them (bound draw colours,
-// k_colors.cu) and with `points` a region of path data after those (bound path points, k_points.cu), then slack.
-inline size_t scene_bytes(const VbLayout &L, size_t scene_words, uint32_t regions, bool colors = false, bool points = false) {
-    return (scene_words + regions * 6u * (size_t)n_transforms(L, scene_words) + (colors ? n_draw_data(L, scene_words) : 0u) +
-            (points ? n_path_data(L, scene_words) : 0u)) * 4u + 64u;
+inline bool draw_data_bound(const VbBound &b) { return b.rows[VB_BIND_COLORS].rows || b.rows[VB_BIND_STOPS].rows; }
+
+// The regions frames write past a scene's words, in this order, each present or not: the bound transforms (bound instance
+// transforms, k_compose.cu, and bound transforms, k_transforms.cu, share it), the viewed transforms (k_view.cu), the bound
+// draw data (bound colours or stops, k_colors.cu) and the bound path data (bound points, k_points.cu). This is the one place
+// that knows the order: prepare places a frame's regions with it, scene allocations are sized with it, and the bind calls
+// check 32-bit word offsets with it.
+enum { REGION_BOUND_XF, REGION_VIEW, REGION_DRAW_DATA, REGION_PATH_DATA, N_REGIONS };
+struct Regions {
+    uint64_t base[N_REGIONS]; // each region's first word
+    uint64_t len[N_REGIONS];  // its words, 0 when absent
+    uint64_t words;           // the scene's words and its present regions': the frame's scene_words
+    size_t bytes;             // the scene slot's allocation: those words, then slack
+};
+inline Regions regions_of(const VbLayout &L, size_t scene_words, bool bound_xf, bool view, bool draw_data, bool path_data) {
+    const uint64_t xf = 6u * (uint64_t)n_transforms(L, scene_words);
+    const uint64_t full[N_REGIONS] = {xf, xf, n_draw_data(L, scene_words), n_path_data(L, scene_words)};
+    const bool on[N_REGIONS] = {bound_xf, view, draw_data, path_data};
+    Regions g;
+    g.words = scene_words;
+    for (int i = 0; i < N_REGIONS; i++) {
+        g.base[i] = g.words;
+        g.len[i] = on[i] ? full[i] : 0u;
+        g.words += g.len[i];
+    }
+    g.bytes = g.words * 4u + 64u;
+    return g;
 }
 
 // vb_frame.cu

@@ -21,6 +21,39 @@ struct FlJob;
 struct CmpXform; // an instance's transform (k_compose.cu, below)
 struct VbUdiff;  // the upload diff's state (k_upload_diff.cu, below)
 
+// The bindings of a scene to device rows that every frame reads (vb_bind_*): instance transforms, draw colours, path points,
+// gradient stops, transforms and visibility. Binding k's rows are `n` rows `pitch` bytes apart from `rows`, null while unbound.
+enum { VB_BIND_INSTANCES, VB_BIND_COLORS, VB_BIND_POINTS, VB_BIND_STOPS, VB_BIND_TRANSFORMS, VB_BIND_VISIBILITY, VB_N_BINDINGS };
+struct VbRows {
+    const uint8_t *rows;
+    uint32_t n, pitch;
+};
+// What is bound, as the renderer keeps it and each frame reads it (VbFrameBufs::bound): the rows, and the tables each binding
+// made at bind time (vb_compose.cu), null or 0 while it is unbound.
+struct VbBound {
+    VbRows rows[VB_N_BINDINGS];
+    // instances (k_instance_transforms): the exclusive prefix of their transform counts (n + 1), their compose-time transforms
+    // (n), the fragments' untransformed transforms, and their draw prefix for damage tracking (n + 1: instance k draws draw
+    // objects inst_draw[k] .. inst_draw[k + 1])
+    const uint32_t *inst_prefix;
+    const CmpXform *inst_xf;
+    const uint32_t *inst_src, *inst_draw;
+    // colours or stops (k_draw_colors): per draw-data word of the scene, the colour row whose conversion replaces it,
+    // VB_GRAD_SLOT | g for bound gradient g's ramp word, or VB_COLOR_NONE; null while neither is bound
+    const uint32_t *col_slots;
+    // stops (k_bound_ramps): the bound gradients (rs_grads_n RsRamp records over the scene's stop indices), their encoded
+    // stops, and per draw object its bound gradient or VB_COLOR_NONE (k_damage). Gradient g's ramp row is ramps + (rs_ramp0 +
+    // g) * 512.
+    const RsRamp *rs_grads;
+    const RsStop *rs_stops;
+    const uint32_t *rs_draw;
+    // points (k_path_points): each path's first point (layout.n_paths + 1; k_damage maps changed points to paths with it)
+    const uint32_t *pt_first;
+    // transforms: the range of transforms each path reads (layout.n_paths {t_lo, t_hi}; k_damage)
+    const uint2 *xf_range;
+    uint32_t rs_grads_n, rs_ramp0;
+};
+
 // The device buffers a frame's launches read and write: the current scene slot's inputs, every intermediate and arena, and
 // the look-back regions of the control block with their partition counts. prepare() (vb_frame.cu) fills it once every buffer
 // has its size. It is part of the key of a captured frame (GraphKey), so it holds launch inputs only, and no padding.
@@ -30,42 +63,10 @@ struct VbFrameBufs {
     const uint8_t *atlas;
     const uint32_t *mask8, *mask16;
     const float *view; // the view's six f32 coefficients (vb_set_view), written in stream order; read by k_view_transforms
-    // bound instance transforms (vb_bind_instance_transforms), read by k_instance_transforms: the caller's rows (instance k's
-    // at inst_rows + k * inst_pitch bytes) and the binding's tables: the exclusive prefix of the instances' transform counts
-    // (inst_n + 1), their compose-time transforms (inst_n) and the fragments' untransformed transforms. Null while unbound.
-    const uint8_t *inst_rows;
-    const uint32_t *inst_prefix;
-    const CmpXform *inst_xf;
-    const uint32_t *inst_src;
-    // the bound draw-data region, written by k_draw_colors with bound colours (vb_bind_draw_colors) or bound gradient stops
-    // (vb_bind_gradient_stops): the caller's colour rows (draw object k's at col_rows + k * col_pitch bytes; null while colours
-    // are unbound), the slot table (per draw-data word of the scene: the colour row whose conversion replaces it, VB_GRAD_SLOT
-    // | g for bound gradient g's ramp word, or VB_COLOR_NONE) and the scene's own draw data, the region's source. col_slots and
-    // col_src are null while neither is bound.
-    const uint8_t *col_rows;
-    const uint32_t *col_slots, *col_src;
-    // bound gradient stops (vb_bind_gradient_stops), read by k_bound_ramps: the caller's rows (stop k's at rs_rows + k *
-    // rs_pitch bytes), the bound gradients (rs_grads_n RsRamp records over the scene's stop indices) with their encoded stops,
-    // and per draw object its bound gradient or VB_COLOR_NONE (k_damage). Gradient g's ramp row is ramps + (rs_ramp0 + g) *
-    // 512. Null while unbound.
-    const uint8_t *rs_rows;
-    const RsRamp *rs_grads;
-    const RsStop *rs_stops;
-    const uint32_t *rs_draw;
-    // bound path points (vb_bind_path_points), read by k_path_points: the caller's rows (point k's at pt_rows + k * pt_pitch
-    // bytes), the binding's table of each path's first point (layout.n_paths + 1; k_damage maps changed points to paths with
-    // it) and the scene's own path data, the region's source. Null while unbound.
-    const uint8_t *pt_rows;
-    const uint32_t *pt_first, *pt_src;
-    // bound transforms (vb_bind_transforms), read by k_bound_transforms: the caller's rows (entry k's at xf_rows + k * xf_pitch
-    // bytes), the binding's range of transforms each path reads (layout.n_paths: {t_lo, t_hi}; k_damage) and the scene's own
-    // transforms, the bound region's source without bound instance transforms. Null while unbound.
-    const uint8_t *xf_rows;
-    const uint2 *xf_range;
-    const uint32_t *xf_src;
-    // bound visibility (vb_bind_draw_visibility), read by k_draw_visibility into the mask at VbConfig::vis: the caller's rows
-    // (draw object k's byte at vis_rows + k * vis_pitch). Null while unbound.
-    const uint8_t *vis_rows;
+    // what is bound to device rows (VbBound), and the scene's own words the bound regions are made from: its draw data, path
+    // data and transforms (the bound transform region's source without bound instance transforms). Null while unbound.
+    VbBound bound;
+    const uint32_t *col_src, *pt_src, *xf_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -91,14 +92,11 @@ struct VbFrameBufs {
     uint32_t *ptcl, *blend_spill;
     // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
     // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
-    // of the frame's transform words, draw boxes, colour words of the col_n bound draw objects, words of the pt_n bound
-    // points, ramp rows of the bound gradients and the visibility mask), one changed flag per bound instance, with points or
-    // visibility bound one per path and with transforms bound one per
-    // transform, and the composed scene's draw prefix (inst_n + 1: instance k draws draw objects inst_draw[k] .. inst_draw[k +
-    // 1]; null while unbound)
+    // of the frame's transform words, draw boxes, colour words of the bound draw objects, words of the bound points, ramp rows
+    // of the bound gradients and the visibility mask), one changed flag per bound instance, with points or visibility bound one
+    // per path and with transforms bound one per transform
     uint8_t *dmg_mask, *dmg_pending;
     uint32_t *dmg_snap, *dmg_changed, *dmg_paths, *dmg_xf;
-    const uint32_t *inst_draw;
     // recompose damage (vb_recompose; k_recompose.cu), set only for the first frame after a recompose that tracking follows,
     // null otherwise: the base frame's draw boxes (rcmp_old_draws), and the tables [old draw prefix (rcmp_n_old + 1)] [new draw
     // prefix (rcmp_n_new + 1)] [new instance -> old instance, or VB_RCMP_NONE (rcmp_n_new)] [old instance unmatched (rcmp_n_old)]
@@ -113,13 +111,10 @@ struct VbFrameBufs {
     size_t ctl_words;
     uint32_t *lb_pathtag, *lb_flatten, *lb_draw, *lb_tile, *lb_clip, *lb_backdrop;
     uint32_t parts_pathtag, parts_flatten, parts_draw, parts_tile, parts_backdrop;
-    uint32_t inst_n, inst_pitch; // bound instances and their row pitch in bytes; 0 while unbound
-    uint32_t col_n, col_pitch; // bound colour rows and their pitch in bytes; 0 while unbound
-    uint32_t pt_n, pt_pitch;   // bound point rows and their pitch in bytes; 0 while unbound
-    uint32_t xf_n, xf_pitch;   // bound transform rows and their pitch in bytes; 0 while unbound
-    uint32_t rs_n, rs_pitch;   // bound stop rows and their pitch in bytes; 0 while unbound
-    uint32_t rs_grads_n, rs_ramp0; // bound gradients and the ramp row of the first; 0 while unbound
-    uint32_t vis_n, vis_pitch;     // bound visibility rows and their pitch in bytes; 0 while unbound
+    // the lengths of the regions prepare reserved past the scene's streams (regions_of, vb_renderer.h), 0 for an absent one:
+    // the transforms of each transform region (the bound one and the viewed one), the words of the bound draw data and of the
+    // bound path data. A launcher that writes a region writes this many and no more.
+    uint32_t xf_len, dd_len, pd_len, pad;
     // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
     // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
     uint32_t dmg_mode, dmg_n_xf;
@@ -130,19 +125,9 @@ struct VbFrameBufs {
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
 };
 
-// The regions prepare (vb_frame.cu) reserves past the scene's streams, in this order: the bound instance transforms, the viewed
-// transforms, the bound draw data, the bound path data, each present only with its binding or view. A region ends where the
-// next present one begins, the last at scene_words. Each launcher that writes one takes its length from here, never from
-// scene_words alone, so that it writes its own region and no later one.
-static inline uint32_t vb_transform_regions_end(const VbConfig &cfg, const VbFrameBufs &b) {
-    return b.col_slots ? cfg.layout.draw_data_base : b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
-}
 // The words of the visibility mask of a scene: one bit per draw object, and per path (path p is draw object p).
 static inline uint32_t vb_vis_words(const VbLayout &L) {
     return ((L.n_draw_objects > L.n_paths ? L.n_draw_objects : L.n_paths) + 31u) / 32u;
-}
-static inline uint32_t vb_draw_data_region_end(const VbConfig &cfg, const VbFrameBufs &b) {
-    return b.pt_rows ? cfg.layout.path_data_base : cfg.scene_words;
 }
 
 // k_exchange.cu: flatten sharded by tag range, lines and path boxes exchanged through peer memory

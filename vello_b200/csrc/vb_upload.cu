@@ -61,8 +61,8 @@ void vb_host::drop_registrations(vb_renderer *r) {
 }
 
 // Install the scene the current slot's buffers now hold, and drop what depended on the one before: a new scene is one cell
-// until vb_set_cells says otherwise, hit testing has no frame of it yet, and no instance transforms, draw colours, path points,
-// gradient stops or transforms are bound to it. Its stops are unknown until the installer that has them keeps them (keep_stops).
+// until vb_set_cells says otherwise, hit testing has no frame of it yet, and nothing is bound to it (VbBound). Its stops are
+// unknown until the installer that has them keeps them (keep_stops).
 void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, uint32_t n_ramps, uint32_t atlas_w, uint32_t atlas_h,
                       std::vector<vb_renderer::SceneSlot::OverridePlace> overridden, bool composed) {
     vb_renderer::SceneSlot &s = *r->cur;
@@ -83,12 +83,7 @@ void vb_host::set_scene(vb_renderer *r, const VbLayout &L, size_t scene_words, u
     s.stops.clear();
     s.have_scene = true;
     r->cells.clear();
-    r->bound = vb_renderer::Binding{};
-    r->colors = vb_renderer::ColorBinding{};
-    r->points = vb_renderer::PointBinding{};
-    r->stops = vb_renderer::StopBinding{};
-    r->xforms = vb_renderer::TransformBinding{};
-    r->vis = vb_renderer::VisBinding{};
+    r->bound = VbBound{};
     r->dmg.epoch++;
     // a diff begun for this installation (diff_begin) makes the next frame of this epoch incremental; any other ends it
     vb_renderer::Damage::Diff &X = r->dmg.diff;
@@ -129,7 +124,7 @@ static int upload_diff_begin(vb_renderer *r, cudaStream_t st, const VbLayout &L,
     if (!r->upload_diff || r->hit.bufs.scene != (const uint32_t *)s.scene.p || !base_diffable(r)) return VB_OK;
     const uint32_t n_old = s.layout.n_draw_objects, n_new = L.n_draw_objects;
     int rc;
-    if ((rc = ensure(r, r->spare_scene, scene_bytes(L, scene_words, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->spare_scene, regions_of(L, scene_words, false, r->view.on, false, false).bytes))) return rc;
     if ((rc = ensure(r, r->spare_ramps, (size_t)n_ramps * 512 * 4))) return rc;
     if ((rc = ensure(r, r->spare_atlas, (size_t)atlas_w * atlas_h * 4))) return rc;
     if ((rc = diff_begin(r, st, true, n_old, n_new, n_new))) return rc;
@@ -179,7 +174,7 @@ int vb_host::upload_on(vb_renderer *r, cudaStream_t st, const uint8_t *scene, si
     int rc;
     DiffedUpload guard;
     if (diff && (rc = upload_diff_begin(r, st, L, scene_len / 4, ramp_h, atlas_w, atlas_h, guard))) return rc;
-    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, scene_len / 4, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->cur->scene, regions_of(L, scene_len / 4, false, r->view.on, false, false).bytes))) return rc;
     if (scene_len) CK(cudaMemcpyAsync(r->cur->scene.p, scene, scene_len, cudaMemcpyHostToDevice, st));
     if ((rc = ensure(r, r->cur->ramps, (size_t)ramp_h * 512 * 4))) return rc;
     if (ramp_h) CK(cudaMemcpyAsync(r->cur->ramps.p, ramps, (size_t)ramp_h * 512 * 4, cudaMemcpyHostToDevice, st));
@@ -676,7 +671,7 @@ extern "C" int vb_scene_upload_streams(vb_renderer *r, const vb_encoding_streams
     if ((rc = upload_diff_begin(r, st, L, plan.words, (uint32_t)ramps.size(), plan.atlas_w, plan.atlas_h, guard))) return rc;
 
     // the six streams go straight to their places in the packed buffer
-    if ((rc = ensure(r, r->cur->scene, scene_bytes(L, plan.words, r->view.on)))) return rc;
+    if ((rc = ensure(r, r->cur->scene, regions_of(L, plan.words, false, r->view.on, false, false).bytes))) return rc;
     char *base = (char *)r->cur->scene.p;
     if (e->n_path_tags) CK(cudaMemcpyAsync(base, e->path_tags, e->n_path_tags, cudaMemcpyHostToDevice, st));
     if (e->n_path_data) CK(cudaMemcpyAsync(base + (size_t)L.path_data_base * 4, e->path_data, (size_t)e->n_path_data * 4, cudaMemcpyHostToDevice, st));

@@ -348,6 +348,10 @@ def _params_struct(p: RenderParams, bin_rows=(0, 0), tile_rows=(0, 0)) -> _Param
 class Renderer:
     """`vello::Renderer`: `Renderer(options)`, then `render_to_texture(scene, params)`."""
 
+    # the device arrays the bind_* methods hold while bound (_bind), None while unbound: of bind_instance_transforms,
+    # bind_draw_colors, bind_path_points, bind_gradient_stops, bind_transforms and bind_draw_visibility
+    _bound = _colors = _points = _stops = _xforms = _visibility = None
+
     def __init__(self, options: Optional[RendererOptions] = None):
         self.lib = load_library()
         options = options or RendererOptions()
@@ -363,12 +367,6 @@ class Renderer:
         self._owner = None
         self._device_images = {}  # key -> the device array an override of this renderer reads (kept alive while in use)
         self._fragment_pixels = {}  # id(pixel array) -> its contiguous copy while it lives: keys of upload_fragment's non-contiguous images
-        self._bound = None  # the device array of bind_instance_transforms
-        self._colors = None  # the device array of bind_draw_colors
-        self._points = None  # the device array of bind_path_points
-        self._stops = None  # the device array of bind_gradient_stops
-        self._xforms = None  # the device array of bind_transforms
-        self._visibility = None  # the device array of bind_draw_visibility
         self._destinations = {}  # key -> the device array a registered destination writes (kept alive while registered)
         self._background = None  # the device array of set_background
         self._background_shape = None  # (cells, H, W, 4-D) of a linear background: what _check_background compares frames with
@@ -387,12 +385,6 @@ class Renderer:
         r._destinations = {}
         r._background = None
         r._background_shape = None
-        r._bound = None
-        r._colors = None
-        r._points = None
-        r._stops = None
-        r._xforms = None
-        r._visibility = None
         r._frame_size = None
         r._cells = 1
         r._hit_extent = None
@@ -542,19 +534,21 @@ class Renderer:
                      L.draw_data_base, L.transform_base, L.style_base)
         return lay, [int(v) for v in offs]
 
+    def _bind(self, name, held, t, rows_of):
+        """The body of the bind_* methods: bind `t` with vb_<name>, from the (pointer, rows, row pitch) that rows_of(t) checks
+        and returns, or unbind for None; and hold `t` in the attribute `held` while it is bound."""
+        fn = "vb_" + name
+        ptr, n, pitch = (None, 0, 0) if t is None else rows_of(t)
+        self._check(getattr(self.lib, fn)(self.handle, ptr, n, pitch), fn)
+        setattr(self, held, t)
+
     def bind_instance_transforms(self, t):
         """Render instance k of the last `compose` under row k of the device array `t` in every frame from now on, read when
         the frame runs (`vb_bind_instance_transforms`): `t` is float32 (n, 6) [a b c d e f] rows, one per composed instance, with
         `__cuda_array_interface__` (e.g. a torch CUDA tensor, or columns of a larger one such as `state[:, 2:8]`). Write it on
         `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. A row that is not
         finite leaves its instance as composed. `t` is held while bound; None unbinds. A new scene (upload, compose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_instance_transforms(self.handle, None, 0, 0), "vb_bind_instance_transforms")
-            self._bound = None
-            return
-        ptr, n, pitch = _device_rows(t, "bind_instance_transforms", "transforms", 6)
-        self._check(self.lib.vb_bind_instance_transforms(self.handle, ptr, n, pitch), "vb_bind_instance_transforms")
-        self._bound = t
+        self._bind("bind_instance_transforms", "_bound", t, lambda t: _device_rows(t, "bind_instance_transforms", "transforms", 6))
 
     def bind_draw_colors(self, t):
         """Render draw object k of the installed scene, for every row k of the device array `t`, as if it had been encoded with
@@ -565,13 +559,7 @@ class Renderer:
         are ignored, and draw objects from n on keep their encoded colour, as does one whose row is not finite. Write it on
         `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. `t` is held
         while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_draw_colors(self.handle, None, 0, 0), "vb_bind_draw_colors")
-            self._colors = None
-            return
-        ptr, n, pitch = _device_rows(t, "bind_draw_colors", "colours", 4)
-        self._check(self.lib.vb_bind_draw_colors(self.handle, ptr, n, pitch), "vb_bind_draw_colors")
-        self._colors = t
+        self._bind("bind_draw_colors", "_colors", t, lambda t: _device_rows(t, "bind_draw_colors", "colours", 4))
 
     def bind_path_points(self, t):
         """Take point k of the installed scene's path data from row k of the device array `t` in every frame from now on, read
@@ -581,13 +569,7 @@ class Renderer:
         uploading the scene with those words overwritten would render; points from n on, and a point whose row is not finite,
         keep their encoded values. Write it on `self.stream` (or synchronise) before a frame, never while one runs; frames then
         need no further call. `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_path_points(self.handle, None, 0, 0), "vb_bind_path_points")
-            self._points = None
-            return
-        ptr, n, pitch = _device_rows(t, "bind_path_points", "points", 2)
-        self._check(self.lib.vb_bind_path_points(self.handle, ptr, n, pitch), "vb_bind_path_points")
-        self._points = t
+        self._bind("bind_path_points", "_points", t, lambda t: _device_rows(t, "bind_path_points", "points", 2))
 
     def bind_gradient_stops(self, t):
         """Take stop k of the installed scene's gradients from row k of the device array `t` in every frame from now on, read
@@ -599,13 +581,7 @@ class Renderer:
         stops (`upload_scene`, `NativeScene.upload_device`, `compose`), not as packed bytes. Write it on `self.stream` (or
         synchronise) before a frame, never while one runs; frames then need no further call. `t` is held while bound; None
         unbinds. A new scene (any upload, compose or recompose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_gradient_stops(self.handle, None, 0, 0), "vb_bind_gradient_stops")
-            self._stops = None
-            return
-        ptr, n, pitch = _device_rows(t, "bind_gradient_stops", "stops", 5)
-        self._check(self.lib.vb_bind_gradient_stops(self.handle, ptr, n, pitch), "vb_bind_gradient_stops")
-        self._stops = t
+        self._bind("bind_gradient_stops", "_stops", t, lambda t: _device_rows(t, "bind_gradient_stops", "stops", 5))
 
     def bind_transforms(self, t):
         """Take transform-stream entry k of the installed scene from row k of the device array `t` in every frame from now on,
@@ -618,13 +594,7 @@ class Renderer:
         and a view still apply (a view on top). Any installed scene can be bound, packed ones included. Write it on
         `self.stream` (or synchronise) before a frame, never while one runs; frames then need no further call. `t` is held
         while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_transforms(self.handle, None, 0, 0), "vb_bind_transforms")
-            self._xforms = None
-            return
-        ptr, n, pitch = _device_rows(t, "bind_transforms", "transforms", 6)
-        self._check(self.lib.vb_bind_transforms(self.handle, ptr, n, pitch), "vb_bind_transforms")
-        self._xforms = t
+        self._bind("bind_transforms", "_xforms", t, lambda t: _device_rows(t, "bind_transforms", "transforms", 6))
 
     def bind_draw_visibility(self, t):
         """Show draw object k of the installed scene only while byte k of the device array `t` is nonzero, in every frame from
@@ -642,13 +612,7 @@ class Renderer:
             r.bind_draw_visibility(mask_inst.repeat_interleave(counts))
 
         `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
-        if t is None:
-            self._check(self.lib.vb_bind_draw_visibility(self.handle, None, 0, 0), "vb_bind_draw_visibility")
-            self._visibility = None
-            return
-        ptr, n, pitch = _device_flags(t, "bind_draw_visibility")
-        self._check(self.lib.vb_bind_draw_visibility(self.handle, ptr, n, pitch), "vb_bind_draw_visibility")
-        self._visibility = t
+        self._bind("bind_draw_visibility", "_visibility", t, lambda t: _device_flags(t, "bind_draw_visibility"))
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
