@@ -567,9 +567,9 @@ extern "C" uint32_t vb_launch_coarse(const VbConfig &cfg, const VbFrameBufs &b, 
     if (cfg.n_cells > 1u) rows *= cfg.n_cells; // a batch has no window: every cell's bin rows, stacked
     if (width_in_bins == 0 || rows == 0) return 0;
     dim3 grid(width_in_bins * 2u, rows * 2u); // four quadrant CTAs per bin
-    if (b.dmg_mode == VB_DMG_INCREMENTAL)
+    if (b.dmg.mode == VB_DMG_INCREMENTAL)
         k_coarse<true><<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
-                                                    b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows, b.dmg_mask);
+                                                    b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows, b.dmg.mask);
     else
         k_coarse<false><<<grid, CO_THREADS, 0, st>>>(cfg, b.scene, b.draw_monoids, b.bin_headers, b.info_bin_data, b.paths, b.tiles, b.bump(), b.ptcl,
                                                      b.tile_start, b.cls_list, cfg.width_in_tiles * cfg.tile_rows, nullptr);

@@ -36,22 +36,13 @@
 #include "vb_stages.h"
 
 #define DM_THREADS 256u
-#define DM_HEADER_WORDS 4u // [generation, pad x3]
-#define DM_RECTS 64u       // caller rectangles per k_damage_rects launch
-
-// a slot: [the transform words (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw objects] [the
-// words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)] [the n_vis words of the
-// visibility mask]
-extern "C" size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads, uint32_t n_vis) {
-    return DM_HEADER_WORDS +
-           2u * (6u * (size_t)n_xf + 4u * (size_t)n_draw + n_col + 2u * (size_t)n_pt + 512u * (size_t)n_grads + n_vis);
-}
+#define DM_RECTS 64u // caller rectangles per k_damage_rects launch
 
 // the snapshot slot the last successful frame wrote (old) and the one this frame writes (nxt)
 __device__ __forceinline__ void dm_slots(uint32_t *snap, size_t slot_words, const uint32_t **old, uint32_t **nxt) {
     const uint32_t gen = *(volatile uint32_t *)snap;
-    *old = snap + DM_HEADER_WORDS + (gen & 1u) * slot_words;
-    *nxt = snap + DM_HEADER_WORDS + ((gen + 1u) & 1u) * slot_words;
+    *old = snap + VB_DMG_HEADER_WORDS + (gen & 1u) * slot_words;
+    *nxt = snap + VB_DMG_HEADER_WORDS + ((gen + 1u) & 1u) * slot_words;
 }
 
 // A full frame damages every tile; otherwise the frame starts from the caller's rectangles. No instance or path has changed yet.
@@ -63,48 +54,60 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
     if (i < n_paths) paths[i] = 0u;
 }
 
+// The inputs of k_damage_mark and k_damage: the snapshot `snap`, laid out by L (its flag arrays: L.changed, L.paths, L.xf), the
+// frame's mask, the words the frame reads and the bindings' tables (VbBound). The mask words `vis` are null without bound
+// visibility, `grad` (VbBound::rs_draw) without a bound gradient, and `xf_range` without bound transforms.
+struct DmArgs {
+    VbDmgLayout L;
+    uint32_t *snap;
+    uint8_t *mask;
+    const uint32_t *xf, *pd, *vis, *draw_tags, *dd; // transforms, path data, visibility mask, draw tags, draw data
+    const VbBbox4 *draw_bboxes;
+    const VbDrawMonoid *draw_monoids;
+    const uint32_t *inst_prefix, *inst_draw, *pt_first, *grad, *ramps; // ramps: the bound gradients' rows
+    const uint2 *xf_range;
+    uint32_t compare, wt, ht;
+};
+
 // One thread per transform u of the frame: its six words against the snapshot, and into the next slot. A difference marks
 // the instance holding u (the binding's prefix of the instances' transform counts). The same thread takes bound point u, when
-// there is one: its two words in the frame's path data (`pd`, the bound region), at `at_pt` of the slot (after the colour
-// words). A difference marks the path holding u (`first`, the binding's first point of each path). A non-finite row left the
-// encoded words in the region, so it is a change only if the words are. With bound transforms, xf_changed[u] records whether
-// transform u differs (a non-finite row that left an unchanged word does not). The same thread takes word u of the visibility
-// mask (`vis`, n_vis words, at `at_vis` of the slot), when there is one: each bit that differs marks its draw object, path d
-// being draw object d. The mask holds normalised bits, so a row going from 1 to 2 is no change.
-__global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__restrict__ xf, uint32_t *snap, size_t slot_words, uint32_t n_xf,
-                                                            uint32_t compare, const uint32_t *__restrict__ prefix, uint32_t n_inst, uint32_t *changed,
-                                                            const uint32_t *__restrict__ pd, size_t at_pt, uint32_t n_pt,
-                                                            const uint32_t *__restrict__ first, uint32_t n_paths, uint32_t *paths,
-                                                            uint32_t *xf_changed, const uint32_t *__restrict__ vis, size_t at_vis,
-                                                            uint32_t n_vis) {
+// there is one: its two words in the frame's path data (`pd`, the bound region). A difference marks the path holding u
+// (`pt_first`, the binding's first point of each path). A non-finite row left the encoded words in the region, so it is a
+// change only if the words are. With bound transforms, flag u records whether transform u differs (a non-finite row that left
+// an unchanged word does not). The same thread takes word u of the visibility mask, when there is one: each bit that differs
+// marks its draw object, path d being draw object d. The mask holds normalised bits, so a row going from 1 to 2 is no change.
+__global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const DmArgs a) {
+    const VbDmgLayout &L = a.L;
     const uint32_t u = blockIdx.x * DM_THREADS + threadIdx.x;
-    if (u >= n_xf && u >= n_pt && u >= n_vis) return;
+    const uint32_t n_paths = L.paths ? L.n_paths : 0u, n_pt = n_paths ? L.n_pt : 0u;
+    if (u >= L.n_xf && u >= n_pt && u >= L.n_vis) return;
     const uint32_t *old;
     uint32_t *nxt;
-    dm_slots(snap, slot_words, &old, &nxt);
-    if (u < n_xf) {
+    dm_slots(a.snap, L.slot_words, &old, &nxt);
+    uint32_t *changed = a.snap + L.changed, *paths = a.snap + L.paths, *xf_changed = a.snap + L.xf;
+    if (u < L.n_xf) {
         bool diff = false;
 #pragma unroll
         for (uint32_t i = 0; i < 6u; i++) {
-            const uint32_t w = __ldg(xf + 6u * u + i);
+            const uint32_t w = __ldg(a.xf + 6u * u + i);
             diff = diff || w != old[6u * u + i];
             nxt[6u * u + i] = w;
         }
-        if (compare && diff && n_inst) changed[cp_find(prefix, 0u, n_inst - 1u, u)] = 1u;
-        if (compare && xf_changed) xf_changed[u] = diff ? 1u : 0u;
+        if (a.compare && diff && L.n_inst) changed[cp_find(a.inst_prefix, 0u, L.n_inst - 1u, u)] = 1u;
+        if (a.compare && L.xf) xf_changed[u] = diff ? 1u : 0u;
     }
     if (u < n_pt) {
-        const uint32_t x = __ldg(pd + 2u * u), y = __ldg(pd + 2u * u + 1u);
-        const size_t o = at_pt + 2u * (size_t)u;
+        const uint32_t x = __ldg(a.pd + 2u * u), y = __ldg(a.pd + 2u * u + 1u);
+        const size_t o = L.pt + 2u * (size_t)u;
         const bool diff = x != old[o] || y != old[o + 1u];
         nxt[o] = x;
         nxt[o + 1u] = y;
-        if (compare && diff) paths[cp_find(first, 0u, n_paths - 1u, u)] = 1u;
+        if (a.compare && diff) paths[cp_find(a.pt_first, 0u, n_paths - 1u, u)] = 1u;
     }
-    if (u < n_vis) {
-        const uint32_t w = __ldg(vis + u);
-        uint32_t flips = compare ? w ^ old[at_vis + u] : 0u;
-        nxt[at_vis + u] = w;
+    if (u < L.n_vis) {
+        const uint32_t w = __ldg(a.vis + u);
+        uint32_t flips = a.compare ? w ^ old[L.vis + u] : 0u;
+        nxt[L.vis + u] = w;
         while (flips != 0u) {
             const uint32_t d = 32u * u + (uint32_t)(__ffs((int)flips) - 1);
             flips &= flips - 1u;
@@ -113,41 +116,34 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const uint32_t *__re
     }
 }
 
-// One warp per draw object: its box, below n_col its colour word and, for a bound gradient (`grad`: the draw object's gradient
-// g or VB_COLOR_NONE, non-null with stops bound), its ramp row (`rows` + 512 g, at `at_rg` + 512 g of the slot) into the next
-// slot; when its instance (n_inst > 0), its colour word, its ramp row or its path's points (`paths`, non-null with points
-// bound) or one of its path's transforms (`xf_range`, non-null with transforms bound: path d reads transforms xf_range[d].x ..
-// .y, each flagged in `xf_changed`) changed, its old and new boxes into the mask. A draw object whose paint is not one colour
-// has colour word 0: its bound row is never read. Its colour word is at its draw monoid's offset in the frame's draw data
-// (`dd`, the bound region).
-__global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict__ draw_bboxes, uint32_t n_draw, uint32_t *snap, size_t slot_words,
-                                                       uint32_t n_xf, uint32_t compare, const uint32_t *__restrict__ inst_draw, uint32_t n_inst,
-                                                       const uint32_t *__restrict__ changed, uint8_t *mask, uint32_t wt, uint32_t ht,
-                                                       const uint32_t *__restrict__ draw_tags, const uint32_t *__restrict__ dd,
-                                                       const VbDrawMonoid *__restrict__ draw_monoids, uint32_t n_col,
-                                                       const uint32_t *__restrict__ paths, uint32_t n_paths, const uint32_t *__restrict__ grad,
-                                                       const uint32_t *__restrict__ rows, size_t at_rg, const uint2 *__restrict__ xf_range,
-                                                       const uint32_t *__restrict__ xf_changed) {
+// One warp per draw object: its box, below L.n_col its colour word and, for a bound gradient (`grad`: the draw object's
+// gradient g or VB_COLOR_NONE), its ramp row (`ramps` + 512 g) into the next slot; when its instance (L.n_inst > 0), its colour
+// word, its ramp row or its path's points (flagged with points or visibility bound) or one of its path's transforms (path d
+// reads transforms xf_range[d].x .. .y, each flagged with transforms bound) changed, its old and new boxes into the mask. A draw
+// object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's
+// offset in the frame's draw data (`dd`, the bound region).
+__global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
+    const VbDmgLayout &L = a.L;
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
-    if (d >= n_draw) return;
+    if (d >= L.n_draw) return;
     const uint32_t *old;
     uint32_t *nxt;
-    dm_slots(snap, slot_words, &old, &nxt);
-    const VbBbox4 now = draw_bboxes[d];
-    const VbBbox4 was = reinterpret_cast<const VbBbox4 *>(old + 6u * (size_t)n_xf)[d];
+    dm_slots(a.snap, L.slot_words, &old, &nxt);
+    const VbBbox4 *box = a.draw_bboxes + d;
+    const VbBbox4 now = {__ldg(&box->x0), __ldg(&box->y0), __ldg(&box->x1), __ldg(&box->y1)};
+    const VbBbox4 was = reinterpret_cast<const VbBbox4 *>(old + L.box)[d];
     bool hit = false;
-    if (d < n_col) {
-        const uint32_t tag = __ldg(draw_tags + d);
+    if (d < L.n_col) {
+        const uint32_t tag = __ldg(a.draw_tags + d);
         const bool one_colour = tag == VB_DRAWTAG_FILL_COLOR || tag == VB_DRAWTAG_BLURRED_ROUNDED_RECT;
-        const uint32_t col = one_colour ? __ldg(dd + draw_monoids[d].scene_offset) : 0u;
-        const size_t at = 6u * (size_t)n_xf + 4u * (size_t)n_draw + d;
-        hit = col != old[at];
-        if (lane == 0u) nxt[at] = col;
+        const uint32_t col = one_colour ? __ldg(a.dd + __ldg(&a.draw_monoids[d].scene_offset)) : 0u;
+        hit = col != old[L.col + d];
+        if (lane == 0u) nxt[L.col + d] = col;
     }
-    const uint32_t g = grad ? __ldg(grad + d) : VB_COLOR_NONE;
+    const uint32_t g = a.grad ? __ldg(a.grad + d) : VB_COLOR_NONE;
     if (g != VB_COLOR_NONE) {
-        const uint32_t *row = rows + 512u * (size_t)g;
-        const size_t at = at_rg + 512u * (size_t)g;
+        const uint32_t *row = a.ramps + 512u * (size_t)g;
+        const size_t at = L.ramp + 512u * (size_t)g;
         bool diff = false;
         for (uint32_t i = lane; i < 512u; i += 32u) {
             const uint32_t w = __ldg(row + i);
@@ -157,23 +153,24 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const VbBbox4 *__restrict
         hit = __any_sync(0xffffffffu, diff) || hit;
     }
     __syncwarp();
-    if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + 6u * (size_t)n_xf)[d] = now;
-    if (!compare) return;
-    if (!hit && paths && d < n_paths) hit = paths[d] != 0u; // path d is draw object d
-    if (!hit && xf_range && d < n_paths && n_xf) {
-        const uint2 t = xf_range[d];
-        const uint64_t hi = t.y < n_xf ? t.y : n_xf - 1u;
+    if (lane == 0u) reinterpret_cast<VbBbox4 *>(nxt + L.box)[d] = now;
+    if (!a.compare) return;
+    const uint32_t *changed = a.snap + L.changed, *paths = a.snap + L.paths, *xf_changed = a.snap + L.xf;
+    if (!hit && L.paths && d < L.n_paths) hit = __ldg(paths + d) != 0u; // path d is draw object d
+    if (!hit && a.xf_range && d < L.n_paths && L.n_xf) {
+        const uint2 t = __ldg(a.xf_range + d);
+        const uint64_t hi = t.y < L.n_xf ? t.y : L.n_xf - 1u;
         bool any = false;
-        for (uint64_t i = (uint64_t)t.x + lane; i <= hi; i += 32u) any = any || xf_changed[i] != 0u;
+        for (uint64_t i = (uint64_t)t.x + lane; i <= hi; i += 32u) any = any || __ldg(xf_changed + i) != 0u;
         hit = __any_sync(0xffffffffu, any);
     }
     if (!hit) {
         // draw objects past the last instance (the END_CLIPs closing open clips) belong to no instance
-        if (n_inst == 0u || d >= __ldg(inst_draw + n_inst)) return;
-        if (changed[cp_find(inst_draw, 0u, n_inst - 1u, d)] == 0u) return;
+        if (L.n_inst == 0u || d >= __ldg(a.inst_draw + L.n_inst)) return;
+        if (__ldg(changed + cp_find(a.inst_draw, 0u, L.n_inst - 1u, d)) == 0u) return;
     }
-    dm_or_box(mask, was, wt, ht, lane);
-    dm_or_box(mask, now, wt, ht, lane);
+    dm_or_box(a.mask, was, a.wt, a.ht, lane);
+    dm_or_box(a.mask, now, a.wt, a.ht, lane);
 }
 
 // The frame's last kernel: a frame that succeeded becomes the base of the next one (its snapshot slot is current, the caller's
@@ -198,48 +195,42 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_rects(uint8_t *pending, D
 }
 
 extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (b.dmg_mode == VB_DMG_OFF) return 0u;
+    const VbDamage &D = b.dmg;
+    if (D.mode == VB_DMG_OFF) return 0u;
     const VbBound &B = b.bound;
-    const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, n_inst = B.rows[VB_BIND_INSTANCES].n;
-    const uint32_t n_col = B.rows[VB_BIND_COLORS].n, n_pt_rows = B.rows[VB_BIND_POINTS].n;
-    const bool xf_bound = B.rows[VB_BIND_TRANSFORMS].rows != nullptr;
-    const uint32_t n_draw = cfg.layout.n_draw_objects, full = b.dmg_mode == VB_DMG_FULL;
-    const uint32_t n_paths = b.dmg_paths ? cfg.layout.n_paths : 0u, n_vis = cfg.vis ? vb_vis_words(cfg.layout) : 0u;
-    const uint32_t n = std::max(std::max(n_tiles, n_inst), n_paths);
-    k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.dmg_mask, b.dmg_pending, n_tiles, full, b.dmg_changed, n_inst,
-                                                                              b.dmg_paths, n_paths);
+    const VbDmgLayout L = vb_dmg_layout(B, cfg.layout, D.n_xf);
+    const uint32_t wt = cfg.width_in_tiles, ht = cfg.height_in_tiles, n_tiles = wt * ht, full = D.mode == VB_DMG_FULL;
+    const uint32_t n_paths = L.paths ? L.n_paths : 0u, n = std::max(std::max(n_tiles, L.n_inst), n_paths);
+    k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(D.mask, D.pending, n_tiles, full, D.snap + L.changed, L.n_inst,
+                                                                              D.snap + L.paths, n_paths);
     // neither instance transforms, colours, points, stops, transforms nor visibility bound: nothing changes without a call that
     // makes the frame full
-    if (n_inst == 0u && n_col == 0u && n_pt_rows == 0u && B.rs_grads_n == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && n_vis == 0u) return 1u;
-    const size_t at_pt = 6u * (size_t)b.dmg_n_xf + 4u * (size_t)n_draw + n_col, at_rg = at_pt + 2u * (size_t)n_pt_rows;
-    const size_t at_vis = at_rg + 512u * (size_t)B.rs_grads_n, slot_words = at_vis + n_vis;
+    if (L.n_inst == 0u && L.n_col == 0u && L.n_pt == 0u && L.n_grads == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && L.n_vis == 0u) return 1u;
+    DmArgs a;
+    a.L = L, a.snap = D.snap, a.mask = D.mask, a.compare = !full, a.wt = wt, a.ht = ht;
+    a.xf = b.scene + cfg.layout.transform_base, a.pd = b.scene + cfg.layout.path_data_base, a.vis = cfg.vis;
+    a.draw_tags = b.scene + cfg.layout.draw_tag_base, a.dd = b.scene + cfg.layout.draw_data_base;
+    a.draw_bboxes = b.draw_bboxes, a.draw_monoids = b.draw_monoids, a.ramps = b.ramps + 512u * (size_t)B.rs_ramp0;
+    a.inst_prefix = B.inst_prefix, a.inst_draw = B.inst_draw, a.pt_first = B.pt_first, a.grad = L.n_grads ? B.rs_draw : nullptr;
+    a.xf_range = B.rows[VB_BIND_TRANSFORMS].rows ? B.xf_range : nullptr;
     uint32_t launches = 1u;
-    const uint32_t n_pt = n_paths ? n_pt_rows : 0u, n_mark = std::max(std::max(b.dmg_n_xf, n_pt), n_vis);
+    const uint32_t n_mark = std::max(std::max(L.n_xf, n_paths ? L.n_pt : 0u), L.n_vis);
     if (n_mark) {
-        k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.scene + cfg.layout.transform_base, b.dmg_snap, slot_words,
-                                                                                      b.dmg_n_xf, !full, B.inst_prefix, n_inst, b.dmg_changed,
-                                                                                      b.scene + cfg.layout.path_data_base, at_pt, n_pt, B.pt_first,
-                                                                                      n_paths, b.dmg_paths, xf_bound ? b.dmg_xf : nullptr,
-                                                                                      cfg.vis, at_vis, n_vis);
+        k_damage_mark<<<(n_mark + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(a);
         launches++;
     }
-    if (n_draw) {
+    if (L.n_draw) {
         const uint32_t per = DM_THREADS / 32u;
-        k_damage<<<(n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(b.draw_bboxes, n_draw, b.dmg_snap, slot_words, b.dmg_n_xf, !full, B.inst_draw,
-                                                                   n_inst, b.dmg_changed, b.dmg_mask, wt, ht, b.scene + cfg.layout.draw_tag_base,
-                                                                   b.scene + cfg.layout.draw_data_base, b.draw_monoids, n_col, b.dmg_paths,
-                                                                   cfg.layout.n_paths, B.rs_grads_n ? B.rs_draw : nullptr,
-                                                                   b.ramps + 512u * (size_t)B.rs_ramp0, at_rg, xf_bound ? B.xf_range : nullptr,
-                                                                   b.dmg_xf);
+        k_damage<<<(L.n_draw + per - 1u) / per, DM_THREADS, 0, st>>>(a);
         launches++;
     }
     return launches;
 }
 
 extern "C" uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (b.dmg_mode == VB_DMG_OFF) return 0u;
+    if (b.dmg.mode == VB_DMG_OFF) return 0u;
     const uint32_t n_tiles = cfg.width_in_tiles * cfg.height_in_tiles;
-    k_damage_commit<<<(n_tiles + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.bump(), b.dmg_snap, b.dmg_pending, n_tiles);
+    k_damage_commit<<<(n_tiles + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(b.bump(), b.dmg.snap, b.dmg.pending, n_tiles);
     return 1u;
 }
 

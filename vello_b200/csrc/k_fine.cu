@@ -1517,7 +1517,7 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     A.texel = o.texel;
     A.premul = o.premul;
     A.bg = bg;
-    const bool dmg = b.dmg_mode == VB_DMG_INCREMENTAL && cls_order; // the damaged tiles of coarse's lists only
+    const bool dmg = b.dmg.mode == VB_DMG_INCREMENTAL && cls_order; // the damaged tiles of coarse's lists only
     if (bg.on) {
         // always the FI_DST store (a plain pointer as linear RGBA8, straight alpha, bytes in place), never FI_DMG: a frame with a
         // background is full (damage_prepare)

@@ -20,24 +20,24 @@ __device__ __forceinline__ bool rc_same_box(const VbBbox4 a, const VbBbox4 b) {
            __float_as_uint(a.x1) == __float_as_uint(b.x1) && __float_as_uint(a.y1) == __float_as_uint(b.y1);
 }
 
-// One warp per draw object: the new composition's first, then the old one's. Tables as in VbFrameBufs::rcmp_tables.
+// One warp per draw object: the new composition's first, then the old one's. Tables as vb_rcmp_tables lays them out.
 __global__ void __launch_bounds__(RC_THREADS)
 k_recompose_damage(const VbBbox4 *__restrict__ now_boxes, const VbBbox4 *__restrict__ old_boxes, const uint32_t *__restrict__ tables,
                    uint32_t n_old, uint32_t n_new, uint32_t old_draws, uint32_t new_draws, uint8_t *mask, uint32_t wt, uint32_t ht) {
     const uint32_t w = blockIdx.x * (RC_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
-    const uint32_t *old_pre = tables, *new_pre = old_pre + n_old + 1u, *map = new_pre + n_new + 1u, *unmatched = map + n_new;
-    const uint32_t old_end = __ldg(old_pre + n_old), new_end = __ldg(new_pre + n_new); // the trailing END_CLIPs start here
+    const VbRcmpTables<const uint32_t> T = vb_rcmp_tables(tables, n_old, n_new);
+    const uint32_t old_end = __ldg(T.old_pre + n_old), new_end = __ldg(T.new_pre + n_new); // the trailing END_CLIPs start here
     if (w < new_draws) {
         const uint32_t d = w;
         const VbBbox4 now = now_boxes[d];
         uint32_t od;
         if (d < new_end) {
-            const uint32_t k = cp_find(new_pre, 0u, n_new - 1u, d), m = __ldg(map + k);
+            const uint32_t k = cp_find(T.new_pre, 0u, n_new - 1u, d), m = __ldg(T.map + k);
             if (m == VB_RCMP_NONE) {
                 dm_or_box(mask, now, wt, ht, lane);
                 return;
             }
-            od = __ldg(old_pre + m) + (d - __ldg(new_pre + k));
+            od = __ldg(T.old_pre + m) + (d - __ldg(T.new_pre + k));
         } else {
             const uint32_t t = new_draws - d; // 1 for the last END_CLIP
             if (t > old_draws - old_end) {
@@ -55,16 +55,16 @@ k_recompose_damage(const VbBbox4 *__restrict__ now_boxes, const VbBbox4 *__restr
     const uint32_t d = w - new_draws;
     if (d >= old_draws) return;
     // a matched old draw object is handled with its counterpart above
-    const bool gone = d < old_end ? __ldg(unmatched + cp_find(old_pre, 0u, n_old - 1u, d)) != 0u : old_draws - d > new_draws - new_end;
+    const bool gone = d < old_end ? __ldg(T.unmatched + cp_find(T.old_pre, 0u, n_old - 1u, d)) != 0u : old_draws - d > new_draws - new_end;
     if (gone) dm_or_box(mask, old_boxes[d], wt, ht, lane);
 }
 
 extern "C" uint32_t vb_launch_recompose_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.rcmp_tables) return 0u;
-    const uint32_t warps = b.rcmp_new_draws + b.rcmp_old_draws, per = RC_THREADS / 32u;
+    const VbDamage &D = b.dmg;
+    if (!D.tables) return 0u;
+    const uint32_t warps = D.new_draws + D.old_draws, per = RC_THREADS / 32u;
     if (warps == 0u) return 0u;
-    k_recompose_damage<<<(warps + per - 1u) / per, RC_THREADS, 0, st>>>(b.draw_bboxes, b.rcmp_old_boxes, b.rcmp_tables, b.rcmp_n_old, b.rcmp_n_new,
-                                                                        b.rcmp_old_draws, b.rcmp_new_draws, b.dmg_mask, cfg.width_in_tiles,
-                                                                        cfg.height_in_tiles);
+    k_recompose_damage<<<(warps + per - 1u) / per, RC_THREADS, 0, st>>>(b.draw_bboxes, D.old_boxes, D.tables, D.n_old, D.n_new, D.old_draws,
+                                                                        D.new_draws, D.mask, cfg.width_in_tiles, cfg.height_in_tiles);
     return 1u;
 }

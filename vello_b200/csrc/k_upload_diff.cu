@@ -170,7 +170,7 @@ k_upload_eq(VbUdiff *h, const VbUdRec *__restrict__ old_rec, const VbUdRec *__re
     if (!e) atomicMin(pos ? &h->prefix : &h->suffix, k);
 }
 
-// One thread per index up to max(n_old, n_new): k_recompose_damage's tables (VbFrameBufs::rcmp_tables).
+// One thread per index up to max(n_old, n_new): k_recompose_damage's tables (vb_rcmp_tables).
 __global__ void __launch_bounds__(UD_THREADS)
 k_upload_tables(const VbUdiff *h, const uint32_t *__restrict__ eq, uint32_t *tables, uint32_t n_old, uint32_t n_new) {
     const uint32_t t = blockIdx.x * UD_THREADS + threadIdx.x;
@@ -181,12 +181,12 @@ k_upload_tables(const VbUdiff *h, const uint32_t *__restrict__ eq, uint32_t *tab
         const uint32_t p = min(h->prefix, m);
         s = min(h->suffix, m - p);
     }
-    uint32_t *old_pre = tables, *new_pre = old_pre + n_old + 1u, *map = new_pre + n_new + 1u, *unmatched = map + n_new;
-    if (t <= n_old) old_pre[t] = t;
-    if (t <= n_new) new_pre[t] = t;
+    const VbRcmpTables<uint32_t> T = vb_rcmp_tables(tables, n_old, n_new);
+    if (t <= n_old) T.old_pre[t] = t;
+    if (t <= n_new) T.new_pre[t] = t;
     // the prefix lies inside [0, m - s) with eq set, so the middle's rule covers it
-    if (t < n_new) map[t] = t >= n_new - s ? t + n_old - n_new : t < m - s && eq[t] ? t : VB_RCMP_NONE;
-    if (t < n_old) unmatched[t] = t >= n_old - s || (t < m - s && eq[t]) ? 0u : 1u;
+    if (t < n_new) T.map[t] = t >= n_new - s ? t + n_old - n_new : t < m - s && eq[t] ? t : VB_RCMP_NONE;
+    if (t < n_old) T.unmatched[t] = t >= n_old - s || (t < m - s && eq[t]) ? 0u : 1u;
 }
 
 extern "C" uint32_t vb_launch_upload_records(const uint32_t *scene, uint32_t path_tag_base, uint32_t draw_tag_base, uint32_t n_tag_words,
@@ -199,21 +199,21 @@ extern "C" uint32_t vb_launch_upload_records(const uint32_t *scene, uint32_t pat
 }
 
 extern "C" uint32_t vb_launch_upload_diff(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
-    if (!b.udiff) return 0u;
-    const uint32_t n_old = b.rcmp_n_old, n_new = b.rcmp_n_new, m = n_old < n_new ? n_old : n_new;
+    if (!b.dmg.udiff) return 0u;
+    const uint32_t n_old = b.dmg.n_old, n_new = b.dmg.n_new, m = n_old < n_new ? n_old : n_new;
     const VbUdLayout U = vb_udiff_layout(n_old, n_new);
-    char *base = (char *)b.udiff;
+    char *base = (char *)b.dmg.udiff;
     const VbUdRec *old_rec = (const VbUdRec *)(base + U.old_rec);
     VbUdRec *new_rec = (VbUdRec *)(base + U.new_rec);
     uint32_t *eq = (uint32_t *)(base + U.eq), *tables = (uint32_t *)(base + U.tables);
     uint32_t launches = vb_launch_upload_records(b.scene, cfg.layout.path_tag_base, cfg.layout.draw_tag_base, cfg.n_tag_words, n_new, b.tag_monoids,
-                                                 b.draw_monoids, new_rec, &b.udiff->prefix, m, st);
+                                                 b.draw_monoids, new_rec, &b.dmg.udiff->prefix, m, st);
     const uint32_t pairs = n_old != n_new ? 2u * m : m, per = UD_THREADS / 32u;
     if (pairs) {
-        k_upload_eq<<<(pairs + per - 1u) / per, UD_THREADS, 0, st>>>(b.udiff, old_rec, new_rec, eq, n_old, n_new);
+        k_upload_eq<<<(pairs + per - 1u) / per, UD_THREADS, 0, st>>>(b.dmg.udiff, old_rec, new_rec, eq, n_old, n_new);
         launches++;
     }
     const uint32_t n = (n_old > n_new ? n_old : n_new) + 1u;
-    k_upload_tables<<<(n + UD_THREADS - 1u) / UD_THREADS, UD_THREADS, 0, st>>>(b.udiff, eq, tables, n_old, n_new);
+    k_upload_tables<<<(n + UD_THREADS - 1u) / UD_THREADS, UD_THREADS, 0, st>>>(b.dmg.udiff, eq, tables, n_old, n_new);
     return launches + 1u;
 }

@@ -454,8 +454,8 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     // the tables, staged through pinned memory: k_compose_streams' (cmp_tables), patches, ramp descriptors
     const size_t o_pat = cmp_tables(n).bytes;
     const size_t o_ramp = up16(o_pat + patches.size() * sizeof(RsPatch)), staged = o_ramp + ramps.size() * sizeof(RsRamp);
-    // vb_recompose's tables (VbFrameBufs::rcmp_tables), staged after compose's
-    const size_t o_rc = up16(staged), rc_bytes = arm ? ((size_t)n_old + 1u + n + 1u + n + n_old) * 4u : 0u, host_bytes = o_rc + rc_bytes;
+    // vb_recompose's tables (vb_rcmp_tables), staged after compose's
+    const size_t o_rc = up16(staged), rc_bytes = arm ? vb_rcmp_tables((uint32_t *)nullptr, n_old, n).words * 4u : 0u, host_bytes = o_rc + rc_bytes;
     if ((rc = compose_room(r, r->compose_tmp, staged))) return rc;
     char *tmp = (char *)r->compose_tmp.p;
     PinnedStage &stage = r->pinned[PIN_COMPOSE];
@@ -467,11 +467,11 @@ static int compose(vb_renderer *r, const char *fn, const vb_instance *inst, uint
     if (!ramps.empty()) memcpy(h + o_ramp, ramps.data(), ramps.size() * sizeof(RsRamp));
     if (draw_offsets) memcpy(draw_offsets, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
     if (arm) {
-        uint32_t *t = (uint32_t *)(h + o_rc);
-        memcpy(t, was.inst_draw.data(), ((size_t)n_old + 1u) * 4u);
-        memcpy(t + n_old + 1u, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
-        if (n) memcpy(t + n_old + 1u + n + 1u, match.data(), (size_t)n * 4u);
-        if (n_old) memcpy(t + n_old + 1u + n + 1u + n, unmatched.data(), (size_t)n_old * 4u);
+        const VbRcmpTables<uint32_t> t = vb_rcmp_tables((uint32_t *)(h + o_rc), n_old, n);
+        memcpy(t.old_pre, was.inst_draw.data(), ((size_t)n_old + 1u) * 4u);
+        memcpy(t.new_pre, pre + (size_t)CMP_DRAW_TAGS * (n + 1u), ((size_t)n + 1u) * 4u);
+        if (n) memcpy(t.map, match.data(), (size_t)n * 4u);
+        if (n_old) memcpy(t.unmatched, unmatched.data(), (size_t)n_old * 4u);
     }
 
     if ((rc = compose_room(r, slot.scene, regions_of(L, total_words, false, r->view.on, false, false).bytes))) return rc;

@@ -10,8 +10,10 @@
 // After prepare, pick_out and resolve_background: is the frame incremental, full, or outside damage tracking (a batch, a window,
 // a background, the exchange: mode VB_DMG_OFF, and no base for the next frame)? A background frame is full because nothing tells
 // which of the background's pixels changed since the base frame. The decision is the same for every re-run of the frame, because the base
-// and the forcing flags change only when a frame succeeds (damage_succeeded). Allocates the mask, the staged rectangles and
-// the snapshot; their sizes follow from the frame size and the scene, so they never move under an incremental frame.
+// and the forcing flags change only when a frame succeeds (damage_succeeded). Allocates the mask, the staged rectangles and,
+// while anything is bound, the snapshot with its flags (vb_dmg_layout). The mask's size follows from the frame size, which an
+// incremental frame shares with its base; the snapshot's from the scene and what is bound, which change only through an
+// installation or a binding. Both advance the epoch and so make the next frame full: no buffer moves under an incremental frame.
 int vb_host::damage_prepare(vb_renderer *r) {
     vb_renderer::Damage &D = r->dmg;
     const VbConfig &c = r->cfg;
@@ -38,38 +40,29 @@ int vb_host::damage_prepare(vb_renderer *r) {
     // this frame rewrites the mask: the last successful frame's can be reported again only if this one succeeds (a frame that
     // fails for good, or a streamed one, which the host does not follow frame by frame, leaves nothing to report)
     if (D.last.mode == VB_DMG_INCREMENTAL) D.have_last = false;
-    const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles, n_draw = r->cur->layout.n_draw_objects;
+    const uint32_t n_tiles = c.width_in_tiles * c.height_in_tiles;
     const VbRows *rows = r->bound.rows;
-    const bool xf = rows[VB_BIND_TRANSFORMS].rows != nullptr;
-    const uint32_t n_xf = rows[VB_BIND_INSTANCES].rows || xf ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
-    const uint32_t n_vis = rows[VB_BIND_VISIBILITY].rows ? vb_vis_words(r->cur->layout) : 0u;
-    const bool snap = any_binding(r->bound), per_path = rows[VB_BIND_POINTS].rows || rows[VB_BIND_VISIBILITY].rows;
+    const uint32_t n_xf = rows[VB_BIND_INSTANCES].rows || rows[VB_BIND_TRANSFORMS].rows ? n_transforms(r->cur->layout, r->cur->scene_words) : 0u;
+    const bool snap = any_binding(r->bound);
     int rc;
     if ((rc = ensure(r, r->dmg_mask, n_tiles))) return rc;
     if ((rc = ensure(r, r->dmg_pending, n_tiles))) return rc;
-    if (snap && (rc = ensure(r, r->dmg_snap, vb_damage_snap_words(n_xf, n_draw, rows[VB_BIND_COLORS].n, rows[VB_BIND_POINTS].n,
-                                                                      r->bound.rs_grads_n, n_vis) * 4u))) return rc;
-    if (rows[VB_BIND_INSTANCES].rows && (rc = ensure(r, r->dmg_changed, (size_t)rows[VB_BIND_INSTANCES].n * 4u))) return rc;
-    if (per_path && (rc = ensure(r, r->dmg_paths, (size_t)r->cur->layout.n_paths * 4u))) return rc;
-    if (xf && (rc = ensure(r, r->dmg_xf, (size_t)n_xf * 4u))) return rc;
-    VbFrameBufs &b = r->bufs;
-    b.dmg_mask = (uint8_t *)r->dmg_mask.p;
-    b.dmg_pending = (uint8_t *)r->dmg_pending.p;
-    if (snap) b.dmg_snap = (uint32_t *)r->dmg_snap.p;
-    if (per_path) b.dmg_paths = (uint32_t *)r->dmg_paths.p;
-    if (xf) b.dmg_xf = (uint32_t *)r->dmg_xf.p;
-    if (rows[VB_BIND_INSTANCES].rows) b.dmg_changed = (uint32_t *)r->dmg_changed.p;
-    b.dmg_mode = f.mode;
-    b.dmg_n_xf = n_xf;
+    if (snap && (rc = ensure(r, r->dmg_snap, vb_dmg_layout(r->bound, r->cur->layout, n_xf).bytes))) return rc;
+    VbDamage &dm = r->bufs.dmg;
+    dm.mask = (uint8_t *)r->dmg_mask.p;
+    dm.pending = (uint8_t *)r->dmg_pending.p;
+    if (snap) dm.snap = (uint32_t *)r->dmg_snap.p;
+    dm.mode = f.mode;
+    dm.n_xf = n_xf;
     if (incremental && diff) { // k_recompose_damage's inputs; an upload's tables are built by the frame (k_upload_diff.cu)
         const char *p = (const char *)r->dmg_diff.p;
-        if (X.upload) b.udiff = (VbUdiff *)r->dmg_diff.p;
-        b.rcmp_old_boxes = (const VbBbox4 *)(p + X.o_boxes);
-        b.rcmp_tables = (const uint32_t *)(p + X.o_tables);
-        b.rcmp_n_old = X.n_old;
-        b.rcmp_n_new = X.n_new;
-        b.rcmp_old_draws = X.old_draws;
-        b.rcmp_new_draws = X.new_draws;
+        if (X.upload) dm.udiff = (VbUdiff *)r->dmg_diff.p;
+        dm.old_boxes = (const VbBbox4 *)(p + X.o_boxes);
+        dm.tables = (const uint32_t *)(p + X.o_tables);
+        dm.n_old = X.n_old;
+        dm.n_new = X.n_new;
+        dm.old_draws = X.old_draws;
+        dm.new_draws = X.new_draws;
     }
     D.frame = f;
     return VB_OK;
@@ -92,7 +85,7 @@ int vb_host::diff_begin(vb_renderer *r, cudaStream_t st, bool upload, uint32_t n
     const size_t box_bytes = (size_t)old_draws * sizeof(VbBbox4);
     const VbUdLayout U = vb_udiff_layout(n_old, n_new);
     const size_t o_boxes = upload ? U.boxes : 0u, o_tables = upload ? U.tables : (box_bytes + 15u) & ~(size_t)15u;
-    const size_t bytes = o_tables + ((size_t)n_old + 1u + n_new + 1u + n_new + n_old) * 4u; // k_recompose_damage's tables
+    const size_t bytes = o_tables + vb_rcmp_tables((uint32_t *)nullptr, n_old, n_new).words * 4u;
     if (r->dmg_diff.cap < bytes) CK(cudaStreamSynchronize(st)); // growing: copies enqueued into it may not have run yet
     int rc;
     if ((rc = ensure(r, r->dmg_diff, bytes))) return rc;

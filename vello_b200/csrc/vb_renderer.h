@@ -358,8 +358,8 @@ struct vb_renderer {
             size_t o_boxes = 0, o_tables = 0;
         } diff;
     } dmg;
-    DevBuf dmg_mask, dmg_pending, dmg_snap, dmg_changed, dmg_paths, dmg_xf;
-    DevBuf dmg_diff; // the diff's buffer: [the base frame's draw boxes, at o_boxes] [the tables, at o_tables] (VbFrameBufs::rcmp_*)
+    DevBuf dmg_mask, dmg_pending, dmg_snap; // VbDamage::mask, pending and snap
+    DevBuf dmg_diff; // the diff's buffer: [the base frame's draw boxes, at o_boxes] [the tables, at o_tables] (VbDamage)
     // upload diff (vb_set_upload_diff): the switch; and the spare scene, ramps and atlas buffers an upload that tracking follows
     // writes, while the current slot's (the base frame's scene) are kept and swapped into the spare set. The diff's buffer is laid
     // out by vb_udiff_layout, behind a head (VbUdiff) written from ud_head.
@@ -384,7 +384,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
                            &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
                            &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask,
-                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_changed, &r->dmg_paths, &r->dmg_xf, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
+                           &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
 }

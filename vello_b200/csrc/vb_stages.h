@@ -54,6 +54,28 @@ struct VbBound {
     uint32_t rs_grads_n, rs_ramp0;
 };
 
+// Damage tracking's state of a frame (vb_set_damage_tracking; k_damage.cu), filled by damage_prepare (vb_damage.cu) and all
+// zero while tracking is off.
+struct VbDamage {
+    // the frame's damage (one byte per tile), the caller's rectangles staged for the next frame (vb_add_damage), and while
+    // anything is bound the snapshot (vb_dmg_layout)
+    uint8_t *mask, *pending;
+    uint32_t *snap;
+    // set only for the first frame after a diff that tracking follows, null otherwise: a recompose's (vb_recompose;
+    // k_recompose.cu) or an upload's (vb_set_upload_diff; k_upload_diff.cu). The base frame's draw boxes and k_recompose_damage's
+    // tables (vb_rcmp_tables); for an upload also the diff's buffer (VbUdiff, then vb_udiff_layout), whose tables describe one
+    // draw object per "instance".
+    const VbBbox4 *old_boxes;
+    const uint32_t *tables;
+    VbUdiff *udiff;
+    // VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and fine only for damaged
+    // tiles); the transforms the frame reads (at layout.transform_base)
+    uint32_t mode, n_xf;
+    // the diff's old and new instances and draw objects (the END_CLIPs after the last instance included)
+    uint32_t n_old, n_new, old_draws, new_draws;
+};
+static_assert(sizeof(VbDamage) == 6 * sizeof(void *) + 6 * sizeof(uint32_t), "VbDamage has no padding (GraphKey is compared bytewise)");
+
 // The device buffers a frame's launches read and write: the current scene slot's inputs, every intermediate and arena, and
 // the look-back regions of the control block with their partition counts. prepare() (vb_frame.cu) fills it once every buffer
 // has its size. It is part of the key of a captured frame (GraphKey), so it holds launch inputs only, and no padding.
@@ -90,22 +112,7 @@ struct VbFrameBufs {
     VbSegmentCount *seg_counts;
     VbSegment *segments;
     uint32_t *ptcl, *blend_spill;
-    // damage tracking (vb_set_damage_tracking; k_damage.cu), all null while it is off: the frame's damage (one byte per tile),
-    // the caller's rectangles staged for the next frame (vb_add_damage), the snapshot ([generation word, 3 pad] then two slots
-    // of the frame's transform words, draw boxes, colour words of the bound draw objects, words of the bound points, ramp rows
-    // of the bound gradients and the visibility mask), one changed flag per bound instance, with points or visibility bound one
-    // per path and with transforms bound one per transform
-    uint8_t *dmg_mask, *dmg_pending;
-    uint32_t *dmg_snap, *dmg_changed, *dmg_paths, *dmg_xf;
-    // recompose damage (vb_recompose; k_recompose.cu), set only for the first frame after a recompose that tracking follows,
-    // null otherwise: the base frame's draw boxes (rcmp_old_draws), and the tables [old draw prefix (rcmp_n_old + 1)] [new draw
-    // prefix (rcmp_n_new + 1)] [new instance -> old instance, or VB_RCMP_NONE (rcmp_n_new)] [old instance unmatched (rcmp_n_old)]
-    const VbBbox4 *rcmp_old_boxes;
-    const uint32_t *rcmp_tables;
-    // upload diff (vb_set_upload_diff; k_upload_diff.cu), set only for the first frame after an upload that tracking follows,
-    // null otherwise: the diff's buffer (VbUdiff, then vb_udiff_layout). The rcmp_* fields then point into it and describe one
-    // draw object per "instance", so that k_recompose_damage computes the damage.
-    VbUdiff *udiff;
+    VbDamage dmg;
     // control block: [VbBump, header words (vb_types.h)] [look-back states], zeroed at the start of every frame
     uint32_t *ctl;
     size_t ctl_words;
@@ -115,11 +122,6 @@ struct VbFrameBufs {
     // the transforms of each transform region (the bound one and the viewed one), the words of the bound draw data and of the
     // bound path data. A launcher that writes a region writes this many and no more.
     uint32_t xf_len, dd_len, pd_len, pad;
-    // damage tracking: VB_DMG_OFF, VB_DMG_FULL (render everything, record the snapshot) or VB_DMG_INCREMENTAL (coarse and
-    // fine only for damaged tiles); the transforms the frame reads (at layout.transform_base)
-    uint32_t dmg_mode, dmg_n_xf;
-    // recompose damage: the old and new compositions' instances and draw objects (the END_CLIPs after the last instance included)
-    uint32_t rcmp_n_old, rcmp_n_new, rcmp_old_draws, rcmp_new_draws;
     int sm_count; // the grids of the persistent and grid-stride kernels are sized from it
 
     VbBump *bump() const { return reinterpret_cast<VbBump *>(ctl); }
@@ -282,12 +284,60 @@ uint32_t vb_launch_draw_visibility(const VbConfig &cfg, const VbFrameBufs &b, cu
 uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_commit(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const uint32_t *tile_rects, uint32_t n, cudaStream_t st);
-size_t vb_damage_snap_words(uint32_t n_xf, uint32_t n_draw, uint32_t n_col, uint32_t n_pt, uint32_t n_grads, uint32_t n_vis);
-// k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg_mask right after vb_launch_damage: the boxes
+// The damage snapshot (VbDamage::snap) of a frame with the bindings B, of the scene of layout S, reading n_xf transforms. It
+// exists while anything is bound (any_binding): [generation, pad x3] [slot 0] [slot 1] [flags]. A slot holds
+//   [the transform words the frame reads (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw
+//   objects] [the words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)] [the
+//   n_vis words of the visibility mask].
+// The flags, which k_damage_begin and k_damage_mark rewrite every frame, are one per bound instance, with points or visibility
+// bound one per path, and with transforms bound one per transform. Offsets are in words: a section's from the start of its
+// slot, a flag array's from the start of the snapshot (0: absent).
+#define VB_DMG_HEADER_WORDS 4u
+struct VbDmgLayout {
+    uint32_t n_xf, n_draw, n_col, n_pt, n_grads, n_vis, n_inst, n_paths;
+    size_t box, col, pt, ramp, vis, slot_words;
+    size_t changed, paths, xf, bytes;
+};
+static inline VbDmgLayout vb_dmg_layout(const VbBound &B, const VbLayout &S, uint32_t n_xf) {
+    const VbRows *k = B.rows;
+    VbDmgLayout L;
+    L.n_xf = n_xf, L.n_draw = S.n_draw_objects, L.n_inst = k[VB_BIND_INSTANCES].n, L.n_paths = S.n_paths;
+    L.n_col = k[VB_BIND_COLORS].n, L.n_pt = k[VB_BIND_POINTS].n, L.n_grads = B.rs_grads_n;
+    L.n_vis = k[VB_BIND_VISIBILITY].rows ? vb_vis_words(S) : 0u;
+    L.box = 6u * (size_t)n_xf;
+    L.col = L.box + 4u * (size_t)L.n_draw;
+    L.pt = L.col + L.n_col;
+    L.ramp = L.pt + 2u * (size_t)L.n_pt;
+    L.vis = L.ramp + 512u * (size_t)L.n_grads;
+    L.slot_words = L.vis + L.n_vis;
+    size_t end = VB_DMG_HEADER_WORDS + 2u * L.slot_words;
+    L.changed = k[VB_BIND_INSTANCES].rows ? end : 0u;
+    end += L.changed ? L.n_inst : 0u;
+    L.paths = k[VB_BIND_POINTS].rows || k[VB_BIND_VISIBILITY].rows ? end : 0u;
+    end += L.paths ? L.n_paths : 0u;
+    L.xf = k[VB_BIND_TRANSFORMS].rows ? end : 0u;
+    L.bytes = (end + (L.xf ? n_xf : 0u)) * 4u;
+    return L;
+}
+// k_recompose.cu: the damage of the first frame after vb_recompose, ORed into dmg.mask right after vb_launch_damage: the boxes
 // of unmatched instances' draw objects, and both boxes of matched draw objects whose boxes differ; nothing while the tables
 // are null
 #define VB_RCMP_NONE 0xffffffffu
 uint32_t vb_launch_recompose_damage(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+// k_recompose_damage's tables at `base` for n_old instances of the base frame's scene and n_new of this frame's: [old draw
+// prefix (n_old + 1)] [new draw prefix (n_new + 1)] [new instance -> old instance, or VB_RCMP_NONE (n_new)] [old instance
+// unmatched (n_old)], `words` in all. Instance k draws draw objects prefix[k] .. prefix[k + 1]. W is uint32_t or const
+// uint32_t, as the caller writes or reads them; sizing passes a null base and reads `words` alone.
+extern "C++" {
+template <class W> struct VbRcmpTables {
+    W *old_pre, *new_pre, *map, *unmatched;
+    size_t words;
+};
+template <class W> __host__ __device__ inline VbRcmpTables<W> vb_rcmp_tables(W *base, uint32_t n_old, uint32_t n_new) {
+    const size_t at_new = (size_t)n_old + 1u, at_map = at_new + n_new + 1u, at_unmatched = at_map + n_new;
+    return VbRcmpTables<W>{base, base + at_new, base + at_map, base + at_unmatched, at_unmatched + n_old};
+}
+}
 
 // k_upload_diff.cu: the damage of the first frame after an upload that tracking follows (vb_set_upload_diff). The upload keeps
 // the base frame's scene (the renderer's spare buffers), copies its draw boxes and runs vb_launch_upload_records on its
@@ -310,7 +360,7 @@ struct VbUdiff {
     uint32_t prefix, suffix, pad[2];
 };
 // The diff's buffer after the head: the base frame's draw boxes (n_old), the records of both scenes (n_old, n_new), the
-// positional equality flags (min(n_old, n_new)) and k_recompose_damage's tables (rcmp_tables: identity draw prefixes,
+// positional equality flags (min(n_old, n_new)) and k_recompose_damage's tables (vb_rcmp_tables: identity draw prefixes,
 // new -> old or VB_RCMP_NONE, old unmatched).
 struct VbUdLayout { size_t boxes, old_rec, new_rec, eq, tables, bytes; };
 static inline VbUdLayout vb_udiff_layout(uint32_t n_old, uint32_t n_new) {
@@ -321,7 +371,7 @@ static inline VbUdLayout vb_udiff_layout(uint32_t n_old, uint32_t n_new) {
     u.new_rec = u.old_rec + (size_t)n_old * sizeof(VbUdRec);
     u.eq = u.new_rec + (size_t)n_new * sizeof(VbUdRec);
     u.tables = u.eq + m * 4u;
-    u.bytes = u.tables + ((size_t)n_old + 1u + n_new + 1u + n_new + n_old) * 4u;
+    u.bytes = u.tables + vb_rcmp_tables((uint32_t *)nullptr, n_old, n_new).words * 4u;
     return u;
 }
 // the records of a scene's n_draw draw objects from its tag and draw monoids; `init` (nullable) gets [m, m], the starting
@@ -330,7 +380,7 @@ uint32_t vb_launch_upload_records(const uint32_t *scene, uint32_t path_tag_base,
                                   const VbTagMonoid *tag_monoids, const VbDrawMonoid *draw_monoids, VbUdRec *out, uint32_t *init, uint32_t m,
                                   cudaStream_t st);
 // the new scene's records, the equality of the draw objects paired by position and from the end, and the tables; nothing while
-// b.udiff is null
+// b.dmg.udiff is null
 uint32_t vb_launch_upload_diff(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_atlas.cu: images in device memory copied into the atlas, all rectangles in one launch (also called through ctypes by
