@@ -734,6 +734,49 @@ int vb_bind_transforms(vb_renderer *, const float *device_affines, uint32_t n, s
  * memory); a pitch of 0, or of 4 GiB or more; a renderer of a vb_group or with the exchange configured; a call between
  * vb_render_enqueue and vb_frame_finish. */
 int vb_bind_draw_visibility(vb_renderer *, const uint8_t *device_flags, uint32_t n, size_t row_pitch_bytes);
+/* Bind the line widths of the installed scene's strokes to device memory (an addition; no vello counterpart). Maps, charts and
+ * node editors keep road outlines, grid lines and graph edges one width on screen while a view zooms; flow maps and graph
+ * layouts draw data-driven widths; hover and selection widen one edge. Each without re-encoding or re-uploading the scene
+ * (which would unbind every binding), and without a host call per frame:
+ *  - Rows. Row k is the f32 at device_widths + k * row_pitch_bytes and belongs to draw object k of the installed scene, which is
+ *    path k: the indices of vb_hit_test and Scene.n_draw_objects, global in a composed scene and in cell order in a batch. Rows
+ *    are per draw object, not per style entry: the encoders push a style entry only when it differs from the previous one, so
+ *    consecutive strokes of equal width share one entry, and each of them still has a row of its own.
+ *  - A row is a line width in the stroke's own coordinates: it plays the part of Stroke::width, and the path's transform,
+ *    bound instance transforms, bound transforms and a view all still apply on top. For a constant on-screen width under a
+ *    uniform zoom z, write w / z.
+ *  - Which rows apply. Row k applies when draw object k is a stroke (it is no layer's BEGIN_CLIP or END_CLIP, and the style
+ *    entry in effect at its path's end tag has the STYLE bit), k < n, and the row is finite and > 0. Rows of fills, images, blurred rectangles, layers and END_CLIPs are
+ *    ignored. A non-finite, zero or negative row keeps the encoded width for that frame (hiding is vb_bind_draw_visibility's
+ *    job). Joins, caps, miter limit and dashes keep their encoded values; dashes are cut on the host along the centreline, so
+ *    each dash takes the bound width, and its caps follow.
+ *  - What a frame renders. When every bound stroke has a style entry of its own (as when the encoded widths all differ), a
+ *    bound frame is byte for byte, in all three AA modes, the frame that installing the scene renders after overwriting the
+ *    width word (style_base + 2 s + 1) of that stroke's entry s with the row's bits. In general it is what the scene re-encoded
+ *    with those widths renders: byte for byte in MSAA8 and MSAA16, and in Area up to the last-bit differences the order of a
+ *    tile's segments makes in its area sums.
+ *  - Culling under a view or a window uses the bound width (the reach of a stroke's hull is 0.5 |width| x miter limit), so a
+ *    thin stroke just outside the frame that a row widens into it appears.
+ *  - Hit tests and hit maps answer from the frame's lines, so they follow the bound widths.
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage, into a snapshot of
+ *    its own (vb_debug_download("stroke_widths"): per draw object the width flatten used, 0 where the encoded width applied),
+ *    and a vb_run_stages range that contains flatten reads them again. The caller orders its writes before the frame, on
+ *    vb_stream or with a synchronisation. A blocking frame that is re-run after an arena overflow reads the rows again; an
+ *    enqueued frame is never re-run. Flatten and damage tracking read only the snapshot, so rows written while a frame runs
+ *    cannot make its kernels disagree. The caller keeps the memory alive while it is bound. Changing only the contents replays
+ *    the captured frame graph. Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next
+ *    frame captures its graph anew. With nothing bound a frame launches, configures and captures exactly what it would without
+ *    this call; bound, it launches one kernel more.
+ *  - Scope. Any installed scene can be bound, packed bytes included. Every scene installation unbinds: every upload form,
+ *    vb_render, vb_render_begin, vb_compose and vb_recompose. The binding survives vb_set_view, vb_set_cells, the six other
+ *    bindings and hit tests; all seven can be active together. device_widths NULL unbinds.
+ *  - The call makes nothing but the snapshot's buffer, and does not synchronise unless that grows. Damage tracking follows the
+ *    rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the scene's draw-object count; a pointer that is not device memory of the renderer's device (or managed
+ * memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 4, or 4 GiB or more; a renderer of a vb_group or
+ * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish. */
+int vb_bind_stroke_widths(vb_renderer *, const float *device_widths, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -776,6 +819,10 @@ int vb_bind_draw_visibility(vb_renderer *, const uint8_t *device_flags, uint32_t
  *    differs from the last successful frame's: only shown or hidden counts, so a row going from 1 to 2 is no change. The damage
  *    is the tiles of its clipped box in the last frame and in this one; a hidden draw object's box is empty, so that is the box
  *    it has while shown. A shown or hidden layer is covered by its BEGIN_CLIP's box, which holds everything inside the layer.
+ *  - Automatic damage, for bound stroke widths (vb_bind_stroke_widths). Draw object d changed if the width its frame used
+ *    differs bit for bit from the last successful frame's: a fill's row, or a row that falls back to an unchanged encoded
+ *    width, is no change. The damage is the tiles of its clipped box in the last frame and in this one; a widened stroke's box
+ *    grows, so the new box covers it.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to

@@ -19,7 +19,11 @@
 //   + with bound visibility (vb_bind_draw_visibility), for every draw object whose bit of the frame's mask (the one flatten
 //     reads) differs from the last successful frame's, its tile box in that frame and in this one. A hidden draw object's box
 //     is empty, so the union is the box it has while shown; a hidden layer is covered by its BEGIN_CLIP's box, which holds
-//     every box inside the layer and the pixels its blend touches.
+//     every box inside the layer and the pixels its blend touches
+//   + with bound stroke widths (vb_bind_stroke_widths), for every draw object below the bound count whose width (the one
+//     flatten used: its snapshot entry, or for an entry of 0 its style's width word) differs bit for bit from the last successful
+//     frame's, its tile box in that frame and in this one. A fill's entry is always 0 and its style word never changes, so its
+//     row is no change; neither is a row that falls back to an unchanged encoded width. A wider stroke's new box holds it.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -56,7 +60,8 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
 
 // The inputs of k_damage_mark and k_damage: the snapshot `snap`, laid out by L (its flag arrays: L.changed, L.paths, L.xf), the
 // frame's mask, the words the frame reads and the bindings' tables (VbBound). The mask words `vis` are null without bound
-// visibility, `grad` (VbBound::rs_draw) without a bound gradient, and `xf_range` without bound transforms.
+// visibility, `grad` (VbBound::rs_draw) without a bound gradient, `xf_range` without bound transforms, and the stroke-width
+// snapshot `widths` without bound widths (`styles`: the scene's n_style style words, `path_draw`: pathtag's path table).
 struct DmArgs {
     VbDmgLayout L;
     uint32_t *snap;
@@ -66,7 +71,10 @@ struct DmArgs {
     const VbDrawMonoid *draw_monoids;
     const uint32_t *inst_prefix, *inst_draw, *pt_first, *grad, *ramps; // ramps: the bound gradients' rows
     const uint2 *xf_range;
-    uint32_t compare, wt, ht;
+    const float *widths;
+    const uint2 *path_draw;
+    const uint32_t *styles;
+    uint32_t compare, wt, ht, n_style;
 };
 
 // One thread per transform u of the frame: its six words against the snapshot, and into the next slot. A difference marks
@@ -121,7 +129,8 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const DmArgs a) {
 // word, its ramp row or its path's points (flagged with points or visibility bound) or one of its path's transforms (path d
 // reads transforms xf_range[d].x .. .y, each flagged with transforms bound) changed, its old and new boxes into the mask. A draw
 // object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's
-// offset in the frame's draw data (`dd`, the bound region).
+// offset in the frame's draw data (`dd`, the bound region). Below L.n_wid, its stroke width: the snapshot entry, or for 0 the
+// width word of its path's style (path d is draw object d).
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
     const VbDmgLayout &L = a.L;
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
@@ -139,6 +148,15 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
         const uint32_t col = one_colour ? __ldg(a.dd + __ldg(&a.draw_monoids[d].scene_offset)) : 0u;
         hit = col != old[L.col + d];
         if (lane == 0u) nxt[L.col + d] = col;
+    }
+    if (d < L.n_wid) {
+        uint32_t w = __float_as_uint(__ldg(a.widths + d));
+        if (w == 0u && d < L.n_paths) {
+            const uint32_t s = __ldg(&a.path_draw[d].x) + 1u;
+            w = s < a.n_style ? __ldg(a.styles + s) : 0u;
+        }
+        hit = w != old[L.wid + d] || hit;
+        if (lane == 0u) nxt[L.wid + d] = w;
     }
     const uint32_t g = a.grad ? __ldg(a.grad + d) : VB_COLOR_NONE;
     if (g != VB_COLOR_NONE) {
@@ -203,9 +221,11 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     const uint32_t n_paths = L.paths ? L.n_paths : 0u, n = std::max(std::max(n_tiles, L.n_inst), n_paths);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(D.mask, D.pending, n_tiles, full, D.snap + L.changed, L.n_inst,
                                                                               D.snap + L.paths, n_paths);
-    // neither instance transforms, colours, points, stops, transforms nor visibility bound: nothing changes without a call that
-    // makes the frame full
-    if (L.n_inst == 0u && L.n_col == 0u && L.n_pt == 0u && L.n_grads == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && L.n_vis == 0u) return 1u;
+    // neither instance transforms, colours, points, stops, transforms, visibility nor stroke widths bound: nothing changes
+    // without a call that makes the frame full
+    if (L.n_inst == 0u && L.n_col == 0u && L.n_pt == 0u && L.n_grads == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && L.n_vis == 0u &&
+        L.n_wid == 0u)
+        return 1u;
     DmArgs a;
     a.L = L, a.snap = D.snap, a.mask = D.mask, a.compare = !full, a.wt = wt, a.ht = ht;
     a.xf = b.scene + cfg.layout.transform_base, a.pd = b.scene + cfg.layout.path_data_base, a.vis = cfg.vis;
@@ -213,6 +233,8 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     a.draw_bboxes = b.draw_bboxes, a.draw_monoids = b.draw_monoids, a.ramps = b.ramps + 512u * (size_t)B.rs_ramp0;
     a.inst_prefix = B.inst_prefix, a.inst_draw = B.inst_draw, a.pt_first = B.pt_first, a.grad = L.n_grads ? B.rs_draw : nullptr;
     a.xf_range = B.rows[VB_BIND_TRANSFORMS].rows ? B.xf_range : nullptr;
+    a.widths = cfg.widths, a.path_draw = b.path_draw, a.styles = b.scene + cfg.layout.style_base;
+    a.n_style = cfg.scene_words > cfg.layout.style_base ? cfg.scene_words - cfg.layout.style_base : 0u;
     uint32_t launches = 1u;
     const uint32_t n_mark = std::max(std::max(L.n_xf, n_paths ? L.n_pt : 0u), L.n_vis);
     if (n_mark) {

@@ -572,7 +572,6 @@ __device__ void flatten_arc(F &f, fv2 begin, fv2 end, fv2 center, float angle, c
     f.write_line(p0, p1);
 }
 
-#define STYLE_FLAGS_STYLE 0x80000000u
 #define STYLE_MITER_LIMIT_MASK 0xFFFFu
 #define STYLE_FLAGS_START_CAP_MASK 0x0C000000u
 #define STYLE_FLAGS_END_CAP_MASK 0x03000000u
@@ -768,6 +767,15 @@ struct TagPlan {
     float edge_y;
 };
 
+// A stroke's line width: bound stroke widths' snapshot entry of its path when it is > 0 (k_widths.cu), else its style's word.
+__device__ __forceinline__ float stroke_width(const VbConfig &cfg, const uint32_t *__restrict__ scene, const PathTagData &tag) {
+    if (cfg.widths != nullptr) {
+        const float w = __ldg(cfg.widths + tag.path_ix);
+        if (w > 0.f) return w;
+    }
+    return __uint_as_float(vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix + 1u));
+}
+
 // false: the tag emits nothing (and, with plan.edge, only extends its path's box).
 __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, const uint32_t *__restrict__ scene,
                                          const VbTagMonoid *__restrict__ tag_monoids, const PathTagData &tag, uint32_t ix,
@@ -804,7 +812,7 @@ __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, con
         const float y_3 = fmaf(transform.m1, pts.p3.x, fmaf(transform.m3, pts.p3.y, transform.ty));
         float grow = 1.0f;
         if (is_stroke) {
-            const float lw = __uint_as_float(vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix + 1u));
+            const float lw = stroke_width(cfg, scene, tag);
             const float lim = fmaxf(f16_bits_to_f32(style_flags & STYLE_MITER_LIMIT_MASK), 1.5f);
             grow += 0.5f * fabsf(lw) * lim * (fabsf(transform.m0) + fabsf(transform.m1) + fabsf(transform.m2) + fabsf(transform.m3));
         }
@@ -846,7 +854,7 @@ __device__ __forceinline__ bool plan_tag(TagPlan &plan, const VbConfig &cfg, con
     tail.arc_begin = tail.arc_end = tail.arc_center = F2(0.f, 0.f);
     tail.a0 = tail.b0 = tail.a1 = tail.b1 = tail.a2 = tail.b2 = F2(0.f, 0.f);
     if (is_stroke) {
-        float linewidth = __uint_as_float(vb_scene(scene, cfg, cfg.layout.style_base + tag.style_ix + 1u));
+        float linewidth = stroke_width(cfg, scene, tag);
         offset = 0.5f * linewidth;
         bool is_open = seg_type != 1u;
         bool is_stroke_cap_marker = (tag.tag_byte & 4u) != 0u;

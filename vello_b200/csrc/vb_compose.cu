@@ -574,7 +574,7 @@ static std::string draw_tags_outside(const Slot &s, uint64_t n) {
     if ((uint64_t)s.layout.draw_tag_base + n > s.scene_words) return "the scene's draw tags do not lie inside its words";
     return {};
 }
-static std::string colors_check(const vb_renderer *r, uint32_t n) { return draw_tags_outside(*r->cur, n); }
+static std::string draw_tags_check(const vb_renderer *r, uint32_t n) { return draw_tags_outside(*r->cur, n); }
 static std::string path_tags_outside(const vb_renderer *r, uint32_t) {
     const VbLayout &L = r->cur->layout;
     if (L.path_data_base < L.path_tag_base || L.path_data_base > r->cur->scene_words) return "the scene's path tags do not lie inside its words";
@@ -722,6 +722,11 @@ static int transform_tables(vb_renderer *r, uint32_t, VbBound &b, std::string &)
 static int visibility_mask(vb_renderer *r, uint32_t, VbBound &, std::string &) {
     return compose_room(r, r->vis_mask, (size_t)vb_vis_words(r->cur->layout) * 4u);
 }
+// Bound stroke widths (k_widths.cu): only the snapshot is sized, which every frame reads the caller's rows into, and which
+// flatten takes the bound strokes' widths from. The call does not synchronise unless the snapshot grows.
+static int width_snapshot(vb_renderer *r, uint32_t, VbBound &, std::string &) {
+    return compose_room(r, r->width_snap, (size_t)vb_width_entries(r->cur->layout) * 4u);
+}
 static int no_tables(vb_renderer *, uint32_t, VbBound &, std::string &) { return VB_OK; }
 
 // The draw-data slot table of bound colours and bound gradient stops (k_colors.cu), made from b whenever either changes and
@@ -763,11 +768,12 @@ struct BindKind {
 };
 static const BindKind BIND_KINDS[VB_N_BINDINGS] = {
     {"vb_bind_instance_transforms", true, composed_scene, n_instances, true, " instances", 24u, true, freed_fragment, instance_tables},
-    {"vb_bind_draw_colors", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 16u, true, colors_check, no_tables},
+    {"vb_bind_draw_colors", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 16u, true, draw_tags_check, no_tables},
     {"vb_bind_path_points", false, any_scene, n_points, false, " points (1 .. n_points)", 8u, true, path_tags_outside, point_tables},
     {"vb_bind_gradient_stops", false, scene_with_stops, n_stops, false, " gradient stops (1 .. n_stops)", 20u, true, stops_check, stop_tables},
     {"vb_bind_transforms", false, any_scene, n_xforms, false, " transforms (1 .. n_transforms)", 24u, true, path_tags_outside, transform_tables},
     {"vb_bind_draw_visibility", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 1u, false, no_check, visibility_mask},
+    {"vb_bind_stroke_widths", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, false, draw_tags_check, width_snapshot},
 };
 
 // Unbind `kind` in b: its rows and the tables only it reads
@@ -850,4 +856,7 @@ extern "C" int vb_bind_transforms(vb_renderer *r, const float *device_affines, u
 }
 extern "C" int vb_bind_draw_visibility(vb_renderer *r, const uint8_t *device_flags, uint32_t n, size_t row_pitch_bytes) {
     return bind_rows(r, VB_BIND_VISIBILITY, device_flags, n, row_pitch_bytes);
+}
+extern "C" int vb_bind_stroke_widths(vb_renderer *r, const float *device_widths, uint32_t n, size_t row_pitch_bytes) {
+    return bind_rows(r, VB_BIND_WIDTHS, device_widths, n, row_pitch_bytes);
 }

@@ -67,6 +67,9 @@ static std::vector<NamedBuf> named(vb_renderer *r) {
     // the path-data words the last frame read from its path_data_base: the bound points' region, else the scene's stream
     const size_t p_off = (size_t)c.layout.path_data_base * 4u, p_cap = r->cur->scene.cap > p_off ? r->cur->scene.cap - p_off : 0u;
     v.push_back({"path_data", &r->cur->scene, std::min<size_t>(4u * (size_t)n_path_data(r->cur->layout, r->cur->scene_words), p_cap), p_off});
+    // the stroke widths the last frame read (k_widths.cu): one float per draw object, 0 where the encoded width applies; empty
+    // while unbound
+    v.push_back({"stroke_widths", &r->width_snap, c.widths ? (size_t)vb_width_entries(c.layout) * 4u : 0u});
     // an arena's buffer up to what the last attempt used of it, at most the capacity the kernels saw
     const uint32_t *size = &c.lines_size;
     for (int a = 0; a < N_ARENAS; a++) {

@@ -209,8 +209,9 @@ __device__ __forceinline__ uint32_t vb_span(float a, float b) {
 __device__ __forceinline__ uint32_t vb_scene(const uint32_t *__restrict__ scene, const VbConfig &cfg, uint32_t ix) {
     return ix < cfg.scene_words ? __ldg(scene + ix) : 0u;
 }
-// a style word's fill-rule bit (the path's draw flags; read by flatten and draw)
+// a style word's fill-rule bit (the path's draw flags; read by flatten and draw), and its stroke bit (flatten, k_stroke_widths)
 #define STYLE_FLAGS_FILL 0x40000000u
+#define STYLE_FLAGS_STYLE 0x80000000u
 // A tile after backdrop, as coarse and hit testing read it. k_backdrop wrote ~(first slot of the slice) into every tile of the
 // arena in tile order, so a tile's segment count is the distance to the next tile's slice; the arena's last tile ends at
 // bump.segments.

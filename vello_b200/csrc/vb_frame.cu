@@ -425,6 +425,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     c.tile_rows = c.height_in_tiles * n_cells;
     c.cell_draw = n_cells > 1u ? (const uint32_t *)r->cell_draw.p : nullptr;
     c.vis = B.rows[VB_BIND_VISIBILITY].rows ? (const uint32_t *)r->vis_mask.p : nullptr; // the mask k_draw_visibility writes
+    c.widths = B.rows[VB_BIND_WIDTHS].rows ? (const float *)r->width_snap.p : nullptr; // the snapshot k_stroke_widths writes
     r->params = *p;
 
     const uint32_t n_draw = c.layout.n_draw_objects, n_tiles = c.width_in_tiles * c.tile_rows;
@@ -577,8 +578,8 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // first, inside flatten's stage events, what the bindings (VbBound) and the view make of the scene: the regions past
             // its streams in regions_of's order, the bound transforms before the viewed ones (their source; instances, then
             // transform rows), the draw data (read by draw, coarse and fine) and the path data (read by flatten alone); the bound
-            // gradients' ramp rows (read by fine); and the visibility mask (read by flatten and damage tracking). Each launcher
-            // launches nothing while its binding is unbound.
+            // gradients' ramp rows (read by fine); the visibility mask and the stroke widths' snapshot (read by flatten and
+            // damage tracking). Each launcher launches nothing while its binding is unbound.
             launches += vb_launch_instance_transforms(c, b, st);
             launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
@@ -586,6 +587,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             launches += vb_launch_bound_ramps(c, b, st);
             launches += vb_launch_path_points(c, b, st);
             launches += vb_launch_draw_visibility(c, b, st);
+            launches += vb_launch_stroke_widths(c, b, st);
             if (fork_draw) {
                 CK(cudaEventRecord(r->draw_fork, st));
                 CK(cudaStreamWaitEvent(r->tiling_stream, r->draw_fork, 0));

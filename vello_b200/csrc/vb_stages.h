@@ -22,8 +22,9 @@ struct CmpXform; // an instance's transform (k_compose.cu, below)
 struct VbUdiff;  // the upload diff's state (k_upload_diff.cu, below)
 
 // The bindings of a scene to device rows that every frame reads (vb_bind_*): instance transforms, draw colours, path points,
-// gradient stops, transforms and visibility. Binding k's rows are `n` rows `pitch` bytes apart from `rows`, null while unbound.
-enum { VB_BIND_INSTANCES, VB_BIND_COLORS, VB_BIND_POINTS, VB_BIND_STOPS, VB_BIND_TRANSFORMS, VB_BIND_VISIBILITY, VB_N_BINDINGS };
+// gradient stops, transforms, visibility and stroke widths. Binding k's rows are `n` rows `pitch` bytes apart from `rows`, null
+// while unbound.
+enum { VB_BIND_INSTANCES, VB_BIND_COLORS, VB_BIND_POINTS, VB_BIND_STOPS, VB_BIND_TRANSFORMS, VB_BIND_VISIBILITY, VB_BIND_WIDTHS, VB_N_BINDINGS };
 struct VbRows {
     const uint8_t *rows;
     uint32_t n, pitch;
@@ -275,6 +276,13 @@ uint32_t vb_launch_bound_transforms(const VbConfig &cfg, const VbFrameBufs &b, c
 // every k from b.vis_n on), which flatten and damage tracking read; nothing while unbound.
 uint32_t vb_launch_draw_visibility(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// The entries of the stroke-width snapshot of a scene: one per draw object, and per path (path p is draw object p).
+static inline uint32_t vb_width_entries(const VbLayout &L) { return L.n_draw_objects > L.n_paths ? L.n_draw_objects : L.n_paths; }
+// k_widths.cu: bound stroke widths (vb_bind_stroke_widths). Per frame, at the start of flatten's stage after the visibility
+// mask: entry k of the snapshot at cfg.widths (vb_width_entries floats) is row k when draw object k is a stroke, k < b.rows.n
+// and the row is finite and > 0, else 0 (the encoded width); flatten and damage tracking read it; nothing while unbound.
+uint32_t vb_launch_stroke_widths(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
 // k_damage.cu: damage tracking. vb_launch_damage runs between binning and coarse: the frame's damage mask, and the snapshot
 // the next frame compares against; vb_launch_damage_commit, the frame's last kernel, makes that snapshot current when the frame
 // succeeded. vb_launch_damage_rects stages caller rectangles (tile ranges x0 y0 x1 y1, clipped) into `pending` in stream order.
@@ -288,14 +296,15 @@ uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const
 // exists while anything is bound (any_binding): [generation, pad x3] [slot 0] [slot 1] [flags]. A slot holds
 //   [the transform words the frame reads (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw
 //   objects] [the words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)] [the
-//   n_vis words of the visibility mask].
+//   n_vis words of the visibility mask] [the stroke widths the first n_wid draw objects were drawn with (their snapshot entry,
+//   or for 0 the encoded width word of their path's style)].
 // The flags, which k_damage_begin and k_damage_mark rewrite every frame, are one per bound instance, with points or visibility
 // bound one per path, and with transforms bound one per transform. Offsets are in words: a section's from the start of its
 // slot, a flag array's from the start of the snapshot (0: absent).
 #define VB_DMG_HEADER_WORDS 4u
 struct VbDmgLayout {
-    uint32_t n_xf, n_draw, n_col, n_pt, n_grads, n_vis, n_inst, n_paths;
-    size_t box, col, pt, ramp, vis, slot_words;
+    uint32_t n_xf, n_draw, n_col, n_pt, n_grads, n_vis, n_wid, n_inst, n_paths;
+    size_t box, col, pt, ramp, vis, wid, slot_words;
     size_t changed, paths, xf, bytes;
 };
 static inline VbDmgLayout vb_dmg_layout(const VbBound &B, const VbLayout &S, uint32_t n_xf) {
@@ -304,12 +313,14 @@ static inline VbDmgLayout vb_dmg_layout(const VbBound &B, const VbLayout &S, uin
     L.n_xf = n_xf, L.n_draw = S.n_draw_objects, L.n_inst = k[VB_BIND_INSTANCES].n, L.n_paths = S.n_paths;
     L.n_col = k[VB_BIND_COLORS].n, L.n_pt = k[VB_BIND_POINTS].n, L.n_grads = B.rs_grads_n;
     L.n_vis = k[VB_BIND_VISIBILITY].rows ? vb_vis_words(S) : 0u;
+    L.n_wid = k[VB_BIND_WIDTHS].n;
     L.box = 6u * (size_t)n_xf;
     L.col = L.box + 4u * (size_t)L.n_draw;
     L.pt = L.col + L.n_col;
     L.ramp = L.pt + 2u * (size_t)L.n_pt;
     L.vis = L.ramp + 512u * (size_t)L.n_grads;
-    L.slot_words = L.vis + L.n_vis;
+    L.wid = L.vis + L.n_vis;
+    L.slot_words = L.wid + L.n_wid;
     size_t end = VB_DMG_HEADER_WORDS + 2u * L.slot_words;
     L.changed = k[VB_BIND_INSTANCES].rows ? end : 0u;
     end += L.changed ? L.n_inst : 0u;

@@ -74,6 +74,10 @@ typedef struct {
      * k_draw_visibility at the start of flatten's stage; flatten emits nothing for a tag of a path whose bit is clear
      * (plan_tag). Null while unbound. */
     const uint32_t *vis;
+    /* Bound stroke widths (vb_bind_stroke_widths): one float per draw object (path p is draw object p), written by k_stroke_widths
+     * at the start of flatten's stage; a path whose entry is > 0 is stroked that wide, any other with its style's width word
+     * (plan_tag). Null while unbound. */
+    const float *widths;
 } VbConfig;
 
 /* One rectangle of k_atlas_blit (k_atlas.cu): w x h RGBA8 texels from device memory (rows src_pitch bytes apart, 4-byte

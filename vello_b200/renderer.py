@@ -179,6 +179,7 @@ def load_library() -> C.CDLL:
     lib.vb_bind_gradient_stops.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_draw_visibility.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_stroke_widths.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -202,20 +203,27 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
-                    "vb_set_background", "vb_bind_draw_visibility"]
+                    "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths"]
 
 
-def _device_rows(t, who: str, what: str, cols: int):
+def _device_rows(t, who: str, what: str, cols: int, vector: bool = False):
     """(pointer, rows, row pitch in bytes) of an (n, cols) float32 device array bound by a `bind_*` method, from its
     `__cuda_array_interface__` (a torch CUDA tensor, or columns of a larger one): columns 4 bytes apart and rows any multiple of
-    4 bytes, at least 4 * cols, apart. `who` names the method and `what` the rows in the errors."""
+    4 bytes, at least 4 * cols, apart. With `vector` (cols = 1) an (n,) array is taken as (n, 1), so a column of a larger
+    tensor such as `state[:, 5]` binds with its row stride. `who` names the method and `what` the rows in the errors."""
     cai = getattr(t, "__cuda_array_interface__", None)
     if cai is None:
         raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device {what} are needed")
     shape = tuple(int(v) for v in cai["shape"])
-    if len(shape) != 2 or shape[0] == 0 or shape[1] != cols or cai["typestr"] != "<f4":
-        raise ValueError(f"{who}: {what} must be (n, {cols}) float32, not {shape} {cai['typestr']}")
-    strides = cai.get("strides") or (4 * cols, 4)
+    strides = cai.get("strides")
+    rows = shape
+    if vector and len(shape) == 1:
+        rows, strides = shape + (1,), strides and (strides[0], 4)
+    if len(rows) != 2 or rows[0] == 0 or rows[1] != cols or cai["typestr"] != "<f4":
+        form = f"(n,) or (n, {cols})" if vector else f"(n, {cols})"
+        raise ValueError(f"{who}: {what} must be {form} float32, not {shape} {cai['typestr']}")
+    shape = rows
+    strides = strides or (4 * cols, 4)
     pitch = int(strides[0]) if shape[0] > 1 else 4 * cols  # the pitch of a single row is never used
     if int(strides[1]) != 4 or pitch % 4 or pitch < 4 * cols:
         raise ValueError(f"{who}: columns 4 bytes apart and rows a multiple of 4 bytes, at least {4 * cols}, apart; "
@@ -349,8 +357,8 @@ class Renderer:
     """`vello::Renderer`: `Renderer(options)`, then `render_to_texture(scene, params)`."""
 
     # the device arrays the bind_* methods hold while bound (_bind), None while unbound: of bind_instance_transforms,
-    # bind_draw_colors, bind_path_points, bind_gradient_stops, bind_transforms and bind_draw_visibility
-    _bound = _colors = _points = _stops = _xforms = _visibility = None
+    # bind_draw_colors, bind_path_points, bind_gradient_stops, bind_transforms, bind_draw_visibility and bind_stroke_widths
+    _bound = _colors = _points = _stops = _xforms = _visibility = _widths = None
 
     def __init__(self, options: Optional[RendererOptions] = None):
         self.lib = load_library()
@@ -613,6 +621,19 @@ class Renderer:
 
         `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
         self._bind("bind_draw_visibility", "_visibility", t, lambda t: _device_flags(t, "bind_draw_visibility"))
+
+    def bind_stroke_widths(self, t):
+        """Stroke draw object k of the installed scene with the line width in row k of the device array `t`, in every frame from
+        now on, read when the frame runs (`vb_bind_stroke_widths`): `t` is float32 (n,) or (n, 1), n at most the scene's
+        `Scene.n_draw_objects`, with `__cuda_array_interface__` and rows any multiple of 4 bytes apart (e.g. a torch CUDA
+        tensor, or a column of a larger one such as `state[:, 5]`). Index k is the draw object of `hit_test`, global in a
+        composed scene or a batch. A row is a width in the stroke's own coordinates, as `Stroke.width` is: the path's transform,
+        bound transforms and a view still apply (for a constant on-screen width under a zoom z, write w / z). It applies to
+        strokes only; rows of other draw objects are ignored, and draw objects from n on, and a stroke whose row is not finite
+        and > 0, keep their encoded width. Joins, caps, miter limit and dashes keep theirs. Every frame renders what the scene
+        re-encoded with those widths renders. Write `t` on `self.stream` (or synchronise) before a frame; frames then need no
+        further call. `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        self._bind("bind_stroke_widths", "_widths", t, lambda t: _device_rows(t, "bind_stroke_widths", "widths", 1, vector=True))
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
