@@ -32,6 +32,9 @@
 #define CO_STAGE 3 // tile records each of a tile's three helpers stages per emission window
 #endif
 #define CO_W (3 * CO_STAGE) // elements of a tile emitted per window (2 x 64 x CO_W x 12 B of shared memory)
+// The top bit of a tile's cost estimate: a command from its occlusion start on is a clip, blend, gradient, image or blurred
+// rectangle, so fine's lean kernel (k_fine_solid) cannot paint it. Moving the occlusion start resets the estimate and the bit.
+#define CO_FLAGGED 0x80000000u
 
 // Phase timing (tools/coarse_phases.py), off by default so the shipped kernel is unchanged: built with -DVB_COARSE_PHASES,
 // thread 0 of every CTA reads %globaltimer after the CTA-wide barrier that ends each phase of each 256-draw chunk and adds the
@@ -215,7 +218,8 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     uint32_t rd_ix = 0u, wr_ix = 0u, part_start_ix = 0u, ready_ix = 0u;
     uint32_t render_blend_depth = 0u, max_blend_depth = 0u;
     uint32_t cull_start = 0u; // PTCL offset of the CMD_SOLID of this tile's last opaque full-tile cover (0: none)
-    uint32_t cost = 0u;       // estimated work of fine on this tile from its occlusion start (orders fine's tile queue)
+    uint32_t cost = 0u;       // estimated work of fine on this tile from its occlusion start (orders fine's tile queue), and
+                              // CO_FLAGGED: a command from there on is not FILL / SOLID / COLOR / JUMP (fine's lean kernel skips it)
     uint32_t emitted = 0u;    // segments of the CMD_FILLs written for this tile
     st.cmd_offset += 1u; // the tile's first word: its blend scratch offset, written last
     if (owns_tile) {
@@ -411,7 +415,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                         cost += 2u;
                         if (solid_at != 0u && (rgba >> 24) == 0xffu && render_blend_depth == 0u) {
                             cull_start = solid_at;
-                            cost = 3u; // fine starts here: everything before is never executed
+                            cost = 3u; // fine starts here: everything before is never executed (nor flags the tile)
                         }
                         break;
                     }
@@ -422,7 +426,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                         co_put(ptcl, st.cmd_offset + 1u, di + 1u);
                         co_put(ptcl, st.cmd_offset + 2u, sh_paint[el_ix]);
                         st.cmd_offset += 3u;
-                        cost += 24u;
+                        cost = (cost + 24u) | CO_FLAGGED;
                         break;
                     case VB_DRAWTAG_FILL_LIN_GRADIENT:
                     case VB_DRAWTAG_FILL_RAD_GRADIENT:
@@ -435,7 +439,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                         co_put(ptcl, st.cmd_offset + 1u, sh_paint[el_ix]);
                         co_put(ptcl, st.cmd_offset + 2u, di + 1u);
                         st.cmd_offset += 3u;
-                        cost += 8u;
+                        cost = (cost + 8u) | CO_FLAGGED;
                         break;
                     }
                     case VB_DRAWTAG_FILL_IMAGE:
@@ -444,7 +448,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                         co_put(ptcl, st.cmd_offset, VB_CMD_IMAGE);
                         co_put(ptcl, st.cmd_offset + 1u, di + 1u);
                         st.cmd_offset += 2u;
-                        cost += 16u;
+                        cost = (cost + 16u) | CO_FLAGGED;
                         break;
                     case VB_DRAWTAG_BEGIN_CLIP: {
                         const bool even_odd = (draw_flags & 1u) != 0u;
@@ -457,7 +461,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                             st.cmd_offset += 1u;
                             render_blend_depth += 1u;
                             max_blend_depth = max(max_blend_depth, render_blend_depth);
-                            cost += 4u;
+                            cost = (cost + 4u) | CO_FLAGGED;
                         }
                         clip_depth += 1u;
                         break;
@@ -471,7 +475,7 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
                         co_put(ptcl, st.cmd_offset + 2u, sh_paint1[el_ix]);
                         st.cmd_offset += 3u;
                         render_blend_depth -= 1u;
-                        cost += 8u;
+                        cost = (cost + 8u) | CO_FLAGGED;
                         break;
                     default: break;
                     }
@@ -511,18 +515,19 @@ k_coarse(VbConfig cfg, const uint32_t *__restrict__ scene, const VbDrawMonoid *_
     } else if (owns_tile) {
         co_flush(ptcl);
     }
-    // fine's tile queue, heaviest first: every tile of the window goes into one of VB_FINE_CLASSES lists by its estimated cost
-    // (one atomic per warp and class; fine walks the lists in class order, so the long tiles start at time zero instead of
-    // turning up at the tail of a persistent kernel that has nothing left to overlap them with)
+    // fine's tile queue, heaviest first: every tile of the window goes into one of VB_FINE_CLASSES classes by its estimated cost
+    // (one atomic per warp and list; fine walks the lists in class order, so the long tiles start at time zero instead of
+    // turning up at the tail of a persistent kernel that has nothing left to overlap them with). Each class is two lists: list
+    // 2k holds the tiles that fine's lean kernel paints, list 2k + 1 the flagged ones (CO_FLAGGED).
     if (lid < 64u) { // the two owner warps, whole
         const uint32_t ty = bin_tile_y + tile_y, tx = bin_tile_x + tile_x; // ty: row in the cell; the list takes frame rows
         const bool in_win = tx < cfg.width_in_tiles && ty >= cfg.win_ty0 && ty < cfg.win_ty1 && ty < cfg.height_in_tiles && (!DMG || sh_damaged[lid] != 0u);
         // classes by powers of two of the estimate: >= 1024, 512, 256, 128, 64, 32, 16, rest
-        const uint32_t lg = 31u - (uint32_t)__clz((int)max(cost, 1u));
-        const uint32_t cls = lg >= 10u ? 0u : (lg <= 3u ? 7u : 10u - lg);
+        const uint32_t lg = 31u - (uint32_t)__clz((int)max(cost & ~CO_FLAGGED, 1u));
+        const uint32_t cls = 2u * (lg >= 10u ? 0u : (lg <= 3u ? 7u : 10u - lg)) + (cost >> 31);
         const uint32_t lane = lid & 31u;
 #pragma unroll
-        for (uint32_t k = 0; k < VB_FINE_CLASSES; k++) {
+        for (uint32_t k = 0; k < VB_FINE_LISTS; k++) {
             const uint32_t m = __ballot_sync(VB_FULL, in_win && cls == k);
             if (m == 0u) continue;
             uint32_t base = 0u;

@@ -30,6 +30,7 @@
 // Algorithmic bytes: 4 B/pixel stored + 4 B per PTCL word + 24 B per segment referenced.
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "vb_detmath.h"
@@ -44,6 +45,15 @@
 #define FI_MINB 2
 #endif
 #define FI_MAX_THREADS (32 * FI_MAX_WARPS)
+// k_fine_solid: FI_SOLID_MINB CTAs of FI_SOLID_WARPS warps per SM, 24 resident warps at 80 registers. Measured on the headline
+// frame (H100 SXM, 700 W): 16 warps at 64 registers and 14 at 72 hold more warps but spill the pixels around the fill, and
+// paint slower (DESIGN §8).
+#ifndef FI_SOLID_WARPS
+#define FI_SOLID_WARPS 12
+#endif
+#ifndef FI_SOLID_MINB
+#define FI_SOLID_MINB 2
+#endif
 #define PX 8                       // pixels per lane
 #define ONE_MINUS_ULP 0.99999994f
 #define ROBUST_EPSILON 2e-7f
@@ -89,6 +99,7 @@ struct FineArgs {
     const uint32_t *cls_count;  // their fill counts (control block); NULL: natural tile order
     uint32_t cls_stride;
     uint32_t cull;              // 1: start each tile there
+    uint32_t lists;             // FI_LISTS_*: which of those lists the launch walks
 };
 // The arguments of the FI_DST instantiations: FineArgs, then a registered destination's (vb_launch_fine's VbFineOut): the
 // __byte_perm selector of the stored byte order, the texel size (4: 8-bit, 8: RGBA16F, 16: RGBA32F), premultiplied or straight
@@ -718,6 +729,23 @@ __device__ void fill_path_ms(const FineArgs &A, WarpMs<AA> &S, const uint32_t *_
         area[i] = (float)((cov[i >> 2] >> ((i & 3u) * 8u)) & 0xffu) * (AA == 2 ? 0.0625f : 0.125f);
 }
 
+// ---------------- CMD_FILL, CMD_SOLID, CMD_COLOR: the commands both interpreters run (k_fine and k_fine_solid) ----------------
+template <int AA>
+__device__ __forceinline__ void fine_cmd_fill(const FineArgs &A, WarpMs<AA == 0 ? 1 : AA> &S, const uint32_t *__restrict__ lut, uint32_t sr,
+                                              uint32_t sd, int32_t bd, uint32_t lane, float (&area)[PX]) {
+    if (AA == 0) fill_path_area(A, sr, sd, bd, (float)((lane & 1u) * 8u), (float)(lane >> 1), area);
+    else fill_path_ms<AA == 0 ? 1 : AA>(A, S, lut, sr, sd, bd, lane, area);
+}
+__device__ __forceinline__ void fine_cmd_solid(float (&area)[PX]) {
+#pragma unroll
+    for (int i = 0; i < PX; i++) area[i] = 1.0f;
+}
+__device__ __forceinline__ void fine_cmd_color(uint32_t rgba8, rgba_t (&rgba)[PX], const float (&area)[PX]) {
+    const rgba_t fg = unpack4x8unorm_uniform(rgba8);
+#pragma unroll
+    for (int i = 0; i < PX; i++) rgba[i] = over(rgba[i], rg_scale(fg, area[i]));
+}
+
 // ---------------- blend.wgsl ----------------
 struct v3 { float x, y, z; };
 __device__ __forceinline__ v3 V3(float x, float y, float z) { v3 r; r.x = x; r.y = y; r.z = z; return r; }
@@ -924,31 +952,96 @@ struct FineSmem {
 static_assert(sizeof(WarpIo) % 16 == 0 && sizeof(WarpMs<1>) % 16 == 0 && sizeof(WarpMs<2>) % 16 == 0, "16-byte aligned smem blocks");
 
 // MODE: the AA mode (0 area, 1 MSAA8, 2 MSAA16), plus FI_DMG for damage tracking (k_damage.cu): coarse listed only the
-// damaged tiles, and those lists are the whole queue, so no other pixel is written. Without FI_DMG the kernel is the one it was
-// before damage tracking existed. FI_DST: a registered destination (vb_register_destination) in BGRA8 order, with premultiplied
-// alpha, in a float format or in a CUDA array; only the store differs. FI_BG (always with FI_DST, never with FI_DMG): every tile
-// starts from a background's pixels (vb_set_background) instead of the base colour. These three instantiations are compiled
-// into k_fine_bg.o (VB_FINE_BG), so that k_fine.o holds exactly the others.
+// damaged tiles, and those lists are the whole queue, so no other pixel is written. FI_DST: a registered destination
+// (vb_register_destination) in BGRA8 order, with premultiplied alpha, in a float format or in a CUDA array; only the store
+// differs. FI_BG (always with FI_DST, never with FI_DMG): every tile starts from a background's pixels (vb_set_background)
+// instead of the base colour. These three instantiations are compiled into k_fine_bg.o (VB_FINE_BG), so that k_fine.o holds
+// exactly the others.
 #define FI_DMG 16
 #define FI_DST 32
 #define FI_BG 64
 template <int MODE>
 using FineArgsOf = typename std::conditional<(MODE & FI_BG) != 0, FineBgArgs,
                                              typename std::conditional<(MODE & FI_DST) != 0, FineDstArgs, FineArgs>::type>::type;
-template <int MODE>
-__global__ void __launch_bounds__(FI_MAX_THREADS, FI_MINB)
-k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
-    constexpr int AA = MODE & 15;
-    constexpr bool DMG = (MODE & FI_DMG) != 0;
-    constexpr bool DST = (MODE & FI_DST) != 0;
-    constexpr bool BG = (MODE & FI_BG) != 0;
-    static_assert(!BG || (DST && !DMG), "FI_BG goes with FI_DST and without FI_DMG");
+
+// Which of coarse's tile lists a launch walks (FineArgs::lists). coarse puts each tile of the window into one of
+// VB_FINE_CLASSES cost classes, and each class into two lists: list 2k holds the tiles whose commands from their occlusion
+// start are only FILL / SOLID / COLOR / JUMP, list 2k + 1 the others (flagged). A frame is painted either by one k_fine over
+// every list, or by k_fine_solid over the simple lists followed by k_fine over the flagged ones.
+#define FI_LISTS_ALL 0u
+#define FI_LISTS_SIMPLE 1u
+#define FI_LISTS_FLAGGED 2u
+
+// ---- the tile queue: queue position -> {tile of the window, occlusion start}. Walking the launch's lists in class order
+// makes the heavy tiles the FIRST ones every warp takes (longest-processing-time-first), which is what bounds a persistent
+// kernel's tail when a stripe has only a few tiles per warp. Lane l < VB_FINE_LISTS holds the first queue position of list l
+// when the launch walks it (~0 otherwise), so the list of a position is the last lane whose start is at or below it.
+struct FineQueue {
+    uint32_t n_tiles; // queue positions of the launch (warp-uniform)
+    uint32_t cpre;    // this lane's list's first queue position
+    bool ordered;     // false: the window's tiles in their natural order, with their occlusion starts from tile_start
+};
+template <bool DMG>
+__device__ __forceinline__ FineQueue fine_queue(const VbConfig &cfg, const FineArgs &A, uint32_t lane) {
+    FineQueue q;
+    q.n_tiles = cfg.width_in_tiles * (cfg.win_ty1 - cfg.win_ty0);
+    q.cpre = ~0u;
+    q.ordered = A.cls_count != nullptr;
+    if (q.ordered) {
+        const uint32_t c = lane < VB_FINE_LISTS ? min(__ldg(A.cls_count + lane), A.cls_stride) : 0u;
+        const bool walked = lane < VB_FINE_LISTS && (A.lists == FI_LISTS_ALL || (lane & 1u) == (A.lists == FI_LISTS_FLAGGED ? 1u : 0u));
+        const uint32_t incl = vb_warp_incl_scan(walked ? c : 0u);
+        if (walked) q.cpre = incl - c;
+        q.ordered = DMG || vb_warp_sum(c) == q.n_tiles; // a launch over part of the window (read-back bands) keeps the natural order
+        if (q.ordered) q.n_tiles = __shfl_sync(VB_FULL, incl, 31);
+    }
+    if (!q.ordered && A.lists == FI_LISTS_SIMPLE) q.n_tiles = 0u; // the k_fine after it paints every tile then
+    return q;
+}
+__device__ __forceinline__ uint2 fine_entry(const VbConfig &cfg, const FineArgs &A, const FineQueue &q, uint32_t pos) {
+    if (q.ordered) {
+        const uint32_t l = 31u - (uint32_t)__clz((int)__ballot_sync(VB_FULL, pos >= q.cpre));
+        return __ldg(A.cls_list + (size_t)l * A.cls_stride + (pos - __shfl_sync(VB_FULL, q.cpre, l)));
+    }
+    return make_uint2(pos, A.cull != 0u ? __ldg(A.tile_start + cfg.win_ty0 * cfg.width_in_tiles + pos) : 0u);
+}
+
+// ---- the command windows
+__device__ __forceinline__ void fine_wait(WarpIo &io, uint32_t buf, uint32_t &phase) {
+    mbar_wait(&io.mbar[buf], (phase >> buf) & 1u);
+    phase ^= 1u << buf;
+}
+// The command word at cmd_ix and its (up to 3) operands, from the staged window; when the pointer leaves the window (a list
+// longer than the window, CMD_JUMP into another chunk) the window is staged again there.
+__device__ __forceinline__ const uint32_t *fine_cmd_words(WarpIo &io, const uint32_t *ptcl, uint32_t cmd_ix, uint32_t &win_base, uint32_t buf,
+                                                          uint32_t &phase, uint32_t lane) {
+    uint32_t off = cmd_ix - win_base;
+    if (off > WIN_WORDS - 4u) {
+        win_base = cmd_ix & ~3u;
+        __syncwarp();
+        if (lane == 0u) {
+            mbar_expect_tx(&io.mbar[buf], WIN_WORDS * 4u);
+            bulk_g2s(io.ptcl[buf], ptcl + win_base, WIN_WORDS * 4u, &io.mbar[buf]);
+        }
+        fine_wait(io, buf, phase);
+        off = cmd_ix - win_base;
+    }
+    return io.ptcl[buf] + off;
+}
+
+// ---- the persistent tile loop of both kernels. For every tile of the launch's queue it calls
+// paint(io, S, lut, tile_ix, cell, gx, gy, start, buf, phase): the warp's command windows and MSAA state, the mask LUT, the
+// tile's index in the frame's tile grid, the cell of a batch, the lane's pixels (cell row gy, columns gx..gx+7), the PTCL
+// offset the tile starts at, and the window its commands are staged in (wait for it with fine_wait).
+template <int AA, bool DMG, class Paint>
+__device__ __forceinline__ void fine_tiles(const VbConfig &cfg, const FineArgs &A, Paint &&paint) {
     extern __shared__ __align__(16) unsigned char smem[];
     typedef WarpMs<AA == 0 ? 1 : AA> Ms;
-    const uint32_t *__restrict__ ptcl = A.ptcl;
-    const uint32_t *__restrict__ info = A.info;
     if (A.bump->failed != 0u) return; // upstream failure (the reference flags it through ptcl[0], path_tiling_setup.wgsl:25; see vb_frame.cu)
     const uint32_t lane = vb_lane(), warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+    const FineQueue q = fine_queue<DMG>(cfg, A, lane);
+    // a CTA none of whose warps has a tile leaves before its set-up (k_fine after k_fine_solid when few or no tiles are flagged)
+    if (blockIdx.x * n_warps >= q.n_tiles) return;
     uint32_t *lut = reinterpret_cast<uint32_t *>(smem);
     uint64_t *lut_bar = reinterpret_cast<uint64_t *>(smem + FineSmem<AA>::LUT_WORDS * 4u);
     WarpIo &io = *reinterpret_cast<WarpIo *>(smem + FineSmem<AA>::LUT_WORDS * 4u + 16u + warp * (uint32_t)sizeof(WarpIo));
@@ -970,54 +1063,29 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
         }
     }
 
-    // ---- tile queue. Tiles of the window are numbered row-major; warp g of G takes tiles g and g + G, then whatever
-    // the queue hands out (2G + atomicAdd). The pipeline is three tiles deep: while tile k is painted, the command
-    // window of tile k+1 is in flight (bulk copy), the occlusion start of tile k+2 is being loaded and the queue
-    // ticket of tile k+3 is being taken, so none of those latencies is exposed.
+    // ---- tile queue. Warp g of G takes queue positions g and g + G, then whatever the queue hands out (2G + atomicAdd). The
+    // pipeline is three tiles deep: while tile k is painted, the command window of tile k+1 is in flight (bulk copy), the
+    // occlusion start of tile k+2 is being loaded and the queue ticket of tile k+3 is being taken, so none of those latencies
+    // is exposed.
     const uint32_t wt = cfg.width_in_tiles;
-    uint32_t n_tiles = wt * (cfg.win_ty1 - cfg.win_ty0);
+    const uint32_t n_tiles = q.n_tiles;
     const uint32_t G = gridDim.x * n_warps, g = blockIdx.x * n_warps + warp;
     const uint32_t first_tile = cfg.win_ty0 * wt;
 #define START_OF(t, s0) ((s0) != 0u && A.cull != 0u ? (s0) : (first_tile + (t)) * VB_PTCL_INITIAL_ALLOC + 1u)
-    // Queue position -> {tile of the window, occlusion start}. coarse sorted the window's tiles into VB_FINE_CLASSES lists by
-    // estimated cost; walking them in class order makes the heavy tiles the FIRST ones every warp takes (longest-processing-
-    // time-first), which is what bounds a persistent kernel's tail when a stripe has only a few tiles per warp.
-    uint32_t cpre[VB_FINE_CLASSES]; // first queue position of each class
-    bool ordered = A.cls_count != nullptr;
-    if (ordered) {
-        uint32_t acc = 0u;
-#pragma unroll
-        for (uint32_t k = 0; k < VB_FINE_CLASSES; k++) {
-            cpre[k] = acc;
-            acc += min(__ldg(A.cls_count + k), A.cls_stride);
-        }
-        if (DMG) n_tiles = acc;
-        ordered = DMG || acc == n_tiles; // a launch over part of the window (read-back bands) keeps the natural order
-    }
-    auto entry_of = [&](uint32_t pos) -> uint2 {
-        if (ordered) {
-            uint32_t k = 0u;
-#pragma unroll
-            for (uint32_t q = 1; q < VB_FINE_CLASSES; q++)
-                if (pos >= cpre[q]) k = q;
-            return __ldg(A.cls_list + (size_t)k * A.cls_stride + (pos - cpre[k]));
-        }
-        return make_uint2(pos, A.cull != 0u ? __ldg(A.tile_start + first_tile + pos) : 0u);
-    };
     uint32_t p_cur = g, p_nxt = g + G; // queue positions
     uint32_t buf = 0u, phase = 0u; // phase: bit b = parity to wait for on mbar[b]
     uint32_t t_cur = 0u, start_cur = 0u, ticket = 0u;
     uint2 e_nxt = make_uint2(0u, 0u);
     if (p_cur < n_tiles) {
-        const uint2 e = entry_of(p_cur);
+        const uint2 e = fine_entry(cfg, A, q, p_cur);
         t_cur = e.x;
         start_cur = START_OF(e.x, e.y);
         if (lane == 0u) {
             mbar_expect_tx(&io.mbar[0], WIN_WORDS * 4u);
-            bulk_g2s(io.ptcl[0], ptcl + (start_cur & ~3u), WIN_WORDS * 4u, &io.mbar[0]);
+            bulk_g2s(io.ptcl[0], A.ptcl + (start_cur & ~3u), WIN_WORDS * 4u, &io.mbar[0]);
             ticket = atomicAdd(A.queue, 1u);
         }
-        if (p_nxt < n_tiles) e_nxt = entry_of(p_nxt);
+        if (p_nxt < n_tiles) e_nxt = fine_entry(cfg, A, q, p_nxt);
     }
     if (AA != 0) mbar_wait(lut_bar, 0u); // every thread of the CTA observes the LUT copy before its first use
 
@@ -1028,12 +1096,12 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
         const uint32_t start_nxt = START_OF(e_nxt.x, e_nxt.y);
         if (p_nxt < n_tiles && lane == 0u) {
             mbar_expect_tx(&io.mbar[buf ^ 1u], WIN_WORDS * 4u);
-            bulk_g2s(io.ptcl[buf ^ 1u], ptcl + (start_nxt & ~3u), WIN_WORDS * 4u, &io.mbar[buf ^ 1u]);
+            bulk_g2s(io.ptcl[buf ^ 1u], A.ptcl + (start_nxt & ~3u), WIN_WORDS * 4u, &io.mbar[buf ^ 1u]);
         }
         const uint32_t p_nn = 2u * G + __shfl_sync(VB_FULL, ticket, 0);
         uint2 e_nn = make_uint2(0u, 0u);
         if (p_nn < n_tiles) {
-            e_nn = entry_of(p_nn);
+            e_nn = fine_entry(cfg, A, q, p_nn);
             if (lane == 0u) ticket = atomicAdd(A.queue, 1u);
         }
 
@@ -1044,6 +1112,101 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
         uint32_t cell = 0u;
         if (cfg.n_cells > 1u) cell = tile_y / cfg.height_in_tiles;
         const uint32_t gx = tile_x * 16u + h * 8u, gy = (tile_y - cell * cfg.height_in_tiles) * 16u + ly;
+        paint(io, S, lut, tile_ix, cell, gx, gy, start_cur, buf, phase);
+        __syncwarp();
+        p_cur = p_nxt; t_cur = t_nxt; start_cur = start_nxt;
+        p_nxt = p_nn; e_nxt = e_nn;
+        buf ^= 1u;
+    }
+#undef START_OF
+}
+
+// ---- store: rgba8unorm with separated alpha (fine.wgsl:1386-1397). When every pixel of the warp is opaque (the common case)
+// a_inv is exactly 1 and the three multiplications are identities, so they are skipped. FI_DST also stores premultiplied alpha
+// (unorm8 of each channel) and float texels (store_float).
+template <bool DST, class Args>
+__device__ __forceinline__ void fine_store(const VbConfig &cfg, const Args &A, rgba_t (&rgba)[PX], uint32_t tile_ix, uint32_t gx, uint32_t gy) {
+    bool opaque = true;
+#pragma unroll
+    for (int i = 0; i < PX; i++) opaque = opaque && rgba[i].a == 1.0f;
+    const bool all_opaque = __all_sync(VB_FULL, opaque);
+    bool float_texels = false, premul = false; // FI_DST: a float destination, premultiplied alpha
+    if constexpr (DST) {
+        float_texels = A.texel != 4u;
+        premul = A.premul != 0u;
+    }
+    if (float_texels && gy < cfg.target_height && gy >= cfg.out_row0) {
+        if constexpr (DST) store_float(A, cfg, rgba, gx, gy, all_opaque);
+    } else if (gy < cfg.target_height && gy >= cfg.out_row0) {
+        uint32_t px[PX];
+        if (all_opaque) {
+#pragma unroll
+            for (int i = 0; i < PX; i++) px[i] = unorm8(rgba[i].r) | (unorm8(rgba[i].g) << 8) | (unorm8(rgba[i].b) << 16) | 0xff000000u;
+        } else if (premul) {
+#pragma unroll
+            for (int i = 0; i < PX; i++) px[i] = pack4x8unorm(rgba[i]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < PX; i++) {
+                const rgba_t fg = rgba[i];
+                const float a_inv = 1.0f / fmaxf(fg.a, 1e-6f);
+                px[i] = unorm8(fg.r * a_inv) | (unorm8(fg.g * a_inv) << 8) | (unorm8(fg.b * a_inv) << 16) | (unorm8(fg.a) << 24);
+            }
+        }
+        bool stored = false;
+        if constexpr (DST) {
+#pragma unroll
+            for (int i = 0; i < PX; i++) px[i] = __byte_perm(px[i], 0u, A.swz);
+            if (A.array) {
+                // gy is the frame's own row, also in a window. Texels out of the array's range are dropped
+                // (cudaBoundaryModeZero), though the host refuses a frame that does not fit before it is enqueued.
+                const uint32_t x = A.x0 + gx, y = A.y0 + gy;
+                if (gx + 7u < cfg.target_width && (x & 3u) == 0u) {
+                    // two 128-bit stores: 32 contiguous bytes of one texel row per lane
+                    surf2Dwrite(make_uint4(px[0], px[1], px[2], px[3]), A.surf, (int)(x * 4u), (int)y, cudaBoundaryModeZero);
+                    surf2Dwrite(make_uint4(px[4], px[5], px[6], px[7]), A.surf, (int)(x * 4u + 16u), (int)y, cudaBoundaryModeZero);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < PX; i++)
+                        if (gx + i < cfg.target_width) surf2Dwrite(px[i], A.surf, (int)((x + i) * 4u), (int)y, cudaBoundaryModeZero);
+                }
+                stored = true;
+            }
+        }
+        if (!stored) {
+            // the cell again, from the tile index (keeping it live across the interpreter would cost a register)
+            const uint32_t out_cell = cfg.n_cells > 1u ? tile_ix / cfg.width_in_tiles / cfg.height_in_tiles : 0u;
+            uint32_t *row = A.out + ((size_t)out_cell * cfg.target_height + (gy - cfg.out_row0)) * cfg.out_pitch_px;
+            if (gx + 7u < cfg.target_width && (cfg.out_pitch_px & 3u) == 0u && ((uintptr_t)A.out & 15u) == 0u) {
+                // two 128-bit stores: 32 contiguous bytes of one pixel row per lane
+                uint4 *dst = reinterpret_cast<uint4 *>(row + gx);
+                dst[0] = make_uint4(px[0], px[1], px[2], px[3]);
+                dst[1] = make_uint4(px[4], px[5], px[6], px[7]);
+            } else {
+#pragma unroll
+                for (int i = 0; i < PX; i++)
+                    if (gx + i < cfg.target_width) row[gx + i] = px[i];
+            }
+        }
+    }
+}
+
+// ---- k_fine: the whole interpreter. It paints every tile of a frame, or only the flagged ones after k_fine_solid.
+template <int MODE>
+__global__ void __launch_bounds__(FI_MAX_THREADS, FI_MINB)
+k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
+    constexpr int AA = MODE & 15;
+    constexpr bool DMG = (MODE & FI_DMG) != 0;
+    constexpr bool DST = (MODE & FI_DST) != 0;
+    constexpr bool BG = (MODE & FI_BG) != 0;
+    static_assert(!BG || (DST && !DMG), "FI_BG goes with FI_DST and without FI_DMG");
+    typedef WarpMs<AA == 0 ? 1 : AA> Ms;
+    const uint32_t *__restrict__ ptcl = A.ptcl;
+    const uint32_t *__restrict__ info = A.info;
+    const uint32_t lane = vb_lane();
+    const uint32_t ly = lane >> 1, h = lane & 1u;
+    fine_tiles<AA, DMG>(cfg, A, [&](WarpIo &io, Ms &S, const uint32_t *lut, uint32_t tile_ix, uint32_t cell, uint32_t gx, uint32_t gy,
+                                    uint32_t start_cur, uint32_t buf, uint32_t &phase) {
         // pixel coordinates are small integers: (float)(gx + i) is exactly the WGSL's xy.x + f32(i) of either 4-pixel group
 #define xyy ((float)gy)
 #define xyx0 ((float)gx)
@@ -1072,50 +1235,29 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
         uint32_t clip_depth = 0u;
         uint32_t cmd_ix = start_cur;
         uint32_t win_base = start_cur & ~3u;
-        mbar_wait(&io.mbar[buf], (phase >> buf) & 1u);
-        phase ^= 1u << buf;
+        fine_wait(io, buf, phase);
 #define PXX(i) ((((i) < 4) ? xyx0 : xyx1) + (float)((i) & 3))
         // The rarely used brushes loop over the lane's pixels WITHOUT unrolling (code size); they work on a copy in local
         // memory so that rgba[] / area[] themselves are only ever indexed by constants and live in registers.
 #define PIX_TO_LOCAL() _Pragma("unroll") for (int q_ = 0; q_ < PX; q_++) { t_rgba[q_] = rgba[q_]; t_area[q_] = area[q_]; }
 #define PIX_FROM_LOCAL() _Pragma("unroll") for (int q_ = 0; q_ < PX; q_++) rgba[q_] = t_rgba[q_]
         for (;;) {
-            // the command word and its (up to 3) operands come from the staged window; when the pointer leaves the
-            // window (a list longer than the window, CMD_JUMP into another chunk) the window is staged again there
-            uint32_t off = cmd_ix - win_base;
-            if (off > WIN_WORDS - 4u) {
-                win_base = cmd_ix & ~3u;
-                __syncwarp();
-                if (lane == 0u) {
-                    mbar_expect_tx(&io.mbar[buf], WIN_WORDS * 4u);
-                    bulk_g2s(io.ptcl[buf], ptcl + win_base, WIN_WORDS * 4u, &io.mbar[buf]);
-                }
-                mbar_wait(&io.mbar[buf], (phase >> buf) & 1u);
-                phase ^= 1u << buf;
-                off = cmd_ix - win_base;
-            }
-            const uint32_t *cw = io.ptcl[buf] + off;
+            const uint32_t *cw = fine_cmd_words(io, ptcl, cmd_ix, win_base, buf, phase, lane);
             const uint32_t tag = cw[0];
             const uint32_t w1 = cw[1], w2 = cw[2], w3 = cw[3];
             if (tag == VB_CMD_END) break;
             switch (tag) {
             case VB_CMD_FILL: {
-                const uint32_t sr = w1, sd = w2;
-                const int32_t bd = (int32_t)w3;
-                if (AA == 0) fill_path_area(A, sr, sd, bd, (float)(h * 8u), (float)ly, area);
-                else fill_path_ms<AA == 0 ? 1 : AA>(A, S, lut, sr, sd, bd, lane, area);
+                fine_cmd_fill<AA>(A, S, lut, w1, w2, (int32_t)w3, lane, area);
                 cmd_ix += 4u;
                 break;
             }
             case VB_CMD_SOLID:
-#pragma unroll
-                for (int i = 0; i < PX; i++) area[i] = 1.0f;
+                fine_cmd_solid(area);
                 cmd_ix += 1u;
                 break;
             case VB_CMD_COLOR: {
-                const rgba_t fg = unpack4x8unorm_uniform(w1);
-#pragma unroll
-                for (int i = 0; i < PX; i++) rgba[i] = over(rgba[i], rg_scale(fg, area[i]));
+                fine_cmd_color(w1, rgba, area);
                 cmd_ix += 2u;
                 break;
             }
@@ -1365,83 +1507,60 @@ k_fine(VbConfig cfg, FineArgsOf<MODE> A) {
 #undef xyy
 #undef xyx0
 #undef xyx1
-        // ---- store: rgba8unorm with separated alpha (fine.wgsl:1386-1397). When every pixel of the warp is opaque
-        // (the common case) a_inv is exactly 1 and the three multiplications are identities, so they are skipped. FI_DST also
-        // stores premultiplied alpha (unorm8 of each channel) and float texels (store_float).
-        bool opaque = true;
+        fine_store<DST>(cfg, A, rgba, tile_ix, gx, gy);
+    });
+}
+
+// ---- k_fine_solid: the lean interpreter of the tiles that run only FILL / SOLID / COLOR / JUMP from their occlusion start
+// (coarse's simple lists), with the same tile loop, commands and store as k_fine, so a tile's pixels are the same bits
+// whichever kernel paints it. Without the blend stack, the brushes' pixel copies and their code it needs no stack and fits
+// FI_SOLID_WARPS x FI_SOLID_MINB resident warps per SM (DESIGN §3 "fine").
+template <int AA>
+__global__ void __launch_bounds__(32 * FI_SOLID_WARPS, FI_SOLID_MINB)
+k_fine_solid(VbConfig cfg, FineArgs A) {
+    typedef WarpMs<AA == 0 ? 1 : AA> Ms;
+    const uint32_t lane = vb_lane();
+    fine_tiles<AA, false>(cfg, A, [&](WarpIo &io, Ms &S, const uint32_t *lut, uint32_t tile_ix, uint32_t, uint32_t gx, uint32_t gy,
+                                      uint32_t start_cur, uint32_t buf, uint32_t &phase) {
+        rgba_t rgba[PX];
+        float area[PX];
+        {
+            const rgba_t base = unpack4x8unorm_uniform(cfg.base_color);
 #pragma unroll
-        for (int i = 0; i < PX; i++) opaque = opaque && rgba[i].a == 1.0f;
-        const bool all_opaque = __all_sync(VB_FULL, opaque);
-        bool float_texels = false, premul = false; // FI_DST: a float destination, premultiplied alpha
-        if constexpr (DST) {
-            float_texels = A.texel != 4u;
-            premul = A.premul != 0u;
+            for (int i = 0; i < PX; i++) { rgba[i] = base; area[i] = 0.0f; }
         }
-        if (float_texels && gy < cfg.target_height && gy >= cfg.out_row0) {
-            if constexpr (DST) store_float(A, cfg, rgba, gx, gy, all_opaque);
-        } else if (gy < cfg.target_height && gy >= cfg.out_row0) {
-            uint32_t px[PX];
-            if (all_opaque) {
-#pragma unroll
-                for (int i = 0; i < PX; i++) px[i] = unorm8(rgba[i].r) | (unorm8(rgba[i].g) << 8) | (unorm8(rgba[i].b) << 16) | 0xff000000u;
-            } else if (premul) {
-#pragma unroll
-                for (int i = 0; i < PX; i++) px[i] = pack4x8unorm(rgba[i]);
+        uint32_t cmd_ix = start_cur;
+        uint32_t win_base = start_cur & ~3u;
+        fine_wait(io, buf, phase);
+        for (;;) {
+            const uint32_t *cw = fine_cmd_words(io, A.ptcl, cmd_ix, win_base, buf, phase, lane);
+            const uint32_t tag = cw[0];
+            if (tag == VB_CMD_END) break;
+            if (tag == VB_CMD_FILL) {
+                fine_cmd_fill<AA>(A, S, lut, cw[1], cw[2], (int32_t)cw[3], lane, area);
+                cmd_ix += 4u;
+            } else if (tag == VB_CMD_SOLID) {
+                fine_cmd_solid(area);
+                cmd_ix += 1u;
+            } else if (tag == VB_CMD_COLOR) {
+                fine_cmd_color(cw[1], rgba, area);
+                cmd_ix += 2u;
+            } else if (tag == VB_CMD_JUMP) {
+                cmd_ix = cw[1];
             } else {
-#pragma unroll
-                for (int i = 0; i < PX; i++) {
-                    const rgba_t fg = rgba[i];
-                    const float a_inv = 1.0f / fmaxf(fg.a, 1e-6f);
-                    px[i] = unorm8(fg.r * a_inv) | (unorm8(fg.g * a_inv) << 8) | (unorm8(fg.b * a_inv) << 16) | (unorm8(fg.a) << 24);
-                }
-            }
-            bool stored = false;
-            if constexpr (DST) {
-#pragma unroll
-                for (int i = 0; i < PX; i++) px[i] = __byte_perm(px[i], 0u, A.swz);
-                if (A.array) {
-                    // gy is the frame's own row, also in a window. Texels out of the array's range are dropped
-                    // (cudaBoundaryModeZero), though the host refuses a frame that does not fit before it is enqueued.
-                    const uint32_t x = A.x0 + gx, y = A.y0 + gy;
-                    if (gx + 7u < cfg.target_width && (x & 3u) == 0u) {
-                        // two 128-bit stores: 32 contiguous bytes of one texel row per lane
-                        surf2Dwrite(make_uint4(px[0], px[1], px[2], px[3]), A.surf, (int)(x * 4u), (int)y, cudaBoundaryModeZero);
-                        surf2Dwrite(make_uint4(px[4], px[5], px[6], px[7]), A.surf, (int)(x * 4u + 16u), (int)y, cudaBoundaryModeZero);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < PX; i++)
-                            if (gx + i < cfg.target_width) surf2Dwrite(px[i], A.surf, (int)((x + i) * 4u), (int)y, cudaBoundaryModeZero);
-                    }
-                    stored = true;
-                }
-            }
-            if (!stored) {
-                // the cell again, from the tile index (keeping it live across the interpreter would cost a register)
-                const uint32_t out_cell = cfg.n_cells > 1u ? tile_ix / wt / cfg.height_in_tiles : 0u;
-                uint32_t *row = A.out + ((size_t)out_cell * cfg.target_height + (gy - cfg.out_row0)) * cfg.out_pitch_px;
-                if (gx + 7u < cfg.target_width && (cfg.out_pitch_px & 3u) == 0u && ((uintptr_t)A.out & 15u) == 0u) {
-                    // two 128-bit stores: 32 contiguous bytes of one pixel row per lane
-                    uint4 *dst = reinterpret_cast<uint4 *>(row + gx);
-                    dst[0] = make_uint4(px[0], px[1], px[2], px[3]);
-                    dst[1] = make_uint4(px[4], px[5], px[6], px[7]);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < PX; i++)
-                        if (gx + i < cfg.target_width) row[gx + i] = px[i];
-                }
+                cmd_ix += 1u; // not in a simple list (k_fine's default)
             }
         }
-        __syncwarp();
-        p_cur = p_nxt; t_cur = t_nxt; start_cur = start_nxt;
-        p_nxt = p_nn; e_nxt = e_nn;
-        buf ^= 1u;
-    }
-#undef START_OF
+        fine_store<false>(cfg, A, rgba, tile_ix, gx, gy);
+    });
 }
 
 typedef cudaError_t (*FineInit)();
 template <int MODE> static cudaError_t fine_smem_limit() {
     return cudaFuncSetAttribute(k_fine<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<MODE & 15>::bytes(FI_MAX_WARPS));
+}
+template <int AA> static cudaError_t fine_solid_smem_limit() {
+    return cudaFuncSetAttribute(k_fine_solid<AA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FineSmem<AA>::bytes(FI_SOLID_WARPS));
 }
 // c_unorm of this object (k_fine.o and k_fine_bg.o each have their own), and the shared-memory limits of the kernels in `set`
 static cudaError_t fine_init(const FineInit *set, int n) {
@@ -1480,25 +1599,30 @@ extern "C" int vb_fine_init_constants(void) {
     const FineInit set[] = {
         fine_smem_limit<0>, fine_smem_limit<0 + FI_DMG>, fine_smem_limit<0 + FI_DST>, fine_smem_limit<0 + FI_DST + FI_DMG>,
         fine_smem_limit<1>, fine_smem_limit<1 + FI_DMG>, fine_smem_limit<1 + FI_DST>, fine_smem_limit<1 + FI_DST + FI_DMG>,
-        fine_smem_limit<2>, fine_smem_limit<2 + FI_DMG>, fine_smem_limit<2 + FI_DST>, fine_smem_limit<2 + FI_DST + FI_DMG>};
-    const cudaError_t e = fine_init(set, 12);
+        fine_smem_limit<2>, fine_smem_limit<2 + FI_DMG>, fine_smem_limit<2 + FI_DST>, fine_smem_limit<2 + FI_DST + FI_DMG>,
+        fine_solid_smem_limit<0>, fine_solid_smem_limit<1>, fine_solid_smem_limit<2>};
+    const cudaError_t e = fine_init(set, 15);
     return e != cudaSuccess ? (int)e : vb_fine_bg_init();
 }
 
+// Persistent grid of `max_warps`-warp CTAs, `minb` per SM, for n tiles: small frames get smaller CTAs so that their tiles still
+// spread over the SMs.
+static void fine_grid(uint32_t n, int sm_count, uint32_t max_warps, uint32_t minb, uint32_t *grid, uint32_t *warps) {
+    uint32_t w = max_warps;
+    while (w > 2u && (n + w - 1u) / w < (uint32_t)sm_count * minb) w >>= 1;
+    *warps = w;
+    *grid = std::min((n + w - 1u) / w, (uint32_t)sm_count * minb * (max_warps / w));
+}
+
 // The launch's tile queue is control-block word VB_CTL_FINE_QUEUE + band, zeroed with the control block (8 of them, one per
-// read-back band).
+// read-back band); the k_fine after k_fine_solid takes VB_CTL_FINE_QUEUE_FLAGGED.
 extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, const VbFineOut &o, const VbFineBg &bg, int aa, uint32_t cull,
                                    uint32_t band, bool cls_order, cudaStream_t st) {
     uint32_t rows = cfg.win_ty1 - cfg.win_ty0;
     uint32_t n = cfg.width_in_tiles * rows;
     if (n == 0) return 0;
-    // persistent grid: FI_MINB CTAs per SM; small frames get smaller CTAs so that their tiles still spread over the SMs
-    const int sm_count = b.sm_count;
-    uint32_t warps = FI_MAX_WARPS;
-    while (warps > 2u && (n + warps - 1u) / warps < (uint32_t)sm_count * FI_MINB) warps >>= 1;
-    uint32_t grid = (n + warps - 1u) / warps;
-    const uint32_t resident = (uint32_t)sm_count * FI_MINB * (FI_MAX_WARPS / warps);
-    if (grid > resident) grid = resident;
+    uint32_t grid, warps;
+    fine_grid(n, b.sm_count, FI_MAX_WARPS, FI_MINB, &grid, &warps);
     FineBgArgs A;
     A.segments = b.segments; A.ptcl = b.ptcl; A.info = b.info_bin_data; A.blend_spill = b.blend_spill; A.out = o.out; A.ramps = b.ramps; A.atlas = b.atlas;
     A.mask_lut = aa == 2 ? b.mask16 : b.mask8;
@@ -1509,6 +1633,7 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     A.cls_list = b.cls_list;
     A.cls_count = cls_order ? b.ctl + VB_CTL_FINE_CLASS : nullptr;
     A.cls_stride = cfg.width_in_tiles * cfg.tile_rows;
+    A.lists = FI_LISTS_ALL;
     A.surf = o.surf;
     A.swz = o.swz;
     A.array = o.array;
@@ -1529,9 +1654,24 @@ extern "C" uint32_t vb_launch_fine(const VbConfig &cfg, const VbFrameBufs &b, co
     } else if (o.dst) {
         if (dmg) launch_fine<FI_DST + FI_DMG>(aa, grid, warps, st, cfg, A);
         else launch_fine<FI_DST>(aa, grid, warps, st, cfg, A);
+    } else if (dmg) {
+        launch_fine<FI_DMG>(aa, grid, warps, st, cfg, A);
+    } else if (cls_order && cull != 0u) {
+        // the simple tiles' lists in k_fine_solid, then the flagged ones in k_fine, whose tile count is read on the device (its
+        // CTAs leave at once when there are none). Both grids are the machine's: only the lists say which tiles each paints.
+        uint32_t grid_s, warps_s;
+        fine_grid(n, b.sm_count, FI_SOLID_WARPS, FI_SOLID_MINB, &grid_s, &warps_s);
+        FineArgs As = A;
+        As.lists = FI_LISTS_SIMPLE;
+        if (aa == 0) k_fine_solid<0><<<grid_s, 32u * warps_s, FineSmem<0>::bytes(warps_s), st>>>(cfg, As);
+        else if (aa == 1) k_fine_solid<1><<<grid_s, 32u * warps_s, FineSmem<1>::bytes(warps_s), st>>>(cfg, As);
+        else k_fine_solid<2><<<grid_s, 32u * warps_s, FineSmem<2>::bytes(warps_s), st>>>(cfg, As);
+        A.lists = FI_LISTS_FLAGGED;
+        A.queue = b.ctl + VB_CTL_FINE_QUEUE_FLAGGED;
+        launch_fine<0>(aa, grid, warps, st, cfg, A);
+        return 2;
     } else {
-        if (dmg) launch_fine<FI_DMG>(aa, grid, warps, st, cfg, A);
-        else launch_fine<0>(aa, grid, warps, st, cfg, A);
+        launch_fine<0>(aa, grid, warps, st, cfg, A);
     }
     return 1;
 }

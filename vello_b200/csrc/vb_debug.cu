@@ -166,6 +166,13 @@ extern "C" int vb_debug_download(vb_renderer *r, const char *name, void *dst, si
         if (dst && cap >= 4) CK(cudaMemcpy(dst, (const uint32_t *)r->fb[FB_CTL].p + VB_CTL_SEG_HOLES, 4, cudaMemcpyDeviceToHost));
         return VB_OK;
     }
+    // the tile counts of fine's lists in the last frame (k_coarse.cu): VB_FINE_LISTS words, list 2k + 1 the flagged tiles of class k
+    if (!strcmp(name, "fine_lists")) {
+        if (bytes) *bytes = VB_FINE_LISTS * 4;
+        if (dst && cap >= VB_FINE_LISTS * 4)
+            CK(cudaMemcpy(dst, (const uint32_t *)r->fb[FB_CTL].p + VB_CTL_FINE_CLASS, VB_FINE_LISTS * 4, cudaMemcpyDeviceToHost));
+        return VB_OK;
+    }
     if (!strcmp(name, "config")) {
         if (bytes) *bytes = sizeof(VbConfig);
         if (dst && cap >= sizeof(VbConfig)) memcpy(dst, &r->cfg, sizeof(VbConfig));

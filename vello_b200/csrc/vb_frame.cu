@@ -109,7 +109,7 @@ const FrameBufDesc vb_host::FRAME_BUFS[N_FRAME_BUFS] = {
      [](const FrameCounts &n, bool download) { return (download ? n.draws : (size_t)n.draw_parts * 256u) * sizeof(VbPath); }},
     {"tile_start", FIELD(tile_start), false, [](const FrameCounts &n, bool) { return ((size_t)n.tiles + 256) * 4; }},
     // fine's cost-ordered tile lists
-    {"cls_list", FIELD(cls_list), false, [](const FrameCounts &n, bool) { return (size_t)VB_FINE_CLASSES * n.tiles * 8; }},
+    {"cls_list", FIELD(cls_list), true, [](const FrameCounts &n, bool) { return (size_t)VB_FINE_LISTS * n.tiles * 8; }},
     {"flatten_parts", FIELD(flatten_parts), false, [](const FrameCounts &n, bool) { return vb_flatten_part_words(n.flatten_parts) * 4; }},
     {"ctl", FIELD(ctl), false, [](const FrameCounts &n, bool) { return n.ctl_words * 4; }},
     // the arenas' buffers, from FB_LINES on
@@ -552,9 +552,9 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
         launches++;
     }
     else if (clear_queues) {
-        if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_QUEUE, 0, 8 * sizeof(uint32_t), st));
+        if (last >= VB_STAGE_ID_FINE) CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_QUEUE, 0, 9 * sizeof(uint32_t), st)); // and the flagged queue
         if (first <= VB_STAGE_ID_COARSE && last >= VB_STAGE_ID_COARSE)
-            CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_CLASSES * sizeof(uint32_t), st));
+            CK(cudaMemsetAsync(b.ctl + VB_CTL_FINE_CLASS, 0, VB_FINE_LISTS * sizeof(uint32_t), st));
         if (first <= VB_STAGE_ID_BACKDROP && last >= VB_STAGE_ID_BACKDROP)
             CK(cudaMemsetAsync(b.lb_backdrop, 0, VB_LB_ZERO_WORDS(b.parts_backdrop) * sizeof(uint32_t), st));
     }

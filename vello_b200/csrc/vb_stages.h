@@ -103,7 +103,7 @@ struct VbFrameBufs {
     VbBinHeader *bin_headers;
     VbPath *paths;
     uint32_t *tile_start;
-    uint2 *cls_list; // fine's cost-ordered tile lists, written by coarse: VB_FINE_CLASSES x (width_in_tiles * tile_rows)
+    uint2 *cls_list; // fine's cost-ordered tile lists, written by coarse: VB_FINE_LISTS x (width_in_tiles * tile_rows)
     // bump arenas, and flatten's scratch arenas sized from the lines capacity
     VbLineSoup *lines;
     FlLit *line_scratch;

@@ -33,9 +33,13 @@ typedef struct { uint32_t failed, binning, ptcl, tile, seg_counts, segments, ble
 #define VB_CTL_SEG_HOLES 8
 /* words 16..23: fine's tile queues, one per launch of a frame (up to 8 read-back bands); the header is 32 words */
 #define VB_CTL_FINE_QUEUE 16
-/* words 24..31: fill counts of fine's cost-class tile lists (written by coarse) */
-#define VB_CTL_FINE_CLASS 24
+/* word 24: the tile queue of the full fine kernel that follows the lean one (k_fine.cu, FI_LISTS_FLAGGED) */
+#define VB_CTL_FINE_QUEUE_FLAGGED 24
+/* words 48..63: fill counts of fine's tile lists (written by coarse): VB_FINE_CLASSES cost classes, each split into the tiles
+ * that run only FILL / SOLID / COLOR / JUMP from their occlusion start (list 2k) and the others (list 2k + 1) */
+#define VB_CTL_FINE_CLASS 48
 #define VB_FINE_CLASSES 8
+#define VB_FINE_LISTS (2 * VB_FINE_CLASSES)
 /* words 32..47: per-destination counts and cursors of the multi-GPU line routing (k_exchange.cu) */
 #define VB_CTL_XCHG_SCRATCH 32
 #define VB_CTL_HEADER_WORDS 64
