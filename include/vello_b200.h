@@ -777,6 +777,52 @@ int vb_bind_draw_visibility(vb_renderer *, const uint8_t *device_flags, uint32_t
  * memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 4, or 4 GiB or more; a renderer of a vb_group or
  * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish. */
 int vb_bind_stroke_widths(vb_renderer *, const float *device_widths, uint32_t n, size_t row_pitch_bytes);
+/* Bind the opacity of the installed scene's layers and images to device memory (an addition; no vello counterpart). Panels,
+ * map layers, tooltips and Lottie-style groups fade, and images or video frames cross-fade, without re-encoding or re-uploading
+ * the scene (which would unbind every binding), and without a host call per frame. A layer's alpha cannot be made from bound
+ * colours: a group's alpha is not the product of its children's alphas where they overlap, and gradient and image children
+ * have no bound colour.
+ *  - Rows. Row k is the f32 at device_alpha + k * row_pitch_bytes and belongs to draw object k of the installed scene: the
+ *    indices of vb_hit_test and Scene.n_draw_objects, global in a composed scene and in cell order in a batch. Draw objects
+ *    from n on keep their encoded values.
+ *  - Which rows apply. A row applies only when it is finite; a NaN or infinite row keeps the encoded words for that frame. A
+ *    finite row is first clamped to [0, 1], as vb_scene_push_layer clamps its alpha.
+ *     - A layer (the BEGIN_CLIP of any push_*_layer: blend, luminance-mask and clip layers): its alpha becomes the row. The
+ *       row of its END_CLIP is ignored.
+ *     - A clip layer (blend word CLIP_BLEND_MODE, 0x8003) with a row below 1 is also drawn as a Normal / SrcOver layer (blend
+ *       word 3): the frame renders what push_layer(Mix::Normal, Compose::SrcOver, row, ...) renders in place of
+ *       push_clip_layer. A clip layer's blend skips the tiles wholly inside its clip, so without the change only its edge tiles
+ *       would fade. With a row of 1 the clip layer is drawn exactly as encoded.
+ *     - An image (draw_image, or an image brush): the low byte of its sample word becomes int(row * 255 + 0.5), the encoders'
+ *       conversion with each step rounded on its own. The row takes the place of the image's alpha times the brush alpha; the
+ *       format, alpha type, quality and extends are kept.
+ *     - Rows of solid fills, strokes, gradients and blurred rectangles are ignored: bind their colours or stops instead.
+ *  - What a frame renders. While rows are bound, every frame renders what installing the scene re-encoded with those alphas
+ *    renders (the clip-layer rule included): byte for byte in MSAA8 and MSAA16, and in Area up to the last-bit differences the
+ *    order of a tile's segments makes in its area sums. Opacity changes no geometry, so hit tests and hit maps answer as
+ *    unbound, even at row 0 (hiding is vb_bind_draw_visibility's job).
+ *  - How. The frame reads its draw data from the region past the scene's streams that bound colours and stops write
+ *    (vb_debug_download("draw_data")): at the start of flatten's stage a kernel copies the scene's draw data there, bound
+ *    colours applied, and another one writes the bound alpha, blend and sample words into it. A vb_run_stages range that
+ *    starts at draw writes them again.
+ *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage. The caller orders its
+ *    writes before the frame, on vb_stream or with a synchronisation, and does not write the rows while a frame that reads
+ *    them is running. A blocking frame that is re-run after an arena overflow reads the rows again; an enqueued frame is never
+ *    re-run. The caller keeps the memory alive while it is bound. Changing only the contents replays the captured frame graph.
+ *    Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next frame captures its graph
+ *    anew. With nothing bound a frame launches, configures and captures exactly what it would without this call; bound, it
+ *    launches one kernel more, and one more again when neither colours nor stops are bound (the draw-data copy).
+ *  - Scope. Any installed scene can be bound, packed bytes included. Every scene installation unbinds: every upload form,
+ *    vb_render, vb_render_begin, vb_compose and vb_recompose. The binding survives vb_set_view, vb_set_cells, the seven other
+ *    bindings and hit tests; all eight can be active together. device_alpha NULL unbinds.
+ *  - The call finds the bound words once, with one kernel over the draw tags, and does not synchronise unless its table grows.
+ *    Damage tracking follows the rows (see below).
+ * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
+ * pointer, or n above the scene's draw-object count; a pointer that is not device memory of the renderer's device (or managed
+ * memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 4, or 4 GiB or more; a renderer of a vb_group or
+ * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose draw data passes 2^30
+ * words, or whose regions past its streams would pass 32-bit word offsets. */
+int vb_bind_draw_opacity(vb_renderer *, const float *device_alpha, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello
  * repaints every frame in full) ----
@@ -823,6 +869,11 @@ int vb_bind_stroke_widths(vb_renderer *, const float *device_widths, uint32_t n,
  *    differs bit for bit from the last successful frame's: a fill's row, or a row that falls back to an unchanged encoded
  *    width, is no change. The damage is the tiles of its clipped box in the last frame and in this one; a widened stroke's box
  *    grows, so the new box covers it.
+ *  - Automatic damage, for bound opacity (vb_bind_draw_opacity). Draw object d changed if its opacity word in the frame's draw
+ *    data (a layer's alpha word, an image's sample word) differs bit for bit from the last successful frame's: a row that
+ *    converts to the same word, a non-finite row that falls back to an unchanged encoded word, and the row of any other draw
+ *    object are no change. The damage is the tiles of its clipped box in the last frame and in this one; a layer's is its
+ *    BEGIN_CLIP's box, which holds everything inside the layer and the pixels its blend touches.
  *  - vb_set_damage_tracking(on): switching it on, or calling it again with 1, makes the next frame full. VB_E_INVALID on a
  *    renderer of a vb_group or with the exchange configured.
  *  - vb_add_damage: n half-open pixel rectangles rects[4i .. 4i + 3] = x0 y0 x1 y1, clamped to the frame and rounded out to

@@ -23,7 +23,12 @@
 //   + with bound stroke widths (vb_bind_stroke_widths), for every draw object below the bound count whose width (the one
 //     flatten used: its snapshot entry, or for an entry of 0 its style's width word) differs bit for bit from the last successful
 //     frame's, its tile box in that frame and in this one. A fill's entry is always 0 and its style word never changes, so its
-//     row is no change; neither is a row that falls back to an unchanged encoded width. A wider stroke's new box holds it.
+//     row is no change; neither is a row that falls back to an unchanged encoded width. A wider stroke's new box holds it
+//   + with bound opacity (vb_bind_draw_opacity), for every draw object below the bound count whose opacity word (the one the
+//     frame's draw data holds after k_draw_opacity: a layer's alpha word, an image's sample word) differs bit for bit from the
+//     last successful frame's, its tile box in that frame and in this one. A clip layer's blend word follows from its alpha, and
+//     a layer is covered by its BEGIN_CLIP's box, which holds everything inside the layer and the pixels its blend touches.
+//     Other draw objects have no opacity word, so their rows are no change.
 // Draw boxes are binning's clipped boxes, rounded out to tiles exactly as tile_alloc rounds them, so a draw object paints no
 // pixel outside its box. A moved open clip changes the boxes of later instances' draw objects, but only inside its own old
 // and new box, which its BEGIN_CLIP contributes.
@@ -60,8 +65,9 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
 
 // The inputs of k_damage_mark and k_damage: the snapshot `snap`, laid out by L (its flag arrays: L.changed, L.paths, L.xf), the
 // frame's mask, the words the frame reads and the bindings' tables (VbBound). The mask words `vis` are null without bound
-// visibility, `grad` (VbBound::rs_draw) without a bound gradient, `xf_range` without bound transforms, and the stroke-width
-// snapshot `widths` without bound widths (`styles`: the scene's n_style style words, `path_draw`: pathtag's path table).
+// visibility, `grad` (VbBound::rs_draw) without a bound gradient, `xf_range` without bound transforms, the stroke-width
+// snapshot `widths` without bound widths (`styles`: the scene's n_style style words, `path_draw`: pathtag's path table), and
+// `op_slots` (VbBound::op_slots) without bound opacity.
 struct DmArgs {
     VbDmgLayout L;
     uint32_t *snap;
@@ -73,7 +79,7 @@ struct DmArgs {
     const uint2 *xf_range;
     const float *widths;
     const uint2 *path_draw;
-    const uint32_t *styles;
+    const uint32_t *styles, *op_slots;
     uint32_t compare, wt, ht, n_style;
 };
 
@@ -130,7 +136,7 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const DmArgs a) {
 // reads transforms xf_range[d].x .. .y, each flagged with transforms bound) changed, its old and new boxes into the mask. A draw
 // object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's
 // offset in the frame's draw data (`dd`, the bound region). Below L.n_wid, its stroke width: the snapshot entry, or for 0 the
-// width word of its path's style (path d is draw object d).
+// width word of its path's style (path d is draw object d). Below L.n_op, its opacity word in `dd` (`op_slots`), or 0.
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
     const VbDmgLayout &L = a.L;
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
@@ -157,6 +163,12 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
         }
         hit = w != old[L.wid + d] || hit;
         if (lane == 0u) nxt[L.wid + d] = w;
+    }
+    if (d < L.n_op) {
+        const uint32_t e = __ldg(a.op_slots + d);
+        const uint32_t w = e == VB_COLOR_NONE ? 0u : __ldg(a.dd + (e >> 2));
+        hit = w != old[L.op + d] || hit;
+        if (lane == 0u) nxt[L.op + d] = w;
     }
     const uint32_t g = a.grad ? __ldg(a.grad + d) : VB_COLOR_NONE;
     if (g != VB_COLOR_NONE) {
@@ -221,10 +233,10 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     const uint32_t n_paths = L.paths ? L.n_paths : 0u, n = std::max(std::max(n_tiles, L.n_inst), n_paths);
     k_damage_begin<<<(n + DM_THREADS - 1u) / DM_THREADS, DM_THREADS, 0, st>>>(D.mask, D.pending, n_tiles, full, D.snap + L.changed, L.n_inst,
                                                                               D.snap + L.paths, n_paths);
-    // neither instance transforms, colours, points, stops, transforms, visibility nor stroke widths bound: nothing changes
-    // without a call that makes the frame full
+    // neither instance transforms, colours, points, stops, transforms, visibility, stroke widths nor opacity bound: nothing
+    // changes without a call that makes the frame full
     if (L.n_inst == 0u && L.n_col == 0u && L.n_pt == 0u && L.n_grads == 0u && B.rows[VB_BIND_TRANSFORMS].n == 0u && L.n_vis == 0u &&
-        L.n_wid == 0u)
+        L.n_wid == 0u && L.n_op == 0u)
         return 1u;
     DmArgs a;
     a.L = L, a.snap = D.snap, a.mask = D.mask, a.compare = !full, a.wt = wt, a.ht = ht;
@@ -235,6 +247,7 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     a.xf_range = B.rows[VB_BIND_TRANSFORMS].rows ? B.xf_range : nullptr;
     a.widths = cfg.widths, a.path_draw = b.path_draw, a.styles = b.scene + cfg.layout.style_base;
     a.n_style = cfg.scene_words > cfg.layout.style_base ? cfg.scene_words - cfg.layout.style_base : 0u;
+    a.op_slots = B.op_slots;
     uint32_t launches = 1u;
     const uint32_t n_mark = std::max(std::max(L.n_xf, n_paths ? L.n_pt : 0u), L.n_vis);
     if (n_mark) {

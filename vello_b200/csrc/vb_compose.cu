@@ -591,6 +591,12 @@ static std::string stops_check(const vb_renderer *r, uint32_t n) {
     if ((uint64_t)s.n_ramps + bound_grads(s, n) > (1ull << 30)) return "the scene's ramps and one per bound gradient pass the 30 bits of the ramp word";
     return draw_tags_outside(s, s.layout.n_draw_objects);
 }
+// bound opacity's table packs a draw-data word offset and a 2-bit kind into a word (VB_OP_ENTRY)
+static std::string opacity_check(const vb_renderer *r, uint32_t n) {
+    const Slot &s = *r->cur;
+    if (n_draw_data(s.layout, s.scene_words) >= (1u << 30)) return "the scene's draw data passes the 30 bits of the opacity table";
+    return draw_tags_outside(s, n);
+}
 static std::string no_check(const vb_renderer *, uint32_t) { return {}; }
 
 // The kinds' bind-time work: the tables of n rows in b. `why` is set for a refusal that only the work finds.
@@ -727,11 +733,26 @@ static int visibility_mask(vb_renderer *r, uint32_t, VbBound &, std::string &) {
 static int width_snapshot(vb_renderer *r, uint32_t, VbBound &, std::string &) {
     return compose_room(r, r->width_snap, (size_t)vb_width_entries(r->cur->layout) * 4u);
 }
+// Bound opacity (k_opacity.cu): the word each of the n bound draw objects patches, by one k_draw_opacity_slots over the scene's
+// draw tags and draw data. The call does not synchronise unless the table grows. The draw-data slot table follows (bind_rows).
+static int opacity_table(vb_renderer *r, uint32_t n, VbBound &b, std::string &) {
+    const Slot &slot = *r->cur;
+    const VbLayout &L = slot.layout;
+    int rc;
+    if ((rc = compose_room(r, r->op_slots, (size_t)n * 4u))) return rc;
+    uint32_t *table = (uint32_t *)r->op_slots.p;
+    const uint32_t *scene = (const uint32_t *)slot.scene.p;
+    vb_launch_draw_opacity_slots(scene + L.draw_tag_base, scene + L.draw_data_base, n, n_draw_data(L, slot.scene_words), table, r->stream);
+    CK(cudaGetLastError());
+    b.op_slots = table;
+    return VB_OK;
+}
 static int no_tables(vb_renderer *, uint32_t, VbBound &, std::string &) { return VB_OK; }
 
-// The draw-data slot table of bound colours and bound gradient stops (k_colors.cu), made from b whenever either changes and
-// one of them stays bound: every word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col draw tags and one
-// k_gradient_slots for the bound gradients, whose draw objects it writes to rs_draw.
+// The draw-data slot table of bound colours and bound gradient stops (k_colors.cu), made from b whenever one of them or bound
+// opacity changes and one of the three stays bound: every word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col
+// draw tags and one k_gradient_slots for the bound gradients, whose draw objects it writes to rs_draw. With opacity alone
+// every word stays VB_COLOR_NONE, so k_draw_colors copies the scene's draw data for k_draw_opacity to patch.
 static int draw_data_slots(vb_renderer *r, VbBound &b) {
     b.col_slots = nullptr;
     if (!draw_data_bound(b)) return VB_OK;
@@ -774,6 +795,7 @@ static const BindKind BIND_KINDS[VB_N_BINDINGS] = {
     {"vb_bind_transforms", false, any_scene, n_xforms, false, " transforms (1 .. n_transforms)", 24u, true, path_tags_outside, transform_tables},
     {"vb_bind_draw_visibility", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 1u, false, no_check, visibility_mask},
     {"vb_bind_stroke_widths", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, false, draw_tags_check, width_snapshot},
+    {"vb_bind_draw_opacity", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, true, opacity_check, opacity_table},
 };
 
 // Unbind `kind` in b: its rows and the tables only it reads
@@ -783,6 +805,7 @@ static void unbind(VbBound &b, int kind) {
     if (kind == VB_BIND_POINTS) b.pt_first = nullptr;
     if (kind == VB_BIND_STOPS) b.rs_grads = nullptr, b.rs_stops = nullptr, b.rs_draw = nullptr, b.rs_grads_n = b.rs_ramp0 = 0u;
     if (kind == VB_BIND_TRANSFORMS) b.xf_range = nullptr;
+    if (kind == VB_BIND_OPACITY) b.op_slots = nullptr;
 }
 
 // Bind n rows of `pitch` bytes from `ptr` as `kind` (null: unbind it), for every frame from now on
@@ -798,7 +821,8 @@ static int bind_rows(vb_renderer *r, int kind, const void *ptr, uint32_t n, size
                                   : "not available for a renderer of a vb_group or with the exchange");
     if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
     VbBound nb = r->bound;
-    const bool draw_data = kind == VB_BIND_COLORS || kind == VB_BIND_STOPS; // the draw-data slot table follows them
+    // the draw-data slot table follows them (draw_data_bound)
+    const bool draw_data = kind == VB_BIND_COLORS || kind == VB_BIND_STOPS || kind == VB_BIND_OPACITY;
     int rc;
     if (!ptr) {
         const bool was = nb.rows[kind].rows != nullptr;
@@ -859,4 +883,7 @@ extern "C" int vb_bind_draw_visibility(vb_renderer *r, const uint8_t *device_fla
 }
 extern "C" int vb_bind_stroke_widths(vb_renderer *r, const float *device_widths, uint32_t n, size_t row_pitch_bytes) {
     return bind_rows(r, VB_BIND_WIDTHS, device_widths, n, row_pitch_bytes);
+}
+extern "C" int vb_bind_draw_opacity(vb_renderer *r, const float *device_alpha, uint32_t n, size_t row_pitch_bytes) {
+    return bind_rows(r, VB_BIND_OPACITY, device_alpha, n, row_pitch_bytes);
 }

@@ -406,8 +406,8 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     // The frame reads its transforms, draw data and path data from the regions past the scene's streams that it writes itself
     // (regions_of): the bound transforms from the caller's instance rows and transform rows, the viewed transforms from the
     // transforms before them (view_src; the region is empty for a layout whose transforms do not lie inside the uploaded words),
-    // the draw data from the scene's, the colour rows and the bound gradients' ramp rows, the path data from the scene's and
-    // the point rows. Reserving them can move the scene.
+    // the draw data from the scene's, the colour rows, the bound gradients' ramp rows and the opacity rows, the path data from
+    // the scene's and the point rows. Reserving them can move the scene.
     const bool bound_xf = B.rows[VB_BIND_INSTANCES].rows || B.rows[VB_BIND_TRANSFORMS].rows;
     const Regions g = regions_of(r->cur->layout, r->cur->scene_words, bound_xf, r->view.on, draw_data_bound(B),
                                  B.rows[VB_BIND_POINTS].rows != nullptr);
@@ -579,11 +579,13 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // its streams in regions_of's order, the bound transforms before the viewed ones (their source; instances, then
             // transform rows), the draw data (read by draw, coarse and fine) and the path data (read by flatten alone); the bound
             // gradients' ramp rows (read by fine); the visibility mask and the stroke widths' snapshot (read by flatten and
-            // damage tracking). Each launcher launches nothing while its binding is unbound.
+            // damage tracking). Bound opacity patches the draw data once it is written. Each launcher launches nothing while
+            // its binding is unbound.
             launches += vb_launch_instance_transforms(c, b, st);
             launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
             launches += vb_launch_draw_colors(c, b, st);
+            launches += vb_launch_draw_opacity(c, b, st);
             launches += vb_launch_bound_ramps(c, b, st);
             launches += vb_launch_path_points(c, b, st);
             launches += vb_launch_draw_visibility(c, b, st);
@@ -615,6 +617,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_colors(c, b, st);
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_opacity(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_ramps(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);

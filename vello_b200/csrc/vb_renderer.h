@@ -326,8 +326,9 @@ struct vb_renderer {
     //  - xform_ranges: each path's transform range {t_lo, t_hi} (layout.n_paths uint2, k_points.cu)
     //  - vis_mask: the bit mask (vb_vis_words) each frame packs the visibility rows into (k_visibility.cu)
     //  - width_snap: the snapshot (vb_width_entries floats) each frame reads the stroke-width rows into (k_widths.cu)
+    //  - op_slots: one word per bound draw object, the draw-data word its opacity row replaces (VbBound::op_slots, k_opacity.cu)
     VbBound bound{};
-    DevBuf inst_tables, color_slots, point_slots, stop_tables, stop_ramps, xform_ranges, vis_mask, width_snap;
+    DevBuf inst_tables, color_slots, point_slots, stop_tables, stop_ramps, xform_ranges, vis_mask, width_snap, op_slots;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -384,7 +385,7 @@ template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
                            &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
-                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap,
+                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap, &r->op_slots,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);
@@ -459,12 +460,15 @@ inline bool any_binding(const VbBound &b) {
         if (k.rows) return true;
     return false;
 }
-// Whether frames read their draw data from the region past the scene's streams: with bound colours or bound gradient stops.
-inline bool draw_data_bound(const VbBound &b) { return b.rows[VB_BIND_COLORS].rows || b.rows[VB_BIND_STOPS].rows; }
+// Whether frames read their draw data from the region past the scene's streams: with bound colours, bound gradient stops or
+// bound opacity.
+inline bool draw_data_bound(const VbBound &b) {
+    return b.rows[VB_BIND_COLORS].rows || b.rows[VB_BIND_STOPS].rows || b.rows[VB_BIND_OPACITY].rows;
+}
 
 // The regions frames write past a scene's words, in this order, each present or not: the bound transforms (bound instance
 // transforms, k_compose.cu, and bound transforms, k_transforms.cu, share it), the viewed transforms (k_view.cu), the bound
-// draw data (bound colours or stops, k_colors.cu) and the bound path data (bound points, k_points.cu). This is the one place
+// draw data (bound colours, stops or opacity, k_colors.cu) and the bound path data (bound points, k_points.cu). This is the one place
 // that knows the order: prepare places a frame's regions with it, scene allocations are sized with it, and the bind calls
 // check 32-bit word offsets with it.
 enum { REGION_BOUND_XF, REGION_VIEW, REGION_DRAW_DATA, REGION_PATH_DATA, N_REGIONS };

@@ -22,9 +22,10 @@ struct CmpXform; // an instance's transform (k_compose.cu, below)
 struct VbUdiff;  // the upload diff's state (k_upload_diff.cu, below)
 
 // The bindings of a scene to device rows that every frame reads (vb_bind_*): instance transforms, draw colours, path points,
-// gradient stops, transforms, visibility and stroke widths. Binding k's rows are `n` rows `pitch` bytes apart from `rows`, null
-// while unbound.
-enum { VB_BIND_INSTANCES, VB_BIND_COLORS, VB_BIND_POINTS, VB_BIND_STOPS, VB_BIND_TRANSFORMS, VB_BIND_VISIBILITY, VB_BIND_WIDTHS, VB_N_BINDINGS };
+// gradient stops, transforms, visibility, stroke widths and opacity. Binding k's rows are `n` rows `pitch` bytes apart from
+// `rows`, null while unbound.
+enum { VB_BIND_INSTANCES, VB_BIND_COLORS, VB_BIND_POINTS, VB_BIND_STOPS, VB_BIND_TRANSFORMS, VB_BIND_VISIBILITY, VB_BIND_WIDTHS, VB_BIND_OPACITY,
+       VB_N_BINDINGS };
 struct VbRows {
     const uint8_t *rows;
     uint32_t n, pitch;
@@ -52,6 +53,9 @@ struct VbBound {
     const uint32_t *pt_first;
     // transforms: the range of transforms each path reads (layout.n_paths {t_lo, t_hi}; k_damage)
     const uint2 *xf_range;
+    // opacity (k_draw_opacity): per bound draw object the draw-data word its row replaces and its kind (VB_OP_ENTRY), or
+    // VB_COLOR_NONE
+    const uint32_t *op_slots;
     uint32_t rs_grads_n, rs_ramp0;
 };
 
@@ -254,6 +258,19 @@ uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b
 uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n, uint32_t *slots, uint32_t n_words, cudaStream_t st);
 uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
+// k_opacity.cu: bound opacity (vb_bind_draw_opacity). The binding's table, once at bind time: table[k] for each draw object
+// k < n, from the scene's draw tags at `tags` and its draw data at `dd` (n_words words): VB_OP_ENTRY(w, kind) for a layer's
+// alpha word w (kind VB_OP_CLIP for a clip layer, whose blend word is w - 1, else VB_OP_LAYER) and an image's sample word w
+// (VB_OP_IMAGE), VB_COLOR_NONE for any other draw object. Per frame, in flatten's stage right after k_draw_colors has written
+// the frame's draw data (draw_data_bound holds while opacity is bound): each bound word with a finite row replaced by the row's
+// conversion; nothing while unbound.
+#define VB_OP_LAYER 1u
+#define VB_OP_CLIP 2u
+#define VB_OP_IMAGE 3u
+#define VB_OP_ENTRY(w, kind) (((w) << 2) | (kind))
+uint32_t vb_launch_draw_opacity_slots(const uint32_t *tags, const uint32_t *dd, uint32_t n, uint32_t n_words, uint32_t *table, cudaStream_t st);
+uint32_t vb_launch_draw_opacity(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+
 // k_points.cu: bound path points (vb_bind_path_points). The binding's table, once at bind time, from the n_words path tag words
 // at `tags`: first[p] = the first point of path p for p <= n_paths (first[n_paths]: the scene's points), and *i16 = 1 when a
 // segment tag lacks the F32 bit. Per frame, in flatten's stage after the draw data (prepare reserved the region, vb_frame.cu):
@@ -297,14 +314,15 @@ uint32_t vb_launch_damage_rects(uint8_t *pending, uint32_t width_in_tiles, const
 //   [the transform words the frame reads (6 n_xf)] [the draw boxes (4 n_draw)] [the colour words of the first n_col draw
 //   objects] [the words of the first n_pt points (2 n_pt)] [the ramp rows of the n_grads bound gradients (512 n_grads)] [the
 //   n_vis words of the visibility mask] [the stroke widths the first n_wid draw objects were drawn with (their snapshot entry,
-//   or for 0 the encoded width word of their path's style)].
+//   or for 0 the encoded width word of their path's style)] [the opacity words the first n_op draw objects were drawn with (a
+//   layer's alpha word, an image's sample word, 0 for any other draw object)].
 // The flags, which k_damage_begin and k_damage_mark rewrite every frame, are one per bound instance, with points or visibility
 // bound one per path, and with transforms bound one per transform. Offsets are in words: a section's from the start of its
 // slot, a flag array's from the start of the snapshot (0: absent).
 #define VB_DMG_HEADER_WORDS 4u
 struct VbDmgLayout {
-    uint32_t n_xf, n_draw, n_col, n_pt, n_grads, n_vis, n_wid, n_inst, n_paths;
-    size_t box, col, pt, ramp, vis, wid, slot_words;
+    uint32_t n_xf, n_draw, n_col, n_pt, n_grads, n_vis, n_wid, n_op, n_inst, n_paths;
+    size_t box, col, pt, ramp, vis, wid, op, slot_words;
     size_t changed, paths, xf, bytes;
 };
 static inline VbDmgLayout vb_dmg_layout(const VbBound &B, const VbLayout &S, uint32_t n_xf) {
@@ -314,13 +332,15 @@ static inline VbDmgLayout vb_dmg_layout(const VbBound &B, const VbLayout &S, uin
     L.n_col = k[VB_BIND_COLORS].n, L.n_pt = k[VB_BIND_POINTS].n, L.n_grads = B.rs_grads_n;
     L.n_vis = k[VB_BIND_VISIBILITY].rows ? vb_vis_words(S) : 0u;
     L.n_wid = k[VB_BIND_WIDTHS].n;
+    L.n_op = k[VB_BIND_OPACITY].n;
     L.box = 6u * (size_t)n_xf;
     L.col = L.box + 4u * (size_t)L.n_draw;
     L.pt = L.col + L.n_col;
     L.ramp = L.pt + 2u * (size_t)L.n_pt;
     L.vis = L.ramp + 512u * (size_t)L.n_grads;
     L.wid = L.vis + L.n_vis;
-    L.slot_words = L.wid + L.n_wid;
+    L.op = L.wid + L.n_wid;
+    L.slot_words = L.op + L.n_op;
     size_t end = VB_DMG_HEADER_WORDS + 2u * L.slot_words;
     L.changed = k[VB_BIND_INSTANCES].rows ? end : 0u;
     end += L.changed ? L.n_inst : 0u;

@@ -180,6 +180,7 @@ def load_library() -> C.CDLL:
     lib.vb_bind_transforms.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_draw_visibility.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_bind_stroke_widths.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
+    lib.vb_bind_draw_opacity.argtypes = [vp, vp, C.c_uint32, C.c_size_t]
     lib.vb_set_damage_tracking.argtypes = [vp, C.c_int]
     lib.vb_set_upload_diff.argtypes = [vp, C.c_int]
     lib.vb_add_damage.argtypes = [vp, vp, C.c_uint32]
@@ -203,7 +204,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
-                    "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths"]
+                    "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths", "vb_bind_draw_opacity"]
 
 
 def _device_rows(t, who: str, what: str, cols: int, vector: bool = False):
@@ -357,8 +358,9 @@ class Renderer:
     """`vello::Renderer`: `Renderer(options)`, then `render_to_texture(scene, params)`."""
 
     # the device arrays the bind_* methods hold while bound (_bind), None while unbound: of bind_instance_transforms,
-    # bind_draw_colors, bind_path_points, bind_gradient_stops, bind_transforms, bind_draw_visibility and bind_stroke_widths
-    _bound = _colors = _points = _stops = _xforms = _visibility = _widths = None
+    # bind_draw_colors, bind_path_points, bind_gradient_stops, bind_transforms, bind_draw_visibility, bind_stroke_widths and
+    # bind_draw_opacity
+    _bound = _colors = _points = _stops = _xforms = _visibility = _widths = _opacity = None
 
     def __init__(self, options: Optional[RendererOptions] = None):
         self.lib = load_library()
@@ -634,6 +636,20 @@ class Renderer:
         re-encoded with those widths renders. Write `t` on `self.stream` (or synchronise) before a frame; frames then need no
         further call. `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
         self._bind("bind_stroke_widths", "_widths", t, lambda t: _device_rows(t, "bind_stroke_widths", "widths", 1, vector=True))
+
+    def bind_draw_opacity(self, t):
+        """Draw layer or image k of the installed scene with the alpha in row k of the device array `t`, in every frame from now
+        on, read when the frame runs (`vb_bind_draw_opacity`): `t` is float32 (n,) or (n, 1), n at most the scene's
+        `Scene.n_draw_objects`, with `__cuda_array_interface__` and rows any multiple of 4 bytes apart (e.g. a torch CUDA
+        tensor, or a column of a larger one such as `state[:, 5]`). Index k is the draw object of `hit_test`, global in a
+        composed scene or a batch. A finite row is clamped to [0, 1] and becomes the alpha of a push_*_layer's draw object (the
+        pop_layer's row is ignored) or of an image (in place of the image's alpha times the brush alpha). A push_clip_layer with
+        a row below 1 is drawn as push_layer(MIX_NORMAL, COMPOSE_SRC_OVER, row), so its whole layer fades; at 1 it is drawn as
+        encoded. Rows of fills, strokes, gradients and blurred rectangles are ignored, and draw objects from n on, and a row
+        that is not finite, keep their encoded values. Every frame renders what the scene re-encoded with those alphas renders;
+        hit tests do not change. Write `t` on `self.stream` (or synchronise) before a frame; frames then need no further call.
+        `t` is held while bound; None unbinds. A new scene (any upload, compose or recompose) unbinds."""
+        self._bind("bind_draw_opacity", "_opacity", t, lambda t: _device_rows(t, "bind_draw_opacity", "alphas", 1, vector=True))
 
     def mark_override_image_dirty(self, image: Image):
         """Copy the overridden image's device pixels into the atlas again, in front of the next frame."""
