@@ -478,6 +478,52 @@ typedef struct {
 } vb_instance;
 int vb_fragment_upload(vb_renderer *, const vb_encoding_streams *, uint32_t *fragment_out);
 int vb_fragment_free(vb_renderer *, uint32_t fragment);
+/* A fragment built on the device from ragged arrays in device memory (an addition; no vello counterpart): polygons a model
+ * predicts, a time series that grows, a simulation's outlines or a filtered map layer, in the points / offsets layout of
+ * GeoArrow, shapely and ragged tensors, with no host loop over their rows and no copy to the host. Path i is rings
+ * path_offsets[i] .. path_offsets[i + 1] - 1 (path_offsets NULL: ring i alone, n_paths = n_rings); ring r is points
+ * ring_offsets[r] .. ring_offsets[r + 1] - 1, each an (x, y) f32 pair point_pitch_bytes apart; path i's colour is the
+ * straight-alpha r g b a f32 row i, color_pitch_bytes apart. The fragment is word for word what vb_fragment_upload receives from
+ * a fresh Scene that, for each path i in order, calls
+ *     fill(fill_rule, IDENTITY, Color(colors[i]), None, shape_i)      kind 0
+ *     stroke(Stroke{width, join, miter_limit, start_cap, end_cap}, IDENTITY, Color(colors[i]), None, shape_i)   kind 1
+ * where shape_i is, for each ring of path i, M p_first, L p for every following point, then Z (fills always; strokes when
+ * `closed`). So the encoders' rules hold: a point EPS-close (1e-12) to the last kept one writes nothing, a ring of fewer than
+ * two distinct points writes nothing, a ring closes with a line when its last kept point differs bit for bit from its first,
+ * strokes end each ring with a cap marker, and a path whose rings all write nothing draws nothing. Its one TRANSFORM (identity)
+ * and STYLE come first when n_paths > 0; n_paths = 0 is the empty fragment. join and caps are vb_stroke's (VB_JOIN_*,
+ * VB_CAP_*, vello_b200_scene.h); dashes, curves, brushes other than one colour per path, and clips are not part of it.
+ * *n_draw_objects_out (optional) receives the fragment's draw objects; draw_index (optional, n_paths int32 entries, device
+ * memory) receives path i's draw object within the fragment, or -1 for a path that draws nothing. Which path-data rows a
+ * point lands in depends on the points dropped, so bind points of such a fragment (vb_bind_path_points) only with rows made
+ * from its own encoding.
+ *  - The result is an ordinary fragment: vb_compose and vb_recompose take it beside uploaded ones, instance transforms, views,
+ *    hit tests and every binding apply, vb_fragment_free frees it, and its id is never reused. A base layer uploaded once and
+ *    an overlay rebuilt from device arrays every frame are one vb_compose([base, overlay]).
+ *  - The arrays are read on vb_stream: order the writes to them before the call (on vb_stream, or with a synchronisation).
+ *    The call is synchronous like vb_fragment_upload: the streams' lengths depend on the data, so after its kernels it reads
+ *    the totals back and synchronises vb_stream once. The allocation is sized for the worst case of the counts (a tag and two
+ *    words per point, a closing line and a cap marker per ring, a PATH tag and a draw object per path).
+ *  - A compose whose stream lengths differ from the last one's captures its frame graph anew (DESIGN.md gives the cost).
+ * VB_E_INVALID (vb_last_error says why), with no fragment made and the renderer as it was: NULL pointers where a count is not
+ * zero, or path_offsets NULL with n_paths != n_rings; an array that is not 4-byte aligned device or managed memory of the
+ * renderer's device; a point pitch below 8 or a colour pitch below 16 bytes, a pitch that is not a multiple of 4 or is 4 GiB
+ * or more; a count past int32; a bad kind, fill rule, join or cap; a width that is not finite and > 0, or a miter limit that
+ * is not finite; a worst case past 32-bit word offsets; a renderer of a vb_group or with the exchange; a call between
+ * vb_render_enqueue and vb_frame_finish. Checked on the device, naming the first offending row: ring_offsets not starting
+ * at 0, decreasing, or not ending at n_points; path_offsets likewise over the rings; a coordinate or a colour component that
+ * is not finite. */
+typedef struct {
+    const float *points;       uint32_t n_points;  size_t point_pitch_bytes; /* x y f32 rows */
+    const int32_t *ring_offsets; uint32_t n_rings;  /* n_rings + 1 entries */
+    const int32_t *path_offsets; uint32_t n_paths;  /* n_paths + 1 entries over rings; NULL: one ring per path (n_paths = n_rings) */
+    const float *colors;       size_t color_pitch_bytes; /* n_paths rows of straight-alpha sRGB r g b a */
+    uint32_t kind;             /* 0 fill, 1 stroke */
+    uint32_t fill_rule;        /* fills: 0 non-zero, 1 even-odd (VB_FILL_NON_ZERO / VB_FILL_EVEN_ODD) */
+    float width, miter_limit;  uint32_t join, start_cap, end_cap, closed; /* strokes: kurbo Stroke without dashes */
+    int32_t *draw_index;       /* optional out, n_paths entries: path i's draw object in the fragment, or -1 */
+} vb_device_paths;
+int vb_fragment_from_device_paths(vb_renderer *, const vb_device_paths *, uint32_t *fragment_out, uint32_t *n_draw_objects_out);
 int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
 /* vb_recompose: vb_compose, followed by a frame that repaints only what the new instance list changed (an addition; no vello
  * counterpart). It installs exactly the scene vb_compose would (scene, layout, ramps, atlas and draw offsets, byte for byte),

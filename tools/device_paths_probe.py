@@ -1,0 +1,188 @@
+"""Fragments from device arrays (Renderer.upload_device_paths, vb_fragment_from_device_paths) against the host route, on two
+inputs: about 30k paris-like polygons (1.5M points, a few with holes, filled) in a 4096^2 frame, and one 1M-point polyline
+(stroked). Prints, with the card, its power limit and SM clock:
+  call_ms     the call's wall time (it ends with its one synchronisation), and kernel_ms, the span of its work on vb_stream
+              from CUDA events recorded around it (scratch clears, the four kernels and the read-back of the totals)
+  host_ms     the host route for the same rows: the arrays copied to the host, one vb_scene_fill / vb_scene_stroke per path
+              (ctypes calls over views of one verb and one coordinate array), and vb_scene_upload_fragment
+  frames      a per-frame loop at 4096^2 MSAA16 of build + compose + render against native encode + upload + compose + render;
+              both change the geometry every frame (points moved by the frame number on the device, or on the host), so the
+              compose's stream lengths may change and the frame graph is captured anew (graph_captures counts it); and
+              the cost of that capture: frames that cycle through six row counts (new lengths every frame, more than
+              the four cached graphs, so a capture every frame), with frame graphs on and off
+With --out the result also goes to DIR/device_paths_probe.json:
+    python tools/device_paths_probe.py [--reps 10] [--frames 20] [--out DIR]"""
+import argparse
+import ctypes as C
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from compose_probe import card  # noqa: E402
+from vello_b200.config import AA_MSAA16, RenderParams  # noqa: E402
+from vello_b200.encoding import BLACK, FILL_NON_ZERO, Stroke  # noqa: E402
+from vello_b200.renderer import Renderer  # noqa: E402
+from vello_b200.scene_native import NativeScene, _Brush, _Color, _Path, _Stroke, _affine  # noqa: E402
+from vello_b200.shapes import Affine  # noqa: E402
+
+SIZE = 4096
+
+
+def polygons(n=30_000, seed=1):
+    """Paris-like blocks: n polygons of 20..80 points around random centres, every 10th with a hole."""
+    rng = np.random.default_rng(seed)
+    pts, roff, poff = [], [0], [0]
+    for i in range(n):
+        c = rng.uniform(0, SIZE, 2)
+        for hole in range(2 if i % 10 == 0 else 1):
+            k = int(rng.integers(20, 81))
+            t = np.sort(rng.uniform(0, 2 * np.pi, k))
+            rad = rng.uniform(20, 60, k) * (0.3 if hole else 1.0)
+            pts.append(np.stack([c[0] + rad * np.cos(t), c[1] + rad * np.sin(t)], 1))
+            roff.append(roff[-1] + k)
+        poff.append(len(roff) - 1)
+    cols = rng.uniform(0, 1, (n, 4)).astype(np.float32)
+    cols[:, 3] = 0.8
+    return np.concatenate(pts).astype(np.float32), np.array(roff, np.int32), np.array(poff, np.int32), cols
+
+
+def polyline(n=1_000_000, seed=2):
+    rng = np.random.default_rng(seed)
+    x = np.linspace(8, SIZE - 8, n)
+    y = SIZE / 2 + SIZE / 3 * np.sin(x / 300.0) + rng.normal(0, 3, n)
+    return np.stack([x, y], 1).astype(np.float32), np.array([0, n], np.int32), None, np.array([[1, 0.9, 0.2, 1]], np.float32)
+
+
+def host_route(r, pts, roff, poff, cols, style):
+    """Copy the device arrays to the host, encode one fill or stroke per path through the native scene, upload the fragment."""
+    p, ro, po, co = (t.cpu().numpy() if t is not None else None for t in (pts, roff, poff, cols))
+    s = NativeScene()
+    lib, h = s.lib, s.handle
+    n_paths = len(po) - 1 if po is not None else len(ro) - 1
+    # one verb and one coordinate array: per ring M, L..., Z (strokes here are open: no Z)
+    stroke = isinstance(style, Stroke)
+    ring_len = np.diff(ro)
+    verbs = []
+    for k in ring_len:
+        verbs += [ord("M")] + [ord("L")] * (int(k) - 1) + ([] if stroke else [ord("Z")])
+    verbs = np.array(verbs, np.uint8)
+    coords = p.astype(np.float64).reshape(-1)
+    vstart = np.concatenate([[0], np.cumsum(ring_len + (0 if stroke else 1))])
+    ident = _affine(Affine.IDENTITY)
+    st = _Stroke(style.width, style.join, style.start_cap, style.end_cap, style.miter_limit, None, 0, 0.0) if stroke else None
+    for i in range(n_paths):
+        r0, r1 = (int(po[i]), int(po[i + 1])) if po is not None else (i, i + 1)
+        b = _Brush()
+        b.kind, b.color = 0, _Color(*[float(v) for v in co[i]])
+        path = _Path(verbs.ctypes.data + int(vstart[r0]), int(vstart[r1] - vstart[r0]), coords.ctypes.data + 16 * int(ro[r0]))
+        if stroke:
+            lib.vb_scene_stroke(h, C.byref(st), ident, C.byref(b), None, C.byref(path))
+        else:
+            lib.vb_scene_fill(h, FILL_NON_ZERO, ident, C.byref(b), None, C.byref(path))
+    return r.upload_fragment(s)
+
+
+def measure(r, name, data, style, reps, n_frames):
+    pts, roff, poff, cols = (torch.as_tensor(a).cuda() if a is not None else None for a in data)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    st = torch.cuda.ExternalStream(r.stream)
+    kw = dict(path_offsets=poff, style=style, closed=False)
+    f, n = r.upload_device_paths(pts, roff, cols, **kw)  # warm-up
+    r.free_fragment(f)
+    call, kern = [], []
+    for _ in range(reps):
+        ev0.record(st)
+        t0 = time.perf_counter()
+        f, n = r.upload_device_paths(pts, roff, cols, **kw)
+        call.append((time.perf_counter() - t0) * 1e3)
+        ev1.record(st)
+        ev1.synchronize()
+        kern.append(ev0.elapsed_time(ev1))
+        r.free_fragment(f)
+    host = []
+    for _ in range(max(2, reps // 3)):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        f = host_route(r, pts, roff, poff, cols, style)
+        host.append((time.perf_counter() - t0) * 1e3)
+        r.free_fragment(f)
+    # frames: the geometry moves every frame (by 0.25 px per frame), rebuilt on the device or encoded on the host
+    p = RenderParams(BLACK, SIZE, SIZE, AA_MSAA16)
+    out = {}
+    for route in ("device", "host"):
+        cap0 = r.debug_graph_captures()
+        torch.cuda.synchronize()
+        t0 = None
+        for k in range(n_frames + 3):
+            if k == 3:
+                torch.cuda.synchronize()
+                t0, cap0 = time.perf_counter(), r.debug_graph_captures()
+            with torch.cuda.stream(st):
+                moved = pts + 0.25 * (k % 8)
+            if route == "device":
+                f, _ = r.upload_device_paths(moved, roff, cols, **kw)
+            else:
+                f = host_route(r, moved, roff, poff, cols, style)
+            r.compose([(f, None)])
+            r.render_resident(p)
+            r.free_fragment(f)
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t0) * 1e3 / n_frames
+        out[route] = {"fps": round(1e3 / ms, 2), "ms_per_frame": round(ms, 3), "graph_captures": r.debug_graph_captures() - cap0}
+    # recapture: the frames cycle through fragments of six stream lengths (all the rows, then 5/6 .. 1/6 of them), more than
+    # the renderer's four cached frame graphs, so every frame captures its graph anew; against the same cycle without graphs
+    def part(v):
+        if poff is None:
+            q = pts.shape[0] * (6 - v) // 6
+            return pts[:q], torch.tensor([0, q], dtype=torch.int32, device="cuda"), None, cols
+        n_p = (len(poff) - 1) * (6 - v) // 6
+        n_r = int(poff[n_p])
+        return pts[:int(roff[n_r])], roff[:n_r + 1], poff[:n_p + 1], cols[:n_p]
+    halves = [part(v) for v in range(6)]
+    for graphs in (True, False):
+        r.set_cuda_graph(graphs)
+        for k in range(n_frames + 3):
+            if k == 3:
+                torch.cuda.synchronize()
+                t0, cap0 = time.perf_counter(), r.debug_graph_captures()
+            q, ro, po, co = halves[k % 6]
+            f, _ = r.upload_device_paths(q, ro, co, path_offsets=po, style=style, closed=False)
+            r.compose([(f, None)])
+            r.render_resident(p)
+            r.free_fragment(f)
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t0) * 1e3 / n_frames
+        out["cycling_graphs" if graphs else "cycling_no_graphs"] = {
+            "fps": round(1e3 / ms, 2), "ms_per_frame": round(ms, 3), "graph_captures": r.debug_graph_captures() - cap0}
+    r.set_cuda_graph(True)
+    return {"input": name, "points": int(pts.shape[0]), "paths": int(cols.shape[0]), "draw_objects": n,
+            "call_ms_median": round(float(np.median(call)), 3), "kernel_ms_median": round(float(np.median(kern)), 3),
+            "host_ms_median": round(float(np.median(host)), 3), "frames": out}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    r = Renderer()
+    res = {"card": card(), "results": [measure(r, "polygons_30k", polygons(), FILL_NON_ZERO, a.reps, a.frames),
+                                       measure(r, "polyline_1m", polyline(), Stroke(2.0), a.reps, a.frames)],
+           "card_after": card()}
+    print(json.dumps(res, indent=1))
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "device_paths_probe.json"), "w") as fh:
+            json.dump(res, fh, indent=1)
+    r.close()
+
+
+if __name__ == "__main__":
+    main()

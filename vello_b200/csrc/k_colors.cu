@@ -14,22 +14,6 @@
 #define DC_THREADS 256u
 #define DC_SLOT_THREADS 1024u
 
-// Color::premultiply().to_rgba8().to_u32() (draw.rs:76-84; vb_scene.cpp's premul_rgba8, encoding.py's premul_rgba8_u32): r is the
-// low byte. Each product and the + 0.5 are rounded on their own, as the encoder rounds them: a fused multiply-add gives other
-// bytes next to the ties.
-__device__ __forceinline__ uint32_t dc_premul_rgba8(float r, float g, float b, float a) {
-    const float p[4] = {__fmul_rn(r, a), __fmul_rn(g, a), __fmul_rn(b, a), a};
-    uint32_t out = 0u;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        float v = floorf(__fadd_rn(__fmul_rn(p[i], 255.0f), 0.5f));
-        if (!(v > 0.0f)) v = 0.0f;
-        if (v > 255.0f) v = 255.0f;
-        out |= (uint32_t)v << (8 * i);
-    }
-    return out;
-}
-
 // One CTA walks the first n draw tags a chunk at a time: the exclusive scan of their draw-data sizes (draw.rs's DrawTag, as
 // k_draw's monoid has it) gives each draw object's first word, which is its colour for FILL_COLOR and BLURRED_ROUNDED_RECT.
 __global__ void __launch_bounds__(DC_SLOT_THREADS) k_draw_color_slots(const uint32_t *__restrict__ tags, uint32_t n, uint32_t *slots,

@@ -1,13 +1,15 @@
 // vb_compose.cu -- composition of resident fragments: vb_fragment_upload / vb_fragment_free, vb_compose and vb_recompose
 // (k_compose.cu, k_recompose.cu), bound instance transforms (vb_bind_instance_transforms), bound draw colours
 // (vb_bind_draw_colors, k_colors.cu), bound path points (vb_bind_path_points, k_points.cu), bound gradient stops
-// (vb_bind_gradient_stops, k_resolve.cu) and bound transforms (vb_bind_transforms, k_transforms.cu).
+// (vb_bind_gradient_stops, k_resolve.cu) and bound transforms (vb_bind_transforms, k_transforms.cu); fragments built from
+// device arrays (vb_fragment_from_device_paths, k_device_paths.cu).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
 
 #include <algorithm>
 
+#include "vb_device.cuh"
 #include "vb_diff.h"
 #include "vb_renderer.h"
 #include "vb_resolve.h"
@@ -152,6 +154,47 @@ static void reap_freed(vb_renderer *r) {
     }
 }
 
+// A fragment's allocation (k_compose.cu reads it): the header of CMP_HEADER_WORDS words, each stream's word offset, then the
+// streams back to back in CMP_* order, the path tags padded to whole words. `units` are the streams' lengths as Fragment::len
+// counts them (tag bytes, words, draw tags, words, transforms, style words); off[] gets the header and the result is the
+// allocation's bytes for them (0 when past 32-bit word offsets), before any image pixels.
+static size_t fragment_layout(const uint64_t units[CMP_STREAMS], uint64_t off[CMP_HEADER_WORDS]) {
+    const uint64_t words[CMP_STREAMS] = {(units[CMP_TAGS] + 3u) / 4u, units[CMP_PATH_DATA], units[CMP_DRAW_TAGS], units[CMP_DRAW_DATA],
+                                         6u * units[CMP_TRANSFORMS], units[CMP_STYLES]};
+    uint64_t w = CMP_HEADER_WORDS;
+    for (int s = 0; s < (int)CMP_HEADER_WORDS; s++) off[s] = 0u;
+    for (int s = 0; s < CMP_STREAMS; s++) {
+        off[s] = w;
+        w += words[s];
+    }
+    if (w + 4u > 0xfffffff0ull) return 0u;
+    return ((size_t)(w + 4u) * 4u + 15u) & ~(size_t)15u;
+}
+
+// Account and register the fragment f, whose allocation holds its streams of lengths `units` (fragment_layout): the renderer
+// owns it from now on under a new id, which is returned.
+static uint32_t fragment_register(vb_renderer *r, std::unique_ptr<Fragment> f, const uint64_t units[CMP_STREAMS], uint32_t n_paths,
+                                  uint32_t n_clips, uint32_t n_open_clips, uint32_t info) {
+    for (int s = 0; s < CMP_STREAMS; s++) f->len[s] = (uint32_t)units[s];
+    f->n_paths = n_paths;
+    f->n_clips = n_clips;
+    f->n_open_clips = n_open_clips;
+    f->info = info;
+    f->id = r->next_fragment++;
+    r->fragment_bytes += f->bytes;
+    const uint32_t id = f->id;
+    r->fragments[id] = std::move(f);
+    return id;
+}
+
+static size_t up16(size_t v) { return (v + 15u) & ~(size_t)15u; }
+// Grow a buffer compose writes. Work already enqueued may read it: growing waits for the renderer's stream.
+static int compose_room(vb_renderer *r, DevBuf &b, size_t bytes) {
+    if (b.cap >= std::max<size_t>(bytes, 256)) return VB_OK;
+    CK(cudaStreamSynchronize(r->stream));
+    return ensure(r, b, bytes);
+}
+
 extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, uint32_t *fragment_out) {
     if (!r) return VB_E_INVALID;
     auto bad = [&](const char *why) {
@@ -160,21 +203,14 @@ extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, 
     };
     if (!e || !fragment_out) return bad("NULL streams or id");
     if (check_streams(r, e, "vb_fragment_upload")) return VB_E_INVALID;
-    // the allocation: header, the six streams (tags padded to whole words), then one copy of each image key's pixels
-    uint64_t off[CMP_HEADER_WORDS] = {};
-    uint64_t w = CMP_HEADER_WORDS;
-    const uint64_t words[CMP_STREAMS] = {((uint64_t)e->n_path_tags + 3u) / 4u, e->n_path_data, e->n_draw_tags, e->n_draw_data,
-                                         6ull * e->n_transforms, 2ull * e->n_styles};
-    for (int s = 0; s < CMP_STREAMS; s++) {
-        off[s] = w;
-        w += words[s];
-    }
-    if (w + 4u > 0xfffffff0ull) return bad("the fragment's streams exceed 32-bit word offsets");
+    // the allocation: header, the six streams, then one copy of each image key's pixels
+    uint64_t off[CMP_HEADER_WORDS];
+    const uint64_t units[CMP_STREAMS] = {e->n_path_tags, e->n_path_data, e->n_draw_tags, e->n_draw_data, e->n_transforms, 2ull * e->n_styles};
+    size_t bytes = fragment_layout(units, off);
+    if (!bytes) return bad("the fragment's streams exceed 32-bit word offsets");
     CK(cudaSetDevice(r->device));
     reap_freed(r);
     std::unique_ptr<Fragment> f(new Fragment());
-    size_t bytes = (size_t)(w + 4u) * 4u;
-    bytes = (bytes + 15u) & ~(size_t)15u;
     std::vector<std::pair<size_t, const Fragment::Image *>> copies; // (offset in the allocation, image) per key with pixels
     std::unordered_map<const ImageKey *, size_t> at;
     std::map<std::tuple<const void *, uint32_t, uint32_t>, uint64_t> hashed; // each of this fragment's images is read once
@@ -236,20 +272,8 @@ extern "C" int vb_fragment_upload(vb_renderer *r, const vb_encoding_streams *e, 
         r->err = std::string("vb_fragment_upload: copying the streams: ") + cudaGetErrorString(ce);
         return VB_E_CUDA;
     }
-    f->len[CMP_TAGS] = e->n_path_tags;
-    f->len[CMP_PATH_DATA] = e->n_path_data;
-    f->len[CMP_DRAW_TAGS] = e->n_draw_tags;
-    f->len[CMP_DRAW_DATA] = e->n_draw_data;
-    f->len[CMP_TRANSFORMS] = e->n_transforms;
-    f->len[CMP_STYLES] = 2u * e->n_styles;
-    f->n_paths = e->n_paths;
-    f->n_clips = e->n_clips;
-    f->n_open_clips = e->n_open_clips;
-    f->info = (uint32_t)vb_draw_info_sum(e->draw_tags, e->n_draw_tags);
-    f->id = r->next_fragment++;
-    r->fragment_bytes += bytes;
-    *fragment_out = f->id;
-    r->fragments[f->id] = std::move(f);
+    *fragment_out = fragment_register(r, std::move(f), units, e->n_paths, e->n_clips, e->n_open_clips,
+                                      (uint32_t)vb_draw_info_sum(e->draw_tags, e->n_draw_tags));
     return VB_OK;
 }
 
@@ -277,12 +301,137 @@ extern "C" int vb_fragment_free(vb_renderer *r, uint32_t fragment) {
     return VB_OK;
 }
 
-// Grow a buffer compose writes. Work already enqueued may read it: growing waits for the renderer's stream.
-static int compose_room(vb_renderer *r, DevBuf &b, size_t bytes) {
-    if (b.cap >= std::max<size_t>(bytes, 256)) return VB_OK;
-    CK(cudaStreamSynchronize(r->stream));
-    return ensure(r, b, bytes);
+// ---- fragments from device arrays: vb_fragment_from_device_paths (k_device_paths.cu) -----------------------------------------
+// The streams' lengths depend on the data (dropped points, closing lines, cap markers), so the fragment is allocated for the
+// worst case of the counts, the four launches write it, and the totals and the error word come back through pinned memory
+// after one synchronisation of the renderer's stream.
+static const uint32_t STROKE_JOINS[3] = {0u, 0x10000000u, 0x20000000u}, STROKE_CAPS[3] = {0u, 0x01000000u, 0x02000000u}; // path.rs:30-66
+static bool one_of(uint32_t v, const uint32_t (&set)[3]) { return v == set[0] || v == set[1] || v == set[2]; }
+
+extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_paths *d, uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
+    if (!r) return VB_E_INVALID;
+    auto bad = [&](const std::string &why) {
+        r->err = "vb_fragment_from_device_paths: " + why;
+        return VB_E_INVALID;
+    };
+    if (!d || !fragment_out) return bad("NULL paths or id");
+    if (r->grouped || r->xc.enabled || r->xc.configured) return bad("not available for a renderer of a vb_group or with the exchange");
+    if (r->frame_pending) return bad("a frame is enqueued and not finished (vb_frame_finish)");
+    const uint64_t P = d->n_points, R = d->n_rings, N = d->n_paths;
+    if (P > 0x7fffffffu || R > 0x7fffffffu || N > 0x7fffffffu) return bad("n_points, n_rings and n_paths must fit int32 offsets");
+    if ((P && !d->points) || ((P || R) && !d->ring_offsets) || (N && !d->colors)) return bad("NULL points, ring_offsets or colors with a non-zero count");
+    if (!d->path_offsets && N != R) return bad("without path_offsets every ring is a path: n_paths must equal n_rings");
+    if (d->point_pitch_bytes < 8u || d->point_pitch_bytes % 4u || d->point_pitch_bytes > 0xffffffffu)
+        return bad("the point pitch must be a multiple of 4 bytes, at least 8 and below 4 GiB");
+    if (d->color_pitch_bytes < 16u || d->color_pitch_bytes % 4u || d->color_pitch_bytes > 0xffffffffu)
+        return bad("the colour pitch must be a multiple of 4 bytes, at least 16 and below 4 GiB");
+    uint32_t flags = 0u, width = 0u;
+    if (d->kind == 0u) {
+        if (d->fill_rule > 1u) return bad("fill_rule must be 0 (non-zero) or 1 (even-odd)");
+        flags = d->fill_rule ? 0x40000000u : 0u; // style_from_fill
+    } else if (d->kind == 1u) {
+        if (!one_of(d->join, STROKE_JOINS)) return bad("join must be VB_JOIN_BEVEL, VB_JOIN_MITER or VB_JOIN_ROUND");
+        if (!one_of(d->start_cap, STROKE_CAPS) || !one_of(d->end_cap, STROKE_CAPS)) return bad("the caps must be VB_CAP_BUTT, VB_CAP_SQUARE or VB_CAP_ROUND");
+        if (!(isfinite(d->width) && d->width > 0.0f)) return bad("the stroke width must be finite and > 0");
+        if (!isfinite(d->miter_limit)) return bad("the miter limit must be finite");
+        flags = 0x80000000u | d->join | (d->start_cap << 2) | d->end_cap | vb_f32_to_f16(d->miter_limit); // style_from_stroke
+        memcpy(&width, &d->width, 4);
+    } else {
+        return bad("kind must be 0 (fill) or 1 (stroke)");
+    }
+    // the worst case: a tag per point, the closing line and a cap marker per ring, a PATH tag per path, the TRANSFORM and STYLE
+    // tags; 2 words per point and 4 per ring (closing line and cap line, or cap quad); a draw object per path
+    uint64_t off[CMP_HEADER_WORDS];
+    const uint64_t worst[CMP_STREAMS] = {N ? 2u + P + 2u * R + N : 0u, 2u * P + 4u * R, N, N, N ? 1u : 0u, N ? 2u : 0u};
+    const size_t bytes = fragment_layout(worst, off);
+    if (!bytes) return bad("the fragment's worst-case streams exceed 32-bit word offsets");
+    CK(cudaSetDevice(r->device));
+    const void *ptrs[5] = {d->points, d->ring_offsets, d->path_offsets, d->colors, d->draw_index};
+    for (const void *p : ptrs)
+        if (p && ((uintptr_t)p % 4u || !device_memory_of(r, p)))
+            return bad("every array must be 4-byte aligned device or managed memory of the renderer's device");
+    reap_freed(r);
+
+    // the scratch (DpArgs): [err, ring_first] set to all ones, [totals, ring_last, ring_odd, path_kept, the look-back's leading
+    // words] to zero, then the rest of the look-back, the partitions' prefixes, the ring records and the keep bytes
+    const uint32_t parts = vb_device_paths_parts((uint32_t)P);
+    const size_t lb_words = vb_lookback_words(parts, 3);
+    const size_t o_first = 16u, o_zero = up16(o_first + 4u * R), o_last = o_zero + 16u, o_odd = o_last + 4u * R, o_kept = o_odd + 4u * R;
+    const size_t o_lb = up16(o_kept + 4u * N), o_excl = up16(o_lb + 4u * lb_words), o_rings = up16(o_excl + 12u * parts);
+    const size_t o_keep = o_rings + 16u * R, scratch = o_keep + P;
+    int rc;
+    if ((rc = compose_room(r, r->paths_tmp, scratch))) return rc;
+    char *t = (char *)r->paths_tmp.p;
+    std::unique_ptr<Fragment> f(new Fragment());
+    const cudaError_t ce = cudaMalloc(&f->mem, bytes);
+    if (ce != cudaSuccess) {
+        r->err = std::string("vb_fragment_from_device_paths: cudaMalloc: ") + cudaGetErrorString(ce);
+        return VB_E_CUDA;
+    }
+    f->bytes = bytes;
+    DpArgs a;
+    memset(&a, 0, sizeof a);
+    a.points = d->points;
+    a.ring_offsets = d->ring_offsets;
+    a.path_offsets = d->path_offsets;
+    a.colors = d->colors;
+    a.point_pitch = d->point_pitch_bytes;
+    a.color_pitch = d->color_pitch_bytes;
+    a.n_points = (uint32_t)P, a.n_rings = (uint32_t)R, a.n_paths = (uint32_t)N, a.n_parts = parts;
+    a.kind = d->kind, a.closed = d->closed ? 1u : 0u, a.style_flags = flags, a.style_width = width;
+    a.err = (unsigned long long *)t;
+    a.ring_first = (uint32_t *)(t + o_first);
+    a.totals = (uint32_t *)(t + o_zero);
+    a.ring_last = (uint32_t *)(t + o_last);
+    a.ring_odd = (uint32_t *)(t + o_odd);
+    a.path_kept = (uint32_t *)(t + o_kept);
+    a.lookback = (uint32_t *)(t + o_lb);
+    a.part_excl = (uint32_t *)(t + o_excl);
+    a.rings = (uint4 *)(t + o_rings);
+    a.keep_fix = (uint8_t *)(t + o_keep);
+    a.fragment = (uint32_t *)f->mem;
+    a.draw_index = d->draw_index;
+    cudaStream_t st = r->stream;
+    PinnedStage &stage = r->pinned[PIN_COMPOSE];
+    uint8_t *h;
+    auto fail = [&](int code) {
+        cudaFree(f->mem);
+        return code;
+    };
+    if ((rc = stage_host(r, stage, 32u, &h))) return fail(rc);
+    cudaError_t e2 = cudaMemsetAsync(t, 0xff, o_zero, st);
+    if (e2 == cudaSuccess) e2 = cudaMemsetAsync(t + o_zero, 0, o_lb - o_zero + 4u * VB_LB_ZERO_WORDS(parts), st);
+    if (e2 == cudaSuccess) {
+        vb_launch_device_paths(a, st);
+        e2 = cudaGetLastError();
+    }
+    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(h, t, 8u, cudaMemcpyDeviceToHost, st);
+    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(h + 8u, t + o_zero, 12u, cudaMemcpyDeviceToHost, st);
+    if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(st);
+    if (e2 != cudaSuccess) {
+        r->err = std::string("vb_fragment_from_device_paths: ") + cudaGetErrorString(e2);
+        return fail(VB_E_CUDA);
+    }
+    unsigned long long err;
+    uint32_t tot[3];
+    memcpy(&err, h, 8u);
+    memcpy(tot, h + 8u, 12u);
+    if (err != ~0ull) {
+        const uint32_t row = (uint32_t)err;
+        const uint32_t kind = (uint32_t)(err >> 32);
+        const std::string at = std::to_string(row);
+        fail(0);
+        if (kind == VB_DP_ERR_RING_OFFSETS) return bad("ring_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_points");
+        if (kind == VB_DP_ERR_PATH_OFFSETS) return bad("path_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_rings");
+        if (kind == VB_DP_ERR_POINTS) return bad("point " + at + " is not finite");
+        return bad("the colour of path " + at + " is not finite");
+    }
+    const uint64_t units[CMP_STREAMS] = {N ? 2u + tot[0] : 0u, tot[1], tot[2], tot[2], N ? 1u : 0u, N ? 2u : 0u};
+    *fragment_out = fragment_register(r, std::move(f), units, tot[2], 0u, 0u, tot[2]); // FILL_COLOR has one info word
+    if (n_draw_objects_out) *n_draw_objects_out = tot[2];
+    return VB_OK;
 }
+
 
 // The resident fragment of an id; nullptr when there is none (never uploaded, or freed).
 static const Fragment *find_fragment(const vb_renderer *r, uint32_t id) {
@@ -290,7 +439,6 @@ static const Fragment *find_fragment(const vb_renderer *r, uint32_t id) {
     return it == r->fragments.end() ? nullptr : it->second.get();
 }
 
-static size_t up16(size_t v) { return (v + 15u) & ~(size_t)15u; }
 // The tables k_compose_streams reads for n instances: [the per-stream exclusive prefix of the instances' lengths,
 // CMP_STREAMS x (n + 1) words] [the fragments' addresses, at o_src] [the transforms, at o_xf]; `bytes` in all.
 struct CmpTables {

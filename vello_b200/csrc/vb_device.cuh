@@ -238,6 +238,22 @@ __device__ __forceinline__ uint32_t vb_cell_of(const VbConfig &cfg, uint32_t ix)
     }
     return lo;
 }
+// Color::premultiply().to_rgba8().to_u32() (draw.rs:76-84; vb_scene.cpp's premul_rgba8, encoding.py's premul_rgba8_u32): r is the
+// low byte. Each product and the + 0.5 are rounded on their own, as the encoder rounds them: a fused multiply-add gives other
+// bytes next to the ties. Bound draw colours (k_colors.cu) and fragments from device arrays (k_device_paths.cu) write it.
+__device__ __forceinline__ uint32_t dc_premul_rgba8(float r, float g, float b, float a) {
+    const float p[4] = {__fmul_rn(r, a), __fmul_rn(g, a), __fmul_rn(b, a), a};
+    uint32_t out = 0u;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        float v = floorf(__fadd_rn(__fmul_rn(p[i], 255.0f), 0.5f));
+        if (!(v > 0.0f)) v = 0.0f;
+        if (v > 255.0f) v = 255.0f;
+        out |= (uint32_t)v << (8 * i);
+    }
+    return out;
+}
+
 // Transform * Transform (vello_encoding/src/math.rs:51-73) in f32, in its association and without FMA contraction: the
 // arithmetic of Encoding::append (encoding.py's Encoding.append, vb_scene.cpp's vb_scene_append), so a transform composed on
 // the device has the bits a host-side append produces. r = a * b; used by views (k_view.cu) and composition (k_compose.cu).

@@ -149,7 +149,6 @@ struct ImageKey {
 // A resident fragment: its streams in one device allocation, back to back behind a header of their word offsets (k_compose.cu
 // reads it), followed by a copy of the pixels of each image key it draws. Patch words are as the encoder wrote them.
 enum { CMP_TAGS, CMP_PATH_DATA, CMP_DRAW_TAGS, CMP_DRAW_DATA, CMP_TRANSFORMS, CMP_STYLES, CMP_STREAMS };
-#define CMP_HEADER_WORDS 8u
 #define CMP_FROM_OVERRIDE 0xffffffffu // the source of an atlas slot filled from an override (fragment ids start at 1, count up)
 // An image's atlas slot in a composition: (image-key id << 32 | pixel source), as in SceneSlot::atlas_keys, and x << 16 | y.
 struct ImgPlace {
@@ -315,6 +314,7 @@ struct vb_renderer {
     uint32_t next_image_key = 1;
     uint64_t compose_seq = 0;
     DevBuf compose_tmp;                  // compose's tables, staged through pinned[PIN_COMPOSE]
+    DevBuf paths_tmp;                    // the scratch of vb_fragment_from_device_paths (DpArgs, k_device_paths.cu)
     // What is bound to device rows (vb_bind_*, vb_compose.cu), with the device tables the bindings made at bind time (VbBound,
     // vb_stages.h), which point into the buffers below. Every scene installation unbinds (set_scene).
     //  - inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n)] [the fragments'
@@ -384,7 +384,7 @@ struct vb_renderer {
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
-                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->paths_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
                            &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap, &r->op_slots,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);

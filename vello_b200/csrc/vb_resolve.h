@@ -20,6 +20,31 @@ static inline uint64_t vb_draw_info_sum(const uint32_t *draw_tags, size_t n) {
     return info;
 }
 
+// f32 -> f16 (math.rs:93-127, float_to_half_fast3): the miter limit in a stroke's style word. The native scene front end
+// (vb_scene.cpp) and fragments from device arrays (vb_compose.cu) encode it.
+static inline uint32_t vb_f32_to_f16(float val) {
+    const uint32_t INF_32 = 255u << 23, INF_16 = 31u << 23, MAGIC = 15u << 23, ROUND_MASK = ~0xFFFu;
+    uint32_t u;
+    memcpy(&u, &val, 4);
+    const uint32_t sign = u & 0x80000000u;
+    u ^= sign;
+    uint32_t out;
+    if (u >= INF_32) {
+        out = u > INF_32 ? 0x7E00u : 0x7C00u;
+    } else {
+        u &= ROUND_MASK;
+        float f, magic;
+        memcpy(&f, &u, 4);
+        memcpy(&magic, &MAGIC, 4);
+        f = f * magic;
+        memcpy(&u, &f, 4);
+        u -= ROUND_MASK;
+        if (u > INF_16) u = INF_16;
+        out = (u >> 13) & 0xFFFFu;
+    }
+    return out | (sign >> 16);
+}
+
 // The packed scene's layout from the sizes of its streams (resolve.rs:107-154): the tag bytes and one PATH tag per open clip,
 // padded to 4 * PATH_REDUCE_WG bytes (resolve.rs:625, config.rs:237); path data; draw tags and one END_CLIP per open clip; draw
 // data; 6 words per transform; 2 per style. Sets *padded_tags (bytes) and *words (the whole scene). False when the scene, with

@@ -39,24 +39,6 @@ constexpr float EPS = 1e-12f; // path.rs:841
 inline uint32_t f32_bits(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
 inline float bits_f32(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 
-uint32_t f32_to_f16(float val) { // math.rs:93-127 (float_to_half_fast3)
-    const uint32_t INF_32 = 255u << 23, INF_16 = 31u << 23, MAGIC = 15u << 23, ROUND_MASK = ~0xFFFu;
-    uint32_t u = f32_bits(val);
-    const uint32_t sign = u & 0x80000000u;
-    u ^= sign;
-    uint32_t out;
-    if (u >= INF_32) {
-        out = u > INF_32 ? 0x7E00u : 0x7C00u;
-    } else {
-        u &= ROUND_MASK;
-        u = f32_bits(bits_f32(u) * bits_f32(MAGIC));
-        u -= ROUND_MASK;
-        if (u > INF_16) u = INF_16;
-        out = (u >> 13) & 0xFFFFu;
-    }
-    return out | (sign >> 16);
-}
-
 struct Color { float r, g, b, a; };
 inline Color multiply_alpha(Color c, float m) { return Color{c.r, c.g, c.b, c.a * m}; }
 uint32_t premul_rgba8(Color c) { // premultiply().to_rgba8().to_u32(), draw.rs:76-84; r is the low byte
@@ -112,7 +94,7 @@ struct Encoding {
     void encode_fill_style(uint32_t fill) { encode_style(Style{fill == VB_FILL_EVEN_ODD ? STYLE_FLAGS_FILL_BIT : 0u, 0.0f}); }
     bool encode_stroke_style(const vb_stroke &s) { // path.rs:70-120
         if (s.width == 0.0) return false;
-        const uint32_t flags = STYLE_FLAGS_STYLE_BIT | s.join | (s.start_cap << 2) | s.end_cap | f32_to_f16((float)s.miter_limit);
+        const uint32_t flags = STYLE_FLAGS_STYLE_BIT | s.join | (s.start_cap << 2) | s.end_cap | vb_f32_to_f16((float)s.miter_limit);
         encode_style(Style{flags, (float)s.width});
         return true;
     }

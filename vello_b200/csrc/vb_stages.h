@@ -244,6 +244,37 @@ struct CmpArgs {
     uint32_t cta0[6];             // first CTA of each stream (set by the launcher)
 };
 uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
+// A fragment's allocation starts with CMP_HEADER_WORDS words: the word offset of each of its six streams, then two zeros.
+#define CMP_HEADER_WORDS 8u
+
+// k_device_paths.cu: a fragment built from device arrays (vb_fragment_from_device_paths). The caller's arrays, the style, the
+// scratch the four launches share and the fragment they write. The scratch: per ring its first and last kept point (set to
+// all ones and zero), a flag for a ring the encoders' walk must decide (zero), its record {last kept point, code, start tangent
+// end}; a keep byte per point of a walked ring; a kept flag per path (zero); the error (all ones until a check fails: (kind
+// << 32) | first row); the look-back (vb_lookback_words(n_parts, 3), its leading words zero); each partition's exclusive
+// prefix (3 words); the totals of tag bytes, path-data words and draw objects (zero), which the caller reads back.
+#define VB_DP_ERR_RING_OFFSETS 1u
+#define VB_DP_ERR_PATH_OFFSETS 2u
+#define VB_DP_ERR_POINTS 3u
+#define VB_DP_ERR_COLOR 4u
+struct DpArgs {
+    const float *points;
+    const int32_t *ring_offsets, *path_offsets; // path_offsets null: one ring per path
+    const float *colors;
+    size_t point_pitch, color_pitch; // bytes
+    uint32_t n_points, n_rings, n_paths, n_parts;
+    uint32_t kind, closed, style_flags, style_width; // kind 0 fill, 1 stroke; the style entry's two words
+    uint32_t *ring_first, *ring_last, *ring_odd;
+    uint4 *rings;
+    uint8_t *keep_fix;
+    uint32_t *path_kept;
+    unsigned long long *err;
+    uint32_t *lookback, *part_excl, *totals;
+    uint32_t *fragment;
+    int32_t *draw_index; // optional
+};
+uint32_t vb_device_paths_parts(uint32_t n_points);
+uint32_t vb_launch_device_paths(const DpArgs &a, cudaStream_t st);
 // bound instance transforms: row_k * T of every transform T of the composed scene into the frame's bound region (prepare,
 // vb_frame.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);

@@ -65,6 +65,14 @@ class _EncodingStreams(C.Structure):
                 ("ramp_patches", C.c_void_p), ("n_ramp_patches", C.c_uint32), ("image_patches", C.c_void_p), ("n_image_patches", C.c_uint32)]
 
 
+class _DevicePaths(C.Structure):
+    _fields_ = [("points", C.c_void_p), ("n_points", C.c_uint32), ("point_pitch_bytes", C.c_size_t),
+                ("ring_offsets", C.c_void_p), ("n_rings", C.c_uint32), ("path_offsets", C.c_void_p), ("n_paths", C.c_uint32),
+                ("colors", C.c_void_p), ("color_pitch_bytes", C.c_size_t), ("kind", C.c_uint32), ("fill_rule", C.c_uint32),
+                ("width", C.c_float), ("miter_limit", C.c_float), ("join", C.c_uint32), ("start_cap", C.c_uint32),
+                ("end_cap", C.c_uint32), ("closed", C.c_uint32), ("draw_index", C.c_void_p)]
+
+
 class _Instance(C.Structure):
     _fields_ = [("fragment", C.c_uint32), ("has_transform", C.c_uint32), ("transform", C.c_double * 6)]
 
@@ -169,6 +177,7 @@ def load_library() -> C.CDLL:
     lib.vb_hit_map.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, C.c_size_t, C.c_uint32]
     lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
+    lib.vb_fragment_from_device_paths.argtypes = [vp, C.POINTER(_DevicePaths), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_recompose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_debug_match_instances.argtypes = [vp, C.c_uint32, vp, C.c_uint32, vp]
@@ -204,14 +213,16 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_bind_instance_transforms", "vb_set_damage_tracking", "vb_add_damage", "vb_last_damage",
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
-                    "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths", "vb_bind_draw_opacity"]
+                    "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths", "vb_bind_draw_opacity",
+                    "vb_fragment_from_device_paths"]
 
 
-def _device_rows(t, who: str, what: str, cols: int, vector: bool = False):
+def _device_rows(t, who: str, what: str, cols: int, vector: bool = False, empty: bool = False):
     """(pointer, rows, row pitch in bytes) of an (n, cols) float32 device array bound by a `bind_*` method, from its
     `__cuda_array_interface__` (a torch CUDA tensor, or columns of a larger one): columns 4 bytes apart and rows any multiple of
     4 bytes, at least 4 * cols, apart. With `vector` (cols = 1) an (n,) array is taken as (n, 1), so a column of a larger
-    tensor such as `state[:, 5]` binds with its row stride. `who` names the method and `what` the rows in the errors."""
+    tensor such as `state[:, 5]` binds with its row stride. With `empty`, n = 0 is taken (a null pointer and the least pitch).
+    `who` names the method and `what` the rows in the errors."""
     cai = getattr(t, "__cuda_array_interface__", None)
     if cai is None:
         raise TypeError(f"{type(t).__name__} has no __cuda_array_interface__: device {what} are needed")
@@ -220,9 +231,11 @@ def _device_rows(t, who: str, what: str, cols: int, vector: bool = False):
     rows = shape
     if vector and len(shape) == 1:
         rows, strides = shape + (1,), strides and (strides[0], 4)
-    if len(rows) != 2 or rows[0] == 0 or rows[1] != cols or cai["typestr"] != "<f4":
+    if len(rows) != 2 or (rows[0] == 0 and not empty) or rows[1] != cols or cai["typestr"] != "<f4":
         form = f"(n,) or (n, {cols})" if vector else f"(n, {cols})"
         raise ValueError(f"{who}: {what} must be {form} float32, not {shape} {cai['typestr']}")
+    if rows[0] == 0:
+        return None, 0, 4 * cols
     shape = rows
     strides = strides or (4 * cols, 4)
     pitch = int(strides[0]) if shape[0] > 1 else 4 * cols  # the pitch of a single row is never used
@@ -230,6 +243,23 @@ def _device_rows(t, who: str, what: str, cols: int, vector: bool = False):
         raise ValueError(f"{who}: columns 4 bytes apart and rows a multiple of 4 bytes, at least {4 * cols}, apart; "
                          f"not strides {tuple(strides)}")
     return C.c_void_p(int(cai["data"][0])), shape[0], pitch
+
+
+def _device_offsets(t, who: str, what: str, dtype: str = "<i4"):
+    """(pointer, entries) of a contiguous 1-D int32 device array, from its `__cuda_array_interface__`. int64 offsets (torch's
+    default integer type) are refused with the conversion to make. `who` names the method and `what` the array in the errors."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{who}: {type(t).__name__} has no __cuda_array_interface__: device {what} are needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if cai["typestr"] == "<i8" and dtype == "<i4":
+        raise ValueError(f"{who}: {what} are int64; convert them to int32 (e.g. `t.to(torch.int32)`)")
+    if len(shape) != 1 or cai["typestr"] != dtype:
+        raise ValueError(f"{who}: {what} must be a 1-D int32 array, not {shape} {cai['typestr']}")
+    strides = cai.get("strides")
+    if strides is not None and shape[0] > 1 and tuple(strides) != (4,):
+        raise ValueError(f"{who}: {what} must be contiguous, not strides {tuple(strides)}")
+    return (C.c_void_p(int(cai["data"][0])) if shape[0] else None), shape[0]
 
 
 def _device_flags(t, who: str):
@@ -508,6 +538,49 @@ class Renderer:
             except TypeError:  # not weakly referenceable: a copy for this upload only
                 pass
         return int(copy.ctypes.data)
+
+    def upload_device_paths(self, points, ring_offsets, colors, *, path_offsets=None, style=0, closed: bool = True,
+                            draw_index=None):
+        """Build a fragment on the device from ragged device arrays (`vb_fragment_from_device_paths`) and return (fragment id,
+        draw objects). `points` is float32 (P, 2) x y rows, `ring_offsets` int32 (R + 1,): ring r is points ring_offsets[r] ..
+        ring_offsets[r + 1] - 1; `path_offsets` int32 (N + 1,) over rings (None: each ring is a path); `colors` float32 (N, 4)
+        straight-alpha r g b a, one row per path. Arrays come through `__cuda_array_interface__` (e.g. torch CUDA tensors); points
+        and colours may be columns of larger arrays (rows any multiple of 4 bytes apart), offsets are contiguous. `style` is a
+        fill rule (FILL_NON_ZERO, FILL_EVEN_ODD) or an undashed `Stroke`; `closed` closes a stroke's rings (fills always close).
+        The fragment is word for word `upload_fragment` of a Scene that fills (or strokes) each path i with Color(colors[i]) under
+        the identity, its shape being, per ring, a move to the first point, lines to the others and, when closed, a close.
+        `draw_index` (optional, int32 (N,) device array) receives each path's draw object in the fragment, or -1 for a path that
+        encodes nothing. Write the arrays on `self.stream` (or synchronise) before the call; it returns once the fragment is
+        built."""
+        from .encoding import Stroke
+        who = "upload_device_paths"
+        pts, n_pts, pitch = _device_rows(points, who, "points", 2, empty=True)
+        rings, n_roff = _device_offsets(ring_offsets, who, "ring_offsets")
+        if n_roff == 0:
+            raise ValueError(f"{who}: ring_offsets has n_rings + 1 entries, at least 1")
+        paths, n_poff = (None, n_roff) if path_offsets is None else _device_offsets(path_offsets, who, "path_offsets")
+        if n_poff == 0:
+            raise ValueError(f"{who}: path_offsets has n_paths + 1 entries, at least 1")
+        cols, n_cols, cpitch = _device_rows(colors, who, "colours", 4, empty=True)
+        if n_cols != n_poff - 1:
+            raise ValueError(f"{who}: {n_cols} colours for {n_poff - 1} paths")
+        d = _DevicePaths(pts, n_pts, pitch, rings, n_roff - 1, paths, n_poff - 1, cols, cpitch)
+        if isinstance(style, Stroke):
+            if style.dash_pattern:
+                raise ValueError(f"{who}: dashed strokes are not built on the device; encode them with Scene.stroke")
+            d.kind, d.width, d.miter_limit = 1, style.width, style.miter_limit
+            d.join, d.start_cap, d.end_cap, d.closed = style.join, style.start_cap, style.end_cap, 1 if closed else 0
+        else:
+            d.kind, d.fill_rule = 0, int(style)
+        if draw_index is not None:
+            idx, n_idx = _device_offsets(draw_index, who, "draw_index")
+            if n_idx != n_poff - 1:
+                raise ValueError(f"{who}: draw_index has {n_idx} entries for {n_poff - 1} paths")
+            d.draw_index = idx
+        fid, n_draws = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.lib.vb_fragment_from_device_paths(self.handle, C.byref(d), C.byref(fid), C.byref(n_draws)),
+                    "vb_fragment_from_device_paths")
+        return int(fid.value), int(n_draws.value)
 
     def free_fragment(self, fragment: int):
         """Release a fragment (after the work already enqueued that reads it). Composed scenes are copies: they stay."""
