@@ -492,7 +492,8 @@ int vb_fragment_free(vb_renderer *, uint32_t fragment);
  * two distinct points writes nothing, a ring closes with a line when its last kept point differs bit for bit from its first,
  * strokes end each ring with a cap marker, and a path whose rings all write nothing draws nothing. Its one TRANSFORM (identity)
  * and STYLE come first when n_paths > 0; n_paths = 0 is the empty fragment. join and caps are vb_stroke's (VB_JOIN_*,
- * VB_CAP_*, vello_b200_scene.h); dashes, curves, brushes other than one colour per path, and clips are not part of it.
+ * VB_CAP_*, vello_b200_scene.h); dashes, brushes other than one colour per path, and clips are not part of it (curves are
+ * vb_fragment_from_device_curves, below).
  * *n_draw_objects_out (optional) receives the fragment's draw objects; draw_index (optional, n_paths int32 entries, device
  * memory) receives path i's draw object within the fragment, or -1 for a path that draws nothing. Which path-data rows a
  * point lands in depends on the points dropped, so bind points of such a fragment (vb_bind_path_points) only with rows made
@@ -524,6 +525,30 @@ typedef struct {
     int32_t *draw_index;       /* optional out, n_paths entries: path i's draw object in the fragment, or -1 */
 } vb_device_paths;
 int vb_fragment_from_device_paths(vb_renderer *, const vb_device_paths *, uint32_t *fragment_out, uint32_t *n_draw_objects_out);
+/* vb_fragment_from_device_curves: vb_fragment_from_device_paths of quadratic and cubic Bézier paths (an addition; no vello
+ * counterpart): glyph outlines (TrueType quadratics, CFF cubics), the control points a vector-graphics model outputs, circle
+ * and ellipse markers, splines. point_kinds holds one byte per point (n_points, device or managed memory of the renderer's
+ * device, any alignment): 0 on-curve, 1 off-curve. Within a ring each on-curve point after the first ends one segment, chosen
+ * by the k off-curve points in front of it: k = 0 L e, k = 1 Q c e, k = 2 C c1 c2 e. The fragment is word for word what
+ * vb_fragment_upload receives from the Scene loop above, shape_i being, for each ring of path i, M p_first, those segments in
+ * order, then Z (fills always; strokes when `closed`). A curved closing segment repeats the first point as its end: Z then adds
+ * no line, the points being equal bit for bit. point_kinds NULL is vb_fragment_from_device_paths. The encoders' rules hold bit
+ * for bit:
+ *  - before a ring's first kept segment, a segment is kept when one of its points is EPS-far (1e-12 in x or y) from the ring's
+ *    first point (start_tangent_for_line / _quad / _curve); that segment gives the start tangent's end (a line: p0 + 1/3 (e -
+ *    p0); a quad: c + 1/3 (p0 - c), or c + 1/3 (e - c) when c is EPS-close to p0; a cubic: the first of c1, c2, e EPS-far from
+ *    p0). This is not the span test: with p0.x = 0, c.x = 8e-13 and e.x = -8e-13 the quad is dropped;
+ *  - after it, a segment is kept when the span of the last kept end point and the segment's points exceeds EPS in x or y;
+ *  - the closing line, the cap markers, SUBPATH_END, the PATH tag, the draw object and draw_index are as above, the last kept
+ *    end point standing for the last kept point.
+ * The worst case of the allocation does not change: a kept segment's points write two words each, and its tag belongs to its
+ * end point. Which path-data rows a point lands in depends on the segments dropped, as above.
+ * VB_E_INVALID as vb_fragment_from_device_paths, and also: point_kinds that is not device or managed memory of the renderer's
+ * device; checked on the device, naming the first offending row: a kind other than 0 or 1, a ring whose first or last point is
+ * off-curve, a third off-curve point in a row. Arcs, TrueType's implied on-curve midpoints (the caller inserts them), dashes and
+ * other brushes are not part of it. */
+int vb_fragment_from_device_curves(vb_renderer *, const vb_device_paths *, const uint8_t *point_kinds, uint32_t *fragment_out,
+                                   uint32_t *n_draw_objects_out);
 int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
 /* vb_recompose: vb_compose, followed by a frame that repaints only what the new instance list changed (an addition; no vello
  * counterpart). It installs exactly the scene vb_compose would (scene, layout, ramps, atlas and draw offsets, byte for byte),

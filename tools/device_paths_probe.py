@@ -1,6 +1,7 @@
-"""Fragments from device arrays (Renderer.upload_device_paths, vb_fragment_from_device_paths) against the host route, on two
-inputs: about 30k paris-like polygons (1.5M points, a few with holes, filled) in a 4096^2 frame, and one 1M-point polyline
-(stroked). Prints, with the card, its power limit and SM clock:
+"""Fragments from device arrays (Renderer.upload_device_paths, vb_fragment_from_device_paths / _curves) against the host
+route, on four inputs in a 4096^2 frame: about 30k paris-like polygons (1.5M points, a few with holes, filled), one 1M-point
+polyline (stroked), 100k circles of four cubics each (1.3M points, filled, with point_kinds) and 20k glyph-like quadratic
+contours (an outer contour and a counter each, filled, with point_kinds). Prints, with the card, its power limit and SM clock:
   call_ms     the call's wall time (it ends with its one synchronisation), and kernel_ms, the span of its work on vb_stream
               from CUDA events recorded around it (scratch clears, the four kernels and the read-back of the totals)
   host_ms     the host route for the same rows: the arrays copied to the host, one vb_scene_fill / vb_scene_stroke per path
@@ -10,8 +11,8 @@ inputs: about 30k paris-like polygons (1.5M points, a few with holes, filled) in
               compose's stream lengths may change and the frame graph is captured anew (graph_captures counts it); and
               the cost of that capture: frames that cycle through six row counts (new lengths every frame, more than
               the four cached graphs, so a capture every frame), with frame graphs on and off
-With --out the result also goes to DIR/device_paths_probe.json:
-    python tools/device_paths_probe.py [--reps 10] [--frames 20] [--out DIR]"""
+--inputs picks some of the inputs by name. With --out the result also goes to DIR/device_paths_probe.json:
+    python tools/device_paths_probe.py [--reps 10] [--frames 20] [--inputs polygons_30k,...] [--out DIR]"""
 import argparse
 import ctypes as C
 import json
@@ -59,21 +60,57 @@ def polyline(n=1_000_000, seed=2):
     return np.stack([x, y], 1).astype(np.float32), np.array([0, n], np.int32), None, np.array([[1, 0.9, 0.2, 1]], np.float32)
 
 
-def host_route(r, pts, roff, poff, cols, style):
+def circles(n=100_000, seed=3):
+    """n circles of radius 4..40, each M and the four cubics of shapes.path_elements(Circle) (13 points, the last the first)."""
+    rng = np.random.default_rng(seed)
+    arm, unit = 0.551915024494, [(1.0, 0.0)]
+    for ix in range(1, 5):
+        th0, th1 = (ix - 1) * np.pi / 2, ix * np.pi / 2
+        s0, c0 = np.sin(th0), np.cos(th0)
+        s1, c1 = (0.0, 1.0) if ix == 4 else (np.sin(th1), np.cos(th1))
+        unit += [(c0 - arm * s0, s0 + arm * c0), (c1 + arm * s1, s1 - arm * c1), (c1, s1)]
+    c, rad = rng.uniform(0, SIZE, (n, 2)), rng.uniform(4, 40, n)
+    pts = (c[:, None, :] + rad[:, None, None] * np.array(unit)[None]).reshape(-1, 2).astype(np.float32)
+    kinds = np.tile(np.array([0] + [1, 1, 0] * 4, np.uint8), n)
+    cols = rng.uniform(0, 1, (n, 4)).astype(np.float32)
+    return pts, np.arange(0, 13 * n + 1, 13, dtype=np.int32), None, cols, kinds
+
+
+def glyphs(n=20_000, seed=4):
+    """n glyph-like outlines of 20..60 px: an outer quadratic contour of 8 quads and a counter wound the other way, with
+    TrueType's implied on-curve points inserted (17 points a contour, the last the first)."""
+    rng = np.random.default_rng(seed)
+    t = np.linspace(0, 2 * np.pi, 17)
+    rad = np.where(np.arange(17) % 2 == 0, 1.0, 1.0 / np.cos(np.pi / 8))  # control points on the tangents' crossings
+    unit = np.stack([np.cos(t) * rad, np.sin(t) * rad], 1)
+    unit[-1] = unit[0]
+    s, c = rng.uniform(10, 30, n), rng.uniform(0, SIZE, (n, 2))
+    outer = c[:, None, :] + s[:, None, None] * unit[None] * (1.0, 1.3)
+    inner = c[:, None, :] + 0.5 * s[:, None, None] * unit[None, ::-1]
+    pts = np.concatenate([outer, inner], 1).reshape(-1, 2).astype(np.float32)
+    kinds = np.tile((np.arange(17) % 2).astype(np.uint8), 2 * n)
+    cols = rng.uniform(0, 1, (n, 4)).astype(np.float32)
+    return pts, np.arange(0, 34 * n + 1, 17, dtype=np.int32), np.arange(0, 2 * n + 1, 2, dtype=np.int32), cols, kinds
+
+
+def host_route(r, pts, roff, poff, cols, style, kinds=None):
     """Copy the device arrays to the host, encode one fill or stroke per path through the native scene, upload the fragment."""
-    p, ro, po, co = (t.cpu().numpy() if t is not None else None for t in (pts, roff, poff, cols))
+    p, ro, po, co, ki = (t.cpu().numpy() if t is not None else None for t in (pts, roff, poff, cols, kinds))
     s = NativeScene()
     lib, h = s.lib, s.handle
     n_paths = len(po) - 1 if po is not None else len(ro) - 1
-    # one verb and one coordinate array: per ring M, L..., Z (strokes here are open: no Z)
+    # one verb and one coordinate array: per ring M, then L, Q or C per on-curve point after the first (the coordinates are
+    # the points, in order), then Z (strokes here are open: no Z)
     stroke = isinstance(style, Stroke)
-    ring_len = np.diff(ro)
-    verbs = []
-    for k in ring_len:
-        verbs += [ord("M")] + [ord("L")] * (int(k) - 1) + ([] if stroke else [ord("Z")])
-    verbs = np.array(verbs, np.uint8)
+    on = np.ones(len(p), bool) if ki is None else ki == 0
+    verb_of = np.frombuffer(b"?LQC", np.uint8)
+    verbs, vstart = [], [0]
+    for a, b in zip(ro[:-1], ro[1:]):
+        ends = np.flatnonzero(on[a:b])
+        verbs.append(np.concatenate([[ord("M")], verb_of[np.diff(ends)], [] if stroke else [ord("Z")]]).astype(np.uint8))
+        vstart.append(vstart[-1] + len(verbs[-1]))
+    verbs = np.concatenate(verbs)
     coords = p.astype(np.float64).reshape(-1)
-    vstart = np.concatenate([[0], np.cumsum(ring_len + (0 if stroke else 1))])
     ident = _affine(Affine.IDENTITY)
     st = _Stroke(style.width, style.join, style.start_cap, style.end_cap, style.miter_limit, None, 0, 0.0) if stroke else None
     for i in range(n_paths):
@@ -89,10 +126,12 @@ def host_route(r, pts, roff, poff, cols, style):
 
 
 def measure(r, name, data, style, reps, n_frames):
-    pts, roff, poff, cols = (torch.as_tensor(a).cuda() if a is not None else None for a in data)
+    pts, roff, poff, cols, kinds = (torch.as_tensor(a).cuda() if a is not None else None for a in (tuple(data) + (None,))[:5])
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     st = torch.cuda.ExternalStream(r.stream)
     kw = dict(path_offsets=poff, style=style, closed=False)
+    if kinds is not None:
+        kw["point_kinds"] = kinds
     f, n = r.upload_device_paths(pts, roff, cols, **kw)  # warm-up
     r.free_fragment(f)
     call, kern = [], []
@@ -109,7 +148,7 @@ def measure(r, name, data, style, reps, n_frames):
     for _ in range(max(2, reps // 3)):
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        f = host_route(r, pts, roff, poff, cols, style)
+        f = host_route(r, pts, roff, poff, cols, style, kinds)
         host.append((time.perf_counter() - t0) * 1e3)
         r.free_fragment(f)
     # frames: the geometry moves every frame (by 0.25 px per frame), rebuilt on the device or encoded on the host
@@ -128,7 +167,7 @@ def measure(r, name, data, style, reps, n_frames):
             if route == "device":
                 f, _ = r.upload_device_paths(moved, roff, cols, **kw)
             else:
-                f = host_route(r, moved, roff, poff, cols, style)
+                f = host_route(r, moved, roff, poff, cols, style, kinds)
             r.compose([(f, None)])
             r.render_resident(p)
             r.free_fragment(f)
@@ -138,12 +177,13 @@ def measure(r, name, data, style, reps, n_frames):
     # recapture: the frames cycle through fragments of six stream lengths (all the rows, then 5/6 .. 1/6 of them), more than
     # the renderer's four cached frame graphs, so every frame captures its graph anew; against the same cycle without graphs
     def part(v):
-        if poff is None:
+        if poff is None and len(roff) == 2:
             q = pts.shape[0] * (6 - v) // 6
-            return pts[:q], torch.tensor([0, q], dtype=torch.int32, device="cuda"), None, cols
-        n_p = (len(poff) - 1) * (6 - v) // 6
-        n_r = int(poff[n_p])
-        return pts[:int(roff[n_r])], roff[:n_r + 1], poff[:n_p + 1], cols[:n_p]
+            return pts[:q], torch.tensor([0, q], dtype=torch.int32, device="cuda"), None, cols, None
+        n_p = (len(cols)) * (6 - v) // 6
+        n_r = int(poff[n_p]) if poff is not None else n_p
+        q = int(roff[n_r])
+        return pts[:q], roff[:n_r + 1], None if poff is None else poff[:n_p + 1], cols[:n_p], None if kinds is None else kinds[:q]
     halves = [part(v) for v in range(6)]
     for graphs in (True, False):
         r.set_cuda_graph(graphs)
@@ -151,8 +191,8 @@ def measure(r, name, data, style, reps, n_frames):
             if k == 3:
                 torch.cuda.synchronize()
                 t0, cap0 = time.perf_counter(), r.debug_graph_captures()
-            q, ro, po, co = halves[k % 6]
-            f, _ = r.upload_device_paths(q, ro, co, path_offsets=po, style=style, closed=False)
+            q, ro, po, co, ki = halves[k % 6]
+            f, _ = r.upload_device_paths(q, ro, co, path_offsets=po, style=style, closed=False, **({} if ki is None else {"point_kinds": ki}))
             r.compose([(f, None)])
             r.render_resident(p)
             r.free_fragment(f)
@@ -170,11 +210,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--inputs", default="polygons_30k,polyline_1m,circles_100k,glyphs_20k")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    inputs = {"polygons_30k": (polygons, FILL_NON_ZERO), "polyline_1m": (polyline, Stroke(2.0)),
+              "circles_100k": (circles, FILL_NON_ZERO), "glyphs_20k": (glyphs, FILL_NON_ZERO)}
     r = Renderer()
-    res = {"card": card(), "results": [measure(r, "polygons_30k", polygons(), FILL_NON_ZERO, a.reps, a.frames),
-                                       measure(r, "polyline_1m", polyline(), Stroke(2.0), a.reps, a.frames)],
+    res = {"card": card(), "results": [measure(r, k, inputs[k][0](), inputs[k][1], a.reps, a.frames) for k in a.inputs.split(",")],
            "card_after": card()}
     print(json.dumps(res, indent=1))
     if a.out:

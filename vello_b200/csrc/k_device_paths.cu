@@ -1,38 +1,49 @@
-// k_device_paths.cu -- fragments from device arrays (vb_fragment_from_device_paths): the encoding of ragged polygons or
-// polylines held in device memory (points, ring offsets, optional path offsets, colours), built on the device, word for word
-// what the host encoder writes for
+// k_device_paths.cu -- fragments from device arrays (vb_fragment_from_device_paths, vb_fragment_from_device_curves): the
+// encoding of ragged polygons, polylines or Bézier paths held in device memory (points, optional point kinds, ring offsets,
+// optional path offsets, colours), built on the device, word for word what the host encoder writes for
 //     for each path i: scene.fill(rule, IDENTITY, Color(colors[i]), None, shape_i)   (or scene.stroke(stroke, ...))
-// where shape_i is, for each ring of path i, M p_first, L p for every following point, then Z (fills always, strokes when
-// `closed`). The PathEncoder's rules (encoding.py's PathEncoder, vb_scene.cpp's) decide what each point writes:
-//  - a line to a point EPS-close (1e-12 on the f32 differences) to the last KEPT point writes nothing;
-//  - a ring that keeps no line writes nothing at all (its move-to is replaced or dropped);
-//  - a kept ring ends with the closing line when its last kept point differs bit for bit from its first point (fills and
+// where shape_i is, for each ring of path i, M p_first, then one segment per following on-curve point e (kind 0), chosen by
+// the off-curve points (kind 1) in front of it: none L e, one Q c e, two C c1 c2 e; then Z (fills always, strokes when
+// `closed`). Without kinds every point is on-curve: M p_first, L p... The PathEncoder's rules (encoding.py's PathEncoder,
+// vb_scene.cpp's) decide what each segment writes:
+//  - before a ring's first kept segment (MoveTo state) a segment is kept when one of its points is EPS-far (1e-12 on the f32
+//    differences) from the ring's first point (the start-tangent tests); that segment gives the ring's start tangent end;
+//  - after it, a segment is kept when the EPS span of the last kept end point and the segment's points exceeds EPS in x or y
+//    (is_zero_length_segment);
+//  - a ring that keeps no segment writes nothing at all (its move-to is replaced or dropped);
+//  - a kept ring ends with the closing line when its last kept end point differs bit for bit from its first point (fills and
 //    closed strokes), then for a stroke its cap marker (closed: a line to the start tangent's end; open: a quad through the
 //    first point to it), which is itself dropped when EPS-close to where the ring stands; its last tag gets SUBPATH_END;
 //  - a path that keeps a ring ends with a PATH tag and draws one FILL_COLOR draw object.
+// A kept segment's points write their own two path-data words each, and its tag byte belongs to its end point.
 //
 // Four launches, in stream order, all sized from the caller's counts:
 //  1. k_device_paths_points, one thread per point, per ring offset, per path offset and per colour row: the device-side
-//     checks (one 64-bit atomicMin of (kind << 32 | row), so the first offending row of the first kind wins), and each point's
-//     neighbour test p_j != p_{j-1}. The keep rule "differs from the last kept point" equals it unless a neighbouring pair is
-//     EPS-close but unequal in value (coordinates below about 1.7e-5): such rings are flagged. +0 beside -0 is equal in value
-//     and its differences are the same, so it needs no walk; the closing line compares bits on either route. Warp-aggregated
-//     atomics give each ring its first and last kept point.
+//     checks (one 64-bit atomicMin of (kind << 32 | row), so the first offending row of the first kind wins), and for each
+//     point: the start-tangent test against the ring's first point, and for an on-curve point the span test of its segment
+//     against the segment's own start (the previous on-curve point). Warp-aggregated atomics give each ring its first kept
+//     segment (the lowest end point whose segment passes the tangent test: exact, with no sequential dependency), the last end
+//     point that passes the span test, and the last end point whose segment fails it while ending unequal in value to its
+//     start. The span rule "against the last kept end point" equals the test against the segment's own start unless such a
+//     dropped segment lies after the first kept one (coordinates below about 1.7e-5): only those rings are walked. +0 beside
+//     -0 is equal in value and its differences are the same, so it needs no walk; the closing line compares bits on either
+//     route.
 //  2. k_device_paths_rings, one thread per ring: a flagged ring is walked in order with the exact rule (its keep flags go to
-//     a byte per point); then the ring's record: kept or not, last kept point, closing line, cap marker, start tangent. A kept
-//     ring marks its path kept.
+//     a byte per end point); then the ring's record: kept or not, last kept end point, closing line, cap marker, start tangent
+//     end. A kept ring marks its path kept.
 //  3. k_device_paths_count, 256 points per partition in ticket order: each point's tag bytes, path-data words and draw objects
 //     (the ring-end and path-end contributions belong to the ring's and the path's last point), summed with one packed block
 //     scan and the decoupled look-back (K = 3). The last partition writes the totals.
 //  4. k_device_paths_emit: the header and the six streams, straight into the fragment's allocation in vb_fragment_upload's
 //     layout (the header's word offsets, then the streams back to back, tags padded to whole words with zero bytes), and
 //     draw_index.
-// Every launch after the first returns at once when a check failed: the offsets are then not trusted to index anything.
+// Every launch after the first returns at once when a check failed: the offsets and kinds are then not trusted to index
+// anything.
 #include "vb_device.cuh"
 #include "vb_stages.h"
 
 #define DP_THREADS 256u
-#define DP_TAG_LINE 0x09u
+#define DP_TAG_LINE 0x09u // + 1 per control point: QUAD 0x0a, CUBIC 0x0b
 #define DP_TAG_QUAD 0x0au
 #define DP_TAG_PATH 0x10u
 #define DP_TAG_TRANSFORM 0x20u
@@ -40,7 +51,7 @@
 #define DP_SUBPATH_END 0x04u
 #define DP_EPS 1e-12f // path.rs:841; f32(1e-12) < 1e-12, so `d > DP_EPS` is the encoders' test for every f32 d
 
-// a ring record (DpArgs::rings) is {last kept point, code, start tangent end x, y}; the code's bits:
+// a ring record (DpArgs::rings) is {last kept end point, code, start tangent end x, y}; the code's bits:
 #define DP_KEPT 1u
 #define DP_CLOSE 2u   // the closing line to the first point
 #define DP_CAP_LINE 4u
@@ -51,6 +62,8 @@ __device__ __forceinline__ float2 dp_point(const DpArgs &a, uint32_t j) {
     const float *p = reinterpret_cast<const float *>(reinterpret_cast<const uint8_t *>(a.points) + (size_t)j * a.point_pitch);
     return make_float2(__ldg(p), __ldg(p + 1));
 }
+// a point's kind: 0 on-curve, 1 off-curve; without kinds every point is on-curve
+__device__ __forceinline__ uint32_t dp_kind(const DpArgs &a, uint32_t j) { return a.kinds ? (uint32_t)__ldg(a.kinds + j) : 0u; }
 // the encoders' EPS test of two points (PathEncoder._neq; _zero_len of a line)
 __device__ __forceinline__ bool dp_neq(float2 p, float2 q) {
     return fabsf(__fsub_rn(p.x, q.x)) > DP_EPS || fabsf(__fsub_rn(p.y, q.y)) > DP_EPS;
@@ -58,6 +71,32 @@ __device__ __forceinline__ bool dp_neq(float2 p, float2 q) {
 __device__ __forceinline__ float dp_span3(float a, float b, float c) { return __fsub_rn(fmaxf(fmaxf(a, b), c), fminf(fminf(a, b), c)); }
 __device__ __forceinline__ bool dp_same_bits(float2 p, float2 q) {
     return __float_as_uint(p.x) == __float_as_uint(q.x) && __float_as_uint(p.y) == __float_as_uint(q.y);
+}
+// the segment that point j (b0 < j < b1) belongs to ends at the first on-curve point at or after j; with checked kinds that is
+// j, j + 1 or j + 2, and before the checks it stays inside the ring
+__device__ __forceinline__ uint32_t dp_seg_end(const DpArgs &a, uint32_t j, uint32_t b1) {
+    uint32_t e = j;
+    if (a.kinds)
+        while (e + 1u < b1 && e < j + 2u && dp_kind(a, e) == 1u) e++;
+    return e;
+}
+// the degree of the segment ending at on-curve point e (b0 < e): 1 + the off-curve points in front of it, at most 3, never
+// reaching the ring's first point. Its start is point e - degree.
+__device__ __forceinline__ uint32_t dp_degree(const DpArgs &a, uint32_t b0, uint32_t e) {
+    uint32_t d = 1u;
+    if (a.kinds)
+        while (d < 3u && e - d > b0 && dp_kind(a, e - d) == 1u) d++;
+    return d;
+}
+// is_zero_length_segment, negated: the EPS span of `at` (where the ring stands) and points s + 1 .. e exceeds EPS in x or y;
+// pe is point e (a line reads no other point)
+__device__ __forceinline__ bool dp_span_keeps(const DpArgs &a, float2 at, uint32_t s, uint32_t e, float2 pe) {
+    float x0 = fminf(at.x, pe.x), x1 = fmaxf(at.x, pe.x), y0 = fminf(at.y, pe.y), y1 = fmaxf(at.y, pe.y);
+    for (uint32_t k = s + 1u; k < e; k++) {
+        const float2 q = dp_point(a, k);
+        x0 = fminf(x0, q.x), x1 = fmaxf(x1, q.x), y0 = fminf(y0, q.y), y1 = fmaxf(y1, q.y);
+    }
+    return __fsub_rn(x1, x0) > DP_EPS || __fsub_rn(y1, y0) > DP_EPS;
 }
 // the last k in [0, n) with off[k] <= x (offsets checked: non-decreasing from 0). n >= 1: the launches after the first run only
 // when the checks passed, and then points imply a ring (ring_offsets[0] = 0 < n_points = ring_offsets[n_rings]) and rings a
@@ -88,28 +127,41 @@ __global__ void __launch_bounds__(DP_THREADS) k_device_paths_points(DpArgs a) {
         const float *c = reinterpret_cast<const float *>(reinterpret_cast<const uint8_t *>(a.colors) + (size_t)g * a.color_pitch);
         if (!(isfinite(__ldg(c)) && isfinite(__ldg(c + 1)) && isfinite(__ldg(c + 2)) && isfinite(__ldg(c + 3)))) dp_fail(a, VB_DP_ERR_COLOR, g);
     }
-    // points: every lane of the warp takes part in the aggregation below
-    uint32_t ring = 0xffffffffu, kept = 0u, odd = 0u;
+    // points: every lane of the warp takes part in the aggregation below. `tangent` is the end point of this point's segment
+    // when the point is EPS-far from the ring's first one; `span` an end point whose segment passes the span test against its
+    // own start; `odd` one whose segment fails it but ends unequal in value to its start.
+    uint32_t ring = 0xffffffffu, tangent = 0xffffffffu, span = 0u, odd = 0u;
     if (g < a.n_points && a.n_rings) {
         const float2 p = dp_point(a, g);
         if (!(isfinite(p.x) && isfinite(p.y))) dp_fail(a, VB_DP_ERR_POINTS, g);
         ring = dp_find(a.ring_offsets, a.n_rings, g);
         const int32_t first = __ldg(a.ring_offsets + ring);
+        const uint32_t b1 = a.kinds ? min((uint32_t)__ldg(a.ring_offsets + ring + 1u), a.n_points) : 0u; // unchecked yet
+        if (a.kinds) {
+            // a value other than 0 or 1; an off-curve point first or last in its ring, or third in a row (a run across rings
+            // has an off-curve last point at a lower row, so the first offending row is the same)
+            const uint32_t k = dp_kind(a, g);
+            if (k > 1u || (k == 1u && ((int32_t)g == first || g + 1u == b1 || (g >= 2u && dp_kind(a, g - 1u) == 1u && dp_kind(a, g - 2u) == 1u))))
+                dp_fail(a, VB_DP_ERR_KINDS, g);
+        }
         if (first >= 0 && (uint32_t)first < g) {
-            const float2 q = dp_point(a, g - 1u);
-            kept = dp_neq(p, q) ? 1u : 0u;
-            odd = !kept && !(p.x == q.x && p.y == q.y) ? 1u : 0u; // EPS-close but unequal: the neighbour test may not hold
+            const uint32_t b0 = (uint32_t)first;
+            if (dp_neq(p, dp_point(a, b0))) tangent = a.kinds ? dp_seg_end(a, g, b1) : g;
+            if (dp_kind(a, g) == 0u) {
+                const uint32_t s = g - dp_degree(a, b0, g);
+                const float2 q = dp_point(a, s);
+                if (dp_span_keeps(a, q, s, g, p)) span = g;
+                else if (!(p.x == q.x && p.y == q.y)) odd = g;
+            }
         }
     }
     const uint32_t group = __match_any_sync(VB_FULL, ring);
-    const uint32_t lo = __reduce_min_sync(group, kept ? g : 0xffffffffu), hi = __reduce_max_sync(group, kept ? g : 0u);
-    const uint32_t any_odd = __reduce_or_sync(group, odd);
+    const uint32_t lo = __reduce_min_sync(group, tangent), hi = __reduce_max_sync(group, span);
+    const uint32_t last_odd = __reduce_max_sync(group, odd);
     if (ring != 0xffffffffu && vb_lane() == (uint32_t)__ffs(group) - 1u) {
-        if (lo != 0xffffffffu) {
-            atomicMin(a.ring_first + ring, lo);
-            atomicMax(a.ring_last + ring, hi);
-        }
-        if (any_odd) atomicOr(a.ring_odd + ring, 1u);
+        if (lo != 0xffffffffu) atomicMin(a.ring_first + ring, lo);
+        if (hi) atomicMax(a.ring_last + ring, hi);
+        if (last_odd) atomicMax(a.ring_odd + ring, last_odd);
     }
 }
 
@@ -117,28 +169,44 @@ __global__ void __launch_bounds__(DP_THREADS) k_device_paths_rings(DpArgs a) {
     const uint32_t r = blockIdx.x * DP_THREADS + threadIdx.x;
     if (r >= a.n_rings || dp_failed(a)) return;
     const uint32_t b0 = (uint32_t)__ldg(a.ring_offsets + r), b1 = (uint32_t)__ldg(a.ring_offsets + r + 1u);
-    uint32_t first = a.ring_first[r], last = a.ring_last[r], code = 0u;
-    if (a.ring_odd[r]) { // the encoders' walk: a point is kept when it differs from the last kept point
-        code |= DP_WALKED;
-        first = 0xffffffffu;
-        float2 at = dp_point(a, b0);
-        for (uint32_t j = b0 + 1u; j < b1; j++) {
-            const float2 p = dp_point(a, j);
-            const bool k = dp_neq(p, at);
-            a.keep_fix[j] = k ? 1u : 0u;
-            if (k) {
-                if (first == 0xffffffffu) first = j;
-                last = j;
-                at = p;
-            }
-        }
-    }
+    const uint32_t first = a.ring_first[r];
+    uint32_t last = a.ring_last[r], code = 0u;
     float2 ste = make_float2(0.0f, 0.0f);
     if (first != 0xffffffffu) {
         code |= DP_KEPT;
-        const float2 p0 = dp_point(a, b0), pf = dp_point(a, first), pl = dp_point(a, last);
+        if (a.ring_odd[r] > first) { // the encoders' walk after the first kept segment: the span against the last kept end
+            code |= DP_WALKED;
+            last = first;
+            float2 at = dp_point(a, first);
+            for (uint32_t e = first + 1u; e < b1; e++) {
+                if (dp_kind(a, e) != 0u) continue;
+                const float2 pe = dp_point(a, e);
+                const bool k = dp_span_keeps(a, at, e - dp_degree(a, b0, e), e, pe);
+                a.keep_fix[e] = k ? 1u : 0u;
+                if (k) {
+                    last = e;
+                    at = pe;
+                }
+            }
+        } else if (last < first) {
+            last = first;
+        }
+        // the start tangent's end, from the first kept segment (start_tangent_for_line / _quad / _curve)
+        const uint32_t d = dp_degree(a, b0, first);
+        const float2 p0 = dp_point(a, b0), pe = dp_point(a, first), pl = dp_point(a, last);
         const float third = __fdiv_rn(1.0f, 3.0f);
-        ste = make_float2(__fadd_rn(p0.x, __fmul_rn(third, __fsub_rn(pf.x, p0.x))), __fadd_rn(p0.y, __fmul_rn(third, __fsub_rn(pf.y, p0.y))));
+        auto toward = [&](float2 from, float2 to) {
+            return make_float2(__fadd_rn(from.x, __fmul_rn(third, __fsub_rn(to.x, from.x))), __fadd_rn(from.y, __fmul_rn(third, __fsub_rn(to.y, from.y))));
+        };
+        if (d == 1u) {
+            ste = toward(p0, pe);
+        } else if (d == 2u) {
+            const float2 c = dp_point(a, first - 1u);
+            ste = dp_neq(c, p0) ? toward(c, p0) : toward(c, pe);
+        } else {
+            const float2 c1 = dp_point(a, first - 2u), c2 = dp_point(a, first - 1u);
+            ste = dp_neq(c1, p0) ? c1 : (dp_neq(c2, p0) ? c2 : pe);
+        }
         const bool closes = a.kind == 0u || a.closed;
         if (closes && !dp_same_bits(pl, p0)) code |= DP_CLOSE;
         if (a.kind == 1u) {
@@ -172,10 +240,19 @@ __device__ __forceinline__ DpOut dp_out(const DpArgs &a, uint32_t j) {
         const uint32_t tail = code & (DP_CLOSE | DP_CAP_LINE | DP_CAP_QUAD);
         if (j == b0) {
             o.main = 1u;
-        } else if ((code & DP_WALKED) ? a.keep_fix[j] != 0u : dp_neq(o.p, dp_point(a, j - 1u))) {
-            o.main = 1u;
-            o.tag_bytes = DP_TAG_LINE | (j == rec.x && !tail ? DP_SUBPATH_END : 0u);
-            o.tags = 1u;
+        } else {
+            // the segment of point j: kept when it is the first kept one, or after it and kept by the span test
+            const uint32_t e = dp_seg_end(a, j, b1), first = a.ring_first[r], d = dp_degree(a, b0, e);
+            bool keep = e == first;
+            if (e > first)
+                keep = (code & DP_WALKED) ? a.keep_fix[e] != 0u : dp_span_keeps(a, dp_point(a, e - d), e - d, e, e == j ? o.p : dp_point(a, e));
+            if (keep) {
+                o.main = 1u;
+                if (j == e) {
+                    o.tag_bytes = (DP_TAG_LINE + d - 1u) | (j == rec.x && !tail ? DP_SUBPATH_END : 0u);
+                    o.tags = 1u;
+                }
+            }
         }
         o.words = 2u * o.main;
         if (j == b1 - 1u && tail) {
@@ -201,7 +278,8 @@ __device__ __forceinline__ DpOut dp_out(const DpArgs &a, uint32_t j) {
     }
     return o;
 }
-// one point's counts packed for the block scan: tags (<= 4 a point) in bits 0..10, words (<= 6) in 11..21, draws in 22..31
+// one point's counts packed for the block scan: tags (<= 4 a point: its segment's, the closing line, the cap marker, PATH) in
+// bits 0..10, words (<= 6: its own, then a closing line and a cap line, or a cap quad) in 11..21, draws in 22..31
 __device__ __forceinline__ uint32_t dp_pack(const DpOut &o) { return o.tags | (o.words << 11) | (o.draws << 22); }
 
 __global__ void __launch_bounds__(DP_THREADS) k_device_paths_count(DpArgs a) {

@@ -301,17 +301,19 @@ extern "C" int vb_fragment_free(vb_renderer *r, uint32_t fragment) {
     return VB_OK;
 }
 
-// ---- fragments from device arrays: vb_fragment_from_device_paths (k_device_paths.cu) -----------------------------------------
+// ---- fragments from device arrays: vb_fragment_from_device_paths / _curves (k_device_paths.cu) ------------------------------
 // The streams' lengths depend on the data (dropped points, closing lines, cap markers), so the fragment is allocated for the
 // worst case of the counts, the four launches write it, and the totals and the error word come back through pinned memory
 // after one synchronisation of the renderer's stream.
 static const uint32_t STROKE_JOINS[3] = {0u, 0x10000000u, 0x20000000u}, STROKE_CAPS[3] = {0u, 0x01000000u, 0x02000000u}; // path.rs:30-66
 static bool one_of(uint32_t v, const uint32_t (&set)[3]) { return v == set[0] || v == set[1] || v == set[2]; }
 
-extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_paths *d, uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
+// vb_fragment_from_device_paths (kinds NULL: every point on-curve) and vb_fragment_from_device_curves; `fn` names the call.
+static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d, const uint8_t *kinds, uint32_t *fragment_out,
+                       uint32_t *n_draw_objects_out) {
     if (!r) return VB_E_INVALID;
     auto bad = [&](const std::string &why) {
-        r->err = "vb_fragment_from_device_paths: " + why;
+        r->err = std::string(fn) + ": " + why;
         return VB_E_INVALID;
     };
     if (!d || !fragment_out) return bad("NULL paths or id");
@@ -350,6 +352,7 @@ extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_pat
     for (const void *p : ptrs)
         if (p && ((uintptr_t)p % 4u || !device_memory_of(r, p)))
             return bad("every array must be 4-byte aligned device or managed memory of the renderer's device");
+    if (kinds && d->n_points && !device_memory_of(r, kinds)) return bad("point_kinds must be device or managed memory of the renderer's device");
     reap_freed(r);
 
     // the scratch (DpArgs): [err, ring_first] set to all ones, [totals, ring_last, ring_odd, path_kept, the look-back's leading
@@ -365,13 +368,14 @@ extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_pat
     std::unique_ptr<Fragment> f(new Fragment());
     const cudaError_t ce = cudaMalloc(&f->mem, bytes);
     if (ce != cudaSuccess) {
-        r->err = std::string("vb_fragment_from_device_paths: cudaMalloc: ") + cudaGetErrorString(ce);
+        r->err = std::string(fn) + ": cudaMalloc: " + cudaGetErrorString(ce);
         return VB_E_CUDA;
     }
     f->bytes = bytes;
     DpArgs a;
     memset(&a, 0, sizeof a);
     a.points = d->points;
+    a.kinds = d->n_points ? kinds : nullptr;
     a.ring_offsets = d->ring_offsets;
     a.path_offsets = d->path_offsets;
     a.colors = d->colors;
@@ -409,7 +413,7 @@ extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_pat
     if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(h + 8u, t + o_zero, 12u, cudaMemcpyDeviceToHost, st);
     if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(st);
     if (e2 != cudaSuccess) {
-        r->err = std::string("vb_fragment_from_device_paths: ") + cudaGetErrorString(e2);
+        r->err = std::string(fn) + ": " + cudaGetErrorString(e2);
         return fail(VB_E_CUDA);
     }
     unsigned long long err;
@@ -424,12 +428,22 @@ extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_pat
         if (kind == VB_DP_ERR_RING_OFFSETS) return bad("ring_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_points");
         if (kind == VB_DP_ERR_PATH_OFFSETS) return bad("path_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_rings");
         if (kind == VB_DP_ERR_POINTS) return bad("point " + at + " is not finite");
+        if (kind == VB_DP_ERR_KINDS)
+            return bad("point_kinds[" + at + "] breaks the kinds: each is 0 (on-curve) or 1 (off-curve), a ring starts and ends on-curve, "
+                       "and at most two off-curve points come in a row");
         return bad("the colour of path " + at + " is not finite");
     }
     const uint64_t units[CMP_STREAMS] = {N ? 2u + tot[0] : 0u, tot[1], tot[2], tot[2], N ? 1u : 0u, N ? 2u : 0u};
     *fragment_out = fragment_register(r, std::move(f), units, tot[2], 0u, 0u, tot[2]); // FILL_COLOR has one info word
     if (n_draw_objects_out) *n_draw_objects_out = tot[2];
     return VB_OK;
+}
+extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_paths *d, uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
+    return from_device(r, "vb_fragment_from_device_paths", d, nullptr, fragment_out, n_draw_objects_out);
+}
+extern "C" int vb_fragment_from_device_curves(vb_renderer *r, const vb_device_paths *d, const uint8_t *point_kinds, uint32_t *fragment_out,
+                                              uint32_t *n_draw_objects_out) {
+    return from_device(r, "vb_fragment_from_device_curves", d, point_kinds, fragment_out, n_draw_objects_out);
 }
 
 

@@ -247,18 +247,21 @@ uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
 // A fragment's allocation starts with CMP_HEADER_WORDS words: the word offset of each of its six streams, then two zeros.
 #define CMP_HEADER_WORDS 8u
 
-// k_device_paths.cu: a fragment built from device arrays (vb_fragment_from_device_paths). The caller's arrays, the style, the
-// scratch the four launches share and the fragment they write. The scratch: per ring its first and last kept point (set to
-// all ones and zero), a flag for a ring the encoders' walk must decide (zero), its record {last kept point, code, start tangent
-// end}; a keep byte per point of a walked ring; a kept flag per path (zero); the error (all ones until a check fails: (kind
-// << 32) | first row); the look-back (vb_lookback_words(n_parts, 3), its leading words zero); each partition's exclusive
-// prefix (3 words); the totals of tag bytes, path-data words and draw objects (zero), which the caller reads back.
+// k_device_paths.cu: a fragment built from device arrays (vb_fragment_from_device_paths, vb_fragment_from_device_curves). The
+// caller's arrays, the style, the scratch the four launches share and the fragment they write. The scratch: per ring the end
+// point of its first kept segment and the last end point kept by the span test (set to all ones and zero), the last end point
+// of a dropped segment that may need the encoders' walk (zero), its record {last kept end point, code, start tangent end}; a
+// keep byte per end point of a walked ring; a kept flag per path (zero); the error (all ones until a check fails: (kind << 32)
+// | first row); the look-back (vb_lookback_words(n_parts, 3), its leading words zero); each partition's exclusive prefix (3
+// words); the totals of tag bytes, path-data words and draw objects (zero), which the caller reads back.
 #define VB_DP_ERR_RING_OFFSETS 1u
 #define VB_DP_ERR_PATH_OFFSETS 2u
 #define VB_DP_ERR_POINTS 3u
 #define VB_DP_ERR_COLOR 4u
+#define VB_DP_ERR_KINDS 5u // a kind other than 0 or 1; an off-curve point first or last in its ring, or third in a row
 struct DpArgs {
     const float *points;
+    const uint8_t *kinds; // null: every point on-curve
     const int32_t *ring_offsets, *path_offsets; // path_offsets null: one ring per path
     const float *colors;
     size_t point_pitch, color_pitch; // bytes

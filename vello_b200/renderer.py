@@ -178,6 +178,7 @@ def load_library() -> C.CDLL:
     lib.vb_fragment_upload.argtypes = [vp, C.POINTER(_EncodingStreams), C.POINTER(C.c_uint32)]
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_fragment_from_device_paths.argtypes = [vp, C.POINTER(_DevicePaths), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    lib.vb_fragment_from_device_curves.argtypes = [vp, C.POINTER(_DevicePaths), vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_recompose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_debug_match_instances.argtypes = [vp, C.c_uint32, vp, C.c_uint32, vp]
@@ -214,7 +215,7 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
                     "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths", "vb_bind_draw_opacity",
-                    "vb_fragment_from_device_paths"]
+                    "vb_fragment_from_device_paths", "vb_fragment_from_device_curves"]
 
 
 def _device_rows(t, who: str, what: str, cols: int, vector: bool = False, empty: bool = False):
@@ -277,6 +278,23 @@ def _device_flags(t, who: str):
     if pitch <= 0:
         raise ValueError(f"{who}: rows a positive number of bytes apart, not strides {tuple(strides)}")
     return C.c_void_p(int(cai["data"][0])), shape[0], pitch
+
+
+def _device_kinds(t, n_points: int, who: str):
+    """The pointer of `point_kinds`: a contiguous 1-D uint8 or bool device array of `n_points` entries, from its
+    `__cuda_array_interface__` (0 on-curve, 1 off-curve; True is 1)."""
+    cai = getattr(t, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{who}: {type(t).__name__} has no __cuda_array_interface__: device point_kinds are needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 1 or cai["typestr"] not in ("|b1", "|u1", "<u1", ">u1"):
+        raise ValueError(f"{who}: point_kinds must be a 1-D uint8 or bool array, not {shape} {cai['typestr']}")
+    if shape[0] != n_points:
+        raise ValueError(f"{who}: point_kinds has {shape[0]} entries for {n_points} points")
+    strides = cai.get("strides")
+    if strides is not None and shape[0] > 1 and tuple(strides) != (1,):
+        raise ValueError(f"{who}: point_kinds must be contiguous, not strides {tuple(strides)}")
+    return C.c_void_p(int(cai["data"][0])) if shape[0] else None
 
 
 def _device_image(t, typestr="|u1"):
@@ -540,7 +558,7 @@ class Renderer:
         return int(copy.ctypes.data)
 
     def upload_device_paths(self, points, ring_offsets, colors, *, path_offsets=None, style=0, closed: bool = True,
-                            draw_index=None):
+                            draw_index=None, point_kinds=None):
         """Build a fragment on the device from ragged device arrays (`vb_fragment_from_device_paths`) and return (fragment id,
         draw objects). `points` is float32 (P, 2) x y rows, `ring_offsets` int32 (R + 1,): ring r is points ring_offsets[r] ..
         ring_offsets[r + 1] - 1; `path_offsets` int32 (N + 1,) over rings (None: each ring is a path); `colors` float32 (N, 4)
@@ -550,8 +568,11 @@ class Renderer:
         The fragment is word for word `upload_fragment` of a Scene that fills (or strokes) each path i with Color(colors[i]) under
         the identity, its shape being, per ring, a move to the first point, lines to the others and, when closed, a close.
         `draw_index` (optional, int32 (N,) device array) receives each path's draw object in the fragment, or -1 for a path that
-        encodes nothing. Write the arrays on `self.stream` (or synchronise) before the call; it returns once the fragment is
-        built."""
+        encodes nothing. `point_kinds` (optional, uint8 or bool (P,) device array) makes the paths curved
+        (`vb_fragment_from_device_curves`): 0 marks an on-curve point, 1 an off-curve one, and each on-curve point after a ring's
+        first ends a segment chosen by the off-curve points in front of it: none a line, one a quad, two a cubic. A ring starts
+        and ends on-curve; a curved closing segment ends on a repeat of the first point. None makes every point on-curve. Write
+        the arrays on `self.stream` (or synchronise) before the call; it returns once the fragment is built."""
         from .encoding import Stroke
         who = "upload_device_paths"
         pts, n_pts, pitch = _device_rows(points, who, "points", 2, empty=True)
@@ -564,6 +585,7 @@ class Renderer:
         cols, n_cols, cpitch = _device_rows(colors, who, "colours", 4, empty=True)
         if n_cols != n_poff - 1:
             raise ValueError(f"{who}: {n_cols} colours for {n_poff - 1} paths")
+        kinds = None if point_kinds is None else _device_kinds(point_kinds, n_pts, who)
         d = _DevicePaths(pts, n_pts, pitch, rings, n_roff - 1, paths, n_poff - 1, cols, cpitch)
         if isinstance(style, Stroke):
             if style.dash_pattern:
@@ -578,8 +600,12 @@ class Renderer:
                 raise ValueError(f"{who}: draw_index has {n_idx} entries for {n_poff - 1} paths")
             d.draw_index = idx
         fid, n_draws = C.c_uint32(0), C.c_uint32(0)
-        self._check(self.lib.vb_fragment_from_device_paths(self.handle, C.byref(d), C.byref(fid), C.byref(n_draws)),
-                    "vb_fragment_from_device_paths")
+        if point_kinds is None:
+            self._check(self.lib.vb_fragment_from_device_paths(self.handle, C.byref(d), C.byref(fid), C.byref(n_draws)),
+                        "vb_fragment_from_device_paths")
+        else:
+            self._check(self.lib.vb_fragment_from_device_curves(self.handle, C.byref(d), kinds, C.byref(fid), C.byref(n_draws)),
+                        "vb_fragment_from_device_curves")
         return int(fid.value), int(n_draws.value)
 
     def free_fragment(self, fragment: int):
