@@ -873,16 +873,16 @@ int vb_bind_stroke_widths(vb_renderer *, const float *device_widths, uint32_t n,
  *    order of a tile's segments makes in its area sums. Opacity changes no geometry, so hit tests and hit maps answer as
  *    unbound, even at row 0 (hiding is vb_bind_draw_visibility's job).
  *  - How. The frame reads its draw data from the region past the scene's streams that bound colours and stops write
- *    (vb_debug_download("draw_data")): at the start of flatten's stage a kernel copies the scene's draw data there, bound
- *    colours applied, and another one writes the bound alpha, blend and sample words into it. A vb_run_stages range that
- *    starts at draw writes them again.
+ *    (vb_debug_download("draw_data")): at the start of flatten's stage one kernel writes the scene's draw data there, with the
+ *    bound colour, ramp, alpha, blend and sample words in place of the encoded ones. A vb_run_stages range that starts at draw
+ *    writes it again.
  *  - When rows are read. A frame reads the rows when it runs on vb_stream, at the start of flatten's stage. The caller orders its
  *    writes before the frame, on vb_stream or with a synchronisation, and does not write the rows while a frame that reads
  *    them is running. A blocking frame that is re-run after an arena overflow reads the rows again; an enqueued frame is never
  *    re-run. The caller keeps the memory alive while it is bound. Changing only the contents replays the captured frame graph.
  *    Binding, unbinding, or binding another pointer, n or pitch changes the frame's key, so the next frame captures its graph
  *    anew. With nothing bound a frame launches, configures and captures exactly what it would without this call; bound, it
- *    launches one kernel more, and one more again when neither colours nor stops are bound (the draw-data copy).
+ *    launches one kernel more (the draw-data pass) when neither colours nor stops are bound, and none more when they are.
  *  - Scope. Any installed scene can be bound, packed bytes included. Every scene installation unbinds: every upload form,
  *    vb_render, vb_render_begin, vb_compose and vb_recompose. The binding survives vb_set_view, vb_set_cells, the seven other
  *    bindings and hit tests; all eight can be active together. device_alpha NULL unbinds.
@@ -891,8 +891,8 @@ int vb_bind_stroke_widths(vb_renderer *, const float *device_widths, uint32_t n,
  * VB_E_INVALID (vb_last_error says why), with any previous binding left as it was: no scene installed; n = 0 with a non-NULL
  * pointer, or n above the scene's draw-object count; a pointer that is not device memory of the renderer's device (or managed
  * memory), or not 4-byte aligned; a pitch that is not a multiple of 4, below 4, or 4 GiB or more; a renderer of a vb_group or
- * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose draw data passes 2^30
- * words, or whose regions past its streams would pass 32-bit word offsets. */
+ * with the exchange configured; a call between vb_render_enqueue and vb_frame_finish; a scene whose regions past its streams
+ * would pass 32-bit word offsets. */
 int vb_bind_draw_opacity(vb_renderer *, const float *device_alpha, uint32_t n, size_t row_pitch_bytes);
 
 /* ---- damage tracking: repaint only the tiles that changed since the last frame in the same destination (an addition; vello

@@ -46,6 +46,12 @@ BUDGETS = [
     Budget("k_flatten.o", "k_flatten_emit", 1, regs=(4, 256), smem=4),
     Budget("k_compose.o", "k_compose_streams", 1),
     Budget("k_compose.o", "k_instance_transforms", 1),
+    # the bound draw data's per-frame pass and bind-time slot walk (k_colors.cu); the device resolve and the bound ramps
+    Budget("k_colors.o", "k_draw_data", 1),
+    Budget("k_colors.o", "k_draw_data_slots", 1),
+    Budget("k_resolve.o", "k_resolve_finish", 1),
+    Budget("k_resolve.o", "k_make_ramps", 1),
+    Budget("k_resolve.o", "k_bound_ramps", 1),
     Budget("k_damage.o", "k_damage*", 5),
     Budget("k_recompose.o", "k_recompose_damage", 1),
     Budget("k_upload_diff.o", "k_upload_*", 3),

@@ -1,6 +1,6 @@
-"""Bound draw colours without a GPU: the conversion the tests hold k_draw_colors to is the encoder's, Renderer.bind_draw_colors
-refuses what the library would refuse before calling it, and the compiled kernels keep their conversion and their data in
-registers."""
+"""Bound draw colours without a GPU: the conversion the tests hold k_draw_data to is the encoder's, Renderer.bind_draw_colors
+refuses what the library would refuse before calling it, and the compiled kernel rounds each step of its conversions on its
+own (its registers: test_compiled_kernels.py)."""
 import os
 import re
 import shutil
@@ -143,21 +143,13 @@ def built():
 
 
 @needs_cuobjdump
-def test_colour_kernels_stay_in_registers(built):
-    res = subprocess.run(["cuobjdump", "-res-usage", os.path.join(built, "k_colors.o")], capture_output=True, text=True, check=True).stdout
-    fns = dict((fn, (int(st), int(loc))) for fn, st, loc in re.findall(r"Function (\S+):\s*\n\s*REG:\d+ STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", res))
-    names = sorted(re.match(r"_Z\d+(\w+?)P", fn).group(1) for fn in fns)
-    assert names == ["k_draw_color_slots", "k_draw_colors"], names
-    for fn, (stack, local) in fns.items():
-        assert stack == 0 and local == 0, f"{fn}: {stack} bytes of stack, {local} bytes of local memory"
-
-
-@needs_cuobjdump
-def test_conversion_has_no_fused_multiply_add(built):
+def test_draw_data_conversions_have_no_fused_multiply_add(built):
     sass = subprocess.run(["cuobjdump", "-sass", os.path.join(built, "k_colors.o")], capture_output=True, text=True, check=True).stdout
-    body = sass[sass.index("Function : _Z13k_draw_colors"):]
+    body = sass[sass.index("Function : _Z11k_draw_data"):]
     body = body[:body.index("..........")] if ".........." in body else body
     ops = re.findall(r"/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9.]+)", body)
-    # three premultiplications and four scalings by 255, each its own rounding
-    assert ops.count("FRND.FLOOR") == 4 and ops.count("FMUL") == 7 and ops.count("FADD") == 4, ops
+    # a colour: three premultiplications and four scalings by 255, each its own rounding, floored and truncated per byte; an
+    # image's alpha byte (bound opacity): one scaling by 255 and one + 0.5, each its own rounding, then a truncation
+    assert ops.count("FRND.FLOOR") == 4 and ops.count("FMUL") == 8 and ops.count("FADD") == 5, ops
+    assert sum(op.startswith("F2I") for op in ops) == 5, ops
     assert not any(op.startswith(("FFMA", "HFMA", "DFMA")) for op in ops), "the conversion contracts a multiply and an add"

@@ -217,7 +217,7 @@ def test_updates_on_the_stream_replay_the_graph(rr):
         if caps is None:
             caps = r.debug_graph_captures()
         assert r.debug_graph_captures() == caps, f"frame {j} captured a graph"
-        # the draw-data region (k_draw_colors) and the rows (k_bound_ramps)
+        # the draw-data region (k_draw_data) and the rows (k_bound_ramps)
         assert st.kernel_launches == unbound + 2
         ref.upload_scene(substituted(s, seq[j]))
         assert (r.download_target(p) == frame(ref)[0]).all(), f"frame {j}"

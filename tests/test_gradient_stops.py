@@ -201,16 +201,6 @@ def _functions(sass):
 
 
 @needs_cuobjdump
-def test_stop_kernels_stay_in_registers(built):
-    res = subprocess.run(["cuobjdump", "-res-usage", os.path.join(built, "k_resolve.o")], capture_output=True, text=True, check=True).stdout
-    fns = dict((fn, (int(st), int(loc))) for fn, st, loc in re.findall(r"Function (\S+):\s*\n\s*REG:\d+ STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", res))
-    names = sorted(re.match(r"_Z\d+(\w+?)P", fn).group(1) for fn in fns)
-    assert names == ["k_bound_ramps", "k_gradient_slots", "k_make_ramps", "k_resolve_finish"], names
-    for fn, (stack, local) in fns.items():
-        assert stack == 0 and local == 0, f"{fn}: {stack} bytes of stack, {local} bytes of local memory"
-
-
-@needs_cuobjdump
 def test_bound_ramps_run_the_resolves_arithmetic(built):
     """k_bound_ramps and k_make_ramps share one walk: the same floating-point operations, and the only FFMAs are those of the
     correctly rounded divisions (u = i / 511 and 1 / alpha), which the compiler expands the same way in both."""

@@ -1,11 +1,7 @@
 """Bound opacity without a GPU (Renderer.bind_draw_opacity): the Python row checks, with a stub `__cuda_array_interface__` and
-a stub library; a float32 restatement of what k_draw_opacity writes, tied to both scene front ends at every rounding edge of
-the image alpha byte; the re-encoded scene the GPU tests (test_gpu_opacity.py) compare with; and the compiled kernels."""
-import os
-import re
-import shutil
-import subprocess
-
+a stub library; a float32 restatement of the words bound opacity writes into the frame's draw data (k_draw_data), tied to
+both scene front ends at every rounding edge of the image alpha byte; and the re-encoded scene the GPU tests
+(test_gpu_opacity.py) compare with. The compiled kernel is checked in test_compiled_kernels.py and test_draw_colors.py."""
 import numpy as np
 import pytest
 
@@ -18,8 +14,6 @@ from vello_b200.shapes import Affine, Circle, Rect, RoundedRect
 
 from .test_visibility import _Cai, _NoLib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BUILD = os.path.join(ROOT, "vello_b200", "csrc", "build")
 f32 = np.float32
 NORMAL_SRC_OVER = (MIX_NORMAL << 8) | COMPOSE_SRC_OVER
 
@@ -37,8 +31,8 @@ def image_byte(a):
 
 
 def opacity_slots(packed):
-    """Per draw object, the restatement of k_draw_opacity_slots: (word, kind) with the word relative to the draw data that its
-    row replaces, kind "layer", "clip" or "image", or None for a draw object whose row is ignored."""
+    """Per draw object, where bound opacity writes (k_draw_data_slots): (word, kind) with the word relative to the draw data
+    that its row replaces, kind "layer", "clip" or "image", or None for a draw object whose row is ignored."""
     L = packed.layout
     scene = np.asarray(packed.scene, dtype=np.uint32)
     tags = scene[L.draw_tag_base:L.draw_tag_base + L.n_draw_objects]
@@ -382,35 +376,3 @@ def test_python_accepts_vectors_columns_and_strided_rows():
     assert got[-1] == (1 << 20, 6, 24)
     r.bind_draw_opacity(None)
     assert got[-1] == (None, 0, 0) and r._opacity is None
-
-
-# ---- the compiled kernels ----------------------------------------------------------------------------------------------------
-needs_cuobjdump = pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="CUDA binary utilities not installed")
-
-
-@pytest.fixture(scope="module")
-def built():
-    import __graft_entry__ as g
-    g.build()
-    return BUILD
-
-
-@needs_cuobjdump
-def test_opacity_kernels_stay_in_registers(built):
-    res = subprocess.run(["cuobjdump", "-res-usage", os.path.join(built, "k_opacity.o")], capture_output=True, text=True, check=True).stdout
-    fns = dict((fn, (int(st), int(loc))) for fn, st, loc in re.findall(r"Function (\S+):\s*\n\s*REG:\d+ STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", res))
-    names = sorted(re.match(r"_Z\d+(\w+?)P", fn).group(1) for fn in fns)
-    assert names == ["k_draw_opacity", "k_draw_opacity_slots"], names
-    for fn, (stack, local) in fns.items():
-        assert stack == 0 and local == 0, f"{fn}: {stack} bytes of stack, {local} bytes of local memory"
-
-
-@needs_cuobjdump
-def test_image_conversion_has_no_fused_multiply_add(built):
-    sass = subprocess.run(["cuobjdump", "-sass", os.path.join(built, "k_opacity.o")], capture_output=True, text=True, check=True).stdout
-    body = sass[sass.index("Function : _Z14k_draw_opacity"):]
-    body = body[:body.index("Function :", 1)] if "Function :" in body[1:] else body
-    ops = re.findall(r"/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9.]+)", body)
-    # one scaling by 255 and one + 0.5, each its own rounding, then a truncation
-    assert ops.count("FMUL") == 1 and ops.count("FADD") == 1 and any(op.startswith("F2I") for op in ops), ops
-    assert not any(op.startswith(("FFMA", "HFMA", "DFMA")) for op in ops), "the conversion contracts a multiply and an add"

@@ -7,7 +7,7 @@ frames/s and ms per frame (host wall time of --steps blocking frames after --war
                    uploaded again (vb_scene_upload), then the frame
   (d) bound_damage as (b), but 1 % of the rows changed per frame and damage tracking on into a device destination; also the
                    mean damaged tile count per frame
-and the device time of one k_draw_colors from torch.profiler (a separate pass). (b) and (c) check one frame's pixels against
+and the device time of one k_draw_data from torch.profiler (a separate pass). (b) and (c) check one frame's pixels against
 each other. With --out the result also goes to DIR/color_probe.json:
     python tools/color_probe.py [--steps 50] [--warmup 5] [--out DIR]"""
 import argparse
@@ -68,7 +68,7 @@ def kernel_us(r, t, all_rows, p, steps):
                 t.copy_(all_rows[s % all_rows.shape[0]])
             r.render_resident(p)
     for e in prof.key_averages():
-        if "k_draw_colors" in e.key:
+        if e.key.startswith("k_draw_data("):
             us = getattr(e, "device_time_total", None)
             if us is None:
                 us = getattr(e, "cuda_time_total", 0.0)
@@ -153,7 +153,7 @@ def main():
     tiles = ((size + 15) // 16) ** 2
     res["d_bound_damage"].update(rows_changed=m, damaged_tiles_mean=round(float(np.mean(damaged)), 1), tiles=tiles)
     r.set_damage_tracking(False)
-    res["k_draw_colors_us"] = kernel_us(r, t, all_rows, p, 20)
+    res["k_draw_data_us"] = kernel_us(r, t, all_rows, p, 20)
     r.close()
     res["card_after"] = card()
     print(json.dumps(res, indent=1))

@@ -7,7 +7,8 @@ the card, its power limit and SM clock, frames/s and ms per frame of four routes
   host      the host route for the rows of 0.5: re-encoding the scene (Python encoder and resolve), uploading it and its frame,
             each timed alone, and their sum as the cost of one frame; and the pixels of the last bound frame against the
             re-encoded scene's (must be equal)
-and the device time of k_draw_opacity and of the draw-data copy (k_draw_colors) per frame (torch.profiler, in a run of its own).
+and the device time per frame of k_draw_data, which writes the frame's draw data with the bound words (torch.profiler, in a
+run of its own).
 With --out the result also goes to DIR/opacity_probe.json:
     python tools/opacity_probe.py [--steps 30] [--warmup 5] [--out DIR]"""
 import argparse
@@ -144,7 +145,7 @@ def main():
             t.copy_(rows[s % 2])
         r.render_resident(p)
 
-    res["kernel_us"] = kernel_us(bound05, a.steps, ["k_draw_opacity", "k_draw_colors"])
+    res["kernel_us"] = kernel_us(bound05, a.steps, ["k_draw_data"])
     for k in ("unbound", "bound_1", "bound_05", "host"):
         print(f"{k:9s} {res[k]['fps']:9.2f} frames/s {res[k]['ms_per_frame']:9.3f} ms/frame", flush=True)
     print(f"host route: encode+resolve {encode_ms:.0f} ms, upload {res['host']['upload_ms']:.3f} ms, frame "

@@ -8,7 +8,7 @@ ending in a synchronise) of:
                    installed again (vb_scene_upload_streams, which resolves and makes the ramps on the device), then the frame
   (d) bound_damage as (b), but the stops of 1 % of the gradients changed per frame and damage tracking on into a device
                    destination; also the mean damaged tile count per frame
-and the device time of one k_bound_ramps from torch.profiler (a separate pass). (b) and (c) check one frame's pixels against
+and the device time of one k_bound_ramps and one k_draw_data from torch.profiler (a separate pass). (b) and (c) check one frame's pixels against
 each other. With --out the result also goes to DIR/stops_probe.json:
     python tools/stops_probe.py [--steps 50] [--warmup 5] [--out DIR]"""
 import argparse
@@ -67,8 +67,8 @@ def kernel_us(r, t, all_rows, p, steps):
             r.render_resident(p)
     out = {}
     for e in prof.key_averages():
-        for name in ("k_bound_ramps", "k_draw_colors"):
-            if name in e.key:
+        for name in ("k_bound_ramps", "k_draw_data"):
+            if e.key.startswith(name + "("):
                 us = getattr(e, "device_time_total", None)
                 if us is None:
                     us = getattr(e, "cuda_time_total", 0.0)

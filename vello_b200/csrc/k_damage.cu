@@ -24,8 +24,8 @@
 //     flatten used: its snapshot entry, or for an entry of 0 its style's width word) differs bit for bit from the last successful
 //     frame's, its tile box in that frame and in this one. A fill's entry is always 0 and its style word never changes, so its
 //     row is no change; neither is a row that falls back to an unchanged encoded width. A wider stroke's new box holds it
-//   + with bound opacity (vb_bind_draw_opacity), for every draw object below the bound count whose opacity word (the one the
-//     frame's draw data holds after k_draw_opacity: a layer's alpha word, an image's sample word) differs bit for bit from the
+//   + with bound opacity (vb_bind_draw_opacity), for every draw object below the bound count whose opacity word (the one
+//     coarse and fine read from the frame's draw data: a layer's alpha word, an image's sample word) differs bit for bit from the
 //     last successful frame's, its tile box in that frame and in this one. A clip layer's blend word follows from its alpha, and
 //     a layer is covered by its BEGIN_CLIP's box, which holds everything inside the layer and the pixels its blend touches.
 //     Other draw objects have no opacity word, so their rows are no change.
@@ -66,8 +66,8 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_begin(uint8_t *mask, cons
 // The inputs of k_damage_mark and k_damage: the snapshot `snap`, laid out by L (its flag arrays: L.changed, L.paths, L.xf), the
 // frame's mask, the words the frame reads and the bindings' tables (VbBound). The mask words `vis` are null without bound
 // visibility, `grad` (VbBound::rs_draw) without a bound gradient, `xf_range` without bound transforms, the stroke-width
-// snapshot `widths` without bound widths (`styles`: the scene's n_style style words, `path_draw`: pathtag's path table), and
-// `op_slots` (VbBound::op_slots) without bound opacity.
+// snapshot `widths` without bound widths (`styles`: the scene's n_style style words, `path_draw`: pathtag's path table). The
+// frame's draw data `dd` has n_dd words.
 struct DmArgs {
     VbDmgLayout L;
     uint32_t *snap;
@@ -79,8 +79,8 @@ struct DmArgs {
     const uint2 *xf_range;
     const float *widths;
     const uint2 *path_draw;
-    const uint32_t *styles, *op_slots;
-    uint32_t compare, wt, ht, n_style;
+    const uint32_t *styles;
+    uint32_t compare, wt, ht, n_style, n_dd;
 };
 
 // One thread per transform u of the frame: its six words against the snapshot, and into the next slot. A difference marks
@@ -136,7 +136,8 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage_mark(const DmArgs a) {
 // reads transforms xf_range[d].x .. .y, each flagged with transforms bound) changed, its old and new boxes into the mask. A draw
 // object whose paint is not one colour has colour word 0: its bound row is never read. Its colour word is at its draw monoid's
 // offset in the frame's draw data (`dd`, the bound region). Below L.n_wid, its stroke width: the snapshot entry, or for 0 the
-// width word of its path's style (path d is draw object d). Below L.n_op, its opacity word in `dd` (`op_slots`), or 0.
+// width word of its path's style (path d is draw object d). Below L.n_op, its opacity word in `dd` (a BEGIN_CLIP's alpha word
+// right after its draw monoid's offset, an image's sample word two after it), or 0 for any other draw object.
 __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
     const VbDmgLayout &L = a.L;
     const uint32_t d = blockIdx.x * (DM_THREADS / 32u) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
@@ -165,8 +166,10 @@ __global__ void __launch_bounds__(DM_THREADS) k_damage(const DmArgs a) {
         if (lane == 0u) nxt[L.wid + d] = w;
     }
     if (d < L.n_op) {
-        const uint32_t e = __ldg(a.op_slots + d);
-        const uint32_t w = e == VB_COLOR_NONE ? 0u : __ldg(a.dd + (e >> 2));
+        const uint32_t tag = __ldg(a.draw_tags + d);
+        const uint32_t at = tag == VB_DRAWTAG_BEGIN_CLIP ? 1u : tag == VB_DRAWTAG_FILL_IMAGE ? 2u : 0u;
+        const uint32_t o = __ldg(&a.draw_monoids[d].scene_offset) + at;
+        const uint32_t w = at && o < a.n_dd ? __ldg(a.dd + o) : 0u;
         hit = w != old[L.op + d] || hit;
         if (lane == 0u) nxt[L.op + d] = w;
     }
@@ -247,7 +250,7 @@ extern "C" uint32_t vb_launch_damage(const VbConfig &cfg, const VbFrameBufs &b, 
     a.xf_range = B.rows[VB_BIND_TRANSFORMS].rows ? B.xf_range : nullptr;
     a.widths = cfg.widths, a.path_draw = b.path_draw, a.styles = b.scene + cfg.layout.style_base;
     a.n_style = cfg.scene_words > cfg.layout.style_base ? cfg.scene_words - cfg.layout.style_base : 0u;
-    a.op_slots = B.op_slots;
+    a.n_dd = b.dd_len;
     uint32_t launches = 1u;
     const uint32_t n_mark = std::max(std::max(L.n_xf, n_paths ? L.n_pt : 0u), L.n_vis);
     if (n_mark) {

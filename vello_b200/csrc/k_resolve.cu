@@ -96,34 +96,8 @@ k_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t *out) {
 // ---- bound gradient stops (vb_bind_gradient_stops) ------------------------------------------------------------------------------
 // A bound gradient renders from a ramp row of its own: resolves share one row between gradients whose stops are equal, and
 // bound rows may part them. The binding gives bound gradient g row ramp0 + g of a renderer-owned copy of the scene's ramps,
-// and k_draw_colors writes that row into the gradient's ramp word in the frame's draw data (VB_GRAD_SLOT). No pipeline kernel
+// and k_draw_data (k_colors.cu) writes that row into the gradient's ramp word in the frame's draw data. No pipeline kernel
 // changes: fine reads the row as any other, bounded by cfg.n_ramps.
-
-// One CTA: the bound gradients' ramp words into the draw-data slot table, then a walk over every draw tag (the exclusive scan
-// of their draw-data sizes, as k_draw_color_slots has it) that finds the draw object each of those words belongs to.
-#define RS_SLOT_THREADS 1024u
-__global__ void __launch_bounds__(RS_SLOT_THREADS) k_gradient_slots(const uint32_t *__restrict__ tags, uint32_t n_draw, const uint32_t *__restrict__ dd,
-                                                                    uint32_t n_grads, uint32_t *slots, uint32_t n_words, uint32_t *draw_grad) {
-    __shared__ uint32_t sh[RS_SLOT_THREADS / 32u + 1u];
-    for (uint32_t g = threadIdx.x; g < n_grads; g += RS_SLOT_THREADS) {
-        const uint32_t w = __ldg(dd + g);
-        if (w < n_words) slots[w] = VB_GRAD_SLOT | g;
-    }
-    __syncthreads();
-    uint32_t base = 0u;
-    for (uint32_t c = 0u; c < n_draw; c += RS_SLOT_THREADS) {
-        const uint32_t k = c + threadIdx.x;
-        const uint32_t tag = k < n_draw ? __ldg(tags + k) : VB_DRAWTAG_NOP;
-        uint32_t total;
-        const uint32_t off = base + vb_block_excl_scan((tag >> 2) & 7u, sh, &total);
-        const bool gradient = tag == VB_DRAWTAG_FILL_LIN_GRADIENT || tag == VB_DRAWTAG_FILL_RAD_GRADIENT || tag == VB_DRAWTAG_FILL_SWEEP_GRADIENT;
-        if (gradient && off < n_words) {
-            const uint32_t s = slots[off];
-            if (s != VB_COLOR_NONE && (s & VB_GRAD_SLOT)) draw_grad[k] = s & ~VB_GRAD_SLOT;
-        }
-        base += total;
-    }
-}
 
 // One CTA per bound gradient, one thread per texel: its ramp row from its stops, stop k (global over the scene's ramp patches)
 // read from the caller's row when k < n_rows and all five values are finite, else as encoded.
@@ -153,12 +127,6 @@ extern "C" void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, 
 }
 extern "C" void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st) {
     if (n_ramps) k_make_ramps<<<n_ramps, RS_SAMPLES, 0, st>>>(ramps, stops, out);
-}
-extern "C" uint32_t vb_launch_gradient_slots(const uint32_t *tags, uint32_t n_draw, const uint32_t *dd, uint32_t n_grads, uint32_t *slots,
-                                             uint32_t n_words, uint32_t *draw_grad, cudaStream_t st) {
-    if (n_grads == 0u) return 0u;
-    k_gradient_slots<<<1, RS_SLOT_THREADS, 0, st>>>(tags, n_draw, dd, n_grads, slots, n_words, draw_grad);
-    return 1u;
 }
 extern "C" uint32_t vb_launch_bound_ramps(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st) {
     const VbRows &rows = b.bound.rows[VB_BIND_STOPS];

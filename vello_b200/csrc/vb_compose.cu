@@ -753,12 +753,6 @@ static std::string stops_check(const vb_renderer *r, uint32_t n) {
     if ((uint64_t)s.n_ramps + bound_grads(s, n) > (1ull << 30)) return "the scene's ramps and one per bound gradient pass the 30 bits of the ramp word";
     return draw_tags_outside(s, s.layout.n_draw_objects);
 }
-// bound opacity's table packs a draw-data word offset and a 2-bit kind into a word (VB_OP_ENTRY)
-static std::string opacity_check(const vb_renderer *r, uint32_t n) {
-    const Slot &s = *r->cur;
-    if (n_draw_data(s.layout, s.scene_words) >= (1u << 30)) return "the scene's draw data passes the 30 bits of the opacity table";
-    return draw_tags_outside(s, n);
-}
 static std::string no_check(const vb_renderer *, uint32_t) { return {}; }
 
 // The kinds' bind-time work: the tables of n rows in b. `why` is set for a refusal that only the work finds.
@@ -895,44 +889,28 @@ static int visibility_mask(vb_renderer *r, uint32_t, VbBound &, std::string &) {
 static int width_snapshot(vb_renderer *r, uint32_t, VbBound &, std::string &) {
     return compose_room(r, r->width_snap, (size_t)vb_width_entries(r->cur->layout) * 4u);
 }
-// Bound opacity (k_opacity.cu): the word each of the n bound draw objects patches, by one k_draw_opacity_slots over the scene's
-// draw tags and draw data. The call does not synchronise unless the table grows. The draw-data slot table follows (bind_rows).
-static int opacity_table(vb_renderer *r, uint32_t n, VbBound &b, std::string &) {
-    const Slot &slot = *r->cur;
-    const VbLayout &L = slot.layout;
-    int rc;
-    if ((rc = compose_room(r, r->op_slots, (size_t)n * 4u))) return rc;
-    uint32_t *table = (uint32_t *)r->op_slots.p;
-    const uint32_t *scene = (const uint32_t *)slot.scene.p;
-    vb_launch_draw_opacity_slots(scene + L.draw_tag_base, scene + L.draw_data_base, n, n_draw_data(L, slot.scene_words), table, r->stream);
-    CK(cudaGetLastError());
-    b.op_slots = table;
-    return VB_OK;
-}
 static int no_tables(vb_renderer *, uint32_t, VbBound &, std::string &) { return VB_OK; }
 
-// The draw-data slot table of bound colours and bound gradient stops (k_colors.cu), made from b whenever one of them or bound
-// opacity changes and one of the three stays bound: every word VB_COLOR_NONE, then one k_draw_color_slots over the first n_col
-// draw tags and one k_gradient_slots for the bound gradients, whose draw objects it writes to rs_draw. With opacity alone
-// every word stays VB_COLOR_NONE, so k_draw_colors copies the scene's draw data for k_draw_opacity to patch.
+// The draw-data slot table of bound colours, bound gradient stops and bound opacity (k_colors.cu), made from b whenever one
+// of them changes and one of them stays bound: every word VB_COLOR_NONE, then one k_draw_data_slots over the draw tags the
+// bound rows reach, which also writes the bound gradients' draw objects to rs_draw. The call does not synchronise unless the
+// table grows.
 static int draw_data_slots(vb_renderer *r, VbBound &b) {
-    b.col_slots = nullptr;
+    b.dd_slots = nullptr;
     if (!draw_data_bound(b)) return VB_OK;
     const Slot &slot = *r->cur;
     const VbLayout &L = slot.layout;
     const uint32_t n_dd = n_draw_data(L, slot.scene_words);
     int rc;
-    if ((rc = compose_room(r, r->color_slots, (size_t)n_dd * 4u))) return rc;
+    if ((rc = compose_room(r, r->dd_slots, (size_t)n_dd * 4u))) return rc;
     cudaStream_t st = r->stream;
-    uint32_t *slots = (uint32_t *)r->color_slots.p;
+    uint32_t *slots = (uint32_t *)r->dd_slots.p;
     if (n_dd) CK(cudaMemsetAsync(slots, 0xff, (size_t)n_dd * 4u, st));
-    const uint32_t *tags = (const uint32_t *)slot.scene.p + L.draw_tag_base;
-    const bool stops = b.rows[VB_BIND_STOPS].rows != nullptr;
-    vb_launch_draw_color_slots(tags, b.rows[VB_BIND_COLORS].n, slots, n_dd, st);
-    vb_launch_gradient_slots(tags, L.n_draw_objects, stops ? (const uint32_t *)r->stop_tables.p : nullptr, b.rs_grads_n, slots, n_dd,
-                             const_cast<uint32_t *>(b.rs_draw), st);
+    const uint32_t *scene = (const uint32_t *)slot.scene.p;
+    const uint32_t *grad_dd = b.rows[VB_BIND_STOPS].rows ? (const uint32_t *)r->stop_tables.p : nullptr;
+    vb_launch_draw_data_slots(b, scene + L.draw_tag_base, scene + L.draw_data_base, n_dd, L.n_draw_objects, grad_dd, slots, st);
     CK(cudaGetLastError());
-    b.col_slots = slots;
+    b.dd_slots = slots;
     return VB_OK;
 }
 
@@ -957,7 +935,7 @@ static const BindKind BIND_KINDS[VB_N_BINDINGS] = {
     {"vb_bind_transforms", false, any_scene, n_xforms, false, " transforms (1 .. n_transforms)", 24u, true, path_tags_outside, transform_tables},
     {"vb_bind_draw_visibility", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 1u, false, no_check, visibility_mask},
     {"vb_bind_stroke_widths", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, false, draw_tags_check, width_snapshot},
-    {"vb_bind_draw_opacity", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, true, opacity_check, opacity_table},
+    {"vb_bind_draw_opacity", false, any_scene, n_draws, false, " draw objects (1 .. n_draw_objects)", 4u, true, draw_tags_check, no_tables},
 };
 
 // Unbind `kind` in b: its rows and the tables only it reads
@@ -967,7 +945,6 @@ static void unbind(VbBound &b, int kind) {
     if (kind == VB_BIND_POINTS) b.pt_first = nullptr;
     if (kind == VB_BIND_STOPS) b.rs_grads = nullptr, b.rs_stops = nullptr, b.rs_draw = nullptr, b.rs_grads_n = b.rs_ramp0 = 0u;
     if (kind == VB_BIND_TRANSFORMS) b.xf_range = nullptr;
-    if (kind == VB_BIND_OPACITY) b.op_slots = nullptr;
 }
 
 // Bind n rows of `pitch` bytes from `ptr` as `kind` (null: unbind it), for every frame from now on

@@ -479,7 +479,7 @@ static int prepare(vb_renderer *r, const vb_params *p) {
     b.view = r->view.on ? (const float *)r->view_coef.p : nullptr;
     // the bindings, and what depends on where the scene lives now: the regions' sources and lengths, the bound gradients' ramps
     b.bound = B;
-    if (draw_data_bound(B)) b.col_src = b.scene + r->cur->layout.draw_data_base;
+    if (draw_data_bound(B)) b.dd_src = b.scene + r->cur->layout.draw_data_base;
     if (B.rows[VB_BIND_POINTS].rows) b.pt_src = b.scene + r->cur->layout.path_data_base;
     if (B.rows[VB_BIND_TRANSFORMS].rows) b.xf_src = b.scene + r->cur->layout.transform_base;
     if (B.rows[VB_BIND_STOPS].rows) b.ramps = (const uint32_t *)r->stop_ramps.p;
@@ -579,13 +579,11 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             // its streams in regions_of's order, the bound transforms before the viewed ones (their source; instances, then
             // transform rows), the draw data (read by draw, coarse and fine) and the path data (read by flatten alone); the bound
             // gradients' ramp rows (read by fine); the visibility mask and the stroke widths' snapshot (read by flatten and
-            // damage tracking). Bound opacity patches the draw data once it is written. Each launcher launches nothing while
-            // its binding is unbound.
+            // damage tracking). Each launcher launches nothing while its binding is unbound.
             launches += vb_launch_instance_transforms(c, b, st);
             launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on) launches += vb_launch_view_transforms(c, b, st);
-            launches += vb_launch_draw_colors(c, b, st);
-            launches += vb_launch_draw_opacity(c, b, st);
+            launches += vb_launch_draw_data(c, b, st);
             launches += vb_launch_bound_ramps(c, b, st);
             launches += vb_launch_path_points(c, b, st);
             launches += vb_launch_draw_visibility(c, b, st);
@@ -616,8 +614,7 @@ static int enqueue_direct(vb_renderer *r, int first, int last, const Dest &d, bo
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_instance_transforms(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_transforms(c, b, st);
             if (r->view.on && first == VB_STAGE_ID_DRAW) launches += vb_launch_view_transforms(c, b, st);
-            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_colors(c, b, st);
-            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_opacity(c, b, st);
+            if (first == VB_STAGE_ID_DRAW) launches += vb_launch_draw_data(c, b, st);
             if (first == VB_STAGE_ID_DRAW) launches += vb_launch_bound_ramps(c, b, st);
             if (r->xc.enabled) // second half of the exchange: my lines and the complete path boxes arrive before draw_leaf reads them
                 launches += vb_launch_exchange_recv(c, b, X, st);

@@ -319,16 +319,16 @@ struct vb_renderer {
     // vb_stages.h), which point into the buffers below. Every scene installation unbinds (set_scene).
     //  - inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n)] [the fragments'
     //    untransformed transforms] [the instances' draw prefix (n + 1)]
-    //  - color_slots: one word per draw-data word of the scene (VbBound::col_slots), while colours or stops are bound
+    //  - dd_slots: one word per draw-data word of the scene (VbBound::dd_slots, k_colors.cu), while colours, stops or opacity
+    //    are bound
     //  - point_slots: the first point of each path (layout.n_paths + 1 words), then the bind-time flag of a 16-bit segment
     //  - stop_tables: [each bound gradient's ramp word in the draw data] [the gradients (RsRamp)] [their encoded stops] [per
     //    draw object its gradient or VB_COLOR_NONE]; stop_ramps: the scene's ramps, then a row per bound gradient (k_resolve.cu)
     //  - xform_ranges: each path's transform range {t_lo, t_hi} (layout.n_paths uint2, k_points.cu)
     //  - vis_mask: the bit mask (vb_vis_words) each frame packs the visibility rows into (k_visibility.cu)
     //  - width_snap: the snapshot (vb_width_entries floats) each frame reads the stroke-width rows into (k_widths.cu)
-    //  - op_slots: one word per bound draw object, the draw-data word its opacity row replaces (VbBound::op_slots, k_opacity.cu)
     VbBound bound{};
-    DevBuf inst_tables, color_slots, point_slots, stop_tables, stop_ramps, xform_ranges, vis_mask, width_snap, op_slots;
+    DevBuf inst_tables, dd_slots, point_slots, stop_tables, stop_ramps, xform_ranges, vis_mask, width_snap;
 
     // damage tracking (vb_set_damage_tracking; k_damage.cu). `epoch` counts what makes the next frame a full one: a scene
     // installation, a binding or unbinding, vb_set_cells, a new view, switching tracking on. A frame is incremental when it
@@ -384,8 +384,8 @@ struct vb_renderer {
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
-                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->paths_tmp, &r->inst_tables, &r->color_slots, &r->point_slots,
-                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap, &r->op_slots,
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->paths_tmp, &r->inst_tables, &r->dd_slots, &r->point_slots,
+                           &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);
     for (DevBuf &b : r->fb) f(b);

@@ -40,12 +40,12 @@ struct VbBound {
     const uint32_t *inst_prefix;
     const CmpXform *inst_xf;
     const uint32_t *inst_src, *inst_draw;
-    // colours or stops (k_draw_colors): per draw-data word of the scene, the colour row whose conversion replaces it,
-    // VB_GRAD_SLOT | g for bound gradient g's ramp word, or VB_COLOR_NONE; null while neither is bound
-    const uint32_t *col_slots;
+    // colours, stops or opacity (k_draw_data): per draw-data word of the scene, the draw object whose binding replaces it, or
+    // VB_COLOR_NONE; null while none of them is bound
+    const uint32_t *dd_slots;
     // stops (k_bound_ramps): the bound gradients (rs_grads_n RsRamp records over the scene's stop indices), their encoded
-    // stops, and per draw object its bound gradient or VB_COLOR_NONE (k_damage). Gradient g's ramp row is ramps + (rs_ramp0 +
-    // g) * 512.
+    // stops, and per draw object its bound gradient or VB_COLOR_NONE (k_draw_data, k_damage). Gradient g's ramp row is ramps +
+    // (rs_ramp0 + g) * 512.
     const RsRamp *rs_grads;
     const RsStop *rs_stops;
     const uint32_t *rs_draw;
@@ -53,9 +53,6 @@ struct VbBound {
     const uint32_t *pt_first;
     // transforms: the range of transforms each path reads (layout.n_paths {t_lo, t_hi}; k_damage)
     const uint2 *xf_range;
-    // opacity (k_draw_opacity): per bound draw object the draw-data word its row replaces and its kind (VB_OP_ENTRY), or
-    // VB_COLOR_NONE
-    const uint32_t *op_slots;
     uint32_t rs_grads_n, rs_ramp0;
 };
 
@@ -93,7 +90,7 @@ struct VbFrameBufs {
     // what is bound to device rows (VbBound), and the scene's own words the bound regions are made from: its draw data, path
     // data and transforms (the bound transform region's source without bound instance transforms). Null while unbound.
     VbBound bound;
-    const uint32_t *col_src, *pt_src, *xf_src;
+    const uint32_t *dd_src, *pt_src, *xf_src;
     // fixed-size intermediates
     VbTagMonoid *tag_monoids;
     VbPathBbox *path_bboxes;
@@ -220,14 +217,9 @@ uint32_t vb_launch_hit_map(const VbConfig &cfg, const VbFrameBufs &b, uint32_t x
 void vb_launch_resolve_finish(uint32_t *scene, uint32_t n_tag_bytes, uint32_t n_open_clips, uint32_t padded_tag_bytes, uint32_t end_clip_word0,
                               const RsPatch *patches, uint32_t n_patches, cudaStream_t st);
 void vb_launch_make_ramps(const RsRamp *ramps, const RsStop *stops, uint32_t n_ramps, uint32_t *out, cudaStream_t st);
-// bound gradient stops (vb_bind_gradient_stops). The binding's tables, once at bind time: slots[dd[g]] = VB_GRAD_SLOT | g for
-// each of the n_grads bound gradients (dd: its ramp word, relative to the draw data), then from the scene's n_draw draw tags at
-// `tags`, draw_grad[k] = g for the gradient draw object k whose ramp word that is; the caller sets both tables to
-// VB_COLOR_NONE first. Per frame, in flatten's stage after the draw data (vb_frame.cu): each bound gradient's ramp row from its
-// stops, each read from the caller's row when it is bound and finite, else as encoded; nothing while unbound.
-#define VB_GRAD_SLOT 0x80000000u
-uint32_t vb_launch_gradient_slots(const uint32_t *tags, uint32_t n_draw, const uint32_t *dd, uint32_t n_grads, uint32_t *slots, uint32_t n_words,
-                                  uint32_t *draw_grad, cudaStream_t st);
+// bound gradient stops (vb_bind_gradient_stops). Per frame, in flatten's stage after the draw data (vb_frame.cu): each bound
+// gradient's ramp row from its stops, each read from the caller's row when it is bound and finite, else as encoded; nothing
+// while unbound. k_draw_data (k_colors.cu) points each bound gradient's ramp word at its row.
 uint32_t vb_launch_bound_ramps(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_compose.cu: the six streams of a composition of resident fragments (vb_compose), staged by vb_compose.cu
@@ -282,28 +274,18 @@ uint32_t vb_launch_device_paths(const DpArgs &a, cudaStream_t st);
 // vb_frame.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
-// k_colors.cu: bound draw colours (vb_bind_draw_colors). The binding's slot table, once at bind time: slots[w] = k for the colour
-// word w (relative to the draw data) of each draw object k < n whose paint is one colour (FILL_COLOR, BLURRED_ROUNDED_RECT),
-// from the scene's draw tags at `tags`; the caller sets the n_words words of the table to VB_COLOR_NONE first. Per frame, in
-// flatten's stage after the transforms (prepare reserved the region, vb_frame.cu): the scene's draw data into the frame's
-// region at layout.draw_data_base, each colour slot's word replaced by its row's premultiplied RGBA8 word and each gradient
-// slot's ramp id by its bound row (b.rs_ramp0 + g; VB_GRAD_SLOT, k_resolve.cu); nothing while neither is bound.
+// k_colors.cu: the bound draw data of bound colours (vb_bind_draw_colors), gradient stops (vb_bind_gradient_stops) and opacity
+// (vb_bind_draw_opacity). The bindings' slot table, once at bind time, from the scene's draw tags at `tags` and its n_words words
+// of draw data at `dd`: slots[w] = k for each draw-data word w that b's bindings replace, draw object k's colour, ramp, alpha,
+// clip-layer blend or image sample word; and b.rs_draw[k] = g for the gradient draw object k whose ramp word is bound gradient
+// g's (grad_dd[g], relative to the draw data). It reads at most n_draw tags, and the caller sets both tables to VB_COLOR_NONE
+// first. Per frame, in flatten's stage after the transforms (prepare reserved the region, vb_frame.cu): the scene's draw data
+// into the frame's region at layout.draw_data_base, each slot's word replaced by the word its binding makes from its row;
+// nothing while none of the three is bound.
 #define VB_COLOR_NONE 0xffffffffu
-uint32_t vb_launch_draw_color_slots(const uint32_t *tags, uint32_t n, uint32_t *slots, uint32_t n_words, cudaStream_t st);
-uint32_t vb_launch_draw_colors(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
-
-// k_opacity.cu: bound opacity (vb_bind_draw_opacity). The binding's table, once at bind time: table[k] for each draw object
-// k < n, from the scene's draw tags at `tags` and its draw data at `dd` (n_words words): VB_OP_ENTRY(w, kind) for a layer's
-// alpha word w (kind VB_OP_CLIP for a clip layer, whose blend word is w - 1, else VB_OP_LAYER) and an image's sample word w
-// (VB_OP_IMAGE), VB_COLOR_NONE for any other draw object. Per frame, in flatten's stage right after k_draw_colors has written
-// the frame's draw data (draw_data_bound holds while opacity is bound): each bound word with a finite row replaced by the row's
-// conversion; nothing while unbound.
-#define VB_OP_LAYER 1u
-#define VB_OP_CLIP 2u
-#define VB_OP_IMAGE 3u
-#define VB_OP_ENTRY(w, kind) (((w) << 2) | (kind))
-uint32_t vb_launch_draw_opacity_slots(const uint32_t *tags, const uint32_t *dd, uint32_t n, uint32_t n_words, uint32_t *table, cudaStream_t st);
-uint32_t vb_launch_draw_opacity(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
+uint32_t vb_launch_draw_data_slots(const VbBound &b, const uint32_t *tags, const uint32_t *dd, uint32_t n_words, uint32_t n_draw,
+                                   const uint32_t *grad_dd, uint32_t *slots, cudaStream_t st);
+uint32_t vb_launch_draw_data(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);
 
 // k_points.cu: bound path points (vb_bind_path_points). The binding's table, once at bind time, from the n_words path tag words
 // at `tags`: first[p] = the first point of path p for p <= n_paths (first[n_paths]: the scene's points), and *i16 = 1 when a
