@@ -549,6 +549,37 @@ int vb_fragment_from_device_paths(vb_renderer *, const vb_device_paths *, uint32
  * other brushes are not part of it. */
 int vb_fragment_from_device_curves(vb_renderer *, const vb_device_paths *, const uint8_t *point_kinds, uint32_t *fragment_out,
                                    uint32_t *n_draw_objects_out);
+/* vb_fragment_from_device_dashes: dashed strokes of the paths above (an addition; no vello counterpart): chart grid lines and
+ * threshold series, map borders and trails, focus rings and animated "marching ants". d->kind must be 1; point_kinds is as for
+ * vb_fragment_from_device_curves (NULL: polylines). The fragment is word for word what vb_fragment_upload receives from a fresh
+ * Scene that, for each path i in order, calls
+ *     stroke(Stroke{width, join, miter_limit, start_cap, end_cap, pattern, offset_i}, IDENTITY, Color(colors[i]), None, shape_i)
+ * offset_i being (double) offsets[i], or `offset` when offsets is NULL, and shape_i the shape of vb_fragment_from_device_curves
+ * with one exception: a ring of fewer than two points contributes no element. (The host dasher, kurbo's DashIterator as
+ * restated here, turns a closed one-point ring `M p Z` into Z and a segment left over from the rings before it; the undashed
+ * calls write nothing for such rings.) So the dashes are the host's bit for bit: each ring is dashed on its own, the phase
+ * starting again at each ring; every cut is made in f64 (pieces are sub-segments, their ends rounded to f32 like the host's);
+ * the first dash of a ring broken into several comes last, continuing the last dash when a closed ring ends inside one; and a
+ * closed ring that stays inside one dash comes out as M p0, its segments but the last, Z, then the last segment, which the
+ * encoder draws again from p0 when the path has already kept a segment (visible for a curved closing segment). That last
+ * behaviour is the host encoder's, which this call reproduces; it is not checked against kurbo itself. The fragment's
+ * allocation is the worst case of vb_fragment_from_device_paths for the dashes' points and sub-rings. The call synchronises
+ * vb_stream twice: once to size the dashes, once for the fragment's totals. An animated offset is a new fragment (and a
+ * recompose) per frame. Each ring's walk is serial, one warp per ring: a single long ring takes as long as its dashes.
+ * VB_E_INVALID as vb_fragment_from_device_curves, and also: dash NULL; kind 0; a pattern NULL, empty, with an entry that is not
+ * finite or is below 0, or whose entries sum to 0; a scalar offset that is not finite or lies more than 2^24 pattern entries
+ * before the pattern's start; offsets not 4-byte aligned device or managed memory of the renderer's device, or a pitch that is
+ * not a multiple of 4, below 4 or 4 GiB or more; dashes of more than 2^31 - 1 points or sub-rings, a ring whose control
+ * polygon's length allows 2^31 dash breaks (n_pattern (1.01 length / the pattern's sum + 2), refused before it is walked), or a
+ * worst case past 32-bit word offsets. Checked on the device, naming the first offending path: an offset that is not finite or lies more than 2^24
+ * pattern entries before the start; a piece's point that is not finite once rounded to f32. */
+typedef struct {
+    const double *pattern; uint32_t n_pattern; /* host memory: dash, gap, dash, ... lengths */
+    double offset;                             /* every path's offset when offsets is NULL */
+    const float *offsets; size_t offset_pitch_bytes; /* optional device f32, n_paths rows: path i's offset */
+} vb_dash;
+int vb_fragment_from_device_dashes(vb_renderer *, const vb_device_paths *, const uint8_t *point_kinds, const vb_dash *dash,
+                                   uint32_t *fragment_out, uint32_t *n_draw_objects_out);
 int vb_compose(vb_renderer *, const vb_instance *, uint32_t n, vb_layout *layout_out, uint32_t *draw_offsets);
 /* vb_recompose: vb_compose, followed by a frame that repaints only what the new instance list changed (an addition; no vello
  * counterpart). It installs exactly the scene vb_compose would (scene, layout, ramps, atlas and draw offsets, byte for byte),

@@ -11,8 +11,13 @@ contours (an outer contour and a counter each, filled, with point_kinds). Prints
               compose's stream lengths may change and the frame graph is captured anew (graph_captures counts it); and
               the cost of that capture: frames that cycle through six row counts (new lengths every frame, more than
               the four cached graphs, so a capture every frame), with frame graphs on and off
+Dashed strokes (Renderer.upload_device_dashes, vb_fragment_from_device_dashes) on three more inputs: the 30k polygons' outlines
+with pattern (6, 3), the 1M-point polyline with (4, 4) and the 100k circles with (2, 2). For each: call_ms and kernel_ms as
+above; kernels_us, each kernel's time per call from torch.profiler; host_ms, the host route with vb_scene_stroke's dashes (on
+the first `host_fraction` of the paths for the circles, whose host dash takes minutes); and `animated`, frames of build with
+the dash offset moved by 0.5 per frame + recompose + render at 4096^2 MSAA16, with frame graphs on and off.
 --inputs picks some of the inputs by name. With --out the result also goes to DIR/device_paths_probe.json:
-    python tools/device_paths_probe.py [--reps 10] [--frames 20] [--inputs polygons_30k,...] [--out DIR]"""
+    python tools/device_paths_probe.py [--reps 10] [--frames 20] [--inputs polygons_30k,...,dashes_polygons_30k] [--out DIR]"""
 import argparse
 import ctypes as C
 import json
@@ -206,18 +211,116 @@ def measure(r, name, data, style, reps, n_frames):
             "host_ms_median": round(float(np.median(host)), 3), "frames": out}
 
 
+def host_dash_route(r, pts, roff, poff, cols, stroke, kinds, closed, n_paths):
+    """The host route of a dashed stroke for the first n_paths paths: arrays to the host, one dashed vb_scene_stroke per path."""
+    p, ro, po, co, ki = (t.cpu().numpy() if t is not None else None for t in (pts, roff, poff, cols, kinds))
+    s = NativeScene()
+    lib, h = s.lib, s.handle
+    on = np.ones(len(p), bool) if ki is None else ki == 0
+    verb_of = np.frombuffer(b"?LQC", np.uint8)
+    verbs, vstart = [], [0]
+    for a, b in zip(ro[:-1], ro[1:]):
+        ends = np.flatnonzero(on[a:b])
+        verbs.append(np.concatenate([[ord("M")], verb_of[np.diff(ends)], [ord("Z")] if closed else []]).astype(np.uint8))
+        vstart.append(vstart[-1] + len(verbs[-1]))
+    verbs = np.concatenate(verbs)
+    coords = p.astype(np.float64).reshape(-1)
+    ident = _affine(Affine.IDENTITY)
+    pat = (C.c_double * len(stroke.dash_pattern))(*stroke.dash_pattern)
+    st = _Stroke(stroke.width, stroke.join, stroke.start_cap, stroke.end_cap, stroke.miter_limit, C.cast(pat, C.c_void_p),
+                 len(stroke.dash_pattern), stroke.dash_offset)
+    for i in range(n_paths):
+        r0, r1 = (int(po[i]), int(po[i + 1])) if po is not None else (i, i + 1)
+        b = _Brush()
+        b.kind, b.color = 0, _Color(*[float(v) for v in co[i]])
+        path = _Path(verbs.ctypes.data + int(vstart[r0]), int(vstart[r1] - vstart[r0]), coords.ctypes.data + 16 * int(ro[r0]))
+        lib.vb_scene_stroke(h, C.byref(st), ident, C.byref(b), None, C.byref(path))
+    return r.upload_fragment(s)
+
+
+def measure_dashes(r, name, data, stroke, closed, reps, n_frames, host_fraction=1.0):
+    pts, roff, poff, cols, kinds = (torch.as_tensor(a).cuda() if a is not None else None for a in (tuple(data) + (None,))[:5])
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    st = torch.cuda.ExternalStream(r.stream)
+    kw = dict(path_offsets=poff, closed=closed, point_kinds=kinds)
+    f, n = r.upload_device_dashes(pts, roff, cols, stroke, **kw)  # warm-up
+    r.free_fragment(f)
+    call, kern = [], []
+    for _ in range(reps):
+        ev0.record(st)
+        t0 = time.perf_counter()
+        f, n = r.upload_device_dashes(pts, roff, cols, stroke, **kw)
+        call.append((time.perf_counter() - t0) * 1e3)
+        ev1.record(st)
+        ev1.synchronize()
+        kern.append(ev0.elapsed_time(ev1))
+        r.free_fragment(f)
+    prof_calls = max(1, min(reps, 5))
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(prof_calls):
+            f, _ = r.upload_device_dashes(pts, roff, cols, stroke, **kw)
+            r.free_fragment(f)
+        torch.cuda.synchronize()
+    kernels = {}
+    for e in prof.key_averages():
+        if "k_device_" in e.key:
+            total = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0.0)
+            kernels[e.key.split("(")[0]] = round(total / prof_calls, 1)
+    n_paths = len(cols)
+    n_host = max(1, int(n_paths * host_fraction))
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    f = host_dash_route(r, pts, roff, poff, cols, stroke, kinds, closed, n_host)
+    host = (time.perf_counter() - t0) * 1e3
+    r.free_fragment(f)
+    # an animated dash offset: a new fragment each frame, recomposed beside nothing else and rendered
+    p = RenderParams(BLACK, SIZE, SIZE, AA_MSAA16)
+    anim = {}
+    for graphs in (True, False):
+        r.set_cuda_graph(graphs)
+        t0 = None
+        for k in range(n_frames + 3):
+            if k == 3:
+                torch.cuda.synchronize()
+                t0, cap0 = time.perf_counter(), r.debug_graph_captures()
+            moving = Stroke(stroke.width, stroke.join, stroke.miter_limit, stroke.start_cap, stroke.end_cap, stroke.dash_pattern,
+                            0.5 * k)
+            f, _ = r.upload_device_dashes(pts, roff, cols, moving, **kw)
+            r.recompose([(f, None)])
+            r.render_resident(p)
+            r.free_fragment(f)
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t0) * 1e3 / n_frames
+        anim["graphs" if graphs else "no_graphs"] = {"fps": round(1e3 / ms, 2), "ms_per_frame": round(ms, 3),
+                                                      "graph_captures": r.debug_graph_captures() - cap0}
+    r.set_cuda_graph(True)
+    return {"input": name, "pattern": list(stroke.dash_pattern), "points": int(pts.shape[0]), "paths": n_paths,
+            "draw_objects": n, "call_ms": [round(v, 3) for v in call], "kernel_ms": [round(v, 3) for v in kern],
+            "kernels_us": kernels, "host_ms": round(host, 1), "host_fraction": n_host / n_paths, "animated": anim}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--frames", type=int, default=20)
-    ap.add_argument("--inputs", default="polygons_30k,polyline_1m,circles_100k,glyphs_20k")
+    ap.add_argument("--inputs", default="polygons_30k,polyline_1m,circles_100k,glyphs_20k,dashes_polygons_30k,dashes_polyline_1m,"
+                                        "dashes_circles_100k")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     inputs = {"polygons_30k": (polygons, FILL_NON_ZERO), "polyline_1m": (polyline, Stroke(2.0)),
               "circles_100k": (circles, FILL_NON_ZERO), "glyphs_20k": (glyphs, FILL_NON_ZERO)}
+    dashes = {"dashes_polygons_30k": (polygons, Stroke(1.5, dash_pattern=(6.0, 3.0)), True, 1.0),
+              "dashes_polyline_1m": (polyline, Stroke(2.0, dash_pattern=(4.0, 4.0)), False, 1.0),
+              "dashes_circles_100k": (circles, Stroke(1.5, dash_pattern=(2.0, 2.0)), True, 0.05)}
     r = Renderer()
-    res = {"card": card(), "results": [measure(r, k, inputs[k][0](), inputs[k][1], a.reps, a.frames) for k in a.inputs.split(",")],
-           "card_after": card()}
+    results = []
+    for k in a.inputs.split(","):
+        if k in dashes:
+            make, stroke, closed, frac = dashes[k]
+            results.append(measure_dashes(r, k, make(), stroke, closed, a.reps, a.frames, frac))
+        else:
+            results.append(measure(r, k, inputs[k][0](), inputs[k][1], a.reps, a.frames))
+    res = {"card": card(), "results": results, "card_after": card()}
     print(json.dumps(res, indent=1))
     if a.out:
         os.makedirs(a.out, exist_ok=True)

@@ -39,6 +39,10 @@
 //     draw_index.
 // Every launch after the first returns at once when a check failed: the offsets and kinds are then not trusted to index
 // anything.
+// With ring_flags (the sub-rings of vb_fragment_from_device_dashes, k_device_dashes.cu) a ring closes by its flag instead of
+// `kind == 0 || closed`, and a conditional ring (the segment a dasher's walk pushes after Z) is kept only when a lower,
+// unconditional ring of its path keeps a segment (path_min): the encoder draws it from the first point only after the path
+// has encoded a segment.
 #include "vb_device.cuh"
 #include "vb_stages.h"
 
@@ -207,7 +211,8 @@ __global__ void __launch_bounds__(DP_THREADS) k_device_paths_rings(DpArgs a) {
             const float2 c1 = dp_point(a, first - 2u), c2 = dp_point(a, first - 1u);
             ste = dp_neq(c1, p0) ? c1 : (dp_neq(c2, p0) ? c2 : pe);
         }
-        const bool closes = a.kind == 0u || a.closed;
+        const uint32_t flags = a.ring_flags ? (uint32_t)a.ring_flags[r] : 0u;
+        const bool closes = a.ring_flags ? (flags & VB_DP_RING_CLOSED) != 0u : (a.kind == 0u || a.closed);
         if (closes && !dp_same_bits(pl, p0)) code |= DP_CLOSE;
         if (a.kind == 1u) {
             if (closes) {
@@ -216,7 +221,12 @@ __global__ void __launch_bounds__(DP_THREADS) k_device_paths_rings(DpArgs a) {
                 code |= DP_CAP_QUAD;
             }
         }
-        a.path_kept[a.path_offsets ? dp_find(a.path_offsets, a.n_paths, r) : r] = 1u;
+        // a conditional ring is kept after a kept unconditional one of its path (dp_out), which has marked the path
+        if (!(flags & VB_DP_RING_CONDITIONAL)) {
+            const uint32_t i = a.path_offsets ? dp_find(a.path_offsets, a.n_paths, r) : r;
+            a.path_kept[i] = 1u;
+            if (a.ring_flags) atomicMin(a.path_min + i, r);
+        }
     }
     a.rings[r] = make_uint4(last, code, __float_as_uint(ste.x), __float_as_uint(ste.y));
 }
@@ -235,7 +245,10 @@ __device__ __forceinline__ DpOut dp_out(const DpArgs &a, uint32_t j) {
     const uint32_t r = dp_find(a.ring_offsets, a.n_rings, j);
     const uint4 rec = a.rings[r];
     const uint32_t b0 = (uint32_t)__ldg(a.ring_offsets + r), b1 = (uint32_t)__ldg(a.ring_offsets + r + 1u), code = rec.y;
-    if (code & DP_KEPT) {
+    bool kept = code & DP_KEPT;
+    if (kept && a.ring_flags && (a.ring_flags[r] & VB_DP_RING_CONDITIONAL))
+        kept = a.path_min[dp_find(a.path_offsets, a.n_paths, r)] < r; // ring_flags come with path_offsets
+    if (kept) {
         o.p = dp_point(a, j);
         const uint32_t tail = code & (DP_CLOSE | DP_CAP_LINE | DP_CAP_QUAD);
         if (j == b0) {
@@ -353,14 +366,17 @@ __global__ void __launch_bounds__(DP_THREADS) k_device_paths_emit(DpArgs a) {
 }
 
 extern "C" uint32_t vb_launch_device_paths(const DpArgs &a, cudaStream_t st) {
-    const uint32_t checks = a.n_points > a.n_rings + 1u ? a.n_points : a.n_rings + 1u;
-    const uint32_t rows = checks > a.n_paths + 1u ? checks : a.n_paths + 1u;
-    k_device_paths_points<<<(rows + DP_THREADS - 1u) / DP_THREADS, DP_THREADS, 0, st>>>(a);
-    uint32_t n = 1u;
+    uint32_t n = vb_launch_device_paths_checks(a, st);
     if (a.n_rings) k_device_paths_rings<<<(a.n_rings + DP_THREADS - 1u) / DP_THREADS, DP_THREADS, 0, st>>>(a), n++;
     if (a.n_parts) k_device_paths_count<<<a.n_parts, DP_THREADS, 0, st>>>(a), n++;
     const uint32_t path_ctas = (a.n_paths + DP_THREADS - 1u) / DP_THREADS;
     k_device_paths_emit<<<a.n_parts > path_ctas ? a.n_parts : (path_ctas ? path_ctas : 1u), DP_THREADS, 0, st>>>(a);
     return n + 1u;
+}
+extern "C" uint32_t vb_launch_device_paths_checks(const DpArgs &a, cudaStream_t st) {
+    const uint32_t checks = a.n_points > a.n_rings + 1u ? a.n_points : a.n_rings + 1u;
+    const uint32_t rows = checks > a.n_paths + 1u ? checks : a.n_paths + 1u;
+    k_device_paths_points<<<(rows + DP_THREADS - 1u) / DP_THREADS, DP_THREADS, 0, st>>>(a);
+    return 1u;
 }
 extern "C" uint32_t vb_device_paths_parts(uint32_t n_points) { return (n_points + DP_THREADS - 1u) / DP_THREADS; }

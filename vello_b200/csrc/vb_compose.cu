@@ -301,16 +301,156 @@ extern "C" int vb_fragment_free(vb_renderer *r, uint32_t fragment) {
     return VB_OK;
 }
 
-// ---- fragments from device arrays: vb_fragment_from_device_paths / _curves (k_device_paths.cu) ------------------------------
+// ---- fragments from device arrays: vb_fragment_from_device_paths / _curves / _dashes (k_device_paths.cu, k_device_dashes.cu) --
 // The streams' lengths depend on the data (dropped points, closing lines, cap markers), so the fragment is allocated for the
 // worst case of the counts, the four launches write it, and the totals and the error word come back through pinned memory
 // after one synchronisation of the renderer's stream.
 static const uint32_t STROKE_JOINS[3] = {0u, 0x10000000u, 0x20000000u}, STROKE_CAPS[3] = {0u, 0x01000000u, 0x02000000u}; // path.rs:30-66
 static bool one_of(uint32_t v, const uint32_t (&set)[3]) { return v == set[0] || v == set[1] || v == set[2]; }
 
-// vb_fragment_from_device_paths (kinds NULL: every point on-curve) and vb_fragment_from_device_curves; `fn` names the call.
-static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d, const uint8_t *kinds, uint32_t *fragment_out,
-                       uint32_t *n_draw_objects_out) {
+// What a device check's error word says (VB_DP_ERR_*), naming the first offending row `at`.
+static std::string device_paths_error(uint32_t kind, const std::string &at) {
+    if (kind == VB_DP_ERR_RING_OFFSETS) return "ring_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_points";
+    if (kind == VB_DP_ERR_PATH_OFFSETS) return "path_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_rings";
+    if (kind == VB_DP_ERR_POINTS) return "point " + at + " is not finite";
+    if (kind == VB_DP_ERR_KINDS)
+        return "point_kinds[" + at + "] breaks the kinds: each is 0 (on-curve) or 1 (off-curve), a ring starts and ends on-curve, "
+               "and at most two off-curve points come in a row";
+    if (kind == VB_DP_ERR_DASH_OFFSETS)
+        return "the dash offset of path " + at + " is not finite, or is more than 2^24 pattern entries before the pattern's start";
+    return "the colour of path " + at + " is not finite";
+}
+
+// A dash offset's pre-roll into the pattern (dash_path in vb_scene.cpp): the dash index, bit 31 set when that dash is not drawn,
+// and what remains of it; false past the native front end's 2^24 steps.
+static bool dash_phase(const double *pattern, uint32_t n, double offset, uint32_t *ix, double *rem) {
+    uint32_t i = 0u, inactive = 0u;
+    double r = pattern[0] - offset;
+    for (uint32_t guard = 0u; r < 0.0; guard++) {
+        if (guard > (1u << 24)) return false;
+        i = (i + 1u) % n;
+        r += pattern[i];
+        inactive ^= 1u;
+    }
+    *ix = i | (inactive << 31);
+    *rem = r;
+    return true;
+}
+
+// The dashes of vb_fragment_from_device_dashes, cut on the device (k_device_dashes.cu) into an intermediate of sub-rings in
+// r->dashes_mid: *mid gets d with its points, offsets and counts replaced by the intermediate's, *mid_kinds its point kinds and
+// *mid_flags its VB_DP_RING_* flags. The arguments are checked; the device checks the arrays, then the totals come back through
+// pinned memory after one synchronisation of the renderer's stream.
+static int dash_intermediate(vb_renderer *r, const char *fn, const vb_device_paths *d, const uint8_t *kinds, const vb_dash *dash,
+                             vb_device_paths *mid, const uint8_t **mid_kinds, const uint8_t **mid_flags) {
+    auto bad = [&](const std::string &why) {
+        r->err = std::string(fn) + ": " + why;
+        return VB_E_INVALID;
+    };
+    const uint64_t P = d->n_points, R = d->n_rings, N = d->n_paths, D = dash->n_pattern;
+    // the scratch: [err, ring_first] set to all ones; [ring_last, ring_odd, the rings' prefixes and totals, the look-back's
+    // leading words] to zero; the rest of the look-back, the ring records, the paths' phases, the pattern
+    const uint32_t parts = vb_device_dashes_parts((uint32_t)R);
+    const size_t o_first = 16u, o_zero = up16(o_first + 4u * R), o_odd = o_zero + 4u * R, o_excl = up16(o_odd + 4u * R);
+    const size_t o_lb = up16(o_excl + 8u * (R + 1u)), o_rec = up16(o_lb + 4u * vb_lookback_words(parts, 2)), o_rem = o_rec + 16u * R;
+    const size_t o_ix = o_rem + 8u * N, o_pat = up16(o_ix + 4u * N), scratch = o_pat + 8u * D;
+    int rc;
+    if ((rc = compose_room(r, r->dashes_tmp, scratch))) return rc;
+    char *t = (char *)r->dashes_tmp.p;
+    DpArgs c;
+    memset(&c, 0, sizeof c);
+    c.points = d->points;
+    c.kinds = d->n_points ? kinds : nullptr;
+    c.ring_offsets = d->ring_offsets;
+    c.path_offsets = d->path_offsets;
+    c.colors = d->colors;
+    c.point_pitch = d->point_pitch_bytes;
+    c.color_pitch = d->color_pitch_bytes;
+    c.n_points = (uint32_t)P, c.n_rings = (uint32_t)R, c.n_paths = (uint32_t)N;
+    c.kind = d->kind;
+    c.err = (unsigned long long *)t;
+    c.ring_first = (uint32_t *)(t + o_first);
+    c.ring_last = (uint32_t *)(t + o_zero);
+    c.ring_odd = (uint32_t *)(t + o_odd);
+    DdArgs a;
+    memset(&a, 0, sizeof a);
+    a.points = d->points;
+    a.kinds = c.kinds;
+    a.ring_offsets = d->ring_offsets;
+    a.path_offsets = d->path_offsets;
+    a.point_pitch = d->point_pitch_bytes;
+    a.n_points = (uint32_t)P, a.n_rings = (uint32_t)R, a.n_paths = (uint32_t)N, a.n_parts = parts;
+    a.closed = d->closed ? 1u : 0u, a.n_pattern = (uint32_t)D;
+    a.pattern = (const double *)(t + o_pat);
+    for (uint32_t k = 0; k < dash->n_pattern; k++) a.pattern_period += dash->pattern[k];
+    a.err = c.err;
+    a.rec = (uint4 *)(t + o_rec);
+    a.excl = (uint2 *)(t + o_excl);
+    a.lookback = (uint32_t *)(t + o_lb);
+    if (dash->offsets) {
+        a.offsets = dash->offsets;
+        a.offset_pitch = dash->offset_pitch_bytes;
+        a.phase_rem = (double *)(t + o_rem);
+        a.phase_ix = (uint32_t *)(t + o_ix);
+    } else {
+        dash_phase(dash->pattern, dash->n_pattern, dash->offset, &a.scalar_ix, &a.scalar_rem); // checked by the caller
+    }
+    cudaStream_t st = r->stream;
+    PinnedStage &stage = r->pinned[PIN_COMPOSE];
+    uint8_t *h;
+    if ((rc = stage_host(r, stage, 16u + 8u * D, &h))) return rc;
+    memcpy(h + 16u, dash->pattern, 8u * D);
+    cudaError_t e2 = cudaMemsetAsync(t, 0xff, o_zero, st);
+    if (e2 == cudaSuccess) e2 = cudaMemsetAsync(t + o_zero, 0, o_lb - o_zero + 4u * VB_LB_ZERO_WORDS(parts), st);
+    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(t + o_pat, h + 16u, 8u * D, cudaMemcpyHostToDevice, st);
+    if (e2 == cudaSuccess && (rc = stage_copied(r, stage))) return rc;
+    if (e2 == cudaSuccess) {
+        vb_launch_device_dashes(c, a, st);
+        e2 = cudaGetLastError();
+    }
+    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(h, t, 8u, cudaMemcpyDeviceToHost, st);
+    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(h + 8u, t + o_excl + 8u * R, 8u, cudaMemcpyDeviceToHost, st);
+    if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(st);
+    if (e2 != cudaSuccess) {
+        r->err = std::string(fn) + ": " + cudaGetErrorString(e2);
+        return VB_E_CUDA;
+    }
+    unsigned long long err;
+    uint32_t tot[2];
+    memcpy(&err, h, 8u);
+    memcpy(tot, h + 8u, 8u);
+    if (err != ~0ull) return bad(device_paths_error((uint32_t)(err >> 32), std::to_string((uint32_t)err)));
+    if (tot[0] > 0x7fffffffu || tot[1] > 0x7fffffffu) return bad("the dashes' points or sub-rings exceed int32 offsets (a ring is refused before its walk "
+                                                                   "when its control polygon's length allows 2^31 dash breaks)");
+    // the intermediate: points, ring offsets, path offsets, then the kind and flag bytes
+    const uint64_t MP = tot[0], MR = tot[1];
+    const size_t o_roff = 8u * MP, o_poff = o_roff + 4u * (MR + 1u), o_kinds = o_poff + 4u * (N + 1u), o_flags = o_kinds + MP;
+    if ((rc = compose_room(r, r->dashes_mid, o_flags + MR))) return rc;
+    char *m = (char *)r->dashes_mid.p;
+    a.out_points = (float *)m;
+    a.out_ring_offsets = (int32_t *)(m + o_roff);
+    a.out_path_offsets = (int32_t *)(m + o_poff);
+    a.out_kinds = (uint8_t *)(m + o_kinds);
+    a.out_flags = (uint8_t *)(m + o_flags);
+    vb_launch_device_dashes_emit(a, st);
+    if ((e2 = cudaGetLastError()) != cudaSuccess) {
+        r->err = std::string(fn) + ": " + cudaGetErrorString(e2);
+        return VB_E_CUDA;
+    }
+    *mid = *d;
+    mid->points = a.out_points, mid->n_points = (uint32_t)MP, mid->point_pitch_bytes = 8u;
+    mid->ring_offsets = a.out_ring_offsets, mid->n_rings = (uint32_t)MR;
+    mid->path_offsets = a.out_path_offsets;
+    mid->closed = 0u;
+    *mid_kinds = a.out_kinds;
+    *mid_flags = a.out_flags;
+    return VB_OK;
+}
+
+// vb_fragment_from_device_paths (kinds NULL: every point on-curve), vb_fragment_from_device_curves and, with `dash`,
+// vb_fragment_from_device_dashes; `fn` names the call.
+static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d, const uint8_t *kinds, const vb_dash *dash,
+                       uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
     if (!r) return VB_E_INVALID;
     auto bad = [&](const std::string &why) {
         r->err = std::string(fn) + ": " + why;
@@ -341,28 +481,59 @@ static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d,
     } else {
         return bad("kind must be 0 (fill) or 1 (stroke)");
     }
+    if (dash) {
+        if (d->kind != 1u) return bad("dashes apply to strokes: kind must be 1");
+        if (!dash->pattern || !dash->n_pattern) return bad("the dash pattern is empty");
+        double sum = 0.0;
+        for (uint32_t k = 0; k < dash->n_pattern; k++) {
+            if (!(isfinite(dash->pattern[k]) && dash->pattern[k] >= 0.0)) return bad("the dash pattern's entries must be finite and >= 0");
+            sum += dash->pattern[k];
+        }
+        if (!(sum > 0.0)) return bad("the dash pattern's entries sum to 0");
+        if (dash->offsets) {
+            if (dash->offset_pitch_bytes < 4u || dash->offset_pitch_bytes % 4u || dash->offset_pitch_bytes > 0xffffffffu)
+                return bad("the dash offsets' pitch must be a multiple of 4 bytes, at least 4 and below 4 GiB");
+        } else {
+            uint32_t ix;
+            double rem;
+            if (!isfinite(dash->offset) || !dash_phase(dash->pattern, dash->n_pattern, dash->offset, &ix, &rem))
+                return bad("the dash offset is not finite, or is more than 2^24 pattern entries before the pattern's start");
+        }
+    }
     // the worst case: a tag per point, the closing line and a cap marker per ring, a PATH tag per path, the TRANSFORM and STYLE
-    // tags; 2 words per point and 4 per ring (closing line and cap line, or cap quad); a draw object per path
+    // tags; 2 words per point and 4 per ring (closing line and cap line, or cap quad); a draw object per path (for dashes, of
+    // the intermediate's counts, below)
     uint64_t off[CMP_HEADER_WORDS];
     const uint64_t worst[CMP_STREAMS] = {N ? 2u + P + 2u * R + N : 0u, 2u * P + 4u * R, N, N, N ? 1u : 0u, N ? 2u : 0u};
-    const size_t bytes = fragment_layout(worst, off);
-    if (!bytes) return bad("the fragment's worst-case streams exceed 32-bit word offsets");
+    size_t bytes = fragment_layout(worst, off);
+    if (!bytes && !dash) return bad("the fragment's worst-case streams exceed 32-bit word offsets");
     CK(cudaSetDevice(r->device));
-    const void *ptrs[5] = {d->points, d->ring_offsets, d->path_offsets, d->colors, d->draw_index};
+    const void *ptrs[6] = {d->points, d->ring_offsets, d->path_offsets, d->colors, d->draw_index, dash ? dash->offsets : nullptr};
     for (const void *p : ptrs)
         if (p && ((uintptr_t)p % 4u || !device_memory_of(r, p)))
             return bad("every array must be 4-byte aligned device or managed memory of the renderer's device");
     if (kinds && d->n_points && !device_memory_of(r, kinds)) return bad("point_kinds must be device or managed memory of the renderer's device");
     reap_freed(r);
 
-    // the scratch (DpArgs): [err, ring_first] set to all ones, [totals, ring_last, ring_odd, path_kept, the look-back's leading
-    // words] to zero, then the rest of the look-back, the partitions' prefixes, the ring records and the keep bytes
-    const uint32_t parts = vb_device_paths_parts((uint32_t)P);
-    const size_t lb_words = vb_lookback_words(parts, 3);
-    const size_t o_first = 16u, o_zero = up16(o_first + 4u * R), o_last = o_zero + 16u, o_odd = o_last + 4u * R, o_kept = o_odd + 4u * R;
-    const size_t o_lb = up16(o_kept + 4u * N), o_excl = up16(o_lb + 4u * lb_words), o_rings = up16(o_excl + 12u * parts);
-    const size_t o_keep = o_rings + 16u * R, scratch = o_keep + P;
+    vb_device_paths mid;
+    const uint8_t *ring_flags = nullptr;
     int rc;
+    if (dash) {
+        if ((rc = dash_intermediate(r, fn, d, kinds, dash, &mid, &kinds, &ring_flags))) return rc;
+        d = &mid;
+        const uint64_t MP = d->n_points, MR = d->n_rings;
+        const uint64_t mworst[CMP_STREAMS] = {N ? 2u + MP + 2u * MR + N : 0u, 2u * MP + 4u * MR, N, N, N ? 1u : 0u, N ? 2u : 0u};
+        if (!(bytes = fragment_layout(mworst, off))) return bad("the fragment's worst-case streams exceed 32-bit word offsets");
+    }
+    const uint64_t MP = d->n_points, MR = d->n_rings;
+    // the scratch (DpArgs): [err, ring_first, path_min] set to all ones, [totals, ring_last, ring_odd, path_kept, the look-back's
+    // leading words] to zero, then the rest of the look-back, the partitions' prefixes, the ring records and the keep bytes
+    const uint32_t parts = vb_device_paths_parts((uint32_t)MP);
+    const size_t lb_words = vb_lookback_words(parts, 3);
+    const size_t o_first = 16u, o_min = o_first + 4u * MR, o_zero = up16(o_min + (ring_flags ? 4u * N : 0u)), o_last = o_zero + 16u;
+    const size_t o_odd = o_last + 4u * MR, o_kept = o_odd + 4u * MR;
+    const size_t o_lb = up16(o_kept + 4u * N), o_excl = up16(o_lb + 4u * lb_words), o_rings = up16(o_excl + 12u * parts);
+    const size_t o_keep = o_rings + 16u * MR, scratch = o_keep + MP;
     if ((rc = compose_room(r, r->paths_tmp, scratch))) return rc;
     char *t = (char *)r->paths_tmp.p;
     std::unique_ptr<Fragment> f(new Fragment());
@@ -381,7 +552,7 @@ static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d,
     a.colors = d->colors;
     a.point_pitch = d->point_pitch_bytes;
     a.color_pitch = d->color_pitch_bytes;
-    a.n_points = (uint32_t)P, a.n_rings = (uint32_t)R, a.n_paths = (uint32_t)N, a.n_parts = parts;
+    a.n_points = (uint32_t)MP, a.n_rings = (uint32_t)MR, a.n_paths = (uint32_t)N, a.n_parts = parts;
     a.kind = d->kind, a.closed = d->closed ? 1u : 0u, a.style_flags = flags, a.style_width = width;
     a.err = (unsigned long long *)t;
     a.ring_first = (uint32_t *)(t + o_first);
@@ -395,6 +566,8 @@ static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d,
     a.keep_fix = (uint8_t *)(t + o_keep);
     a.fragment = (uint32_t *)f->mem;
     a.draw_index = d->draw_index;
+    a.ring_flags = ring_flags;
+    a.path_min = ring_flags ? (uint32_t *)(t + o_min) : nullptr;
     cudaStream_t st = r->stream;
     PinnedStage &stage = r->pinned[PIN_COMPOSE];
     uint8_t *h;
@@ -421,17 +594,11 @@ static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d,
     memcpy(&err, h, 8u);
     memcpy(tot, h + 8u, 12u);
     if (err != ~0ull) {
-        const uint32_t row = (uint32_t)err;
-        const uint32_t kind = (uint32_t)(err >> 32);
-        const std::string at = std::to_string(row);
+        const std::string at = std::to_string((uint32_t)err);
         fail(0);
-        if (kind == VB_DP_ERR_RING_OFFSETS) return bad("ring_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_points");
-        if (kind == VB_DP_ERR_PATH_OFFSETS) return bad("path_offsets[" + at + "] breaks the offsets: they start at 0, never decrease and end at n_rings");
-        if (kind == VB_DP_ERR_POINTS) return bad("point " + at + " is not finite");
-        if (kind == VB_DP_ERR_KINDS)
-            return bad("point_kinds[" + at + "] breaks the kinds: each is 0 (on-curve) or 1 (off-curve), a ring starts and ends on-curve, "
-                       "and at most two off-curve points come in a row");
-        return bad("the colour of path " + at + " is not finite");
+        // the dashes' intermediate passed the arrays' checks: only a piece's point can fail, rounded to f32 past its range
+        if (dash) return bad("point " + at + " of the dashes is not finite in f32");
+        return bad(device_paths_error((uint32_t)(err >> 32), at));
     }
     const uint64_t units[CMP_STREAMS] = {N ? 2u + tot[0] : 0u, tot[1], tot[2], tot[2], N ? 1u : 0u, N ? 2u : 0u};
     *fragment_out = fragment_register(r, std::move(f), units, tot[2], 0u, 0u, tot[2]); // FILL_COLOR has one info word
@@ -439,11 +606,20 @@ static int from_device(vb_renderer *r, const char *fn, const vb_device_paths *d,
     return VB_OK;
 }
 extern "C" int vb_fragment_from_device_paths(vb_renderer *r, const vb_device_paths *d, uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
-    return from_device(r, "vb_fragment_from_device_paths", d, nullptr, fragment_out, n_draw_objects_out);
+    return from_device(r, "vb_fragment_from_device_paths", d, nullptr, nullptr, fragment_out, n_draw_objects_out);
 }
 extern "C" int vb_fragment_from_device_curves(vb_renderer *r, const vb_device_paths *d, const uint8_t *point_kinds, uint32_t *fragment_out,
                                               uint32_t *n_draw_objects_out) {
-    return from_device(r, "vb_fragment_from_device_curves", d, point_kinds, fragment_out, n_draw_objects_out);
+    return from_device(r, "vb_fragment_from_device_curves", d, point_kinds, nullptr, fragment_out, n_draw_objects_out);
+}
+extern "C" int vb_fragment_from_device_dashes(vb_renderer *r, const vb_device_paths *d, const uint8_t *point_kinds, const vb_dash *dash,
+                                              uint32_t *fragment_out, uint32_t *n_draw_objects_out) {
+    if (!r) return VB_E_INVALID;
+    if (!dash) {
+        r->err = "vb_fragment_from_device_dashes: NULL dash";
+        return VB_E_INVALID;
+    }
+    return from_device(r, "vb_fragment_from_device_dashes", d, point_kinds, dash, fragment_out, n_draw_objects_out);
 }
 
 

@@ -315,6 +315,8 @@ struct vb_renderer {
     uint64_t compose_seq = 0;
     DevBuf compose_tmp;                  // compose's tables, staged through pinned[PIN_COMPOSE]
     DevBuf paths_tmp;                    // the scratch of vb_fragment_from_device_paths (DpArgs, k_device_paths.cu)
+    DevBuf dashes_tmp;                   // the scratch of vb_fragment_from_device_dashes' walk (DdArgs, k_device_dashes.cu)
+    DevBuf dashes_mid;                   // its intermediate of sub-rings, which k_device_paths.cu encodes
     // What is bound to device rows (vb_bind_*, vb_compose.cu), with the device tables the bindings made at bind time (VbBound,
     // vb_stages.h), which point into the buffers below. Every scene installation unbinds (set_scene).
     //  - inst_tables: [prefix of the instances' transform counts (n + 1)] [compose-time transforms (n)] [the fragments'
@@ -384,7 +386,7 @@ struct vb_renderer {
 template <class F> static void for_each_buf(vb_renderer *r, F f) {
     DevBuf *const all[] = {&r->slot[0].scene, &r->slot[0].ramps, &r->slot[0].atlas, &r->slot[1].scene, &r->slot[1].ramps, &r->slot[1].atlas,
                            &r->mask8, &r->mask16, &r->cell_draw, &r->target, &r->target_alt, &r->resolve_tmp, &r->blit_rects, &r->xc.arena,
-                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->paths_tmp, &r->inst_tables, &r->dd_slots, &r->point_slots,
+                           &r->view_coef, &r->hit_io, &r->stop_pool, &r->compose_tmp, &r->paths_tmp, &r->dashes_tmp, &r->dashes_mid, &r->inst_tables, &r->dd_slots, &r->point_slots,
                            &r->stop_tables, &r->stop_ramps, &r->xform_ranges, &r->vis_mask, &r->width_snap,
                            &r->dmg_mask, &r->dmg_pending, &r->dmg_snap, &r->dmg_diff, &r->spare_scene, &r->spare_ramps, &r->spare_atlas};
     for (DevBuf *b : all) f(*b);

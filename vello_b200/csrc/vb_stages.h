@@ -246,11 +246,17 @@ uint32_t vb_launch_compose(CmpArgs a, cudaStream_t st);
 // keep byte per end point of a walked ring; a kept flag per path (zero); the error (all ones until a check fails: (kind << 32)
 // | first row); the look-back (vb_lookback_words(n_parts, 3), its leading words zero); each partition's exclusive prefix (3
 // words); the totals of tag bytes, path-data words and draw objects (zero), which the caller reads back.
+// ring_flags (optional, one byte per ring; the dashes' sub-rings, k_device_dashes.cu) replaces the uniform closing: a ring
+// closes when it has VB_DP_RING_CLOSED, and a VB_DP_RING_CONDITIONAL ring is kept only after a kept unconditional ring of its
+// path: path_min (all ones) gets each path's lowest such ring.
 #define VB_DP_ERR_RING_OFFSETS 1u
 #define VB_DP_ERR_PATH_OFFSETS 2u
 #define VB_DP_ERR_POINTS 3u
 #define VB_DP_ERR_COLOR 4u
 #define VB_DP_ERR_KINDS 5u // a kind other than 0 or 1; an off-curve point first or last in its ring, or third in a row
+#define VB_DP_ERR_DASH_OFFSETS 6u // a dash offset that is not finite, or whose pre-roll into the pattern passes 2^24 steps
+#define VB_DP_RING_CLOSED 1u
+#define VB_DP_RING_CONDITIONAL 2u
 struct DpArgs {
     const float *points;
     const uint8_t *kinds; // null: every point on-curve
@@ -267,9 +273,46 @@ struct DpArgs {
     uint32_t *lookback, *part_excl, *totals;
     uint32_t *fragment;
     int32_t *draw_index; // optional
+    const uint8_t *ring_flags; // optional: VB_DP_RING_* per ring
+    uint32_t *path_min;
 };
 uint32_t vb_device_paths_parts(uint32_t n_points);
 uint32_t vb_launch_device_paths(const DpArgs &a, cudaStream_t st);
+// the first launch alone: the checks (and the per-ring tables they fill, ring_first, ring_last and ring_odd)
+uint32_t vb_launch_device_paths_checks(const DpArgs &a, cudaStream_t st);
+
+// k_device_dashes.cu: the dashes of vb_fragment_from_device_dashes, cut on the device into an intermediate of sub-rings that
+// k_device_paths.cu encodes (ring_flags). The input arrays (as DpArgs), the pattern (device f64) and the offsets: per path
+// (offsets, f32 rows) or one pre-rolled phase for all (scalar_rem, scalar_ix: the dash index, bit 31 set when not drawn). The
+// scratch: per path its pre-rolled phase; the error word DpArgs::err; per ring its record {points, sub-rings, S's points, S's
+// sub-rings} and its exclusive prefix {points, sub-rings}, entry n_rings the totals (zero when there is no ring), saturating at
+// 2^31; the look-back (vb_lookback_words(n_parts, 2), its leading words zero). The intermediate: f32 points (8 bytes apart),
+// a kind per point, ring offsets (totals.y + 1), path offsets over the sub-rings (n_paths + 1) and a VB_DP_RING_* per sub-ring.
+struct DdArgs {
+    const float *points;
+    const uint8_t *kinds;
+    const int32_t *ring_offsets, *path_offsets;
+    size_t point_pitch;
+    uint32_t n_points, n_rings, n_paths, n_parts, closed, n_pattern;
+    const double *pattern;
+    double pattern_period; // the sum of the pattern's entries (> 0)
+    const float *offsets;
+    size_t offset_pitch;
+    double scalar_rem;
+    uint32_t scalar_ix;
+    double *phase_rem;
+    uint32_t *phase_ix;
+    unsigned long long *err;
+    uint4 *rec;
+    uint2 *excl;
+    uint32_t *lookback;
+    float *out_points;
+    uint8_t *out_kinds, *out_flags;
+    int32_t *out_ring_offsets, *out_path_offsets;
+};
+uint32_t vb_device_dashes_parts(uint32_t n_rings);
+uint32_t vb_launch_device_dashes(const DpArgs &checks, const DdArgs &a, cudaStream_t st); // the checks, phases, counts and scan
+uint32_t vb_launch_device_dashes_emit(const DdArgs &a, cudaStream_t st);
 // bound instance transforms: row_k * T of every transform T of the composed scene into the frame's bound region (prepare,
 // vb_frame.cu), in flatten's stage before the view's transforms; nothing while unbound
 uint32_t vb_launch_instance_transforms(const VbConfig &cfg, const VbFrameBufs &b, cudaStream_t st);

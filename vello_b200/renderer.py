@@ -73,6 +73,11 @@ class _DevicePaths(C.Structure):
                 ("end_cap", C.c_uint32), ("closed", C.c_uint32), ("draw_index", C.c_void_p)]
 
 
+class _Dash(C.Structure):
+    _fields_ = [("pattern", C.c_void_p), ("n_pattern", C.c_uint32), ("offset", C.c_double), ("offsets", C.c_void_p),
+                ("offset_pitch_bytes", C.c_size_t)]
+
+
 class _Instance(C.Structure):
     _fields_ = [("fragment", C.c_uint32), ("has_transform", C.c_uint32), ("transform", C.c_double * 6)]
 
@@ -179,6 +184,8 @@ def load_library() -> C.CDLL:
     lib.vb_fragment_free.argtypes = [vp, C.c_uint32]
     lib.vb_fragment_from_device_paths.argtypes = [vp, C.POINTER(_DevicePaths), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     lib.vb_fragment_from_device_curves.argtypes = [vp, C.POINTER(_DevicePaths), vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    lib.vb_fragment_from_device_dashes.argtypes = [vp, C.POINTER(_DevicePaths), vp, C.POINTER(_Dash), C.POINTER(C.c_uint32),
+                                                   C.POINTER(C.c_uint32)]
     lib.vb_compose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_recompose.argtypes = [vp, vp, C.c_uint32, C.POINTER(_Layout), vp]
     lib.vb_debug_match_instances.argtypes = [vp, C.c_uint32, vp, C.c_uint32, vp]
@@ -215,7 +222,8 @@ EXPORTED_SYMBOLS = ["vb_renderer_new", "vb_renderer_free", "vb_strerror", "vb_la
                     "vb_recompose", "vb_set_upload_diff", "vb_register_destination", "vb_unregister_destination",
                     "vb_bind_draw_colors", "vb_bind_path_points", "vb_bind_gradient_stops", "vb_bind_transforms",
                     "vb_set_background", "vb_bind_draw_visibility", "vb_bind_stroke_widths", "vb_bind_draw_opacity",
-                    "vb_fragment_from_device_paths", "vb_fragment_from_device_curves"]
+                    "vb_fragment_from_device_paths", "vb_fragment_from_device_curves",
+                    "vb_fragment_from_device_dashes"]
 
 
 def _device_rows(t, who: str, what: str, cols: int, vector: bool = False, empty: bool = False):
@@ -575,6 +583,53 @@ class Renderer:
         the arrays on `self.stream` (or synchronise) before the call; it returns once the fragment is built."""
         from .encoding import Stroke
         who = "upload_device_paths"
+        d, kinds = self._device_paths(who, points, ring_offsets, colors, path_offsets, draw_index, point_kinds)
+        if isinstance(style, Stroke):
+            if style.dash_pattern:
+                raise ValueError(f"{who}: dashed strokes are built by upload_device_dashes (or encode them with Scene.stroke)")
+            self._device_stroke(d, style, closed)
+        else:
+            d.kind, d.fill_rule = 0, int(style)
+        fid, n_draws = C.c_uint32(0), C.c_uint32(0)
+        if point_kinds is None:
+            self._check(self.lib.vb_fragment_from_device_paths(self.handle, C.byref(d), C.byref(fid), C.byref(n_draws)),
+                        "vb_fragment_from_device_paths")
+        else:
+            self._check(self.lib.vb_fragment_from_device_curves(self.handle, C.byref(d), kinds, C.byref(fid), C.byref(n_draws)),
+                        "vb_fragment_from_device_curves")
+        return int(fid.value), int(n_draws.value)
+
+    def upload_device_dashes(self, points, ring_offsets, colors, stroke, *, path_offsets=None, closed: bool = True,
+                             draw_index=None, point_kinds=None, dash_offsets=None):
+        """Build a fragment of dashed strokes on the device (`vb_fragment_from_device_dashes`) and return (fragment id, draw
+        objects). The arrays are those of `upload_device_paths` (with `point_kinds`, curved paths); `stroke` is a dashed
+        `Stroke`, whose pattern and offset cut every path, or, with `dash_offsets` (float32 (N,) device array, or a column of a
+        larger one), path i's offset is dash_offsets[i]: an animated offset is a new fragment per frame. The fragment is word for
+        word `upload_fragment` of a Scene that strokes each path i with Color(colors[i]) under the identity, with `stroke` and
+        dash offset float(dash_offsets[i]) (or stroke.dash_offset), its shape being `upload_device_paths`' with the rings of fewer
+        than two points left out. Write the arrays on `self.stream` (or synchronise) before the call; it returns once the
+        fragment is built."""
+        from .encoding import Stroke
+        who = "upload_device_dashes"
+        if not isinstance(stroke, Stroke) or not stroke.dash_pattern:
+            raise ValueError(f"{who}: stroke must be a Stroke with a dash pattern")
+        d, kinds = self._device_paths(who, points, ring_offsets, colors, path_offsets, draw_index, point_kinds)
+        self._device_stroke(d, stroke, closed)
+        pattern = (C.c_double * len(stroke.dash_pattern))(*(float(v) for v in stroke.dash_pattern))
+        dash = _Dash(C.cast(pattern, C.c_void_p), len(stroke.dash_pattern), float(stroke.dash_offset), None, 4)
+        if dash_offsets is not None:
+            ptr, n, pitch = _device_rows(dash_offsets, who, "dash offsets", 1, vector=True, empty=True)
+            if n != d.n_paths:
+                raise ValueError(f"{who}: {n} dash offsets for {d.n_paths} paths")
+            dash.offsets, dash.offset_pitch_bytes = ptr, pitch
+        fid, n_draws = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.lib.vb_fragment_from_device_dashes(self.handle, C.byref(d), kinds, C.byref(dash), C.byref(fid),
+                                                            C.byref(n_draws)), "vb_fragment_from_device_dashes")
+        return int(fid.value), int(n_draws.value)
+
+    @staticmethod
+    def _device_paths(who, points, ring_offsets, colors, path_offsets, draw_index, point_kinds):
+        """The checked arrays of `upload_device_paths` and `upload_device_dashes`: (_DevicePaths without its style, kinds)."""
         pts, n_pts, pitch = _device_rows(points, who, "points", 2, empty=True)
         rings, n_roff = _device_offsets(ring_offsets, who, "ring_offsets")
         if n_roff == 0:
@@ -587,26 +642,17 @@ class Renderer:
             raise ValueError(f"{who}: {n_cols} colours for {n_poff - 1} paths")
         kinds = None if point_kinds is None else _device_kinds(point_kinds, n_pts, who)
         d = _DevicePaths(pts, n_pts, pitch, rings, n_roff - 1, paths, n_poff - 1, cols, cpitch)
-        if isinstance(style, Stroke):
-            if style.dash_pattern:
-                raise ValueError(f"{who}: dashed strokes are not built on the device; encode them with Scene.stroke")
-            d.kind, d.width, d.miter_limit = 1, style.width, style.miter_limit
-            d.join, d.start_cap, d.end_cap, d.closed = style.join, style.start_cap, style.end_cap, 1 if closed else 0
-        else:
-            d.kind, d.fill_rule = 0, int(style)
         if draw_index is not None:
             idx, n_idx = _device_offsets(draw_index, who, "draw_index")
             if n_idx != n_poff - 1:
                 raise ValueError(f"{who}: draw_index has {n_idx} entries for {n_poff - 1} paths")
             d.draw_index = idx
-        fid, n_draws = C.c_uint32(0), C.c_uint32(0)
-        if point_kinds is None:
-            self._check(self.lib.vb_fragment_from_device_paths(self.handle, C.byref(d), C.byref(fid), C.byref(n_draws)),
-                        "vb_fragment_from_device_paths")
-        else:
-            self._check(self.lib.vb_fragment_from_device_curves(self.handle, C.byref(d), kinds, C.byref(fid), C.byref(n_draws)),
-                        "vb_fragment_from_device_curves")
-        return int(fid.value), int(n_draws.value)
+        return d, kinds
+
+    @staticmethod
+    def _device_stroke(d, stroke, closed):
+        d.kind, d.width, d.miter_limit = 1, stroke.width, stroke.miter_limit
+        d.join, d.start_cap, d.end_cap, d.closed = stroke.join, stroke.start_cap, stroke.end_cap, 1 if closed else 0
 
     def free_fragment(self, fragment: int):
         """Release a fragment (after the work already enqueued that reads it). Composed scenes are copies: they stay."""
